@@ -1,4 +1,4 @@
-"""Builds the C-ABI shared library in-tree: nvcc, sm_100a only.
+"""Builds the C-ABI shared library in-tree: nvcc, sm_90a (H100) only.
 
 Translation units (compiled in parallel, then linked into libbsched.so):
   engine.cu            the C ABI, host sequencing and every kernel but the dominant one
@@ -55,7 +55,7 @@ def build(force: bool = False, verbose: bool = False, lib: str = None, extra=Non
     extra = list(extra or []) + os.environ.get("BS_NVCC_EXTRA", "").split()
     objdir = OBJ if lib == LIB and not extra else OBJ + "_" + os.path.splitext(os.path.basename(lib))[0]
     os.makedirs(objdir, exist_ok=True)
-    base = [nvcc_path(), "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+    base = [nvcc_path(), "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
             "-Xcompiler", "-fPIC,-Wall,-fopenmp", "-fmad=false", "-diag-suppress=186,550"] + extra
     if verbose:
         base.insert(1, "-Xptxas=-v")
@@ -71,7 +71,7 @@ def build(force: bool = False, verbose: bool = False, lib: str = None, extra=Non
 
     with ThreadPoolExecutor(max_workers=max(1, min(os.cpu_count() or 1, len(_units())))) as ex:
         objs = list(ex.map(compile_one, _units()))
-    subprocess.check_call([nvcc_path(), "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", lib] + objs +
+    subprocess.check_call([nvcc_path(), "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", lib] + objs +
                           ["-lgomp"], cwd=CSRC)
     return lib
 

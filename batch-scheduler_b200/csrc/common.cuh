@@ -1,4 +1,4 @@
-// common.cuh — constants and lane-layout types shared by every sm_100a translation unit of the engine.
+// common.cuh — constants and lane-layout types shared by every sm_90a translation unit of the engine.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -68,22 +68,13 @@ static_assert(TILE_WORDS <= 16, "best-node key: score (27 bits) + word index (4 
 #define BS_FIT_STAGES 2
 #endif
 constexpr int FIT_STAGES = BS_FIT_STAGES;               // TMA ring depth (full/empty mbarrier pairs)
-// Score rows leave the SMs with 8-byte streaming stores (BS_FIT_STG, default).  -DBS_FIT_TMA_STORE stages them in
-// shared memory and hands FIT_SEG-node row segments to the TMA engine instead (cp.async.bulk shared -> global):
-// built, parity-tested and measured in round 2 — 3 % slower in the kernel (the per-segment proxy fence and
-// issue cost more than the cleaner HBM burst pattern returns), see profiles/README.md.
-#if !defined(BS_FIT_TMA_STORE) && !defined(BS_FIT_STG)
-#define BS_FIT_STG 1
-#endif
+// Score rows are staged in shared memory and leave the SMs as FIT_SEG-node row segments handed to the TMA engine
+// (cp.async.bulk shared -> global).  -DBS_FIT_STG writes them with 8-byte streaming stores instead: measured on an
+// H100, 3 % slower in the score-mode kernel (gang_fit 3.95 vs 3.83 ms on the bench workload, profiles/README.md).
 #ifndef BS_FIT_SEG
-#ifdef BS_FIT_STG
-#define BS_FIT_SEG BS_FIT_TILE
-#else
 #define BS_FIT_SEG 128
 #endif
-#endif
 constexpr int FIT_SEG = BS_FIT_SEG;                     // nodes per score store segment (one bulk store per pod row)
-constexpr int SEG_WORDS = FIT_SEG / 32;
 static_assert(NODE_TILE % FIT_SEG == 0 && FIT_SEG % 128 == 0, "a tile is a whole number of 128-node-multiple segments");
 #ifndef BS_FIT_NB
 #define BS_FIT_NB 2

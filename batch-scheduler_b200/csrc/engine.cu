@@ -1,4 +1,4 @@
-// engine.cu — C ABI (include/bsched.h) of the B200 gang-scheduling feasibility engine.
+// engine.cu — C ABI (include/bsched.h) of the H100 gang-scheduling feasibility engine.
 //
 // Host side: table validation + upload, class de-duplication of the pre-encoded
 // selector/toleration masks, kernel sequencing on one CUDA stream (the queue sort
@@ -988,8 +988,8 @@ int evaluate_async_locked(bs_engine* e) {
         // Two builds of the same kernel.  Beside a long fit kernel the sort is hidden anyway and must stay out of its
         // way (32 registers: its CTAs share their SMs with the fit CTAs); when the fit kernel is the shorter of the two
         // (a small shard, few nodes) the round waits for the sort, and the build with 16 gathers in flight per thread
-        // is the faster one.  Estimate: pairs x the measured per-pair time of the output mode.
-        const double est_fit_ms = (double)P * (double)e->N * ((e->out_flags & BS_OUT_SCORE) ? 1.4e-9 : 0.8e-9);
+        // is the faster one.  Estimate: pairs x the per-pair time of the output mode measured on an H100.
+        const double est_fit_ms = (double)P * (double)e->N * ((e->out_flags & BS_OUT_SCORE) ? 3.8e-9 : 0.9e-9);
         const bool lean = e->sort_variant == 1 || (e->sort_variant == 0 && est_fit_ms > 0.6);
         const void* fn = lean ? (const void*)queue_sort_kernel<SORT_LEAN_GROUP> : (const void*)queue_sort_kernel<SORT_WIDE_GROUP>;
         CK(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(SORT_THREADS), params, 0, e->s2));

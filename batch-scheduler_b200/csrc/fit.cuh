@@ -24,14 +24,15 @@ namespace bsk {
 //   INPUT: the producer lane streams the tiles of the residual table into a FIT_STAGES-deep
 //     shared-memory ring with 1-D TMA bulk copies (cp.async.bulk global->shared, one per lane
 //     row), guarded by full/empty mbarrier pairs; consumers never meet at a CTA-wide barrier.
-//   OUTPUT (round 2): score rows do NOT leave through the LSU.  A warp writes the NODE_TILE
-//     scores of each of its pods into a private staging slab in shared memory (st.shared.u64,
-//     conflict-free) and one lane hands every row segment — NODE_TILE*8 contiguous bytes of one
+//   OUTPUT: score rows do NOT leave through the LSU.  A warp writes the FIT_SEG scores of a
+//     segment for each of its pods into a private staging slab in shared memory (st.shared.u64,
+//     conflict-free) and one lane hands every row segment — FIT_SEG*8 contiguous bytes of one
 //     matrix row — to the TMA engine (cp.async.bulk shared->global, bulk_group completion);
 //     FIT_NB slabs per warp rotate, a slab is refilled once its bulk reads have finished
-//     (cp.async.bulk.wait_group.read).  HBM then sees 2 KB bursts per row instead of 256-byte
-//     pieces of four interleaved rows: the store pattern alone went from 1.34 ms to 1.14 ms for
-//     the 8 GB matrix of the bench workload (profiles/microbench/store_pattern2.cu; cudaMemset 1.09).
+//     (cp.async.bulk.wait_group.read).  HBM then sees 1 KB bursts per row instead of 256-byte
+//     pieces of four interleaved rows: on an H100 the store pattern alone takes 2.61 ms instead of
+//     2.73 ms for the 8 GB matrix of the bench workload (profiles/microbench/store_pattern2.cu;
+//     cudaMemset 2.44).
 // A lane owns nodes lane, lane+32, ... of the tile, keeps their `left` in registers and evaluates
 // PODS_PER_WARP pods against them at a time.
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
@@ -160,7 +161,7 @@ template <> struct BestT<true> { using type = int32_t; };
 // OUT: what leaves the SMs besides the per-pod results — 0 nothing (decisions only: feasible counts come from a
 // predicated add, no ballot), 1 the fit bitmap, 2 the score matrix (+ the bitmap when its pointer is set).
 enum { FIT_OUT_NONE = 0, FIT_OUT_BITMAP = 1, FIT_OUT_SCORE = 2 };
-template <int LW, int LN, int LS, int OUT>
+template <int LW, int LN, int LS, int OUT, int SEGW /*words of the segment*/>
 __device__ __forceinline__ void fit_seg(const FitArgs& a, const int64_t* __restrict__ tlw,
                                          const int32_t* __restrict__ tln,
                                          const int64_t (&rqw)[PODS_PER_WARP][LW > 0 ? LW : 1],
@@ -180,7 +181,7 @@ __device__ __forceinline__ void fit_seg(const FitArgs& a, const int64_t* __restr
   uint32_t sp = slab + lane * 8;
   int32_t jrem = TILE_WORDS - 1 - j0;   // best-node key: low KEY_BITS bits = TILE_WORDS-1-j (earlier node wins a tie)
 #pragma unroll 1
-  for (int jb = j0; jb < j0 + SEG_WORDS; jb += 4) {
+  for (int jb = j0; jb < j0 + SEGW; jb += 4) {
 #pragma unroll
     for (int jj = 0; jj < 4; ++jj) {
       int64_t lfw[LW > 0 ? LW : 1];
@@ -226,7 +227,7 @@ __device__ __forceinline__ void fit_seg(const FitArgs& a, const int64_t* __restr
           // (scores of fitting pairs are < 2^27), -1 = none; decoded once per tile
           const int32_t key = (int32_t)(m32 << KEY_BITS) + (jrem - jj);
           if (fit) kb[r] = max(kb[r], key);
-#ifdef BS_FIT_STG     // (experiment: scores straight to HBM with 8-byte streaming stores, no staging / TMA)
+#ifdef BS_FIT_STG     // (-DBS_FIT_STG: scores straight to HBM with 8-byte streaming stores, no staging / TMA)
           if (SCORE && (uint32_t)(node + jj * 32) < a.N)
             __stcs(reinterpret_cast<unsigned long long*>(a.score) + (size_t)(stg_row0 + r) * a.score_pitch + (node + jj * 32),
                    (unsigned long long)(fit ? m32 : 0u) | ((unsigned long long)(fit ? 0u : 0x80000000u) << 32));
@@ -275,7 +276,7 @@ __host__ __device__ constexpr size_t fit_smem_front(int LW, int LN, int LS, int 
 __host__ __device__ constexpr size_t fit_smem_total(int LW, int LN, int LS, bool score, int stages) {
   return fit_smem_front(LW, LN, LS, stages) + (score ? (size_t)FIT_WARPS * FIT_NB * fit_slab_bytes() : 0);
 }
-// input ring depth: FIT_STAGES where the CTA's shared memory allows it (227 KB per CTA on sm_100a), else 2
+// input ring depth: FIT_STAGES where the CTA's shared memory allows it (227 KB per CTA on sm_90a), else 2
 constexpr size_t FIT_SMEM_MAX = 227 * 1024;
 __host__ __device__ constexpr int fit_stages(int LW, int LN, int LS, bool score) {
   return fit_smem_total(LW, LN, LS, score, FIT_STAGES) <= FIT_SMEM_MAX ? FIT_STAGES : 2;
@@ -425,21 +426,24 @@ __global__ void __launch_bounds__(FIT_THREADS, OUT == FIT_OUT_SCORE ? BS_FIT_MIN
     const int32_t* tln = reinterpret_cast<const int32_t*>(s_tile + stage * STAGE_BYTES + (size_t)LW * NODE_TILE * 8);
     const uint32_t node_base = tile * NODE_TILE;
     const uint32_t wbase = (tile % TILES_PER_LINE) * TILE_WORDS;
-    // the tile in store segments of FIT_SEG nodes: each goes to the next of the warp's FIT_NB staging slabs and
-    // leaves as PODS_PER_WARP bulk stores (one per matrix row) while the following segment is computed
-#pragma unroll 1
-    for (int sg = 0; sg < NODE_TILE / FIT_SEG; ++sg) {
-      const uint32_t slab = slab0 + sb * (uint32_t)fit_slab_bytes();
 #ifdef BS_FIT_STG
-      constexpr bool STAGE = false;
+    constexpr bool STAGE = false;
 #else
-      constexpr bool STAGE = SCORE;
+    constexpr bool STAGE = SCORE;
 #endif
+    // staged scores: the tile in store segments of FIT_SEG nodes, each goes to the next of the warp's FIT_NB staging
+    // slabs and leaves as PODS_PER_WARP bulk stores (one per matrix row) while the following segment is computed;
+    // nothing to stage: the tile in one piece
+    constexpr int SEG_NODES = STAGE ? FIT_SEG : NODE_TILE;
+#pragma unroll 1
+    for (int sg = 0; sg < NODE_TILE / SEG_NODES; ++sg) {
+      const uint32_t slab = slab0 + sb * (uint32_t)fit_slab_bytes();
       if (STAGE && nseg >= (uint32_t)FIT_NB) {
         if (lane == 0) bulk_wait_read<FIT_NB - 1>();   // the bulk stores that last read this slab are done with it
         __syncwarp();
       }
-      fit_seg<LW, LN, LS, OUT>(a, tlw, tln, rqw, rqn, colbits, slab, s_words, wbase, node_base, lane, sg * SEG_WORDS, best_s, best_n, kb, cnt, wpod0);
+      fit_seg<LW, LN, LS, OUT, SEG_NODES / 32>(a, tlw, tln, rqw, rqn, colbits, slab, s_words, wbase, node_base, lane,
+                                               sg * (SEG_NODES / 32), best_s, best_n, kb, cnt, wpod0);
       if (STAGE) {
         fence_async_smem();
         __syncwarp();
@@ -483,7 +487,7 @@ __global__ void __launch_bounds__(FIT_THREADS, OUT == FIT_OUT_SCORE ? BS_FIT_MIN
     if (lane == 0) mbar_arrive(&s_empty[stage]);   // this warp no longer reads the stage
     // Fit bitmap: the ballot words of TILES_PER_LINE tiles make one 128-byte line per pod (the bitmap's row
     // pitch is a multiple of 32 words), written with one fully coalesced store — 4-byte pieces of unaligned rows
-    // cost 0.15 ms on the bench workload (partial sectors), a full aligned line costs nothing measurable.
+    // would write partial sectors.
     if (WORDS && ((tile + 1) % TILES_PER_LINE == 0 || tile + 1 == tile_hi)) {
       const uint32_t line = tile / TILES_PER_LINE;
       const uint32_t valid = (tile % TILES_PER_LINE + 1) * TILE_WORDS;   // words assembled in this line

@@ -1,4 +1,4 @@
-// kernels.cuh — sm_100a kernels of the gang-scheduling feasibility engine.
+// kernels.cuh — sm_90a kernels of the gang-scheduling feasibility engine.
 //
 // Every kernel cites the reference lines it restates (tenstack/batch-scheduler,
 // pkg/scheduler/core/core.go).  All arithmetic is int64 / uint32 / one float32

@@ -19,14 +19,16 @@ through NCCL is timed beside it at N > 1).
   roofline      gang_fit kernel, algorithmic bytes / its CUDA-event time vs measured HBM peak
   cpu_baseline  the CPU oracle (port of the reference algorithm) on the host cores, bounded sample
 
-Timing: W warm-up steps, then a barrier + synchronize, then the timed steps with one CUDA event
-per step on the engine's stream, then the exchange stream joined, a final event, barrier +
-synchronize.  The timed region runs --steps K steps or --min-time seconds of device time, whichever
-is MORE (a 30 ms region cannot be timed across 8 ranks); `steps` in the line is what ran,
-`steps_requested` what was asked.  MAX over ranks.  Clocks are sampled through NVML inside the
-process (no nvidia-smi subprocess between the barrier and the first step).
+Timing: W warm-up steps, then a barrier + synchronize, then exactly K = --steps timed steps with
+one CUDA event per step on the engine's stream, then the exchange stream joined, a final event,
+barrier + synchronize.  MAX over ranks.  Clocks are sampled through NVML inside the process (no
+nvidia-smi subprocess between the barrier and the first step).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+--dump-outputs DIR writes what the headline path returned in its last timed step to DIR/<name>.npy
+(float64, exact for these integer values): every decision vector, and the fit bitmap and score
+matrix rows of a fixed, seeded sample of pods.  The synthetic inputs depend on the arguments only.
+
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 """
 from __future__ import annotations
 
@@ -57,10 +59,10 @@ def load_peaks():
         try:
             with open(p) as f:
                 d = json.load(f)
-            return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)", float(d.get("sm_max_mhz", 1965.0))
+            return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)", float(d.get("sm_max_mhz", 1980.0))
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)", 1965.0
+    return 3350.0, "data sheet (H100 SXM HBM3 3.35 TB/s), not measured", 1980.0
 
 
 def usable_threads() -> int:
@@ -85,8 +87,8 @@ def usable_threads() -> int:
 
 
 class ClockSampler:
-    """SM clock + throttle reasons of one GPU, sampled in-process through NVML every 50 ms (a thread: about 20 samples
-    inside the >= 1 s timed region; NVML queries take driver locks, so no more often than that);
+    """SM clock + throttle reasons of one GPU, sampled in-process through NVML every 50 ms (a thread: 20 samples per
+    second of timed region; NVML queries take driver locks, so no more often than that);
     `window(t0, t1)` summarises the samples taken inside a perf_counter interval.  Falls back to one
     nvidia-smi -lms subprocess (started long before the timed region) when NVML is unavailable."""
 
@@ -197,6 +199,12 @@ class ClockSampler:
                 "reasons": sorted(v for k, v in self.REASONS.items() if mask & k),
                 "power_w_max": max(pw) if pw else None, "source": self.src}
 
+    def power_limit_w(self):
+        try:
+            return self.nv.nvmlDeviceGetEnforcedPowerLimit(self.h) / 1000.0 if self.nv is not None else None
+        except Exception:
+            return None
+
     def stop(self):
         self.stop_flag = True
         if self.proc is not None:
@@ -234,7 +242,7 @@ def workload_config(scale: float):
                         "(BASELINE.json configs[3] snapshot per GPU)",
             "pods_per_gpu": P, "nodes": N, "groups_per_gpu": G, "lanes": 5,
             "outputs": "score matrix int64 PxN + fit bitmap + decisions",
-            "l2": "each step streams an %.1f GB score matrix (>> 126 MB L2): working set larger than L2, "
+            "l2": "each step streams an %.1f GB score matrix (>> 50 MB L2): working set larger than L2, "
                   "no explicit flush" % (8.0 * P * N / 1e9),
             "scale": scale}
 
@@ -339,27 +347,15 @@ class Harness:
         self.dist.all_reduce(t, op=self.dist.ReduceOp.SUM)
         return float(t.item())
 
-    def timed(self, eng, step, steps_req, warmup, min_time_s, join=None, sampler=None):
-        """W warm-up steps; barrier; K timed steps (K = max(steps_req, what min_time_s needs), the same on
-        every rank) with an event per step on the engine stream; `join` (exchange stream) before the last
-        event; barrier.  Returns total ms (max over ranks), steps, per-step ms of this rank, clock window."""
+    def timed(self, eng, step, steps, warmup, join=None, sampler=None):
+        """W warm-up steps; barrier; exactly `steps` timed steps with an event per step on the engine stream;
+        `join` (exchange stream) before the last event; barrier.  Returns total ms (max over ranks), steps,
+        per-step ms of this rank, clock window."""
         torch = self.torch
         ext = torch.cuda.ExternalStream(eng.stream(), device=self.local_rank)
         for _ in range(warmup):
             step()
         self.full_sync(eng)
-        # pilot: how long is a step?  (same count on every rank: max over ranks)
-        p0, p1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        p0.record(ext)
-        for _ in range(3):
-            step()
-        if join:
-            join()
-        p1.record(ext)
-        self.full_sync(eng)
-        est_ms = self.max_over_ranks(p0.elapsed_time(p1) / 3.0)
-        steps = int(max(steps_req, math.ceil(min_time_s * 1e3 / max(est_ms, 1e-3))))
-        steps = int(self.max_over_ranks(steps))
         evs = [torch.cuda.Event(enable_timing=True) for _ in range(steps + 1)]
         end = torch.cuda.Event(enable_timing=True)
         self.full_sync(eng)                      # barrier + synchronize; nothing but the loop follows
@@ -389,6 +385,29 @@ class Harness:
 def step_stats(per):
     return {"p50_ms": float(np.percentile(per, 50)), "p99_ms": float(np.percentile(per, 99)),
             "max_ms": float(per.max()), "mean_ms": float(per.mean())}
+
+
+DUMP_BYTES = 48 << 20     # --dump-outputs stays below 64 MB in all
+
+
+def dump_outputs(out_dir, eng):
+    """What a caller of the timed path receives after its last step, as float64 .npy files (every value is INT64_MIN
+    or an integer below 2^53 in magnitude, so the conversion is exact): the decision vectors whole, and the fit
+    bitmap / score matrix rows of pods drawn with a fixed seed (the whole P x N matrices are gigabytes)."""
+    os.makedirs(out_dir, exist_ok=True)
+    res = eng.fetch()
+    arrays = {f: getattr(res, f) for f in ("prefilter", "feasible_count", "best_node", "best_score", "admit", "admit_bitmap",
+                                           "new_denied", "order", "rank")}
+    arrays["max_group"], arrays["max_finished"] = np.array([res.max_group]), np.array([res.max_finished])
+    left = DUMP_BYTES - sum(a.size * 8 for a in arrays.values())
+    W = (eng.N + 31) // 32
+    n_rows = int(min(eng.P, 256, max(1, left // (8 * (eng.N + W + 1)))))
+    rows = np.sort(np.random.default_rng(0).choice(eng.P, n_rows, replace=False))
+    arrays["sample_pods"] = rows
+    arrays["fit_bitmap_rows"] = np.concatenate([eng.fit_rows(int(p), 1) for p in rows])
+    arrays["score_rows"] = np.concatenate([eng.score_rows(int(p), 1) for p in rows])
+    for k, a in arrays.items():
+        np.save(os.path.join(out_dir, k + ".npy"), np.asarray(a, dtype=np.float64))
 
 
 def make_nccl_exchange(H, eng, capi):
@@ -421,7 +440,7 @@ def peer_setup(H, eng, words):
     H.dist.barrier()
 
 
-def strong_leg(H, pkg, cfg, scale, steps_req, warmup, min_time_s, score=True):
+def strong_leg(H, pkg, cfg, scale, steps_req, warmup, score=True):
     """ONE snapshot (BASELINE configs[cfg-1]) group-sharded over the ranks: first-pod capture resolved
     globally, contiguous group ranges balanced by pod count, node and group tables replicated, admit
     bitmap all-gathered every step by the engine's peer-memory exchange."""
@@ -432,13 +451,13 @@ def strong_leg(H, pkg, cfg, scale, steps_req, warmup, min_time_s, score=True):
     eng = pkg.Engine(L, H.local_rank, fit_bitmap=True, score=score)
     eng.upload(local)
     peer_setup(H, eng, (G + 31) // 32)
-    total_ms, steps, per, _ = H.timed(eng, eng.evaluate_async, steps_req, warmup, min_time_s, join=eng.peer_join)
+    total_ms, steps, per, _ = H.timed(eng, eng.evaluate_async, steps_req, warmup, join=eng.peer_join)
     pairs = H.sum_over_ranks(float(P) * N)
     # the same shard with no exchange and no peers: what the rank's own work takes
     H.dist.barrier()
     eng.peer_detach()
     H.dist.barrier()
-    solo_ms, solo_steps, _, _ = H.timed(eng, eng.evaluate_async, max(5, min(steps_req, 20)), 2, 0.2)
+    solo_ms, solo_steps, _, _ = H.timed(eng, eng.evaluate_async, max(5, min(steps_req, 20)), 2)
     eng.close()
     ranks = H.gather_objects({"rank": H.rank, "pods": int(P), **step_stats(per)})
     out = {"config": {"workload": full.name, "pods": int(full.pods.n), "nodes": int(N), "groups": int(G), "lanes": int(L),
@@ -491,10 +510,10 @@ def strong_parity(H, pkg, cfg, scale):
                     "max_group == oracle's unsharded round"}
 
 
-def sass_issue_roofline(pairs, ms, clock_mhz):
+def sass_issue_roofline(pairs, ms, clock_mhz, sms):
     """Decisions-only regime (SURVEY 8(d) R2): instruction-issue roofline.  Ops per (pod,node) pair are
     counted from the committed SASS of the decisions-only kernel (profiles/sass_ops_r2.json, written by
-    profiles/tools/sass_count.py): peak = 148 SMs x 4 schedulers x 32 lanes x clock / issued ops per pair;
+    profiles/tools/sass_count.py): peak = SMs x 4 schedulers x 32 lanes x clock / issued ops per pair;
     the ALU-pipe bound uses the 64 lanes/clk/SM of the integer ALU pipe and the ALU ops per pair."""
     p = os.path.join(ROOT, "profiles", "sass_ops_r2.json")
     if not os.path.exists(p):
@@ -505,8 +524,8 @@ def sass_issue_roofline(pairs, ms, clock_mhz):
     except Exception:
         return None
     clk = clock_mhz * 1e6
-    peak_issue = 148 * 128 * clk / issue
-    peak_alu = 148 * 64 * clk / alu
+    peak_issue = sms * 128 * clk / issue
+    peak_alu = sms * 64 * clk / alu
     achieved = pairs / (ms * 1e-3)
     return {"bound": "int-issue", "achieved": achieved, "peak": peak_issue, "unit": UNIT, "frac": achieved / peak_issue,
             "issue_ops_per_pair": issue, "alu_pipe_ops_per_pair": alu, "alu_pipe_peak": peak_alu,
@@ -521,8 +540,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=None)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--scale", type=float, default=1.0, help="shrink the workload (debug only; marks the line)")
-    ap.add_argument("--min-time", type=float, default=1.0,
-                    help="the timed region lasts at least this many seconds of device time (more steps than --steps if needed)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the headline path's outputs of its last timed step to DIR/<name>.npy")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-replay", action="store_true", help="skip the multi-round admission leg")
     ap.add_argument("--no-strong", action="store_true", help="N>1: skip the strong-scaling legs")
@@ -589,18 +608,20 @@ def main():
         def step_nccl():
             eng.evaluate_async()
             exch_nccl()
-        tot, st, per, clk = H.timed(eng, step_nccl, steps_req, warmup, args.min_time, sampler=sampler)
+        tot, st, per, clk = H.timed(eng, step_nccl, steps_req, warmup, sampler=sampler)
         legs["nccl"] = {"ms_total": tot, "steps": st, "per": per, "clocks": clk}
     if use_p2p:
         peer_setup(H, eng, (G + 31) // 32)
     if world == 1 or use_p2p:
         launches0 = eng.launch_count()
-        tot, st, per, clk = H.timed(eng, eng.evaluate_async, steps_req, warmup, args.min_time,
+        tot, st, per, clk = H.timed(eng, eng.evaluate_async, steps_req, warmup,
                                     join=eng.peer_join if use_p2p else None, sampler=sampler)
         legs["p2p" if use_p2p else "single"] = {"ms_total": tot, "steps": st, "per": per, "clocks": clk}
-        launches_per_step = (eng.launch_count() - launches0) / float(st + warmup + 3)
+        launches_per_step = (eng.launch_count() - launches0) / float(st + warmup)
     else:
         launches_per_step = None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, eng)
     head_key = "p2p" if use_p2p else ("single" if world == 1 else "nccl")
     head = legs[head_key]
     total_pairs = H.sum_over_ranks(float(P) * N)
@@ -636,22 +657,13 @@ def main():
     narrow = (shape["LN"] + shape["LS"]) if shape else 0
     alg = gang_fit_alg_bytes(P, N, G, L, 64, narrow)
     achieved = alg / (fit_ms * 1e-3) / 1e9 if fit_ms > 0 else 0.0
-    traffic, traffic_src = None, None
-    tp = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if os.path.exists(tp):
-        try:
-            tj = json.load(open(tp))
-            traffic = tj.get(f"cfg{WORKLOAD_CFG}_gang_fit_dram_bytes")
-            traffic_src = "static: profiles/ncu_traffic.json (" + str(tj.get("source")) + "), not measured in this run"
-        except Exception:
-            traffic = None
 
     # ---- decisions-only regime (SURVEY 8(d) R2): same round, no P x N matrix leaves the SMs ------
     fused = None
     if world == 1:
         eng2 = pkg.Engine(L, local_rank, fit_bitmap=False, score=False)
         eng2.upload(snap)
-        ftot, fst, fper, fclk = H.timed(eng2, eng2.evaluate_async, max(10, min(steps_req, 50)), 3, min(args.min_time, 0.3),
+        ftot, fst, fper, fclk = H.timed(eng2, eng2.evaluate_async, max(10, min(steps_req, 50)), 3,
                                         sampler=sampler)
         eng2.set_profiling(True)
         fk = []
@@ -665,7 +677,8 @@ def main():
                  "gang_fit_ms": float(np.mean(fk)),
                  "what": "same round with out_flags=0: prefilter/admit/order/feasible-count/best-node only; "
                          "the tables are L2-resident, so the bound is instruction issue, not HBM",
-                 "roofline": sass_issue_roofline(float(P) * N, float(np.mean(fk)), clk_mhz)}
+                 "roofline": sass_issue_roofline(float(P) * N, float(np.mean(fk)), clk_mhz,
+                                                 torch.cuda.get_device_properties(local_rank).multi_processor_count)}
         eng2.close()
 
     # ---- multi-round admission (SURVEY 8(f) row 4): the whole queue through bs_replay, once ----
@@ -778,13 +791,13 @@ def main():
     strong = None
     if world > 1 and not args.no_strong:
         strong = {}
-        s4 = strong_leg(H, pkg, 4, args.scale, steps_req, 3, min(args.min_time, 0.5))
+        s4 = strong_leg(H, pkg, 4, args.scale, steps_req, 3)
         strong["cfg4"] = s4
         # cfg5: 1M pods x 50k nodes; a rank's int64 score shard is (1M / world) x 50k x 8 B
         shard_gb = 1e6 * args.scale / world * 50000 * args.scale * 8 / 1e9
         free_gb = torch.cuda.mem_get_info()[0] / 1e9
         with_score = shard_gb < 0.85 * free_gb
-        s5 = strong_leg(H, pkg, 5, args.scale, max(5, min(steps_req, 20)), 2, min(args.min_time, 0.5), score=with_score)
+        s5 = strong_leg(H, pkg, 5, args.scale, max(5, min(steps_req, 20)), 2, score=with_score)
         if not with_score:
             s5["note"] = f"score shard {shard_gb:.0f} GB does not fit {free_gb:.0f} GB free: fit bitmap + decisions only"
         strong["cfg5"] = s5
@@ -816,7 +829,7 @@ def main():
             "sharding": ("groups/pods per rank, node table replicated, admit bitmap all-gathered every step by "
                          + ("the engine's peer-memory kernels over NVLink (CUDA IPC): a push kernel closes the round, the wait "
                             "runs on a side stream one round deep" if use_p2p else "one NCCL all-gather")) if world > 1 else "single GPU",
-            "timing": {"min_time_s": args.min_time, "per_rank": per_rank,
+            "timing": {"per_rank": per_rank,
                        "what": "CUDA events on the engine stream, one per step; barrier + synchronize on both sides; max over ranks"},
             "exchange": exchange_lines,
             "admit_decisions_per_s": admit_rate,
@@ -834,12 +847,13 @@ def main():
             "replay": replay,
             "strong": strong,
             "roofline": {"bound": "hbm", "kernel": "gang_fit_kernel" + (str(shape) if shape else ""), "achieved": achieved,
-                         "peak": peak, "unit": "GB/s", "frac": achieved / peak if peak else None, "traffic": traffic,
-                         "traffic_source": traffic_src, "peak_source": peak_src, "alg_bytes_per_launch": int(alg),
+                         "peak": peak, "unit": "GB/s", "frac": achieved / peak if peak else None,
+                         "peak_source": peak_src, "alg_bytes_per_launch": int(alg),
                          "kernel_ms": fit_ms},
             "cpu_baseline": cpu,
             "cpu_baseline_1thread": cpu1,
             "clocks": head["clocks"],
+            "gpu": {"name": torch.cuda.get_device_name(local_rank), "power_limit_w": sampler.power_limit_w()},
         }
         print(json.dumps(line), flush=True)
     if world > 1:

@@ -1,5 +1,5 @@
 /*
- * bsched.h — C ABI of the B200 gang-scheduling feasibility engine.
+ * bsched.h — C ABI of the H100 gang-scheduling feasibility engine.
  *
  * This is the drop-in boundary for the PreFilter / Permit / Less hot path of
  * tenstack/batch-scheduler.  Every entry point names the reference interface it

@@ -1,4 +1,4 @@
-// store_pattern.cu — what bounds a write-only P x N int64 matrix kernel on B200?
+// store_pattern.cu — what bounds a write-only P x N int64 matrix kernel on H100?
 // Every variant writes the same 100000 x 10000 x 8 B = 8.0 GB with 8-byte streaming stores:
 //   fill      : flat grid-stride fill (cudaMemset-like reference)
 //   rows32    : the gang_fit pattern — CTA owns 32 rows, 8 warps x 4 rows, sweeps 512-node tiles,
@@ -6,7 +6,7 @@
 //   rows32_po : same ownership, pods-outer: a warp finishes a row's 4 KB tile segment before the next row
 //   cta_row   : CTA owns 32 rows but all 8 warps cooperate on ONE row at a time (2 KB per step)
 //   rows8     : CTA owns 8 rows (1 per warp), 4x more CTAs
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o store_pattern store_pattern.cu
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o store_pattern store_pattern.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -63,7 +63,7 @@ int main() {
   long long* d;
   cudaMalloc(&d, n * 8);
   auto rep = [&](const char* name, float ms) { printf("%-10s %.3f ms  %.0f GB/s\n", name, ms, n * 8 / ms / 1e6); };
-  rep("fill", timeit([&] { fill<<<148 * 8, 256>>>(d, n); }));
+  rep("fill", timeit([&] { fill<<<132 * 8, 256>>>(d, n); }));
   rep("rows32", timeit([&] { rows<4, false><<<(P + 31) / 32, 256>>>(d, P, N); }));
   rep("rows32_po", timeit([&] { rows<4, true><<<(P + 31) / 32, 256>>>(d, P, N); }));
   rep("cta_row", timeit([&] { cta_row<<<(P + 31) / 32, 256>>>(d, P, N); }));

@@ -1,5 +1,5 @@
 // store_pattern2.cu — round 2: which OUTPUT PATH lets a P x N int64 matrix kernel approach the HBM
-// write ceiling on B200?  Every variant writes the same 100000 x 10000 x 8 B = 8.0 GB.
+// write ceiling on H100?  Every variant writes the same 100000 x 10000 x 8 B = 8.0 GB.
 //
 //   fill          flat grid-stride 8-byte streaming stores (reference)
 //   rows<R>       round-1 gang_fit pattern: warp owns R rows, 512-node tiles, st.global.cs 8 B per lane
@@ -10,7 +10,7 @@
 //   tmacta<R,T,NB> CTA-level variant: the 8 warps fill a CTA slab (32 rows x T) and one thread issues
 //                 all 32 bulk stores (larger bursts per issue, one bar.sync per tile)
 //
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o store_pattern2 store_pattern2.cu
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o store_pattern2 store_pattern2.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -180,7 +180,7 @@ void run_tmacta(const char* name) {
 int main() {
   const size_t n = (size_t)P * N;
   cudaMalloc(&d, n * 8 + (1 << 20));
-  rep("fill", timeit([&] { fill<<<148 * 8, 256>>>(d, n); }));
+  rep("fill", timeit([&] { fill<<<132 * 8, 256>>>(d, n); }));
   rep("memset", timeit([&] { cudaMemsetAsync(d, 1, n * 8); }));
   rep("rows<4> (round-1 pattern)", timeit([&] { rows<4><<<(P + 31) / 32, 256>>>(d, P, N); }));
   rep("rows<1> 8 rows/CTA", timeit([&] { rows<1><<<(P + 7) / 8, 256>>>(d, P, N); }));

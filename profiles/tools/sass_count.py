@@ -3,10 +3,10 @@
 instructions: one trip = 4 nodes per lane x PODS_PER_WARP pods) and writes profiles/sass_ops_r2.json, the
 op counts behind the decisions-only instruction roofline in bench.py (SURVEY 8(d) R2).
 
-    python profiles/tools/sass_count.py [--lib batch-scheduler_b200/libbsched.so] [--kernel ILi0ELi3ELi2ELb0E]
+    python profiles/tools/sass_count.py [--lib batch-scheduler_b200/libbsched.so] [--kernel ILi0ELi3ELi2ELi0E]
                                         [--ppw 4] [--dump profiles/sass_gang_fit_r2.txt]
 
-Pipe classes (sm_100a, as ncu groups them): the integer ALU pipe takes add/logic/shift/compare/select/
+Pipe classes (sm_90a, as ncu groups them): the integer ALU pipe takes add/logic/shift/compare/select/
 min-max/vote-free predicate ops at 64 lanes/clk/SM (16 per scheduler); IMAD* go to the FMA pipe; LDS/STS/
 LDG/STG to the LSU; U* ops to the uniform datapath.  Every instruction costs one issue slot."""
 import argparse, json, os, re, subprocess, sys
@@ -39,7 +39,7 @@ def classify(mn):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--lib", default=os.path.join(ROOT, "batch-scheduler_b200", "libbsched.so"))
-    ap.add_argument("--kernel", default="ILi0ELi3ELi2ELb0E", help="substring of the mangled gang_fit_kernel instance")
+    ap.add_argument("--kernel", default="ILi0ELi3ELi2ELi0E", help="substring of the mangled gang_fit_kernel instance")
     ap.add_argument("--ppw", type=int, default=4)
     ap.add_argument("--marks-per-pair", type=int, default=4, help="VIADDMNMX per pair: (LN - 1) + LS, 4 for the bench shape (0,3,2)")
     ap.add_argument("--dump", default=None)
