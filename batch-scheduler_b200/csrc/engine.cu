@@ -268,8 +268,6 @@ struct bs_engine {
   DevBuf d_gk0, d_gk1, d_pk0, d_pk1, d_idx_a, d_idx_b, d_ghist, d_group_rank, d_tilecnt, d_sort_barrier;
   uint32_t sort_max_grid = 1;
   DevBuf d_sort_arena;            // the sort scratch buffers above are views into it
-  size_t sort_arena_bytes = 0;
-  size_t l2_persist_bytes = 0, l2_window_max = 0;   // persisting-L2 set-aside for the sort scratch (0 = off)
 
   // host copies for the per-call mirrors and class building
   std::vector<int32_t> h_gid, h_prio;
@@ -837,9 +835,9 @@ int ensure_round_buffers(bs_engine* e) {
     if (fresh) CK(cudaMemsetAsync(e->d_pre_done.p, 0, e->d_pre_done.cap, e->s));
     CK(e->d_max_partial.ensure((size_t)cdiv(G, FINDMAX_THREADS * FINDMAX_PER_THREAD) * sizeof(MaxState)));
   }
-  // sort scratch: ONE arena, so that one L2 access-policy window on the sort stream covers it.  The queue sort
-  // gathers its key words at random while gang_fit streams 8 GB of scores through the same L2: marked persisting,
-  // the sort's few megabytes stay resident instead of turning into DRAM reads in the middle of a write stream.
+  // sort scratch: one arena.  No persisting-L2 window over it: the set-aside such a window needs cost the score-mode
+  // gang_fit kernel 0.9 ms of 3.85 on an H100 (its 8 GB score stream through a smaller L2), and the sort was no
+  // faster with it.
   {
     const uint32_t M = std::max(P, G);
     struct F { DevBuf* d; size_t bytes; };
@@ -849,24 +847,11 @@ int ensure_round_buffers(bs_engine* e) {
                   {&e->d_sort_barrier, sizeof(unsigned int)}, {&e->d_group_rank, (size_t)G * 4}};
     size_t total = 0;
     for (auto& f : fields) total += (f.bytes + 255) & ~(size_t)255;
-    const void* old_base = e->d_sort_arena.p;
     CK(e->d_sort_arena.ensure(total));
     size_t off = 0;
     for (auto& f : fields) {
       f.d->alias(static_cast<char*>(e->d_sort_arena.p) + off, f.bytes);
       off += (f.bytes + 255) & ~(size_t)255;
-    }
-    if (e->d_sort_arena.p != old_base || total != e->sort_arena_bytes) {
-      e->sort_arena_bytes = total;
-      if (e->l2_persist_bytes) {
-        cudaStreamAttrValue v{};
-        v.accessPolicyWindow.base_ptr = e->d_sort_arena.p;
-        v.accessPolicyWindow.num_bytes = std::min(total, e->l2_window_max);
-        v.accessPolicyWindow.hitRatio = total <= e->l2_persist_bytes ? 1.0f : (float)((double)e->l2_persist_bytes / (double)total);
-        v.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-        v.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-        if (cudaStreamSetAttribute(e->s2, cudaStreamAttributeAccessPolicyWindow, &v) != cudaSuccess) cudaGetLastError();   // a hint only
-      }
     }
   }
   return BS_OK;
@@ -985,7 +970,7 @@ int evaluate_async_locked(bs_engine* e) {
         // way (32 registers: its CTAs share their SMs with the fit CTAs); when the fit kernel is the shorter of the two
         // (a small shard, few nodes) the round waits for the sort, and the build with 16 gathers in flight per thread
         // is the faster one.  Estimate: pairs x the per-pair time of the output mode measured on an H100.
-        const double est_fit_ms = (double)P * (double)e->N * ((e->out_flags & BS_OUT_SCORE) ? 3.8e-9 : 0.9e-9);
+        const double est_fit_ms = (double)P * (double)e->N * ((e->out_flags & BS_OUT_SCORE) ? 3.0e-9 : 0.9e-9);
         const bool lean = est_fit_ms > 0.6;
         const void* fn = lean ? (const void*)queue_sort_kernel<SORT_LEAN_GROUP> : (const void*)queue_sort_kernel<SORT_WIDE_GROUP>;
         CK(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(SORT_THREADS), params, 0, e->s2));
@@ -1271,21 +1256,6 @@ int bs_create(const bs_config* cfg, bs_engine** out) {
     // the sort shares the GPU with the fit kernel on the other stream: one CTA per SM is plenty
     per_sm = std::min(per_sm, per_sm_wide);
     e->sort_max_grid = (uint32_t)std::max(1, std::min(per_sm * sms, sms));
-    // persisting-L2 set-aside for the sort scratch (BS_SORT_L2_PERSIST_MB, default 16, 0 = off); a hint: failures are ignored
-    int max_persist = 0, max_window = 0;
-    size_t want_mb = 16;
-    if (const char* lp = getenv("BS_SORT_L2_PERSIST_MB")) want_mb = (size_t)std::max(0, atoi(lp));
-    if (want_mb && cudaDeviceGetAttribute(&max_persist, cudaDevAttrMaxPersistingL2CacheSize, cfg->device) == cudaSuccess &&
-        cudaDeviceGetAttribute(&max_window, cudaDevAttrMaxAccessPolicyWindowSize, cfg->device) == cudaSuccess &&
-        max_persist > 0 && max_window > 0) {
-      const size_t want = std::min<size_t>(want_mb << 20, (size_t)max_persist);
-      if (cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, want) == cudaSuccess) {
-        e->l2_persist_bytes = want;
-        e->l2_window_max = (size_t)max_window;
-      } else {
-        cudaGetLastError();
-      }
-    }
   }
   if (!ok) {
     bs_destroy(e);
