@@ -10,6 +10,7 @@
 #include <omp.h>
 
 #include <algorithm>
+#include <array>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -31,57 +32,93 @@ using namespace bsk;
 
 namespace {
 
-struct DevBuf {
+struct DeviceAlloc {
+  static cudaError_t alloc(void** p, size_t bytes) { return cudaMalloc(p, bytes); }
+  static void free(void* p) { cudaFree(p); }
+};
+struct PinnedAlloc {
+  static cudaError_t alloc(void** p, size_t bytes) { return cudaHostAlloc(p, bytes, cudaHostAllocDefault); }
+  static void free(void* p) { cudaFreeHost(p); }
+};
+
+// A block of device or pinned host memory that frees itself.  ensure() only grows it (at least 256 bytes)
+// and does not keep the contents when it does.
+template <class A>
+struct Buf {
   void* p = nullptr;
   size_t cap = 0;
-  bool owned = true;    // false: a view into an arena (alias), never freed here
-  void alias(void* ptr, size_t bytes) { p = ptr; cap = bytes; owned = false; }
+  Buf() = default;
+  Buf(Buf&& o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); }
+  Buf& operator=(Buf&& o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); return *this; }
+  ~Buf() { reset(); }
+  void reset() {
+    if (p) A::free(p);
+    p = nullptr;
+    cap = 0;
+  }
   cudaError_t ensure(size_t bytes) {
     if (bytes <= cap) return cudaSuccess;
-    if (p && owned) cudaFree(p);
-    owned = true;
-    p = nullptr;
-    cap = 0;
+    reset();
     const size_t want = std::max<size_t>(bytes, 256);
-    cudaError_t e = cudaMalloc(&p, want);
+    cudaError_t e = A::alloc(&p, want);
     if (e == cudaSuccess) cap = want;
+    else p = nullptr;
     return e;
   }
-  void release() {
-    if (p && owned) cudaFree(p);
-    p = nullptr;
-    cap = 0;
-    owned = true;
-  }
+  template <class T>
+  T* as() const { return reinterpret_cast<T*>(p); }
+};
+using DevBuf = Buf<DeviceAlloc>;
+using PinBuf = Buf<PinnedAlloc>;
+
+// A field of an arena (carve): it neither allocates nor frees.
+struct View {
+  void* p = nullptr;
+  size_t bytes = 0;
   template <class T>
   T* as() const { return reinterpret_cast<T*>(p); }
 };
 
-struct PinBuf {
-  void* p = nullptr;
-  size_t cap = 0;
-  bool owned = true;
-  void alias(void* ptr, size_t bytes) { p = ptr; cap = bytes; owned = false; }
-  cudaError_t ensure(size_t bytes) {
-    if (bytes <= cap) return cudaSuccess;
-    if (p && owned) cudaFreeHost(p);
-    owned = true;
-    p = nullptr;
-    cap = 0;
-    const size_t want = std::max<size_t>(bytes, 256);
-    cudaError_t e = cudaHostAlloc(&p, want, cudaHostAllocDefault);
-    if (e == cudaSuccess) cap = want;
-    return e;
-  }
-  void release() {
-    if (p && owned) cudaFreeHost(p);
-    p = nullptr;
-    cap = 0;
-    owned = true;
-  }
-  template <class T>
-  T* as() const { return reinterpret_cast<T*>(p); }
+struct Field {
+  View* v;
+  size_t bytes;
+  View* mirror = nullptr;   // the same field in the mirror arena
 };
+
+// Lays the fields out back to back in `arena`, each at a 256-byte aligned offset, and points every view
+// at its field.  With a `mirror`, the same layout is carved into it for the mirror views.  An arena that
+// has to grow loses its contents.  *used gets the bytes the layout takes.
+template <size_t K>
+cudaError_t carve(DevBuf& arena, const Field (&fields)[K], PinBuf* mirror = nullptr, size_t* used = nullptr) {
+  size_t total = 0;
+  for (const Field& f : fields) total += (f.bytes + 255) & ~(size_t)255;
+  cudaError_t er = arena.ensure(total);
+  if (er == cudaSuccess && mirror) er = mirror->ensure(total);
+  if (er != cudaSuccess) return er;
+  size_t off = 0;
+  for (const Field& f : fields) {
+    *f.v = View{arena.as<char>() + off, f.bytes};
+    if (mirror) *f.mirror = View{mirror->as<char>() + off, f.bytes};
+    off += (f.bytes + 255) & ~(size_t)255;
+  }
+  if (used) *used = total;
+  return cudaSuccess;
+}
+
+// A CUDA stream or event that is destroyed with its owner; it converts to the handle the runtime takes.
+template <class H, cudaError_t (*destroy)(H)>
+struct Handle {
+  H h = nullptr;
+  Handle() = default;
+  Handle(const Handle&) = delete;
+  Handle& operator=(const Handle&) = delete;
+  ~Handle() {
+    if (h) destroy(h);
+  }
+  operator H() const { return h; }
+};
+using Stream = Handle<cudaStream_t, cudaStreamDestroy>;
+using Event = Handle<cudaEvent_t, cudaEventDestroy>;
 
 // a resizable array in pinned host memory: what is DMA'd every round must not be staged through
 // pageable memory
@@ -97,7 +134,6 @@ struct PinVec {
   T* data() const { return buf.as<T>(); }
   T& operator[](size_t i) const { return buf.as<T>()[i]; }
   size_t size() const { return n; }
-  void release() { buf.release(); n = 0; }
 };
 
 // (sel, tol, non-zero scalar request mask): the pre-encoded predicates a pod class shares
@@ -211,8 +247,8 @@ struct bs_engine {
   std::mutex mu;
   int device = 0;
   uint32_t L = 0, out_flags = 0;
-  cudaStream_t s = nullptr, s2 = nullptr, s3 = nullptr, s4 = nullptr;   // main; queue sort; PreFilter chain (high priority); peer wait
-  cudaEvent_t ev_fork = nullptr, ev_join = nullptr, ev_pre = nullptr, ev_push = nullptr, ev_gath = nullptr;
+  Stream s, s2, s3, s4;   // main; queue sort; PreFilter chain (high priority); peer wait
+  Event ev_fork, ev_join, ev_pre, ev_push, ev_gath;
   std::string err;
   uint64_t launches = 0;
 
@@ -223,7 +259,7 @@ struct bs_engine {
 
   // node table (device, padded to Npad) + derived
   DevBuf d_alloc, d_requested, d_pod_count, d_apres, d_rpres, d_label, d_taint, d_nflags;
-  DevBuf d_left_w, d_left_n, d_left_present, d_classfit, d_left_plain, d_filter_bitmap, d_filter_code;
+  DevBuf d_left_w, d_left_n, d_left_present, d_classfit, d_left_plain, d_filter_bitmap;
   LaneMap lane_map{};
   bool lane_map_valid = false;
   // per-lane maxima of |value| (lane classification wide / narrow)
@@ -257,17 +293,17 @@ struct bs_engine {
   uint32_t n_fit_classes = 0, n_rep_classes = 0;
   // effective group state + round scratch
   DevBuf d_eflags, d_emin_res, d_emrpres, d_erep_class, d_first_pod, d_in_round, d_contrib, d_done, d_okA;
-  DevBuf d_state, d_pre, d_pre_present, d_pre_stats, d_max_partial, d_pre_part, d_pre_part_pres, d_pre_cstats, d_pre_done;
+  DevBuf d_pre, d_pre_present, d_pre_stats, d_max_partial, d_pre_part, d_pre_part_pres, d_pre_cstats;
+  DevBuf d_pre_done;   // kept between rounds: zeroed only when it is allocated
   uint32_t prefix_slots = 0;
   // outputs
-  DevBuf u_buf[9];        // bs_update_nodes / bs_update_groups: device scratch of the changed rows
+  DevBuf d_stage;         // bs_update_nodes / bs_update_groups: device staging of the changed rows
   DevBuf d_best_packed;   // gang_fit tail pieces: max((score + 1) << 32 | ~node) per pod
-  DevBuf d_prefilter, d_feasible, d_best_node, d_best_score, d_admit, d_admit_bitmap, d_new_denied,
-      d_fit_bitmap, d_score, d_order, d_rank;
-  // sort scratch
-  DevBuf d_gk0, d_gk1, d_pk0, d_pk1, d_idx_a, d_idx_b, d_ghist, d_group_rank, d_tilecnt, d_sort_barrier;
+  DevBuf d_fit_bitmap, d_score;
+  // sort scratch: views into one arena
+  View d_gk0, d_gk1, d_pk0, d_pk1, d_idx_a, d_idx_b, d_ghist, d_group_rank, d_tilecnt, d_sort_barrier;
   uint32_t sort_max_grid = 1;
-  DevBuf d_sort_arena;            // the sort scratch buffers above are views into it
+  DevBuf d_sort_arena;
 
   // host copies for the per-call mirrors and class building
   std::vector<int32_t> h_gid, h_prio;
@@ -278,7 +314,7 @@ struct bs_engine {
   // (sel, tol) of pods and carried-in group representatives
   ClassIndex fit_index, rep_index;
   PinVec<uint32_t> h_pfc, h_prc, h_grc;   // pinned: DMA'd whenever the classes change
-  cudaEvent_t ev_classes = nullptr;       // the last class-table DMA out of them
+  Event ev_classes;                       // the last class-table DMA out of them
   bool group_classes_dirty = true;   // every group's representative id has to be looked up again
   bool group_ids_dirty = false;      // some ids in h_grc changed in place (bs_update_groups): DMA them again
   std::vector<int64_t> h_wait_ns;
@@ -294,19 +330,19 @@ struct bs_engine {
   bool host_prof = false;
   std::vector<std::pair<const char*, double>> hp_log;
   std::chrono::steady_clock::time_point hp_t;
-  // pinned result cache
-  PinBuf h_prefilter, h_feasible, h_best_node, h_best_score, h_admit, h_admit_bitmap, h_new_denied,
-      h_order, h_rank, h_state, h_filter_code;
-  bool fetched = false;
   // decision arena: every per-round decision vector lives in ONE device block and ONE pinned block with the
-  // same layout (the d_* / h_* buffers above are views into them), so bs_fetch is a single D2H copy
+  // same layout (d_* views, and their h_* pinned mirrors), so bs_fetch is a single D2H copy
+  View d_state, d_prefilter, d_feasible, d_best_node, d_best_score, d_admit, d_admit_bitmap, d_new_denied, d_order,
+      d_rank, d_filter_code;
+  View h_state, h_prefilter, h_feasible, h_best_node, h_best_score, h_admit, h_admit_bitmap, h_new_denied, h_order,
+      h_rank, h_filter_code;
   DevBuf d_arena;
   PinBuf h_arena;
   size_t arena_bytes = 0;
+  bool fetched = false;
 
-  // bs_replay scratch (kept between calls: cudaMalloc/cudaFree per call would dominate small queues)
-  DevBuf r_req, r_pc, r_rp, r_matched, r_gflags, r_grc, r_minres, r_mrp, r_queue, r_pf, r_node, r_ready, r_status,
-      r_sum, r_max, r_keys, r_left0, r_left1, r_both, r_fit, r_stat;
+  // bs_replay scratch (kept between calls: an allocation per call would dominate small queues)
+  DevBuf d_replay;
 
   // peer exchange (admit bitmap all-gather over NVLink peer memory)
   DevBuf d_gather, d_peer_err;
@@ -318,7 +354,7 @@ struct bs_engine {
 
   // profiling
   bool profiling = false;
-  cudaEvent_t ev_a[BS_K_COUNT] = {}, ev_b[BS_K_COUNT] = {};
+  Event ev_a[BS_K_COUNT], ev_b[BS_K_COUNT];
   uint32_t k_launches[BS_K_COUNT] = {};
   bool k_valid[BS_K_COUNT] = {};
 };
@@ -340,48 +376,10 @@ int fail(bs_engine* e, int code, const char* msg) {
   return code;
 }
 
-// per-lane max |value| of a [L][n] table; false if any value is outside +-BS_VALUE_LIMIT
-bool lane_maxima(const int64_t* a, uint32_t L, size_t n, int64_t* out) {
-  bool ok = true;
-  for (uint32_t d = 0; d < L; ++d) {
-    const int64_t* row = a + (size_t)d * n;
-    int64_t lo = 0, hi = 0;
-#pragma omp parallel for reduction(min : lo) reduction(max : hi) if (n > 65536) num_threads(host_threads())
-    for (size_t i = 0; i < n; ++i) {
-      lo = std::min(lo, row[i]);
-      hi = std::max(hi, row[i]);
-    }
-    ok = ok && lo >= -BS_VALUE_LIMIT && hi <= BS_VALUE_LIMIT;
-    out[d] = std::max(hi, lo == INT64_MIN ? INT64_MAX : -lo);
-  }
-  return ok;
-}
-
-// Host restatement of singleNodeResource's per-lane residual at percent 1.0 (core.go:647-668) for the
-// lane statistics only: OR of the values (common power-of-two factor) and max |value| per lane.
-// (float)alloc is the RN convert, * 1.0f is exact, the cast back truncates — the device's scale_f32.
-void left_stats(const bs_node_table* t, uint32_t L, uint32_t n, uint64_t* or_out, int64_t* max_out) {
-  for (uint32_t d = 0; d < L; ++d) {
-    uint64_t o = 0;
-    int64_t mx = 0;
-    const int64_t* al = t->alloc + (size_t)d * n;
-    const int64_t* rq = t->requested + (size_t)d * n;
-    for (uint32_t i = 0; i < n; ++i) {
-      if (d >= 4 && !((t->alloc_present[i] & t->req_present[i]) >> d & 1u)) continue;   // key absent: sentinel
-      int64_t used = rq[i];
-      if (d == (uint32_t)LANE_PODS && used == 0) used = t->pod_count[i];
-      const int64_t v = (int64_t)((float)al[i] * 1.0f) - used;
-      o |= (uint64_t)v;
-      mx = std::max(mx, v < 0 ? -v : v);
-    }
-    or_out[d] |= o;
-    max_out[d] = std::max(max_out[d], mx);
-  }
-}
-
-// Everything bs_upload_nodes needs from the host columns in ONE chunked pass (an omp team for big tables):
-// |value| maxima of alloc / requested (range check + lane classification), max |pod_count| and the
-// residual statistics of left_stats.
+// Everything bs_upload_nodes / bs_update_nodes need from the host columns in ONE chunked pass (an omp team
+// for big tables): |value| maxima of alloc / requested (range check + lane classification), max |pod_count|,
+// and per lane the OR and max |value| of the residual at percent 1.0 (singleNodeResource, core.go:647-668;
+// the OR gives the common power-of-two factor).
 struct NodeHostStats {
   int64_t mx_a[BS_MAX_LANES] = {}, mx_r[BS_MAX_LANES] = {}, mx_l[BS_MAX_LANES] = {};
   uint64_t or_l[BS_MAX_LANES] = {};
@@ -405,8 +403,9 @@ NodeHostStats node_host_pass(const bs_node_table* t, uint32_t L, uint32_t N) {
         alo = std::min(alo, al[i]); ahi = std::max(ahi, al[i]);
         rlo = std::min(rlo, rq[i]); rhi = std::max(rhi, rq[i]);
       }
-      for (uint32_t i = a0; i < a1; ++i) {   // left_stats' body
-        if (d >= 4 && !((t->alloc_present[i] & t->req_present[i]) >> d & 1u)) continue;
+      // (float)alloc is the RN convert, * 1.0f is exact, the cast back truncates: the device's scale_f32
+      for (uint32_t i = a0; i < a1; ++i) {
+        if (d >= 4 && !((t->alloc_present[i] & t->req_present[i]) >> d & 1u)) continue;   // key absent: sentinel
         int64_t used = rq[i];
         if (d == (uint32_t)LANE_PODS && used == 0) used = t->pod_count[i];
         const int64_t v = (int64_t)((float)al[i] * 1.0f) - used;
@@ -446,21 +445,75 @@ LaneMap classify_lanes(const bs_engine* e);
 
 inline uint32_t cdiv(uint32_t a, uint32_t b) { return (a + b - 1) / b; }
 
-// upload a [L][n] lane-major host table into a [L][npad] device table
-int upload_lanes(bs_engine* e, DevBuf& dst, const int64_t* src, uint32_t L, uint32_t n, uint32_t npad) {
-  CK(dst.ensure((size_t)L * npad * 8));
-  if (npad != n) CK(cudaMemsetAsync(dst.p, 0, (size_t)L * npad * 8, e->s));
-  if (n)
-    CK(cudaMemcpy2DAsync(dst.p, (size_t)npad * 8, src, (size_t)n * 8, (size_t)n * 8, L,
-                         cudaMemcpyHostToDevice, e->s));
-  return BS_OK;
+// A table column: the caller's host column ([lanes][rows]) and the resident device column ([lanes][padded rows]).
+struct Col {
+  const void* host;
+  DevBuf* dev;
+  uint32_t elem, lanes;   // element bytes, lanes
+};
+template <class T>
+Col col(const T* host, DevBuf& dev, uint32_t lanes = 1) { return Col{host, &dev, (uint32_t)sizeof(T), lanes}; }
+
+// the columns bs_upload_nodes / bs_update_nodes move to the device
+std::array<Col, 8> node_cols(bs_engine* e, const bs_node_table* t) {
+  return {col(t->alloc, e->d_alloc, e->L), col(t->requested, e->d_requested, e->L), col(t->pod_count, e->d_pod_count),
+          col(t->alloc_present, e->d_apres), col(t->req_present, e->d_rpres), col(t->label_mask, e->d_label),
+          col(t->taint_mask, e->d_taint), col(t->flags, e->d_nflags)};
+}
+// the columns bs_upload_groups / bs_update_groups move to the device (the representative columns stay on the host)
+std::array<Col, 8> group_cols(bs_engine* e, const bs_group_table* t) {
+  return {col(t->min_member, e->d_min_member), col(t->scheduled, e->d_scheduled), col(t->matched, e->d_matched),
+          col(t->flags, e->d_gflags), col(t->min_res, e->d_min_res, e->L), col(t->min_res_present, e->d_mrpres),
+          col(t->creation_ns, e->d_creation), col(t->name_rank, e->d_name_rank)};
+}
+template <size_t K>
+bool null_column(const std::array<Col, K>& cols) {
+  return std::any_of(cols.begin(), cols.end(), [](const Col& c) { return !c.host; });
 }
 
+// upload a host column of n rows into its device column padded to npad rows (rows >= n zero)
+int upload_col(bs_engine* e, const Col& c, uint32_t n, uint32_t npad) {
+  const size_t row = (size_t)c.elem * n, prow = (size_t)c.elem * npad;
+  CK(c.dev->ensure(prow * c.lanes));
+  if (npad != n) CK(cudaMemsetAsync(c.dev->p, 0, prow * c.lanes, e->s));
+  if (n && c.lanes == 1) CK(cudaMemcpyAsync(c.dev->p, c.host, row, cudaMemcpyHostToDevice, e->s));
+  else if (n) CK(cudaMemcpy2DAsync(c.dev->p, prow, c.host, row, row, c.lanes, cudaMemcpyHostToDevice, e->s));
+  return BS_OK;
+}
+template <size_t K>
+int upload_cols(bs_engine* e, const std::array<Col, K>& cols, uint32_t n, uint32_t npad) {
+  int rc;
+  for (const Col& c : cols)
+    if ((rc = upload_col(e, c, n, npad))) return rc;
+  return BS_OK;
+}
 template <class T>
 int upload_vec(bs_engine* e, DevBuf& dst, const T* src, uint32_t n, uint32_t npad) {
-  CK(dst.ensure((size_t)npad * sizeof(T)));
-  if (npad != n) CK(cudaMemsetAsync(dst.p, 0, (size_t)npad * sizeof(T), e->s));
-  if (n) CK(cudaMemcpyAsync(dst.p, src, (size_t)n * sizeof(T), cudaMemcpyHostToDevice, e->s));
+  return upload_col(e, col(src, dst), n, npad);
+}
+
+// Stages the n changed rows of every column, and idx, in d_stage, and scatters row k of each column to row
+// idx[k] of its device column (pitch rows per lane).  The caller synchronises before its arrays are reused.
+template <size_t K>
+int scatter_rows(bs_engine* e, const std::array<Col, K>& cols, const uint32_t* idx, uint32_t n, uint32_t pitch) {
+  static_assert(K <= SCATTER_MAX_COLS, "one ScatterCols slot per column");
+  View stage[K + 1];
+  Field fields[K + 1];
+  for (size_t c = 0; c < K; ++c) fields[c] = Field{&stage[c], (size_t)cols[c].elem * cols[c].lanes * n};
+  fields[K] = Field{&stage[K], (size_t)n * 4};
+  CK(carve(e->d_stage, fields));
+  ScatterCols sc{};
+  sc.n_cols = K;
+  for (size_t c = 0; c < K; ++c) {
+    CK(cudaMemcpyAsync(stage[c].p, cols[c].host, stage[c].bytes, cudaMemcpyHostToDevice, e->s));
+    sc.dst[c] = static_cast<uint8_t*>(cols[c].dev->p);
+    sc.src[c] = static_cast<const uint8_t*>(stage[c].p);
+    sc.elem[c] = cols[c].elem;
+    sc.lanes[c] = cols[c].lanes;
+  }
+  CK(cudaMemcpyAsync(stage[K].p, idx, stage[K].bytes, cudaMemcpyHostToDevice, e->s));
+  row_scatter_kernel<<<cdiv(n, 256), 256, 0, e->s>>>(sc, pitch, static_cast<const uint32_t*>(stage[K].p), n);
+  e->launches++;
   return BS_OK;
 }
 
@@ -780,32 +833,19 @@ int ensure_round_buffers(bs_engine* e) {
   CK(e->d_contrib.ensure((size_t)G * 4));
   CK(e->d_done.ensure((size_t)G * 4));
   CK(e->d_okA.ensure(G));
-  {
-    // decision arena layout (256-byte aligned fields)
-    struct F { DevBuf* d; PinBuf* h; size_t bytes; };
-    F fields[] = {{&e->d_state, &e->h_state, sizeof(RoundState)},
-                  {&e->d_prefilter, &e->h_prefilter, P},
-                  {&e->d_feasible, &e->h_feasible, (size_t)P * 4},
-                  {&e->d_best_node, &e->h_best_node, (size_t)P * 4},
-                  {&e->d_best_score, &e->h_best_score, (size_t)P * 8},
-                  {&e->d_admit, &e->h_admit, G},
-                  {&e->d_admit_bitmap, &e->h_admit_bitmap, (size_t)cdiv(G, 32) * 4},
-                  {&e->d_new_denied, &e->h_new_denied, G},
-                  {&e->d_order, &e->h_order, (size_t)P * 4},
-                  {&e->d_rank, &e->h_rank, (size_t)P * 4},
-                  {&e->d_filter_code, &e->h_filter_code, (e->out_flags & BS_OUT_FILTER) ? (size_t)P : 0}};
-    size_t total = 0;
-    for (auto& f : fields) total += (f.bytes + 255) & ~(size_t)255;
-    CK(e->d_arena.ensure(total));
-    CK(e->h_arena.ensure(total));
-    size_t off = 0;
-    for (auto& f : fields) {
-      f.d->alias(static_cast<char*>(e->d_arena.p) + off, f.bytes);
-      f.h->alias(static_cast<char*>(e->h_arena.p) + off, f.bytes);
-      off += (f.bytes + 255) & ~(size_t)255;
-    }
-    e->arena_bytes = total;
-  }
+  CK(carve(e->d_arena,
+           {{&e->d_state, sizeof(RoundState), &e->h_state},
+            {&e->d_prefilter, P, &e->h_prefilter},
+            {&e->d_feasible, (size_t)P * 4, &e->h_feasible},
+            {&e->d_best_node, (size_t)P * 4, &e->h_best_node},
+            {&e->d_best_score, (size_t)P * 8, &e->h_best_score},
+            {&e->d_admit, G, &e->h_admit},
+            {&e->d_admit_bitmap, (size_t)cdiv(G, 32) * 4, &e->h_admit_bitmap},
+            {&e->d_new_denied, G, &e->h_new_denied},
+            {&e->d_order, (size_t)P * 4, &e->h_order},
+            {&e->d_rank, (size_t)P * 4, &e->h_rank},
+            {&e->d_filter_code, (e->out_flags & BS_OUT_FILTER) ? (size_t)P : 0, &e->h_filter_code}},
+           &e->h_arena, &e->arena_bytes));
   CK(e->d_best_packed.ensure((size_t)P * 8));
   // rows padded to a whole CTA of pods: the fit kernel writes pods >= P without a guard
   const size_t Prows = (size_t)cdiv(std::max(e->P, 1u), PODS_PER_CTA) * PODS_PER_CTA;
@@ -838,22 +878,12 @@ int ensure_round_buffers(bs_engine* e) {
   // sort scratch: one arena.  No persisting-L2 window over it: the set-aside such a window needs cost the score-mode
   // gang_fit kernel 0.9 ms of 3.85 on an H100 (its 8 GB score stream through a smaller L2), and the sort was no
   // faster with it.
-  {
-    const uint32_t M = std::max(P, G);
-    struct F { DevBuf* d; size_t bytes; };
-    F fields[] = {{&e->d_gk0, (size_t)G * 8}, {&e->d_gk1, (size_t)G * 8}, {&e->d_pk0, (size_t)P * 8}, {&e->d_pk1, (size_t)P * 8},
-                  {&e->d_idx_a, (size_t)M * 4}, {&e->d_idx_b, (size_t)M * 4},
-                  {&e->d_ghist, (size_t)3 * 256 * cdiv(M, SORT_TILE) * 4}, {&e->d_tilecnt, (size_t)cdiv(M, SORT_TILE) * 4},
-                  {&e->d_sort_barrier, sizeof(unsigned int)}, {&e->d_group_rank, (size_t)G * 4}};
-    size_t total = 0;
-    for (auto& f : fields) total += (f.bytes + 255) & ~(size_t)255;
-    CK(e->d_sort_arena.ensure(total));
-    size_t off = 0;
-    for (auto& f : fields) {
-      f.d->alias(static_cast<char*>(e->d_sort_arena.p) + off, f.bytes);
-      off += (f.bytes + 255) & ~(size_t)255;
-    }
-  }
+  const uint32_t M = std::max(P, G);
+  CK(carve(e->d_sort_arena,
+           {{&e->d_gk0, (size_t)G * 8}, {&e->d_gk1, (size_t)G * 8}, {&e->d_pk0, (size_t)P * 8}, {&e->d_pk1, (size_t)P * 8},
+            {&e->d_idx_a, (size_t)M * 4}, {&e->d_idx_b, (size_t)M * 4},
+            {&e->d_ghist, (size_t)3 * 256 * cdiv(M, SORT_TILE) * 4}, {&e->d_tilecnt, (size_t)cdiv(M, SORT_TILE) * 4},
+            {&e->d_sort_barrier, sizeof(unsigned int)}, {&e->d_group_rank, (size_t)G * 4}}));
   return BS_OK;
 }
 
@@ -1059,8 +1089,8 @@ int evaluate_async_locked(bs_engine* e) {
       a.P = P; a.N = e->N; a.Npad = e->Npad; a.W = e->W;
       a.best_packed = e->d_best_packed.as<unsigned long long>();
       uint32_t nl = 1;
-      CK(launch_fit(a, cdiv(P, PODS_PER_CTA), e->s, &nl, e->profiling ? e->ev_a[BS_K_GANG_FIT] : nullptr,
-                    e->profiling ? e->ev_b[BS_K_GANG_FIT] : nullptr));
+      CK(launch_fit(a, cdiv(P, PODS_PER_CTA), e->s, &nl, e->profiling ? e->ev_a[BS_K_GANG_FIT].h : nullptr,
+                    e->profiling ? e->ev_b[BS_K_GANG_FIT].h : nullptr));
       if (e->profiling) e->k_valid[BS_K_GANG_FIT] = true;
       tm.launched(nl);
     }
@@ -1167,7 +1197,7 @@ int fetch_locked(bs_engine* e, bs_results* out, bool view = false) {
     out->max_group = st->max_group;
     out->max_finished = st->max_finished;
   } else if (out) {
-    auto cp = [](void* dst, const PinBuf& src, size_t bytes) {
+    auto cp = [](void* dst, const View& src, size_t bytes) {
       if (dst && bytes) memcpy(dst, src.p, bytes);
     };
     cp(out->prefilter, e->h_prefilter, P);
@@ -1235,18 +1265,18 @@ int bs_create(const bs_config* cfg, bs_engine** out) {
   int prio_lo = 0, prio_hi = 0;
   cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);   // the small kernels of the PreFilter chain must get the
                                                           // SM slots the fit kernel's retiring CTAs free
-  bool ok = cudaStreamCreateWithFlags(&e->s, cudaStreamNonBlocking) == cudaSuccess &&
-            cudaStreamCreateWithFlags(&e->s2, cudaStreamNonBlocking) == cudaSuccess &&
-            cudaStreamCreateWithPriority(&e->s3, cudaStreamNonBlocking, prio_hi) == cudaSuccess &&
-            cudaStreamCreateWithPriority(&e->s4, cudaStreamNonBlocking, prio_hi) == cudaSuccess &&
-            cudaEventCreateWithFlags(&e->ev_pre, cudaEventDisableTiming) == cudaSuccess &&
-            cudaEventCreateWithFlags(&e->ev_push, cudaEventDisableTiming) == cudaSuccess &&
-            cudaEventCreateWithFlags(&e->ev_gath, cudaEventDisableTiming) == cudaSuccess &&
-            cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming) == cudaSuccess &&
-            cudaEventCreateWithFlags(&e->ev_join, cudaEventDisableTiming) == cudaSuccess &&
-            cudaEventCreateWithFlags(&e->ev_classes, cudaEventDisableTiming) == cudaSuccess;
+  bool ok = cudaStreamCreateWithFlags(&e->s.h, cudaStreamNonBlocking) == cudaSuccess &&
+            cudaStreamCreateWithFlags(&e->s2.h, cudaStreamNonBlocking) == cudaSuccess &&
+            cudaStreamCreateWithPriority(&e->s3.h, cudaStreamNonBlocking, prio_hi) == cudaSuccess &&
+            cudaStreamCreateWithPriority(&e->s4.h, cudaStreamNonBlocking, prio_hi) == cudaSuccess &&
+            cudaEventCreateWithFlags(&e->ev_pre.h, cudaEventDisableTiming) == cudaSuccess &&
+            cudaEventCreateWithFlags(&e->ev_push.h, cudaEventDisableTiming) == cudaSuccess &&
+            cudaEventCreateWithFlags(&e->ev_gath.h, cudaEventDisableTiming) == cudaSuccess &&
+            cudaEventCreateWithFlags(&e->ev_fork.h, cudaEventDisableTiming) == cudaSuccess &&
+            cudaEventCreateWithFlags(&e->ev_join.h, cudaEventDisableTiming) == cudaSuccess &&
+            cudaEventCreateWithFlags(&e->ev_classes.h, cudaEventDisableTiming) == cudaSuccess;
   for (int k = 0; ok && k < BS_K_COUNT; ++k)
-    ok = cudaEventCreate(&e->ev_a[k]) == cudaSuccess && cudaEventCreate(&e->ev_b[k]) == cudaSuccess;
+    ok = cudaEventCreate(&e->ev_a[k].h) == cudaSuccess && cudaEventCreate(&e->ev_b[k].h) == cudaSuccess;
   if (ok) {
     int per_sm = 0, sms = 0;
     int per_sm_wide = 0;
@@ -1273,48 +1303,7 @@ void bs_destroy(bs_engine* e) {
   if (e->s4) cudaStreamSynchronize(e->s4);
   for (uint32_t r = 0; r < e->peer_world; ++r)
     if (r != e->peer_rank && e->peer_ptr[r]) cudaIpcCloseMemHandle(e->peer_ptr[r]);
-  e->d_gather.release();
-  e->d_peer_err.release();
-  DevBuf* bufs[] = {&e->d_alloc, &e->d_requested, &e->d_pod_count, &e->d_apres, &e->d_rpres, &e->d_label,
-                    &e->d_taint, &e->d_nflags, &e->d_left_w, &e->d_left_n, &e->d_left_present, &e->d_left_plain, &e->d_filter_bitmap, &e->d_filter_code, &e->d_classfit, &e->d_req,
-                    &e->d_ppres, &e->d_gid, &e->d_prio, &e->d_ts, &e->d_pflags, &e->d_pod_fit_class,
-                    &e->d_pod_rep_class, &e->d_min_member, &e->d_scheduled, &e->d_matched, &e->d_gflags,
-                    &e->d_min_res, &e->d_mrpres, &e->d_creation, &e->d_name_rank, &e->d_group_rep_class,
-                    &e->d_fsel, &e->d_ftol, &e->d_fnz, &e->d_faff, &e->d_rsel, &e->d_rtol, &e->d_raff, &e->d_aff_bits, &e->d_eflags, &e->d_emin_res,
-                    &e->d_emrpres, &e->d_erep_class, &e->d_first_pod, &e->d_in_round, &e->d_contrib,
-                    &e->d_done, &e->d_okA, &e->d_state, &e->d_pre, &e->d_pre_present, &e->d_pre_stats, &e->d_max_partial, &e->d_pre_part,
-                    &e->d_pre_part_pres, &e->d_pre_cstats, &e->d_pre_done,
-                    &e->d_best_packed, &e->d_prefilter, &e->d_feasible, &e->d_best_node, &e->d_best_score, &e->d_admit,
-                    &e->d_admit_bitmap, &e->d_new_denied, &e->d_fit_bitmap, &e->d_score, &e->d_order,
-                    &e->d_rank, &e->d_gk0, &e->d_gk1, &e->d_pk0, &e->d_pk1, &e->d_idx_a, &e->d_idx_b,
-                    &e->d_ghist, &e->d_group_rank, &e->d_tilecnt, &e->d_sort_barrier,
-                    &e->r_req, &e->r_pc, &e->r_rp, &e->r_matched, &e->r_gflags, &e->r_grc, &e->r_minres, &e->r_mrp,
-                    &e->r_queue, &e->r_pf, &e->r_node, &e->r_ready, &e->r_status, &e->r_sum, &e->r_max, &e->r_keys,
-                    &e->r_left0, &e->r_left1, &e->r_both, &e->r_fit, &e->r_stat};
-  for (DevBuf* b : bufs) b->release();
-  e->d_sort_arena.release();
-  e->d_arena.release();
-  e->h_arena.release();
-  for (DevBuf& b : e->u_buf) b.release();
-  PinBuf* pins[] = {&e->h_prefilter, &e->h_feasible, &e->h_best_node, &e->h_best_score, &e->h_admit,
-                    &e->h_admit_bitmap, &e->h_new_denied, &e->h_order, &e->h_rank, &e->h_state, &e->h_filter_code};
-  for (PinBuf* b : pins) b->release();
-  for (int k = 0; k < BS_K_COUNT; ++k) {
-    if (e->ev_a[k]) cudaEventDestroy(e->ev_a[k]);
-    if (e->ev_b[k]) cudaEventDestroy(e->ev_b[k]);
-  }
-  if (e->ev_fork) cudaEventDestroy(e->ev_fork);
-  if (e->ev_join) cudaEventDestroy(e->ev_join);
-  if (e->ev_pre) cudaEventDestroy(e->ev_pre);
-  if (e->ev_push) cudaEventDestroy(e->ev_push);
-  if (e->ev_gath) cudaEventDestroy(e->ev_gath);
-  if (e->s3) cudaStreamDestroy(e->s3);
-  if (e->s4) cudaStreamDestroy(e->s4);
-  if (e->ev_classes) cudaEventDestroy(e->ev_classes);
-  e->h_pfc.release(); e->h_prc.release(); e->h_grc.release();
-  if (e->s) cudaStreamDestroy(e->s);
-  if (e->s2) cudaStreamDestroy(e->s2);
-  delete e;
+  delete e;   // the members free their buffers, streams and events on the engine's device (the guard is still alive)
 }
 
 int bs_upload_nodes(bs_engine* e, const bs_node_table* t) {
@@ -1322,9 +1311,8 @@ int bs_upload_nodes(bs_engine* e, const bs_node_table* t) {
   std::lock_guard<std::mutex> lk(e->mu);
   if (t->n_lanes != e->L) return fail(e, BS_E_INVAL, "bs_upload_nodes: n_lanes differs from the engine's");
   const uint32_t N = t->n_nodes, L = e->L;
-  if (N && (!t->alloc || !t->requested || !t->pod_count || !t->alloc_present || !t->req_present ||
-            !t->label_mask || !t->taint_mask || !t->flags))
-    return fail(e, BS_E_INVAL, "bs_upload_nodes: null column");
+  const auto cols = node_cols(e, t);
+  if (N && null_column(cols)) return fail(e, BS_E_INVAL, "bs_upload_nodes: null column");
   HP_BEGIN(e);
   const NodeHostStats hs = node_host_pass(t, L, N);
   if (!hs.ok) return fail(e, BS_E_RANGE, "bs_upload_nodes: value outside +-2^56");
@@ -1332,14 +1320,7 @@ int bs_upload_nodes(bs_engine* e, const bs_node_table* t) {
   BS_DEVICE_GUARD(e);
   const uint32_t Npad = std::max(1u, cdiv(N, NODE_TILE)) * NODE_TILE;
   int rc;
-  if ((rc = upload_lanes(e, e->d_alloc, t->alloc, L, N, Npad))) return rc;
-  if ((rc = upload_lanes(e, e->d_requested, t->requested, L, N, Npad))) return rc;
-  if ((rc = upload_vec(e, e->d_pod_count, t->pod_count, N, Npad))) return rc;
-  if ((rc = upload_vec(e, e->d_apres, t->alloc_present, N, Npad))) return rc;
-  if ((rc = upload_vec(e, e->d_rpres, t->req_present, N, Npad))) return rc;
-  if ((rc = upload_vec(e, e->d_label, t->label_mask, N, Npad))) return rc;
-  if ((rc = upload_vec(e, e->d_taint, t->taint_mask, N, Npad))) return rc;
-  if ((rc = upload_vec(e, e->d_nflags, t->flags, N, Npad))) return rc;
+  if ((rc = upload_cols(e, cols, N, Npad))) return rc;
   HP(e, "nodes:dma-enqueue");
   CK(cudaStreamSynchronize(e->s));
   HP(e, "nodes:dma-wait");
@@ -1369,61 +1350,29 @@ int bs_update_nodes(bs_engine* e, const uint32_t* idx, const bs_node_table* t) {
   if (t->n_lanes != e->L) return fail(e, BS_E_INVAL, "bs_update_nodes: n_lanes differs from the engine's");
   const uint32_t n = t->n_nodes, L = e->L;
   if (!n) return BS_OK;
-  if (!t->alloc || !t->requested || !t->pod_count || !t->alloc_present || !t->req_present || !t->label_mask ||
-      !t->taint_mask || !t->flags)
-    return fail(e, BS_E_INVAL, "bs_update_nodes: null column");
+  const auto cols = node_cols(e, t);
+  if (null_column(cols)) return fail(e, BS_E_INVAL, "bs_update_nodes: null column");
   for (uint32_t k = 0; k < n; ++k)
     if (idx[k] >= e->N) return BS_E_INDEX;
-  int64_t mx_a[BS_MAX_LANES] = {}, mx_r[BS_MAX_LANES] = {};
-  if (!lane_maxima(t->alloc, L, n, mx_a) || !lane_maxima(t->requested, L, n, mx_r))
-    return fail(e, BS_E_RANGE, "bs_update_nodes: value outside +-2^56");
+  const NodeHostStats hs = node_host_pass(t, L, n);
+  if (!hs.ok) return fail(e, BS_E_RANGE, "bs_update_nodes: value outside +-2^56");
   BS_DEVICE_GUARD(e);
   HP_BEGIN(e);
-  // scratch of the changed rows: kept in the engine (cudaMalloc / cudaFree per call would cost more than the scatter)
-  DevBuf &da = e->u_buf[0], &dr = e->u_buf[1], &dpc = e->u_buf[2], &dap = e->u_buf[3], &drp = e->u_buf[4], &dl = e->u_buf[5],
-         &dt = e->u_buf[6], &df = e->u_buf[7], &di = e->u_buf[8];
-  cudaError_t er = da.ensure((size_t)L * n * 8);
-  if (er == cudaSuccess) er = dr.ensure((size_t)L * n * 8);
-  if (er == cudaSuccess) er = dpc.ensure((size_t)n * 4);
-  if (er == cudaSuccess) er = dap.ensure((size_t)n * 4);
-  if (er == cudaSuccess) er = drp.ensure((size_t)n * 4);
-  if (er == cudaSuccess) er = dl.ensure((size_t)n * 8);
-  if (er == cudaSuccess) er = dt.ensure((size_t)n * 8);
-  if (er == cudaSuccess) er = df.ensure(n);
-  if (er == cudaSuccess) er = di.ensure((size_t)n * 4);
-  auto h2d = [&](DevBuf& d, const void* src, size_t bytes) {
-    if (er == cudaSuccess) er = cudaMemcpyAsync(d.p, src, bytes, cudaMemcpyHostToDevice, e->s);
-  };
-  h2d(da, t->alloc, (size_t)L * n * 8); h2d(dr, t->requested, (size_t)L * n * 8);
-  h2d(dpc, t->pod_count, (size_t)n * 4); h2d(dap, t->alloc_present, (size_t)n * 4);
-  h2d(drp, t->req_present, (size_t)n * 4); h2d(dl, t->label_mask, (size_t)n * 8);
-  h2d(dt, t->taint_mask, (size_t)n * 8); h2d(df, t->flags, n); h2d(di, idx, (size_t)n * 4);
-  if (er == cudaSuccess) {
-    NodeTabMut dst{e->d_alloc.as<int64_t>(), e->d_requested.as<int64_t>(), e->d_pod_count.as<int32_t>(),
-                   e->d_apres.as<uint32_t>(), e->d_rpres.as<uint32_t>(), e->d_label.as<uint64_t>(),
-                   e->d_taint.as<uint64_t>(), e->d_nflags.as<uint8_t>()};
-    NodeTab src{};
-    src.alloc = da.as<int64_t>(); src.requested = dr.as<int64_t>(); src.pod_count = dpc.as<int32_t>();
-    src.alloc_present = dap.as<uint32_t>(); src.req_present = drp.as<uint32_t>(); src.label = dl.as<uint64_t>();
-    src.taint = dt.as<uint64_t>(); src.flags = df.as<uint8_t>();
-    node_scatter_kernel<<<cdiv(n, 256), 256, 0, e->s>>>(dst, e->Npad, L, src, di.as<uint32_t>(), n);
-    e->launches++;
-    HP(e, "upd-nodes:enqueue");
-    er = cudaStreamSynchronize(e->s);
-  }
-  CK(er);
+  int rc;
+  if ((rc = scatter_rows(e, cols, idx, n, e->Npad))) return rc;
+  HP(e, "upd-nodes:enqueue");
+  CK(cudaStreamSynchronize(e->s));
   HP(e, "upd-nodes:wait");
   // lane maxima only ever grow here (a conservative bound keeps the wide/narrow split exact); the OR
   // of the residuals only gains bits (fewer common trailing zeros: a smaller unit, still exact)
-  left_stats(t, L, n, e->or_left, e->max_left);
   for (uint32_t d = 0; d < L; ++d) {
-    e->max_alloc[d] = std::max(e->max_alloc[d], mx_a[d]);
-    e->max_requested[d] = std::max(e->max_requested[d], mx_r[d]);
+    e->max_alloc[d] = std::max(e->max_alloc[d], hs.mx_a[d]);
+    e->max_requested[d] = std::max(e->max_requested[d], hs.mx_r[d]);
+    e->max_left[d] = std::max(e->max_left[d], hs.mx_l[d]);
+    e->or_left[d] |= hs.or_l[d];
   }
-  for (uint32_t k = 0; k < n; ++k) {
-    e->max_pod_count = std::max<int64_t>(e->max_pod_count, std::abs((int64_t)t->pod_count[k]));
-    e->h_nflags[idx[k]] = t->flags[k];
-  }
+  e->max_pod_count = std::max(e->max_pod_count, hs.mx_pc);
+  for (uint32_t k = 0; k < n; ++k) e->h_nflags[idx[k]] = t->flags[k];
   e->nodes_dirty = true;
   e->evaluated = false;
   return BS_OK;
@@ -1434,9 +1383,8 @@ int bs_upload_groups(bs_engine* e, const bs_group_table* t) {
   std::lock_guard<std::mutex> lk(e->mu);
   if (t->n_lanes != e->L) return fail(e, BS_E_INVAL, "bs_upload_groups: n_lanes differs from the engine's");
   const uint32_t G = t->n_groups, L = e->L;
-  if (G && (!t->min_member || !t->scheduled || !t->matched || !t->flags || !t->min_res ||
-            !t->min_res_present || !t->rep_sel || !t->rep_tol || !t->creation_ns || !t->name_rank))
-    return fail(e, BS_E_INVAL, "bs_upload_groups: null column");
+  const auto cols = group_cols(e, t);
+  if (G && (null_column(cols) || !t->rep_sel || !t->rep_tol)) return fail(e, BS_E_INVAL, "bs_upload_groups: null column");
   // the DMAs go first (asynchronous from pinned tables) and run under the host checks below; a table
   // that then fails validation is dropped (have_groups = false)
   BS_DEVICE_GUARD(e);
@@ -1445,14 +1393,7 @@ int bs_upload_groups(bs_engine* e, const bs_group_table* t) {
   e->evaluated = false;
   const uint32_t Gp = std::max(G, 1u);
   int rc;
-  if ((rc = upload_vec(e, e->d_min_member, t->min_member, G, Gp))) return rc;
-  if ((rc = upload_vec(e, e->d_scheduled, t->scheduled, G, Gp))) return rc;
-  if ((rc = upload_vec(e, e->d_matched, t->matched, G, Gp))) return rc;
-  if ((rc = upload_vec(e, e->d_gflags, t->flags, G, Gp))) return rc;
-  if ((rc = upload_lanes(e, e->d_min_res, t->min_res, L, G, Gp))) return rc;
-  if ((rc = upload_vec(e, e->d_mrpres, t->min_res_present, G, Gp))) return rc;
-  if ((rc = upload_vec(e, e->d_creation, t->creation_ns, G, Gp))) return rc;
-  if ((rc = upload_vec(e, e->d_name_rank, t->name_rank, G, Gp))) return rc;
+  if ((rc = upload_cols(e, cols, G, Gp))) return rc;
   HP(e, "groups:dma-enqueue");
   // one chunked pass over the host columns (an omp team for big tables): |min_res| range, the varying bits of the
   // sort-key words, creation sentinel, and whether the representative columns moved since their ids were assigned
@@ -1535,48 +1476,21 @@ int bs_update_groups(bs_engine* e, const uint32_t* idx, const bs_group_table* t)
   if (t->n_lanes != e->L) return fail(e, BS_E_INVAL, "bs_update_groups: n_lanes differs from the engine's");
   const uint32_t n = t->n_groups, L = e->L, G = e->G;
   if (!n) return BS_OK;
-  if (!t->min_member || !t->scheduled || !t->matched || !t->flags || !t->min_res || !t->min_res_present ||
-      !t->rep_sel || !t->rep_tol || !t->creation_ns || !t->name_rank)
-    return fail(e, BS_E_INVAL, "bs_update_groups: null column");
+  const auto cols = group_cols(e, t);
+  if (null_column(cols) || !t->rep_sel || !t->rep_tol) return fail(e, BS_E_INVAL, "bs_update_groups: null column");
   for (uint32_t k = 0; k < n; ++k)
     if (idx[k] >= G) return BS_E_INDEX;
-  {
-    int64_t mx[BS_MAX_LANES] = {};
-    if (!lane_maxima(t->min_res, L, n, mx)) return fail(e, BS_E_RANGE, "bs_update_groups: value outside +-2^56");
-  }
+  if (!std::all_of(t->min_res, t->min_res + (size_t)L * n,
+                   [](int64_t v) { return v >= -BS_VALUE_LIMIT && v <= BS_VALUE_LIMIT; }))
+    return fail(e, BS_E_RANGE, "bs_update_groups: value outside +-2^56");
   for (uint32_t k = 0; k < n; ++k)
     if (t->creation_ns[k] == INT64_MAX) return fail(e, BS_E_RANGE, "bs_update_groups: creation_ns == INT64_MAX");
   BS_DEVICE_GUARD(e);
   HP_BEGIN(e);
-  DevBuf &dmm = e->u_buf[0], &dsc = e->u_buf[1], &dma = e->u_buf[2], &dfl = e->u_buf[3], &dmr = e->u_buf[4], &dmp = e->u_buf[5],
-         &dcr = e->u_buf[6], &dnr = e->u_buf[7], &di = e->u_buf[8];
-  cudaError_t er = dmm.ensure((size_t)n * 4);
-  if (er == cudaSuccess) er = dsc.ensure((size_t)n * 4);
-  if (er == cudaSuccess) er = dma.ensure((size_t)n * 4);
-  if (er == cudaSuccess) er = dfl.ensure(n);
-  if (er == cudaSuccess) er = dmr.ensure((size_t)L * n * 8);
-  if (er == cudaSuccess) er = dmp.ensure((size_t)n * 4);
-  if (er == cudaSuccess) er = dcr.ensure((size_t)n * 8);
-  if (er == cudaSuccess) er = dnr.ensure((size_t)n * 4);
-  if (er == cudaSuccess) er = di.ensure((size_t)n * 4);
-  auto h2d = [&](DevBuf& d, const void* src, size_t bytes) {
-    if (er == cudaSuccess) er = cudaMemcpyAsync(d.p, src, bytes, cudaMemcpyHostToDevice, e->s);
-  };
-  h2d(dmm, t->min_member, (size_t)n * 4); h2d(dsc, t->scheduled, (size_t)n * 4); h2d(dma, t->matched, (size_t)n * 4);
-  h2d(dfl, t->flags, n); h2d(dmr, t->min_res, (size_t)L * n * 8); h2d(dmp, t->min_res_present, (size_t)n * 4);
-  h2d(dcr, t->creation_ns, (size_t)n * 8); h2d(dnr, t->name_rank, (size_t)n * 4); h2d(di, idx, (size_t)n * 4);
-  if (er == cudaSuccess) {
-    GroupCols dst{e->d_min_member.as<uint32_t>(), e->d_scheduled.as<uint32_t>(), e->d_matched.as<uint32_t>(),
-                  e->d_gflags.as<uint8_t>(), e->d_min_res.as<int64_t>(), e->d_mrpres.as<uint32_t>(),
-                  e->d_creation.as<int64_t>(), e->d_name_rank.as<uint32_t>()};
-    GroupCols src{dmm.as<uint32_t>(), dsc.as<uint32_t>(), dma.as<uint32_t>(), dfl.as<uint8_t>(), dmr.as<int64_t>(),
-                  dmp.as<uint32_t>(), dcr.as<int64_t>(), dnr.as<uint32_t>()};
-    group_scatter_kernel<<<cdiv(n, 256), 256, 0, e->s>>>(dst, std::max(G, 1u), L, src, di.as<uint32_t>(), n);
-    e->launches++;
-    HP(e, "upd-groups:enqueue");
-    er = cudaStreamSynchronize(e->s);
-  }
-  CK(er);
+  int rc;
+  if ((rc = scatter_rows(e, cols, idx, n, std::max(G, 1u)))) return rc;
+  HP(e, "upd-groups:enqueue");
+  CK(cudaStreamSynchronize(e->s));
   HP(e, "upd-groups:wait");
   // sort-key digits that vary: the accumulated OR / AND only widen (a superset costs a pass, never an error)
   for (uint32_t k = 0; k < n; ++k) {
@@ -1640,7 +1554,7 @@ int bs_upload_pods(bs_engine* e, const bs_pod_table* t) {
   e->evaluated = false;
   const uint32_t Pp = std::max(P, 1u);
   int rc;
-  if ((rc = upload_lanes(e, e->d_req, t->req, L, P, Pp))) return rc;
+  if ((rc = upload_col(e, col(t->req, e->d_req, L), P, Pp))) return rc;
   if ((rc = upload_vec(e, e->d_ppres, t->req_present, P, Pp))) return rc;
   if ((rc = upload_vec(e, e->d_gid, t->gid, P, Pp))) return rc;
   if ((rc = upload_vec(e, e->d_prio, t->priority, P, Pp))) return rc;
@@ -2168,12 +2082,9 @@ int bs_node_left(bs_engine* e, uint64_t sel, uint64_t tol, float percent, int64_
   node_left_class_kernel<<<cdiv(N, 256), 256, 0, e->s>>>(node_tab(e), sel, tol, percent, dl.as<int64_t>(),
                                                          dp.as<uint32_t>());
   e->launches++;
-  cudaError_t er = cudaMemcpyAsync(left, dl.p, (size_t)L * N * 8, cudaMemcpyDeviceToHost, e->s);
-  if (er == cudaSuccess) er = cudaMemcpyAsync(present, dp.p, (size_t)N * 4, cudaMemcpyDeviceToHost, e->s);
-  if (er == cudaSuccess) er = cudaStreamSynchronize(e->s);
-  dl.release();
-  dp.release();
-  CK(er);
+  CK(cudaMemcpyAsync(left, dl.p, (size_t)L * N * 8, cudaMemcpyDeviceToHost, e->s));
+  CK(cudaMemcpyAsync(present, dp.p, (size_t)N * 4, cudaMemcpyDeviceToHost, e->s));
+  CK(cudaStreamSynchronize(e->s));
   return BS_OK;
 }
 
@@ -2189,38 +2100,27 @@ int bs_cluster_check(bs_engine* e, uint64_t sel, uint64_t tol, float percent, co
     memset(ok, 0, n_needs);  // empty snapshot list: the loop never runs (core.go:604,631)
     return BS_OK;
   }
-  DevBuf pre, pp, stats, dn, dnp, dok, spart, spres, scst, sdone;
+  DevBuf scratch;
+  View pre, pp, stats, dn, dnp, dok, spart, spres, scst, sdone;
   const size_t n_chunks = cdiv(N, PREFIX_CHUNK);
-  cudaError_t er = pre.ensure((size_t)L * N * 8);
-  if (er == cudaSuccess) er = spart.ensure(n_chunks * BS_MAX_LANES * 8);
-  if (er == cudaSuccess) er = spres.ensure(n_chunks * 4);
-  if (er == cudaSuccess) er = scst.ensure(n_chunks * sizeof(ClassStats));
-  if (er == cudaSuccess) er = sdone.ensure(4);
-  if (er == cudaSuccess) er = cudaMemsetAsync(sdone.p, 0, 4, e->s);
-  if (er == cudaSuccess) er = pp.ensure((size_t)N * 4);
-  if (er == cudaSuccess) er = stats.ensure(sizeof(ClassStats));
-  if (er == cudaSuccess) er = dn.ensure((size_t)L * n_needs * 8);
-  if (er == cudaSuccess) er = dnp.ensure((size_t)n_needs * 4);
-  if (er == cudaSuccess) er = dok.ensure(n_needs);
-  if (er == cudaSuccess) er = cudaMemcpyAsync(dn.p, need, (size_t)L * n_needs * 8, cudaMemcpyHostToDevice, e->s);
-  if (er == cudaSuccess) er = cudaMemcpyAsync(dnp.p, need_present, (size_t)n_needs * 4, cudaMemcpyHostToDevice, e->s);
-  if (er == cudaSuccess) {
-    PrefixOut po{pre.as<int64_t>(), pp.as<uint32_t>(), stats.as<ClassStats>()};
-    NodeTab t = node_tab(e);
-    PrefixSel ps{nullptr, nullptr, nullptr, 0, 2, sel, tol, percent, nullptr};
-    PrefixScratch psc{spart.as<int64_t>(), spres.as<uint32_t>(), scst.as<ClassStats>(), sdone.as<uint32_t>()};
-    launch_prefix(L, t, ps, psc, po, 1, e->s);
-    const uint64_t threads = (uint64_t)n_needs * 32;
-    needs_check_kernel<<<(uint32_t)((threads + 255) / 256), 256, 0, e->s>>>(
-        t, po, dn.as<int64_t>(), dnp.as<uint32_t>(), n_needs, dok.as<uint8_t>());
-    e->launches += 3;
-    er = cudaMemcpyAsync(ok, dok.p, n_needs, cudaMemcpyDeviceToHost, e->s);
-  }
-  if (er == cudaSuccess) er = cudaStreamSynchronize(e->s);
-  if (er == cudaSuccess) er = cudaGetLastError();
-  pre.release(); pp.release(); stats.release(); dn.release(); dnp.release(); dok.release();
-  spart.release(); spres.release(); scst.release(); sdone.release();
-  CK(er);
+  CK(carve(scratch, {{&pre, (size_t)L * N * 8}, {&spart, n_chunks * BS_MAX_LANES * 8}, {&spres, n_chunks * 4},
+                     {&scst, n_chunks * sizeof(ClassStats)}, {&sdone, 4}, {&pp, (size_t)N * 4}, {&stats, sizeof(ClassStats)},
+                     {&dn, (size_t)L * n_needs * 8}, {&dnp, (size_t)n_needs * 4}, {&dok, n_needs}}));
+  CK(cudaMemsetAsync(sdone.p, 0, 4, e->s));
+  CK(cudaMemcpyAsync(dn.p, need, (size_t)L * n_needs * 8, cudaMemcpyHostToDevice, e->s));
+  CK(cudaMemcpyAsync(dnp.p, need_present, (size_t)n_needs * 4, cudaMemcpyHostToDevice, e->s));
+  PrefixOut po{pre.as<int64_t>(), pp.as<uint32_t>(), stats.as<ClassStats>()};
+  NodeTab t = node_tab(e);
+  PrefixSel ps{nullptr, nullptr, nullptr, 0, 2, sel, tol, percent, nullptr};
+  PrefixScratch psc{spart.as<int64_t>(), spres.as<uint32_t>(), scst.as<ClassStats>(), sdone.as<uint32_t>()};
+  launch_prefix(L, t, ps, psc, po, 1, e->s);
+  const uint64_t threads = (uint64_t)n_needs * 32;
+  needs_check_kernel<<<(uint32_t)((threads + 255) / 256), 256, 0, e->s>>>(
+      t, po, dn.as<int64_t>(), dnp.as<uint32_t>(), n_needs, dok.as<uint8_t>());
+  e->launches += 3;
+  CK(cudaMemcpyAsync(ok, dok.p, n_needs, cudaMemcpyDeviceToHost, e->s));
+  CK(cudaStreamSynchronize(e->s));
+  CK(cudaGetLastError());
   return BS_OK;
 }
 
@@ -2239,128 +2139,112 @@ int bs_replay(bs_engine* e, const uint32_t* queue, uint32_t n_queue, bs_replay_r
   int rc;
   if (e->classes_dirty && (rc = rebuild_classes(e))) return rc;
 
-  // scratch copies of everything the cycle mutates
-  DevBuf &s_req = e->r_req, &s_pc = e->r_pc, &s_rp = e->r_rp, &s_matched = e->r_matched, &s_gflags = e->r_gflags,
-         &s_grc = e->r_grc, &s_minres = e->r_minres, &s_mrp = e->r_mrp, &d_queue = e->r_queue, &d_pf = e->r_pf,
-         &d_node = e->r_node, &d_ready = e->r_ready, &d_status = e->r_status, &c_sum = e->r_sum, &c_max = e->r_max,
-         &c_keys = e->r_keys, &n_left0 = e->r_left0, &n_left1 = e->r_left1, &n_both = e->r_both, &n_fit = e->r_fit,
-         &n_stat = e->r_stat;
+  // scratch copies of everything the cycle mutates, the queue and the outputs, and the compact node state and
+  // block cache the kernel builds (replay.cuh)
   const uint32_t Gp = std::max(G, 1u), Qp = std::max(n_queue, 1u);
-  cudaError_t er = s_req.ensure((size_t)L * Npad * 8);
-  auto dup = [&](DevBuf& dst, const DevBuf& src, size_t bytes) {
-    if (er == cudaSuccess) er = dst.ensure(std::max<size_t>(bytes, 4));
-    if (er == cudaSuccess && bytes) er = cudaMemcpyAsync(dst.p, src.p, bytes, cudaMemcpyDeviceToDevice, e->s);
+  const bool fitmask = e->n_rep_classes <= (uint32_t)REPLAY_MAX_CLASSES;
+  // block cache of the cluster scan: every running sum must stay below 2^62.  A pod is only assumed where it
+  // fits, so a node's `requested` never passes its capacity by more than one request; only negative requests
+  // accumulate without that limit.
+  long double worst = 0;
+  for (uint32_t d = 0; d < L; ++d)
+    worst = std::max(worst, (long double)e->max_alloc[d] + (long double)e->max_requested[d] + (long double)e->max_req[d] +
+                                (long double)e->neg_req[d] * (long double)n_queue + (long double)e->max_pod_count + n_queue);
+  const bool safe = worst * (long double)std::max(N, 1u) < 4.0e18L;
+  const uint32_t n_blocks = cdiv(N, REPLAY_BLOCK);
+  const bool cache = safe && fitmask && n_blocks >= 1 && n_blocks <= (uint32_t)REPLAY_MAX_BLOCKS;
+  const size_t rows = cache ? (size_t)2 * e->n_rep_classes * n_blocks : 0, maxl = replay_maxl(L);
+  View s_req, s_pc, s_rp, s_matched, s_gflags, s_grc, s_minres, s_mrp, d_queue, d_pf, d_node, d_ready, d_status,
+      n_left0, n_left1, n_both, n_stat, n_fit, c_sum, c_max, c_keys;
+  // The node state and block cache every step reads come first: carved behind the copies, the same kernel took
+  // 2 % longer at the bench shape on an H100.
+  CK(carve(e->d_replay,
+           {{&n_left0, (size_t)L * Npad * 8}, {&n_left1, (size_t)L * Npad * 8}, {&n_both, (size_t)Npad * 4},
+            {&n_stat, Npad}, {&n_fit, fitmask ? (size_t)Npad * 4 : 0}, {&c_sum, rows * maxl * 8},
+            {&c_max, rows * maxl * 8}, {&c_keys, rows * 4}, {&s_req, (size_t)L * Npad * 8}, {&s_pc, (size_t)Npad * 4},
+            {&s_rp, (size_t)Npad * 4}, {&s_matched, (size_t)Gp * 4}, {&s_gflags, Gp}, {&s_grc, (size_t)Gp * 4},
+            {&s_minres, (size_t)L * Gp * 8}, {&s_mrp, (size_t)Gp * 4}, {&d_queue, (size_t)Qp * 4}, {&d_pf, Qp},
+            {&d_node, (size_t)Qp * 4}, {&d_ready, Qp}, {&d_status, 128}}));
+  auto dup = [&](const View& dst, const DevBuf& src, size_t bytes) {
+    return bytes ? cudaMemcpyAsync(dst.p, src.p, bytes, cudaMemcpyDeviceToDevice, e->s) : cudaSuccess;
   };
-  dup(s_req, e->d_requested, (size_t)L * Npad * 8);
-  dup(s_pc, e->d_pod_count, (size_t)Npad * 4);
-  dup(s_rp, e->d_rpres, (size_t)Npad * 4);
-  dup(s_matched, e->d_matched, (size_t)G * 4);
-  dup(s_gflags, e->d_gflags, (size_t)G);
-  dup(s_grc, e->d_group_rep_class, (size_t)G * 4);
-  dup(s_minres, e->d_min_res, (size_t)L * G * 8);
-  dup(s_mrp, e->d_mrpres, (size_t)G * 4);
-  if (er == cudaSuccess) er = d_queue.ensure((size_t)Qp * 4);
-  if (er == cudaSuccess && queue && n_queue)
-    er = cudaMemcpyAsync(d_queue.p, queue, (size_t)n_queue * 4, cudaMemcpyHostToDevice, e->s);
-  if (er == cudaSuccess) er = d_pf.ensure(Qp);
-  if (er == cudaSuccess) er = d_node.ensure((size_t)Qp * 4);
-  if (er == cudaSuccess) er = d_ready.ensure(Qp);
-  if (er == cudaSuccess) er = d_status.ensure(128);
-  if (er == cudaSuccess) er = cudaMemsetAsync(d_status.p, 0, 128, e->s);
-  int32_t status = 0;
-  if (er == cudaSuccess) {
-    ReplayArgs a{};
-    a.nt = node_tab(e);
-    a.nt.requested = s_req.as<int64_t>();
-    a.nt.pod_count = s_pc.as<int32_t>();
-    a.nt.req_present = s_rp.as<uint32_t>();
-    a.requested = s_req.as<int64_t>();
-    a.pod_count = s_pc.as<int32_t>();
-    a.req_present = s_rp.as<uint32_t>();
-    a.pt = pod_tab(e);
-    // compact node state the kernel builds and maintains (replay.cuh)
-    er = n_left0.ensure((size_t)L * Npad * 8);
-    if (er == cudaSuccess) er = n_left1.ensure((size_t)L * Npad * 8);
-    if (er == cudaSuccess) er = n_both.ensure((size_t)Npad * 4);
-    if (er == cudaSuccess) er = n_stat.ensure((size_t)Npad);
-    if (er == cudaSuccess && e->n_rep_classes <= (uint32_t)REPLAY_MAX_CLASSES) er = n_fit.ensure((size_t)Npad * 4);
-    a.left[0] = n_left0.as<int64_t>();
-    a.left[1] = n_left1.as<int64_t>();
-    a.both = n_both.as<uint32_t>();
-    a.nstat = n_stat.as<uint8_t>();
-    a.fitmask = e->n_rep_classes <= (uint32_t)REPLAY_MAX_CLASSES ? n_fit.as<uint32_t>() : nullptr;
-    a.rsel = e->d_rsel.as<uint64_t>();
-    a.rtol = e->d_rtol.as<uint64_t>();
-    a.raff = e->d_raff.as<uint32_t>();
-    a.n_rep = e->n_rep_classes;
-    {
-      // block cache of the cluster scan (replay.cuh): every running sum must stay below 2^62.
-      // A pod is only assumed where it fits, so a node's `requested` never passes its capacity by
-      // more than one request; only negative requests accumulate without that limit.
-      long double worst = 0;
-      for (uint32_t d = 0; d < L; ++d)
-        worst = std::max(worst, (long double)e->max_alloc[d] + (long double)e->max_requested[d] + (long double)e->max_req[d] +
-                                    (long double)e->neg_req[d] * (long double)n_queue + (long double)e->max_pod_count + n_queue);
-      const bool safe = worst * (long double)std::max(N, 1u) < 4.0e18L;
-      const uint32_t n_blocks = cdiv(N, REPLAY_BLOCK);
-      const uint32_t maxl = replay_maxl(L);
-      a.cache_ok = 0;
-      if (er == cudaSuccess && safe && a.n_rep <= (uint32_t)REPLAY_MAX_CLASSES && n_blocks >= 1 && n_blocks <= (uint32_t)REPLAY_MAX_BLOCKS) {
-        const size_t rows = (size_t)2 * a.n_rep * n_blocks;
-        er = c_sum.ensure(rows * maxl * 8);
-        if (er == cudaSuccess) er = c_max.ensure(rows * maxl * 8);
-        if (er == cudaSuccess) er = c_keys.ensure(rows * 4);
-        a.blk_sum = c_sum.as<int64_t>();
-        a.blk_max = c_max.as<int64_t>();
-        a.blk_keys = c_keys.as<uint32_t>();
-        a.cache_ok = 1;
-      }
-    }
-    a.min_member = e->d_min_member.as<uint32_t>();
-    a.scheduled = e->d_scheduled.as<uint32_t>();
-    a.matched = s_matched.as<uint32_t>();
-    a.gflags = s_gflags.as<uint8_t>();
-    a.grc = s_grc.as<uint32_t>();
-    a.min_res = s_minres.as<int64_t>();
-    a.mrpres = s_mrp.as<uint32_t>();
-    a.G = G;
-    a.queue = queue ? d_queue.as<uint32_t>() : nullptr;
-    a.n_queue = n_queue;
-    a.prefilter = d_pf.as<uint8_t>();
-    a.node = d_node.as<int32_t>();
-    a.ready = d_ready.as<uint8_t>();
-    a.status = d_status.as<int32_t>();
-    if (er == cudaSuccess) {
-      StageTimer tm(e, BS_K_REPLAY, e->s);
-      launch_replay(L, a, e->s);
-      tm.launched();
-      er = cudaGetLastError();
-    }
+  CK(dup(s_req, e->d_requested, (size_t)L * Npad * 8));
+  CK(dup(s_pc, e->d_pod_count, (size_t)Npad * 4));
+  CK(dup(s_rp, e->d_rpres, (size_t)Npad * 4));
+  CK(dup(s_matched, e->d_matched, (size_t)G * 4));
+  CK(dup(s_gflags, e->d_gflags, (size_t)G));
+  CK(dup(s_grc, e->d_group_rep_class, (size_t)G * 4));
+  CK(dup(s_minres, e->d_min_res, (size_t)L * G * 8));
+  CK(dup(s_mrp, e->d_mrpres, (size_t)G * 4));
+  if (queue && n_queue) CK(cudaMemcpyAsync(d_queue.p, queue, (size_t)n_queue * 4, cudaMemcpyHostToDevice, e->s));
+  CK(cudaMemsetAsync(d_status.p, 0, 128, e->s));
+  ReplayArgs a{};
+  a.nt = node_tab(e);
+  a.nt.requested = s_req.as<int64_t>();
+  a.nt.pod_count = s_pc.as<int32_t>();
+  a.nt.req_present = s_rp.as<uint32_t>();
+  a.requested = s_req.as<int64_t>();
+  a.pod_count = s_pc.as<int32_t>();
+  a.req_present = s_rp.as<uint32_t>();
+  a.pt = pod_tab(e);
+  a.left[0] = n_left0.as<int64_t>();
+  a.left[1] = n_left1.as<int64_t>();
+  a.both = n_both.as<uint32_t>();
+  a.nstat = n_stat.as<uint8_t>();
+  a.fitmask = fitmask ? n_fit.as<uint32_t>() : nullptr;
+  a.rsel = e->d_rsel.as<uint64_t>();
+  a.rtol = e->d_rtol.as<uint64_t>();
+  a.raff = e->d_raff.as<uint32_t>();
+  a.n_rep = e->n_rep_classes;
+  a.cache_ok = cache ? 1 : 0;
+  if (cache) {
+    a.blk_sum = c_sum.as<int64_t>();
+    a.blk_max = c_max.as<int64_t>();
+    a.blk_keys = c_keys.as<uint32_t>();
   }
+  a.min_member = e->d_min_member.as<uint32_t>();
+  a.scheduled = e->d_scheduled.as<uint32_t>();
+  a.matched = s_matched.as<uint32_t>();
+  a.gflags = s_gflags.as<uint8_t>();
+  a.grc = s_grc.as<uint32_t>();
+  a.min_res = s_minres.as<int64_t>();
+  a.mrpres = s_mrp.as<uint32_t>();
+  a.G = G;
+  a.queue = queue ? d_queue.as<uint32_t>() : nullptr;
+  a.n_queue = n_queue;
+  a.prefilter = d_pf.as<uint8_t>();
+  a.node = d_node.as<int32_t>();
+  a.ready = d_ready.as<uint8_t>();
+  a.status = d_status.as<int32_t>();
+  {
+    StageTimer tm(e, BS_K_REPLAY, e->s);
+    launch_replay(L, a, e->s);
+    tm.launched();
+    CK(cudaGetLastError());
+  }
+  int32_t status = 0;
   std::vector<uint32_t> grc;
-  auto d2h = [&](void* dst, const DevBuf& src, size_t bytes) {
-    if (er == cudaSuccess && dst && bytes) er = cudaMemcpyAsync(dst, src.p, bytes, cudaMemcpyDeviceToHost, e->s);
+  auto d2h = [&](void* dst, const View& src, size_t bytes) {
+    return dst && bytes ? cudaMemcpyAsync(dst, src.p, bytes, cudaMemcpyDeviceToHost, e->s) : cudaSuccess;
   };
-  d2h(&status, d_status, 4);
-  d2h(out->prefilter, d_pf, n_queue);
-  d2h(out->node, d_node, (size_t)n_queue * 4);
-  d2h(out->ready, d_ready, n_queue);
-  if (er == cudaSuccess && out->node_requested && N)
-    er = cudaMemcpy2DAsync(out->node_requested, (size_t)N * 8, s_req.p, (size_t)Npad * 8, (size_t)N * 8, L,
-                           cudaMemcpyDeviceToHost, e->s);
-  d2h(out->node_pod_count, s_pc, (size_t)N * 4);
-  d2h(out->node_req_present, s_rp, (size_t)N * 4);
-  d2h(out->group_matched, s_matched, (size_t)G * 4);
-  d2h(out->group_flags, s_gflags, (size_t)G);
-  d2h(out->group_min_res, s_minres, (size_t)L * G * 8);
-  d2h(out->group_min_res_present, s_mrp, (size_t)G * 4);
+  CK(d2h(&status, d_status, 4));
+  CK(d2h(out->prefilter, d_pf, n_queue));
+  CK(d2h(out->node, d_node, (size_t)n_queue * 4));
+  CK(d2h(out->ready, d_ready, n_queue));
+  if (out->node_requested && N)
+    CK(cudaMemcpy2DAsync(out->node_requested, (size_t)N * 8, s_req.p, (size_t)Npad * 8, (size_t)N * 8, L,
+                         cudaMemcpyDeviceToHost, e->s));
+  CK(d2h(out->node_pod_count, s_pc, (size_t)N * 4));
+  CK(d2h(out->node_req_present, s_rp, (size_t)N * 4));
+  CK(d2h(out->group_matched, s_matched, (size_t)G * 4));
+  CK(d2h(out->group_flags, s_gflags, (size_t)G));
+  CK(d2h(out->group_min_res, s_minres, (size_t)L * G * 8));
+  CK(d2h(out->group_min_res_present, s_mrp, (size_t)G * 4));
   if (out->group_rep_sel || out->group_rep_tol) {
     grc.resize(Gp);
-    d2h(grc.data(), s_grc, (size_t)G * 4);
+    CK(d2h(grc.data(), s_grc, (size_t)G * 4));
   }
-  if (er == cudaSuccess) er = cudaStreamSynchronize(e->s);
-  CK(er);
-  (void)Gp;
+  CK(cudaStreamSynchronize(e->s));
   if (status) return fail(e, BS_E_REF_PANIC, "bs_replay: findMaxPG would divide by MinMember == 0 (core.go:716)");
   for (uint32_t g = 0; g < G && (out->group_rep_sel || out->group_rep_tol); ++g) {
     const ClassKey& k = e->rep_index.keys[grc[g]];
@@ -2465,7 +2349,7 @@ int bs_peer_init(bs_engine* e, uint32_t rank, uint32_t world, uint32_t words_per
   BS_DEVICE_GUARD(e);
   if (e->peer_attached) return fail(e, BS_E_STATE, "bs_peer_init: detach first");
   const size_t bytes = peer_buf_words(world, words_per_rank) * 4;
-  e->d_gather.release();   // a fresh allocation: the IPC handle names this exact block
+  e->d_gather.reset();   // a fresh allocation: the IPC handle names this exact block
   CK(e->d_gather.ensure(bytes));
   CK(e->d_peer_err.ensure(sizeof(int)));
   CK(cudaMemsetAsync(e->d_gather.p, 0, e->d_gather.cap, e->s));

@@ -171,58 +171,28 @@ __global__ void node_left_kernel(NodeTab t, LaneMap lm, int64_t* __restrict__ le
   left_present[i] = both;
 }
 
-// scatter of changed node rows into the resident node table (bs_update_nodes)
-struct NodeTabMut {
-  int64_t* alloc;
-  int64_t* requested;
-  int32_t* pod_count;
-  uint32_t* alloc_present;
-  uint32_t* req_present;
-  uint64_t* label;
-  uint64_t* taint;
-  uint8_t* flags;
+// scatter of changed rows into a resident table (bs_update_nodes / bs_update_groups): column c has elem[c]-byte
+// elements, [lanes[c]][n] compact in src[c] and [lanes[c]][pitch] in dst[c]; row k goes to row idx[k]
+constexpr int SCATTER_MAX_COLS = 8;
+struct ScatterCols {
+  uint8_t* dst[SCATTER_MAX_COLS];
+  const uint8_t* src[SCATTER_MAX_COLS];
+  uint32_t elem[SCATTER_MAX_COLS], lanes[SCATTER_MAX_COLS];
+  uint32_t n_cols;
 };
-__global__ void node_scatter_kernel(NodeTabMut dst, uint32_t Npad, uint32_t L, NodeTab src /*compact, Npad = n*/,
-                                    const uint32_t* __restrict__ idx, uint32_t n) {
+__global__ void row_scatter_kernel(ScatterCols c, uint32_t pitch, const uint32_t* __restrict__ idx, uint32_t n) {
   const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n) return;
   const uint32_t i = idx[k];
-  for (uint32_t d = 0; d < L; ++d) {
-    dst.alloc[(size_t)d * Npad + i] = src.alloc[(size_t)d * n + k];
-    dst.requested[(size_t)d * Npad + i] = src.requested[(size_t)d * n + k];
-  }
-  dst.pod_count[i] = src.pod_count[k];
-  dst.alloc_present[i] = src.alloc_present[k];
-  dst.req_present[i] = src.req_present[k];
-  dst.label[i] = src.label[k];
-  dst.taint[i] = src.taint[k];
-  dst.flags[i] = src.flags[k];
-}
-
-// scatter of changed group rows into the resident group table (bs_update_groups)
-struct GroupCols {
-  uint32_t* min_member;
-  uint32_t* scheduled;
-  uint32_t* matched;
-  uint8_t* flags;
-  int64_t* min_res;   // [L][pitch]
-  uint32_t* min_res_present;
-  int64_t* creation;
-  uint32_t* name_rank;
-};
-__global__ void group_scatter_kernel(GroupCols dst, uint32_t G, uint32_t L, GroupCols src /*compact, pitch n*/,
-                                     const uint32_t* __restrict__ idx, uint32_t n) {
-  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k >= n) return;
-  const uint32_t g = idx[k];
-  dst.min_member[g] = src.min_member[k];
-  dst.scheduled[g] = src.scheduled[k];
-  dst.matched[g] = src.matched[k];
-  dst.flags[g] = src.flags[k];
-  for (uint32_t d = 0; d < L; ++d) dst.min_res[(size_t)d * G + g] = src.min_res[(size_t)d * n + k];
-  dst.min_res_present[g] = src.min_res_present[k];
-  dst.creation[g] = src.creation[k];
-  dst.name_rank[g] = src.name_rank[k];
+  for (uint32_t j = 0; j < c.n_cols; ++j)
+    for (uint32_t d = 0; d < c.lanes[j]; ++d) {
+      const size_t s = (size_t)d * n + k, t = (size_t)d * pitch + i;
+      switch (c.elem[j]) {
+        case 1: c.dst[j][t] = c.src[j][s]; break;
+        case 4: reinterpret_cast<uint32_t*>(c.dst[j])[t] = reinterpret_cast<const uint32_t*>(c.src[j])[s]; break;
+        default: reinterpret_cast<uint64_t*>(c.dst[j])[t] = reinterpret_cast<const uint64_t*>(c.src[j])[s]; break;
+      }
+    }
 }
 
 // generic singleNodeResource table for one class (bs_node_left): left[L][N], present[N]
