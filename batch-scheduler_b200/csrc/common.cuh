@@ -47,7 +47,7 @@ constexpr int NODE_TILE = 512;                          // nodes per shared-memo
 constexpr int FIT_WARPS = 8;                            // consumer warps (each sweeps PODS_PER_WARP pods)
 constexpr int FIT_THREADS = (FIT_WARPS + 1) * 32;       // + one producer warp that only drives the TMA ring
 constexpr int FIT_MIN_BLOCKS = 2;                       // resident CTAs per SM the fit kernel's launch bounds ask for
-constexpr int PODS_PER_WARP = 4;                        // pods evaluated together per node (ILP)
+constexpr int PODS_PER_WARP = 4;                        // pods per consumer warp (evaluated together per node, except in score mode)
 constexpr int PODS_PER_CTA = FIT_WARPS * PODS_PER_WARP; // 32
 constexpr int TILE_WORDS = NODE_TILE / 32;              // ballot words per tile and pod
 static_assert(TILE_WORDS <= 32 && 32 % TILE_WORDS == 0, "a 32-word bitmap line is a whole number of tiles");
@@ -56,11 +56,10 @@ constexpr int KEY_BITS = 4;                             // log2(TILE_WORDS)
 static_assert((1 << KEY_BITS) == TILE_WORDS, "the best-node key holds a word index of the tile in KEY_BITS bits");
 static_assert(FIT_CAP_LOG2 + KEY_BITS <= 31, "best-node key: score (27 bits) + word index must fit 31 bits");
 constexpr int FIT_STAGES = 2;                           // TMA ring depth (full/empty mbarrier pairs)
-// Score rows are staged in shared memory and leave the SMs as FIT_SEG-node row segments handed to the TMA engine
+static_assert(TILE_WORDS % 4 == 0, "the fit kernel sweeps a tile 4 words at a time");
+// Score rows are staged in shared memory and leave the SMs as NODE_TILE-node row segments handed to the TMA engine
 // (cp.async.bulk shared -> global).
-constexpr int FIT_SEG = 128;                            // nodes per score store segment (one bulk store per pod row)
-static_assert(NODE_TILE % FIT_SEG == 0 && FIT_SEG % 128 == 0, "a tile is a whole number of 128-node-multiple segments");
-constexpr int FIT_NB = 2;                               // score staging slabs (segments) per warp in flight
+constexpr int FIT_NB = 2;                               // score staging slabs (one tile of one row each) per warp in flight
 using ColBits = uint16_t;                               // class bits of the TILE_WORDS nodes a lane owns in one tile
 static_assert(sizeof(ColBits) * 8 == TILE_WORDS, "one class bit per ballot word of a tile");
 

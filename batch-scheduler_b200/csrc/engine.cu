@@ -1000,7 +1000,7 @@ int evaluate_async_locked(bs_engine* e) {
         // way (32 registers: its CTAs share their SMs with the fit CTAs); when the fit kernel is the shorter of the two
         // (a small shard, few nodes) the round waits for the sort, and the build with 16 gathers in flight per thread
         // is the faster one.  Estimate: pairs x the per-pair time of the output mode measured on an H100.
-        const double est_fit_ms = (double)P * (double)e->N * ((e->out_flags & BS_OUT_SCORE) ? 3.0e-9 : 0.9e-9);
+        const double est_fit_ms = (double)P * (double)e->N * ((e->out_flags & BS_OUT_SCORE) ? 2.9e-9 : 0.9e-9);
         const bool lean = est_fit_ms > 0.6;
         const void* fn = lean ? (const void*)queue_sort_kernel<SORT_LEAN_GROUP> : (const void*)queue_sort_kernel<SORT_WIDE_GROUP>;
         CK(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(SORT_THREADS), params, 0, e->s2));

@@ -21,17 +21,22 @@ namespace bsk {
 //   INPUT: the producer lane streams the tiles of the residual table into a FIT_STAGES-deep
 //     shared-memory ring with 1-D TMA bulk copies (cp.async.bulk global->shared, one per lane
 //     row), guarded by full/empty mbarrier pairs; consumers never meet at a CTA-wide barrier.
-//   OUTPUT: score rows do NOT leave through the LSU.  A warp writes the FIT_SEG scores of a
-//     segment for each of its pods into a private staging slab in shared memory (st.shared.u64,
-//     conflict-free) and one lane hands every row segment — FIT_SEG*8 contiguous bytes of one
-//     matrix row — to the TMA engine (cp.async.bulk shared->global, bulk_group completion);
-//     FIT_NB slabs per warp rotate, a slab is refilled once its bulk reads have finished
-//     (cp.async.bulk.wait_group.read).  HBM then sees 1 KB bursts per row instead of 256-byte
-//     pieces of four interleaved rows: on an H100 the store pattern alone takes 2.61 ms instead of
-//     2.73 ms for the 8 GB matrix of the bench workload (profiles/microbench/store_pattern2.cu;
-//     cudaMemset 2.44).
-// A lane owns nodes lane, lane+32, ... of the tile, keeps their `left` in registers and evaluates
-// PODS_PER_WARP pods against them at a time.
+//   OUTPUT: score rows do NOT leave through the LSU.  In score mode a warp sweeps each tile one
+//     pod at a time, writes that pod's NODE_TILE scores into a private staging slab in shared
+//     memory (st.shared.u64, conflict-free) and one lane hands the row segment — NODE_TILE*8 =
+//     4 KB contiguous bytes of one matrix row — to the TMA engine (cp.async.bulk shared->global,
+//     bulk_group completion); FIT_NB slabs per warp rotate, a slab is refilled once its bulk read
+//     has finished (cp.async.bulk.wait_group.read).  On an H100, at the kernel's occupancy of two
+//     CTAs per SM, writing the 8 GB matrix of the bench workload this way takes 2.49 ms, against
+//     2.60 ms for slabs of the same size holding 1 KB pieces of four rows and 2.44 ms for
+//     cudaMemset (profiles/microbench/store_pattern2.cu).  The stores carry an L2 evict_first
+//     policy: nothing in the round reads the matrix back, so its lines need not displace what the
+//     queue sort (beside it on another stream) and the kernel's own inputs keep in L2.  On an H100
+//     at 700 W the hint takes the round from 3.00 to 2.83 ms, gang_fit from 2.93 to 2.78 ms and
+//     the sort from 2.1 to 1.6 ms (profiles/fit_l2_hint_ab_h100.jsonl).
+// A lane owns nodes lane, lane+32, ... of the tile.  The bitmap and decisions-only modes evaluate
+// the warp's PODS_PER_WARP pods against each node's `left` in registers; the score sweep reads a
+// node's `left` from the stage once per pod.
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return (uint32_t)__cvta_generic_to_shared(p);
 }
@@ -66,9 +71,17 @@ __device__ __forceinline__ void tma_bulk_g2s(void* dst_smem, const void* src_gme
       "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar))
       : "memory");
 }
-// shared -> global bulk store (TMA), completion tracked by the issuing thread's bulk async-group
-__device__ __forceinline__ void tma_bulk_s2g(void* dst_gmem, uint32_t src_smem, uint32_t bytes) {
-  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst_gmem), "r"(src_smem), "r"(bytes)
+// L2 policy: lines written under it are the first to be evicted.  volatile: made at each use, so that the
+// compiler does not keep it in two registers across the sweep
+__device__ __forceinline__ uint64_t l2_evict_first() {
+  uint64_t pol;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+  return pol;
+}
+// shared -> global bulk store (TMA) under L2 policy `pol`, completion tracked by the issuing thread's bulk async-group
+__device__ __forceinline__ void tma_bulk_s2g(void* dst_gmem, uint32_t src_smem, uint32_t bytes, uint64_t pol) {
+  asm volatile("cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, %3;" ::"l"(dst_gmem),
+               "r"(src_smem), "r"(bytes), "l"(pol)
                : "memory");
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
@@ -138,37 +151,39 @@ struct FitArgs {
 template <bool NARROW> struct BestT { using type = int64_t; };
 template <> struct BestT<true> { using type = int32_t; };
 
-// One node tile for the PODS_PER_WARP pods of a warp.
+// One node tile for pods R0 .. R0+RN-1 of a warp's PODS_PER_WARP (the score sweep calls it with one pod at a
+// time, the other modes with all of them).
 //   narrow lanes: one 32-bit VIADDMNMX (fused subtract+min) each;
 //   scaled lanes: x = min(left' - req', C) (one VIADDMNMX: the clamp keeps x << k below 2^31), its sign
 //     joins the fit test, x << k (exact original units, or 2^27 = "cannot be the minimum") joins the min;
 //   wide lanes: 64-bit subtract, sign through the high word, low word when the high word is 0.
 // Ballot words go to a per-warp shared-memory slab (one STS per pair, every lane writes the same word);
-// scores go to the warp's staging slab (SCORE) as int64: fit ? m : INT64_MIN.
+// scores go to the warp's staging slab (SCORE, RN == 1: one matrix row segment, node j*32 + lane at slab
+// element j*32 + lane) as int64: fit ? m : INT64_MIN.
 // OUT: what leaves the SMs besides the per-pod results — 0 nothing (decisions only: feasible counts come from a
 // predicated add, no ballot), 1 the fit bitmap, 2 the score matrix (+ the bitmap when its pointer is set).
 enum { FIT_OUT_NONE = 0, FIT_OUT_BITMAP = 1, FIT_OUT_SCORE = 2 };
-template <int LW, int LN, int LS, int OUT, int SEGW /*words of the segment*/>
-__device__ __forceinline__ void fit_seg(const FitArgs& a, const int64_t* __restrict__ tlw,
+template <int LW, int LN, int LS, int OUT, int RN>
+__device__ __forceinline__ void fit_tile(const FitArgs& a, const int64_t* __restrict__ tlw,
                                          const int32_t* __restrict__ tln,
                                          const int64_t (&rqw)[PODS_PER_WARP][LW > 0 ? LW : 1],
                                          const int32_t (&rqn)[PODS_PER_WARP][LN + LS > 0 ? LN + LS : 1],
-                                         const ColBits (&colbits)[PODS_PER_WARP], uint32_t slab /*smem addr*/,
+                                         const ColBits (&colbits)[PODS_PER_WARP], int R0, uint32_t slab /*smem addr*/,
                                          uint32_t* s_words, uint32_t wbase /*tile's first word in the line*/, uint32_t node_base, uint32_t lane,
-                                         int j0 /*first word of the segment*/,
                                          typename BestT<(LN > 0)>::type (&best_s)[PODS_PER_WARP],
                                          int32_t (&best_n)[PODS_PER_WARP], int32_t (&kb)[PODS_PER_WARP],
                                          uint32_t (&cnt)[PODS_PER_WARP]) {
   constexpr bool SCORE = OUT == FIT_OUT_SCORE;
   constexpr bool WORDS = OUT != FIT_OUT_NONE;
-  const int64_t* tpw = tlw + lane + j0 * 32;
-  const int32_t* tpn = tln + lane + j0 * 32;
-  int32_t node = (int32_t)(node_base + lane) + j0 * 32;
-  uint32_t wp = smem_u32(s_words) + (wbase + j0) * 4;   // word (wbase + j) of the 32-word line being assembled
+  static_assert(!SCORE || RN == 1, "a staging slab holds one matrix row");
+  const int64_t* tpw = tlw + lane;
+  const int32_t* tpn = tln + lane;
+  int32_t node = (int32_t)(node_base + lane);
+  uint32_t wp = smem_u32(s_words) + wbase * 4;   // word (wbase + j) of the 32-word line being assembled
   uint32_t sp = slab + lane * 8;
-  int32_t jrem = TILE_WORDS - 1 - j0;   // best-node key: low KEY_BITS bits = TILE_WORDS-1-j (earlier node wins a tie)
+  int32_t jrem = TILE_WORDS - 1;   // best-node key: low KEY_BITS bits = TILE_WORDS-1-j (earlier node wins a tie)
 #pragma unroll 1
-  for (int jb = j0; jb < j0 + SEGW; jb += 4) {
+  for (int jb = 0; jb < TILE_WORDS; jb += 4) {
 #pragma unroll
     for (int jj = 0; jj < 4; ++jj) {
       int64_t lfw[LW > 0 ? LW : 1];
@@ -178,7 +193,8 @@ __device__ __forceinline__ void fit_seg(const FitArgs& a, const int64_t* __restr
 #pragma unroll
       for (int d = 0; d < LN + LS; ++d) lfn[d] = tpn[d * NODE_TILE + jj * 32];
 #pragma unroll
-      for (int r = 0; r < PODS_PER_WARP; ++r) {
+      for (int i = 0; i < RN; ++i) {
+        const int r = R0 + i;
         if (LN > 0) {
           // Narrow fast path.  t = min over the narrow lanes is a REAL difference (the narrow set
           // holds a fixed lane) with |t| < 2^27, and the pair's score m = min over all lanes <= t.
@@ -209,7 +225,7 @@ __device__ __forceinline__ void fit_seg(const FitArgs& a, const int64_t* __restr
           // (scores of fitting pairs are < 2^27), -1 = none; decoded once per tile
           const int32_t key = (int32_t)(m32 << KEY_BITS) + (jrem - jj);
           if (fit) kb[r] = max(kb[r], key);
-          if (SCORE) sts_v2u32(sp + (r * FIT_SEG + jj * 32) * 8, fit ? m32 : 0u, fit ? 0u : 0x80000000u);
+          if (SCORE) sts_v2u32(sp + jj * 32 * 8, fit ? m32 : 0u, fit ? 0u : 0x80000000u);
         } else {
           int64_t m = lfw[0] - rqw[r][0];
 #pragma unroll
@@ -218,7 +234,7 @@ __device__ __forceinline__ void fit_seg(const FitArgs& a, const int64_t* __restr
           if (WORDS) sts_u32(wp + (r * 32 + jj) * 4, __ballot_sync(0xffffffffu, fit));
           else if (fit) ++cnt[r];
           if (fit && m > best_s[r]) { best_s[r] = m; best_n[r] = node + jj * 32; }
-          if (SCORE) sts_u64(sp + (r * FIT_SEG + jj * 32) * 8, fit ? (long long)m : (long long)INT64_MIN);
+          if (SCORE) sts_u64(sp + jj * 32 * 8, fit ? (long long)m : (long long)INT64_MIN);
         }
       }
     }
@@ -234,7 +250,7 @@ __device__ __forceinline__ void fit_seg(const FitArgs& a, const int64_t* __restr
 __host__ __device__ constexpr size_t fit_tile_bytes(int LW, int LN, int LS) {
   return (size_t)NODE_TILE * (8 * LW + 4 * (LN + LS));
 }
-__host__ __device__ constexpr size_t fit_slab_bytes() { return (size_t)PODS_PER_WARP * FIT_SEG * 8; }
+__host__ __device__ constexpr size_t fit_slab_bytes() { return (size_t)NODE_TILE * 8; }   // one tile of one score row
 // shared-memory layout: [stages]{[LW][NODE_TILE] i64, [LN+LS][NODE_TILE] i32} | req_w | req_n | mbarriers |
 //                       ballot words | (SCORE) [FIT_WARPS][FIT_NB] staging slabs, 128-byte aligned
 __host__ __device__ constexpr size_t fit_smem_front(int LW, int LN, int LS) {
@@ -377,36 +393,36 @@ __global__ void __launch_bounds__(FIT_THREADS, FIT_MIN_BLOCKS) gang_fit_kernel(F
     const int32_t* tln = reinterpret_cast<const int32_t*>(s_tile + stage * STAGE_BYTES + (size_t)LW * NODE_TILE * 8);
     const uint32_t node_base = tile * NODE_TILE;
     const uint32_t wbase = (tile % TILES_PER_LINE) * TILE_WORDS;
-    // staged scores: the tile in store segments of FIT_SEG nodes, each goes to the next of the warp's FIT_NB staging
-    // slabs and leaves as PODS_PER_WARP bulk stores (one per matrix row) while the following segment is computed;
-    // nothing to stage: the tile in one piece
-    constexpr int SEG_NODES = SCORE ? FIT_SEG : NODE_TILE;
-#pragma unroll 1
-    for (int sg = 0; sg < NODE_TILE / SEG_NODES; ++sg) {
-      const uint32_t slab = slab0 + sb * (uint32_t)fit_slab_bytes();
-      if (SCORE && nseg >= (uint32_t)FIT_NB) {
-        if (lane == 0) bulk_wait_read<FIT_NB - 1>();   // the bulk stores that last read this slab are done with it
-        __syncwarp();
-      }
-      fit_seg<LW, LN, LS, OUT, SEG_NODES / 32>(a, tlw, tln, rqw, rqn, colbits, slab, s_words, wbase, node_base, lane,
-                                               sg * (SEG_NODES / 32), best_s, best_n, kb, cnt);
-      if (SCORE) {
+    if constexpr (SCORE) {
+      // staged scores, one pod at a time: the pod's row of the tile goes to the next of the warp's FIT_NB staging
+      // slabs and leaves as one NODE_TILE*8-byte bulk store while the next pod is computed.  Each node's `left` is
+      // read from the stage once per pod instead of once per warp, for row segments 4x as long as a 4-row slab of
+      // the same size would give.
+#pragma unroll
+      for (int r = 0; r < PODS_PER_WARP; ++r) {
+        const uint32_t slab = slab0 + sb * (uint32_t)fit_slab_bytes();
+        if (nseg >= (uint32_t)FIT_NB) {
+          if (lane == 0) bulk_wait_read<FIT_NB - 1>();   // the bulk store that last read this slab is done with it
+          __syncwarp();
+        }
+        fit_tile<LW, LN, LS, OUT, 1>(a, tlw, tln, rqw, rqn, colbits, r, slab, s_words, wbase, node_base, lane, best_s,
+                                     best_n, kb, cnt);
         fence_async_smem();
         __syncwarp();
         if (lane == 0) {
-          // row segments: FIT_SEG scores, or what is left of the row (pitch is even: 16-byte sizes)
-          const uint32_t col0 = node_base + sg * FIT_SEG;
-          if (col0 < (uint32_t)a.score_pitch) {
-            const uint32_t cols = min((uint32_t)FIT_SEG, (uint32_t)a.score_pitch - col0);
-#pragma unroll
-            for (int r = 0; r < PODS_PER_WARP; ++r)
-              tma_bulk_s2g(srow + (size_t)r * a.score_pitch + col0, slab + r * (FIT_SEG * 8), cols * 8);
+          // the tile's scores, or what is left of the row (pitch is even: 16-byte sizes)
+          if (node_base < (uint32_t)a.score_pitch) {
+            const uint32_t cols = min((uint32_t)NODE_TILE, (uint32_t)a.score_pitch - node_base);
+            tma_bulk_s2g(srow + (size_t)r * a.score_pitch + node_base, slab, cols * 8, l2_evict_first());
           }
           bulk_commit();
         }
         ++nseg;
         if (++sb == FIT_NB) sb = 0;
       }
+    } else {
+      fit_tile<LW, LN, LS, OUT, PODS_PER_WARP>(a, tlw, tln, rqw, rqn, colbits, 0, 0, s_words, wbase, node_base, lane,
+                                               best_s, best_n, kb, cnt);
     }
     if (LN > 0) {
       // a tile's best key beats the running best iff key >= (best_s + 1) << KEY_BITS: strictly greater score

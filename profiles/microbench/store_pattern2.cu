@@ -11,8 +11,11 @@
 //                 all 32 bulk stores (larger bursts per issue, one bar.sync per tile)
 //
 // build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o store_pattern2 store_pattern2.cu
+// run:   ./store_pattern2        every variant at its own shared-memory size
+//        ./store_pattern2 occ2   the 4 KB-slab TMA shapes padded to the fit kernel's shared memory, alternated
 #include <cstdio>
 #include <cstdint>
+#include <cstring>
 #include <cuda_runtime.h>
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -141,9 +144,10 @@ static void rep(const char* name, float ms) {
   printf(" %-28s %.3f ms  %.0f GB/s  %s\n", name, ms, (double)P * N * 8 / ms / 1e6, e == cudaSuccess ? "" : cudaGetErrorString(e));
 }
 
+// smem_pad > 0: ask for that much dynamic shared memory instead of the slabs' own size (occupancy of another kernel)
 template <int R, int T, int NB, int WARPS>
-void run_tma(const char* name) {
-  const size_t smem = (size_t)WARPS * NB * R * T * 8;
+void run_tma(const char* name, size_t smem_pad = 0) {
+  const size_t smem = smem_pad ? smem_pad : (size_t)WARPS * NB * R * T * 8;
   cudaFuncSetAttribute(tma<R, T, NB, WARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   int occ = 0;
   cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, tma<R, T, NB, WARPS>, WARPS * 32, smem);
@@ -177,9 +181,23 @@ void run_tmacta(const char* name) {
   rep(buf, ms);
 }
 
-int main() {
+int main(int argc, char** argv) {
   const size_t n = (size_t)P * N;
   cudaMalloc(&d, n * 8 + (1 << 20));
+  if (argc > 1 && !strcmp(argv[1], "occ2")) {
+    // the three 4 KB-slab shapes at the score-mode fit kernel's shared memory (cfg4 lanes: 90880 B, 2 CTAs per SM),
+    // alternated so that drift over the run hits each alike
+    constexpr size_t FIT_SMEM = 90880;
+    for (int k = 0; k < 3; ++k) {
+      run_tma<4, 128, 2, 8>("tma R4 T128 NB2 W8 pad", FIT_SMEM);
+      run_tma<1, 512, 2, 8>("tma R1 T512 NB2 W8 pad", FIT_SMEM);
+      run_tma<2, 256, 2, 8>("tma R2 T256 NB2 W8 pad", FIT_SMEM);
+    }
+    rep("memset", timeit([&] { cudaMemsetAsync(d, 1, n * 8); }));
+    cudaError_t e = cudaDeviceSynchronize();
+    printf("status: %s\n", cudaGetErrorString(e));
+    return 0;
+  }
   rep("fill", timeit([&] { fill<<<132 * 8, 256>>>(d, n); }));
   rep("memset", timeit([&] { cudaMemsetAsync(d, 1, n * 8); }));
   rep("rows<4> (round-1 pattern)", timeit([&] { rows<4><<<(P + 31) / 32, 256>>>(d, P, N); }));

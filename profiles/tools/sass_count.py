@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Counts the SASS instructions of gang_fit_kernel's hot loop (the innermost loop that holds the VOTE
-instructions: one trip = 4 nodes per lane x PODS_PER_WARP pods) and writes profiles/sass_ops_r2.json, the
+instructions: one trip = 4 nodes per lane x --ppw pods) and writes profiles/sass_ops_r2.json, the
 op counts behind the decisions-only instruction roofline in bench.py (SURVEY 8(d) R2).
 
     python profiles/tools/sass_count.py [--lib batch-scheduler_b200/libbsched.so] [--kernel ILi0ELi3ELi2ELi0E]
@@ -40,7 +40,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--lib", default=os.path.join(ROOT, "batch-scheduler_b200", "libbsched.so"))
     ap.add_argument("--kernel", default="ILi0ELi3ELi2ELi0E", help="substring of the mangled gang_fit_kernel instance")
-    ap.add_argument("--ppw", type=int, default=4)
+    ap.add_argument("--ppw", type=int, default=4, help="pods per trip of the loop: 4 (PODS_PER_WARP), 1 for a score-mode kernel")
     ap.add_argument("--marks-per-pair", type=int, default=4, help="VIADDMNMX per pair: (LN - 1) + LS, 4 for the bench shape (0,3,2)")
     ap.add_argument("--dump", default=None)
     ap.add_argument("--out", default=os.path.join(ROOT, "profiles", "sass_ops_r2.json"))
@@ -86,7 +86,7 @@ def main():
     if best is None:
         sys.exit("no loop with the lane arithmetic found")
     lo, hi, inside, marks = best
-    pairs = 4 * a.ppw      # one trip = 4 nodes per lane x PODS_PER_WARP pods (the 4-word unrolled body)
+    pairs = 4 * a.ppw      # one trip = 4 nodes per lane x --ppw pods (the 4-word unrolled body)
     by_class, by_mn = {}, {}
     for addr, mn, t in inside:
         c = classify(mn)
@@ -98,9 +98,10 @@ def main():
            "alu_pipe_ops_per_pair": by_class.get("alu", 0) / pairs, "fma_pipe_ops_per_pair": by_class.get("fma", 0) / pairs,
            "lsu_ops_per_pair": by_class.get("lsu", 0) / pairs, "by_class": by_class,
            "by_mnemonic": dict(sorted(by_mn.items(), key=lambda kv: -kv[1])),
-           "note": "static count of the innermost loop that holds the lane arithmetic; with FIT_SEG = 128 nodes the 4-word "
-                   "compute loop is fully unrolled into the segment loop, so the count INCLUDES the per-segment staging overhead "
-                   "(fence, bulk-store issue) in score mode; per-tile / per-sweep instructions outside it are not counted"}
+           "note": "static count of the innermost loop that holds the lane arithmetic (one trip = 4 nodes per lane x "
+                   "pods_per_trip / 4 pods: all PODS_PER_WARP pods in the bitmap and decisions-only modes, one pod in score "
+                   "mode, --ppw 1); per-tile instructions outside it are not counted, and in score mode neither is the "
+                   "per-slab staging (fence, bulk-store issue, once per pod and tile)"}
     with open(a.out, "w") as f:
         json.dump(out, f, indent=1)
     print(json.dumps({k: out[k] for k in ("kernel", "instructions_in_loop", "pairs_per_trip", "issue_ops_per_pair",
