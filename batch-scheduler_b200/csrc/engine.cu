@@ -211,34 +211,129 @@ inline int host_threads() {
   return n;
 }
 
-// out[i] = id of key_of(i) in `global` (ids stable across calls: the index only grows).
-// Two parallel passes: thread-local indices, a small sequential merge, then a remap.
-template <class KeyFn>
-void assign_classes(ClassIndex& global, uint32_t n, KeyFn key_of, uint32_t* out) {
-  if (global.slots.empty()) global.clear();
-  const int T = n < 8192 ? 1 : host_threads();
-  // T fixed CHUNKS, not T threads: num_threads(T) is only a request (OMP_THREAD_LIMIT, OMP_DYNAMIC, a failed
-  // thread creation give a smaller team), so the chunks are shared out with an omp for
-  std::vector<ClassIndex> local(T);
-  std::vector<std::vector<uint32_t>> remap(T);
-  const uint32_t chunk = (n + T - 1) / T;
-#pragma omp parallel for schedule(static, 1) num_threads(T)
-  for (int t = 0; t < T; ++t) {
-    ClassIndex& li = local[t];
-    li.clear();
-    const uint32_t a = std::min(n, (uint32_t)t * chunk), b = std::min(n, a + chunk);
-    for (uint32_t i = a; i < b; ++i) out[i] = li.get_or_add(key_of(i));
+// The rows [0, n) of a host pass cut into T fixed chunks: one chunk below `serial_below` rows, else host_threads().
+// T fixed CHUNKS, not T threads: num_threads(T) is only a request (OMP_THREAD_LIMIT, OMP_DYNAMIC, a failed thread
+// creation give a smaller team), so the chunks are shared out with an omp for and a smaller team still covers them.
+struct Chunks {
+  uint32_t n;
+  int T;
+  Chunks(uint32_t n_, uint32_t serial_below) : n(n_), T(n_ < serial_below ? 1 : host_threads()) {}
+  // body(chunk, first row, end row) for every chunk
+  template <class F>
+  void run(F body) const {
+    const uint32_t chunk = (n + T - 1) / T;
+#pragma omp parallel for schedule(static, 1) num_threads(T) if (T > 1)
+    for (int t = 0; t < T; ++t) {
+      const uint32_t a = std::min(n, (uint32_t)t * chunk);
+      body(t, a, std::min(n, a + chunk));
+    }
   }
-  for (int t = 0; t < T; ++t) {
+  // body(chunk, first row, end row, the chunk's statistics) for every chunk; returns the chunks' statistics merged
+  template <class S, class F>
+  S reduce(F body) const {
+    std::vector<S> part(T);
+    run([&](int t, uint32_t a, uint32_t b) { body(t, a, b, part[t]); });
+    S r;
+    for (const S& s : part) r.merge(s);
+    return r;
+  }
+};
+
+// What the node pass (node_host_pass) gathers: |value| maxima of alloc / requested (range check + lane classification,
+// wide / narrow), max |pod_count|, and per lane the OR and max |value| of the residual at percent 1.0
+// (singleNodeResource, core.go:647-668; the OR's trailing zeros are the power of two every residual is a multiple of:
+// scaled lanes).  A row update only widens them (a conservative bound keeps the lane split exact; more OR bits give a
+// smaller unit, still exact).
+struct NodeStats {
+  int64_t max_alloc[BS_MAX_LANES] = {}, max_requested[BS_MAX_LANES] = {}, max_left[BS_MAX_LANES] = {};
+  uint64_t or_left[BS_MAX_LANES] = {};
+  int64_t max_pod_count = 0;
+  bool bad_range = false;   // an alloc / requested value outside +-2^56
+  void merge(const NodeStats& o) {
+    for (uint32_t d = 0; d < BS_MAX_LANES; ++d) {
+      max_alloc[d] = std::max(max_alloc[d], o.max_alloc[d]);
+      max_requested[d] = std::max(max_requested[d], o.max_requested[d]);
+      max_left[d] = std::max(max_left[d], o.max_left[d]);
+      or_left[d] |= o.or_left[d];
+    }
+    max_pod_count = std::max(max_pod_count, o.max_pod_count);
+    bad_range = bad_range || o.bad_range;
+  }
+};
+
+// What the group pass (group_host_pass) gathers: the OR / AND of the two sort-key words (creation_ns, ~name_rank) and
+// the checks.  A row update widens the OR / AND: a superset of the varying bits costs a radix pass, never an error.
+struct GroupStats {
+  uint64_t or_creation = 0, and_creation = ~0ull, or_name = 0, and_name = ~0ull;
+  bool bad_range = false;      // a min_res value outside +-2^56
+  bool bad_creation = false;   // creation_ns == INT64_MAX
+  bool reps_differ = false;    // the representative columns differ from the engine's
+  void merge(const GroupStats& o) {
+    or_creation |= o.or_creation; and_creation &= o.and_creation;
+    or_name |= o.or_name; and_name &= o.and_name;
+    bad_range = bad_range || o.bad_range;
+    bad_creation = bad_creation || o.bad_creation;
+    reps_differ = reps_differ || o.reps_differ;
+  }
+  // bits that differ between rows of each sort-key word (a constant byte needs no radix pass); AND is a subset of OR
+  // once a row was seen, so OR & ~AND is OR ^ AND there and 0 for an empty table
+  uint64_t vary_creation() const { return or_creation & ~and_creation; }
+  uint64_t vary_name() const { return or_name & ~and_name; }
+};
+
+// What the pod pass gathers: per lane max |req| and the largest negative request (0 when none; the replay's
+// overflow bound), the OR of every request (scaled lanes), the OR / AND of the sort-key columns, whether a pod sorts
+// as ungrouped (lister miss or gid < BS_GID_NONE) and the largest gid.
+struct PodStats {
+  int64_t max_req[BS_MAX_LANES] = {}, neg_req[BS_MAX_LANES] = {};
+  uint64_t or_req[BS_MAX_LANES] = {};
+  uint64_t or_ts = 0, and_ts = ~0ull;
+  uint32_t or_prio = 0, and_prio = ~0u;
+  bool lister_miss = false;
+  int32_t max_gid = -1;
+  bool bad_range = false;   // a request outside +-2^56
+  void merge(const PodStats& o) {
+    for (uint32_t d = 0; d < BS_MAX_LANES; ++d) {
+      max_req[d] = std::max(max_req[d], o.max_req[d]);
+      neg_req[d] = std::max(neg_req[d], o.neg_req[d]);
+      or_req[d] |= o.or_req[d];
+    }
+    or_ts |= o.or_ts; and_ts &= o.and_ts;
+    or_prio |= o.or_prio; and_prio &= o.and_prio;
+    lister_miss = lister_miss || o.lister_miss;
+    max_gid = std::max(max_gid, o.max_gid);
+    bad_range = bad_range || o.bad_range;
+  }
+  uint64_t vary_ts() const { return or_ts & ~and_ts; }   // as GroupStats::vary_creation
+  uint64_t vary_prio() const { return or_prio & ~and_prio; }
+};
+
+// Merges the chunks' thread-local class indices into `global` (ids of known classes are stable: the index only
+// grows), then rewrites every ids[i], an id in the local index of row i's chunk, as its id in `global`.
+void merge_classes(ClassIndex& global, const std::vector<ClassIndex>& local, const Chunks& ch, uint32_t* ids) {
+  std::vector<std::vector<uint32_t>> remap(local.size());
+  for (size_t t = 0; t < local.size(); ++t) {
     remap[t].resize(local[t].size());
     for (size_t j = 0; j < local[t].size(); ++j) remap[t][j] = global.get_or_add(local[t].keys[j]);
   }
-#pragma omp parallel for schedule(static, 1) num_threads(T)
-  for (int t = 0; t < T; ++t) {
-    const uint32_t a = std::min(n, (uint32_t)t * chunk), b = std::min(n, a + chunk);
+  ch.run([&](int t, uint32_t a, uint32_t b) {
     const uint32_t* rm = remap[t].data();
-    for (uint32_t i = a; i < b; ++i) out[i] = rm[out[i]];
-  }
+    for (uint32_t i = a; i < b; ++i) ids[i] = rm[ids[i]];
+  });
+}
+
+// out[i] = id of key_of(i) in `global`: thread-local indices in parallel, then merge_classes.
+template <class KeyFn>
+void assign_classes(ClassIndex& global, uint32_t n, KeyFn key_of, uint32_t* out) {
+  if (global.slots.empty()) global.clear();
+  const Chunks ch(n, 8192);
+  std::vector<ClassIndex> local(ch.T);
+  ch.run([&](int t, uint32_t a, uint32_t b) {
+    ClassIndex& li = local[t];
+    li.clear();
+    for (uint32_t i = a; i < b; ++i) out[i] = li.get_or_add(key_of(i));
+  });
+  merge_classes(global, local, ch, out);
 }
 
 }  // namespace
@@ -262,14 +357,10 @@ struct bs_engine {
   DevBuf d_left_w, d_left_n, d_left_present, d_classfit, d_left_plain, d_filter_bitmap;
   LaneMap lane_map{};
   bool lane_map_valid = false;
-  // per-lane maxima of |value| (lane classification wide / narrow)
-  int64_t max_alloc[BS_MAX_LANES] = {}, max_requested[BS_MAX_LANES] = {}, max_req[BS_MAX_LANES] = {};
-  int64_t max_pod_count = 0;
-  int64_t neg_req[BS_MAX_LANES] = {};   // largest negative request per lane (0 when none)
-  // scaled-lane classification: OR of every residual (percent 1.0) / request value of a lane (its
-  // trailing zeros = the power of two every value is a multiple of) and max |residual|
-  uint64_t or_left[BS_MAX_LANES] = {}, or_req[BS_MAX_LANES] = {};
-  int64_t max_left[BS_MAX_LANES] = {};
+  // statistics of the tables as uploaded, widened by row updates (lane classification, sort passes, replay bound)
+  NodeStats node_stats;
+  GroupStats group_stats;
+  PodStats pod_stats;
   uint32_t score_pitch = 0;             // elements per score row: N rounded up to even
   uint32_t bitmap_pitch = 0;            // words per fit-bitmap row: ceil(N/32) rounded up to 32 (whole 128-byte lines)
   // pod table
@@ -319,11 +410,6 @@ struct bs_engine {
   bool group_ids_dirty = false;      // some ids in h_grc changed in place (bs_update_groups): DMA them again
   std::vector<int64_t> h_wait_ns;
   int64_t default_wait_ns = 0;
-  // bits that differ between rows of each sort key word (a constant byte needs no radix pass)
-  bool any_lister_miss = true;
-  int32_t max_gid = -1;
-  uint64_t vary_ts = ~0ull, vary_prio = ~0ull, vary_creation = ~0ull, vary_name = ~0ull;
-  uint64_t g_or1 = 0, g_and1 = ~0ull, g_or0 = 0, g_and0 = ~0ull;   // OR / AND of the group key words seen so far
   bool pod_classes_dirty = true;
   double last_classes_us = 0;
   // BS_HOST_PROFILE: host-side segment times (label, us) since the last bs_evaluate, printed there
@@ -376,24 +462,9 @@ int fail(bs_engine* e, int code, const char* msg) {
   return code;
 }
 
-// Everything bs_upload_nodes / bs_update_nodes need from the host columns in ONE chunked pass (an omp team
-// for big tables): |value| maxima of alloc / requested (range check + lane classification), max |pod_count|,
-// and per lane the OR and max |value| of the residual at percent 1.0 (singleNodeResource, core.go:647-668;
-// the OR gives the common power-of-two factor).
-struct NodeHostStats {
-  int64_t mx_a[BS_MAX_LANES] = {}, mx_r[BS_MAX_LANES] = {}, mx_l[BS_MAX_LANES] = {};
-  uint64_t or_l[BS_MAX_LANES] = {};
-  int64_t mx_pc = 0;
-  bool ok = true;
-};
-NodeHostStats node_host_pass(const bs_node_table* t, uint32_t L, uint32_t N) {
-  const int T = N < 4096 ? 1 : host_threads();
-  std::vector<NodeHostStats> part(T);
-  const uint32_t chunk = (N + T - 1) / std::max(T, 1);
-#pragma omp parallel for schedule(static, 1) num_threads(T) if (T > 1)
-  for (int tk = 0; tk < T; ++tk) {
-    NodeHostStats st;
-    const uint32_t a0 = std::min(N, (uint32_t)tk * chunk), a1 = std::min(N, a0 + chunk);
+// Everything bs_upload_nodes / bs_update_nodes need from the N rows of host columns, in ONE chunked pass.
+NodeStats node_host_pass(const bs_node_table* t, uint32_t L, uint32_t N) {
+  return Chunks(N, 4096).reduce<NodeStats>([&](int, uint32_t a0, uint32_t a1, NodeStats& st) {
     for (uint32_t d = 0; d < L; ++d) {
       const int64_t* al = t->alloc + (size_t)d * N;
       const int64_t* rq = t->requested + (size_t)d * N;
@@ -412,29 +483,49 @@ NodeHostStats node_host_pass(const bs_node_table* t, uint32_t L, uint32_t N) {
         o |= (uint64_t)v;
         mx = std::max(mx, v < 0 ? -v : v);
       }
-      st.ok = st.ok && alo >= -BS_VALUE_LIMIT && ahi <= BS_VALUE_LIMIT && rlo >= -BS_VALUE_LIMIT && rhi <= BS_VALUE_LIMIT;
-      st.mx_a[d] = std::max(ahi, alo == INT64_MIN ? INT64_MAX : -alo);
-      st.mx_r[d] = std::max(rhi, rlo == INT64_MIN ? INT64_MAX : -rlo);
-      st.or_l[d] = o;
-      st.mx_l[d] = mx;
+      st.bad_range = st.bad_range || alo < -BS_VALUE_LIMIT || ahi > BS_VALUE_LIMIT || rlo < -BS_VALUE_LIMIT ||
+                     rhi > BS_VALUE_LIMIT;
+      st.max_alloc[d] = std::max(ahi, alo == INT64_MIN ? INT64_MAX : -alo);
+      st.max_requested[d] = std::max(rhi, rlo == INT64_MIN ? INT64_MAX : -rlo);
+      st.or_left[d] = o;
+      st.max_left[d] = mx;
     }
     int64_t pc = 0;
     for (uint32_t i = a0; i < a1; ++i) pc = std::max<int64_t>(pc, std::abs((int64_t)t->pod_count[i]));
-    st.mx_pc = pc;
-    part[tk] = st;
-  }
-  NodeHostStats r;
-  for (int tk = 0; tk < T; ++tk) {
-    r.ok = r.ok && part[tk].ok;
-    r.mx_pc = std::max(r.mx_pc, part[tk].mx_pc);
+    st.max_pod_count = pc;
+  });
+}
+
+// Everything bs_upload_groups / bs_update_groups need from the n rows of host columns, in ONE chunked pass: the
+// |min_res| range, the creation sentinel, the OR / AND of the sort-key words and, with `reps` (an engine whose
+// representative columns have n rows), whether the table's representative columns differ from that engine's.
+GroupStats group_host_pass(const bs_group_table* t, uint32_t L, uint32_t n, const bs_engine* reps) {
+  return Chunks(n, 8192).reduce<GroupStats>([&](int, uint32_t g0, uint32_t g1, GroupStats& st) {
     for (uint32_t d = 0; d < L; ++d) {
-      r.mx_a[d] = std::max(r.mx_a[d], part[tk].mx_a[d]);
-      r.mx_r[d] = std::max(r.mx_r[d], part[tk].mx_r[d]);
-      r.mx_l[d] = std::max(r.mx_l[d], part[tk].mx_l[d]);
-      r.or_l[d] |= part[tk].or_l[d];
+      const int64_t* row = t->min_res + (size_t)d * n;
+      int64_t lo = 0, hi = 0;
+      for (uint32_t g = g0; g < g1; ++g) { lo = std::min(lo, row[g]); hi = std::max(hi, row[g]); }
+      st.bad_range = st.bad_range || lo < -BS_VALUE_LIMIT || hi > BS_VALUE_LIMIT;
     }
-  }
-  return r;
+    uint64_t lo1 = 0, la1 = ~0ull, lo0 = 0, la0 = ~0ull;
+    bool bc = false;
+    for (uint32_t g = g0; g < g1; ++g) {
+      const uint64_t c = (uint64_t)t->creation_ns[g], nm = (uint64_t)(~t->name_rank[g]);
+      lo1 |= c; la1 &= c; lo0 |= nm; la0 &= nm;
+      bc = bc || t->creation_ns[g] == INT64_MAX;
+    }
+    st.or_creation = lo1; st.and_creation = la1; st.or_name = lo0; st.and_name = la0; st.bad_creation = bc;
+    if (reps && g1 > g0) {
+      const size_t k = g1 - g0;
+      bool df = memcmp(reps->h_gsel.data() + g0, t->rep_sel + g0, k * 8) != 0 ||
+                memcmp(reps->h_gtol.data() + g0, t->rep_tol + g0, k * 8) != 0;
+      const uint32_t* ha = reps->h_gaff.data();
+      if (t->rep_aff_class) df = df || memcmp(ha + g0, t->rep_aff_class + g0, k * 4) != 0;
+      else
+        for (uint32_t g = g0; g < g1 && !df; ++g) df = ha[g] != BS_AFF_NONE;
+      st.reps_differ = df;
+    }
+  });
 }
 
 // Lane classification for the fit kernel (kernels.cuh "Narrow lanes"): lane d is narrow when every
@@ -683,12 +774,14 @@ LaneMap classify_lanes(const bs_engine* e) {
   uint32_t unit[BS_MAX_LANES] = {};
   bool fixed_narrow = false;
   uint32_t ln = 0, ls = 0;
+  const NodeStats& ns = e->node_stats;
+  const PodStats& ps = e->pod_stats;
   for (uint32_t d = 0; d < L; ++d) {
     // |left| <= |scale(alloc)| + |requested| (pods lane: + len(Pods())); float32 rounding of a
     // value <= 2^26 is exact, so the bound 2^26 + 2^26 = 2^27 holds.
-    int64_t used = e->max_requested[d];
-    if (d == LANE_PODS) used = std::max(used, e->max_pod_count);
-    const bool narrow = e->max_alloc[d] <= (NARROW_LIMIT >> 1) && used <= (NARROW_LIMIT >> 1) && e->max_req[d] <= NARROW_LIMIT;
+    int64_t used = ns.max_requested[d];
+    if (d == LANE_PODS) used = std::max(used, ns.max_pod_count);
+    const bool narrow = ns.max_alloc[d] <= (NARROW_LIMIT >> 1) && used <= (NARROW_LIMIT >> 1) && ps.max_req[d] <= NARROW_LIMIT;
     kind[d] = narrow ? NARROW : WIDE;
     if (narrow) {
       ++ln;
@@ -697,8 +790,8 @@ LaneMap classify_lanes(const bs_engine* e) {
     }
     // scaled: every residual and every request of the lane is a multiple of 2^k (k from the OR of all
     // values seen at upload) and fits 2^29 in those units; the smallest such k is taken
-    const uint32_t k_avail = std::min(ctz64(e->or_left[d]), ctz64(e->or_req[d]));
-    const int64_t mx = std::max(e->max_left[d], e->max_req[d]);
+    const uint32_t k_avail = std::min(ctz64(ns.or_left[d]), ctz64(ps.or_req[d]));
+    const int64_t mx = std::max(ns.max_left[d], ps.max_req[d]);
     uint32_t k_need = 0;
     while (k_need < 63 && (mx >> k_need) > SCALED_LIMIT) ++k_need;
     if (k_need <= k_avail) {
@@ -981,11 +1074,12 @@ int evaluate_async_locked(bs_engine* e) {
       sa.tilecnt = e->d_tilecnt.as<uint32_t>();
       sa.barrier = e->d_sort_barrier.as<unsigned int>();
       sa.ntiles_max = cdiv(std::max(std::max(P, G), 1u), SORT_TILE);
-      sa.n_gpass = build_passes(e->vary_name, e->vary_creation, sa.gpass);
+      sa.n_gpass = build_passes(e->group_stats.vary_name(), e->group_stats.vary_creation(), sa.gpass);
       // word1 = [~biased prio : 32][grouped : 1][group rank or 0x7fffffff : 31]
-      const uint64_t vary1 = (e->vary_prio << 32) | 0x80000000ull |
-                             ((e->any_lister_miss || e->max_gid >= (int64_t)G) ? 0x7fffffffull : low_bits_mask(G));
-      sa.n_ppass = build_passes(e->vary_ts, vary1, sa.ppass);
+      const PodStats& ps = e->pod_stats;
+      const uint64_t vary1 = (ps.vary_prio() << 32) | 0x80000000ull |
+                             ((ps.lister_miss || ps.max_gid >= (int64_t)G) ? 0x7fffffffull : low_bits_mask(G));
+      sa.n_ppass = build_passes(ps.vary_ts(), vary1, sa.ppass);
       if (std::max(P, G) <= (uint32_t)SORT_SMALL_MAX) {
         // small tables: one CTA, the same radix passes with the index arrays in shared memory
         const size_t smem = sort_small_smem();
@@ -1314,8 +1408,8 @@ int bs_upload_nodes(bs_engine* e, const bs_node_table* t) {
   const auto cols = node_cols(e, t);
   if (N && null_column(cols)) return fail(e, BS_E_INVAL, "bs_upload_nodes: null column");
   HP_BEGIN(e);
-  const NodeHostStats hs = node_host_pass(t, L, N);
-  if (!hs.ok) return fail(e, BS_E_RANGE, "bs_upload_nodes: value outside +-2^56");
+  const NodeStats ns = node_host_pass(t, L, N);
+  if (ns.bad_range) return fail(e, BS_E_RANGE, "bs_upload_nodes: value outside +-2^56");
   HP(e, "nodes:host-pass");
   BS_DEVICE_GUARD(e);
   const uint32_t Npad = std::max(1u, cdiv(N, NODE_TILE)) * NODE_TILE;
@@ -1325,11 +1419,7 @@ int bs_upload_nodes(bs_engine* e, const bs_node_table* t) {
   CK(cudaStreamSynchronize(e->s));
   HP(e, "nodes:dma-wait");
   e->h_nflags.assign(t->flags, t->flags + N);
-  memcpy(e->max_alloc, hs.mx_a, sizeof(hs.mx_a));
-  memcpy(e->max_requested, hs.mx_r, sizeof(hs.mx_r));
-  memcpy(e->or_left, hs.or_l, sizeof(hs.or_l));
-  memcpy(e->max_left, hs.mx_l, sizeof(hs.mx_l));
-  e->max_pod_count = hs.mx_pc;
+  e->node_stats = ns;
   e->N = N;
   e->score_pitch = (N + 1u) & ~1u;
   e->bitmap_pitch = (cdiv(N, 32) + 31u) & ~31u;
@@ -1354,8 +1444,8 @@ int bs_update_nodes(bs_engine* e, const uint32_t* idx, const bs_node_table* t) {
   if (null_column(cols)) return fail(e, BS_E_INVAL, "bs_update_nodes: null column");
   for (uint32_t k = 0; k < n; ++k)
     if (idx[k] >= e->N) return BS_E_INDEX;
-  const NodeHostStats hs = node_host_pass(t, L, n);
-  if (!hs.ok) return fail(e, BS_E_RANGE, "bs_update_nodes: value outside +-2^56");
+  const NodeStats ns = node_host_pass(t, L, n);
+  if (ns.bad_range) return fail(e, BS_E_RANGE, "bs_update_nodes: value outside +-2^56");
   BS_DEVICE_GUARD(e);
   HP_BEGIN(e);
   int rc;
@@ -1363,15 +1453,7 @@ int bs_update_nodes(bs_engine* e, const uint32_t* idx, const bs_node_table* t) {
   HP(e, "upd-nodes:enqueue");
   CK(cudaStreamSynchronize(e->s));
   HP(e, "upd-nodes:wait");
-  // lane maxima only ever grow here (a conservative bound keeps the wide/narrow split exact); the OR
-  // of the residuals only gains bits (fewer common trailing zeros: a smaller unit, still exact)
-  for (uint32_t d = 0; d < L; ++d) {
-    e->max_alloc[d] = std::max(e->max_alloc[d], hs.mx_a[d]);
-    e->max_requested[d] = std::max(e->max_requested[d], hs.mx_r[d]);
-    e->max_left[d] = std::max(e->max_left[d], hs.mx_l[d]);
-    e->or_left[d] |= hs.or_l[d];
-  }
-  e->max_pod_count = std::max(e->max_pod_count, hs.mx_pc);
+  e->node_stats.merge(ns);
   for (uint32_t k = 0; k < n; ++k) e->h_nflags[idx[k]] = t->flags[k];
   e->nodes_dirty = true;
   e->evaluated = false;
@@ -1395,58 +1477,20 @@ int bs_upload_groups(bs_engine* e, const bs_group_table* t) {
   int rc;
   if ((rc = upload_cols(e, cols, G, Gp))) return rc;
   HP(e, "groups:dma-enqueue");
-  // one chunked pass over the host columns (an omp team for big tables): |min_res| range, the varying bits of the
-  // sort-key words, creation sentinel, and whether the representative columns moved since their ids were assigned
-  uint64_t o1 = 0, a1 = ~0ull, o0 = 0, a0 = ~0ull;
-  int bad_creation = 0, bad_range = 0, reps_differ = 0;
-  {
-    const bool cmp_reps = e->h_gsel.size() == G && e->h_gtol.size() == G && e->h_grc.size() == G && e->h_gaff.size() == G;
-    if (!cmp_reps) reps_differ = 1;
-    const int T = G < 8192 ? 1 : host_threads();
-    const uint32_t chunk = (G + T - 1) / std::max(T, 1);
-    const uint64_t* hs = e->h_gsel.data();
-    const uint64_t* ht = e->h_gtol.data();
-    const uint32_t* ha = e->h_gaff.data();
-#pragma omp parallel for schedule(static, 1) num_threads(T) if (T > 1) reduction(| : o1, o0, bad_creation, bad_range, reps_differ) reduction(& : a1, a0)
-    for (int tk = 0; tk < T; ++tk) {
-      const uint32_t g0 = std::min(G, (uint32_t)tk * chunk), g1 = std::min(G, g0 + chunk);
-      for (uint32_t d = 0; d < L; ++d) {
-        const int64_t* row = t->min_res + (size_t)d * G;
-        int64_t lo = 0, hi = 0;
-        for (uint32_t g = g0; g < g1; ++g) { lo = std::min(lo, row[g]); hi = std::max(hi, row[g]); }
-        bad_range |= (lo < -BS_VALUE_LIMIT || hi > BS_VALUE_LIMIT) ? 1 : 0;
-      }
-      uint64_t lo1 = 0, la1 = ~0ull, lo0 = 0, la0 = ~0ull;
-      int bc = 0;
-      for (uint32_t g = g0; g < g1; ++g) {
-        const uint64_t c = (uint64_t)t->creation_ns[g], nm = (uint64_t)(~t->name_rank[g]);
-        lo1 |= c; la1 &= c; lo0 |= nm; la0 &= nm;
-        bc |= t->creation_ns[g] == INT64_MAX ? 1 : 0;
-      }
-      o1 |= lo1; a1 &= la1; o0 |= lo0; a0 &= la0; bad_creation |= bc;
-      if (cmp_reps && g1 > g0) {
-        int df = memcmp(hs + g0, t->rep_sel + g0, (size_t)(g1 - g0) * 8) != 0 || memcmp(ht + g0, t->rep_tol + g0, (size_t)(g1 - g0) * 8) != 0;
-        if (t->rep_aff_class) df = df || memcmp(ha + g0, t->rep_aff_class + g0, (size_t)(g1 - g0) * 4) != 0;
-        else
-          for (uint32_t g = g0; g < g1 && !df; ++g) df = ha[g] != BS_AFF_NONE;
-        reps_differ |= df;
-      }
-    }
-  }
-  if (bad_range) {
+  // the representative columns are compared with the engine's when it has ids assigned for a table of this length
+  const bool cmp_reps = e->h_gsel.size() == G && e->h_gtol.size() == G && e->h_grc.size() == G && e->h_gaff.size() == G;
+  const GroupStats gs = group_host_pass(t, L, G, cmp_reps ? e : nullptr);
+  if (gs.bad_range) {
     cudaStreamSynchronize(e->s);
     return fail(e, BS_E_RANGE, "bs_upload_groups: value outside +-2^56");
   }
-  if (bad_creation) {
+  if (gs.bad_creation) {
     cudaStreamSynchronize(e->s);
     return fail(e, BS_E_RANGE, "bs_upload_groups: creation_ns == INT64_MAX");
   }
-  e->vary_creation = G ? (o1 ^ a1) : 0;
-  e->vary_name = G ? (o0 ^ a0) : 0;
-  e->g_or1 = o1; e->g_and1 = a1; e->g_or0 = o0; e->g_and0 = a0;
+  e->group_stats = gs;
   // representative (sel, tol, affinity) columns unchanged since the ids were assigned: nothing to look up again
-  const bool same_reps = !reps_differ;
-  if (!same_reps) {
+  if (!cmp_reps || gs.reps_differ) {
     e->h_gsel.assign(t->rep_sel, t->rep_sel + G);
     e->h_gtol.assign(t->rep_tol, t->rep_tol + G);
     e->h_gaff.resize(G);
@@ -1480,11 +1524,9 @@ int bs_update_groups(bs_engine* e, const uint32_t* idx, const bs_group_table* t)
   if (null_column(cols) || !t->rep_sel || !t->rep_tol) return fail(e, BS_E_INVAL, "bs_update_groups: null column");
   for (uint32_t k = 0; k < n; ++k)
     if (idx[k] >= G) return BS_E_INDEX;
-  if (!std::all_of(t->min_res, t->min_res + (size_t)L * n,
-                   [](int64_t v) { return v >= -BS_VALUE_LIMIT && v <= BS_VALUE_LIMIT; }))
-    return fail(e, BS_E_RANGE, "bs_update_groups: value outside +-2^56");
-  for (uint32_t k = 0; k < n; ++k)
-    if (t->creation_ns[k] == INT64_MAX) return fail(e, BS_E_RANGE, "bs_update_groups: creation_ns == INT64_MAX");
+  const GroupStats gs = group_host_pass(t, L, n, nullptr);
+  if (gs.bad_range) return fail(e, BS_E_RANGE, "bs_update_groups: value outside +-2^56");
+  if (gs.bad_creation) return fail(e, BS_E_RANGE, "bs_update_groups: creation_ns == INT64_MAX");
   BS_DEVICE_GUARD(e);
   HP_BEGIN(e);
   int rc;
@@ -1492,10 +1534,8 @@ int bs_update_groups(bs_engine* e, const uint32_t* idx, const bs_group_table* t)
   HP(e, "upd-groups:enqueue");
   CK(cudaStreamSynchronize(e->s));
   HP(e, "upd-groups:wait");
-  // sort-key digits that vary: the accumulated OR / AND only widen (a superset costs a pass, never an error)
+  e->group_stats.merge(gs);
   for (uint32_t k = 0; k < n; ++k) {
-    const uint64_t c = (uint64_t)t->creation_ns[k], nm = (uint64_t)(~t->name_rank[k]);
-    e->g_or1 |= c; e->g_and1 &= c; e->g_or0 |= nm; e->g_and0 &= nm;
     e->h_gsel[idx[k]] = t->rep_sel[k];
     e->h_gtol[idx[k]] = t->rep_tol[k];
     e->h_gaff[idx[k]] = t->rep_aff_class ? t->rep_aff_class[k] : BS_AFF_NONE;
@@ -1504,8 +1544,6 @@ int bs_update_groups(bs_engine* e, const uint32_t* idx, const bs_group_table* t)
     e->h_matched_up[idx[k]] = t->matched[k];
     e->h_gflags_up[idx[k]] = t->flags[k];
   }
-  e->vary_creation = e->g_or1 ^ e->g_and1;
-  e->vary_name = e->g_or0 ^ e->g_and0;
   e->classes_dirty = true;         // the class tables go to the device again (new classes may have appeared); the pods' ids stay
   if (!e->group_classes_dirty && e->h_grc.size() == G) {
     // the other groups' ids are current: look up only the changed rows (the index keeps ids stable)
@@ -1532,17 +1570,8 @@ int bs_upload_pods(bs_engine* e, const bs_pod_table* t) {
   // wide/narrow lane classification), the varying bits of the sort keys, thread-local class indices
   // (fit class = (sel, tol, scalar keys requested with a non-zero amount, core.go:688-690);
   // representative class = (sel, tol)), and the host copies the per-call mirrors read.
-  const int T = P < 8192 ? 1 : host_threads();
-  struct Part {
-    int64_t lo[BS_MAX_LANES], hi[BS_MAX_LANES];
-    uint64_t orq[BS_MAX_LANES];
-    uint64_t ot = 0, at = ~0ull;
-    uint32_t op = 0, apr = ~0u;
-    int miss = 0;
-    int32_t mg = -1;
-    ClassIndex fit, rep;
-  };
-  std::vector<Part> part(T);
+  const Chunks ch(P, 8192);
+  std::vector<ClassIndex> fit_local(ch.T), rep_local(ch.T);
   HP_BEGIN(e);
   e->h_gid.resize(P); e->h_prio.resize(P); e->h_pflags.resize(P);
   BS_DEVICE_GUARD(e);
@@ -1561,19 +1590,15 @@ int bs_upload_pods(bs_engine* e, const bs_pod_table* t) {
   if ((rc = upload_vec(e, e->d_ts, t->ts_ns, P, Pp))) return rc;
   if ((rc = upload_vec(e, e->d_pflags, t->flags, P, Pp))) return rc;
   HP(e, "pods:dma-enqueue");
-  // T fixed chunks handed out by an omp for: a team smaller than requested still covers every chunk
-  const uint32_t chunk = (P + T - 1) / std::max(T, 1);
-#pragma omp parallel for schedule(static, 1) num_threads(T)
-  for (int tk = 0; tk < T; ++tk) {
-    Part& pt = part[tk];
-    for (uint32_t d = 0; d < BS_MAX_LANES; ++d) { pt.lo[d] = 0; pt.hi[d] = 0; pt.orq[d] = 0; }
-    const uint32_t a0 = std::min(P, (uint32_t)tk * chunk), a1 = std::min(P, a0 + chunk);
+  const PodStats ps = ch.reduce<PodStats>([&](int tk, uint32_t a0, uint32_t a1, PodStats& st) {
     for (uint32_t d = 0; d < L; ++d) {
       const int64_t* row = t->req + (size_t)d * P;
       int64_t lo = 0, hi = 0;
       uint64_t o = 0;
       for (uint32_t p = a0; p < a1; ++p) { lo = std::min(lo, row[p]); hi = std::max(hi, row[p]); o |= (uint64_t)row[p]; }
-      pt.lo[d] = lo; pt.hi[d] = hi; pt.orq[d] = o;
+      const int64_t neg = lo == INT64_MIN ? INT64_MAX : -lo;
+      st.bad_range = st.bad_range || lo < -BS_VALUE_LIMIT || hi > BS_VALUE_LIMIT;
+      st.max_req[d] = std::max(hi, neg); st.neg_req[d] = neg; st.or_req[d] = o;
     }
     {
       // reductions in locals and the plain column copies as memcpy: a byte store inside the loop would make the
@@ -1590,7 +1615,7 @@ int bs_upload_pods(bs_engine* e, const bs_pod_table* t) {
         miss |= ((g < BS_GID_NONE) || (t->flags[p] & BS_POD_LISTER_MISS)) ? 1 : 0;
         mg = std::max(mg, g);
       }
-      pt.ot = ot; pt.at = at; pt.op = op; pt.apr = apr; pt.miss = miss; pt.mg = mg;
+      st.or_ts = ot; st.and_ts = at; st.or_prio = op; st.and_prio = apr; st.lister_miss = miss != 0; st.max_gid = mg;
       if (a1 > a0) {
         memcpy(e->h_gid.data() + a0, t->gid + a0, (size_t)(a1 - a0) * 4);
         memcpy(e->h_prio.data() + a0, t->priority + a0, (size_t)(a1 - a0) * 4);
@@ -1616,73 +1641,33 @@ int bs_upload_pods(bs_engine* e, const bs_pod_table* t) {
         pfc[p] = fc;
         prc[p] = rep_of_fit[fc];
       }
-      pt.fit = std::move(fit);
-      pt.rep = std::move(rep);
+      fit_local[tk] = std::move(fit);
+      rep_local[tk] = std::move(rep);
     }
-  }
+  });
   HP(e, "pods:host-pass");
-  int64_t mx_q[BS_MAX_LANES] = {}, neg_q[BS_MAX_LANES] = {};
-  uint64_t or_q[BS_MAX_LANES] = {};
-  {
-    uint64_t ot = 0, at = ~0ull;
-    uint32_t op = 0, apr = ~0u;
-    int miss = 0;
-    int32_t mg = -1;
-    bool ok = true;
-    for (int k = 0; k < T; ++k) {
-      const Part& pt = part[k];
-      for (uint32_t d = 0; d < L; ++d) {
-        ok = ok && pt.lo[d] >= -BS_VALUE_LIMIT && pt.hi[d] <= BS_VALUE_LIMIT;
-        mx_q[d] = std::max(mx_q[d], std::max(pt.hi[d], pt.lo[d] == INT64_MIN ? INT64_MAX : -pt.lo[d]));
-        neg_q[d] = std::max(neg_q[d], pt.lo[d] == INT64_MIN ? INT64_MAX : -pt.lo[d]);
-        or_q[d] |= pt.orq[d];
-      }
-      ot |= pt.ot; at &= pt.at; op |= pt.op; apr &= pt.apr; miss |= pt.miss; mg = std::max(mg, pt.mg);
-    }
-    if (!ok) {   // the device and host-side columns were already overwritten: the table stays dropped
-      cudaStreamSynchronize(e->s);
-      return fail(e, BS_E_RANGE, "bs_upload_pods: value outside +-2^56");
-    }
-    e->vary_ts = P ? (ot ^ at) : 0;
-    e->vary_prio = P ? (uint64_t)(op ^ apr) : 0;
-    e->any_lister_miss = miss != 0;
-    e->max_gid = mg;
+  if (ps.bad_range) {   // the device and host-side columns were already overwritten: the table stays dropped
+    cudaStreamSynchronize(e->s);
+    return fail(e, BS_E_RANGE, "bs_upload_pods: value outside +-2^56");
   }
   // Merge the thread-local class indices into the engine's and remap the ids while the DMA is in
   // flight.  The engine's indices persist across uploads (ids of known classes are stable, so the
   // groups' representative ids stay valid); they restart only when mostly stale.
   {
     size_t lf = 0, lr = 0;
-    for (int k = 0; k < T; ++k) { lf += part[k].fit.size(); lr += part[k].rep.size(); }
+    for (int k = 0; k < ch.T; ++k) { lf += fit_local[k].size(); lr += rep_local[k].size(); }
     if (e->fit_index.size() > std::max<size_t>(4096, 4 * lf)) e->fit_index.clear();
     if (e->rep_index.size() > std::max<size_t>(4096, 4 * lr)) {
       e->rep_index.clear();
       e->group_classes_dirty = true;   // the groups' ids referred to the old index
     }
   }
-  {
-    std::vector<std::vector<uint32_t>> rf(T), rr(T);
-    for (int k = 0; k < T; ++k) {
-      rf[k].resize(part[k].fit.size());
-      rr[k].resize(part[k].rep.size());
-      for (size_t j = 0; j < part[k].fit.size(); ++j) rf[k][j] = e->fit_index.get_or_add(part[k].fit.keys[j]);
-      for (size_t j = 0; j < part[k].rep.size(); ++j) rr[k][j] = e->rep_index.get_or_add(part[k].rep.keys[j]);
-    }
-#pragma omp parallel for schedule(static, 1) num_threads(T)
-    for (int k = 0; k < T; ++k) {
-      const uint32_t a0 = std::min(P, (uint32_t)k * chunk), a1 = std::min(P, a0 + chunk);
-      for (uint32_t p = a0; p < a1; ++p) {
-        e->h_pfc[p] = rf[k][e->h_pfc[p]];
-        e->h_prc[p] = rr[k][e->h_prc[p]];
-      }
-    }
-  }
+  merge_classes(e->fit_index, fit_local, ch, e->h_pfc.data());
+  merge_classes(e->rep_index, rep_local, ch, e->h_prc.data());
   HP(e, "pods:class-merge");
   CK(cudaStreamSynchronize(e->s));
   HP(e, "pods:dma-wait");
-  memcpy(e->max_req, mx_q, sizeof(mx_q));
-  memcpy(e->neg_req, neg_q, sizeof(neg_q));
-  memcpy(e->or_req, or_q, sizeof(or_q));
+  e->pod_stats = ps;
   e->P = P;
   e->have_pods = true;
   e->classes_dirty = true;
@@ -2147,9 +2132,11 @@ int bs_replay(bs_engine* e, const uint32_t* queue, uint32_t n_queue, bs_replay_r
   // fits, so a node's `requested` never passes its capacity by more than one request; only negative requests
   // accumulate without that limit.
   long double worst = 0;
+  const NodeStats& ns = e->node_stats;
+  const PodStats& ps = e->pod_stats;
   for (uint32_t d = 0; d < L; ++d)
-    worst = std::max(worst, (long double)e->max_alloc[d] + (long double)e->max_requested[d] + (long double)e->max_req[d] +
-                                (long double)e->neg_req[d] * (long double)n_queue + (long double)e->max_pod_count + n_queue);
+    worst = std::max(worst, (long double)ns.max_alloc[d] + (long double)ns.max_requested[d] + (long double)ps.max_req[d] +
+                                (long double)ps.neg_req[d] * (long double)n_queue + (long double)ns.max_pod_count + n_queue);
   const bool safe = worst * (long double)std::max(N, 1u) < 4.0e18L;
   const uint32_t n_blocks = cdiv(N, REPLAY_BLOCK);
   const bool cache = safe && fitmask && n_blocks >= 1 && n_blocks <= (uint32_t)REPLAY_MAX_BLOCKS;

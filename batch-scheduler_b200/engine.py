@@ -26,6 +26,22 @@ class RoundResult:
     filter_code: np.ndarray = None
 
 
+_TABLE_C = {
+    NodeTable: (capi.NodeTableC, ("alloc", "requested", "pod_count", "alloc_present", "req_present", "label_mask",
+                                  "taint_mask", "flags")),
+    GroupTable: (capi.GroupTableC, ("min_member", "scheduled", "matched", "flags", "min_res", "min_res_present",
+                                    "rep_sel", "rep_tol", "creation_ns", "name_rank", "rep_aff")),
+    PodTable: (capi.PodTableC, ("req", "req_present", "gid", "sel_mask", "tol_mask", "priority", "ts_ns", "flags",
+                                "aff_class")),
+}
+
+
+def _table_c(table):
+    """The C struct of a table, for uploads and row updates alike: its columns in field order, alive for the call."""
+    cls, cols = _TABLE_C[type(table)]
+    return cls(table.n, table.lanes, *(capi.ptr(getattr(table, c)) for c in cols))
+
+
 class Engine:
     def __init__(self, n_lanes: int, device: int = 0, fit_bitmap: bool = True, score: bool = False,
                  filter: bool = False):
@@ -61,44 +77,27 @@ class Engine:
 
     # -- uploads ---------------------------------------------------------------------------
     def upload_nodes(self, nt: NodeTable):
-        t = capi.NodeTableC(nt.n, nt.lanes, capi.ptr(nt.alloc), capi.ptr(nt.requested), capi.ptr(nt.pod_count),
-                            capi.ptr(nt.alloc_present), capi.ptr(nt.req_present), capi.ptr(nt.label_mask),
-                            capi.ptr(nt.taint_mask), capi.ptr(nt.flags))
-        self._check(self.lib.bs_upload_nodes(self.h, C.byref(t)))
+        self._check(self.lib.bs_upload_nodes(self.h, C.byref(_table_c(nt))))
         self.N = nt.n
 
     def update_nodes(self, idx, rows: NodeTable):
         """Overwrites rows `idx` of the resident node table with `rows` (a compact NodeTable)."""
         idx = np.ascontiguousarray(idx, dtype=np.uint32)
         assert len(idx) == rows.n
-        t = capi.NodeTableC(rows.n, rows.lanes, capi.ptr(rows.alloc), capi.ptr(rows.requested),
-                            capi.ptr(rows.pod_count), capi.ptr(rows.alloc_present), capi.ptr(rows.req_present),
-                            capi.ptr(rows.label_mask), capi.ptr(rows.taint_mask), capi.ptr(rows.flags))
-        self._check(self.lib.bs_update_nodes(self.h, capi.ptr(idx), C.byref(t)))
+        self._check(self.lib.bs_update_nodes(self.h, capi.ptr(idx), C.byref(_table_c(rows))))
 
     def upload_groups(self, gt: GroupTable):
-        t = capi.GroupTableC(gt.n, gt.lanes, capi.ptr(gt.min_member), capi.ptr(gt.scheduled), capi.ptr(gt.matched),
-                             capi.ptr(gt.flags), capi.ptr(gt.min_res), capi.ptr(gt.min_res_present),
-                             capi.ptr(gt.rep_sel), capi.ptr(gt.rep_tol), capi.ptr(gt.creation_ns),
-                             capi.ptr(gt.name_rank), capi.ptr(gt.rep_aff))
-        self._check(self.lib.bs_upload_groups(self.h, C.byref(t)))
+        self._check(self.lib.bs_upload_groups(self.h, C.byref(_table_c(gt))))
         self.G = gt.n
 
     def update_groups(self, idx, rows: GroupTable):
         """Overwrites rows `idx` of the resident group table with `rows` (a compact GroupTable)."""
         idx = np.ascontiguousarray(idx, dtype=np.uint32)
         assert len(idx) == rows.n
-        t = capi.GroupTableC(rows.n, rows.lanes, capi.ptr(rows.min_member), capi.ptr(rows.scheduled),
-                             capi.ptr(rows.matched), capi.ptr(rows.flags), capi.ptr(rows.min_res),
-                             capi.ptr(rows.min_res_present), capi.ptr(rows.rep_sel), capi.ptr(rows.rep_tol),
-                             capi.ptr(rows.creation_ns), capi.ptr(rows.name_rank))
-        self._check(self.lib.bs_update_groups(self.h, capi.ptr(idx), C.byref(t)))
+        self._check(self.lib.bs_update_groups(self.h, capi.ptr(idx), C.byref(_table_c(rows))))
 
     def upload_pods(self, pt: PodTable):
-        t = capi.PodTableC(pt.n, pt.lanes, capi.ptr(pt.req), capi.ptr(pt.req_present), capi.ptr(pt.gid),
-                           capi.ptr(pt.sel_mask), capi.ptr(pt.tol_mask), capi.ptr(pt.priority),
-                           capi.ptr(pt.ts_ns), capi.ptr(pt.flags), capi.ptr(pt.aff_class))
-        self._check(self.lib.bs_upload_pods(self.h, C.byref(t)))
+        self._check(self.lib.bs_upload_pods(self.h, C.byref(_table_c(pt))))
         self.P = pt.n
 
     def upload_affinity(self, bits):
