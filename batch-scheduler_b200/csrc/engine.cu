@@ -342,6 +342,7 @@ struct bs_engine {
   std::mutex mu;
   int device = 0;
   uint32_t L = 0, out_flags = 0;
+  uint32_t topk = 0;   // list length K of BS_OUT_TOPK, 0 without it
   Stream s, s2, s3, s4;   // main; queue sort; PreFilter chain (high priority); peer wait
   Event ev_fork, ev_join, ev_pre, ev_push, ev_gath;
   std::string err;
@@ -391,6 +392,7 @@ struct bs_engine {
   DevBuf d_stage;         // bs_update_nodes / bs_update_groups: device staging of the changed rows
   DevBuf d_best_packed;   // gang_fit tail pieces: max((score + 1) << 32 | ~node) per pod
   DevBuf d_fit_bitmap, d_score;
+  DevBuf d_topk_node, d_topk_score;   // BS_OUT_TOPK: [Prows][topk] lists
   // sort scratch: views into one arena
   View d_gk0, d_gk1, d_pk0, d_pk1, d_idx_a, d_idx_b, d_ghist, d_group_rank, d_tilecnt, d_sort_barrier;
   uint32_t sort_max_grid = 1;
@@ -759,7 +761,7 @@ void launch_replay(uint32_t L, const ReplayArgs& a, cudaStream_t s) {
 }
 
 cudaError_t launch_fit(const FitArgs& a, uint32_t units, cudaStream_t s, uint32_t* launches, cudaEvent_t ev_a, cudaEvent_t ev_b) {
-  const int out = a.score ? FIT_OUT_SCORE : (a.fit_bitmap ? FIT_OUT_BITMAP : FIT_OUT_NONE);
+  const int out = a.score ? FIT_OUT_SCORE : a.topk_node ? FIT_OUT_TOPK : a.fit_bitmap ? FIT_OUT_BITMAP : FIT_OUT_NONE;
   FitFn fn = fit_lookup(a.lm.LW, a.lm.LN, a.lm.LS, out);
   return fn ? fn(a, units, s, launches, ev_a, ev_b) : cudaErrorInvalidValue;
 }
@@ -944,6 +946,10 @@ int ensure_round_buffers(bs_engine* e) {
   const size_t Prows = (size_t)cdiv(std::max(e->P, 1u), PODS_PER_CTA) * PODS_PER_CTA;
   if (e->out_flags & BS_OUT_FIT_BITMAP) CK(e->d_fit_bitmap.ensure(Prows * std::max(e->bitmap_pitch, 32u) * 4));
   if (e->out_flags & BS_OUT_SCORE) CK(e->d_score.ensure(Prows * std::max(e->score_pitch, 2u) * 8));
+  if (e->out_flags & BS_OUT_TOPK) {
+    CK(e->d_topk_node.ensure(Prows * e->topk * 4));
+    CK(e->d_topk_score.ensure(Prows * e->topk * 8));
+  }
   if (e->out_flags & BS_OUT_FILTER) {
     CK(e->d_filter_bitmap.ensure(Prows * std::max(e->W, 1u) * 4));
   }
@@ -1093,8 +1099,10 @@ int evaluate_async_locked(bs_engine* e) {
         // Two builds of the same kernel.  Beside a long fit kernel the sort is hidden anyway and must stay out of its
         // way (32 registers: its CTAs share their SMs with the fit CTAs); when the fit kernel is the shorter of the two
         // (a small shard, few nodes) the round waits for the sort, and the build with 16 gathers in flight per thread
-        // is the faster one.  Estimate: pairs x the per-pair time of the output mode measured on an H100.
-        const double est_fit_ms = (double)P * (double)e->N * ((e->out_flags & BS_OUT_SCORE) ? 2.9e-9 : 0.9e-9);
+        // is the faster one.  Estimate: pairs x the per-pair time of the output mode measured on an H100 (top-K: K = 16
+        // at cfg4, profiles/topk_h100.jsonl).
+        const double per_pair_ms = (e->out_flags & BS_OUT_SCORE) ? 2.9e-9 : (e->out_flags & BS_OUT_TOPK) ? 2.0e-9 : 0.9e-9;
+        const double est_fit_ms = (double)P * (double)e->N * per_pair_ms;
         const bool lean = est_fit_ms > 0.6;
         const void* fn = lean ? (const void*)queue_sort_kernel<SORT_LEAN_GROUP> : (const void*)queue_sort_kernel<SORT_WIDE_GROUP>;
         CK(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(SORT_THREADS), params, 0, e->s2));
@@ -1182,6 +1190,10 @@ int evaluate_async_locked(bs_engine* e) {
       a.bitmap_pitch = e->bitmap_pitch;
       a.P = P; a.N = e->N; a.Npad = e->Npad; a.W = e->W;
       a.best_packed = e->d_best_packed.as<unsigned long long>();
+      const bool topk = (e->out_flags & BS_OUT_TOPK) != 0;
+      a.topk_node = topk ? e->d_topk_node.as<int32_t>() : nullptr;
+      a.topk_score = topk ? e->d_topk_score.as<int64_t>() : nullptr;
+      a.topk_k = e->topk;
       uint32_t nl = 1;
       CK(launch_fit(a, cdiv(P, PODS_PER_CTA), e->s, &nl, e->profiling ? e->ev_a[BS_K_GANG_FIT].h : nullptr,
                     e->profiling ? e->ev_b[BS_K_GANG_FIT].h : nullptr));
@@ -1342,6 +1354,10 @@ int bs_create(const bs_config* cfg, bs_engine** out) {
   if (!cfg || !out) return BS_E_INVAL;
   *out = nullptr;
   if (cfg->n_lanes < BS_FIXED_LANES || cfg->n_lanes > BS_MAX_LANES) return BS_E_INVAL;
+  // top-K lists: 1..BS_TOPK_MAX entries with the flag, none without; the score matrix already holds them
+  if ((cfg->out_flags & BS_OUT_TOPK) ? (cfg->topk < 1 || cfg->topk > BS_TOPK_MAX || (cfg->out_flags & BS_OUT_SCORE))
+                                     : cfg->topk != 0)
+    return BS_E_INVAL;
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) {
     cudaGetLastError();
@@ -1355,6 +1371,7 @@ int bs_create(const bs_config* cfg, bs_engine** out) {
   e->device = cfg->device;
   e->L = cfg->n_lanes;
   e->out_flags = cfg->out_flags;
+  e->topk = cfg->topk;
   e->host_prof = getenv("BS_HOST_PROFILE") != nullptr;
   int prio_lo = 0, prio_hi = 0;
   cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);   // the small kernels of the PreFilter chain must get the
@@ -2326,6 +2343,21 @@ int bs_fetch_score_rows(bs_engine* e, uint32_t pod0, uint32_t n, int64_t* scores
   if (n && e->N)
     CK(cudaMemcpy2DAsync(scores, (size_t)e->N * 8, e->d_score.as<int64_t>() + (size_t)pod0 * e->score_pitch,
                          (size_t)e->score_pitch * 8, (size_t)e->N * 8, n, cudaMemcpyDeviceToHost, e->s));
+  CK(cudaStreamSynchronize(e->s));
+  return BS_OK;
+}
+
+int bs_fetch_topk_rows(bs_engine* e, uint32_t pod0, uint32_t n, int32_t* nodes, int64_t* scores) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!e->evaluated || !(e->out_flags & BS_OUT_TOPK)) return fail(e, BS_E_STATE, "no top-K lists materialised");
+  if ((uint64_t)pod0 + n > e->P) return BS_E_INDEX;
+  BS_DEVICE_GUARD(e);
+  const size_t off = (size_t)pod0 * e->topk, cnt = (size_t)n * e->topk;   // device rows are dense [Prows][K]
+  if (cnt && nodes)
+    CK(cudaMemcpyAsync(nodes, e->d_topk_node.as<int32_t>() + off, cnt * 4, cudaMemcpyDeviceToHost, e->s));
+  if (cnt && scores)
+    CK(cudaMemcpyAsync(scores, e->d_topk_score.as<int64_t>() + off, cnt * 8, cudaMemcpyDeviceToHost, e->s));
   CK(cudaStreamSynchronize(e->s));
   return BS_OK;
 }

@@ -144,6 +144,11 @@ struct FitArgs {
   // Pieces combine their per-pod results with atomics (count add, packed (score+1, ~node) max).
   uint32_t n_full, tail_split;
   unsigned long long* best_packed;   // [P] or null (tail_split == 1)
+  // top-K lists (FIT_OUT_TOPK, else null): per pod its topk_k best fitting nodes, score descending then node
+  // ascending, padded with node -1 / score INT64_MIN
+  int32_t* topk_node;     // [Ppad][topk_k]
+  int64_t* topk_score;    // [Ppad][topk_k]
+  uint32_t topk_k;        // 1..BS_TOPK_MAX
 };
 
 // running best score of a lane: int32 on the narrow fast path (scores of fitting pairs are < 2^27,
@@ -161,8 +166,45 @@ template <> struct BestT<true> { using type = int32_t; };
 // scores go to the warp's staging slab (SCORE, RN == 1: one matrix row segment, node j*32 + lane at slab
 // element j*32 + lane) as int64: fit ? m : INT64_MIN.
 // OUT: what leaves the SMs besides the per-pod results — 0 nothing (decisions only: feasible counts come from a
-// predicated add, no ballot), 1 the fit bitmap, 2 the score matrix (+ the bitmap when its pointer is set).
-enum { FIT_OUT_NONE = 0, FIT_OUT_BITMAP = 1, FIT_OUT_SCORE = 2 };
+// predicated add, no ballot), 1 the fit bitmap, 2 the score matrix (+ the bitmap when its pointer is set), 3 each
+// pod's top-K list (counts as in mode 0; + the bitmap when its pointer is set).
+enum { FIT_OUT_NONE = 0, FIT_OUT_BITMAP = 1, FIT_OUT_SCORE = 2, FIT_OUT_TOPK = 3 };
+
+// Top-K selection (FIT_OUT_TOPK).  Each pod keeps a running list of its best fitting nodes in shared memory (32
+// entries of (score, node), lane i of the warp owns entry i) ordered by score descending, then node ascending — the
+// strict total order best_node uses.  Unfilled entries hold (-1, -1): every fitting pair has a score >= 0, so they
+// come after every real entry.  In registers the pod keeps only its threshold, the score of entry K-1.  A pair is a
+// candidate when it fits and its score is greater than the threshold: nodes are swept in ascending index order, so
+// a node met later never beats an entry of equal score.  A warp ballot per word and pod collects the candidates;
+// this out-of-line path inserts them one at a time.  A candidate's place is the number of entries before it under
+// the total order (lexicographic on (score, node), popcount of a ballot); the entries from there on move up one
+// lane; entries past K-1 are never read out.  The top K of a set under a strict total order do not depend on the
+// order in which its elements are inserted, so the list is exact whatever order the sweep meets the nodes in.
+// Returns the new threshold.
+template <typename S>
+__device__ __forceinline__ S topk_insert(S* __restrict__ ls_p, int32_t* __restrict__ ln_p, uint32_t K, uint32_t cb,
+                                         S s, int32_t n0 /*node of lane 0's pair*/, uint32_t lane) {
+  S ls = ls_p[lane];
+  int32_t ln = ln_p[lane];
+#pragma unroll 1
+  do {
+    const uint32_t src = __ffs(cb) - 1;
+    cb &= cb - 1;
+    const S cs = __shfl_sync(0xffffffffu, s, src);
+    const int32_t cn = n0 + (int32_t)src;
+    const uint32_t pos = __popc(__ballot_sync(0xffffffffu, ls > cs || (ls == cs && ln < cn)));
+    if (pos < K) {
+      const S us = __shfl_up_sync(0xffffffffu, ls, 1);
+      const int32_t un = __shfl_up_sync(0xffffffffu, ln, 1);
+      if (lane == pos) { ls = cs; ln = cn; }
+      else if (lane > pos) { ls = us; ln = un; }
+    }
+  } while (cb);
+  ls_p[lane] = ls;
+  ln_p[lane] = ln;
+  return __shfl_sync(0xffffffffu, ls, K - 1);
+}
+
 template <int LW, int LN, int LS, int OUT, int RN>
 __device__ __forceinline__ void fit_tile(const FitArgs& a, const int64_t* __restrict__ tlw,
                                          const int32_t* __restrict__ tln,
@@ -172,9 +214,13 @@ __device__ __forceinline__ void fit_tile(const FitArgs& a, const int64_t* __rest
                                          uint32_t* s_words, uint32_t wbase /*tile's first word in the line*/, uint32_t node_base, uint32_t lane,
                                          typename BestT<(LN > 0)>::type (&best_s)[PODS_PER_WARP],
                                          int32_t (&best_n)[PODS_PER_WARP], int32_t (&kb)[PODS_PER_WARP],
-                                         uint32_t (&cnt)[PODS_PER_WARP]) {
+                                         uint32_t (&cnt)[PODS_PER_WARP],
+                                         typename BestT<(LN > 0)>::type* tks, int32_t* tkn /*TOPK: the warp's lists*/,
+                                         typename BestT<(LN > 0)>::type (&thr)[PODS_PER_WARP]) {
   constexpr bool SCORE = OUT == FIT_OUT_SCORE;
-  constexpr bool WORDS = OUT != FIT_OUT_NONE;
+  constexpr bool TOPK = OUT == FIT_OUT_TOPK;
+  constexpr bool WORDS = OUT == FIT_OUT_BITMAP || SCORE;
+  using S = typename BestT<(LN > 0)>::type;
   static_assert(!SCORE || RN == 1, "a staging slab holds one matrix row");
   const int64_t* tpw = tlw + lane;
   const int32_t* tpn = tln + lane;
@@ -221,11 +267,16 @@ __device__ __forceinline__ void fit_tile(const FitArgs& a, const int64_t* __rest
           const bool fit = (sgn >= 0) && ((colbits[r] >> (jb + jj)) & 1u);
           if (WORDS) sts_u32(wp + (r * 32 + jj) * 4, __ballot_sync(0xffffffffu, fit));
           else if (fit) ++cnt[r];
+          if (TOPK && a.fit_bitmap) sts_u32(wp + (r * 32 + jj) * 4, __ballot_sync(0xffffffffu, fit));
           // best node of the tile as ONE running max: key = score * 2^KEY_BITS + (TILE_WORDS-1-j) < 2^31
           // (scores of fitting pairs are < 2^27), -1 = none; decoded once per tile
           const int32_t key = (int32_t)(m32 << KEY_BITS) + (jrem - jj);
-          if (fit) kb[r] = max(kb[r], key);
+          if (!TOPK && fit) kb[r] = max(kb[r], key);
           if (SCORE) sts_v2u32(sp + jj * 32 * 8, fit ? m32 : 0u, fit ? 0u : 0x80000000u);
+          if (TOPK) {
+            const uint32_t cb = __ballot_sync(0xffffffffu, fit && (int32_t)m32 > thr[r]);
+            if (cb) thr[r] = topk_insert<S>(tks + r * 32, tkn + r * 32, a.topk_k, cb, (int32_t)m32, node + jj * 32 - (int32_t)lane, lane);
+          }
         } else {
           int64_t m = lfw[0] - rqw[r][0];
 #pragma unroll
@@ -233,8 +284,13 @@ __device__ __forceinline__ void fit_tile(const FitArgs& a, const int64_t* __rest
           const bool fit = (hi32(m) >= 0) && ((colbits[r] >> (jb + jj)) & 1u);
           if (WORDS) sts_u32(wp + (r * 32 + jj) * 4, __ballot_sync(0xffffffffu, fit));
           else if (fit) ++cnt[r];
-          if (fit && m > best_s[r]) { best_s[r] = m; best_n[r] = node + jj * 32; }
+          if (TOPK && a.fit_bitmap) sts_u32(wp + (r * 32 + jj) * 4, __ballot_sync(0xffffffffu, fit));
+          if (!TOPK && fit && m > best_s[r]) { best_s[r] = m; best_n[r] = node + jj * 32; }
           if (SCORE) sts_u64(sp + jj * 32 * 8, fit ? (long long)m : (long long)INT64_MIN);
+          if (TOPK) {
+            const uint32_t cb = __ballot_sync(0xffffffffu, fit && m > thr[r]);
+            if (cb) thr[r] = topk_insert<S>(tks + r * 32, tkn + r * 32, a.topk_k, cb, m, node + jj * 32 - (int32_t)lane, lane);
+          }
         }
       }
     }
@@ -251,23 +307,31 @@ __host__ __device__ constexpr size_t fit_tile_bytes(int LW, int LN, int LS) {
   return (size_t)NODE_TILE * (8 * LW + 4 * (LN + LS));
 }
 __host__ __device__ constexpr size_t fit_slab_bytes() { return (size_t)NODE_TILE * 8; }   // one tile of one score row
+// the top-K lists of a CTA: [PODS_PER_CTA][32] scores (8 bytes each; int32 in the first half on the narrow path,
+// whose fitting scores are < 2^27), then [PODS_PER_CTA][32] i32 nodes (12 KB)
+__host__ __device__ constexpr size_t fit_topk_bytes() { return (size_t)PODS_PER_CTA * BS_TOPK_MAX * 12; }
+static_assert(BS_TOPK_MAX == 32, "a top-K list holds one entry per lane");
 // shared-memory layout: [stages]{[LW][NODE_TILE] i64, [LN+LS][NODE_TILE] i32} | req_w | req_n | mbarriers |
 //                       ballot words | (SCORE) [FIT_WARPS][FIT_NB] staging slabs, 128-byte aligned
+//                                    | (TOPK) the top-K lists
 __host__ __device__ constexpr size_t fit_smem_front(int LW, int LN, int LS) {
   size_t b = FIT_STAGES * fit_tile_bytes(LW, LN, LS) + (size_t)PODS_PER_CTA * (8 * LW + 4 * (LN + LS));
   b = (b + 7) & ~(size_t)7;
   b += 2 * FIT_STAGES * sizeof(uint64_t) + (size_t)PODS_PER_CTA * 32 * sizeof(uint32_t);
   return (b + 127) & ~(size_t)127;
 }
-__host__ __device__ constexpr size_t fit_smem_total(int LW, int LN, int LS, bool score) {
-  return fit_smem_front(LW, LN, LS) + (score ? (size_t)FIT_WARPS * FIT_NB * fit_slab_bytes() : 0);
+__host__ __device__ constexpr size_t fit_smem_total(int LW, int LN, int LS, int out) {
+  return fit_smem_front(LW, LN, LS) + (out == FIT_OUT_SCORE  ? (size_t)FIT_WARPS * FIT_NB * fit_slab_bytes()
+                                       : out == FIT_OUT_TOPK ? fit_topk_bytes()
+                                                             : 0);
 }
 constexpr size_t FIT_SMEM_MAX = 227 * 1024;   // dynamic shared memory one CTA may use on sm_90a
 
 template <int LW, int LN, int LS, int OUT>
 __global__ void __launch_bounds__(FIT_THREADS, FIT_MIN_BLOCKS) gang_fit_kernel(FitArgs a) {
   constexpr bool SCORE = OUT == FIT_OUT_SCORE;
-  constexpr bool WORDS = OUT != FIT_OUT_NONE;
+  constexpr bool TOPK = OUT == FIT_OUT_TOPK;
+  constexpr bool WORDS = OUT == FIT_OUT_BITMAP || SCORE;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   constexpr size_t STAGE_BYTES = fit_tile_bytes(LW, LN, LS);
   constexpr int LNS = LN + LS;
@@ -357,12 +421,19 @@ __global__ void __launch_bounds__(FIT_THREADS, FIT_MIN_BLOCKS) gang_fit_kernel(F
   typename BestT<(LN > 0)>::type best_s[PODS_PER_WARP];
   int32_t best_n[PODS_PER_WARP];
   int32_t kb[PODS_PER_WARP], kthr[PODS_PER_WARP];   // tile-local best key; smallest key that beats best_s
+  typename BestT<(LN > 0)>::type thr[PODS_PER_WARP];   // TOPK: score of list entry K-1 (-1 while the list is not full)
   int64_t rqw[PODS_PER_WARP][LW > 0 ? LW : 1];
   int32_t rqn[PODS_PER_WARP][LNS > 0 ? LNS : 1];
   uint32_t coff[PODS_PER_WARP];
+  // TOPK: the warp's PODS_PER_WARP lists of 32 entries (after the ballot words, where score mode has its slabs)
+  typename BestT<(LN > 0)>::type* tks =
+      reinterpret_cast<typename BestT<(LN > 0)>::type*>(smem_raw + fit_smem_front(LW, LN, LS)) + wid * PODS_PER_WARP * 32;
+  int32_t* tkn = reinterpret_cast<int32_t*>(smem_raw + fit_smem_front(LW, LN, LS) + (size_t)PODS_PER_CTA * 32 * 8) +
+                 wid * PODS_PER_WARP * 32;
 #pragma unroll
   for (int r = 0; r < PODS_PER_WARP; ++r) {
-    cnt[r] = 0; best_n[r] = -1; kb[r] = -1; kthr[r] = 0;
+    cnt[r] = 0; best_n[r] = -1; kb[r] = -1; kthr[r] = 0; thr[r] = -1;
+    if (TOPK) { tks[r * 32 + lane] = -1; tkn[r * 32 + lane] = -1; }
     best_s[r] = LN > 0 ? (typename BestT<(LN > 0)>::type)(-1) : (typename BestT<(LN > 0)>::type)INT64_MIN;
     const uint32_t p = wpod0 + r;
     coff[r] = (p < a.P ? a.fit_class[p] : 0u) * n_tiles * 32 + lane;
@@ -406,7 +477,7 @@ __global__ void __launch_bounds__(FIT_THREADS, FIT_MIN_BLOCKS) gang_fit_kernel(F
           __syncwarp();
         }
         fit_tile<LW, LN, LS, OUT, 1>(a, tlw, tln, rqw, rqn, colbits, r, slab, s_words, wbase, node_base, lane, best_s,
-                                     best_n, kb, cnt);
+                                     best_n, kb, cnt, tks, tkn, thr);
         fence_async_smem();
         __syncwarp();
         if (lane == 0) {
@@ -422,9 +493,9 @@ __global__ void __launch_bounds__(FIT_THREADS, FIT_MIN_BLOCKS) gang_fit_kernel(F
       }
     } else {
       fit_tile<LW, LN, LS, OUT, PODS_PER_WARP>(a, tlw, tln, rqw, rqn, colbits, 0, 0, s_words, wbase, node_base, lane,
-                                               best_s, best_n, kb, cnt);
+                                               best_s, best_n, kb, cnt, tks, tkn, thr);
     }
-    if (LN > 0) {
+    if (LN > 0 && !TOPK) {
       // a tile's best key beats the running best iff key >= (best_s + 1) << KEY_BITS: strictly greater score
       // (an equal score in a later tile loses to the earlier node)
 #pragma unroll
@@ -442,14 +513,14 @@ __global__ void __launch_bounds__(FIT_THREADS, FIT_MIN_BLOCKS) gang_fit_kernel(F
     // Fit bitmap: the ballot words of TILES_PER_LINE tiles make one 128-byte line per pod (the bitmap's row
     // pitch is a multiple of 32 words), written with one fully coalesced store — 4-byte pieces of unaligned rows
     // would write partial sectors.
-    if (WORDS && ((tile + 1) % TILES_PER_LINE == 0 || tile + 1 == tile_hi)) {
+    if ((WORDS || (TOPK && want_bitmap)) && ((tile + 1) % TILES_PER_LINE == 0 || tile + 1 == tile_hi)) {
       const uint32_t line = tile / TILES_PER_LINE;
       const uint32_t valid = (tile % TILES_PER_LINE + 1) * TILE_WORDS;   // words assembled in this line
       if (lane < valid) {
 #pragma unroll
         for (int r = 0; r < PODS_PER_WARP; ++r) {
           const uint32_t w = s_words[r * 32 + lane];
-          cnt[r] += __popc(w);
+          if (WORDS) cnt[r] += __popc(w);
           if (want_bitmap) a.fit_bitmap[(size_t)(wpod0 + r) * a.bitmap_pitch + line * 32 + lane] = w;
         }
       }
@@ -458,12 +529,23 @@ __global__ void __launch_bounds__(FIT_THREADS, FIT_MIN_BLOCKS) gang_fit_kernel(F
     if (++stage == FIT_STAGES) { stage = 0; phase ^= 1; }
   }
   if (SCORE && lane == 0) bulk_wait_read<0>();      // the slabs must outlive their bulk reads
+  if (TOPK && lane < a.topk_k) {
+    // the lists leave as [Ppad][K] rows (padded rows: no pod guard); lane i writes entry i
+#pragma unroll
+    for (int r = 0; r < PODS_PER_WARP; ++r) {
+      const size_t o = (size_t)(wpod0 + r) * a.topk_k + lane;
+      const int32_t n = tkn[r * 32 + lane];
+      a.topk_node[o] = n;
+      a.topk_score[o] = n < 0 ? INT64_MIN : (int64_t)tks[r * 32 + lane];
+    }
+  }
 
   // per-pod reductions across the warp: best = max score, lowest node on ties
 #pragma unroll
   for (int k = 0; k < PODS_PER_WARP; ++k) {
-    int32_t n = best_n[k];
-    int64_t s = n < 0 ? INT64_MIN : (int64_t)best_s[k];
+    // TOPK: the best node is entry 0 of the list (same order), read by every lane; the sweep keeps no running best
+    int32_t n = TOPK ? tkn[k * 32] : best_n[k];
+    int64_t s = n < 0 ? INT64_MIN : TOPK ? (int64_t)tks[k * 32] : (int64_t)best_s[k];
     uint32_t c = cnt[k];
     for (int o = 16; o; o >>= 1) {
       const int64_t os = __shfl_xor_sync(0xffffffffu, s, o);

@@ -14,7 +14,7 @@ namespace {
 
 template <int LW, int LN, int LS, int OUT>
 cudaError_t launch_fit_t(const FitArgs& a0, uint32_t units, cudaStream_t s, uint32_t* launches, cudaEvent_t ev_a, cudaEvent_t ev_b) {
-  constexpr size_t smem = fit_smem_total(LW, LN, LS, OUT == FIT_OUT_SCORE);
+  constexpr size_t smem = fit_smem_total(LW, LN, LS, OUT);
   static_assert(smem <= FIT_SMEM_MAX, "the fit kernel's shared memory exceeds what one CTA may use");
   // per launch, not cached: the attribute is per device and one process may drive several GPUs
   cudaError_t er = cudaFuncSetAttribute(gang_fit_kernel<LW, LN, LS, OUT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -25,8 +25,8 @@ cudaError_t launch_fit_t(const FitArgs& a0, uint32_t units, cudaStream_t s, uint
   a.tail_split = 1;
   // Tail balance (FitArgs): whole waves of resident CTA slots run full-range units; the units of the last,
   // partial wave are cut into node-range pieces so that every SM gets a share of it.  Narrow shapes only
-  // (the packed best needs scores below 2^31).
-  if (LN > 0 && a.best_packed && units) {
+  // (the packed best needs scores below 2^31), and not in top-K mode (a piece's list covers its node range only).
+  if (LN > 0 && OUT != FIT_OUT_TOPK && a.best_packed && units) {
     int per_sm = 0, dev = 0, sms = 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gang_fit_kernel<LW, LN, LS, OUT>, FIT_THREADS, smem) == cudaSuccess &&
         cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess &&
@@ -66,8 +66,12 @@ cudaError_t launch_fit_t(const FitArgs& a0, uint32_t units, cudaStream_t s, uint
 
 template <int LW, int LN, int LS>
 FitFn pick(int out) {
-  return out == FIT_OUT_SCORE ? launch_fit_t<LW, LN, LS, FIT_OUT_SCORE>
-                              : (out == FIT_OUT_BITMAP ? launch_fit_t<LW, LN, LS, FIT_OUT_BITMAP> : launch_fit_t<LW, LN, LS, FIT_OUT_NONE>);
+  switch (out) {
+    case FIT_OUT_SCORE: return launch_fit_t<LW, LN, LS, FIT_OUT_SCORE>;
+    case FIT_OUT_BITMAP: return launch_fit_t<LW, LN, LS, FIT_OUT_BITMAP>;
+    case FIT_OUT_TOPK: return launch_fit_t<LW, LN, LS, FIT_OUT_TOPK>;
+  }
+  return launch_fit_t<LW, LN, LS, FIT_OUT_NONE>;
 }
 
 }  // namespace

@@ -692,12 +692,11 @@ Status BatchSchedulingPlugin::Pack(const std::vector<const NodeInfo*>& snapshot,
   return pack_impl(snapshot, pending, gi, extra_pod_flags, default_wait_ns, out);
 }
 
-BatchSchedulingPlugin::BatchSchedulingPlugin(int device, int64_t max_schedule_time_ns, uint32_t out_flags)
+BatchSchedulingPlugin::BatchSchedulingPlugin(int device, int64_t max_schedule_time_ns, uint32_t out_flags, uint32_t topk)
     : max_schedule_time_ns_(max_schedule_time_ns) {
-  (void)device;
-  (void)out_flags;
   device_ = device;
-  out_flags_ = out_flags;
+  out_flags_ = out_flags | (topk ? BS_OUT_TOPK : 0u);
+  topk_ = topk;
 }
 
 BatchSchedulingPlugin::~BatchSchedulingPlugin() {
@@ -878,7 +877,7 @@ Status BatchSchedulingPlugin::BeginRound(const std::vector<const NodeInfo*>& sna
   if (!eng_ || eng_lanes_ != packed_.lanes) {
     // a new scalar resource changed the lane count: a fresh engine takes over the gang state of the old one
     bs_engine* fresh = nullptr;
-    bs_config cfg{device_, packed_.lanes, out_flags_, 0};
+    bs_config cfg{device_, packed_.lanes, out_flags_, topk_};
     int rc = bs_create(&cfg, &fresh);
     if (rc) return fail(rc);
     if (eng_) { bs_state_move(fresh, eng_); bs_destroy(eng_); }
@@ -911,6 +910,7 @@ Status BatchSchedulingPlugin::BeginRound(const std::vector<const NodeInfo*>& sna
   r.prefilter = prefilter_.data(); r.feasible_count = feasible_.data(); r.best_node = best_node_.data();
   r.admit = admit_.data(); r.new_denied = new_denied_.data(); r.order = order_.data(); r.rank = rank_.data();
   if ((rc = bs_evaluate(eng_, &r))) return fail(rc);
+  if ((rc = FetchTopK())) return fail(rc);
   last_device_ms_ = now_ms() - t1;
 
   // side effects the reference performs while it walks the pods:
@@ -1012,8 +1012,29 @@ Status BatchSchedulingPlugin::Reevaluate() {
   r.admit = admit_.data(); r.new_denied = new_denied_.data(); r.order = order_.data(); r.rank = rank_.data();
   int rc = bs_begin_cycle(eng_, now_ns_);   // matched / flags columns follow the engine's tables at now
   if (!rc) rc = bs_evaluate(eng_, &r);
+  if (!rc) rc = FetchTopK();
   if (rc) return Status{BS_CODE_ERROR, std::string("bsched: ") + bs_strerror(rc) + " (" + bs_last_error(eng_) + ")"};
   return Status{};   // (new_denied groups were deny-listed by the engine's fetch, core.go:142,163)
+}
+
+int BatchSchedulingPlugin::FetchTopK() {
+  if (!topk_) return BS_OK;
+  const uint32_t P = packed_.n_pods;
+  topk_node_.assign((size_t)P * topk_, -1);
+  topk_score_.assign((size_t)P * topk_, INT64_MIN);
+  return bs_fetch_topk_rows(eng_, 0, P, topk_node_.data(), topk_score_.data());
+}
+
+std::vector<std::pair<std::string, int64_t>> BatchSchedulingPlugin::TopNodes(const std::string& uid) const {
+  std::vector<std::pair<std::string, int64_t>> out;
+  const int32_t row = pod_row_.find(uid);
+  if (row < 0 || !topk_ || topk_node_.size() < ((size_t)row + 1) * topk_) return out;
+  for (uint32_t i = 0; i < topk_; ++i) {
+    const int32_t n = topk_node_[(size_t)row * topk_ + i];
+    if (n < 0) break;   // padding: the pod fits on fewer nodes
+    out.emplace_back((size_t)n < node_names_.size() ? node_names_[n] : std::string(), topk_score_[(size_t)row * topk_ + i]);
+  }
+  return out;
 }
 
 Status BatchSchedulingPlugin::UpdateRound(const std::vector<std::pair<uint32_t, const NodeInfo*>>& changed_nodes,

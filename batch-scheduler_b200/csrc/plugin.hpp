@@ -219,7 +219,8 @@ class StrIndex {
 class BatchSchedulingPlugin {
  public:
   // batch.New (batchscheduler.go:377): max_schedule_time from the plugin args (Configuration, :71-75)
-  BatchSchedulingPlugin(int device, int64_t max_schedule_time_ns, uint32_t out_flags = BS_OUT_FIT_BITMAP);
+  // topk > 0 adds BS_OUT_TOPK: each round also keeps every pending pod's topk best fitting nodes (TopNodes)
+  BatchSchedulingPlugin(int device, int64_t max_schedule_time_ns, uint32_t out_flags = BS_OUT_FIT_BITMAP, uint32_t topk = 0);
   ~BatchSchedulingPlugin();
   BatchSchedulingPlugin(const BatchSchedulingPlugin&) = delete;
   BatchSchedulingPlugin& operator=(const BatchSchedulingPlugin&) = delete;
@@ -276,6 +277,9 @@ class BatchSchedulingPlugin {
   const std::vector<uint32_t>& queue_order() const { return order_; }
   const std::vector<uint32_t>& feasible_counts() const { return feasible_; }
   const std::vector<int32_t>& best_nodes() const { return best_node_; }
+  // the pod's best fitting nodes of the last round (plugin created with topk > 0): (node name, residual score),
+  // score descending, then snapshot order; at most topk of them, empty for an unknown uid
+  std::vector<std::pair<std::string, int64_t>> TopNodes(const std::string& uid) const;
   int group_index(const std::string& ns_name) const;
   double last_pack_ms() const { return last_pack_ms_; }
   double last_device_ms() const { return last_device_ms_; }
@@ -329,7 +333,7 @@ class BatchSchedulingPlugin {
   bs_engine* eng_ = nullptr;
   bool state_ready_ = false;   // bs_state_reset has run for this plugin's engine lineage
   int device_ = 0;
-  uint32_t out_flags_ = 0, eng_lanes_ = 0;
+  uint32_t out_flags_ = 0, eng_lanes_ = 0, topk_ = 0;
   std::string init_error_;
   int64_t max_schedule_time_ns_;
   std::map<std::string, GroupState> groups_;                        // ordered: canonical table order
@@ -347,9 +351,12 @@ class BatchSchedulingPlugin {
   std::vector<uint8_t> prefilter_, admit_, new_denied_;
   std::vector<uint32_t> order_, rank_, feasible_;
   std::vector<int32_t> best_node_;
+  std::vector<int32_t> topk_node_;                                  // [P][topk_] (BS_OUT_TOPK)
+  std::vector<int64_t> topk_score_;
   int64_t now_ns_ = 0;
   double last_pack_ms_ = 0, last_device_ms_ = 0;
   Status Reevaluate();   // bs_evaluate into the round's result vectors + the deny side effect (core.go:142,163)
+  int FetchTopK();       // the round's top-K lists into topk_node_ / topk_score_ (no-op without topk)
 };
 
 }  // namespace bsched

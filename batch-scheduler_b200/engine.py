@@ -44,12 +44,15 @@ def _table_c(table):
 
 class Engine:
     def __init__(self, n_lanes: int, device: int = 0, fit_bitmap: bool = True, score: bool = False,
-                 filter: bool = False):
+                 filter: bool = False, topk: int = 0):
+        """topk > 0 also keeps each pod's `topk` best fitting nodes and their scores (BS_OUT_TOPK, read with
+        topk_rows); it cannot be combined with score=True, whose matrix holds them already."""
         self.lib = capi.load()
         self.n_lanes = n_lanes
+        self.topk = topk
         self.out_flags = ((capi.OUT_FIT_BITMAP if fit_bitmap else 0) | (capi.OUT_SCORE if score else 0) |
-                          (capi.OUT_FILTER if filter else 0))
-        cfg = capi.Config(device, n_lanes, self.out_flags, 0)
+                          (capi.OUT_FILTER if filter else 0) | (capi.OUT_TOPK if topk else 0))
+        cfg = capi.Config(device, n_lanes, self.out_flags, topk)
         h = C.c_void_p()
         rc = self.lib.bs_create(C.byref(cfg), C.byref(h))
         if rc != 0:
@@ -223,6 +226,15 @@ class Engine:
         out = np.zeros((n, self.N), np.int64)
         self._check(self.lib.bs_fetch_score_rows(self.h, pod0, n, capi.ptr(out)))
         return out
+
+    def topk_rows(self, pod0=0, n=None):
+        """(nodes [n, K] int32, scores [n, K] int64): each pod's fitting nodes by score descending, then node index
+        ascending; min(K, feasible_count) entries, padded with node -1 and score INT64_MIN."""
+        n = self.P - pod0 if n is None else n
+        nodes = np.zeros((n, self.topk), np.int32)
+        scores = np.zeros((n, self.topk), np.int64)
+        self._check(self.lib.bs_fetch_topk_rows(self.h, pod0, n, capi.ptr(nodes), capi.ptr(scores)))
+        return nodes, scores
 
     # -- standalone kernels ------------------------------------------------------------------
     def node_left(self, sel: int, tol: int, percent: float):

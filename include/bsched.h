@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define BS_ABI_VERSION 6
+#define BS_ABI_VERSION 7
 #define BS_FIXED_LANES 4
 #define BS_MAX_LANES 16
 /* |value| bound accepted for every int64 table entry (validated at upload):
@@ -174,12 +174,15 @@ typedef struct {
 #define BS_OUT_SCORE 0x2u      /* P x N int64 residual-capacity scores            */
 #define BS_OUT_FILTER 0x4u     /* P x ceil(N/32) u32: Filter verdict bit per (pod,node) — ScheduleOperation.Filter /
                                   computeResourceSatisfied (core.go:170-191, 514-564) against the round's max group */
+#define BS_OUT_TOPK 0x8u       /* P x K: each pod's K best fitting nodes and their scores (bs_fetch_topk_rows),
+                                  without the score matrix; not combinable with BS_OUT_SCORE */
+#define BS_TOPK_MAX 32         /* largest list length K */
 
 typedef struct {
   int32_t device;      /* CUDA device ordinal */
   uint32_t n_lanes;    /* lanes of every table uploaded to this engine */
   uint32_t out_flags;  /* BS_OUT_* */
-  uint32_t reserved;
+  uint32_t topk;       /* list length K: 1..BS_TOPK_MAX with BS_OUT_TOPK, 0 without (else bs_create -> BS_E_INVAL) */
 } bs_config;
 
 /* Host result buffers; any pointer may be NULL (that output is not copied back). */
@@ -399,6 +402,10 @@ uint32_t bs_bitmap_pitch(const bs_engine* e);
 int bs_fetch_fit_rows(bs_engine* e, uint32_t pod0, uint32_t n, uint32_t* words);
 int bs_fetch_score_rows(bs_engine* e, uint32_t pod0, uint32_t n, int64_t* scores);
 int bs_fetch_filter_rows(bs_engine* e, uint32_t pod0, uint32_t n, uint32_t* words);
+/* copy the top-K lists of pods [pod0, pod0+n) to the host as dense [n][K] rows (BS_OUT_TOPK).  Row p holds the
+ * fitting nodes of pod p ordered by score descending, then node index ascending (entry 0 = best_node / best_score),
+ * min(K, feasible_count[p]) of them, padded with node -1 and score INT64_MIN.  Either pointer may be NULL. */
+int bs_fetch_topk_rows(bs_engine* e, uint32_t pod0, uint32_t n, int32_t* nodes, int64_t* scores);
 
 /* ---- multi-GPU exchange of the admit bitmap over peer memory (NVLink / NVSwitch) ----
  * The path shards over groups (one process per GPU); the only exchange is the all-gather of the

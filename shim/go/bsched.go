@@ -23,7 +23,10 @@ import (
 
 // Engine wraps one bs_engine (one GPU).  Thread-safe: the C side serialises calls per handle, as the reference
 // calls Less / Permit from several goroutines (batchscheduler.go:165,214).
-type Engine struct{ h *C.bs_engine }
+type Engine struct {
+	h    *C.bs_engine
+	topk int // list length of BS_OUT_TOPK, 0 without it
+}
 
 // ID turns a pod UID or a "namespace/name" into the 64-bit id the gang-state calls take (FNV-1a, as
 // BatchSchedulingPlugin::IdOf does in csrc/plugin.cpp).
@@ -34,13 +37,21 @@ func ID(s string) uint64 {
 }
 
 // New replaces core.NewScheduleOperation (core.go:64-77).
-func New(device, lanes int, outFlags uint32) (*Engine, error) {
-	cfg := C.bs_config{device: C.int32_t(device), n_lanes: C.uint32_t(lanes), out_flags: C.uint32_t(outFlags)}
+func New(device, lanes int, outFlags uint32) (*Engine, error) { return NewTopK(device, lanes, outFlags, 0) }
+
+// NewTopK is New with each round also keeping every pod's topk best fitting nodes (BS_OUT_TOPK, 1..BS_TOPK_MAX;
+// 0 = none), read with TopNodes.
+func NewTopK(device, lanes int, outFlags uint32, topk int) (*Engine, error) {
+	if topk > 0 {
+		outFlags |= C.BS_OUT_TOPK
+	}
+	cfg := C.bs_config{device: C.int32_t(device), n_lanes: C.uint32_t(lanes), out_flags: C.uint32_t(outFlags),
+		topk: C.uint32_t(topk)}
 	var h *C.bs_engine
 	if rc := C.bs_create(&cfg, &h); rc != 0 {
 		return nil, fmt.Errorf("bs_create: %s", C.GoString(C.bs_strerror(rc)))
 	}
-	return &Engine{h}, nil
+	return &Engine{h, topk}, nil
 }
 
 func (e *Engine) Close() { C.bs_destroy(e.h) }
@@ -114,6 +125,18 @@ func (e *Engine) EvaluateView(nPods, nGroups int) (Round, error) {
 		Order:     unsafe.Slice((*uint32)(unsafe.Pointer(r.order)), nPods),
 		Rank:      unsafe.Slice((*uint32)(unsafe.Pointer(r.rank)), nPods),
 	}, nil
+}
+
+// TopNodes returns the top-K lists of pods [pod0, pod0+n) of the last round as dense [n][K] rows: each pod's
+// fitting nodes by score descending, then node index ascending, padded with node -1 and score math.MinInt64.
+func (e *Engine) TopNodes(pod0, n int) ([]int32, []int64, error) {
+	nodes, scores := make([]int32, n*e.topk), make([]int64, n*e.topk)
+	if len(nodes) == 0 {
+		return nodes, scores, e.rc(C.bs_fetch_topk_rows(e.h, C.uint32_t(pod0), C.uint32_t(n), nil, nil))
+	}
+	err := e.rc(C.bs_fetch_topk_rows(e.h, C.uint32_t(pod0), C.uint32_t(n), (*C.int32_t)(unsafe.Pointer(&nodes[0])),
+		(*C.int64_t)(unsafe.Pointer(&scores[0]))))
+	return nodes, scores, err
 }
 
 // PreFilter mirrors ScheduleOperation.PreFilter(pod) error (core.go:88): nil == pass.
