@@ -637,7 +637,8 @@ __global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(ReplayArgs a)
         if (tid >= 32 && tid < 32 + 2u * REPLAY_MAX_CLASSES)   // the node's block summaries are stale for every class
           sm.valid[tid - 32][(n / REPLAY_BLOCK) >> 5] &= ~(1u << ((n / REPLAY_BLOCK) & 31));
         if (tid == 32) {
-          const uint32_t rp = a.req_present[n] | req_keys;
+          // NodeInfo.AddPod adds the request's keys of lanes 4..L-1 only: a table has no lane >= L
+          const uint32_t rp = a.req_present[n] | (req_keys & ((1u << L) - 1u));
           a.req_present[n] = rp;
           a.both[n] = a.nt.alloc_present[n] & rp & ~0xFu;
         }

@@ -365,11 +365,11 @@ typedef struct bs_replay_result {
   uint8_t* ready;              /* [n_queue] Permit returned ready (core.go:303) */
   int64_t* node_requested;     /* [n_lanes][n_nodes] or NULL */
   int32_t* node_pod_count;     /* [n_nodes] or NULL */
-  uint32_t* node_req_present;  /* [n_nodes] or NULL */
+  uint32_t* node_req_present;  /* [n_nodes] or NULL; an assumed pod adds its keys of lanes 4..n_lanes-1 only */
   uint32_t* group_matched;     /* [n_groups] or NULL */
   uint8_t* group_flags;        /* [n_groups] or NULL (BS_GROUP_*) */
   int64_t* group_min_res;      /* [n_lanes][n_groups] or NULL */
-  uint32_t* group_min_res_present; /* [n_groups] or NULL */
+  uint32_t* group_min_res_present; /* [n_groups] or NULL; a group's first pod gives its whole mask, bits 0..3 cleared */
   uint64_t* group_rep_sel;     /* [n_groups] or NULL */
   uint64_t* group_rep_tol;     /* [n_groups] or NULL */
 } bs_replay_result;
