@@ -217,39 +217,51 @@ bs_group_table PackedSnapshot::group_table() const {
 
 namespace {
 
+// What encoding one row gave, in the order a caller must see them: the std::min of two results is the one to report.
+// kNeedsFull: the row holds a name the round's dictionaries have no lane or bit for (in a full pack, which built its
+// dictionaries from every row, an internal error).
+enum Encoded { kNeedsFull, kBadRequested, kBadAllocatable, kBadMinResources, kBadContainers, kEncoded };
+const char* const kEncodeError[] = {"a row outside the round's own dictionaries", "bad quantity in requested",
+                                    "bad quantity in allocatable", "bad quantity in MinResources",
+                                    "bad quantity in a pod's containers"};
+
+constexpr int kLaneIgnored = -1, kLaneUnknown = -2;
+
 struct LaneTable {
   std::vector<std::string> scalars;
   std::unordered_map<std::string, uint32_t> lane_of;
-  bool overflow = false;
-  int lane(const std::string& name, bool create) {
+  bool add(const std::string& scalar) {   // false: the lanes are used up
+    if (lane_of.count(scalar)) return true;
+    if (BS_FIXED_LANES + scalars.size() >= BS_MAX_LANES) return false;
+    lane_of.emplace(scalar, BS_FIXED_LANES + (uint32_t)scalars.size());
+    scalars.push_back(scalar);
+    return true;
+  }
+  int lane(const std::string& name) const {   // kLaneUnknown: a scalar resource without a lane
     if (name == "cpu") return kLaneCpu;
     if (name == "memory") return kLaneMem;
     if (name == "ephemeral-storage") return kLaneEph;
     if (name == "pods") return kLanePods;
-    if (!IsScalarResourceName(name)) return -1;  // Resource.Add ignores it
+    if (!IsScalarResourceName(name)) return kLaneIgnored;  // Resource.Add ignores it
     auto it = lane_of.find(name);
-    if (it != lane_of.end()) return (int)it->second;
-    if (!create) return -1;
-    if (BS_FIXED_LANES + scalars.size() >= BS_MAX_LANES) { overflow = true; return -1; }
-    const uint32_t l = BS_FIXED_LANES + (uint32_t)scalars.size();
-    scalars.push_back(name);
-    lane_of.emplace(name, l);
-    return (int)l;
+    return it == lane_of.end() ? kLaneUnknown : (int)it->second;
   }
-  void scan(const ResourceList& rl) { for (auto& kv : rl) lane(kv.first, true); }
 };
 
-// nodeinfo.Resource.Add(rl): v[lane] += quantity (cpu in milli), scalar keys become present
-bool add_list(LaneTable& lt, const ResourceList& rl, int64_t* v, uint32_t* present) {
+// nodeinfo.Resource.Add(rl): v[lane] += quantity (cpu in milli), scalar keys become present.  A scalar without a lane
+// gives kNeedsFull even after a malformed quantity (which gives `bad`): a full pack would have given it a lane.
+Encoded add_list(const LaneTable& lt, const ResourceList& rl, int64_t* v, uint32_t* present, Encoded bad) {
+  Encoded r = kEncoded;
   for (auto& kv : rl) {
-    const int l = lt.lane(kv.first, false);
+    const int l = lt.lane(kv.first);
+    if (l == kLaneUnknown) return kNeedsFull;
     if (l < 0) continue;
     int64_t q;
-    if (l == kLaneCpu ? !QuantityMilliValue(kv.second, &q) : !QuantityValue(kv.second, &q)) return false;
+    if (l == kLaneCpu ? !QuantityMilliValue(kv.second, &q) : !QuantityValue(kv.second, &q)) { r = bad; continue; }
     v[l] += q;
     if (l >= (int)BS_FIXED_LANES) *present |= 1u << l;
   }
-  return true;
+  return r;
 }
 
 const ResourceList& container_demand(const Container& c) { return c.has_limits ? c.limits : c.requests; }  // core.go:765-769
@@ -262,6 +274,9 @@ bool tolerates(const Toleration& t, const Taint& taint) {
   if (t.op == "Exists") return true;
   return false;
 }
+
+bool hard_taint(const Taint& t) { return t.effect == "NoSchedule" || t.effect == "NoExecute"; }  // PodToleratesNodeTaints
+bool same_taint(const Taint& a, const Taint& b) { return a.key == b.key && a.value == b.value && a.effect == b.effect; }
 
 // threads for the packer: BS_HOST_THREADS, else up to 8 (small inputs stay single-threaded)
 int pack_threads(size_t objects) {
@@ -313,15 +328,129 @@ bool aff_class_matches(const PackedSnapshot::AffClassDef& c, const Node& nd) {
   return !c.has_required_affinity || MatchNodeSelectorTerms(c.terms, nd.labels, nd.name);
 }
 
-struct PackGroupIn {
-  const PodGroup* pg;
-  uint32_t matched;
-  uint8_t flags;        // BS_GROUP_SCHEDULED | BS_GROUP_HAS_POD | BS_GROUP_DENIED (HAS_MINRES derived)
-  const Pod* rep_pod;   // pgs.Pod or nullptr
+// The row encoding of one round, from the dictionaries a full pack keeps in its PackedSnapshot (scalar_names,
+// sel_pairs, taint_list, sel_in_table, aff_signatures).  The full pack and the row re-packs both encode through it,
+// so a re-packed row carries exactly the bits the full pack gives the same object.  The constructor sizes the node
+// and group columns of `out` for out.n_nodes / out.n_groups rows, at the values of a row or field the methods leave
+// out; the methods write the columns at (row, lane stride) and change nothing else, so rows may be encoded from
+// several threads at once.
+class RowEncoder {
+ public:
+  RowEncoder(const PackedSnapshot& dict, PackedSnapshot& out) : dict_(dict), out_(out) {
+    for (auto& nm : dict.scalar_names) lanes_.add(nm);
+    for (size_t b = 0; b < dict.sel_pairs.size(); ++b) sel_bit_.emplace(dict.sel_pairs[b], (int)b);
+    for (size_t c = 0; c < dict.aff_signatures.size(); ++c) aff_class_.emplace(dict.aff_signatures[c], (uint32_t)c);
+    const size_t L = dict.lanes, N = out.n_nodes, G = out.n_groups;
+    out.alloc.assign(L * N, 0); out.requested.assign(L * N, 0);
+    out.pod_count.assign(N, 0); out.alloc_present.assign(N, 0); out.req_present.assign(N, 0);
+    out.label_mask.assign(N, 0); out.taint_mask.assign(N, 0); out.node_flags.assign(N, 0);
+    out.min_member.assign(G, 0); out.scheduled.assign(G, 0); out.matched.assign(G, 0); out.group_flags.assign(G, 0);
+    out.min_res.assign(L * G, 0); out.min_res_present.assign(G, 0); out.rep_sel.assign(G, 0);
+    out.rep_tol.assign(G, 0); out.creation_ns.assign(G, 0); out.name_rank.assign(G, 0); out.wait_ns.assign(G, 0);
+    out.rep_aff.assign(G, BS_AFF_NONE);
+  }
+
+  Encoded node(const NodeInfo* ni, uint32_t i, uint32_t stride) const {
+    if (!ni) { out_.node_flags[i] = BS_NODE_NIL; return kEncoded; }                   // core.go:606
+    const Node* nd = ni->node;
+    int64_t req[BS_MAX_LANES] = {}, alloc[BS_MAX_LANES] = {};
+    uint32_t req_pres = 0, alloc_pres = 0;
+    const Encoded r = std::min(add_list(lanes_, ni->requested, req, &req_pres, kBadRequested),
+                               nd ? add_list(lanes_, nd->allocatable, alloc, &alloc_pres, kBadAllocatable) : kEncoded);
+    if (r != kEncoded) return r;
+    uint8_t fl = 0;
+    if (!nd) fl |= BS_NODE_NO_NODE;                                                    // core.go:610
+    if (ni->taints_error) fl |= BS_NODE_TAINTS_ERR;                                    // core.go:639
+    if (nd && nd->unschedulable) fl |= BS_NODE_UNSCHEDULABLE;                          // core.go:615
+    out_.node_flags[i] = fl;
+    out_.pod_count[i] = ni->num_pods;
+    for (uint32_t d = 0; d < dict_.lanes; ++d) {
+      out_.requested[(size_t)d * stride + i] = req[d];
+      out_.alloc[(size_t)d * stride + i] = alloc[d];
+    }
+    out_.req_present[i] = req_pres;
+    out_.alloc_present[i] = alloc_pres;
+    if (!nd) return kEncoded;
+    for (size_t b = 0; b < dict_.sel_pairs.size(); ++b) {
+      auto it = nd->labels.find(dict_.sel_pairs[b].first);
+      if (it != nd->labels.end() && it->second == dict_.sel_pairs[b].second) out_.label_mask[i] |= 1ull << b;
+    }
+    for (auto& t : nd->taints) {
+      if (!hard_taint(t)) continue;
+      const int b = taint_bit(t);
+      if (b < 0) return kNeedsFull;   // a taint no toleration mask of the round has a bit for
+      out_.taint_mask[i] |= 1ull << b;
+    }
+    return kEncoded;
+  }
+
+  // everything of a group's row but name_rank, which depends on the other groups' names
+  Encoded group(const BatchSchedulingPlugin::GroupDelta& gd, uint32_t k, uint32_t stride, int64_t default_wait_ns) const {
+    const PodGroup& pg = *gd.pg;
+    out_.min_member[k] = pg.min_member;
+    out_.scheduled[k] = pg.scheduled;
+    out_.matched[k] = gd.matched;
+    out_.creation_ns[k] = pg.creation_ns;
+    // util.GetWaitTimeDuration (k8s.go:82-91): Spec.MaxScheduleTime wins, else the plugin default
+    out_.wait_ns[k] = pg.max_schedule_time_ns >= 0 ? pg.max_schedule_time_ns : default_wait_ns;
+    uint8_t fl = gd.flags & (BS_GROUP_SCHEDULED | BS_GROUP_HAS_POD | BS_GROUP_DENIED);
+    if (pg.has_min_resources) {
+      fl |= BS_GROUP_HAS_MINRES;
+      int64_t v[BS_MAX_LANES] = {};
+      uint32_t pres = 0;
+      const Encoded r = add_list(lanes_, pg.min_resources, v, &pres, kBadMinResources);
+      if (r != kEncoded) return r;
+      for (uint32_t d = 0; d < dict_.lanes; ++d) out_.min_res[(size_t)d * stride + k] = v[d];
+      out_.min_res_present[k] = pres;
+    }
+    if (gd.rep_pod) {
+      fl |= BS_GROUP_HAS_POD;
+      const std::string sig = aff_signature(*gd.rep_pod, dict_.sel_in_table);
+      if (!sig.empty()) {
+        auto it = aff_class_.find(sig);
+        if (it == aff_class_.end()) return kNeedsFull;   // a predicate the round's table has no row for
+        out_.rep_aff[k] = it->second;
+      }
+      const Encoded r = pod_masks(*gd.rep_pod, &out_.rep_sel[k], &out_.rep_tol[k]);
+      if (r != kEncoded) return r;
+    }
+    out_.group_flags[k] = fl;
+    return kEncoded;
+  }
+
+  // nodeSelector pairs -> selector bits (none while the selectors live in the affinity table), tolerations -> the
+  // bits of the taints they tolerate
+  Encoded pod_masks(const Pod& p, uint64_t* sel, uint64_t* tol) const {
+    *sel = 0;
+    *tol = 0;
+    if (!dict_.sel_in_table)
+      for (auto& kv : p.node_selector) {
+        auto it = sel_bit_.find(kv);
+        if (it == sel_bit_.end()) return kNeedsFull;   // the nodes' label masks have no bit for this pair
+        *sel |= 1ull << it->second;
+      }
+    for (size_t b = 0; b < dict_.taint_list.size(); ++b)
+      for (auto& tl : p.tolerations)
+        if (tolerates(tl, dict_.taint_list[b])) { *tol |= 1ull << b; break; }
+    return kEncoded;
+  }
+
+ private:
+  int taint_bit(const Taint& t) const {
+    for (size_t b = 0; b < dict_.taint_list.size(); ++b)
+      if (same_taint(dict_.taint_list[b], t)) return (int)b;
+    return -1;
+  }
+
+  const PackedSnapshot& dict_;
+  PackedSnapshot& out_;
+  LaneTable lanes_;
+  std::map<std::pair<std::string, std::string>, int> sel_bit_;
+  std::unordered_map<std::string, uint32_t> aff_class_;
 };
 
 Status pack_impl(const std::vector<const NodeInfo*>& snapshot, const std::vector<const Pod*>& pending,
-                 const std::vector<PackGroupIn>& groups, const std::vector<uint8_t>& pod_flags_in,
+                 const std::vector<BatchSchedulingPlugin::GroupDelta>& groups, const std::vector<uint8_t>& pod_flags_in,
                  int64_t default_wait_ns, PackedSnapshot* out) {
   Status bad{BS_CODE_ERROR, ""};
   PackedSnapshot& ps = *out;
@@ -346,8 +475,7 @@ Status pack_impl(const std::vector<const NodeInfo*>& snapshot, const std::vector
     auto note = [&](std::vector<Seen>& mine, uint64_t pos, const ResourceList& rl) {
       for (auto& kv : rl) {
         const std::string& nm = kv.first;
-        if (nm == "cpu" || nm == "memory" || nm == "ephemeral-storage" || nm == "pods") continue;
-        if (!IsScalarResourceName(nm)) continue;
+        if (lt.lane(nm) != kLaneUnknown) continue;   // lt stays empty until the merge: only the scalars are noted
         bool dup = false;
         for (auto& s2 : mine) if (s2.name == nm) { dup = true; break; }
         if (!dup) mine.push_back(Seen{pos, nm});
@@ -377,9 +505,9 @@ Status pack_impl(const std::vector<const NodeInfo*>& snapshot, const std::vector
     std::vector<Seen> all;
     for (auto& v : seen) all.insert(all.end(), v.begin(), v.end());
     std::stable_sort(all.begin(), all.end(), [](const Seen& a, const Seen& b) { return a.pos < b.pos; });
-    for (auto& s2 : all) lt.lane(s2.name, true);
+    for (auto& s2 : all)
+      if (!lt.add(s2.name)) { bad.message = "more than 12 scalar resources"; return bad; }
   }
-  if (lt.overflow) { bad.message = "more than 12 scalar resources"; return bad; }
   phase("lane scan");
   const uint32_t L = BS_FIXED_LANES + (uint32_t)lt.scalars.size();
   ps.lanes = L;
@@ -387,15 +515,13 @@ Status pack_impl(const std::vector<const NodeInfo*>& snapshot, const std::vector
   ps.n_nodes = N; ps.n_pods = P; ps.n_groups = G;
 
   // ---- selector pairs and taints -> bits
-  std::map<std::pair<std::string, std::string>, int> sel_bit;
-  auto scan_sel = [&](const Pod* p) { for (auto& kv : p->node_selector) sel_bit.emplace(kv, 0); };
-  for (auto* p : pending) scan_sel(p);
-  for (auto& g : groups) if (g.rep_pod) scan_sel(g.rep_pod);
+  std::set<std::pair<std::string, std::string>> pairs;
+  for (auto* p : pending) pairs.insert(p->node_selector.begin(), p->node_selector.end());
+  for (auto& g : groups) if (g.rep_pod) pairs.insert(g.rep_pod->node_selector.begin(), g.rep_pod->node_selector.end());
   // more than 64 distinct pairs: every nodeSelector moves into the affinity table (one class per distinct
   // selector map), the 64-bit masks stay zero
-  ps.sel_in_table = sel_bit.size() > 64;
-  if (ps.sel_in_table) sel_bit.clear();
-  { int b = 0; for (auto& kv : sel_bit) kv.second = b++; }
+  ps.sel_in_table = pairs.size() > 64;
+  if (!ps.sel_in_table) ps.sel_pairs.assign(pairs.begin(), pairs.end());
   // ---- affinity classes: first-seen order over the pending pods, then the groups' representatives
   {
     std::unordered_map<std::string, uint32_t> cls;
@@ -415,73 +541,34 @@ Status pack_impl(const std::vector<const NodeInfo*>& snapshot, const std::vector
       return id;
     };
     ps.aff_class.assign(P, BS_AFF_NONE);
-    ps.rep_aff.assign(G, BS_AFF_NONE);
     bool any = ps.sel_in_table;
     for (uint32_t i = 0; i < P && !any; ++i) any = pending[i]->has_required_affinity;
     for (uint32_t g = 0; g < G && !any; ++g) any = groups[g].rep_pod && groups[g].rep_pod->has_required_affinity;
     if (any) {
       for (uint32_t i = 0; i < P; ++i) ps.aff_class[i] = class_of(*pending[i]);
-      for (uint32_t g = 0; g < G; ++g) if (groups[g].rep_pod) ps.rep_aff[g] = class_of(*groups[g].rep_pod);
+      for (uint32_t g = 0; g < G; ++g) if (groups[g].rep_pod) class_of(*groups[g].rep_pod);   // rep_aff: RowEncoder::group
     }
   }
-  std::vector<Taint> taints;
-  auto taint_bit = [&](const Taint& t) -> int {
-    for (size_t i = 0; i < taints.size(); ++i)
-      if (taints[i].key == t.key && taints[i].value == t.value && taints[i].effect == t.effect) return (int)i;
-    taints.push_back(t);
-    return (int)taints.size() - 1;
-  };
-  // ---- nodes
-  ps.alloc.assign((size_t)L * N, 0); ps.requested.assign((size_t)L * N, 0);
-  ps.pod_count.assign(N, 0); ps.alloc_present.assign(N, 0); ps.req_present.assign(N, 0);
-  ps.label_mask.assign(N, 0); ps.taint_mask.assign(N, 0); ps.node_flags.assign(N, 0);
   phase("selectors");
-  // taints: sequential pre-pass (first-seen order defines the bit), then the nodes in parallel
+  // taints: first-seen order defines the bit
   for (uint32_t i = 0; i < N; ++i) {
     const NodeInfo* ni = snapshot[i];
     if (!ni || !ni->node) continue;
     for (auto& t : ni->node->taints)
-      if (t.effect == "NoSchedule" || t.effect == "NoExecute") taint_bit(t);   // PodToleratesNodeTaints filter
+      if (hard_taint(t) && std::none_of(ps.taint_list.begin(), ps.taint_list.end(), [&](const Taint& u) { return same_taint(u, t); }))
+        ps.taint_list.push_back(t);
   }
-  if (taints.size() > 64) { bad.message = "more than 64 distinct taints in one round"; return bad; }
-  ps.sel_pairs.resize(sel_bit.size());
-  for (auto& kv : sel_bit) ps.sel_pairs[kv.second] = kv.first;
-  ps.taint_list = taints;
-  std::atomic<int> err{0};
+  if (ps.taint_list.size() > 64) { bad.message = "more than 64 distinct taints in one round"; return bad; }
+  // ---- rows, through the encoding PackNodeRows / PackGroupRows use
+  const RowEncoder enc(ps, ps);
+  std::atomic<int> err{kEncoded};
+  auto failed = [&] { bad.message = kEncodeError[err]; return bad; };
 #pragma omp parallel for num_threads(T) schedule(static)
   for (uint32_t i = 0; i < N; ++i) {
-    const NodeInfo* ni = snapshot[i];
-    if (!ni) { ps.node_flags[i] = BS_NODE_NIL; continue; }              // core.go:606
-    int64_t tmp[BS_MAX_LANES] = {};
-    if (!ni->node) ps.node_flags[i] |= BS_NODE_NO_NODE;                 // core.go:610
-    if (ni->taints_error) ps.node_flags[i] |= BS_NODE_TAINTS_ERR;       // core.go:639
-    ps.pod_count[i] = ni->num_pods;
-    uint32_t pres = 0;
-    if (!add_list(lt, ni->requested, tmp, &pres)) { err = 1; continue; }
-    for (uint32_t d = 0; d < L; ++d) ps.requested[(size_t)d * N + i] = tmp[d];
-    ps.req_present[i] = pres;
-    if (!ni->node) continue;
-    const Node& nd = *ni->node;
-    if (nd.unschedulable) ps.node_flags[i] |= BS_NODE_UNSCHEDULABLE;    // core.go:615
-    pres = 0;
-    std::fill(tmp, tmp + BS_MAX_LANES, 0);
-    if (!add_list(lt, nd.allocatable, tmp, &pres)) { err = 2; continue; }
-    for (uint32_t d = 0; d < L; ++d) ps.alloc[(size_t)d * N + i] = tmp[d];
-    ps.alloc_present[i] = pres;
-    for (auto& kv : sel_bit) {
-      auto it = nd.labels.find(kv.first.first);
-      if (it != nd.labels.end() && it->second == kv.first.second) ps.label_mask[i] |= 1ull << kv.second;
-    }
-    for (auto& t : nd.taints) {
-      if (t.effect != "NoSchedule" && t.effect != "NoExecute") continue;
-      for (size_t b = 0; b < taints.size(); ++b)
-        if (taints[b].key == t.key && taints[b].value == t.value && taints[b].effect == t.effect) {
-          ps.taint_mask[i] |= 1ull << b;
-          break;
-        }
-    }
+    const Encoded r = enc.node(snapshot[i], i, N);
+    if (r != kEncoded) err = r;
   }
-  if (err) { bad.message = err == 1 ? "bad quantity in requested" : "bad quantity in allocatable"; return bad; }
+  if (err != kEncoded) return failed();
   phase("nodes");
   // ---- (affinity class, node) verdicts, evaluated on the host once per class and node
   {
@@ -499,23 +586,14 @@ Status pack_impl(const std::vector<const NodeInfo*>& snapshot, const std::vector
       }
   }
   phase("affinity");
-  auto pod_masks = [&](const Pod& p, uint64_t* sel, uint64_t* tol) {
-    *sel = 0; *tol = 0;
-    if (!ps.sel_in_table)
-      for (auto& kv : p.node_selector) *sel |= 1ull << sel_bit.at(kv);
-    for (size_t b = 0; b < taints.size(); ++b)
-      for (auto& t : p.tolerations)
-        if (tolerates(t, taints[b])) { *tol |= 1ull << b; break; }
-  };
-  auto pod_demand = [&](const Pod& p, int64_t* v, uint32_t* pres) -> bool {  // getPodResourceRequire core.go:761-772
-    for (auto& c : p.containers)
-      if (!add_list(lt, container_demand(c), v, pres)) return false;
-    return true;
+  auto pod_demand = [&](const Pod& p, int64_t* v, uint32_t* pres) {  // getPodResourceRequire core.go:761-772
+    for (auto& c : p.containers) {
+      const Encoded r = add_list(lt, container_demand(c), v, pres, kBadContainers);
+      if (r != kEncoded) return r;
+    }
+    return kEncoded;
   };
   // ---- groups
-  ps.min_member.assign(G, 0); ps.scheduled.assign(G, 0); ps.matched.assign(G, 0); ps.group_flags.assign(G, 0);
-  ps.min_res.assign((size_t)L * G, 0); ps.min_res_present.assign(G, 0); ps.rep_sel.assign(G, 0);
-  ps.rep_tol.assign(G, 0); ps.creation_ns.assign(G, 0); ps.name_rank.assign(G, 0); ps.wait_ns.assign(G, 0);
   // bare-name ranks, byte-wise ascending (Go string compare); equal names share a rank (core.go:404)
   // (sorted on the big-endian first 8 bytes as an integer; the strings are compared only where those tie)
   std::vector<uint32_t> by_name(G);
@@ -583,29 +661,11 @@ Status pack_impl(const std::vector<const NodeInfo*>& snapshot, const std::vector
   };
 #pragma omp parallel for num_threads(T) schedule(static)
   for (uint32_t g = 0; g < G; ++g) {
-    const PodGroup& pg = *groups[g].pg;
-    int64_t tmp[BS_MAX_LANES] = {};
-    ps.min_member[g] = pg.min_member;
-    ps.scheduled[g] = pg.scheduled;
-    ps.matched[g] = groups[g].matched;
-    ps.group_flags[g] = groups[g].flags & (BS_GROUP_SCHEDULED | BS_GROUP_HAS_POD | BS_GROUP_DENIED);
-    ps.creation_ns[g] = pg.creation_ns;
     ps.name_rank[g] = rank_of_group[g];
-    // util.GetWaitTimeDuration (k8s.go:82-91): Spec.MaxScheduleTime wins, else the plugin default
-    ps.wait_ns[g] = pg.max_schedule_time_ns >= 0 ? pg.max_schedule_time_ns : default_wait_ns;
-    if (pg.has_min_resources) {
-      ps.group_flags[g] |= BS_GROUP_HAS_MINRES;
-      uint32_t pres = 0;
-      if (!add_list(lt, pg.min_resources, tmp, &pres)) { err = 3; continue; }
-      for (uint32_t d = 0; d < L; ++d) ps.min_res[(size_t)d * G + g] = tmp[d];
-      ps.min_res_present[g] = pres;
-    }
-    if (groups[g].rep_pod) {
-      ps.group_flags[g] |= BS_GROUP_HAS_POD;
-      pod_masks(*groups[g].rep_pod, &ps.rep_sel[g], &ps.rep_tol[g]);
-    }
+    const Encoded r = enc.group(groups[g], g, G, default_wait_ns);
+    if (r != kEncoded) err = r;
   }
-  if (err) { bad.message = "bad quantity in MinResources"; return bad; }
+  if (err != kEncoded) return failed();
   phase("groups");
   // ---- pods (arrival order): demand / masks / group lookup in parallel, then the occupancy
   // rule sequentially, as fillOccupiedObj is order dependent (core.go:494-511)
@@ -617,10 +677,11 @@ Status pack_impl(const std::vector<const NodeInfo*>& snapshot, const std::vector
     const Pod& p = *pending[i];
     uint32_t pres = 0;
     int64_t tmp[BS_MAX_LANES] = {};
-    if (!pod_demand(p, tmp, &pres)) { err = 4; continue; }
+    Encoded r = pod_demand(p, tmp, &pres);
+    if (r == kEncoded) r = enc.pod_masks(p, &ps.sel_mask[i], &ps.tol_mask[i]);
+    if (r != kEncoded) { err = r; continue; }
     for (uint32_t d = 0; d < L; ++d) ps.req[(size_t)d * P + i] = tmp[d];
     ps.pod_req_present[i] = pres;
-    pod_masks(p, &ps.sel_mask[i], &ps.tol_mask[i]);
     ps.priority[i] = p.priority;
     ps.ts_ns[i] = p.queue_ts_ns;
     uint8_t fl = i < pod_flags_in.size() ? pod_flags_in[i] : 0;
@@ -632,7 +693,7 @@ Status pack_impl(const std::vector<const NodeInfo*>& snapshot, const std::vector
     }
     ps.pod_flags[i] = fl;
   }
-  if (err) { bad.message = "bad quantity in a pod's containers"; return bad; }
+  if (err != kEncoded) return failed();
   phase("pods par");
   // fillOccupiedObj runs when a pod is popped, i.e. in QUEUE order (Less = Compare, core.go:368-411), not in
   // arrival order: with an empty OccupiedBy and pods of one group carrying different ownerRefs, the first pod
@@ -685,11 +746,19 @@ Status BatchSchedulingPlugin::Pack(const std::vector<const NodeInfo*>& snapshot,
                                    const std::vector<uint8_t>& extra_group_flags,
                                    const std::vector<uint8_t>& extra_pod_flags, int64_t default_wait_ns,
                                    PackedSnapshot* out) {
-  std::vector<PackGroupIn> gi(groups.size());
+  std::vector<GroupDelta> gd(groups.size());
   for (size_t g = 0; g < groups.size(); ++g)
-    gi[g] = PackGroupIn{&groups[g], g < matched.size() ? matched[g] : 0u,
-                        g < extra_group_flags.size() ? extra_group_flags[g] : (uint8_t)0, nullptr};
-  return pack_impl(snapshot, pending, gi, extra_pod_flags, default_wait_ns, out);
+    gd[g] = GroupDelta{(uint32_t)g, &groups[g], g < matched.size() ? matched[g] : 0u,
+                       g < extra_group_flags.size() ? extra_group_flags[g] : (uint8_t)0, nullptr};
+  return Pack(snapshot, pending, gd, extra_pod_flags, default_wait_ns, out);
+}
+
+Status BatchSchedulingPlugin::Pack(const std::vector<const NodeInfo*>& snapshot, const std::vector<const Pod*>& pending,
+                                   const std::vector<GroupDelta>& groups, const std::vector<uint8_t>& extra_pod_flags,
+                                   int64_t default_wait_ns, PackedSnapshot* out) {
+  for (auto& g : groups)
+    if (!g.pg) return Status{BS_CODE_ERROR, "Pack: null PodGroup"};
+  return pack_impl(snapshot, pending, groups, extra_pod_flags, default_wait_ns, out);
 }
 
 BatchSchedulingPlugin::BatchSchedulingPlugin(int device, int64_t max_schedule_time_ns, uint32_t out_flags, uint32_t topk)
@@ -823,13 +892,13 @@ Status BatchSchedulingPlugin::BeginRound(const std::vector<const NodeInfo*>& sna
     const int rc = bs_state_view(eng_, now_ns, Gn, st_matched.data(), st_flags.data());
     if (rc) return Status{BS_CODE_ERROR, std::string("bsched: ") + bs_strerror(rc)};
   }
-  std::vector<PackGroupIn> gin;
+  std::vector<GroupDelta> gin;
   gin.reserve(Gn);
   {
     uint32_t g = 0;
     for (auto& kv : groups_) {
       GroupState& gs = kv.second;
-      gin.push_back(PackGroupIn{&gs.pg, st_matched[g], st_flags[g], gs.has_pod ? &gs.rep_pod : nullptr});
+      gin.push_back(GroupDelta{g, &gs.pg, st_matched[g], st_flags[g], gs.has_pod ? &gs.rep_pod : nullptr});
       ++g;
     }
   }
@@ -943,8 +1012,8 @@ Status BatchSchedulingPlugin::PackNodeRows(const PackedSnapshot& ctx, const std:
   *needs_full = false;
   PackedSnapshot& ps = *out;
   ps = PackedSnapshot();
-  const uint32_t n = (uint32_t)rows.size(), L = ctx.lanes;
-  ps.lanes = L; ps.scalar_names = ctx.scalar_names; ps.sel_pairs = ctx.sel_pairs; ps.taint_list = ctx.taint_list;
+  const uint32_t n = (uint32_t)rows.size();
+  ps.lanes = ctx.lanes; ps.scalar_names = ctx.scalar_names; ps.sel_pairs = ctx.sel_pairs; ps.taint_list = ctx.taint_list;
   ps.n_nodes = n;
   // affinity verdicts of the changed rows: aff_bits[c * n + k] = 0 / 1 (one word per (class, row); the
   // caller patches the round's bit table with them)
@@ -955,53 +1024,11 @@ Status BatchSchedulingPlugin::PackNodeRows(const PackedSnapshot& ctx, const std:
   for (uint32_t c = 0; c < ctx.n_aff(); ++c)
     for (uint32_t k = 0; k < n; ++k)
       if (rows[k] && rows[k]->node && aff_class_matches(ctx.aff_classes[c], *rows[k]->node)) ps.aff_bits[(size_t)c * n + k] = 1;
-  LaneTable lt;   // the lanes of the full pack, nothing may be added
-  for (auto& nm : ctx.scalar_names) lt.lane(nm, true);
-  auto known = [&](const ResourceList& rl) {
-    for (auto& kv : rl) {
-      const std::string& nm = kv.first;
-      if (nm == "cpu" || nm == "memory" || nm == "ephemeral-storage" || nm == "pods") continue;
-      if (IsScalarResourceName(nm) && lt.lane(nm, false) < 0) return false;
-    }
-    return true;
-  };
-  ps.alloc.assign((size_t)L * n, 0); ps.requested.assign((size_t)L * n, 0);
-  ps.pod_count.assign(n, 0); ps.alloc_present.assign(n, 0); ps.req_present.assign(n, 0);
-  ps.label_mask.assign(n, 0); ps.taint_mask.assign(n, 0); ps.node_flags.assign(n, 0);
+  const RowEncoder enc(ctx, ps);
   for (uint32_t i = 0; i < n; ++i) {
-    const NodeInfo* ni = rows[i];
-    if (!ni) { ps.node_flags[i] = BS_NODE_NIL; continue; }              // core.go:606
-    if (!known(ni->requested) || (ni->node && !known(ni->node->allocatable))) { *needs_full = true; return Status{}; }
-    int64_t tmp[BS_MAX_LANES] = {};
-    if (!ni->node) ps.node_flags[i] |= BS_NODE_NO_NODE;                 // core.go:610
-    if (ni->taints_error) ps.node_flags[i] |= BS_NODE_TAINTS_ERR;       // core.go:639
-    ps.pod_count[i] = ni->num_pods;
-    uint32_t pres = 0;
-    if (!add_list(lt, ni->requested, tmp, &pres)) return Status{BS_CODE_ERROR, "bad quantity in requested"};
-    for (uint32_t d = 0; d < L; ++d) ps.requested[(size_t)d * n + i] = tmp[d];
-    ps.req_present[i] = pres;
-    if (!ni->node) continue;
-    const Node& nd = *ni->node;
-    if (nd.unschedulable) ps.node_flags[i] |= BS_NODE_UNSCHEDULABLE;    // core.go:615
-    pres = 0;
-    std::fill(tmp, tmp + BS_MAX_LANES, 0);
-    if (!add_list(lt, nd.allocatable, tmp, &pres)) return Status{BS_CODE_ERROR, "bad quantity in allocatable"};
-    for (uint32_t d = 0; d < L; ++d) ps.alloc[(size_t)d * n + i] = tmp[d];
-    ps.alloc_present[i] = pres;
-    for (size_t b = 0; b < ctx.sel_pairs.size(); ++b) {
-      auto it = nd.labels.find(ctx.sel_pairs[b].first);
-      if (it != nd.labels.end() && it->second == ctx.sel_pairs[b].second) ps.label_mask[i] |= 1ull << b;
-    }
-    for (auto& t : nd.taints) {
-      if (t.effect != "NoSchedule" && t.effect != "NoExecute") continue;   // PodToleratesNodeTaints filter
-      bool found = false;
-      for (size_t b = 0; b < ctx.taint_list.size() && !found; ++b)
-        if (ctx.taint_list[b].key == t.key && ctx.taint_list[b].value == t.value && ctx.taint_list[b].effect == t.effect) {
-          ps.taint_mask[i] |= 1ull << b;
-          found = true;
-        }
-      if (!found) { *needs_full = true; return Status{}; }   // a taint no toleration mask of the round knows
-    }
+    const Encoded r = enc.node(rows[i], i, n);
+    if (r == kNeedsFull) { *needs_full = true; return Status{}; }
+    if (r != kEncoded) return Status{BS_CODE_ERROR, kEncodeError[r]};
   }
   return Status{};
 }
@@ -1099,63 +1126,17 @@ Status BatchSchedulingPlugin::PackGroupRows(const PackedSnapshot& ctx, const std
   *needs_full = false;
   PackedSnapshot& ps = *out;
   ps = PackedSnapshot();
-  const uint32_t n = (uint32_t)rows.size(), L = ctx.lanes;
-  ps.lanes = L; ps.scalar_names = ctx.scalar_names; ps.sel_pairs = ctx.sel_pairs; ps.taint_list = ctx.taint_list;
+  const uint32_t n = (uint32_t)rows.size();
+  ps.lanes = ctx.lanes; ps.scalar_names = ctx.scalar_names; ps.sel_pairs = ctx.sel_pairs; ps.taint_list = ctx.taint_list;
   ps.n_groups = n;
-  LaneTable lt;
-  for (auto& nm : ctx.scalar_names) lt.lane(nm, true);
-  ps.min_member.assign(n, 0); ps.scheduled.assign(n, 0); ps.matched.assign(n, 0); ps.group_flags.assign(n, 0);
-  ps.min_res.assign((size_t)L * n, 0); ps.min_res_present.assign(n, 0); ps.rep_sel.assign(n, 0);
-  ps.rep_tol.assign(n, 0); ps.creation_ns.assign(n, 0); ps.name_rank.assign(n, 0); ps.wait_ns.assign(n, 0);
-  ps.rep_aff.assign(n, BS_AFF_NONE);
+  const RowEncoder enc(ctx, ps);
   for (uint32_t k = 0; k < n; ++k) {
     const GroupDelta& gd = rows[k];
     if (!gd.pg || gd.index >= ctx.n_groups) return Status{BS_CODE_ERROR, "PackGroupRows: bad row"};
-    const PodGroup& pg = *gd.pg;
-    ps.min_member[k] = pg.min_member;
-    ps.scheduled[k] = pg.scheduled;
-    ps.matched[k] = gd.matched;
-    ps.group_flags[k] = gd.flags & (BS_GROUP_SCHEDULED | BS_GROUP_HAS_POD | BS_GROUP_DENIED);
-    ps.creation_ns[k] = pg.creation_ns;
     ps.name_rank[k] = ctx.name_rank[gd.index];   // the name of an object does not change
-    ps.wait_ns[k] = pg.max_schedule_time_ns >= 0 ? pg.max_schedule_time_ns : default_wait_ns;   // k8s.go:82-91
-    if (pg.has_min_resources) {
-      for (auto& kv : pg.min_resources) {
-        const std::string& nm = kv.first;
-        if (nm == "cpu" || nm == "memory" || nm == "ephemeral-storage" || nm == "pods") continue;
-        if (IsScalarResourceName(nm) && lt.lane(nm, false) < 0) { *needs_full = true; return Status{}; }
-      }
-      ps.group_flags[k] |= BS_GROUP_HAS_MINRES;
-      int64_t tmp[BS_MAX_LANES] = {};
-      uint32_t pres = 0;
-      if (!add_list(lt, pg.min_resources, tmp, &pres)) return Status{BS_CODE_ERROR, "bad quantity in MinResources"};
-      for (uint32_t d = 0; d < L; ++d) ps.min_res[(size_t)d * n + k] = tmp[d];
-      ps.min_res_present[k] = pres;
-    }
-    if (gd.rep_pod) {
-      ps.group_flags[k] |= BS_GROUP_HAS_POD;
-      const std::string sig = aff_signature(*gd.rep_pod, ctx.sel_in_table);
-      if (!sig.empty()) {
-        uint32_t cid = BS_AFF_NONE;
-        for (uint32_t c = 0; c < ctx.n_aff(); ++c)
-          if (ctx.aff_signatures[c] == sig) { cid = c; break; }
-        if (cid == BS_AFF_NONE) { *needs_full = true; return Status{}; }   // a predicate the round's table has no row for
-        ps.rep_aff[k] = cid;
-      }
-      for (auto& kv : gd.rep_pod->node_selector) {
-        if (ctx.sel_in_table) break;
-        bool found = false;
-        for (size_t b = 0; b < ctx.sel_pairs.size() && !found; ++b)
-          if (ctx.sel_pairs[b] == std::pair<std::string, std::string>(kv.first, kv.second)) {
-            ps.rep_sel[k] |= 1ull << b;
-            found = true;
-          }
-        if (!found) { *needs_full = true; return Status{}; }   // the nodes' label masks have no bit for this pair
-      }
-      for (size_t b = 0; b < ctx.taint_list.size(); ++b)
-        for (auto& t : gd.rep_pod->tolerations)
-          if (tolerates(t, ctx.taint_list[b])) { ps.rep_tol[k] |= 1ull << b; break; }
-    }
+    const Encoded r = enc.group(gd, k, n, default_wait_ns);
+    if (r == kNeedsFull) { *needs_full = true; return Status{}; }
+    if (r != kEncoded) return Status{BS_CODE_ERROR, kEncodeError[r]};
   }
   return Status{};
 }

@@ -320,6 +320,11 @@ class BatchSchedulingPlugin {
                      const std::vector<PodGroup>& groups, const std::vector<uint32_t>& matched,
                      const std::vector<uint8_t>& extra_group_flags, const std::vector<uint8_t>& extra_pod_flags,
                      int64_t default_wait_ns, PackedSnapshot* out);
+  // the same with each group given as a GroupDelta (object, matched count, flags, representative pod); a group's
+  // row is its position in `groups`, GroupDelta::index is not read
+  static Status Pack(const std::vector<const NodeInfo*>& snapshot, const std::vector<const Pod*>& pending,
+                     const std::vector<GroupDelta>& groups, const std::vector<uint8_t>& extra_pod_flags,
+                     int64_t default_wait_ns, PackedSnapshot* out);
 
  private:
   // MatchedPodNodes / PodNameUIDs / pgs.Scheduled and the deny / permitted caches live in the ENGINE (bs_state_*,
