@@ -17,11 +17,14 @@ AFF_NONE = 0xffffffff
 BS_OK, BS_E_INVAL, BS_E_NODEVICE, BS_E_CUDA, BS_E_NOMEM, BS_E_RANGE, BS_E_STATE, BS_E_REF_PANIC, BS_E_INDEX, BS_E_PEER = \
     0, -1, -2, -3, -4, -5, -6, -7, -8, -9
 CODE_SUCCESS, CODE_ERROR, CODE_UNSCHEDULABLE, CODE_UNSCHEDULABLE_AND_UNRESOLVABLE, CODE_WAIT, CODE_SKIP = range(6)
-OUT_FIT_BITMAP, OUT_SCORE, OUT_FILTER, OUT_TOPK = 0x1, 0x2, 0x4, 0x8
+OUT_FIT_BITMAP, OUT_SCORE, OUT_FILTER, OUT_TOPK, OUT_REASONS = 0x1, 0x2, 0x4, 0x8, 0x10
+# bins of a reason row (BS_OUT_REASONS): [unschedulable, unavailable, selector, taints, lane 0, lane 1, ...]
+REASON_UNSCHEDULABLE, REASON_UNAVAILABLE, REASON_SELECTOR, REASON_TAINTS, REASON_LANE0 = range(5)
 TOPK_MAX = 32   # BS_TOPK_MAX: longest top-K list
 FILTER_PASS, FILTER_NOT_FOUND, FILTER_NOT_ENOUGH, FILTER_NO_SNAPSHOT, FILTER_REF_PANIC = range(5)
 BUF_FIT_BITMAP, BUF_SCORE, BUF_ADMIT_BITMAP, BUF_PREFILTER, BUF_ADMIT, BUF_ORDER, BUF_GATHERED_ADMIT = range(7)
-K_NODE_LEFT, K_FIND_MAX, K_CLASS_PREFIX, K_PREFILTER, K_GANG_FIT, K_SORT, K_FILTER, K_PEER, K_REPLAY, K_COUNT = range(10)
+K_NODE_LEFT, K_FIND_MAX, K_CLASS_PREFIX, K_PREFILTER, K_GANG_FIT, K_SORT, K_FILTER, K_PEER, K_REPLAY, K_REASONS, K_COUNT = \
+    range(11)
 KERNEL_NAMES = ["node_left", "find_max", "class_prefix", "prefilter", "gang_fit", "sort", "filter", "peer", "replay"]
 
 
@@ -126,6 +129,8 @@ SYMBOLS = {
     "bs_fetch_score_rows": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]),
     "bs_fetch_filter_rows": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]),
     "bs_fetch_topk_rows": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p]),
+    "bs_fetch_reason_rows": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]),
+    "bs_format_fit_error": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_char_p, C.c_size_t]),
     "bs_peer_init": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32]),
     "bs_peer_handle": (C.c_int, [C.c_void_p, C.c_void_p]),
     "bs_peer_attach": (C.c_int, [C.c_void_p, C.c_void_p]),

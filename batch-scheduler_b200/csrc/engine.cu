@@ -393,6 +393,9 @@ struct bs_engine {
   DevBuf d_best_packed;   // gang_fit tail pieces: max((score + 1) << 32 | ~node) per pod
   DevBuf d_fit_bitmap, d_score;
   DevBuf d_topk_node, d_topk_score;   // BS_OUT_TOPK: [Prows][topk] lists
+  // BS_OUT_REASONS: full-width residuals [L][Npad], per fit class the gate bitmap [classes][Npad/32] and bins 0-3
+  // [classes][4] (rebuilt with the class fit bits), and the rows [P][4 + L]
+  DevBuf d_left_full, d_reason_gate, d_reason_class, d_reasons;
   // sort scratch: views into one arena
   View d_gk0, d_gk1, d_pk0, d_pk1, d_idx_a, d_idx_b, d_ghist, d_group_rank, d_tilecnt, d_sort_barrier;
   uint32_t sort_max_grid = 1;
@@ -953,6 +956,7 @@ int ensure_round_buffers(bs_engine* e) {
   if (e->out_flags & BS_OUT_FILTER) {
     CK(e->d_filter_bitmap.ensure(Prows * std::max(e->W, 1u) * 4));
   }
+  if (e->out_flags & BS_OUT_REASONS) CK(e->d_reasons.ensure((size_t)P * (4 + L) * 4));
   // prefix scratch: as many rep-class slots as fit a 1 GiB budget
   const size_t per_class = (size_t)N * (8 * L + 4);
   // BS_PREFIX_BUDGET_BYTES (default 1 GiB) bounds the scratch; classes beyond it are processed in chunks
@@ -994,12 +998,15 @@ int prepare_nodes(bs_engine* e) {
   CK(e->d_left_n.ensure((size_t)std::max(e->lane_map.LN + e->lane_map.LS, 1u) * e->Npad * 4));
   CK(e->d_left_present.ensure((size_t)e->Npad * 4));
   if (e->out_flags & BS_OUT_FILTER) CK(e->d_left_plain.ensure((size_t)4 * e->Npad * 8));
+  const bool reasons = (e->out_flags & BS_OUT_REASONS) != 0;
+  if (reasons) CK(e->d_left_full.ensure((size_t)e->L * e->Npad * 8));
   const uint32_t n_tiles = e->Npad / NODE_TILE;
   CK(e->d_classfit.ensure((size_t)e->n_fit_classes * n_tiles * 32 * sizeof(ColBits)));
   node_left_kernel<<<cdiv(e->Npad, 256), 256, 0, e->s>>>(t, e->lane_map, e->d_left_w.as<int64_t>(),
                                                          e->d_left_n.as<int32_t>(),
                                                          e->d_left_present.as<uint32_t>(),
-                                                         (e->out_flags & BS_OUT_FILTER) ? e->d_left_plain.as<int64_t>() : nullptr);
+                                                         (e->out_flags & BS_OUT_FILTER) ? e->d_left_plain.as<int64_t>() : nullptr,
+                                                         reasons ? e->d_left_full.as<int64_t>() : nullptr);
   tm.launched();
   {
     for (uint32_t c0 = 0; c0 < e->n_fit_classes; c0 += 32768) {
@@ -1007,6 +1014,21 @@ int prepare_nodes(bs_engine* e) {
       class_fit_kernel<<<grid, 256, 0, e->s>>>(t, e->d_left_present.as<uint32_t>(), e->d_fsel.as<uint64_t>(),
                                                e->d_ftol.as<uint64_t>(), e->d_fnz.as<uint32_t>(), e->d_faff.as<uint32_t>(),
                                                e->n_fit_classes, n_tiles, e->d_classfit.as<ColBits>(), c0);
+      tm.launched();
+    }
+  }
+  if (reasons) {
+    // the class half of the reason rows follows the same inputs as the class fit bits
+    const uint32_t Wg = e->Npad / 32;
+    CK(e->d_reason_gate.ensure((size_t)e->n_fit_classes * Wg * 4));
+    CK(e->d_reason_class.ensure((size_t)e->n_fit_classes * 4 * 4));
+    CK(cudaMemsetAsync(e->d_reason_class.p, 0, (size_t)e->n_fit_classes * 4 * 4, e->s));
+    for (uint32_t c0 = 0; c0 < e->n_fit_classes; c0 += 32768) {
+      dim3 grid(cdiv(Wg * 32, REASON_CLASS_THREADS), std::min(32768u, e->n_fit_classes - c0));
+      reason_class_kernel<<<grid, REASON_CLASS_THREADS, 0, e->s>>>(t, e->d_fsel.as<uint64_t>(), e->d_ftol.as<uint64_t>(),
+                                                                   e->d_faff.as<uint32_t>(), e->n_fit_classes, Wg,
+                                                                   e->d_reason_gate.as<uint32_t>(),
+                                                                   e->d_reason_class.as<uint32_t>(), c0);
       tm.launched();
     }
   }
@@ -1234,6 +1256,23 @@ int evaluate_async_locked(bs_engine* e) {
       fa.P = P; fa.N = e->N; fa.Npad = e->Npad; fa.W = e->W; fa.G = G; fa.L = L;
       const uint32_t warps = cdiv(P, FILTER_PPW);
       filter_kernel<<<cdiv(warps * 32, 256), 256, 0, e->s>>>(fa);
+      tm.launched();
+    }
+  }
+  {
+    StageTimer tm(e, BS_K_REASONS, e->s);
+    if (P && (e->out_flags & BS_OUT_REASONS)) {
+      ReasonArgs ra;
+      ra.left = e->d_left_full.as<int64_t>();
+      ra.left_present = e->d_left_present.as<uint32_t>();
+      ra.gate = e->d_reason_gate.as<uint32_t>();
+      ra.class_bins = e->d_reason_class.as<uint32_t>();
+      ra.req = e->d_req.as<int64_t>();
+      ra.req_present = e->d_ppres.as<uint32_t>();
+      ra.fit_class = e->d_pod_fit_class.as<uint32_t>();
+      ra.rows = e->d_reasons.as<uint32_t>();
+      ra.P = P; ra.N = e->N; ra.Npad = e->Npad; ra.Wg = e->Npad / 32; ra.L = L;
+      reason_pod_kernel<<<cdiv(P, REASON_PODS_PER_CTA), REASON_THREADS, 0, e->s>>>(ra);
       tm.launched();
     }
   }
@@ -2071,6 +2110,38 @@ int bs_format_message(const bs_status* st, const char* ns_name, const char* occu
   return BS_OK;
 }
 
+// kube-scheduler v1.17.5's predicate reasons (restated) and FitError.Error(): "0/N nodes are available: " + the
+// sorted "<count> <reason>" entries joined by ", " + "."
+int bs_format_fit_error(const uint32_t* counts, uint32_t n_lanes, uint32_t n_nodes, const char* const* scalar_names,
+                        char* buf, size_t buf_len) {
+  if (!counts || !buf || !buf_len || n_lanes < BS_FIXED_LANES || n_lanes > BS_MAX_LANES) return BS_E_INVAL;
+  static const char* const kFixed[4] = {"node(s) were unschedulable", "node(s) were unavailable",
+                                        "node(s) didn't match node selector",
+                                        "node(s) had taints that the pod didn't tolerate"};
+  static const char* const kLane[4] = {"cpu", "memory", "ephemeral-storage", "pods"};
+  std::vector<std::string> entries;
+  for (uint32_t b = 0; b < 4 + n_lanes; ++b) {
+    if (!counts[b]) continue;
+    std::string text;
+    if (b < 4) text = kFixed[b];
+    else {
+      const uint32_t d = b - 4;
+      text = "Insufficient ";
+      if (d < 4) text += kLane[d];
+      else if (scalar_names && scalar_names[d - 4]) text += scalar_names[d - 4];
+      else text += "lane" + std::to_string(d);
+    }
+    entries.push_back(std::to_string(counts[b]) + " " + text);
+  }
+  std::sort(entries.begin(), entries.end());   // byte-wise, as Go's sort.Strings
+  std::string msg = "0/" + std::to_string(n_nodes) + " nodes are available: ";
+  for (size_t k = 0; k < entries.size(); ++k) msg += (k ? ", " : "") + entries[k];
+  msg += ".";
+  if (msg.size() + 1 > buf_len) return BS_E_INVAL;
+  memcpy(buf, msg.c_str(), msg.size() + 1);
+  return BS_OK;
+}
+
 int bs_node_left(bs_engine* e, uint64_t sel, uint64_t tol, float percent, int64_t* left, uint32_t* present) {
   if (!e || !left || !present) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
@@ -2358,6 +2429,19 @@ int bs_fetch_topk_rows(bs_engine* e, uint32_t pod0, uint32_t n, int32_t* nodes, 
     CK(cudaMemcpyAsync(nodes, e->d_topk_node.as<int32_t>() + off, cnt * 4, cudaMemcpyDeviceToHost, e->s));
   if (cnt && scores)
     CK(cudaMemcpyAsync(scores, e->d_topk_score.as<int64_t>() + off, cnt * 8, cudaMemcpyDeviceToHost, e->s));
+  CK(cudaStreamSynchronize(e->s));
+  return BS_OK;
+}
+
+int bs_fetch_reason_rows(bs_engine* e, uint32_t pod0, uint32_t n, uint32_t* counts) {
+  if (!e || !counts) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!e->evaluated || !(e->out_flags & BS_OUT_REASONS)) return fail(e, BS_E_STATE, "no reason rows materialised");
+  if ((uint64_t)pod0 + n > e->P) return BS_E_INDEX;
+  BS_DEVICE_GUARD(e);
+  const size_t R = 4 + e->L;
+  if (n) CK(cudaMemcpyAsync(counts, e->d_reasons.as<uint32_t>() + (size_t)pod0 * R, (size_t)n * R * 4,
+                            cudaMemcpyDeviceToHost, e->s));
   CK(cudaStreamSynchronize(e->s));
   return BS_OK;
 }

@@ -118,10 +118,12 @@ __device__ __forceinline__ bool compare_res(const int64_t* left, uint32_t lpres,
 // class-independent (checkFit is applied per pod class by class_fit_kernel), split into the
 // wide (int64) and narrow (int32) lane tables of the round's LaneMap.
 // Restates singleNodeResource core.go:647-668.  Padding nodes (>= N) get zeros.
+// left_full (reason rows, BS_OUT_REASONS): every lane in original order as int64, 0 where the key is absent.
 __global__ void node_left_kernel(NodeTab t, LaneMap lm, int64_t* __restrict__ left_w /*[LW][Npad]*/,
                                  int32_t* __restrict__ left_n /*[LN+LS][Npad]: narrow lanes, then scaled lanes*/,
                                  uint32_t* __restrict__ left_present /*[Npad]*/,
-                                 int64_t* __restrict__ left_plain /*[4][Npad] getLeftResource, or null*/) {
+                                 int64_t* __restrict__ left_plain /*[4][Npad] getLeftResource, or null*/,
+                                 int64_t* __restrict__ left_full /*[L][Npad], or null*/) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= t.Npad) return;
   if (left_plain) {
@@ -139,6 +141,8 @@ __global__ void node_left_kernel(NodeTab t, LaneMap lm, int64_t* __restrict__ le
   if (i >= t.N) {
     for (uint32_t k = 0; k < lm.LW; ++k) left_w[(size_t)k * t.Npad + i] = 0;
     for (uint32_t k = 0; k < lm.LN + lm.LS; ++k) left_n[(size_t)k * t.Npad + i] = 0;
+    if (left_full)
+      for (uint32_t d = 0; d < t.L; ++d) left_full[(size_t)d * t.Npad + i] = 0;
     left_present[i] = 0;
     return;
   }
@@ -168,6 +172,12 @@ __global__ void node_left_kernel(NodeTab t, LaneMap lm, int64_t* __restrict__ le
     const int64_t v = lane_left(lm.scaled[k], pres);
     left_n[(size_t)(lm.LN + k) * t.Npad + i] = pres ? (int32_t)(v >> lm.sunit[k]) : ABSENT_LEFTS;
   }
+  if (left_full)
+    for (uint32_t d = 0; d < t.L; ++d) {
+      bool pres;
+      const int64_t v = lane_left(d, pres);
+      left_full[(size_t)d * t.Npad + i] = pres ? v : 0;
+    }
   left_present[i] = both;
 }
 
@@ -237,6 +247,141 @@ __global__ void class_fit_kernel(NodeTab t, const uint32_t* __restrict__ left_pr
     bits |= (ColBits)(ok ? 1u : 0u) << j;
   }
   classfit[(size_t)c * n_tiles * 32 + slot] = bits;
+}
+
+// ---------------------------------------------------------------------------
+// K1c reason_class_kernel — the class half of a reason row (BS_OUT_REASONS): per fit class, how many nodes are
+// unschedulable / unavailable (the guards of core.go:606-617 and :639, in that precedence) and, among the nodes
+// past the guards, how many fail the selector (label bits or the affinity-class bit) and the taints (checkFit,
+// core.go:741-759; both predicates' reasons count).  Also the class's gate bitmap [c][Wg]: bit n%32 of word n/32
+// = node n passes the guards and checkFit, the only nodes whose lanes a reason row inspects.  One thread per node
+// (Wg * 32 threads cover the padded table: gate bits of padding nodes are 0), one ballot per warp and bin, one
+// global atomic per CTA and bin into class_bins[c][4] (zeroed before the launch).
+constexpr int REASON_CLASS_THREADS = 256;
+__global__ void __launch_bounds__(REASON_CLASS_THREADS)
+reason_class_kernel(NodeTab t, const uint64_t* __restrict__ csel, const uint64_t* __restrict__ ctol,
+                    const uint32_t* __restrict__ caff, uint32_t n_classes, uint32_t Wg,
+                    uint32_t* __restrict__ gate, uint32_t* __restrict__ class_bins, uint32_t class0) {
+  const uint32_t c = class0 + blockIdx.y;   // gridDim.y is capped at 65535: classes go in chunks
+  if (c >= n_classes) return;
+  __shared__ uint32_t s_bins[4];
+  if (threadIdx.x < 4) s_bins[threadIdx.x] = 0;
+  __syncthreads();
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x, lane = threadIdx.x & 31;
+  bool unsched = false, unavail = false, sel_bad = false, taint_bad = false, pass = false;
+  if (i < t.N) {
+    const uint8_t f = t.flags[i];
+    if (node_skipped(f) || (f & BS_NODE_TAINTS_ERR)) {
+      unsched = !(f & (BS_NODE_NIL | BS_NODE_NO_NODE)) && (f & BS_NODE_UNSCHEDULABLE);
+      unavail = !unsched;
+    } else {
+      const uint64_t sel = csel[c], tol = ctol[c];
+      const uint64_t label = t.label[i], taint = t.taint[i];
+      // check_fit's two predicates one at a time: a neutral taint / label side leaves only the other
+      sel_bad = !check_fit(label, 0, sel, 0) || !aff_ok(t, caff[c], i);
+      taint_bad = !check_fit(~0ull, taint, 0, tol);
+      pass = !sel_bad && !taint_bad;
+    }
+  }
+  const uint32_t gw = __ballot_sync(0xffffffffu, pass);
+  if (lane == 0 && (i >> 5) < Wg) gate[(size_t)c * Wg + (i >> 5)] = gw;
+  const uint32_t b0 = __popc(__ballot_sync(0xffffffffu, unsched)), b1 = __popc(__ballot_sync(0xffffffffu, unavail));
+  const uint32_t b2 = __popc(__ballot_sync(0xffffffffu, sel_bad)), b3 = __popc(__ballot_sync(0xffffffffu, taint_bad));
+  if (lane == 0) {
+    if (b0) atomicAdd(&s_bins[0], b0);
+    if (b1) atomicAdd(&s_bins[1], b1);
+    if (b2) atomicAdd(&s_bins[2], b2);
+    if (b3) atomicAdd(&s_bins[3], b3);
+  }
+  __syncthreads();
+  if (threadIdx.x < 4 && s_bins[threadIdx.x]) atomicAdd(&class_bins[(size_t)c * 4 + threadIdx.x], s_bins[threadIdx.x]);
+}
+
+// K1d reason_pod_kernel — the lane bins of a reason row.  A warp takes REASON_PPW pods and sweeps every node 32 at a
+// time (lane k owns node base + k); a node counts only when the pod's class gate bit is set.  Lane d is short under
+// compareResourceAndRequire's rules (core.go:672-699) with `left` at percent 1.0 from node_left_kernel (left_full,
+// left_present): lanes 0-3 when left < req; a scalar lane the pod requests when the node's left lacks the key and
+// req != 0, or when req > left.  Every short lane counts (the reference stops at the first).  Counters stay in
+// registers, are summed across the warp once at the end, and each (pod, bin) is stored once; bins 0-3 are copied
+// from the pod's class.
+constexpr int REASON_THREADS = 256;
+constexpr int REASON_PPW = 4;                                         // pods per warp
+constexpr int REASON_PODS_PER_CTA = (REASON_THREADS / 32) * REASON_PPW;
+struct ReasonArgs {
+  const int64_t* left;          // [L][Npad] left_full
+  const uint32_t* left_present; // [Npad]
+  const uint32_t* gate;         // [classes][Wg]
+  const uint32_t* class_bins;   // [classes][4]
+  const int64_t* req;           // [L][P]
+  const uint32_t* req_present;  // [P]
+  const uint32_t* fit_class;    // [P]
+  uint32_t* rows;               // [P][4 + L]
+  uint32_t P, N, Npad, Wg, L;
+};
+__global__ void __launch_bounds__(REASON_THREADS) reason_pod_kernel(ReasonArgs a) {
+  __shared__ int64_t s_req[REASON_THREADS / 32][REASON_PPW][BS_MAX_LANES];
+  const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const uint32_t p0 = (blockIdx.x * (REASON_THREADS / 32) + wid) * REASON_PPW;
+  const int L = (int)a.L;
+  for (uint32_t k = lane; k < REASON_PPW * BS_MAX_LANES; k += 32) {
+    const uint32_t j = k / BS_MAX_LANES, d = k % BS_MAX_LANES, p = p0 + j;
+    s_req[wid][j][d] = (p < a.P && d < a.L) ? a.req[(size_t)d * a.P + p] : 0;
+  }
+  __syncwarp();
+  uint32_t rmask[REASON_PPW];   // lanes compared: 0-3 always, scalar lanes the pod requests
+  const uint32_t* grow[REASON_PPW];
+#pragma unroll
+  for (int j = 0; j < REASON_PPW; ++j) {
+    const uint32_t p = p0 + j;
+    const bool ok = p < a.P;
+    rmask[j] = ok ? (a.req_present[p] | 0xFu) : 0u;
+    grow[j] = a.gate + (size_t)(ok ? a.fit_class[p] : 0u) * a.Wg;
+  }
+  uint32_t cnt[REASON_PPW][BS_MAX_LANES];
+#pragma unroll
+  for (int j = 0; j < REASON_PPW; ++j)
+#pragma unroll
+    for (int d = 0; d < BS_MAX_LANES; ++d) cnt[j][d] = 0;
+  for (uint32_t base = 0; base < a.N; base += 32) {
+    const uint32_t i = base + lane, w = base >> 5;
+    bool g[REASON_PPW];
+    uint32_t any = 0;
+#pragma unroll
+    for (int j = 0; j < REASON_PPW; ++j) {
+      const uint32_t gw = rmask[j] ? grow[j][w] : 0u;   // the word of the padded table: bits >= N are 0
+      any |= gw;
+      g[j] = (gw >> lane) & 1u;
+    }
+    if (!any) continue;   // warp-uniform: no pod of the warp looks at these 32 nodes
+    const uint32_t lp = a.left_present[i] | 0xFu;   // i < Npad: the padded table is readable
+#pragma unroll
+    for (int d = 0; d < BS_MAX_LANES; ++d) {
+      if (d >= L) break;
+      const int64_t v = a.left[(size_t)d * a.Npad + i];
+      const bool pres = (lp >> d) & 1u;
+#pragma unroll
+      for (int j = 0; j < REASON_PPW; ++j) {
+        const int64_t r = s_req[wid][j][d];
+        const bool shrt = g[j] && ((rmask[j] >> d) & 1u) && (pres ? v < r : r != 0);
+        cnt[j][d] += shrt ? 1u : 0u;
+      }
+    }
+  }
+  const uint32_t R = 4 + a.L;
+#pragma unroll
+  for (int j = 0; j < REASON_PPW; ++j) {
+    const uint32_t p = p0 + j;
+    uint32_t mine = 0;
+#pragma unroll
+    for (int d = 0; d < BS_MAX_LANES; ++d) {
+      const uint32_t s = __reduce_add_sync(0xffffffffu, cnt[j][d]);
+      if (lane == 4 + d) mine = s;
+    }
+    if (p < a.P) {
+      if (lane < 4) mine = a.class_bins[(size_t)a.fit_class[p] * 4 + lane];
+      if (lane < R) a.rows[(size_t)p * R + lane] = mine;
+    }
+  }
 }
 
 // ---------------------------------------------------------------------------

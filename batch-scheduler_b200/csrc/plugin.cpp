@@ -980,6 +980,7 @@ Status BatchSchedulingPlugin::BeginRound(const std::vector<const NodeInfo*>& sna
   r.admit = admit_.data(); r.new_denied = new_denied_.data(); r.order = order_.data(); r.rank = rank_.data();
   if ((rc = bs_evaluate(eng_, &r))) return fail(rc);
   if ((rc = FetchTopK())) return fail(rc);
+  if ((rc = FetchReasons())) return fail(rc);
   last_device_ms_ = now_ms() - t1;
 
   // side effects the reference performs while it walks the pods:
@@ -1040,6 +1041,7 @@ Status BatchSchedulingPlugin::Reevaluate() {
   int rc = bs_begin_cycle(eng_, now_ns_);   // matched / flags columns follow the engine's tables at now
   if (!rc) rc = bs_evaluate(eng_, &r);
   if (!rc) rc = FetchTopK();
+  if (!rc) rc = FetchReasons();
   if (rc) return Status{BS_CODE_ERROR, std::string("bsched: ") + bs_strerror(rc) + " (" + bs_last_error(eng_) + ")"};
   return Status{};   // (new_denied groups were deny-listed by the engine's fetch, core.go:142,163)
 }
@@ -1062,6 +1064,37 @@ std::vector<std::pair<std::string, int64_t>> BatchSchedulingPlugin::TopNodes(con
     out.emplace_back((size_t)n < node_names_.size() ? node_names_[n] : std::string(), topk_score_[(size_t)row * topk_ + i]);
   }
   return out;
+}
+
+int BatchSchedulingPlugin::FetchReasons() {
+  if (!(out_flags_ & BS_OUT_REASONS)) return BS_OK;
+  const uint32_t P = packed_.n_pods;
+  reasons_.assign((size_t)P * (4 + packed_.lanes), 0);
+  return bs_fetch_reason_rows(eng_, 0, P, reasons_.data());
+}
+
+std::vector<uint32_t> BatchSchedulingPlugin::ReasonCounts(const std::string& uid) const {
+  const int32_t row = pod_row_.find(uid);
+  const size_t R = 4 + packed_.lanes;
+  if (row < 0 || reasons_.size() < ((size_t)row + 1) * R) return {};
+  return std::vector<uint32_t>(reasons_.begin() + (size_t)row * R, reasons_.begin() + ((size_t)row + 1) * R);
+}
+
+std::string BatchSchedulingPlugin::FitError(const std::string& uid) const {
+  const int32_t row = pod_row_.find(uid);
+  if (row < 0 || (size_t)row >= feasible_.size() || feasible_[row] != 0) return "";
+  const std::vector<uint32_t> counts = ReasonCounts(uid);
+  if (counts.empty()) return "";
+  std::vector<const char*> names;
+  for (auto& nm : packed_.scalar_names) names.push_back(nm.c_str());
+  std::vector<char> buf(256);
+  for (;;) {   // grows until the whole message fits
+    const int rc = bs_format_fit_error(counts.data(), packed_.lanes, packed_.n_nodes, names.empty() ? nullptr : names.data(),
+                                       buf.data(), buf.size());
+    if (rc == BS_OK) return std::string(buf.data());
+    if (buf.size() > (1u << 20)) return "";
+    buf.resize(buf.size() * 4);
+  }
 }
 
 Status BatchSchedulingPlugin::UpdateRound(const std::vector<std::pair<uint32_t, const NodeInfo*>>& changed_nodes,

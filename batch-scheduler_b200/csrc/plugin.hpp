@@ -280,6 +280,11 @@ class BatchSchedulingPlugin {
   // the pod's best fitting nodes of the last round (plugin created with topk > 0): (node name, residual score),
   // score descending, then snapshot order; at most topk of them, empty for an unknown uid
   std::vector<std::pair<std::string, int64_t>> TopNodes(const std::string& uid) const;
+  // plugin created with BS_OUT_REASONS in out_flags: the pod's reason row of the last round, 4 + lanes counters in the
+  // bins of BS_REASON_* (empty for an unknown uid), and the FailedScheduling message built from it
+  // ("0/N nodes are available: ..."; lanes >= 4 by their resource names) for a pod that fits no node, "" otherwise
+  std::vector<uint32_t> ReasonCounts(const std::string& uid) const;
+  std::string FitError(const std::string& uid) const;
   int group_index(const std::string& ns_name) const;
   double last_pack_ms() const { return last_pack_ms_; }
   double last_device_ms() const { return last_device_ms_; }
@@ -358,10 +363,12 @@ class BatchSchedulingPlugin {
   std::vector<int32_t> best_node_;
   std::vector<int32_t> topk_node_;                                  // [P][topk_] (BS_OUT_TOPK)
   std::vector<int64_t> topk_score_;
+  std::vector<uint32_t> reasons_;                                   // [P][4 + lanes] (BS_OUT_REASONS)
   int64_t now_ns_ = 0;
   double last_pack_ms_ = 0, last_device_ms_ = 0;
   Status Reevaluate();   // bs_evaluate into the round's result vectors + the deny side effect (core.go:142,163)
   int FetchTopK();       // the round's top-K lists into topk_node_ / topk_score_ (no-op without topk)
+  int FetchReasons();    // the round's reason rows into reasons_ (no-op without BS_OUT_REASONS)
 };
 
 }  // namespace bsched

@@ -44,14 +44,16 @@ def _table_c(table):
 
 class Engine:
     def __init__(self, n_lanes: int, device: int = 0, fit_bitmap: bool = True, score: bool = False,
-                 filter: bool = False, topk: int = 0):
+                 filter: bool = False, topk: int = 0, reasons: bool = False):
         """topk > 0 also keeps each pod's `topk` best fitting nodes and their scores (BS_OUT_TOPK, read with
-        topk_rows); it cannot be combined with score=True, whose matrix holds them already."""
+        topk_rows); it cannot be combined with score=True, whose matrix holds them already.  reasons=True also counts,
+        per pod, the nodes that reject it for each reason (BS_OUT_REASONS, read with reason_rows)."""
         self.lib = capi.load()
         self.n_lanes = n_lanes
         self.topk = topk
         self.out_flags = ((capi.OUT_FIT_BITMAP if fit_bitmap else 0) | (capi.OUT_SCORE if score else 0) |
-                          (capi.OUT_FILTER if filter else 0) | (capi.OUT_TOPK if topk else 0))
+                          (capi.OUT_FILTER if filter else 0) | (capi.OUT_TOPK if topk else 0) |
+                          (capi.OUT_REASONS if reasons else 0))
         cfg = capi.Config(device, n_lanes, self.out_flags, topk)
         h = C.c_void_p()
         rc = self.lib.bs_create(C.byref(cfg), C.byref(h))
@@ -236,6 +238,23 @@ class Engine:
         self._check(self.lib.bs_fetch_topk_rows(self.h, pod0, n, capi.ptr(nodes), capi.ptr(scores)))
         return nodes, scores
 
+    def reason_rows(self, pod0=0, n=None) -> np.ndarray:
+        """[n, 4 + L] uint32: bin b of row p = the nodes that reject pod pod0 + p for reason b (capi.REASON_*)."""
+        n = self.P - pod0 if n is None else n
+        out = np.zeros((n, 4 + self.n_lanes), np.uint32)
+        self._check(self.lib.bs_fetch_reason_rows(self.h, pod0, n, capi.ptr(out)))
+        return out
+
+    def fit_error(self, counts, n_nodes: int, scalar_names=None) -> str:
+        """The "0/N nodes are available: ..." message of one reason row (bs_format_fit_error)."""
+        return format_fit_error(counts, self.n_lanes, n_nodes, scalar_names)
+
+    def reasons_ms(self) -> float:
+        """Milliseconds of the last round's reason-row stage (profiling on)."""
+        ms, n = C.c_float(), C.c_uint32()
+        self._check(self.lib.bs_kernel_ms(self.h, capi.K_REASONS, C.byref(ms), C.byref(n)))
+        return float(ms.value)
+
     # -- standalone kernels ------------------------------------------------------------------
     def node_left(self, sel: int, tol: int, percent: float):
         left = np.zeros((self.n_lanes, self.N), np.int64)
@@ -398,3 +417,21 @@ class Engine:
 
     def launch_count(self) -> int:
         return int(self.lib.bs_launch_count(self.h))
+
+
+def format_fit_error(counts, n_lanes: int, n_nodes: int, scalar_names=None, buf_len: int = 4096) -> str:
+    """kube-scheduler's FailedScheduling text for one reason row; needs no engine and no device.  scalar_names: the
+    names of lanes 4.. (None: "lane<d>")."""
+    lib = capi.load()
+    row = np.ascontiguousarray(counts, dtype=np.uint32)
+    if row.shape != (4 + n_lanes,):
+        raise ValueError("a reason row has 4 + n_lanes bins")
+    names = None
+    if scalar_names is not None:
+        names = (C.c_char_p * max(1, n_lanes - 4))(*[s.encode() for s in scalar_names])
+    buf = C.create_string_buffer(buf_len)
+    rc = lib.bs_format_fit_error(capi.ptr(row), n_lanes, n_nodes, C.cast(names, C.c_void_p) if names is not None else None,
+                                 buf, buf_len)
+    if rc != 0:
+        raise capi.BsError(rc, lib.bs_strerror(rc).decode())
+    return buf.value.decode()

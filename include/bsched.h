@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define BS_ABI_VERSION 7
+#define BS_ABI_VERSION 8
 #define BS_FIXED_LANES 4
 #define BS_MAX_LANES 16
 /* |value| bound accepted for every int64 table entry (validated at upload):
@@ -177,6 +177,19 @@ typedef struct {
 #define BS_OUT_TOPK 0x8u       /* P x K: each pod's K best fitting nodes and their scores (bs_fetch_topk_rows),
                                   without the score matrix; not combinable with BS_OUT_SCORE */
 #define BS_TOPK_MAX 32         /* largest list length K */
+#define BS_OUT_REASONS 0x10u   /* P x (4 + n_lanes) u32: per pod, how many nodes reject it for each reason
+                                  (bs_fetch_reason_rows); combines with every other flag */
+
+/* Bins of a reason row.  A node counts in no bin <=> the pod fits it (fit bitmap bit set); a guarded node counts in
+ * exactly one of bins 0-1 (precedence nil, Node()==nil, unschedulable, Taints() error, core.go:606-617,639); a node
+ * passing the guards may count in both bins 2 and 3 (checkFit appends both predicates' reasons, core.go:741-759);
+ * only a node passing the guards and checkFit counts in lane bins, in every lane that is short
+ * (compareResourceAndRequire's rules at percent 1.0, core.go:672-699, without its early return). */
+#define BS_REASON_UNSCHEDULABLE 0 /* Spec.Unschedulable (and not nil / no Node())          */
+#define BS_REASON_UNAVAILABLE 1   /* nil info, nil Node(), or Taints() returned an error    */
+#define BS_REASON_SELECTOR 2      /* node selector / required node affinity not matched     */
+#define BS_REASON_TAINTS 3        /* a NoSchedule / NoExecute taint not tolerated           */
+#define BS_REASON_LANE0 4         /* + d: resource lane d short ("Insufficient <resource>") */
 
 typedef struct {
   int32_t device;      /* CUDA device ordinal */
@@ -406,6 +419,16 @@ int bs_fetch_filter_rows(bs_engine* e, uint32_t pod0, uint32_t n, uint32_t* word
  * fitting nodes of pod p ordered by score descending, then node index ascending (entry 0 = best_node / best_score),
  * min(K, feasible_count[p]) of them, padded with node -1 and score INT64_MIN.  Either pointer may be NULL. */
 int bs_fetch_topk_rows(bs_engine* e, uint32_t pod0, uint32_t n, int32_t* nodes, int64_t* scores);
+/* copy the reason rows of pods [pod0, pod0+n) to the host as dense [n][4 + n_lanes] counters (BS_OUT_REASONS): bin b
+ * of row p = the number of snapshot nodes that reject pod p for reason b (BS_REASON_*) */
+int bs_fetch_reason_rows(bs_engine* e, uint32_t pod0, uint32_t n, uint32_t* counts);
+/* kube-scheduler's FailedScheduling text for one reason row (no engine, no device):
+ *     "0/<n_nodes> nodes are available: <count> <reason>, ... ."
+ * one entry per non-zero bin, entries sorted as whole strings byte-wise ascending (Go's sort.Strings), joined by
+ * ", ".  Lane d >= 4 reads "Insufficient <scalar_names[d - 4]>", or "Insufficient lane<d>" when scalar_names is NULL.
+ * A buffer too small for the whole message is BS_E_INVAL (nothing is truncated). */
+int bs_format_fit_error(const uint32_t* counts, uint32_t n_lanes, uint32_t n_nodes, const char* const* scalar_names,
+                        char* buf, size_t buf_len);
 
 /* ---- multi-GPU exchange of the admit bitmap over peer memory (NVLink / NVSwitch) ----
  * The path shards over groups (one process per GPU); the only exchange is the all-gather of the
@@ -446,7 +469,9 @@ typedef enum {
   BS_K_FILTER = 6,     /* optional Filter matrix (BS_OUT_FILTER) */
   BS_K_PEER = 7,       /* admit-bitmap exchange over peer memory */
   BS_K_REPLAY = 8,     /* bs_replay: the pod-at-a-time cycle in one persistent kernel */
-  BS_K_COUNT = 9
+  BS_K_REASONS = 9,    /* reason rows (BS_OUT_REASONS): the per-pod lane sweep; the per-class bins and gate bitmap are
+                          rebuilt with the class fit bits and counted in BS_K_NODE_LEFT */
+  BS_K_COUNT = 10
 } bs_kernel_id;
 int bs_set_profiling(bs_engine* e, int on); /* record CUDA events around each stage */
 /* milliseconds of stage k in the last evaluation, and launches it took */

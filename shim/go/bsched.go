@@ -24,8 +24,9 @@ import (
 // Engine wraps one bs_engine (one GPU).  Thread-safe: the C side serialises calls per handle, as the reference
 // calls Less / Permit from several goroutines (batchscheduler.go:165,214).
 type Engine struct {
-	h    *C.bs_engine
-	topk int // list length of BS_OUT_TOPK, 0 without it
+	h     *C.bs_engine
+	topk  int // list length of BS_OUT_TOPK, 0 without it
+	lanes int // resource lanes of every table: a reason row has 4 + lanes bins
 }
 
 // ID turns a pod UID or a "namespace/name" into the 64-bit id the gang-state calls take (FNV-1a, as
@@ -51,7 +52,7 @@ func NewTopK(device, lanes int, outFlags uint32, topk int) (*Engine, error) {
 	if rc := C.bs_create(&cfg, &h); rc != 0 {
 		return nil, fmt.Errorf("bs_create: %s", C.GoString(C.bs_strerror(rc)))
 	}
-	return &Engine{h, topk}, nil
+	return &Engine{h, topk, lanes}, nil
 }
 
 func (e *Engine) Close() { C.bs_destroy(e.h) }
@@ -137,6 +138,49 @@ func (e *Engine) TopNodes(pod0, n int) ([]int32, []int64, error) {
 	err := e.rc(C.bs_fetch_topk_rows(e.h, C.uint32_t(pod0), C.uint32_t(n), (*C.int32_t)(unsafe.Pointer(&nodes[0])),
 		(*C.int64_t)(unsafe.Pointer(&scores[0]))))
 	return nodes, scores, err
+}
+
+// Reasons returns the reason rows of pods [pod0, pod0+n) of the last round (engine created with BS_OUT_REASONS) as
+// dense [n][4+lanes] counters: bin b of a row = the nodes that reject the pod for reason b (BS_REASON_*).
+func (e *Engine) Reasons(pod0, n int) ([]uint32, error) {
+	counts := make([]uint32, n*(4+e.lanes))
+	if len(counts) == 0 {
+		var none C.uint32_t
+		return counts, e.rc(C.bs_fetch_reason_rows(e.h, C.uint32_t(pod0), C.uint32_t(n), &none))
+	}
+	err := e.rc(C.bs_fetch_reason_rows(e.h, C.uint32_t(pod0), C.uint32_t(n), (*C.uint32_t)(unsafe.Pointer(&counts[0]))))
+	return counts, err
+}
+
+// FitError formats one reason row (4 + lanes counters) as kube-scheduler's FailedScheduling message,
+// "0/<nNodes> nodes are available: ...", naming lanes 4.. by scalarNames (nil: "lane<d>").  Needs no engine.
+func FitError(counts []uint32, nNodes int, scalarNames []string) (string, error) {
+	lanes := len(counts) - 4
+	if lanes < C.BS_FIXED_LANES {
+		return "", fmt.Errorf("bs_format_fit_error: a reason row has 4 + lanes bins")
+	}
+	var names **C.char
+	if len(scalarNames) > 0 {
+		arr := C.malloc(C.size_t(len(scalarNames)) * C.size_t(unsafe.Sizeof(uintptr(0))))
+		defer C.free(arr)
+		view := unsafe.Slice((**C.char)(arr), len(scalarNames))
+		for i, s := range scalarNames {
+			view[i] = C.CString(s)
+			defer C.free(unsafe.Pointer(view[i]))
+		}
+		names = (**C.char)(arr)
+	}
+	for size := 512; size <= 1<<20; size *= 4 {
+		buf := (*C.char)(C.malloc(C.size_t(size)))
+		rc := C.bs_format_fit_error((*C.uint32_t)(unsafe.Pointer(&counts[0])), C.uint32_t(lanes), C.uint32_t(nNodes),
+			names, buf, C.size_t(size))
+		msg := C.GoString(buf)
+		C.free(unsafe.Pointer(buf))
+		if rc == 0 {
+			return msg, nil
+		}
+	}
+	return "", fmt.Errorf("bs_format_fit_error: %s", C.GoString(C.bs_strerror(C.BS_E_INVAL)))
 }
 
 // PreFilter mirrors ScheduleOperation.PreFilter(pod) error (core.go:88): nil == pass.
