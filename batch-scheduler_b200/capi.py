@@ -21,6 +21,9 @@ OUT_FIT_BITMAP, OUT_SCORE, OUT_FILTER, OUT_TOPK, OUT_REASONS = 0x1, 0x2, 0x4, 0x
 # bins of a reason row (BS_OUT_REASONS): [unschedulable, unavailable, selector, taints, lane 0, lane 1, ...]
 REASON_UNSCHEDULABLE, REASON_UNAVAILABLE, REASON_SELECTOR, REASON_TAINTS, REASON_LANE0 = range(5)
 TOPK_MAX = 32   # BS_TOPK_MAX: longest top-K list
+# core.PreemptRemovePod verdicts (bs_remove_code) and the bound-pod flag
+REMOVE_ALLOW, REMOVE_OFFLINE_ONLINE, REMOVE_NOT_FOUND, REMOVE_LOCKED, REMOVE_SAME_GROUP = range(5)
+BOUND_GROUP_LOCKED = 0x01
 FILTER_PASS, FILTER_NOT_FOUND, FILTER_NOT_ENOUGH, FILTER_NO_SNAPSHOT, FILTER_REF_PANIC = range(5)
 BUF_FIT_BITMAP, BUF_SCORE, BUF_ADMIT_BITMAP, BUF_PREFILTER, BUF_ADMIT, BUF_ORDER, BUF_GATHERED_ADMIT = range(7)
 K_NODE_LEFT, K_FIND_MAX, K_CLASS_PREFIX, K_PREFILTER, K_GANG_FIT, K_SORT, K_FILTER, K_PEER, K_REPLAY, K_REASONS, K_COUNT = \
@@ -67,6 +70,18 @@ class ReplayResultC(C.Structure):
                 ("node_requested", C.c_void_p), ("node_pod_count", C.c_void_p), ("node_req_present", C.c_void_p),
                 ("group_matched", C.c_void_p), ("group_flags", C.c_void_p), ("group_min_res", C.c_void_p),
                 ("group_min_res_present", C.c_void_p), ("group_rep_sel", C.c_void_p), ("group_rep_tol", C.c_void_p)]
+
+
+class BoundTableC(C.Structure):
+    _fields_ = [("n_pods", C.c_uint32), ("n_lanes", C.c_uint32), ("node", C.c_void_p), ("req", C.c_void_p),
+                ("req_present", C.c_void_p), ("gid", C.c_void_p), ("priority", C.c_void_p), ("start_ns", C.c_void_p),
+                ("flags", C.c_void_p)]
+
+
+class PreemptResultC(C.Structure):
+    _fields_ = [("node", C.c_void_p), ("n_victims", C.c_void_p), ("n_candidates", C.c_void_p),
+                ("victim_offset", C.c_void_p), ("victims", C.c_void_p), ("victims_cap", C.c_uint32),
+                ("victims_total", C.c_uint32)]
 
 
 class StatusC(C.Structure):
@@ -121,6 +136,10 @@ SYMBOLS = {
     "bs_replay": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, _p(ReplayResultC)]),
     "bs_cluster_check": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, C.c_float, C.c_void_p, C.c_void_p,
                                    C.c_uint32, C.c_void_p]),
+    "bs_upload_bound_pods": (C.c_int, [C.c_void_p, _p(BoundTableC)]),
+    "bs_preempt": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, _p(PreemptResultC)]),
+    "bs_remove_pod": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, _p(StatusC)]),
+    "bs_format_remove_message": (C.c_int, [_p(StatusC), C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_size_t]),
     "bs_device_buffer": (C.c_int, [C.c_void_p, C.c_int, _p(C.c_void_p), _p(C.c_size_t)]),
     "bs_stream": (C.c_void_p, [C.c_void_p]),
     "bs_score_pitch": (C.c_uint32, [C.c_void_p]),

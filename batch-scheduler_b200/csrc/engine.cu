@@ -27,6 +27,7 @@
 #include "gang_state.hpp"
 #include "sort.cuh"
 #include "replay.cuh"
+#include "preempt.cuh"
 
 using namespace bsk;
 
@@ -434,6 +435,21 @@ struct bs_engine {
 
   // bs_replay scratch (kept between calls: an allocation per call would dominate small queues)
   DevBuf d_replay;
+
+  // bound-pod table (bs_upload_bound_pods): CSR by node in MoreImportantPod order, its suffix sums and counts, and
+  // the residuals it is read against (node_left_kernel's full-width table, kept apart from the round's); dropped
+  // with the node snapshot and with the group table
+  bool have_bound = false;
+  uint32_t V = 0;
+  int32_t bound_max_gid = -1;
+  std::vector<int32_t> h_bgid;        // by bound-table index: bs_remove_pod
+  std::vector<uint8_t> h_bflags;
+  std::vector<int32_t> h_npc;         // node pod_count and req_present as uploaded (bound-table validation)
+  std::vector<uint32_t> h_nrpres;
+  DevBuf d_brow, d_bprio, d_bstart, d_bgid, d_bflags, d_bidx, d_breq, d_bsuf, d_bsuf_online, d_bsuf_bad;
+  DevBuf d_pl_left, d_pl_present;
+  // bs_preempt scratch
+  DevBuf d_pp, d_ptiles, d_pnode, d_pnv, d_pcand, d_poff, d_pvict;
 
   // peer exchange (admit bitmap all-gather over NVLink peer memory)
   DevBuf d_gather, d_peer_err;
@@ -1364,6 +1380,38 @@ int fetch_locked(bs_engine* e, bs_results* out, bool view = false) {
   return BS_OK;
 }
 
+// ---- preemption (preempt.cuh) ----
+// Launches a MAXL instance of a preemption kernel: 5, 9 or 16 lanes of registers
+template <template <int> class K, class... A>
+void launch_maxl(uint32_t L, A&&... args) {
+  if (L <= 5) K<5>::go(args...);
+  else if (L <= 9) K<9>::go(args...);
+  else K<16>::go(args...);
+}
+template <int MAXL>
+struct PreemptNodeLaunch {
+  static void go(dim3 grid, cudaStream_t s, const PreemptArgs& a) {
+    preempt_node_kernel<MAXL><<<grid, PREEMPT_THREADS, 0, s>>>(a);
+  }
+};
+template <int MAXL>
+struct PreemptEmitLaunch {
+  static void go(dim3 grid, cudaStream_t s, const PreemptArgs& a) { preempt_emit_kernel<MAXL><<<grid, 256, 0, s>>>(a); }
+};
+
+// What the bound-table pass finds wrong, in the order the errors are reported.
+struct BoundStats {
+  bool bad_index = false, bad_count = false, bad_keys = false, bad_range = false;   // bad_index: node or gid
+  int32_t max_gid = -1;
+  void merge(const BoundStats& o) {
+    bad_index = bad_index || o.bad_index;
+    bad_count = bad_count || o.bad_count;
+    bad_keys = bad_keys || o.bad_keys;
+    bad_range = bad_range || o.bad_range;
+    max_gid = std::max(max_gid, o.max_gid);
+  }
+};
+
 }  // namespace
 
 // ============================================================================
@@ -1475,6 +1523,9 @@ int bs_upload_nodes(bs_engine* e, const bs_node_table* t) {
   CK(cudaStreamSynchronize(e->s));
   HP(e, "nodes:dma-wait");
   e->h_nflags.assign(t->flags, t->flags + N);
+  e->h_npc.assign(t->pod_count, t->pod_count + N);
+  e->h_nrpres.assign(t->req_present, t->req_present + N);
+  e->have_bound = false;   // the bound-pod table belongs to the node snapshot
   e->node_stats = ns;
   e->N = N;
   e->score_pitch = (N + 1u) & ~1u;
@@ -1510,7 +1561,12 @@ int bs_update_nodes(bs_engine* e, const uint32_t* idx, const bs_node_table* t) {
   CK(cudaStreamSynchronize(e->s));
   HP(e, "upd-nodes:wait");
   e->node_stats.merge(ns);
-  for (uint32_t k = 0; k < n; ++k) e->h_nflags[idx[k]] = t->flags[k];
+  for (uint32_t k = 0; k < n; ++k) {
+    e->h_nflags[idx[k]] = t->flags[k];
+    e->h_npc[idx[k]] = t->pod_count[k];
+    e->h_nrpres[idx[k]] = t->req_present[k];
+  }
+  e->have_bound = false;
   e->nodes_dirty = true;
   e->evaluated = false;
   return BS_OK;
@@ -1528,6 +1584,7 @@ int bs_upload_groups(bs_engine* e, const bs_group_table* t) {
   BS_DEVICE_GUARD(e);
   HP_BEGIN(e);
   e->have_groups = false;
+  e->have_bound = false;   // the bound rows' group indices refer to the old table
   e->evaluated = false;
   const uint32_t Gp = std::max(G, 1u);
   int rc;
@@ -2326,6 +2383,261 @@ int bs_replay(bs_engine* e, const uint32_t* queue, uint32_t n_queue, bs_replay_r
     if (out->group_rep_sel) out->group_rep_sel[g] = k.sel;
     if (out->group_rep_tol) out->group_rep_tol[g] = k.tol;
   }
+  return BS_OK;
+}
+
+// ---- preemption: bs_upload_bound_pods, bs_preempt, bs_remove_pod (preempt.cuh) ----
+int bs_upload_bound_pods(bs_engine* e, const bs_bound_table* t) {
+  if (!e || !t) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!e->have_nodes) return fail(e, BS_E_STATE, "bs_upload_bound_pods: upload nodes first");
+  if (t->n_lanes != e->L) return fail(e, BS_E_INVAL, "bs_upload_bound_pods: n_lanes differs from the engine's");
+  const uint32_t V = t->n_pods, L = e->L, N = e->N;
+  if (V && (!t->node || !t->req || !t->req_present || !t->gid || !t->priority || !t->start_ns || !t->flags))
+    return fail(e, BS_E_INVAL, "bs_upload_bound_pods: null column");
+  e->have_bound = false;   // a failing table is dropped
+  // rows: node index, scalar keys within the node's, value range
+  BoundStats bs = Chunks(V, 8192).reduce<BoundStats>([&](int, uint32_t a0, uint32_t a1, BoundStats& st) {
+    for (uint32_t v = a0; v < a1; ++v) {
+      const uint32_t n = t->node[v];
+      if (n >= N) { st.bad_index = true; continue; }
+      st.bad_keys = st.bad_keys || (t->req_present[v] & ~0xFu & ~e->h_nrpres[n]) != 0;
+      st.max_gid = std::max(st.max_gid, t->gid[v]);
+      st.bad_index = st.bad_index || t->gid[v] < BS_GID_MISSING;   // neither a group, BS_GID_NONE nor BS_GID_MISSING
+    }
+    for (uint32_t d = 0; d < L; ++d) {
+      if (d == (uint32_t)LANE_PODS) continue;
+      const int64_t* r = t->req + (size_t)d * V;
+      int64_t lo = 0, hi = 0;
+      for (uint32_t v = a0; v < a1; ++v) { lo = std::min(lo, r[v]); hi = std::max(hi, r[v]); }
+      st.bad_range = st.bad_range || lo < -BS_VALUE_LIMIT || hi > BS_VALUE_LIMIT;
+    }
+  });
+  if (bs.bad_index) return fail(e, BS_E_INDEX, "bs_upload_bound_pods: node index outside the snapshot or gid < BS_GID_MISSING");
+  // CSR by node
+  std::vector<uint32_t> row(N + 1, 0), order(V);
+  for (uint32_t v = 0; v < V; ++v) row[t->node[v] + 1]++;
+  for (uint32_t n = 0; n < N; ++n) {
+    bs.bad_count = bs.bad_count || (int64_t)row[n + 1] > (int64_t)e->h_npc[n];
+    row[n + 1] += row[n];
+  }
+  if (bs.bad_count) return fail(e, BS_E_INVAL, "bs_upload_bound_pods: more bound pods on a node than its pod_count");
+  if (bs.bad_keys) return fail(e, BS_E_INVAL, "bs_upload_bound_pods: scalar keys outside the node's req_present");
+  if (bs.bad_range) return fail(e, BS_E_RANGE, "bs_upload_bound_pods: value outside +-2^56");
+  {
+    std::vector<uint32_t> fill(row.begin(), row.end() - 1);
+    for (uint32_t v = 0; v < V; ++v) order[fill[t->node[v]]++] = v;   // table order within a node
+  }
+  // per node: MoreImportantPod order (priority descending, start ascending, index ascending) and the suffix range
+  const int64_t* req = t->req;
+  const bool suffix_bad = Chunks(N, 1024).reduce<BoundStats>([&](int, uint32_t n0, uint32_t n1, BoundStats& st) {
+    for (uint32_t n = n0; n < n1; ++n) {
+      uint32_t* a = order.data() + row[n];
+      std::sort(a, order.data() + row[n + 1], [&](uint32_t x, uint32_t y) {
+        if (t->priority[x] != t->priority[y]) return t->priority[x] > t->priority[y];
+        if (t->start_ns[x] != t->start_ns[y]) return t->start_ns[x] < t->start_ns[y];
+        return x < y;
+      });
+      for (uint32_t d = 0; d < L && !st.bad_range; ++d) {
+        if (d == (uint32_t)LANE_PODS) continue;
+        int64_t s = 0;
+        for (uint32_t k = row[n + 1]; k-- > row[n];) {
+          const uint32_t v = order[k];
+          if (d >= 4 && !((t->req_present[v] >> d) & 1u)) continue;
+          s += req[(size_t)d * V + v];
+          st.bad_range = st.bad_range || s < -BS_VALUE_LIMIT || s > BS_VALUE_LIMIT;
+        }
+      }
+    }
+  }).bad_range;
+  if (suffix_bad) return fail(e, BS_E_RANGE, "bs_upload_bound_pods: a per-node suffix sum outside +-2^56");
+  // columns in CSR order: lane 3 and scalar lanes the row has no key for are not removed
+  const size_t Vp = std::max(V, 1u);
+  std::vector<int32_t> prio(Vp, 0), gid(Vp, 0);
+  std::vector<int64_t> start(Vp, 0), breq((size_t)L * Vp, 0);
+  std::vector<uint8_t> flags(Vp, 0);
+  Chunks(V, 8192).run([&](int, uint32_t k0, uint32_t k1) {
+    for (uint32_t k = k0; k < k1; ++k) {
+      const uint32_t v = order[k];
+      prio[k] = t->priority[v];
+      gid[k] = t->gid[v];
+      start[k] = t->start_ns[v];
+      flags[k] = t->flags[v];
+      for (uint32_t d = 0; d < L; ++d)
+        if (d != (uint32_t)LANE_PODS && (d < 4 || ((t->req_present[v] >> d) & 1u))) breq[(size_t)d * V + k] = req[(size_t)d * V + v];
+    }
+  });
+  BS_DEVICE_GUARD(e);
+  int rc;
+  if ((rc = upload_vec(e, e->d_brow, row.data(), N + 1, N + 1))) return rc;
+  if ((rc = upload_vec(e, e->d_bprio, prio.data(), V, (uint32_t)Vp))) return rc;
+  if ((rc = upload_vec(e, e->d_bstart, start.data(), V, (uint32_t)Vp))) return rc;
+  if ((rc = upload_vec(e, e->d_bgid, gid.data(), V, (uint32_t)Vp))) return rc;
+  if ((rc = upload_vec(e, e->d_bflags, flags.data(), V, (uint32_t)Vp))) return rc;
+  if ((rc = upload_vec(e, e->d_bidx, order.data(), V, (uint32_t)Vp))) return rc;
+  if ((rc = upload_col(e, col(breq.data(), e->d_breq, L), (uint32_t)Vp, (uint32_t)Vp))) return rc;
+  CK(e->d_bsuf.ensure((size_t)L * Vp * 8));
+  CK(e->d_bsuf_online.ensure(Vp * 4));
+  CK(e->d_bsuf_bad.ensure(Vp * 4));
+  // the residuals the bound table is read against: node_left_kernel with no lane-class tables, into buffers of
+  // its own (the round's tables stay as they are)
+  CK(e->d_pl_left.ensure((size_t)L * e->Npad * 8));
+  CK(e->d_pl_present.ensure((size_t)e->Npad * 4));
+  if (N) {
+    preempt_prep_kernel<<<cdiv(N, 256), 256, 0, e->s>>>(e->d_brow.as<uint32_t>(), e->d_bgid.as<int32_t>(),
+                                                       e->d_bflags.as<uint8_t>(), e->d_breq.as<int64_t>(),
+                                                       e->d_bsuf.as<int64_t>(), e->d_bsuf_online.as<uint32_t>(),
+                                                       e->d_bsuf_bad.as<uint32_t>(), N, (uint32_t)Vp, L);
+    ++e->launches;
+  }
+  node_left_kernel<<<cdiv(e->Npad, 256), 256, 0, e->s>>>(node_tab(e), LaneMap{}, nullptr, nullptr,
+                                                         e->d_pl_present.as<uint32_t>(), nullptr,
+                                                         e->d_pl_left.as<int64_t>());
+  ++e->launches;
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(e->s));   // the host vectors die here
+  e->h_bgid.assign(t->gid, t->gid + V);
+  e->h_bflags.assign(t->flags, t->flags + V);
+  e->V = V;
+  e->bound_max_gid = bs.max_gid;
+  e->have_bound = true;
+  return BS_OK;
+}
+
+int bs_preempt(bs_engine* e, const uint32_t* pods, uint32_t n, bs_preempt_result* out) {
+  if (!e || !out || (n && (!pods || !out->node || !out->n_victims || !out->n_candidates)) || !out->victim_offset)
+    return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!e->have_nodes || !e->have_groups || !e->have_pods || !e->have_bound)
+    return fail(e, BS_E_STATE, "bs_preempt: upload nodes, groups, pods and the bound-pod table first");
+  if (e->bound_max_gid >= (int32_t)e->G) return fail(e, BS_E_INDEX, "bs_preempt: a bound pod's group index >= n_groups");
+  const uint32_t L = e->L, N = e->N;
+  std::vector<PreemptPod> pp(std::max(n, 1u));
+  for (uint32_t i = 0; i < n; ++i) {
+    const uint32_t p = pods[i];
+    if (p >= e->P) return fail(e, BS_E_INDEX, "bs_preempt: pod index outside the pod table");
+    const ClassKey& k = e->fit_index.keys[e->h_pfc[p]];
+    if (k.aff != BS_AFF_NONE && k.aff >= e->n_aff)
+      return fail(e, BS_E_INDEX, "bs_preempt: affinity class outside the uploaded table");
+    pp[i] = PreemptPod{k.sel, k.tol, p, k.nz, k.aff, e->h_prio[p], e->h_gid[p]};
+  }
+  out->victim_offset[0] = 0;
+  out->victims_total = 0;
+  if (!n) return BS_OK;
+  BS_DEVICE_GUARD(e);
+  CK(e->d_pp.ensure((size_t)n * sizeof(PreemptPod)));
+  CK(e->d_pnode.ensure((size_t)n * 4));
+  CK(e->d_pnv.ensure((size_t)n * 4));
+  CK(e->d_pcand.ensure((size_t)n * 4));
+  CK(e->d_poff.ensure((size_t)n * 4));
+  CK(cudaMemcpyAsync(e->d_pp.p, pp.data(), (size_t)n * sizeof(PreemptPod), cudaMemcpyHostToDevice, e->s));
+  PreemptArgs a{};
+  a.t = node_tab(e);
+  a.left = e->d_pl_left.as<int64_t>();
+  a.left_present = e->d_pl_present.as<uint32_t>();
+  a.b = BoundTab{e->d_brow.as<uint32_t>(), e->d_bprio.as<int32_t>(), e->d_bstart.as<int64_t>(), e->d_bgid.as<int32_t>(),
+                 e->d_bflags.as<uint8_t>(), e->d_bidx.as<uint32_t>(), e->d_breq.as<int64_t>(), e->d_bsuf.as<int64_t>(),
+                 e->d_bsuf_online.as<uint32_t>(), e->d_bsuf_bad.as<uint32_t>(), std::max(e->V, 1u)};
+  a.pp = e->d_pp.as<PreemptPod>();
+  a.preq = e->d_req.as<int64_t>();
+  a.preq_present = e->d_ppres.as<uint32_t>();
+  a.P = e->P;
+  a.n = n;
+  a.out_node = e->d_pnode.as<int32_t>();
+  a.out_nv = e->d_pnv.as<uint32_t>();
+  a.out_cand = e->d_pcand.as<uint32_t>();
+  a.n_tiles = cdiv(N, PREEMPT_THREADS);
+  if (!N) {
+    CK(cudaMemsetAsync(a.out_node, 0xff, (size_t)n * 4, e->s));
+    CK(cudaMemsetAsync(a.out_nv, 0, (size_t)n * 4, e->s));
+    CK(cudaMemsetAsync(a.out_cand, 0, (size_t)n * 4, e->s));
+  } else {
+    // preemptors in chunks: one grid row each (gridDim.y <= 65535), per-tile keys within a 256 MiB budget
+    const size_t per = (size_t)a.n_tiles * sizeof(PickKey);
+    const uint32_t chunk = (uint32_t)std::max<size_t>(1, std::min<size_t>({(size_t)65535, (size_t)n, ((size_t)256 << 20) / per}));
+    CK(e->d_ptiles.ensure((size_t)chunk * per));
+    a.tiles = e->d_ptiles.as<PickKey>();
+    for (uint32_t p0 = 0; p0 < n; p0 += chunk) {
+      const uint32_t cnt = std::min(chunk, n - p0);
+      a.p0 = p0;
+      launch_maxl<PreemptNodeLaunch>(L, dim3(a.n_tiles, cnt), (cudaStream_t)e->s, a);
+      preempt_reduce_kernel<<<cdiv(cnt, 256), 256, 0, e->s>>>(a, cnt);
+      e->launches += 2;
+    }
+  }
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(out->node, a.out_node, (size_t)n * 4, cudaMemcpyDeviceToHost, e->s));
+  CK(cudaMemcpyAsync(out->n_victims, a.out_nv, (size_t)n * 4, cudaMemcpyDeviceToHost, e->s));
+  CK(cudaMemcpyAsync(out->n_candidates, a.out_cand, (size_t)n * 4, cudaMemcpyDeviceToHost, e->s));
+  CK(cudaStreamSynchronize(e->s));
+  uint64_t total = 0;
+  for (uint32_t i = 0; i < n; ++i) {
+    out->victim_offset[i] = (uint32_t)std::min<uint64_t>(total, UINT32_MAX);
+    total += out->n_victims[i];
+  }
+  out->victim_offset[n] = (uint32_t)std::min<uint64_t>(total, UINT32_MAX);
+  out->victims_total = (uint32_t)std::min<uint64_t>(total, UINT32_MAX);
+  if (total > out->victims_cap) return fail(e, BS_E_INVAL, "bs_preempt: victims_cap is smaller than victims_total");
+  if (!total) return BS_OK;
+  if (!out->victims) return fail(e, BS_E_INVAL, "bs_preempt: null victims buffer");
+  CK(e->d_pvict.ensure((size_t)total * 4));
+  CK(cudaMemcpyAsync(e->d_poff.p, out->victim_offset, (size_t)n * 4, cudaMemcpyHostToDevice, e->s));
+  a.offset = e->d_poff.as<uint32_t>();
+  a.victims = e->d_pvict.as<uint32_t>();
+  launch_maxl<PreemptEmitLaunch>(L, dim3(cdiv(n, 256)), (cudaStream_t)e->s, a);
+  ++e->launches;
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(out->victims, a.victims, (size_t)total * 4, cudaMemcpyDeviceToHost, e->s));
+  CK(cudaStreamSynchronize(e->s));
+  return BS_OK;
+}
+
+// core.PreemptRemovePod (core.go:203-260).  "Offline" = carries the group label (VerifyPodLabelSatisfied,
+// k8s.go:62-70): gid >= 0 or BS_GID_MISSING.  The same-group test (:251) compares fullNameToRemove, which is "" when
+// checkPreemption failed, so a victim of p's own group whose group is locked reports the phase message.
+int bs_remove_pod(bs_engine* e, uint32_t pod, uint32_t bound, bs_status* st) {
+  if (!e || !st) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!e->have_pods || !e->have_groups || !e->have_bound)
+    return fail(e, BS_E_STATE, "bs_remove_pod: upload groups, pods and the bound-pod table first");
+  if (pod >= e->P || bound >= e->V) return fail(e, BS_E_INDEX, "bs_remove_pod: index out of range");
+  const int32_t gp = e->h_gid[pod], gv = e->h_bgid[bound];
+  if (gv >= (int32_t)e->G) return fail(e, BS_E_INDEX, "bs_remove_pod: the bound pod's group index >= n_groups");
+  const bool off_p = gp != BS_GID_NONE, off_v = gv != BS_GID_NONE;
+  int reason = BS_REMOVE_ALLOW;
+  if (!off_p && !off_v) reason = BS_REMOVE_ALLOW;                               // :213-215
+  else if (off_p && !off_v) reason = BS_REMOVE_OFFLINE_ONLINE;                  // :216-218
+  else {
+    int check = BS_REMOVE_ALLOW;                                                // checkPreemption :220-240
+    if (gv < 0) check = BS_REMOVE_NOT_FOUND;                                    // :222-225
+    else if (e->h_bflags[bound] & BS_BOUND_GROUP_LOCKED) check = BS_REMOVE_LOCKED;   // :234-238
+    if (!off_p) reason = check;                                                 // :245-247
+    else if (check == BS_REMOVE_ALLOW && gp >= 0 && gp == gv) reason = BS_REMOVE_SAME_GROUP;   // :250-253
+    else reason = check;                                                        // :254-256
+  }
+  st->reason = reason;
+  st->code = reason == BS_REMOVE_ALLOW ? BS_CODE_SUCCESS : BS_CODE_UNSCHEDULABLE;   // batchscheduler.go:137-143
+  st->group = off_v && gv >= 0 ? gv : -1;
+  return BS_OK;
+}
+
+int bs_format_remove_message(const bs_status* st, const char* pod_name, const char* victim_name,
+                             const char* victim_ns_name, char* buf, size_t buf_len) {
+  if (!st || !buf || !buf_len) return BS_E_INVAL;
+  std::string m;
+  switch (st->reason) {
+    case BS_REMOVE_ALLOW: break;
+    case BS_REMOVE_OFFLINE_ONLINE:
+      m = std::string("offline pods ") + (pod_name ? pod_name : "") + " are forbidden to preempt online " +
+          (victim_name ? victim_name : "");
+      break;
+    case BS_REMOVE_NOT_FOUND: m = std::string("can not found pod group: ") + (victim_ns_name ? victim_ns_name : ""); break;
+    case BS_REMOVE_LOCKED: m = "pod belongs to Scheduled or Running pod group can not be scheduled"; break;
+    case BS_REMOVE_SAME_GROUP: m = "podToSchedule and podToRemove belong to same pod group, do not preempt"; break;
+    default: return BS_E_INVAL;
+  }
+  if (m.size() + 1 > buf_len) return BS_E_INVAL;
+  memcpy(buf, m.c_str(), m.size() + 1);
   return BS_OK;
 }
 

@@ -929,6 +929,9 @@ Status BatchSchedulingPlugin::BeginRound(const std::vector<const NodeInfo*>& sna
   node_row_.build(snapshot.size(), [&](size_t i) { return snapshot[i] && snapshot[i]->node ? &snapshot[i]->node->name : nullptr; },
                   pack_threads(snapshot.size()));
   node_names_.assign(snapshot.size(), std::string());
+  snapshot_ = snapshot;
+  pending_uid_.resize(pending.size());
+  for (size_t i = 0; i < pending.size(); ++i) pending_uid_[i] = pending[i]->uid;
   for (size_t i = 0; i < snapshot.size(); ++i)
     if (snapshot[i] && snapshot[i]->node) node_names_[i] = snapshot[i]->node->name;
   lap("node rows");
@@ -961,6 +964,10 @@ Status BatchSchedulingPlugin::BeginRound(const std::vector<const NodeInfo*>& sna
   if (packed_.n_aff() && (rc = bs_upload_affinity(eng_, packed_.n_aff(), packed_.aff_bits.data()))) return fail(rc);
   if ((rc = bs_upload_groups(eng_, &gt))) return fail(rc);
   if ((rc = bs_upload_pods(eng_, &pt))) return fail(rc);
+  {
+    Status bst = UploadBound();   // after the groups: the bound rows' group indices refer to this table
+    if (!bst.ok()) return bst;
+  }
   if ((rc = bs_set_wait_time(eng_, max_schedule_time_ns_, packed_.wait_ns.data(), packed_.n_groups))) return fail(rc);
   if (!state_ready_) {
     if ((rc = bs_state_reset(eng_))) return fail(rc);
@@ -1148,7 +1155,10 @@ Status BatchSchedulingPlugin::UpdateNodes(const std::vector<std::pair<uint32_t, 
     packed_.pod_count[i] = delta.pod_count[k]; packed_.alloc_present[i] = delta.alloc_present[k];
     packed_.req_present[i] = delta.req_present[k]; packed_.label_mask[i] = delta.label_mask[k];
     packed_.taint_mask[i] = delta.taint_mask[k]; packed_.node_flags[i] = delta.node_flags[k];
+    if (i < snapshot_.size()) snapshot_[i] = rows[k];
   }
+  st = UploadBound();   // bs_update_nodes dropped the bound-pod table: the changed NodeInfos list their pods again
+  if (!st.ok()) return st;
   // the round's decisions follow the new snapshot: same pods, same groups, same result vectors
   return evaluate ? Reevaluate() : Status{};
 }
@@ -1218,7 +1228,153 @@ Status BatchSchedulingPlugin::UpdateGroups(const std::vector<std::string>& ns_na
   }
   if ((rc = bs_set_wait_time(eng_, max_schedule_time_ns_, packed_.wait_ns.data(), G)))
     return Status{BS_CODE_ERROR, std::string("bsched: ") + bs_strerror(rc)};
+  st = UploadBound();   // a changed Status.Phase locks or unlocks the bound pods of its group
+  if (!st.ok()) return st;
   return evaluate ? Reevaluate() : Status{};
+}
+
+// ---- preemption: the bound-pod table, RemovePod, Preempt ----
+bs_bound_table PackedBound::table() const {
+  return bs_bound_table{n, lanes, node.data(), req.data(), req_present.data(), gid.data(), priority.data(),
+                        start_ns.data(), flags.data()};
+}
+
+Status BatchSchedulingPlugin::PackBoundPods(const PackedSnapshot& ctx, const std::vector<const NodeInfo*>& snapshot,
+                                            const std::unordered_map<std::string, uint32_t>& group_row,
+                                            const std::vector<uint8_t>& locked, PackedBound* out) {
+  if (!out) return Status{BS_CODE_ERROR, "PackBoundPods: null output"};
+  PackedBound& b = *out;
+  b = PackedBound();
+  b.lanes = ctx.lanes;
+  LaneTable lt;
+  for (auto& s : ctx.scalar_names) lt.add(s);   // lane 4 + k, as in the round
+  for (uint32_t i = 0; i < snapshot.size(); ++i)
+    if (snapshot[i])
+      for (const Pod* p : snapshot[i]->pods)
+        if (p) b.pods.push_back(p), b.node.push_back(i);
+  const uint32_t V = b.n = (uint32_t)b.pods.size(), L = b.lanes;
+  b.req.assign((size_t)L * V, 0);
+  b.req_present.assign(V, 0); b.gid.assign(V, BS_GID_NONE); b.priority.assign(V, 0); b.start_ns.assign(V, 0);
+  b.flags.assign(V, 0);
+  std::vector<int64_t> v(L);
+  for (uint32_t k = 0; k < V; ++k) {
+    const Pod& p = *b.pods[k];
+    std::fill(v.begin(), v.end(), 0);
+    for (const Container& c : p.containers) {
+      // NodeInfo.RemovePod subtracts the pod's Requests (calculateResource, [upstream, from memory]), never its Limits
+      const Encoded r = add_list(lt, c.requests, v.data(), &b.req_present[k], kBadContainers);
+      if (r == kNeedsFull)
+        return Status{BS_CODE_ERROR, "PackBoundPods: pod " + p.ns + "/" + p.name + " requests a scalar resource its node's requested lacks"};
+      if (r != kEncoded) return Status{BS_CODE_ERROR, std::string("PackBoundPods: ") + kEncodeError[r]};
+    }
+    for (uint32_t d = 0; d < L; ++d) b.req[(size_t)d * V + k] = d == (uint32_t)kLanePods ? 0 : v[d];
+    b.priority[k] = p.priority;
+    b.start_ns[k] = p.start_ns;
+    auto lb = p.labels.find(kPodGroupLabel);   // VerifyPodLabelSatisfied (k8s.go:62-70)
+    if (lb != p.labels.end() && !lb->second.empty()) {
+      auto it = group_row.find(p.ns + "/" + lb->second);   // checkPreemption's fullNameToRemove (core.go:221)
+      if (it == group_row.end()) b.gid[k] = BS_GID_MISSING;
+      else {
+        b.gid[k] = (int32_t)it->second;
+        if (it->second < locked.size() && locked[it->second]) b.flags[k] = BS_BOUND_GROUP_LOCKED;
+      }
+    }
+  }
+  return Status{};
+}
+
+Status BatchSchedulingPlugin::UploadBound() {
+  bool any = false;
+  for (const NodeInfo* ni : snapshot_) any = any || (ni && !ni->pods.empty());
+  if (!any) {
+    bound_ = PackedBound();
+    bound_row_.clear();
+    return Status{};
+  }
+  std::vector<uint8_t> locked(group_names_.size(), 0);
+  for (size_t g = 0; g < group_names_.size(); ++g) {
+    auto it = groups_.find(group_names_[g]);
+    if (it != groups_.end()) locked[g] = it->second.pg.phase == "Scheduled" || it->second.pg.phase == "Running";
+  }
+  Status st = PackBoundPods(packed_, snapshot_, group_row_, locked, &bound_);
+  if (!st.ok()) return st;
+  bound_row_.build(bound_.n, [&](size_t k) { return &bound_.pods[k]->uid; }, pack_threads(bound_.n));
+  const bs_bound_table t = bound_.table();
+  const int rc = bs_upload_bound_pods(eng_, &t);
+  if (rc) return Status{BS_CODE_ERROR, std::string("bsched: ") + bs_strerror(rc) + " (" + bs_last_error(eng_) + ")"};
+  return Status{};
+}
+
+Status BatchSchedulingPlugin::RemovePod(const Pod& preemptor, const Pod& victim) {
+  std::lock_guard<std::mutex> lk(mu_);
+  const int32_t p = pod_row_.find(preemptor.uid), v = bound_row_.find(victim.uid);
+  if (!eng_ || p < 0 || v < 0) return Status{BS_CODE_ERROR, "RemovePod: the pods are not part of the round"};
+  bs_status st{};
+  int rc = bs_remove_pod(eng_, (uint32_t)p, (uint32_t)v, &st);
+  if (rc) return Status{BS_CODE_ERROR, std::string("bsched: ") + bs_strerror(rc) + " (" + bs_last_error(eng_) + ")"};
+  if (st.code == BS_CODE_SUCCESS) return Status{};
+  auto lb = victim.labels.find(kPodGroupLabel);
+  const std::string victim_group = victim.ns + "/" + (lb == victim.labels.end() ? std::string() : lb->second);
+  char buf[1024];
+  rc = bs_format_remove_message(&st, preemptor.name.c_str(), victim.name.c_str(), victim_group.c_str(), buf, sizeof buf);
+  if (rc) return Status{BS_CODE_ERROR, "RemovePod: message does not fit"};
+  return Status{st.code, buf};   // framework.NewStatus(framework.Unschedulable, err.Error()) (batchscheduler.go:137-141)
+}
+
+Status BatchSchedulingPlugin::RunPreempt(const std::vector<uint32_t>& rows, std::vector<Preemption>* out) {
+  const uint32_t n = (uint32_t)rows.size();
+  std::vector<int32_t> node(n);
+  std::vector<uint32_t> nv(n), cand(n), off(n + 1);
+  std::vector<uint32_t> vict;
+  bs_preempt_result r{node.data(), nv.data(), cand.data(), off.data(), nullptr, 0, 0};
+  int rc = bs_preempt(eng_, rows.data(), n, &r);
+  if (rc == BS_E_INVAL && r.victims_total > 0) {   // the first call sized the victim list
+    vict.resize(r.victims_total);
+    r.victims = vict.data();
+    r.victims_cap = r.victims_total;
+    rc = bs_preempt(eng_, rows.data(), n, &r);
+  }
+  if (rc) return Status{BS_CODE_ERROR, std::string("bsched: ") + bs_strerror(rc) + " (" + bs_last_error(eng_) + ")"};
+  out->resize(n);
+  for (uint32_t i = 0; i < n; ++i) {
+    Preemption& pr = (*out)[i];
+    pr.node = node[i] >= 0 ? node_names_[node[i]] : std::string();
+    pr.victims.clear();
+    for (uint32_t k = off[i]; k < off[i + 1]; ++k) pr.victims.push_back(bound_.pods[vict[k]]->uid);
+  }
+  return Status{};
+}
+
+Status BatchSchedulingPlugin::Preempt(const std::string& uid, std::string* node, std::vector<std::string>* victim_uids) {
+  std::lock_guard<std::mutex> lk(mu_);
+  const int32_t p = pod_row_.find(uid);
+  if (!eng_ || p < 0) return Status{BS_CODE_ERROR, "Preempt: " + uid + " is not a pending pod of the round"};
+  if (!bound_.n) {   // no NodeInfo lists pods: nothing to evict, the table was never uploaded
+    if (node) node->clear();
+    if (victim_uids) victim_uids->clear();
+    return Status{};
+  }
+  std::vector<Preemption> res;
+  Status st = RunPreempt({(uint32_t)p}, &res);
+  if (!st.ok()) return st;
+  if (node) *node = res[0].node;
+  if (victim_uids) *victim_uids = res[0].victims;
+  return Status{};
+}
+
+Status BatchSchedulingPlugin::PreemptAll(std::vector<Preemption>* out) {
+  std::lock_guard<std::mutex> lk(mu_);
+  if (!eng_ || !out) return Status{BS_CODE_ERROR, "PreemptAll: no round has been started"};
+  out->clear();
+  if (!bound_.n) return Status{};
+  std::vector<uint32_t> rows;
+  for (uint32_t i = 0; i < packed_.n_pods; ++i)
+    if (prefilter_[i] == BS_PF_PASS && feasible_[i] == 0) rows.push_back(i);
+  if (rows.empty()) return Status{};
+  Status st = RunPreempt(rows, out);
+  if (!st.ok()) return st;
+  for (size_t k = 0; k < rows.size(); ++k) (*out)[k].uid = pending_uid_[rows[k]];
+  return Status{};
 }
 
 Status BatchSchedulingPlugin::ReplayQueue(std::vector<ReplayDecision>* out) {

@@ -64,6 +64,7 @@ struct Pod {
   std::vector<std::string> owner_uids;  // OwnerReferences[].UID (core.go:483-485)
   int32_t priority = 0;                 // podutil.GetPodPriority
   int64_t queue_ts_ns = 0;              // framework.PodInfo.Timestamp
+  int64_t start_ns = 0;                 // Status.StartTime of a bound pod (preemption: MoreImportantPod)
 };
 struct Node {
   std::string name;
@@ -77,6 +78,7 @@ struct NodeInfo {          // k8s.io/kubernetes/pkg/scheduler/nodeinfo.NodeInfo,
   ResourceList requested;      // info.RequestedResource()
   int32_t num_pods = 0;        // len(info.Pods())
   bool taints_error = false;   // info.Taints() returned an error (core.go:639)
+  std::vector<const Pod*> pods;   // info.Pods(): the pods bound to the node, what preemption may evict (may be empty)
 };
 struct PodGroup {          // pkg/apis/podgroup/v1/types.go:62-130 (fields on the path)
   std::string ns, name;
@@ -87,6 +89,7 @@ struct PodGroup {          // pkg/apis/podgroup/v1/types.go:62-130 (fields on th
   uint32_t scheduled = 0;             // Status.Scheduled
   std::string occupied_by;            // Status.OccupiedBy
   int64_t creation_ns = 0;
+  std::string phase;                  // Status.Phase ("Scheduled" / "Running" lock its pods against preemption, core.go:235-236)
 };
 
 struct Status {  // framework.Status
@@ -157,6 +160,17 @@ struct PackedSnapshot {
 // string -> row index of one round, built in one go: the keys are copied into ONE arena (no allocation per key),
 // hashed in parallel, and a later duplicate overwrites an earlier one, as `map[key] = row` in a loop would.
 // Lookups are exact (the arena bytes are compared), not by hash alone.
+// The bound-pod table of a round (bs_bound_table): every pod NodeInfo.Pods() lists, in snapshot order.
+struct PackedBound {
+  uint32_t lanes = BS_FIXED_LANES, n = 0;
+  std::vector<uint32_t> node, req_present;
+  std::vector<int64_t> req, start_ns;   // req: [lanes][n], the containers' Requests
+  std::vector<int32_t> gid, priority;
+  std::vector<uint8_t> flags;
+  std::vector<const Pod*> pods;
+  bs_bound_table table() const;
+};
+
 class StrIndex {
  public:
   // key_at(i) -> const std::string* (nullptr: row i has no key)
@@ -321,6 +335,29 @@ class BatchSchedulingPlugin {
   Status UpdateGroups(const std::vector<std::string>& ns_names, int64_t now_ns, bool evaluate = true);
 
   // the packer alone (no GPU): objects -> tables
+  // The bound pods of `snapshot` against the lanes of `ctx`: demand = the containers' Requests (NodeInfo.RemovePod
+  // subtracts what AddPod added: Requests, not Limits); gid from the group label and "ns/<label>" in group_row
+  // (BS_GID_NONE without the label, BS_GID_MISSING when the group is not in the table); BS_BOUND_GROUP_LOCKED when
+  // that group's row is in `locked` (Status.Phase Scheduled or Running).
+  static Status PackBoundPods(const PackedSnapshot& ctx, const std::vector<const NodeInfo*>& snapshot,
+                              const std::unordered_map<std::string, uint32_t>& group_row,
+                              const std::vector<uint8_t>& locked, PackedBound* out);
+  // batchSchedulingPluginExtension.RemovePod (batchscheduler.go:132-144) -> core.PreemptRemovePod (core.go:203-260):
+  // the preemptor must be a pending pod of the round, the victim a pod some NodeInfo of the round lists
+  Status RemovePod(const Pod& preemptor, const Pod& victim);
+  // PreemptAddPod always succeeds (core.go:194-196)
+  Status AddPod(const Pod&, const Pod&) { return Status{}; }
+  // genericScheduler.Preempt for one pending pod of the round against the round's snapshot: the node preemption would
+  // pick ("" none) and the uids of the pods it would evict there, most important first
+  Status Preempt(const std::string& uid, std::string* node, std::vector<std::string>* victim_uids);
+  struct Preemption {
+    std::string uid, node;
+    std::vector<std::string> victims;
+  };
+  // Preempt for every pending pod that passed PreFilter and fits no node (upstream preempts only on a FitError)
+  Status PreemptAll(std::vector<Preemption>* out);
+  const PackedBound& bound() const { return bound_; }
+
   static Status Pack(const std::vector<const NodeInfo*>& snapshot, const std::vector<const Pod*>& pending,
                      const std::vector<PodGroup>& groups, const std::vector<uint32_t>& matched,
                      const std::vector<uint8_t>& extra_group_flags, const std::vector<uint8_t>& extra_pod_flags,
@@ -369,6 +406,12 @@ class BatchSchedulingPlugin {
   Status Reevaluate();   // bs_evaluate into the round's result vectors + the deny side effect (core.go:142,163)
   int FetchTopK();       // the round's top-K lists into topk_node_ / topk_score_ (no-op without topk)
   int FetchReasons();    // the round's reason rows into reasons_ (no-op without BS_OUT_REASONS)
+  Status UploadBound();  // packs and uploads the bound-pod table of snapshot_ (no-op when no NodeInfo lists pods)
+  Status RunPreempt(const std::vector<uint32_t>& rows, std::vector<Preemption>* out);
+  std::vector<const NodeInfo*> snapshot_;                           // the round's NodeInfos (bound pods)
+  std::vector<std::string> pending_uid_;                            // pending index -> uid
+  PackedBound bound_;
+  StrIndex bound_row_;                                              // uid -> bound-table row
 };
 
 }  // namespace bsched

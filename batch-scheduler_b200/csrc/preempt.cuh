@@ -1,0 +1,274 @@
+// preempt.cuh — sm_90a kernels of bs_preempt: for each preemptor, the node kube-scheduler's preemption would pick and
+// the victims it would evict there (genericScheduler.Preempt -> selectVictimsOnNode -> pickOneNodeForPreemption,
+// k8s v1.17.5 [upstream, from memory]; DESIGN.md §2 "Preemption"), with the plugin's RemovePod rule
+// (core.PreemptRemovePod, core.go:203-260) as the gate on every potential victim.
+//
+// The bound pods of a node are stored as one CSR segment in MoreImportantPod order (priority descending, start time
+// ascending, table index ascending), so the potential victims of a preemptor (priority strictly lower) are a SUFFIX
+// of the segment.  preempt_prep_kernel builds, per CSR position, the suffix sums of the removable lanes and the
+// suffix counts of the rows RemovePod refuses for some preemptor; the hot kernel answers "all victims removed"
+// with one binary search and one suffix read per (preemptor, node) and walks the suffix only for the pairs that
+// survive that test.  The oracles in the tests mutate a copy of the node instead: the two must agree.
+#pragma once
+#include "kernels.cuh"
+
+namespace bsk {
+
+// bound-pod table grouped by node (CSR), columns in CSR position order
+struct BoundTab {
+  const uint32_t* row;      // [N + 1] segment of node n: [row[n], row[n + 1])
+  const int32_t* prio;      // [V]
+  const int64_t* start;     // [V]
+  const int32_t* gid;       // [V]
+  const uint8_t* flags;     // [V] BS_BOUND_*
+  const uint32_t* idx;      // [V] bound-table index
+  const int64_t* req;       // [L][V] removable amounts: lanes 0-2 and the row's scalar keys, 0 elsewhere
+  const int64_t* suf;       // [L][V] sum of req over positions k .. end of the segment
+  const uint32_t* suf_online;   // [V] rows without a group label in k .. end
+  const uint32_t* suf_bad;      // [V] rows whose group is missing or Scheduled / Running in k .. end
+  uint32_t V;
+};
+
+// one preemptor, as the host resolves it from the pod table and its fit class
+struct PreemptPod {
+  uint64_t sel, tol;
+  uint32_t pod;   // pod-table index
+  uint32_t nz;    // scalar keys requested with a non-zero amount (the class-fit presence rule)
+  uint32_t aff;   // affinity class or BS_AFF_NONE
+  int32_t prio, gid;
+};
+
+// pickOneNodeForPreemption's order over candidate nodes; the smaller key wins.  A candidate without victims wins
+// at once (lowest index); otherwise: highest victim priority, sum of (priority + 2^31), victim count, LATEST start
+// of the first (most important) victim, node index.  node = -1: no candidate.
+struct PickKey {
+  int64_t sum;
+  int64_t start;
+  int32_t hp;
+  uint32_t nv;
+  int32_t node;
+  uint32_t cand;   // candidates counted into this key (not part of the order)
+};
+
+__device__ __forceinline__ bool pick_less(const PickKey& a, const PickKey& b) {
+  if (a.node < 0) return false;
+  if (b.node < 0) return true;
+  if ((a.nv == 0) != (b.nv == 0)) return a.nv == 0;
+  if (a.nv != 0) {
+    if (a.hp != b.hp) return a.hp < b.hp;
+    if (a.sum != b.sum) return a.sum < b.sum;
+    if (a.nv != b.nv) return a.nv < b.nv;
+    if (a.start != b.start) return a.start > b.start;
+  }
+  return a.node < b.node;
+}
+
+__device__ __forceinline__ PickKey pick_min(const PickKey& a, const PickKey& b) {
+  PickKey r = pick_less(b, a) ? b : a;
+  r.cand = a.cand + b.cand;
+  return r;
+}
+
+__device__ __forceinline__ PickKey pick_none() {
+  PickKey k;
+  k.sum = 0; k.start = 0; k.hp = 0; k.nv = 0; k.node = -1; k.cand = 0;
+  return k;
+}
+
+// ---------------------------------------------------------------------------
+// preempt_prep_kernel — once per bound-table upload, one thread per node: suffix sums of the removable lanes and
+// suffix counts of the online and the missing-or-locked rows, walking the node's segment from its end.
+__global__ void preempt_prep_kernel(const uint32_t* __restrict__ row, const int32_t* __restrict__ gid,
+                                    const uint8_t* __restrict__ flags, const int64_t* __restrict__ req,
+                                    int64_t* __restrict__ suf, uint32_t* __restrict__ suf_online,
+                                    uint32_t* __restrict__ suf_bad, uint32_t N, uint32_t V, uint32_t L) {
+  const uint32_t n = blockIdx.x * blockDim.x + threadIdx.x;
+  if (n >= N) return;
+  const uint32_t b = row[n], e = row[n + 1];
+  uint32_t on = 0, bad = 0;
+  for (uint32_t k = e; k-- > b;) {
+    const int32_t g = gid[k];
+    on += g == BS_GID_NONE ? 1u : 0u;
+    bad += (g == BS_GID_MISSING || (g >= 0 && (flags[k] & BS_BOUND_GROUP_LOCKED))) ? 1u : 0u;
+    suf_online[k] = on;
+    suf_bad[k] = bad;
+  }
+  for (uint32_t d = 0; d < L; ++d) {
+    int64_t s = 0;
+    for (uint32_t k = e; k-- > b;) {
+      s += req[(size_t)d * V + k];
+      suf[(size_t)d * V + k] = s;
+    }
+  }
+}
+
+struct PreemptArgs {
+  NodeTab t;                  // node table (guards, masks, affinity bits, requested lane 3)
+  const int64_t* left;        // [L][Npad] node_left_kernel's full-width residuals at percent 1.0 (0 = key absent)
+  const uint32_t* left_present;   // [Npad] scalar keys of `left`
+  BoundTab b;
+  const PreemptPod* pp;       // [n] the preemptors
+  const int64_t* preq;        // [L][P] pod-table requests
+  const uint32_t* preq_present;   // [P]
+  uint32_t P, n;
+  uint32_t p0;                // first preemptor of this launch (grid.y covers [p0, p0 + gridDim.y))
+  PickKey* tiles;             // [gridDim.y][n_tiles] per-(preemptor, node tile) best keys
+  uint32_t n_tiles;
+  // reduce + emit
+  int32_t* out_node;
+  uint32_t* out_nv;
+  uint32_t* out_cand;
+  const uint32_t* offset;     // [n] exclusive scan of out_nv (emit)
+  uint32_t* victims;          // emit output
+};
+
+constexpr int PREEMPT_THREADS = 256;   // nodes per tile of the hot kernel
+
+// The fit predicate of the round (bso_fit_eval / the fit bitmap), on a node from which `freed` (per lane) and
+// `count` pods have been removed: left[d] + freed[d] >= req[d] on lanes 0-2 and on the scalar keys both sides have,
+// and on the pods lane left + count >= req when requested[3] == 0 (len(Pods()) is the pod count then, core.go:650-653),
+// else left >= req (lane 3 of requested is not touched by a removal).  The guards, checkFit and the absent-key rule
+// do not change under removal (victims' keys are a subset of the node's): they are the gate.
+template <int MAXL>
+__device__ __forceinline__ bool fits_freed(const int64_t* left, const int64_t* freed, const int64_t* req,
+                                           uint32_t cmask, int64_t pods_left, int64_t pods_req) {
+  bool ok = pods_left >= pods_req;
+#pragma unroll
+  for (int d = 0; d < MAXL; ++d)
+    if (d != LANE_PODS && ((cmask >> d) & 1u)) ok &= left[d] + freed[d] >= req[d];
+  return ok;
+}
+
+// selectVictimsOnNode for preemptor slot i on node n.  Returns false when the node is not a candidate; else the
+// key of the node, and with EMIT the victims' bound-table indices at out[0..).
+template <int MAXL, bool EMIT>
+__device__ bool select_victims(const PreemptArgs& a, const PreemptPod& q, const int64_t* req, uint32_t rpres,
+                               uint32_t n, PickKey& key, uint32_t* out) {
+  const NodeTab& t = a.t;
+  const uint8_t f = t.flags[n];
+  // the gate: the pod's fit-class bit (guards core.go:606-617 and :639, checkFit :741-759, absent-key rule :688-690)
+  if (node_skipped(f) || (f & BS_NODE_TAINTS_ERR) || !check_fit(t.label[n], t.taint[n], q.sel, q.tol) ||
+      !aff_ok(t, q.aff, n) || (q.nz & ~a.left_present[n]) != 0)
+    return false;
+  const uint32_t beg = a.b.row[n], end = a.b.row[n + 1];
+  // potential victims: priority strictly below the preemptor's, a suffix of the segment
+  uint32_t lo = beg, hi = end;
+  while (lo < hi) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (a.b.prio[mid] < q.prio) hi = mid;
+    else lo = mid + 1;
+  }
+  const uint32_t s = lo;
+  const bool offline = q.gid != BS_GID_NONE;
+  if (s < end) {
+    // RemovePod refuses some potential victim -> the node is dropped (upstream aborts its selection)
+    if (a.b.suf_bad[s] != 0) return false;
+    if (offline && a.b.suf_online[s] != 0) return false;
+    if (offline && q.gid >= 0)
+      for (uint32_t k = s; k < end; ++k)
+        if (a.b.gid[k] == q.gid) return false;
+  }
+  const uint32_t cmask = 0x7u | (rpres & a.left_present[n] & ~0xFu);
+  const bool pods_by_count = t.requested[(size_t)LANE_PODS * t.Npad + n] == 0;
+  int64_t left[MAXL], freed[MAXL];
+#pragma unroll
+  for (int d = 0; d < MAXL; ++d) {
+    left[d] = d < (int)t.L ? a.left[(size_t)d * t.Npad + n] : 0;
+    freed[d] = (d < (int)t.L && s < end) ? a.b.suf[(size_t)d * a.b.V + s] : 0;
+  }
+  const int64_t pods_left = left[LANE_PODS], pods_req = req[LANE_PODS];
+  uint32_t removed = end - s;
+  if (!fits_freed<MAXL>(left, freed, req, cmask, pods_left + (pods_by_count ? removed : 0), pods_req)) return false;
+  // reprieve, most important first: add each back; keep it when the pod still fits, else it is a victim
+  key = pick_none();
+  key.node = (int32_t)n;
+  key.cand = 1;
+  for (uint32_t k = s; k < end; ++k) {
+#pragma unroll
+    for (int d = 0; d < MAXL; ++d)
+      if (d < (int)t.L) freed[d] -= a.b.req[(size_t)d * a.b.V + k];
+    --removed;
+    if (fits_freed<MAXL>(left, freed, req, cmask, pods_left + (pods_by_count ? removed : 0), pods_req)) continue;
+#pragma unroll
+    for (int d = 0; d < MAXL; ++d)
+      if (d < (int)t.L) freed[d] += a.b.req[(size_t)d * a.b.V + k];
+    ++removed;
+    const int32_t pr = a.b.prio[k];
+    if (key.nv == 0) {
+      key.hp = pr;
+      key.start = a.b.start[k];
+    }
+    key.sum += (int64_t)pr + ((int64_t)1 << 31);
+    if (EMIT) out[key.nv] = a.b.idx[k];
+    ++key.nv;
+  }
+  return true;
+}
+
+template <int MAXL>
+__device__ __forceinline__ uint32_t load_req(const PreemptArgs& a, const PreemptPod& q, int64_t* req) {
+#pragma unroll
+  for (int d = 0; d < MAXL; ++d) req[d] = d < (int)a.t.L ? a.preq[(size_t)d * a.P + q.pod] : 0;
+  return a.preq_present[q.pod];
+}
+
+// preempt_node_kernel — the hot path: block (tile, preemptor) evaluates PREEMPT_THREADS nodes for one preemptor and
+// writes the tile's best key (and its candidate count).  The key is a total order (the node index decides last),
+// so the tree below gives the same winner as a walk in node order.
+template <int MAXL>
+__global__ void __launch_bounds__(PREEMPT_THREADS) preempt_node_kernel(PreemptArgs a) {
+  const uint32_t i = a.p0 + blockIdx.y;
+  const uint32_t n = blockIdx.x * PREEMPT_THREADS + threadIdx.x;
+  const PreemptPod q = a.pp[i];
+  int64_t req[MAXL];
+  const uint32_t rpres = load_req<MAXL>(a, q, req);
+  PickKey key = pick_none();
+  if (n < a.t.N && !select_victims<MAXL, false>(a, q, req, rpres, n, key, nullptr)) key = pick_none();
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    PickKey k2;
+    k2.sum = __shfl_down_sync(0xffffffffu, key.sum, o);
+    k2.start = __shfl_down_sync(0xffffffffu, key.start, o);
+    k2.hp = __shfl_down_sync(0xffffffffu, key.hp, o);
+    k2.nv = __shfl_down_sync(0xffffffffu, key.nv, o);
+    k2.node = __shfl_down_sync(0xffffffffu, key.node, o);
+    k2.cand = __shfl_down_sync(0xffffffffu, key.cand, o);
+    key = pick_min(key, k2);
+  }
+  __shared__ PickKey s_key[PREEMPT_THREADS / 32];
+  if ((threadIdx.x & 31) == 0) s_key[threadIdx.x >> 5] = key;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    PickKey r = s_key[0];
+    for (int w = 1; w < PREEMPT_THREADS / 32; ++w) r = pick_min(r, s_key[w]);
+    a.tiles[(size_t)blockIdx.y * a.n_tiles + blockIdx.x] = r;
+  }
+}
+
+// preempt_reduce_kernel — one thread per preemptor of the launch: the tiles in node order
+__global__ void preempt_reduce_kernel(PreemptArgs a, uint32_t count) {
+  const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= count) return;
+  PickKey r = pick_none();
+  for (uint32_t tl = 0; tl < a.n_tiles; ++tl) r = pick_min(r, a.tiles[(size_t)j * a.n_tiles + tl]);
+  const uint32_t i = a.p0 + j;
+  a.out_node[i] = r.node;
+  a.out_nv[i] = r.node >= 0 ? r.nv : 0u;
+  a.out_cand[i] = r.cand;
+}
+
+// preempt_emit_kernel — one thread per preemptor with a node: the reprieve again on that node, writing the victims
+template <int MAXL>
+__global__ void preempt_emit_kernel(PreemptArgs a) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= a.n) return;
+  const int32_t n = a.out_node[i];
+  if (n < 0 || a.out_nv[i] == 0) return;
+  const PreemptPod q = a.pp[i];
+  int64_t req[MAXL];
+  const uint32_t rpres = load_req<MAXL>(a, q, req);
+  PickKey key;
+  select_victims<MAXL, true>(a, q, req, rpres, (uint32_t)n, key, a.victims + a.offset[i]);
+}
+
+}  // namespace bsk

@@ -7,7 +7,21 @@ from dataclasses import dataclass
 import numpy as np
 
 from . import capi
-from .snapshot import NodeTable, PodTable, GroupTable, Snapshot
+from .snapshot import BoundPodTable, NodeTable, PodTable, GroupTable, Snapshot
+
+
+@dataclass
+class PreemptResult:
+    """bs_preempt's outputs: per preemptor the chosen node (-1 none), its victims (bound-table indices, reprieve order)
+    at victims[victim_offset[i]:victim_offset[i + 1]], and the number of candidate nodes."""
+    node: np.ndarray           # int32 [n]
+    n_victims: np.ndarray      # uint32 [n]
+    n_candidates: np.ndarray   # uint32 [n]
+    victim_offset: np.ndarray  # uint32 [n + 1]
+    victims: np.ndarray        # uint32 [victims_total]
+
+    def victims_of(self, i):
+        return self.victims[self.victim_offset[i]:self.victim_offset[i + 1]].tolist()
 
 
 @dataclass
@@ -31,6 +45,7 @@ _TABLE_C = {
                                   "taint_mask", "flags")),
     GroupTable: (capi.GroupTableC, ("min_member", "scheduled", "matched", "flags", "min_res", "min_res_present",
                                     "rep_sel", "rep_tol", "creation_ns", "name_rank", "rep_aff")),
+    BoundPodTable: (capi.BoundTableC, ("node", "req", "req_present", "gid", "priority", "start_ns", "flags")),
     PodTable: (capi.PodTableC, ("req", "req_present", "gid", "sel_mask", "tol_mask", "priority", "ts_ns", "flags",
                                 "aff_class")),
 }
@@ -292,6 +307,35 @@ class Engine:
         self._check(self.lib.bs_replay(self.h, None if q is None else capi.ptr(q), n, C.byref(r)))
         return out
 
+    # -- preemption ---------------------------------------------------------------------------
+    def upload_bound_pods(self, bt: BoundPodTable):
+        """The pods bound to the uploaded nodes (upload nodes and groups first; either upload drops this table)."""
+        self._check(self.lib.bs_upload_bound_pods(self.h, C.byref(_table_c(bt))))
+
+    def preempt(self, pods, victims_cap=None) -> PreemptResult:
+        """For every pod index in `pods`: the node preemption would pick and the pods it would evict there.
+        victims_cap: capacity of the victim list (None: as large as the answer needs, found with a first call)."""
+        idx = np.ascontiguousarray(pods, dtype=np.uint32)
+        n = len(idx)
+        node, nv, cand = np.zeros(n, np.int32), np.zeros(n, np.uint32), np.zeros(n, np.uint32)
+        off = np.zeros(n + 1, np.uint32)
+        cap = 0 if victims_cap is None else victims_cap
+        while True:
+            vict = np.zeros(max(cap, 1), np.uint32)
+            r = capi.PreemptResultC(capi.ptr(node), capi.ptr(nv), capi.ptr(cand), capi.ptr(off), capi.ptr(vict), cap, 0)
+            rc = self.lib.bs_preempt(self.h, capi.ptr(idx) if n else None, n, C.byref(r))
+            if rc == capi.BS_E_INVAL and victims_cap is None and r.victims_total > cap:
+                cap = r.victims_total
+                continue
+            self._check(rc)
+            return PreemptResult(node, nv, cand, off, vict[:r.victims_total].copy())
+
+    def remove_pod(self, pod: int, bound: int):
+        """batchSchedulingPluginExtension.RemovePod for pod `pod` and bound pod `bound`: (code, reason, group)."""
+        st = capi.StatusC()
+        self._check(self.lib.bs_remove_pod(self.h, pod, bound, C.byref(st)))
+        return st.code, st.reason, st.group
+
     # -- per-call mirrors ------------------------------------------------------------------
     def prefilter(self, pod: int):
         st = capi.StatusC()
@@ -417,6 +461,19 @@ class Engine:
 
     def launch_count(self) -> int:
         return int(self.lib.bs_launch_count(self.h))
+
+
+def format_remove_message(reason: int, pod_name: str = "", victim_name: str = "", victim_ns_name: str = "",
+                          buf_len: int = 512) -> str:
+    """The reference's RemovePod error text for a bs_remove_code ("" for REMOVE_ALLOW); needs no engine and no device."""
+    lib = capi.load()
+    st = capi.StatusC(0, reason, -1)
+    buf = C.create_string_buffer(buf_len)
+    rc = lib.bs_format_remove_message(C.byref(st), pod_name.encode(), victim_name.encode(), victim_ns_name.encode(),
+                                      buf, buf_len)
+    if rc != 0:
+        raise capi.BsError(rc, lib.bs_strerror(rc).decode())
+    return buf.value.decode()
 
 
 def format_fit_error(counts, n_lanes: int, n_nodes: int, scalar_names=None, buf_len: int = 4096) -> str:

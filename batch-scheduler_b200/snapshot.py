@@ -172,6 +172,48 @@ class GroupTable:
         return GroupTable(*(None if getattr(self, f) is None else getattr(self, f).copy() for f in self.__dataclass_fields__))
 
 
+BOUND_GROUP_LOCKED = 0x01   # the bound pod's PodGroup Status.Phase is Scheduled or Running
+
+
+@dataclass
+class BoundPodTable:
+    """The pods already bound to the snapshot's nodes (NodeInfo.Pods()): what preemption may evict."""
+    node: np.ndarray         # uint32 [V] node index
+    req: np.ndarray          # int64 [L, V] the containers' Requests (lane 3 ignored)
+    req_present: np.ndarray  # uint32 [V] scalar keys, a subset of the node's req_present
+    gid: np.ndarray          # int32 [V] group index, GID_NONE (no group label) or GID_MISSING
+    priority: np.ndarray     # int32 [V]
+    start_ns: np.ndarray     # int64 [V] Status.StartTime
+    flags: np.ndarray        # uint8 [V] BOUND_*
+
+    def __post_init__(self):
+        self.node = _c(self.node, np.uint32)
+        self.req = _c(self.req, np.int64)
+        self.req_present = _c(self.req_present, np.uint32)
+        self.gid = _c(self.gid, np.int32)
+        self.priority = _c(self.priority, np.int32)
+        self.start_ns = _c(self.start_ns, np.int64)
+        self.flags = _c(self.flags, np.uint8)
+        assert self.req.ndim == 2 and self.req.shape[1] == len(self.node)
+
+    @property
+    def n(self):
+        return self.req.shape[1]
+
+    @property
+    def lanes(self):
+        return self.req.shape[0]
+
+    @staticmethod
+    def empty(n, lanes):
+        z = lambda dt: np.zeros(n, dt)
+        return BoundPodTable(z(np.uint32), np.zeros((lanes, n), np.int64), z(np.uint32), z(np.int32), z(np.int32),
+                             z(np.int64), z(np.uint8))
+
+    def copy(self):
+        return BoundPodTable(*(getattr(self, f).copy() for f in self.__dataclass_fields__))
+
+
 @dataclass
 class Snapshot:
     nodes: NodeTable
@@ -248,6 +290,49 @@ class Snapshot:
                      dict(self.meta), self.aff_bits)
         s.meta.update(group_range=(g0, g1), pod_index=idx)
         return s
+
+
+def bound_pods(snap: Snapshot, seed: int, fill: float = 1.0, max_per_node: int = None,
+               priorities=(-10, 0, 0, 5, 100, 1000), n_starts: int = 8, online: float = 0.3, missing: float = 0.03,
+               locked: float = 0.2) -> BoundPodTable:
+    """A bound-pod table consistent with the node table: node n gets round(fill * pod_count[n]) pods (at most
+    max_per_node) whose lanes 0-2 split the node's requested amounts (the last pod takes the remainder) and whose scalar
+    keys are a random subset of the node's req_present.  Priorities are drawn from `priorities`, start times from
+    n_starts values (ties on purpose); a pod is online (no group label) with probability `online`, in a missing group
+    with `missing`, else in a random group of the snapshot, locked (Scheduled / Running) with `locked`."""
+    rng = np.random.default_rng(seed)
+    nt, G, L = snap.nodes, snap.groups.n, snap.nodes.lanes
+    k = np.round(np.clip(nt.pod_count.astype(np.int64), 0, None) * fill).astype(np.int64)
+    if max_per_node is not None:
+        k = np.minimum(k, max_per_node)
+    node = np.repeat(np.arange(nt.n, dtype=np.int64), k)
+    V = len(node)
+    bt = BoundPodTable.empty(V, L)
+    bt.node = node.astype(np.uint32)
+    if V:
+        last = np.cumsum(k)[k > 0] - 1   # the last row of each non-empty node
+        w = rng.random(V) + 0.1
+        wsum = np.bincount(node, weights=w, minlength=nt.n)
+        for d in range(3):
+            total = nt.requested[d][node]
+            part = np.floor(total.astype(np.float64) * (w / wsum[node])).astype(np.int64)
+            part[last] = 0
+            part[last] = nt.requested[d][node[last]] - np.bincount(node, weights=part, minlength=nt.n)[node[last]].astype(np.int64)
+            bt.req[d] = part
+        pres = np.zeros(V, np.uint32)
+        for d in range(4, L):
+            has = ((nt.req_present[node] >> np.uint32(d)) & 1).astype(bool) & (rng.random(V) < 0.6)
+            pres |= has.astype(np.uint32) << np.uint32(d)
+            bt.req[d] = np.where(has, rng.integers(0, 4, V), 0)
+        bt.req_present = pres
+        bt.priority = rng.choice(np.asarray(priorities, np.int64), V).astype(np.int32)
+        bt.start_ns = (1_600_000_000 * 10**9 + rng.integers(0, n_starts, V) * 10**9).astype(np.int64)
+        u = rng.random(V)
+        gid = rng.integers(0, G, V) if G else np.full(V, GID_NONE)
+        gid = np.where(u < online, GID_NONE, np.where(u < online + missing, GID_MISSING, gid))
+        bt.gid = gid.astype(np.int32)
+        bt.flags = np.where((gid >= 0) & (rng.random(V) < locked), BOUND_GROUP_LOCKED, 0).astype(np.uint8)
+    return bt
 
 
 # ----------------------------------------------------------------------------

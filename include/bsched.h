@@ -430,6 +430,61 @@ int bs_fetch_reason_rows(bs_engine* e, uint32_t pod0, uint32_t n, uint32_t* coun
 int bs_format_fit_error(const uint32_t* counts, uint32_t n_lanes, uint32_t n_nodes, const char* const* scalar_names,
                         char* buf, size_t buf_len);
 
+/* ---- preemption: PreFilterExtensions.RemovePod and the node / victims kube-scheduler's preemption would pick ----
+ * The bound-pod table lists the pods already running on the snapshot's nodes (NodeInfo.Pods()).  Rows may come in
+ * any order; the engine groups them by node in MoreImportantPod order (priority descending, start time ascending,
+ * then table index ascending).  Validation: node >= n_nodes or gid < BS_GID_MISSING is BS_E_INDEX; more rows on a node than its pod_count,
+ * or scalar keys that are not a subset of the node's req_present, BS_E_INVAL; a value or any per-node suffix sum of
+ * a lane beyond +-BS_VALUE_LIMIT, BS_E_RANGE.  A failing table is dropped.  The table belongs to the node snapshot:
+ * bs_upload_nodes, bs_update_nodes and bs_upload_groups drop it (BS_E_STATE until it is uploaded again). */
+#define BS_BOUND_GROUP_LOCKED 0x01u /* the pod's PodGroup Status.Phase is Scheduled or Running (core.go:235-236) */
+typedef struct {
+  uint32_t n_pods, n_lanes;
+  const uint32_t* node;        /* [V] snapshot index of the node it is bound to (NodeInfo.Pods())              */
+  const int64_t* req;          /* [n_lanes][V] what NodeInfo.RemovePod subtracts: the containers' Requests (not
+                                  Limits: calculateResource, [upstream, from memory]); lane 3 ignored             */
+  const uint32_t* req_present; /* [V] scalar keys; must be a subset of its node's req_present                     */
+  const int32_t* gid;          /* [V] group index, BS_GID_NONE (online) or BS_GID_MISSING                          */
+  const int32_t* priority;     /* [V] GetPodPriority */
+  const int64_t* start_ns;     /* [V] Status.StartTime */
+  const uint8_t* flags;        /* [V] BS_BOUND_* */
+} bs_bound_table;
+int bs_upload_bound_pods(bs_engine* e, const bs_bound_table* t);
+
+/* Result of bs_preempt.  Per preemptor: the node genericScheduler.Preempt -> pickOneNodeForPreemption would pick
+ * (-1 none) and, in victims[victim_offset[i] .. victim_offset[i + 1]), the bound-table indices of the pods
+ * selectVictimsOnNode would evict there, in reprieve order (most important first). */
+typedef struct {
+  int32_t* node;            /* [n] chosen node, -1 none                                              */
+  uint32_t* n_victims;      /* [n]                                                                   */
+  uint32_t* n_candidates;   /* [n] nodes where removing every lower-priority pod lets the pod fit    */
+  uint32_t* victim_offset;  /* [n + 1] exclusive scan of n_victims                                   */
+  uint32_t* victims;        /* [victims_cap] bound-table indices, per preemptor in reprieve order      */
+  uint32_t victims_cap;
+  uint32_t victims_total;   /* out, always written; > victims_cap -> BS_E_INVAL, victims untouched   */
+} bs_preempt_result;
+/* Every pods[i] (an index of the uploaded pod table) is an independent what-if against the uploaded node and bound
+ * tables (DESIGN.md §2 "Preemption").  Needs nodes, groups, pods and the bound table; does not depend on, and does not
+ * change, any round's state or outputs. */
+int bs_preempt(bs_engine* e, const uint32_t* pods, uint32_t n, bs_preempt_result* out);
+
+/* RemovePod verdicts (core.PreemptRemovePod, core.go:203-260) */
+typedef enum {
+  BS_REMOVE_ALLOW = 0,
+  BS_REMOVE_OFFLINE_ONLINE = 1, /* "offline pods %v are forbidden to preempt online %v"                     :217 */
+  BS_REMOVE_NOT_FOUND = 2,      /* "can not found pod group: %v"                                            :224 */
+  BS_REMOVE_LOCKED = 3,         /* "pod belongs to Scheduled or Running pod group can not be scheduled"     :237 */
+  BS_REMOVE_SAME_GROUP = 4      /* "podToSchedule and podToRemove belong to same pod group, do not preempt" :252 */
+} bs_remove_code;
+/* batchSchedulingPluginExtension.RemovePod (batchscheduler.go:132-144) -> core.PreemptRemovePod (core.go:203-260) for
+ * pod `pod` of the pod table and row `bound` of the bound table.  st->reason is a bs_remove_code, st->code Success or
+ * Unschedulable, st->group the victim's group or -1.  PreemptAddPod always succeeds (core.go:194-196). */
+int bs_remove_pod(bs_engine* e, uint32_t pod, uint32_t bound, bs_status* st);
+/* The reference's error text of a RemovePod status ("" for BS_REMOVE_ALLOW); victim_ns_name is "namespace/pgName" of
+ * the victim's group.  A buffer too small for the whole message is BS_E_INVAL. */
+int bs_format_remove_message(const bs_status* st, const char* pod_name, const char* victim_name,
+                             const char* victim_ns_name, char* buf, size_t buf_len);
+
 /* ---- multi-GPU exchange of the admit bitmap over peer memory (NVLink / NVSwitch) ----
  * The path shards over groups (one process per GPU); the only exchange is the all-gather of the
  * per-rank admit bitmaps.  Instead of a separate NCCL launch, bs_evaluate_async ends with a push

@@ -201,6 +201,73 @@ func (e *Engine) PreFilter(pod uint32, nsName, occupiedBy string) error {
 	return fmt.Errorf("%s", C.GoString(buf)) // the adapter turns it into framework.Unschedulable (batchscheduler.go:104-107)
 }
 
+// UploadBoundPods uploads the pods bound to the snapshot's nodes (NodeInfo.Pods()): what preemption may evict.
+// Upload nodes and groups first; either upload, and UpdateNodes, drop the table.
+func (e *Engine) UploadBoundPods(t *C.bs_bound_table) error { return e.rc(C.bs_upload_bound_pods(e.h, t)) }
+
+// RemovePod mirrors batchSchedulingPluginExtension.RemovePod (batchscheduler.go:132-144) ->
+// core.PreemptRemovePod (core.go:203-260) for pod row `pod` and bound-pod row `bound`: nil == the victim may go.
+// victimGroup is "namespace/pgName" of the victim's group (the not-found message names it).
+func (e *Engine) RemovePod(pod, bound uint32, podName, victimName, victimGroup string) error {
+	var st C.bs_status
+	if err := e.rc(C.bs_remove_pod(e.h, C.uint32_t(pod), C.uint32_t(bound), &st)); err != nil {
+		return err
+	}
+	if st.reason == C.BS_REMOVE_ALLOW {
+		return nil
+	}
+	buf := (*C.char)(C.malloc(1024))
+	defer C.free(unsafe.Pointer(buf))
+	cp, cv, cg := C.CString(podName), C.CString(victimName), C.CString(victimGroup)
+	defer C.free(unsafe.Pointer(cp))
+	defer C.free(unsafe.Pointer(cv))
+	defer C.free(unsafe.Pointer(cg))
+	if err := e.rc(C.bs_format_remove_message(&st, cp, cv, cg, buf, 1024)); err != nil {
+		return err
+	}
+	return fmt.Errorf("%s", C.GoString(buf)) // the adapter turns it into framework.Unschedulable (batchscheduler.go:137-141)
+}
+
+// Preemption is one preemptor's answer: the snapshot index of the node preemption would pick (-1 none) and the
+// bound-pod rows it would evict there, most important first.
+type Preemption struct {
+	Node       int32
+	Victims    []uint32
+	Candidates uint32
+}
+
+// Preempt mirrors genericScheduler.Preempt's node and victim choice for every pod row in pods, against the uploaded
+// snapshot and bound-pod table (bs_preempt; DESIGN.md §2 "Preemption").
+func (e *Engine) Preempt(pods []uint32) ([]Preemption, error) {
+	n := len(pods)
+	out := make([]Preemption, n)
+	if n == 0 {
+		return out, nil
+	}
+	node := make([]int32, n)
+	nv := make([]uint32, n)
+	cand := make([]uint32, n)
+	off := make([]uint32, n+1)
+	r := C.bs_preempt_result{node: (*C.int32_t)(unsafe.Pointer(&node[0])), n_victims: (*C.uint32_t)(unsafe.Pointer(&nv[0])),
+		n_candidates: (*C.uint32_t)(unsafe.Pointer(&cand[0])), victim_offset: (*C.uint32_t)(unsafe.Pointer(&off[0]))}
+	p := (*C.uint32_t)(unsafe.Pointer(&pods[0]))
+	rc := C.bs_preempt(e.h, p, C.uint32_t(n), &r)
+	var victims []uint32
+	if rc == C.BS_E_INVAL && r.victims_total > 0 { // the first call sized the victim list
+		victims = make([]uint32, int(r.victims_total))
+		r.victims = (*C.uint32_t)(unsafe.Pointer(&victims[0]))
+		r.victims_cap = r.victims_total
+		rc = C.bs_preempt(e.h, p, C.uint32_t(n), &r)
+	}
+	if err := e.rc(rc); err != nil {
+		return nil, err
+	}
+	for i := 0; i < n; i++ {
+		out[i] = Preemption{Node: node[i], Victims: append([]uint32(nil), victims[off[i]:off[i+1]]...), Candidates: cand[i]}
+	}
+	return out, nil
+}
+
 // Permit mirrors batchSchedulingPlugin.Permit (batchscheduler.go:165-202) with core.Permit's bookkeeping
 // (core.go:268-309) against the engine's tables: ready only once len(MatchedPodNodes.Items()) reaches
 // MinMember - Status.Scheduled.
