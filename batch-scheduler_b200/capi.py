@@ -17,10 +17,11 @@ AFF_NONE = 0xffffffff
 BS_OK, BS_E_INVAL, BS_E_NODEVICE, BS_E_CUDA, BS_E_NOMEM, BS_E_RANGE, BS_E_STATE, BS_E_REF_PANIC, BS_E_INDEX, BS_E_PEER = \
     0, -1, -2, -3, -4, -5, -6, -7, -8, -9
 CODE_SUCCESS, CODE_ERROR, CODE_UNSCHEDULABLE, CODE_UNSCHEDULABLE_AND_UNRESOLVABLE, CODE_WAIT, CODE_SKIP = range(6)
-OUT_FIT_BITMAP, OUT_SCORE, OUT_FILTER, OUT_TOPK, OUT_REASONS = 0x1, 0x2, 0x4, 0x8, 0x10
+OUT_FIT_BITMAP, OUT_SCORE, OUT_FILTER, OUT_TOPK, OUT_REASONS, OUT_PRIORITY = 0x1, 0x2, 0x4, 0x8, 0x10, 0x20
 # bins of a reason row (BS_OUT_REASONS): [unschedulable, unavailable, selector, taints, lane 0, lane 1, ...]
 REASON_UNSCHEDULABLE, REASON_UNAVAILABLE, REASON_SELECTOR, REASON_TAINTS, REASON_LANE0 = range(5)
 TOPK_MAX = 32   # BS_TOPK_MAX: longest top-K list
+NONZERO_MAX = 1 << 56   # BS_NONZERO_MAX: largest non-zero request a priority column may hold
 # core.PreemptRemovePod verdicts (bs_remove_code) and the bound-pod flag
 REMOVE_ALLOW, REMOVE_OFFLINE_ONLINE, REMOVE_NOT_FOUND, REMOVE_LOCKED, REMOVE_SAME_GROUP = range(5)
 BOUND_GROUP_LOCKED = 0x01
@@ -150,6 +151,10 @@ SYMBOLS = {
     "bs_fetch_topk_rows": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p]),
     "bs_fetch_reason_rows": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]),
     "bs_format_fit_error": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_char_p, C.c_size_t]),
+    "bs_set_score_weights": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32]),
+    "bs_upload_node_nonzero": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p]),
+    "bs_upload_pod_nonzero": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p]),
+    "bs_fetch_priority_rows": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p]),
     "bs_peer_init": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32]),
     "bs_peer_handle": (C.c_int, [C.c_void_p, C.c_void_p]),
     "bs_peer_attach": (C.c_int, [C.c_void_p, C.c_void_p]),

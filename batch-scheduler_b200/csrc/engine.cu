@@ -28,6 +28,7 @@
 #include "sort.cuh"
 #include "replay.cuh"
 #include "preempt.cuh"
+#include "priority.cuh"
 
 using namespace bsk;
 
@@ -397,6 +398,11 @@ struct bs_engine {
   // BS_OUT_REASONS: full-width residuals [L][Npad], per fit class the gate bitmap [classes][Npad/32] and bins 0-3
   // [classes][4] (rebuilt with the class fit bits), and the rows [P][4 + L]
   DevBuf d_left_full, d_reason_gate, d_reason_class, d_reasons;
+  // BS_OUT_PRIORITY: the non-zero request columns (node [2][Npad] zero-padded, pod [2][P]; each dropped with its
+  // table), the score weights, and the lists [P][topk]; the fit set is the reason rows' (d_left_full, d_reason_gate)
+  DevBuf d_nz_node, d_nz_pod, d_prio_node, d_prio_score;
+  bool have_nz_node = false, have_nz_pod = false;
+  ScoreWeights weights{1, 0, 1};
   // sort scratch: views into one arena
   View d_gk0, d_gk1, d_pk0, d_pk1, d_idx_a, d_idx_b, d_ghist, d_group_rank, d_tilecnt, d_sort_barrier;
   uint32_t sort_max_grid = 1;
@@ -973,6 +979,10 @@ int ensure_round_buffers(bs_engine* e) {
     CK(e->d_filter_bitmap.ensure(Prows * std::max(e->W, 1u) * 4));
   }
   if (e->out_flags & BS_OUT_REASONS) CK(e->d_reasons.ensure((size_t)P * (4 + L) * 4));
+  if (e->out_flags & BS_OUT_PRIORITY) {
+    CK(e->d_prio_node.ensure((size_t)P * e->topk * 4));
+    CK(e->d_prio_score.ensure((size_t)P * e->topk * 8));
+  }
   // prefix scratch: as many rep-class slots as fit a 1 GiB budget
   const size_t per_class = (size_t)N * (8 * L + 4);
   // BS_PREFIX_BUDGET_BYTES (default 1 GiB) bounds the scratch; classes beyond it are processed in chunks
@@ -1014,7 +1024,8 @@ int prepare_nodes(bs_engine* e) {
   CK(e->d_left_n.ensure((size_t)std::max(e->lane_map.LN + e->lane_map.LS, 1u) * e->Npad * 4));
   CK(e->d_left_present.ensure((size_t)e->Npad * 4));
   if (e->out_flags & BS_OUT_FILTER) CK(e->d_left_plain.ensure((size_t)4 * e->Npad * 8));
-  const bool reasons = (e->out_flags & BS_OUT_REASONS) != 0;
+  // the reason rows' residuals and gate bitmap: also the fit set of the priority lists
+  const bool reasons = (e->out_flags & (BS_OUT_REASONS | BS_OUT_PRIORITY)) != 0;
   if (reasons) CK(e->d_left_full.ensure((size_t)e->L * e->Npad * 8));
   const uint32_t n_tiles = e->Npad / NODE_TILE;
   CK(e->d_classfit.ensure((size_t)e->n_fit_classes * n_tiles * 32 * sizeof(ColBits)));
@@ -1056,6 +1067,8 @@ int prepare_nodes(bs_engine* e) {
 int evaluate_async_locked(bs_engine* e) {
   if (!e->have_nodes || !e->have_pods || !e->have_groups)
     return fail(e, BS_E_STATE, "bs_evaluate: upload nodes, groups and pods first");
+  if ((e->out_flags & BS_OUT_PRIORITY) && !(e->have_nz_node && e->have_nz_pod))
+    return fail(e, BS_E_STATE, "bs_evaluate: BS_OUT_PRIORITY needs the node and pod non-zero columns");
   if (e->peer_broken)
     return fail(e, BS_E_PEER, "peer exchange is broken (a rank did not arrive): bs_peer_detach on every rank, then init/attach again");
   BS_DEVICE_GUARD(e);
@@ -1292,6 +1305,27 @@ int evaluate_async_locked(bs_engine* e) {
       tm.launched();
     }
   }
+  if (P && (e->out_flags & BS_OUT_PRIORITY)) {
+    PriorityArgs pa;
+    pa.left = e->d_left_full.as<int64_t>();
+    pa.left_present = e->d_left_present.as<uint32_t>();
+    pa.gate = e->d_reason_gate.as<uint32_t>();
+    pa.req = e->d_req.as<int64_t>();
+    pa.req_present = e->d_ppres.as<uint32_t>();
+    pa.fit_class = e->d_pod_fit_class.as<uint32_t>();
+    pa.alloc = e->d_alloc.as<int64_t>();
+    pa.node_nz = e->d_nz_node.as<int64_t>();
+    pa.pod_nz = e->d_nz_pod.as<int64_t>();
+    pa.out_node = e->d_prio_node.as<int32_t>();
+    pa.out_score = e->d_prio_score.as<int64_t>();
+    pa.w = e->weights;
+    pa.P = P; pa.N = e->N; pa.Npad = e->Npad; pa.Wg = e->Npad / 32; pa.L = L; pa.K = e->topk;
+    const uint32_t grid = cdiv(P, PRIO_PODS_PER_CTA);
+    if (L <= 5) priority_pod_kernel<5><<<grid, PRIO_THREADS, 0, e->s>>>(pa);
+    else if (L <= 9) priority_pod_kernel<9><<<grid, PRIO_THREADS, 0, e->s>>>(pa);
+    else priority_pod_kernel<16><<<grid, PRIO_THREADS, 0, e->s>>>(pa);
+    e->launches += 1;
+  }
   if (e->peer_attached) {
     // admit-bitmap all-gather over peer memory (kernels.cuh K8): the push is the round's last kernel on
     // the main stream, ordered behind the PREVIOUS round's wait (slot reuse rule); the wait for this
@@ -1442,8 +1476,10 @@ int bs_create(const bs_config* cfg, bs_engine** out) {
   *out = nullptr;
   if (cfg->n_lanes < BS_FIXED_LANES || cfg->n_lanes > BS_MAX_LANES) return BS_E_INVAL;
   // top-K lists: 1..BS_TOPK_MAX entries with the flag, none without; the score matrix already holds them
-  if ((cfg->out_flags & BS_OUT_TOPK) ? (cfg->topk < 1 || cfg->topk > BS_TOPK_MAX || (cfg->out_flags & BS_OUT_SCORE))
-                                     : cfg->topk != 0)
+  // (the priority lists share K; they combine with every flag)
+  if ((cfg->out_flags & (BS_OUT_TOPK | BS_OUT_PRIORITY))
+          ? (cfg->topk < 1 || cfg->topk > BS_TOPK_MAX || ((cfg->out_flags & BS_OUT_TOPK) && (cfg->out_flags & BS_OUT_SCORE)))
+          : cfg->topk != 0)
     return BS_E_INVAL;
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) {
@@ -1507,6 +1543,7 @@ void bs_destroy(bs_engine* e) {
 int bs_upload_nodes(bs_engine* e, const bs_node_table* t) {
   if (!e || !t) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
+  e->have_nz_node = false;   // the non-zero column belongs to the node snapshot
   if (t->n_lanes != e->L) return fail(e, BS_E_INVAL, "bs_upload_nodes: n_lanes differs from the engine's");
   const uint32_t N = t->n_nodes, L = e->L;
   const auto cols = node_cols(e, t);
@@ -1544,6 +1581,7 @@ int bs_update_nodes(bs_engine* e, const uint32_t* idx, const bs_node_table* t) {
   if (!e || !t || (t->n_nodes && !idx)) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
   if (!e->have_nodes) return fail(e, BS_E_STATE, "bs_update_nodes: upload nodes first");
+  e->have_nz_node = false;   // the changed rows' non-zero requests come with a new column
   if (t->n_lanes != e->L) return fail(e, BS_E_INVAL, "bs_update_nodes: n_lanes differs from the engine's");
   const uint32_t n = t->n_nodes, L = e->L;
   if (!n) return BS_OK;
@@ -1674,6 +1712,7 @@ int bs_update_groups(bs_engine* e, const uint32_t* idx, const bs_group_table* t)
 int bs_upload_pods(bs_engine* e, const bs_pod_table* t) {
   if (!e || !t) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
+  e->have_nz_pod = false;   // the non-zero column belongs to the pod table
   if (t->n_lanes != e->L) return fail(e, BS_E_INVAL, "bs_upload_pods: n_lanes differs from the engine's");
   const uint32_t P = t->n_pods, L = e->L;
   if (P && (!t->req || !t->req_present || !t->gid || !t->sel_mask || !t->tol_mask || !t->priority ||
@@ -2754,6 +2793,68 @@ int bs_fetch_reason_rows(bs_engine* e, uint32_t pod0, uint32_t n, uint32_t* coun
   const size_t R = 4 + e->L;
   if (n) CK(cudaMemcpyAsync(counts, e->d_reasons.as<uint32_t>() + (size_t)pod0 * R, (size_t)n * R * 4,
                             cudaMemcpyDeviceToHost, e->s));
+  CK(cudaStreamSynchronize(e->s));
+  return BS_OK;
+}
+
+// ---- resource priorities (BS_OUT_PRIORITY, priority.cuh) ----
+int bs_set_score_weights(bs_engine* e, uint32_t least, uint32_t most, uint32_t balanced) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  e->weights = ScoreWeights{least, most, balanced};
+  return BS_OK;
+}
+
+namespace {
+// One non-zero column [2][n] into dst ([2][pitch], zero beyond n).  The caller has dropped the column already; it is
+// marked present only when every value lies in [0, BS_NONZERO_MAX].
+int upload_nonzero(bs_engine* e, DevBuf& dst, uint32_t n, uint32_t pitch, const int64_t* nz, const char* who) {
+  if (n && !nz) return fail(e, BS_E_INVAL, who);
+  for (size_t k = 0; k < (size_t)2 * n; ++k)
+    if (nz[k] < 0 || nz[k] > BS_NONZERO_MAX) return fail(e, BS_E_RANGE, "non-zero request outside [0, 2^56]");
+  BS_DEVICE_GUARD(e);
+  CK(dst.ensure((size_t)2 * std::max(pitch, 1u) * 8));
+  if (pitch > n) CK(cudaMemsetAsync(dst.p, 0, (size_t)2 * pitch * 8, e->s));
+  if (n)
+    CK(cudaMemcpy2DAsync(dst.p, (size_t)pitch * 8, nz, (size_t)n * 8, (size_t)n * 8, 2, cudaMemcpyHostToDevice, e->s));
+  CK(cudaStreamSynchronize(e->s));
+  return BS_OK;
+}
+}  // namespace
+
+int bs_upload_node_nonzero(bs_engine* e, uint32_t n_nodes, const int64_t* nz) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  e->have_nz_node = false;
+  if (!e->have_nodes) return fail(e, BS_E_STATE, "bs_upload_node_nonzero: upload nodes first");
+  if (n_nodes != e->N) return fail(e, BS_E_INVAL, "bs_upload_node_nonzero: n_nodes differs from the node table's");
+  const int rc = upload_nonzero(e, e->d_nz_node, n_nodes, e->Npad, nz, "bs_upload_node_nonzero: null column");
+  e->have_nz_node = rc == BS_OK;
+  return rc;
+}
+
+int bs_upload_pod_nonzero(bs_engine* e, uint32_t n_pods, const int64_t* nz) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  e->have_nz_pod = false;
+  if (!e->have_pods) return fail(e, BS_E_STATE, "bs_upload_pod_nonzero: upload pods first");
+  if (n_pods != e->P) return fail(e, BS_E_INVAL, "bs_upload_pod_nonzero: n_pods differs from the pod table's");
+  const int rc = upload_nonzero(e, e->d_nz_pod, n_pods, n_pods, nz, "bs_upload_pod_nonzero: null column");
+  e->have_nz_pod = rc == BS_OK;
+  return rc;
+}
+
+int bs_fetch_priority_rows(bs_engine* e, uint32_t pod0, uint32_t n, int32_t* nodes, int64_t* scores) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!e->evaluated || !(e->out_flags & BS_OUT_PRIORITY)) return fail(e, BS_E_STATE, "no priority lists materialised");
+  if ((uint64_t)pod0 + n > e->P) return BS_E_INDEX;
+  BS_DEVICE_GUARD(e);
+  const size_t off = (size_t)pod0 * e->topk, cnt = (size_t)n * e->topk;   // device rows are dense [P][K]
+  if (cnt && nodes)
+    CK(cudaMemcpyAsync(nodes, e->d_prio_node.as<int32_t>() + off, cnt * 4, cudaMemcpyDeviceToHost, e->s));
+  if (cnt && scores)
+    CK(cudaMemcpyAsync(scores, e->d_prio_score.as<int64_t>() + off, cnt * 8, cudaMemcpyDeviceToHost, e->s));
   CK(cudaStreamSynchronize(e->s));
   return BS_OK;
 }

@@ -112,6 +112,14 @@ __device__ __forceinline__ bool compare_res(const int64_t* left, uint32_t lpres,
   return ok;
 }
 
+// One lane of compareResourceAndRequire (core.go:672-699) against node_left_kernel's full-width residuals (left_full,
+// left_present | 0xF): short when the key is present and left < req (:694), or absent and req != 0 (:688-692).  The
+// caller applies it to lanes 0-3 and to the scalar lanes the pod requests.  Reason rows count the short lanes; the
+// priority lists take a node as fitting when its gate bit is set and no lane is short.
+__device__ __forceinline__ bool lane_short(bool present, int64_t left, int64_t req) {
+  return present ? left < req : req != 0;
+}
+
 // ---------------------------------------------------------------------------
 // K1  node_left_kernel — per node: residual capacity at percent 1.0 in the
 // sentinel form the fit kernel consumes (absent scalar lane -> ABSENT_LEFT / ABSENT_LEFT32),
@@ -362,7 +370,7 @@ __global__ void __launch_bounds__(REASON_THREADS) reason_pod_kernel(ReasonArgs a
 #pragma unroll
       for (int j = 0; j < REASON_PPW; ++j) {
         const int64_t r = s_req[wid][j][d];
-        const bool shrt = g[j] && ((rmask[j] >> d) & 1u) && (pres ? v < r : r != 0);
+        const bool shrt = g[j] && ((rmask[j] >> d) & 1u) && lane_short(pres, v, r);
         cnt[j][d] += shrt ? 1u : 0u;
       }
     }

@@ -761,11 +761,14 @@ Status BatchSchedulingPlugin::Pack(const std::vector<const NodeInfo*>& snapshot,
   return pack_impl(snapshot, pending, groups, extra_pod_flags, default_wait_ns, out);
 }
 
-BatchSchedulingPlugin::BatchSchedulingPlugin(int device, int64_t max_schedule_time_ns, uint32_t out_flags, uint32_t topk)
+BatchSchedulingPlugin::BatchSchedulingPlugin(int device, int64_t max_schedule_time_ns, uint32_t out_flags, uint32_t topk,
+                                             uint32_t priority_k)
     : max_schedule_time_ns_(max_schedule_time_ns) {
   device_ = device;
-  out_flags_ = out_flags | (topk ? BS_OUT_TOPK : 0u);
+  out_flags_ = out_flags | (topk ? BS_OUT_TOPK : 0u) | (priority_k ? BS_OUT_PRIORITY : 0u);
   topk_ = topk;
+  priority_k_ = priority_k;
+  if (topk && priority_k && topk != priority_k) init_error_ = "topk and priority_k share one list length: they must be equal";
 }
 
 BatchSchedulingPlugin::~BatchSchedulingPlugin() {
@@ -846,6 +849,7 @@ int BatchSchedulingPlugin::group_index(const std::string& ns_name) const {
 Status BatchSchedulingPlugin::BeginRound(const std::vector<const NodeInfo*>& snapshot,
                                          const std::vector<const Pod*>& pending, int64_t now_ns) {
   const double t0 = now_ms();
+  if (!init_error_.empty()) return Status{BS_CODE_ERROR, init_error_};
   std::lock_guard<std::mutex> lk(mu_);
   now_ns_ = now_ns;
   const bool prof = getenv("BS_PACK_PROFILE") != nullptr;
@@ -949,7 +953,7 @@ Status BatchSchedulingPlugin::BeginRound(const std::vector<const NodeInfo*>& sna
   if (!eng_ || eng_lanes_ != packed_.lanes) {
     // a new scalar resource changed the lane count: a fresh engine takes over the gang state of the old one
     bs_engine* fresh = nullptr;
-    bs_config cfg{device_, packed_.lanes, out_flags_, topk_};
+    bs_config cfg{device_, packed_.lanes, out_flags_, topk_ ? topk_ : priority_k_};
     int rc = bs_create(&cfg, &fresh);
     if (rc) return fail(rc);
     if (eng_) { bs_state_move(fresh, eng_); bs_destroy(eng_); }
@@ -964,6 +968,10 @@ Status BatchSchedulingPlugin::BeginRound(const std::vector<const NodeInfo*>& sna
   if (packed_.n_aff() && (rc = bs_upload_affinity(eng_, packed_.n_aff(), packed_.aff_bits.data()))) return fail(rc);
   if ((rc = bs_upload_groups(eng_, &gt))) return fail(rc);
   if ((rc = bs_upload_pods(eng_, &pt))) return fail(rc);
+  {
+    Status nst = UploadNonZero(&pending);
+    if (!nst.ok()) return nst;
+  }
   {
     Status bst = UploadBound();   // after the groups: the bound rows' group indices refer to this table
     if (!bst.ok()) return bst;
@@ -988,6 +996,7 @@ Status BatchSchedulingPlugin::BeginRound(const std::vector<const NodeInfo*>& sna
   if ((rc = bs_evaluate(eng_, &r))) return fail(rc);
   if ((rc = FetchTopK())) return fail(rc);
   if ((rc = FetchReasons())) return fail(rc);
+  if ((rc = FetchPriority())) return fail(rc);
   last_device_ms_ = now_ms() - t1;
 
   // side effects the reference performs while it walks the pods:
@@ -1049,6 +1058,7 @@ Status BatchSchedulingPlugin::Reevaluate() {
   if (!rc) rc = bs_evaluate(eng_, &r);
   if (!rc) rc = FetchTopK();
   if (!rc) rc = FetchReasons();
+  if (!rc) rc = FetchPriority();
   if (rc) return Status{BS_CODE_ERROR, std::string("bsched: ") + bs_strerror(rc) + " (" + bs_last_error(eng_) + ")"};
   return Status{};   // (new_denied groups were deny-listed by the engine's fetch, core.go:142,163)
 }
@@ -1078,6 +1088,94 @@ int BatchSchedulingPlugin::FetchReasons() {
   const uint32_t P = packed_.n_pods;
   reasons_.assign((size_t)P * (4 + packed_.lanes), 0);
   return bs_fetch_reason_rows(eng_, 0, P, reasons_.data());
+}
+
+int BatchSchedulingPlugin::FetchPriority() {
+  if (!priority_k_) return BS_OK;
+  const uint32_t P = packed_.n_pods;
+  prio_node_.assign((size_t)P * priority_k_, -1);
+  prio_score_.assign((size_t)P * priority_k_, INT64_MIN);
+  return bs_fetch_priority_rows(eng_, 0, P, prio_node_.data(), prio_score_.data());
+}
+
+std::vector<std::pair<std::string, int64_t>> BatchSchedulingPlugin::PriorityNodes(const std::string& uid) const {
+  std::vector<std::pair<std::string, int64_t>> out;
+  const int32_t row = pod_row_.find(uid);
+  if (row < 0 || !priority_k_ || prio_node_.size() < ((size_t)row + 1) * priority_k_) return out;
+  for (uint32_t i = 0; i < priority_k_; ++i) {
+    const int32_t n = prio_node_[(size_t)row * priority_k_ + i];
+    if (n < 0) break;   // padding: the pod fits on fewer nodes
+    out.emplace_back((size_t)n < node_names_.size() ? node_names_[n] : std::string(), prio_score_[(size_t)row * priority_k_ + i]);
+  }
+  return out;
+}
+
+void BatchSchedulingPlugin::SetScoreWeights(uint32_t least, uint32_t most, uint32_t balanced) {
+  std::lock_guard<std::mutex> lk(mu_);
+  weights_[0] = least; weights_[1] = most; weights_[2] = balanced;
+  if (eng_) bs_set_score_weights(eng_, least, most, balanced);
+}
+
+namespace {
+// GetNonzeroRequestForResource [upstream, from memory]: the Requests' cpu (MilliValue) / memory (Value), 100 m /
+// 200 MiB when the key is absent; a key listed twice counts its last entry, as a map assignment would
+constexpr int64_t kDefaultMilliCpuRequest = 100, kDefaultMemoryRequest = 200ll * 1024 * 1024;
+bool nonzero_of(const Pod& p, int64_t* cpu, int64_t* mem) {
+  *cpu = *mem = 0;
+  for (const Container& c : p.containers) {
+    const std::string *qc = nullptr, *qm = nullptr;
+    for (auto& kv : c.requests) {
+      if (kv.first == "cpu") qc = &kv.second;
+      else if (kv.first == "memory") qm = &kv.second;
+    }
+    int64_t vc = kDefaultMilliCpuRequest, vm = kDefaultMemoryRequest;
+    if (qc && !QuantityMilliValue(*qc, &vc)) return false;
+    if (qm && !QuantityValue(*qm, &vm)) return false;
+    *cpu += vc;
+    *mem += vm;
+  }
+  return true;
+}
+}  // namespace
+
+Status BatchSchedulingPlugin::PackNonZero(const std::vector<const NodeInfo*>& snapshot, const std::vector<const Pod*>& pending,
+                                          std::vector<int64_t>* node_nz, std::vector<int64_t>* pod_nz) {
+  auto bad = [](const Pod& p) { return Status{BS_CODE_ERROR, "PackNonZero: malformed request quantity in pod " + p.ns + "/" + p.name}; };
+  if (node_nz) {
+    const size_t N = snapshot.size();
+    node_nz->assign(2 * N, 0);
+    for (size_t i = 0; i < N; ++i) {
+      if (!snapshot[i]) continue;
+      for (const Pod* p : snapshot[i]->pods) {   // NodeInfo.NonZeroRequest(): the same sum over the node's pods
+        int64_t c, m;
+        if (!p) continue;
+        if (!nonzero_of(*p, &c, &m)) return bad(*p);
+        (*node_nz)[i] += c;
+        (*node_nz)[N + i] += m;
+      }
+    }
+  }
+  if (pod_nz) {
+    const size_t P = pending.size();
+    pod_nz->assign(2 * P, 0);
+    for (size_t i = 0; i < P; ++i) {
+      if (!pending[i]) continue;
+      if (!nonzero_of(*pending[i], &(*pod_nz)[i], &(*pod_nz)[P + i])) return bad(*pending[i]);
+    }
+  }
+  return Status{};
+}
+
+Status BatchSchedulingPlugin::UploadNonZero(const std::vector<const Pod*>* pending) {
+  if (!priority_k_) return Status{};
+  std::vector<int64_t> node_nz, pod_nz;
+  Status st = PackNonZero(snapshot_, pending ? *pending : std::vector<const Pod*>(), &node_nz, pending ? &pod_nz : nullptr);
+  if (!st.ok()) return st;
+  int rc = bs_upload_node_nonzero(eng_, (uint32_t)snapshot_.size(), node_nz.data());
+  if (!rc && pending) rc = bs_upload_pod_nonzero(eng_, (uint32_t)pending->size(), pod_nz.data());
+  if (!rc) rc = bs_set_score_weights(eng_, weights_[0], weights_[1], weights_[2]);
+  if (rc) return Status{BS_CODE_ERROR, std::string("bsched: ") + bs_strerror(rc) + " (" + bs_last_error(eng_) + ")"};
+  return Status{};
 }
 
 std::vector<uint32_t> BatchSchedulingPlugin::ReasonCounts(const std::string& uid) const {
@@ -1158,6 +1256,8 @@ Status BatchSchedulingPlugin::UpdateNodes(const std::vector<std::pair<uint32_t, 
     if (i < snapshot_.size()) snapshot_[i] = rows[k];
   }
   st = UploadBound();   // bs_update_nodes dropped the bound-pod table: the changed NodeInfos list their pods again
+  if (!st.ok()) return st;
+  st = UploadNonZero(nullptr);   // ... and the node non-zero column: the changed NodeInfos' pods count again
   if (!st.ok()) return st;
   // the round's decisions follow the new snapshot: same pods, same groups, same result vectors
   return evaluate ? Reevaluate() : Status{};

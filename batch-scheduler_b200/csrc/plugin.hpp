@@ -234,7 +234,10 @@ class BatchSchedulingPlugin {
  public:
   // batch.New (batchscheduler.go:377): max_schedule_time from the plugin args (Configuration, :71-75)
   // topk > 0 adds BS_OUT_TOPK: each round also keeps every pending pod's topk best fitting nodes (TopNodes)
-  BatchSchedulingPlugin(int device, int64_t max_schedule_time_ns, uint32_t out_flags = BS_OUT_FIT_BITMAP, uint32_t topk = 0);
+  // priority_k > 0 adds BS_OUT_PRIORITY: each round also keeps every pending pod's priority_k best fitting nodes under
+  // kube-scheduler's resource priorities (PriorityNodes); with topk too, the two must be equal (else init_error())
+  BatchSchedulingPlugin(int device, int64_t max_schedule_time_ns, uint32_t out_flags = BS_OUT_FIT_BITMAP, uint32_t topk = 0,
+                        uint32_t priority_k = 0);
   ~BatchSchedulingPlugin();
   BatchSchedulingPlugin(const BatchSchedulingPlugin&) = delete;
   BatchSchedulingPlugin& operator=(const BatchSchedulingPlugin&) = delete;
@@ -299,6 +302,13 @@ class BatchSchedulingPlugin {
   // ("0/N nodes are available: ..."; lanes >= 4 by their resource names) for a pod that fits no node, "" otherwise
   std::vector<uint32_t> ReasonCounts(const std::string& uid) const;
   std::string FitError(const std::string& uid) const;
+  // plugin created with priority_k > 0: the pod's best fitting nodes of the last round under the resource priorities
+  // (node name, score), score descending, then snapshot order; at most priority_k of them, empty for an unknown uid.
+  // Entry 0 is where kube-scheduler's default profile would bind the pod, as far as these priorities decide it.
+  std::vector<std::pair<std::string, int64_t>> PriorityNodes(const std::string& uid) const;
+  // weights of NodeResourcesLeastAllocated, NodeResourcesMostAllocated and NodeResourcesBalancedAllocation (default
+  // 1, 0, 1), from the next round or delta round on
+  void SetScoreWeights(uint32_t least, uint32_t most, uint32_t balanced);
   int group_index(const std::string& ns_name) const;
   double last_pack_ms() const { return last_pack_ms_; }
   double last_device_ms() const { return last_device_ms_; }
@@ -357,6 +367,12 @@ class BatchSchedulingPlugin {
   // Preempt for every pending pod that passed PreFilter and fits no node (upstream preempts only on a FitError)
   Status PreemptAll(std::vector<Preemption>* out);
   const PackedBound& bound() const { return bound_; }
+  // The non-zero request columns of the resource priorities (no GPU): per pending pod and per NodeInfo (over
+  // NodeInfo::pods), [2][n] int64 — cpu millicores, memory bytes — summed over the containers' Requests, a container
+  // without a cpu key counting 100 m and without a memory key 200 MiB (an explicit zero stays zero).  Init containers
+  // and pod overhead are not modelled.
+  static Status PackNonZero(const std::vector<const NodeInfo*>& snapshot, const std::vector<const Pod*>& pending,
+                            std::vector<int64_t>* node_nz, std::vector<int64_t>* pod_nz);
 
   static Status Pack(const std::vector<const NodeInfo*>& snapshot, const std::vector<const Pod*>& pending,
                      const std::vector<PodGroup>& groups, const std::vector<uint32_t>& matched,
@@ -380,7 +396,8 @@ class BatchSchedulingPlugin {
   bs_engine* eng_ = nullptr;
   bool state_ready_ = false;   // bs_state_reset has run for this plugin's engine lineage
   int device_ = 0;
-  uint32_t out_flags_ = 0, eng_lanes_ = 0, topk_ = 0;
+  uint32_t out_flags_ = 0, eng_lanes_ = 0, topk_ = 0, priority_k_ = 0;
+  uint32_t weights_[3] = {1, 0, 1};
   std::string init_error_;
   int64_t max_schedule_time_ns_;
   std::map<std::string, GroupState> groups_;                        // ordered: canonical table order
@@ -401,11 +418,16 @@ class BatchSchedulingPlugin {
   std::vector<int32_t> topk_node_;                                  // [P][topk_] (BS_OUT_TOPK)
   std::vector<int64_t> topk_score_;
   std::vector<uint32_t> reasons_;                                   // [P][4 + lanes] (BS_OUT_REASONS)
+  std::vector<int32_t> prio_node_;                                  // [P][priority_k_] (BS_OUT_PRIORITY)
+  std::vector<int64_t> prio_score_;
   int64_t now_ns_ = 0;
   double last_pack_ms_ = 0, last_device_ms_ = 0;
   Status Reevaluate();   // bs_evaluate into the round's result vectors + the deny side effect (core.go:142,163)
   int FetchTopK();       // the round's top-K lists into topk_node_ / topk_score_ (no-op without topk)
   int FetchReasons();    // the round's reason rows into reasons_ (no-op without BS_OUT_REASONS)
+  int FetchPriority();   // the round's priority lists into prio_node_ / prio_score_ (no-op without priority_k)
+  Status UploadNonZero(const std::vector<const Pod*>* pending);   // node column of snapshot_ (+ the pods'); no-op without
+                                                                  // priority_k
   Status UploadBound();  // packs and uploads the bound-pod table of snapshot_ (no-op when no NodeInfo lists pods)
   Status RunPreempt(const std::vector<uint32_t>& rows, std::vector<Preemption>* out);
   std::vector<const NodeInfo*> snapshot_;                           // the round's NodeInfos (bound pods)

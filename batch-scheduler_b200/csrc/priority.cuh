@@ -1,0 +1,179 @@
+// priority.cuh — the resource priorities of a round (BS_OUT_PRIORITY): each pod's K best fitting nodes under
+// kube-scheduler v1.17's NodeResourcesLeastAllocated, NodeResourcesMostAllocated and
+// NodeResourcesBalancedAllocation (include/bsched.h, DESIGN.md §2 "Resource priorities").
+//
+// The fit set is the reason rows' (kernels.cuh K1c/K1d): a node fits a pod when its class gate bit is set and no lane
+// is short (lane_short over node_left_kernel's full-width residuals), the invariant DESIGN §2 states for reason rows.
+// The lists are kept with gang_fit's topk_insert (fit.cuh).
+#pragma once
+#include "kernels.cuh"
+#include "fit.cuh"
+
+namespace bsk {
+
+// floor(100 r / c) for 0 <= r <= c, 0 < c <= 2^56 (the node table's bound), and whether the division is exact.  The
+// quotient lies in [0, 100]; a float32 estimate (both operands rounded to nearest, then __fdividef: relative error below 2^-21 in all) is within
+// 100 * 2^-21 of it, so its truncation is the quotient or one off, and one exact int64 remainder test corrects it.
+// No 64-bit division subroutine runs.
+__device__ __forceinline__ int64_t pct_quotient(int64_t r, int64_t c, bool& exact) {
+  const int64_t num = r * 100;   // <= 100 * 2^56 < 2^63
+  int64_t q = (int64_t)__float2int_rz(__fdividef(__ll2float_rn(num), __ll2float_rn(c)));
+  int64_t rem = num - q * c;
+  if (rem < 0) { --q; rem += c; }
+  else if (rem >= c) { ++q; rem -= c; }
+  exact = rem == 0;
+  return q;
+}
+
+// fractionOfCapacity [upstream, from memory]: capacity 0 counts as full; else IEEE binary64 r / c, round to nearest
+__device__ __forceinline__ double cap_fraction(int64_t r, int64_t c) {
+  return c == 0 ? 1.0 : __ddiv_rn(__ll2double_rn(r), __ll2double_rn(c));
+}
+
+struct ScoreWeights {
+  uint32_t least, most, balanced;
+};
+
+// The weighted score of one (pod, node) pair, r = non-zero requests with the pod added, c = allocatable (unscaled):
+//   least(r, c) = (c - r) * 100 / c = 100 - ceil(100 r / c),  most(r, c) = floor(100 r / c)   (0 when c == 0 or r > c)
+//   Balanced = (1 - |fc - fm|) * 100 truncated toward zero (0 when a fraction is >= 1); __double2ll_rz saturates, so a
+//   product below -2^63 (a negative allocatable) gives INT64_MIN
+// and the sum w_least * Least + w_most * Most + w_balanced * Balanced wraps in two's complement.
+__device__ __forceinline__ int64_t pair_score(int64_t r_cpu, int64_t c_cpu, int64_t r_mem, int64_t c_mem, ScoreWeights w) {
+  uint64_t s = 0;
+  if (w.least | w.most) {
+    int64_t least = 0, most = 0;
+    if (c_cpu != 0 && r_cpu <= c_cpu) {
+      bool ex;
+      const int64_t q = pct_quotient(r_cpu, c_cpu, ex);
+      most += q;
+      least += 100 - q - (ex ? 0 : 1);
+    }
+    if (c_mem != 0 && r_mem <= c_mem) {
+      bool ex;
+      const int64_t q = pct_quotient(r_mem, c_mem, ex);
+      most += q;
+      least += 100 - q - (ex ? 0 : 1);
+    }
+    s += (uint64_t)w.least * (uint64_t)(least / 2) + (uint64_t)w.most * (uint64_t)(most / 2);
+  }
+  if (w.balanced) {
+    const double fc = cap_fraction(r_cpu, c_cpu), fm = cap_fraction(r_mem, c_mem);
+    int64_t b = 0;
+    if (!(fc >= 1.0 || fm >= 1.0)) b = __double2ll_rz(__dmul_rn(__dsub_rn(1.0, fabs(__dsub_rn(fc, fm))), 100.0));
+    s += (uint64_t)w.balanced * (uint64_t)b;
+  }
+  return (int64_t)s;
+}
+
+// K1e priority_pod_kernel — a warp takes PRIO_PPW pods and sweeps every node 32 at a time (lane k owns node
+// base + k), as reason_pod_kernel does.  A node fits when the pod's class gate bit is set and no lane it compares is
+// short; each fitting pair is scored and offered to the pod's list.  Lists live in shared memory, 32 (score, node)
+// entries per pod ordered by score descending, then node ascending; unfilled entries are (INT64_MIN, PRIO_EMPTY) and
+// rank after every real entry, including one that scores INT64_MIN.  A fitting pair is a candidate while the list has
+// fewer than K fitting nodes, or when it beats the score of entry K-1: nodes come in ascending order, so a later node
+// never displaces an equal score.  MAXL bounds the lanes held in registers (5, 9 or 16).
+constexpr int PRIO_THREADS = 256;
+constexpr int PRIO_PPW = 4;                                           // pods per warp
+constexpr int PRIO_PODS_PER_CTA = (PRIO_THREADS / 32) * PRIO_PPW;
+constexpr int32_t PRIO_EMPTY = 0x7fffffff;                            // node of an unfilled list entry
+struct PriorityArgs {
+  const int64_t* left;          // [L][Npad] left_full
+  const uint32_t* left_present; // [Npad]
+  const uint32_t* gate;         // [classes][Wg]
+  const int64_t* req;           // [L][P]
+  const uint32_t* req_present;  // [P]
+  const uint32_t* fit_class;    // [P]
+  const int64_t* alloc;         // [L][Npad] the node table's allocatable: rows 0 (cpu) and 1 (memory)
+  const int64_t* node_nz;       // [2][Npad] non-zero requests on the node (padding 0)
+  const int64_t* pod_nz;        // [2][P]
+  int32_t* out_node;            // [P][K]
+  int64_t* out_score;           // [P][K]
+  ScoreWeights w;
+  uint32_t P, N, Npad, Wg, L, K;
+};
+template <int MAXL>
+__global__ void __launch_bounds__(PRIO_THREADS) priority_pod_kernel(PriorityArgs a) {
+  constexpr int WARPS = PRIO_THREADS / 32;
+  __shared__ int64_t s_req[WARPS][PRIO_PPW][MAXL];
+  __shared__ int64_t s_ls[WARPS][PRIO_PPW][32];
+  __shared__ int32_t s_ln[WARPS][PRIO_PPW][32];
+  const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const uint32_t p0 = (blockIdx.x * WARPS + wid) * PRIO_PPW;
+  const int L = (int)a.L;
+  for (uint32_t k = lane; k < PRIO_PPW * MAXL; k += 32) {
+    const uint32_t j = k / MAXL, d = k % MAXL, p = p0 + j;
+    s_req[wid][j][d] = (p < a.P && d < a.L) ? a.req[(size_t)d * a.P + p] : 0;
+  }
+#pragma unroll
+  for (int j = 0; j < PRIO_PPW; ++j) {
+    s_ls[wid][j][lane] = INT64_MIN;
+    s_ln[wid][j][lane] = PRIO_EMPTY;
+  }
+  __syncwarp();
+  uint32_t rmask[PRIO_PPW];   // lanes compared: 0-3 always, scalar lanes the pod requests; 0 = no pod
+  const uint32_t* grow[PRIO_PPW];
+  int64_t nz_cpu[PRIO_PPW], nz_mem[PRIO_PPW], thr[PRIO_PPW];
+  uint32_t nfit[PRIO_PPW];
+#pragma unroll
+  for (int j = 0; j < PRIO_PPW; ++j) {
+    const uint32_t p = p0 + j;
+    const bool ok = p < a.P;
+    rmask[j] = ok ? (a.req_present[p] | 0xFu) : 0u;
+    grow[j] = a.gate + (size_t)(ok ? a.fit_class[p] : 0u) * a.Wg;
+    nz_cpu[j] = ok ? a.pod_nz[p] : 0;
+    nz_mem[j] = ok ? a.pod_nz[(size_t)a.P + p] : 0;
+    thr[j] = INT64_MIN;
+    nfit[j] = 0;
+  }
+  for (uint32_t base = 0; base < a.N; base += 32) {
+    const uint32_t i = base + lane, w = base >> 5;
+    bool g[PRIO_PPW];
+    uint32_t any = 0;
+#pragma unroll
+    for (int j = 0; j < PRIO_PPW; ++j) {
+      const uint32_t gw = rmask[j] ? grow[j][w] : 0u;   // the word of the padded table: bits >= N are 0
+      any |= gw;
+      g[j] = (gw >> lane) & 1u;
+    }
+    if (!any) continue;   // warp-uniform: no pod of the warp looks at these 32 nodes
+    const uint32_t lp = a.left_present[i] | 0xFu;   // i < Npad: the padded tables are readable
+#pragma unroll
+    for (int d = 0; d < MAXL; ++d) {
+      if (d >= L) break;
+      const int64_t v = a.left[(size_t)d * a.Npad + i];
+      const bool pres = (lp >> d) & 1u;
+#pragma unroll
+      for (int j = 0; j < PRIO_PPW; ++j)
+        if (((rmask[j] >> d) & 1u) && lane_short(pres, v, s_req[wid][j][d])) g[j] = false;
+    }
+    uint32_t fw[PRIO_PPW], anyfit = 0;
+#pragma unroll
+    for (int j = 0; j < PRIO_PPW; ++j) {
+      fw[j] = __ballot_sync(0xffffffffu, g[j]);
+      anyfit |= fw[j];
+    }
+    if (!anyfit) continue;
+    const int64_t c_cpu = a.alloc[i], c_mem = a.alloc[(size_t)a.Npad + i];
+    const int64_t n_cpu = a.node_nz[i], n_mem = a.node_nz[(size_t)a.Npad + i];
+#pragma unroll
+    for (int j = 0; j < PRIO_PPW; ++j) {
+      if (!fw[j]) continue;   // warp-uniform
+      const int64_t s = g[j] ? pair_score(n_cpu + nz_cpu[j], c_cpu, n_mem + nz_mem[j], c_mem, a.w) : INT64_MIN;
+      const uint32_t cb = __ballot_sync(0xffffffffu, g[j] && (nfit[j] < a.K || s > thr[j]));
+      if (cb) thr[j] = topk_insert<int64_t>(s_ls[wid][j], s_ln[wid][j], a.K, cb, s, (int32_t)base, lane);
+      nfit[j] += __popc(fw[j]);
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < PRIO_PPW; ++j) {
+    const uint32_t p = p0 + j;
+    if (p < a.P && lane < a.K) {
+      const int32_t n = s_ln[wid][j][lane];
+      a.out_node[(size_t)p * a.K + lane] = n == PRIO_EMPTY ? -1 : n;
+      a.out_score[(size_t)p * a.K + lane] = n == PRIO_EMPTY ? INT64_MIN : s_ls[wid][j][lane];
+    }
+  }
+}
+
+}  // namespace bsk

@@ -59,17 +59,22 @@ def _table_c(table):
 
 class Engine:
     def __init__(self, n_lanes: int, device: int = 0, fit_bitmap: bool = True, score: bool = False,
-                 filter: bool = False, topk: int = 0, reasons: bool = False):
+                 filter: bool = False, topk: int = 0, reasons: bool = False, priority_k: int = 0):
         """topk > 0 also keeps each pod's `topk` best fitting nodes and their scores (BS_OUT_TOPK, read with
         topk_rows); it cannot be combined with score=True, whose matrix holds them already.  reasons=True also counts,
-        per pod, the nodes that reject it for each reason (BS_OUT_REASONS, read with reason_rows)."""
+        per pod, the nodes that reject it for each reason (BS_OUT_REASONS, read with reason_rows).  priority_k > 0 also
+        keeps each pod's priority_k best fitting nodes under kube-scheduler's resource priorities (BS_OUT_PRIORITY, read
+        with priority_rows; needs upload_nonzero before each round); with topk too, both lists have the same length."""
+        if topk and priority_k and topk != priority_k:
+            raise ValueError("topk and priority_k share the list length K: they must be equal")
         self.lib = capi.load()
         self.n_lanes = n_lanes
         self.topk = topk
+        self.priority_k = priority_k
         self.out_flags = ((capi.OUT_FIT_BITMAP if fit_bitmap else 0) | (capi.OUT_SCORE if score else 0) |
                           (capi.OUT_FILTER if filter else 0) | (capi.OUT_TOPK if topk else 0) |
-                          (capi.OUT_REASONS if reasons else 0))
-        cfg = capi.Config(device, n_lanes, self.out_flags, topk)
+                          (capi.OUT_REASONS if reasons else 0) | (capi.OUT_PRIORITY if priority_k else 0))
+        cfg = capi.Config(device, n_lanes, self.out_flags, topk or priority_k)
         h = C.c_void_p()
         rc = self.lib.bs_create(C.byref(cfg), C.byref(h))
         if rc != 0:
@@ -259,6 +264,30 @@ class Engine:
         out = np.zeros((n, 4 + self.n_lanes), np.uint32)
         self._check(self.lib.bs_fetch_reason_rows(self.h, pod0, n, capi.ptr(out)))
         return out
+
+    # -- resource priorities (BS_OUT_PRIORITY) -------------------------------------------------
+    def set_score_weights(self, least: int = 1, most: int = 0, balanced: int = 1):
+        """Weights of LeastAllocated, MostAllocated and BalancedAllocation for the next rounds (default 1, 0, 1)."""
+        self._check(self.lib.bs_set_score_weights(self.h, least, most, balanced))
+
+    def upload_nonzero(self, node=None, pods=None):
+        """The non-zero request columns: node [2, N] and/or pods [2, P] int64 (row 0 cpu millicores, row 1 memory
+        bytes).  Uploading nodes (or updating node rows) drops the node column, uploading pods the pod column."""
+        if node is not None:
+            a = np.ascontiguousarray(node, dtype=np.int64)
+            self._check(self.lib.bs_upload_node_nonzero(self.h, a.shape[1] if a.ndim == 2 else 0, capi.ptr(a)))
+        if pods is not None:
+            a = np.ascontiguousarray(pods, dtype=np.int64)
+            self._check(self.lib.bs_upload_pod_nonzero(self.h, a.shape[1] if a.ndim == 2 else 0, capi.ptr(a)))
+
+    def priority_rows(self, pod0=0, n=None):
+        """(nodes [n, K] int32, scores [n, K] int64): each pod's fitting nodes by priority score descending, then node
+        index ascending; min(K, feasible_count) entries, padded with node -1 and score INT64_MIN."""
+        n = self.P - pod0 if n is None else n
+        nodes = np.zeros((n, self.priority_k), np.int32)
+        scores = np.zeros((n, self.priority_k), np.int64)
+        self._check(self.lib.bs_fetch_priority_rows(self.h, pod0, n, capi.ptr(nodes), capi.ptr(scores)))
+        return nodes, scores
 
     def fit_error(self, counts, n_nodes: int, scalar_names=None) -> str:
         """The "0/N nodes are available: ..." message of one reason row (bs_format_fit_error)."""

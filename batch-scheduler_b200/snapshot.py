@@ -335,6 +335,30 @@ def bound_pods(snap: Snapshot, seed: int, fill: float = 1.0, max_per_node: int =
     return bt
 
 
+DEFAULT_MILLI_CPU_REQUEST = 100                 # GetNonzeroRequests: a container without a cpu request
+DEFAULT_MEMORY_REQUEST = 200 * 1024 * 1024      # ... and without a memory request
+NONZERO_MAX = 1 << 56
+
+
+def nonzero_requests(snap: Snapshot, seed: int, explicit_zero: float = 0.1, unset_on_node: int = 4):
+    """Seeded non-zero request columns (BS_OUT_PRIORITY) for a table without containers: (node [2, N], pod [2, P])
+    int64, row 0 cpu (millicores), row 1 memory (bytes).  The stand-in: a pod is one container whose Requests are its
+    req lanes 0-1; a zero there is an absent key (counted as 100 m / 200 MiB) except with probability `explicit_zero`,
+    where it is an explicit zero and stays 0.  A node's column is its requested lanes 0-1 plus 0..unset_on_node pods
+    without any request (each counted at both defaults).  Values are clipped into [0, 2^56]."""
+    rng = np.random.default_rng(seed)
+    nt, pt = snap.nodes, snap.pods
+    pod = np.zeros((2, pt.n), np.int64)
+    for row, lane, dflt in ((0, LANE_CPU, DEFAULT_MILLI_CPU_REQUEST), (1, LANE_MEM, DEFAULT_MEMORY_REQUEST)):
+        r = pt.req[lane].astype(np.int64)
+        absent = (r == 0) & (rng.random(pt.n) >= explicit_zero)
+        pod[row] = np.where(absent, dflt, r)
+    unset = rng.integers(0, unset_on_node + 1, nt.n).astype(np.int64)
+    node = np.stack([nt.requested[LANE_CPU].astype(np.int64) + unset * DEFAULT_MILLI_CPU_REQUEST,
+                     nt.requested[LANE_MEM].astype(np.int64) + unset * DEFAULT_MEMORY_REQUEST])
+    return np.clip(node, 0, NONZERO_MAX), np.clip(pod, 0, NONZERO_MAX)
+
+
 # ----------------------------------------------------------------------------
 # splitmix64 stream (vectorised): value i of the stream with seed s is
 # mix(s + (i+1)*0x9E3779B97F4A7C15).

@@ -179,6 +179,8 @@ typedef struct {
 #define BS_TOPK_MAX 32         /* largest list length K */
 #define BS_OUT_REASONS 0x10u   /* P x (4 + n_lanes) u32: per pod, how many nodes reject it for each reason
                                   (bs_fetch_reason_rows); combines with every other flag */
+#define BS_OUT_PRIORITY 0x20u  /* P x K: each pod's K best fitting nodes under kube-scheduler's resource priorities
+                                  (bs_fetch_priority_rows); combines with every other flag, K = bs_config.topk */
 
 /* Bins of a reason row.  A node counts in no bin <=> the pod fits it (fit bitmap bit set); a guarded node counts in
  * exactly one of bins 0-1 (precedence nil, Node()==nil, unschedulable, Taints() error, core.go:606-617,639); a node
@@ -195,7 +197,8 @@ typedef struct {
   int32_t device;      /* CUDA device ordinal */
   uint32_t n_lanes;    /* lanes of every table uploaded to this engine */
   uint32_t out_flags;  /* BS_OUT_* */
-  uint32_t topk;       /* list length K: 1..BS_TOPK_MAX with BS_OUT_TOPK, 0 without (else bs_create -> BS_E_INVAL) */
+  uint32_t topk;       /* list length K: 1..BS_TOPK_MAX with BS_OUT_TOPK or BS_OUT_PRIORITY, 0 without either (else
+                          bs_create -> BS_E_INVAL); with both flags both lists have length K */
 } bs_config;
 
 /* Host result buffers; any pointer may be NULL (that output is not copied back). */
@@ -429,6 +432,34 @@ int bs_fetch_reason_rows(bs_engine* e, uint32_t pod0, uint32_t n, uint32_t* coun
  * A buffer too small for the whole message is BS_E_INVAL (nothing is truncated). */
 int bs_format_fit_error(const uint32_t* counts, uint32_t n_lanes, uint32_t n_nodes, const char* const* scalar_names,
                         char* buf, size_t buf_len);
+
+/* ---- resource priorities (BS_OUT_PRIORITY): kube-scheduler v1.17's NodeResourcesLeastAllocated,
+ *      NodeResourcesMostAllocated and NodeResourcesBalancedAllocation over each pod's fitting nodes ----
+ * For pod p and node n, with cap = alloc[0..1][n] (unscaled) and req = node_nz[n] + pod_nz[p] per resource:
+ *     least(r, c) = c == 0 || r > c ? 0 : (c - r) * 100 / c      most(r, c) = c == 0 || r > c ? 0 : r * 100 / c
+ *     Least = (least(cpu) + least(mem)) / 2        Most = (most(cpu) + most(mem)) / 2        (int64, truncating)
+ *     frac(r, c) = c == 0 ? 1.0 : (double)r / (double)c                      (IEEE binary64, round to nearest)
+ *     Balanced = fc >= 1 || fm >= 1 ? 0 : (int64)((1.0 - fabs(fc - fm)) * 100.0)   (toward zero; below -2^63:
+ *                INT64_MIN)
+ *     score = w_least * Least + w_most * Most + w_balanced * Balanced        (int64, two's complement wrap)
+ * Only the pod's fitting nodes are scored (fit bitmap bit set).  The non-zero columns are caller-supplied: per pod
+ * the sum over its containers of the Requests with an absent cpu key counted as 100 (millicores) and an absent memory
+ * key as 209715200 (bytes; an explicit zero stays zero); per node the same sum over the pods on it
+ * (NodeInfo.NonZeroRequest()).  Values lie in [0, BS_NONZERO_MAX]. */
+#define BS_NONZERO_MAX (1ll << 56)
+/* weights of the three scores (default 1, 0, 1: v1.17's default provider); any time, read by the next evaluation */
+int bs_set_score_weights(bs_engine* e, uint32_t least, uint32_t most, uint32_t balanced);
+/* nz[2][n_nodes]: row 0 cpu (millicores), row 1 memory (bytes).  n_nodes must equal the uploaded node table's
+ * (else BS_E_INVAL); a value outside [0, BS_NONZERO_MAX] is BS_E_RANGE and drops the column.  The column belongs to the
+ * node snapshot: bs_upload_nodes and bs_update_nodes drop it. */
+int bs_upload_node_nonzero(bs_engine* e, uint32_t n_nodes, const int64_t* nz);
+/* nz[2][n_pods], the same for the pod table; bs_upload_pods drops it.  An evaluation with BS_OUT_PRIORITY and either
+ * column missing is BS_E_STATE before anything is launched. */
+int bs_upload_pod_nonzero(bs_engine* e, uint32_t n_pods, const int64_t* nz);
+/* copy the priority lists of pods [pod0, pod0+n) to the host as dense [n][K] rows (BS_OUT_PRIORITY).  Row p holds
+ * the fitting nodes of pod p ordered by score descending, then node index ascending, min(K, feasible_count[p]) of
+ * them, padded with node -1 and score INT64_MIN.  Either pointer may be NULL. */
+int bs_fetch_priority_rows(bs_engine* e, uint32_t pod0, uint32_t n, int32_t* nodes, int64_t* scores);
 
 /* ---- preemption: PreFilterExtensions.RemovePod and the node / victims kube-scheduler's preemption would pick ----
  * The bound-pod table lists the pods already running on the snapshot's nodes (NodeInfo.Pods()).  Rows may come in

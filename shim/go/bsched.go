@@ -55,6 +55,19 @@ func NewTopK(device, lanes int, outFlags uint32, topk int) (*Engine, error) {
 	return &Engine{h, topk, lanes}, nil
 }
 
+// NewPriority is New with each round also keeping every pod's k best fitting nodes under kube-scheduler's resource
+// priorities (BS_OUT_PRIORITY, 1..BS_TOPK_MAX), read with PriorityNodes.  outFlags may hold BS_OUT_TOPK too: both
+// lists then have length k.
+func NewPriority(device, lanes int, outFlags uint32, k int) (*Engine, error) {
+	cfg := C.bs_config{device: C.int32_t(device), n_lanes: C.uint32_t(lanes),
+		out_flags: C.uint32_t(outFlags | C.BS_OUT_PRIORITY), topk: C.uint32_t(k)}
+	var h *C.bs_engine
+	if rc := C.bs_create(&cfg, &h); rc != 0 {
+		return nil, fmt.Errorf("bs_create: %s", C.GoString(C.bs_strerror(rc)))
+	}
+	return &Engine{h, k, lanes}, nil
+}
+
 func (e *Engine) Close() { C.bs_destroy(e.h) }
 
 func (e *Engine) rc(code C.int) error {
@@ -136,6 +149,43 @@ func (e *Engine) TopNodes(pod0, n int) ([]int32, []int64, error) {
 		return nodes, scores, e.rc(C.bs_fetch_topk_rows(e.h, C.uint32_t(pod0), C.uint32_t(n), nil, nil))
 	}
 	err := e.rc(C.bs_fetch_topk_rows(e.h, C.uint32_t(pod0), C.uint32_t(n), (*C.int32_t)(unsafe.Pointer(&nodes[0])),
+		(*C.int64_t)(unsafe.Pointer(&scores[0]))))
+	return nodes, scores, err
+}
+
+// SetScoreWeights sets the weights of NodeResourcesLeastAllocated, NodeResourcesMostAllocated and
+// NodeResourcesBalancedAllocation (default 1, 0, 1) for the next rounds.
+func (e *Engine) SetScoreWeights(least, most, balanced uint32) error {
+	return e.rc(C.bs_set_score_weights(e.h, C.uint32_t(least), C.uint32_t(most), C.uint32_t(balanced)))
+}
+
+// UploadNodeNonZero / UploadPodNonZero: the non-zero request columns, nz[2][n] (cpu millicores, then memory bytes):
+// per pod the sum over its containers of GetNonzeroRequestForResource(Requests), per node NodeInfo.NonZeroRequest().
+// UploadNodes / UpdateNodes drop the node column and UploadPods the pod column: upload them again before Evaluate.
+func (e *Engine) UploadNodeNonZero(nz []int64) error {
+	n := len(nz) / 2
+	if n == 0 {
+		return e.rc(C.bs_upload_node_nonzero(e.h, 0, nil))
+	}
+	return e.rc(C.bs_upload_node_nonzero(e.h, C.uint32_t(n), (*C.int64_t)(unsafe.Pointer(&nz[0]))))
+}
+func (e *Engine) UploadPodNonZero(nz []int64) error {
+	n := len(nz) / 2
+	if n == 0 {
+		return e.rc(C.bs_upload_pod_nonzero(e.h, 0, nil))
+	}
+	return e.rc(C.bs_upload_pod_nonzero(e.h, C.uint32_t(n), (*C.int64_t)(unsafe.Pointer(&nz[0]))))
+}
+
+// PriorityNodes returns the priority lists of pods [pod0, pod0+n) of the last round (engine from NewPriority) as dense
+// [n][K] rows: each pod's fitting nodes by priority score descending, then node index ascending, padded with node -1
+// and score math.MinInt64.  Entry 0 is the node to bind or nominate.
+func (e *Engine) PriorityNodes(pod0, n int) ([]int32, []int64, error) {
+	nodes, scores := make([]int32, n*e.topk), make([]int64, n*e.topk)
+	if len(nodes) == 0 {
+		return nodes, scores, e.rc(C.bs_fetch_priority_rows(e.h, C.uint32_t(pod0), C.uint32_t(n), nil, nil))
+	}
+	err := e.rc(C.bs_fetch_priority_rows(e.h, C.uint32_t(pod0), C.uint32_t(n), (*C.int32_t)(unsafe.Pointer(&nodes[0])),
 		(*C.int64_t)(unsafe.Pointer(&scores[0]))))
 	return nodes, scores, err
 }
