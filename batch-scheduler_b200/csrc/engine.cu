@@ -402,6 +402,7 @@ struct bs_engine {
   // table), the score weights, and the lists [P][topk]; the fit set is the reason rows' (d_left_full, d_reason_gate)
   DevBuf d_nz_node, d_nz_pod, d_prio_node, d_prio_score;
   bool have_nz_node = false, have_nz_pod = false;
+  int64_t nz_node_max[2] = {0, 0}, nz_pod_max[2] = {0, 0};   // per row, of the uploaded columns (bs_replay_priority)
   ScoreWeights weights{1, 0, 1};
   // sort scratch: views into one arena
   View d_gk0, d_gk1, d_pk0, d_pk1, d_idx_a, d_idx_b, d_ghist, d_group_rank, d_tilecnt, d_sort_barrier;
@@ -775,13 +776,16 @@ void launch_prefix(uint32_t L, NodeTab t, PrefixSel ps, PrefixScratch sc, Prefix
 }
 
 template <int MAXL>
-void launch_replay_t(const ReplayArgs& a, cudaStream_t s) { replay_kernel<MAXL><<<1, REPLAY_THREADS, 0, s>>>(a); }
+void launch_replay_t(const ReplayArgs& a, bool scored, cudaStream_t s) {
+  if (scored) replay_kernel<MAXL, true><<<1, REPLAY_THREADS, 0, s>>>(a);
+  else replay_kernel<MAXL, false><<<1, REPLAY_THREADS, 0, s>>>(a);
+}
 inline uint32_t replay_maxl(uint32_t L) { return L <= 5 ? 5u : L <= 9 ? 9u : 16u; }
-void launch_replay(uint32_t L, const ReplayArgs& a, cudaStream_t s) {
+void launch_replay(uint32_t L, const ReplayArgs& a, bool scored, cudaStream_t s) {
   switch (replay_maxl(L)) {
-    case 5: launch_replay_t<5>(a, s); break;
-    case 9: launch_replay_t<9>(a, s); break;
-    default: launch_replay_t<16>(a, s); break;
+    case 5: launch_replay_t<5>(a, scored, s); break;
+    case 9: launch_replay_t<9>(a, scored, s); break;
+    default: launch_replay_t<16>(a, scored, s); break;
   }
 }
 
@@ -2293,18 +2297,28 @@ int bs_cluster_check(bs_engine* e, uint64_t sel, uint64_t tol, float percent, co
   return BS_OK;
 }
 
-int bs_replay(bs_engine* e, const uint32_t* queue, uint32_t n_queue, bs_replay_result* out) {
-  if (!e || !out) return BS_E_INVAL;
-  std::lock_guard<std::mutex> lk(e->mu);
+namespace {
+// bs_replay and bs_replay_priority (replay.cuh): the checks, the scratch copies, the walk and the read-back.  `scored`
+// selects bs_replay_priority's node choice, which also needs both non-zero columns and reads the live node column back
+// into nz_after ([2][N], or NULL).  The caller holds the engine's lock.
+int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n_queue, bs_replay_result* out,
+                bool scored, int64_t* nz_after) {
+  const std::string w(who);
   if (!e->have_nodes || !e->have_pods || !e->have_groups)
-    return fail(e, BS_E_STATE, "bs_replay: upload nodes, groups and pods first");
+    return fail(e, BS_E_STATE, (w + ": upload nodes, groups and pods first").c_str());
+  if (scored && !(e->have_nz_node && e->have_nz_pod))
+    return fail(e, BS_E_STATE, (w + ": upload both non-zero request columns first").c_str());
   BS_DEVICE_GUARD(e);
   const uint32_t N = e->N, Npad = e->Npad, P = e->P, G = e->G, L = e->L;
   if (!queue) n_queue = P;
   if (n_queue && (!out->prefilter || !out->node || !out->ready)) return BS_E_INVAL;
   if (queue)
     for (uint32_t i = 0; i < n_queue; ++i)
-      if (queue[i] >= P) return fail(e, BS_E_INDEX, "bs_replay: queue entry is not a pod of the table");
+      if (queue[i] >= P) return fail(e, BS_E_INDEX, (w + ": queue entry is not a pod of the table").c_str());
+  // the live non-zero sums: at most the node column's maximum plus every queued pod's
+  for (int r = 0; r < 2 && scored; ++r)
+    if ((long double)e->nz_node_max[r] + (long double)n_queue * (long double)e->nz_pod_max[r] > 0x1p62L)
+      return fail(e, BS_E_RANGE, (w + ": live non-zero requests could pass 2^62").c_str());
   int rc;
   if (e->classes_dirty && (rc = rebuild_classes(e))) return rc;
 
@@ -2326,7 +2340,7 @@ int bs_replay(bs_engine* e, const uint32_t* queue, uint32_t n_queue, bs_replay_r
   const bool cache = safe && fitmask && n_blocks >= 1 && n_blocks <= (uint32_t)REPLAY_MAX_BLOCKS;
   const size_t rows = cache ? (size_t)2 * e->n_rep_classes * n_blocks : 0, maxl = replay_maxl(L);
   View s_req, s_pc, s_rp, s_matched, s_gflags, s_grc, s_minres, s_mrp, d_queue, d_pf, d_node, d_ready, d_status,
-      n_left0, n_left1, n_both, n_stat, n_fit, c_sum, c_max, c_keys;
+      n_left0, n_left1, n_both, n_stat, n_fit, c_sum, c_max, c_keys, n_nz;
   // The node state and block cache every step reads come first: carved behind the copies, the same kernel took
   // 2 % longer at the bench shape on an H100.
   CK(carve(e->d_replay,
@@ -2335,7 +2349,7 @@ int bs_replay(bs_engine* e, const uint32_t* queue, uint32_t n_queue, bs_replay_r
             {&c_max, rows * maxl * 8}, {&c_keys, rows * 4}, {&s_req, (size_t)L * Npad * 8}, {&s_pc, (size_t)Npad * 4},
             {&s_rp, (size_t)Npad * 4}, {&s_matched, (size_t)Gp * 4}, {&s_gflags, Gp}, {&s_grc, (size_t)Gp * 4},
             {&s_minres, (size_t)L * Gp * 8}, {&s_mrp, (size_t)Gp * 4}, {&d_queue, (size_t)Qp * 4}, {&d_pf, Qp},
-            {&d_node, (size_t)Qp * 4}, {&d_ready, Qp}, {&d_status, 128}}));
+            {&d_node, (size_t)Qp * 4}, {&d_ready, Qp}, {&d_status, 128}, {&n_nz, scored ? (size_t)2 * Npad * 8 : 0}}));
   auto dup = [&](const View& dst, const DevBuf& src, size_t bytes) {
     return bytes ? cudaMemcpyAsync(dst.p, src.p, bytes, cudaMemcpyDeviceToDevice, e->s) : cudaSuccess;
   };
@@ -2347,6 +2361,7 @@ int bs_replay(bs_engine* e, const uint32_t* queue, uint32_t n_queue, bs_replay_r
   CK(dup(s_grc, e->d_group_rep_class, (size_t)G * 4));
   CK(dup(s_minres, e->d_min_res, (size_t)L * G * 8));
   CK(dup(s_mrp, e->d_mrpres, (size_t)G * 4));
+  if (scored) CK(dup(n_nz, e->d_nz_node, (size_t)2 * Npad * 8));
   if (queue && n_queue) CK(cudaMemcpyAsync(d_queue.p, queue, (size_t)n_queue * 4, cudaMemcpyHostToDevice, e->s));
   CK(cudaMemsetAsync(d_status.p, 0, 128, e->s));
   ReplayArgs a{};
@@ -2387,9 +2402,14 @@ int bs_replay(bs_engine* e, const uint32_t* queue, uint32_t n_queue, bs_replay_r
   a.node = d_node.as<int32_t>();
   a.ready = d_ready.as<uint8_t>();
   a.status = d_status.as<int32_t>();
+  if (scored) {
+    a.nz_live = n_nz.as<int64_t>();
+    a.pod_nz = e->d_nz_pod.as<int64_t>();
+    a.w = e->weights;
+  }
   {
     StageTimer tm(e, BS_K_REPLAY, e->s);
-    launch_replay(L, a, e->s);
+    launch_replay(L, a, scored, e->s);
     tm.launched();
     CK(cudaGetLastError());
   }
@@ -2411,18 +2431,35 @@ int bs_replay(bs_engine* e, const uint32_t* queue, uint32_t n_queue, bs_replay_r
   CK(d2h(out->group_flags, s_gflags, (size_t)G));
   CK(d2h(out->group_min_res, s_minres, (size_t)L * G * 8));
   CK(d2h(out->group_min_res_present, s_mrp, (size_t)G * 4));
+  if (scored && nz_after && N)
+    CK(cudaMemcpy2DAsync(nz_after, (size_t)N * 8, n_nz.p, (size_t)Npad * 8, (size_t)N * 8, 2, cudaMemcpyDeviceToHost,
+                         e->s));
   if (out->group_rep_sel || out->group_rep_tol) {
     grc.resize(Gp);
     CK(d2h(grc.data(), s_grc, (size_t)G * 4));
   }
   CK(cudaStreamSynchronize(e->s));
-  if (status) return fail(e, BS_E_REF_PANIC, "bs_replay: findMaxPG would divide by MinMember == 0 (core.go:716)");
+  if (status) return fail(e, BS_E_REF_PANIC, (w + ": findMaxPG would divide by MinMember == 0 (core.go:716)").c_str());
   for (uint32_t g = 0; g < G && (out->group_rep_sel || out->group_rep_tol); ++g) {
     const ClassKey& k = e->rep_index.keys[grc[g]];
     if (out->group_rep_sel) out->group_rep_sel[g] = k.sel;
     if (out->group_rep_tol) out->group_rep_tol[g] = k.tol;
   }
   return BS_OK;
+}
+}  // namespace
+
+int bs_replay(bs_engine* e, const uint32_t* queue, uint32_t n_queue, bs_replay_result* out) {
+  if (!e || !out) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  return replay_walk(e, "bs_replay", queue, n_queue, out, false, nullptr);
+}
+
+int bs_replay_priority(bs_engine* e, const uint32_t* queue, uint32_t n_queue, bs_replay_result* out,
+                       int64_t* node_nonzero_after) {
+  if (!e || !out) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  return replay_walk(e, "bs_replay_priority", queue, n_queue, out, true, node_nonzero_after);
 }
 
 // ---- preemption: bs_upload_bound_pods, bs_preempt, bs_remove_pod (preempt.cuh) ----
@@ -2807,11 +2844,17 @@ int bs_set_score_weights(bs_engine* e, uint32_t least, uint32_t most, uint32_t b
 
 namespace {
 // One non-zero column [2][n] into dst ([2][pitch], zero beyond n).  The caller has dropped the column already; it is
-// marked present only when every value lies in [0, BS_NONZERO_MAX].
-int upload_nonzero(bs_engine* e, DevBuf& dst, uint32_t n, uint32_t pitch, const int64_t* nz, const char* who) {
+// marked present only when every value lies in [0, BS_NONZERO_MAX].  mx gets each row's maximum (bs_replay_priority's
+// overflow bound).
+int upload_nonzero(bs_engine* e, DevBuf& dst, uint32_t n, uint32_t pitch, const int64_t* nz, const char* who,
+                   int64_t (&mx)[2]) {
   if (n && !nz) return fail(e, BS_E_INVAL, who);
-  for (size_t k = 0; k < (size_t)2 * n; ++k)
+  mx[0] = mx[1] = 0;
+  for (size_t k = 0; k < (size_t)2 * n; ++k) {
     if (nz[k] < 0 || nz[k] > BS_NONZERO_MAX) return fail(e, BS_E_RANGE, "non-zero request outside [0, 2^56]");
+    int64_t& m = mx[k >= n];
+    m = std::max(m, nz[k]);
+  }
   BS_DEVICE_GUARD(e);
   CK(dst.ensure((size_t)2 * std::max(pitch, 1u) * 8));
   if (pitch > n) CK(cudaMemsetAsync(dst.p, 0, (size_t)2 * pitch * 8, e->s));
@@ -2828,7 +2871,8 @@ int bs_upload_node_nonzero(bs_engine* e, uint32_t n_nodes, const int64_t* nz) {
   e->have_nz_node = false;
   if (!e->have_nodes) return fail(e, BS_E_STATE, "bs_upload_node_nonzero: upload nodes first");
   if (n_nodes != e->N) return fail(e, BS_E_INVAL, "bs_upload_node_nonzero: n_nodes differs from the node table's");
-  const int rc = upload_nonzero(e, e->d_nz_node, n_nodes, e->Npad, nz, "bs_upload_node_nonzero: null column");
+  const int rc = upload_nonzero(e, e->d_nz_node, n_nodes, e->Npad, nz, "bs_upload_node_nonzero: null column",
+                                e->nz_node_max);
   e->have_nz_node = rc == BS_OK;
   return rc;
 }
@@ -2839,7 +2883,8 @@ int bs_upload_pod_nonzero(bs_engine* e, uint32_t n_pods, const int64_t* nz) {
   e->have_nz_pod = false;
   if (!e->have_pods) return fail(e, BS_E_STATE, "bs_upload_pod_nonzero: upload pods first");
   if (n_pods != e->P) return fail(e, BS_E_INVAL, "bs_upload_pod_nonzero: n_pods differs from the pod table's");
-  const int rc = upload_nonzero(e, e->d_nz_pod, n_pods, n_pods, nz, "bs_upload_pod_nonzero: null column");
+  const int rc = upload_nonzero(e, e->d_nz_pod, n_pods, n_pods, nz, "bs_upload_pod_nonzero: null column",
+                                e->nz_pod_max);
   e->have_nz_pod = rc == BS_OK;
   return rc;
 }

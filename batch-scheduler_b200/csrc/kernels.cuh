@@ -121,6 +121,66 @@ __device__ __forceinline__ bool lane_short(bool present, int64_t left, int64_t r
 }
 
 // ---------------------------------------------------------------------------
+// The resource priorities (include/bsched.h, DESIGN.md §2 "Resource priorities"): kube-scheduler v1.17's
+// NodeResourcesLeastAllocated, NodeResourcesMostAllocated and NodeResourcesBalancedAllocation for one (pod, node)
+// pair.  Shared by the round's priority lists (priority.cuh) and bs_replay_priority's node choice (replay.cuh).
+
+// floor(100 r / c) for 0 <= r <= c, 0 < c <= 2^56 (the node table's bound), and whether the division is exact.  The
+// quotient lies in [0, 100]; a float32 estimate (both operands rounded to nearest, then __fdividef: relative error below 2^-21 in all) is within
+// 100 * 2^-21 of it, so its truncation is the quotient or one off, and one exact int64 remainder test corrects it.
+// No 64-bit division subroutine runs.
+__device__ __forceinline__ int64_t pct_quotient(int64_t r, int64_t c, bool& exact) {
+  const int64_t num = r * 100;   // <= 100 * 2^56 < 2^63
+  int64_t q = (int64_t)__float2int_rz(__fdividef(__ll2float_rn(num), __ll2float_rn(c)));
+  int64_t rem = num - q * c;
+  if (rem < 0) { --q; rem += c; }
+  else if (rem >= c) { ++q; rem -= c; }
+  exact = rem == 0;
+  return q;
+}
+
+// fractionOfCapacity [upstream, from memory]: capacity 0 counts as full; else IEEE binary64 r / c, round to nearest
+__device__ __forceinline__ double cap_fraction(int64_t r, int64_t c) {
+  return c == 0 ? 1.0 : __ddiv_rn(__ll2double_rn(r), __ll2double_rn(c));
+}
+
+struct ScoreWeights {
+  uint32_t least, most, balanced;
+};
+
+// The weighted score of one (pod, node) pair, r = non-zero requests with the pod added, c = allocatable (unscaled):
+//   least(r, c) = (c - r) * 100 / c = 100 - ceil(100 r / c),  most(r, c) = floor(100 r / c)   (0 when c == 0 or r > c)
+//   Balanced = (1 - |fc - fm|) * 100 truncated toward zero (0 when a fraction is >= 1); __double2ll_rz saturates, so a
+//   product below -2^63 (a negative allocatable) gives INT64_MIN
+// and the sum w_least * Least + w_most * Most + w_balanced * Balanced wraps in two's complement.
+__device__ __forceinline__ int64_t pair_score(int64_t r_cpu, int64_t c_cpu, int64_t r_mem, int64_t c_mem, ScoreWeights w) {
+  uint64_t s = 0;
+  if (w.least | w.most) {
+    int64_t least = 0, most = 0;
+    if (c_cpu != 0 && r_cpu <= c_cpu) {
+      bool ex;
+      const int64_t q = pct_quotient(r_cpu, c_cpu, ex);
+      most += q;
+      least += 100 - q - (ex ? 0 : 1);
+    }
+    if (c_mem != 0 && r_mem <= c_mem) {
+      bool ex;
+      const int64_t q = pct_quotient(r_mem, c_mem, ex);
+      most += q;
+      least += 100 - q - (ex ? 0 : 1);
+    }
+    s += (uint64_t)w.least * (uint64_t)(least / 2) + (uint64_t)w.most * (uint64_t)(most / 2);
+  }
+  if (w.balanced) {
+    const double fc = cap_fraction(r_cpu, c_cpu), fm = cap_fraction(r_mem, c_mem);
+    int64_t b = 0;
+    if (!(fc >= 1.0 || fm >= 1.0)) b = __double2ll_rz(__dmul_rn(__dsub_rn(1.0, fabs(__dsub_rn(fc, fm))), 100.0));
+    s += (uint64_t)w.balanced * (uint64_t)b;
+  }
+  return (int64_t)s;
+}
+
+// ---------------------------------------------------------------------------
 // K1  node_left_kernel — per node: residual capacity at percent 1.0 in the
 // sentinel form the fit kernel consumes (absent scalar lane -> ABSENT_LEFT / ABSENT_LEFT32),
 // class-independent (checkFit is applied per pod class by class_fit_kernel), split into the

@@ -1477,15 +1477,19 @@ Status BatchSchedulingPlugin::PreemptAll(std::vector<Preemption>* out) {
   return Status{};
 }
 
-Status BatchSchedulingPlugin::ReplayQueue(std::vector<ReplayDecision>* out) {
+Status BatchSchedulingPlugin::ReplayQueue(std::vector<ReplayDecision>* out, ReplayNodeChoice choice) {
   if (!out) return Status{BS_CODE_ERROR, "ReplayQueue: null output"};
   if (!eng_) return Status{BS_CODE_ERROR, "ReplayQueue: no round has been started"};
+  const bool prio = choice == ReplayNodeChoice::kPriority;
+  if (prio && !priority_k_)
+    return Status{BS_CODE_ERROR, "ReplayQueue: kPriority needs a plugin created with priority_k > 0 (its rounds upload "
+                                 "the non-zero request columns)"};
   const uint32_t P = packed_.n_pods;
   std::vector<uint8_t> pf(P), rd(P);
   std::vector<int32_t> nd(P);
   bs_replay_result r{};
   r.prefilter = pf.data(); r.node = nd.data(); r.ready = rd.data();
-  const int rc = bs_replay(eng_, order_.data(), P, &r);
+  const int rc = prio ? bs_replay_priority(eng_, order_.data(), P, &r, nullptr) : bs_replay(eng_, order_.data(), P, &r);
   if (rc) return Status{BS_CODE_ERROR, std::string("bsched: ") + bs_strerror(rc) + " (" + bs_last_error(eng_) + ")"};
   out->assign(P, ReplayDecision{});
   for (uint32_t qi = 0; qi < P; ++qi) (*out)[order_[qi]] = ReplayDecision{pf[qi], nd[qi], rd[qi] != 0, qi};

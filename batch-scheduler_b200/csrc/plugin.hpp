@@ -276,7 +276,7 @@ class BatchSchedulingPlugin {
   static uint64_t IdOf(const std::string& s);   // FNV-1a 64: uids and "ns/name"s cross the C ABI as ids
 
   // The whole pending queue of the last BeginRound walked through the reference's pod-at-a-time cycle
-  // (PreFilter against live state -> first fitting node -> assume -> Permit, core.go:88-167,268-309)
+  // (PreFilter against live state -> node choice -> assume -> Permit, core.go:88-167,268-309)
   // on the device, in the order Less defines (bs_replay; SURVEY 8(f) row 4).  A what-if: neither the
   // plugin's caches nor the uploaded tables change.  out is indexed like `pending`.
   struct ReplayDecision {
@@ -285,7 +285,14 @@ class BatchSchedulingPlugin {
     bool ready = false;       // Permit found the gang complete with this pod (core.go:303)
     uint32_t position = 0;    // place in the walked queue
   };
-  Status ReplayQueue(std::vector<ReplayDecision>* out);
+  // where the walk places a pod that passes PreFilter
+  enum class ReplayNodeChoice {
+    kFirstFit,   // the first fitting node in snapshot order (bs_replay)
+    kPriority,   // the best fitting node under the resource priorities (SetScoreWeights) on the live state
+                 // (bs_replay_priority); needs a plugin created with priority_k > 0, whose rounds upload the non-zero
+                 // request columns; otherwise ReplayQueue returns an error
+  };
+  Status ReplayQueue(std::vector<ReplayDecision>* out, ReplayNodeChoice choice = ReplayNodeChoice::kFirstFit);
 
   // results of the last round, by pending index
   const PackedSnapshot& packed() const { return packed_; }

@@ -25,13 +25,19 @@
 //                      hold a satisfying prefix and is skipped, the others are scanned exactly, in
 //                      order.  A stale first block is scanned exactly before anything else: where
 //                      the cluster has room the need is met there;
-//   node choice        first node in list order where the pod fits, the stand-in for the upstream
-//                      filter/selectHost the oracle uses too.  Requests only grow `requested`, so a
-//                      leading run of nodes no pod of the table can ever fit again (or that is
-//                      skipped) is remembered and not rescanned;
-//   assume + Permit    a handful of stores by the first lanes.
+//   node choice        bs_replay (SCORED = false): first node in list order where the pod fits, the
+//                      stand-in for the upstream filter/selectHost the oracle uses too.
+//                      bs_replay_priority (SCORED = true): every fitting node is scored with
+//                      pair_score on the live non-zero column and the best one wins (score
+//                      descending, then index ascending): each thread keeps the best of its four
+//                      nodes over the sweep, one block reduction picks the winner.  In both,
+//                      requests only grow `requested`, so a leading run of nodes no pod of the table
+//                      can ever fit again (or that is skipped) is remembered and not rescanned; such
+//                      a node never fits, so it never scores either;
+//   assume + Permit    a handful of stores by the first lanes (SCORED: the chosen node's live
+//                      non-zero column grows by the pod's, NodeInfo.AddPod's nonzeroRequest).
 // Mutable state lives in scratch copies (requested, pod_count, req_present, matched, group flags,
-// representative class, MinResources); the uploaded tables are untouched.
+// representative class, MinResources, the live non-zero column); the uploaded tables are untouched.
 #pragma once
 #include "kernels.cuh"
 
@@ -81,6 +87,10 @@ struct ReplayArgs {
   int32_t* node;              // [n_queue]
   uint8_t* ready;             // [n_queue]
   int32_t* status;            // [0]: findMaxPG would have divided by zero (core.go:716)
+  // bs_replay_priority only (SCORED): the live node column, the pod column and the weights of the node choice
+  int64_t* nz_live;           // [2][Npad] scratch copy of the uploaded node column
+  const int64_t* pod_nz;      // [2][P]
+  ScoreWeights w;
 };
 
 template <int MAXL>
@@ -199,7 +209,7 @@ __device__ __forceinline__ void block_scan(ReplaySmem<MAXL>& sm, int64_t (&v)[RE
   for (int k = 0; k < REPLAY_NPT; ++k) keys[k] |= fk;
 }
 
-template <int MAXL>
+template <int MAXL, bool SCORED>
 __global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(ReplayArgs a) {
   __shared__ ReplaySmem<MAXL> sm;
   const uint32_t tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
@@ -288,6 +298,9 @@ __global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(ReplayArgs a)
   for (uint32_t k = tid; k < 2u * REPLAY_MAX_CLASSES * (REPLAY_MAX_BLOCKS / 32); k += REPLAY_THREADS) (&sm.valid[0][0])[k] = 0;
 
   // pod columns of the NEXT step are fetched one step ahead (the walk is latency-bound)
+  // SCORED: the pod's non-zero pair (cpu, memory), one slot per step parity like sm.req; a separate array, so that the
+  // first-fit kernel's shared memory stays as it is
+  __shared__ int64_t s_pod_nz[2][2];
   struct PodRow { uint32_t p; int32_t g; uint8_t pf; uint32_t keys, rc; };
   auto load_row = [&](uint32_t qi, int slot) {
     PodRow r;
@@ -297,6 +310,8 @@ __global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(ReplayArgs a)
     const uint32_t ppres = a.pt.req_present[r.p];
     r.keys = ppres & ~0xFu;
     r.rc = a.pt.rep_class[r.p];
+    if constexpr (SCORED)
+      if (tid < 2) s_pod_nz[slot][tid] = a.pod_nz[(size_t)tid * P + r.p];
     if (tid < L)   // getPodResourceRequire (core.go:761-772): the packer summed the containers
       sm.req[slot][tid] = (tid < 4 || ((ppres >> tid) & 1u)) ? a.pt.req[(size_t)tid * P + r.p] : 0;
     return r;
@@ -582,9 +597,12 @@ __global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(ReplayArgs a)
     int32_t chosen = -1;
     uint8_t rdy = 0;
     if (code == BS_PF_PASS) {
-      // ---- node choice: first node (list order) where the pod fits, A5 at percent 1.0 ----
+      // ---- node choice among the nodes where the pod fits (A5 at percent 1.0): the first in list order, or
+      // (SCORED) the best-scoring ----
       const uint32_t rc = cur.rc;   // the pod's own (selector, tolerations) class
       const uint64_t sel = a.rsel[rc], tol = a.rtol[rc];
+      int64_t best_s = INT64_MIN;   // SCORED: this thread's best (score, node) so far; node -1 = none
+      int32_t best_n = -1;
       for (uint32_t base = lo; base < N; base += REPLAY_BLOCK) {
         int64_t v[REPLAY_NPT][MAXL];
         uint32_t keys[REPLAY_NPT], vis, tok, cf;
@@ -599,17 +617,52 @@ __global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(ReplayArgs a)
           if (((usable & cf) >> k) & 1u)
             if (compare_lanes<MAXL>(v[k], keys[k], req, req_keys)) fit |= 1u << k;
         }
-        if (__syncthreads_or(fit ? 1 : 0)) {
-          const uint32_t b = __ballot_sync(0xffffffffu, fit != 0);
-          if (b && lane == (uint32_t)(__ffs(b) - 1))
-            atomicMin(&sm.first[par], (int32_t)(base + REPLAY_NPT * tid + (uint32_t)(__ffs(fit) - 1)));
-          __syncthreads();
-          chosen = sm.first[par];
-          break;
+        if constexpr (SCORED) {
+          // nodes come in ascending order per thread: only a strictly higher score replaces the best
+          const int64_t pnz0 = s_pod_nz[par][0], pnz1 = s_pod_nz[par][1];
+#pragma unroll
+          for (int k = 0; k < REPLAY_NPT; ++k) {
+            if (!((fit >> k) & 1u)) continue;
+            const uint32_t n = base + REPLAY_NPT * tid + k;
+            const int64_t s = pair_score(a.nz_live[n] + pnz0, a.nt.alloc[n], a.nz_live[(size_t)Npad + n] + pnz1,
+                                         a.nt.alloc[(size_t)Npad + n], a.w);
+            if (best_n < 0 || s > best_s) { best_s = s; best_n = (int32_t)n; }
+          }
+        } else {
+          if (__syncthreads_or(fit ? 1 : 0)) {
+            const uint32_t b = __ballot_sync(0xffffffffu, fit != 0);
+            if (b && lane == (uint32_t)(__ffs(b) - 1))
+              atomicMin(&sm.first[par], (int32_t)(base + REPLAY_NPT * tid + (uint32_t)(__ffs(fit) - 1)));
+            __syncthreads();
+            chosen = sm.first[par];
+            break;
+          }
         }
         if (monotone && base == lo) {
           if (__syncthreads_and(dead == (1u << REPLAY_NPT) - 1u ? 1 : 0)) lo = base + REPLAY_BLOCK;
         }
+      }
+      if constexpr (SCORED) {
+        // the block's best: score descending, then node ascending (node -1 ranks last)
+        __shared__ int64_t s_best_s[REPLAY_WARPS];
+        __shared__ int32_t s_best_n[REPLAY_WARPS];
+        auto better = [](int64_t s, int32_t n, int64_t s2, int32_t n2) {
+          return n2 >= 0 && (n < 0 || s2 > s || (s2 == s && n2 < n));
+        };
+#pragma unroll
+        for (int o = 16; o; o >>= 1) {
+          const int64_t s2 = __shfl_xor_sync(0xffffffffu, best_s, o);
+          const int32_t n2 = __shfl_xor_sync(0xffffffffu, best_n, o);
+          if (better(best_s, best_n, s2, n2)) { best_s = s2; best_n = n2; }
+        }
+        if (lane == 0) { s_best_s[wid] = best_s; s_best_n[wid] = best_n; }
+        __syncthreads();
+        best_s = s_best_s[0];
+        best_n = s_best_n[0];
+#pragma unroll
+        for (int w = 1; w < REPLAY_WARPS; ++w)
+          if (better(best_s, best_n, s_best_s[w], s_best_n[w])) { best_s = s_best_s[w]; best_n = s_best_n[w]; }
+        chosen = best_n;   // uniform; the slots are rewritten only after the barrier that ends this step
       }
       if (chosen >= 0) {
         // assume: NodeInfo.AddPod adds the pod's request to `requested` (pods lane: the pod list
@@ -642,6 +695,8 @@ __global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(ReplayArgs a)
           a.req_present[n] = rp;
           a.both[n] = a.nt.alloc_present[n] & rp & ~0xFu;
         }
+        if constexpr (SCORED)   // NodeInfo.AddPod grows the node's non-zero requests by the pod's
+          if (tid >= 96 && tid < 98) a.nz_live[(size_t)(tid - 96) * Npad + n] += s_pod_nz[par][tid - 96];
         if (tid == 0) {
           // ---- Permit (core.go:268-309) ----
           if (g < 0 || (uint32_t)g >= G) {

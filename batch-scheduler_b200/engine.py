@@ -316,10 +316,13 @@ class Engine:
         return ok.astype(bool)
 
     # -- multi-round admission (SURVEY 8(f) row 4) -------------------------------------------
-    def replay(self, queue=None, after_state=True):
+    def replay(self, queue=None, after_state=True, priority=False):
         """The reference's pod-at-a-time cycle over the uploaded tables, on the device, in queue order.
         Returns a dict: prefilter / node / ready per queue position and, with after_state, the mutated
-        node and group columns (the uploaded tables themselves are left untouched)."""
+        node and group columns (the uploaded tables themselves are left untouched).
+        priority=True places each passing pod on its best node under the resource priorities on the live
+        state (bs_replay_priority; needs upload_nonzero, weights from set_score_weights) instead of the first
+        fitting one; with after_state the dict also holds the live non-zero column node_nonzero [2, N]."""
         q = None if queue is None else np.ascontiguousarray(queue, dtype=np.uint32)
         n = self.P if q is None else len(q)
         L, N, G = self.n_lanes, self.N, self.G
@@ -333,7 +336,14 @@ class Engine:
                        group_rep_tol=np.zeros(G, np.uint64))
         for k, v in out.items():
             setattr(r, k, capi.ptr(v))
-        self._check(self.lib.bs_replay(self.h, None if q is None else capi.ptr(q), n, C.byref(r)))
+        qp = None if q is None else capi.ptr(q)
+        if priority:
+            nz = np.zeros((2, N), np.int64) if after_state else None
+            self._check(self.lib.bs_replay_priority(self.h, qp, n, C.byref(r), None if nz is None else capi.ptr(nz)))
+            if after_state:
+                out["node_nonzero"] = nz
+        else:
+            self._check(self.lib.bs_replay(self.h, qp, n, C.byref(r)))
         return out
 
     # -- preemption ---------------------------------------------------------------------------

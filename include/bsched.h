@@ -374,7 +374,9 @@ int bs_cluster_check(bs_engine* e, uint64_t sel, uint64_t tol, float percent,
  * Filter/Score/selectHost the repo's oracle uses as well).  Sequential by nature: one GPU, no
  * sharding ("replicas only").
  * Outputs per queue position; the optional after-state arrays (NULL = not wanted) return the
- * mutated copies so that the caller can continue from them (bs_upload_* / bs_update_nodes). */
+ * mutated copies so that the caller can continue from them (bs_upload_* / bs_update_nodes).
+ * bs_replay_priority (below, after the resource priorities) is the same walk with kube-scheduler's
+ * node choice in place of first-fit. */
 typedef struct bs_replay_result {
   uint8_t* prefilter;          /* [n_queue] bs_prefilter_code */
   int32_t* node;               /* [n_queue] assumed node, -1 none */
@@ -460,6 +462,17 @@ int bs_upload_pod_nonzero(bs_engine* e, uint32_t n_pods, const int64_t* nz);
  * the fitting nodes of pod p ordered by score descending, then node index ascending, min(K, feasible_count[p]) of
  * them, padded with node -1 and score INT64_MIN.  Either pointer may be NULL. */
 int bs_fetch_priority_rows(bs_engine* e, uint32_t pod0, uint32_t n, int32_t* nodes, int64_t* scores);
+/* bs_replay with kube-scheduler's node choice: the same walk (PreFilter on live state, fillOccupiedObj, findMaxPG, the
+ * cluster scans, assume, Permit, the after-state), except that a passing pod goes to the node with the highest score
+ * above among the nodes where it fits on the live state (visited, Taints() ok, checkFit of its own class, every lane
+ * at percent 1.0), ties to the lower node index, -1 when none fits: entry 0 of a BS_OUT_PRIORITY list computed on the
+ * live state, with the weights of bs_set_score_weights.  Assume debits `requested` by the pod table's request as
+ * bs_replay does and adds the pod's non-zero column to the chosen node's live one; node_nonzero_after ([2][n_nodes] or
+ * NULL) returns that column.  Both non-zero columns must be uploaded (else BS_E_STATE before anything is launched;
+ * BS_OUT_PRIORITY at bs_create is not needed); they stay untouched.  BS_E_RANGE when, for either row, the column
+ * maxima give max(node) + n_queue * max(pod) > 2^62.  Timed under BS_K_REPLAY. */
+int bs_replay_priority(bs_engine* e, const uint32_t* queue, uint32_t n_queue, bs_replay_result* out,
+                       int64_t* node_nonzero_after);
 
 /* ---- preemption: PreFilterExtensions.RemovePod and the node / victims kube-scheduler's preemption would pick ----
  * The bound-pod table lists the pods already running on the snapshot's nodes (NodeInfo.Pods()).  Rows may come in

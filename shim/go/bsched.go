@@ -368,6 +368,16 @@ func (e *Engine) Replay(queue []uint32, prefilter *C.uint8_t, node *C.int32_t, r
 	return e.rc(C.bs_replay(e.h, (*C.uint32_t)(unsafe.Pointer(&queue[0])), C.uint32_t(len(queue)), &r))
 }
 
+// ReplayPriority is Replay with kube-scheduler's node choice: each passing pod goes to its best fitting node under the
+// resource priorities (SetScoreWeights) on the live state.  Both non-zero columns must be uploaded
+// (UploadNodeNonZero, UploadPodNonZero).  nodeNonZeroAfter ([2][n_nodes], C-allocated) may be nil.
+func (e *Engine) ReplayPriority(queue []uint32, prefilter *C.uint8_t, node *C.int32_t, ready *C.uint8_t,
+	nodeNonZeroAfter *C.int64_t) error {
+	r := C.bs_replay_result{prefilter: prefilter, node: node, ready: ready}
+	return e.rc(C.bs_replay_priority(e.h, (*C.uint32_t)(unsafe.Pointer(&queue[0])), C.uint32_t(len(queue)), &r,
+		nodeNonZeroAfter))
+}
+
 // ---- several GPUs: one process per GPU, groups sharded; the admit bitmaps are all-gathered over NVLink peer
 // memory at the end of every round.
 func (e *Engine) PeerInit(rank, world, words uint32) error {
