@@ -156,6 +156,8 @@ SYMBOLS = {
     "bs_upload_pod_nonzero": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p]),
     "bs_fetch_priority_rows": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p]),
     "bs_replay_priority": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, _p(ReplayResultC), C.c_void_p]),
+    "bs_set_ratio_priority": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32,
+                                        C.c_void_p, C.c_uint32]),
     "bs_peer_init": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32]),
     "bs_peer_handle": (C.c_int, [C.c_void_p, C.c_void_p]),
     "bs_peer_attach": (C.c_int, [C.c_void_p, C.c_void_p]),

@@ -404,6 +404,9 @@ struct bs_engine {
   bool have_nz_node = false, have_nz_pod = false;
   int64_t nz_node_max[2] = {0, 0}, nz_pod_max[2] = {0, 0};   // per row, of the uploaded columns (bs_replay_priority)
   ScoreWeights weights{1, 0, 1};
+  // RequestedToCapacityRatio (bs_set_ratio_priority): weight 0 = off; the shape table lives in d_ratio_tab
+  RatioSetting ratio{};
+  DevBuf d_ratio_tab;
   // sort scratch: views into one arena
   View d_gk0, d_gk1, d_pk0, d_pk1, d_idx_a, d_idx_b, d_ghist, d_group_rank, d_tilecnt, d_sort_barrier;
   uint32_t sort_max_grid = 1;
@@ -777,7 +780,8 @@ void launch_prefix(uint32_t L, NodeTab t, PrefixSel ps, PrefixScratch sc, Prefix
 
 template <int MAXL>
 void launch_replay_t(const ReplayArgs& a, bool scored, cudaStream_t s) {
-  if (scored) replay_kernel<MAXL, true><<<1, REPLAY_THREADS, 0, s>>>(a);
+  if (scored && a.ratio.weight) replay_kernel<MAXL, true, true><<<1, REPLAY_THREADS, 0, s>>>(a);
+  else if (scored) replay_kernel<MAXL, true><<<1, REPLAY_THREADS, 0, s>>>(a);
   else replay_kernel<MAXL, false><<<1, REPLAY_THREADS, 0, s>>>(a);
 }
 inline uint32_t replay_maxl(uint32_t L) { return L <= 5 ? 5u : L <= 9 ? 9u : 16u; }
@@ -1310,7 +1314,7 @@ int evaluate_async_locked(bs_engine* e) {
     }
   }
   if (P && (e->out_flags & BS_OUT_PRIORITY)) {
-    PriorityArgs pa;
+    PriorityRatioArgs pa;
     pa.left = e->d_left_full.as<int64_t>();
     pa.left_present = e->d_left_present.as<uint32_t>();
     pa.gate = e->d_reason_gate.as<uint32_t>();
@@ -1324,10 +1328,21 @@ int evaluate_async_locked(bs_engine* e) {
     pa.out_score = e->d_prio_score.as<int64_t>();
     pa.w = e->weights;
     pa.P = P; pa.N = e->N; pa.Npad = e->Npad; pa.Wg = e->Npad / 32; pa.L = L; pa.K = e->topk;
+    pa.node_requested = e->d_requested.as<int64_t>();
+    pa.node_alloc_present = e->d_apres.as<uint32_t>();
+    pa.node_req_present = e->d_rpres.as<uint32_t>();
+    pa.ratio = e->ratio;
     const uint32_t grid = cdiv(P, PRIO_PODS_PER_CTA);
-    if (L <= 5) priority_pod_kernel<5><<<grid, PRIO_THREADS, 0, e->s>>>(pa);
-    else if (L <= 9) priority_pod_kernel<9><<<grid, PRIO_THREADS, 0, e->s>>>(pa);
-    else priority_pod_kernel<16><<<grid, PRIO_THREADS, 0, e->s>>>(pa);
+    if (e->ratio.weight) {
+      if (L <= 5) priority_pod_kernel<5, true><<<grid, PRIO_THREADS, 0, e->s>>>(pa);
+      else if (L <= 9) priority_pod_kernel<9, true><<<grid, PRIO_THREADS, 0, e->s>>>(pa);
+      else priority_pod_kernel<16, true><<<grid, PRIO_THREADS, 0, e->s>>>(pa);
+    } else {
+      const PriorityArgs& pb = pa;
+      if (L <= 5) priority_pod_kernel<5, false><<<grid, PRIO_THREADS, 0, e->s>>>(pb);
+      else if (L <= 9) priority_pod_kernel<9, false><<<grid, PRIO_THREADS, 0, e->s>>>(pb);
+      else priority_pod_kernel<16, false><<<grid, PRIO_THREADS, 0, e->s>>>(pb);
+    }
     e->launches += 1;
   }
   if (e->peer_attached) {
@@ -2406,6 +2421,7 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
     a.nz_live = n_nz.as<int64_t>();
     a.pod_nz = e->d_nz_pod.as<int64_t>();
     a.w = e->weights;
+    a.ratio = e->ratio;
   }
   {
     StageTimer tm(e, BS_K_REPLAY, e->s);
@@ -2839,6 +2855,54 @@ int bs_set_score_weights(bs_engine* e, uint32_t least, uint32_t most, uint32_t b
   if (!e) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
   e->weights = ScoreWeights{least, most, balanced};
+  return BS_OK;
+}
+
+int bs_set_ratio_priority(bs_engine* e, uint32_t weight, uint32_t n_points, const uint32_t* utilization,
+                          const uint32_t* score, uint32_t n_lanes, const uint32_t* lane_weight, uint32_t absent_weight) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  const char* who = "bs_set_ratio_priority";
+  auto bad = [&](const char* why) { return fail(e, BS_E_INVAL, (std::string(who) + ": " + why).c_str()); };
+  if (n_points < 1 || n_points > (uint32_t)RATIO_TABLE) return bad("the shape needs 1 to 101 points");
+  if (!utilization || !score || !lane_weight) return bad("null argument");
+  for (uint32_t i = 0; i < n_points; ++i) {
+    if (utilization[i] > 100 || score[i] > 100) return bad("utilization and score lie in [0, 100]");
+    if (i && utilization[i] <= utilization[i - 1]) return bad("utilization must be strictly ascending");
+  }
+  if (n_lanes != e->L) return bad("n_lanes differs from the engine's");
+  if (lane_weight[LANE_PODS]) return bad("lane 3 (pods) must weigh 0: pass its weight in absent_weight");
+  uint64_t sum = absent_weight;
+  for (uint32_t d = 0; d < n_lanes; ++d) sum += lane_weight[d];
+  if (sum > (1u << 24)) return bad("the weights sum to more than 2^24");
+  // buildBrokenLinearFunction [upstream, from memory] at every utilization 0..100, int64 truncating toward zero
+  int32_t tab[RATIO_TABLE];
+  for (int64_t p = 0; p < RATIO_TABLE; ++p) {
+    int64_t v = score[n_points - 1];
+    for (uint32_t i = 0; i < n_points; ++i) {
+      if (p > (int64_t)utilization[i]) continue;
+      if (i == 0) v = score[0];
+      else {
+        const int64_t s0 = score[i - 1], s1 = score[i], u0 = utilization[i - 1], u1 = utilization[i];
+        v = s0 + (s1 - s0) * (p - u0) / (u1 - u0);
+      }
+      break;
+    }
+    tab[p] = (int32_t)v;
+  }
+  BS_DEVICE_GUARD(e);
+  CK(e->d_ratio_tab.ensure(sizeof tab));
+  CK(cudaMemcpyAsync(e->d_ratio_tab.p, tab, sizeof tab, cudaMemcpyHostToDevice, e->s));
+  CK(cudaStreamSynchronize(e->s));
+  RatioSetting r{};
+  r.table = e->d_ratio_tab.as<int32_t>();
+  for (uint32_t d = 0; d < n_lanes; ++d) {
+    r.lane_w[d] = lane_weight[d];
+    if (lane_weight[d]) r.mask |= 1u << d;
+  }
+  r.weight = weight;
+  if (tab[100] > 0) { r.num0 = (uint32_t)tab[100] * absent_weight; r.den0 = absent_weight; }
+  e->ratio = r;
   return BS_OK;
 }
 

@@ -180,6 +180,67 @@ __device__ __forceinline__ int64_t pair_score(int64_t r_cpu, int64_t c_cpu, int6
   return (int64_t)s;
 }
 
+// kube-scheduler v1.17's RequestedToCapacityRatio priority (include/bsched.h bs_set_ratio_priority, DESIGN.md §2).
+// The shape is expanded once on the host into table[u] = shape(u), u = 0..100; the kernels copy it to shared memory
+// (the index varies per thread: constant memory would serialize the reads).
+constexpr int RATIO_TABLE = 101;
+struct RatioSetting {
+  const int32_t* table;             // [RATIO_TABLE] in device memory
+  uint32_t lane_w[BS_MAX_LANES];    // weight per lane, 0 = not scored (lane 3 and lanes >= L are always 0)
+  uint32_t mask;                    // lanes with a non-zero weight
+  uint32_t weight;                  // the priority's weight in the total
+  uint32_t num0, den0;              // the resources with capacity 0 everywhere: shape(100) * absent_weight and
+                                    // absent_weight, or 0 and 0 when shape(100) == 0
+};
+
+// One resource's score shape(util) [upstream, from memory]:
+//   util = c == 0 || r > c ? 100 : 100 - (c - r) * 100 / c     (int64, wrapping, division truncating toward zero)
+// For 0 <= r <= c (so 0 < c <= 2^56) that is ceil(100 r / c) = q + (exact ? 0 : 1) with pct_quotient's q.  Any
+// other pair (r < 0, which also covers c < 0) takes the exact path in Go's wrapping arithmetic; it is rare.
+// The clamp to [0, 100] before the lookup is exact: util < 0 lies below the first point, whose utilization is >= 0,
+// so shape gives s_0 = shape(0); util > 100 lies above the last point, so shape gives the last score = shape(100).
+__device__ __forceinline__ int32_t ratio_lane_score(const int32_t* tab, int64_t r, int64_t c) {
+  int64_t util = 100;
+  if (c != 0 && r <= c) {
+    if (r >= 0) {
+      bool ex;
+      const int64_t q = pct_quotient(r, c, ex);
+      util = q + (ex ? 0 : 1);
+    } else {
+      const int64_t prod = (int64_t)(((uint64_t)c - (uint64_t)r) * 100u);
+      const int64_t q = c == -1 ? (int64_t)(0 - (uint64_t)prod) : prod / c;   // Go: x / -1 wraps, never traps
+      util = (int64_t)(100u - (uint64_t)q);
+    }
+  }
+  return tab[util < 0 ? 0 : util > 100 ? 100 : util];
+}
+
+// Adds one weighted resource to the average: a resource that scores 0 drops out (upstream's resourceScore > 0).
+__device__ __forceinline__ void ratio_accumulate(int32_t s, uint32_t w, uint32_t& num, uint32_t& den) {
+  if (s > 0) { num += (uint32_t)s * w; den += w; }
+}
+
+// Ratio = math.Round(float64(num) / float64(den)), 0 when den == 0.  With den <= 2^24 and num <= 100 den, this is
+// floor((2 num + den) / (2 den)): num and den are exact in binary64, and the rounded quotient is within 100 * 2^-53
+// of num / den, while a quotient that is not a half-integer lies at least 1 / (2 den) >= 2^-25 from one; so the
+// binary64 quotient sits on the same side of every half-integer as the exact one, and an exact half-integer rounds
+// away from zero in both.  The division: a float32 estimate (relative error below 2^-21, quotient <= 100.5) is the
+// quotient or one off, and one exact remainder test corrects it, as in pct_quotient.
+__device__ __forceinline__ int64_t ratio_round(uint32_t num, uint32_t den) {
+  if (!den) return 0;
+  const int64_t x = 2 * (int64_t)num + den, y = 2 * (int64_t)den;
+  int64_t q = (int64_t)__float2int_rz(__fdividef(__ll2float_rn(x), __ll2float_rn(y)));
+  const int64_t rem = x - q * y;
+  if (rem < 0) --q;
+  else if (rem >= y) ++q;
+  return q;
+}
+
+// weight * Ratio as the unsigned addend of a score (the total wraps in two's complement)
+__device__ __forceinline__ uint64_t ratio_term(uint32_t weight, uint32_t num, uint32_t den) {
+  return (uint64_t)weight * (uint64_t)ratio_round(num, den);
+}
+
 // ---------------------------------------------------------------------------
 // K1  node_left_kernel — per node: residual capacity at percent 1.0 in the
 // sentinel form the fit kernel consumes (absent scalar lane -> ABSENT_LEFT / ABSENT_LEFT32),

@@ -1116,6 +1116,54 @@ void BatchSchedulingPlugin::SetScoreWeights(uint32_t least, uint32_t most, uint3
   if (eng_) bs_set_score_weights(eng_, least, most, balanced);
 }
 
+Status BatchSchedulingPlugin::SetRatioPriority(uint32_t weight, const std::vector<std::pair<uint32_t, uint32_t>>& shape,
+                                               const std::map<std::string, uint32_t>& resources) {
+  std::lock_guard<std::mutex> lk(mu_);
+  auto bad = [](const std::string& why) { return Status{BS_CODE_ERROR, "SetRatioPriority: " + why}; };
+  if (shape.empty() || shape.size() > 101) return bad("the shape needs 1 to 101 points");
+  std::vector<uint32_t> util, score;
+  for (size_t i = 0; i < shape.size(); ++i) {
+    if (shape[i].first > 100 || shape[i].second > 10) return bad("utilization lies in 0..100 and score in 0..10");
+    if (i && shape[i].first <= shape[i - 1].first) return bad("utilization must be strictly ascending");
+    util.push_back(shape[i].first);
+    score.push_back(shape[i].second * 10);   // MaxNodeScore / MaxCustomPriorityScore
+  }
+  for (auto& kv : resources)
+    if (kv.second < 1 || kv.second > 100) return bad("resource weights lie in 1..100 (" + kv.first + ")");
+  const uint32_t old_weight = ratio_weight_;
+  std::vector<uint32_t> old_util = ratio_util_, old_score = ratio_score_;
+  std::map<std::string, uint32_t> old_res = ratio_resources_;
+  ratio_weight_ = weight;
+  ratio_util_ = util;
+  ratio_score_ = score;
+  ratio_resources_ = resources.empty() ? std::map<std::string, uint32_t>{{"cpu", 1}, {"memory", 1}} : resources;
+  const int rc = eng_ ? PushRatio() : BS_OK;
+  if (rc) {
+    ratio_weight_ = old_weight; ratio_util_ = old_util; ratio_score_ = old_score; ratio_resources_ = old_res;
+    return Status{BS_CODE_ERROR, std::string("bsched: ") + bs_strerror(rc) + " (" + bs_last_error(eng_) + ")"};
+  }
+  return Status{};
+}
+
+int BatchSchedulingPlugin::PushRatio() {
+  const uint32_t L = eng_lanes_;
+  std::vector<uint32_t> lane_w(L, 0);
+  uint32_t absent = 0;
+  for (auto& kv : ratio_resources_) {
+    int lane = -1;
+    if (kv.first == "cpu") lane = 0;
+    else if (kv.first == "memory") lane = 1;
+    else if (kv.first == "ephemeral-storage") lane = 2;
+    else
+      for (size_t k = 0; k < packed_.scalar_names.size(); ++k)
+        if (packed_.scalar_names[k] == kv.first && 4 + k < L) lane = (int)(4 + k);
+    if (lane < 0) absent += kv.second;   // `pods` and names without a lane: capacity 0 on every node
+    else lane_w[lane] += kv.second;
+  }
+  return bs_set_ratio_priority(eng_, ratio_weight_, (uint32_t)ratio_util_.size(), ratio_util_.data(), ratio_score_.data(),
+                               L, lane_w.data(), absent);
+}
+
 namespace {
 // GetNonzeroRequestForResource [upstream, from memory]: the Requests' cpu (MilliValue) / memory (Value), 100 m /
 // 200 MiB when the key is absent; a key listed twice counts its last entry, as a map assignment would
@@ -1174,6 +1222,7 @@ Status BatchSchedulingPlugin::UploadNonZero(const std::vector<const Pod*>* pendi
   int rc = bs_upload_node_nonzero(eng_, (uint32_t)snapshot_.size(), node_nz.data());
   if (!rc && pending) rc = bs_upload_pod_nonzero(eng_, (uint32_t)pending->size(), pod_nz.data());
   if (!rc) rc = bs_set_score_weights(eng_, weights_[0], weights_[1], weights_[2]);
+  if (!rc) rc = PushRatio();   // the lanes of this round's scalar resources
   if (rc) return Status{BS_CODE_ERROR, std::string("bsched: ") + bs_strerror(rc) + " (" + bs_last_error(eng_) + ")"};
   return Status{};
 }

@@ -316,6 +316,15 @@ class BatchSchedulingPlugin {
   // weights of NodeResourcesLeastAllocated, NodeResourcesMostAllocated and NodeResourcesBalancedAllocation (default
   // 1, 0, 1), from the next round or delta round on
   void SetScoreWeights(uint32_t least, uint32_t most, uint32_t balanced);
+  // kube-scheduler v1.17's RequestedToCapacityRatio priority (bs_set_ratio_priority), added to PriorityNodes and
+  // ReplayQueue(kPriority) with `weight` (0 = off, the default), from the next round or delta round on.  `shape` holds
+  // (utilization 0..100, score 0..10) points as the policy file gives them, utilization strictly ascending; the scores
+  // are multiplied by 10 (MaxNodeScore / MaxCustomPriorityScore).  `resources` maps a resource name to a weight in
+  // 1..100; empty means cpu 1, memory 1.  Every round maps the names onto its lanes: cpu, memory and ephemeral-storage
+  // to lanes 0-2, a scalar resource of the round to its lane, and `pods` or a name no node of the round carries to the
+  // weight of resources with capacity 0 everywhere.  An invalid setting returns an error and the previous one stays.
+  Status SetRatioPriority(uint32_t weight, const std::vector<std::pair<uint32_t, uint32_t>>& shape,
+                          const std::map<std::string, uint32_t>& resources);
   int group_index(const std::string& ns_name) const;
   double last_pack_ms() const { return last_pack_ms_; }
   double last_device_ms() const { return last_device_ms_; }
@@ -405,6 +414,9 @@ class BatchSchedulingPlugin {
   int device_ = 0;
   uint32_t out_flags_ = 0, eng_lanes_ = 0, topk_ = 0, priority_k_ = 0;
   uint32_t weights_[3] = {1, 0, 1};
+  uint32_t ratio_weight_ = 0;                          // SetRatioPriority: shape in engine units, weights by name
+  std::vector<uint32_t> ratio_util_{0, 100}, ratio_score_{100, 0};
+  std::map<std::string, uint32_t> ratio_resources_{{"cpu", 1}, {"memory", 1}};
   std::string init_error_;
   int64_t max_schedule_time_ns_;
   std::map<std::string, GroupState> groups_;                        // ordered: canonical table order
@@ -432,6 +444,7 @@ class BatchSchedulingPlugin {
   Status Reevaluate();   // bs_evaluate into the round's result vectors + the deny side effect (core.go:142,163)
   int FetchTopK();       // the round's top-K lists into topk_node_ / topk_score_ (no-op without topk)
   int FetchReasons();    // the round's reason rows into reasons_ (no-op without BS_OUT_REASONS)
+  int PushRatio();      // the ratio setting with this round's lane mapping (bs_set_ratio_priority)
   int FetchPriority();   // the round's priority lists into prio_node_ / prio_score_ (no-op without priority_k)
   Status UploadNonZero(const std::vector<const Pod*>* pending);   // node column of snapshot_ (+ the pods'); no-op without
                                                                   // priority_k

@@ -4,10 +4,13 @@
 //
 // The fit set is the reason rows' (kernels.cuh K1c/K1d): a node fits a pod when its class gate bit is set and no lane
 // is short (lane_short over node_left_kernel's full-width residuals), the invariant DESIGN §2 states for reason rows.
-// The lists are kept with gang_fit's topk_insert (fit.cuh); the pair scorer pair_score is kernels.cuh's.
+// The lists are kept with gang_fit's topk_insert (fit.cuh); the pair scorer pair_score is kernels.cuh's, and with RATIO
+// the RequestedToCapacityRatio term (kernels.cuh ratio_*) is added to it.
 #pragma once
 #include "kernels.cuh"
 #include "fit.cuh"
+
+#include <type_traits>
 
 namespace bsk {
 
@@ -17,7 +20,9 @@ namespace bsk {
 // entries per pod ordered by score descending, then node ascending; unfilled entries are (INT64_MIN, PRIO_EMPTY) and
 // rank after every real entry, including one that scores INT64_MIN.  A fitting pair is a candidate while the list has
 // fewer than K fitting nodes, or when it beats the score of entry K-1: nodes come in ascending order, so a later node
-// never displaces an equal score.  MAXL bounds the lanes held in registers (5, 9 or 16).
+// never displaces an equal score.  MAXL bounds the lanes held in registers (5, 9 or 16).  RATIO (chosen by the host
+// when the ratio weight is non-zero) adds w_ratio * Ratio to each score; the node's columns of a weighted lane are read
+// once per 32-node step and shared by the warp's pods.
 constexpr int PRIO_THREADS = 256;
 constexpr int PRIO_PPW = 4;                                           // pods per warp
 constexpr int PRIO_PODS_PER_CTA = (PRIO_THREADS / 32) * PRIO_PPW;
@@ -37,12 +42,28 @@ struct PriorityArgs {
   ScoreWeights w;
   uint32_t P, N, Npad, Wg, L, K;
 };
-template <int MAXL>
-__global__ void __launch_bounds__(PRIO_THREADS) priority_pod_kernel(PriorityArgs a) {
+// RATIO's arguments: also the node table's requested and key masks, and the setting.  A separate type, so that the
+// kernel without the ratio term keeps its parameter block (a larger one changed its SASS).
+struct PriorityRatioArgs : PriorityArgs {
+  const int64_t* node_requested;        // [L][Npad]
+  const uint32_t* node_alloc_present;   // [Npad]
+  const uint32_t* node_req_present;     // [Npad]
+  RatioSetting ratio;
+};
+template <int MAXL, bool RATIO>
+__global__ void __launch_bounds__(PRIO_THREADS)
+priority_pod_kernel(std::conditional_t<RATIO, PriorityRatioArgs, PriorityArgs> a) {
   constexpr int WARPS = PRIO_THREADS / 32;
   __shared__ int64_t s_req[WARPS][PRIO_PPW][MAXL];
   __shared__ int64_t s_ls[WARPS][PRIO_PPW][32];
   __shared__ int32_t s_ln[WARPS][PRIO_PPW][32];
+  [[maybe_unused]] const int32_t* tab = nullptr;   // RATIO: shape(util) in shared memory
+  if constexpr (RATIO) {
+    __shared__ int32_t s_tab[RATIO_TABLE];
+    for (uint32_t k = threadIdx.x; k < (uint32_t)RATIO_TABLE; k += PRIO_THREADS) s_tab[k] = a.ratio.table[k];
+    __syncthreads();
+    tab = s_tab;
+  }
   const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const uint32_t p0 = (blockIdx.x * WARPS + wid) * PRIO_PPW;
   const int L = (int)a.L;
@@ -101,10 +122,39 @@ __global__ void __launch_bounds__(PRIO_THREADS) priority_pod_kernel(PriorityArgs
     if (!anyfit) continue;
     const int64_t c_cpu = a.alloc[i], c_mem = a.alloc[(size_t)a.Npad + i];
     const int64_t n_cpu = a.node_nz[i], n_mem = a.node_nz[(size_t)a.Npad + i];
+    [[maybe_unused]] uint32_t rnum[PRIO_PPW], rden[PRIO_PPW];   // RATIO: the weighted sum and weight sum of each pod's average
+    if constexpr (RATIO) {
+#pragma unroll
+      for (int j = 0; j < PRIO_PPW; ++j) { rnum[j] = a.ratio.num0; rden[j] = a.ratio.den0; }
+      const uint32_t ap = a.node_alloc_present[i], rp = a.node_req_present[i];
+#pragma unroll
+      for (int d = 0; d < MAXL; ++d) {
+        const uint32_t wd = a.ratio.lane_w[d];
+        if (!wd) continue;   // uniform; lanes 3 and >= L weigh 0
+        // capacity and the node's term: cpu / memory from the non-zero column; lane 2 and the scalar lanes from the
+        // node table, 0 for a key the node lacks
+        int64_t c, rn;
+        if (d == LANE_CPU) { c = c_cpu; rn = n_cpu; }
+        else if (d == LANE_MEM) { c = c_mem; rn = n_mem; }
+        else {
+          c = (d < 4 || ((ap >> d) & 1u)) ? a.alloc[(size_t)d * a.Npad + i] : 0;
+          rn = (d < 4 || ((rp >> d) & 1u)) ? a.node_requested[(size_t)d * a.Npad + i] : 0;
+        }
+#pragma unroll
+        for (int j = 0; j < PRIO_PPW; ++j) {
+          if (!fw[j]) continue;   // warp-uniform
+          const int64_t rq = d == LANE_CPU ? nz_cpu[j] : d == LANE_MEM ? nz_mem[j]
+                                                       : (((rmask[j] >> d) & 1u) ? s_req[wid][j][d] : 0);
+          ratio_accumulate(ratio_lane_score(tab, (int64_t)((uint64_t)rn + (uint64_t)rq), c), wd, rnum[j], rden[j]);
+        }
+      }
+    }
 #pragma unroll
     for (int j = 0; j < PRIO_PPW; ++j) {
       if (!fw[j]) continue;   // warp-uniform
-      const int64_t s = g[j] ? pair_score(n_cpu + nz_cpu[j], c_cpu, n_mem + nz_mem[j], c_mem, a.w) : INT64_MIN;
+      int64_t s = g[j] ? pair_score(n_cpu + nz_cpu[j], c_cpu, n_mem + nz_mem[j], c_mem, a.w) : INT64_MIN;
+      if constexpr (RATIO)
+        if (g[j]) s = (int64_t)((uint64_t)s + ratio_term(a.ratio.weight, rnum[j], rden[j]));
       const uint32_t cb = __ballot_sync(0xffffffffu, g[j] && (nfit[j] < a.K || s > thr[j]));
       if (cb) thr[j] = topk_insert<int64_t>(s_ls[wid][j], s_ln[wid][j], a.K, cb, s, (int32_t)base, lane);
       nfit[j] += __popc(fw[j]);

@@ -30,7 +30,9 @@
 //                      bs_replay_priority (SCORED = true): every fitting node is scored with
 //                      pair_score on the live non-zero column and the best one wins (score
 //                      descending, then index ascending): each thread keeps the best of its four
-//                      nodes over the sweep, one block reduction picks the winner.  In both,
+//                      nodes over the sweep, one block reduction picks the winner.  RATIO (a non-zero
+//                      bs_set_ratio_priority weight) adds the RequestedToCapacityRatio term over the
+//                      live `requested` and key mask (lanes >= 2) and the live non-zero column.  In both,
 //                      requests only grow `requested`, so a leading run of nodes no pod of the table
 //                      can ever fit again (or that is skipped) is remembered and not rescanned; such
 //                      a node never fits, so it never scores either;
@@ -91,6 +93,7 @@ struct ReplayArgs {
   int64_t* nz_live;           // [2][Npad] scratch copy of the uploaded node column
   const int64_t* pod_nz;      // [2][P]
   ScoreWeights w;
+  RatioSetting ratio;         // RATIO only
 };
 
 template <int MAXL>
@@ -209,9 +212,11 @@ __device__ __forceinline__ void block_scan(ReplaySmem<MAXL>& sm, int64_t (&v)[RE
   for (int k = 0; k < REPLAY_NPT; ++k) keys[k] |= fk;
 }
 
-template <int MAXL, bool SCORED>
+template <int MAXL, bool SCORED, bool RATIO = false>
 __global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(ReplayArgs a) {
+  static_assert(SCORED || !RATIO, "the ratio term belongs to the scored node choice");
   __shared__ ReplaySmem<MAXL> sm;
+  __shared__ int32_t s_tab[RATIO_TABLE];   // RATIO: shape(util)
   const uint32_t tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   const uint32_t N = a.nt.N, Npad = a.nt.Npad, G = a.G, P = a.pt.P;
   const uint32_t L = a.nt.L;
@@ -316,6 +321,8 @@ __global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(ReplayArgs a)
       sm.req[slot][tid] = (tid < 4 || ((ppres >> tid) & 1u)) ? a.pt.req[(size_t)tid * P + r.p] : 0;
     return r;
   };
+  if constexpr (RATIO)
+    for (uint32_t k = tid; k < (uint32_t)RATIO_TABLE; k += REPLAY_THREADS) s_tab[k] = a.ratio.table[k];
   if (tid == 0) { sm.first[0] = 0x7fffffff; sm.first[1] = 0x7fffffff; sm.panic = 0; }
   if (tid < MAXL) { sm.req[0][tid] = 0; sm.req[1][tid] = 0; sm.need[tid] = 0; }
   __syncthreads();
@@ -624,8 +631,30 @@ __global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(ReplayArgs a)
           for (int k = 0; k < REPLAY_NPT; ++k) {
             if (!((fit >> k) & 1u)) continue;
             const uint32_t n = base + REPLAY_NPT * tid + k;
-            const int64_t s = pair_score(a.nz_live[n] + pnz0, a.nt.alloc[n], a.nz_live[(size_t)Npad + n] + pnz1,
-                                         a.nt.alloc[(size_t)Npad + n], a.w);
+            const int64_t r_cpu = a.nz_live[n] + pnz0, r_mem = a.nz_live[(size_t)Npad + n] + pnz1;
+            const int64_t c_cpu = a.nt.alloc[n], c_mem = a.nt.alloc[(size_t)Npad + n];
+            int64_t s = pair_score(r_cpu, c_cpu, r_mem, c_mem, a.w);
+            if constexpr (RATIO) {
+              // lanes >= 2: the live requested and key mask (assume grows them) plus the pod's request, which
+              // sm.req already holds as 0 for a key the pod lacks
+              uint32_t num = a.ratio.num0, den = a.ratio.den0;
+              const uint32_t ap = a.nt.alloc_present[n], rp = a.req_present[n];
+#pragma unroll
+              for (int d = 0; d < MAXL; ++d) {
+                const uint32_t wd = a.ratio.lane_w[d];
+                if (!wd) continue;   // uniform; lanes 3 and >= L weigh 0
+                int64_t r, c;
+                if (d == LANE_CPU) { r = r_cpu; c = c_cpu; }
+                else if (d == LANE_MEM) { r = r_mem; c = c_mem; }
+                else {
+                  c = (d < 4 || ((ap >> d) & 1u)) ? a.nt.alloc[(size_t)d * Npad + n] : 0;
+                  const int64_t rn = (d < 4 || ((rp >> d) & 1u)) ? a.requested[(size_t)d * Npad + n] : 0;
+                  r = (int64_t)((uint64_t)rn + (uint64_t)req[d]);
+                }
+                ratio_accumulate(ratio_lane_score(s_tab, r, c), wd, num, den);
+              }
+              s = (int64_t)((uint64_t)s + (uint64_t)a.ratio.weight * (uint64_t)ratio_round(num, den));
+            }
             if (best_n < 0 || s > best_s) { best_s = s; best_n = (int32_t)n; }
           }
         } else {

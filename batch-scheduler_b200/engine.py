@@ -270,6 +270,21 @@ class Engine:
         """Weights of LeastAllocated, MostAllocated and BalancedAllocation for the next rounds (default 1, 0, 1)."""
         self._check(self.lib.bs_set_score_weights(self.h, least, most, balanced))
 
+    def set_ratio_priority(self, weight: int, shape, lane_weights, absent_weight: int = 0):
+        """kube-scheduler's RequestedToCapacityRatio priority, added to the priority score with `weight` (0 = off).
+        shape: (utilization, score) pairs in engine units (both 0..100, utilization strictly ascending); lane_weights:
+        one weight per lane (lane 3 must be 0); absent_weight: the weights of resources no node has.  Read by the next
+        rounds' priority lists and by replay(priority=True)."""
+        pts = np.asarray(shape, dtype=np.int64).reshape(-1, 2)
+        lw = np.asarray(lane_weights, dtype=np.int64).reshape(-1)
+        if (pts < 0).any() or (pts > 0xFFFFFFFF).any() or (lw < 0).any() or (lw > 0xFFFFFFFF).any():
+            raise ValueError("shape points and lane weights are unsigned 32-bit values")
+        util = np.ascontiguousarray(pts[:, 0], dtype=np.uint32)
+        score = np.ascontiguousarray(pts[:, 1], dtype=np.uint32)
+        lw = np.ascontiguousarray(lw, dtype=np.uint32)
+        self._check(self.lib.bs_set_ratio_priority(self.h, weight, len(util), capi.ptr(util), capi.ptr(score), len(lw),
+                                                   capi.ptr(lw), absent_weight))
+
     def upload_nonzero(self, node=None, pods=None):
         """The non-zero request columns: node [2, N] and/or pods [2, P] int64 (row 0 cpu millicores, row 1 memory
         bytes).  Uploading nodes (or updating node rows) drops the node column, uploading pods the pod column."""

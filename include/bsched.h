@@ -473,6 +473,25 @@ int bs_fetch_priority_rows(bs_engine* e, uint32_t pod0, uint32_t n, int32_t* nod
  * maxima give max(node) + n_queue * max(pod) > 2^62.  Timed under BS_K_REPLAY. */
 int bs_replay_priority(bs_engine* e, const uint32_t* queue, uint32_t n_queue, bs_replay_result* out,
                        int64_t* node_nonzero_after);
+/* kube-scheduler v1.17's RequestedToCapacityRatio priority, added to the BS_OUT_PRIORITY score with weight `weight`
+ * (0 = off, the default).  Shape: n_points (1..101) points, utilization strictly ascending in [0, 100], score in
+ * [0, 100] (node-score units).  lane_weight[n_lanes] (n_lanes = the engine's), lane 3 must be 0; absent_weight = the
+ * weights of resources with capacity 0 on every node.  Sum of lane weights + absent_weight <= 2^24.  Else BS_E_INVAL,
+ * and the previous setting stays.  Read by the next evaluation and by bs_replay_priority.
+ * Per (pod p, node n) and weighted lane d [upstream, from memory]:
+ *     c = alloc[d][n] (unscaled); r = node_nz[n] + pod_nz[p] on lanes 0-1, requested[d][n] + req[d][p] on lane 2 and
+ *         the scalar lanes, a scalar key absent on a side counting 0 there (alloc_present / req_present); the pod side
+ *         is the pod table's request (Limits else Requests), which for extended resources and hugepages equals
+ *         Requests
+ *     util = c == 0 || r > c ? 100 : 100 - (c - r) * 100 / c     (int64, wrapping, truncating toward zero)
+ *     s_d = shape(util): s_0 at or below u_0, s_last above the last point, else on the segment u_{i-1} < util <= u_i
+ *           s_{i-1} + (s_i - s_{i-1}) * (util - u_{i-1}) / (u_i - u_{i-1})  (int64, truncating toward zero)
+ *     Ratio = round(sum s_d * w_d / sum w_d) over the resources with s_d > 0 (half away from zero; 0 without any);
+ *             absent_weight joins both sums with s = shape(100) when shape(100) > 0
+ *     score = w_least * Least + w_most * Most + w_balanced * Balanced + weight * Ratio   (int64, two's complement wrap)
+ * v1.17's policy file gives shape scores in 0..10 and the scheduler multiplies them by 10: the caller scales. */
+int bs_set_ratio_priority(bs_engine* e, uint32_t weight, uint32_t n_points, const uint32_t* utilization,
+                          const uint32_t* score, uint32_t n_lanes, const uint32_t* lane_weight, uint32_t absent_weight);
 
 /* ---- preemption: PreFilterExtensions.RemovePod and the node / victims kube-scheduler's preemption would pick ----
  * The bound-pod table lists the pods already running on the snapshot's nodes (NodeInfo.Pods()).  Rows may come in

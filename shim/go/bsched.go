@@ -159,6 +159,34 @@ func (e *Engine) SetScoreWeights(least, most, balanced uint32) error {
 	return e.rc(C.bs_set_score_weights(e.h, C.uint32_t(least), C.uint32_t(most), C.uint32_t(balanced)))
 }
 
+// RatioPoint is one point of a RequestedToCapacityRatio shape in engine units: utilization and score both 0..100.
+type RatioPoint struct{ Utilization, Score uint32 }
+
+// SetRatioPriority adds kube-scheduler's RequestedToCapacityRatio priority to the priority score with weight `weight`
+// (0 = off).  The v1.17 policy file gives shape scores in 0..10: multiply them by 10 before calling.  laneWeights has
+// one weight per lane of the engine (lane 3, pods, must be 0); absentWeight is the weight of the resources no node of
+// the round has (pods and names that are not a lane of the round).  An invalid setting keeps the previous one.
+func (e *Engine) SetRatioPriority(weight uint32, shape []RatioPoint, laneWeights []uint32, absentWeight uint32) error {
+	util := make([]C.uint32_t, len(shape))
+	score := make([]C.uint32_t, len(shape))
+	for i, p := range shape {
+		util[i], score[i] = C.uint32_t(p.Utilization), C.uint32_t(p.Score)
+	}
+	lw := make([]C.uint32_t, len(laneWeights))
+	for i, w := range laneWeights {
+		lw[i] = C.uint32_t(w)
+	}
+	var up, sp, lp *C.uint32_t
+	if len(shape) > 0 {
+		up, sp = &util[0], &score[0]
+	}
+	if len(lw) > 0 {
+		lp = &lw[0]
+	}
+	return e.rc(C.bs_set_ratio_priority(e.h, C.uint32_t(weight), C.uint32_t(len(shape)), up, sp, C.uint32_t(len(lw)), lp,
+		C.uint32_t(absentWeight)))
+}
+
 // UploadNodeNonZero / UploadPodNonZero: the non-zero request columns, nz[2][n] (cpu millicores, then memory bytes):
 // per pod the sum over its containers of GetNonzeroRequestForResource(Requests), per node NodeInfo.NonZeroRequest().
 // UploadNodes / UpdateNodes drop the node column and UploadPods the pod column: upload them again before Evaluate.
