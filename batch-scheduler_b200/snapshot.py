@@ -74,6 +74,11 @@ class NodeTable:
     def copy(self):
         return NodeTable(*(getattr(self, f).copy() for f in self.__dataclass_fields__))
 
+    def take(self, idx):
+        idx = np.asarray(idx)
+        return NodeTable(self.alloc[:, idx], self.requested[:, idx], self.pod_count[idx], self.alloc_present[idx],
+                         self.req_present[idx], self.label_mask[idx], self.taint_mask[idx], self.flags[idx])
+
 
 @dataclass
 class PodTable:
@@ -170,6 +175,13 @@ class GroupTable:
 
     def copy(self):
         return GroupTable(*(None if getattr(self, f) is None else getattr(self, f).copy() for f in self.__dataclass_fields__))
+
+    def take(self, idx):
+        idx = np.asarray(idx)
+        return GroupTable(self.min_member[idx], self.scheduled[idx], self.matched[idx], self.flags[idx],
+                          self.min_res[:, idx], self.min_res_present[idx], self.rep_sel[idx], self.rep_tol[idx],
+                          self.creation_ns[idx], self.name_rank[idx],
+                          None if self.rep_aff is None else self.rep_aff[idx])
 
 
 BOUND_GROUP_LOCKED = 0x01   # the bound pod's PodGroup Status.Phase is Scheduled or Running

@@ -1,7 +1,7 @@
 /* fit_reasons_ref.c — TEST INFRASTRUCTURE: the CPU restatement of the reason rows (include/bsched.h BS_OUT_REASONS),
  * built on the oracle's line-by-line helpers (oracle/bs_oracle.h: bso_check_fit, bso_single_node_resource,
- * bso_pod_require) and linked against oracle/libbs_oracle.so.  tests/fit_reasons_ref.py compiles it into a temporary
- * directory and binds it. */
+ * bso_pod_require) and linked against oracle/libbs_oracle.so.  tests/native.py compiles it with the other
+ * restatements and tests/fit_reasons_ref.py binds it. */
 #include <stdint.h>
 #include <string.h>
 

@@ -1,6 +1,6 @@
 /* preempt_ref.c — TEST INFRASTRUCTURE: the CPU restatement of bs_remove_pod and bs_preempt (include/bsched.h), built on
  * the oracle's fit predicate (oracle/bs_oracle.h: bso_fit_eval) and linked against oracle/libbs_oracle.so.
- * tests/preempt_ref.py compiles it into a temporary directory and binds it.
+ * tests/native.py compiles it with the other restatements and tests/preempt_ref.py binds it.
  *
  * Preemption is restated the way upstream does it (k8s v1.17.5 genericScheduler.Preempt -> selectVictimsOnNode ->
  * pickOneNodeForPreemption, [upstream, from memory]): on a MUTATED one-node copy of each node, removing and re-adding

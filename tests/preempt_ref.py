@@ -2,24 +2,18 @@
 
 tests/preempt_ref.c mutates a one-node copy of each node and calls the oracle's fit predicate (bso_fit_eval) after
 every removal and re-add, the way upstream's selectVictimsOnNode does, with OpenMP over the preemptors.  It is
-compiled into a temporary directory on first use, because the tree may be read-only, and linked against
-oracle/libbs_oracle.so.
+compiled on first use into tests/native.py's library of the C restatements.
 """
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
-import tempfile
+import functools
 from dataclasses import dataclass
 
 import numpy as np
 
+import native
 from oracle import oracle
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_ORACLE_DIR = os.path.join(os.path.dirname(_HERE), "oracle")
-_lib_h = None
 
 ALLOW, OFFLINE_ONLINE, NOT_FOUND, LOCKED, SAME_GROUP = range(5)
 BOUND_GROUP_LOCKED = 0x01
@@ -31,23 +25,15 @@ class _Bound(C.Structure):
                 ("flags", C.c_void_p)]
 
 
+@functools.cache
 def _lib():
-    global _lib_h
-    if _lib_h is None:
-        so = oracle.build()
-        out = os.path.join(tempfile.mkdtemp(prefix="preempt_ref_"), "libpreempt_ref.so")
-        subprocess.check_call(["gcc", "-O2", "-std=c11", "-fPIC", "-Wall", "-Wextra", "-fopenmp", "-shared", "-o", out,
-                               os.path.join(_HERE, "preempt_ref.c"), "-I" + _ORACLE_DIR, so,
-                               "-Wl,-rpath," + os.path.dirname(so)])
-        oracle.lib()   # the oracle library first, so that its symbols resolve
-        lib = C.CDLL(out)
-        lib.bsr_remove_pod.restype = C.c_int
-        lib.bsr_remove_pod.argtypes = [C.c_int32, C.c_int32, C.c_uint8]
-        lib.bsr_preempt.restype = None
-        lib.bsr_preempt.argtypes = [C.POINTER(oracle._Nodes), C.POINTER(oracle._Pods), C.POINTER(_Bound), C.c_void_p,
-                                    C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_int]
-        _lib_h = lib
-    return _lib_h
+    lib = native.ref_lib()
+    lib.bsr_remove_pod.restype = C.c_int
+    lib.bsr_remove_pod.argtypes = [C.c_int32, C.c_int32, C.c_uint8]
+    lib.bsr_preempt.restype = None
+    lib.bsr_preempt.argtypes = [C.POINTER(oracle._Nodes), C.POINTER(oracle._Pods), C.POINTER(_Bound), C.c_void_p,
+                                C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_int]
+    return lib
 
 
 def remove_pod(gid_p: int, gid_v: int, flags_v: int) -> int:

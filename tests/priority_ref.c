@@ -1,13 +1,14 @@
 /* priority_ref.c — TEST INFRASTRUCTURE: the CPU restatement of the priority lists (include/bsched.h BS_OUT_PRIORITY).
  * The fit set comes from the oracle's bso_fit_eval (oracle/bs_oracle.h); the three scorers restate kube-scheduler
  * v1.17's NodeResourcesLeastAllocated, NodeResourcesMostAllocated and NodeResourcesBalancedAllocation [upstream, from
- * memory].  Compiled with -ffp-contract=off, so every double operation rounds on its own.  tests/priority_ref.py
- * compiles it into a temporary directory and binds it. */
+ * memory].  Compiled with -ffp-contract=off, so every double operation rounds on its own.  tests/native.py compiles
+ * it with the other restatements and tests/priority_ref.py binds it. */
 #include <math.h>
 #include <stddef.h>
 #include <stdint.h>
 
 #include "bs_oracle.h"
+#include "bs_ref.h"
 
 /* leastRequestedScore / mostRequestedScore: int64, truncating */
 static int64_t least_score(int64_t r, int64_t c) {

@@ -1,45 +1,31 @@
 """TEST INFRASTRUCTURE — the CPU restatement of the priority lists (include/bsched.h BS_OUT_PRIORITY).
 
 tests/priority_ref.c takes each pod's fit set from the oracle's bso_fit_eval and restates the three resource scorers in
-C.  It is compiled with -ffp-contract=off into a temporary directory on first use, because the tree may be read-only,
-and linked against oracle/libbs_oracle.so.
+C.  It is compiled with -ffp-contract=off on first use into tests/native.py's library of the C restatements.
 """
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
-import tempfile
+import functools
 
 import numpy as np
 
+import native
 from oracle import oracle
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_ORACLE_DIR = os.path.join(os.path.dirname(_HERE), "oracle")
-_lib_cache = None
 
 DEFAULT_WEIGHTS = (1, 0, 1)
 
 
+@functools.cache
 def _lib():
-    global _lib_cache
-    if _lib_cache is None:
-        so = oracle.build()
-        out = os.path.join(tempfile.mkdtemp(prefix="priority_ref_"), "libpriority_ref.so")
-        subprocess.check_call(["gcc", "-O2", "-std=c11", "-fPIC", "-Wall", "-Wextra", "-ffp-contract=off", "-shared",
-                               "-o", out, os.path.join(_HERE, "priority_ref.c"), "-I" + _ORACLE_DIR, so, "-lm",
-                               "-Wl,-rpath," + os.path.dirname(so)])
-        oracle.lib()   # the oracle library first, so that its symbols resolve
-        lib = C.CDLL(out)
-        lib.bsr_priority_rows.restype = None
-        lib.bsr_priority_rows.argtypes = [C.POINTER(oracle._Nodes), C.POINTER(oracle._Pods), C.c_void_p, C.c_void_p,
-                                          C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p,
-                                          C.c_void_p]
-        lib.bsr_priority_score.restype = C.c_int64
-        lib.bsr_priority_score.argtypes = [C.c_int64] * 4 + [C.c_uint32] * 3
-        _lib_cache = lib
-    return _lib_cache
+    lib = native.ref_lib()
+    lib.bsr_priority_rows.restype = None
+    lib.bsr_priority_rows.argtypes = [C.POINTER(oracle._Nodes), C.POINTER(oracle._Pods), C.c_void_p, C.c_void_p,
+                                      C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p,
+                                      C.c_void_p]
+    lib.bsr_priority_score.restype = C.c_int64
+    lib.bsr_priority_score.argtypes = [C.c_int64] * 4 + [C.c_uint32] * 3
+    return lib
 
 
 def score(r_cpu, c_cpu, r_mem, c_mem, weights=DEFAULT_WEIGHTS) -> int:

@@ -4,21 +4,14 @@
  * from the broken-line definition at each utilization, not from a table, and the average is rounded with C's round()
  * (half away from zero, Go's math.Round) on binary64.  The score is bsr_priority_score (tests/priority_ref.c) plus
  * weight * Ratio.  Provides the priority-list builder over bso_fit_eval and a chooser / assume hook pair for
- * bsr_replay_choose (tests/replay_priority_ref.c).  Compiled with -ffp-contract=off; tests/ratio_priority_ref.py
- * compiles it with both files into a temporary directory and binds it. */
+ * bsr_replay_choose (tests/replay_priority_ref.c).  Compiled with -ffp-contract=off; tests/native.py compiles it
+ * with the other restatements and tests/ratio_priority_ref.py binds it. */
 #include <math.h>
 #include <stddef.h>
 #include <stdint.h>
 
 #include "bs_oracle.h"
-
-int64_t bsr_priority_score(int64_t r_cpu, int64_t c_cpu, int64_t r_mem, int64_t c_mem, uint32_t w_least, uint32_t w_most,
-                           uint32_t w_balanced);
-typedef int32_t (*bsr_choose_fn)(void* ctx, const bso_nodes* nd, const bso_pods* pd, uint32_t p);
-typedef void (*bsr_assumed_fn)(void* ctx, const bso_nodes* nd, const bso_pods* pd, uint32_t p, uint32_t n);
-int bsr_replay_choose(bso_nodes* nd, const bso_pods* pd, bso_groups* gr, const uint32_t* queue, uint32_t n_queue,
-                      uint8_t* prefilter_out, int32_t* node_out, uint8_t* ready_out, bsr_choose_fn choose,
-                      bsr_assumed_fn assumed, void* ctx);
+#include "bs_ref.h"
 
 /* the setting of bs_set_ratio_priority, in engine units */
 typedef struct {

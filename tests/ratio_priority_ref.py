@@ -3,23 +3,18 @@ bs_set_ratio_priority) in the priority lists and in bs_replay_priority.
 
 tests/ratio_priority_ref.c restates the ratio term from the broken-line definition and adds it to tests/priority_ref.c's
 scorer; its list builder takes the fit set from the oracle's bso_fit_eval, and its chooser / assume hooks drive
-tests/replay_priority_ref.c's walk.  The three files are compiled with -ffp-contract=off into a temporary directory on
-first use, because the tree may be read-only, and linked against oracle/libbs_oracle.so.
+tests/replay_priority_ref.c's walk.  The three files are compiled with -ffp-contract=off on first use into
+tests/native.py's library of the C restatements.
 """
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
-import tempfile
+import functools
 
 import numpy as np
 
+import native
 from oracle import oracle
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_ORACLE_DIR = os.path.join(os.path.dirname(_HERE), "oracle")
-_lib_cache = None
 
 DEFAULT_WEIGHTS = (1, 0, 1)
 DEFAULT_SHAPE = ((0, 100), (100, 0))   # v1.17's default {(0, 10), (100, 0)} in node-score units
@@ -43,31 +38,22 @@ def setting(weight, shape, lane_weights, absent_weight=0):
     return s
 
 
+@functools.cache
 def _lib():
-    global _lib_cache
-    if _lib_cache is None:
-        so = oracle.build()
-        out = os.path.join(tempfile.mkdtemp(prefix="ratio_priority_ref_"), "libratio_priority_ref.so")
-        subprocess.check_call(["gcc", "-O2", "-std=c11", "-fPIC", "-Wall", "-Wextra", "-ffp-contract=off", "-shared",
-                               "-o", out, os.path.join(_HERE, "ratio_priority_ref.c"),
-                               os.path.join(_HERE, "replay_priority_ref.c"), os.path.join(_HERE, "priority_ref.c"),
-                               "-I" + _ORACLE_DIR, so, "-lm", "-Wl,-rpath," + os.path.dirname(so)])
-        oracle.lib()   # the oracle library first, so that its symbols resolve
-        lib = C.CDLL(out)
-        P, S = C.c_void_p, C.POINTER(_Setting)
-        lib.bsr_ratio_shape.restype = C.c_int64
-        lib.bsr_ratio_shape.argtypes = [S, C.c_int64]
-        lib.bsr_ratio_util.restype = C.c_int64
-        lib.bsr_ratio_util.argtypes = [C.c_int64, C.c_int64]
-        lib.bsr_ratio_of.restype = C.c_int64
-        lib.bsr_ratio_of.argtypes = [S, P, P]
-        lib.bsr_ratio_rows.restype = None
-        lib.bsr_ratio_rows.argtypes = [S, C.POINTER(oracle._Nodes), C.POINTER(oracle._Pods), P, P, C.c_uint32,
-                                       C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, P, P]
-        lib.bsr_replay_ratio.argtypes = [C.POINTER(oracle._Nodes), C.POINTER(oracle._Pods), C.POINTER(oracle._Groups),
-                                         P, C.c_uint32, P, P, P, P, P, C.c_uint32, C.c_uint32, C.c_uint32, S]
-        _lib_cache = lib
-    return _lib_cache
+    lib = native.ref_lib()
+    P, S = C.c_void_p, C.POINTER(_Setting)
+    lib.bsr_ratio_shape.restype = C.c_int64
+    lib.bsr_ratio_shape.argtypes = [S, C.c_int64]
+    lib.bsr_ratio_util.restype = C.c_int64
+    lib.bsr_ratio_util.argtypes = [C.c_int64, C.c_int64]
+    lib.bsr_ratio_of.restype = C.c_int64
+    lib.bsr_ratio_of.argtypes = [S, P, P]
+    lib.bsr_ratio_rows.restype = None
+    lib.bsr_ratio_rows.argtypes = [S, C.POINTER(oracle._Nodes), C.POINTER(oracle._Pods), P, P, C.c_uint32,
+                                   C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, P, P]
+    lib.bsr_replay_ratio.argtypes = [C.POINTER(oracle._Nodes), C.POINTER(oracle._Pods), C.POINTER(oracle._Groups),
+                                     P, C.c_uint32, P, P, P, P, P, C.c_uint32, C.c_uint32, C.c_uint32, S]
+    return lib
 
 
 def shape_at(shape, p) -> int:

@@ -5,21 +5,16 @@
  * tables, or -1, and is told which node the pod was assumed onto.  With bsr_first_fit it is bso_replay, which the
  * tests check; with bsr_priority_choose it is bs_replay_priority: among the fitting nodes the highest
  * bsr_priority_score (tests/priority_ref.c) over a live copy of the node non-zero column, ties to the lower index.
- * tests/replay_priority_ref.py compiles it with priority_ref.c into a temporary directory and binds it. */
+ * tests/native.py compiles it with the other restatements and tests/replay_priority_ref.py binds it. */
 #include <stddef.h>
 #include <stdint.h>
 
 #include "bs_oracle.h"
+#include "bs_ref.h"
 
 #define LANE_PODS 3
 #define POD_AFF(pd, p) ((pd)->aff_class ? (pd)->aff_class[p] : BSO_AFF_NONE)
 #define GROUP_AFF(gr, g) ((gr)->rep_aff ? (gr)->rep_aff[g] : BSO_AFF_NONE)
-
-int64_t bsr_priority_score(int64_t r_cpu, int64_t c_cpu, int64_t r_mem, int64_t c_mem, uint32_t w_least, uint32_t w_most,
-                           uint32_t w_balanced);
-
-typedef int32_t (*bsr_choose_fn)(void* ctx, const bso_nodes* nd, const bso_pods* pd, uint32_t p);
-typedef void (*bsr_assumed_fn)(void* ctx, const bso_nodes* nd, const bso_pods* pd, uint32_t p, uint32_t n);
 
 /* bso_replay's node choice: the first node in list order where the pod fits */
 int32_t bsr_first_fit(void* ctx, const bso_nodes* nd, const bso_pods* pd, uint32_t p) {

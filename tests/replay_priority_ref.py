@@ -2,48 +2,33 @@
 
 tests/replay_priority_ref.c restates the oracle's pod-at-a-time walk over the oracle's public helpers with the node
 choice as a hook, and the scoring chooser over tests/priority_ref.c's scorer.  Both files are compiled with
--ffp-contract=off into a temporary directory on first use, because the tree may be read-only, and linked against
-oracle/libbs_oracle.so.
+-ffp-contract=off on first use into tests/native.py's library of the C restatements.
 """
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
-import tempfile
+import functools
 
 import numpy as np
 
+import native
 from oracle import oracle
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_ORACLE_DIR = os.path.join(os.path.dirname(_HERE), "oracle")
-_lib_cache = None
 
 DEFAULT_WEIGHTS = (1, 0, 1)
 
 
+@functools.cache
 def _lib():
-    global _lib_cache
-    if _lib_cache is None:
-        so = oracle.build()
-        out = os.path.join(tempfile.mkdtemp(prefix="replay_priority_ref_"), "libreplay_priority_ref.so")
-        subprocess.check_call(["gcc", "-O2", "-std=c11", "-fPIC", "-Wall", "-Wextra", "-ffp-contract=off", "-shared",
-                               "-o", out, os.path.join(_HERE, "replay_priority_ref.c"),
-                               os.path.join(_HERE, "priority_ref.c"), "-I" + _ORACLE_DIR, so, "-lm",
-                               "-Wl,-rpath," + os.path.dirname(so)])
-        oracle.lib()   # the oracle library first, so that its symbols resolve
-        lib = C.CDLL(out)
-        P = C.c_void_p
-        lib.bsr_replay_priority.argtypes = [C.POINTER(oracle._Nodes), C.POINTER(oracle._Pods),
-                                            C.POINTER(oracle._Groups), P, C.c_uint32, P, P, P, P, P,
-                                            C.c_uint32, C.c_uint32, C.c_uint32]
-        lib.bsr_replay_choose.argtypes = [C.POINTER(oracle._Nodes), C.POINTER(oracle._Pods),
-                                          C.POINTER(oracle._Groups), P, C.c_uint32, P, P, P, P, P, P]
-        lib.bsr_first_fit.restype = C.c_int32
-        lib.bsr_priority_choose.restype = C.c_int32
-        _lib_cache = lib
-    return _lib_cache
+    lib = native.ref_lib()
+    P = C.c_void_p
+    lib.bsr_replay_priority.argtypes = [C.POINTER(oracle._Nodes), C.POINTER(oracle._Pods),
+                                        C.POINTER(oracle._Groups), P, C.c_uint32, P, P, P, P, P,
+                                        C.c_uint32, C.c_uint32, C.c_uint32]
+    lib.bsr_replay_choose.argtypes = [C.POINTER(oracle._Nodes), C.POINTER(oracle._Pods),
+                                      C.POINTER(oracle._Groups), P, C.c_uint32, P, P, P, P, P, P]
+    lib.bsr_first_fit.restype = C.c_int32
+    lib.bsr_priority_choose.restype = C.c_int32
+    return lib
 
 
 def _walk(snap, queue, call):

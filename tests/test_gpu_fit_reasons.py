@@ -2,7 +2,6 @@
 (built on the oracle's helpers), in every lane layout, at unaligned sizes, beside every other output mode, after row
 updates, at cfg4 size, and through the C++ plugin's FitError."""
 import json
-import os
 import subprocess
 
 import numpy as np
@@ -10,17 +9,9 @@ import pytest
 
 import fit_reasons_ref
 import lane_cases
+import native
 import reason_cases
 from randsnap import S, random_snapshot
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _sub(table, idx):
-    """The compact table of rows `idx` (row updates)."""
-    return type(table)(*(None if getattr(table, f) is None else
-                         (getattr(table, f)[:, idx] if getattr(table, f).ndim == 2 else getattr(table, f)[idx])
-                         for f in table.__dataclass_fields__))
 
 
 def _fit_matrix(words, N):
@@ -110,7 +101,7 @@ def test_affinity_tables(pkg, oracle, aff):
 def test_unaligned_sizes(pkg, oracle, N, P):
     snap = random_snapshot(N * 7 + P, P=P, N=max(N, 1), G=9, L=6, aff=3)
     if N == 0:
-        snap.nodes = _sub(snap.nodes, np.zeros(0, np.int64))
+        snap.nodes = snap.nodes.take(np.zeros(0, np.int64))
         snap.aff_bits = None
         snap.pods.aff_class = None
         snap.groups.rep_aff = None
@@ -185,7 +176,7 @@ def test_row_updates_and_affinity_replacement(pkg, oracle):
         nodes.requested[0, nidx[20:30]] = 0
         nodes.requested[0, nidx[30:]] = nodes.alloc[0, nidx[30:]] + 1
         nodes.req_present[nidx[30:]] ^= np.uint32(1 << 5)
-        eng.update_nodes(nidx, _sub(nodes, nidx))
+        eng.update_nodes(nidx, nodes.take(nidx))
         snap.nodes = nodes
         res = eng.evaluate()
         _check(oracle, snap, res, eng.reason_rows(), eng.fit_rows())
@@ -194,7 +185,7 @@ def test_row_updates_and_affinity_replacement(pkg, oracle):
         groups = snap.groups.copy()
         groups.matched[gidx] += 1
         groups.flags[gidx] ^= np.uint8(S.GROUP_DENIED)
-        eng.update_groups(gidx, _sub(groups, gidx))
+        eng.update_groups(gidx, groups.take(gidx))
         snap.groups = groups
         res = eng.evaluate()
         _check(oracle, snap, res, eng.reason_rows(), eng.fit_rows())
@@ -274,13 +265,8 @@ def test_fetch_errors(pkg):
 
 
 @pytest.mark.gpu
-def test_plugin_fit_error(pkg, tmp_path):
-    pkg.capi.load()
-    src = os.path.join(ROOT, "tests", "cpp", "plugin_reasons_test.cpp")
-    libdir = os.path.join(ROOT, "batch-scheduler_b200")
-    binary = str(tmp_path / "plugin_reasons_test")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-o", binary, src, "-L" + libdir, "-lbsched",
-                           "-Wl,-rpath," + libdir, "-L/usr/local/cuda/lib64", "-Wl,-rpath,/usr/local/cuda/lib64"])
+def test_plugin_fit_error():
+    binary = native.cpp_program("plugin_reasons_test")
     first, second = json.loads(subprocess.check_output([binary, "reasons"], text=True))
     taints = "1 node(s) had taints that the pod didn't tolerate"
     assert first["lanes"] == second["lanes"] == 5

@@ -194,7 +194,7 @@ def test_lifecycle_drops_table():
         if drop == "nodes":
             eng.upload_nodes(snap.nodes)
         elif drop == "update":
-            eng.update_nodes([0], S.NodeTable(*(getattr(snap.nodes, f)[..., :1] for f in snap.nodes.__dataclass_fields__)))
+            eng.update_nodes([0], snap.nodes.take([0]))
         else:
             eng.upload_groups(snap.groups)
         with pytest.raises(capi.BsError) as ex:

@@ -4,24 +4,16 @@ beside every other output mode (whose outputs do not change), after row updates,
 of the C ABI, and through the C++ plugin's PriorityNodes."""
 import importlib
 import json
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
+import native
 import priority_ref
 from randsnap import S, random_snapshot
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 WEIGHTS = [(1, 0, 1), (0, 1, 0), (3, 2, 5), (0, 0, 0)]
-
-
-def _sub(table, idx):
-    """The compact table of rows `idx` (row updates)."""
-    return type(table)(*(None if getattr(table, f) is None else
-                         (getattr(table, f)[:, idx] if getattr(table, f).ndim == 2 else getattr(table, f)[idx])
-                         for f in table.__dataclass_fields__))
 
 
 def _fit_matrix(words, N):
@@ -111,7 +103,7 @@ def test_narrow_shape_with_ties(pkg, oracle):
 def test_unaligned_sizes(pkg, oracle, N, K):
     snap = random_snapshot(N * 7 + K, P=70, N=max(N, 1), G=9, L=6, aff=3)
     if N == 0:
-        snap.nodes = _sub(snap.nodes, np.zeros(0, np.int64))
+        snap.nodes = snap.nodes.take(np.zeros(0, np.int64))
         snap.aff_bits = None
         snap.pods.aff_class = None
         snap.groups.rep_aff = None
@@ -195,7 +187,7 @@ def test_row_updates_and_weight_changes(pkg, oracle):
         nodes.flags[nidx[:10]] = S.NODE_UNSCHEDULABLE
         nodes.requested[0, nidx[20:30]] = 0
         nodes.alloc[1, nidx[30:]] = -nodes.alloc[1, nidx[30:]]   # negative allocatable memory
-        eng.update_nodes(nidx, _sub(nodes, nidx))
+        eng.update_nodes(nidx, nodes.take(nidx))
         snap.nodes = nodes
         node_nz = node_nz.copy()
         node_nz[:, nidx[20:30]] = 0
@@ -299,7 +291,7 @@ def test_errors(pkg):
         assert code(eng.evaluate) == c.BS_E_STATE
         eng.upload_nonzero(pods=pod_nz)
         eng.evaluate()
-        eng.update_nodes(np.array([3]), _sub(snap.nodes, np.array([3])))
+        eng.update_nodes(np.array([3]), snap.nodes.take(np.array([3])))
         assert code(eng.evaluate) == c.BS_E_STATE
         eng.upload_nonzero(node=node_nz)
         eng.evaluate()
@@ -312,14 +304,8 @@ def test_errors(pkg):
 
 
 @pytest.mark.gpu
-def test_plugin_priority_nodes(pkg, tmp_path):
-    pkg.capi.load()
-    src = os.path.join(ROOT, "tests", "cpp", "plugin_priority_test.cpp")
-    libdir = os.path.join(ROOT, "batch-scheduler_b200")
-    binary = str(tmp_path / "plugin_priority_test")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-o", binary, src, "-L" + libdir, "-lbsched",
-                           "-Wl,-rpath," + libdir, "-L/usr/local/cuda/lib64", "-Wl,-rpath,/usr/local/cuda/lib64"])
-    o = json.loads(subprocess.check_output([binary, "round"], text=True))
+def test_plugin_priority_nodes():
+    o = json.loads(subprocess.check_output([native.cpp_program("plugin_priority_test"), "round"], text=True))
     least, most = o["begin"]
     # the min-residual rule picks node-0 (most pod slots left); LeastAllocated + Balanced picks node-1, MostAllocated
     # node-2 (scores worked by hand: DESIGN §2's formulas on cpu 8 / memory 32Gi nodes and a 500m / 1Gi pod)

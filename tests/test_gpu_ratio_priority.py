@@ -3,31 +3,24 @@ bs_replay_priority, bit-exact against the CPU restatement tests/ratio_priority_r
 list lengths, shapes, weight sets, extreme and negative values; weight 0 is the engine without the priority; every
 BS_E_INVAL case keeps the previous setting; and the C++ plugin's SetRatioPriority."""
 import json
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
+import native
 import priority_ref
 import ratio_priority_ref as rr
 from randsnap import S, random_snapshot
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SHAPES = {"default": rr.DEFAULT_SHAPE, "binpack": rr.BIN_PACK, "single": ((50, 40),),
           "full": tuple((u, (u * 37) % 101) for u in range(101)), "falling": ((0, 100), (30, 0)),
           "rising": ((10, 20), (40, 90), (60, 30), (100, 70))}
 WEIGHTS = [(0, 0, 0), (1, 0, 1), (0, 1, 0)]
 AFTER = ("node_requested", "node_pod_count", "node_req_present", "group_matched", "group_flags", "group_min_res",
          "group_min_res_present", "group_rep_sel", "group_rep_tol")
-
-
-def _sub(table, idx):
-    return type(table)(*(None if getattr(table, f) is None else
-                         (getattr(table, f)[:, idx] if getattr(table, f).ndim == 2 else getattr(table, f)[idx])
-                         for f in table.__dataclass_fields__))
 
 
 def _lane_weights(L, seed, gpu_only=False):
@@ -82,7 +75,7 @@ def test_weight_sets_and_lengths(pkg, oracle, w, K):
 def test_unaligned_sizes(pkg, oracle, N):
     snap = random_snapshot(N * 5 + 1, P=70, N=max(N, 1), G=9, L=6)
     if N == 0:
-        snap.nodes = _sub(snap.nodes, np.zeros(0, np.int64))
+        snap.nodes = snap.nodes.take(np.zeros(0, np.int64))
     nodes, _ = _check_rows(pkg, snap, 7, (1, 0, 1), (1, rr.BIN_PACK, [1, 1, 1, 0, 2, 2], 1), seed=N)
     if N == 0:
         assert (nodes == -1).all()
@@ -264,17 +257,11 @@ def test_replay_errors_still_hold(pkg):
         eng.close()
 
 
-def test_plugin_ratio_priority(pkg, tmp_path):
+def test_plugin_ratio_priority():
     """BatchSchedulingPlugin::SetRatioPriority through tests/cpp/plugin_ratio_priority_test.cpp: the lane mapping over
     two rounds whose scalar lanes come in different orders, pods and unknown names in absent_weight, the x10 scaling,
     and PriorityNodes / ReplayQueue(kPriority) equal to the engine called directly."""
-    pkg.capi.load()
-    src = os.path.join(ROOT, "tests", "cpp", "plugin_ratio_priority_test.cpp")
-    libdir = os.path.join(ROOT, "batch-scheduler_b200")
-    binary = str(tmp_path / "plugin_ratio_priority_test")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-o", binary, src, "-L" + libdir, "-lbsched",
-                           "-Wl,-rpath," + libdir, "-L/usr/local/cuda/lib64", "-Wl,-rpath,/usr/local/cuda/lib64"])
-    o = json.loads(subprocess.check_output([binary], text=True))
+    o = json.loads(subprocess.check_output([native.cpp_program("plugin_ratio_priority_test")], text=True))
     for r in o["rounds"]:
         assert r["plugin_nodes"] == r["engine_nodes"] and r["plugin_scores"] == r["engine_scores"], r
         assert r["plugin_replay"] == r["engine_replay"], r

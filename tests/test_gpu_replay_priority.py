@@ -3,20 +3,18 @@ restatement tests/replay_priority_ref.c per queue position and on the whole afte
 column, in every lane build, for several weight sets, with the cross-layer and error checks of the C ABI and full-size
 properties at cfg4."""
 import json
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
+import native
 import priority_ref
 import pyref_priority
 import replay_priority_ref as rpr
 from randsnap import S, random_snapshot
 
 pytestmark = pytest.mark.gpu
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 WEIGHTS = [(1, 0, 1), (0, 1, 0), (1, 1, 1), (3, 0, 7)]
 AFTER = ("node_requested", "node_pod_count", "node_req_present", "group_matched", "group_flags", "group_min_res",
@@ -133,9 +131,7 @@ def test_negative_allocatable_and_requests(pkg, oracle):
 
 def test_no_nodes(pkg, oracle):
     snap = random_snapshot(5, P=50, N=1, G=8, L=5, case="mixed")
-    idx = np.zeros(0, np.int64)
-    snap.nodes = type(snap.nodes)(*(getattr(snap.nodes, f)[:, idx] if getattr(snap.nodes, f).ndim == 2
-                                    else getattr(snap.nodes, f)[idx] for f in snap.nodes.__dataclass_fields__))
+    snap.nodes = snap.nodes.take(np.zeros(0, np.int64))
     nz = (np.zeros((2, 0), np.int64), S.nonzero_requests(snap, 5)[1])
     got = walk_both(pkg, snap, None, (1, 0, 1), nz=nz)
     assert (got["node"] == -1).all() and got["node_nonzero"].shape == (2, 0)
@@ -215,9 +211,7 @@ def test_errors(pkg):
         assert code(eng.replay, priority=True) == c.BS_E_STATE            # no pod column
         eng.upload_nonzero(pods=pod_nz)
         eng.replay(priority=True)
-        eng.update_nodes(np.array([3]), type(snap.nodes)(*(getattr(snap.nodes, f)[:, [3]] if getattr(snap.nodes, f).ndim == 2
-                                                           else getattr(snap.nodes, f)[[3]]
-                                                           for f in snap.nodes.__dataclass_fields__)))
+        eng.update_nodes(np.array([3]), snap.nodes.take([3]))
         assert code(eng.replay, priority=True) == c.BS_E_STATE            # row updates drop the node column
         eng.upload_nonzero(node=node_nz)
         eng.replay(priority=True)
@@ -266,17 +260,11 @@ def test_full_size_cfg4(pkg, snapshot_mod):
                                   got["node_pod_count"] - snap.nodes.pod_count)
 
 
-def test_plugin_replay_queue_choices(pkg, tmp_path):
+def test_plugin_replay_queue_choices():
     """BatchSchedulingPlugin::ReplayQueue: two empty 4-cpu / 8Gi nodes, four 500m / 1Gi pods.  First-fit packs node 0;
     kPriority under (1, 0, 1) alternates (87 + 100 on both empty nodes, then 175 against 187, ...), under (0, 1, 0)
     packs node 0; without priority_k kPriority is an error."""
-    pkg.capi.load()
-    src = os.path.join(ROOT, "tests", "cpp", "plugin_replay_priority_test.cpp")
-    libdir = os.path.join(ROOT, "batch-scheduler_b200")
-    binary = str(tmp_path / "plugin_replay_priority_test")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-o", binary, src, "-L" + libdir, "-lbsched",
-                           "-Wl,-rpath," + libdir, "-L/usr/local/cuda/lib64", "-Wl,-rpath,/usr/local/cuda/lib64"])
-    o = json.loads(subprocess.check_output([binary], text=True))
+    o = json.loads(subprocess.check_output([native.cpp_program("plugin_replay_priority_test")], text=True))
     assert o["first_fit"] == o["plain_first_fit"] == [0, 0, 0, 0]
     assert o["least_balanced"] == [0, 1, 0, 1] and o["positions"] == [0, 1, 2, 3]
     assert o["most"] == [0, 0, 0, 0]

@@ -11,6 +11,7 @@ import subprocess
 import numpy as np
 import pytest
 
+import native
 from parity import assert_round_equal
 from randsnap import random_snapshot
 
@@ -243,19 +244,13 @@ def test_topk_row_updates(pkg, oracle):
         for d in range(3):
             rows.requested[d, nidx] = 0                  # the changed nodes free up
         rows.flags[nidx[:2]] = 0
-        sub = type(rows)(*(None if getattr(rows, f) is None else
-                           (getattr(rows, f)[:, nidx] if getattr(rows, f).ndim == 2 else getattr(rows, f)[nidx])
-                           for f in rows.__dataclass_fields__))
-        eng.update_nodes(nidx, sub)
+        eng.update_nodes(nidx, rows.take(nidx))
         snap.nodes = rows
         gidx = np.sort(rng.choice(snap.groups.n, 5, replace=False))
         groups = snap.groups.copy()
         groups.matched[gidx] += 1
         groups.flags[gidx] ^= 0x8                          # toggles GROUP_DENIED
-        gsub = type(groups)(*(None if getattr(groups, f) is None else
-                              (getattr(groups, f)[:, gidx] if getattr(groups, f).ndim == 2 else getattr(groups, f)[gidx])
-                              for f in groups.__dataclass_fields__))
-        eng.update_groups(gidx, gsub)
+        eng.update_groups(gidx, groups.take(gidx))
         snap.groups = groups
         res = eng.evaluate()
         nodes, scores = eng.topk_rows()
@@ -297,17 +292,9 @@ def test_topk_full_size_cfg4(pkg, oracle, snapshot_mod):
 
 
 @pytest.mark.gpu
-def test_plugin_top_nodes(pkg):
-    pkg.capi.load()
-    src = os.path.join(ROOT, "tests", "cpp", "plugin_topk_test.cpp")
-    binary = os.path.join(ROOT, "tests", "cpp", "plugin_topk_test")
-    libdir = os.path.join(ROOT, "batch-scheduler_b200")
-    lib = os.path.join(libdir, "libbsched.so")
-    if not os.path.exists(binary) or os.path.getmtime(binary) < max(os.path.getmtime(src), os.path.getmtime(lib)):
-        subprocess.check_call(["g++", "-std=c++17", "-O2", "-o", binary, src, "-L" + libdir, "-lbsched",
-                               "-Wl,-rpath," + libdir, "-L/usr/local/cuda/lib64", "-Wl,-rpath,/usr/local/cuda/lib64"])
+def test_plugin_top_nodes():
     K = 8
-    rounds = json.loads(subprocess.check_output([binary, "topk", str(K)], text=True))
+    rounds = json.loads(subprocess.check_output([native.cpp_program("plugin_topk_test"), "topk", str(K)], text=True))
     assert len(rounds) == 2                            # BeginRound, then UpdateRound
     for rd in rounds:
         assert rd["rc"] == 0 and rd["unknown"] == 0

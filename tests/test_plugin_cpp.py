@@ -1,26 +1,17 @@
 """The C++ host mirror (batch-scheduler_b200/csrc/plugin.{hpp,cpp}): resource.Quantity parsing and the
 snapshot packer on CPU; the README scenario pod-by-pod through BatchSchedulingPlugin on the GPU."""
 import json
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-BIN = os.path.join(ROOT, "tests", "cpp", "plugin_test")
+import native
 
 
 @pytest.fixture(scope="module")
-def plugin_bin(pkg):
-    pkg.capi.load()  # makes sure libbsched.so exists
-    src = os.path.join(ROOT, "tests", "cpp", "plugin_test.cpp")
-    libdir = os.path.join(ROOT, "batch-scheduler_b200")
-    lib = os.path.join(libdir, "libbsched.so")
-    if (not os.path.exists(BIN) or os.path.getmtime(BIN) < max(os.path.getmtime(src), os.path.getmtime(lib))):
-        subprocess.check_call(["g++", "-std=c++17", "-O2", "-o", BIN, src, "-L" + libdir, "-lbsched",
-                               "-Wl,-rpath," + libdir, "-L/usr/local/cuda/lib64", "-Wl,-rpath,/usr/local/cuda/lib64"])
-    return BIN
+def plugin_bin():
+    return native.cpp_program("plugin_test")
 
 
 def _run(binary, *args):

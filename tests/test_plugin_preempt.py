@@ -1,24 +1,18 @@
 """Preemption through the C++ plugin (tests/cpp/plugin_preempt_test.cpp): the bound-pod packer on the CPU, and a
 scripted gang scenario through BatchSchedulingPlugin on the GPU."""
 import json
-import os
 import subprocess
 
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+import native
+
 LOCKED_MSG = "pod belongs to Scheduled or Running pod group can not be scheduled"
 
 
 @pytest.fixture(scope="module")
-def binary(pkg, tmp_path_factory):
-    pkg.capi.load()
-    src = os.path.join(ROOT, "tests", "cpp", "plugin_preempt_test.cpp")
-    libdir = os.path.join(ROOT, "batch-scheduler_b200")
-    out = str(tmp_path_factory.mktemp("plugin_preempt") / "plugin_preempt_test")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-o", out, src, "-L" + libdir, "-lbsched",
-                           "-Wl,-rpath," + libdir, "-L/usr/local/cuda/lib64", "-Wl,-rpath,/usr/local/cuda/lib64"])
-    return out
+def binary():
+    return native.cpp_program("plugin_preempt_test")
 
 
 def test_pack_bound_pods(binary):

@@ -9,6 +9,7 @@ import subprocess
 import numpy as np
 import pytest
 
+import native
 import priority_ref
 import pyref_priority
 from randsnap import random_snapshot
@@ -210,19 +211,8 @@ def test_engine_rejects_unequal_list_lengths(pkg):
 
 
 # -- the packer -------------------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def priority_bin(pkg, tmp_path_factory):
-    pkg.capi.load()
-    src = os.path.join(ROOT, "tests", "cpp", "plugin_priority_test.cpp")
-    libdir = os.path.join(ROOT, "batch-scheduler_b200")
-    binary = str(tmp_path_factory.mktemp("plugin_priority") / "plugin_priority_test")   # the tree may be read-only
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-o", binary, src, "-L" + libdir, "-lbsched",
-                           "-Wl,-rpath," + libdir, "-L/usr/local/cuda/lib64", "-Wl,-rpath,/usr/local/cuda/lib64"])
-    return binary
-
-
-def test_packer_nonzero_columns(priority_bin):
-    o = json.loads(subprocess.check_output([priority_bin, "pack"], text=True))
+def test_packer_nonzero_columns():
+    o = json.loads(subprocess.check_output([native.cpp_program("plugin_priority_test"), "pack"], text=True))
     d_cpu, d_mem = 100, 200 << 20
     # pods: no containers; one container without requests; explicit zeros; set values; cpu only; two containers;
     # limits only (Requests, not Limits, count)
