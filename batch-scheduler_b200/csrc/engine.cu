@@ -411,6 +411,8 @@ struct bs_engine {
   View d_gk0, d_gk1, d_pk0, d_pk1, d_idx_a, d_idx_b, d_ghist, d_group_rank, d_tilecnt, d_sort_barrier;
   uint32_t sort_max_grid = 1;
   DevBuf d_sort_arena;
+  // what the last round's sort launched (bs_sort_shape): kernel 0 none, 1 single-CTA, 2 persistent lean, 3 persistent wide
+  struct SortShape { bool valid = false; uint32_t kernel = 0, grid = 0, group_passes = 0, pod_passes = 0; } sort_shape;
 
   // host copies for the per-call mirrors and class building
   std::vector<int32_t> h_gid, h_prio;
@@ -1116,6 +1118,8 @@ int evaluate_async_locked(bs_engine* e) {
   {
     StageTimer tm(e, BS_K_SORT, e->s2);
     // one persistent kernel: group keys -> sort -> dense group rank -> pod keys -> sort -> order + rank
+    e->sort_shape = {};
+    e->sort_shape.valid = true;
     if (P || G) {
       SortArgs sa{};
       sa.creation = e->d_creation.as<int64_t>();
@@ -1151,6 +1155,8 @@ int evaluate_async_locked(bs_engine* e) {
         CK(cudaFuncSetAttribute(queue_sort_small_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         queue_sort_small_kernel<<<1, SORT_SMALL_THREADS, smem, e->s2>>>(sa);
         CK(cudaGetLastError());
+        e->sort_shape.kernel = 1;
+        e->sort_shape.grid = 1;
       } else {
         CK(cudaMemsetAsync(sa.barrier, 0, sizeof(unsigned int), e->s2));
         const uint32_t grid = std::max(1u, std::min(sa.ntiles_max, e->sort_max_grid));
@@ -1165,7 +1171,11 @@ int evaluate_async_locked(bs_engine* e) {
         const bool lean = est_fit_ms > 0.6;
         const void* fn = lean ? (const void*)queue_sort_kernel<SORT_LEAN_GROUP> : (const void*)queue_sort_kernel<SORT_WIDE_GROUP>;
         CK(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(SORT_THREADS), params, 0, e->s2));
+        e->sort_shape.kernel = lean ? 2 : 3;
+        e->sort_shape.grid = grid;
       }
+      e->sort_shape.group_passes = sa.n_gpass;
+      e->sort_shape.pod_passes = sa.n_ppass;
       tm.launched();
     }
   }
@@ -3091,6 +3101,17 @@ int bs_fit_shape(bs_engine* e, uint32_t* wide, uint32_t* narrow, uint32_t* scale
   if (wide) *wide = e->lane_map.LW;
   if (narrow) *narrow = e->lane_map.LN;
   if (scaled) *scaled = e->lane_map.LS;
+  return BS_OK;
+}
+
+int bs_sort_shape(bs_engine* e, uint32_t* kernel, uint32_t* grid, uint32_t* group_passes, uint32_t* pod_passes) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!e->sort_shape.valid) return fail(e, BS_E_STATE, "bs_sort_shape: evaluate first");
+  if (kernel) *kernel = e->sort_shape.kernel;
+  if (grid) *grid = e->sort_shape.grid;
+  if (group_passes) *group_passes = e->sort_shape.group_passes;
+  if (pod_passes) *pod_passes = e->sort_shape.pod_passes;
   return BS_OK;
 }
 

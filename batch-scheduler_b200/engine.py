@@ -510,6 +510,14 @@ class Engine:
         self._check(self.lib.bs_fit_shape(self.h, C.byref(w), C.byref(n), C.byref(sc)))
         return {"LW": int(w.value), "LN": int(n.value), "LS": int(sc.value)}
 
+    def sort_shape(self) -> dict:
+        """What the last evaluation's queue sort launched: kernel (0 none, 1 single-CTA, 2 persistent lean,
+        3 persistent wide), its grid in CTAs, and the radix passes kept for the group and the pod table."""
+        k, g, gp, pp = C.c_uint32(), C.c_uint32(), C.c_uint32(), C.c_uint32()
+        self._check(self.lib.bs_sort_shape(self.h, C.byref(k), C.byref(g), C.byref(gp), C.byref(pp)))
+        return {"kernel": int(k.value), "grid": int(g.value), "group_passes": int(gp.value),
+                "pod_passes": int(pp.value)}
+
     def score_pitch(self) -> int:
         return int(self.lib.bs_score_pitch(self.h))
 

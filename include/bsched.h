@@ -599,6 +599,12 @@ uint64_t bs_launch_count(const bs_engine* e); /* kernels launched since bs_creat
  * |value| <= 2^27) and int32 in exact power-of-two units (scaled: every value of the lane a multiple of
  * 2^k, |value| >> k <= 2^29); wide + narrow + scaled == n_lanes */
 int bs_fit_shape(bs_engine* e, uint32_t* wide, uint32_t* narrow, uint32_t* scaled);
+/* what the last evaluation's queue sort launched: kernel 0 none (both tables empty), 1 the single-CTA kernel
+ * (max(n_pods, n_groups) <= 16384), 2 the persistent kernel's lean build (4 keys in flight per thread, beside a long
+ * fit kernel), 3 its wide build (16 in flight); the grid in CTAs (4096-key tiles are shared out round-robin when there
+ * are more tiles than CTAs); and the radix passes kept for the group and the pod table, one per key byte that varies
+ * over the table.  BS_E_STATE before the first evaluation. */
+int bs_sort_shape(bs_engine* e, uint32_t* kernel, uint32_t* grid, uint32_t* group_passes, uint32_t* pod_passes);
 
 #ifdef __cplusplus
 }

@@ -238,6 +238,30 @@ def prefilter_round(snap):
     return codes, denied, m
 
 
+def queue_order(pt, gt):
+    """The queue order by Compare's key (core.go:379-408), ties in table order, and each pod's dense rank: the number
+    of key changes before it along the order.  Lister misses sort after the resolvable groups."""
+    P, G = pt.n, gt.n
+
+    def key(p):
+        g = int(pt.gid[p])
+        if g == -1:
+            return (-int(pt.priority[p]), 0, 0, 0, int(pt.ts_ns[p]))
+        miss = g < 0 or g >= G or bool(pt.flags[p] & 0x08)
+        creation = (1 << 63) - 1 if miss else int(gt.creation_ns[g])
+        name = 0 if miss else -int(gt.name_rank[g])
+        return (-int(pt.priority[p]), 1, creation, name, int(pt.ts_ns[p]))
+
+    order = np.array(sorted(range(P), key=key), np.uint32)   # sorted() is stable
+    rank = np.zeros(P, np.uint32)
+    r = 0
+    for i in range(P):
+        if i and key(int(order[i])) != key(int(order[i - 1])):
+            r += 1
+        rank[order[i]] = r
+    return order, rank
+
+
 def round_outputs(snap):
     """The rest of a snapshot round (DESIGN.md §2) from the Go-like objects: fit matrix (the composite
     of core_test.go:108-110 behind the node guards and checkFit), builder-defined score, per-pod
@@ -287,22 +311,7 @@ def round_outputs(snap):
         else:
             admit[g] = 0 if cnt >= ((int(gt.min_member[g]) - int(gt.scheduled[g])) & M32) else 1
 
-    def key(p):  # Compare's lexicographic key (core.go:379-408); lister misses after the resolvable groups
-        g = int(pt.gid[p])
-        if g == -1:
-            return (-int(pt.priority[p]), 0, 0, 0, int(pt.ts_ns[p]))
-        miss = g < 0 or g >= G or bool(pt.flags[p] & 0x08)
-        creation = (1 << 63) - 1 if miss else int(gt.creation_ns[g])
-        name = 0 if miss else -int(gt.name_rank[g])
-        return (-int(pt.priority[p]), 1, creation, name, int(pt.ts_ns[p]))
-
-    order = np.array(sorted(range(P), key=key), np.uint32)   # sorted() is stable
-    rank = np.zeros(P, np.uint32)
-    r = 0
-    for i in range(P):
-        if i and key(int(order[i])) != key(int(order[i - 1])):
-            r += 1
-        rank[order[i]] = r
+    order, rank = queue_order(pt, gt)
     return dict(fit=fit, score=score, feasible_count=feasible, best_node=best_node, best_score=best_score,
                 admit=admit, order=order, rank=rank)
 

@@ -586,17 +586,3 @@ def test_view_results_match_copies(pkg, oracle, snapshot_mod):
             assert np.array_equal(getattr(v2, f), getattr(c, f)), f
         assert (v.max_group, v.max_finished) == (c.max_group, c.max_finished)
     eng.close()
-
-
-@pytest.mark.parametrize("P,G", [(140000, 2500), (40000, 20000), (17000, 9000)])
-def test_queue_sort_table_sizes(pkg, oracle, snapshot_mod, P, G):
-    """Compare / queue order (core.go:368-411) across the sort kernel's regimes: more than 32 tiles of 4096 pods
-    (tile histograms read from global memory instead of the staged copy), several tiles per table with the
-    rank phases reusing a staged tile, and tables just above the single-CTA kernel's limit; ties in every key
-    field (few priorities, shared creation times, equal timestamps) so that stability decides the order."""
-    rng = np.random.default_rng(P)
-    snap = random_snapshot(7700 + G, P=P, N=48, G=G, L=5)
-    snap.pods.priority = rng.choice([0, 5, -3], snap.pods.n).astype(np.int32)
-    snap.pods.ts_ns = (rng.integers(0, 4000, snap.pods.n) * 1000003 + (1 << 40)).astype(np.int64)
-    snap.groups.creation_ns = (rng.integers(0, 300, snap.groups.n) * 7919 + (1 << 33)).astype(np.int64)
-    run_and_compare(pkg, oracle, snap, score=False)
