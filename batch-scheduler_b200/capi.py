@@ -22,6 +22,8 @@ OUT_FIT_BITMAP, OUT_SCORE, OUT_FILTER, OUT_TOPK, OUT_REASONS, OUT_PRIORITY = 0x1
 REASON_UNSCHEDULABLE, REASON_UNAVAILABLE, REASON_SELECTOR, REASON_TAINTS, REASON_LANE0 = range(5)
 TOPK_MAX = 32   # BS_TOPK_MAX: longest top-K list
 NONZERO_MAX = 1 << 56   # BS_NONZERO_MAX: largest non-zero request a priority column may hold
+PREF_NONE = 0xffffffff   # BS_PREF_NONE: pref_class of a pod without preferred node-affinity terms
+PREF_TABLE_MAX_BYTES = 1 << 30   # BS_PREF_TABLE_MAX_BYTES: cap of the class x node weight table
 # core.PreemptRemovePod verdicts (bs_remove_code) and the bound-pod flag
 REMOVE_ALLOW, REMOVE_OFFLINE_ONLINE, REMOVE_NOT_FOUND, REMOVE_LOCKED, REMOVE_SAME_GROUP = range(5)
 BOUND_GROUP_LOCKED = 0x01
@@ -158,6 +160,9 @@ SYMBOLS = {
     "bs_replay_priority": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, _p(ReplayResultC), C.c_void_p]),
     "bs_set_ratio_priority": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32,
                                         C.c_void_p, C.c_uint32]),
+    "bs_set_node_priority_weights": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32]),
+    "bs_upload_node_preferences": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p]),
+    "bs_upload_pod_preferences": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]),
     "bs_peer_init": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32]),
     "bs_peer_handle": (C.c_int, [C.c_void_p, C.c_void_p]),
     "bs_peer_attach": (C.c_int, [C.c_void_p, C.c_void_p]),

@@ -407,6 +407,15 @@ struct bs_engine {
   // RequestedToCapacityRatio (bs_set_ratio_priority): weight 0 = off; the shape table lives in d_ratio_tab
   RatioSetting ratio{};
   DevBuf d_ratio_tab;
+  // TaintToleration and preferred NodeAffinity (bs_set_node_priority_weights; 0, 0 = off): the node side
+  // (PreferNoSchedule masks [Npad], the class x node weights [classes][Npad]; dropped with the node table) and the pod
+  // side (tolerated masks [P], the class of each pod [P]; dropped with the pod table).  pref_class_max: the largest
+  // class a pod names (-1 none), checked against pref_classes at evaluation.
+  uint32_t w_taint = 0, w_naff = 0;
+  DevBuf d_prefer_taints, d_pref_weights, d_prefer_tol, d_pref_class;
+  bool have_pref_node = false, have_pref_pod = false;
+  uint32_t pref_classes = 0;
+  int64_t pref_class_max = -1;
   // sort scratch: views into one arena
   View d_gk0, d_gk1, d_pk0, d_pk1, d_idx_a, d_idx_b, d_ghist, d_group_rank, d_tilecnt, d_sort_barrier;
   uint32_t sort_max_grid = 1;
@@ -1079,6 +1088,12 @@ int evaluate_async_locked(bs_engine* e) {
     return fail(e, BS_E_STATE, "bs_evaluate: upload nodes, groups and pods first");
   if ((e->out_flags & BS_OUT_PRIORITY) && !(e->have_nz_node && e->have_nz_pod))
     return fail(e, BS_E_STATE, "bs_evaluate: BS_OUT_PRIORITY needs the node and pod non-zero columns");
+  if ((e->out_flags & BS_OUT_PRIORITY) && (e->w_taint || e->w_naff)) {
+    if (!(e->have_pref_node && e->have_pref_pod))
+      return fail(e, BS_E_STATE, "bs_evaluate: a non-zero node priority weight needs the node and pod preference columns");
+    if (e->w_naff && e->pref_class_max >= (int64_t)e->pref_classes)
+      return fail(e, BS_E_INDEX, "bs_evaluate: a pod's preference class is outside the uploaded weight table");
+  }
   if (e->peer_broken)
     return fail(e, BS_E_PEER, "peer exchange is broken (a rank did not arrive): bs_peer_detach on every rank, then init/attach again");
   BS_DEVICE_GUARD(e);
@@ -1343,15 +1358,33 @@ int evaluate_async_locked(bs_engine* e) {
     pa.node_req_present = e->d_rpres.as<uint32_t>();
     pa.ratio = e->ratio;
     const uint32_t grid = cdiv(P, PRIO_PODS_PER_CTA);
-    if (e->ratio.weight) {
-      if (L <= 5) priority_pod_kernel<5, true><<<grid, PRIO_THREADS, 0, e->s>>>(pa);
-      else if (L <= 9) priority_pod_kernel<9, true><<<grid, PRIO_THREADS, 0, e->s>>>(pa);
-      else priority_pod_kernel<16, true><<<grid, PRIO_THREADS, 0, e->s>>>(pa);
+    if (e->w_taint || e->w_naff) {
+      PriorityPrefArgs pp;
+      static_cast<PriorityRatioArgs&>(pp) = pa;
+      pp.prefer_taints = e->d_prefer_taints.as<uint64_t>();
+      pp.pref_weights = e->d_pref_weights.as<int32_t>();
+      pp.prefer_tol = e->d_prefer_tol.as<uint64_t>();
+      pp.pref_class = e->d_pref_class.as<uint32_t>();
+      pp.w_taint = e->w_taint;
+      pp.w_naff = e->w_naff;
+      if (e->ratio.weight) {
+        if (L <= 5) priority_pod_kernel<5, true, true><<<grid, PRIO_THREADS, 0, e->s>>>(pp);
+        else if (L <= 9) priority_pod_kernel<9, true, true><<<grid, PRIO_THREADS, 0, e->s>>>(pp);
+        else priority_pod_kernel<16, true, true><<<grid, PRIO_THREADS, 0, e->s>>>(pp);
+      } else {
+        if (L <= 5) priority_pod_kernel<5, false, true><<<grid, PRIO_THREADS, 0, e->s>>>(pp);
+        else if (L <= 9) priority_pod_kernel<9, false, true><<<grid, PRIO_THREADS, 0, e->s>>>(pp);
+        else priority_pod_kernel<16, false, true><<<grid, PRIO_THREADS, 0, e->s>>>(pp);
+      }
+    } else if (e->ratio.weight) {
+      if (L <= 5) priority_pod_kernel<5, true, false><<<grid, PRIO_THREADS, 0, e->s>>>(pa);
+      else if (L <= 9) priority_pod_kernel<9, true, false><<<grid, PRIO_THREADS, 0, e->s>>>(pa);
+      else priority_pod_kernel<16, true, false><<<grid, PRIO_THREADS, 0, e->s>>>(pa);
     } else {
       const PriorityArgs& pb = pa;
-      if (L <= 5) priority_pod_kernel<5, false><<<grid, PRIO_THREADS, 0, e->s>>>(pb);
-      else if (L <= 9) priority_pod_kernel<9, false><<<grid, PRIO_THREADS, 0, e->s>>>(pb);
-      else priority_pod_kernel<16, false><<<grid, PRIO_THREADS, 0, e->s>>>(pb);
+      if (L <= 5) priority_pod_kernel<5, false, false><<<grid, PRIO_THREADS, 0, e->s>>>(pb);
+      else if (L <= 9) priority_pod_kernel<9, false, false><<<grid, PRIO_THREADS, 0, e->s>>>(pb);
+      else priority_pod_kernel<16, false, false><<<grid, PRIO_THREADS, 0, e->s>>>(pb);
     }
     e->launches += 1;
   }
@@ -1573,6 +1606,7 @@ int bs_upload_nodes(bs_engine* e, const bs_node_table* t) {
   if (!e || !t) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
   e->have_nz_node = false;   // the non-zero column belongs to the node snapshot
+  e->have_pref_node = false;   // and so do the PreferNoSchedule masks and the preferred-affinity table
   if (t->n_lanes != e->L) return fail(e, BS_E_INVAL, "bs_upload_nodes: n_lanes differs from the engine's");
   const uint32_t N = t->n_nodes, L = e->L;
   const auto cols = node_cols(e, t);
@@ -1611,6 +1645,7 @@ int bs_update_nodes(bs_engine* e, const uint32_t* idx, const bs_node_table* t) {
   std::lock_guard<std::mutex> lk(e->mu);
   if (!e->have_nodes) return fail(e, BS_E_STATE, "bs_update_nodes: upload nodes first");
   e->have_nz_node = false;   // the changed rows' non-zero requests come with a new column
+  e->have_pref_node = false;   // ... and so do their taints and labels: the node preference side is uploaded again
   if (t->n_lanes != e->L) return fail(e, BS_E_INVAL, "bs_update_nodes: n_lanes differs from the engine's");
   const uint32_t n = t->n_nodes, L = e->L;
   if (!n) return BS_OK;
@@ -1742,6 +1777,7 @@ int bs_upload_pods(bs_engine* e, const bs_pod_table* t) {
   if (!e || !t) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
   e->have_nz_pod = false;   // the non-zero column belongs to the pod table
+  e->have_pref_pod = false;   // and so does the pod preference side
   if (t->n_lanes != e->L) return fail(e, BS_E_INVAL, "bs_upload_pods: n_lanes differs from the engine's");
   const uint32_t P = t->n_pods, L = e->L;
   if (P && (!t->req || !t->req_present || !t->gid || !t->sel_mask || !t->tol_mask || !t->priority ||
@@ -2485,6 +2521,9 @@ int bs_replay_priority(bs_engine* e, const uint32_t* queue, uint32_t n_queue, bs
                        int64_t* node_nonzero_after) {
   if (!e || !out) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
+  if (e->w_taint || e->w_naff)   // their maxima would have to follow the walk's live fit set, which is not built yet
+    return fail(e, BS_E_INVAL, "bs_replay_priority: TaintToleration and NodeAffinity are not supported in the walk; "
+                               "set both weights of bs_set_node_priority_weights to 0");
   return replay_walk(e, "bs_replay_priority", queue, n_queue, out, true, node_nonzero_after);
 }
 
@@ -2961,6 +3000,72 @@ int bs_upload_pod_nonzero(bs_engine* e, uint32_t n_pods, const int64_t* nz) {
                                 e->nz_pod_max);
   e->have_nz_pod = rc == BS_OK;
   return rc;
+}
+
+int bs_set_node_priority_weights(bs_engine* e, uint32_t taint_toleration, uint32_t node_affinity) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  e->w_taint = taint_toleration;
+  e->w_naff = node_affinity;
+  return BS_OK;
+}
+
+int bs_upload_node_preferences(bs_engine* e, uint32_t n_nodes, const uint64_t* prefer_taints, uint32_t n_classes,
+                               const int32_t* pref_weights) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  const char* who = "bs_upload_node_preferences";
+  auto bad = [&](int rc, const char* why) { return fail(e, rc, (std::string(who) + ": " + why).c_str()); };
+  e->have_pref_node = false;
+  if (!e->have_nodes) return bad(BS_E_STATE, "upload nodes first");
+  if (n_nodes != e->N) return bad(BS_E_INVAL, "n_nodes differs from the node table's");
+  const uint32_t Npad = e->Npad;
+  if ((uint64_t)n_classes * Npad * 4 > BS_PREF_TABLE_MAX_BYTES)
+    return bad(BS_E_INVAL, "n_classes x padded nodes x 4 bytes exceeds BS_PREF_TABLE_MAX_BYTES");
+  if (n_nodes && !prefer_taints) return bad(BS_E_INVAL, "null prefer_taints");
+  if (n_classes && n_nodes && !pref_weights) return bad(BS_E_INVAL, "null pref_weights");
+  for (size_t k = 0; k < (size_t)n_classes * n_nodes; ++k)
+    if (pref_weights[k] < 0) return bad(BS_E_RANGE, "a preferred-affinity weight is negative");
+  BS_DEVICE_GUARD(e);
+  CK(e->d_prefer_taints.ensure((size_t)std::max(Npad, 1u) * 8));
+  CK(cudaMemsetAsync(e->d_prefer_taints.p, 0, (size_t)Npad * 8, e->s));
+  if (n_nodes) CK(cudaMemcpyAsync(e->d_prefer_taints.p, prefer_taints, (size_t)n_nodes * 8, cudaMemcpyHostToDevice, e->s));
+  if (n_classes) {
+    CK(e->d_pref_weights.ensure((size_t)n_classes * Npad * 4));
+    CK(cudaMemsetAsync(e->d_pref_weights.p, 0, (size_t)n_classes * Npad * 4, e->s));
+    if (n_nodes)
+      CK(cudaMemcpy2DAsync(e->d_pref_weights.p, (size_t)Npad * 4, pref_weights, (size_t)n_nodes * 4, (size_t)n_nodes * 4,
+                           n_classes, cudaMemcpyHostToDevice, e->s));
+  }
+  CK(cudaStreamSynchronize(e->s));
+  e->pref_classes = n_classes;
+  e->have_pref_node = true;
+  return BS_OK;
+}
+
+int bs_upload_pod_preferences(bs_engine* e, uint32_t n_pods, const uint64_t* prefer_tol, const uint32_t* pref_class) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  const char* who = "bs_upload_pod_preferences";
+  auto bad = [&](int rc, const char* why) { return fail(e, rc, (std::string(who) + ": " + why).c_str()); };
+  e->have_pref_pod = false;
+  if (!e->have_pods) return bad(BS_E_STATE, "upload pods first");
+  if (n_pods != e->P) return bad(BS_E_INVAL, "n_pods differs from the pod table's");
+  if (n_pods && (!prefer_tol || !pref_class)) return bad(BS_E_INVAL, "null column");
+  int64_t mx = -1;
+  for (uint32_t p = 0; p < n_pods; ++p)
+    if (pref_class[p] != BS_PREF_NONE) mx = std::max(mx, (int64_t)pref_class[p]);
+  BS_DEVICE_GUARD(e);
+  CK(e->d_prefer_tol.ensure((size_t)std::max(n_pods, 1u) * 8));
+  CK(e->d_pref_class.ensure((size_t)std::max(n_pods, 1u) * 4));
+  if (n_pods) {
+    CK(cudaMemcpyAsync(e->d_prefer_tol.p, prefer_tol, (size_t)n_pods * 8, cudaMemcpyHostToDevice, e->s));
+    CK(cudaMemcpyAsync(e->d_pref_class.p, pref_class, (size_t)n_pods * 4, cudaMemcpyHostToDevice, e->s));
+  }
+  CK(cudaStreamSynchronize(e->s));
+  e->pref_class_max = mx;
+  e->have_pref_pod = true;
+  return BS_OK;
 }
 
 int bs_fetch_priority_rows(bs_engine* e, uint32_t pod0, uint32_t n, int32_t* nodes, int64_t* scores) {

@@ -935,6 +935,7 @@ Status BatchSchedulingPlugin::BeginRound(const std::vector<const NodeInfo*>& sna
   node_names_.assign(snapshot.size(), std::string());
   snapshot_ = snapshot;
   pending_uid_.resize(pending.size());
+  pending_ = pending;
   for (size_t i = 0; i < pending.size(); ++i) pending_uid_[i] = pending[i]->uid;
   for (size_t i = 0; i < snapshot.size(); ++i)
     if (snapshot[i] && snapshot[i]->node) node_names_[i] = snapshot[i]->node->name;
@@ -970,6 +971,8 @@ Status BatchSchedulingPlugin::BeginRound(const std::vector<const NodeInfo*>& sna
   if ((rc = bs_upload_pods(eng_, &pt))) return fail(rc);
   {
     Status nst = UploadNonZero(&pending);
+    if (!nst.ok()) return nst;
+    nst = UploadPreferences();
     if (!nst.ok()) return nst;
   }
   {
@@ -1227,6 +1230,116 @@ Status BatchSchedulingPlugin::UploadNonZero(const std::vector<const Pod*>* pendi
   return Status{};
 }
 
+void BatchSchedulingPlugin::SetNodePriorityWeights(uint32_t taint_toleration, uint32_t node_affinity) {
+  std::lock_guard<std::mutex> lk(mu_);
+  node_prio_weights_[0] = taint_toleration;
+  node_prio_weights_[1] = node_affinity;
+}
+
+namespace {
+// canonical text of a pod's preferred terms of non-zero weight ("" = none): the class key of PackPreferences
+std::string preference_signature(const Pod& p) {
+  std::string s;
+  for (auto& t : p.preferred_affinity) {
+    if (t.weight == 0) continue;   // CalculateNodeAffinityPriorityMap skips it
+    s += 'W'; s += std::to_string(t.weight); s += '\x1f';
+    for (auto& r : t.preference.match_expressions) {
+      s += 'E'; s += r.key; s += '\x1f'; s += r.op; s += '\x1f';
+      for (auto& v : r.values) { s += v; s += '\x1d'; }
+      s += '\x1e';
+    }
+  }
+  return s;
+}
+}  // namespace
+
+Status BatchSchedulingPlugin::PackPreferences(const std::vector<const NodeInfo*>& snapshot,
+                                              const std::vector<const Pod*>& pending, PackedPreferences* out) {
+  if (!out) return Status{BS_CODE_ERROR, "PackPreferences: null output"};
+  PackedPreferences& pp = *out;
+  pp = PackedPreferences();
+  const size_t N = snapshot.size(), P = pending.size();
+  // the round's PreferNoSchedule dictionary: one bit per distinct (key, value)
+  pp.prefer_taints.assign(N, 0);
+  for (size_t i = 0; i < N; ++i) {
+    if (!snapshot[i] || !snapshot[i]->node) continue;
+    for (const Taint& t : snapshot[i]->node->taints) {
+      if (t.effect != "PreferNoSchedule") continue;
+      size_t b = 0;
+      while (b < pp.taints.size() && !(pp.taints[b].key == t.key && pp.taints[b].value == t.value)) ++b;
+      if (b == pp.taints.size()) {
+        if (b == 64) return Status{BS_CODE_ERROR, "PackPreferences: more than 64 distinct PreferNoSchedule taints in one round"};
+        pp.taints.push_back(t);
+      }
+      pp.prefer_taints[i] |= 1ull << b;
+    }
+  }
+  // each pod's tolerated bits (getAllTolerationPreferNoSchedule, then ToleratesTaint) and preferred class
+  pp.prefer_tol.assign(P, 0);
+  pp.pref_class.assign(P, BS_PREF_NONE);
+  std::unordered_map<std::string, uint32_t> class_of;
+  std::vector<const Pod*> class_pod;   // the first pod of each class
+  for (size_t p = 0; p < P; ++p) {
+    if (!pending[p]) continue;
+    const Pod& pod = *pending[p];
+    for (size_t b = 0; b < pp.taints.size(); ++b)
+      for (const Toleration& tol : pod.tolerations)
+        if ((tol.effect.empty() || tol.effect == "PreferNoSchedule") && tolerates(tol, pp.taints[b])) {
+          pp.prefer_tol[p] |= 1ull << b;
+          break;
+        }
+    for (auto& t : pod.preferred_affinity)
+      if (t.weight < 0) return Status{BS_CODE_ERROR, "PackPreferences: negative preferred-term weight in pod " + pod.ns + "/" + pod.name};
+    std::string sig = preference_signature(pod);
+    if (sig.empty()) continue;
+    auto it = class_of.find(sig);
+    if (it == class_of.end()) {
+      it = class_of.emplace(sig, (uint32_t)pp.class_signatures.size()).first;
+      pp.class_signatures.push_back(std::move(sig));
+      class_pod.push_back(&pod);
+    }
+    pp.pref_class[p] = it->second;
+  }
+  // the class x node table: terms whose (non-empty) match_expressions all match the node's labels
+  const uint32_t C = pp.n_classes();
+  pp.pref_weights.assign((size_t)C * N, 0);
+  for (uint32_t c = 0; c < C; ++c)
+    for (size_t i = 0; i < N; ++i) {
+      if (!snapshot[i] || !snapshot[i]->node) continue;
+      const auto& labels = snapshot[i]->node->labels;
+      int64_t sum = 0;
+      for (auto& t : class_pod[c]->preferred_affinity) {
+        if (t.weight == 0 || t.preference.match_expressions.empty()) continue;   // labels.Nothing()
+        bool ok = true, valid = true;
+        for (auto& r : t.preference.match_expressions) {
+          ok = requirement_matches(r, labels, &valid) && valid;   // an invalid requirement: the term counts 0
+          if (!ok) break;
+        }
+        if (ok) sum += t.weight;
+      }
+      if (sum > INT32_MAX) return Status{BS_CODE_ERROR, "PackPreferences: preferred-term weights above INT32_MAX"};
+      pp.pref_weights[(size_t)c * N + i] = (int32_t)sum;
+    }
+  return Status{};
+}
+
+Status BatchSchedulingPlugin::UploadPreferences() {
+  if (!priority_k_) return Status{};
+  auto fail = [&](int rc) {
+    return Status{BS_CODE_ERROR, std::string("bsched: ") + bs_strerror(rc) + " (" + bs_last_error(eng_) + ")"};
+  };
+  int rc = bs_set_node_priority_weights(eng_, node_prio_weights_[0], node_prio_weights_[1]);
+  if (rc) return fail(rc);
+  if (!node_prio_weights_[0] && !node_prio_weights_[1]) return Status{};
+  PackedPreferences pp;
+  Status st = PackPreferences(snapshot_, pending_, &pp);
+  if (!st.ok()) return st;
+  rc = bs_upload_node_preferences(eng_, (uint32_t)snapshot_.size(), pp.prefer_taints.data(), pp.n_classes(),
+                                  pp.pref_weights.data());
+  if (!rc) rc = bs_upload_pod_preferences(eng_, (uint32_t)pending_.size(), pp.prefer_tol.data(), pp.pref_class.data());
+  return rc ? fail(rc) : Status{};
+}
+
 std::vector<uint32_t> BatchSchedulingPlugin::ReasonCounts(const std::string& uid) const {
   const int32_t row = pod_row_.find(uid);
   const size_t R = 4 + packed_.lanes;
@@ -1259,6 +1372,10 @@ Status BatchSchedulingPlugin::UpdateRound(const std::vector<std::pair<uint32_t, 
   if (!st.ok()) return st;
   st = UpdateGroups(changed_groups, now_ns, false);
   if (!st.ok()) return st;
+  if (changed_nodes.empty()) {   // UpdateNodes uploaded the preferences and weights when it changed rows
+    st = UploadPreferences();
+    if (!st.ok()) return st;
+  }
   return Reevaluate();
 }
 
@@ -1307,6 +1424,8 @@ Status BatchSchedulingPlugin::UpdateNodes(const std::vector<std::pair<uint32_t, 
   st = UploadBound();   // bs_update_nodes dropped the bound-pod table: the changed NodeInfos list their pods again
   if (!st.ok()) return st;
   st = UploadNonZero(nullptr);   // ... and the node non-zero column: the changed NodeInfos' pods count again
+  if (!st.ok()) return st;
+  st = UploadPreferences();      // ... and the node preference side (its taint dictionary may change: both sides)
   if (!st.ok()) return st;
   // the round's decisions follow the new snapshot: same pods, same groups, same result vectors
   return evaluate ? Reevaluate() : Status{};
@@ -1533,6 +1652,9 @@ Status BatchSchedulingPlugin::ReplayQueue(std::vector<ReplayDecision>* out, Repl
   if (prio && !priority_k_)
     return Status{BS_CODE_ERROR, "ReplayQueue: kPriority needs a plugin created with priority_k > 0 (its rounds upload "
                                  "the non-zero request columns)"};
+  if (prio && (node_prio_weights_[0] || node_prio_weights_[1]))
+    return Status{BS_CODE_ERROR, "ReplayQueue: kPriority does not support TaintToleration and NodeAffinity yet "
+                                 "(SetNodePriorityWeights(0, 0) first)"};
   const uint32_t P = packed_.n_pods;
   std::vector<uint8_t> pf(P), rd(P);
   std::vector<int32_t> nd(P);

@@ -53,12 +53,19 @@ struct NodeSelectorTerm {
   std::vector<NodeSelectorRequirement> match_expressions;  // against node labels
   std::vector<NodeSelectorRequirement> match_fields;       // against node fields (metadata.name)
 };
+// v1.PreferredSchedulingTerm: one term of Spec.Affinity.NodeAffinity.PreferredDuringSchedulingIgnoredDuringExecution,
+// which kube-scheduler's NodeAffinity priority sums by weight over the nodes its preference matches
+struct PreferredSchedulingTerm {
+  int32_t weight = 0;               // 1..100 upstream; a term of weight 0 is skipped
+  NodeSelectorTerm preference;      // only match_expressions are read; an empty list matches nothing
+};
 struct Pod {
   std::string ns, name, uid;
   std::map<std::string, std::string> labels;
   std::map<std::string, std::string> node_selector;
   bool has_required_affinity = false;                 // the required node-affinity field is non-nil
   std::vector<NodeSelectorTerm> required_affinity;    // its terms, ORed; an empty term matches nothing
+  std::vector<PreferredSchedulingTerm> preferred_affinity;   // the PREFERRED node-affinity terms (NodeAffinity priority)
   std::vector<Toleration> tolerations;
   std::vector<Container> containers;
   std::vector<std::string> owner_uids;  // OwnerReferences[].UID (core.go:483-485)
@@ -155,6 +162,20 @@ struct PackedSnapshot {
   bs_node_table node_table() const;
   bs_pod_table pod_table() const;
   bs_group_table group_table() const;
+};
+
+// The columns of the TaintToleration and preferred NodeAffinity priorities of one round (bs_upload_node_preferences,
+// bs_upload_pod_preferences): the round's dictionary of distinct PreferNoSchedule taints (key, value), each node's bits
+// of it and each pending pod's tolerated bits; the pods' distinct preferred-affinity classes (by the canonical text of
+// their weighted terms) and the class x node table of summed weights.
+struct PackedPreferences {
+  std::vector<Taint> taints;                    // bit b of the masks
+  std::vector<uint64_t> prefer_taints;          // [n_nodes]
+  std::vector<uint64_t> prefer_tol;             // [n_pods]
+  std::vector<uint32_t> pref_class;             // [n_pods], BS_PREF_NONE = no preferred term of non-zero weight
+  std::vector<std::string> class_signatures;    // canonical text of each class
+  std::vector<int32_t> pref_weights;            // [n_classes][n_nodes]
+  uint32_t n_classes() const { return (uint32_t)class_signatures.size(); }
 };
 
 // string -> row index of one round, built in one go: the keys are copied into ONE arena (no allocation per key),
@@ -325,6 +346,11 @@ class BatchSchedulingPlugin {
   // weight of resources with capacity 0 everywhere.  An invalid setting returns an error and the previous one stays.
   Status SetRatioPriority(uint32_t weight, const std::vector<std::pair<uint32_t, uint32_t>>& shape,
                           const std::map<std::string, uint32_t>& resources);
+  // weights of kube-scheduler v1.17's TaintToleration and preferred NodeAffinity priorities in PriorityNodes
+  // (bs_set_node_priority_weights; 0, 0 = off, the default; v1.17's default profile is 1, 1), from the next round or
+  // delta round on, on a plugin created with priority_k > 0.  While either is non-zero, ReplayQueue(kPriority) returns
+  // an error.
+  void SetNodePriorityWeights(uint32_t taint_toleration, uint32_t node_affinity);
   int group_index(const std::string& ns_name) const;
   double last_pack_ms() const { return last_pack_ms_; }
   double last_device_ms() const { return last_device_ms_; }
@@ -389,6 +415,13 @@ class BatchSchedulingPlugin {
   // and pod overhead are not modelled.
   static Status PackNonZero(const std::vector<const NodeInfo*>& snapshot, const std::vector<const Pod*>& pending,
                             std::vector<int64_t>* node_nz, std::vector<int64_t>* pod_nz);
+  // The columns of the TaintToleration and preferred NodeAffinity priorities (no GPU): a node's PreferNoSchedule taints
+  // as bits of the round's dictionary (more than 64 distinct ones is an error); a pod tolerates a bit when one of its
+  // tolerations with an empty or PreferNoSchedule effect tolerates the taint (ToleratesTaint); a class's weight on a
+  // node sums the weights of its terms whose match_expressions all match the node's labels.  A term with an invalid
+  // requirement counts 0 there (upstream, it fails the pod's scoring); a negative weight is an error.
+  static Status PackPreferences(const std::vector<const NodeInfo*>& snapshot, const std::vector<const Pod*>& pending,
+                                PackedPreferences* out);
 
   static Status Pack(const std::vector<const NodeInfo*>& snapshot, const std::vector<const Pod*>& pending,
                      const std::vector<PodGroup>& groups, const std::vector<uint32_t>& matched,
@@ -417,6 +450,7 @@ class BatchSchedulingPlugin {
   uint32_t ratio_weight_ = 0;                          // SetRatioPriority: shape in engine units, weights by name
   std::vector<uint32_t> ratio_util_{0, 100}, ratio_score_{100, 0};
   std::map<std::string, uint32_t> ratio_resources_{{"cpu", 1}, {"memory", 1}};
+  uint32_t node_prio_weights_[2] = {0, 0};             // SetNodePriorityWeights: TaintToleration, NodeAffinity
   std::string init_error_;
   int64_t max_schedule_time_ns_;
   std::map<std::string, GroupState> groups_;                        // ordered: canonical table order
@@ -448,10 +482,13 @@ class BatchSchedulingPlugin {
   int FetchPriority();   // the round's priority lists into prio_node_ / prio_score_ (no-op without priority_k)
   Status UploadNonZero(const std::vector<const Pod*>* pending);   // node column of snapshot_ (+ the pods'); no-op without
                                                                   // priority_k
+  Status UploadPreferences();   // both preference sides of snapshot_ and pending_ and the two weights; the columns only
+                                // while a weight is non-zero; no-op without priority_k
   Status UploadBound();  // packs and uploads the bound-pod table of snapshot_ (no-op when no NodeInfo lists pods)
   Status RunPreempt(const std::vector<uint32_t>& rows, std::vector<Preemption>* out);
   std::vector<const NodeInfo*> snapshot_;                           // the round's NodeInfos (bound pods)
   std::vector<std::string> pending_uid_;                            // pending index -> uid
+  std::vector<const Pod*> pending_;                                 // the round's pending pods (preferences)
   PackedBound bound_;
   StrIndex bound_row_;                                              // uid -> bound-table row
 };

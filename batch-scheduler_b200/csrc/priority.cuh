@@ -5,7 +5,8 @@
 // The fit set is the reason rows' (kernels.cuh K1c/K1d): a node fits a pod when its class gate bit is set and no lane
 // is short (lane_short over node_left_kernel's full-width residuals), the invariant DESIGN §2 states for reason rows.
 // The lists are kept with gang_fit's topk_insert (fit.cuh); the pair scorer pair_score is kernels.cuh's, and with RATIO
-// the RequestedToCapacityRatio term (kernels.cuh ratio_*) is added to it.
+// the RequestedToCapacityRatio term (kernels.cuh ratio_*) is added to it; with PREF the TaintToleration and preferred
+// NodeAffinity terms (bs_set_node_priority_weights), normalized over the pod's fit set.
 #pragma once
 #include "kernels.cuh"
 #include "fit.cuh"
@@ -50,9 +51,42 @@ struct PriorityRatioArgs : PriorityArgs {
   const uint32_t* node_req_present;     // [Npad]
   RatioSetting ratio;
 };
-template <int MAXL, bool RATIO>
+// PREF's arguments (bs_upload_node_preferences / bs_upload_pod_preferences): the PreferNoSchedule taints of each node
+// and the tolerated ones of each pod, the preferred-affinity class of each pod and the class x node weight table, and
+// the two weights.  Derived from the ratio's type for the same reason; the ratio fields are read only with RATIO.
+constexpr uint32_t PREF_NONE = 0xffffffffu;   // BS_PREF_NONE
+struct PriorityPrefArgs : PriorityRatioArgs {
+  const uint64_t* prefer_taints;   // [Npad] (padding 0)
+  const int32_t* pref_weights;     // [classes][Npad] (padding 0)
+  const uint64_t* prefer_tol;      // [P]
+  const uint32_t* pref_class;      // [P] row of pref_weights or PREF_NONE
+  uint32_t w_taint, w_naff;
+};
+// The raw counts of PREF for one (pod, node): t = PreferNoSchedule taints of the node the pod does not tolerate,
+// a = the summed weights of the pod's preferred terms the node matches.  A weight of 0 skips its read (uniform).
+__device__ __forceinline__ void pref_counts(const PriorityPrefArgs& a, uint64_t taints, uint64_t tol, uint32_t cls,
+                                            uint32_t i, uint32_t& t, uint32_t& aw) {
+  t = a.w_taint ? (uint32_t)__popcll(taints & ~tol) : 0u;
+  aw = (a.w_naff && cls != PREF_NONE) ? (uint32_t)a.pref_weights[(size_t)cls * a.Npad + i] : 0u;
+}
+// TaintToleration + NodeAffinity of one fitting pair, normalized by the pod's maxima over its fit set (NormalizeReduce
+// with MaxNodeScore 100; reversed for the taints), weighted, int64 wrapping
+__device__ __forceinline__ uint64_t pref_term(const PriorityPrefArgs& a, uint32_t t, uint32_t aw, uint32_t mt,
+                                              uint32_t ma) {
+  const int64_t tt = mt == 0 ? 100 : 100 - (int64_t)100 * t / mt;
+  const int64_t na = ma == 0 ? 0 : (int64_t)100 * aw / ma;
+  return (uint64_t)a.w_taint * (uint64_t)tt + (uint64_t)a.w_naff * (uint64_t)na;
+}
+
+// PREF (chosen by the host when either weight of bs_set_node_priority_weights is non-zero) adds w_taint * TT +
+// w_naff * NA.  Both are normalized by the maximum raw count over the pod's fit set, and floor(100 * a / Ma) re-orders
+// nodes already seen when Ma grows, so every maximum has to be known before the first pair is scored: the warp first
+// sweeps the nodes once with the same fit test, keeping the largest t and a of each of its pods over the nodes that
+// fit, and reduces them across its lanes.  The sweep lives in the kernel (not a [2][P] pre-pass) because its fit test
+// needs the pod's requests and gate row, which the warp has already loaded for the scoring sweep.
+template <int MAXL, bool RATIO, bool PREF>
 __global__ void __launch_bounds__(PRIO_THREADS)
-priority_pod_kernel(std::conditional_t<RATIO, PriorityRatioArgs, PriorityArgs> a) {
+priority_pod_kernel(std::conditional_t<PREF, PriorityPrefArgs, std::conditional_t<RATIO, PriorityRatioArgs, PriorityArgs>> a) {
   constexpr int WARPS = PRIO_THREADS / 32;
   __shared__ int64_t s_req[WARPS][PRIO_PPW][MAXL];
   __shared__ int64_t s_ls[WARPS][PRIO_PPW][32];
@@ -91,6 +125,54 @@ priority_pod_kernel(std::conditional_t<RATIO, PriorityRatioArgs, PriorityArgs> a
     nz_mem[j] = ok ? a.pod_nz[(size_t)a.P + p] : 0;
     thr[j] = INT64_MIN;
     nfit[j] = 0;
+  }
+  [[maybe_unused]] uint64_t ptol[PRIO_PPW];
+  [[maybe_unused]] uint32_t pcls[PRIO_PPW], mt[PRIO_PPW], ma[PRIO_PPW];   // PREF: the pod's maxima over its fit set
+  if constexpr (PREF) {
+#pragma unroll
+    for (int j = 0; j < PRIO_PPW; ++j) {
+      const uint32_t p = p0 + j;
+      ptol[j] = rmask[j] && a.w_taint ? a.prefer_tol[p] : 0;   // a column whose weight is 0 may be missing
+      pcls[j] = rmask[j] && a.w_naff ? a.pref_class[p] : PREF_NONE;
+      mt[j] = ma[j] = 0;
+    }
+    // the first sweep: the fit test of the scoring sweep below, then the raw counts of the fitting nodes
+    for (uint32_t base = 0; base < a.N; base += 32) {
+      const uint32_t i = base + lane, w = base >> 5;
+      bool g[PRIO_PPW];
+      uint32_t any = 0;
+#pragma unroll
+      for (int j = 0; j < PRIO_PPW; ++j) {
+        const uint32_t gw = rmask[j] ? grow[j][w] : 0u;
+        any |= gw;
+        g[j] = (gw >> lane) & 1u;
+      }
+      if (!any) continue;   // warp-uniform
+      const uint32_t lp = a.left_present[i] | 0xFu;
+#pragma unroll
+      for (int d = 0; d < MAXL; ++d) {
+        if (d >= L) break;
+        const int64_t v = a.left[(size_t)d * a.Npad + i];
+        const bool pres = (lp >> d) & 1u;
+#pragma unroll
+        for (int j = 0; j < PRIO_PPW; ++j)
+          if (((rmask[j] >> d) & 1u) && lane_short(pres, v, s_req[wid][j][d])) g[j] = false;
+      }
+      const uint64_t taints = a.w_taint ? a.prefer_taints[i] : 0;
+#pragma unroll
+      for (int j = 0; j < PRIO_PPW; ++j) {
+        if (!g[j]) continue;
+        uint32_t t, aw;
+        pref_counts(a, taints, ptol[j], pcls[j], i, t, aw);
+        mt[j] = max(mt[j], t);
+        ma[j] = max(ma[j], aw);
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < PRIO_PPW; ++j) {
+      mt[j] = __reduce_max_sync(0xffffffffu, mt[j]);
+      ma[j] = __reduce_max_sync(0xffffffffu, ma[j]);
+    }
   }
   for (uint32_t base = 0; base < a.N; base += 32) {
     const uint32_t i = base + lane, w = base >> 5;
@@ -155,6 +237,12 @@ priority_pod_kernel(std::conditional_t<RATIO, PriorityRatioArgs, PriorityArgs> a
       int64_t s = g[j] ? pair_score(n_cpu + nz_cpu[j], c_cpu, n_mem + nz_mem[j], c_mem, a.w) : INT64_MIN;
       if constexpr (RATIO)
         if (g[j]) s = (int64_t)((uint64_t)s + ratio_term(a.ratio.weight, rnum[j], rden[j]));
+      if constexpr (PREF)
+        if (g[j]) {
+          uint32_t t, aw;
+          pref_counts(a, a.w_taint ? a.prefer_taints[i] : 0, ptol[j], pcls[j], i, t, aw);
+          s = (int64_t)((uint64_t)s + pref_term(a, t, aw, mt[j], ma[j]));
+        }
       const uint32_t cb = __ballot_sync(0xffffffffu, g[j] && (nfit[j] < a.K || s > thr[j]));
       if (cb) thr[j] = topk_insert<int64_t>(s_ls[wid][j], s_ln[wid][j], a.K, cb, s, (int32_t)base, lane);
       nfit[j] += __popc(fw[j]);

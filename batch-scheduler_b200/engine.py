@@ -295,6 +295,32 @@ class Engine:
             a = np.ascontiguousarray(pods, dtype=np.int64)
             self._check(self.lib.bs_upload_pod_nonzero(self.h, a.shape[1] if a.ndim == 2 else 0, capi.ptr(a)))
 
+    def set_node_priority_weights(self, taint_toleration: int = 0, node_affinity: int = 0):
+        """Weights of kube-scheduler's TaintToleration and preferred NodeAffinity priorities in the priority score
+        (0, 0 = off, the default; v1.17's default profile is 1, 1).  A non-zero weight needs upload_preferences before
+        each round, and makes replay(priority=True) refuse to run."""
+        self._check(self.lib.bs_set_node_priority_weights(self.h, taint_toleration, node_affinity))
+
+    def upload_preferences(self, node=None, pods=None):
+        """The columns of the two node priorities.  node = (prefer_taints [N] uint64, pref_weights [C, N] int32): bit b
+        of prefer_taints is PreferNoSchedule taint b of the round's dictionary, pref_weights[c, n] the summed weights of
+        class c's preferred terms that node n matches.  pods = (prefer_tol [P] uint64, pref_class [P] uint32): the bits
+        each pod tolerates and its class (capi.PREF_NONE: no preferred terms).  Uploading nodes (or updating node rows)
+        drops the node side, uploading pods the pod side."""
+        if node is not None:
+            taints = np.ascontiguousarray(node[0], dtype=np.uint64).reshape(-1)
+            w = np.ascontiguousarray(node[1], dtype=np.int32)
+            if w.ndim != 2 or w.shape[1] != len(taints):
+                raise ValueError("pref_weights must be [classes, N] with N = len(prefer_taints)")
+            self._check(self.lib.bs_upload_node_preferences(self.h, len(taints), capi.ptr(taints), w.shape[0],
+                                                            capi.ptr(w)))
+        if pods is not None:
+            tol = np.ascontiguousarray(pods[0], dtype=np.uint64).reshape(-1)
+            cls = np.ascontiguousarray(pods[1], dtype=np.uint32).reshape(-1)
+            if len(tol) != len(cls):
+                raise ValueError("prefer_tol and pref_class must have one entry per pod")
+            self._check(self.lib.bs_upload_pod_preferences(self.h, len(tol), capi.ptr(tol), capi.ptr(cls)))
+
     def priority_rows(self, pod0=0, n=None):
         """(nodes [n, K] int32, scores [n, K] int64): each pod's fitting nodes by priority score descending, then node
         index ascending; min(K, feasible_count) entries, padded with node -1 and score INT64_MIN."""

@@ -371,6 +371,37 @@ def nonzero_requests(snap: Snapshot, seed: int, explicit_zero: float = 0.1, unse
     return np.clip(node, 0, NONZERO_MAX), np.clip(pod, 0, NONZERO_MAX)
 
 
+PREF_NONE = 0xFFFFFFFF   # BS_PREF_NONE
+
+
+def node_preferences(snap: Snapshot, seed: int, n_bits: int = 6, tainted: float = 0.3, tolerate: float = 0.4,
+                     tolerate_all: float = 0.1, n_classes: int = 5, terms: int = 3, match: float = 0.3,
+                     no_class: float = 0.3):
+    """Seeded columns of the TaintToleration and preferred NodeAffinity priorities for a table without objects:
+    (prefer_taints [N] uint64, pref_weights [n_classes, N] int32, prefer_tol [P] uint64, pref_class [P] uint32).
+    A share `tainted` of the nodes carries a random non-empty subset of n_bits PreferNoSchedule taints; a pod tolerates
+    each bit with probability `tolerate`, or every bit with `tolerate_all`.  A class is `terms` preferred terms of
+    weight 1..100, each matching a node with probability `match`; a pod has no class (PREF_NONE) with `no_class`."""
+    rng = np.random.default_rng(seed)
+    N, P = snap.nodes.n, snap.pods.n
+    bits = rng.random((N, n_bits)) < 0.5
+    bits[np.arange(N), rng.integers(0, max(n_bits, 1), N)] = True   # non-empty
+    taint_bits = (bits & (rng.random(N) < tainted)[:, None]) if n_bits else np.zeros((N, 0), bool)
+    weights_of_bits = np.uint64(1) << np.arange(n_bits, dtype=np.uint64)
+    prefer_taints = (taint_bits.astype(np.uint64) * weights_of_bits).sum(axis=1, dtype=np.uint64)
+    tol_bits = (rng.random((P, n_bits)) < tolerate) | (rng.random(P) < tolerate_all)[:, None]
+    prefer_tol = (tol_bits.astype(np.uint64) * weights_of_bits).sum(axis=1, dtype=np.uint64)
+    pref_weights = np.zeros((n_classes, N), np.int64)
+    for c in range(n_classes):
+        for _ in range(terms):
+            pref_weights[c] += np.where(rng.random(N) < match, int(rng.integers(1, 101)), 0)
+    pref_class = rng.integers(0, max(n_classes, 1), P).astype(np.uint32)
+    if n_classes == 0:
+        pref_class[:] = PREF_NONE
+    pref_class[rng.random(P) < no_class] = PREF_NONE
+    return prefer_taints.astype(np.uint64), pref_weights.astype(np.int32), prefer_tol.astype(np.uint64), pref_class
+
+
 # ----------------------------------------------------------------------------
 # splitmix64 stream (vectorised): value i of the stream with seed s is
 # mix(s + (i+1)*0x9E3779B97F4A7C15).

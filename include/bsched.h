@@ -492,6 +492,31 @@ int bs_replay_priority(bs_engine* e, const uint32_t* queue, uint32_t n_queue, bs
  * v1.17's policy file gives shape scores in 0..10 and the scheduler multiplies them by 10: the caller scales. */
 int bs_set_ratio_priority(bs_engine* e, uint32_t weight, uint32_t n_points, const uint32_t* utilization,
                           const uint32_t* score, uint32_t n_lanes, const uint32_t* lane_weight, uint32_t absent_weight);
+/* kube-scheduler v1.17's TaintToleration and (preferred) NodeAffinity priorities, added to the BS_OUT_PRIORITY score
+ * with weights taint_toleration and node_affinity (0, 0 = off, the default; v1.17's default profile is 1, 1).  Any
+ * time, read by the next evaluation.  Per (pod p, node n) [upstream, from memory]:
+ *     t(p, n) = popcount(prefer_taints[n] & ~prefer_tol[p])   the node's PreferNoSchedule taints p does not tolerate
+ *     a(p, n) = pref_weights[pref_class[p]][n], 0 for BS_PREF_NONE   the weights of p's preferred terms n matches
+ *     Mt, Ma = the maxima of t and a over the pod's fit set (the nodes of its fit-bitmap row; no other node counts)
+ *     TT = Mt == 0 ? 100 : 100 - 100 * t / Mt         NA = Ma == 0 ? 0 : 100 * a / Ma       (int64, truncating)
+ *     score = <the score above> + taint_toleration * TT + node_affinity * NA                 (int64, two's complement wrap)
+ * An evaluation with BS_OUT_PRIORITY and a non-zero weight is BS_E_STATE before anything is launched when a column it
+ * needs is missing (taint_toleration: both masks; node_affinity: the weight table and the class column), and
+ * BS_E_INDEX when node_affinity is non-zero and a pod's class is >= n_classes.  bs_replay_priority refuses to run
+ * (BS_E_INVAL) while either weight is non-zero. */
+int bs_set_node_priority_weights(bs_engine* e, uint32_t taint_toleration, uint32_t node_affinity);
+#define BS_PREF_NONE 0xffffffffu                 /* pref_class of a pod without preferred terms (a = 0) */
+#define BS_PREF_TABLE_MAX_BYTES (1ull << 30)     /* n_classes x Npad x 4 (Npad: n_nodes rounded up) at most 1 GiB */
+/* prefer_taints[n_nodes]: bit b = the node carries the round's PreferNoSchedule taint b (the caller's dictionary of
+ * distinct key/value pairs, at most 64); pref_weights[n_classes][n_nodes]: a(class, node), each in [0, INT32_MAX].
+ * n_nodes must equal the node table's (else BS_E_INVAL), a table above BS_PREF_TABLE_MAX_BYTES is BS_E_INVAL, a
+ * negative weight BS_E_RANGE; a failing call leaves the side dropped.  The side belongs to the node snapshot:
+ * bs_upload_nodes and bs_update_nodes drop it. */
+int bs_upload_node_preferences(bs_engine* e, uint32_t n_nodes, const uint64_t* prefer_taints, uint32_t n_classes,
+                               const int32_t* pref_weights);
+/* prefer_tol[n_pods]: the bits of the dictionary each pod tolerates; pref_class[n_pods]: its row of pref_weights or
+ * BS_PREF_NONE.  n_pods must equal the pod table's (else BS_E_INVAL); bs_upload_pods drops the side. */
+int bs_upload_pod_preferences(bs_engine* e, uint32_t n_pods, const uint64_t* prefer_tol, const uint32_t* pref_class);
 
 /* ---- preemption: PreFilterExtensions.RemovePod and the node / victims kube-scheduler's preemption would pick ----
  * The bound-pod table lists the pods already running on the snapshot's nodes (NodeInfo.Pods()).  Rows may come in

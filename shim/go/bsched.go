@@ -187,6 +187,39 @@ func (e *Engine) SetRatioPriority(weight uint32, shape []RatioPoint, laneWeights
 		C.uint32_t(absentWeight)))
 }
 
+// SetNodePriorityWeights adds kube-scheduler's TaintToleration and preferred NodeAffinity priorities to the priority
+// score (0, 0 = off; v1.17's default profile is 1, 1).  While either is non-zero ReplayPriority is refused.
+func (e *Engine) SetNodePriorityWeights(taintToleration, nodeAffinity uint32) error {
+	return e.rc(C.bs_set_node_priority_weights(e.h, C.uint32_t(taintToleration), C.uint32_t(nodeAffinity)))
+}
+
+// UploadNodePreferences: per node the bits of the round's PreferNoSchedule taint dictionary it carries, and the
+// class x node table prefWeights[nClasses][n] of summed preferred-term weights.  UploadNodes / UpdateNodes drop it.
+func (e *Engine) UploadNodePreferences(preferTaints []uint64, prefWeights []int32) error {
+	n := len(preferTaints)
+	if n == 0 {
+		return e.rc(C.bs_upload_node_preferences(e.h, 0, nil, 0, nil))
+	}
+	classes := len(prefWeights) / n
+	var wp *C.int32_t
+	if classes > 0 {
+		wp = (*C.int32_t)(unsafe.Pointer(&prefWeights[0]))
+	}
+	return e.rc(C.bs_upload_node_preferences(e.h, C.uint32_t(n), (*C.uint64_t)(unsafe.Pointer(&preferTaints[0])),
+		C.uint32_t(classes), wp))
+}
+
+// UploadPodPreferences: per pod the dictionary bits it tolerates and its row of the class table (BS_PREF_NONE for a
+// pod without preferred terms).  UploadPods drops it.
+func (e *Engine) UploadPodPreferences(preferTol []uint64, prefClass []uint32) error {
+	n := len(preferTol)
+	if n == 0 || len(prefClass) != n {
+		return e.rc(C.bs_upload_pod_preferences(e.h, C.uint32_t(n), nil, nil))
+	}
+	return e.rc(C.bs_upload_pod_preferences(e.h, C.uint32_t(n), (*C.uint64_t)(unsafe.Pointer(&preferTol[0])),
+		(*C.uint32_t)(unsafe.Pointer(&prefClass[0]))))
+}
+
 // UploadNodeNonZero / UploadPodNonZero: the non-zero request columns, nz[2][n] (cpu millicores, then memory bytes):
 // per pod the sum over its containers of GetNonzeroRequestForResource(Requests), per node NodeInfo.NonZeroRequest().
 // UploadNodes / UpdateNodes drop the node column and UploadPods the pod column: upload them again before Evaluate.
