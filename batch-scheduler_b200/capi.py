@@ -173,6 +173,7 @@ SYMBOLS = {
     "bs_kernel_ms": (C.c_int, [C.c_void_p, C.c_int, _p(C.c_float), _p(C.c_uint32)]),
     "bs_launch_count": (C.c_uint64, [C.c_void_p]),
     "bs_fit_shape": (C.c_int, [C.c_void_p, _p(C.c_uint32), _p(C.c_uint32), _p(C.c_uint32)]),
+    "bs_fit_lanes": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "bs_sort_shape": (C.c_int, [C.c_void_p, _p(C.c_uint32), _p(C.c_uint32), _p(C.c_uint32), _p(C.c_uint32)]),
 }
 

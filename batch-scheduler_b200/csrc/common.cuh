@@ -39,8 +39,8 @@ struct LaneMap {
   uint8_t narrow[BS_MAX_LANES];  // original lane index of narrow slot k (k < LN)
   uint8_t scaled[BS_MAX_LANES];  // original lane index of scaled slot k (k < LS)
   uint8_t sunit[BS_MAX_LANES];   // k: the slot's unit is 2^k
-  uint8_t sshift[BS_MAX_LANES];  // min(k, 28): shift back to original units after the clamp
-  uint32_t sclamp[BS_MAX_LANES]; // C = 2^(28-k), or 1 when k > 28
+  uint8_t sshift[BS_MAX_LANES];  // min(k, FIT_CAP_LOG2 = 27): shift back to original units after the clamp
+  uint32_t sclamp[BS_MAX_LANES]; // C = 2^(27-k), or 1 when k > 27
   uint32_t LW, LN, LS;
 };
 constexpr int NODE_TILE = 512;                          // nodes per shared-memory tile

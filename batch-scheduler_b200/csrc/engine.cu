@@ -3209,6 +3209,24 @@ int bs_fit_shape(bs_engine* e, uint32_t* wide, uint32_t* narrow, uint32_t* scale
   return BS_OK;
 }
 
+int bs_fit_lanes(bs_engine* e, uint8_t* kind, uint8_t* unit) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!e->lane_map_valid) return fail(e, BS_E_STATE, "bs_fit_lanes: evaluate first");
+  const LaneMap& lm = e->lane_map;
+  uint8_t k[BS_MAX_LANES] = {}, u[BS_MAX_LANES] = {};
+  for (uint32_t s = 0; s < lm.LN; ++s) k[lm.narrow[s]] = 1;
+  for (uint32_t s = 0; s < lm.LS; ++s) {
+    k[lm.scaled[s]] = 2;
+    u[lm.scaled[s]] = lm.sunit[s];
+  }
+  for (uint32_t d = 0; d < e->L; ++d) {
+    if (kind) kind[d] = k[d];
+    if (unit) unit[d] = u[d];
+  }
+  return BS_OK;
+}
+
 int bs_sort_shape(bs_engine* e, uint32_t* kernel, uint32_t* grid, uint32_t* group_passes, uint32_t* pod_passes) {
   if (!e) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);

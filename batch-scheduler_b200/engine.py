@@ -536,6 +536,13 @@ class Engine:
         self._check(self.lib.bs_fit_shape(self.h, C.byref(w), C.byref(n), C.byref(sc)))
         return {"LW": int(w.value), "LN": int(n.value), "LS": int(sc.value)}
 
+    def fit_lanes(self):
+        """(kind [L] uint8, unit [L] uint8) of the last evaluation's fit kernel: kind 0 wide, 1 narrow, 2 scaled;
+        unit k of a scaled lane (its values in units of 2^k), 0 otherwise."""
+        kind, unit = np.zeros(self.n_lanes, np.uint8), np.zeros(self.n_lanes, np.uint8)
+        self._check(self.lib.bs_fit_lanes(self.h, capi.ptr(kind), capi.ptr(unit)))
+        return kind, unit
+
     def sort_shape(self) -> dict:
         """What the last evaluation's queue sort launched: kernel (0 none, 1 single-CTA, 2 persistent lean,
         3 persistent wide), its grid in CTAs, and the radix passes kept for the group and the pod table."""

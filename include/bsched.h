@@ -624,6 +624,9 @@ uint64_t bs_launch_count(const bs_engine* e); /* kernels launched since bs_creat
  * |value| <= 2^27) and int32 in exact power-of-two units (scaled: every value of the lane a multiple of
  * 2^k, |value| >> k <= 2^29); wide + narrow + scaled == n_lanes */
 int bs_fit_shape(bs_engine* e, uint32_t* wide, uint32_t* narrow, uint32_t* scaled);
+/* per lane of the last evaluation's fit kernel: kind[d] 0 wide / 1 narrow / 2 scaled, unit[d] = k of a scaled lane
+ * (0 otherwise); BS_E_STATE before the first evaluation */
+int bs_fit_lanes(bs_engine* e, uint8_t* kind /*[n_lanes]*/, uint8_t* unit /*[n_lanes]*/);
 /* what the last evaluation's queue sort launched: kernel 0 none (both tables empty), 1 the single-CTA kernel
  * (max(n_pods, n_groups) <= 16384), 2 the persistent kernel's lean build (4 keys in flight per thread, beside a long
  * fit kernel), 3 its wide build (16 in flight); the grid in CTAs (4096-key tiles are shared out round-robin when there
