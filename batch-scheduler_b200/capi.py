@@ -24,6 +24,11 @@ TOPK_MAX = 32   # BS_TOPK_MAX: longest top-K list
 NONZERO_MAX = 1 << 56   # BS_NONZERO_MAX: largest non-zero request a priority column may hold
 PREF_NONE = 0xffffffff   # BS_PREF_NONE: pref_class of a pod without preferred node-affinity terms
 PREF_TABLE_MAX_BYTES = 1 << 30   # BS_PREF_TABLE_MAX_BYTES: cap of the class x node weight table
+IMAGE_NONE = 0xffffffff   # BS_IMAGE_NONE: image_class of a pod without dictionary images
+AVOID_NONE = 0xff         # BS_AVOID_NONE: avoid_bit of a pod without an RC / RS controller
+IMAGE_SIZE_MAX = 1 << 48  # BS_IMAGE_SIZE_MAX: largest image size in bytes
+LOC_CLASS_MAX = 64        # BS_LOC_CLASS_MAX: ids one image class may list
+LOC_TABLE_MAX_BYTES = 1 << 30   # BS_LOC_TABLE_MAX_BYTES: cap of the image bit rows and of the class x node IL table
 # core.PreemptRemovePod verdicts (bs_remove_code) and the bound-pod flag
 REMOVE_ALLOW, REMOVE_OFFLINE_ONLINE, REMOVE_NOT_FOUND, REMOVE_LOCKED, REMOVE_SAME_GROUP = range(5)
 BOUND_GROUP_LOCKED = 0x01
@@ -163,6 +168,10 @@ SYMBOLS = {
     "bs_set_node_priority_weights": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32]),
     "bs_upload_node_preferences": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p]),
     "bs_upload_pod_preferences": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]),
+    "bs_set_locality_weights": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32]),
+    "bs_upload_node_locality": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "bs_upload_pod_locality": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p,
+                                         C.c_void_p]),
     "bs_peer_init": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32]),
     "bs_peer_handle": (C.c_int, [C.c_void_p, C.c_void_p]),
     "bs_peer_attach": (C.c_int, [C.c_void_p, C.c_void_p]),

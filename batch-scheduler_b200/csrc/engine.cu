@@ -416,6 +416,18 @@ struct bs_engine {
   bool have_pref_node = false, have_pref_pod = false;
   uint32_t pref_classes = 0;
   int64_t pref_class_max = -1;
+  // ImageLocality and NodePreferAvoidPods (bs_set_locality_weights; 0, 0 = off): the node side (the image bit rows
+  // [n_images][ceil(N/32)] and sizes, the preferAvoidPods masks [Npad]; dropped with the node table) and the pod side
+  // (each pod's image class [P], the classes' CSR, each pod's controller bit [P]; dropped with the pod table); each
+  // side has its image part and its avoid part.  d_img_scaled and the class x node IL table d_loc_il are built on the
+  // device when loc_dirty (priority.cuh image_spread_kernel, locality_class_kernel).  loc_class_max / loc_image_max:
+  // the largest class a pod names and the largest id a class lists (-1 none), checked at evaluation.
+  uint32_t w_img = 0, w_avoid = 0;
+  DevBuf d_img_bits, d_img_size, d_img_scaled, d_avoid_mask, d_loc_class, d_loc_off, d_loc_ids, d_avoid_bit, d_loc_il;
+  bool have_img_node = false, have_avoid_node = false, have_img_pod = false, have_avoid_pod = false;
+  bool loc_dirty = true;
+  uint32_t loc_images = 0, loc_classes = 0;
+  int64_t loc_class_max = -1, loc_image_max = -1;
   // sort scratch: views into one arena
   View d_gk0, d_gk1, d_pk0, d_pk1, d_idx_a, d_idx_b, d_ghist, d_group_rank, d_tilecnt, d_sort_barrier;
   uint32_t sort_max_grid = 1;
@@ -789,18 +801,23 @@ void launch_prefix(uint32_t L, NodeTab t, PrefixSel ps, PrefixScratch sc, Prefix
   }
 }
 
+// loc: the scored walk with the locality terms (a is then a ReplayLocArgs)
 template <int MAXL>
-void launch_replay_t(const ReplayArgs& a, bool scored, cudaStream_t s) {
-  if (scored && a.ratio.weight) replay_kernel<MAXL, true, true><<<1, REPLAY_THREADS, 0, s>>>(a);
+void launch_replay_t(const ReplayArgs& a, bool scored, bool loc, cudaStream_t s) {
+  if (loc) {
+    const ReplayLocArgs& la = static_cast<const ReplayLocArgs&>(a);
+    if (a.ratio.weight) replay_kernel<MAXL, true, true, true><<<1, REPLAY_THREADS, 0, s>>>(la);
+    else replay_kernel<MAXL, true, false, true><<<1, REPLAY_THREADS, 0, s>>>(la);
+  } else if (scored && a.ratio.weight) replay_kernel<MAXL, true, true><<<1, REPLAY_THREADS, 0, s>>>(a);
   else if (scored) replay_kernel<MAXL, true><<<1, REPLAY_THREADS, 0, s>>>(a);
   else replay_kernel<MAXL, false><<<1, REPLAY_THREADS, 0, s>>>(a);
 }
 inline uint32_t replay_maxl(uint32_t L) { return L <= 5 ? 5u : L <= 9 ? 9u : 16u; }
-void launch_replay(uint32_t L, const ReplayArgs& a, bool scored, cudaStream_t s) {
+void launch_replay(uint32_t L, const ReplayArgs& a, bool scored, bool loc, cudaStream_t s) {
   switch (replay_maxl(L)) {
-    case 5: launch_replay_t<5>(a, scored, s); break;
-    case 9: launch_replay_t<9>(a, scored, s); break;
-    default: launch_replay_t<16>(a, scored, s); break;
+    case 5: launch_replay_t<5>(a, scored, loc, s); break;
+    case 9: launch_replay_t<9>(a, scored, loc, s); break;
+    default: launch_replay_t<16>(a, scored, loc, s); break;
   }
 }
 
@@ -1083,7 +1100,45 @@ int prepare_nodes(bs_engine* e) {
   return BS_OK;
 }
 
+// The columns a non-zero bs_set_locality_weights weight reads (BS_E_STATE when one is missing) and the ids they hold
+// (BS_E_INDEX), checked before anything is launched.
+int locality_check(bs_engine* e, const char* who) {
+  const std::string w(who);
+  if (e->w_img) {
+    if (!(e->have_img_node && e->have_img_pod))
+      return fail(e, BS_E_STATE, (w + ": a non-zero ImageLocality weight needs the node and pod image columns").c_str());
+    if (e->loc_class_max >= (int64_t)e->loc_classes)
+      return fail(e, BS_E_INDEX, (w + ": a pod's image class is outside the uploaded classes").c_str());
+    if (e->loc_image_max >= (int64_t)e->loc_images)
+      return fail(e, BS_E_INDEX, (w + ": an image class lists an id outside the node side's image dictionary").c_str());
+    // the pod side outlives node uploads: its class x node table is checked against the node table of now
+    if ((uint64_t)e->loc_classes * e->Npad > BS_LOC_TABLE_MAX_BYTES)
+      return fail(e, BS_E_INVAL, (w + ": n_classes x padded nodes bytes exceeds BS_LOC_TABLE_MAX_BYTES").c_str());
+  }
+  if (e->w_avoid && !(e->have_avoid_node && e->have_avoid_pod))
+    return fail(e, BS_E_STATE, (w + ": a non-zero NodePreferAvoidPods weight needs the node and pod avoid columns").c_str());
+  return BS_OK;
+}
+
+// The LOC pre-pass on the main stream: each name's scaled size, then the class x node IL table.  Only after either
+// side or a weight changed, and only while the ImageLocality weight is non-zero (else the table is not read).
+int locality_prepass(bs_engine* e) {
+  if (!e->loc_dirty || !e->w_img) return BS_OK;
+  const uint32_t C = e->loc_classes, I = e->loc_images;
+  if (C && e->Npad) {
+    CK(e->d_loc_il.ensure((size_t)C * e->Npad));
+    CK(e->d_img_scaled.ensure((size_t)std::max(I, 1u) * 8));
+    CK(launch_locality_prepass(e->d_img_bits.as<uint32_t>(), e->d_img_size.as<int64_t>(), e->d_img_scaled.as<int64_t>(),
+                               I, e->d_loc_off.as<uint32_t>(), e->d_loc_ids.as<uint32_t>(), e->d_loc_il.as<uint8_t>(), C,
+                               e->N, e->Npad, e->s));
+    e->launches += 2;
+  }
+  e->loc_dirty = false;
+  return BS_OK;
+}
+
 int evaluate_async_locked(bs_engine* e) {
+  int rc;
   if (!e->have_nodes || !e->have_pods || !e->have_groups)
     return fail(e, BS_E_STATE, "bs_evaluate: upload nodes, groups and pods first");
   if ((e->out_flags & BS_OUT_PRIORITY) && !(e->have_nz_node && e->have_nz_pod))
@@ -1094,10 +1149,10 @@ int evaluate_async_locked(bs_engine* e) {
     if (e->w_naff && e->pref_class_max >= (int64_t)e->pref_classes)
       return fail(e, BS_E_INDEX, "bs_evaluate: a pod's preference class is outside the uploaded weight table");
   }
+  if ((e->out_flags & BS_OUT_PRIORITY) && (rc = locality_check(e, "bs_evaluate"))) return rc;
   if (e->peer_broken)
     return fail(e, BS_E_PEER, "peer exchange is broken (a rank did not arrive): bs_peer_detach on every rank, then init/attach again");
   BS_DEVICE_GUARD(e);
-  int rc;
   bool reprepare = e->nodes_dirty;
   if (e->classes_dirty) {
     const bool pods_changed = e->pod_classes_dirty;   // the fit classes (class_fit bits) come from the pods only
@@ -1358,34 +1413,25 @@ int evaluate_async_locked(bs_engine* e) {
     pa.node_req_present = e->d_rpres.as<uint32_t>();
     pa.ratio = e->ratio;
     const uint32_t grid = cdiv(P, PRIO_PODS_PER_CTA);
-    if (e->w_taint || e->w_naff) {
-      PriorityPrefArgs pp;
-      static_cast<PriorityRatioArgs&>(pp) = pa;
-      pp.prefer_taints = e->d_prefer_taints.as<uint64_t>();
-      pp.pref_weights = e->d_pref_weights.as<int32_t>();
-      pp.prefer_tol = e->d_prefer_tol.as<uint64_t>();
-      pp.pref_class = e->d_pref_class.as<uint32_t>();
-      pp.w_taint = e->w_taint;
-      pp.w_naff = e->w_naff;
-      if (e->ratio.weight) {
-        if (L <= 5) priority_pod_kernel<5, true, true><<<grid, PRIO_THREADS, 0, e->s>>>(pp);
-        else if (L <= 9) priority_pod_kernel<9, true, true><<<grid, PRIO_THREADS, 0, e->s>>>(pp);
-        else priority_pod_kernel<16, true, true><<<grid, PRIO_THREADS, 0, e->s>>>(pp);
-      } else {
-        if (L <= 5) priority_pod_kernel<5, false, true><<<grid, PRIO_THREADS, 0, e->s>>>(pp);
-        else if (L <= 9) priority_pod_kernel<9, false, true><<<grid, PRIO_THREADS, 0, e->s>>>(pp);
-        else priority_pod_kernel<16, false, true><<<grid, PRIO_THREADS, 0, e->s>>>(pp);
-      }
-    } else if (e->ratio.weight) {
-      if (L <= 5) priority_pod_kernel<5, true, false><<<grid, PRIO_THREADS, 0, e->s>>>(pa);
-      else if (L <= 9) priority_pod_kernel<9, true, false><<<grid, PRIO_THREADS, 0, e->s>>>(pa);
-      else priority_pod_kernel<16, true, false><<<grid, PRIO_THREADS, 0, e->s>>>(pa);
-    } else {
-      const PriorityArgs& pb = pa;
-      if (L <= 5) priority_pod_kernel<5, false, false><<<grid, PRIO_THREADS, 0, e->s>>>(pb);
-      else if (L <= 9) priority_pod_kernel<9, false, false><<<grid, PRIO_THREADS, 0, e->s>>>(pb);
-      else priority_pod_kernel<16, false, false><<<grid, PRIO_THREADS, 0, e->s>>>(pb);
+    PriorityLocArgs la;
+    static_cast<PriorityRatioArgs&>(la) = pa;
+    la.prefer_taints = e->d_prefer_taints.as<uint64_t>();
+    la.pref_weights = e->d_pref_weights.as<int32_t>();
+    la.prefer_tol = e->d_prefer_tol.as<uint64_t>();
+    la.pref_class = e->d_pref_class.as<uint32_t>();
+    la.w_taint = e->w_taint;
+    la.w_naff = e->w_naff;
+    const bool pref = e->w_taint || e->w_naff, ratio = e->ratio.weight != 0;
+    if (e->w_img || e->w_avoid) {   // (the pre-pass runs on the same stream, ahead of the kernel)
+      if ((rc = locality_prepass(e))) return rc;
+      la.il = e->d_loc_il.as<uint8_t>();
+      la.avoid_mask = e->d_avoid_mask.as<uint64_t>();
+      la.loc_class = e->d_loc_class.as<uint32_t>();
+      la.avoid_bit = e->d_avoid_bit.as<uint8_t>();
+      la.w_img = e->w_img;
+      la.w_avoid = e->w_avoid;
     }
+    CK(launch_priority(L, grid, ratio, pref, e->w_img || e->w_avoid, la, e->s));
     e->launches += 1;
   }
   if (e->peer_attached) {
@@ -1607,6 +1653,7 @@ int bs_upload_nodes(bs_engine* e, const bs_node_table* t) {
   std::lock_guard<std::mutex> lk(e->mu);
   e->have_nz_node = false;   // the non-zero column belongs to the node snapshot
   e->have_pref_node = false;   // and so do the PreferNoSchedule masks and the preferred-affinity table
+  e->have_img_node = e->have_avoid_node = false;   // and the image rows and preferAvoidPods masks
   if (t->n_lanes != e->L) return fail(e, BS_E_INVAL, "bs_upload_nodes: n_lanes differs from the engine's");
   const uint32_t N = t->n_nodes, L = e->L;
   const auto cols = node_cols(e, t);
@@ -1646,6 +1693,7 @@ int bs_update_nodes(bs_engine* e, const uint32_t* idx, const bs_node_table* t) {
   if (!e->have_nodes) return fail(e, BS_E_STATE, "bs_update_nodes: upload nodes first");
   e->have_nz_node = false;   // the changed rows' non-zero requests come with a new column
   e->have_pref_node = false;   // ... and so do their taints and labels: the node preference side is uploaded again
+  e->have_img_node = e->have_avoid_node = false;   // ... and their images and annotations: so is the locality side
   if (t->n_lanes != e->L) return fail(e, BS_E_INVAL, "bs_update_nodes: n_lanes differs from the engine's");
   const uint32_t n = t->n_nodes, L = e->L;
   if (!n) return BS_OK;
@@ -1778,6 +1826,7 @@ int bs_upload_pods(bs_engine* e, const bs_pod_table* t) {
   std::lock_guard<std::mutex> lk(e->mu);
   e->have_nz_pod = false;   // the non-zero column belongs to the pod table
   e->have_pref_pod = false;   // and so does the pod preference side
+  e->have_img_pod = e->have_avoid_pod = false;   // and the pod locality side
   if (t->n_lanes != e->L) return fail(e, BS_E_INVAL, "bs_upload_pods: n_lanes differs from the engine's");
   const uint32_t P = t->n_pods, L = e->L;
   if (P && (!t->req || !t->req_present || !t->gid || !t->sel_mask || !t->tol_mask || !t->priority ||
@@ -2369,6 +2418,9 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
     return fail(e, BS_E_STATE, (w + ": upload nodes, groups and pods first").c_str());
   if (scored && !(e->have_nz_node && e->have_nz_pod))
     return fail(e, BS_E_STATE, (w + ": upload both non-zero request columns first").c_str());
+  const bool loc = scored && (e->w_img || e->w_avoid);
+  int rc;
+  if (loc && (rc = locality_check(e, who))) return rc;
   BS_DEVICE_GUARD(e);
   const uint32_t N = e->N, Npad = e->Npad, P = e->P, G = e->G, L = e->L;
   if (!queue) n_queue = P;
@@ -2380,8 +2432,8 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
   for (int r = 0; r < 2 && scored; ++r)
     if ((long double)e->nz_node_max[r] + (long double)n_queue * (long double)e->nz_pod_max[r] > 0x1p62L)
       return fail(e, BS_E_RANGE, (w + ": live non-zero requests could pass 2^62").c_str());
-  int rc;
   if (e->classes_dirty && (rc = rebuild_classes(e))) return rc;
+  if (loc && (rc = locality_prepass(e))) return rc;
 
   // scratch copies of everything the cycle mutates, the queue and the outputs, and the compact node state and
   // block cache the kernel builds (replay.cuh)
@@ -2425,7 +2477,8 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
   if (scored) CK(dup(n_nz, e->d_nz_node, (size_t)2 * Npad * 8));
   if (queue && n_queue) CK(cudaMemcpyAsync(d_queue.p, queue, (size_t)n_queue * 4, cudaMemcpyHostToDevice, e->s));
   CK(cudaMemsetAsync(d_status.p, 0, 128, e->s));
-  ReplayArgs a{};
+  ReplayLocArgs la{};
+  ReplayArgs& a = la;
   a.nt = node_tab(e);
   a.nt.requested = s_req.as<int64_t>();
   a.nt.pod_count = s_pc.as<int32_t>();
@@ -2469,9 +2522,17 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
     a.w = e->weights;
     a.ratio = e->ratio;
   }
+  if (loc) {
+    la.il = e->d_loc_il.as<uint8_t>();
+    la.avoid_mask = e->d_avoid_mask.as<uint64_t>();
+    la.loc_class = e->d_loc_class.as<uint32_t>();
+    la.avoid_bit = e->d_avoid_bit.as<uint8_t>();
+    la.w_img = e->w_img;
+    la.w_avoid = e->w_avoid;
+  }
   {
     StageTimer tm(e, BS_K_REPLAY, e->s);
-    launch_replay(L, a, scored, e->s);
+    launch_replay(L, a, scored, loc, e->s);
     tm.launched();
     CK(cudaGetLastError());
   }
@@ -3065,6 +3126,101 @@ int bs_upload_pod_preferences(bs_engine* e, uint32_t n_pods, const uint64_t* pre
   CK(cudaStreamSynchronize(e->s));
   e->pref_class_max = mx;
   e->have_pref_pod = true;
+  return BS_OK;
+}
+
+int bs_set_locality_weights(bs_engine* e, uint32_t image_locality, uint32_t prefer_avoid_pods) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (image_locality != e->w_img || prefer_avoid_pods != e->w_avoid) e->loc_dirty = true;
+  e->w_img = image_locality;
+  e->w_avoid = prefer_avoid_pods;
+  return BS_OK;
+}
+
+int bs_upload_node_locality(bs_engine* e, uint32_t n_nodes, uint32_t n_images, const int64_t* image_size,
+                            const uint32_t* image_bits, const uint64_t* avoid_mask) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  const char* who = "bs_upload_node_locality";
+  auto bad = [&](int rc, const char* why) { return fail(e, rc, (std::string(who) + ": " + why).c_str()); };
+  e->have_img_node = e->have_avoid_node = false;
+  e->loc_dirty = true;
+  if (!e->have_nodes) return bad(BS_E_STATE, "upload nodes first");
+  if (n_nodes != e->N) return bad(BS_E_INVAL, "n_nodes differs from the node table's");
+  const uint32_t Npad = e->Npad, words = cdiv(n_nodes, 32);
+  const bool img = image_size && image_bits;
+  if (img && (uint64_t)n_images * words * 4 > BS_LOC_TABLE_MAX_BYTES)
+    return bad(BS_E_INVAL, "n_images x ceil(n_nodes / 32) x 4 bytes exceeds BS_LOC_TABLE_MAX_BYTES");
+  for (uint32_t i = 0; img && i < n_images; ++i)
+    if (image_size[i] < 0 || image_size[i] > BS_IMAGE_SIZE_MAX) return bad(BS_E_RANGE, "an image size is outside [0, 2^48]");
+  BS_DEVICE_GUARD(e);
+  if (img) {
+    CK(e->d_img_size.ensure((size_t)std::max(n_images, 1u) * 8));
+    CK(e->d_img_bits.ensure((size_t)std::max<uint64_t>((uint64_t)n_images * words, 1) * 4));
+    if (n_images) {
+      CK(cudaMemcpyAsync(e->d_img_size.p, image_size, (size_t)n_images * 8, cudaMemcpyHostToDevice, e->s));
+      if (words) CK(cudaMemcpyAsync(e->d_img_bits.p, image_bits, (size_t)n_images * words * 4, cudaMemcpyHostToDevice, e->s));
+    }
+  }
+  if (avoid_mask) {
+    CK(e->d_avoid_mask.ensure((size_t)std::max(Npad, 1u) * 8));
+    CK(cudaMemsetAsync(e->d_avoid_mask.p, 0, (size_t)Npad * 8, e->s));
+    if (n_nodes) CK(cudaMemcpyAsync(e->d_avoid_mask.p, avoid_mask, (size_t)n_nodes * 8, cudaMemcpyHostToDevice, e->s));
+  }
+  CK(cudaStreamSynchronize(e->s));
+  e->loc_images = img ? n_images : 0;
+  e->have_img_node = img;
+  e->have_avoid_node = avoid_mask != nullptr;
+  return BS_OK;
+}
+
+int bs_upload_pod_locality(bs_engine* e, uint32_t n_pods, const uint32_t* image_class, uint32_t n_classes,
+                           const uint32_t* class_offset, const uint32_t* class_images, const uint8_t* avoid_bit) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  const char* who = "bs_upload_pod_locality";
+  auto bad = [&](int rc, const char* why) { return fail(e, rc, (std::string(who) + ": " + why).c_str()); };
+  e->have_img_pod = e->have_avoid_pod = false;
+  e->loc_dirty = true;
+  if (!e->have_pods) return bad(BS_E_STATE, "upload pods first");
+  if (n_pods != e->P) return bad(BS_E_INVAL, "n_pods differs from the pod table's");
+  const bool img = image_class && class_offset && class_images;
+  int64_t cmax = -1, imax = -1;
+  uint32_t nnz = 0;
+  if (img) {
+    if ((uint64_t)n_classes * e->Npad > BS_LOC_TABLE_MAX_BYTES)
+      return bad(BS_E_INVAL, "n_classes x padded nodes bytes exceeds BS_LOC_TABLE_MAX_BYTES");
+    if (class_offset[0] != 0) return bad(BS_E_INVAL, "class_offset[0] is not 0");
+    for (uint32_t c = 0; c < n_classes; ++c)
+      if (class_offset[c + 1] < class_offset[c] || class_offset[c + 1] - class_offset[c] > BS_LOC_CLASS_MAX)
+        return bad(BS_E_INVAL, "class_offset is not ascending, or a class lists more than BS_LOC_CLASS_MAX ids");
+    nnz = class_offset[n_classes];
+    for (uint32_t k = 0; k < nnz; ++k) imax = std::max(imax, (int64_t)class_images[k]);
+    for (uint32_t p = 0; p < n_pods; ++p)
+      if (image_class[p] != BS_IMAGE_NONE) cmax = std::max(cmax, (int64_t)image_class[p]);
+  }
+  for (uint32_t p = 0; avoid_bit && p < n_pods; ++p)
+    if (avoid_bit[p] > 63 && avoid_bit[p] != BS_AVOID_NONE) return bad(BS_E_RANGE, "an avoid bit is outside 0..63");
+  BS_DEVICE_GUARD(e);
+  if (img) {
+    CK(e->d_loc_class.ensure((size_t)std::max(n_pods, 1u) * 4));
+    CK(e->d_loc_off.ensure((size_t)(n_classes + 1) * 4));
+    CK(e->d_loc_ids.ensure((size_t)std::max(nnz, 1u) * 4));
+    if (n_pods) CK(cudaMemcpyAsync(e->d_loc_class.p, image_class, (size_t)n_pods * 4, cudaMemcpyHostToDevice, e->s));
+    CK(cudaMemcpyAsync(e->d_loc_off.p, class_offset, (size_t)(n_classes + 1) * 4, cudaMemcpyHostToDevice, e->s));
+    if (nnz) CK(cudaMemcpyAsync(e->d_loc_ids.p, class_images, (size_t)nnz * 4, cudaMemcpyHostToDevice, e->s));
+  }
+  if (avoid_bit) {
+    CK(e->d_avoid_bit.ensure(std::max(n_pods, 1u)));
+    if (n_pods) CK(cudaMemcpyAsync(e->d_avoid_bit.p, avoid_bit, n_pods, cudaMemcpyHostToDevice, e->s));
+  }
+  CK(cudaStreamSynchronize(e->s));
+  e->loc_classes = img ? n_classes : 0;
+  e->loc_class_max = cmax;
+  e->loc_image_max = imax;
+  e->have_img_pod = img;
+  e->have_avoid_pod = avoid_bit != nullptr;
   return BS_OK;
 }
 

@@ -241,6 +241,9 @@ __device__ __forceinline__ uint64_t ratio_term(uint32_t weight, uint32_t num, ui
   return (uint64_t)weight * (uint64_t)ratio_round(num, den);
 }
 
+// The round's kernels.  A translation unit that needs only the helpers above (priority_inst.cu) defines
+// BS_KERNELS_HELPERS_ONLY, so that these external kernels are defined once, in engine.cu.
+#ifndef BS_KERNELS_HELPERS_ONLY
 // ---------------------------------------------------------------------------
 // K1  node_left_kernel — per node: residual capacity at percent 1.0 in the
 // sentinel form the fit kernel consumes (absent scalar lane -> ABSENT_LEFT / ABSENT_LEFT32),
@@ -1414,5 +1417,7 @@ __global__ void __launch_bounds__(32) peer_wait_kernel(PeerArgs a) {
   __threadfence_system();
   if (!ok) *a.err = 1;
 }
+
+#endif  // BS_KERNELS_HELPERS_ONLY
 
 }  // namespace bsk

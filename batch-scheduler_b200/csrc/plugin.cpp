@@ -974,6 +974,8 @@ Status BatchSchedulingPlugin::BeginRound(const std::vector<const NodeInfo*>& sna
     if (!nst.ok()) return nst;
     nst = UploadPreferences();
     if (!nst.ok()) return nst;
+    nst = UploadLocality();
+    if (!nst.ok()) return nst;
   }
   {
     Status bst = UploadBound();   // after the groups: the bound rows' group indices refer to this table
@@ -1340,6 +1342,129 @@ Status BatchSchedulingPlugin::UploadPreferences() {
   return rc ? fail(rc) : Status{};
 }
 
+void BatchSchedulingPlugin::SetLocalityWeights(uint32_t image_locality, uint32_t prefer_avoid_pods) {
+  std::lock_guard<std::mutex> lk(mu_);
+  locality_weights_[0] = image_locality;
+  locality_weights_[1] = prefer_avoid_pods;
+}
+
+std::string normalized_image_name(const std::string& name) {
+  const size_t colon = name.rfind(':'), slash = name.rfind('/');
+  // strings.LastIndex gives -1 where rfind gives npos: compare as "position + 1"
+  const size_t c1 = colon == std::string::npos ? 0 : colon + 1, s1 = slash == std::string::npos ? 0 : slash + 1;
+  return c1 <= s1 ? name + ":latest" : name;
+}
+
+namespace {
+bool rc_or_rs(const std::string& kind) { return kind == "ReplicationController" || kind == "ReplicaSet"; }
+}  // namespace
+
+Status BatchSchedulingPlugin::PackLocality(const std::vector<const NodeInfo*>& snapshot,
+                                           const std::vector<const Pod*>& pending, PackedLocality* out) {
+  if (!out) return Status{BS_CODE_ERROR, "PackLocality: null output"};
+  PackedLocality& pl = *out;
+  pl = PackedLocality();
+  const size_t N = snapshot.size(), P = pending.size(), W = (N + 31) / 32;
+  // the names some pending pod's normalized container image asks for
+  std::unordered_map<std::string, uint32_t> wanted;   // name -> dictionary id (UINT32_MAX: not reported yet)
+  for (const Pod* pod : pending)
+    if (pod)
+      for (const Container& c : pod->containers) wanted.emplace(normalized_image_name(c.image), UINT32_MAX);
+  // the dictionary in node order: a name's size is the first (lowest-index) node's that reports it
+  for (size_t i = 0; i < N; ++i) {
+    if (!snapshot[i] || !snapshot[i]->node) continue;
+    for (const ContainerImage& im : snapshot[i]->node->images)
+      for (const std::string& name : im.names) {
+        auto it = wanted.find(name);
+        if (it == wanted.end()) continue;
+        if (it->second == UINT32_MAX) {
+          if (im.size_bytes < 0 || im.size_bytes > BS_IMAGE_SIZE_MAX)
+            return Status{BS_CODE_ERROR, "PackLocality: image " + name + " has a size outside [0, 2^48]"};
+          it->second = (uint32_t)pl.names.size();
+          pl.names.push_back(name);
+          pl.image_size.push_back(im.size_bytes);
+          pl.image_bits.resize(pl.image_bits.size() + W, 0u);
+        }
+        pl.image_bits[(size_t)it->second * W + i / 32] |= 1u << (i % 32);
+      }
+  }
+  // each pod's class: its containers' dictionary ids, sorted (a repeated image stays repeated), deduplicated
+  pl.image_class.assign(P, BS_IMAGE_NONE);
+  std::map<std::vector<uint32_t>, uint32_t> class_of;
+  for (size_t p = 0; p < P; ++p) {
+    if (!pending[p]) continue;
+    std::vector<uint32_t> ids;
+    for (const Container& c : pending[p]->containers) {
+      const uint32_t id = wanted.at(normalized_image_name(c.image));
+      if (id != UINT32_MAX) ids.push_back(id);
+    }
+    if (ids.empty()) continue;
+    if (ids.size() > BS_LOC_CLASS_MAX)
+      return Status{BS_CODE_ERROR, "PackLocality: pod " + pending[p]->ns + "/" + pending[p]->name +
+                                       " has more than 64 containers with reported images"};
+    std::sort(ids.begin(), ids.end());
+    auto it = class_of.find(ids);
+    if (it == class_of.end()) {
+      it = class_of.emplace(ids, pl.n_classes()).first;
+      pl.class_images.insert(pl.class_images.end(), ids.begin(), ids.end());
+      pl.class_offset.push_back((uint32_t)pl.class_images.size());
+    }
+    pl.image_class[p] = it->second;
+  }
+  // the avoid dictionary: RC / RS controllers of pending pods that some node's annotation lists, in node order
+  std::set<std::pair<std::string, std::string>> controlling;
+  for (const Pod* pod : pending)
+    if (pod && rc_or_rs(pod->controller_kind)) controlling.emplace(pod->controller_kind, pod->controller_uid);
+  pl.avoid_mask.assign(N, 0);
+  std::map<std::pair<std::string, std::string>, uint32_t> bit_of;
+  for (size_t i = 0; i < N; ++i) {
+    if (!snapshot[i] || !snapshot[i]->node) continue;
+    for (const PodController& pc : snapshot[i]->node->prefer_avoid_pods) {
+      const auto key = std::make_pair(pc.kind, pc.uid);
+      if (!controlling.count(key)) continue;
+      auto it = bit_of.find(key);
+      if (it == bit_of.end()) {
+        if (pl.controllers.size() == 64)
+          return Status{BS_CODE_ERROR, "PackLocality: more than 64 avoided controllers of pending pods in one round"};
+        it = bit_of.emplace(key, (uint32_t)pl.controllers.size()).first;
+        pl.controllers.push_back(pc);
+      }
+      pl.avoid_mask[i] |= 1ull << it->second;
+    }
+  }
+  pl.avoid_bit.assign(P, BS_AVOID_NONE);
+  for (size_t p = 0; p < P; ++p) {
+    if (!pending[p] || !rc_or_rs(pending[p]->controller_kind)) continue;
+    auto it = bit_of.find(std::make_pair(pending[p]->controller_kind, pending[p]->controller_uid));
+    if (it != bit_of.end()) pl.avoid_bit[p] = (uint8_t)it->second;
+  }
+  return Status{};
+}
+
+Status BatchSchedulingPlugin::UploadLocality() {
+  if (!priority_k_) return Status{};
+  auto fail = [&](int rc) {
+    return Status{BS_CODE_ERROR, std::string("bsched: ") + bs_strerror(rc) + " (" + bs_last_error(eng_) + ")"};
+  };
+  int rc = bs_set_locality_weights(eng_, locality_weights_[0], locality_weights_[1]);
+  if (rc) return fail(rc);
+  if (!locality_weights_[0] && !locality_weights_[1]) return Status{};
+  PackedLocality pl;
+  Status st = PackLocality(snapshot_, pending_, &pl);
+  if (!st.ok()) return st;
+  // empty vectors may have null data(): the parts are present, so point them at something
+  static const uint64_t none = 0;
+  auto nz = [](const void* p) { return p ? p : (const void*)&none; };
+  rc = bs_upload_node_locality(eng_, (uint32_t)snapshot_.size(), (uint32_t)pl.names.size(),
+                               (const int64_t*)nz(pl.image_size.data()), (const uint32_t*)nz(pl.image_bits.data()),
+                               (const uint64_t*)nz(pl.avoid_mask.data()));
+  if (!rc)
+    rc = bs_upload_pod_locality(eng_, (uint32_t)pending_.size(), (const uint32_t*)nz(pl.image_class.data()),
+                                pl.n_classes(), pl.class_offset.data(), (const uint32_t*)nz(pl.class_images.data()),
+                                (const uint8_t*)nz(pl.avoid_bit.data()));
+  return rc ? fail(rc) : Status{};
+}
+
 std::vector<uint32_t> BatchSchedulingPlugin::ReasonCounts(const std::string& uid) const {
   const int32_t row = pod_row_.find(uid);
   const size_t R = 4 + packed_.lanes;
@@ -1374,6 +1499,8 @@ Status BatchSchedulingPlugin::UpdateRound(const std::vector<std::pair<uint32_t, 
   if (!st.ok()) return st;
   if (changed_nodes.empty()) {   // UpdateNodes uploaded the preferences and weights when it changed rows
     st = UploadPreferences();
+    if (!st.ok()) return st;
+    st = UploadLocality();
     if (!st.ok()) return st;
   }
   return Reevaluate();
@@ -1426,6 +1553,8 @@ Status BatchSchedulingPlugin::UpdateNodes(const std::vector<std::pair<uint32_t, 
   st = UploadNonZero(nullptr);   // ... and the node non-zero column: the changed NodeInfos' pods count again
   if (!st.ok()) return st;
   st = UploadPreferences();      // ... and the node preference side (its taint dictionary may change: both sides)
+  if (!st.ok()) return st;
+  st = UploadLocality();         // ... and the locality side (its dictionaries may change: both sides)
   if (!st.ok()) return st;
   // the round's decisions follow the new snapshot: same pods, same groups, same result vectors
   return evaluate ? Reevaluate() : Status{};

@@ -35,6 +35,7 @@ struct Container {
   bool has_limits = false;  // Resources.Limits != nil  (core.go:765)
   ResourceList limits;
   ResourceList requests;
+  std::string image;        // Spec.Containers[].Image as written (ImageLocality normalizes it)
 };
 struct Toleration {
   std::string key, op /* "", "Equal", "Exists" */, value, effect;
@@ -72,6 +73,18 @@ struct Pod {
   int32_t priority = 0;                 // podutil.GetPodPriority
   int64_t queue_ts_ns = 0;              // framework.PodInfo.Timestamp
   int64_t start_ns = 0;                 // Status.StartTime of a bound pod (preemption: MoreImportantPod)
+  std::string controller_kind, controller_uid;   // metav1.GetControllerOf: the controlling owner ("" = none)
+};
+// v1.ContainerImage: one entry of Status.Images, the names it is known by and its size (ImageLocality)
+struct ContainerImage {
+  std::vector<std::string> names;
+  int64_t size_bytes = 0;
+};
+// v1.PodSignature.PodController of one entry of the scheduler.alpha.kubernetes.io/preferAvoidPods annotation
+// (NodePreferAvoidPods); the adapter parses the annotation (v1helper.GetAvoidPodsFromNodeAnnotations), an annotation
+// that fails to parse giving no entries
+struct PodController {
+  std::string kind, uid;
 };
 struct Node {
   std::string name;
@@ -79,6 +92,8 @@ struct Node {
   std::vector<Taint> taints;
   ResourceList allocatable;
   bool unschedulable = false;
+  std::vector<ContainerImage> images;             // Status.Images
+  std::vector<PodController> prefer_avoid_pods;   // the preferAvoidPods annotation's controllers
 };
 struct NodeInfo {          // k8s.io/kubernetes/pkg/scheduler/nodeinfo.NodeInfo, the fields core.go reads
   const Node* node = nullptr;  // nullptr: info.Node() == nil (core.go:610)
@@ -177,6 +192,26 @@ struct PackedPreferences {
   std::vector<int32_t> pref_weights;            // [n_classes][n_nodes]
   uint32_t n_classes() const { return (uint32_t)class_signatures.size(); }
 };
+
+// The columns of the ImageLocality and NodePreferAvoidPods priorities of one round (bs_upload_node_locality,
+// bs_upload_pod_locality): the dictionary of reported image names that some pending pod's normalized container image
+// matches, with each name's size and bit row over the nodes; each pod's class (its sorted id list, deduplicated); the
+// dictionary of RC / RS controllers listed on some node and controlling some pending pod, each node's bits of it and
+// each pod's bit.
+struct PackedLocality {
+  std::vector<std::string> names;               // id i of the image dictionary
+  std::vector<int64_t> image_size;              // [n_images]
+  std::vector<uint32_t> image_bits;             // [n_images][ceil(n_nodes / 32)]
+  std::vector<uint32_t> image_class;            // [n_pods], BS_IMAGE_NONE = no dictionary image
+  std::vector<uint32_t> class_offset{0};        // [n_classes + 1]
+  std::vector<uint32_t> class_images;           // [class_offset.back()]
+  std::vector<PodController> controllers;       // bit b of the avoid masks
+  std::vector<uint64_t> avoid_mask;             // [n_nodes]
+  std::vector<uint8_t> avoid_bit;               // [n_pods], BS_AVOID_NONE = no listed RC / RS controller
+  uint32_t n_classes() const { return (uint32_t)class_offset.size() - 1; }
+};
+// normalizedImageName (ImageLocality): ":latest" appended when the last ':' does not follow the last '/'
+std::string normalized_image_name(const std::string& name);
 
 // string -> row index of one round, built in one go: the keys are copied into ONE arena (no allocation per key),
 // hashed in parallel, and a later duplicate overwrites an earlier one, as `map[key] = row` in a loop would.
@@ -351,6 +386,10 @@ class BatchSchedulingPlugin {
   // delta round on, on a plugin created with priority_k > 0.  While either is non-zero, ReplayQueue(kPriority) returns
   // an error.
   void SetNodePriorityWeights(uint32_t taint_toleration, uint32_t node_affinity);
+  // weights of kube-scheduler v1.17's ImageLocality and NodePreferAvoidPods priorities in PriorityNodes and in
+  // ReplayQueue(kPriority) (bs_set_locality_weights; 0, 0 = off, the default; v1.17's default profile is 1, 10000),
+  // from the next round or delta round on, on a plugin created with priority_k > 0.
+  void SetLocalityWeights(uint32_t image_locality, uint32_t prefer_avoid_pods);
   int group_index(const std::string& ns_name) const;
   double last_pack_ms() const { return last_pack_ms_; }
   double last_device_ms() const { return last_device_ms_; }
@@ -422,6 +461,12 @@ class BatchSchedulingPlugin {
   // requirement counts 0 there (upstream, it fails the pod's scoring); a negative weight is an error.
   static Status PackPreferences(const std::vector<const NodeInfo*>& snapshot, const std::vector<const Pod*>& pending,
                                 PackedPreferences* out);
+  // The columns of the ImageLocality and NodePreferAvoidPods priorities (no GPU).  Only Spec.Containers count; a name
+  // reported with different sizes takes the size of the lowest node index reporting it; a controller of a kind other
+  // than ReplicationController / ReplicaSet counts as none.  More than BS_LOC_CLASS_MAX dictionary images in one pod,
+  // or more than 64 controllers in the avoid dictionary, is an error.
+  static Status PackLocality(const std::vector<const NodeInfo*>& snapshot, const std::vector<const Pod*>& pending,
+                             PackedLocality* out);
 
   static Status Pack(const std::vector<const NodeInfo*>& snapshot, const std::vector<const Pod*>& pending,
                      const std::vector<PodGroup>& groups, const std::vector<uint32_t>& matched,
@@ -451,6 +496,7 @@ class BatchSchedulingPlugin {
   std::vector<uint32_t> ratio_util_{0, 100}, ratio_score_{100, 0};
   std::map<std::string, uint32_t> ratio_resources_{{"cpu", 1}, {"memory", 1}};
   uint32_t node_prio_weights_[2] = {0, 0};             // SetNodePriorityWeights: TaintToleration, NodeAffinity
+  uint32_t locality_weights_[2] = {0, 0};              // SetLocalityWeights: ImageLocality, NodePreferAvoidPods
   std::string init_error_;
   int64_t max_schedule_time_ns_;
   std::map<std::string, GroupState> groups_;                        // ordered: canonical table order
@@ -484,6 +530,8 @@ class BatchSchedulingPlugin {
                                                                   // priority_k
   Status UploadPreferences();   // both preference sides of snapshot_ and pending_ and the two weights; the columns only
                                 // while a weight is non-zero; no-op without priority_k
+  Status UploadLocality();   // both locality sides of snapshot_ and pending_ and the two weights; the columns only
+                             // while a weight is non-zero; no-op without priority_k
   Status UploadBound();  // packs and uploads the bound-pod table of snapshot_ (no-op when no NodeInfo lists pods)
   Status RunPreempt(const std::vector<uint32_t>& rows, std::vector<Preemption>* out);
   std::vector<const NodeInfo*> snapshot_;                           // the round's NodeInfos (bound pods)

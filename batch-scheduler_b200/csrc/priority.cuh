@@ -6,7 +6,8 @@
 // is short (lane_short over node_left_kernel's full-width residuals), the invariant DESIGN §2 states for reason rows.
 // The lists are kept with gang_fit's topk_insert (fit.cuh); the pair scorer pair_score is kernels.cuh's, and with RATIO
 // the RequestedToCapacityRatio term (kernels.cuh ratio_*) is added to it; with PREF the TaintToleration and preferred
-// NodeAffinity terms (bs_set_node_priority_weights), normalized over the pod's fit set.
+// NodeAffinity terms (bs_set_node_priority_weights), normalized over the pod's fit set; with LOC the ImageLocality and
+// NodePreferAvoidPods terms (bs_set_locality_weights), static per pair, from the pre-pass below.
 #pragma once
 #include "kernels.cuh"
 #include "fit.cuh"
@@ -78,15 +79,54 @@ __device__ __forceinline__ uint64_t pref_term(const PriorityPrefArgs& a, uint32_
   return (uint64_t)a.w_taint * (uint64_t)tt + (uint64_t)a.w_naff * (uint64_t)na;
 }
 
+// LOC's arguments (bs_upload_node_locality / bs_upload_pod_locality): the IL table the pre-pass built, each node's
+// preferAvoidPods mask, each pod's class and controller bit, and the two weights.  Derived from PREF's type for the same
+// reason; the ratio and preference fields are read only with RATIO and PREF.
+constexpr uint32_t IMAGE_NONE = 0xffffffffu;   // BS_IMAGE_NONE
+constexpr uint32_t AVOID_NONE = 0xffu;         // BS_AVOID_NONE
+struct PriorityLocArgs : PriorityPrefArgs {
+  const uint8_t* il;            // [classes][Npad] IL of (class, node), 0..100 (locality_class_kernel)
+  const uint64_t* avoid_mask;   // [Npad] (padding 0)
+  const uint32_t* loc_class;    // [P] row of il or IMAGE_NONE
+  const uint8_t* avoid_bit;     // [P] 0..63 or AVOID_NONE
+  uint32_t w_img, w_avoid;
+};
+// The pod's side of LOC: its row of the IL table (null: IL = 0) and its controller as a one-bit mask (0: none).  A
+// weight of 0 skips the column, which may then be missing.
+__device__ __forceinline__ void loc_pod(const PriorityLocArgs& a, uint32_t p, const uint8_t*& row, uint64_t& amask) {
+  const uint32_t c = a.w_img ? a.loc_class[p] : IMAGE_NONE;
+  row = c == IMAGE_NONE ? nullptr : a.il + (size_t)c * a.Npad;
+  const uint32_t b = a.w_avoid ? a.avoid_bit[p] : AVOID_NONE;
+  amask = b == AVOID_NONE ? 0ull : 1ull << b;
+}
+// w_img * IL + w_avoid * NPA of one pair, int64 wrapping: NPA is 0 when the node's annotation lists the pod's controller
+__device__ __forceinline__ uint64_t loc_term(const PriorityLocArgs& a, const uint8_t* row, uint64_t amask, uint32_t i,
+                                             uint64_t node_avoid) {
+  const uint64_t il = row ? row[i] : 0u;
+  return (uint64_t)a.w_img * il + (uint64_t)a.w_avoid * ((node_avoid & amask) ? 0u : 100u);
+}
+
+// The LOC pre-pass (priority_inst.cu image_spread_kernel, locality_class_kernel) builds the IL table once per
+// change of either side or a weight.
+constexpr int LOC_THREADS = 256;
+
 // PREF (chosen by the host when either weight of bs_set_node_priority_weights is non-zero) adds w_taint * TT +
 // w_naff * NA.  Both are normalized by the maximum raw count over the pod's fit set, and floor(100 * a / Ma) re-orders
 // nodes already seen when Ma grows, so every maximum has to be known before the first pair is scored: the warp first
 // sweeps the nodes once with the same fit test, keeping the largest t and a of each of its pods over the nodes that
 // fit, and reduces them across its lanes.  The sweep lives in the kernel (not a [2][P] pre-pass) because its fit test
 // needs the pod's requests and gate row, which the warp has already loaded for the scoring sweep.
-template <int MAXL, bool RATIO, bool PREF>
-__global__ void __launch_bounds__(PRIO_THREADS)
-priority_pod_kernel(std::conditional_t<PREF, PriorityPrefArgs, std::conditional_t<RATIO, PriorityRatioArgs, PriorityArgs>> a) {
+//
+// LOC (chosen by the host when either weight of bs_set_locality_weights is non-zero) adds w_img * IL + w_avoid * NPA:
+// one byte of the pod's IL row per pair, read by adjacent lanes, and the node's avoid mask, shared by the warp's pods.
+//
+// LOC's kernels ask for two CTAs per SM: left to itself, ptxas gives the PREF + LOC variants up to 145 registers, which
+// fits one 256-thread CTA per SM where the kernels without LOC run two.
+template <int MAXL, bool RATIO, bool PREF, bool LOC = false>
+__global__ void __launch_bounds__(PRIO_THREADS, LOC ? 2 : 0)
+priority_pod_kernel(std::conditional_t<LOC, PriorityLocArgs,
+                                       std::conditional_t<PREF, PriorityPrefArgs,
+                                                          std::conditional_t<RATIO, PriorityRatioArgs, PriorityArgs>>> a) {
   constexpr int WARPS = PRIO_THREADS / 32;
   __shared__ int64_t s_req[WARPS][PRIO_PPW][MAXL];
   __shared__ int64_t s_ls[WARPS][PRIO_PPW][32];
@@ -125,6 +165,16 @@ priority_pod_kernel(std::conditional_t<PREF, PriorityPrefArgs, std::conditional_
     nz_mem[j] = ok ? a.pod_nz[(size_t)a.P + p] : 0;
     thr[j] = INT64_MIN;
     nfit[j] = 0;
+  }
+  [[maybe_unused]] const uint8_t* lrow[PRIO_PPW];   // LOC: the pod's IL row and controller bit
+  [[maybe_unused]] uint64_t lmask[PRIO_PPW];
+  if constexpr (LOC) {
+#pragma unroll
+    for (int j = 0; j < PRIO_PPW; ++j) {
+      lrow[j] = nullptr;
+      lmask[j] = 0;
+      if (rmask[j]) loc_pod(a, p0 + j, lrow[j], lmask[j]);
+    }
   }
   [[maybe_unused]] uint64_t ptol[PRIO_PPW];
   [[maybe_unused]] uint32_t pcls[PRIO_PPW], mt[PRIO_PPW], ma[PRIO_PPW];   // PREF: the pod's maxima over its fit set
@@ -204,6 +254,8 @@ priority_pod_kernel(std::conditional_t<PREF, PriorityPrefArgs, std::conditional_
     if (!anyfit) continue;
     const int64_t c_cpu = a.alloc[i], c_mem = a.alloc[(size_t)a.Npad + i];
     const int64_t n_cpu = a.node_nz[i], n_mem = a.node_nz[(size_t)a.Npad + i];
+    [[maybe_unused]] uint64_t navoid = 0;   // LOC: the node's preferAvoidPods mask
+    if constexpr (LOC) navoid = a.w_avoid ? a.avoid_mask[i] : 0;
     [[maybe_unused]] uint32_t rnum[PRIO_PPW], rden[PRIO_PPW];   // RATIO: the weighted sum and weight sum of each pod's average
     if constexpr (RATIO) {
 #pragma unroll
@@ -243,6 +295,8 @@ priority_pod_kernel(std::conditional_t<PREF, PriorityPrefArgs, std::conditional_
           pref_counts(a, a.w_taint ? a.prefer_taints[i] : 0, ptol[j], pcls[j], i, t, aw);
           s = (int64_t)((uint64_t)s + pref_term(a, t, aw, mt[j], ma[j]));
         }
+      if constexpr (LOC)
+        if (g[j]) s = (int64_t)((uint64_t)s + loc_term(a, lrow[j], lmask[j], i, navoid));
       const uint32_t cb = __ballot_sync(0xffffffffu, g[j] && (nfit[j] < a.K || s > thr[j]));
       if (cb) thr[j] = topk_insert<int64_t>(s_ls[wid][j], s_ln[wid][j], a.K, cb, s, (int32_t)base, lane);
       nfit[j] += __popc(fw[j]);
@@ -258,5 +312,15 @@ priority_pod_kernel(std::conditional_t<PREF, PriorityPrefArgs, std::conditional_
     }
   }
 }
+
+// priority_inst.cu, a translation unit of its own so that the variants compile in parallel with engine.cu:
+// priority_pod_kernel<MAXL, ratio, pref, loc> for the engine's lane count L; `a` is read as the flags' argument type
+// (PriorityArgs without any flag, PriorityRatioArgs with ratio alone, PriorityPrefArgs with pref, all of it with loc).
+cudaError_t launch_priority(uint32_t L, uint32_t grid, bool ratio, bool pref, bool loc, const PriorityLocArgs& a,
+                            cudaStream_t s);
+// the LOC pre-pass: scaled[n_images] from the bit rows and sizes, then il[n_classes][Npad]; 2 launches
+cudaError_t launch_locality_prepass(const uint32_t* bits, const int64_t* size, int64_t* scaled, uint32_t n_images,
+                                    const uint32_t* class_offset, const uint32_t* class_images, uint8_t* il,
+                                    uint32_t n_classes, uint32_t n_nodes, uint32_t Npad, cudaStream_t s);
 
 }  // namespace bsk

@@ -1,0 +1,111 @@
+// priority_inst.cu — the priority lists' kernels (priority.cuh): every priority_pod_kernel variant and the LOC
+// pre-pass.  A translation unit of its own (build.py), compiled in parallel with engine.cu, which reaches the kernels
+// through launch_priority and launch_locality_prepass.
+#define BS_KERNELS_HELPERS_ONLY   // kernels.cuh's round kernels live in engine.cu
+#include "priority.cuh"
+
+namespace bsk {
+namespace {
+
+// The LOC pre-pass.  ImageLocality's per-name score depends on how many snapshot nodes report the name, and its sum
+// over a pod's containers only on the pod's image class, so both are built once per (node side, pod side) and the
+// scoring sweep reads one byte per pair.
+//
+// K1f image_spread_kernel — one warp per dictionary name: NumNodes = the popcount of the name's bit row over the
+// n_nodes real nodes, then scaled = (int64)((double)size * ((double)NumNodes / (double)n_nodes)).  The explicit
+// round-to-nearest intrinsics keep each operation a separate binary64 rounding whatever -fmad says.
+__global__ void __launch_bounds__(LOC_THREADS) image_spread_kernel(const uint32_t* bits, const int64_t* size,
+                                                                   int64_t* scaled, uint32_t n_images, uint32_t n_nodes,
+                                                                   uint32_t words) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t img = (blockIdx.x * LOC_THREADS + threadIdx.x) >> 5;
+  if (img >= n_images) return;   // warp-uniform
+  const uint32_t* row = bits + (size_t)img * words;
+  uint32_t cnt = 0;
+  for (uint32_t w = lane; w < words; w += 32) {
+    uint32_t x = row[w];
+    const uint32_t lo = w * 32;
+    if (lo + 32 > n_nodes) x &= (1u << (n_nodes - lo)) - 1u;   // n_nodes - lo < 32: bits past the last node
+    cnt += __popc(x);
+  }
+  cnt = __reduce_add_sync(0xffffffffu, cnt);
+  if (lane == 0) {
+    const double spread = __ddiv_rn((double)cnt, (double)n_nodes);
+    scaled[img] = __double2ll_rz(__dmul_rn((double)size[img], spread));
+  }
+}
+
+// K1g locality_class_kernel — IL of every (class, node): a thread per node, the class's ids and their scaled sizes in
+// shared memory (at most BS_LOC_CLASS_MAX).  Padding nodes get 0.
+constexpr int64_t IL_MIN = 23ll << 20, IL_MAX = 1000ll << 20;   // ImageLocality's thresholds, 23 MiB and 1000 MiB
+__global__ void __launch_bounds__(LOC_THREADS) locality_class_kernel(const uint32_t* class_offset,
+                                                                     const uint32_t* class_images,
+                                                                     const uint32_t* bits, const int64_t* scaled,
+                                                                     uint8_t* il, uint32_t n_classes, uint32_t n_nodes,
+                                                                     uint32_t Npad, uint32_t words) {
+  __shared__ uint32_t s_img[64];
+  __shared__ int64_t s_scaled[64];
+  const uint32_t i = blockIdx.x * LOC_THREADS + threadIdx.x;
+  for (uint32_t c = blockIdx.y; c < n_classes; c += gridDim.y) {
+    const uint32_t o0 = class_offset[c], n = class_offset[c + 1] - o0;
+    __syncthreads();
+    if (threadIdx.x < n) {
+      const uint32_t id = class_images[o0 + threadIdx.x];
+      s_img[threadIdx.x] = id;
+      s_scaled[threadIdx.x] = scaled[id];
+    }
+    __syncthreads();
+    if (i >= Npad) continue;
+    int64_t sum = 0;
+    if (i < n_nodes)
+      for (uint32_t k = 0; k < n; ++k)
+        if ((bits[(size_t)s_img[k] * words + (i >> 5)] >> (i & 31)) & 1u) sum += s_scaled[k];
+    sum = min(max(sum, IL_MIN), IL_MAX);
+    il[(size_t)c * Npad + i] = i < n_nodes ? (uint8_t)(100 * (sum - IL_MIN) / (IL_MAX - IL_MIN)) : 0;
+  }
+}
+
+template <bool RATIO, bool PREF, bool LOC, class Args>
+void launch_t(uint32_t L, uint32_t grid, const Args& a, cudaStream_t s) {
+  if (L <= 5) priority_pod_kernel<5, RATIO, PREF, LOC><<<grid, PRIO_THREADS, 0, s>>>(a);
+  else if (L <= 9) priority_pod_kernel<9, RATIO, PREF, LOC><<<grid, PRIO_THREADS, 0, s>>>(a);
+  else priority_pod_kernel<16, RATIO, PREF, LOC><<<grid, PRIO_THREADS, 0, s>>>(a);
+}
+
+}  // namespace
+
+cudaError_t launch_priority(uint32_t L, uint32_t grid, bool ratio, bool pref, bool loc, const PriorityLocArgs& a,
+                            cudaStream_t s) {
+  const PriorityPrefArgs& pp = a;
+  const PriorityRatioArgs& pr = a;
+  const PriorityArgs& pb = a;
+  if (loc) {
+    if (pref && ratio) launch_t<true, true, true>(L, grid, a, s);
+    else if (pref) launch_t<false, true, true>(L, grid, a, s);
+    else if (ratio) launch_t<true, false, true>(L, grid, a, s);
+    else launch_t<false, false, true>(L, grid, a, s);
+  } else if (pref) {
+    if (ratio) launch_t<true, true, false>(L, grid, pp, s);
+    else launch_t<false, true, false>(L, grid, pp, s);
+  } else if (ratio) {
+    launch_t<true, false, false>(L, grid, pr, s);
+  } else {
+    launch_t<false, false, false>(L, grid, pb, s);
+  }
+  return cudaGetLastError();
+}
+
+cudaError_t launch_locality_prepass(const uint32_t* bits, const int64_t* size, int64_t* scaled, uint32_t n_images,
+                                    const uint32_t* class_offset, const uint32_t* class_images, uint8_t* il,
+                                    uint32_t n_classes, uint32_t n_nodes, uint32_t Npad, cudaStream_t s) {
+  const uint32_t words = (n_nodes + 31) / 32;
+  if (n_images && n_nodes)
+    image_spread_kernel<<<(n_images + LOC_THREADS / 32 - 1) / (LOC_THREADS / 32), LOC_THREADS, 0, s>>>(
+        bits, size, scaled, n_images, n_nodes, words);
+  const dim3 grid((Npad + LOC_THREADS - 1) / LOC_THREADS, n_classes < 65535u ? n_classes : 65535u);
+  locality_class_kernel<<<grid, LOC_THREADS, 0, s>>>(class_offset, class_images, bits, scaled, il, n_classes, n_nodes,
+                                                     Npad, words);
+  return cudaGetLastError();
+}
+
+}  // namespace bsk

@@ -32,7 +32,9 @@
 //                      descending, then index ascending): each thread keeps the best of its four
 //                      nodes over the sweep, one block reduction picks the winner.  RATIO (a non-zero
 //                      bs_set_ratio_priority weight) adds the RequestedToCapacityRatio term over the
-//                      live `requested` and key mask (lanes >= 2) and the live non-zero column.  In both,
+//                      live `requested` and key mask (lanes >= 2) and the live non-zero column.  LOC (a
+//                      non-zero bs_set_locality_weights weight) adds ImageLocality and NodePreferAvoidPods,
+//                      which the walk does not change: the round's IL table and avoid masks.  In both,
 //                      requests only grow `requested`, so a leading run of nodes no pod of the table
 //                      can ever fit again (or that is skipped) is remembered and not rescanned; such
 //                      a node never fits, so it never scores either;
@@ -42,6 +44,8 @@
 // representative class, MinResources, the live non-zero column); the uploaded tables are untouched.
 #pragma once
 #include "kernels.cuh"
+
+#include <type_traits>
 
 namespace bsk {
 
@@ -94,6 +98,14 @@ struct ReplayArgs {
   const int64_t* pod_nz;      // [2][P]
   ScoreWeights w;
   RatioSetting ratio;         // RATIO only
+};
+// LOC's arguments (priority.cuh PriorityLocArgs): a derived type, so that the kernels without the terms keep theirs
+struct ReplayLocArgs : ReplayArgs {
+  const uint8_t* il;            // [classes][Npad]
+  const uint64_t* avoid_mask;   // [Npad]
+  const uint32_t* loc_class;    // [P]
+  const uint8_t* avoid_bit;     // [P]
+  uint32_t w_img, w_avoid;
 };
 
 template <int MAXL>
@@ -212,9 +224,10 @@ __device__ __forceinline__ void block_scan(ReplaySmem<MAXL>& sm, int64_t (&v)[RE
   for (int k = 0; k < REPLAY_NPT; ++k) keys[k] |= fk;
 }
 
-template <int MAXL, bool SCORED, bool RATIO = false>
-__global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(ReplayArgs a) {
+template <int MAXL, bool SCORED, bool RATIO = false, bool LOC = false>
+__global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(std::conditional_t<LOC, ReplayLocArgs, ReplayArgs> a) {
   static_assert(SCORED || !RATIO, "the ratio term belongs to the scored node choice");
+  static_assert(SCORED || !LOC, "the locality terms belong to the scored node choice");
   __shared__ ReplaySmem<MAXL> sm;
   __shared__ int32_t s_tab[RATIO_TABLE];   // RATIO: shape(util)
   const uint32_t tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
@@ -627,6 +640,14 @@ __global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(ReplayArgs a)
         if constexpr (SCORED) {
           // nodes come in ascending order per thread: only a strictly higher score replaces the best
           const int64_t pnz0 = s_pod_nz[par][0], pnz1 = s_pod_nz[par][1];
+          [[maybe_unused]] const uint8_t* lrow = nullptr;   // LOC: the pod's IL row (null: IL = 0) and controller bit
+          [[maybe_unused]] uint64_t lmask = 0;
+          if constexpr (LOC) {
+            const uint32_t c = a.w_img ? a.loc_class[cur.p] : 0xffffffffu;   // BS_IMAGE_NONE
+            if (c != 0xffffffffu) lrow = a.il + (size_t)c * Npad;
+            const uint32_t b = a.w_avoid ? a.avoid_bit[cur.p] : 0xffu;       // BS_AVOID_NONE
+            if (b != 0xffu) lmask = 1ull << b;
+          }
 #pragma unroll
           for (int k = 0; k < REPLAY_NPT; ++k) {
             if (!((fit >> k) & 1u)) continue;
@@ -654,6 +675,11 @@ __global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(ReplayArgs a)
                 ratio_accumulate(ratio_lane_score(s_tab, r, c), wd, num, den);
               }
               s = (int64_t)((uint64_t)s + (uint64_t)a.ratio.weight * (uint64_t)ratio_round(num, den));
+            }
+            if constexpr (LOC) {
+              const uint64_t il = lrow ? lrow[n] : 0u;
+              const uint64_t nav = a.w_avoid ? a.avoid_mask[n] : 0ull;
+              s = (int64_t)((uint64_t)s + (uint64_t)a.w_img * il + (uint64_t)a.w_avoid * ((nav & lmask) ? 0u : 100u));
             }
             if (best_n < 0 || s > best_s) { best_s = s; best_n = (int32_t)n; }
           }

@@ -321,6 +321,48 @@ class Engine:
                 raise ValueError("prefer_tol and pref_class must have one entry per pod")
             self._check(self.lib.bs_upload_pod_preferences(self.h, len(tol), capi.ptr(tol), capi.ptr(cls)))
 
+    def set_locality_weights(self, image_locality: int = 0, prefer_avoid_pods: int = 0):
+        """Weights of kube-scheduler's ImageLocality and NodePreferAvoidPods priorities in the priority score and in
+        replay(priority=True)'s node choice (0, 0 = off, the default; v1.17's default profile is 1, 10000).  A non-zero
+        weight needs upload_locality before each round."""
+        self._check(self.lib.bs_set_locality_weights(self.h, image_locality, prefer_avoid_pods))
+
+    def upload_locality(self, node=None, pods=None):
+        """The columns of the two locality priorities.  node = (image_size [I] int64, image_bits [I, ceil(N/32)]
+        uint32, avoid_mask [N] uint64): the image dictionary's sizes in bytes, bit n%32 of word n/32 of row i set when
+        node n reports name i, and bit b of avoid_mask when the node's preferAvoidPods annotation lists controller b.
+        pods = (image_class [P] uint32, class_offset [C+1] uint32, class_images [nnz] uint32, avoid_bit [P] uint8):
+        each pod's class (capi.IMAGE_NONE: none), the dictionary ids of each class (CSR), and each pod's controller bit
+        (capi.AVOID_NONE: none).  Either image part or avoid part may be None when its weight is 0.  Uploading nodes
+        (or updating node rows) drops the node side, uploading pods the pod side."""
+        if node is not None:
+            size, bits, avoid = node
+            if size is not None:
+                size = np.ascontiguousarray(size, dtype=np.int64).reshape(-1)
+                bits = np.ascontiguousarray(bits, dtype=np.uint32).reshape(len(size), -1)
+            if avoid is not None:
+                avoid = np.ascontiguousarray(avoid, dtype=np.uint64).reshape(-1)
+            n = len(avoid) if avoid is not None else self.N
+            self._check(self.lib.bs_upload_node_locality(self.h, n, 0 if size is None else len(size), capi.ptr(size),
+                                                         capi.ptr(bits), capi.ptr(avoid)))
+        if pods is not None:
+            cls, off, ids, abit = pods
+            n_classes = 0
+            if cls is not None:
+                cls = np.ascontiguousarray(cls, dtype=np.uint32).reshape(-1)
+                off = np.ascontiguousarray(off, dtype=np.uint32).reshape(-1)
+                ids = np.ascontiguousarray(ids, dtype=np.uint32).reshape(-1)
+                if len(off) < 1 or len(ids) < int(off[-1]):
+                    raise ValueError("class_offset must have C+1 entries and class_images class_offset[C] of them")
+                n_classes = len(off) - 1
+            if abit is not None:
+                abit = np.ascontiguousarray(abit, dtype=np.uint8).reshape(-1)
+            if cls is not None and abit is not None and len(cls) != len(abit):
+                raise ValueError("image_class and avoid_bit must have one entry per pod")
+            n = len(cls) if cls is not None else len(abit) if abit is not None else self.P
+            self._check(self.lib.bs_upload_pod_locality(self.h, n, capi.ptr(cls), n_classes, capi.ptr(off),
+                                                        capi.ptr(ids), capi.ptr(abit)))
+
     def priority_rows(self, pod0=0, n=None):
         """(nodes [n, K] int32, scores [n, K] int64): each pod's fitting nodes by priority score descending, then node
         index ascending; min(K, feasible_count) entries, padded with node -1 and score INT64_MIN."""

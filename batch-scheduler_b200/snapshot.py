@@ -402,6 +402,53 @@ def node_preferences(snap: Snapshot, seed: int, n_bits: int = 6, tainted: float 
     return prefer_taints.astype(np.uint64), pref_weights.astype(np.int32), prefer_tol.astype(np.uint64), pref_class
 
 
+IMAGE_NONE = 0xFFFFFFFF   # BS_IMAGE_NONE
+AVOID_NONE = 0xFF         # BS_AVOID_NONE
+MIB = 1 << 20
+
+
+def node_locality(snap: Snapshot, seed: int, n_images: int = 16, n_classes: int = 8, max_ids: int = 5,
+                  no_image: float = 0.2, n_controllers: int = 8, avoided: float = 0.1, controlled: float = 0.6):
+    """Seeded columns of the ImageLocality and NodePreferAvoidPods priorities for a table without objects:
+    (node, pods) with node = (image_size [I] int64, image_bits [I, ceil(N/32)] uint32, avoid_mask [N] uint64) and
+    pods = (image_class [P] uint32, class_offset [C+1] uint32, class_images [nnz] uint32, avoid_bit [P] uint8).
+    Sizes span 0 to 20 GiB; four names lie on every node at 23 MiB, 23 MiB + 1, 1000 MiB - 1 and 1000 MiB, so that
+    sums land on and next to both thresholds; the others are reported by a share of the nodes drawn from
+    {1 node, 5 %, 30 %, 70 %, all}.  A class lists 1..max_ids ids drawn with replacement (duplicates count twice); a
+    pod has no class (IMAGE_NONE) with `no_image`.  A share `avoided` of the nodes lists 1-2 of n_controllers
+    controllers, and a pod has a controller bit with `controlled`, else AVOID_NONE."""
+    rng = np.random.default_rng(seed)
+    N, P = snap.nodes.n, snap.pods.n
+    W = (N + 31) // 32
+    fixed = [23 * MIB, 23 * MIB + 1, 1000 * MIB - 1, 1000 * MIB]
+    size = np.zeros(n_images, np.int64)
+    size[:min(4, n_images)] = fixed[:min(4, n_images)]
+    rest = max(n_images - 4, 0)
+    size[4:] = np.where(rng.random(rest) < 0.15, 0, (rng.random(rest) ** 3 * (20 << 30)).astype(np.int64))
+    present = np.zeros((n_images, N), bool)
+    present[:4] = True
+    for i in range(4, n_images):
+        share = rng.choice([-1.0, 0.05, 0.3, 0.7, 1.0])
+        present[i] = rng.random(N) < share if share >= 0 else np.arange(N) == rng.integers(0, max(N, 1))
+    padded = np.zeros((n_images, W * 32), bool)
+    padded[:, :N] = present
+    bits = (padded.reshape(n_images, W, 32).astype(np.uint64) << np.arange(32, dtype=np.uint64)).sum(
+        axis=2, dtype=np.uint64).astype(np.uint32)
+    lens = rng.integers(1, max_ids + 1, n_classes)
+    off = np.concatenate([[0], np.cumsum(lens)]).astype(np.uint32)
+    ids = rng.integers(0, max(n_images, 1), int(off[-1])).astype(np.uint32)
+    if n_classes and lens[0] >= 2 and n_images:
+        ids[1] = ids[0]   # a duplicate image within a class
+    cls = rng.integers(0, max(n_classes, 1), P).astype(np.uint32)
+    cls[(rng.random(P) < no_image) | (n_classes == 0)] = IMAGE_NONE
+    ctrl = rng.integers(0, n_controllers, (N, 2))
+    avoid = (np.uint64(1) << ctrl[:, 0].astype(np.uint64)) | np.where(
+        rng.random(N) < 0.5, np.uint64(1) << ctrl[:, 1].astype(np.uint64), np.uint64(0))
+    avoid = np.where(rng.random(N) < avoided, avoid, np.uint64(0)).astype(np.uint64)
+    abit = np.where(rng.random(P) < controlled, rng.integers(0, n_controllers, P), AVOID_NONE).astype(np.uint8)
+    return (size, bits, avoid), (cls, off, ids, abit)
+
+
 # ----------------------------------------------------------------------------
 # splitmix64 stream (vectorised): value i of the stream with seed s is
 # mix(s + (i+1)*0x9E3779B97F4A7C15).

@@ -517,6 +517,51 @@ int bs_upload_node_preferences(bs_engine* e, uint32_t n_nodes, const uint64_t* p
 /* prefer_tol[n_pods]: the bits of the dictionary each pod tolerates; pref_class[n_pods]: its row of pref_weights or
  * BS_PREF_NONE.  n_pods must equal the pod table's (else BS_E_INVAL); bs_upload_pods drops the side. */
 int bs_upload_pod_preferences(bs_engine* e, uint32_t n_pods, const uint64_t* prefer_tol, const uint32_t* pref_class);
+/* kube-scheduler v1.17's ImageLocality and NodePreferAvoidPods priorities, added to the BS_OUT_PRIORITY score and to
+ * bs_replay_priority's node choice with weights image_locality and prefer_avoid_pods (0, 0 = off, the default;
+ * v1.17's default profile is 1, 10000).  Any time, read by the next evaluation and by bs_replay_priority.  Both terms
+ * are static per (pod, node): nothing is normalized over the fit set.  Per (pod p, node n) [upstream, from memory]:
+ *     NumNodes(i) = the snapshot nodes whose bit of name i is set (every node of the table counts, fitting or not)
+ *     scaled(i) = (int64)((double)image_size[i] * ((double)NumNodes(i) / (double)n_nodes))
+ *                 (binary64, round to nearest, then truncation toward zero)
+ *     sum = the sum of scaled(i) over the ids i of p's class (a repeated id counts again) whose bit is set on n
+ *     IL = 100 * (clamp(sum, 23 MiB, 1000 MiB) - 23 MiB) / 977 MiB       (int64, truncating; 0 for BS_IMAGE_NONE)
+ *     NPA = avoid_bit[p] != BS_AVOID_NONE && bit avoid_bit[p] of avoid_mask[n] is set ? 0 : 100
+ *     score = <the score above> + image_locality * IL + prefer_avoid_pods * NPA   (int64, two's complement wrap)
+ * The caller builds the image dictionary from the names the nodes report (Status.Images[].Names, as reported) that
+ * some pod's normalized container image matches (":latest" appended when the last ':' is not after the last '/'); only
+ * Spec.Containers count.  Builder-defined: NumNodes is counted over the current snapshot, and a name reported with
+ * different sizes takes the size of the lowest node index that reports it.  avoid_bit is the pod's controller of kind
+ * ReplicationController or ReplicaSet in the caller's controller dictionary (at most 64); the caller parses the nodes'
+ * preferAvoidPods annotations, one that fails to parse listing nothing.
+ * An evaluation with BS_OUT_PRIORITY, or bs_replay_priority, with a non-zero weight is BS_E_STATE before anything is
+ * launched when a column it needs is missing (image_locality: the bit rows and sizes, and the pod classes;
+ * prefer_avoid_pods: the avoid masks and the pod bits), and BS_E_INDEX when image_locality is non-zero and a pod's
+ * class is >= n_classes or a class lists an id >= n_images, and BS_E_INVAL when image_locality is non-zero and
+ * n_classes x Npad passes BS_LOC_TABLE_MAX_BYTES for the node table of now.  The class x node IL table is rebuilt on the device at the
+ * first evaluation (or walk) after either side or a weight changes. */
+int bs_set_locality_weights(bs_engine* e, uint32_t image_locality, uint32_t prefer_avoid_pods);
+#define BS_IMAGE_NONE 0xffffffffu                /* image_class of a pod without dictionary images (IL = 0) */
+#define BS_AVOID_NONE 0xffu                      /* avoid_bit of a pod without an RC / RS controller (NPA = 100) */
+#define BS_IMAGE_SIZE_MAX (1ll << 48)            /* largest image size, in bytes */
+#define BS_LOC_CLASS_MAX 64                      /* ids one image class may list: every sum stays below 2^54 */
+#define BS_LOC_TABLE_MAX_BYTES (1ull << 30)      /* n_images x ceil(n_nodes/32) x 4, and n_classes x Npad, each <= 1 GiB */
+/* image_size[n_images]: bytes, each in [0, BS_IMAGE_SIZE_MAX] (else BS_E_RANGE); image_bits[n_images][ceil(n_nodes/32)]:
+ * bit n%32 of word n/32 of row i = node n reports name i; avoid_mask[n_nodes]: bit b = the node's preferAvoidPods
+ * annotation lists controller b of the round's dictionary.  image_size and image_bits may be NULL while image_locality
+ * is 0, avoid_mask while prefer_avoid_pods is 0 (the side then lacks that part).  n_nodes must equal the node table's
+ * (else BS_E_INVAL), a bit table above BS_LOC_TABLE_MAX_BYTES is BS_E_INVAL; a failing call leaves the side dropped.
+ * The side belongs to the node snapshot: bs_upload_nodes and bs_update_nodes drop it. */
+int bs_upload_node_locality(bs_engine* e, uint32_t n_nodes, uint32_t n_images, const int64_t* image_size,
+                            const uint32_t* image_bits, const uint64_t* avoid_mask);
+/* image_class[n_pods]: the pod's class or BS_IMAGE_NONE; class_offset[n_classes + 1] (ascending from 0) and
+ * class_images[class_offset[n_classes]]: the dictionary ids of each class, at most BS_LOC_CLASS_MAX per class (else
+ * BS_E_INVAL); avoid_bit[n_pods]: 0..63 or BS_AVOID_NONE (else BS_E_RANGE).  image_class, class_offset and
+ * class_images may be NULL while image_locality is 0, avoid_bit while prefer_avoid_pods is 0.  n_pods must equal the
+ * pod table's, n_classes x Npad bytes may not pass BS_LOC_TABLE_MAX_BYTES (else BS_E_INVAL); a failing call leaves the
+ * side dropped.  bs_upload_pods drops the side. */
+int bs_upload_pod_locality(bs_engine* e, uint32_t n_pods, const uint32_t* image_class, uint32_t n_classes,
+                           const uint32_t* class_offset, const uint32_t* class_images, const uint8_t* avoid_bit);
 
 /* ---- preemption: PreFilterExtensions.RemovePod and the node / victims kube-scheduler's preemption would pick ----
  * The bound-pod table lists the pods already running on the snapshot's nodes (NodeInfo.Pods()).  Rows may come in

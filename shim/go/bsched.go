@@ -220,6 +220,83 @@ func (e *Engine) UploadPodPreferences(preferTol []uint64, prefClass []uint32) er
 		(*C.uint32_t)(unsafe.Pointer(&prefClass[0]))))
 }
 
+// SetLocalityWeights: kube-scheduler v1.17's ImageLocality and NodePreferAvoidPods weights in the priority lists and
+// in ReplayPriority (0, 0 = off; v1.17's default profile is 1, 10000).
+func (e *Engine) SetLocalityWeights(imageLocality, preferAvoidPods uint32) error {
+	return e.rc(C.bs_set_locality_weights(e.h, C.uint32_t(imageLocality), C.uint32_t(preferAvoidPods)))
+}
+
+// A nil slice is a missing part (NULL), an empty one a part without entries (a non-NULL pointer to locDummy).
+var locDummy [8]byte
+
+func locP(isNil bool, n int, first func() unsafe.Pointer) unsafe.Pointer {
+	if isNil {
+		return nil
+	}
+	if n == 0 {
+		return unsafe.Pointer(&locDummy[0])
+	}
+	return first()
+}
+func locI64(v []int64) *C.int64_t {
+	return (*C.int64_t)(locP(v == nil, len(v), func() unsafe.Pointer { return unsafe.Pointer(&v[0]) }))
+}
+func locU32(v []uint32) *C.uint32_t {
+	return (*C.uint32_t)(locP(v == nil, len(v), func() unsafe.Pointer { return unsafe.Pointer(&v[0]) }))
+}
+func locU64(v []uint64) *C.uint64_t {
+	return (*C.uint64_t)(locP(v == nil, len(v), func() unsafe.Pointer { return unsafe.Pointer(&v[0]) }))
+}
+func locU8(v []uint8) *C.uint8_t {
+	return (*C.uint8_t)(locP(v == nil, len(v), func() unsafe.Pointer { return unsafe.Pointer(&v[0]) }))
+}
+
+// UploadNodeLocality: the image dictionary's sizes (bytes, [0, 2^48]) and bit rows imageBits[len(imageSize)][(n+31)/32]
+// (bit n%32 of word n/32: node n reports the name), and avoidMask[n], per node the bits of the round's controller
+// dictionary that its preferAvoidPods annotation lists.  imageSize and imageBits may both be nil while the
+// ImageLocality weight is 0, avoidMask while the NodePreferAvoidPods weight is 0.  Slices of the wrong length are an
+// error before anything is passed to C.  UploadNodes / UpdateNodes drop it.
+func (e *Engine) UploadNodeLocality(n int, imageSize []int64, imageBits []uint32, avoidMask []uint64) error {
+	if (imageSize == nil) != (imageBits == nil) {
+		return fmt.Errorf("UploadNodeLocality: imageSize and imageBits must both be given or both be nil")
+	}
+	if imageSize != nil && len(imageBits) != len(imageSize)*((n+31)/32) {
+		return fmt.Errorf("UploadNodeLocality: len(imageBits) = %d, want len(imageSize) * ((n + 31) / 32) = %d",
+			len(imageBits), len(imageSize)*((n+31)/32))
+	}
+	if avoidMask != nil && len(avoidMask) != n {
+		return fmt.Errorf("UploadNodeLocality: len(avoidMask) = %d, want n = %d", len(avoidMask), n)
+	}
+	return e.rc(C.bs_upload_node_locality(e.h, C.uint32_t(n), C.uint32_t(len(imageSize)),
+		locI64(imageSize), locU32(imageBits), locU64(avoidMask)))
+}
+
+// UploadPodLocality: imageClass[n], each pod's image class (BS_IMAGE_NONE: none), the classes as
+// classOffset[nClasses+1] into classImages, and avoidBit[n], each pod's controller bit (BS_AVOID_NONE: none).  The
+// three image parts may be nil together while the ImageLocality weight is 0, avoidBit while the NodePreferAvoidPods
+// weight is 0.  Slices of the wrong length are an error before anything is passed to C.  UploadPods drops it.
+func (e *Engine) UploadPodLocality(n int, imageClass, classOffset, classImages []uint32, avoidBit []uint8) error {
+	classes := 0
+	if imageClass != nil || classOffset != nil || classImages != nil {
+		if imageClass == nil || classOffset == nil || classImages == nil {
+			return fmt.Errorf("UploadPodLocality: imageClass, classOffset and classImages must all be given or all be nil")
+		}
+		if len(imageClass) != n {
+			return fmt.Errorf("UploadPodLocality: len(imageClass) = %d, want n = %d", len(imageClass), n)
+		}
+		if len(classOffset) < 1 || int(classOffset[len(classOffset)-1]) > len(classImages) {
+			return fmt.Errorf("UploadPodLocality: classOffset needs nClasses + 1 entries and classImages " +
+				"classOffset[nClasses] of them")
+		}
+		classes = len(classOffset) - 1
+	}
+	if avoidBit != nil && len(avoidBit) != n {
+		return fmt.Errorf("UploadPodLocality: len(avoidBit) = %d, want n = %d", len(avoidBit), n)
+	}
+	return e.rc(C.bs_upload_pod_locality(e.h, C.uint32_t(n), locU32(imageClass), C.uint32_t(classes), locU32(classOffset),
+		locU32(classImages), locU8(avoidBit)))
+}
+
 // UploadNodeNonZero / UploadPodNonZero: the non-zero request columns, nz[2][n] (cpu millicores, then memory bytes):
 // per pod the sum over its containers of GetNonzeroRequestForResource(Requests), per node NodeInfo.NonZeroRequest().
 // UploadNodes / UpdateNodes drop the node column and UploadPods the pod column: upload them again before Evaluate.
