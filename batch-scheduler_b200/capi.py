@@ -184,6 +184,7 @@ SYMBOLS = {
     "bs_fit_shape": (C.c_int, [C.c_void_p, _p(C.c_uint32), _p(C.c_uint32), _p(C.c_uint32)]),
     "bs_fit_lanes": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "bs_sort_shape": (C.c_int, [C.c_void_p, _p(C.c_uint32), _p(C.c_uint32), _p(C.c_uint32), _p(C.c_uint32)]),
+    "bs_replay_shape": (C.c_int, [C.c_void_p] + [_p(C.c_uint32)] * 8),
 }
 
 _lib = None

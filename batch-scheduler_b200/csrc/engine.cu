@@ -434,6 +434,11 @@ struct bs_engine {
   DevBuf d_sort_arena;
   // what the last round's sort launched (bs_sort_shape): kernel 0 none, 1 single-CTA, 2 persistent lean, 3 persistent wide
   struct SortShape { bool valid = false; uint32_t kernel = 0, grid = 0, group_passes = 0, pod_passes = 0; } sort_shape;
+  // the regime of the last bs_replay / bs_replay_priority walk (bs_replay_shape)
+  struct ReplayShape {
+    bool valid = false;
+    uint32_t cached = 0, fitmask = 0, n_rep = 0, n_blocks = 0, bucket_size = 0, n_buckets = 0, lo = 0, monotone = 0;
+  } replay_shape;
 
   // host copies for the per-call mirrors and class building
   std::vector<int32_t> h_gid, h_prio;
@@ -2536,12 +2541,12 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
     tm.launched();
     CK(cudaGetLastError());
   }
-  int32_t status = 0;
+  int32_t status[3] = {};   // panic, final lo, monotone
   std::vector<uint32_t> grc;
   auto d2h = [&](void* dst, const View& src, size_t bytes) {
     return dst && bytes ? cudaMemcpyAsync(dst, src.p, bytes, cudaMemcpyDeviceToHost, e->s) : cudaSuccess;
   };
-  CK(d2h(&status, d_status, 4));
+  CK(d2h(status, d_status, sizeof(status)));
   CK(d2h(out->prefilter, d_pf, n_queue));
   CK(d2h(out->node, d_node, (size_t)n_queue * 4));
   CK(d2h(out->ready, d_ready, n_queue));
@@ -2562,7 +2567,13 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
     CK(d2h(grc.data(), s_grc, (size_t)G * 4));
   }
   CK(cudaStreamSynchronize(e->s));
-  if (status) return fail(e, BS_E_REF_PANIC, (w + ": findMaxPG would divide by MinMember == 0 (core.go:716)").c_str());
+  {
+    // the findMaxPG buckets as replay_kernel cuts them
+    const uint32_t per = cdiv(G, 32u * REPLAY_MAX_BUCKETS), S = 32u * std::max(per, 1u);
+    e->replay_shape = {true, cache, fitmask, e->n_rep_classes, n_blocks, S, cdiv(G, S), (uint32_t)status[1],
+                       (uint32_t)status[2]};
+  }
+  if (status[0]) return fail(e, BS_E_REF_PANIC, (w + ": findMaxPG would divide by MinMember == 0 (core.go:716)").c_str());
   for (uint32_t g = 0; g < G && (out->group_rep_sel || out->group_rep_tol); ++g) {
     const ClassKey& k = e->rep_index.keys[grc[g]];
     if (out->group_rep_sel) out->group_rep_sel[g] = k.sel;
@@ -3391,6 +3402,23 @@ int bs_sort_shape(bs_engine* e, uint32_t* kernel, uint32_t* grid, uint32_t* grou
   if (grid) *grid = e->sort_shape.grid;
   if (group_passes) *group_passes = e->sort_shape.group_passes;
   if (pod_passes) *pod_passes = e->sort_shape.pod_passes;
+  return BS_OK;
+}
+
+int bs_replay_shape(bs_engine* e, uint32_t* cached, uint32_t* fitmask, uint32_t* n_rep, uint32_t* n_blocks,
+                    uint32_t* bucket_size, uint32_t* n_buckets, uint32_t* lo, uint32_t* monotone) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  const auto& r = e->replay_shape;
+  if (!r.valid) return fail(e, BS_E_STATE, "bs_replay_shape: walk first");
+  if (cached) *cached = r.cached;
+  if (fitmask) *fitmask = r.fitmask;
+  if (n_rep) *n_rep = r.n_rep;
+  if (n_blocks) *n_blocks = r.n_blocks;
+  if (bucket_size) *bucket_size = r.bucket_size;
+  if (n_buckets) *n_buckets = r.n_buckets;
+  if (lo) *lo = r.lo;
+  if (monotone) *monotone = r.monotone;
   return BS_OK;
 }
 

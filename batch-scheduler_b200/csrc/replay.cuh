@@ -92,7 +92,8 @@ struct ReplayArgs {
   uint8_t* prefilter;         // [n_queue]
   int32_t* node;              // [n_queue]
   uint8_t* ready;             // [n_queue]
-  int32_t* status;            // [0]: findMaxPG would have divided by zero (core.go:716)
+  int32_t* status;            // [0]: findMaxPG would have divided by zero (core.go:716); [1] the final `lo` of
+                              // the dead-node skip, [2] `monotone` (bs_replay_shape)
   // bs_replay_priority only (SCORED): the live node column, the pod column and the weights of the node choice
   int64_t* nz_live;           // [2][Npad] scratch copy of the uploaded node column
   const int64_t* pod_nz;      // [2][P]
@@ -774,7 +775,7 @@ __global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(std::conditio
       max_dirty = true;
     }
   }
-  if (tid == 0) a.status[0] = sm.panic;
+  if (tid == 0) { a.status[0] = sm.panic; a.status[1] = (int32_t)lo; a.status[2] = sm.monotone; }
 }
 
 }  // namespace bsk

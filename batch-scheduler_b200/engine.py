@@ -593,6 +593,15 @@ class Engine:
         return {"kernel": int(k.value), "grid": int(g.value), "group_passes": int(gp.value),
                 "pod_passes": int(pp.value)}
 
+    def replay_shape(self) -> dict:
+        """The regime of the last replay walk (bs_replay_shape): cached (block-summary cache on), fitmask (checkFit
+        bits per class), n_rep classes, n_blocks of 1024 nodes, findMaxPG's bucket_size and n_buckets, the final lo
+        of the dead-node skip and monotone (no negative fixed-lane request)."""
+        names = ("cached", "fitmask", "n_rep", "n_blocks", "bucket_size", "n_buckets", "lo", "monotone")
+        v = [C.c_uint32() for _ in names]
+        self._check(self.lib.bs_replay_shape(self.h, *[C.byref(x) for x in v]))
+        return {k: int(x.value) for k, x in zip(names, v)}
+
     def score_pitch(self) -> int:
         return int(self.lib.bs_score_pitch(self.h))
 

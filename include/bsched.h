@@ -678,6 +678,15 @@ int bs_fit_lanes(bs_engine* e, uint8_t* kind /*[n_lanes]*/, uint8_t* unit /*[n_l
  * are more tiles than CTAs); and the radix passes kept for the group and the pod table, one per key byte that varies
  * over the table.  BS_E_STATE before the first evaluation. */
 int bs_sort_shape(bs_engine* e, uint32_t* kernel, uint32_t* grid, uint32_t* group_passes, uint32_t* pod_passes);
+/* the regime of the last bs_replay / bs_replay_priority walk (also one that returned BS_E_REF_PANIC): cached 1 when
+ * the cluster check kept per-block summaries (fitmask, every running sum below 2^62, 1 <= n_blocks <= 1024),
+ * fitmask 1 when n_rep <= 32 representative classes had a checkFit bit per node, n_blocks = ceil(n_nodes / 1024),
+ * findMaxPG's n_buckets buckets of bucket_size = 32 * ceil(n_groups / 32768) groups, the walk's final lo (the leading
+ * nodes the node choice stopped visiting because no pod of the table can fit there again) and monotone 1 when no pod
+ * of the table has a negative cpu, memory or ephemeral-storage request (the only case lo advances).  BS_E_STATE
+ * before the first walk. */
+int bs_replay_shape(bs_engine* e, uint32_t* cached, uint32_t* fitmask, uint32_t* n_rep, uint32_t* n_blocks,
+                    uint32_t* bucket_size, uint32_t* n_buckets, uint32_t* lo, uint32_t* monotone);
 
 #ifdef __cplusplus
 }

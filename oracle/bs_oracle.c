@@ -648,6 +648,7 @@ int bso_round(const bso_nodes* nd, const bso_pods* pd, const bso_groups* gr, bso
 int bso_replay(bso_nodes* nd, const bso_pods* pd, bso_groups* gr, const uint32_t* queue,
                uint32_t n_queue, uint8_t* prefilter_out, int32_t* node_out, uint8_t* ready_out) {
   const uint32_t N = nd->n, L = nd->lanes;
+  int panic_at = -1;
   for (uint32_t qi = 0; qi < n_queue; ++qi) {
     const uint32_t p = queue[qi];
     const int g = pd->gid[p];
@@ -681,6 +682,7 @@ int bso_replay(bso_nodes* nd, const bso_pods* pd, bso_groups* gr, const uint32_t
       uint32_t mf;
       int pn;
       const int m = bso_find_max_pg(gr, &mf, &pn);
+      if (pn && panic_at < 0) panic_at = (int)qi;
       if (m < 0) break;
       const uint32_t matched = gr->matched[m];
       bso_resource need, req;
@@ -725,5 +727,5 @@ int bso_replay(bso_nodes* nd, const bso_pods* pd, bso_groups* gr, const uint32_t
       ready_out[qi] = 1;
     }
   }
-  return 0;
+  return panic_at;
 }

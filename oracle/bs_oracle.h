@@ -156,7 +156,9 @@ int bso_round(const bso_nodes* nd, const bso_pods* pd, const bso_groups* gr, bso
  * Pods are processed in queue order; state (requested, pod_count, matched,
  * scheduled, flags) is mutated in place like the reference's caches.  A pod that
  * passes PreFilter is assumed onto the first node (list order) where it fits.
- * prefilter_out[P], node_out[P] (-1 none), ready_out[P].  Returns 0. */
+ * prefilter_out[P], node_out[P] (-1 none), ready_out[P].  Returns the first queue position whose findMaxPG would
+ * divide by MinMember == 0 (core.go:716, where the reference panics), or -1; the walk goes on past it as if that group
+ * were left out, so every output is as without the check. */
 int bso_replay(bso_nodes* nd, const bso_pods* pd, bso_groups* gr, const uint32_t* queue,
                uint32_t n_queue, uint8_t* prefilter_out, int32_t* node_out, uint8_t* ready_out);
 

@@ -250,8 +250,10 @@ def round(snap, want_bitmap=True, want_score=False, faithful=False, threads=0, w
     return r
 
 
-def replay(snap, queue=None):
-    """Sequential pod-at-a-time replay on COPIES of the tables; returns (prefilter, node, ready, snap_after)."""
+def replay(snap, queue=None, panic=False):
+    """Sequential pod-at-a-time replay on COPIES of the tables; returns (prefilter, node, ready, snap_after) and, with
+    panic=True, a fifth value: the first queue position where findMaxPG would divide by MinMember == 0 (the reference
+    panics there; bs_replay returns BS_E_REF_PANIC), or None."""
     s = snap.copy()
     nt, pt, gt = s.nodes, s.pods, s.groups
     q = np.ascontiguousarray(np.arange(pt.n) if queue is None else queue, dtype=np.uint32)
@@ -262,10 +264,13 @@ def replay(snap, queue=None):
         gt.rep_aff = np.full(gt.n, AFF_NONE, np.uint32)   # the walk records the first pod's class here
     nd, pd, gr = _nodes(nt, getattr(s, "aff_bits", None)), _pods(pt), _groups(gt)
     f = lib().bso_replay
+    f.restype = C.c_int
     f.argtypes = [_p(_Nodes), _p(_Pods), _p(_Groups), _p(C.c_uint32), C.c_uint32, _p(C.c_uint8),
                   _p(C.c_int32), _p(C.c_uint8)]
-    f(C.byref(nd), C.byref(pd), C.byref(gr), _ptr(q, C.c_uint32), len(q), _ptr(pf, C.c_uint8),
-      _ptr(node, C.c_int32), _ptr(ready, C.c_uint8))
+    at = f(C.byref(nd), C.byref(pd), C.byref(gr), _ptr(q, C.c_uint32), len(q), _ptr(pf, C.c_uint8),
+           _ptr(node, C.c_int32), _ptr(ready, C.c_uint8))
+    if panic:
+        return pf, node, ready, s, (None if at < 0 else int(at))
     return pf, node, ready, s
 
 
