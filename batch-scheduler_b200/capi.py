@@ -29,6 +29,11 @@ AVOID_NONE = 0xff         # BS_AVOID_NONE: avoid_bit of a pod without an RC / RS
 IMAGE_SIZE_MAX = 1 << 48  # BS_IMAGE_SIZE_MAX: largest image size in bytes
 LOC_CLASS_MAX = 64        # BS_LOC_CLASS_MAX: ids one image class may list
 LOC_TABLE_MAX_BYTES = 1 << 30   # BS_LOC_TABLE_MAX_BYTES: cap of the image bit rows and of the class x node IL table
+SPREAD_NONE = 0xffffffff  # BS_SPREAD_NONE: spread_class of a pod without selectors
+ZONE_NONE = 0xff          # BS_ZONE_NONE: zone of a node without a zone key
+SPREAD_ZONE_MAX = 64      # BS_SPREAD_ZONE_MAX: zones of one node side
+SPREAD_COUNT_MAX = 1 << 24   # BS_SPREAD_COUNT_MAX: largest selector count
+SPREAD_TABLE_MAX_BYTES = 1 << 30   # BS_SPREAD_TABLE_MAX_BYTES: cap of the class x node count table
 # core.PreemptRemovePod verdicts (bs_remove_code) and the bound-pod flag
 REMOVE_ALLOW, REMOVE_OFFLINE_ONLINE, REMOVE_NOT_FOUND, REMOVE_LOCKED, REMOVE_SAME_GROUP = range(5)
 BOUND_GROUP_LOCKED = 0x01
@@ -172,6 +177,9 @@ SYMBOLS = {
     "bs_upload_node_locality": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "bs_upload_pod_locality": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p,
                                          C.c_void_p]),
+    "bs_set_spread_weight": (C.c_int, [C.c_void_p, C.c_uint32]),
+    "bs_upload_node_spread": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p]),
+    "bs_upload_pod_spread": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p]),
     "bs_peer_init": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32]),
     "bs_peer_handle": (C.c_int, [C.c_void_p, C.c_void_p]),
     "bs_peer_attach": (C.c_int, [C.c_void_p, C.c_void_p]),

@@ -428,6 +428,14 @@ struct bs_engine {
   bool loc_dirty = true;
   uint32_t loc_images = 0, loc_classes = 0;
   int64_t loc_class_max = -1, loc_image_max = -1;
+  // SelectorSpread (bs_set_spread_weight; 0 = off): the node side (each node's zone [Npad], the class x node counts
+  // [classes][Npad]; dropped with the node table) and the pod side (each pod's class [P]; dropped with the pod table).
+  // spread_class_max: the largest class a pod names (-1 none), checked against spread_classes at evaluation.
+  uint32_t w_spread = 0;
+  DevBuf d_spread_zone, d_spread_counts, d_spread_class;
+  bool have_spread_node = false, have_spread_pod = false;
+  uint32_t spread_classes = 0;
+  int64_t spread_class_max = -1;
   // sort scratch: views into one arena
   View d_gk0, d_gk1, d_pk0, d_pk1, d_idx_a, d_idx_b, d_ghist, d_group_rank, d_tilecnt, d_sort_barrier;
   uint32_t sort_max_grid = 1;
@@ -1155,6 +1163,12 @@ int evaluate_async_locked(bs_engine* e) {
       return fail(e, BS_E_INDEX, "bs_evaluate: a pod's preference class is outside the uploaded weight table");
   }
   if ((e->out_flags & BS_OUT_PRIORITY) && (rc = locality_check(e, "bs_evaluate"))) return rc;
+  if ((e->out_flags & BS_OUT_PRIORITY) && e->w_spread) {
+    if (!(e->have_spread_node && e->have_spread_pod))
+      return fail(e, BS_E_STATE, "bs_evaluate: a non-zero SelectorSpread weight needs the node and pod spread columns");
+    if (e->spread_class_max >= (int64_t)e->spread_classes)
+      return fail(e, BS_E_INDEX, "bs_evaluate: a pod's spread class is outside the uploaded count table");
+  }
   if (e->peer_broken)
     return fail(e, BS_E_PEER, "peer exchange is broken (a rank did not arrive): bs_peer_detach on every rank, then init/attach again");
   BS_DEVICE_GUARD(e);
@@ -1418,7 +1432,7 @@ int evaluate_async_locked(bs_engine* e) {
     pa.node_req_present = e->d_rpres.as<uint32_t>();
     pa.ratio = e->ratio;
     const uint32_t grid = cdiv(P, PRIO_PODS_PER_CTA);
-    PriorityLocArgs la;
+    PrioritySpreadArgs la;
     static_cast<PriorityRatioArgs&>(la) = pa;
     la.prefer_taints = e->d_prefer_taints.as<uint64_t>();
     la.pref_weights = e->d_pref_weights.as<int32_t>();
@@ -1436,7 +1450,13 @@ int evaluate_async_locked(bs_engine* e) {
       la.w_img = e->w_img;
       la.w_avoid = e->w_avoid;
     }
-    CK(launch_priority(L, grid, ratio, pref, e->w_img || e->w_avoid, la, e->s));
+    if (e->w_spread) {
+      la.spread_zone = e->d_spread_zone.as<uint8_t>();
+      la.spread_counts = e->d_spread_counts.as<int32_t>();
+      la.spread_class = e->d_spread_class.as<uint32_t>();
+      la.w_spread = e->w_spread;
+    }
+    CK(launch_priority(L, grid, ratio, pref, e->w_img || e->w_avoid, e->w_spread != 0, la, e->s));
     e->launches += 1;
   }
   if (e->peer_attached) {
@@ -1659,6 +1679,7 @@ int bs_upload_nodes(bs_engine* e, const bs_node_table* t) {
   e->have_nz_node = false;   // the non-zero column belongs to the node snapshot
   e->have_pref_node = false;   // and so do the PreferNoSchedule masks and the preferred-affinity table
   e->have_img_node = e->have_avoid_node = false;   // and the image rows and preferAvoidPods masks
+  e->have_spread_node = false;   // and the zones and selector counts (counts change when pods bind)
   if (t->n_lanes != e->L) return fail(e, BS_E_INVAL, "bs_upload_nodes: n_lanes differs from the engine's");
   const uint32_t N = t->n_nodes, L = e->L;
   const auto cols = node_cols(e, t);
@@ -1699,6 +1720,7 @@ int bs_update_nodes(bs_engine* e, const uint32_t* idx, const bs_node_table* t) {
   e->have_nz_node = false;   // the changed rows' non-zero requests come with a new column
   e->have_pref_node = false;   // ... and so do their taints and labels: the node preference side is uploaded again
   e->have_img_node = e->have_avoid_node = false;   // ... and their images and annotations: so is the locality side
+  e->have_spread_node = false;   // ... and the pods on them and their zone labels: so is the spread side
   if (t->n_lanes != e->L) return fail(e, BS_E_INVAL, "bs_update_nodes: n_lanes differs from the engine's");
   const uint32_t n = t->n_nodes, L = e->L;
   if (!n) return BS_OK;
@@ -1832,6 +1854,7 @@ int bs_upload_pods(bs_engine* e, const bs_pod_table* t) {
   e->have_nz_pod = false;   // the non-zero column belongs to the pod table
   e->have_pref_pod = false;   // and so does the pod preference side
   e->have_img_pod = e->have_avoid_pod = false;   // and the pod locality side
+  e->have_spread_pod = false;   // and the pod spread side
   if (t->n_lanes != e->L) return fail(e, BS_E_INVAL, "bs_upload_pods: n_lanes differs from the engine's");
   const uint32_t P = t->n_pods, L = e->L;
   if (P && (!t->req || !t->req_present || !t->gid || !t->sel_mask || !t->tol_mask || !t->priority ||
@@ -2596,6 +2619,9 @@ int bs_replay_priority(bs_engine* e, const uint32_t* queue, uint32_t n_queue, bs
   if (e->w_taint || e->w_naff)   // their maxima would have to follow the walk's live fit set, which is not built yet
     return fail(e, BS_E_INVAL, "bs_replay_priority: TaintToleration and NodeAffinity are not supported in the walk; "
                                "set both weights of bs_set_node_priority_weights to 0");
+  if (e->w_spread)   // its maxima and zone sums would follow the live fit set and the live counts, likewise
+    return fail(e, BS_E_INVAL, "bs_replay_priority: SelectorSpread is not supported in the walk; "
+                               "set bs_set_spread_weight to 0");
   return replay_walk(e, "bs_replay_priority", queue, n_queue, out, true, node_nonzero_after);
 }
 
@@ -3232,6 +3258,70 @@ int bs_upload_pod_locality(bs_engine* e, uint32_t n_pods, const uint32_t* image_
   e->loc_image_max = imax;
   e->have_img_pod = img;
   e->have_avoid_pod = avoid_bit != nullptr;
+  return BS_OK;
+}
+
+int bs_set_spread_weight(bs_engine* e, uint32_t selector_spread) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  e->w_spread = selector_spread;
+  return BS_OK;
+}
+
+int bs_upload_node_spread(bs_engine* e, uint32_t n_nodes, uint32_t n_zones, const uint8_t* zone, uint32_t n_classes,
+                          const int32_t* counts) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  const char* who = "bs_upload_node_spread";
+  auto bad = [&](int rc, const char* why) { return fail(e, rc, (std::string(who) + ": " + why).c_str()); };
+  e->have_spread_node = false;
+  if (!e->have_nodes) return bad(BS_E_STATE, "upload nodes first");
+  if (n_nodes != e->N) return bad(BS_E_INVAL, "n_nodes differs from the node table's");
+  if (n_zones > BS_SPREAD_ZONE_MAX) return bad(BS_E_INVAL, "n_zones exceeds BS_SPREAD_ZONE_MAX");
+  const uint32_t Npad = e->Npad;
+  if ((uint64_t)n_classes * Npad * 4 > BS_SPREAD_TABLE_MAX_BYTES)
+    return bad(BS_E_INVAL, "n_classes x padded nodes x 4 bytes exceeds BS_SPREAD_TABLE_MAX_BYTES");
+  if (n_nodes && !zone) return bad(BS_E_INVAL, "null zone");
+  if (n_classes && n_nodes && !counts) return bad(BS_E_INVAL, "null counts");
+  for (uint32_t i = 0; i < n_nodes; ++i)
+    if (zone[i] >= n_zones && zone[i] != BS_ZONE_NONE) return bad(BS_E_INDEX, "a zone id is >= n_zones");
+  for (size_t k = 0; k < (size_t)n_classes * n_nodes; ++k)
+    if (counts[k] < 0 || counts[k] > BS_SPREAD_COUNT_MAX) return bad(BS_E_RANGE, "a count is outside [0, 2^24]");
+  BS_DEVICE_GUARD(e);
+  CK(e->d_spread_zone.ensure(std::max(Npad, 1u)));
+  CK(cudaMemsetAsync(e->d_spread_zone.p, BS_ZONE_NONE, Npad, e->s));   // padding nodes have no zone (and never fit)
+  if (n_nodes) CK(cudaMemcpyAsync(e->d_spread_zone.p, zone, n_nodes, cudaMemcpyHostToDevice, e->s));
+  if (n_classes) {
+    CK(e->d_spread_counts.ensure((size_t)n_classes * Npad * 4));
+    CK(cudaMemsetAsync(e->d_spread_counts.p, 0, (size_t)n_classes * Npad * 4, e->s));
+    if (n_nodes)
+      CK(cudaMemcpy2DAsync(e->d_spread_counts.p, (size_t)Npad * 4, counts, (size_t)n_nodes * 4, (size_t)n_nodes * 4,
+                           n_classes, cudaMemcpyHostToDevice, e->s));
+  }
+  CK(cudaStreamSynchronize(e->s));
+  e->spread_classes = n_classes;
+  e->have_spread_node = true;
+  return BS_OK;
+}
+
+int bs_upload_pod_spread(bs_engine* e, uint32_t n_pods, const uint32_t* spread_class) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  const char* who = "bs_upload_pod_spread";
+  auto bad = [&](int rc, const char* why) { return fail(e, rc, (std::string(who) + ": " + why).c_str()); };
+  e->have_spread_pod = false;
+  if (!e->have_pods) return bad(BS_E_STATE, "upload pods first");
+  if (n_pods != e->P) return bad(BS_E_INVAL, "n_pods differs from the pod table's");
+  if (n_pods && !spread_class) return bad(BS_E_INVAL, "null spread_class");
+  int64_t mx = -1;
+  for (uint32_t p = 0; p < n_pods; ++p)
+    if (spread_class[p] != BS_SPREAD_NONE) mx = std::max(mx, (int64_t)spread_class[p]);
+  BS_DEVICE_GUARD(e);
+  CK(e->d_spread_class.ensure((size_t)std::max(n_pods, 1u) * 4));
+  if (n_pods) CK(cudaMemcpyAsync(e->d_spread_class.p, spread_class, (size_t)n_pods * 4, cudaMemcpyHostToDevice, e->s));
+  CK(cudaStreamSynchronize(e->s));
+  e->spread_class_max = mx;
+  e->have_spread_pod = true;
   return BS_OK;
 }
 

@@ -976,6 +976,8 @@ Status BatchSchedulingPlugin::BeginRound(const std::vector<const NodeInfo*>& sna
     if (!nst.ok()) return nst;
     nst = UploadLocality();
     if (!nst.ok()) return nst;
+    nst = UploadSpread();
+    if (!nst.ok()) return nst;
   }
   {
     Status bst = UploadBound();   // after the groups: the bound rows' group indices refer to this table
@@ -1465,6 +1467,188 @@ Status BatchSchedulingPlugin::UploadLocality() {
   return rc ? fail(rc) : Status{};
 }
 
+void BatchSchedulingPlugin::SetSpreadSelectors(SpreadSelectors selectors) {
+  std::lock_guard<std::mutex> lk(mu_);
+  spread_selectors_ = std::move(selectors);
+}
+
+void BatchSchedulingPlugin::SetSelectorSpreadWeight(uint32_t selector_spread) {
+  std::lock_guard<std::mutex> lk(mu_);
+  spread_weight_ = selector_spread;
+}
+
+namespace {
+// one requirement of a converted selector (labels.Requirement): Equals from a map or matchLabels, or a
+// LabelSelectorRequirement's operator
+struct SpreadReq {
+  std::string key, op;
+  std::vector<std::string> values;   // sorted: the set of the requirement
+};
+using SpreadSel = std::vector<SpreadReq>;   // ANDed; sorted by key, then operator
+
+bool spread_req_matches(const SpreadReq& r, const std::map<std::string, std::string>& labels) {
+  const auto it = labels.find(r.key);
+  const bool has = it != labels.end();
+  auto in = [&] { return has && std::binary_search(r.values.begin(), r.values.end(), it->second); };
+  if (r.op == "=" || r.op == "In") return in();
+  if (r.op == "NotIn") return !in();
+  if (r.op == "Exists") return has;
+  return !has;   // DoesNotExist
+}
+bool spread_sel_matches(const SpreadSel& s, const std::map<std::string, std::string>& labels) {
+  for (const SpreadReq& r : s)
+    if (!spread_req_matches(r, labels)) return false;
+  return true;
+}
+void sort_sel(SpreadSel* s) {
+  for (SpreadReq& r : *s) std::sort(r.values.begin(), r.values.end());
+  std::sort(s->begin(), s->end(), [](const SpreadReq& a, const SpreadReq& b) {
+    return a.key != b.key ? a.key < b.key : a.op != b.op ? a.op < b.op : a.values < b.values;
+  });
+}
+// labels.SelectorFromSet of a Service or RC selector (an empty map: Everything)
+SpreadSel sel_from_map(const std::map<std::string, std::string>& m) {
+  SpreadSel s;
+  for (auto& kv : m) s.push_back(SpreadReq{kv.first, "=", {kv.second}});
+  return s;
+}
+// metav1.LabelSelectorAsSelector of a non-nil selector; false when a requirement fails to convert
+bool sel_from_label_selector(const LabelSelector& ls, SpreadSel* out) {
+  SpreadSel s = sel_from_map(ls.match_labels);
+  for (const LabelSelectorRequirement& r : ls.match_expressions) {
+    if (r.op == "In" || r.op == "NotIn") {
+      if (r.values.empty()) return false;
+    } else if (r.op == "Exists" || r.op == "DoesNotExist") {
+      if (!r.values.empty()) return false;
+    } else {
+      return false;
+    }
+    s.push_back(SpreadReq{r.key, r.op, r.values});
+  }
+  sort_sel(&s);
+  *out = std::move(s);
+  return true;
+}
+// the canonical text of a converted selector (a class key part)
+std::string sel_text(const SpreadSel& s) {
+  std::string t;
+  for (const SpreadReq& r : s) {
+    t += r.key; t += '\x1f'; t += r.op; t += '\x1f';
+    for (auto& v : r.values) { t += v; t += '\x1d'; }
+    t += '\x1e';
+  }
+  return t;
+}
+}  // namespace
+
+Status BatchSchedulingPlugin::PackSpread(const std::vector<const NodeInfo*>& snapshot,
+                                         const std::vector<const Pod*>& pending, const SpreadSelectors& selectors,
+                                         PackedSpread* out) {
+  if (!out) return Status{BS_CODE_ERROR, "PackSpread: null output"};
+  PackedSpread& ps = *out;
+  ps = PackedSpread();
+  const size_t N = snapshot.size(), P = pending.size();
+  // the zone dictionary (utilnode.GetZoneKey: the beta region and zone labels), in order of first appearance
+  ps.zone.assign(N, BS_ZONE_NONE);
+  std::unordered_map<std::string, uint8_t> zone_of;
+  for (size_t i = 0; i < N; ++i) {
+    if (!snapshot[i] || !snapshot[i]->node) continue;
+    const auto& labels = snapshot[i]->node->labels;
+    const auto r = labels.find("failure-domain.beta.kubernetes.io/region");
+    const auto z = labels.find("failure-domain.beta.kubernetes.io/zone");
+    const std::string region = r == labels.end() ? "" : r->second, zone = z == labels.end() ? "" : z->second;
+    if (region.empty() && zone.empty()) continue;
+    const std::string key = region + std::string(":\0:", 3) + zone;
+    auto it = zone_of.find(key);
+    if (it == zone_of.end()) {
+      if (ps.zones.size() == BS_SPREAD_ZONE_MAX)
+        return Status{BS_CODE_ERROR, "PackSpread: more than 64 zones in one round"};
+      it = zone_of.emplace(key, (uint8_t)ps.zones.size()).first;
+      ps.zones.push_back(key);
+    }
+    ps.zone[i] = it->second;
+  }
+  // the converted selectors of the listers' objects, once: (namespace, selector) of those that can select a pod
+  struct Cand {
+    const std::string* ns;
+    SpreadSel sel;
+    bool needs_labels;   // RC / RS / StatefulSet: their listers return an error for a pod without labels
+  };
+  std::vector<Cand> cands;
+  for (const Service& s : selectors.services)
+    if (s.has_selector) cands.push_back(Cand{&s.ns, sel_from_map(s.selector), false});   // nil: matches nothing
+  for (const ReplicationController& c : selectors.controllers)
+    if (c.has_selector && !c.selector.empty()) cands.push_back(Cand{&c.ns, sel_from_map(c.selector), true});
+  auto add_ls = [&](const std::string& ns, bool has, const LabelSelector& ls) {
+    if (!has || (ls.match_labels.empty() && ls.match_expressions.empty())) return;   // nil or empty: nothing
+    SpreadSel s;
+    if (sel_from_label_selector(ls, &s)) cands.push_back(Cand{&ns, std::move(s), true});
+  };
+  for (const ReplicaSet& r : selectors.replica_sets) add_ls(r.ns, r.has_selector, r.selector);
+  for (const StatefulSet& r : selectors.stateful_sets) add_ls(r.ns, r.has_selector, r.selector);
+  // each pod's class: its namespace and the sorted set of its selectors' texts
+  ps.spread_class.assign(P, BS_SPREAD_NONE);
+  std::unordered_map<std::string, uint32_t> class_of;
+  std::vector<std::pair<const std::string*, std::vector<const SpreadSel*>>> class_sels;
+  for (size_t p = 0; p < P; ++p) {
+    if (!pending[p]) continue;
+    const Pod& pod = *pending[p];
+    std::vector<std::pair<std::string, const SpreadSel*>> mine;
+    for (const Cand& c : cands)
+      if (*c.ns == pod.ns && (!c.needs_labels || !pod.labels.empty()) && spread_sel_matches(c.sel, pod.labels))
+        mine.emplace_back(sel_text(c.sel), &c.sel);
+    if (mine.empty()) continue;
+    std::sort(mine.begin(), mine.end(), [](auto& a, auto& b) { return a.first < b.first; });
+    mine.erase(std::unique(mine.begin(), mine.end(), [](auto& a, auto& b) { return a.first == b.first; }), mine.end());
+    std::string sig = pod.ns;
+    for (auto& m : mine) { sig += '\x1c'; sig += m.first; }
+    auto it = class_of.find(sig);
+    if (it == class_of.end()) {
+      it = class_of.emplace(sig, ps.n_classes()).first;
+      ps.class_signatures.push_back(std::move(sig));
+      std::vector<const SpreadSel*> sels;
+      for (auto& m : mine) sels.push_back(m.second);
+      class_sels.emplace_back(&pod.ns, std::move(sels));
+    }
+    ps.spread_class[p] = it->second;
+  }
+  // countMatchingPods over NodeInfo::pods
+  const uint32_t C = ps.n_classes();
+  ps.counts.assign((size_t)C * N, 0);
+  for (uint32_t c = 0; c < C; ++c)
+    for (size_t i = 0; i < N; ++i) {
+      if (!snapshot[i]) continue;
+      int64_t n = 0;
+      for (const Pod* bp : snapshot[i]->pods) {
+        if (!bp || bp->ns != *class_sels[c].first || bp->terminating) continue;
+        bool ok = true;
+        for (const SpreadSel* s : class_sels[c].second)
+          if (!spread_sel_matches(*s, bp->labels)) { ok = false; break; }
+        n += ok;
+      }
+      if (n > BS_SPREAD_COUNT_MAX) return Status{BS_CODE_ERROR, "PackSpread: a count above BS_SPREAD_COUNT_MAX"};
+      ps.counts[(size_t)c * N + i] = (int32_t)n;
+    }
+  return Status{};
+}
+
+Status BatchSchedulingPlugin::UploadSpread() {
+  if (!priority_k_) return Status{};
+  auto fail = [&](int rc) {
+    return Status{BS_CODE_ERROR, std::string("bsched: ") + bs_strerror(rc) + " (" + bs_last_error(eng_) + ")"};
+  };
+  int rc = bs_set_spread_weight(eng_, spread_weight_);
+  if (rc) return fail(rc);
+  if (!spread_weight_) return Status{};
+  PackedSpread ps;
+  Status st = PackSpread(snapshot_, pending_, spread_selectors_, &ps);
+  if (!st.ok()) return st;
+  rc = bs_upload_node_spread(eng_, (uint32_t)snapshot_.size(), (uint32_t)ps.zones.size(), ps.zone.data(), ps.n_classes(),
+                             ps.counts.data());
+  if (!rc) rc = bs_upload_pod_spread(eng_, (uint32_t)pending_.size(), ps.spread_class.data());
+  return rc ? fail(rc) : Status{};
+}
+
 std::vector<uint32_t> BatchSchedulingPlugin::ReasonCounts(const std::string& uid) const {
   const int32_t row = pod_row_.find(uid);
   const size_t R = 4 + packed_.lanes;
@@ -1501,6 +1685,8 @@ Status BatchSchedulingPlugin::UpdateRound(const std::vector<std::pair<uint32_t, 
     st = UploadPreferences();
     if (!st.ok()) return st;
     st = UploadLocality();
+    if (!st.ok()) return st;
+    st = UploadSpread();
     if (!st.ok()) return st;
   }
   return Reevaluate();
@@ -1555,6 +1741,8 @@ Status BatchSchedulingPlugin::UpdateNodes(const std::vector<std::pair<uint32_t, 
   st = UploadPreferences();      // ... and the node preference side (its taint dictionary may change: both sides)
   if (!st.ok()) return st;
   st = UploadLocality();         // ... and the locality side (its dictionaries may change: both sides)
+  if (!st.ok()) return st;
+  st = UploadSpread();           // ... and the spread side (the changed NodeInfos' pods and zones: both sides)
   if (!st.ok()) return st;
   // the round's decisions follow the new snapshot: same pods, same groups, same result vectors
   return evaluate ? Reevaluate() : Status{};
@@ -1784,6 +1972,9 @@ Status BatchSchedulingPlugin::ReplayQueue(std::vector<ReplayDecision>* out, Repl
   if (prio && (node_prio_weights_[0] || node_prio_weights_[1]))
     return Status{BS_CODE_ERROR, "ReplayQueue: kPriority does not support TaintToleration and NodeAffinity yet "
                                  "(SetNodePriorityWeights(0, 0) first)"};
+  if (prio && spread_weight_)
+    return Status{BS_CODE_ERROR, "ReplayQueue: kPriority does not support SelectorSpread yet "
+                                 "(SetSelectorSpreadWeight(0) first)"};
   const uint32_t P = packed_.n_pods;
   std::vector<uint8_t> pf(P), rd(P);
   std::vector<int32_t> nd(P);

@@ -74,6 +74,48 @@ struct Pod {
   int64_t queue_ts_ns = 0;              // framework.PodInfo.Timestamp
   int64_t start_ns = 0;                 // Status.StartTime of a bound pod (preemption: MoreImportantPod)
   std::string controller_kind, controller_uid;   // metav1.GetControllerOf: the controlling owner ("" = none)
+  bool terminating = false;             // DeletionTimestamp != nil (SelectorSpread does not count the pod)
+};
+// metav1.LabelSelectorRequirement / metav1.LabelSelector: the selectors of ReplicaSets and StatefulSets
+// (SelectorSpread).  An In / NotIn requirement without values, an Exists / DoesNotExist one with values, or another
+// operator fails LabelSelectorAsSelector.
+struct LabelSelectorRequirement {
+  std::string key, op /* In | NotIn | Exists | DoesNotExist */;
+  std::vector<std::string> values;
+};
+struct LabelSelector {
+  std::map<std::string, std::string> match_labels;
+  std::vector<LabelSelectorRequirement> match_expressions;
+};
+// The objects whose selectors SelectorSpread spreads by: Services and ReplicationControllers select with a map,
+// ReplicaSets and StatefulSets with a LabelSelector.  has_selector = false is a nil selector, kept distinct from an
+// empty one (an empty Service selector matches every pod; an empty RC, RS or StatefulSet selector matches none).
+struct Service {
+  std::string ns, name;
+  bool has_selector = false;
+  std::map<std::string, std::string> selector;
+};
+struct ReplicationController {
+  std::string ns, name;
+  bool has_selector = false;
+  std::map<std::string, std::string> selector;
+};
+struct ReplicaSet {
+  std::string ns, name;
+  bool has_selector = false;
+  LabelSelector selector;
+};
+struct StatefulSet {
+  std::string ns, name;
+  bool has_selector = false;
+  LabelSelector selector;
+};
+// what the Service, ReplicationController, ReplicaSet and StatefulSet listers hold (SetSpreadSelectors)
+struct SpreadSelectors {
+  std::vector<Service> services;
+  std::vector<ReplicationController> controllers;
+  std::vector<ReplicaSet> replica_sets;
+  std::vector<StatefulSet> stateful_sets;
 };
 // v1.ContainerImage: one entry of Status.Images, the names it is known by and its size (ImageLocality)
 struct ContainerImage {
@@ -209,6 +251,18 @@ struct PackedLocality {
   std::vector<uint64_t> avoid_mask;             // [n_nodes]
   std::vector<uint8_t> avoid_bit;               // [n_pods], BS_AVOID_NONE = no listed RC / RS controller
   uint32_t n_classes() const { return (uint32_t)class_offset.size() - 1; }
+};
+// The columns of the SelectorSpread priority of one round (bs_upload_node_spread, bs_upload_pod_spread): the zone
+// dictionary (GetZoneKey of each node, in order of first appearance, at most 64) and each node's zone; each pending
+// pod's class (its namespace and the sorted set of its selectors' canonical texts; BS_SPREAD_NONE without selectors)
+// and the class x node table of matching pods over NodeInfo::pods.
+struct PackedSpread {
+  std::vector<std::string> zones;               // id z of the zone dictionary
+  std::vector<uint8_t> zone;                    // [n_nodes], BS_ZONE_NONE = no zone key
+  std::vector<uint32_t> spread_class;           // [n_pods], BS_SPREAD_NONE = no selector
+  std::vector<std::string> class_signatures;    // namespace and selector texts of each class
+  std::vector<int32_t> counts;                  // [n_classes][n_nodes]
+  uint32_t n_classes() const { return (uint32_t)class_signatures.size(); }
 };
 // normalizedImageName (ImageLocality): ":latest" appended when the last ':' does not follow the last '/'
 std::string normalized_image_name(const std::string& name);
@@ -390,6 +444,11 @@ class BatchSchedulingPlugin {
   // ReplayQueue(kPriority) (bs_set_locality_weights; 0, 0 = off, the default; v1.17's default profile is 1, 10000),
   // from the next round or delta round on, on a plugin created with priority_k > 0.
   void SetLocalityWeights(uint32_t image_locality, uint32_t prefer_avoid_pods);
+  // the content of the Service, ReplicationController, ReplicaSet and StatefulSet listers, read by the next round
+  void SetSpreadSelectors(SpreadSelectors selectors);
+  // weight of kube-scheduler v1.17's SelectorSpread priority in PriorityNodes (bs_set_spread_weight; 0 = off, the
+  // default; v1.17's default profile is 1), read by the next round; ReplayQueue(kPriority) refuses a non-zero weight
+  void SetSelectorSpreadWeight(uint32_t selector_spread);
   int group_index(const std::string& ns_name) const;
   double last_pack_ms() const { return last_pack_ms_; }
   double last_device_ms() const { return last_device_ms_; }
@@ -467,6 +526,13 @@ class BatchSchedulingPlugin {
   // or more than 64 controllers in the avoid dictionary, is an error.
   static Status PackLocality(const std::vector<const NodeInfo*>& snapshot, const std::vector<const Pod*>& pending,
                              PackedLocality* out);
+  // The columns of the SelectorSpread priority (no GPU).  A pod's selectors are those of getSelectors: the Services of
+  // its namespace whose non-nil selector matches its labels, and, when it has labels, the RCs, ReplicaSets and
+  // StatefulSets of its namespace whose non-empty selector matches them (a selector that fails to convert is
+  // skipped).  count(class, node) = the pods of NodeInfo::pods in the class's namespace, not terminating, that every
+  // selector matches.  More than 64 zones, or a count above BS_SPREAD_COUNT_MAX, is an error.
+  static Status PackSpread(const std::vector<const NodeInfo*>& snapshot, const std::vector<const Pod*>& pending,
+                           const SpreadSelectors& selectors, PackedSpread* out);
 
   static Status Pack(const std::vector<const NodeInfo*>& snapshot, const std::vector<const Pod*>& pending,
                      const std::vector<PodGroup>& groups, const std::vector<uint32_t>& matched,
@@ -497,6 +563,8 @@ class BatchSchedulingPlugin {
   std::map<std::string, uint32_t> ratio_resources_{{"cpu", 1}, {"memory", 1}};
   uint32_t node_prio_weights_[2] = {0, 0};             // SetNodePriorityWeights: TaintToleration, NodeAffinity
   uint32_t locality_weights_[2] = {0, 0};              // SetLocalityWeights: ImageLocality, NodePreferAvoidPods
+  uint32_t spread_weight_ = 0;                          // SetSelectorSpreadWeight
+  SpreadSelectors spread_selectors_;                    // SetSpreadSelectors
   std::string init_error_;
   int64_t max_schedule_time_ns_;
   std::map<std::string, GroupState> groups_;                        // ordered: canonical table order
@@ -530,6 +598,8 @@ class BatchSchedulingPlugin {
                                                                   // priority_k
   Status UploadPreferences();   // both preference sides of snapshot_ and pending_ and the two weights; the columns only
                                 // while a weight is non-zero; no-op without priority_k
+  Status UploadSpread();     // both spread sides of snapshot_ and pending_ and the weight; the columns only while the
+                             // weight is non-zero; no-op without priority_k
   Status UploadLocality();   // both locality sides of snapshot_ and pending_ and the two weights; the columns only
                              // while a weight is non-zero; no-op without priority_k
   Status UploadBound();  // packs and uploads the bound-pod table of snapshot_ (no-op when no NodeInfo lists pods)

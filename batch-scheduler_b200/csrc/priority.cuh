@@ -7,7 +7,8 @@
 // The lists are kept with gang_fit's topk_insert (fit.cuh); the pair scorer pair_score is kernels.cuh's, and with RATIO
 // the RequestedToCapacityRatio term (kernels.cuh ratio_*) is added to it; with PREF the TaintToleration and preferred
 // NodeAffinity terms (bs_set_node_priority_weights), normalized over the pod's fit set; with LOC the ImageLocality and
-// NodePreferAvoidPods terms (bs_set_locality_weights), static per pair, from the pre-pass below.
+// NodePreferAvoidPods terms (bs_set_locality_weights), static per pair, from the pre-pass below; with SPREAD the
+// SelectorSpread term (bs_set_spread_weight), normalized over the pod's fit set and its zones.
 #pragma once
 #include "kernels.cuh"
 #include "fit.cuh"
@@ -106,6 +107,31 @@ __device__ __forceinline__ uint64_t loc_term(const PriorityLocArgs& a, const uin
   return (uint64_t)a.w_img * il + (uint64_t)a.w_avoid * ((node_avoid & amask) ? 0u : 100u);
 }
 
+// SPREAD's arguments (bs_upload_node_spread / bs_upload_pod_spread): each node's zone, the class x node counts, each
+// pod's class, and the weight.  Derived from LOC's type for the same reason; the fields of the other flags are read only
+// with their flags.
+constexpr uint32_t SPREAD_NONE = 0xffffffffu;   // BS_SPREAD_NONE
+constexpr uint32_t ZONE_NONE = 0xffu;           // BS_ZONE_NONE
+constexpr int SPREAD_ZONES = 64;                // BS_SPREAD_ZONE_MAX
+struct PrioritySpreadArgs : PriorityLocArgs {
+  const uint8_t* spread_zone;     // [Npad] 0..63 or ZONE_NONE (padding ZONE_NONE)
+  const int32_t* spread_counts;   // [classes][Npad] (padding 0)
+  const uint32_t* spread_class;   // [P] row of spread_counts or SPREAD_NONE
+  uint32_t w_spread;
+};
+// SelectorSpread of one fitting pair (CalculateSpreadPriorityReduce): cnt = the pair's count, mn = the pod's maximum
+// over its fit set, zsum / mz = the sum of the node's zone and the largest zone sum (zoned: the node has a zone).  Every operation is a binary64 rounding of its own whatever -fmad says, and the
+// result is truncated toward zero.
+__device__ __forceinline__ int64_t spread_score(uint32_t cnt, uint32_t mn, bool zoned, uint64_t zsum, uint64_t mz) {
+  constexpr double ZW = 2.0 / 3.0;   // zoneWeighting
+  double f = mn > 0 ? __dmul_rn(100.0, __ddiv_rn((double)(mn - cnt), (double)mn)) : 100.0;
+  if (zoned) {
+    const double zs = mz > 0 ? __dmul_rn(100.0, __ddiv_rn(__ull2double_rn(mz - zsum), __ull2double_rn(mz))) : 100.0;
+    f = __dadd_rn(__dmul_rn(f, 1.0 - ZW), __dmul_rn(ZW, zs));
+  }
+  return __double2ll_rz(f);
+}
+
 // The LOC pre-pass (priority_inst.cu image_spread_kernel, locality_class_kernel) builds the IL table once per
 // change of either side or a weight.
 constexpr int LOC_THREADS = 256;
@@ -120,13 +146,23 @@ constexpr int LOC_THREADS = 256;
 // LOC (chosen by the host when either weight of bs_set_locality_weights is non-zero) adds w_img * IL + w_avoid * NPA:
 // one byte of the pod's IL row per pair, read by adjacent lanes, and the node's avoid mask, shared by the warp's pods.
 //
-// LOC's kernels ask for two CTAs per SM: left to itself, ptxas gives the PREF + LOC variants up to 145 registers, which
-// fits one 256-thread CTA per SM where the kernels without LOC run two.
-template <int MAXL, bool RATIO, bool PREF, bool LOC = false>
-__global__ void __launch_bounds__(PRIO_THREADS, LOC ? 2 : 0)
-priority_pod_kernel(std::conditional_t<LOC, PriorityLocArgs,
+// SPREAD (chosen by the host when bs_set_spread_weight is non-zero) adds w_spread * SS.  Like PREF it needs the pod's
+// maxima over its fit set before the first pair is scored, so the first sweep (one sweep for PREF, SPREAD or both)
+// also keeps, per pod, the largest count (a register per lane, reduced after the sweep) and each zone's sum of counts
+// over the fitting nodes (s_zs, shared memory).  A node with count 0 adds nothing to its zone, so only nodes with a
+// count reach s_zs: the lanes with the same zone add theirs with __match_any_sync and __reduce_add_sync, and one lane
+// of each zone adds the result with one shared atomic.  After the sweep the warp takes each pod's largest zone sum.
+// haveZones needs no state of its own: it only changes the score of a fitting node with a zone, and that node makes it
+// true.  A pod without selectors (SPREAD_NONE) scores 100 and reads nothing.
+//
+// LOC's and SPREAD's kernels ask for two CTAs per SM: left to itself, ptxas gives the PREF + LOC variants up to 145
+// registers, which fits one 256-thread CTA per SM where the kernels without LOC run two.
+template <int MAXL, bool RATIO, bool PREF, bool LOC = false, bool SPREAD = false>
+__global__ void __launch_bounds__(PRIO_THREADS, (LOC || SPREAD) ? 2 : 0)
+priority_pod_kernel(std::conditional_t<SPREAD, PrioritySpreadArgs,
+                    std::conditional_t<LOC, PriorityLocArgs,
                                        std::conditional_t<PREF, PriorityPrefArgs,
-                                                          std::conditional_t<RATIO, PriorityRatioArgs, PriorityArgs>>> a) {
+                                                          std::conditional_t<RATIO, PriorityRatioArgs, PriorityArgs>>>> a) {
   constexpr int WARPS = PRIO_THREADS / 32;
   __shared__ int64_t s_req[WARPS][PRIO_PPW][MAXL];
   __shared__ int64_t s_ls[WARPS][PRIO_PPW][32];
@@ -178,13 +214,30 @@ priority_pod_kernel(std::conditional_t<LOC, PriorityLocArgs,
   }
   [[maybe_unused]] uint64_t ptol[PRIO_PPW];
   [[maybe_unused]] uint32_t pcls[PRIO_PPW], mt[PRIO_PPW], ma[PRIO_PPW];   // PREF: the pod's maxima over its fit set
-  if constexpr (PREF) {
+  // SPREAD: the pod's class, its largest count and largest zone sum over its fit set
+  [[maybe_unused]] uint32_t scls[PRIO_PPW], mn[PRIO_PPW];
+  [[maybe_unused]] uint64_t mz[PRIO_PPW];
+  [[maybe_unused]] uint64_t (*zs)[SPREAD_ZONES] = nullptr;   // SPREAD: the warp's zone sums, [PRIO_PPW][64]
+  if constexpr (SPREAD) {
+    __shared__ uint64_t s_zs[WARPS][PRIO_PPW][SPREAD_ZONES];
+    zs = s_zs[wid];
+    for (uint32_t k = lane; k < PRIO_PPW * SPREAD_ZONES; k += 32) zs[k / SPREAD_ZONES][k % SPREAD_ZONES] = 0;
 #pragma unroll
     for (int j = 0; j < PRIO_PPW; ++j) {
-      const uint32_t p = p0 + j;
-      ptol[j] = rmask[j] && a.w_taint ? a.prefer_tol[p] : 0;   // a column whose weight is 0 may be missing
-      pcls[j] = rmask[j] && a.w_naff ? a.pref_class[p] : PREF_NONE;
-      mt[j] = ma[j] = 0;
+      scls[j] = rmask[j] ? a.spread_class[p0 + j] : SPREAD_NONE;
+      mn[j] = 0;
+    }
+    __syncwarp();
+  }
+  if constexpr (PREF || SPREAD) {
+    if constexpr (PREF) {
+#pragma unroll
+      for (int j = 0; j < PRIO_PPW; ++j) {
+        const uint32_t p = p0 + j;
+        ptol[j] = rmask[j] && a.w_taint ? a.prefer_tol[p] : 0;   // a column whose weight is 0 may be missing
+        pcls[j] = rmask[j] && a.w_naff ? a.pref_class[p] : PREF_NONE;
+        mt[j] = ma[j] = 0;
+      }
     }
     // the first sweep: the fit test of the scoring sweep below, then the raw counts of the fitting nodes
     for (uint32_t base = 0; base < a.N; base += 32) {
@@ -208,20 +261,52 @@ priority_pod_kernel(std::conditional_t<LOC, PriorityLocArgs,
         for (int j = 0; j < PRIO_PPW; ++j)
           if (((rmask[j] >> d) & 1u) && lane_short(pres, v, s_req[wid][j][d])) g[j] = false;
       }
-      const uint64_t taints = a.w_taint ? a.prefer_taints[i] : 0;
+      if constexpr (PREF) {
+        const uint64_t taints = a.w_taint ? a.prefer_taints[i] : 0;
 #pragma unroll
-      for (int j = 0; j < PRIO_PPW; ++j) {
-        if (!g[j]) continue;
-        uint32_t t, aw;
-        pref_counts(a, taints, ptol[j], pcls[j], i, t, aw);
-        mt[j] = max(mt[j], t);
-        ma[j] = max(ma[j], aw);
+        for (int j = 0; j < PRIO_PPW; ++j) {
+          if (!g[j]) continue;
+          uint32_t t, aw;
+          pref_counts(a, taints, ptol[j], pcls[j], i, t, aw);
+          mt[j] = max(mt[j], t);
+          ma[j] = max(ma[j], aw);
+        }
+      }
+      if constexpr (SPREAD) {
+        const uint32_t z = a.spread_zone[i];   // i < Npad: padding is ZONE_NONE
+#pragma unroll
+        for (int j = 0; j < PRIO_PPW; ++j) {
+          if (scls[j] == SPREAD_NONE) continue;   // warp-uniform
+          const uint32_t cnt = g[j] ? (uint32_t)a.spread_counts[(size_t)scls[j] * a.Npad + i] : 0u;
+          mn[j] = max(mn[j], cnt);
+          // zone sums: one shared atomic per zone that some lane's count reaches
+          const bool add = cnt != 0 && z != ZONE_NONE;
+          if (!__any_sync(0xffffffffu, add)) continue;   // warp-uniform
+          const uint32_t peers = __match_any_sync(0xffffffffu, add ? z : 0xffffffffu);
+          if (add) {
+            const uint32_t sum = __reduce_add_sync(peers, cnt);   // at most 32 x 2^24: no wrap
+            if (lane == (uint32_t)(__ffs(peers) - 1)) atomicAdd((unsigned long long*)&zs[j][z], (unsigned long long)sum);
+          }
+        }
       }
     }
+    if constexpr (PREF) {
 #pragma unroll
-    for (int j = 0; j < PRIO_PPW; ++j) {
-      mt[j] = __reduce_max_sync(0xffffffffu, mt[j]);
-      ma[j] = __reduce_max_sync(0xffffffffu, ma[j]);
+      for (int j = 0; j < PRIO_PPW; ++j) {
+        mt[j] = __reduce_max_sync(0xffffffffu, mt[j]);
+        ma[j] = __reduce_max_sync(0xffffffffu, ma[j]);
+      }
+    }
+    if constexpr (SPREAD) {
+      __syncwarp();
+#pragma unroll
+      for (int j = 0; j < PRIO_PPW; ++j) {
+        mn[j] = __reduce_max_sync(0xffffffffu, mn[j]);
+        uint64_t m = max(zs[j][lane], zs[j][lane + 32]);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
+        mz[j] = m;
+      }
     }
   }
   for (uint32_t base = 0; base < a.N; base += 32) {
@@ -256,6 +341,8 @@ priority_pod_kernel(std::conditional_t<LOC, PriorityLocArgs,
     const int64_t n_cpu = a.node_nz[i], n_mem = a.node_nz[(size_t)a.Npad + i];
     [[maybe_unused]] uint64_t navoid = 0;   // LOC: the node's preferAvoidPods mask
     if constexpr (LOC) navoid = a.w_avoid ? a.avoid_mask[i] : 0;
+    [[maybe_unused]] uint32_t nzone = ZONE_NONE;   // SPREAD: the node's zone
+    if constexpr (SPREAD) nzone = a.spread_zone[i];
     [[maybe_unused]] uint32_t rnum[PRIO_PPW], rden[PRIO_PPW];   // RATIO: the weighted sum and weight sum of each pod's average
     if constexpr (RATIO) {
 #pragma unroll
@@ -297,6 +384,16 @@ priority_pod_kernel(std::conditional_t<LOC, PriorityLocArgs,
         }
       if constexpr (LOC)
         if (g[j]) s = (int64_t)((uint64_t)s + loc_term(a, lrow[j], lmask[j], i, navoid));
+      if constexpr (SPREAD)
+        if (g[j]) {
+          int64_t ss = 100;
+          if (scls[j] != SPREAD_NONE) {
+            const bool zoned = nzone != ZONE_NONE;   // a fitting node with a zone: haveZones holds
+            ss = spread_score((uint32_t)a.spread_counts[(size_t)scls[j] * a.Npad + i], mn[j], zoned,
+                              zoned ? zs[j][nzone] : 0ull, mz[j]);
+          }
+          s = (int64_t)((uint64_t)s + (uint64_t)a.w_spread * (uint64_t)ss);
+        }
       const uint32_t cb = __ballot_sync(0xffffffffu, g[j] && (nfit[j] < a.K || s > thr[j]));
       if (cb) thr[j] = topk_insert<int64_t>(s_ls[wid][j], s_ln[wid][j], a.K, cb, s, (int32_t)base, lane);
       nfit[j] += __popc(fw[j]);
@@ -314,10 +411,15 @@ priority_pod_kernel(std::conditional_t<LOC, PriorityLocArgs,
 }
 
 // priority_inst.cu, a translation unit of its own so that the variants compile in parallel with engine.cu:
-// priority_pod_kernel<MAXL, ratio, pref, loc> for the engine's lane count L; `a` is read as the flags' argument type
-// (PriorityArgs without any flag, PriorityRatioArgs with ratio alone, PriorityPrefArgs with pref, all of it with loc).
-cudaError_t launch_priority(uint32_t L, uint32_t grid, bool ratio, bool pref, bool loc, const PriorityLocArgs& a,
-                            cudaStream_t s);
+// priority_pod_kernel<MAXL, ratio, pref, loc, spread> for the engine's lane count L; `a` is read as the flags' argument
+// type (PriorityArgs without any flag, PriorityRatioArgs with ratio alone, PriorityPrefArgs with pref, PriorityLocArgs
+// with loc, all of it with spread).
+cudaError_t launch_priority(uint32_t L, uint32_t grid, bool ratio, bool pref, bool loc, bool spread,
+                            const PrioritySpreadArgs& a, cudaStream_t s);
+// priority_spread_inst.cu, one translation unit per MAXL (-DBS_PRIO_SPREAD_MAXL): the SPREAD variants, reached through
+// launch_priority
+template <int MAXL>
+void launch_priority_spread(uint32_t grid, bool ratio, bool pref, bool loc, const PrioritySpreadArgs& a, cudaStream_t s);
 // the LOC pre-pass: scaled[n_images] from the bit rows and sizes, then il[n_classes][Npad]; 2 launches
 cudaError_t launch_locality_prepass(const uint32_t* bits, const int64_t* size, int64_t* scaled, uint32_t n_images,
                                     const uint32_t* class_offset, const uint32_t* class_images, uint8_t* il,

@@ -1,6 +1,6 @@
 // priority_inst.cu — the priority lists' kernels (priority.cuh): every priority_pod_kernel variant and the LOC
-// pre-pass.  A translation unit of its own (build.py), compiled in parallel with engine.cu, which reaches the kernels
-// through launch_priority and launch_locality_prepass.
+// pre-pass, except the SPREAD variants (priority_spread_inst.cu).  A translation unit of its own (build.py), compiled in
+// parallel with engine.cu, which reaches the kernels through launch_priority and launch_locality_prepass.
 #define BS_KERNELS_HELPERS_ONLY   // kernels.cuh's round kernels live in engine.cu
 #include "priority.cuh"
 
@@ -74,16 +74,21 @@ void launch_t(uint32_t L, uint32_t grid, const Args& a, cudaStream_t s) {
 
 }  // namespace
 
-cudaError_t launch_priority(uint32_t L, uint32_t grid, bool ratio, bool pref, bool loc, const PriorityLocArgs& a,
-                            cudaStream_t s) {
+cudaError_t launch_priority(uint32_t L, uint32_t grid, bool ratio, bool pref, bool loc, bool spread,
+                            const PrioritySpreadArgs& a, cudaStream_t s) {
+  const PriorityLocArgs& pl = a;
   const PriorityPrefArgs& pp = a;
   const PriorityRatioArgs& pr = a;
   const PriorityArgs& pb = a;
-  if (loc) {
-    if (pref && ratio) launch_t<true, true, true>(L, grid, a, s);
-    else if (pref) launch_t<false, true, true>(L, grid, a, s);
-    else if (ratio) launch_t<true, false, true>(L, grid, a, s);
-    else launch_t<false, false, true>(L, grid, a, s);
+  if (spread) {
+    if (L <= 5) launch_priority_spread<5>(grid, ratio, pref, loc, a, s);
+    else if (L <= 9) launch_priority_spread<9>(grid, ratio, pref, loc, a, s);
+    else launch_priority_spread<16>(grid, ratio, pref, loc, a, s);
+  } else if (loc) {
+    if (pref && ratio) launch_t<true, true, true>(L, grid, pl, s);
+    else if (pref) launch_t<false, true, true>(L, grid, pl, s);
+    else if (ratio) launch_t<true, false, true>(L, grid, pl, s);
+    else launch_t<false, false, true>(L, grid, pl, s);
   } else if (pref) {
     if (ratio) launch_t<true, true, false>(L, grid, pp, s);
     else launch_t<false, true, false>(L, grid, pp, s);

@@ -363,6 +363,32 @@ class Engine:
             self._check(self.lib.bs_upload_pod_locality(self.h, n, capi.ptr(cls), n_classes, capi.ptr(off),
                                                         capi.ptr(ids), capi.ptr(abit)))
 
+    def set_spread_weight(self, selector_spread: int = 0):
+        """Weight of kube-scheduler's SelectorSpread priority in the priority score (0 = off, the default; v1.17's
+        default profile is 1).  A non-zero weight needs upload_spread before each round, and makes
+        replay(priority=True) refuse to run."""
+        self._check(self.lib.bs_set_spread_weight(self.h, selector_spread))
+
+    def upload_spread(self, node=None, pods=None, n_zones=None):
+        """The columns of SelectorSpread.  node = (zone [N] uint8, counts [C, N] int32): each node's zone in the round's
+        zone dictionary (capi.ZONE_NONE: no zone) and counts[c, n] the pods on node n that class c's selectors match.
+        n_zones defaults to one more than the largest zone id.  pods = spread_class [P] uint32: each pod's class
+        (capi.SPREAD_NONE: no selectors).  Uploading nodes (or updating node rows) drops the node side, uploading pods
+        the pod side."""
+        if node is not None:
+            zone = np.ascontiguousarray(node[0], dtype=np.uint8).reshape(-1)
+            counts = np.ascontiguousarray(node[1], dtype=np.int32)
+            if counts.ndim != 2 or counts.shape[1] != len(zone):
+                raise ValueError("counts must be [classes, N] with N = len(zone)")
+            if n_zones is None:
+                real = zone[zone != capi.ZONE_NONE]
+                n_zones = int(real.max()) + 1 if len(real) else 0
+            self._check(self.lib.bs_upload_node_spread(self.h, len(zone), n_zones, capi.ptr(zone), counts.shape[0],
+                                                       capi.ptr(counts)))
+        if pods is not None:
+            cls = np.ascontiguousarray(pods, dtype=np.uint32).reshape(-1)
+            self._check(self.lib.bs_upload_pod_spread(self.h, len(cls), capi.ptr(cls)))
+
     def priority_rows(self, pod0=0, n=None):
         """(nodes [n, K] int32, scores [n, K] int64): each pod's fitting nodes by priority score descending, then node
         index ascending; min(K, feasible_count) entries, padded with node -1 and score INT64_MIN."""

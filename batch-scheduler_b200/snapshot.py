@@ -449,6 +449,26 @@ def node_locality(snap: Snapshot, seed: int, n_images: int = 16, n_classes: int 
     return (size, bits, avoid), (cls, off, ids, abit)
 
 
+SPREAD_NONE = 0xFFFFFFFF   # BS_SPREAD_NONE
+ZONE_NONE = 0xFF           # BS_ZONE_NONE
+
+
+def node_spread(snap: Snapshot, seed: int, n_zones: int = 4, unzoned: float = 0.2, n_classes: int = 6,
+                occupied: float = 0.3, max_count: int = 6, no_class: float = 0.25):
+    """Seeded columns of the SelectorSpread priority for a table without objects: (node, pods) with node = (zone [N]
+    uint8, counts [n_classes, N] int32) and pods = spread_class [P] uint32.  A share `unzoned` of the nodes has no zone
+    (ZONE_NONE), the rest lie in one of n_zones zones; a class counts 1..max_count matching pods on a share `occupied`
+    of the nodes and 0 elsewhere; a pod has no class (SPREAD_NONE) with `no_class`."""
+    rng = np.random.default_rng(seed)
+    N, P = snap.nodes.n, snap.pods.n
+    zone = rng.integers(0, max(n_zones, 1), N).astype(np.uint8)
+    zone[(rng.random(N) < unzoned) | (n_zones == 0)] = ZONE_NONE
+    counts = np.where(rng.random((n_classes, N)) < occupied, rng.integers(1, max_count + 1, (n_classes, N)), 0)
+    cls = rng.integers(0, max(n_classes, 1), P).astype(np.uint32)
+    cls[(rng.random(P) < no_class) | (n_classes == 0)] = SPREAD_NONE
+    return (zone, counts.astype(np.int32)), cls
+
+
 # ----------------------------------------------------------------------------
 # splitmix64 stream (vectorised): value i of the stream with seed s is
 # mix(s + (i+1)*0x9E3779B97F4A7C15).

@@ -562,6 +562,42 @@ int bs_upload_node_locality(bs_engine* e, uint32_t n_nodes, uint32_t n_images, c
  * side dropped.  bs_upload_pods drops the side. */
 int bs_upload_pod_locality(bs_engine* e, uint32_t n_pods, const uint32_t* image_class, uint32_t n_classes,
                            const uint32_t* class_offset, const uint32_t* class_images, const uint8_t* avoid_bit);
+/* kube-scheduler v1.17's SelectorSpread priority, added to the BS_OUT_PRIORITY score with weight selector_spread
+ * (0 = off, the default; v1.17's default profile is 1).  Any time, read by the next evaluation.  Per (pod p, node n)
+ * [upstream, from memory]:
+ *     count(p, n) = counts[spread_class[p]][n]: the pods of NodeInfo.Pods() on n in p's namespace, not terminating,
+ *                   whose labels match every selector of p's Services, ReplicationControllers, ReplicaSets and
+ *                   StatefulSets; 0 on every node for BS_SPREAD_NONE (a pod without selectors)
+ *     F = the pod's fit set (the nodes of its fit-bitmap row); no other node counts, for any of the following
+ *     Mn = max count(p, n) over F;  Zn(z) = sum of count(p, n) over the nodes of F in zone z;  Mz = max Zn over zones
+ *     haveZones = some node of F has a zone (zone[n] != BS_ZONE_NONE), whatever its count
+ *     f = Mn > 0 ? 100.0 * ((double)(Mn - count) / (double)Mn) : 100.0
+ *     if haveZones and zone[n] != BS_ZONE_NONE:
+ *         zs = Mz > 0 ? 100.0 * ((double)(Mz - Zn(zone[n])) / (double)Mz) : 100.0
+ *         f = (f * (1.0 - zw)) + (zw * zs)          zw = 2.0 / 3.0 rounded to binary64
+ *     SS = (int64)f                                 (binary64, each operation rounded on its own; truncation)
+ *     score = <the score above> + selector_spread * SS                  (int64, two's complement wrap)
+ * A BS_SPREAD_NONE pod scores SS = 100 on every fitting node.  The caller builds the zone dictionary from the node
+ * labels failure-domain.beta.kubernetes.io/region and /zone (key region + ":\x00:" + zone, none when both are empty)
+ * and the classes from the listers; every fitting node is scored, and ties go to the lower node index.
+ * An evaluation with BS_OUT_PRIORITY and a non-zero weight is BS_E_STATE before anything is launched when either side
+ * is missing, and BS_E_INDEX when a pod's class is >= n_classes.  bs_replay_priority refuses to run (BS_E_INVAL) while
+ * the weight is non-zero. */
+int bs_set_spread_weight(bs_engine* e, uint32_t selector_spread);
+#define BS_SPREAD_NONE 0xffffffffu               /* spread_class of a pod without selectors (SS = 100) */
+#define BS_ZONE_NONE 0xffu                       /* zone of a node without a zone key */
+#define BS_SPREAD_ZONE_MAX 64                    /* zones of one node side */
+#define BS_SPREAD_COUNT_MAX (1 << 24)            /* largest count: every zone sum stays exact in binary64 */
+#define BS_SPREAD_TABLE_MAX_BYTES (1ull << 30)   /* n_classes x Npad x 4 (Npad: n_nodes rounded up) at most 1 GiB */
+/* zone[n_nodes]: 0..n_zones-1 or BS_ZONE_NONE (else BS_E_INDEX); counts[n_classes][n_nodes]: count(class, node), each
+ * in [0, BS_SPREAD_COUNT_MAX] (else BS_E_RANGE).  n_nodes must equal the node table's, n_zones may not pass
+ * BS_SPREAD_ZONE_MAX and the table BS_SPREAD_TABLE_MAX_BYTES (else BS_E_INVAL); a failing call leaves the side dropped.
+ * The side belongs to the node snapshot (counts change when pods bind): bs_upload_nodes and bs_update_nodes drop it. */
+int bs_upload_node_spread(bs_engine* e, uint32_t n_nodes, uint32_t n_zones, const uint8_t* zone, uint32_t n_classes,
+                          const int32_t* counts);
+/* spread_class[n_pods]: the pod's row of counts or BS_SPREAD_NONE.  n_pods must equal the pod table's (else
+ * BS_E_INVAL); a failing call leaves the side dropped.  bs_upload_pods drops the side. */
+int bs_upload_pod_spread(bs_engine* e, uint32_t n_pods, const uint32_t* spread_class);
 
 /* ---- preemption: PreFilterExtensions.RemovePod and the node / victims kube-scheduler's preemption would pick ----
  * The bound-pod table lists the pods already running on the snapshot's nodes (NodeInfo.Pods()).  Rows may come in

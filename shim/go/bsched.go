@@ -297,6 +297,47 @@ func (e *Engine) UploadPodLocality(n int, imageClass, classOffset, classImages [
 		locU32(classImages), locU8(avoidBit)))
 }
 
+// SetSpreadWeight: kube-scheduler v1.17's SelectorSpread weight in the priority lists (0 = off; v1.17's default
+// profile is 1).  ReplayPriority refuses a non-zero weight.
+func (e *Engine) SetSpreadWeight(selectorSpread uint32) error {
+	return e.rc(C.bs_set_spread_weight(e.h, C.uint32_t(selectorSpread)))
+}
+
+// UploadNodeSpread: zone[n], each node's id in the round's zone dictionary of nZones keys (BS_ZONE_NONE: no zone
+// key), and counts[classes][n], per class the pods on each node that its selectors match.  Slices of the wrong length
+// are an error before anything is passed to C.  UploadNodes / UpdateNodes drop it.
+func (e *Engine) UploadNodeSpread(n, nZones int, zone []uint8, counts []int32) error {
+	if len(zone) != n {
+		return fmt.Errorf("UploadNodeSpread: len(zone) = %d, want n = %d", len(zone), n)
+	}
+	classes := 0
+	if n > 0 {
+		if len(counts)%n != 0 {
+			return fmt.Errorf("UploadNodeSpread: len(counts) = %d is not a multiple of n = %d", len(counts), n)
+		}
+		classes = len(counts) / n
+	}
+	var zp *C.uint8_t
+	var cp *C.int32_t
+	if n > 0 {
+		zp = (*C.uint8_t)(unsafe.Pointer(&zone[0]))
+	}
+	if len(counts) > 0 {
+		cp = (*C.int32_t)(unsafe.Pointer(&counts[0]))
+	}
+	return e.rc(C.bs_upload_node_spread(e.h, C.uint32_t(n), C.uint32_t(nZones), zp, C.uint32_t(classes), cp))
+}
+
+// UploadPodSpread: per pod its row of the count table (BS_SPREAD_NONE for a pod without selectors).  UploadPods
+// drops it.
+func (e *Engine) UploadPodSpread(spreadClass []uint32) error {
+	if len(spreadClass) == 0 {
+		return e.rc(C.bs_upload_pod_spread(e.h, 0, nil))
+	}
+	return e.rc(C.bs_upload_pod_spread(e.h, C.uint32_t(len(spreadClass)),
+		(*C.uint32_t)(unsafe.Pointer(&spreadClass[0]))))
+}
+
 // UploadNodeNonZero / UploadPodNonZero: the non-zero request columns, nz[2][n] (cpu millicores, then memory bytes):
 // per pod the sum over its containers of GetNonzeroRequestForResource(Requests), per node NodeInfo.NonZeroRequest().
 // UploadNodes / UpdateNodes drop the node column and UploadPods the pod column: upload them again before Evaluate.
