@@ -34,6 +34,14 @@ ZONE_NONE = 0xff          # BS_ZONE_NONE: zone of a node without a zone key
 SPREAD_ZONE_MAX = 64      # BS_SPREAD_ZONE_MAX: zones of one node side
 SPREAD_COUNT_MAX = 1 << 24   # BS_SPREAD_COUNT_MAX: largest selector count
 SPREAD_TABLE_MAX_BYTES = 1 << 30   # BS_SPREAD_TABLE_MAX_BYTES: cap of the class x node count table
+IPA_NONE = 0xffffffff     # BS_IPA_NONE: class of a pod or bound pod without entries
+TOPO_NONE = 0xffffffff    # BS_TOPO_NONE: topo value of a node without the key
+IPA_KEY_MAX = 64          # BS_IPA_KEY_MAX: topology keys of one node side
+IPA_BOUND_MAX = 1 << 24   # BS_IPA_BOUND_MAX: bound pods of one node side
+IPA_CLASS_MAX = 64        # BS_IPA_CLASS_MAX: entries of one class
+IPA_OWN_MAX = 1 << 16     # BS_IPA_OWN_MAX: largest |own| of one entry
+IPA_TERM_MAX_BYTES = 1 << 30    # BS_IPA_TERM_MAX_BYTES: cap of the (term, value) M / S tables
+IPA_TABLE_MAX_BYTES = 1 << 30   # BS_IPA_TABLE_MAX_BYTES: cap of the pod class x node raw table
 # core.PreemptRemovePod verdicts (bs_remove_code) and the bound-pod flag
 REMOVE_ALLOW, REMOVE_OFFLINE_ONLINE, REMOVE_NOT_FOUND, REMOVE_LOCKED, REMOVE_SAME_GROUP = range(5)
 BOUND_GROUP_LOCKED = 0x01
@@ -89,6 +97,21 @@ class BoundTableC(C.Structure):
     _fields_ = [("n_pods", C.c_uint32), ("n_lanes", C.c_uint32), ("node", C.c_void_p), ("req", C.c_void_p),
                 ("req_present", C.c_void_p), ("gid", C.c_void_p), ("priority", C.c_void_p), ("start_ns", C.c_void_p),
                 ("flags", C.c_void_p)]
+
+
+class InterpodClassesC(C.Structure):
+    _fields_ = [("n_classes", C.c_uint32), ("class_offset", C.c_void_p), ("term", C.c_void_p), ("own", C.c_void_p),
+                ("match", C.c_void_p)]
+
+
+class InterpodNodesC(C.Structure):
+    _fields_ = [("n_nodes", C.c_uint32), ("n_keys", C.c_uint32), ("n_values", C.c_void_p), ("topo", C.c_void_p),
+                ("n_terms", C.c_uint32), ("term_key", C.c_void_p), ("n_bound", C.c_uint32), ("bound_node", C.c_void_p),
+                ("bound_class", C.c_void_p), ("classes", InterpodClassesC)]
+
+
+class InterpodPodsC(C.Structure):
+    _fields_ = [("n_pods", C.c_uint32), ("pod_class", C.c_void_p), ("classes", InterpodClassesC)]
 
 
 class PreemptResultC(C.Structure):
@@ -180,6 +203,9 @@ SYMBOLS = {
     "bs_set_spread_weight": (C.c_int, [C.c_void_p, C.c_uint32]),
     "bs_upload_node_spread": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p]),
     "bs_upload_pod_spread": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p]),
+    "bs_set_interpod_weight": (C.c_int, [C.c_void_p, C.c_uint32]),
+    "bs_upload_node_interpod": (C.c_int, [C.c_void_p, _p(InterpodNodesC)]),
+    "bs_upload_pod_interpod": (C.c_int, [C.c_void_p, _p(InterpodPodsC)]),
     "bs_peer_init": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32]),
     "bs_peer_handle": (C.c_int, [C.c_void_p, C.c_void_p]),
     "bs_peer_attach": (C.c_int, [C.c_void_p, C.c_void_p]),

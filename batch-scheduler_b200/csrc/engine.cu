@@ -436,6 +436,19 @@ struct bs_engine {
   bool have_spread_node = false, have_spread_pod = false;
   uint32_t spread_classes = 0;
   int64_t spread_class_max = -1;
+  // InterPodAffinity (bs_set_interpod_weight; 0 = off): the node side (topology values [keys][N], each term's key and
+  // first (term, value) slot, the bound pods and their class table; dropped with the node table) and the pod side (each
+  // pod's class [P] and the class table; dropped with the pod table).  d_ipa_ms (M and S per slot) and the pod class x
+  // node raw table d_ipa_raw are built on the device when ipa_dirty (ipa_mass_dirty: M and S too).  ipa_term_max: the
+  // largest term a pod class names (-1 none), checked against ipa_terms at evaluation.
+  uint32_t w_ipa = 0;
+  DevBuf d_ipa_topo, d_ipa_term_key, d_ipa_term_off, d_ipa_bound_node, d_ipa_bound_class;
+  DevBuf d_ipa_boff, d_ipa_bterm, d_ipa_bown, d_ipa_bmatch, d_ipa_ms;
+  DevBuf d_ipa_class, d_ipa_poff, d_ipa_pterm, d_ipa_pown, d_ipa_pmatch, d_ipa_raw;
+  bool have_ipa_node = false, have_ipa_pod = false, ipa_dirty = true, ipa_mass_dirty = true;
+  uint32_t ipa_terms = 0, ipa_bound = 0, ipa_bclasses = 0, ipa_pclasses = 0;
+  uint64_t ipa_slots = 0;
+  int64_t ipa_term_max = -1;
   // sort scratch: views into one arena
   View d_gk0, d_gk1, d_pk0, d_pk1, d_idx_a, d_idx_b, d_ghist, d_group_rank, d_tilecnt, d_sort_barrier;
   uint32_t sort_max_grid = 1;
@@ -1150,6 +1163,32 @@ int locality_prepass(bs_engine* e) {
   return BS_OK;
 }
 
+// The IPA pre-pass on the main stream: M and S over the bound pods (after a node-side change), then the pod class x
+// node raw table.  Only after either side changed, and only while the weight is non-zero.
+int interpod_prepass(bs_engine* e) {
+  if (!e->ipa_dirty || !e->w_ipa) return BS_OK;
+  const uint32_t C = e->ipa_pclasses, Npad = e->Npad;
+  if (e->ipa_mass_dirty) {
+    CK(e->d_ipa_ms.ensure((size_t)std::max<uint64_t>(e->ipa_slots, 1) * 16));
+    CK(cudaMemsetAsync(e->d_ipa_ms.p, 0, (size_t)e->ipa_slots * 16, e->s));
+  }
+  if (C && Npad) {
+    CK(e->d_ipa_raw.ensure((size_t)C * Npad * 8));
+    const InterpodClasses bound{e->d_ipa_boff.as<uint32_t>(), e->d_ipa_bterm.as<uint32_t>(), e->d_ipa_bown.as<int32_t>(),
+                                e->d_ipa_bmatch.as<uint8_t>(), e->ipa_bclasses};
+    const InterpodClasses pods{e->d_ipa_poff.as<uint32_t>(), e->d_ipa_pterm.as<uint32_t>(), e->d_ipa_pown.as<int32_t>(),
+                               e->d_ipa_pmatch.as<uint8_t>(), C};
+    CK(launch_interpod_prepass(e->ipa_mass_dirty, e->d_ipa_topo.as<uint32_t>(), e->d_ipa_term_key.as<uint32_t>(),
+                               e->d_ipa_term_off.as<uint32_t>(), e->d_ipa_bound_node.as<uint32_t>(),
+                               e->d_ipa_bound_class.as<uint32_t>(), e->ipa_bound, bound, pods,
+                               e->d_ipa_ms.as<int64_t>(), e->d_ipa_raw.as<int64_t>(), e->N, Npad, e->s));
+    e->launches += (e->ipa_mass_dirty && e->ipa_bound) ? 2 : 1;
+    e->ipa_mass_dirty = false;
+  }
+  e->ipa_dirty = false;
+  return BS_OK;
+}
+
 int evaluate_async_locked(bs_engine* e) {
   int rc;
   if (!e->have_nodes || !e->have_pods || !e->have_groups)
@@ -1168,6 +1207,15 @@ int evaluate_async_locked(bs_engine* e) {
       return fail(e, BS_E_STATE, "bs_evaluate: a non-zero SelectorSpread weight needs the node and pod spread columns");
     if (e->spread_class_max >= (int64_t)e->spread_classes)
       return fail(e, BS_E_INDEX, "bs_evaluate: a pod's spread class is outside the uploaded count table");
+  }
+  if ((e->out_flags & BS_OUT_PRIORITY) && e->w_ipa) {
+    if (!(e->have_ipa_node && e->have_ipa_pod))
+      return fail(e, BS_E_STATE, "bs_evaluate: a non-zero InterPodAffinity weight needs the node and pod inter-pod sides");
+    if (e->ipa_term_max >= (int64_t)e->ipa_terms)
+      return fail(e, BS_E_INDEX, "bs_evaluate: a pod class's term is outside the node side's term dictionary");
+    // the pod side outlives node uploads: its class x node table is checked against the node table of now
+    if ((uint64_t)e->ipa_pclasses * e->Npad * 8 > BS_IPA_TABLE_MAX_BYTES)
+      return fail(e, BS_E_INVAL, "bs_evaluate: pod n_classes x padded nodes x 8 bytes exceeds BS_IPA_TABLE_MAX_BYTES");
   }
   if (e->peer_broken)
     return fail(e, BS_E_PEER, "peer exchange is broken (a rank did not arrive): bs_peer_detach on every rank, then init/attach again");
@@ -1432,7 +1480,7 @@ int evaluate_async_locked(bs_engine* e) {
     pa.node_req_present = e->d_rpres.as<uint32_t>();
     pa.ratio = e->ratio;
     const uint32_t grid = cdiv(P, PRIO_PODS_PER_CTA);
-    PrioritySpreadArgs la;
+    PriorityIpaArgs la;
     static_cast<PriorityRatioArgs&>(la) = pa;
     la.prefer_taints = e->d_prefer_taints.as<uint64_t>();
     la.pref_weights = e->d_pref_weights.as<int32_t>();
@@ -1456,7 +1504,13 @@ int evaluate_async_locked(bs_engine* e) {
       la.spread_class = e->d_spread_class.as<uint32_t>();
       la.w_spread = e->w_spread;
     }
-    CK(launch_priority(L, grid, ratio, pref, e->w_img || e->w_avoid, e->w_spread != 0, la, e->s));
+    if (e->w_ipa) {   // (the pre-pass runs on the same stream, ahead of the kernel)
+      if ((rc = interpod_prepass(e))) return rc;
+      la.ipa_raw = e->d_ipa_raw.as<int64_t>();
+      la.ipa_class = e->d_ipa_class.as<uint32_t>();
+      la.w_ipa = e->w_ipa;
+    }
+    CK(launch_priority(L, grid, ratio, pref, e->w_img || e->w_avoid, e->w_spread != 0, e->w_ipa != 0, la, e->s));
     e->launches += 1;
   }
   if (e->peer_attached) {
@@ -1680,6 +1734,7 @@ int bs_upload_nodes(bs_engine* e, const bs_node_table* t) {
   e->have_pref_node = false;   // and so do the PreferNoSchedule masks and the preferred-affinity table
   e->have_img_node = e->have_avoid_node = false;   // and the image rows and preferAvoidPods masks
   e->have_spread_node = false;   // and the zones and selector counts (counts change when pods bind)
+  e->have_ipa_node = false;   // and the topology values and bound pods of InterPodAffinity
   if (t->n_lanes != e->L) return fail(e, BS_E_INVAL, "bs_upload_nodes: n_lanes differs from the engine's");
   const uint32_t N = t->n_nodes, L = e->L;
   const auto cols = node_cols(e, t);
@@ -1721,6 +1776,7 @@ int bs_update_nodes(bs_engine* e, const uint32_t* idx, const bs_node_table* t) {
   e->have_pref_node = false;   // ... and so do their taints and labels: the node preference side is uploaded again
   e->have_img_node = e->have_avoid_node = false;   // ... and their images and annotations: so is the locality side
   e->have_spread_node = false;   // ... and the pods on them and their zone labels: so is the spread side
+  e->have_ipa_node = false;   // ... and the inter-pod side, for the same reasons
   if (t->n_lanes != e->L) return fail(e, BS_E_INVAL, "bs_update_nodes: n_lanes differs from the engine's");
   const uint32_t n = t->n_nodes, L = e->L;
   if (!n) return BS_OK;
@@ -1855,6 +1911,7 @@ int bs_upload_pods(bs_engine* e, const bs_pod_table* t) {
   e->have_pref_pod = false;   // and so does the pod preference side
   e->have_img_pod = e->have_avoid_pod = false;   // and the pod locality side
   e->have_spread_pod = false;   // and the pod spread side
+  e->have_ipa_pod = false;   // and the pod inter-pod side
   if (t->n_lanes != e->L) return fail(e, BS_E_INVAL, "bs_upload_pods: n_lanes differs from the engine's");
   const uint32_t P = t->n_pods, L = e->L;
   if (P && (!t->req || !t->req_present || !t->gid || !t->sel_mask || !t->tol_mask || !t->priority ||
@@ -2622,6 +2679,9 @@ int bs_replay_priority(bs_engine* e, const uint32_t* queue, uint32_t n_queue, bs
   if (e->w_spread)   // its maxima and zone sums would follow the live fit set and the live counts, likewise
     return fail(e, BS_E_INVAL, "bs_replay_priority: SelectorSpread is not supported in the walk; "
                                "set bs_set_spread_weight to 0");
+  if (e->w_ipa)   // its maxima would follow the live fit set and the live placements, likewise
+    return fail(e, BS_E_INVAL, "bs_replay_priority: InterPodAffinity is not supported in the walk; "
+                               "set bs_set_interpod_weight to 0");
   return replay_walk(e, "bs_replay_priority", queue, n_queue, out, true, node_nonzero_after);
 }
 
@@ -3322,6 +3382,153 @@ int bs_upload_pod_spread(bs_engine* e, uint32_t n_pods, const uint32_t* spread_c
   CK(cudaStreamSynchronize(e->s));
   e->spread_class_max = mx;
   e->have_spread_pod = true;
+  return BS_OK;
+}
+
+int bs_set_interpod_weight(bs_engine* e, uint32_t inter_pod_affinity) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  e->w_ipa = inter_pod_affinity;
+  return BS_OK;
+}
+
+namespace {
+
+// A class table of bs_interpod_classes: the offsets ascending from 0 and at most BS_IPA_CLASS_MAX apart, own and match
+// in range, the terms distinct within a class and (n_terms != UINT32_MAX) below n_terms.  term_max: the largest term.
+int interpod_classes_check(const bs_interpod_classes& c, uint32_t n_terms, int64_t& term_max, const char*& why) {
+  term_max = -1;
+  if (!c.n_classes) return BS_OK;
+  if (!c.class_offset) return why = "null class_offset", BS_E_INVAL;
+  if (c.class_offset[0] != 0) return why = "class_offset[0] is not 0", BS_E_INVAL;
+  for (uint32_t k = 0; k < c.n_classes; ++k)
+    if (c.class_offset[k + 1] < c.class_offset[k] || c.class_offset[k + 1] - c.class_offset[k] > BS_IPA_CLASS_MAX)
+      return why = "class_offset is not ascending, or a class lists more than BS_IPA_CLASS_MAX entries", BS_E_INVAL;
+  const uint32_t nnz = c.class_offset[c.n_classes];
+  if (nnz && !(c.term && c.own && c.match)) return why = "null term, own or match", BS_E_INVAL;
+  for (uint32_t k = 0; k < nnz; ++k) {
+    if (c.match[k] > 1) return why = "a match is not 0 or 1", BS_E_RANGE;
+    if (c.own[k] < -BS_IPA_OWN_MAX || c.own[k] > BS_IPA_OWN_MAX) return why = "an own is outside [-2^16, 2^16]", BS_E_RANGE;
+    if (n_terms != UINT32_MAX && c.term[k] >= n_terms) return why = "a term id is >= n_terms", BS_E_INDEX;
+    term_max = std::max(term_max, (int64_t)c.term[k]);
+  }
+  for (uint32_t k = 0; k < c.n_classes; ++k) {
+    const uint32_t o0 = c.class_offset[k], o1 = c.class_offset[k + 1];
+    for (uint32_t x = o0; x < o1; ++x)
+      for (uint32_t y = x + 1; y < o1; ++y)
+        if (c.term[x] == c.term[y]) return why = "a class lists one term twice", BS_E_INVAL;
+  }
+  return BS_OK;
+}
+
+// Device copies of a checked class table.
+int interpod_classes_upload(bs_engine* e, const bs_interpod_classes& c, DevBuf& off, DevBuf& term, DevBuf& own,
+                            DevBuf& match) {
+  const uint32_t nnz = c.n_classes ? c.class_offset[c.n_classes] : 0;
+  CK(off.ensure((size_t)(c.n_classes + 1) * 4));
+  CK(term.ensure((size_t)std::max(nnz, 1u) * 4));
+  CK(own.ensure((size_t)std::max(nnz, 1u) * 4));
+  CK(match.ensure(std::max(nnz, 1u)));
+  if (c.n_classes) CK(cudaMemcpyAsync(off.p, c.class_offset, (size_t)(c.n_classes + 1) * 4, cudaMemcpyHostToDevice, e->s));
+  else CK(cudaMemsetAsync(off.p, 0, 4, e->s));
+  if (nnz) {
+    CK(cudaMemcpyAsync(term.p, c.term, (size_t)nnz * 4, cudaMemcpyHostToDevice, e->s));
+    CK(cudaMemcpyAsync(own.p, c.own, (size_t)nnz * 4, cudaMemcpyHostToDevice, e->s));
+    CK(cudaMemcpyAsync(match.p, c.match, nnz, cudaMemcpyHostToDevice, e->s));
+  }
+  return BS_OK;
+}
+
+}  // namespace
+
+int bs_upload_node_interpod(bs_engine* e, const bs_interpod_nodes* t) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  const char* who = "bs_upload_node_interpod";
+  auto bad = [&](int rc, const char* why) { return fail(e, rc, (std::string(who) + ": " + why).c_str()); };
+  e->have_ipa_node = false;
+  e->ipa_dirty = e->ipa_mass_dirty = true;
+  if (!t) return bad(BS_E_INVAL, "null table");
+  if (!e->have_nodes) return bad(BS_E_STATE, "upload nodes first");
+  const uint32_t N = t->n_nodes, K = t->n_keys, T = t->n_terms, V = t->n_bound;
+  if (N != e->N) return bad(BS_E_INVAL, "n_nodes differs from the node table's");
+  if (K > BS_IPA_KEY_MAX) return bad(BS_E_INVAL, "n_keys exceeds BS_IPA_KEY_MAX");
+  if (V > BS_IPA_BOUND_MAX) return bad(BS_E_INVAL, "n_bound exceeds BS_IPA_BOUND_MAX");
+  if ((K && !t->n_values) || (K && N && !t->topo) || (T && !t->term_key) || (V && !(t->bound_node && t->bound_class)))
+    return bad(BS_E_INVAL, "null column");
+  for (size_t k = 0; k < (size_t)K * N; ++k)
+    if (t->topo[k] != BS_TOPO_NONE && t->topo[k] >= t->n_values[k / N]) return bad(BS_E_INDEX, "a topo value is >= n_values");
+  std::vector<uint32_t> off(T);
+  uint64_t slots = 0;
+  for (uint32_t k = 0; k < T; ++k) {
+    if (t->term_key[k] >= K) return bad(BS_E_INDEX, "a term_key is >= n_keys");
+    off[k] = (uint32_t)std::min<uint64_t>(slots, UINT32_MAX);
+    slots += t->n_values[t->term_key[k]];
+    if (slots * 16 > BS_IPA_TERM_MAX_BYTES) return bad(BS_E_INVAL, "the term tables exceed BS_IPA_TERM_MAX_BYTES");
+  }
+  for (uint32_t k = 0; k < V; ++k) {
+    if (t->bound_node[k] >= N) return bad(BS_E_INDEX, "a bound_node is >= n_nodes");
+    if (t->bound_class[k] != BS_IPA_NONE && t->bound_class[k] >= t->classes.n_classes)
+      return bad(BS_E_INDEX, "a bound_class is >= n_classes");
+  }
+  int64_t tmax;
+  const char* why = nullptr;
+  if (int rc = interpod_classes_check(t->classes, T, tmax, why)) return bad(rc, why);
+  BS_DEVICE_GUARD(e);
+  CK(e->d_ipa_topo.ensure((size_t)std::max<uint64_t>((uint64_t)K * N, 1) * 4));
+  CK(e->d_ipa_term_key.ensure((size_t)std::max(T, 1u) * 4));
+  CK(e->d_ipa_term_off.ensure((size_t)std::max(T, 1u) * 4));
+  CK(e->d_ipa_bound_node.ensure((size_t)std::max(V, 1u) * 4));
+  CK(e->d_ipa_bound_class.ensure((size_t)std::max(V, 1u) * 4));
+  if (K && N) CK(cudaMemcpyAsync(e->d_ipa_topo.p, t->topo, (size_t)K * N * 4, cudaMemcpyHostToDevice, e->s));
+  if (T) {
+    CK(cudaMemcpyAsync(e->d_ipa_term_key.p, t->term_key, (size_t)T * 4, cudaMemcpyHostToDevice, e->s));
+    CK(cudaMemcpyAsync(e->d_ipa_term_off.p, off.data(), (size_t)T * 4, cudaMemcpyHostToDevice, e->s));
+  }
+  if (V) {
+    CK(cudaMemcpyAsync(e->d_ipa_bound_node.p, t->bound_node, (size_t)V * 4, cudaMemcpyHostToDevice, e->s));
+    CK(cudaMemcpyAsync(e->d_ipa_bound_class.p, t->bound_class, (size_t)V * 4, cudaMemcpyHostToDevice, e->s));
+  }
+  if (int rc = interpod_classes_upload(e, t->classes, e->d_ipa_boff, e->d_ipa_bterm, e->d_ipa_bown, e->d_ipa_bmatch))
+    return rc;
+  CK(cudaStreamSynchronize(e->s));   // the caller's columns may go once the call returns
+  e->ipa_terms = T;
+  e->ipa_slots = slots;
+  e->ipa_bound = V;
+  e->ipa_bclasses = t->classes.n_classes;
+  e->have_ipa_node = true;
+  return BS_OK;
+}
+
+int bs_upload_pod_interpod(bs_engine* e, const bs_interpod_pods* t) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  const char* who = "bs_upload_pod_interpod";
+  auto bad = [&](int rc, const char* why) { return fail(e, rc, (std::string(who) + ": " + why).c_str()); };
+  e->have_ipa_pod = false;
+  e->ipa_dirty = true;
+  if (!t) return bad(BS_E_INVAL, "null table");
+  if (!e->have_pods) return bad(BS_E_STATE, "upload pods first");
+  const uint32_t P = t->n_pods;
+  if (P != e->P) return bad(BS_E_INVAL, "n_pods differs from the pod table's");
+  if (P && !t->pod_class) return bad(BS_E_INVAL, "null pod_class");
+  if ((uint64_t)t->classes.n_classes * e->Npad * 8 > BS_IPA_TABLE_MAX_BYTES)
+    return bad(BS_E_INVAL, "n_classes x padded nodes x 8 bytes exceeds BS_IPA_TABLE_MAX_BYTES");
+  for (uint32_t p = 0; p < P; ++p)
+    if (t->pod_class[p] != BS_IPA_NONE && t->pod_class[p] >= t->classes.n_classes)
+      return bad(BS_E_INDEX, "a pod_class is >= n_classes");
+  int64_t tmax;
+  const char* why = nullptr;
+  if (int rc = interpod_classes_check(t->classes, UINT32_MAX, tmax, why)) return bad(rc, why);
+  BS_DEVICE_GUARD(e);
+  CK(e->d_ipa_class.ensure((size_t)std::max(P, 1u) * 4));
+  if (P) CK(cudaMemcpyAsync(e->d_ipa_class.p, t->pod_class, (size_t)P * 4, cudaMemcpyHostToDevice, e->s));
+  if (int rc = interpod_classes_upload(e, t->classes, e->d_ipa_poff, e->d_ipa_pterm, e->d_ipa_pown, e->d_ipa_pmatch))
+    return rc;
+  CK(cudaStreamSynchronize(e->s));
+  e->ipa_pclasses = t->classes.n_classes;
+  e->ipa_term_max = tmax;
+  e->have_ipa_pod = true;
   return BS_OK;
 }
 

@@ -12,6 +12,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <set>
+#include <tuple>
 
 namespace bsched {
 
@@ -978,6 +979,8 @@ Status BatchSchedulingPlugin::BeginRound(const std::vector<const NodeInfo*>& sna
     if (!nst.ok()) return nst;
     nst = UploadSpread();
     if (!nst.ok()) return nst;
+    nst = UploadInterPodAffinity();
+    if (!nst.ok()) return nst;
   }
   {
     Status bst = UploadBound();   // after the groups: the bound rows' group indices refer to this table
@@ -1649,6 +1652,209 @@ Status BatchSchedulingPlugin::UploadSpread() {
   return rc ? fail(rc) : Status{};
 }
 
+void BatchSchedulingPlugin::SetInterPodAffinityWeight(uint32_t inter_pod_affinity) {
+  std::lock_guard<std::mutex> lk(mu_);
+  interpod_weight_ = inter_pod_affinity;
+}
+
+Status BatchSchedulingPlugin::SetHardPodAffinityWeight(int32_t hard_pod_affinity_weight) {
+  if (hard_pod_affinity_weight < 0 || hard_pod_affinity_weight > 100)
+    return Status{BS_CODE_ERROR, "SetHardPodAffinityWeight: the weight is outside 0..100"};
+  std::lock_guard<std::mutex> lk(mu_);
+  hard_pod_affinity_weight_ = hard_pod_affinity_weight;
+  return Status{};
+}
+
+Status BatchSchedulingPlugin::PackInterPodAffinity(const std::vector<const NodeInfo*>& snapshot,
+                                                   const std::vector<const Pod*>& pending, int32_t hard_weight,
+                                                   PackedInterPodAffinity* out) {
+  if (!out) return Status{BS_CODE_ERROR, "PackInterPodAffinity: null output"};
+  PackedInterPodAffinity& pk = *out;
+  pk = PackedInterPodAffinity();
+  const size_t N = snapshot.size(), P = pending.size();
+  // the dictionaries: keys and terms in order of first appearance; a term keeps its converted selector (nullopt: nil)
+  // and its resolved namespaces for the match tests
+  struct TermInfo {
+    bool has_sel;
+    SpreadSel sel;
+    std::vector<std::string> ns;   // sorted
+  };
+  std::unordered_map<std::string, uint32_t> key_of, term_of;
+  std::vector<TermInfo> terms;
+  // the (term, signed weight) pairs a pod's processing reads; bad = a term's selector fails to convert
+  auto own_of = [&](const Pod& pod, bool bound_side, std::map<uint32_t, int64_t>* own, bool* bad) -> Status {
+    auto add = [&](const PodAffinityTerm& t, int64_t w) -> Status {
+      SpreadSel sel;
+      if (t.has_selector && !sel_from_label_selector(t.selector, &sel)) {
+        *bad = true;
+        return Status{};
+      }
+      if (t.topology_key.empty()) return Status{};   // NodesHaveSameTopologyKey never holds
+      std::vector<std::string> ns = t.namespaces.empty() ? std::vector<std::string>{pod.ns} : t.namespaces;
+      std::sort(ns.begin(), ns.end());
+      ns.erase(std::unique(ns.begin(), ns.end()), ns.end());
+      std::string sig;
+      for (auto& n : ns) { sig += n; sig += '\x1d'; }
+      sig += '\x1c';
+      sig += t.has_selector ? "sel:" + sel_text(sel) : std::string("nil");
+      sig += '\x1c';
+      sig += t.topology_key;
+      auto kit = key_of.find(t.topology_key);
+      if (kit == key_of.end()) {
+        if (pk.keys.size() == BS_IPA_KEY_MAX)
+          return Status{BS_CODE_ERROR, "PackInterPodAffinity: more than BS_IPA_KEY_MAX topology keys"};
+        kit = key_of.emplace(t.topology_key, (uint32_t)pk.keys.size()).first;
+        pk.keys.push_back(t.topology_key);
+      }
+      auto it = term_of.find(sig);
+      if (it == term_of.end()) {
+        it = term_of.emplace(sig, (uint32_t)terms.size()).first;
+        terms.push_back(TermInfo{t.has_selector, std::move(sel), std::move(ns)});
+        pk.term_signatures.push_back(sig);
+        pk.term_key.push_back(kit->second);
+      }
+      (*own)[it->second] += w;
+      return Status{};
+    };
+    Status st;
+    if (bound_side && hard_weight > 0)
+      for (const PodAffinityTerm& t : pod.required_pod_affinity)
+        if (!(st = add(t, hard_weight)).ok()) return st;
+    for (const WeightedPodAffinityTerm& t : pod.preferred_pod_affinity)
+      if (!(st = add(t.term, t.weight)).ok()) return st;
+    for (const WeightedPodAffinityTerm& t : pod.preferred_pod_anti_affinity)
+      if (!(st = add(t.term, -(int64_t)t.weight)).ok()) return st;
+    return Status{};
+  };
+  std::vector<const Pod*> bound;
+  std::vector<std::map<uint32_t, int64_t>> bown, pown(P);
+  bool invalid_bound = false;
+  Status st;
+  for (size_t i = 0; i < N; ++i) {
+    if (!snapshot[i] || !snapshot[i]->node) continue;
+    for (const Pod* bp : snapshot[i]->pods) {
+      if (!bp) continue;
+      if (bound.size() == BS_IPA_BOUND_MAX)
+        return Status{BS_CODE_ERROR, "PackInterPodAffinity: more than BS_IPA_BOUND_MAX bound pods"};
+      bound.push_back(bp);
+      pk.bound_node.push_back((uint32_t)i);
+      bown.emplace_back();
+      bool bad = false;
+      if (!(st = own_of(*bp, true, &bown.back(), &bad)).ok()) return st;
+      invalid_bound = invalid_bound || bad;
+    }
+  }
+  std::vector<uint8_t> pbad(P, 0);
+  for (size_t p = 0; p < P; ++p) {
+    if (!pending[p]) continue;
+    bool bad = false;
+    if (!(st = own_of(*pending[p], false, &pown[p], &bad)).ok()) return st;
+    pbad[p] = bad && !bound.empty();
+  }
+  // the terms each side owns: a pod's match entries are the other side's terms it matches
+  std::vector<uint32_t> b_terms, p_terms;
+  {
+    std::vector<uint8_t> in_b(terms.size(), 0), in_p(terms.size(), 0);
+    for (auto& o : bown) for (auto& kv : o) in_b[kv.first] = 1;
+    for (auto& o : pown) for (auto& kv : o) in_p[kv.first] = 1;
+    for (uint32_t t = 0; t < terms.size(); ++t) {
+      if (in_b[t]) b_terms.push_back(t);
+      if (in_p[t]) p_terms.push_back(t);
+    }
+  }
+  auto matches = [&](const Pod& pod, uint32_t t) {
+    const TermInfo& ti = terms[t];
+    return ti.has_sel && std::binary_search(ti.ns.begin(), ti.ns.end(), pod.ns) && spread_sel_matches(ti.sel, pod.labels);
+  };
+  // a pod's sorted entries as a class, in order of first appearance; no entries: BS_IPA_NONE
+  auto classify = [&](const Pod& pod, const std::map<uint32_t, int64_t>& own, const std::vector<uint32_t>& other,
+                      std::map<std::vector<std::tuple<uint32_t, int32_t, uint8_t>>, uint32_t>& class_of,
+                      PackedInterPodAffinity::Classes& cl, uint32_t* out_class) -> Status {
+    std::map<uint32_t, std::pair<int64_t, uint8_t>> ent;
+    for (auto& kv : own) ent[kv.first].first = kv.second;
+    for (uint32_t t : other)
+      if (matches(pod, t)) ent[t].second = 1;
+    std::vector<std::tuple<uint32_t, int32_t, uint8_t>> key;
+    for (auto& kv : ent) {
+      if (!kv.second.first && !kv.second.second) continue;
+      if (kv.second.first < -BS_IPA_OWN_MAX || kv.second.first > BS_IPA_OWN_MAX)
+        return Status{BS_CODE_ERROR, "PackInterPodAffinity: a pod's summed weight on one term exceeds BS_IPA_OWN_MAX"};
+      key.emplace_back(kv.first, (int32_t)kv.second.first, kv.second.second);
+    }
+    if (key.size() > BS_IPA_CLASS_MAX)
+      return Status{BS_CODE_ERROR, "PackInterPodAffinity: a pod lists more than BS_IPA_CLASS_MAX terms"};
+    *out_class = BS_IPA_NONE;
+    if (key.empty()) return Status{};
+    auto it = class_of.find(key);
+    if (it == class_of.end()) {
+      it = class_of.emplace(key, cl.n_classes()).first;
+      for (auto& e : key) {
+        cl.term.push_back(std::get<0>(e));
+        cl.own.push_back(std::get<1>(e));
+        cl.match.push_back(std::get<2>(e));
+      }
+      cl.offset.push_back((uint32_t)cl.term.size());
+    }
+    *out_class = it->second;
+    return Status{};
+  };
+  std::map<std::vector<std::tuple<uint32_t, int32_t, uint8_t>>, uint32_t> bclass_of, pclass_of;
+  pk.bound_class.assign(bound.size(), BS_IPA_NONE);
+  for (size_t k = 0; k < bound.size(); ++k)
+    if (!(st = classify(*bound[k], bown[k], p_terms, bclass_of, pk.bound_classes, &pk.bound_class[k])).ok()) return st;
+  pk.pod_class.assign(P, BS_IPA_NONE);
+  for (size_t p = 0; p < P; ++p)
+    if (pending[p] && !invalid_bound && !pbad[p])
+      if (!(st = classify(*pending[p], pown[p], b_terms, pclass_of, pk.pod_classes, &pk.pod_class[p])).ok()) return st;
+  // each key's values over the nodes, in order of first appearance
+  const size_t K = pk.keys.size();
+  pk.values.assign(K, {});
+  pk.n_values.assign(K, 0);
+  pk.topo.assign(K * N, BS_TOPO_NONE);
+  for (size_t k = 0; k < K; ++k) {
+    std::unordered_map<std::string, uint32_t> value_of;
+    for (size_t i = 0; i < N; ++i) {
+      if (!snapshot[i] || !snapshot[i]->node) continue;
+      const auto& labels = snapshot[i]->node->labels;
+      const auto l = labels.find(pk.keys[k]);
+      if (l == labels.end()) continue;
+      auto it = value_of.find(l->second);
+      if (it == value_of.end()) {
+        it = value_of.emplace(l->second, (uint32_t)pk.values[k].size()).first;
+        pk.values[k].push_back(l->second);
+      }
+      pk.topo[k * N + i] = it->second;
+    }
+    pk.n_values[k] = (uint32_t)pk.values[k].size();
+  }
+  return Status{};
+}
+
+Status BatchSchedulingPlugin::UploadInterPodAffinity() {
+  if (!priority_k_) return Status{};
+  auto fail = [&](int rc) {
+    return Status{BS_CODE_ERROR, std::string("bsched: ") + bs_strerror(rc) + " (" + bs_last_error(eng_) + ")"};
+  };
+  int rc = bs_set_interpod_weight(eng_, interpod_weight_);
+  if (rc) return fail(rc);
+  if (!interpod_weight_) return Status{};
+  PackedInterPodAffinity pk;
+  Status st = PackInterPodAffinity(snapshot_, pending_, hard_pod_affinity_weight_, &pk);
+  if (!st.ok()) return st;
+  auto classes = [](const PackedInterPodAffinity::Classes& c) {
+    return bs_interpod_classes{c.n_classes(), c.offset.data(), c.term.data(), c.own.data(), c.match.data()};
+  };
+  bs_interpod_nodes nt{(uint32_t)snapshot_.size(), (uint32_t)pk.keys.size(), pk.n_values.data(), pk.topo.data(),
+                       (uint32_t)pk.term_key.size(), pk.term_key.data(), (uint32_t)pk.bound_node.size(),
+                       pk.bound_node.data(), pk.bound_class.data(), classes(pk.bound_classes)};
+  rc = bs_upload_node_interpod(eng_, &nt);
+  if (!rc) {
+    bs_interpod_pods pt{(uint32_t)pending_.size(), pk.pod_class.data(), classes(pk.pod_classes)};
+    rc = bs_upload_pod_interpod(eng_, &pt);
+  }
+  return rc ? fail(rc) : Status{};
+}
+
 std::vector<uint32_t> BatchSchedulingPlugin::ReasonCounts(const std::string& uid) const {
   const int32_t row = pod_row_.find(uid);
   const size_t R = 4 + packed_.lanes;
@@ -1687,6 +1893,8 @@ Status BatchSchedulingPlugin::UpdateRound(const std::vector<std::pair<uint32_t, 
     st = UploadLocality();
     if (!st.ok()) return st;
     st = UploadSpread();
+    if (!st.ok()) return st;
+    st = UploadInterPodAffinity();
     if (!st.ok()) return st;
   }
   return Reevaluate();
@@ -1743,6 +1951,8 @@ Status BatchSchedulingPlugin::UpdateNodes(const std::vector<std::pair<uint32_t, 
   st = UploadLocality();         // ... and the locality side (its dictionaries may change: both sides)
   if (!st.ok()) return st;
   st = UploadSpread();           // ... and the spread side (the changed NodeInfos' pods and zones: both sides)
+  if (!st.ok()) return st;
+  st = UploadInterPodAffinity();   // ... and the inter-pod side (the changed NodeInfos' pods and labels: both sides)
   if (!st.ok()) return st;
   // the round's decisions follow the new snapshot: same pods, same groups, same result vectors
   return evaluate ? Reevaluate() : Status{};
@@ -1975,6 +2185,9 @@ Status BatchSchedulingPlugin::ReplayQueue(std::vector<ReplayDecision>* out, Repl
   if (prio && spread_weight_)
     return Status{BS_CODE_ERROR, "ReplayQueue: kPriority does not support SelectorSpread yet "
                                  "(SetSelectorSpreadWeight(0) first)"};
+  if (prio && interpod_weight_)
+    return Status{BS_CODE_ERROR, "ReplayQueue: kPriority does not support InterPodAffinity yet "
+                                 "(SetInterPodAffinityWeight(0) first)"};
   const uint32_t P = packed_.n_pods;
   std::vector<uint8_t> pf(P), rd(P);
   std::vector<int32_t> nd(P);

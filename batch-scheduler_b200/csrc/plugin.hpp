@@ -60,6 +60,30 @@ struct PreferredSchedulingTerm {
   int32_t weight = 0;               // 1..100 upstream; a term of weight 0 is skipped
   NodeSelectorTerm preference;      // only match_expressions are read; an empty list matches nothing
 };
+// metav1.LabelSelectorRequirement / metav1.LabelSelector: the selectors of ReplicaSets and StatefulSets
+// (SelectorSpread) and of pod-affinity terms (InterPodAffinity).  An In / NotIn requirement without values, an Exists / DoesNotExist one with values, or another
+// operator fails LabelSelectorAsSelector.
+struct LabelSelectorRequirement {
+  std::string key, op /* In | NotIn | Exists | DoesNotExist */;
+  std::vector<std::string> values;
+};
+struct LabelSelector {
+  std::map<std::string, std::string> match_labels;
+  std::vector<LabelSelectorRequirement> match_expressions;
+};
+// v1.PodAffinityTerm (InterPodAffinity): has_selector = false is a nil selector, which matches no pod; an empty one
+// matches every pod.  An empty namespaces list means the namespace of the pod that defines the term.
+struct PodAffinityTerm {
+  LabelSelector selector;
+  bool has_selector = false;
+  std::vector<std::string> namespaces;
+  std::string topology_key;
+};
+// v1.WeightedPodAffinityTerm: one preferred pod-affinity or pod-anti-affinity term and its weight (1..100 upstream)
+struct WeightedPodAffinityTerm {
+  int32_t weight = 0;
+  PodAffinityTerm term;
+};
 struct Pod {
   std::string ns, name, uid;
   std::map<std::string, std::string> labels;
@@ -75,17 +99,10 @@ struct Pod {
   int64_t start_ns = 0;                 // Status.StartTime of a bound pod (preemption: MoreImportantPod)
   std::string controller_kind, controller_uid;   // metav1.GetControllerOf: the controlling owner ("" = none)
   bool terminating = false;             // DeletionTimestamp != nil (SelectorSpread does not count the pod)
-};
-// metav1.LabelSelectorRequirement / metav1.LabelSelector: the selectors of ReplicaSets and StatefulSets
-// (SelectorSpread).  An In / NotIn requirement without values, an Exists / DoesNotExist one with values, or another
-// operator fails LabelSelectorAsSelector.
-struct LabelSelectorRequirement {
-  std::string key, op /* In | NotIn | Exists | DoesNotExist */;
-  std::vector<std::string> values;
-};
-struct LabelSelector {
-  std::map<std::string, std::string> match_labels;
-  std::vector<LabelSelectorRequirement> match_expressions;
+  // Spec.Affinity.PodAffinity / PodAntiAffinity (InterPodAffinity): the required pod-affinity terms and the preferred
+  // pod-affinity and pod-anti-affinity terms; required anti-affinity is not read
+  std::vector<PodAffinityTerm> required_pod_affinity;
+  std::vector<WeightedPodAffinityTerm> preferred_pod_affinity, preferred_pod_anti_affinity;
 };
 // The objects whose selectors SelectorSpread spreads by: Services and ReplicationControllers select with a map,
 // ReplicaSets and StatefulSets with a LabelSelector.  has_selector = false is a nil selector, kept distinct from an
@@ -263,6 +280,29 @@ struct PackedSpread {
   std::vector<std::string> class_signatures;    // namespace and selector texts of each class
   std::vector<int32_t> counts;                  // [n_classes][n_nodes]
   uint32_t n_classes() const { return (uint32_t)class_signatures.size(); }
+};
+// The columns of the InterPodAffinity priority of one round (bs_upload_node_interpod, bs_upload_pod_interpod): the
+// topology keys and each key's values in order of first appearance; the term dictionary (term_signatures: the
+// resolved, sorted namespaces, the selector's canonical text and the key); the bound pods of NodeInfo::pods and their
+// classes; each pending pod's class.  A class is a sorted list of (term, own, match).
+struct PackedInterPodAffinity {
+  struct Classes {
+    std::vector<uint32_t> offset{0};            // [n_classes + 1]
+    std::vector<uint32_t> term;
+    std::vector<int32_t> own;
+    std::vector<uint8_t> match;
+    uint32_t n_classes() const { return (uint32_t)offset.size() - 1; }
+  };
+  std::vector<std::string> keys;                // key id -> topology key
+  std::vector<std::vector<std::string>> values; // [key] value id -> label value
+  std::vector<uint32_t> n_values;               // [n_keys]
+  std::vector<uint32_t> topo;                   // [n_keys][n_nodes], BS_TOPO_NONE = the node lacks the key
+  std::vector<std::string> term_signatures;     // term id -> signature
+  std::vector<uint32_t> term_key;               // [n_terms]
+  std::vector<uint32_t> bound_node, bound_class;   // [n_bound], BS_IPA_NONE = no entries
+  Classes bound_classes;
+  std::vector<uint32_t> pod_class;              // [n_pods], BS_IPA_NONE = no entries (scores 0)
+  Classes pod_classes;
 };
 // normalizedImageName (ImageLocality): ":latest" appended when the last ':' does not follow the last '/'
 std::string normalized_image_name(const std::string& name);
@@ -449,6 +489,12 @@ class BatchSchedulingPlugin {
   // weight of kube-scheduler v1.17's SelectorSpread priority in PriorityNodes (bs_set_spread_weight; 0 = off, the
   // default; v1.17's default profile is 1), read by the next round; ReplayQueue(kPriority) refuses a non-zero weight
   void SetSelectorSpreadWeight(uint32_t selector_spread);
+  // weight of kube-scheduler v1.17's InterPodAffinity priority in PriorityNodes (bs_set_interpod_weight; 0 = off, the
+  // default; v1.17's default profile is 1), read by the next round; ReplayQueue(kPriority) refuses a non-zero weight
+  void SetInterPodAffinityWeight(uint32_t inter_pod_affinity);
+  // hardPodAffinitySymmetricWeight: the weight of a bound pod's required pod-affinity term in InterPodAffinity,
+  // 0..100 (else an error), default 1; 0 leaves those terms out
+  Status SetHardPodAffinityWeight(int32_t hard_pod_affinity_weight);
   int group_index(const std::string& ns_name) const;
   double last_pack_ms() const { return last_pack_ms_; }
   double last_device_ms() const { return last_device_ms_; }
@@ -533,6 +579,21 @@ class BatchSchedulingPlugin {
   // selector matches.  More than 64 zones, or a count above BS_SPREAD_COUNT_MAX, is an error.
   static Status PackSpread(const std::vector<const NodeInfo*>& snapshot, const std::vector<const Pod*>& pending,
                            const SpreadSelectors& selectors, PackedSpread* out);
+  // The columns of the InterPodAffinity priority (no GPU), from NodeInfo::pods (terminating ones too) and the pending
+  // pods.  Keys and terms are numbered in order of first appearance over the bound pods' terms (required affinity
+  // while hard_weight > 0, preferred affinity, preferred anti-affinity), then the pending pods' (preferred affinity,
+  // preferred anti-affinity); a term is identified by its resolved, sorted namespaces, its converted selector's
+  // canonical text (SelectorSpread's conversion) and its key.  A term with an empty key matches no node and is left
+  // out; so is a term whose selector fails to convert.  Each key's values are numbered in order of first appearance
+  // over the nodes.  A pod lists (t, own, match) for every term it owns (own: its summed signed weights, +hard_weight
+  // per required term of a bound pod) or matches among the other side's terms; a pod without entries has no class,
+  // and classes are numbered in order of first appearance.  A pending pod gets no class (BS_IPA_NONE, score 0), as
+  // upstream fails its score, when a processed term of a bound pod fails to convert, or when one of its own terms does
+  // and a pod is bound.  More than BS_IPA_KEY_MAX keys, BS_IPA_BOUND_MAX bound pods or BS_IPA_CLASS_MAX entries in a
+  // class, or an own outside BS_IPA_OWN_MAX, is an error.
+  static Status PackInterPodAffinity(const std::vector<const NodeInfo*>& snapshot,
+                                     const std::vector<const Pod*>& pending, int32_t hard_weight,
+                                     PackedInterPodAffinity* out);
 
   static Status Pack(const std::vector<const NodeInfo*>& snapshot, const std::vector<const Pod*>& pending,
                      const std::vector<PodGroup>& groups, const std::vector<uint32_t>& matched,
@@ -565,6 +626,8 @@ class BatchSchedulingPlugin {
   uint32_t locality_weights_[2] = {0, 0};              // SetLocalityWeights: ImageLocality, NodePreferAvoidPods
   uint32_t spread_weight_ = 0;                          // SetSelectorSpreadWeight
   SpreadSelectors spread_selectors_;                    // SetSpreadSelectors
+  uint32_t interpod_weight_ = 0;                        // SetInterPodAffinityWeight
+  int32_t hard_pod_affinity_weight_ = 1;                // SetHardPodAffinityWeight
   std::string init_error_;
   int64_t max_schedule_time_ns_;
   std::map<std::string, GroupState> groups_;                        // ordered: canonical table order
@@ -600,6 +663,8 @@ class BatchSchedulingPlugin {
                                 // while a weight is non-zero; no-op without priority_k
   Status UploadSpread();     // both spread sides of snapshot_ and pending_ and the weight; the columns only while the
                              // weight is non-zero; no-op without priority_k
+  Status UploadInterPodAffinity();   // both inter-pod sides of snapshot_ and pending_ and the weight; the columns
+                                    // only while the weight is non-zero; no-op without priority_k
   Status UploadLocality();   // both locality sides of snapshot_ and pending_ and the two weights; the columns only
                              // while a weight is non-zero; no-op without priority_k
   Status UploadBound();  // packs and uploads the bound-pod table of snapshot_ (no-op when no NodeInfo lists pods)

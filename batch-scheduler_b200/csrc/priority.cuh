@@ -8,7 +8,8 @@
 // the RequestedToCapacityRatio term (kernels.cuh ratio_*) is added to it; with PREF the TaintToleration and preferred
 // NodeAffinity terms (bs_set_node_priority_weights), normalized over the pod's fit set; with LOC the ImageLocality and
 // NodePreferAvoidPods terms (bs_set_locality_weights), static per pair, from the pre-pass below; with SPREAD the
-// SelectorSpread term (bs_set_spread_weight), normalized over the pod's fit set and its zones.
+// SelectorSpread term (bs_set_spread_weight), normalized over the pod's fit set and its zones; with IPA the
+// InterPodAffinity term (bs_set_interpod_weight), from the pre-pass below, normalized over the pod's fit set.
 #pragma once
 #include "kernels.cuh"
 #include "fit.cuh"
@@ -132,8 +133,29 @@ __device__ __forceinline__ int64_t spread_score(uint32_t cnt, uint32_t mn, bool 
   return __double2ll_rz(f);
 }
 
+// IPA's arguments (bs_upload_node_interpod / bs_upload_pod_interpod): the class x node raw table the IPA pre-pass
+// built, each pod's class, and the weight.  Derived from SPREAD's type for the same reason; the fields of the other
+// flags are read only with their flags.
+constexpr uint32_t IPA_NONE = 0xffffffffu;   // BS_IPA_NONE
+constexpr uint32_t TOPO_NONE = 0xffffffffu;  // BS_TOPO_NONE
+constexpr int IPA_CLASS_MAX = 64;            // BS_IPA_CLASS_MAX
+struct PriorityIpaArgs : PrioritySpreadArgs {
+  const int64_t* ipa_raw;       // [classes][Npad] raw of (class, node) (padding 0)
+  const uint32_t* ipa_class;    // [P] row of ipa_raw or IPA_NONE
+  uint32_t w_ipa;
+};
+// InterPodAffinity of one fitting pair (CalculateInterPodAffinityPriorityReduce): raw = the pair's raw score, mn / mx =
+// the pod's minimum and maximum over its fit set, both started at 0.  |raw| <= 2^47 (bsched.h), so raw - mn and
+// mx - mn convert exactly; the division and the product are binary64 roundings of their own whatever -fmad says, and
+// the result is truncated toward zero.
+__device__ __forceinline__ int64_t ipa_score(int64_t raw, int64_t mn, int64_t mx) {
+  if (mx - mn <= 0) return 0;
+  return __double2ll_rz(__dmul_rn(100.0, __ddiv_rn(__ll2double_rn(raw - mn), __ll2double_rn(mx - mn))));
+}
+
 // The LOC pre-pass (priority_inst.cu image_spread_kernel, locality_class_kernel) builds the IL table once per
-// change of either side or a weight.
+// change of either side or a weight; the IPA pre-pass (priority_inst.cu interpod_mass_kernel, interpod_class_kernel)
+// builds the raw table once per change of either side.
 constexpr int LOC_THREADS = 256;
 
 // PREF (chosen by the host when either weight of bs_set_node_priority_weights is non-zero) adds w_taint * TT +
@@ -155,14 +177,21 @@ constexpr int LOC_THREADS = 256;
 // haveZones needs no state of its own: it only changes the score of a fitting node with a zone, and that node makes it
 // true.  A pod without selectors (SPREAD_NONE) scores 100 and reads nothing.
 //
-// LOC's and SPREAD's kernels ask for two CTAs per SM: left to itself, ptxas gives the PREF + LOC variants up to 145
-// registers, which fits one 256-thread CTA per SM where the kernels without LOC run two.
-template <int MAXL, bool RATIO, bool PREF, bool LOC = false, bool SPREAD = false>
-__global__ void __launch_bounds__(PRIO_THREADS, (LOC || SPREAD) ? 2 : 0)
-priority_pod_kernel(std::conditional_t<SPREAD, PrioritySpreadArgs,
+// IPA (chosen by the host when bs_set_interpod_weight is non-zero) adds w_ipa * IPA.  The pre-pass has already summed
+// every bound pod's terms into one int64 raw per (class, node), so the pair reads one int64; the normalization needs
+// the pod's minimum and maximum raw over its fit set, which the first sweep (shared with PREF and SPREAD) keeps per lane,
+// both started at 0, and reduces across the warp into shared memory, so that they hold no register in the scoring
+// sweep.  A pod without a class (IPA_NONE) scores 0 and reads nothing.
+//
+// LOC's, SPREAD's and IPA's kernels ask for two CTAs per SM: left to itself, ptxas gives the PREF + LOC variants up to
+// 145 registers, which fits one 256-thread CTA per SM where the kernels without LOC run two.
+template <int MAXL, bool RATIO, bool PREF, bool LOC = false, bool SPREAD = false, bool IPA = false>
+__global__ void __launch_bounds__(PRIO_THREADS, (LOC || SPREAD || IPA) ? 2 : 0)
+priority_pod_kernel(std::conditional_t<IPA, PriorityIpaArgs,
+                    std::conditional_t<SPREAD, PrioritySpreadArgs,
                     std::conditional_t<LOC, PriorityLocArgs,
                                        std::conditional_t<PREF, PriorityPrefArgs,
-                                                          std::conditional_t<RATIO, PriorityRatioArgs, PriorityArgs>>>> a) {
+                                                          std::conditional_t<RATIO, PriorityRatioArgs, PriorityArgs>>>>> a) {
   constexpr int WARPS = PRIO_THREADS / 32;
   __shared__ int64_t s_req[WARPS][PRIO_PPW][MAXL];
   __shared__ int64_t s_ls[WARPS][PRIO_PPW][32];
@@ -229,7 +258,21 @@ priority_pod_kernel(std::conditional_t<SPREAD, PrioritySpreadArgs,
     }
     __syncwarp();
   }
-  if constexpr (PREF || SPREAD) {
+  // IPA: the pod's class, and its minimum and maximum raw over its fit set ([PRIO_PPW][2], the warp's, shared memory)
+  [[maybe_unused]] uint32_t icls[PRIO_PPW];
+  [[maybe_unused]] int64_t (*ipm)[2] = nullptr;
+  if constexpr (IPA) {
+    __shared__ int64_t s_ipm[WARPS][PRIO_PPW][2];
+    ipm = s_ipm[wid];
+#pragma unroll
+    for (int j = 0; j < PRIO_PPW; ++j) icls[j] = rmask[j] ? a.ipa_class[p0 + j] : IPA_NONE;
+  }
+  if constexpr (PREF || SPREAD || IPA) {
+    [[maybe_unused]] int64_t imn[PRIO_PPW], imx[PRIO_PPW];   // IPA: this lane's extremes, both started at 0
+    if constexpr (IPA) {
+#pragma unroll
+      for (int j = 0; j < PRIO_PPW; ++j) imn[j] = imx[j] = 0;
+    }
     if constexpr (PREF) {
 #pragma unroll
       for (int j = 0; j < PRIO_PPW; ++j) {
@@ -289,6 +332,15 @@ priority_pod_kernel(std::conditional_t<SPREAD, PrioritySpreadArgs,
           }
         }
       }
+      if constexpr (IPA) {
+#pragma unroll
+        for (int j = 0; j < PRIO_PPW; ++j) {
+          if (!g[j] || icls[j] == IPA_NONE) continue;
+          const int64_t r = a.ipa_raw[(size_t)icls[j] * a.Npad + i];
+          imn[j] = min(imn[j], r);
+          imx[j] = max(imx[j], r);
+        }
+      }
     }
     if constexpr (PREF) {
 #pragma unroll
@@ -307,6 +359,19 @@ priority_pod_kernel(std::conditional_t<SPREAD, PrioritySpreadArgs,
         for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
         mz[j] = m;
       }
+    }
+    if constexpr (IPA) {
+#pragma unroll
+      for (int j = 0; j < PRIO_PPW; ++j) {
+        int64_t lo = imn[j], hi = imx[j];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+          lo = min(lo, __shfl_xor_sync(0xffffffffu, lo, o));
+          hi = max(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+        }
+        if (lane == 0) { ipm[j][0] = lo; ipm[j][1] = hi; }
+      }
+      __syncwarp();
     }
   }
   for (uint32_t base = 0; base < a.N; base += 32) {
@@ -394,6 +459,11 @@ priority_pod_kernel(std::conditional_t<SPREAD, PrioritySpreadArgs,
           }
           s = (int64_t)((uint64_t)s + (uint64_t)a.w_spread * (uint64_t)ss);
         }
+      if constexpr (IPA)
+        if (g[j] && icls[j] != IPA_NONE) {
+          const int64_t is = ipa_score(a.ipa_raw[(size_t)icls[j] * a.Npad + i], ipm[j][0], ipm[j][1]);
+          s = (int64_t)((uint64_t)s + (uint64_t)a.w_ipa * (uint64_t)is);
+        }
       const uint32_t cb = __ballot_sync(0xffffffffu, g[j] && (nfit[j] < a.K || s > thr[j]));
       if (cb) thr[j] = topk_insert<int64_t>(s_ls[wid][j], s_ln[wid][j], a.K, cb, s, (int32_t)base, lane);
       nfit[j] += __popc(fw[j]);
@@ -411,18 +481,37 @@ priority_pod_kernel(std::conditional_t<SPREAD, PrioritySpreadArgs,
 }
 
 // priority_inst.cu, a translation unit of its own so that the variants compile in parallel with engine.cu:
-// priority_pod_kernel<MAXL, ratio, pref, loc, spread> for the engine's lane count L; `a` is read as the flags' argument
-// type (PriorityArgs without any flag, PriorityRatioArgs with ratio alone, PriorityPrefArgs with pref, PriorityLocArgs
-// with loc, all of it with spread).
-cudaError_t launch_priority(uint32_t L, uint32_t grid, bool ratio, bool pref, bool loc, bool spread,
-                            const PrioritySpreadArgs& a, cudaStream_t s);
+// priority_pod_kernel<MAXL, ratio, pref, loc, spread, ipa> for the engine's lane count L; `a` is read as the flags'
+// argument type (PriorityArgs without any flag, PriorityRatioArgs with ratio alone, PriorityPrefArgs with pref,
+// PriorityLocArgs with loc, PrioritySpreadArgs with spread, all of it with ipa).
+cudaError_t launch_priority(uint32_t L, uint32_t grid, bool ratio, bool pref, bool loc, bool spread, bool ipa,
+                            const PriorityIpaArgs& a, cudaStream_t s);
 // priority_spread_inst.cu, one translation unit per MAXL (-DBS_PRIO_SPREAD_MAXL): the SPREAD variants, reached through
 // launch_priority
 template <int MAXL>
 void launch_priority_spread(uint32_t grid, bool ratio, bool pref, bool loc, const PrioritySpreadArgs& a, cudaStream_t s);
+// priority_interpod_inst.cu, one translation unit per MAXL (-DBS_PRIO_IPA_MAXL): the IPA variants, reached through
+// launch_priority
+template <int MAXL>
+void launch_priority_interpod(uint32_t grid, bool ratio, bool pref, bool loc, bool spread, const PriorityIpaArgs& a,
+                              cudaStream_t s);
 // the LOC pre-pass: scaled[n_images] from the bit rows and sizes, then il[n_classes][Npad]; 2 launches
 cudaError_t launch_locality_prepass(const uint32_t* bits, const int64_t* size, int64_t* scaled, uint32_t n_images,
                                     const uint32_t* class_offset, const uint32_t* class_images, uint8_t* il,
                                     uint32_t n_classes, uint32_t n_nodes, uint32_t Npad, cudaStream_t s);
+// The IPA pre-pass over device copies of the bs_interpod_nodes / bs_interpod_pods columns.  term_off[t]: the first
+// (term, value) slot of term t; ms[slots][2]: M and S, zeroed by the caller.  With mass, the bound pods are summed into
+// ms first (1 launch); then raw[n_pod_classes][Npad] (1 launch).
+struct InterpodClasses {
+  const uint32_t* offset;   // [n_classes + 1]
+  const uint32_t* term;
+  const int32_t* own;
+  const uint8_t* match;
+  uint32_t n_classes;
+};
+cudaError_t launch_interpod_prepass(bool mass, const uint32_t* topo, const uint32_t* term_key, const uint32_t* term_off,
+                                    const uint32_t* bound_node, const uint32_t* bound_class, uint32_t n_bound,
+                                    const InterpodClasses& bound, const InterpodClasses& pods, int64_t* ms,
+                                    int64_t* raw, uint32_t n_nodes, uint32_t Npad, cudaStream_t s);
 
 }  // namespace bsk

@@ -1,6 +1,7 @@
-// priority_inst.cu — the priority lists' kernels (priority.cuh): every priority_pod_kernel variant and the LOC
-// pre-pass, except the SPREAD variants (priority_spread_inst.cu).  A translation unit of its own (build.py), compiled in
-// parallel with engine.cu, which reaches the kernels through launch_priority and launch_locality_prepass.
+// priority_inst.cu — the priority lists' kernels (priority.cuh): every priority_pod_kernel variant and the LOC and IPA
+// pre-passes, except the SPREAD and IPA variants (priority_spread_inst.cu, priority_interpod_inst.cu).  A translation
+// unit of its own (build.py), compiled in parallel with engine.cu, which reaches the kernels through launch_priority,
+// launch_locality_prepass and launch_interpod_prepass.
 #define BS_KERNELS_HELPERS_ONLY   // kernels.cuh's round kernels live in engine.cu
 #include "priority.cuh"
 
@@ -65,6 +66,87 @@ __global__ void __launch_bounds__(LOC_THREADS) locality_class_kernel(const uint3
   }
 }
 
+// The IPA pre-pass.  raw(c, n) = sum over class c's entries (t, own, match) of own * M[t][v] + match * S[t][v], v = n's
+// value of key(t), with M / S the sums of match / own over the bound pods whose node has value v (bsched.h): an
+// identity, grouped by term.  Integer sums in any order give the same table, so the result is bit-exact.
+//
+// K1h interpod_mass_kernel — a thread per bound pod, walking its class's entries in step with its warp: entry k of every
+// lane at once.  Bound pods of one class on nodes with one value of a key hit one (term, value) slot, so the lanes with
+// the same slot add theirs with __match_any_sync and __reduce_add_sync (|own| sum <= 32 x 2^16, no wrap) and one lane
+// of each slot does the two int64 atomics.  Every lane of a warp reaches the warp-wide calls: no lane returns early.
+__global__ void __launch_bounds__(LOC_THREADS) interpod_mass_kernel(const uint32_t* bound_node,
+                                                                    const uint32_t* bound_class, uint32_t n_bound,
+                                                                    InterpodClasses cl, const uint32_t* topo,
+                                                                    const uint32_t* term_key, const uint32_t* term_off,
+                                                                    uint32_t n_nodes, int64_t* ms) {
+  const uint32_t e = blockIdx.x * LOC_THREADS + threadIdx.x, lane = threadIdx.x & 31;
+  const uint32_t c = e < n_bound ? bound_class[e] : IPA_NONE;
+  uint32_t o0 = 0, n = 0, node = 0;
+  if (c != IPA_NONE) {
+    o0 = cl.offset[c];
+    n = cl.offset[c + 1] - o0;
+    node = bound_node[e];
+  }
+  const uint32_t rounds = __reduce_max_sync(0xffffffffu, n);
+  for (uint32_t k = 0; k < rounds; ++k) {
+    uint64_t slot = ~0ull;
+    int32_t own = 0;
+    uint32_t match = 0;
+    if (k < n) {
+      const uint32_t t = cl.term[o0 + k];
+      const uint32_t v = topo[(size_t)term_key[t] * n_nodes + node];
+      if (v != TOPO_NONE) {
+        slot = (uint64_t)term_off[t] + v;
+        own = cl.own[o0 + k];
+        match = cl.match[o0 + k];
+      }
+    }
+    const uint32_t peers = __match_any_sync(0xffffffffu, slot);
+    if (slot != ~0ull) {
+      const uint32_t m = __reduce_add_sync(peers, match);
+      const int32_t w = (int32_t)__reduce_add_sync(peers, (uint32_t)own);
+      if (lane == (uint32_t)(__ffs(peers) - 1)) {
+        if (m) atomicAdd((unsigned long long*)&ms[2 * slot], (unsigned long long)m);
+        if (w) atomicAdd((unsigned long long*)&ms[2 * slot + 1], (unsigned long long)(int64_t)w);
+      }
+    }
+  }
+}
+
+// K1i interpod_class_kernel — raw of every (pod class, node): a thread per node, the class's entries (at most
+// BS_IPA_CLASS_MAX) with their keys and slots in shared memory.  Padding nodes get 0.
+__global__ void __launch_bounds__(LOC_THREADS) interpod_class_kernel(InterpodClasses cl, const uint32_t* topo,
+                                                                     const uint32_t* term_key,
+                                                                     const uint32_t* term_off, const int64_t* ms,
+                                                                     int64_t* raw, uint32_t n_nodes, uint32_t Npad) {
+  __shared__ uint32_t s_key[IPA_CLASS_MAX], s_off[IPA_CLASS_MAX];
+  __shared__ int32_t s_own[IPA_CLASS_MAX];
+  __shared__ uint8_t s_match[IPA_CLASS_MAX];
+  const uint32_t i = blockIdx.x * LOC_THREADS + threadIdx.x;
+  for (uint32_t c = blockIdx.y; c < cl.n_classes; c += gridDim.y) {
+    const uint32_t o0 = cl.offset[c], n = cl.offset[c + 1] - o0;
+    __syncthreads();
+    if (threadIdx.x < n) {
+      const uint32_t t = cl.term[o0 + threadIdx.x];
+      s_key[threadIdx.x] = term_key[t];
+      s_off[threadIdx.x] = term_off[t];
+      s_own[threadIdx.x] = cl.own[o0 + threadIdx.x];
+      s_match[threadIdx.x] = cl.match[o0 + threadIdx.x];
+    }
+    __syncthreads();
+    if (i >= Npad) continue;
+    int64_t r = 0;
+    if (i < n_nodes)
+      for (uint32_t k = 0; k < n; ++k) {
+        const uint32_t v = topo[(size_t)s_key[k] * n_nodes + i];
+        if (v == TOPO_NONE) continue;
+        const longlong2 q = reinterpret_cast<const longlong2*>(ms)[(size_t)s_off[k] + v];
+        r += (int64_t)s_own[k] * q.x + (s_match[k] ? q.y : 0);
+      }
+    raw[(size_t)c * Npad + i] = r;
+  }
+}
+
 template <bool RATIO, bool PREF, bool LOC, class Args>
 void launch_t(uint32_t L, uint32_t grid, const Args& a, cudaStream_t s) {
   if (L <= 5) priority_pod_kernel<5, RATIO, PREF, LOC><<<grid, PRIO_THREADS, 0, s>>>(a);
@@ -74,16 +156,21 @@ void launch_t(uint32_t L, uint32_t grid, const Args& a, cudaStream_t s) {
 
 }  // namespace
 
-cudaError_t launch_priority(uint32_t L, uint32_t grid, bool ratio, bool pref, bool loc, bool spread,
-                            const PrioritySpreadArgs& a, cudaStream_t s) {
+cudaError_t launch_priority(uint32_t L, uint32_t grid, bool ratio, bool pref, bool loc, bool spread, bool ipa,
+                            const PriorityIpaArgs& a, cudaStream_t s) {
+  const PrioritySpreadArgs& ps = a;
   const PriorityLocArgs& pl = a;
   const PriorityPrefArgs& pp = a;
   const PriorityRatioArgs& pr = a;
   const PriorityArgs& pb = a;
-  if (spread) {
-    if (L <= 5) launch_priority_spread<5>(grid, ratio, pref, loc, a, s);
-    else if (L <= 9) launch_priority_spread<9>(grid, ratio, pref, loc, a, s);
-    else launch_priority_spread<16>(grid, ratio, pref, loc, a, s);
+  if (ipa) {
+    if (L <= 5) launch_priority_interpod<5>(grid, ratio, pref, loc, spread, a, s);
+    else if (L <= 9) launch_priority_interpod<9>(grid, ratio, pref, loc, spread, a, s);
+    else launch_priority_interpod<16>(grid, ratio, pref, loc, spread, a, s);
+  } else if (spread) {
+    if (L <= 5) launch_priority_spread<5>(grid, ratio, pref, loc, ps, s);
+    else if (L <= 9) launch_priority_spread<9>(grid, ratio, pref, loc, ps, s);
+    else launch_priority_spread<16>(grid, ratio, pref, loc, ps, s);
   } else if (loc) {
     if (pref && ratio) launch_t<true, true, true>(L, grid, pl, s);
     else if (pref) launch_t<false, true, true>(L, grid, pl, s);
@@ -110,6 +197,18 @@ cudaError_t launch_locality_prepass(const uint32_t* bits, const int64_t* size, i
   const dim3 grid((Npad + LOC_THREADS - 1) / LOC_THREADS, n_classes < 65535u ? n_classes : 65535u);
   locality_class_kernel<<<grid, LOC_THREADS, 0, s>>>(class_offset, class_images, bits, scaled, il, n_classes, n_nodes,
                                                      Npad, words);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_interpod_prepass(bool mass, const uint32_t* topo, const uint32_t* term_key, const uint32_t* term_off,
+                                    const uint32_t* bound_node, const uint32_t* bound_class, uint32_t n_bound,
+                                    const InterpodClasses& bound, const InterpodClasses& pods, int64_t* ms,
+                                    int64_t* raw, uint32_t n_nodes, uint32_t Npad, cudaStream_t s) {
+  if (mass && n_bound)
+    interpod_mass_kernel<<<(n_bound + LOC_THREADS - 1) / LOC_THREADS, LOC_THREADS, 0, s>>>(
+        bound_node, bound_class, n_bound, bound, topo, term_key, term_off, n_nodes, ms);
+  const dim3 grid((Npad + LOC_THREADS - 1) / LOC_THREADS, pods.n_classes < 65535u ? pods.n_classes : 65535u);
+  interpod_class_kernel<<<grid, LOC_THREADS, 0, s>>>(pods, topo, term_key, term_off, ms, raw, n_nodes, Npad);
   return cudaGetLastError();
 }
 

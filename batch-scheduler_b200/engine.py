@@ -389,6 +389,47 @@ class Engine:
             cls = np.ascontiguousarray(pods, dtype=np.uint32).reshape(-1)
             self._check(self.lib.bs_upload_pod_spread(self.h, len(cls), capi.ptr(cls)))
 
+    def set_interpod_weight(self, inter_pod_affinity: int = 0):
+        """Weight of kube-scheduler's InterPodAffinity priority in the priority score (0 = off, the default; v1.17's
+        default profile is 1).  A non-zero weight needs upload_interpod before each round, and makes
+        replay(priority=True) refuse to run."""
+        self._check(self.lib.bs_set_interpod_weight(self.h, inter_pod_affinity))
+
+    def upload_interpod(self, node=None, pods=None):
+        """The columns of InterPodAffinity (include/bsched.h bs_upload_node_interpod).  A class table is
+        (class_offset [C + 1], term, own int32, match uint8).  node = (n_values [K], topo [K, N], term_key [T],
+        bound_node [V], bound_class [V], classes): each key's value count, each node's value of each key
+        (capi.TOPO_NONE: none), each term's key, the bound pods' nodes and classes (capi.IPA_NONE: none) and the bound
+        classes.  pods = (pod_class [P], classes): each pod's class (capi.IPA_NONE: none) and the pod classes.  Uploading
+        nodes (or updating node rows) drops the node side, uploading pods the pod side."""
+        def classes(cl, keep):
+            off, term, own, match = cl
+            a = [np.ascontiguousarray(off, dtype=np.uint32).reshape(-1), np.ascontiguousarray(term, dtype=np.uint32),
+                 np.ascontiguousarray(own, dtype=np.int32), np.ascontiguousarray(match, dtype=np.uint8)]
+            keep += a
+            return capi.InterpodClassesC(max(len(a[0]) - 1, 0), *(capi.ptr(x) for x in a))
+        if node is not None:
+            keep = []
+            nv, topo, tkey, bnode, bcls, cl = node
+            nv = np.ascontiguousarray(nv, dtype=np.uint32).reshape(-1)
+            topo = (np.ascontiguousarray(topo, dtype=np.uint32).reshape(len(nv), -1) if len(nv)
+                    else np.zeros((0, self.N), np.uint32))
+            tkey = np.ascontiguousarray(tkey, dtype=np.uint32).reshape(-1)
+            bnode = np.ascontiguousarray(bnode, dtype=np.uint32).reshape(-1)
+            bcls = np.ascontiguousarray(bcls, dtype=np.uint32).reshape(-1)
+            if len(bnode) != len(bcls):
+                raise ValueError("bound_node and bound_class must have one entry per bound pod")
+            t = capi.InterpodNodesC(topo.shape[1], len(nv), capi.ptr(nv), capi.ptr(topo),
+                                    len(tkey), capi.ptr(tkey), len(bnode), capi.ptr(bnode), capi.ptr(bcls),
+                                    classes(cl, keep))
+            self._check(self.lib.bs_upload_node_interpod(self.h, C.byref(t)))
+        if pods is not None:
+            keep = []
+            pcls, cl = pods
+            pcls = np.ascontiguousarray(pcls, dtype=np.uint32).reshape(-1)
+            t = capi.InterpodPodsC(len(pcls), capi.ptr(pcls), classes(cl, keep))
+            self._check(self.lib.bs_upload_pod_interpod(self.h, C.byref(t)))
+
     def priority_rows(self, pod0=0, n=None):
         """(nodes [n, K] int32, scores [n, K] int64): each pod's fitting nodes by priority score descending, then node
         index ascending; min(K, feasible_count) entries, padded with node -1 and score INT64_MIN."""

@@ -469,6 +469,55 @@ def node_spread(snap: Snapshot, seed: int, n_zones: int = 4, unzoned: float = 0.
     return (zone, counts.astype(np.int32)), cls
 
 
+IPA_NONE = 0xFFFFFFFF    # BS_IPA_NONE
+TOPO_NONE = 0xFFFFFFFF   # BS_TOPO_NONE
+
+
+def interpod_classes(rng, n_classes: int, n_terms: int, max_entries: int, max_weight: int = 100,
+                     hard: int = 1) -> tuple:
+    """A seeded class table (class_offset [C + 1], term, own int32, match uint8): each class lists 1..max_entries
+    distinct terms; own is a preferred affinity (+1..max_weight), a preferred anti-affinity (-1..-max_weight), a
+    required affinity (+hard) or nothing (0), and match is 0 or 1, so both signs and both directions occur."""
+    off, term, own, match = [0], [], [], []
+    for _ in range(n_classes):
+        k = int(rng.integers(1, min(max_entries, max(n_terms, 1)) + 1)) if n_terms else 0
+        ts = rng.choice(n_terms, k, replace=False) if k else []
+        for t in ts:
+            kind = int(rng.integers(0, 4))
+            w = int(rng.integers(1, max_weight + 1))
+            term.append(int(t))
+            own.append((w, -w, hard, 0)[kind])
+            match.append(int(rng.integers(0, 2)))
+        off.append(len(term))
+    return (np.array(off, np.uint32), np.array(term, np.uint32), np.array(own, np.int32), np.array(match, np.uint8))
+
+
+def node_interpod(snap: Snapshot, seed: int, n_zones: int = 8, rack_size: int = 16, unlabelled: float = 0.05,
+                  n_terms: int = 24, n_bound: int = None, n_bclasses: int = 12, n_pclasses: int = 10,
+                  max_entries: int = 6, no_class: float = 0.2, hard: int = 1):
+    """Seeded columns of the InterPodAffinity priority for a table without objects: (node, pods) as Engine.upload_interpod
+    takes them.  Three topology keys: a hostname-like key (one value per node), a zone-like key (n_zones values) and a
+    rack-like key (one value per rack_size nodes); a share `unlabelled` of the nodes lacks the zone and the rack key.
+    n_terms terms over the three keys; n_bound bound pods (default 4 per node) spread over the nodes, of n_bclasses
+    classes; n_pclasses pod classes; a share `no_class` of the pods and of the bound pods has no class (IPA_NONE)."""
+    rng = np.random.default_rng(seed)
+    N, P = snap.nodes.n, snap.pods.n
+    n_bound = 4 * N if n_bound is None else n_bound
+    racks = max((N + rack_size - 1) // rack_size, 1)
+    n_values = np.array([max(N, 1), max(n_zones, 1), racks], np.uint32)
+    topo = np.stack([np.arange(N), rng.integers(0, max(n_zones, 1), N), np.arange(N) // rack_size]).astype(np.uint32)
+    topo[1:, rng.random(N) < unlabelled] = TOPO_NONE
+    term_key = rng.integers(0, 3, n_terms).astype(np.uint32)
+    bound_node = rng.integers(0, max(N, 1), n_bound).astype(np.uint32)
+    bound_class = rng.integers(0, max(n_bclasses, 1), n_bound).astype(np.uint32)
+    bound_class[(rng.random(n_bound) < no_class) | (n_bclasses == 0)] = IPA_NONE
+    bcl = interpod_classes(rng, n_bclasses, n_terms, max_entries, hard=hard)
+    pod_class = rng.integers(0, max(n_pclasses, 1), P).astype(np.uint32)
+    pod_class[(rng.random(P) < no_class) | (n_pclasses == 0)] = IPA_NONE
+    pcl = interpod_classes(rng, n_pclasses, n_terms, max_entries, hard=0)
+    return (n_values, topo, term_key, bound_node, bound_class, bcl), (pod_class, pcl)
+
+
 # ----------------------------------------------------------------------------
 # splitmix64 stream (vectorised): value i of the stream with seed s is
 # mix(s + (i+1)*0x9E3779B97F4A7C15).

@@ -598,6 +598,74 @@ int bs_upload_node_spread(bs_engine* e, uint32_t n_nodes, uint32_t n_zones, cons
 /* spread_class[n_pods]: the pod's row of counts or BS_SPREAD_NONE.  n_pods must equal the pod table's (else
  * BS_E_INVAL); a failing call leaves the side dropped.  bs_upload_pods drops the side. */
 int bs_upload_pod_spread(bs_engine* e, uint32_t n_pods, const uint32_t* spread_class);
+/* kube-scheduler v1.17's InterPodAffinity priority, added to the BS_OUT_PRIORITY score with weight inter_pod_affinity
+ * (0 = off, the default; v1.17's default profile is 1).  Any time, read by the next evaluation.  The caller resolves
+ * the objects into a dictionary of terms t = (namespaces, selector, topology key key(t)) and gives every pod and every
+ * bound pod a class: a list of entries (t, own, match), at most one per term, where
+ *     match = 1 when the pod matches t (its namespace is among t's, t's selector matches its labels), else 0
+ *     own   = the pod's own signed weights on t: +Weight per preferred affinity term, -Weight per preferred
+ *             anti-affinity term and, for a bound pod, +hardPodAffinityWeight per required affinity term.
+ * Per (pod p, node n) [upstream, from memory]:
+ *     raw(p, n) = sum over bound pods e, over entries (t, own_p, match_p) of p's class and (t, own_e, match_e) of e's
+ *                 class, where n and e's node both carry key(t) with the same value, of own_p * match_e + match_p * own_e
+ *     F = the pod's fit set (the nodes of its fit-bitmap row); no other node counts
+ *     max = max(0, max raw over F);  min = min(0, min raw over F)
+ *     IPA = max - min > 0 ? (int64)(100.0 * ((double)(raw - min) / (double)(max - min))) : 0
+ *                                                   (binary64, each operation rounded on its own; truncation)
+ *     score = <the score above> + inter_pod_affinity * IPA                  (int64, two's complement wrap)
+ * The engine computes raw as sum over the class's entries of own * M[t][v] + match * S[t][v], v = n's value of key(t),
+ * with M[t][v] / S[t][v] the sums of match_e / own_e over the bound pods whose node has value v: the same sum, grouped.
+ * A BS_IPA_NONE pod or bound pod has no entries (a pod scores 0 everywhere).  Every fitting node is scored, and ties go
+ * to the lower node index.  An evaluation with BS_OUT_PRIORITY and a non-zero weight is BS_E_STATE before anything is
+ * launched when either side is missing, and BS_E_INDEX when a pod class's term is >= the node side's n_terms.
+ * bs_replay_priority refuses to run (BS_E_INVAL) while the weight is non-zero.
+ *
+ * Exactness: at most BS_IPA_BOUND_MAX bound pods, BS_IPA_CLASS_MAX entries per class with distinct terms,
+ * |own| <= BS_IPA_OWN_MAX and match in {0, 1} give |M| <= 2^24 and |S| <= 2^40, so each entry adds at most 2^41 and a
+ * raw is at most 2^47 in magnitude: raw - min and max - min stay within 2^48 and convert to binary64 exactly. */
+int bs_set_interpod_weight(bs_engine* e, uint32_t inter_pod_affinity);
+#define BS_IPA_NONE 0xffffffffu                 /* class of a pod or bound pod without entries */
+#define BS_TOPO_NONE 0xffffffffu                /* topo value of a node without the key */
+#define BS_IPA_KEY_MAX 64                       /* topology keys of one node side */
+#define BS_IPA_BOUND_MAX (1u << 24)             /* bound pods of one node side */
+#define BS_IPA_CLASS_MAX 64                     /* entries of one class */
+#define BS_IPA_OWN_MAX (1 << 16)                /* largest |own| of one entry */
+#define BS_IPA_TERM_MAX_BYTES (1ull << 30)      /* 16 x sum over terms of n_values[term_key[t]] at most 1 GiB */
+#define BS_IPA_TABLE_MAX_BYTES (1ull << 30)     /* pod n_classes x Npad x 8 (Npad: n_nodes rounded up) at most 1 GiB */
+/* A class table: class c's entries are [class_offset[c], class_offset[c + 1]) of term / own / match. */
+typedef struct {
+  uint32_t n_classes;
+  const uint32_t* class_offset;   /* [n_classes + 1], class_offset[0] = 0, ascending, at most BS_IPA_CLASS_MAX apart */
+  const uint32_t* term;           /* [class_offset[n_classes]] term ids, distinct within a class */
+  const int32_t* own;             /* [...] |own| <= BS_IPA_OWN_MAX */
+  const uint8_t* match;           /* [...] 0 or 1 */
+} bs_interpod_classes;
+typedef struct {
+  uint32_t n_nodes;               /* the node table's */
+  uint32_t n_keys;                /* at most BS_IPA_KEY_MAX */
+  const uint32_t* n_values;       /* [n_keys] values of each key */
+  const uint32_t* topo;           /* [n_keys][n_nodes] value id < n_values[k], or BS_TOPO_NONE */
+  uint32_t n_terms;
+  const uint32_t* term_key;       /* [n_terms] < n_keys */
+  uint32_t n_bound;               /* at most BS_IPA_BOUND_MAX */
+  const uint32_t* bound_node;     /* [n_bound] < n_nodes */
+  const uint32_t* bound_class;    /* [n_bound] < classes.n_classes, or BS_IPA_NONE */
+  bs_interpod_classes classes;    /* the bound pods' classes; terms < n_terms */
+} bs_interpod_nodes;
+typedef struct {
+  uint32_t n_pods;                /* the pod table's */
+  const uint32_t* pod_class;      /* [n_pods] < classes.n_classes, or BS_IPA_NONE */
+  bs_interpod_classes classes;    /* the pods' classes; terms checked against the node side at evaluation */
+} bs_interpod_pods;
+/* The node side.  An id out of range is BS_E_INDEX, an own or match out of range BS_E_RANGE; a wrong n_nodes, more
+ * than BS_IPA_KEY_MAX keys or BS_IPA_BOUND_MAX bound pods, a malformed class table or term tables over
+ * BS_IPA_TERM_MAX_BYTES are BS_E_INVAL; a failing call leaves the side dropped.  The side belongs to the node snapshot
+ * (pods bind, labels change): bs_upload_nodes and bs_update_nodes drop it. */
+int bs_upload_node_interpod(bs_engine* e, const bs_interpod_nodes* t);
+/* The pod side, checked as the node side's classes; the raw table (n_classes x Npad x 8 bytes, at most
+ * BS_IPA_TABLE_MAX_BYTES, else BS_E_INVAL, checked here and at evaluation) is built at the first evaluation after
+ * either side changes.  bs_upload_pods drops the side. */
+int bs_upload_pod_interpod(bs_engine* e, const bs_interpod_pods* t);
 
 /* ---- preemption: PreFilterExtensions.RemovePod and the node / victims kube-scheduler's preemption would pick ----
  * The bound-pod table lists the pods already running on the snapshot's nodes (NodeInfo.Pods()).  Rows may come in

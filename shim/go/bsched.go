@@ -338,6 +338,23 @@ func (e *Engine) UploadPodSpread(spreadClass []uint32) error {
 		(*C.uint32_t)(unsafe.Pointer(&spreadClass[0]))))
 }
 
+// SetInterPodAffinityWeight: kube-scheduler v1.17's InterPodAffinity weight in the priority lists (0 = off; v1.17's
+// default profile is 1).  ReplayPriority refuses a non-zero weight.
+func (e *Engine) SetInterPodAffinityWeight(interPodAffinity uint32) error {
+	return e.rc(C.bs_set_interpod_weight(e.h, C.uint32_t(interPodAffinity)))
+}
+
+// UploadNodeInterPodAffinity / UploadPodInterPodAffinity: the InterPodAffinity sides (topology values, term keys,
+// bound pods and their classes; each pending pod's class), as the packer builds them in C-malloc'd (or pinned)
+// columns, like the other tables: cgo forbids passing a Go struct that holds Go pointers.  UploadNodes / UpdateNodes
+// drop the node side and UploadPods the pod side.
+func (e *Engine) UploadNodeInterPodAffinity(t *C.bs_interpod_nodes) error {
+	return e.rc(C.bs_upload_node_interpod(e.h, t))
+}
+func (e *Engine) UploadPodInterPodAffinity(t *C.bs_interpod_pods) error {
+	return e.rc(C.bs_upload_pod_interpod(e.h, t))
+}
+
 // UploadNodeNonZero / UploadPodNonZero: the non-zero request columns, nz[2][n] (cpu millicores, then memory bytes):
 // per pod the sum over its containers of GetNonzeroRequestForResource(Requests), per node NodeInfo.NonZeroRequest().
 // UploadNodes / UpdateNodes drop the node column and UploadPods the pod column: upload them again before Evaluate.
