@@ -22,6 +22,7 @@
 #include <sched.h>
 #include <vector>
 
+#include "devmem.hpp"
 #include "kernels.cuh"
 #include "fit.cuh"
 #include "gang_state.hpp"
@@ -42,6 +43,26 @@ struct PinnedAlloc {
   static cudaError_t alloc(void** p, size_t bytes) { return cudaHostAlloc(p, bytes, cudaHostAllocDefault); }
   static void free(void* p) { cudaFreeHost(p); }
 };
+// Compressible device memory (devmem.hpp) where the device supports it and the driver grants it, cudaMalloc
+// otherwise.  For the score matrix: every element is INT64_MIN or, on a shape with a narrow lane, a score below 2^27,
+// so at least half its bytes are zero and the L2 sends it to DRAM in fewer bytes (DESIGN §4).
+struct CompressibleAlloc {
+  CompMem m;
+  int supported = 0;   // CU_DEVICE_ATTRIBUTE_GENERIC_COMPRESSION_SUPPORTED at the last allocation
+  cudaError_t alloc(void** p, size_t bytes) {
+    supported = compmem_supported();
+    if (compmem_alloc(&m, bytes)) {
+      *p = m.p;
+      return cudaSuccess;
+    }
+    return cudaMalloc(p, bytes);
+  }
+  void free(void* p) {
+    if (m.p) compmem_free(&m);
+    else cudaFree(p);
+  }
+  bool compressed() const { return m.p != nullptr; }
+};
 
 // A block of device or pinned host memory that frees itself.  ensure() only grows it (at least 256 bytes)
 // and does not keep the contents when it does.
@@ -49,12 +70,13 @@ template <class A>
 struct Buf {
   void* p = nullptr;
   size_t cap = 0;
+  A a;   // the allocator: what it needs to free the block, and what it reports about it
   Buf() = default;
-  Buf(Buf&& o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); }
-  Buf& operator=(Buf&& o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); return *this; }
+  Buf(Buf&& o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); std::swap(a, o.a); }
+  Buf& operator=(Buf&& o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); std::swap(a, o.a); return *this; }
   ~Buf() { reset(); }
   void reset() {
-    if (p) A::free(p);
+    if (p) a.free(p);
     p = nullptr;
     cap = 0;
   }
@@ -62,7 +84,7 @@ struct Buf {
     if (bytes <= cap) return cudaSuccess;
     reset();
     const size_t want = std::max<size_t>(bytes, 256);
-    cudaError_t e = A::alloc(&p, want);
+    cudaError_t e = a.alloc(&p, want);
     if (e == cudaSuccess) cap = want;
     else p = nullptr;
     return e;
@@ -72,6 +94,7 @@ struct Buf {
 };
 using DevBuf = Buf<DeviceAlloc>;
 using PinBuf = Buf<PinnedAlloc>;
+using ScoreBuf = Buf<CompressibleAlloc>;
 
 // A field of an arena (carve): it neither allocates nor frees.
 struct View {
@@ -393,7 +416,8 @@ struct bs_engine {
   // outputs
   DevBuf d_stage;         // bs_update_nodes / bs_update_groups: device staging of the changed rows
   DevBuf d_best_packed;   // gang_fit tail pieces: max((score + 1) << 32 | ~node) per pod
-  DevBuf d_fit_bitmap, d_score;
+  DevBuf d_fit_bitmap;
+  ScoreBuf d_score;   // compressible where granted (bs_score_memory); the fit bitmap gains nothing from it
   DevBuf d_topk_node, d_topk_score;   // BS_OUT_TOPK: [Prows][topk] lists
   // BS_OUT_REASONS: full-width residuals [L][Npad], per fit class the gate bitmap [classes][Npad/32] and bins 0-3
   // [classes][4] (rebuilt with the class fit bits), and the rows [P][4 + L]
@@ -1302,8 +1326,9 @@ int evaluate_async_locked(bs_engine* e) {
         // way (32 registers: its CTAs share their SMs with the fit CTAs); when the fit kernel is the shorter of the two
         // (a small shard, few nodes) the round waits for the sort, and the build with 16 gathers in flight per thread
         // is the faster one.  Estimate: pairs x the per-pair time of the output mode measured on an H100 (top-K: K = 16
-        // at cfg4, profiles/topk_h100.jsonl).
-        const double per_pair_ms = (e->out_flags & BS_OUT_SCORE) ? 2.9e-9 : (e->out_flags & BS_OUT_TOPK) ? 2.0e-9 : 0.9e-9;
+        // at cfg4, profiles/topk_h100.jsonl; score mode on compressible memory: profiles/score_memory_h100.jsonl).
+        const double score_ms = e->d_score.a.compressed() ? 2.2e-9 : 2.9e-9;
+        const double per_pair_ms = (e->out_flags & BS_OUT_SCORE) ? score_ms : (e->out_flags & BS_OUT_TOPK) ? 2.0e-9 : 0.9e-9;
         const double est_fit_ms = (double)P * (double)e->N * per_pair_ms;
         const bool lean = est_fit_ms > 0.6;
         const void* fn = lean ? (const void*)queue_sort_kernel<SORT_LEAN_GROUP> : (const void*)queue_sort_kernel<SORT_WIDE_GROUP>;
@@ -3670,6 +3695,15 @@ int bs_fit_shape(bs_engine* e, uint32_t* wide, uint32_t* narrow, uint32_t* scale
   if (wide) *wide = e->lane_map.LW;
   if (narrow) *narrow = e->lane_map.LN;
   if (scaled) *scaled = e->lane_map.LS;
+  return BS_OK;
+}
+
+int bs_score_memory(bs_engine* e, uint32_t* supported, uint32_t* compressed) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!e->d_score.p) return fail(e, BS_E_STATE, "bs_score_memory: no score matrix (evaluate with BS_OUT_SCORE first)");
+  if (supported) *supported = (uint32_t)e->d_score.a.supported;
+  if (compressed) *compressed = e->d_score.a.compressed() ? 1u : 0u;
   return BS_OK;
 }
 

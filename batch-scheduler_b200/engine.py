@@ -660,6 +660,13 @@ class Engine:
         return {"kernel": int(k.value), "grid": int(g.value), "group_passes": int(gp.value),
                 "pod_passes": int(pp.value)}
 
+    def score_memory(self) -> dict:
+        """The memory behind the last evaluation's score matrix (bs_score_memory): supported (the device's
+        generic-compression attribute) and compressed (compressible memory, else cudaMalloc)."""
+        sup, comp = C.c_uint32(), C.c_uint32()
+        self._check(self.lib.bs_score_memory(self.h, C.byref(sup), C.byref(comp)))
+        return {"supported": int(sup.value), "compressed": bool(comp.value)}
+
     def replay_shape(self) -> dict:
         """The regime of the last replay walk (bs_replay_shape): cached (block-summary cache on), fitmask (checkFit
         bits per class), n_rep classes, n_blocks of 1024 nodes, findMaxPG's bucket_size and n_buckets, the final lo

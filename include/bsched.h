@@ -403,6 +403,8 @@ typedef enum {
   BS_BUF_ORDER = 5,
   BS_BUF_GATHERED_ADMIT = 6
 } bs_buffer;
+/* BS_BUF_SCORE is ordinary device memory to kernels and copies, but where bs_score_memory reports it compressed it
+ * came from cuMemCreate, not cudaMalloc, and cannot be exported through CUDA IPC (cudaIpcGetMemHandle). */
 int bs_device_buffer(bs_engine* e, int which, void** dev_ptr, size_t* bytes);
 void* bs_stream(bs_engine* e); /* the cudaStream_t a round is ordered on: uploads, the fit kernel and the
                                   verdicts run on it, and the two side streams of a round (PreFilter chain,
@@ -776,6 +778,12 @@ int bs_fit_shape(bs_engine* e, uint32_t* wide, uint32_t* narrow, uint32_t* scale
 /* per lane of the last evaluation's fit kernel: kind[d] 0 wide / 1 narrow / 2 scaled, unit[d] = k of a scaled lane
  * (0 otherwise); BS_E_STATE before the first evaluation */
 int bs_fit_lanes(bs_engine* e, uint8_t* kind /*[n_lanes]*/, uint8_t* unit /*[n_lanes]*/);
+/* the memory behind the score matrix (BS_OUT_SCORE) of the last evaluation: supported = the device's
+ * CU_DEVICE_ATTRIBUTE_GENERIC_COMPRESSION_SUPPORTED; compressed 1 when the matrix is compressible memory
+ * (cuMemCreate with CU_MEM_ALLOCATION_COMP_GENERIC: the L2 compresses its lines on their way to DRAM), 0 when
+ * the device does not support it or the driver did not grant it and it came from cudaMalloc.  Either way it is
+ * ordinary device memory to every kernel and copy.  BS_E_STATE before an evaluation with BS_OUT_SCORE. */
+int bs_score_memory(bs_engine* e, uint32_t* supported, uint32_t* compressed);
 /* what the last evaluation's queue sort launched: kernel 0 none (both tables empty), 1 the single-CTA kernel
  * (max(n_pods, n_groups) <= 16384), 2 the persistent kernel's lean build (4 keys in flight per thread, beside a long
  * fit kernel), 3 its wide build (16 in flight); the grid in CTAs (4096-key tiles are shared out round-robin when there

@@ -9,6 +9,8 @@
 //                 engine: cp.async.bulk.global.shared::cta.bulk_group; NB staging slabs per warp in flight
 //   tmacta<R,T,NB> CTA-level variant: the 8 warps fill a CTA slab (32 rows x T) and one thread issues
 //                 all 32 bulk stores (larger bursts per issue, one bar.sync per tile)
+//   tma<...,V>    the same pattern writing another value class (V): 0 small indices (the default), 1 zeros, 2 a
+//                 random 64-bit word per element; fit_attrib.cu includes this file for the two controls 1 and 2
 //
 // build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o store_pattern2 store_pattern2.cu
 // run:   ./store_pattern2        every variant at its own shared-memory size
@@ -59,8 +61,20 @@ __global__ void rowsv2(long long* out, int P, int N) {
       }
 }
 
+// V = 2: a 64-bit word whose halves are two 32-bit hashes of the element's position, so no two lines repeat
+__device__ __forceinline__ uint32_t mix32(uint32_t x) {
+  x *= 0x9e3779b1u; x ^= x >> 15; x *= 0x85ebca77u; x ^= x >> 13; x *= 0xc2b2ae3du; return x ^ (x >> 16);
+}
+template <int V>
+__device__ __forceinline__ long long store_value(long long index_value, int row, int col) {
+  if (V == 0) return index_value;
+  if (V == 1) return 0;
+  const uint32_t k = (uint32_t)row * 10007u + (uint32_t)col;
+  return (long long)(((uint64_t)mix32(k) << 32) | mix32(k ^ 0x5bd1e995u));
+}
+
 // warp-private staging slabs, NB deep
-template <int R, int T, int NB, int WARPS>
+template <int R, int T, int NB, int WARPS, int V = 0>
 __global__ void __launch_bounds__(WARPS * 32) tma(long long* out, int P, int N) {
   extern __shared__ __align__(128) unsigned char smem[];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -78,7 +92,8 @@ __global__ void __launch_bounds__(WARPS * 32) tma(long long* out, int P, int N) 
 #pragma unroll 4
     for (int j = 0; j < T / 32; ++j)
 #pragma unroll
-      for (int r = 0; r < R; ++r) s[r * T + j * 32 + lane] = (long long)(base + j * 32 + lane + r);
+      for (int r = 0; r < R; ++r)
+        s[r * T + j * 32 + lane] = store_value<V>((long long)(base + j * 32 + lane + r), row0 + r, base + j * 32 + lane);
     fence_async_smem();
     __syncwarp();
     if (lane == 0) {
@@ -122,6 +137,7 @@ __global__ void __launch_bounds__(WARPS * 32) tmacta(long long* out, int P, int 
   if (threadIdx.x == 0) bulk_wait_read<0>();
 }
 
+#ifndef STORE_PATTERN2_KERNELS_ONLY
 template <class F>
 float timeit(F f) {
   cudaEvent_t a, b;
@@ -224,3 +240,4 @@ int main(int argc, char** argv) {
   printf("status: %s\n", cudaGetErrorString(e));
   return 0;
 }
+#endif
