@@ -981,18 +981,21 @@ int rebuild_classes(bs_engine* e) {
   std::vector<uint64_t> fsel(e->n_fit_classes), ftol(e->n_fit_classes), rsel(e->n_rep_classes), rtol(e->n_rep_classes);
   std::vector<uint32_t> fnz(e->n_fit_classes), faff(e->n_fit_classes), raff(e->n_rep_classes);
   bool aff_bad = false, any_aff = false;
+  // Stale classes of earlier tables linger in both persistent indices and may name an affinity row the table of now
+  // does not have.  Only the classes in use are checked: a pod's fit and representative class carry its own affinity
+  // id and a group's representative class the group's, so the pods and groups below are checked, not the indices.  A
+  // stale class's bits are never read, so its out-of-range id goes to the device as no constraint: no kernel ever
+  // indexes the table with it (the walk's fit mask covers every representative class).
+  auto aff_row = [e](uint32_t a) { return a != BS_AFF_NONE && a >= e->n_aff ? BS_AFF_NONE : a; };
   for (uint32_t c = 0; c < e->n_fit_classes; ++c) {
     fsel[c] = e->fit_index.keys[c].sel; ftol[c] = e->fit_index.keys[c].tol; fnz[c] = e->fit_index.keys[c].nz;
-    faff[c] = e->fit_index.keys[c].aff;
-    aff_bad = aff_bad || (faff[c] != BS_AFF_NONE && faff[c] >= e->n_aff);
+    faff[c] = aff_row(e->fit_index.keys[c].aff);
   }
   for (uint32_t c = 0; c < e->n_rep_classes; ++c) {
-    rsel[c] = e->rep_index.keys[c].sel; rtol[c] = e->rep_index.keys[c].tol; raff[c] = e->rep_index.keys[c].aff;
-    any_aff = any_aff || raff[c] != BS_AFF_NONE;
+    rsel[c] = e->rep_index.keys[c].sel; rtol[c] = e->rep_index.keys[c].tol; raff[c] = aff_row(e->rep_index.keys[c].aff);
+    any_aff = any_aff || e->rep_index.keys[c].aff != BS_AFF_NONE;
   }
-  // (stale representative classes may linger in the persistent index; only the classes in use are checked, and
-  // every pod / group has its representative class in that index: no affinity id there, nothing to check)
-  if (any_aff) {
+  if (any_aff) {   // else no pod or group names an affinity class: nothing to check
     for (uint32_t p = 0; p < P && !aff_bad; ++p) {
       const uint32_t a = e->rep_index.keys[e->h_prc[p]].aff;
       aff_bad = a != BS_AFF_NONE && a >= e->n_aff;
@@ -1764,6 +1767,14 @@ int bs_upload_nodes(bs_engine* e, const bs_node_table* t) {
   const uint32_t N = t->n_nodes, L = e->L;
   const auto cols = node_cols(e, t);
   if (N && null_column(cols)) return fail(e, BS_E_INVAL, "bs_upload_nodes: null column");
+  // the old table goes before validation and the DMA, with what belongs to it: a table that fails either (BS_E_RANGE,
+  // or an error partway through the copy) leaves no snapshot behind, and the engine answers BS_E_STATE until a valid
+  // one arrives instead of evaluating the previous snapshot (or a half-written one)
+  e->have_nodes = false;
+  e->have_bound = false;   // the bound-pod table belongs to the node snapshot
+  if (e->n_aff) e->classes_dirty = true;   // class ids are validated again: the affinity table belongs to the
+  e->n_aff = 0;                            // node snapshot and goes with it
+  e->evaluated = false;
   HP_BEGIN(e);
   const NodeStats ns = node_host_pass(t, L, N);
   if (ns.bad_range) return fail(e, BS_E_RANGE, "bs_upload_nodes: value outside +-2^56");
@@ -1778,13 +1789,10 @@ int bs_upload_nodes(bs_engine* e, const bs_node_table* t) {
   e->h_nflags.assign(t->flags, t->flags + N);
   e->h_npc.assign(t->pod_count, t->pod_count + N);
   e->h_nrpres.assign(t->req_present, t->req_present + N);
-  e->have_bound = false;   // the bound-pod table belongs to the node snapshot
   e->node_stats = ns;
   e->N = N;
   e->score_pitch = (N + 1u) & ~1u;
   e->bitmap_pitch = (cdiv(N, 32) + 31u) & ~31u;
-  if (e->n_aff) e->classes_dirty = true;   // class ids are validated again: the affinity table belongs to the
-  e->n_aff = 0;                            // node snapshot and goes with it
   e->Npad = Npad;
   e->W = cdiv(N, 32);
   e->have_nodes = true;

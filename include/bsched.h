@@ -245,17 +245,26 @@ const char* bs_last_error(const bs_engine* e);
  *      PreFilter/Permit/Compare (core.go:88,268,368).  Host arrays are copied;
  *      nothing is retained.  The copy runs under the validation pass: a table
  *      that fails it (BS_E_RANGE) is dropped, and the engine answers BS_E_STATE
- *      until a valid table of that kind is uploaded. ---- */
+ *      until a valid table of that kind is uploaded.  A node table is dropped
+ *      with the affinity and bound-pod tables that belong to it, so a failed
+ *      bs_upload_nodes never leaves the previous snapshot live.  A wrong n_lanes
+ *      or a null column (BS_E_INVAL) is refused before anything is dropped,
+ *      except the node-snapshot side columns (bs_upload_nodes) and the pod-table
+ *      side columns (bs_upload_pods), which go first. ---- */
 int bs_upload_nodes(bs_engine* e, const bs_node_table* t);
 /* Incremental snapshot update: overwrite rows idx[0..t->n_nodes) of the uploaded node table with
  * the rows of `t` (a compact table of the changed nodes, same lane layout).  The snapshot's list
- * order and size do not change; between scheduling cycles only a few NodeInfos differ. */
+ * order and size do not change; between scheduling cycles only a few NodeInfos differ.  Every call
+ * drops the node-snapshot side columns first, also one that changes no row or then fails; a failing
+ * call (BS_E_INDEX for an index >= n_nodes, BS_E_RANGE) leaves every row and the bound-pod table as
+ * they were, and only a call that changes rows drops the bound-pod table. */
 int bs_update_nodes(bs_engine* e, const uint32_t* idx, const bs_node_table* t);
 int bs_upload_groups(bs_engine* e, const bs_group_table* t);
 /* The same for PodGroup state: overwrite rows idx[0..t->n_groups) of the uploaded group table.
  * Between cycles a few groups change (matched count, Status.Scheduled, the Scheduled / denied flags,
  * MinResources and the representative pod once the first pod arrived: cache.go:52-67); the table's
- * size and order stay. */
+ * size and order stay.  The bound-pod table stays (its group indices still hold); a failing call
+ * (BS_E_INDEX for an index >= n_groups, BS_E_RANGE) leaves every row as it was. */
 int bs_update_groups(bs_engine* e, const uint32_t* idx, const bs_group_table* t);
 int bs_upload_pods(bs_engine* e, const bs_pod_table* t);
 /* checkFit beyond bit masks (core.go:741-759 -> predicates.PodMatchNodeSelector).  sel_mask / label_mask
@@ -267,7 +276,8 @@ int bs_upload_pods(bs_engine* e, const bs_pod_table* t);
  * A pod fits a node iff the mask test AND its class's bit hold (bs_pod_table.aff_class, BS_AFF_NONE =
  * mask test only); the group's representative pod likewise (bs_group_table.rep_aff_class).  The table
  * belongs to the node snapshot: bs_upload_nodes drops it (upload nodes, then the table), n_classes = 0
- * clears it.  A class id >= n_classes at evaluation time is BS_E_INDEX. */
+ * clears it.  A class id >= n_classes at evaluation time is BS_E_INDEX; only the ids of the pod and group
+ * tables of now count, not those of tables uploaded before them. */
 int bs_upload_affinity(bs_engine* e, uint32_t n_classes, const uint32_t* bits);
 /* max_schedule_time: plugin arg (batchscheduler.go:71-75, util.GetWaitTimeDuration
  * k8s.go:82-91).  per_group_ns may be NULL; entries < 0 mean "unset". */

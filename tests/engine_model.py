@@ -1,0 +1,719 @@
+"""TEST INFRASTRUCTURE — a host model of one long-lived engine's logical state, and a seeded generator of call sequences.
+
+Model.apply(op) follows one call: it updates the tables, side columns and weights the engine keeps between calls and
+returns the error code the engine must answer (None for success).  The drop rules and check orders are
+include/bsched.h's; Model.expect(cfg) gives every output of a round on the current state from the existing CPU
+restatements only (the oracle, the reason rows, the priority lists, the lane classifier, the walks and preemption).
+
+generate(seed) is a list of ops: random uploads, row updates, side columns, weights, failing calls and rounds, plus
+the scripted bursts R1-R6 (every seed runs at least one; across seeds all of them):
+  R1  more than 4096 fit and representative classes, then a table with few (both persistent class indices clear),
+      then bs_update_groups with a new representative class, then a round;
+  R2  node tables of 0, 1, 511, 512, 513 and more nodes, growing and shrinking, every side uploaded again after each;
+  R3  one lane narrow -> scaled -> wide through row updates, a row put back (stays wide), a pod table that changes a
+      scaled lane's unit, a fresh node table (narrow again);
+  R4  each side dropped by the call that owns it: BS_E_STATE with its weight on, the lists without the term with it
+      off, and the term back once the side is uploaded again;
+  R5  a failing upload of each table kind, then a round;
+  R6  every list output at N = 0 and at P = 0 with every term on.
+"""
+from __future__ import annotations
+
+import numpy as np
+
+import fit_reasons_ref as frr
+import fit_shape_cases as fsc
+import interpod_priority_ref as ir
+import locality_priority_ref as lpr
+import preempt_ref
+import ratio_priority_ref as rr
+from oracle import oracle
+from randsnap import S, random_snapshot
+
+E_INVAL, E_RANGE, E_STATE, E_INDEX = -1, -5, -6, -8
+I64_MIN = np.iinfo(np.int64).min
+LIMIT = 1 << 56
+NODE_SIDES = ("nz_node", "pref_node", "loc_node", "spread_node", "ipa_node")
+POD_SIDES = ("nz_pod", "pref_pod", "loc_pod", "spread_pod", "ipa_pod")
+PW, LW, W_SPREAD, W_IPA = (1, 1), (1, 10000), 1, 1
+RATIO_ON = (2, rr.BIN_PACK, None, 1)   # lane weights filled in per lane count
+AFF = 3   # affinity classes of every generated table: pods and groups name classes 0..2 of each node upload's table
+
+
+def expected_topk(score, K):
+    """[P, N] oracle scores (INT64_MIN = does not fit) -> (nodes [P, K] int32, scores [P, K] int64): each row's fitting
+    entries by score descending, then node index ascending, cut to K, padded with node -1 and score INT64_MIN."""
+    P, N = score.shape
+    nodes = np.full((P, K), -1, np.int32)
+    scores = np.full((P, K), I64_MIN, np.int64)
+    if N == 0:
+        return nodes, scores
+    fit = score != I64_MIN
+    key = np.where(fit, score, -1)                     # fitting scores are >= 0
+    idx = np.broadcast_to(np.arange(N), (P, N))
+    order = np.lexsort((idx, -key), axis=1)[:, :K]
+    take = min(K, N)
+    ok = np.take_along_axis(fit, order, axis=1)
+    nodes[:, :take] = np.where(ok, order, -1)
+    scores[:, :take] = np.where(ok, np.take_along_axis(score, order, axis=1), I64_MIN)
+    return nodes, scores
+
+
+def _out_of_range(*arrays):
+    return any(np.size(a) and (np.abs(np.asarray(a, np.int64)) > LIMIT).any() for a in arrays)
+
+
+def _apply_rows(table, idx, rows):
+    """A copy of `table` with rows idx overwritten by the compact table `rows` (the same layout)."""
+    out = table.copy()
+    for f in out.__dataclass_fields__:
+        a, r = getattr(out, f), getattr(rows, f)
+        if a is None or r is None:
+            continue
+        if a.ndim == 2:
+            a[:, idx] = r
+        else:
+            a[idx] = r
+    return out
+
+
+def _max_class(cls, none):
+    c = np.asarray(cls, np.int64)
+    c = c[c != none]
+    return int(c.max()) if c.size else -1
+
+
+class Model:
+    """The logical state of one engine with `lanes` lanes (see the module docstring)."""
+
+    def __init__(self, lanes):
+        self.lanes = lanes
+        self.nodes = self.pods = self.groups = None
+        self.aff = None          # [n_aff, W] bits, or None (no table: n_aff = 0)
+        self.bound = None
+        self.history = []        # node tables replaced by row updates since the last full node upload
+        self.side = dict.fromkeys(NODE_SIDES + POD_SIDES)
+        self.weights = (1, 0, 1)
+        self.ratio = ir.NO_RATIO
+        self.pw, self.lw, self.w_spread, self.w_ipa = (0, 0), (0, 0), 0, 0
+
+    # ---- state ---------------------------------------------------------------------------------------------------
+    def snapshot(self):
+        return S.Snapshot(self.nodes, self.pods, self.groups, aff_bits=self.aff)
+
+    def complete(self):
+        return self.nodes is not None and self.pods is not None and self.groups is not None
+
+    def _drop(self, keys):
+        for k in keys:
+            self.side[k] = None
+
+    # ---- one call ------------------------------------------------------------------------------------------------
+    def apply(self, op):
+        kind = op["op"]
+        f = getattr(self, "_" + kind, None)
+        if f is None:
+            raise ValueError(kind)
+        return f(op)
+
+    def _upload_nodes(self, op):
+        nt = op["table"]
+        self._drop(NODE_SIDES)
+        self.bound, self.aff = None, None   # they belong to the snapshot, also to one that fails validation
+        if _out_of_range(nt.alloc, nt.requested):
+            self.nodes = None
+            return E_RANGE
+        self.nodes, self.history = nt, []
+        return None
+
+    def _update_nodes(self, op):
+        idx, rows = op["idx"], op["rows"]
+        if self.nodes is None:
+            return E_STATE
+        self._drop(NODE_SIDES)   # every call, also one that changes no row or fails (bsched.h bs_update_nodes)
+        if len(idx) == 0:
+            return None
+        if (np.asarray(idx) >= self.nodes.n).any():
+            return E_INDEX
+        if _out_of_range(rows.alloc, rows.requested):
+            return E_RANGE
+        self.history.append(self.nodes)
+        self.nodes = _apply_rows(self.nodes, idx, rows)
+        self.bound = None
+        return None
+
+    def _upload_groups(self, op):
+        gt = op["table"]
+        self.bound = None
+        if _out_of_range(gt.min_res):
+            self.groups = None
+            return E_RANGE
+        self.groups = gt
+        return None
+
+    def _update_groups(self, op):
+        idx, rows = op["idx"], op["rows"]
+        if self.groups is None:
+            return E_STATE
+        if len(idx) == 0:
+            return None
+        if (np.asarray(idx) >= self.groups.n).any():
+            return E_INDEX
+        if _out_of_range(rows.min_res):
+            return E_RANGE
+        self.groups = _apply_rows(self.groups, idx, rows)   # the bound-pod table stays
+        return None
+
+    def _upload_pods(self, op):
+        pt = op["table"]
+        self._drop(POD_SIDES)
+        if _out_of_range(pt.req):
+            self.pods = None
+            return E_RANGE
+        self.pods = pt
+        return None
+
+    def _upload_affinity(self, op):
+        if self.nodes is None:
+            return E_STATE
+        bits = op["bits"]
+        self.aff = None if bits is None or len(bits) == 0 else bits
+        return None
+
+    def _upload_bound(self, op):
+        if self.nodes is None:
+            return E_STATE
+        self.bound = op["table"]
+        return None
+
+    def _side(self, op):
+        """One half of a side: name (nz / pref / loc / spread / ipa), half (node / pod), cols, n (its length)."""
+        key = op["name"] + "_" + op["half"]
+        self.side[key] = None    # a failing call leaves the side dropped
+        table = self.nodes if op["half"] == "node" else self.pods
+        if table is None:
+            return E_STATE
+        if op["n"] != table.n:
+            return E_INVAL
+        self.side[key] = op["cols"]
+        return None
+
+    def _weights(self, op):
+        for k, v in op.items():
+            if k != "op":
+                setattr(self, k, v)
+        return None
+
+    def _evaluate(self, op):
+        """The engine's check order: the tables, then (priority lists only) the non-zero columns, the node
+        priorities, locality, spread and inter-pod, then the affinity class ids."""
+        if not self.complete():
+            return E_STATE
+        if op["priority"]:
+            sd = self.side
+            if sd["nz_node"] is None or sd["nz_pod"] is None:
+                return E_STATE
+            if any(self.pw):
+                if sd["pref_node"] is None or sd["pref_pod"] is None:
+                    return E_STATE
+                if self.pw[1] and _max_class(sd["pref_pod"][1], S.PREF_NONE) >= sd["pref_node"][1].shape[0]:
+                    return E_INDEX
+            rc = self._locality_check()
+            if rc:
+                return rc
+            if self.w_spread:
+                if sd["spread_node"] is None or sd["spread_pod"] is None:
+                    return E_STATE
+                if _max_class(sd["spread_pod"], S.SPREAD_NONE) >= sd["spread_node"][1].shape[0]:
+                    return E_INDEX
+            if self.w_ipa:
+                if sd["ipa_node"] is None or sd["ipa_pod"] is None:
+                    return E_STATE
+                if _max_class(sd["ipa_pod"][1][1], -1) >= len(sd["ipa_node"][2]):
+                    return E_INDEX
+        return self._affinity_check()
+
+    def _locality_check(self):
+        sd = self.side
+        if self.lw[0]:
+            if sd["loc_node"] is None or sd["loc_pod"] is None:
+                return E_STATE
+            cls, off, ids, _ = sd["loc_pod"]
+            if _max_class(cls, S.IMAGE_NONE) >= len(off) - 1 or _max_class(ids, -1) >= len(sd["loc_node"][0]):
+                return E_INDEX
+        if self.lw[1] and (sd["loc_node"] is None or sd["loc_pod"] is None):
+            return E_STATE
+        return None
+
+    def _affinity_check(self):
+        n_aff = 0 if self.aff is None else len(self.aff)
+        for a in (self.pods.aff_class, self.groups.rep_aff):
+            if a is not None and _max_class(a, S.AFF_NONE) >= n_aff:
+                return E_INDEX
+        return None
+
+    def _replay(self, op):
+        if op["priority"] and (any(self.pw) or self.w_spread or self.w_ipa):
+            return E_INVAL     # bs_replay_priority refuses these weights before anything else
+        if not self.complete():
+            return E_STATE
+        if op["priority"]:
+            if self.side["nz_node"] is None or self.side["nz_pod"] is None:
+                return E_STATE
+            rc = self._locality_check() if any(self.lw) else None
+            if rc:
+                return rc
+        return self._affinity_check()
+
+    def _preempt(self, op):
+        if not self.complete() or self.bound is None:
+            return E_STATE
+        n_aff = 0 if self.aff is None else len(self.aff)
+        if self.pods.aff_class is not None and _max_class(self.pods.aff_class, S.AFF_NONE) >= n_aff:
+            return E_INDEX
+        return None
+
+    # ---- what a round gives ----------------------------------------------------------------------------------------
+    def priority_rows(self, K, pods=None):
+        sd, snap = self.side, self.snapshot()
+        N, P = self.nodes.n, self.pods.n
+        zero = (([1], [np.zeros(N)], [0], [], [], ([0], [], [], [])), (np.full(P, S.IPA_NONE), ([0], [], [], [])))
+        interpod = (sd["ipa_node"], sd["ipa_pod"]) if self.w_ipa else zero
+        prefs = sd["pref_node"] + sd["pref_pod"] if any(self.pw) else None
+        loc = (sd["loc_node"], sd["loc_pod"]) if any(self.lw) else None
+        spread = (sd["spread_node"], sd["spread_pod"]) if self.w_spread else None
+        ratio = self.ratio_setting()
+        return ir.priority_rows(snap, sd["nz_node"], sd["nz_pod"], K, interpod, self.w_ipa, ratio, self.weights, prefs,
+                                self.pw, loc, self.lw, spread, self.w_spread, pods=pods)
+
+    def ratio_setting(self):
+        return self.ratio if self.ratio[0] else ir.NO_RATIO
+
+    def expect(self, cfg):
+        """Every output of a round on this state for an engine built with cfg (score, fit_bitmap, filter, reasons,
+        topk, priority_k): a dict of arrays, keyed as the GPU test reads them back."""
+        snap = self.snapshot()
+        orc = oracle.round(snap, want_bitmap=True, want_score=True, want_filter=cfg.get("filter", False))
+        out = {f: getattr(orc, f) for f in ("prefilter", "feasible_count", "best_node", "best_score", "admit",
+                                             "admit_bitmap", "new_denied", "order", "rank")}
+        out["max_group"], out["max_finished"] = orc.max_group, orc.max_finished
+        if cfg.get("fit_bitmap"):
+            out["fit_rows"] = orc.fit_bitmap
+        if cfg.get("score"):
+            out["score_rows"] = orc.score
+        if cfg.get("filter"):
+            out["filter_rows"], out["filter_code"] = orc.filter_bitmap, orc.filter_code
+        if cfg.get("topk"):
+            out["topk_nodes"], out["topk_scores"] = expected_topk(orc.score, cfg["topk"])
+        if cfg.get("reasons"):
+            out["reason_rows"] = frr.fit_reasons(snap)
+        if cfg.get("priority_k"):
+            out["priority_nodes"], out["priority_scores"] = self.priority_rows(cfg["priority_k"])
+        out["lanes"] = fsc.classify(self.nodes, self.pods, self.history)
+        return out
+
+    def expect_walk(self, priority, queue):
+        snap = self.snapshot()
+        if priority:
+            sd = self.side
+            loc = (sd["loc_node"], sd["loc_pod"]) if any(self.lw) else \
+                ((np.zeros(0, np.int64), np.zeros((0, (self.nodes.n + 31) // 32), np.uint32),
+                  np.zeros(self.nodes.n, np.uint64)),
+                 (np.full(self.pods.n, S.IMAGE_NONE, np.uint32), np.zeros(1, np.uint32), np.zeros(0, np.uint32),
+                  np.full(self.pods.n, S.AVOID_NONE, np.uint8)))
+            pf, node, ready, _, _ = lpr.replay_locality(snap, sd["nz_node"], sd["nz_pod"], loc, self.lw,
+                                                        self.ratio_setting(), queue, self.weights)
+        else:
+            pf, node, ready, _ = oracle.replay(snap, queue)
+        return {"prefilter": pf, "node": node, "ready": ready}
+
+    def expect_preempt(self, pods):
+        r = preempt_ref.preempt(self.snapshot(), self.bound, pods)
+        return {"node": r.node, "n_victims": r.n_victims, "n_candidates": r.n_candidates,
+                "victims": np.concatenate([r.victims_of(i) for i in range(len(pods))] + [np.zeros(0, np.uint32)])}
+
+
+# ---- the generator -----------------------------------------------------------------------------------------------
+
+def describe(op):
+    """One line per op for a failure report."""
+    parts = [op["op"]]
+    for k, v in op.items():
+        if k == "op":
+            continue
+        if hasattr(v, "n") and hasattr(v, "lanes"):
+            parts.append(f"{k}=<{type(v).__name__} n={v.n}>")
+        elif isinstance(v, np.ndarray):
+            parts.append(f"{k}=<{v.dtype}[{','.join(map(str, v.shape))}]>")
+        elif k == "cols":
+            parts.append("cols=...")
+        else:
+            parts.append(f"{k}={v!r}")
+    return " ".join(parts)
+
+
+class Generator:
+    """Seeded op sequences over one lane count; the burst methods append scripted regimes."""
+
+    def __init__(self, seed, lanes=6):
+        self.seed, self.L = seed, lanes
+        self.rng = np.random.default_rng(seed)
+        self.model = Model(lanes)   # the generator's own copy: side columns are built on the state of now
+        self.ops = []
+        self.regimes = set()
+        self.max_p = 0
+
+    def _k(self):
+        return int(self.rng.integers(0, 1 << 30))
+
+    def emit(self, op):
+        self.model.apply(op)
+        self.ops.append(op)
+        return op
+
+    # -- tables --
+    def snap(self, P, N, G, aff=0, case=None):
+        return random_snapshot(self._k(), P=P, N=N, G=G, L=self.L, case=case or str(self.rng.choice(["mixed", "A", "B"])),
+                               aff=aff)
+
+    def upload_nodes(self, N, aff=AFF):
+        s = self.snap(1, N, 1, aff=aff)
+        self.emit({"op": "upload_nodes", "table": s.nodes})
+        if aff and s.aff_bits is not None:
+            self.emit({"op": "upload_affinity", "bits": s.aff_bits})
+
+    def upload_pods(self, P, aff=AFF):
+        m = self.model
+        G = m.groups.n if m.groups is not None else 8
+        s = self.snap(P, 1, max(G, 1), aff=aff)
+        pt = s.pods
+        if G == 0:
+            pt.gid[:] = np.where(pt.gid >= 0, 3, pt.gid)   # out-of-range gids: the oracle treats them as missing
+        self.max_p = max(self.max_p, P)
+        self.emit({"op": "upload_pods", "table": pt})
+
+    def upload_groups(self, G, aff=AFF):
+        s = self.snap(1, 1, G, aff=aff)
+        self.emit({"op": "upload_groups", "table": s.groups})
+
+    def update_nodes(self, mode):
+        m = self.model
+        N = m.nodes.n
+        k = int(self.rng.integers(1, min(N, 9) + 1))
+        idx = np.sort(self.rng.choice(N, k, replace=False)).astype(np.uint32)
+        rows = m.nodes.take(idx).copy()
+        if mode == "widen":
+            rows.alloc[0, 0] = 1 << 40
+        elif mode == "back":
+            rows = self._first.take(idx).copy() if getattr(self, "_first", None) is not None and \
+                self._first.n == N else rows
+        elif mode == "flags":
+            rows.flags[:] = self.rng.choice([0, S.NODE_UNSCHEDULABLE, S.NODE_NIL, S.NODE_TAINTS_ERR], k)
+        elif mode == "labels":
+            rows.label_mask[:] = self.rng.integers(0, 16, k)
+            rows.taint_mask[:] = self.rng.integers(0, 4, k)
+        self.emit({"op": "update_nodes", "idx": idx, "rows": rows, "mode": mode})
+
+    def update_groups(self, mode):
+        m = self.model
+        G = m.groups.n
+        k = int(self.rng.integers(1, min(G, 6) + 1))
+        idx = np.sort(self.rng.choice(G, k, replace=False)).astype(np.uint32)
+        rows = m.groups.take(idx).copy()
+        if mode == "rep":
+            rows.rep_sel[0] = np.uint64(0xF0F0 + int(self.rng.integers(0, 1 << 12)))
+            rows.flags[0] |= S.GROUP_HAS_POD
+        else:
+            rows.creation_ns[0] = np.int64(1) << int(self.rng.integers(40, 62))
+            rows.matched[:] = self.rng.integers(0, 3, k)
+        self.emit({"op": "update_groups", "idx": idx, "rows": rows})
+
+    # -- sides --
+    def side(self, name, half, mismatch=False, wrong_len=False):
+        m = self.model
+        table = m.nodes if half == "node" else m.pods
+        if table is None:
+            return
+        snap = S.Snapshot(m.nodes if m.nodes is not None else S.NodeTable.empty(0, self.L),
+                          m.pods if m.pods is not None else S.PodTable.empty(0, self.L),
+                          m.groups if m.groups is not None else S.GroupTable.empty(0, self.L))
+        k = self._k()
+        if name == "nz":
+            cols = S.nonzero_requests(snap, k)[0 if half == "node" else 1]
+            n = cols.shape[1]
+        elif name == "pref":
+            c = S.node_preferences(snap, k, n_classes=2 if mismatch else 5)
+            cols = (c[0], c[1]) if half == "node" else (c[2], c[3])
+            n = len(cols[0])
+        elif name == "loc":
+            node, pods = S.node_locality(snap, k, n_images=3 if mismatch else 16)
+            cols = node if half == "node" else pods
+            n = len(node[2]) if half == "node" else len(pods[0])
+        elif name == "spread":
+            node, pods = S.node_spread(snap, k, n_classes=2 if mismatch else 6)
+            cols = node if half == "node" else pods
+            n = len(node[0]) if half == "node" else len(pods)
+        else:
+            node, pods = S.node_interpod(snap, k, n_terms=3 if mismatch else 24)
+            cols = node if half == "node" else pods
+            n = table.n
+        if wrong_len and name in ("nz", "spread"):   # one entry too many
+            n += 1
+            if name == "nz":
+                cols = np.concatenate([cols, np.zeros((2, 1), np.int64)], axis=1)
+            elif half == "node":
+                cols = (np.r_[cols[0], np.uint8(S.ZONE_NONE)].astype(np.uint8),
+                        np.concatenate([cols[1], np.zeros((cols[1].shape[0], 1), np.int32)], axis=1))
+            else:
+                cols = np.r_[cols, np.uint32(S.SPREAD_NONE)].astype(np.uint32)
+        self.emit({"op": "side", "name": name, "half": half, "n": n, "cols": cols, "wrong_len": wrong_len})
+
+    def all_sides(self, halves=("node", "pod")):
+        for name in ("nz", "pref", "loc", "spread", "ipa"):
+            for half in halves:
+                self.side(name, half)
+
+    def node_sides(self):
+        """The node halves again, as a caller does after bs_update_nodes dropped them."""
+        self.all_sides(("node",))
+
+    def weights(self, on):
+        L = self.L
+        ratio = (RATIO_ON[0], RATIO_ON[1], [1, 1, 0, 0] + [1] * (L - 4), RATIO_ON[3]) if on else ir.NO_RATIO
+        self.emit({"op": "weights", "weights": (1, 0, 1) if on else (2, 1, 3), "ratio": ratio,
+                   "pw": PW if on else (0, 0), "lw": LW if on else (0, 0), "w_spread": W_SPREAD if on else 0,
+                   "w_ipa": W_IPA if on else 0})
+
+    def round(self, how=None):
+        how = how or str(self.rng.choice(["evaluate", "view", "async"]))
+        self.emit({"op": "evaluate", "how": how, "priority": True})
+
+    def walk(self, kind):
+        if kind == "preempt":
+            if self.model.complete() and self.model.nodes is not None and self.model.groups is not None:
+                self.emit({"op": "upload_bound", "table": S.bound_pods(self.model.snapshot(), self._k(), max_per_node=6)})
+            self.emit({"op": "preempt", "pods": np.arange(min(self.model.pods.n if self.model.pods is not None else 0, 40),
+                                                         dtype=np.uint32)})
+        else:
+            self.emit({"op": "replay", "priority": kind == "priority"})
+
+    def base(self, P=150, N=300, G=20):
+        self.upload_nodes(N)
+        self.upload_groups(G)
+        self.upload_pods(P)
+        self.all_sides()
+        self.weights(on=True)
+        self.round()
+
+    # -- the scripted bursts --
+    def r1(self):
+        """Both persistent class indices past 4096 classes, then a small table that clears them, then a group row
+        update whose new representative class is looked up in place in the cleared index."""
+        self.upload_nodes(64)
+        self.upload_groups(40)
+        s = self.snap(5000, 1, 40)
+        pt = s.pods
+        pt.sel_mask = (self.rng.integers(0, 1 << 62, pt.n).astype(np.uint64) & np.uint64(~0xF & (2**64 - 1))) | \
+            self.rng.integers(0, 16, pt.n).astype(np.uint64)
+        pt.sel_mask[::5] = 0
+        pt.tol_mask = self.rng.integers(0, 1 << 40, pt.n).astype(np.uint64)
+        self.emit({"op": "upload_pods", "table": pt})
+        self.all_sides()
+        self.round("evaluate")
+        self.upload_pods(60)
+        self.all_sides()
+        self.round()            # the groups' ids are assigned again in the cleared index
+        self.update_groups("rep")
+        self.round()            # ... so this update looks its new class up in place
+        self.regimes.add("R1")
+
+    def r2(self):
+        for N in (0, 1, 511, 512, 513, 700, 64, 513, 0, 300):
+            self.upload_nodes(N)
+            self.all_sides()
+            self.round()
+        self.regimes.add("R2")
+
+    def r3(self):
+        self.upload_nodes(200)
+        self._first = self.model.nodes
+        self.all_sides()
+        self.round()
+        m = self.model
+        # narrow -> scaled: a lane's values grow past the narrow limit in whole multiples of 2^20
+        idx = np.arange(0, 200, 17, dtype=np.uint32)
+        rows = m.nodes.take(idx).copy()
+        rows.alloc[2] = (np.int64(1) << 40) + (np.arange(len(idx), dtype=np.int64) << 20)
+        rows.requested[2] = 0
+        self.emit({"op": "update_nodes", "idx": idx, "rows": rows, "mode": "scaled"})
+        self.node_sides()
+        self.round()
+        rows = rows.copy()
+        rows.alloc[2, 0] += 1   # an odd value: scaled -> wide
+        self.emit({"op": "update_nodes", "idx": idx, "rows": rows, "mode": "wide"})
+        self.node_sides()
+        self.round()
+        self.emit({"op": "update_nodes", "idx": idx, "rows": self._first.take(idx), "mode": "row back"})   # stays wide
+        self.node_sides()
+        self.round()
+        s = self.snap(m.pods.n if m.pods is not None else 100, 1, m.groups.n if m.groups is not None else 10, aff=AFF)
+        s.pods.req[2] = np.where(self.rng.random(s.pods.n) < 0.3, np.int64(1) << 41, 0)
+        if m.groups is None:
+            self.upload_groups(10)
+        self.emit({"op": "upload_pods", "table": s.pods})   # a pod table that moves a scaled lane's unit
+        self.all_sides()
+        self.round()
+        self.upload_nodes(200)   # a fresh table: narrow again
+        self.all_sides()
+        self.round()
+        self.regimes.add("R3")
+
+    def r4(self):
+        self.base()
+        self.round()
+        m = self.model
+        idx = np.array([0], np.uint32)
+        owners = [("nz", "node", lambda: self.emit({"op": "update_nodes", "idx": idx, "rows": m.nodes.take(idx)})),
+                  ("pref", "node", lambda: self.emit({"op": "update_nodes", "idx": idx, "rows": m.nodes.take(idx)})),
+                  ("loc", "pod", lambda: self.emit({"op": "upload_pods", "table": m.pods})),
+                  ("spread", "node", lambda: self.emit({"op": "upload_nodes", "table": m.nodes})),
+                  ("ipa", "pod", lambda: self.emit({"op": "upload_pods", "table": m.pods}))]
+        for name, half, drop in owners:
+            drop()
+            self.all_sides_but(name)
+            self.round()            # BS_E_STATE while the weight is on (the non-zero columns: always)
+            if name != "nz":
+                self.emit({"op": "weights", **self._off(name)})
+                self.round()        # the lists without the term
+            self.side(name, "node")
+            self.side(name, "pod")
+            self.weights(on=True)
+            self.round()            # the term back
+        self.regimes.add("R4")
+
+    def _off(self, name):
+        return {"pref": {"pw": (0, 0)}, "loc": {"lw": (0, 0)}, "spread": {"w_spread": 0}, "ipa": {"w_ipa": 0}}[name]
+
+    def all_sides_but(self, skip):
+        for name in ("nz", "pref", "loc", "spread", "ipa"):
+            if name == skip:
+                continue
+            for half in ("node", "pod"):
+                if self.model.side[name + "_" + half] is None:
+                    self.side(name, half)
+
+    def r5(self):
+        self.base()
+        m = self.model
+        bad = m.nodes.copy()
+        if bad.n:
+            bad.requested[0, bad.n // 2] = LIMIT + 1
+        else:
+            bad = self.snap(1, 5, 1).nodes
+            bad.alloc[1, 2] = -LIMIT - 1
+        self.emit({"op": "upload_nodes", "table": bad})
+        self.round()                 # BS_E_STATE, never a round on the previous snapshot
+        self.emit({"op": "update_nodes", "idx": np.zeros(1, np.uint32), "rows": bad.take([0])})
+        self.upload_nodes(250)
+        self.all_sides()
+        self.round()
+        bad = m.groups.copy()
+        bad.min_res[0, 0] = -(LIMIT + 1)
+        self.emit({"op": "upload_groups", "table": bad})
+        self.round()
+        self.upload_groups(12)
+        bad = m.pods.copy()
+        bad.req[1, -1] = LIMIT + 1
+        self.emit({"op": "upload_pods", "table": bad})
+        self.round()
+        self.upload_pods(100)
+        self.all_sides()
+        self.round()
+        self.regimes.add("R5")
+
+    def r6(self):
+        self.upload_nodes(0)
+        self.upload_groups(10)
+        self.upload_pods(80)
+        self.all_sides()
+        self.weights(on=True)
+        self.round()
+        self.upload_nodes(130)
+        self.upload_groups(0)
+        self.upload_pods(0)
+        self.all_sides()
+        self.round()
+        self.upload_groups(7)
+        self.upload_pods(90)
+        self.all_sides()
+        self.round()
+        self.regimes.add("R6")
+
+    # -- random ops --
+    def random_op(self):
+        m = self.model
+        r = self.rng.random()
+        if m.nodes is None or m.pods is None or m.groups is None:
+            self.base()
+        elif r < 0.10:   # without its affinity table now and then: the pods' classes are BS_E_INDEX until it comes
+            self.upload_nodes(int(self.rng.choice([1, 33, 511, 512, 513, 900])), aff=AFF if self.rng.random() < 0.85 else 0)
+            self.all_sides(("node",))
+        elif r < 0.18:
+            self.upload_pods(int(self.rng.choice([0, 1, 70, self.max_p + 13])), aff=AFF if self.rng.random() < 0.8 else 0)
+            self.all_sides(("pod",))
+        elif r < 0.22:
+            self.upload_groups(int(self.rng.choice([0, 1, 9, 31])), aff=AFF if self.rng.random() < 0.8 else 0)
+        elif r < 0.34 and m.nodes.n:
+            self.update_nodes(str(self.rng.choice(["widen", "back", "flags", "labels"])))
+            if self.rng.random() < 0.85:   # else the next rounds answer BS_E_STATE until a side op brings them back
+                self.node_sides()
+                self.round()
+        elif r < 0.42 and m.groups.n:
+            self.update_groups(str(self.rng.choice(["rep", "creation"])))
+            self.round()
+        elif r < 0.50:   # a new table (the nodes' class fits change), or none (the pods' classes are out of range)
+            bits = self.snap(1, m.nodes.n, 1, aff=AFF).aff_bits if self.rng.random() < 0.75 else None
+            self.emit({"op": "upload_affinity", "bits": bits})
+            self.round()
+        elif r < 0.62:
+            name = str(self.rng.choice(["nz", "pref", "loc", "spread", "ipa"]))
+            half = str(self.rng.choice(["node", "pod"]))
+            self.side(name, half, mismatch=self.rng.random() < 0.3, wrong_len=self.rng.random() < 0.1)
+        elif r < 0.70:
+            self.weights(on=bool(self.rng.random() < 0.6))
+        elif r < 0.76:
+            kind = str(self.rng.choice(["nodes", "groups", "pods", "index"]))
+            if kind == "index" and m.nodes.n:
+                self.emit({"op": "update_nodes", "idx": np.array([m.nodes.n], np.uint32), "rows": m.nodes.take([0])})
+            elif kind == "groups":
+                bad = m.groups.copy()
+                if bad.n:
+                    bad.min_res[1, -1] = LIMIT + 1
+                self.emit({"op": "upload_groups", "table": bad})
+            elif kind == "pods" and m.pods.n:
+                bad = m.pods.copy()
+                bad.req[0, 0] = -(LIMIT + 1)
+                self.emit({"op": "upload_pods", "table": bad})
+        elif r < 0.84:
+            self.walk(str(self.rng.choice(["first_fit", "priority", "preempt"])))
+        else:
+            self.round()
+
+
+BURSTS = ("r1", "r2", "r3", "r4", "r5", "r6")
+
+
+def generate(seed, n_ops=30, lanes=None):
+    """(ops, regimes): about n_ops random ops around one scripted burst (seed % 6 picks it; seeds >= 6 add another),
+    every op as the dict Model.apply takes; regimes names the bursts the sequence ran."""
+    g = Generator(seed, lanes or [5, 6, 9][seed % 3])
+    bursts = [BURSTS[seed % 6]] + ([BURSTS[(seed // 6 + seed) % 6]] if seed >= 6 else [])
+    at = sorted(int(x) for x in g.rng.integers(0, n_ops, len(bursts)))
+    g.base()
+    for i in range(n_ops):
+        while at and at[0] == i:
+            getattr(g, bursts.pop(0))()
+            at.pop(0)
+        g.random_op()
+    g.round()
+    return g.ops, g.regimes, g.L

@@ -56,7 +56,8 @@ def _lib():
 def _columns(prefs, n_nodes):
     taints, table, tol, cls = prefs
     taints = np.ascontiguousarray(taints, dtype=np.uint64)
-    table = np.ascontiguousarray(table, dtype=np.int32).reshape(-1, n_nodes)
+    table = np.ascontiguousarray(table, dtype=np.int32)
+    table = table.reshape(len(table) if table.ndim == 2 else -1, n_nodes)   # [C, 0] for an empty node table
     tol = np.ascontiguousarray(tol, dtype=np.uint64)
     cls = np.ascontiguousarray(cls, dtype=np.uint32)
     return taints, table, tol, cls

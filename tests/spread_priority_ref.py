@@ -69,7 +69,8 @@ class Columns:
     def __init__(self, spread, n_nodes, w):
         (zone, counts), cls = spread
         self.arrays = [np.ascontiguousarray(zone, dtype=np.uint8).reshape(n_nodes),
-                       np.ascontiguousarray(counts, dtype=np.int32).reshape(-1, n_nodes),
+                       np.ascontiguousarray(counts, dtype=np.int32).reshape(np.shape(counts)[0] if np.ndim(counts) == 2 else -1,
+                                                                          n_nodes),
                        np.ascontiguousarray(cls, dtype=np.uint32)]
         self.q = _Spread(*(a.ctypes.data for a in self.arrays), w)
 

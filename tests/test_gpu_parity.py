@@ -178,7 +178,7 @@ def test_mirrors_prefilter_permit_less(pkg, oracle, snapshot_mod):
     eng.close()
 
 
-def test_value_range_rejected(pkg, snapshot_mod):
+def test_value_range_rejected(pkg, oracle, snapshot_mod):
     snap = snapshot_mod.readme_scenario()
     snap.nodes.alloc[1, 0] = (1 << 56) + 1
     eng = pkg.Engine(snap.lanes)
@@ -203,6 +203,29 @@ def test_value_range_rejected(pkg, snapshot_mod):
     eng.upload_groups(snap.groups)
     assert (eng.evaluate().prefilter == 0).all()
     eng.close()
+    # the same for a node table on an engine that already holds one: the old snapshot, its affinity table and its
+    # bound-pod table go with the failed upload, and no round answers from them
+    snap = random_snapshot(182, P=60, N=40, G=6, L=5, aff=2)
+    eng = pkg.Engine(snap.lanes)
+    eng.upload(snap)
+    eng.upload_bound_pods(snapshot_mod.bound_pods(snap, 182))
+    eng.evaluate()
+    bad = snap.nodes.copy()
+    bad.requested[0, 7] = (1 << 56) + 1
+    calls = [lambda: eng.upload_nodes(bad), eng.evaluate, lambda: eng.update_nodes([0], snap.nodes.take([0])),
+             lambda: eng.upload_affinity(snap.aff_bits), lambda: eng.preempt(np.arange(snap.pods.n))]
+    for k, call in enumerate(calls):
+        with pytest.raises(pkg.capi.BsError) as ei:
+            call()
+        assert ei.value.code == (pkg.capi.BS_E_RANGE if k == 0 else pkg.capi.BS_E_STATE), k
+    eng.upload_nodes(snap.nodes)      # a valid table again: the affinity table has to follow it
+    with pytest.raises(pkg.capi.BsError) as ei:
+        eng.evaluate()
+    assert ei.value.code == pkg.capi.BS_E_INDEX
+    eng.upload_affinity(snap.aff_bits)
+    res = eng.evaluate()
+    eng.close()
+    assert_round_equal(res, None, None, oracle.round(snap))
 
 
 def test_reupload_and_reevaluate(pkg, oracle, snapshot_mod):
@@ -565,6 +588,26 @@ def test_affinity_semantics(pkg, oracle):
             eng.evaluate()
     finally:
         eng.close()
+
+
+def test_stale_affinity_classes_do_not_count(pkg, oracle):
+    """The engine's class indices outlive pod tables, so classes of an earlier table keep affinity ids that the table
+    of now need not have.  A pod table without affinity classes, after a node upload that dropped the affinity table,
+    evaluates and walks as on a fresh engine."""
+    eng = pkg.Engine(5, 0)
+    try:
+        eng.upload(random_snapshot(41, P=90, N=60, G=8, L=5, aff=3))
+        eng.evaluate()
+        plain = random_snapshot(42, P=70, N=60, G=8, L=5)
+        eng.upload(plain)
+        res = eng.evaluate()
+        walk = eng.replay(res.order)
+    finally:
+        eng.close()
+    assert_round_equal(res, None, None, oracle.round(plain))
+    pf, node, ready, _ = oracle.replay(plain, res.order)
+    assert np.array_equal(walk["prefilter"], pf) and np.array_equal(walk["node"], node)
+    assert np.array_equal(walk["ready"], ready)
 
 
 def test_view_results_match_copies(pkg, oracle, snapshot_mod):
