@@ -42,9 +42,10 @@ IPA_CLASS_MAX = 64        # BS_IPA_CLASS_MAX: entries of one class
 IPA_OWN_MAX = 1 << 16     # BS_IPA_OWN_MAX: largest |own| of one entry
 IPA_TERM_MAX_BYTES = 1 << 30    # BS_IPA_TERM_MAX_BYTES: cap of the (term, value) M / S tables
 IPA_TABLE_MAX_BYTES = 1 << 30   # BS_IPA_TABLE_MAX_BYTES: cap of the pod class x node raw table
-# core.PreemptRemovePod verdicts (bs_remove_code) and the bound-pod flag
+# core.PreemptRemovePod verdicts (bs_remove_code) and the bound-pod flags
 REMOVE_ALLOW, REMOVE_OFFLINE_ONLINE, REMOVE_NOT_FOUND, REMOVE_LOCKED, REMOVE_SAME_GROUP = range(5)
 BOUND_GROUP_LOCKED = 0x01
+BOUND_PDB_VIOLATING = 0x02
 FILTER_PASS, FILTER_NOT_FOUND, FILTER_NOT_ENOUGH, FILTER_NO_SNAPSHOT, FILTER_REF_PANIC = range(5)
 BUF_FIT_BITMAP, BUF_SCORE, BUF_ADMIT_BITMAP, BUF_PREFILTER, BUF_ADMIT, BUF_ORDER, BUF_GATHERED_ADMIT = range(7)
 K_NODE_LEFT, K_FIND_MAX, K_CLASS_PREFIX, K_PREFILTER, K_GANG_FIT, K_SORT, K_FILTER, K_PEER, K_REPLAY, K_REASONS, K_COUNT = \

@@ -529,7 +529,7 @@ struct bs_engine {
   std::vector<uint8_t> h_bflags;
   std::vector<int32_t> h_npc;         // node pod_count and req_present as uploaded (bound-table validation)
   std::vector<uint32_t> h_nrpres;
-  DevBuf d_brow, d_bprio, d_bstart, d_bgid, d_bflags, d_bidx, d_breq, d_bsuf, d_bsuf_online, d_bsuf_bad;
+  DevBuf d_brow, d_bprio, d_bstart, d_bgid, d_bflags, d_bidx, d_breq, d_bsuf, d_bsuf_online, d_bsuf_bad, d_bsuf_vio;
   DevBuf d_pl_left, d_pl_present;
   // bs_preempt scratch
   DevBuf d_pp, d_ptiles, d_pnode, d_pnv, d_pcand, d_poff, d_pvict;
@@ -2811,6 +2811,7 @@ int bs_upload_bound_pods(bs_engine* e, const bs_bound_table* t) {
   CK(e->d_bsuf.ensure((size_t)L * Vp * 8));
   CK(e->d_bsuf_online.ensure(Vp * 4));
   CK(e->d_bsuf_bad.ensure(Vp * 4));
+  CK(e->d_bsuf_vio.ensure(Vp * 4));
   // the residuals the bound table is read against: node_left_kernel with no lane-class tables, into buffers of
   // its own (the round's tables stay as they are)
   CK(e->d_pl_left.ensure((size_t)L * e->Npad * 8));
@@ -2819,7 +2820,8 @@ int bs_upload_bound_pods(bs_engine* e, const bs_bound_table* t) {
     preempt_prep_kernel<<<cdiv(N, 256), 256, 0, e->s>>>(e->d_brow.as<uint32_t>(), e->d_bgid.as<int32_t>(),
                                                        e->d_bflags.as<uint8_t>(), e->d_breq.as<int64_t>(),
                                                        e->d_bsuf.as<int64_t>(), e->d_bsuf_online.as<uint32_t>(),
-                                                       e->d_bsuf_bad.as<uint32_t>(), N, (uint32_t)Vp, L);
+                                                       e->d_bsuf_bad.as<uint32_t>(), e->d_bsuf_vio.as<uint32_t>(), N,
+                                                       (uint32_t)Vp, L);
     ++e->launches;
   }
   node_left_kernel<<<cdiv(e->Npad, 256), 256, 0, e->s>>>(node_tab(e), LaneMap{}, nullptr, nullptr,
@@ -2869,7 +2871,8 @@ int bs_preempt(bs_engine* e, const uint32_t* pods, uint32_t n, bs_preempt_result
   a.left_present = e->d_pl_present.as<uint32_t>();
   a.b = BoundTab{e->d_brow.as<uint32_t>(), e->d_bprio.as<int32_t>(), e->d_bstart.as<int64_t>(), e->d_bgid.as<int32_t>(),
                  e->d_bflags.as<uint8_t>(), e->d_bidx.as<uint32_t>(), e->d_breq.as<int64_t>(), e->d_bsuf.as<int64_t>(),
-                 e->d_bsuf_online.as<uint32_t>(), e->d_bsuf_bad.as<uint32_t>(), std::max(e->V, 1u)};
+                 e->d_bsuf_online.as<uint32_t>(), e->d_bsuf_bad.as<uint32_t>(), e->d_bsuf_vio.as<uint32_t>(),
+                 std::max(e->V, 1u)};
   a.pp = e->d_pp.as<PreemptPod>();
   a.preq = e->d_req.as<int64_t>();
   a.preq_present = e->d_ppres.as<uint32_t>();

@@ -1475,6 +1475,11 @@ void BatchSchedulingPlugin::SetSpreadSelectors(SpreadSelectors selectors) {
   spread_selectors_ = std::move(selectors);
 }
 
+void BatchSchedulingPlugin::SetPodDisruptionBudgets(std::vector<PodDisruptionBudget> pdbs) {
+  std::lock_guard<std::mutex> lk(mu_);
+  pdbs_ = std::move(pdbs);
+}
+
 void BatchSchedulingPlugin::SetSelectorSpreadWeight(uint32_t selector_spread) {
   std::lock_guard<std::mutex> lk(mu_);
   spread_weight_ = selector_spread;
@@ -2036,8 +2041,18 @@ bs_bound_table PackedBound::table() const {
 
 Status BatchSchedulingPlugin::PackBoundPods(const PackedSnapshot& ctx, const std::vector<const NodeInfo*>& snapshot,
                                             const std::unordered_map<std::string, uint32_t>& group_row,
-                                            const std::vector<uint8_t>& locked, PackedBound* out) {
+                                            const std::vector<uint8_t>& locked, PackedBound* out,
+                                            const std::vector<PodDisruptionBudget>& pdbs) {
   if (!out) return Status{BS_CODE_ERROR, "PackBoundPods: null output"};
+  // filterPodsWithPDBViolation: only a budget that allows no disruption can make a pod violating; its selector is
+  // converted once here.  A nil or empty selector matches nothing, and one that fails to convert is skipped.
+  std::vector<std::pair<const std::string*, SpreadSel>> exhausted;
+  for (const PodDisruptionBudget& pdb : pdbs) {
+    SpreadSel sel;
+    if (pdb.disruptions_allowed > 0 || !pdb.has_selector || !sel_from_label_selector(pdb.selector, &sel) || sel.empty())
+      continue;
+    exhausted.emplace_back(&pdb.ns, std::move(sel));
+  }
   PackedBound& b = *out;
   b = PackedBound();
   b.lanes = ctx.lanes;
@@ -2074,6 +2089,12 @@ Status BatchSchedulingPlugin::PackBoundPods(const PackedSnapshot& ctx, const std
         if (it->second < locked.size() && locked[it->second]) b.flags[k] = BS_BOUND_GROUP_LOCKED;
       }
     }
+    if (!p.labels.empty())   // a pod without labels matches no budget
+      for (const auto& e : exhausted)
+        if (*e.first == p.ns && spread_sel_matches(e.second, p.labels)) {
+          b.flags[k] |= BS_BOUND_PDB_VIOLATING;
+          break;
+        }
   }
   return Status{};
 }
@@ -2091,7 +2112,7 @@ Status BatchSchedulingPlugin::UploadBound() {
     auto it = groups_.find(group_names_[g]);
     if (it != groups_.end()) locked[g] = it->second.pg.phase == "Scheduled" || it->second.pg.phase == "Running";
   }
-  Status st = PackBoundPods(packed_, snapshot_, group_row_, locked, &bound_);
+  Status st = PackBoundPods(packed_, snapshot_, group_row_, locked, &bound_, pdbs_);
   if (!st.ok()) return st;
   bound_row_.build(bound_.n, [&](size_t k) { return &bound_.pods[k]->uid; }, pack_threads(bound_.n));
   const bs_bound_table t = bound_.table();

@@ -134,6 +134,15 @@ struct SpreadSelectors {
   std::vector<ReplicaSet> replica_sets;
   std::vector<StatefulSet> stateful_sets;
 };
+// policy/v1beta1.PodDisruptionBudget as preemption reads it (filterPodsWithPDBViolation, k8s v1.17.5 [upstream, from
+// memory]): has_selector = false is a nil selector.  A nil or empty selector, or one that fails
+// LabelSelectorAsSelector, matches no pod.  disruptions_allowed is Status.PodDisruptionsAllowed.
+struct PodDisruptionBudget {
+  std::string ns, name;
+  bool has_selector = false;
+  LabelSelector selector;
+  int32_t disruptions_allowed = 0;
+};
 // v1.ContainerImage: one entry of Status.Images, the names it is known by and its size (ImageLocality)
 struct ContainerImage {
   std::vector<std::string> names;
@@ -486,6 +495,9 @@ class BatchSchedulingPlugin {
   void SetLocalityWeights(uint32_t image_locality, uint32_t prefer_avoid_pods);
   // the content of the Service, ReplicationController, ReplicaSet and StatefulSet listers, read by the next round
   void SetSpreadSelectors(SpreadSelectors selectors);
+  // the content of the PodDisruptionBudget lister, read when the bound-pod table is packed next: at the next
+  // BeginRound, UpdateNodes or UpdateGroups (PackBoundPods sets BS_BOUND_PDB_VIOLATING from it)
+  void SetPodDisruptionBudgets(std::vector<PodDisruptionBudget> pdbs);
   // weight of kube-scheduler v1.17's SelectorSpread priority in PriorityNodes (bs_set_spread_weight; 0 = off, the
   // default; v1.17's default profile is 1), read by the next round; ReplayQueue(kPriority) refuses a non-zero weight
   void SetSelectorSpreadWeight(uint32_t selector_spread);
@@ -534,23 +546,28 @@ class BatchSchedulingPlugin {
   // The bound pods of `snapshot` against the lanes of `ctx`: demand = the containers' Requests (NodeInfo.RemovePod
   // subtracts what AddPod added: Requests, not Limits); gid from the group label and "ns/<label>" in group_row
   // (BS_GID_NONE without the label, BS_GID_MISSING when the group is not in the table); BS_BOUND_GROUP_LOCKED when
-  // that group's row is in `locked` (Status.Phase Scheduled or Running).
+  // that group's row is in `locked` (Status.Phase Scheduled or Running).  BS_BOUND_PDB_VIOLATING by
+  // filterPodsWithPDBViolation: the pod has a label and some budget of `pdbs` in its namespace, with a selector that
+  // converts, is not empty and matches the pod's labels, allows <= 0 disruptions.
   static Status PackBoundPods(const PackedSnapshot& ctx, const std::vector<const NodeInfo*>& snapshot,
                               const std::unordered_map<std::string, uint32_t>& group_row,
-                              const std::vector<uint8_t>& locked, PackedBound* out);
+                              const std::vector<uint8_t>& locked, PackedBound* out,
+                              const std::vector<PodDisruptionBudget>& pdbs = {});
   // batchSchedulingPluginExtension.RemovePod (batchscheduler.go:132-144) -> core.PreemptRemovePod (core.go:203-260):
   // the preemptor must be a pending pod of the round, the victim a pod some NodeInfo of the round lists
   Status RemovePod(const Pod& preemptor, const Pod& victim);
   // PreemptAddPod always succeeds (core.go:194-196)
   Status AddPod(const Pod&, const Pod&) { return Status{}; }
   // genericScheduler.Preempt for one pending pod of the round against the round's snapshot: the node preemption would
-  // pick ("" none) and the uids of the pods it would evict there, most important first
+  // pick ("" none) and the uids of the pods it would evict there: those that violate a PodDisruptionBudget
+  // (SetPodDisruptionBudgets) first, then the others, each part most important first
   Status Preempt(const std::string& uid, std::string* node, std::vector<std::string>* victim_uids);
   struct Preemption {
     std::string uid, node;
     std::vector<std::string> victims;
   };
-  // Preempt for every pending pod that passed PreFilter and fits no node (upstream preempts only on a FitError)
+  // Preempt for every pending pod that passed PreFilter and fits no node (upstream preempts only on a FitError), the
+  // victims in Preempt's order
   Status PreemptAll(std::vector<Preemption>* out);
   const PackedBound& bound() const { return bound_; }
   // The non-zero request columns of the resource priorities (no GPU): per pending pod and per NodeInfo (over
@@ -626,6 +643,7 @@ class BatchSchedulingPlugin {
   uint32_t locality_weights_[2] = {0, 0};              // SetLocalityWeights: ImageLocality, NodePreferAvoidPods
   uint32_t spread_weight_ = 0;                          // SetSelectorSpreadWeight
   SpreadSelectors spread_selectors_;                    // SetSpreadSelectors
+  std::vector<PodDisruptionBudget> pdbs_;               // SetPodDisruptionBudgets
   uint32_t interpod_weight_ = 0;                        // SetInterPodAffinityWeight
   int32_t hard_pod_affinity_weight_ = 1;                // SetHardPodAffinityWeight
   std::string init_error_;

@@ -6,9 +6,10 @@
 // The bound pods of a node are stored as one CSR segment in MoreImportantPod order (priority descending, start time
 // ascending, table index ascending), so the potential victims of a preemptor (priority strictly lower) are a SUFFIX
 // of the segment.  preempt_prep_kernel builds, per CSR position, the suffix sums of the removable lanes and the
-// suffix counts of the rows RemovePod refuses for some preemptor; the hot kernel answers "all victims removed"
-// with one binary search and one suffix read per (preemptor, node) and walks the suffix only for the pairs that
-// survive that test.  The oracles in the tests mutate a copy of the node instead: the two must agree.
+// suffix counts of the rows RemovePod refuses for some preemptor and of the PodDisruptionBudget-violating rows; the
+// hot kernel answers "all victims removed" with one binary search and one suffix read per (preemptor, node) and walks
+// the suffix only for the pairs that survive that test.  The oracles in the tests mutate a copy of the node instead:
+// the two must agree.
 #pragma once
 #include "kernels.cuh"
 
@@ -26,6 +27,7 @@ struct BoundTab {
   const int64_t* suf;       // [L][V] sum of req over positions k .. end of the segment
   const uint32_t* suf_online;   // [V] rows without a group label in k .. end
   const uint32_t* suf_bad;      // [V] rows whose group is missing or Scheduled / Running in k .. end
+  const uint32_t* suf_vio;      // [V] rows flagged BS_BOUND_PDB_VIOLATING in k .. end
   uint32_t V;
 };
 
@@ -39,13 +41,15 @@ struct PreemptPod {
 };
 
 // pickOneNodeForPreemption's order over candidate nodes; the smaller key wins.  A candidate without victims wins
-// at once (lowest index); otherwise: highest victim priority, sum of (priority + 2^31), victim count, LATEST start
-// of the first (most important) victim, node index.  node = -1: no candidate.
+// at once (lowest index); otherwise: PDB-violating victims, the priority of the FIRST victim (upstream's "highest",
+// which is the first violating victim when there is one), sum of (priority + 2^31), victim count, LATEST earliest
+// start among the victims of the true maximum priority (GetEarliestPodStartTime), node index.  node = -1: none.
 struct PickKey {
   int64_t sum;
   int64_t start;
   int32_t hp;
   uint32_t nv;
+  uint32_t vio;    // victims flagged BS_BOUND_PDB_VIOLATING (numViolatingVictim)
   int32_t node;
   uint32_t cand;   // candidates counted into this key (not part of the order)
 };
@@ -55,6 +59,7 @@ __device__ __forceinline__ bool pick_less(const PickKey& a, const PickKey& b) {
   if (b.node < 0) return true;
   if ((a.nv == 0) != (b.nv == 0)) return a.nv == 0;
   if (a.nv != 0) {
+    if (a.vio != b.vio) return a.vio < b.vio;
     if (a.hp != b.hp) return a.hp < b.hp;
     if (a.sum != b.sum) return a.sum < b.sum;
     if (a.nv != b.nv) return a.nv < b.nv;
@@ -71,27 +76,32 @@ __device__ __forceinline__ PickKey pick_min(const PickKey& a, const PickKey& b) 
 
 __device__ __forceinline__ PickKey pick_none() {
   PickKey k;
-  k.sum = 0; k.start = 0; k.hp = 0; k.nv = 0; k.node = -1; k.cand = 0;
+  k.sum = 0; k.start = 0; k.hp = 0; k.nv = 0; k.vio = 0; k.node = -1; k.cand = 0;
   return k;
 }
 
 // ---------------------------------------------------------------------------
 // preempt_prep_kernel — once per bound-table upload, one thread per node: suffix sums of the removable lanes and
-// suffix counts of the online and the missing-or-locked rows, walking the node's segment from its end.
+// suffix counts of the online, the missing-or-locked and the PDB-violating rows, walking the node's segment from its
+// end.
 __global__ void preempt_prep_kernel(const uint32_t* __restrict__ row, const int32_t* __restrict__ gid,
                                     const uint8_t* __restrict__ flags, const int64_t* __restrict__ req,
                                     int64_t* __restrict__ suf, uint32_t* __restrict__ suf_online,
-                                    uint32_t* __restrict__ suf_bad, uint32_t N, uint32_t V, uint32_t L) {
+                                    uint32_t* __restrict__ suf_bad, uint32_t* __restrict__ suf_vio, uint32_t N,
+                                    uint32_t V, uint32_t L) {
   const uint32_t n = blockIdx.x * blockDim.x + threadIdx.x;
   if (n >= N) return;
   const uint32_t b = row[n], e = row[n + 1];
-  uint32_t on = 0, bad = 0;
+  uint32_t on = 0, bad = 0, vio = 0;
   for (uint32_t k = e; k-- > b;) {
     const int32_t g = gid[k];
+    const uint8_t f = flags[k];
     on += g == BS_GID_NONE ? 1u : 0u;
-    bad += (g == BS_GID_MISSING || (g >= 0 && (flags[k] & BS_BOUND_GROUP_LOCKED))) ? 1u : 0u;
+    bad += (g == BS_GID_MISSING || (g >= 0 && (f & BS_BOUND_GROUP_LOCKED))) ? 1u : 0u;
+    vio += (f & BS_BOUND_PDB_VIOLATING) ? 1u : 0u;
     suf_online[k] = on;
     suf_bad[k] = bad;
+    suf_vio[k] = vio;
   }
   for (uint32_t d = 0; d < L; ++d) {
     int64_t s = 0;
@@ -139,8 +149,15 @@ __device__ __forceinline__ bool fits_freed(const int64_t* left, const int64_t* f
   return ok;
 }
 
+template <bool B>
+struct BoolC {
+  static constexpr bool value = B;
+};
+
 // selectVictimsOnNode for preemptor slot i on node n.  Returns false when the node is not a candidate; else the
-// key of the node, and with EMIT the victims' bound-table indices at out[0..).
+// key of the node, and with EMIT the victims' bound-table indices at out[0..): the PDB-violating victims first, then
+// the others, each part in MoreImportantPod order (filterPodsWithPDBViolation splits the potential victims and the
+// violating ones are reprieved first).
 template <int MAXL, bool EMIT>
 __device__ bool select_victims(const PreemptArgs& a, const PreemptPod& q, const int64_t* req, uint32_t rpres,
                                uint32_t n, PickKey& key, uint32_t* out) {
@@ -179,16 +196,22 @@ __device__ bool select_victims(const PreemptArgs& a, const PreemptPod& q, const 
   const int64_t pods_left = left[LANE_PODS], pods_req = req[LANE_PODS];
   uint32_t removed = end - s;
   if (!fits_freed<MAXL>(left, freed, req, cmask, pods_left + (pods_by_count ? removed : 0), pods_req)) return false;
-  // reprieve, most important first: add each back; keep it when the pod still fits, else it is a victim
+  // reprieve, most important first: add each back; keep it when the pod still fits, else it is a victim.  With
+  // PDB-violating potential victims, two passes over the suffix: the violating rows, then the others.
   key = pick_none();
   key.node = (int32_t)n;
   key.cand = 1;
-  for (uint32_t k = s; k < end; ++k) {
+  int32_t maxp = 0;   // the highest victim priority so far; key.start is the earliest start among its victims
+  // one reprieve step on row k.  SPLIT: the walk is the two-pass one, whose victims are not in priority order, so
+  // the start criterion follows the running maximum; in the single pass the first victim has the maximum priority
+  // and the earliest start among it.
+  auto reprieve = [&](uint32_t k, bool vio, auto split_c) {
+    constexpr bool SPLIT = decltype(split_c)::value;
 #pragma unroll
     for (int d = 0; d < MAXL; ++d)
       if (d < (int)t.L) freed[d] -= a.b.req[(size_t)d * a.b.V + k];
     --removed;
-    if (fits_freed<MAXL>(left, freed, req, cmask, pods_left + (pods_by_count ? removed : 0), pods_req)) continue;
+    if (fits_freed<MAXL>(left, freed, req, cmask, pods_left + (pods_by_count ? removed : 0), pods_req)) return;
 #pragma unroll
     for (int d = 0; d < MAXL; ++d)
       if (d < (int)t.L) freed[d] += a.b.req[(size_t)d * a.b.V + k];
@@ -197,10 +220,24 @@ __device__ bool select_victims(const PreemptArgs& a, const PreemptPod& q, const 
     if (key.nv == 0) {
       key.hp = pr;
       key.start = a.b.start[k];
+      maxp = pr;
+    } else if (SPLIT && pr >= maxp) {
+      const int64_t st = a.b.start[k];
+      if (pr > maxp || st < key.start) key.start = st;
+      maxp = pr;
     }
     key.sum += (int64_t)pr + ((int64_t)1 << 31);
+    if (SPLIT) key.vio += vio ? 1u : 0u;
     if (EMIT) out[key.nv] = a.b.idx[k];
     ++key.nv;
+  };
+  if (s == end || a.b.suf_vio[s] == 0) {
+    for (uint32_t k = s; k < end; ++k) reprieve(k, false, BoolC<false>{});
+  } else {   // the violating rows first, then the others, each in MoreImportantPod order
+    for (uint32_t k = s; k < end; ++k)
+      if (a.b.flags[k] & BS_BOUND_PDB_VIOLATING) reprieve(k, true, BoolC<true>{});
+    for (uint32_t k = s; k < end; ++k)
+      if (!(a.b.flags[k] & BS_BOUND_PDB_VIOLATING)) reprieve(k, false, BoolC<true>{});
   }
   return true;
 }
@@ -214,9 +251,10 @@ __device__ __forceinline__ uint32_t load_req(const PreemptArgs& a, const Preempt
 
 // preempt_node_kernel — the hot path: block (tile, preemptor) evaluates PREEMPT_THREADS nodes for one preemptor and
 // writes the tile's best key (and its candidate count).  The key is a total order (the node index decides last),
-// so the tree below gives the same winner as a walk in node order.
+// so the tree below gives the same winner as a walk in node order.  At MAXL 5 the bound holds 64 registers, four
+// blocks per SM, without spills (the PDB pass would otherwise take it to 72 and three blocks).
 template <int MAXL>
-__global__ void __launch_bounds__(PREEMPT_THREADS) preempt_node_kernel(PreemptArgs a) {
+__global__ void __launch_bounds__(PREEMPT_THREADS, MAXL <= 5 ? 4 : 1) preempt_node_kernel(PreemptArgs a) {
   const uint32_t i = a.p0 + blockIdx.y;
   const uint32_t n = blockIdx.x * PREEMPT_THREADS + threadIdx.x;
   const PreemptPod q = a.pp[i];
@@ -231,6 +269,7 @@ __global__ void __launch_bounds__(PREEMPT_THREADS) preempt_node_kernel(PreemptAr
     k2.start = __shfl_down_sync(0xffffffffu, key.start, o);
     k2.hp = __shfl_down_sync(0xffffffffu, key.hp, o);
     k2.nv = __shfl_down_sync(0xffffffffu, key.nv, o);
+    k2.vio = __shfl_down_sync(0xffffffffu, key.vio, o);
     k2.node = __shfl_down_sync(0xffffffffu, key.node, o);
     k2.cand = __shfl_down_sync(0xffffffffu, key.cand, o);
     key = pick_min(key, k2);

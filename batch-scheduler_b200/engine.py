@@ -12,8 +12,9 @@ from .snapshot import BoundPodTable, NodeTable, PodTable, GroupTable, Snapshot
 
 @dataclass
 class PreemptResult:
-    """bs_preempt's outputs: per preemptor the chosen node (-1 none), its victims (bound-table indices, reprieve order)
-    at victims[victim_offset[i]:victim_offset[i + 1]], and the number of candidate nodes."""
+    """bs_preempt's outputs: per preemptor the chosen node (-1 none), its victims (bound-table indices, reprieve order:
+    the BOUND_PDB_VIOLATING ones first) at victims[victim_offset[i]:victim_offset[i + 1]], and the number of candidate
+    nodes."""
     node: np.ndarray           # int32 [n]
     n_victims: np.ndarray      # uint32 [n]
     n_candidates: np.ndarray   # uint32 [n]

@@ -185,6 +185,7 @@ class GroupTable:
 
 
 BOUND_GROUP_LOCKED = 0x01   # the bound pod's PodGroup Status.Phase is Scheduled or Running
+BOUND_PDB_VIOLATING = 0x02  # the bound pod violates a PodDisruptionBudget (filterPodsWithPDBViolation)
 
 
 @dataclass
@@ -306,12 +307,14 @@ class Snapshot:
 
 def bound_pods(snap: Snapshot, seed: int, fill: float = 1.0, max_per_node: int = None,
                priorities=(-10, 0, 0, 5, 100, 1000), n_starts: int = 8, online: float = 0.3, missing: float = 0.03,
-               locked: float = 0.2) -> BoundPodTable:
+               locked: float = 0.2, violating: float = 0.0) -> BoundPodTable:
     """A bound-pod table consistent with the node table: node n gets round(fill * pod_count[n]) pods (at most
     max_per_node) whose lanes 0-2 split the node's requested amounts (the last pod takes the remainder) and whose scalar
     keys are a random subset of the node's req_present.  Priorities are drawn from `priorities`, start times from
     n_starts values (ties on purpose); a pod is online (no group label) with probability `online`, in a missing group
-    with `missing`, else in a random group of the snapshot, locked (Scheduled / Running) with `locked`."""
+    with `missing`, else in a random group of the snapshot, locked (Scheduled / Running) with `locked`.  A pod violates
+    a PodDisruptionBudget with probability `violating`, drawn after everything else and only when it is > 0, so that a
+    seed gives the same table with the default as without the parameter."""
     rng = np.random.default_rng(seed)
     nt, G, L = snap.nodes, snap.groups.n, snap.nodes.lanes
     k = np.round(np.clip(nt.pod_count.astype(np.int64), 0, None) * fill).astype(np.int64)
@@ -344,6 +347,8 @@ def bound_pods(snap: Snapshot, seed: int, fill: float = 1.0, max_per_node: int =
         gid = np.where(u < online, GID_NONE, np.where(u < online + missing, GID_MISSING, gid))
         bt.gid = gid.astype(np.int32)
         bt.flags = np.where((gid >= 0) & (rng.random(V) < locked), BOUND_GROUP_LOCKED, 0).astype(np.uint8)
+        if violating > 0:
+            bt.flags |= np.where(rng.random(V) < violating, BOUND_PDB_VIOLATING, 0).astype(np.uint8)
     return bt
 
 

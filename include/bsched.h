@@ -687,6 +687,12 @@ int bs_upload_pod_interpod(bs_engine* e, const bs_interpod_pods* t);
  * a lane beyond +-BS_VALUE_LIMIT, BS_E_RANGE.  A failing table is dropped.  The table belongs to the node snapshot:
  * bs_upload_nodes, bs_update_nodes and bs_upload_groups drop it (BS_E_STATE until it is uploaded again). */
 #define BS_BOUND_GROUP_LOCKED 0x01u /* the pod's PodGroup Status.Phase is Scheduled or Running (core.go:235-236) */
+/* The pod violates a PodDisruptionBudget (filterPodsWithPDBViolation, k8s v1.17.5 [upstream, from memory]): it has a
+ * label, and some PDB of its namespace with a non-empty selector that converts and matches its labels has
+ * Status.PodDisruptionsAllowed <= 0.  bs_preempt reprieves such victims first and ranks nodes by how many it evicts
+ * (DESIGN.md §2 "Preemption").  A table without the bit gives the answers of a cluster without budgets.  Other bits
+ * are ignored. */
+#define BS_BOUND_PDB_VIOLATING 0x02u
 typedef struct {
   uint32_t n_pods, n_lanes;
   const uint32_t* node;        /* [V] snapshot index of the node it is bound to (NodeInfo.Pods())              */
@@ -702,13 +708,14 @@ int bs_upload_bound_pods(bs_engine* e, const bs_bound_table* t);
 
 /* Result of bs_preempt.  Per preemptor: the node genericScheduler.Preempt -> pickOneNodeForPreemption would pick
  * (-1 none) and, in victims[victim_offset[i] .. victim_offset[i + 1]), the bound-table indices of the pods
- * selectVictimsOnNode would evict there, in reprieve order (most important first). */
+ * selectVictimsOnNode would evict there, in reprieve order: the BS_BOUND_PDB_VIOLATING victims first, then the
+ * others, each part most important first. */
 typedef struct {
   int32_t* node;            /* [n] chosen node, -1 none                                              */
   uint32_t* n_victims;      /* [n]                                                                   */
   uint32_t* n_candidates;   /* [n] nodes where removing every lower-priority pod lets the pod fit    */
   uint32_t* victim_offset;  /* [n + 1] exclusive scan of n_victims                                   */
-  uint32_t* victims;        /* [victims_cap] bound-table indices, per preemptor in reprieve order      */
+  uint32_t* victims;        /* [victims_cap] bound-table indices, per preemptor in reprieve order    */
   uint32_t victims_cap;
   uint32_t victims_total;   /* out, always written; > victims_cap -> BS_E_INVAL, victims untouched   */
 } bs_preempt_result;

@@ -447,6 +447,13 @@ func (e *Engine) PreFilter(pod uint32, nsName, occupiedBy string) error {
 	return fmt.Errorf("%s", C.GoString(buf)) // the adapter turns it into framework.Unschedulable (batchscheduler.go:104-107)
 }
 
+// Bound-pod flags (bs_bound_table.flags): the pod's PodGroup is Scheduled or Running; the pod violates a
+// PodDisruptionBudget (filterPodsWithPDBViolation's verdict, which preemption reprieves first and ranks nodes by).
+const (
+	BoundGroupLocked  = C.BS_BOUND_GROUP_LOCKED
+	BoundPDBViolating = C.BS_BOUND_PDB_VIOLATING
+)
+
 // UploadBoundPods uploads the pods bound to the snapshot's nodes (NodeInfo.Pods()): what preemption may evict.
 // Upload nodes and groups first; either upload, and UpdateNodes, drop the table.
 func (e *Engine) UploadBoundPods(t *C.bs_bound_table) error { return e.rc(C.bs_upload_bound_pods(e.h, t)) }
@@ -475,7 +482,8 @@ func (e *Engine) RemovePod(pod, bound uint32, podName, victimName, victimGroup s
 }
 
 // Preemption is one preemptor's answer: the snapshot index of the node preemption would pick (-1 none) and the
-// bound-pod rows it would evict there, most important first.
+// bound-pod rows it would evict there: the BoundPDBViolating ones first, then the others, each part most important
+// first.
 type Preemption struct {
 	Node       int32
 	Victims    []uint32
