@@ -46,6 +46,9 @@ IPA_TABLE_MAX_BYTES = 1 << 30   # BS_IPA_TABLE_MAX_BYTES: cap of the pod class x
 REMOVE_ALLOW, REMOVE_OFFLINE_ONLINE, REMOVE_NOT_FOUND, REMOVE_LOCKED, REMOVE_SAME_GROUP = range(5)
 BOUND_GROUP_LOCKED = 0x01
 BOUND_PDB_VIOLATING = 0x02
+# bs_preempt_walk: the flag and the per-preemptor outcomes (bs_walk_outcome)
+PREEMPT_GANG = 0x1
+WALK_NONE, WALK_NOMINATED, WALK_ROLLED_BACK = range(3)
 FILTER_PASS, FILTER_NOT_FOUND, FILTER_NOT_ENOUGH, FILTER_NO_SNAPSHOT, FILTER_REF_PANIC = range(5)
 BUF_FIT_BITMAP, BUF_SCORE, BUF_ADMIT_BITMAP, BUF_PREFILTER, BUF_ADMIT, BUF_ORDER, BUF_GATHERED_ADMIT = range(7)
 K_NODE_LEFT, K_FIND_MAX, K_CLASS_PREFIX, K_PREFILTER, K_GANG_FIT, K_SORT, K_FILTER, K_PEER, K_REPLAY, K_REASONS, K_COUNT = \
@@ -175,6 +178,8 @@ SYMBOLS = {
                                    C.c_uint32, C.c_void_p]),
     "bs_upload_bound_pods": (C.c_int, [C.c_void_p, _p(BoundTableC)]),
     "bs_preempt": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, _p(PreemptResultC)]),
+    "bs_preempt_walk": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, _p(PreemptResultC), C.c_void_p,
+                                  C.c_void_p]),
     "bs_remove_pod": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, _p(StatusC)]),
     "bs_format_remove_message": (C.c_int, [_p(StatusC), C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_size_t]),
     "bs_device_buffer": (C.c_int, [C.c_void_p, C.c_int, _p(C.c_void_p), _p(C.c_size_t)]),

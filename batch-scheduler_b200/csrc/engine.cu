@@ -533,6 +533,8 @@ struct bs_engine {
   DevBuf d_pl_left, d_pl_present;
   // bs_preempt scratch
   DevBuf d_pp, d_ptiles, d_pnode, d_pnv, d_pcand, d_poff, d_pvict;
+  // bs_preempt_walk scratch: the live copies of the node and bound state, the outputs and the undo log
+  DevBuf d_walk;
 
   // peer exchange (admit bitmap all-gather over NVLink peer memory)
   DevBuf d_gather, d_peer_err;
@@ -1646,6 +1648,12 @@ struct PreemptNodeLaunch {
 template <int MAXL>
 struct PreemptEmitLaunch {
   static void go(dim3 grid, cudaStream_t s, const PreemptArgs& a) { preempt_emit_kernel<MAXL><<<grid, 256, 0, s>>>(a); }
+};
+template <int MAXL>
+struct PreemptCommitLaunch {
+  static void go(cudaStream_t s, const PreemptArgs& a, const WalkArgs& w, uint32_t i) {
+    preempt_commit_kernel<MAXL><<<1, PREEMPT_THREADS, 0, s>>>(a, w, i);
+  }
 };
 
 // What the bound-table pass finds wrong, in the order the errors are reported.
@@ -2838,23 +2846,55 @@ int bs_upload_bound_pods(bs_engine* e, const bs_bound_table* t) {
   return BS_OK;
 }
 
+namespace {
+// bs_preempt and bs_preempt_walk: the state checks and each preemptor as the kernels take it.  The caller holds the
+// engine's lock.
+int preempt_pods(bs_engine* e, const char* who, const uint32_t* pods, uint32_t n, std::vector<PreemptPod>& pp) {
+  const std::string w(who);
+  if (!e->have_nodes || !e->have_groups || !e->have_pods || !e->have_bound)
+    return fail(e, BS_E_STATE, (w + ": upload nodes, groups, pods and the bound-pod table first").c_str());
+  if (e->bound_max_gid >= (int32_t)e->G)
+    return fail(e, BS_E_INDEX, (w + ": a bound pod's group index >= n_groups").c_str());
+  pp.assign(std::max(n, 1u), PreemptPod{});
+  for (uint32_t i = 0; i < n; ++i) {
+    const uint32_t p = pods[i];
+    if (p >= e->P) return fail(e, BS_E_INDEX, (w + ": pod index outside the pod table").c_str());
+    const ClassKey& k = e->fit_index.keys[e->h_pfc[p]];
+    if (k.aff != BS_AFF_NONE && k.aff >= e->n_aff)
+      return fail(e, BS_E_INDEX, (w + ": affinity class outside the uploaded table").c_str());
+    pp[i] = PreemptPod{k.sel, k.tol, p, k.nz, k.aff, e->h_prio[p], e->h_gid[p]};
+  }
+  return BS_OK;
+}
+
+// The kernels' view of the uploaded node and bound tables and of the preemptors in e->d_pp.
+PreemptArgs preempt_args(const bs_engine* e, uint32_t n) {
+  PreemptArgs a{};
+  a.t = node_tab(e);
+  a.left = e->d_pl_left.as<int64_t>();
+  a.left_present = e->d_pl_present.as<uint32_t>();
+  a.b = BoundTab{e->d_brow.as<uint32_t>(), e->d_brow.as<uint32_t>() + 1, e->d_bprio.as<int32_t>(),
+                 e->d_bstart.as<int64_t>(), e->d_bgid.as<int32_t>(), e->d_bflags.as<uint8_t>(), e->d_bidx.as<uint32_t>(),
+                 e->d_breq.as<int64_t>(), e->d_bsuf.as<int64_t>(), e->d_bsuf_online.as<uint32_t>(),
+                 e->d_bsuf_bad.as<uint32_t>(), e->d_bsuf_vio.as<uint32_t>(), std::max(e->V, 1u)};
+  a.pp = e->d_pp.as<PreemptPod>();
+  a.preq = e->d_req.as<int64_t>();
+  a.preq_present = e->d_ppres.as<uint32_t>();
+  a.P = e->P;
+  a.n = n;
+  a.n_tiles = cdiv(e->N, PREEMPT_THREADS);
+  return a;
+}
+}  // namespace
+
 int bs_preempt(bs_engine* e, const uint32_t* pods, uint32_t n, bs_preempt_result* out) {
   if (!e || !out || (n && (!pods || !out->node || !out->n_victims || !out->n_candidates)) || !out->victim_offset)
     return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
-  if (!e->have_nodes || !e->have_groups || !e->have_pods || !e->have_bound)
-    return fail(e, BS_E_STATE, "bs_preempt: upload nodes, groups, pods and the bound-pod table first");
-  if (e->bound_max_gid >= (int32_t)e->G) return fail(e, BS_E_INDEX, "bs_preempt: a bound pod's group index >= n_groups");
+  std::vector<PreemptPod> pp;
+  int rc;
+  if ((rc = preempt_pods(e, "bs_preempt", pods, n, pp))) return rc;
   const uint32_t L = e->L, N = e->N;
-  std::vector<PreemptPod> pp(std::max(n, 1u));
-  for (uint32_t i = 0; i < n; ++i) {
-    const uint32_t p = pods[i];
-    if (p >= e->P) return fail(e, BS_E_INDEX, "bs_preempt: pod index outside the pod table");
-    const ClassKey& k = e->fit_index.keys[e->h_pfc[p]];
-    if (k.aff != BS_AFF_NONE && k.aff >= e->n_aff)
-      return fail(e, BS_E_INDEX, "bs_preempt: affinity class outside the uploaded table");
-    pp[i] = PreemptPod{k.sel, k.tol, p, k.nz, k.aff, e->h_prio[p], e->h_gid[p]};
-  }
   out->victim_offset[0] = 0;
   out->victims_total = 0;
   if (!n) return BS_OK;
@@ -2865,23 +2905,10 @@ int bs_preempt(bs_engine* e, const uint32_t* pods, uint32_t n, bs_preempt_result
   CK(e->d_pcand.ensure((size_t)n * 4));
   CK(e->d_poff.ensure((size_t)n * 4));
   CK(cudaMemcpyAsync(e->d_pp.p, pp.data(), (size_t)n * sizeof(PreemptPod), cudaMemcpyHostToDevice, e->s));
-  PreemptArgs a{};
-  a.t = node_tab(e);
-  a.left = e->d_pl_left.as<int64_t>();
-  a.left_present = e->d_pl_present.as<uint32_t>();
-  a.b = BoundTab{e->d_brow.as<uint32_t>(), e->d_bprio.as<int32_t>(), e->d_bstart.as<int64_t>(), e->d_bgid.as<int32_t>(),
-                 e->d_bflags.as<uint8_t>(), e->d_bidx.as<uint32_t>(), e->d_breq.as<int64_t>(), e->d_bsuf.as<int64_t>(),
-                 e->d_bsuf_online.as<uint32_t>(), e->d_bsuf_bad.as<uint32_t>(), e->d_bsuf_vio.as<uint32_t>(),
-                 std::max(e->V, 1u)};
-  a.pp = e->d_pp.as<PreemptPod>();
-  a.preq = e->d_req.as<int64_t>();
-  a.preq_present = e->d_ppres.as<uint32_t>();
-  a.P = e->P;
-  a.n = n;
+  PreemptArgs a = preempt_args(e, n);
   a.out_node = e->d_pnode.as<int32_t>();
   a.out_nv = e->d_pnv.as<uint32_t>();
   a.out_cand = e->d_pcand.as<uint32_t>();
-  a.n_tiles = cdiv(N, PREEMPT_THREADS);
   if (!N) {
     CK(cudaMemsetAsync(a.out_node, 0xff, (size_t)n * 4, e->s));
     CK(cudaMemsetAsync(a.out_nv, 0, (size_t)n * 4, e->s));
@@ -2922,6 +2949,170 @@ int bs_preempt(bs_engine* e, const uint32_t* pods, uint32_t n, bs_preempt_result
   launch_maxl<PreemptEmitLaunch>(L, dim3(cdiv(n, 256)), (cudaStream_t)e->s, a);
   ++e->launches;
   CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(out->victims, a.victims, (size_t)total * 4, cudaMemcpyDeviceToHost, e->s));
+  CK(cudaStreamSynchronize(e->s));
+  return BS_OK;
+}
+
+int bs_preempt_walk(bs_engine* e, const uint32_t* pods, uint32_t n, uint32_t flags, bs_preempt_result* out,
+                    uint32_t* outcome, int32_t* evicted_by) {
+  if (!e || !out || (n && (!pods || !out->node || !out->n_victims || !out->n_candidates)) || !out->victim_offset)
+    return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (flags & ~BS_PREEMPT_GANG) return fail(e, BS_E_INVAL, "bs_preempt_walk: unknown flag bits");
+  const bool gang = flags & BS_PREEMPT_GANG;
+  std::vector<PreemptPod> pp;
+  int rc;
+  if ((rc = preempt_pods(e, "bs_preempt_walk", pods, n, pp))) return rc;
+  // queue order: every earlier nomination has a priority >= the current preemptor's, so all of them count
+  // (addNominatedPods) and none is ever cleared (getLowerPriorityNominatedPods)
+  std::vector<uint8_t> seen(e->P, 0), closed(gang ? e->G : 0, 0), unit_last(std::max(n, 1u), 1);
+  for (uint32_t i = 0; i < n; ++i) {
+    if (i && pp[i].prio > pp[i - 1].prio)
+      return fail(e, BS_E_INVAL, "bs_preempt_walk: priorities must be non-increasing along the list");
+    if (seen[pp[i].pod]++) return fail(e, BS_E_INVAL, "bs_preempt_walk: a pod is listed twice");
+    // a group index >= n_groups names no group of the table: like BS_GID_MISSING, a unit of one
+    if (!gang || pp[i].gid < 0 || pp[i].gid >= (int32_t)e->G) continue;
+    const int32_t g = pp[i].gid;
+    if (i && pp[i - 1].gid == g) {
+      unit_last[i - 1] = 0;
+    } else {
+      if (closed[g]) return fail(e, BS_E_INVAL, "bs_preempt_walk: the preemptors of a group are not contiguous");
+      closed[g] = 1;
+    }
+  }
+  // the live sums: nominations add requests (negative ones without the fit's bound) and pods
+  const NodeStats& ns = e->node_stats;
+  const PodStats& ps = e->pod_stats;
+  for (uint32_t d = 0; d < e->L; ++d)
+    if ((long double)ns.max_alloc[d] + (long double)ns.max_requested[d] + (long double)ps.max_req[d] +
+            (long double)ps.neg_req[d] * (long double)n + (long double)ns.max_pod_count + n + (long double)BS_VALUE_LIMIT >
+        0x1p62L)
+      return fail(e, BS_E_RANGE, "bs_preempt_walk: live requests could pass 2^62");
+  const uint32_t L = e->L, N = e->N, Npad = e->Npad, V = e->V, Vp = std::max(V, 1u);
+  if (evicted_by) std::fill(evicted_by, evicted_by + V, -1);
+  out->victim_offset[0] = 0;
+  out->victims_total = 0;
+  if (!n) return BS_OK;
+  BS_DEVICE_GUARD(e);
+  PreemptArgs a = preempt_args(e, n);
+  const size_t g_n = gang ? n : 0, g_v = gang ? Vp : 0;
+  View w_pp, w_node, w_nv, w_cand, w_outcome, w_last, w_tiles, w_vict, w_ctl, w_end, w_prio, w_start, w_gid, w_flags,
+      w_idx, w_req, w_suf, w_son, w_sbad, w_svio, w_requested, w_rp, w_pc, w_left, w_lp, w_evby, e_node, e_end, e_nv,
+      e_row, e_req, e_rp, e_pc, r_pos, r_prio, r_start, r_gid, r_flags, r_idx, r_req;
+  CK(carve(e->d_walk,
+           {{&w_pp, (size_t)n * sizeof(PreemptPod)}, {&w_node, (size_t)n * 4}, {&w_nv, (size_t)n * 4},
+            {&w_cand, (size_t)n * 4}, {&w_outcome, (size_t)n * 4}, {&w_last, n}, {&w_tiles, a.n_tiles * sizeof(PickKey)},
+            {&w_vict, (size_t)Vp * 4}, {&w_ctl, sizeof(WalkCtl)}, {&w_end, (size_t)N * 4}, {&w_prio, (size_t)Vp * 4},
+            {&w_start, (size_t)Vp * 8}, {&w_gid, (size_t)Vp * 4}, {&w_flags, Vp}, {&w_idx, (size_t)Vp * 4},
+            {&w_req, (size_t)L * Vp * 8}, {&w_suf, (size_t)L * Vp * 8}, {&w_son, (size_t)Vp * 4},
+            {&w_sbad, (size_t)Vp * 4}, {&w_svio, (size_t)Vp * 4}, {&w_requested, (size_t)L * Npad * 8},
+            {&w_rp, (size_t)Npad * 4}, {&w_pc, (size_t)Npad * 4}, {&w_left, (size_t)L * Npad * 8},
+            {&w_lp, (size_t)Npad * 4}, {&w_evby, (size_t)Vp * 4}, {&e_node, g_n * 4}, {&e_end, g_n * 4},
+            {&e_nv, g_n * 4}, {&e_row, g_n * 4}, {&e_req, L * g_n * 8}, {&e_rp, g_n * 4}, {&e_pc, g_n * 4},
+            {&r_pos, g_v * 4}, {&r_prio, g_v * 4}, {&r_start, g_v * 8}, {&r_gid, g_v * 4}, {&r_flags, g_v},
+            {&r_idx, g_v * 4}, {&r_req, L * g_v * 8}}));
+  auto dup = [&](const View& dst, const void* src, size_t bytes) {
+    return bytes ? cudaMemcpyAsync(dst.p, src, bytes, cudaMemcpyDeviceToDevice, e->s) : cudaSuccess;
+  };
+  CK(cudaMemcpyAsync(w_pp.p, pp.data(), (size_t)n * sizeof(PreemptPod), cudaMemcpyHostToDevice, e->s));
+  CK(cudaMemcpyAsync(w_last.p, unit_last.data(), n, cudaMemcpyHostToDevice, e->s));
+  CK(cudaMemsetAsync(w_ctl.p, 0, sizeof(WalkCtl), e->s));
+  CK(cudaMemsetAsync(w_evby.p, 0xff, (size_t)Vp * 4, e->s));
+  CK(dup(w_end, e->d_brow.as<uint32_t>() + 1, (size_t)N * 4));
+  CK(dup(w_prio, e->d_bprio.p, (size_t)Vp * 4));
+  CK(dup(w_start, e->d_bstart.p, (size_t)Vp * 8));
+  CK(dup(w_gid, e->d_bgid.p, (size_t)Vp * 4));
+  CK(dup(w_flags, e->d_bflags.p, Vp));
+  CK(dup(w_idx, e->d_bidx.p, (size_t)Vp * 4));
+  CK(dup(w_req, e->d_breq.p, (size_t)L * Vp * 8));
+  CK(dup(w_suf, e->d_bsuf.p, (size_t)L * Vp * 8));
+  CK(dup(w_son, e->d_bsuf_online.p, (size_t)Vp * 4));
+  CK(dup(w_sbad, e->d_bsuf_bad.p, (size_t)Vp * 4));
+  CK(dup(w_svio, e->d_bsuf_vio.p, (size_t)Vp * 4));
+  CK(dup(w_requested, e->d_requested.p, (size_t)L * Npad * 8));
+  CK(dup(w_rp, e->d_rpres.p, (size_t)Npad * 4));
+  CK(dup(w_pc, e->d_pod_count.p, (size_t)Npad * 4));
+  CK(dup(w_left, e->d_pl_left.p, (size_t)L * Npad * 8));
+  CK(dup(w_lp, e->d_pl_present.p, (size_t)Npad * 4));
+  WalkArgs w{};
+  w.end = w_end.as<uint32_t>();
+  w.prio = w_prio.as<int32_t>();
+  w.start = w_start.as<int64_t>();
+  w.gid = w_gid.as<int32_t>();
+  w.flags = w_flags.as<uint8_t>();
+  w.idx = w_idx.as<uint32_t>();
+  w.req = w_req.as<int64_t>();
+  w.suf = w_suf.as<int64_t>();
+  w.suf_online = w_son.as<uint32_t>();
+  w.suf_bad = w_sbad.as<uint32_t>();
+  w.suf_vio = w_svio.as<uint32_t>();
+  w.requested = w_requested.as<int64_t>();
+  w.req_present = w_rp.as<uint32_t>();
+  w.pod_count = w_pc.as<int32_t>();
+  w.left = w_left.as<int64_t>();
+  w.left_present = w_lp.as<uint32_t>();
+  w.evicted_by = w_evby.as<int32_t>();
+  w.outcome = w_outcome.as<uint32_t>();
+  w.unit_last = w_last.as<uint8_t>();
+  w.ctl = w_ctl.as<WalkCtl>();
+  if (gang) {
+    w.ent_node = e_node.as<uint32_t>();
+    w.ent_end = e_end.as<uint32_t>();
+    w.ent_nv = e_nv.as<uint32_t>();
+    w.ent_row = e_row.as<uint32_t>();
+    w.ent_req = e_req.as<int64_t>();
+    w.ent_rp = e_rp.as<uint32_t>();
+    w.ent_pc = e_pc.as<int32_t>();
+    w.row_pos = r_pos.as<uint32_t>();
+    w.row_prio = r_prio.as<int32_t>();
+    w.row_start = r_start.as<int64_t>();
+    w.row_gid = r_gid.as<int32_t>();
+    w.row_flags = r_flags.as<uint8_t>();
+    w.row_idx = r_idx.as<uint32_t>();
+    w.row_req = r_req.as<int64_t>();
+  }
+  w.n = n;
+  // the kernels read the live state through PreemptArgs' views
+  a.t.requested = w.requested;
+  a.t.req_present = w.req_present;
+  a.t.pod_count = w.pod_count;
+  a.left = w.left;
+  a.left_present = w.left_present;
+  a.b = BoundTab{a.b.row, w.end, w.prio, w.start, w.gid, w.flags, w.idx, w.req, w.suf, w.suf_online, w.suf_bad,
+                 w.suf_vio, Vp};
+  a.pp = w_pp.as<PreemptPod>();
+  a.tiles = w_tiles.as<PickKey>();
+  a.out_node = w_node.as<int32_t>();
+  a.out_nv = w_nv.as<uint32_t>();
+  a.out_cand = w_cand.as<uint32_t>();
+  a.victims = w_vict.as<uint32_t>();
+  for (uint32_t i = 0; i < n; ++i) {   // stream-ordered: no host synchronisation inside the walk
+    if (N) {
+      a.p0 = i;
+      launch_maxl<PreemptNodeLaunch>(L, dim3(a.n_tiles, 1), (cudaStream_t)e->s, a);
+      ++e->launches;
+    }
+    launch_maxl<PreemptCommitLaunch>(L, (cudaStream_t)e->s, a, w, i);
+    ++e->launches;
+  }
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(out->node, a.out_node, (size_t)n * 4, cudaMemcpyDeviceToHost, e->s));
+  CK(cudaMemcpyAsync(out->n_victims, a.out_nv, (size_t)n * 4, cudaMemcpyDeviceToHost, e->s));
+  CK(cudaMemcpyAsync(out->n_candidates, a.out_cand, (size_t)n * 4, cudaMemcpyDeviceToHost, e->s));
+  if (outcome) CK(cudaMemcpyAsync(outcome, w.outcome, (size_t)n * 4, cudaMemcpyDeviceToHost, e->s));
+  if (evicted_by && V) CK(cudaMemcpyAsync(evicted_by, w.evicted_by, (size_t)V * 4, cudaMemcpyDeviceToHost, e->s));
+  CK(cudaStreamSynchronize(e->s));
+  uint32_t total = 0;   // at most V: a row is evicted once
+  for (uint32_t i = 0; i < n; ++i) {
+    out->victim_offset[i] = total;
+    total += out->n_victims[i];
+  }
+  out->victim_offset[n] = total;
+  out->victims_total = total;
+  if (total > out->victims_cap) return fail(e, BS_E_INVAL, "bs_preempt_walk: victims_cap is smaller than victims_total");
+  if (!total) return BS_OK;
+  if (!out->victims) return fail(e, BS_E_INVAL, "bs_preempt_walk: null victims buffer");
   CK(cudaMemcpyAsync(out->victims, a.victims, (size_t)total * 4, cudaMemcpyDeviceToHost, e->s));
   CK(cudaStreamSynchronize(e->s));
   return BS_OK;

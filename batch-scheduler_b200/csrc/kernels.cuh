@@ -244,6 +244,24 @@ __device__ __forceinline__ uint64_t ratio_term(uint32_t weight, uint32_t num, ui
 // The round's kernels.  A translation unit that needs only the helpers above (priority_inst.cu) defines
 // BS_KERNELS_HELPERS_ONLY, so that these external kernels are defined once, in engine.cu.
 #ifndef BS_KERNELS_HELPERS_ONLY
+// node_left_kernel's per-node code, shared with bs_preempt_walk's commit step: the scalar keys of the residuals
+// (alloc_present & req_present) and lane d's residual at percent 1.0 (singleNodeResource core.go:647-668), or
+// present = false when d is a scalar lane without the key.
+__device__ __forceinline__ uint32_t node_left_keys(const NodeTab& t, uint32_t i) {
+  return t.alloc_present[i] & t.req_present[i] & ~0xFu;
+}
+__device__ __forceinline__ int64_t node_lane_left(const NodeTab& t, uint32_t i, uint32_t both, uint32_t d,
+                                                  bool& present) {
+  present = true;
+  if (d == LANE_PODS) {
+    int64_t pc = t.requested[(size_t)LANE_PODS * t.Npad + i];
+    if (pc == 0) pc = t.pod_count[i];
+    return scale_f32(t.alloc[(size_t)LANE_PODS * t.Npad + i], 1.0f) - pc;
+  }
+  if (d >= 4 && !((both >> d) & 1u)) { present = false; return 0; }
+  return scale_f32(t.alloc[(size_t)d * t.Npad + i], 1.0f) - t.requested[(size_t)d * t.Npad + i];
+}
+
 // ---------------------------------------------------------------------------
 // K1  node_left_kernel — per node: residual capacity at percent 1.0 in the
 // sentinel form the fit kernel consumes (absent scalar lane -> ABSENT_LEFT / ABSENT_LEFT32),
@@ -278,17 +296,8 @@ __global__ void node_left_kernel(NodeTab t, LaneMap lm, int64_t* __restrict__ le
     left_present[i] = 0;
     return;
   }
-  const uint32_t both = t.alloc_present[i] & t.req_present[i] & ~0xFu;
-  auto lane_left = [&](uint32_t d, bool& present) -> int64_t {
-    present = true;
-    if (d == LANE_PODS) {
-      int64_t pc = t.requested[(size_t)LANE_PODS * t.Npad + i];
-      if (pc == 0) pc = t.pod_count[i];
-      return scale_f32(t.alloc[(size_t)LANE_PODS * t.Npad + i], 1.0f) - pc;
-    }
-    if (d >= 4 && !((both >> d) & 1u)) { present = false; return 0; }
-    return scale_f32(t.alloc[(size_t)d * t.Npad + i], 1.0f) - t.requested[(size_t)d * t.Npad + i];
-  };
+  const uint32_t both = node_left_keys(t, i);
+  auto lane_left = [&](uint32_t d, bool& present) -> int64_t { return node_lane_left(t, i, both, d, present); };
   for (uint32_t k = 0; k < lm.LW; ++k) {
     bool pres;
     const int64_t v = lane_left(lm.wide[k], pres);

@@ -2137,18 +2137,23 @@ Status BatchSchedulingPlugin::RemovePod(const Pod& preemptor, const Pod& victim)
   return Status{st.code, buf};   // framework.NewStatus(framework.Unschedulable, err.Error()) (batchscheduler.go:137-141)
 }
 
-Status BatchSchedulingPlugin::RunPreempt(const std::vector<uint32_t>& rows, std::vector<Preemption>* out) {
+Status BatchSchedulingPlugin::RunPreempt(const std::vector<uint32_t>& rows, std::vector<Preemption>* out,
+                                         int walk_flags) {
   const uint32_t n = (uint32_t)rows.size();
   std::vector<int32_t> node(n);
   std::vector<uint32_t> nv(n), cand(n), off(n + 1);
   std::vector<uint32_t> vict;
   bs_preempt_result r{node.data(), nv.data(), cand.data(), off.data(), nullptr, 0, 0};
-  int rc = bs_preempt(eng_, rows.data(), n, &r);
+  auto call = [&] {
+    return walk_flags < 0 ? bs_preempt(eng_, rows.data(), n, &r)
+                          : bs_preempt_walk(eng_, rows.data(), n, (uint32_t)walk_flags, &r, nullptr, nullptr);
+  };
+  int rc = call();
   if (rc == BS_E_INVAL && r.victims_total > 0) {   // the first call sized the victim list
     vict.resize(r.victims_total);
     r.victims = vict.data();
     r.victims_cap = r.victims_total;
-    rc = bs_preempt(eng_, rows.data(), n, &r);
+    rc = call();
   }
   if (rc) return Status{BS_CODE_ERROR, std::string("bsched: ") + bs_strerror(rc) + " (" + bs_last_error(eng_) + ")"};
   out->resize(n);
@@ -2188,6 +2193,40 @@ Status BatchSchedulingPlugin::PreemptAll(std::vector<Preemption>* out) {
     if (prefilter_[i] == BS_PF_PASS && feasible_[i] == 0) rows.push_back(i);
   if (rows.empty()) return Status{};
   Status st = RunPreempt(rows, out);
+  if (!st.ok()) return st;
+  for (size_t k = 0; k < rows.size(); ++k) (*out)[k].uid = pending_uid_[rows[k]];
+  return Status{};
+}
+
+Status BatchSchedulingPlugin::PreemptQueue(std::vector<Preemption>* out, bool gang) {
+  std::lock_guard<std::mutex> lk(mu_);
+  if (!eng_ || !out) return Status{BS_CODE_ERROR, "PreemptQueue: no round has been started"};
+  out->clear();
+  if (!bound_.n) return Status{};
+  // PreemptAll's pods in queue order; with gang units, one unit per group at its first preemptor's place
+  std::vector<std::vector<uint32_t>> units;
+  std::unordered_map<int32_t, size_t> unit_of;
+  for (uint32_t i : order_) {
+    if (prefilter_[i] != BS_PF_PASS || feasible_[i] != 0) continue;
+    const int32_t g = packed_.gid[i];
+    if (gang && g >= 0) {
+      auto it = unit_of.find(g);
+      if (it != unit_of.end()) {
+        std::vector<uint32_t>& u = units[it->second];
+        if (packed_.priority[i] != packed_.priority[u[0]])
+          return Status{BS_CODE_ERROR, "PreemptQueue: the pending pods of group " + group_names_[g] +
+                                           " have different priorities"};
+        u.push_back(i);
+        continue;
+      }
+      unit_of[g] = units.size();
+    }
+    units.push_back({i});
+  }
+  std::vector<uint32_t> rows;
+  for (const std::vector<uint32_t>& u : units) rows.insert(rows.end(), u.begin(), u.end());
+  if (rows.empty()) return Status{};
+  Status st = RunPreempt(rows, out, gang ? (int)BS_PREEMPT_GANG : 0);
   if (!st.ok()) return st;
   for (size_t k = 0; k < rows.size(); ++k) (*out)[k].uid = pending_uid_[rows[k]];
   return Status{};

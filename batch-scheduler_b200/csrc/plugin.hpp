@@ -569,6 +569,11 @@ class BatchSchedulingPlugin {
   // Preempt for every pending pod that passed PreFilter and fits no node (upstream preempts only on a FitError), the
   // victims in Preempt's order
   Status PreemptAll(std::vector<Preemption>* out);
+  // PreemptAll's pods as kube-scheduler preempts them, one per cycle (bs_preempt_walk): in the round's queue_order(),
+  // each seeing the evictions and nominations of those before it.  With `gang`, each group's later preemptors move up
+  // to its first one (the order is kept otherwise) and a group gets nodes for all its preemptors or for none; a group
+  // whose preemptors have different priorities is an error.  Entries in walk order; a rolled-back member has node "".
+  Status PreemptQueue(std::vector<Preemption>* out, bool gang);
   const PackedBound& bound() const { return bound_; }
   // The non-zero request columns of the resource priorities (no GPU): per pending pod and per NodeInfo (over
   // NodeInfo::pods), [2][n] int64 — cpu millicores, memory bytes — summed over the containers' Requests, a container
@@ -686,7 +691,8 @@ class BatchSchedulingPlugin {
   Status UploadLocality();   // both locality sides of snapshot_ and pending_ and the two weights; the columns only
                              // while a weight is non-zero; no-op without priority_k
   Status UploadBound();  // packs and uploads the bound-pod table of snapshot_ (no-op when no NodeInfo lists pods)
-  Status RunPreempt(const std::vector<uint32_t>& rows, std::vector<Preemption>* out);
+  // bs_preempt on `rows`, or with walk_flags >= 0 bs_preempt_walk with those flags
+  Status RunPreempt(const std::vector<uint32_t>& rows, std::vector<Preemption>* out, int walk_flags = -1);
   std::vector<const NodeInfo*> snapshot_;                           // the round's NodeInfos (bound pods)
   std::vector<std::string> pending_uid_;                            // pending index -> uid
   std::vector<const Pod*> pending_;                                 // the round's pending pods (preferences)

@@ -17,7 +17,8 @@ namespace bsk {
 
 // bound-pod table grouped by node (CSR), columns in CSR position order
 struct BoundTab {
-  const uint32_t* row;      // [N + 1] segment of node n: [row[n], row[n + 1])
+  const uint32_t* row;      // [N + 1] segment of node n: [row[n], end[n])
+  const uint32_t* end;      // [N] segment ends: row + 1, or bs_preempt_walk's live ends (evicted rows leave)
   const int32_t* prio;      // [V]
   const int64_t* start;     // [V]
   const int32_t* gid;       // [V]
@@ -80,18 +81,11 @@ __device__ __forceinline__ PickKey pick_none() {
   return k;
 }
 
-// ---------------------------------------------------------------------------
-// preempt_prep_kernel — once per bound-table upload, one thread per node: suffix sums of the removable lanes and
-// suffix counts of the online, the missing-or-locked and the PDB-violating rows, walking the node's segment from its
-// end.
-__global__ void preempt_prep_kernel(const uint32_t* __restrict__ row, const int32_t* __restrict__ gid,
-                                    const uint8_t* __restrict__ flags, const int64_t* __restrict__ req,
-                                    int64_t* __restrict__ suf, uint32_t* __restrict__ suf_online,
-                                    uint32_t* __restrict__ suf_bad, uint32_t* __restrict__ suf_vio, uint32_t N,
-                                    uint32_t V, uint32_t L) {
-  const uint32_t n = blockIdx.x * blockDim.x + threadIdx.x;
-  if (n >= N) return;
-  const uint32_t b = row[n], e = row[n + 1];
+// The suffix sums of the removable lanes and the suffix counts of the online, the missing-or-locked and the
+// PDB-violating rows of one node's segment [b, e), walking it from its end.
+__device__ __forceinline__ void prep_node(uint32_t b, uint32_t e, const int32_t* gid, const uint8_t* flags,
+                                          const int64_t* req, int64_t* suf, uint32_t* suf_online, uint32_t* suf_bad,
+                                          uint32_t* suf_vio, uint32_t V, uint32_t L) {
   uint32_t on = 0, bad = 0, vio = 0;
   for (uint32_t k = e; k-- > b;) {
     const int32_t g = gid[k];
@@ -110,6 +104,18 @@ __global__ void preempt_prep_kernel(const uint32_t* __restrict__ row, const int3
       suf[(size_t)d * V + k] = s;
     }
   }
+}
+
+// ---------------------------------------------------------------------------
+// preempt_prep_kernel — once per bound-table upload, one thread per node: prep_node over the node's segment.
+__global__ void preempt_prep_kernel(const uint32_t* __restrict__ row, const int32_t* __restrict__ gid,
+                                    const uint8_t* __restrict__ flags, const int64_t* __restrict__ req,
+                                    int64_t* __restrict__ suf, uint32_t* __restrict__ suf_online,
+                                    uint32_t* __restrict__ suf_bad, uint32_t* __restrict__ suf_vio, uint32_t N,
+                                    uint32_t V, uint32_t L) {
+  const uint32_t n = blockIdx.x * blockDim.x + threadIdx.x;
+  if (n >= N) return;
+  prep_node(row[n], row[n + 1], gid, flags, req, suf, suf_online, suf_bad, suf_vio, V, L);
 }
 
 struct PreemptArgs {
@@ -167,7 +173,7 @@ __device__ bool select_victims(const PreemptArgs& a, const PreemptPod& q, const 
   if (node_skipped(f) || (f & BS_NODE_TAINTS_ERR) || !check_fit(t.label[n], t.taint[n], q.sel, q.tol) ||
       !aff_ok(t, q.aff, n) || (q.nz & ~a.left_present[n]) != 0)
     return false;
-  const uint32_t beg = a.b.row[n], end = a.b.row[n + 1];
+  const uint32_t beg = a.b.row[n], end = a.b.end[n];
   // potential victims: priority strictly below the preemptor's, a suffix of the segment
   uint32_t lo = beg, hi = end;
   while (lo < hi) {
@@ -249,19 +255,9 @@ __device__ __forceinline__ uint32_t load_req(const PreemptArgs& a, const Preempt
   return a.preq_present[q.pod];
 }
 
-// preempt_node_kernel — the hot path: block (tile, preemptor) evaluates PREEMPT_THREADS nodes for one preemptor and
-// writes the tile's best key (and its candidate count).  The key is a total order (the node index decides last),
-// so the tree below gives the same winner as a walk in node order.  At MAXL 5 the bound holds 64 registers, four
-// blocks per SM, without spills (the PDB pass would otherwise take it to 72 and three blocks).
-template <int MAXL>
-__global__ void __launch_bounds__(PREEMPT_THREADS, MAXL <= 5 ? 4 : 1) preempt_node_kernel(PreemptArgs a) {
-  const uint32_t i = a.p0 + blockIdx.y;
-  const uint32_t n = blockIdx.x * PREEMPT_THREADS + threadIdx.x;
-  const PreemptPod q = a.pp[i];
-  int64_t req[MAXL];
-  const uint32_t rpres = load_req<MAXL>(a, q, req);
-  PickKey key = pick_none();
-  if (n < a.t.N && !select_victims<MAXL, false>(a, q, req, rpres, n, key, nullptr)) key = pick_none();
+// The smallest key of a PREEMPT_THREADS-thread block (pick_min over the warps, then over the warp minima), valid in
+// thread 0.
+__device__ __forceinline__ PickKey block_pick_min(PickKey key) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     PickKey k2;
@@ -277,11 +273,26 @@ __global__ void __launch_bounds__(PREEMPT_THREADS, MAXL <= 5 ? 4 : 1) preempt_no
   __shared__ PickKey s_key[PREEMPT_THREADS / 32];
   if ((threadIdx.x & 31) == 0) s_key[threadIdx.x >> 5] = key;
   __syncthreads();
-  if (threadIdx.x == 0) {
-    PickKey r = s_key[0];
-    for (int w = 1; w < PREEMPT_THREADS / 32; ++w) r = pick_min(r, s_key[w]);
-    a.tiles[(size_t)blockIdx.y * a.n_tiles + blockIdx.x] = r;
-  }
+  if (threadIdx.x == 0)
+    for (int w = 1; w < PREEMPT_THREADS / 32; ++w) key = pick_min(key, s_key[w]);
+  return key;
+}
+
+// preempt_node_kernel — the hot path: block (tile, preemptor) evaluates PREEMPT_THREADS nodes for one preemptor and
+// writes the tile's best key (and its candidate count).  The key is a total order (the node index decides last),
+// so the tree below gives the same winner as a walk in node order.  At MAXL 5 the bound holds 64 registers, four
+// blocks per SM, without spills (the PDB pass would otherwise take it to 72 and three blocks).
+template <int MAXL>
+__global__ void __launch_bounds__(PREEMPT_THREADS, MAXL <= 5 ? 4 : 1) preempt_node_kernel(PreemptArgs a) {
+  const uint32_t i = a.p0 + blockIdx.y;
+  const uint32_t n = blockIdx.x * PREEMPT_THREADS + threadIdx.x;
+  const PreemptPod q = a.pp[i];
+  int64_t req[MAXL];
+  const uint32_t rpres = load_req<MAXL>(a, q, req);
+  PickKey key = pick_none();
+  if (n < a.t.N && !select_victims<MAXL, false>(a, q, req, rpres, n, key, nullptr)) key = pick_none();
+  key = block_pick_min(key);
+  if (threadIdx.x == 0) a.tiles[(size_t)blockIdx.y * a.n_tiles + blockIdx.x] = key;
 }
 
 // preempt_reduce_kernel — one thread per preemptor of the launch: the tiles in node order
@@ -308,6 +319,196 @@ __global__ void preempt_emit_kernel(PreemptArgs a) {
   const uint32_t rpres = load_req<MAXL>(a, q, req);
   PickKey key;
   select_victims<MAXL, true>(a, q, req, rpres, (uint32_t)n, key, a.victims + a.offset[i]);
+}
+
+// ---------------------------------------------------------------------------
+// bs_preempt_walk (DESIGN.md §2 "Preemption"): the preemptors in list order over a private copy of the node and bound
+// state.  Step i is preempt_node_kernel for preemptor i against the live state, then preempt_commit_kernel, which
+// picks the node, writes the victims, evicts them (the segment is compacted in order and its suffixes rebuilt),
+// nominates the preemptor (bs_replay's assume) and rebuilds the node's residuals.  With gang units, every commit of
+// the open unit is logged, and the unit's last step undoes the unit from the log when a member got no node.
+
+enum : uint32_t { WALK_NONE = 0, WALK_NOMINATED = 1, WALK_ROLLED_BACK = 2 };   // BS_WALK_*
+
+// the walk's running counters (device memory, zeroed once per call)
+struct WalkCtl {
+  uint32_t voff;         // victims written so far
+  uint32_t unit_first;   // first step of the open unit
+  uint32_t unit_voff;    // voff when the open unit began
+  uint32_t failed;       // a member of the open unit got no node
+  uint32_t n_ent;        // log entries of the open unit
+  uint32_t n_rows;       // logged rows of the open unit
+};
+
+struct WalkArgs {
+  // the live copies behind PreemptArgs' const views (a.b, a.t.requested / req_present / pod_count, a.left)
+  uint32_t* end;
+  int32_t* prio;
+  int64_t* start;
+  int32_t* gid;
+  uint8_t* flags;
+  uint32_t* idx;
+  int64_t* req;
+  int64_t* suf;
+  uint32_t *suf_online, *suf_bad, *suf_vio;
+  int64_t* requested;       // [L][Npad]
+  uint32_t* req_present;    // [Npad]
+  int32_t* pod_count;       // [Npad]
+  int64_t* left;            // [L][Npad]
+  uint32_t* left_present;   // [Npad]
+  int32_t* evicted_by;      // [V] by bound-table index: the step that evicted the row, -1
+  uint32_t* outcome;        // [n] WALK_*
+  const uint8_t* unit_last; // [n] step i closes its unit
+  WalkCtl* ctl;
+  // the undo log of the open unit (gang units only; null otherwise): per commit the node, its segment end, victim
+  // count and first logged row, and its requested / req_present / pod_count before the commit; per evicted row its
+  // position in the segment before the commit and its columns
+  uint32_t *ent_node, *ent_end, *ent_nv, *ent_row;
+  int64_t* ent_req;         // [L][n]
+  uint32_t* ent_rp;
+  int32_t* ent_pc;
+  uint32_t* row_pos;        // [V]
+  int32_t* row_prio;
+  int64_t* row_start;
+  int32_t* row_gid;
+  uint8_t* row_flags;
+  uint32_t* row_idx;
+  int64_t* row_req;         // [L][V]
+  uint32_t n;
+};
+
+// Rebuilds node n's suffixes and residuals from its live segment and its live requested / req_present / pod_count.
+__device__ __forceinline__ void walk_refresh_node(const PreemptArgs& a, const WalkArgs& w, uint32_t n) {
+  const uint32_t V = a.b.V, L = a.t.L;
+  prep_node(a.b.row[n], w.end[n], w.gid, w.flags, w.req, w.suf, w.suf_online, w.suf_bad, w.suf_vio, V, L);
+  const uint32_t both = node_left_keys(a.t, n);
+  for (uint32_t d = 0; d < L; ++d) {
+    bool pres;
+    const int64_t v = node_lane_left(a.t, n, both, d, pres);
+    w.left[(size_t)d * a.t.Npad + n] = pres ? v : 0;
+  }
+  w.left_present[n] = both;
+}
+
+// Step i's pick, victims, eviction and nomination, and at the end of a failed unit its undo.  One CTA; the tiles of
+// preempt_node_kernel are reduced by the whole block, the rest runs on thread 0 (one node's segment).
+template <int MAXL>
+__global__ void __launch_bounds__(PREEMPT_THREADS) preempt_commit_kernel(PreemptArgs a, WalkArgs w, uint32_t i) {
+  PickKey key = pick_none();
+  for (uint32_t tl = threadIdx.x; tl < a.n_tiles; tl += PREEMPT_THREADS) key = pick_min(key, a.tiles[tl]);
+  key = block_pick_min(key);
+  if (threadIdx.x != 0) return;
+  WalkCtl& c = *w.ctl;
+  const uint32_t L = a.t.L, V = a.b.V, Npad = a.t.Npad;
+  a.out_cand[i] = key.cand;
+  if (key.node < 0) {
+    a.out_node[i] = -1;
+    a.out_nv[i] = 0;
+    w.outcome[i] = WALK_NONE;
+    c.failed = 1;
+  } else {
+    const uint32_t n = (uint32_t)key.node;
+    const PreemptPod q = a.pp[i];
+    int64_t req[MAXL];
+    const uint32_t rpres = load_req<MAXL>(a, q, req);
+    uint32_t* vict = a.victims + c.voff;
+    PickKey k2;
+    select_victims<MAXL, true>(a, q, req, rpres, n, k2, vict);
+    const uint32_t nv = k2.nv;
+    a.out_node[i] = (int32_t)n;
+    a.out_nv[i] = nv;
+    w.outcome[i] = WALK_NOMINATED;
+    c.voff += nv;
+    for (uint32_t j = 0; j < nv; ++j) w.evicted_by[vict[j]] = (int32_t)i;
+    const uint32_t beg = a.b.row[n], end = w.end[n];
+    if (w.ent_node) {   // log the node before the commit
+      const uint32_t e = c.n_ent++;
+      w.ent_node[e] = n;
+      w.ent_end[e] = end;
+      w.ent_nv[e] = nv;
+      w.ent_row[e] = c.n_rows;
+      for (uint32_t d = 0; d < L; ++d) w.ent_req[(size_t)d * w.n + e] = w.requested[(size_t)d * Npad + n];
+      w.ent_rp[e] = w.req_present[n];
+      w.ent_pc[e] = w.pod_count[n];
+    }
+    // evict: the victims leave the segment (order kept) and NodeInfo.RemovePod takes their Requests
+    uint32_t dst = beg;
+    for (uint32_t k = beg; k < end; ++k) {
+      if (w.evicted_by[w.idx[k]] == (int32_t)i) {
+        for (uint32_t d = 0; d < L; ++d) w.requested[(size_t)d * Npad + n] -= w.req[(size_t)d * V + k];
+        if (w.ent_node) {
+          const uint32_t r = c.n_rows++;
+          w.row_pos[r] = k - beg;
+          w.row_prio[r] = w.prio[k];
+          w.row_start[r] = w.start[k];
+          w.row_gid[r] = w.gid[k];
+          w.row_flags[r] = w.flags[k];
+          w.row_idx[r] = w.idx[k];
+          for (uint32_t d = 0; d < L; ++d) w.row_req[(size_t)d * V + r] = w.req[(size_t)d * V + k];
+        }
+        continue;
+      }
+      if (dst != k) {
+        w.prio[dst] = w.prio[k];
+        w.start[dst] = w.start[k];
+        w.gid[dst] = w.gid[k];
+        w.flags[dst] = w.flags[k];
+        w.idx[dst] = w.idx[k];
+        for (uint32_t d = 0; d < L; ++d) w.req[(size_t)d * V + dst] = w.req[(size_t)d * V + k];
+      }
+      ++dst;
+    }
+    w.end[n] = dst;
+    // nominate: bs_replay's assume (NodeInfo.AddPod): the pod's request on every lane but 3 and its scalar keys
+    for (uint32_t d = 0; d < L; ++d)
+      if (d != LANE_PODS && (d < 4 || ((rpres >> d) & 1u)))
+        w.requested[(size_t)d * Npad + n] += a.preq[(size_t)d * a.P + q.pod];
+    w.req_present[n] |= rpres & ~0xFu;
+    w.pod_count[n] += 1 - (int32_t)nv;
+    walk_refresh_node(a, w, n);
+  }
+  if (!w.unit_last[i]) return;
+  if (c.failed && w.ent_node) {   // undo the unit, last commit first
+    for (uint32_t e = c.n_ent; e-- > 0;) {
+      const uint32_t n = w.ent_node[e], beg = a.b.row[n], nv = w.ent_nv[e], r0 = w.ent_row[e];
+      uint32_t src = w.end[n], j = nv;
+      for (uint32_t k = w.ent_end[e]; k-- > beg;) {
+        if (j > 0 && beg + w.row_pos[r0 + j - 1] == k) {
+          const uint32_t r = r0 + --j;
+          w.prio[k] = w.row_prio[r];
+          w.start[k] = w.row_start[r];
+          w.gid[k] = w.row_gid[r];
+          w.flags[k] = w.row_flags[r];
+          w.idx[k] = w.row_idx[r];
+          for (uint32_t d = 0; d < L; ++d) w.req[(size_t)d * V + k] = w.row_req[(size_t)d * V + r];
+          w.evicted_by[w.row_idx[r]] = -1;
+        } else if (--src != k) {
+          w.prio[k] = w.prio[src];
+          w.start[k] = w.start[src];
+          w.gid[k] = w.gid[src];
+          w.flags[k] = w.flags[src];
+          w.idx[k] = w.idx[src];
+          for (uint32_t d = 0; d < L; ++d) w.req[(size_t)d * V + k] = w.req[(size_t)d * V + src];
+        }
+      }
+      w.end[n] = w.ent_end[e];
+      for (uint32_t d = 0; d < L; ++d) w.requested[(size_t)d * Npad + n] = w.ent_req[(size_t)d * w.n + e];
+      w.req_present[n] = w.ent_rp[e];
+      w.pod_count[n] = w.ent_pc[e];
+      walk_refresh_node(a, w, n);
+    }
+    for (uint32_t k = c.unit_first; k <= i; ++k) {
+      a.out_node[k] = -1;
+      a.out_nv[k] = 0;
+      w.outcome[k] = WALK_ROLLED_BACK;
+    }
+    c.voff = c.unit_voff;
+  }
+  c.unit_first = i + 1;
+  c.unit_voff = c.voff;
+  c.failed = 0;
+  c.n_ent = 0;
+  c.n_rows = 0;
 }
 
 }  // namespace bsk

@@ -26,6 +26,14 @@ class PreemptResult:
 
 
 @dataclass
+class PreemptWalkResult(PreemptResult):
+    """bs_preempt_walk's outputs: PreemptResult's fields for the walk, plus per preemptor its outcome (capi.WALK_*)
+    and per bound row the list position whose step evicted it (-1 none)."""
+    outcome: np.ndarray = None      # uint32 [n]
+    evicted_by: np.ndarray = None   # int32 [V]
+
+
+@dataclass
 class RoundResult:
     prefilter: np.ndarray
     feasible_count: np.ndarray
@@ -82,6 +90,7 @@ class Engine:
             raise capi.BsError(rc, self.lib.bs_strerror(rc).decode())
         self.h = h
         self.P = self.N = self.G = 0
+        self._bound_rows = 0   # rows of the last bound-pod table uploaded (preempt_walk's evicted_by)
         self._res = None
 
     # -- lifecycle -------------------------------------------------------------------------
@@ -501,6 +510,7 @@ class Engine:
     def upload_bound_pods(self, bt: BoundPodTable):
         """The pods bound to the uploaded nodes (upload nodes and groups first; either upload drops this table)."""
         self._check(self.lib.bs_upload_bound_pods(self.h, C.byref(_table_c(bt))))
+        self._bound_rows = bt.n
 
     def preempt(self, pods, victims_cap=None) -> PreemptResult:
         """For every pod index in `pods`: the node preemption would pick and the pods it would evict there.
@@ -519,6 +529,28 @@ class Engine:
                 continue
             self._check(rc)
             return PreemptResult(node, nv, cand, off, vict[:r.victims_total].copy())
+
+    def preempt_walk(self, pods, gang=False, victims_cap=None) -> PreemptWalkResult:
+        """The preemptors of `pods` one after another in list order (priorities non-increasing), each seeing the
+        evictions and nominations of those before it; with `gang`, the preemptors of one group (contiguous in the
+        list) are preempted for all together or not at all.  victims_cap as in preempt()."""
+        idx = np.ascontiguousarray(pods, dtype=np.uint32)
+        n = len(idx)
+        node, nv, cand = np.zeros(n, np.int32), np.zeros(n, np.uint32), np.zeros(n, np.uint32)
+        off, outcome = np.zeros(n + 1, np.uint32), np.zeros(n, np.uint32)
+        evicted_by = np.zeros(self._bound_rows, np.int32)
+        flags = capi.PREEMPT_GANG if gang else 0
+        cap = 0 if victims_cap is None else victims_cap
+        while True:
+            vict = np.zeros(max(cap, 1), np.uint32)
+            r = capi.PreemptResultC(capi.ptr(node), capi.ptr(nv), capi.ptr(cand), capi.ptr(off), capi.ptr(vict), cap, 0)
+            rc = self.lib.bs_preempt_walk(self.h, capi.ptr(idx) if n else None, n, flags, C.byref(r),
+                                          capi.ptr(outcome) if n else None, capi.ptr(evicted_by))
+            if rc == capi.BS_E_INVAL and victims_cap is None and r.victims_total > cap:
+                cap = r.victims_total
+                continue
+            self._check(rc)
+            return PreemptWalkResult(node, nv, cand, off, vict[:r.victims_total].copy(), outcome, evicted_by)
 
     def remove_pod(self, pod: int, bound: int):
         """batchSchedulingPluginExtension.RemovePod for pod `pod` and bound pod `bound`: (code, reason, group)."""

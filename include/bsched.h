@@ -724,6 +724,39 @@ typedef struct {
  * change, any round's state or outputs. */
 int bs_preempt(bs_engine* e, const uint32_t* pods, uint32_t n, bs_preempt_result* out);
 
+/* bs_preempt_walk: the preemptors one after another, as kube-scheduler preempts one pod per cycle (DESIGN.md §2
+ * "Preemption").  pods[0..n) is walked in list order over a private copy of the node and bound state: step i is
+ * bs_preempt for pods[i] on the state the steps before it left.  When step i picks a node, its victims leave that
+ * node's bound pods (NodeInfo.RemovePod: Requests on lanes 0-2 and the row's scalar keys, one pod fewer; an evicted
+ * row is never a potential victim again), and the preemptor is nominated there by bs_replay's assume rule (the pod
+ * table's request on every lane but 3, its scalar keys ORed into req_present, one pod more).  A nominated pod is
+ * never a victim.  Victims leave at once (graceful termination is not modelled); PreemptionPolicy is not modelled.
+ *
+ * Rules, each BS_E_INVAL: priorities must be non-increasing along the list (queue order satisfies it; every earlier
+ * nomination then counts for later preemptors and none is ever cleared); a pod listed twice; flag bits other than
+ * BS_PREEMPT_GANG; with BS_PREEMPT_GANG, the preemptors of one group (gid >= 0) not contiguous.
+ *
+ * BS_PREEMPT_GANG: the preemptors of one group form a unit (online and missing-group pods, and pods whose gid is
+ * >= n_groups, are units of one).  When
+ * a unit's last member has been walked and some member got no node, the unit is undone: the state is the one before
+ * it, and every member reports node -1, 0 victims and BS_WALK_ROLLED_BACK.  A gang succeeds when every listed member
+ * got a node, so the caller lists the members the gang needs.
+ *
+ * out is bs_preempt's result: n_candidates counts against the live state; victims come per preemptor in reprieve
+ * order with the same victims_cap / victims_total contract; victims_total <= n_pods of the bound table (each row is
+ * evicted at most once).  outcome[n] (NULL allowed) gets a bs_walk_outcome per preemptor; evicted_by[V] (NULL
+ * allowed, V = the bound table's n_pods) gets the list position whose step evicted bound row v, or -1.  The errors of
+ * bs_preempt apply, and BS_E_RANGE when the live sums could pass 2^62 (bs_replay's bound).  The uploaded tables, the
+ * round's state and bs_preempt's answers are unchanged by the call. */
+#define BS_PREEMPT_GANG 0x1u
+typedef enum {
+  BS_WALK_NONE = 0,        /* no candidate node */
+  BS_WALK_NOMINATED = 1,   /* nominated to out->node[i]; its victims are evicted */
+  BS_WALK_ROLLED_BACK = 2  /* a member of its unit got no node: the unit was undone */
+} bs_walk_outcome;
+int bs_preempt_walk(bs_engine* e, const uint32_t* pods, uint32_t n, uint32_t flags, bs_preempt_result* out,
+                    uint32_t* outcome, int32_t* evicted_by);
+
 /* RemovePod verdicts (core.PreemptRemovePod, core.go:203-260) */
 typedef enum {
   BS_REMOVE_ALLOW = 0,

@@ -522,6 +522,62 @@ func (e *Engine) Preempt(pods []uint32) ([]Preemption, error) {
 	return out, nil
 }
 
+// WalkOutcome is one preemptor's outcome in PreemptWalk (bs_walk_outcome).
+type WalkOutcome uint32
+
+const (
+	WalkNone       WalkOutcome = C.BS_WALK_NONE        // no candidate node
+	WalkNominated  WalkOutcome = C.BS_WALK_NOMINATED   // nominated to Node; its victims are evicted
+	WalkRolledBack WalkOutcome = C.BS_WALK_ROLLED_BACK // a member of its gang unit got no node: the unit was undone
+)
+
+// PreemptWalk preempts for the pod rows of pods one after another, as kube-scheduler does one pod per cycle: each
+// preemptor sees the evictions and nominations of those before it (bs_preempt_walk; DESIGN.md §2 "Preemption").
+// Priorities must not rise along pods.  With gang, the rows of one group must be contiguous, and a group gets nodes
+// for all its rows or for none.  evictedBy[v] is the position in pods whose step evicted bound-pod row v, or -1.
+func (e *Engine) PreemptWalk(pods []uint32, gang bool, nBound int) (out []Preemption, outcome []WalkOutcome,
+	evictedBy []int32, err error) {
+	n := len(pods)
+	out = make([]Preemption, n)
+	outcome = make([]WalkOutcome, n)
+	evictedBy = make([]int32, nBound+1)
+	node := make([]int32, n+1)
+	nv := make([]uint32, n+1)
+	cand := make([]uint32, n+1)
+	off := make([]uint32, n+1)
+	oc := make([]uint32, n+1)
+	flags := C.uint32_t(0)
+	if gang {
+		flags = C.BS_PREEMPT_GANG
+	}
+	r := C.bs_preempt_result{node: (*C.int32_t)(unsafe.Pointer(&node[0])), n_victims: (*C.uint32_t)(unsafe.Pointer(&nv[0])),
+		n_candidates: (*C.uint32_t)(unsafe.Pointer(&cand[0])), victim_offset: (*C.uint32_t)(unsafe.Pointer(&off[0]))}
+	var p *C.uint32_t
+	if n > 0 {
+		p = (*C.uint32_t)(unsafe.Pointer(&pods[0]))
+	}
+	call := func() C.int {
+		return C.bs_preempt_walk(e.h, p, C.uint32_t(n), flags, &r, (*C.uint32_t)(unsafe.Pointer(&oc[0])),
+			(*C.int32_t)(unsafe.Pointer(&evictedBy[0])))
+	}
+	rc := call()
+	var victims []uint32
+	if rc == C.BS_E_INVAL && r.victims_total > 0 { // the first call sized the victim list
+		victims = make([]uint32, int(r.victims_total))
+		r.victims = (*C.uint32_t)(unsafe.Pointer(&victims[0]))
+		r.victims_cap = r.victims_total
+		rc = call()
+	}
+	if err := e.rc(rc); err != nil {
+		return nil, nil, nil, err
+	}
+	for i := 0; i < n; i++ {
+		out[i] = Preemption{Node: node[i], Victims: append([]uint32(nil), victims[off[i]:off[i+1]]...), Candidates: cand[i]}
+		outcome[i] = WalkOutcome(oc[i])
+	}
+	return out, outcome, evictedBy[:nBound], nil
+}
+
 // Permit mirrors batchSchedulingPlugin.Permit (batchscheduler.go:165-202) with core.Permit's bookkeeping
 // (core.go:268-309) against the engine's tables: ready only once len(MatchedPodNodes.Items()) reaches
 // MinMember - Status.Scheduled.
