@@ -21,7 +21,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libbsched.so")
 OBJ = os.path.join(HERE, "build")
-HEADERS = ["devmem.hpp", "common.cuh", "kernels.cuh", "fit.cuh", "sort.cuh", "replay.cuh", "preempt.cuh", "priority.cuh", "plugin.hpp",
+HEADERS = ["devmem.hpp", "common.cuh", "kernels.cuh", "fit.cuh", "sort.cuh", "replay.cuh", "preempt.cuh", "priority.cuh", "interpod_filter.cuh",
+           "plugin.hpp",
            os.path.join("..", "..", "include", "bsched.h")]
 FIT_SLICES = 9
 

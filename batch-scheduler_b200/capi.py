@@ -36,6 +36,8 @@ SPREAD_COUNT_MAX = 1 << 24   # BS_SPREAD_COUNT_MAX: largest selector count
 SPREAD_TABLE_MAX_BYTES = 1 << 30   # BS_SPREAD_TABLE_MAX_BYTES: cap of the class x node count table
 IPA_NONE = 0xffffffff     # BS_IPA_NONE: class of a pod or bound pod without entries
 TOPO_NONE = 0xffffffff    # BS_TOPO_NONE: topo value of a node without the key
+IPF_NONE = 0xffffffff     # BS_IPF_NONE: filter class of a pod without entries (passes every node)
+IPF_AFFINITY, IPF_ANTI, IPF_EXISTING = range(3)   # BS_IPF_*: roles of a pod's filter class entries
 IPA_KEY_MAX = 64          # BS_IPA_KEY_MAX: topology keys of one node side
 IPA_BOUND_MAX = 1 << 24   # BS_IPA_BOUND_MAX: bound pods of one node side
 IPA_CLASS_MAX = 64        # BS_IPA_CLASS_MAX: entries of one class
@@ -116,6 +118,11 @@ class InterpodNodesC(C.Structure):
 
 class InterpodPodsC(C.Structure):
     _fields_ = [("n_pods", C.c_uint32), ("pod_class", C.c_void_p), ("classes", InterpodClassesC)]
+
+
+class InterpodFilterPodsC(C.Structure):
+    _fields_ = [("n_pods", C.c_uint32), ("pod_class", C.c_void_p), ("n_classes", C.c_uint32),
+                ("class_offset", C.c_void_p), ("term", C.c_void_p), ("role", C.c_void_p), ("self_match", C.c_void_p)]
 
 
 class PreemptResultC(C.Structure):
@@ -212,6 +219,12 @@ SYMBOLS = {
     "bs_set_interpod_weight": (C.c_int, [C.c_void_p, C.c_uint32]),
     "bs_upload_node_interpod": (C.c_int, [C.c_void_p, _p(InterpodNodesC)]),
     "bs_upload_pod_interpod": (C.c_int, [C.c_void_p, _p(InterpodPodsC)]),
+    "bs_set_interpod_filter": (C.c_int, [C.c_void_p, C.c_int]),
+    "bs_upload_node_interpod_filter": (C.c_int, [C.c_void_p, _p(InterpodNodesC)]),
+    "bs_upload_pod_interpod_filter": (C.c_int, [C.c_void_p, _p(InterpodFilterPodsC)]),
+    "bs_fetch_interpod_reason_rows": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]),
+    "bs_format_fit_error_interpod": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_char_p,
+                                               C.c_size_t]),
     "bs_peer_init": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32]),
     "bs_peer_handle": (C.c_int, [C.c_void_p, C.c_void_p]),
     "bs_peer_attach": (C.c_int, [C.c_void_p, C.c_void_p]),

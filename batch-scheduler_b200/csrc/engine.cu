@@ -24,6 +24,7 @@
 
 #include "devmem.hpp"
 #include "kernels.cuh"
+#include "interpod_filter.cuh"
 #include "fit.cuh"
 #include "gang_state.hpp"
 #include "sort.cuh"
@@ -166,7 +167,10 @@ struct ClassKey {
   uint64_t sel, tol;
   uint32_t nz;
   uint32_t aff;   // affinity class (row of the bs_upload_affinity table) or BS_AFF_NONE
-  bool operator==(const ClassKey& o) const { return sel == o.sel && tol == o.tol && nz == o.nz && aff == o.aff; }
+  uint32_t ipf = BS_IPF_NONE;   // MatchInterPodAffinity filter class while the filter is on, else BS_IPF_NONE
+  bool operator==(const ClassKey& o) const {
+    return sel == o.sel && tol == o.tol && nz == o.nz && aff == o.aff && ipf == o.ipf;
+  }
 };
 
 // flat open-addressing index ClassKey -> dense id (insertion order)
@@ -178,7 +182,7 @@ struct ClassIndex {
   uint32_t last_id = 0;
   static uint64_t hash(const ClassKey& k) {
     uint64_t h = k.sel * 0x9E3779B97F4A7C15ull ^ (k.tol + 0x7F4A7C15ull) * 0xBF58476D1CE4E5B9ull ^
-                 ((uint64_t)k.nz | ((uint64_t)k.aff << 32)) * 0x94D049BB133111EBull;
+                 ((uint64_t)k.nz | ((uint64_t)k.aff << 32)) * 0x94D049BB133111EBull ^ (uint64_t)(k.ipf + 1u) * 0xD6E8FEB86659FD93ull;
     return h ^ (h >> 29);
   }
   void clear() {
@@ -473,6 +477,23 @@ struct bs_engine {
   uint32_t ipa_terms = 0, ipa_bound = 0, ipa_bclasses = 0, ipa_pclasses = 0;
   uint64_t ipa_slots = 0;
   int64_t ipa_term_max = -1;
+  // MatchInterPodAffinity filter (bs_set_interpod_filter; off by default): the node side (topology values, each term's
+  // key and first slot, the bound pods and their class table; dropped with the node table) and the pod side (each pod's
+  // filter class h_ipf_class, the class table; dropped with the pod table).  The presence planes d_ipf_presence
+  // ([2][words]: match, own), the per-term counts d_ipf_hits and the class planes d_ipf_bits ([3][classes][Npad/32]:
+  // pass, E, A) are built on the device when ipf_dirty.  ipf_assign_dirty: the pods' fit classes have to be assigned
+  // again (with their filter class while the filter is on, else their base class h_pfc_base).  d_fipf: each fit class's
+  // filter class, d_reason_gate_ipf the priority lists' gate, d_ipf_reasons the companion rows [P][3].
+  bool ipf_on = false, ipf_round = false;
+  DevBuf d_ipf_topo, d_ipf_term_key, d_ipf_term_off, d_ipf_bound_node, d_ipf_bound_class;
+  DevBuf d_ipf_boff, d_ipf_bterm, d_ipf_bown, d_ipf_bmatch, d_ipf_presence, d_ipf_hits;
+  DevBuf d_ipf_poff, d_ipf_pterm, d_ipf_prole, d_ipf_pself, d_ipf_bits, d_fipf, d_reason_gate_ipf, d_ipf_reasons;
+  bool have_ipf_node = false, have_ipf_pod = false, ipf_dirty = true, ipf_assign_dirty = false;
+  uint32_t ipf_terms = 0, ipf_bound = 0, ipf_pclasses = 0;
+  uint64_t ipf_slots = 0;
+  int64_t ipf_term_max = -1;
+  std::vector<uint32_t> h_ipf_class, h_pfc_base;   // h_pfc_base: the pods' fit classes without the filter
+  bool pfc_base_valid = false;                     // h_pfc_base holds the classes of the pod table of now
   // sort scratch: views into one arena
   View d_gk0, d_gk1, d_pk0, d_pk1, d_idx_a, d_idx_b, d_ghist, d_group_rank, d_tilecnt, d_sort_barrier;
   uint32_t sort_max_grid = 1;
@@ -958,6 +979,31 @@ inline uint64_t low_bits_mask(uint32_t n) {  // mask covering every value in [0,
   return m;
 }
 
+// The fit index only grows.  While the filter is on, every pod-side upload and every switch adds (class, filter class)
+// keys, so after each re-assignment the index is rebuilt from the classes the pods use when those are a small share
+// of it (the bound bs_upload_pods applies to stale classes); the base ids of h_pfc_base follow.
+void compact_fit_index(bs_engine* e) {
+  ClassIndex& fi = e->fit_index;
+  const uint32_t P = e->P;
+  uint32_t* pfc = e->h_pfc.data();
+  uint32_t* base = e->pfc_base_valid ? e->h_pfc_base.data() : nullptr;
+  std::vector<uint8_t> used(fi.size(), 0);
+  size_t n_used = 0;
+  auto mark = [&](uint32_t id) { n_used += used[id] ? 0 : 1; used[id] = 1; };
+  for (uint32_t p = 0; p < P; ++p) {
+    mark(pfc[p]);
+    if (base) mark(base[p]);
+  }
+  if (fi.size() <= std::max<size_t>(4096, 4 * n_used)) return;
+  ClassIndex ni;
+  ni.clear();
+  for (uint32_t p = 0; p < P; ++p) {
+    if (base) base[p] = ni.get_or_add(fi.keys[base[p]]);
+    pfc[p] = ni.get_or_add(fi.keys[pfc[p]]);
+  }
+  fi = std::move(ni);
+}
+
 int rebuild_classes(bs_engine* e) {
   // Pod classes were indexed while the pod table was uploaded; group representative classes are
   // looked up here (the representative index must already hold the pods' (sel, tol) pairs so that
@@ -976,6 +1022,26 @@ int rebuild_classes(bs_engine* e) {
     e->group_classes_dirty = false;
   }
   HP(e, "classes:assign-groups");
+  if (e->ipf_assign_dirty) {
+    // the pods' fit classes with their filter class while the filter is on, else the classes of the upload
+    uint32_t* pfc = e->h_pfc.data();
+    if (e->ipf_on) {
+      if (!e->pfc_base_valid) e->h_pfc_base.assign(pfc, pfc + P);
+      e->pfc_base_valid = true;
+      const uint32_t* base = e->h_pfc_base.data();
+      const uint32_t* ipf = e->h_ipf_class.data();
+      ClassIndex& fi = e->fit_index;
+      assign_classes(fi, P, [&fi, base, ipf](uint32_t p) {
+        ClassKey k = fi.keys[base[p]];
+        k.ipf = ipf[p];
+        return k;
+      }, pfc);
+    } else if (e->pfc_base_valid) {
+      memcpy(pfc, e->h_pfc_base.data(), (size_t)P * 4);
+    }
+    compact_fit_index(e);
+    e->ipf_assign_dirty = false;
+  }
   if (e->fit_index.size() == 0) e->fit_index.get_or_add(ClassKey{0, 0, 0, BS_AFF_NONE});
   if (e->rep_index.size() == 0) e->rep_index.get_or_add(ClassKey{0, 0, 0, BS_AFF_NONE});
   e->n_fit_classes = (uint32_t)e->fit_index.size();
@@ -1019,6 +1085,15 @@ int rebuild_classes(bs_engine* e) {
   if ((rc = upload_vec(e, e->d_raff, raff.data(), e->n_rep_classes, e->n_rep_classes))) return rc;
   if ((rc = upload_vec(e, e->d_rsel, rsel.data(), e->n_rep_classes, e->n_rep_classes))) return rc;
   if ((rc = upload_vec(e, e->d_rtol, rtol.data(), e->n_rep_classes, e->n_rep_classes))) return rc;
+  if (e->ipf_on) {
+    // a stale class may name a filter class the pod side of now does not have: no pod uses it, so it passes
+    std::vector<uint32_t> fipf(e->n_fit_classes);
+    for (uint32_t c = 0; c < e->n_fit_classes; ++c) {
+      const uint32_t f = e->fit_index.keys[c].ipf;
+      fipf[c] = f < e->ipf_pclasses ? f : BS_IPF_NONE;
+    }
+    if ((rc = upload_vec(e, e->d_fipf, fipf.data(), e->n_fit_classes, e->n_fit_classes))) return rc;
+  }
   if (e->pod_classes_dirty) {   // a group-only change (bs_update_groups) leaves the pods' ids alone
     if ((rc = upload_vec(e, e->d_pod_fit_class, e->h_pfc.data(), P, std::max(P, 1u)))) return rc;
     if ((rc = upload_vec(e, e->d_pod_rep_class, e->h_prc.data(), P, std::max(P, 1u)))) return rc;
@@ -1070,6 +1145,7 @@ int ensure_round_buffers(bs_engine* e) {
     CK(e->d_filter_bitmap.ensure(Prows * std::max(e->W, 1u) * 4));
   }
   if (e->out_flags & BS_OUT_REASONS) CK(e->d_reasons.ensure((size_t)P * (4 + L) * 4));
+  if ((e->out_flags & BS_OUT_REASONS) && e->ipf_on) CK(e->d_ipf_reasons.ensure((size_t)P * 3 * 4));
   if (e->out_flags & BS_OUT_PRIORITY) {
     CK(e->d_prio_node.ensure((size_t)P * e->topk * 4));
     CK(e->d_prio_score.ensure((size_t)P * e->topk * 8));
@@ -1129,9 +1205,11 @@ int prepare_nodes(bs_engine* e) {
   {
     for (uint32_t c0 = 0; c0 < e->n_fit_classes; c0 += 32768) {
       dim3 grid(cdiv(n_tiles * 32, 256), std::min(32768u, e->n_fit_classes - c0));
-      class_fit_kernel<<<grid, 256, 0, e->s>>>(t, e->d_left_present.as<uint32_t>(), e->d_fsel.as<uint64_t>(),
-                                               e->d_ftol.as<uint64_t>(), e->d_fnz.as<uint32_t>(), e->d_faff.as<uint32_t>(),
-                                               e->n_fit_classes, n_tiles, e->d_classfit.as<ColBits>(), c0);
+      auto fn = e->ipf_on ? class_fit_kernel<true> : class_fit_kernel<false>;
+      fn<<<grid, 256, 0, e->s>>>(t, e->d_left_present.as<uint32_t>(), e->d_fsel.as<uint64_t>(), e->d_ftol.as<uint64_t>(),
+                                 e->d_fnz.as<uint32_t>(), e->d_faff.as<uint32_t>(), e->n_fit_classes, n_tiles,
+                                 e->d_classfit.as<ColBits>(), c0, e->d_fipf.as<uint32_t>(),
+                                 e->d_ipf_bits.as<uint32_t>(), e->Npad / 32);
       tm.launched();
     }
   }
@@ -1141,12 +1219,15 @@ int prepare_nodes(bs_engine* e) {
     CK(e->d_reason_gate.ensure((size_t)e->n_fit_classes * Wg * 4));
     CK(e->d_reason_class.ensure((size_t)e->n_fit_classes * 4 * 4));
     CK(cudaMemsetAsync(e->d_reason_class.p, 0, (size_t)e->n_fit_classes * 4 * 4, e->s));
+    if (e->ipf_on) CK(e->d_reason_gate_ipf.ensure((size_t)e->n_fit_classes * Wg * 4));
     for (uint32_t c0 = 0; c0 < e->n_fit_classes; c0 += 32768) {
       dim3 grid(cdiv(Wg * 32, REASON_CLASS_THREADS), std::min(32768u, e->n_fit_classes - c0));
-      reason_class_kernel<<<grid, REASON_CLASS_THREADS, 0, e->s>>>(t, e->d_fsel.as<uint64_t>(), e->d_ftol.as<uint64_t>(),
-                                                                   e->d_faff.as<uint32_t>(), e->n_fit_classes, Wg,
-                                                                   e->d_reason_gate.as<uint32_t>(),
-                                                                   e->d_reason_class.as<uint32_t>(), c0);
+      auto fn = e->ipf_on ? reason_class_kernel<true> : reason_class_kernel<false>;
+      fn<<<grid, REASON_CLASS_THREADS, 0, e->s>>>(t, e->d_fsel.as<uint64_t>(), e->d_ftol.as<uint64_t>(),
+                                                  e->d_faff.as<uint32_t>(), e->n_fit_classes, Wg,
+                                                  e->d_reason_gate.as<uint32_t>(), e->d_reason_class.as<uint32_t>(), c0,
+                                                  e->d_fipf.as<uint32_t>(), e->d_ipf_bits.as<uint32_t>(),
+                                                  e->d_reason_gate_ipf.as<uint32_t>());
       tm.launched();
     }
   }
@@ -1218,6 +1299,55 @@ int interpod_prepass(bs_engine* e) {
   return BS_OK;
 }
 
+// The MatchInterPodAffinity filter's pre-pass on the main stream (interpod_filter.cuh): presence planes and term
+// counts over the bound pods, then the class bit planes.  Only while the filter is on and after a side changed or the
+// filter was switched on.
+int interpod_filter_prepass(bs_engine* e) {
+  if (!e->ipf_on || !e->ipf_dirty) return BS_OK;
+  const uint32_t C = e->ipf_pclasses, Wg = e->Npad / 32;
+  const uint64_t words = (e->ipf_slots + 31) / 32;
+  CK(e->d_ipf_presence.ensure((size_t)std::max<uint64_t>(2 * words, 1) * 4));
+  CK(e->d_ipf_hits.ensure((size_t)std::max(e->ipf_terms, 1u) * 4));
+  CK(e->d_ipf_bits.ensure((size_t)std::max<uint64_t>(3ull * C * Wg, 1) * 4));
+  if (words) CK(cudaMemsetAsync(e->d_ipf_presence.p, 0, (size_t)2 * words * 4, e->s));
+  if (e->ipf_terms) CK(cudaMemsetAsync(e->d_ipf_hits.p, 0, (size_t)e->ipf_terms * 4, e->s));
+  const IpfTopo tp{e->d_ipf_topo.as<uint32_t>(), e->d_ipf_term_key.as<uint32_t>(), e->d_ipf_term_off.as<uint32_t>(), e->N};
+  uint32_t* mbits = e->d_ipf_presence.as<uint32_t>();
+  if (e->ipf_bound) {
+    const IpfBound b{e->d_ipf_bound_node.as<uint32_t>(), e->d_ipf_bound_class.as<uint32_t>(), e->d_ipf_boff.as<uint32_t>(),
+                     e->d_ipf_bterm.as<uint32_t>(), e->d_ipf_bown.as<int32_t>(), e->d_ipf_bmatch.as<uint8_t>(),
+                     e->ipf_bound};
+    ipf_presence_kernel<<<cdiv(e->ipf_bound, IPF_THREADS), IPF_THREADS, 0, e->s>>>(b, tp, mbits, mbits + words,
+                                                                                  e->d_ipf_hits.as<uint32_t>());
+    e->launches += 1;
+  }
+  const IpfPods pc{e->d_ipf_poff.as<uint32_t>(), e->d_ipf_pterm.as<uint32_t>(), e->d_ipf_prole.as<uint8_t>(),
+                   e->d_ipf_pself.as<uint8_t>(), C};
+  for (uint32_t c0 = 0; c0 < C && Wg; c0 += 32768) {
+    const dim3 grid(cdiv(Wg * 32, IPF_THREADS), std::min(32768u, C - c0));
+    ipf_class_kernel<<<grid, IPF_THREADS, 0, e->s>>>(pc, tp, mbits, mbits + words, e->d_ipf_hits.as<uint32_t>(),
+                                                     e->d_ipf_bits.as<uint32_t>(), Wg, c0);
+    e->launches += 1;
+  }
+  CK(cudaGetLastError());
+  e->ipf_dirty = false;
+  return BS_OK;
+}
+
+// The filter's columns (BS_E_STATE when a side is missing), the terms its pod classes name (BS_E_INDEX) and its class
+// planes' size (BS_E_INVAL), checked before anything is launched.
+int interpod_filter_check(bs_engine* e, const char* who) {
+  const std::string w(who);
+  if (!(e->have_ipf_node && e->have_ipf_pod))
+    return fail(e, BS_E_STATE, (w + ": the MatchInterPodAffinity filter needs its node and pod sides").c_str());
+  if (e->ipf_term_max >= (int64_t)e->ipf_terms)
+    return fail(e, BS_E_INDEX, (w + ": a filter class's term is outside the node side's term dictionary").c_str());
+  // the pod side outlives node uploads: its planes are checked against the node table of now
+  if (3ull * e->ipf_pclasses * (e->Npad / 8) > BS_IPF_TABLE_MAX_BYTES)
+    return fail(e, BS_E_INVAL, (w + ": 3 x filter n_classes x padded nodes / 8 bytes exceeds BS_IPF_TABLE_MAX_BYTES").c_str());
+  return BS_OK;
+}
+
 int evaluate_async_locked(bs_engine* e) {
   int rc;
   if (!e->have_nodes || !e->have_pods || !e->have_groups)
@@ -1246,6 +1376,7 @@ int evaluate_async_locked(bs_engine* e) {
     if ((uint64_t)e->ipa_pclasses * e->Npad * 8 > BS_IPA_TABLE_MAX_BYTES)
       return fail(e, BS_E_INVAL, "bs_evaluate: pod n_classes x padded nodes x 8 bytes exceeds BS_IPA_TABLE_MAX_BYTES");
   }
+  if (e->ipf_on && (rc = interpod_filter_check(e, "bs_evaluate"))) return rc;
   if (e->peer_broken)
     return fail(e, BS_E_PEER, "peer exchange is broken (a rank did not arrive): bs_peer_detach on every rank, then init/attach again");
   BS_DEVICE_GUARD(e);
@@ -1267,6 +1398,10 @@ int evaluate_async_locked(bs_engine* e) {
   }
   if ((rc = ensure_round_buffers(e))) return rc;
   for (int k = 0; k < BS_K_COUNT; ++k) e->k_valid[k] = false;
+  if (e->ipf_on && e->ipf_dirty) {   // new pass bits: the class fit bits and gates are built again
+    if ((rc = interpod_filter_prepass(e))) return rc;
+    reprepare = true;
+  }
   if (reprepare && (rc = prepare_nodes(e))) return rc;
 
   const uint32_t P = e->P, G = e->G, L = e->L;
@@ -1486,7 +1621,12 @@ int evaluate_async_locked(bs_engine* e) {
       ra.fit_class = e->d_pod_fit_class.as<uint32_t>();
       ra.rows = e->d_reasons.as<uint32_t>();
       ra.P = P; ra.N = e->N; ra.Npad = e->Npad; ra.Wg = e->Npad / 32; ra.L = L;
-      reason_pod_kernel<<<cdiv(P, REASON_PODS_PER_CTA), REASON_THREADS, 0, e->s>>>(ra);
+      ra.cipf = e->d_fipf.as<uint32_t>();
+      ra.ipf_bits = e->d_ipf_bits.as<uint32_t>();
+      ra.n_ipf = e->ipf_pclasses;
+      ra.ipf_rows = e->d_ipf_reasons.as<uint32_t>();
+      if (e->ipf_on) reason_pod_kernel<true><<<cdiv(P, REASON_PODS_PER_CTA), REASON_THREADS, 0, e->s>>>(ra);
+      else reason_pod_kernel<false><<<cdiv(P, REASON_PODS_PER_CTA), REASON_THREADS, 0, e->s>>>(ra);
       tm.launched();
     }
   }
@@ -1494,7 +1634,7 @@ int evaluate_async_locked(bs_engine* e) {
     PriorityRatioArgs pa;
     pa.left = e->d_left_full.as<int64_t>();
     pa.left_present = e->d_left_present.as<uint32_t>();
-    pa.gate = e->d_reason_gate.as<uint32_t>();
+    pa.gate = e->ipf_on ? e->d_reason_gate_ipf.as<uint32_t>() : e->d_reason_gate.as<uint32_t>();
     pa.req = e->d_req.as<int64_t>();
     pa.req_present = e->d_ppres.as<uint32_t>();
     pa.fit_class = e->d_pod_fit_class.as<uint32_t>();
@@ -1570,6 +1710,7 @@ int evaluate_async_locked(bs_engine* e) {
   }
   CK(cudaStreamWaitEvent(e->s, e->ev_join, 0));
   CK(cudaGetLastError());
+  e->ipf_round = e->ipf_on;
   e->evaluated = true;
   e->fetched = false;
   e->gang_applied = false;
@@ -1771,6 +1912,7 @@ int bs_upload_nodes(bs_engine* e, const bs_node_table* t) {
   e->have_img_node = e->have_avoid_node = false;   // and the image rows and preferAvoidPods masks
   e->have_spread_node = false;   // and the zones and selector counts (counts change when pods bind)
   e->have_ipa_node = false;   // and the topology values and bound pods of InterPodAffinity
+  e->have_ipf_node = false;   // and those of the MatchInterPodAffinity filter
   if (t->n_lanes != e->L) return fail(e, BS_E_INVAL, "bs_upload_nodes: n_lanes differs from the engine's");
   const uint32_t N = t->n_nodes, L = e->L;
   const auto cols = node_cols(e, t);
@@ -1818,6 +1960,7 @@ int bs_update_nodes(bs_engine* e, const uint32_t* idx, const bs_node_table* t) {
   e->have_img_node = e->have_avoid_node = false;   // ... and their images and annotations: so is the locality side
   e->have_spread_node = false;   // ... and the pods on them and their zone labels: so is the spread side
   e->have_ipa_node = false;   // ... and the inter-pod side, for the same reasons
+  e->have_ipf_node = false;   // ... and the filter's
   if (t->n_lanes != e->L) return fail(e, BS_E_INVAL, "bs_update_nodes: n_lanes differs from the engine's");
   const uint32_t n = t->n_nodes, L = e->L;
   if (!n) return BS_OK;
@@ -1953,6 +2096,9 @@ int bs_upload_pods(bs_engine* e, const bs_pod_table* t) {
   e->have_img_pod = e->have_avoid_pod = false;   // and the pod locality side
   e->have_spread_pod = false;   // and the pod spread side
   e->have_ipa_pod = false;   // and the pod inter-pod side
+  e->have_ipf_pod = false;   // and the filter's pod side; the new table's fit classes are its base classes
+  e->pfc_base_valid = false;
+  e->ipf_assign_dirty = false;
   if (t->n_lanes != e->L) return fail(e, BS_E_INVAL, "bs_upload_pods: n_lanes differs from the engine's");
   const uint32_t P = t->n_pods, L = e->L;
   if (P && (!t->req || !t->req_present || !t->gid || !t->sel_mask || !t->tol_mask || !t->priority ||
@@ -2450,6 +2596,11 @@ int bs_format_message(const bs_status* st, const char* ns_name, const char* occu
 // sorted "<count> <reason>" entries joined by ", " + "."
 int bs_format_fit_error(const uint32_t* counts, uint32_t n_lanes, uint32_t n_nodes, const char* const* scalar_names,
                         char* buf, size_t buf_len) {
+  return bs_format_fit_error_interpod(counts, n_lanes, nullptr, n_nodes, scalar_names, buf, buf_len);
+}
+
+int bs_format_fit_error_interpod(const uint32_t* counts, uint32_t n_lanes, const uint32_t* interpod, uint32_t n_nodes,
+                                 const char* const* scalar_names, char* buf, size_t buf_len) {
   if (!counts || !buf || !buf_len || n_lanes < BS_FIXED_LANES || n_lanes > BS_MAX_LANES) return BS_E_INVAL;
   static const char* const kFixed[4] = {"node(s) were unschedulable", "node(s) were unavailable",
                                         "node(s) didn't match node selector",
@@ -2468,6 +2619,15 @@ int bs_format_fit_error(const uint32_t* counts, uint32_t n_lanes, uint32_t n_nod
       else text += "lane" + std::to_string(d);
     }
     entries.push_back(std::to_string(counts[b]) + " " + text);
+  }
+  if (interpod) {   // a node failing MatchInterPodAffinity reports ErrPodAffinityNotMatch and the step's own reason
+    static const char* const kIpf[3] = {"node(s) didn't satisfy existing pods anti-affinity rules",
+                                        "node(s) didn't match pod affinity rules",
+                                        "node(s) didn't match pod anti-affinity rules"};
+    const uint64_t all = (uint64_t)interpod[0] + interpod[1] + interpod[2];
+    if (all) entries.push_back(std::to_string(all) + " node(s) didn't match pod affinity/anti-affinity");
+    for (int k = 0; k < 3; ++k)
+      if (interpod[k]) entries.push_back(std::to_string(interpod[k]) + " " + kIpf[k]);
   }
   std::sort(entries.begin(), entries.end());   // byte-wise, as Go's sort.Strings
   std::string msg = "0/" + std::to_string(n_nodes) + " nodes are available: ";
@@ -2704,9 +2864,17 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
 }
 }  // namespace
 
+// The walks and preemption refuse to run under the MatchInterPodAffinity filter: its presence would have to follow their
+// own placements and victim removals (upstream's metadata AddPod / RemovePod).
+static int interpod_filter_refuse(bs_engine* e, const char* who) {
+  return fail(e, BS_E_INVAL, (std::string(who) + ": the MatchInterPodAffinity filter is not supported here; "
+                              "switch it off with bs_set_interpod_filter").c_str());
+}
+
 int bs_replay(bs_engine* e, const uint32_t* queue, uint32_t n_queue, bs_replay_result* out) {
   if (!e || !out) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
+  if (e->ipf_on) return interpod_filter_refuse(e, "bs_replay");
   return replay_walk(e, "bs_replay", queue, n_queue, out, false, nullptr);
 }
 
@@ -2714,6 +2882,7 @@ int bs_replay_priority(bs_engine* e, const uint32_t* queue, uint32_t n_queue, bs
                        int64_t* node_nonzero_after) {
   if (!e || !out) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
+  if (e->ipf_on) return interpod_filter_refuse(e, "bs_replay_priority");
   if (e->w_taint || e->w_naff)   // their maxima would have to follow the walk's live fit set, which is not built yet
     return fail(e, BS_E_INVAL, "bs_replay_priority: TaintToleration and NodeAffinity are not supported in the walk; "
                                "set both weights of bs_set_node_priority_weights to 0");
@@ -2891,6 +3060,7 @@ int bs_preempt(bs_engine* e, const uint32_t* pods, uint32_t n, bs_preempt_result
   if (!e || !out || (n && (!pods || !out->node || !out->n_victims || !out->n_candidates)) || !out->victim_offset)
     return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
+  if (e->ipf_on) return interpod_filter_refuse(e, "bs_preempt");
   std::vector<PreemptPod> pp;
   int rc;
   if ((rc = preempt_pods(e, "bs_preempt", pods, n, pp))) return rc;
@@ -2959,6 +3129,7 @@ int bs_preempt_walk(bs_engine* e, const uint32_t* pods, uint32_t n, uint32_t fla
   if (!e || !out || (n && (!pods || !out->node || !out->n_victims || !out->n_candidates)) || !out->victim_offset)
     return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
+  if (e->ipf_on) return interpod_filter_refuse(e, "bs_preempt_walk");
   if (flags & ~BS_PREEMPT_GANG) return fail(e, BS_E_INVAL, "bs_preempt_walk: unknown flag bits");
   const bool gang = flags & BS_PREEMPT_GANG;
   std::vector<PreemptPod> pp;
@@ -3756,6 +3927,149 @@ int bs_upload_pod_interpod(bs_engine* e, const bs_interpod_pods* t) {
   e->ipa_pclasses = t->classes.n_classes;
   e->ipa_term_max = tmax;
   e->have_ipa_pod = true;
+  return BS_OK;
+}
+
+int bs_set_interpod_filter(bs_engine* e, int on) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if ((on != 0) == e->ipf_on) return BS_OK;
+  e->ipf_on = on != 0;
+  e->ipf_dirty = true;   // the pass bits are built again at the next evaluation the filter is on for
+  e->ipf_assign_dirty = e->classes_dirty = e->pod_classes_dirty = true;   // and the pods' fit classes follow the switch
+  e->evaluated = false;
+  return BS_OK;
+}
+
+int bs_upload_node_interpod_filter(bs_engine* e, const bs_interpod_nodes* t) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  const char* who = "bs_upload_node_interpod_filter";
+  auto bad = [&](int rc, const char* why) { return fail(e, rc, (std::string(who) + ": " + why).c_str()); };
+  e->have_ipf_node = false;
+  e->ipf_dirty = true;
+  if (!t) return bad(BS_E_INVAL, "null table");
+  if (!e->have_nodes) return bad(BS_E_STATE, "upload nodes first");
+  const uint32_t N = t->n_nodes, K = t->n_keys, T = t->n_terms, V = t->n_bound;
+  if (N != e->N) return bad(BS_E_INVAL, "n_nodes differs from the node table's");
+  if (K > BS_IPA_KEY_MAX) return bad(BS_E_INVAL, "n_keys exceeds BS_IPA_KEY_MAX");
+  if (V > BS_IPF_BOUND_MAX) return bad(BS_E_INVAL, "n_bound exceeds BS_IPF_BOUND_MAX");
+  if ((K && !t->n_values) || (K && N && !t->topo) || (T && !t->term_key) || (V && !(t->bound_node && t->bound_class)))
+    return bad(BS_E_INVAL, "null column");
+  for (size_t k = 0; k < (size_t)K * N; ++k)
+    if (t->topo[k] != BS_TOPO_NONE && t->topo[k] >= t->n_values[k / N]) return bad(BS_E_INDEX, "a topo value is >= n_values");
+  std::vector<uint32_t> off(T);
+  uint64_t slots = 0;
+  for (uint32_t k = 0; k < T; ++k) {
+    if (t->term_key[k] >= K) return bad(BS_E_INDEX, "a term_key is >= n_keys");
+    off[k] = (uint32_t)slots;
+    slots += t->n_values[t->term_key[k]];
+    if ((slots + 31) / 32 * 2 * 4 > BS_IPF_TERM_MAX_BYTES) return bad(BS_E_INVAL, "the presence planes exceed BS_IPF_TERM_MAX_BYTES");
+  }
+  for (uint32_t k = 0; k < V; ++k) {
+    if (t->bound_node[k] >= N) return bad(BS_E_INDEX, "a bound_node is >= n_nodes");
+    if (t->bound_class[k] != BS_IPF_NONE && t->bound_class[k] >= t->classes.n_classes)
+      return bad(BS_E_INDEX, "a bound_class is >= n_classes");
+  }
+  int64_t tmax;
+  const char* why = nullptr;
+  if (int rc = interpod_classes_check(t->classes, T, tmax, why)) return bad(rc, why);
+  const uint32_t nnz = t->classes.n_classes ? t->classes.class_offset[t->classes.n_classes] : 0;
+  for (uint32_t k = 0; k < nnz; ++k)
+    if (t->classes.own[k] != 0 && t->classes.own[k] != 1) return bad(BS_E_RANGE, "an own is not 0 or 1");
+  BS_DEVICE_GUARD(e);
+  CK(e->d_ipf_topo.ensure((size_t)std::max<uint64_t>((uint64_t)K * N, 1) * 4));
+  CK(e->d_ipf_term_key.ensure((size_t)std::max(T, 1u) * 4));
+  CK(e->d_ipf_term_off.ensure((size_t)std::max(T, 1u) * 4));
+  CK(e->d_ipf_bound_node.ensure((size_t)std::max(V, 1u) * 4));
+  CK(e->d_ipf_bound_class.ensure((size_t)std::max(V, 1u) * 4));
+  if (K && N) CK(cudaMemcpyAsync(e->d_ipf_topo.p, t->topo, (size_t)K * N * 4, cudaMemcpyHostToDevice, e->s));
+  if (T) {
+    CK(cudaMemcpyAsync(e->d_ipf_term_key.p, t->term_key, (size_t)T * 4, cudaMemcpyHostToDevice, e->s));
+    CK(cudaMemcpyAsync(e->d_ipf_term_off.p, off.data(), (size_t)T * 4, cudaMemcpyHostToDevice, e->s));
+  }
+  if (V) {
+    CK(cudaMemcpyAsync(e->d_ipf_bound_node.p, t->bound_node, (size_t)V * 4, cudaMemcpyHostToDevice, e->s));
+    CK(cudaMemcpyAsync(e->d_ipf_bound_class.p, t->bound_class, (size_t)V * 4, cudaMemcpyHostToDevice, e->s));
+  }
+  if (int rc = interpod_classes_upload(e, t->classes, e->d_ipf_boff, e->d_ipf_bterm, e->d_ipf_bown, e->d_ipf_bmatch))
+    return rc;
+  CK(cudaStreamSynchronize(e->s));   // the caller's columns may go once the call returns
+  e->ipf_terms = T;
+  e->ipf_slots = slots;
+  e->ipf_bound = V;
+  e->have_ipf_node = true;
+  e->evaluated = false;
+  return BS_OK;
+}
+
+int bs_upload_pod_interpod_filter(bs_engine* e, const bs_interpod_filter_pods* t) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  const char* who = "bs_upload_pod_interpod_filter";
+  auto bad = [&](int rc, const char* why) { return fail(e, rc, (std::string(who) + ": " + why).c_str()); };
+  e->have_ipf_pod = false;
+  e->ipf_dirty = true;
+  if (!t) return bad(BS_E_INVAL, "null table");
+  if (!e->have_pods) return bad(BS_E_STATE, "upload pods first");
+  const uint32_t P = t->n_pods, C = t->n_classes;
+  if (P != e->P) return bad(BS_E_INVAL, "n_pods differs from the pod table's");
+  if (P && !t->pod_class) return bad(BS_E_INVAL, "null pod_class");
+  if (C && !(t->class_offset && t->self_match)) return bad(BS_E_INVAL, "null class_offset or self_match");
+  if (3ull * C * (e->Npad / 8) > BS_IPF_TABLE_MAX_BYTES)
+    return bad(BS_E_INVAL, "3 x n_classes x padded nodes / 8 bytes exceeds BS_IPF_TABLE_MAX_BYTES");
+  if (C && t->class_offset[0] != 0) return bad(BS_E_INVAL, "class_offset[0] is not 0");
+  for (uint32_t k = 0; k < C; ++k)
+    if (t->class_offset[k + 1] < t->class_offset[k] || t->class_offset[k + 1] - t->class_offset[k] > BS_IPF_CLASS_MAX)
+      return bad(BS_E_INVAL, "class_offset is not ascending, or a class lists more than BS_IPF_CLASS_MAX entries");
+  const uint32_t nnz = C ? t->class_offset[C] : 0;
+  if (nnz && !(t->term && t->role)) return bad(BS_E_INVAL, "null term or role");
+  int64_t tmax = -1;
+  for (uint32_t k = 0; k < nnz; ++k) {
+    if (t->role[k] > BS_IPF_EXISTING) return bad(BS_E_INVAL, "a role is not BS_IPF_AFFINITY, BS_IPF_ANTI or BS_IPF_EXISTING");
+    tmax = std::max(tmax, (int64_t)t->term[k]);
+  }
+  for (uint32_t k = 0; k < C; ++k)
+    if (t->self_match[k] > 1) return bad(BS_E_RANGE, "a self_match is not 0 or 1");
+  for (uint32_t p = 0; p < P; ++p)
+    if (t->pod_class[p] != BS_IPF_NONE && t->pod_class[p] >= C) return bad(BS_E_INDEX, "a pod_class is >= n_classes");
+  BS_DEVICE_GUARD(e);
+  CK(e->d_ipf_poff.ensure((size_t)(C + 1) * 4));
+  CK(e->d_ipf_pterm.ensure((size_t)std::max(nnz, 1u) * 4));
+  CK(e->d_ipf_prole.ensure(std::max(nnz, 1u)));
+  CK(e->d_ipf_pself.ensure(std::max(C, 1u)));
+  if (C) {
+    CK(cudaMemcpyAsync(e->d_ipf_poff.p, t->class_offset, (size_t)(C + 1) * 4, cudaMemcpyHostToDevice, e->s));
+    CK(cudaMemcpyAsync(e->d_ipf_pself.p, t->self_match, C, cudaMemcpyHostToDevice, e->s));
+  }
+  if (nnz) {
+    CK(cudaMemcpyAsync(e->d_ipf_pterm.p, t->term, (size_t)nnz * 4, cudaMemcpyHostToDevice, e->s));
+    CK(cudaMemcpyAsync(e->d_ipf_prole.p, t->role, nnz, cudaMemcpyHostToDevice, e->s));
+  }
+  CK(cudaStreamSynchronize(e->s));
+  e->h_ipf_class.assign(t->pod_class, t->pod_class + P);
+  e->ipf_pclasses = C;
+  e->ipf_term_max = tmax;
+  e->have_ipf_pod = true;
+  e->ipf_assign_dirty = e->classes_dirty = e->pod_classes_dirty = true;   // the pods' fit classes carry the filter class
+  e->evaluated = false;
+  return BS_OK;
+}
+
+int bs_fetch_interpod_reason_rows(bs_engine* e, uint32_t pod0, uint32_t n, uint32_t* counts) {
+  if (!e || (n && !counts)) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!e->evaluated || !(e->out_flags & BS_OUT_REASONS)) return fail(e, BS_E_STATE, "no reason rows materialised");
+  if ((uint64_t)pod0 + n > e->P) return BS_E_INDEX;
+  if (!n) return BS_OK;
+  if (!e->ipf_round) {
+    memset(counts, 0, (size_t)n * 3 * 4);
+    return BS_OK;
+  }
+  BS_DEVICE_GUARD(e);
+  CK(cudaMemcpyAsync(counts, e->d_ipf_reasons.as<uint32_t>() + (size_t)pod0 * 3, (size_t)n * 3 * 4,
+                     cudaMemcpyDeviceToHost, e->s));
+  CK(cudaStreamSynchronize(e->s));
   return BS_OK;
 }
 

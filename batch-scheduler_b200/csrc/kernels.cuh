@@ -363,18 +363,23 @@ __global__ void node_left_class_kernel(NodeTab t, uint64_t sel, uint64_t tol, fl
 // (compareResourceAndRequire :688-690).  Layout is TRANSPOSED for the fit kernel:
 // classfit[(c * n_tiles + tile) * 32 + lane] holds, in bit j, the verdict for node
 // tile*NODE_TILE + j*32 + lane — exactly the TILE_WORDS nodes lane `lane` owns in
-// that tile, so the hot loop needs one coalesced 4-byte load per (pod, tile).
+// that tile, so the hot loop needs one coalesced 4-byte load per (pod, tile).  IPF: the MatchInterPodAffinity
+// filter is on, and the bit also needs the pass bit of the class's filter class cipf[c] (interpod_filter.cuh; bit
+// i % 32 of word ipf_pass[cipf[c] * Wg + i / 32]; BS_IPF_NONE passes).  The IPF = false build is the filter-off kernel.
+template <bool IPF>
 __global__ void class_fit_kernel(NodeTab t, const uint32_t* __restrict__ left_present,
                                  const uint64_t* __restrict__ csel, const uint64_t* __restrict__ ctol,
                                  const uint32_t* __restrict__ cnz, const uint32_t* __restrict__ caff,
                                  uint32_t n_classes, uint32_t n_tiles,
-                                 ColBits* __restrict__ classfit, uint32_t class0) {
+                                 ColBits* __restrict__ classfit, uint32_t class0,
+                                 const uint32_t* __restrict__ cipf, const uint32_t* __restrict__ ipf_pass, uint32_t Wg) {
   const uint32_t c = class0 + blockIdx.y;   // gridDim.y is capped at 65535: classes go in chunks
   const uint32_t slot = blockIdx.x * blockDim.x + threadIdx.x;  // tile * 32 + lane
   if (slot >= n_tiles * 32 || c >= n_classes) return;
   const uint32_t tile = slot >> 5, lane = slot & 31;
   const uint64_t sel = csel[c], tol = ctol[c];
   const uint32_t nz = cnz[c], aff = caff[c];
+  const uint32_t ipf = IPF ? cipf[c] : BS_IPF_NONE;
   ColBits bits = 0;
 #pragma unroll
   for (int j = 0; j < TILE_WORDS; ++j) {
@@ -384,6 +389,7 @@ __global__ void class_fit_kernel(NodeTab t, const uint32_t* __restrict__ left_pr
       const uint8_t f = t.flags[i];
       ok = !node_skipped(f) && !(f & BS_NODE_TAINTS_ERR) && check_fit(t.label[i], t.taint[i], sel, tol) &&
            aff_ok(t, aff, i) && ((nz & ~left_present[i]) == 0);
+      if (IPF && ipf != BS_IPF_NONE) ok = ok && ((ipf_pass[(size_t)ipf * Wg + (i >> 5)] >> (i & 31)) & 1u);
     }
     bits |= (ColBits)(ok ? 1u : 0u) << j;
   }
@@ -397,12 +403,18 @@ __global__ void class_fit_kernel(NodeTab t, const uint32_t* __restrict__ left_pr
 // core.go:741-759; both predicates' reasons count).  Also the class's gate bitmap [c][Wg]: bit n%32 of word n/32
 // = node n passes the guards and checkFit, the only nodes whose lanes a reason row inspects.  One thread per node
 // (Wg * 32 threads cover the padded table: gate bits of padding nodes are 0), one ballot per warp and bin, one
-// global atomic per CTA and bin into class_bins[c][4] (zeroed before the launch).
+// global atomic per CTA and bin into class_bins[c][4] (zeroed before the launch).  IPF: the MatchInterPodAffinity
+// filter is on, and the kernel also writes gate_ipf = the gate AND the pass bits of the class's filter class, the fit
+// set's gate of the priority lists; the gate itself stays the lane sweep's.  The IPF = false build is the filter-off
+// kernel.
 constexpr int REASON_CLASS_THREADS = 256;
+template <bool IPF>
 __global__ void __launch_bounds__(REASON_CLASS_THREADS)
 reason_class_kernel(NodeTab t, const uint64_t* __restrict__ csel, const uint64_t* __restrict__ ctol,
                     const uint32_t* __restrict__ caff, uint32_t n_classes, uint32_t Wg,
-                    uint32_t* __restrict__ gate, uint32_t* __restrict__ class_bins, uint32_t class0) {
+                    uint32_t* __restrict__ gate, uint32_t* __restrict__ class_bins, uint32_t class0,
+                    const uint32_t* __restrict__ cipf, const uint32_t* __restrict__ ipf_pass,
+                    uint32_t* __restrict__ gate_ipf) {
   const uint32_t c = class0 + blockIdx.y;   // gridDim.y is capped at 65535: classes go in chunks
   if (c >= n_classes) return;
   __shared__ uint32_t s_bins[4];
@@ -426,6 +438,10 @@ reason_class_kernel(NodeTab t, const uint64_t* __restrict__ csel, const uint64_t
   }
   const uint32_t gw = __ballot_sync(0xffffffffu, pass);
   if (lane == 0 && (i >> 5) < Wg) gate[(size_t)c * Wg + (i >> 5)] = gw;
+  if (IPF && lane == 0 && (i >> 5) < Wg) {
+    const uint32_t ipf = cipf[c];
+    gate_ipf[(size_t)c * Wg + (i >> 5)] = ipf == BS_IPF_NONE ? gw : gw & ipf_pass[(size_t)ipf * Wg + (i >> 5)];
+  }
   const uint32_t b0 = __popc(__ballot_sync(0xffffffffu, unsched)), b1 = __popc(__ballot_sync(0xffffffffu, unavail));
   const uint32_t b2 = __popc(__ballot_sync(0xffffffffu, sel_bad)), b3 = __popc(__ballot_sync(0xffffffffu, taint_bad));
   if (lane == 0) {
@@ -444,7 +460,9 @@ reason_class_kernel(NodeTab t, const uint64_t* __restrict__ csel, const uint64_t
 // left_present): lanes 0-3 when left < req; a scalar lane the pod requests when the node's left lacks the key and
 // req != 0, or when req > left.  Every short lane counts (the reference stops at the first).  Counters stay in
 // registers, are summed across the warp once at the end, and each (pod, bin) is stored once; bins 0-3 are copied
-// from the pod's class.
+// from the pod's class.  IPF: the MatchInterPodAffinity filter is on, and a gated node with no short lane that fails
+// the filter counts in ipf_rows[p][3] by the step that failed it (E, A, N; interpod_filter.cuh's planes).  The
+// IPF = false build is the filter-off kernel.
 constexpr int REASON_THREADS = 256;
 constexpr int REASON_PPW = 4;                                         // pods per warp
 constexpr int REASON_PODS_PER_CTA = (REASON_THREADS / 32) * REASON_PPW;
@@ -458,7 +476,13 @@ struct ReasonArgs {
   const uint32_t* fit_class;    // [P]
   uint32_t* rows;               // [P][4 + L]
   uint32_t P, N, Npad, Wg, L;
+  // IPF only: each fit class's filter class, the planes [3][n_ipf][Wg] (pass, E, A) and the rows [P][3]
+  const uint32_t* cipf;
+  const uint32_t* ipf_bits;
+  uint32_t n_ipf;
+  uint32_t* ipf_rows;
 };
+template <bool IPF>
 __global__ void __launch_bounds__(REASON_THREADS) reason_pod_kernel(ReasonArgs a) {
   __shared__ int64_t s_req[REASON_THREADS / 32][REASON_PPW][BS_MAX_LANES];
   const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -471,18 +495,27 @@ __global__ void __launch_bounds__(REASON_THREADS) reason_pod_kernel(ReasonArgs a
   __syncwarp();
   uint32_t rmask[REASON_PPW];   // lanes compared: 0-3 always, scalar lanes the pod requests
   const uint32_t* grow[REASON_PPW];
+  const uint32_t* frow[REASON_PPW];   // IPF: the pass plane row of the pod's filter class, or null
 #pragma unroll
   for (int j = 0; j < REASON_PPW; ++j) {
     const uint32_t p = p0 + j;
     const bool ok = p < a.P;
     rmask[j] = ok ? (a.req_present[p] | 0xFu) : 0u;
     grow[j] = a.gate + (size_t)(ok ? a.fit_class[p] : 0u) * a.Wg;
+    if (IPF) {
+      const uint32_t f = ok ? a.cipf[a.fit_class[p]] : BS_IPF_NONE;
+      frow[j] = f == BS_IPF_NONE ? nullptr : a.ipf_bits + (size_t)f * a.Wg;
+    }
   }
   uint32_t cnt[REASON_PPW][BS_MAX_LANES];
+  uint32_t icnt[REASON_PPW][3];
 #pragma unroll
-  for (int j = 0; j < REASON_PPW; ++j)
+  for (int j = 0; j < REASON_PPW; ++j) {
 #pragma unroll
     for (int d = 0; d < BS_MAX_LANES; ++d) cnt[j][d] = 0;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) icnt[j][k] = 0;
+  }
   for (uint32_t base = 0; base < a.N; base += 32) {
     const uint32_t i = base + lane, w = base >> 5;
     bool g[REASON_PPW];
@@ -495,6 +528,9 @@ __global__ void __launch_bounds__(REASON_THREADS) reason_pod_kernel(ReasonArgs a
     }
     if (!any) continue;   // warp-uniform: no pod of the warp looks at these 32 nodes
     const uint32_t lp = a.left_present[i] | 0xFu;   // i < Npad: the padded table is readable
+    bool any_short[REASON_PPW];
+#pragma unroll
+    for (int j = 0; j < REASON_PPW; ++j) any_short[j] = false;
 #pragma unroll
     for (int d = 0; d < BS_MAX_LANES; ++d) {
       if (d >= L) break;
@@ -505,6 +541,18 @@ __global__ void __launch_bounds__(REASON_THREADS) reason_pod_kernel(ReasonArgs a
         const int64_t r = s_req[wid][j][d];
         const bool shrt = g[j] && ((rmask[j] >> d) & 1u) && lane_short(pres, v, r);
         cnt[j][d] += shrt ? 1u : 0u;
+        if (IPF) any_short[j] = any_short[j] || shrt;
+      }
+    }
+    if (IPF) {
+      const size_t plane = (size_t)a.n_ipf * a.Wg;
+#pragma unroll
+      for (int j = 0; j < REASON_PPW; ++j) {
+        if (!g[j] || any_short[j] || !frow[j] || ((frow[j][w] >> lane) & 1u)) continue;
+        const bool e_bit = (frow[j][plane + w] >> lane) & 1u, a_bit = (frow[j][2 * plane + w] >> lane) & 1u;
+        icnt[j][0] += e_bit ? 1u : 0u;
+        icnt[j][1] += !e_bit && a_bit ? 1u : 0u;
+        icnt[j][2] += !e_bit && !a_bit ? 1u : 0u;
       }
     }
   }
@@ -521,6 +569,15 @@ __global__ void __launch_bounds__(REASON_THREADS) reason_pod_kernel(ReasonArgs a
     if (p < a.P) {
       if (lane < 4) mine = a.class_bins[(size_t)a.fit_class[p] * 4 + lane];
       if (lane < R) a.rows[(size_t)p * R + lane] = mine;
+    }
+    if (IPF) {
+      uint32_t im = 0;
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        const uint32_t s = __reduce_add_sync(0xffffffffu, icnt[j][k]);
+        if (lane == (uint32_t)k) im = s;
+      }
+      if (p < a.P && lane < 3) a.ipf_rows[(size_t)p * 3 + lane] = im;
     }
   }
 }

@@ -981,6 +981,8 @@ Status BatchSchedulingPlugin::BeginRound(const std::vector<const NodeInfo*>& sna
     if (!nst.ok()) return nst;
     nst = UploadInterPodAffinity();
     if (!nst.ok()) return nst;
+    nst = UploadInterPodFilter();
+    if (!nst.ok()) return nst;
   }
   {
     Status bst = UploadBound();   // after the groups: the bound rows' group indices refer to this table
@@ -1097,7 +1099,11 @@ int BatchSchedulingPlugin::FetchReasons() {
   if (!(out_flags_ & BS_OUT_REASONS)) return BS_OK;
   const uint32_t P = packed_.n_pods;
   reasons_.assign((size_t)P * (4 + packed_.lanes), 0);
-  return bs_fetch_reason_rows(eng_, 0, P, reasons_.data());
+  const int rc = bs_fetch_reason_rows(eng_, 0, P, reasons_.data());
+  ipf_reasons_.clear();
+  if (rc || !interpod_filter_) return rc;
+  ipf_reasons_.assign((size_t)P * 3, 0);
+  return bs_fetch_interpod_reason_rows(eng_, 0, P, ipf_reasons_.data());
 }
 
 int BatchSchedulingPlugin::FetchPriority() {
@@ -1670,6 +1676,60 @@ Status BatchSchedulingPlugin::SetHardPodAffinityWeight(int32_t hard_pod_affinity
   return Status{};
 }
 
+namespace {
+// A pod-affinity term as the inter-pod dictionaries identify it: its namespaces resolved (empty: the owner's), sorted
+// and deduplicated; its selector converted by SelectorSpread's rules (has_sel = false: nil; ok = false: it fails to
+// convert); and the signature of the three with the key.
+struct ResolvedTerm {
+  bool has_sel = false, ok = true;
+  SpreadSel sel;
+  std::vector<std::string> ns;
+  std::string sig;
+};
+ResolvedTerm resolve_term(const PodAffinityTerm& t, const std::string& owner_ns) {
+  ResolvedTerm r;
+  r.has_sel = t.has_selector;
+  r.ok = !t.has_selector || sel_from_label_selector(t.selector, &r.sel);
+  r.ns = t.namespaces.empty() ? std::vector<std::string>{owner_ns} : t.namespaces;
+  std::sort(r.ns.begin(), r.ns.end());
+  r.ns.erase(std::unique(r.ns.begin(), r.ns.end()), r.ns.end());
+  for (auto& n : r.ns) { r.sig += n; r.sig += '\x1d'; }
+  r.sig += '\x1c';
+  r.sig += !r.ok ? std::string("bad") : t.has_selector ? "sel:" + sel_text(r.sel) : std::string("nil");
+  r.sig += '\x1c';
+  r.sig += t.topology_key;
+  return r;
+}
+bool pod_matches_term(const Pod& pod, const ResolvedTerm& r) {
+  return r.has_sel && r.ok && std::binary_search(r.ns.begin(), r.ns.end(), pod.ns) && spread_sel_matches(r.sel, pod.labels);
+}
+// each key's values over the nodes with a Node(), in order of first appearance; topo [keys][nodes]
+void number_topology(const std::vector<const NodeInfo*>& snapshot, const std::vector<std::string>& keys,
+                     std::vector<std::vector<std::string>>* values, std::vector<uint32_t>* n_values,
+                     std::vector<uint32_t>* topo) {
+  const size_t K = keys.size(), N = snapshot.size();
+  values->assign(K, {});
+  n_values->assign(K, 0);
+  topo->assign(K * N, BS_TOPO_NONE);
+  for (size_t k = 0; k < K; ++k) {
+    std::unordered_map<std::string, uint32_t> value_of;
+    for (size_t i = 0; i < N; ++i) {
+      if (!snapshot[i] || !snapshot[i]->node) continue;
+      const auto& labels = snapshot[i]->node->labels;
+      const auto l = labels.find(keys[k]);
+      if (l == labels.end()) continue;
+      auto it = value_of.find(l->second);
+      if (it == value_of.end()) {
+        it = value_of.emplace(l->second, (uint32_t)(*values)[k].size()).first;
+        (*values)[k].push_back(l->second);
+      }
+      (*topo)[k * N + i] = it->second;
+    }
+    (*n_values)[k] = (uint32_t)(*values)[k].size();
+  }
+}
+}  // namespace
+
 Status BatchSchedulingPlugin::PackInterPodAffinity(const std::vector<const NodeInfo*>& snapshot,
                                                    const std::vector<const Pod*>& pending, int32_t hard_weight,
                                                    PackedInterPodAffinity* out) {
@@ -1689,21 +1749,13 @@ Status BatchSchedulingPlugin::PackInterPodAffinity(const std::vector<const NodeI
   // the (term, signed weight) pairs a pod's processing reads; bad = a term's selector fails to convert
   auto own_of = [&](const Pod& pod, bool bound_side, std::map<uint32_t, int64_t>* own, bool* bad) -> Status {
     auto add = [&](const PodAffinityTerm& t, int64_t w) -> Status {
-      SpreadSel sel;
-      if (t.has_selector && !sel_from_label_selector(t.selector, &sel)) {
+      ResolvedTerm r = resolve_term(t, pod.ns);
+      if (!r.ok) {
         *bad = true;
         return Status{};
       }
       if (t.topology_key.empty()) return Status{};   // NodesHaveSameTopologyKey never holds
-      std::vector<std::string> ns = t.namespaces.empty() ? std::vector<std::string>{pod.ns} : t.namespaces;
-      std::sort(ns.begin(), ns.end());
-      ns.erase(std::unique(ns.begin(), ns.end()), ns.end());
-      std::string sig;
-      for (auto& n : ns) { sig += n; sig += '\x1d'; }
-      sig += '\x1c';
-      sig += t.has_selector ? "sel:" + sel_text(sel) : std::string("nil");
-      sig += '\x1c';
-      sig += t.topology_key;
+      const std::string& sig = r.sig;
       auto kit = key_of.find(t.topology_key);
       if (kit == key_of.end()) {
         if (pk.keys.size() == BS_IPA_KEY_MAX)
@@ -1714,7 +1766,7 @@ Status BatchSchedulingPlugin::PackInterPodAffinity(const std::vector<const NodeI
       auto it = term_of.find(sig);
       if (it == term_of.end()) {
         it = term_of.emplace(sig, (uint32_t)terms.size()).first;
-        terms.push_back(TermInfo{t.has_selector, std::move(sel), std::move(ns)});
+        terms.push_back(TermInfo{t.has_selector, std::move(r.sel), std::move(r.ns)});
         pk.term_signatures.push_back(sig);
         pk.term_key.push_back(kit->second);
       }
@@ -1811,28 +1863,195 @@ Status BatchSchedulingPlugin::PackInterPodAffinity(const std::vector<const NodeI
   for (size_t p = 0; p < P; ++p)
     if (pending[p] && !invalid_bound && !pbad[p])
       if (!(st = classify(*pending[p], pown[p], b_terms, pclass_of, pk.pod_classes, &pk.pod_class[p])).ok()) return st;
-  // each key's values over the nodes, in order of first appearance
-  const size_t K = pk.keys.size();
-  pk.values.assign(K, {});
-  pk.n_values.assign(K, 0);
-  pk.topo.assign(K * N, BS_TOPO_NONE);
-  for (size_t k = 0; k < K; ++k) {
-    std::unordered_map<std::string, uint32_t> value_of;
-    for (size_t i = 0; i < N; ++i) {
-      if (!snapshot[i] || !snapshot[i]->node) continue;
-      const auto& labels = snapshot[i]->node->labels;
-      const auto l = labels.find(pk.keys[k]);
-      if (l == labels.end()) continue;
-      auto it = value_of.find(l->second);
-      if (it == value_of.end()) {
-        it = value_of.emplace(l->second, (uint32_t)pk.values[k].size()).first;
-        pk.values[k].push_back(l->second);
-      }
-      pk.topo[k * N + i] = it->second;
-    }
-    pk.n_values[k] = (uint32_t)pk.values[k].size();
-  }
+  number_topology(snapshot, pk.keys, &pk.values, &pk.n_values, &pk.topo);
   return Status{};
+}
+
+void BatchSchedulingPlugin::SetInterPodAffinityFilter(bool on) {
+  std::lock_guard<std::mutex> lk(mu_);
+  interpod_filter_ = on;
+}
+
+Status BatchSchedulingPlugin::PackInterPodFilter(const std::vector<const NodeInfo*>& snapshot,
+                                                 const std::vector<const Pod*>& pending, PackedInterPodFilter* out) {
+  if (!out) return Status{BS_CODE_ERROR, "PackInterPodFilter: null output"};
+  PackedInterPodFilter& pk = *out;
+  pk = PackedInterPodFilter();
+  const size_t N = snapshot.size(), P = pending.size();
+  std::unordered_map<std::string, uint32_t> key_of, term_of;
+  // the dictionary term of signature `sig` (role-prefixed) on `key`; fresh: it is new
+  auto term_id = [&](const std::string& sig, const std::string& key, uint32_t* id, bool* fresh) -> Status {
+    auto kit = key_of.find(key);
+    if (kit == key_of.end()) {
+      if (pk.keys.size() == BS_IPA_KEY_MAX)
+        return Status{BS_CODE_ERROR, "PackInterPodFilter: more than BS_IPA_KEY_MAX topology keys"};
+      kit = key_of.emplace(key, (uint32_t)pk.keys.size()).first;
+      pk.keys.push_back(key);
+    }
+    auto it = term_of.find(sig);
+    *fresh = it == term_of.end();
+    if (*fresh) {
+      it = term_of.emplace(sig, (uint32_t)pk.term_key.size()).first;
+      pk.term_signatures.push_back(sig);
+      pk.term_key.push_back(kit->second);
+    }
+    *id = it->second;
+    return Status{};
+  };
+  // bound pods and their required anti-affinity terms (own = 1)
+  std::vector<const Pod*> bound;
+  std::vector<std::map<uint32_t, std::pair<int32_t, uint8_t>>> bent;   // term -> (own, match)
+  std::vector<std::pair<ResolvedTerm, uint32_t>> existing;             // distinct existing anti terms and their ids
+  Status st;
+  for (size_t i = 0; i < N; ++i) {
+    if (!snapshot[i] || !snapshot[i]->node) continue;
+    for (const Pod* bp : snapshot[i]->pods) {
+      if (!bp) continue;
+      if (bound.size() == BS_IPF_BOUND_MAX)
+        return Status{BS_CODE_ERROR, "PackInterPodFilter: more than BS_IPF_BOUND_MAX bound pods"};
+      bound.push_back(bp);
+      pk.bound_node.push_back((uint32_t)i);
+      bent.emplace_back();
+      for (const PodAffinityTerm& t : bp->required_pod_anti_affinity) {
+        ResolvedTerm r = resolve_term(t, bp->ns);
+        uint32_t id;
+        bool fresh;
+        if (!(st = term_id("x\x1e" + r.sig, t.topology_key, &id, &fresh)).ok()) return st;
+        if (fresh) existing.emplace_back(std::move(r), id);
+        bent.back()[id].first = 1;
+      }
+    }
+  }
+  // pending pods: EXISTING entries, the affinity set's terms, the anti-affinity terms
+  struct Set { std::vector<ResolvedTerm> terms; std::vector<uint32_t> ids; };
+  std::vector<Set> sets;
+  std::vector<std::pair<ResolvedTerm, uint32_t>> antis;
+  std::unordered_map<std::string, size_t> set_of;
+  std::map<std::pair<std::vector<std::pair<uint32_t, uint8_t>>, uint8_t>, uint32_t> class_of;
+  pk.pod_class.assign(P, BS_IPF_NONE);
+  for (size_t p = 0; p < P; ++p) {
+    if (!pending[p]) continue;
+    const Pod& pod = *pending[p];
+    std::set<std::pair<uint32_t, uint8_t>> ent;
+    for (auto& e : existing)
+      if (pod_matches_term(pod, e.first)) ent.emplace(e.second, (uint8_t)BS_IPF_EXISTING);
+    uint8_t self = 0;
+    if (!pod.required_pod_affinity.empty()) {
+      Set set;
+      std::string ssig;
+      for (const PodAffinityTerm& t : pod.required_pod_affinity) {
+        set.terms.push_back(resolve_term(t, pod.ns));
+        ssig += set.terms.back().sig;
+        ssig += '\x1f';
+      }
+      auto it = set_of.find(ssig);
+      if (it == set_of.end()) {
+        for (size_t k = 0; k < set.terms.size(); ++k) {
+          uint32_t id;
+          bool fresh;
+          if (!(st = term_id("a\x1e" + ssig + "\x1e" + std::to_string(k), pod.required_pod_affinity[k].topology_key,
+                             &id, &fresh)).ok())
+            return st;
+          set.ids.push_back(id);
+        }
+        it = set_of.emplace(ssig, sets.size()).first;
+        sets.push_back(std::move(set));
+      }
+      const Set& s = sets[it->second];
+      self = 1;
+      for (size_t k = 0; k < s.terms.size(); ++k) {
+        ent.emplace(s.ids[k], (uint8_t)BS_IPF_AFFINITY);
+        self = self && pod_matches_term(pod, s.terms[k]);
+      }
+    }
+    for (const PodAffinityTerm& t : pod.required_pod_anti_affinity) {
+      ResolvedTerm r = resolve_term(t, pod.ns);
+      uint32_t id;
+      bool fresh;
+      if (!(st = term_id("n\x1e" + r.sig, t.topology_key, &id, &fresh)).ok()) return st;
+      if (fresh) antis.emplace_back(std::move(r), id);
+      ent.emplace(id, (uint8_t)BS_IPF_ANTI);
+    }
+    if (ent.empty()) continue;
+    if (ent.size() > BS_IPF_CLASS_MAX)
+      return Status{BS_CODE_ERROR, "PackInterPodFilter: a pod lists more than BS_IPF_CLASS_MAX terms"};
+    auto key = std::make_pair(std::vector<std::pair<uint32_t, uint8_t>>(ent.begin(), ent.end()), self);
+    auto it = class_of.find(key);
+    if (it == class_of.end()) {
+      it = class_of.emplace(key, pk.n_pod_classes()).first;
+      for (auto& e : key.first) {
+        pk.pod_term.push_back(e.first);
+        pk.pod_role.push_back(e.second);
+      }
+      pk.pod_offset.push_back((uint32_t)pk.pod_term.size());
+      pk.self_match.push_back(self);
+    }
+    pk.pod_class[p] = it->second;
+  }
+  // the bound pods' match entries: a set's terms when they match the whole set, an anti term when they match it
+  for (size_t k = 0; k < bound.size(); ++k) {
+    for (const Set& s : sets) {
+      bool all = true;
+      for (const ResolvedTerm& r : s.terms) all = all && pod_matches_term(*bound[k], r);
+      if (all)
+        for (uint32_t id : s.ids) bent[k][id].second = 1;
+    }
+    for (auto& a : antis)
+      if (pod_matches_term(*bound[k], a.first)) bent[k][a.second].second = 1;
+  }
+  std::map<std::vector<std::tuple<uint32_t, int32_t, uint8_t>>, uint32_t> bclass_of;
+  pk.bound_class.assign(bound.size(), BS_IPF_NONE);
+  for (size_t k = 0; k < bound.size(); ++k) {
+    if (bent[k].empty()) continue;
+    if (bent[k].size() > BS_IPF_CLASS_MAX)
+      return Status{BS_CODE_ERROR, "PackInterPodFilter: a bound pod lists more than BS_IPF_CLASS_MAX terms"};
+    std::vector<std::tuple<uint32_t, int32_t, uint8_t>> key;
+    for (auto& kv : bent[k]) key.emplace_back(kv.first, kv.second.first, kv.second.second);
+    auto it = bclass_of.find(key);
+    if (it == bclass_of.end()) {
+      PackedInterPodAffinity::Classes& cl = pk.bound_classes;
+      it = bclass_of.emplace(key, cl.n_classes()).first;
+      for (auto& e : key) {
+        cl.term.push_back(std::get<0>(e));
+        cl.own.push_back(std::get<1>(e));
+        cl.match.push_back(std::get<2>(e));
+      }
+      cl.offset.push_back((uint32_t)cl.term.size());
+    }
+    pk.bound_class[k] = it->second;
+  }
+  number_topology(snapshot, pk.keys, &pk.values, &pk.n_values, &pk.topo);
+  return Status{};
+}
+
+Status BatchSchedulingPlugin::UploadInterPodFilter() {
+  auto fail = [&](int rc) {
+    return Status{BS_CODE_ERROR, std::string("bsched: ") + bs_strerror(rc) + " (" + bs_last_error(eng_) + ")"};
+  };
+  int rc = bs_set_interpod_filter(eng_, interpod_filter_ ? 1 : 0);
+  if (rc) return fail(rc);
+  if (!interpod_filter_) return Status{};
+  PackedInterPodFilter pk;
+  Status st = PackInterPodFilter(snapshot_, pending_, &pk);
+  if (!st.ok()) return st;
+  const PackedInterPodAffinity::Classes& c = pk.bound_classes;
+  bs_interpod_nodes nt{(uint32_t)snapshot_.size(), (uint32_t)pk.keys.size(), pk.n_values.data(), pk.topo.data(),
+                       (uint32_t)pk.term_key.size(), pk.term_key.data(), (uint32_t)pk.bound_node.size(),
+                       pk.bound_node.data(), pk.bound_class.data(),
+                       bs_interpod_classes{c.n_classes(), c.offset.data(), c.term.data(), c.own.data(), c.match.data()}};
+  rc = bs_upload_node_interpod_filter(eng_, &nt);
+  if (!rc) {
+    bs_interpod_filter_pods pt{(uint32_t)pending_.size(), pk.pod_class.data(), pk.n_pod_classes(), pk.pod_offset.data(),
+                               pk.pod_term.data(), pk.pod_role.data(), pk.self_match.data()};
+    rc = bs_upload_pod_interpod_filter(eng_, &pt);
+  }
+  return rc ? fail(rc) : Status{};
+}
+
+std::vector<uint32_t> BatchSchedulingPlugin::InterPodReasonCounts(const std::string& uid) const {
+  const int32_t row = pod_row_.find(uid);
+  if (row < 0 || ipf_reasons_.size() < ((size_t)row + 1) * 3) return {};
+  return std::vector<uint32_t>(ipf_reasons_.begin() + (size_t)row * 3, ipf_reasons_.begin() + ((size_t)row + 1) * 3);
 }
 
 Status BatchSchedulingPlugin::UploadInterPodAffinity() {
@@ -1874,10 +2093,12 @@ std::string BatchSchedulingPlugin::FitError(const std::string& uid) const {
   if (counts.empty()) return "";
   std::vector<const char*> names;
   for (auto& nm : packed_.scalar_names) names.push_back(nm.c_str());
+  const std::vector<uint32_t> ipf = InterPodReasonCounts(uid);   // empty while the filter is off
   std::vector<char> buf(256);
   for (;;) {   // grows until the whole message fits
-    const int rc = bs_format_fit_error(counts.data(), packed_.lanes, packed_.n_nodes, names.empty() ? nullptr : names.data(),
-                                       buf.data(), buf.size());
+    const int rc = bs_format_fit_error_interpod(counts.data(), packed_.lanes, ipf.empty() ? nullptr : ipf.data(),
+                                                packed_.n_nodes, names.empty() ? nullptr : names.data(), buf.data(),
+                                                buf.size());
     if (rc == BS_OK) return std::string(buf.data());
     if (buf.size() > (1u << 20)) return "";
     buf.resize(buf.size() * 4);
@@ -1900,6 +2121,8 @@ Status BatchSchedulingPlugin::UpdateRound(const std::vector<std::pair<uint32_t, 
     st = UploadSpread();
     if (!st.ok()) return st;
     st = UploadInterPodAffinity();
+    if (!st.ok()) return st;
+    st = UploadInterPodFilter();
     if (!st.ok()) return st;
   }
   return Reevaluate();
@@ -1958,6 +2181,8 @@ Status BatchSchedulingPlugin::UpdateNodes(const std::vector<std::pair<uint32_t, 
   st = UploadSpread();           // ... and the spread side (the changed NodeInfos' pods and zones: both sides)
   if (!st.ok()) return st;
   st = UploadInterPodAffinity();   // ... and the inter-pod side (the changed NodeInfos' pods and labels: both sides)
+  if (!st.ok()) return st;
+  st = UploadInterPodFilter();     // ... and the filter's sides, for the same reasons
   if (!st.ok()) return st;
   // the round's decisions follow the new snapshot: same pods, same groups, same result vectors
   return evaluate ? Reevaluate() : Status{};
@@ -2168,6 +2393,8 @@ Status BatchSchedulingPlugin::RunPreempt(const std::vector<uint32_t>& rows, std:
 
 Status BatchSchedulingPlugin::Preempt(const std::string& uid, std::string* node, std::vector<std::string>* victim_uids) {
   std::lock_guard<std::mutex> lk(mu_);
+  if (interpod_filter_)
+    return Status{BS_CODE_ERROR, "Preempt: the MatchInterPodAffinity filter is on (SetInterPodAffinityFilter(false) first)"};
   const int32_t p = pod_row_.find(uid);
   if (!eng_ || p < 0) return Status{BS_CODE_ERROR, "Preempt: " + uid + " is not a pending pod of the round"};
   if (!bound_.n) {   // no NodeInfo lists pods: nothing to evict, the table was never uploaded
@@ -2186,6 +2413,8 @@ Status BatchSchedulingPlugin::Preempt(const std::string& uid, std::string* node,
 Status BatchSchedulingPlugin::PreemptAll(std::vector<Preemption>* out) {
   std::lock_guard<std::mutex> lk(mu_);
   if (!eng_ || !out) return Status{BS_CODE_ERROR, "PreemptAll: no round has been started"};
+  if (interpod_filter_)
+    return Status{BS_CODE_ERROR, "PreemptAll: the MatchInterPodAffinity filter is on (SetInterPodAffinityFilter(false) first)"};
   out->clear();
   if (!bound_.n) return Status{};
   std::vector<uint32_t> rows;
@@ -2201,6 +2430,8 @@ Status BatchSchedulingPlugin::PreemptAll(std::vector<Preemption>* out) {
 Status BatchSchedulingPlugin::PreemptQueue(std::vector<Preemption>* out, bool gang) {
   std::lock_guard<std::mutex> lk(mu_);
   if (!eng_ || !out) return Status{BS_CODE_ERROR, "PreemptQueue: no round has been started"};
+  if (interpod_filter_)
+    return Status{BS_CODE_ERROR, "PreemptQueue: the MatchInterPodAffinity filter is on (SetInterPodAffinityFilter(false) first)"};
   out->clear();
   if (!bound_.n) return Status{};
   // PreemptAll's pods in queue order; with gang units, one unit per group at its first preemptor's place
@@ -2235,6 +2466,8 @@ Status BatchSchedulingPlugin::PreemptQueue(std::vector<Preemption>* out, bool ga
 Status BatchSchedulingPlugin::ReplayQueue(std::vector<ReplayDecision>* out, ReplayNodeChoice choice) {
   if (!out) return Status{BS_CODE_ERROR, "ReplayQueue: null output"};
   if (!eng_) return Status{BS_CODE_ERROR, "ReplayQueue: no round has been started"};
+  if (interpod_filter_)
+    return Status{BS_CODE_ERROR, "ReplayQueue: the MatchInterPodAffinity filter is on (SetInterPodAffinityFilter(false) first)"};
   const bool prio = choice == ReplayNodeChoice::kPriority;
   if (prio && !priority_k_)
     return Status{BS_CODE_ERROR, "ReplayQueue: kPriority needs a plugin created with priority_k > 0 (its rounds upload "

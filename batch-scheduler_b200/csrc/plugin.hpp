@@ -99,9 +99,10 @@ struct Pod {
   int64_t start_ns = 0;                 // Status.StartTime of a bound pod (preemption: MoreImportantPod)
   std::string controller_kind, controller_uid;   // metav1.GetControllerOf: the controlling owner ("" = none)
   bool terminating = false;             // DeletionTimestamp != nil (SelectorSpread does not count the pod)
-  // Spec.Affinity.PodAffinity / PodAntiAffinity (InterPodAffinity): the required pod-affinity terms and the preferred
-  // pod-affinity and pod-anti-affinity terms; required anti-affinity is not read
-  std::vector<PodAffinityTerm> required_pod_affinity;
+  // Spec.Affinity.PodAffinity / PodAntiAffinity: the required pod-affinity terms (InterPodAffinity's hard weight and
+  // the MatchInterPodAffinity filter), the required pod-anti-affinity terms (the filter) and the preferred
+  // pod-affinity and pod-anti-affinity terms (InterPodAffinity)
+  std::vector<PodAffinityTerm> required_pod_affinity, required_pod_anti_affinity;
   std::vector<WeightedPodAffinityTerm> preferred_pod_affinity, preferred_pod_anti_affinity;
 };
 // The objects whose selectors SelectorSpread spreads by: Services and ReplicationControllers select with a map,
@@ -313,6 +314,26 @@ struct PackedInterPodAffinity {
   std::vector<uint32_t> pod_class;              // [n_pods], BS_IPA_NONE = no entries (scores 0)
   Classes pod_classes;
 };
+// The columns of the MatchInterPodAffinity filter of one round (bs_upload_node_interpod_filter,
+// bs_upload_pod_interpod_filter): keys, values and topo as PackedInterPodAffinity numbers them; the filter's own term
+// dictionary (term_signatures); the bound pods of NodeInfo::pods and their classes of (term, own, match); each pending
+// pod's class of (term, role) with its self_match byte.
+struct PackedInterPodFilter {
+  std::vector<std::string> keys;
+  std::vector<std::vector<std::string>> values;
+  std::vector<uint32_t> n_values;
+  std::vector<uint32_t> topo;                   // [n_keys][n_nodes], BS_TOPO_NONE = the node lacks the key
+  std::vector<std::string> term_signatures;     // term id -> signature
+  std::vector<uint32_t> term_key;               // [n_terms]
+  std::vector<uint32_t> bound_node, bound_class;   // [n_bound], BS_IPF_NONE = no entries
+  PackedInterPodAffinity::Classes bound_classes;
+  std::vector<uint32_t> pod_class;              // [n_pods], BS_IPF_NONE = no entries (passes every node)
+  std::vector<uint32_t> pod_offset{0};          // [n_classes + 1]
+  std::vector<uint32_t> pod_term;
+  std::vector<uint8_t> pod_role;                // BS_IPF_AFFINITY / BS_IPF_ANTI / BS_IPF_EXISTING
+  std::vector<uint8_t> self_match;              // [n_classes]
+  uint32_t n_pod_classes() const { return (uint32_t)pod_offset.size() - 1; }
+};
 // normalizedImageName (ImageLocality): ":latest" appended when the last ':' does not follow the last '/'
 std::string normalized_image_name(const std::string& name);
 
@@ -504,6 +525,13 @@ class BatchSchedulingPlugin {
   // weight of kube-scheduler v1.17's InterPodAffinity priority in PriorityNodes (bs_set_interpod_weight; 0 = off, the
   // default; v1.17's default profile is 1), read by the next round; ReplayQueue(kPriority) refuses a non-zero weight
   void SetInterPodAffinityWeight(uint32_t inter_pod_affinity);
+  // kube-scheduler v1.17's MatchInterPodAffinity filter in every pod's fit set (bs_set_interpod_filter; off by
+  // default), from the next round, delta round or UpdateNodes on: PackInterPodFilter's columns are uploaded with each
+  // of them.  While it is on, ReplayQueue, Preempt, PreemptAll and PreemptQueue return an error.
+  void SetInterPodAffinityFilter(bool on);
+  // the last round's companion reason row of a pending pod (bs_fetch_interpod_reason_rows: the nodes that pass every
+  // other check and fail the filter at E, A, N); empty without BS_OUT_REASONS or for an unknown uid
+  std::vector<uint32_t> InterPodReasonCounts(const std::string& uid) const;
   // hardPodAffinitySymmetricWeight: the weight of a bound pod's required pod-affinity term in InterPodAffinity,
   // 0..100 (else an error), default 1; 0 leaves those terms out
   Status SetHardPodAffinityWeight(int32_t hard_pod_affinity_weight);
@@ -617,6 +645,19 @@ class BatchSchedulingPlugin {
                                      const std::vector<const Pod*>& pending, int32_t hard_weight,
                                      PackedInterPodAffinity* out);
 
+  // The columns of the MatchInterPodAffinity filter (no GPU), from NodeInfo::pods of nodes with a Node() (terminating
+  // ones too) and the pending pods.  Keys and values are numbered as PackInterPodAffinity numbers them, and terms are
+  // identified the same way (resolved, sorted namespaces, SelectorSpread's converted selector text, key).  The
+  // dictionary: the bound pods' required anti-affinity terms (own = 1 on their owners; a pending pod that matches one
+  // lists it as BS_IPF_EXISTING), then per pending pod its required affinity set, one term per set member
+  // (BS_IPF_AFFINITY; a bound pod's match = it matches every member), and its required anti-affinity terms
+  // (BS_IPF_ANTI; match = it matches the term); equal sets and equal anti terms share their terms.  A selector that
+  // fails to convert matches no pod; an empty key is a key no node carries.  self_match: the pending pod matches its
+  // whole set.  Classes are numbered in order of first appearance; a pod without entries has none (BS_IPF_NONE).
+  // More than BS_IPA_KEY_MAX keys, BS_IPF_BOUND_MAX bound pods or BS_IPF_CLASS_MAX entries in a class is an error.
+  static Status PackInterPodFilter(const std::vector<const NodeInfo*>& snapshot, const std::vector<const Pod*>& pending,
+                                   PackedInterPodFilter* out);
+
   static Status Pack(const std::vector<const NodeInfo*>& snapshot, const std::vector<const Pod*>& pending,
                      const std::vector<PodGroup>& groups, const std::vector<uint32_t>& matched,
                      const std::vector<uint8_t>& extra_group_flags, const std::vector<uint8_t>& extra_pod_flags,
@@ -651,6 +692,7 @@ class BatchSchedulingPlugin {
   std::vector<PodDisruptionBudget> pdbs_;               // SetPodDisruptionBudgets
   uint32_t interpod_weight_ = 0;                        // SetInterPodAffinityWeight
   int32_t hard_pod_affinity_weight_ = 1;                // SetHardPodAffinityWeight
+  bool interpod_filter_ = false;                        // SetInterPodAffinityFilter
   std::string init_error_;
   int64_t max_schedule_time_ns_;
   std::map<std::string, GroupState> groups_;                        // ordered: canonical table order
@@ -671,6 +713,7 @@ class BatchSchedulingPlugin {
   std::vector<int32_t> topk_node_;                                  // [P][topk_] (BS_OUT_TOPK)
   std::vector<int64_t> topk_score_;
   std::vector<uint32_t> reasons_;                                   // [P][4 + lanes] (BS_OUT_REASONS)
+  std::vector<uint32_t> ipf_reasons_;                               // [P][3] companion rows (BS_OUT_REASONS)
   std::vector<int32_t> prio_node_;                                  // [P][priority_k_] (BS_OUT_PRIORITY)
   std::vector<int64_t> prio_score_;
   int64_t now_ns_ = 0;
@@ -688,6 +731,7 @@ class BatchSchedulingPlugin {
                              // weight is non-zero; no-op without priority_k
   Status UploadInterPodAffinity();   // both inter-pod sides of snapshot_ and pending_ and the weight; the columns
                                     // only while the weight is non-zero; no-op without priority_k
+  Status UploadInterPodFilter();   // the filter switch and, while it is on, both filter sides of snapshot_ and pending_
   Status UploadLocality();   // both locality sides of snapshot_ and pending_ and the two weights; the columns only
                              // while a weight is non-zero; no-op without priority_k
   Status UploadBound();  // packs and uploads the bound-pod table of snapshot_ (no-op when no NodeInfo lists pods)

@@ -440,6 +440,50 @@ class Engine:
             t = capi.InterpodPodsC(len(pcls), capi.ptr(pcls), classes(cl, keep))
             self._check(self.lib.bs_upload_pod_interpod(self.h, C.byref(t)))
 
+    def set_interpod_filter(self, on: bool = False):
+        """Switch kube-scheduler's MatchInterPodAffinity filter (required pod affinity and anti-affinity) into every
+        pod's fit set (off by default).  While it is on, each round needs upload_interpod_filter's two sides, and
+        replay and preempt refuse to run."""
+        self._check(self.lib.bs_set_interpod_filter(self.h, 1 if on else 0))
+
+    def upload_interpod_filter(self, node=None, pods=None):
+        """The columns of the MatchInterPodAffinity filter (include/bsched.h bs_upload_node_interpod_filter).  node: as
+        upload_interpod's node side, with own 1 for a bound pod's required anti-affinity terms and match 1 for the terms
+        it matches.  pods = (pod_class [P], (class_offset [C + 1], term, role uint8, self_match [C] uint8)): each pod's
+        class (capi.IPF_NONE: none) and the class table with roles capi.IPF_AFFINITY / IPF_ANTI / IPF_EXISTING.
+        Uploading nodes (or updating node rows) drops the node side, uploading pods the pod side."""
+        if node is not None:
+            nv, topo, tkey, bnode, bcls, (off, term, own, match) = node
+            keep = [np.ascontiguousarray(off, dtype=np.uint32).reshape(-1), np.ascontiguousarray(term, dtype=np.uint32),
+                    np.ascontiguousarray(own, dtype=np.int32), np.ascontiguousarray(match, dtype=np.uint8)]
+            nv = np.ascontiguousarray(nv, dtype=np.uint32).reshape(-1)
+            topo = (np.ascontiguousarray(topo, dtype=np.uint32).reshape(len(nv), -1) if len(nv)
+                    else np.zeros((0, self.N), np.uint32))
+            tkey = np.ascontiguousarray(tkey, dtype=np.uint32).reshape(-1)
+            bnode = np.ascontiguousarray(bnode, dtype=np.uint32).reshape(-1)
+            bcls = np.ascontiguousarray(bcls, dtype=np.uint32).reshape(-1)
+            if len(bnode) != len(bcls):
+                raise ValueError("bound_node and bound_class must have one entry per bound pod")
+            cl = capi.InterpodClassesC(max(len(keep[0]) - 1, 0), *(capi.ptr(x) for x in keep))
+            t = capi.InterpodNodesC(topo.shape[1], len(nv), capi.ptr(nv), capi.ptr(topo), len(tkey), capi.ptr(tkey),
+                                    len(bnode), capi.ptr(bnode), capi.ptr(bcls), cl)
+            self._check(self.lib.bs_upload_node_interpod_filter(self.h, C.byref(t)))
+        if pods is not None:
+            pcls, (off, term, role, self_match) = pods
+            a = [np.ascontiguousarray(pcls, dtype=np.uint32).reshape(-1),
+                 np.ascontiguousarray(off, dtype=np.uint32).reshape(-1), np.ascontiguousarray(term, dtype=np.uint32),
+                 np.ascontiguousarray(role, dtype=np.uint8), np.ascontiguousarray(self_match, dtype=np.uint8)]
+            t = capi.InterpodFilterPodsC(len(a[0]), capi.ptr(a[0]), max(len(a[1]) - 1, 0), *(capi.ptr(x) for x in a[1:]))
+            self._check(self.lib.bs_upload_pod_interpod_filter(self.h, C.byref(t)))
+
+    def fetch_interpod_reason_rows(self, pod0=0, n=None) -> np.ndarray:
+        """[n, 3] uint32: the companion of reason_rows, the nodes that fail MatchInterPodAffinity after every other
+        check, by step: existing pods' anti-affinity (E), the pod's affinity (A), the pod's anti-affinity (N)."""
+        n = self.P - pod0 if n is None else n
+        out = np.zeros((n, 3), np.uint32)
+        self._check(self.lib.bs_fetch_interpod_reason_rows(self.h, pod0, n, capi.ptr(out)))
+        return out
+
     def priority_rows(self, pod0=0, n=None):
         """(nodes [n, K] int32, scores [n, K] int64): each pod's fitting nodes by priority score descending, then node
         index ascending; min(K, feasible_count) entries, padded with node -1 and score INT64_MIN."""
@@ -729,9 +773,10 @@ def format_remove_message(reason: int, pod_name: str = "", victim_name: str = ""
     return buf.value.decode()
 
 
-def format_fit_error(counts, n_lanes: int, n_nodes: int, scalar_names=None, buf_len: int = 4096) -> str:
+def format_fit_error(counts, n_lanes: int, n_nodes: int, scalar_names=None, buf_len: int = 4096, interpod=None) -> str:
     """kube-scheduler's FailedScheduling text for one reason row; needs no engine and no device.  scalar_names: the
-    names of lanes 4.. (None: "lane<d>")."""
+    names of lanes 4.. (None: "lane<d>").  interpod: the row's companion (E, A, N) from fetch_interpod_reason_rows, whose
+    MatchInterPodAffinity entries join the message (bs_format_fit_error_interpod)."""
     lib = capi.load()
     row = np.ascontiguousarray(counts, dtype=np.uint32)
     if row.shape != (4 + n_lanes,):
@@ -740,8 +785,15 @@ def format_fit_error(counts, n_lanes: int, n_nodes: int, scalar_names=None, buf_
     if scalar_names is not None:
         names = (C.c_char_p * max(1, n_lanes - 4))(*[s.encode() for s in scalar_names])
     buf = C.create_string_buffer(buf_len)
-    rc = lib.bs_format_fit_error(capi.ptr(row), n_lanes, n_nodes, C.cast(names, C.c_void_p) if names is not None else None,
-                                 buf, buf_len)
+    if interpod is not None:
+        ip = np.ascontiguousarray(interpod, dtype=np.uint32)
+        if ip.shape != (3,):
+            raise ValueError("an inter-pod companion row has 3 counters")
+        rc = lib.bs_format_fit_error_interpod(capi.ptr(row), n_lanes, capi.ptr(ip), n_nodes,
+                                              C.cast(names, C.c_void_p) if names is not None else None, buf, buf_len)
+    else:
+        rc = lib.bs_format_fit_error(capi.ptr(row), n_lanes, n_nodes,
+                                     C.cast(names, C.c_void_p) if names is not None else None, buf, buf_len)
     if rc != 0:
         raise capi.BsError(rc, lib.bs_strerror(rc).decode())
     return buf.value.decode()

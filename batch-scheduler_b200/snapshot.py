@@ -523,6 +523,96 @@ def node_interpod(snap: Snapshot, seed: int, n_zones: int = 8, rack_size: int = 
     return (n_values, topo, term_key, bound_node, bound_class, bcl), (pod_class, pcl)
 
 
+IPF_NONE = 0xFFFFFFFF                           # BS_IPF_NONE
+IPF_AFFINITY, IPF_ANTI, IPF_EXISTING = range(3)  # BS_IPF_* roles
+
+
+def node_interpod_filter(snap: Snapshot, seed: int, n_zones: int = 8, unlabelled: float = 0.05,
+                         one_per_host: float = 0.3, ps_affine: float = 0.2, ps_missing: float = 0.1,
+                         siblings: int = 2, n_blockers: int = 16, blocked: float = 0.1, filler: int = 2,
+                         self_affine: float = 0.4):
+    """Seeded columns of the MatchInterPodAffinity filter for a table without objects: (node, pods) as
+    Engine.upload_interpod_filter takes them.  Two topology keys: a hostname-like key (one value per node) and a
+    zone-like key (n_zones values; a share `unlabelled` of the nodes lacks it).  Per gang:
+    - a share one_per_host carries required anti-affinity on the hostname key against its own job label, with up to
+      `siblings` of its pods already bound;
+    - a share ps_affine needs the zone of its labelled "ps" pod (required affinity, the workers do not match it
+      themselves); for a share ps_missing of those the ps pod is not bound, so no node passes;
+    - a share self_affine needs the zone of its own job (required affinity the workers match themselves, self_match 1)
+      with up to `siblings` of its pods bound: none bound, or bound only on nodes without the zone key, leaves the
+      first-pod exception to let every node pass.
+    n_blockers bound pods carry required anti-affinity on the zone key, each against a label that the pods of a share
+    `blocked` of the gangs carry.  `filler` bound pods per node have no class.  Own generator: other draws keep their
+    seeds."""
+    rng = np.random.default_rng(seed)
+    N, G = snap.nodes.n, snap.groups.n
+    gid = snap.pods.gid
+    n_values = np.array([max(N, 1), max(n_zones, 1)], np.uint32)
+    topo = np.stack([np.arange(N), rng.integers(0, max(n_zones, 1), N)]).astype(np.uint32)
+    topo[1, rng.random(N) < unlabelled] = TOPO_NONE
+    term_key, bnode, bcls = [], [], []
+    boff, bterm, bown, bmatch = [0], [], [], []
+
+    def term(key):
+        term_key.append(key)
+        return len(term_key) - 1
+
+    def bound(node, entries):   # one bound pod with a class of its own: entries (term, own, match)
+        for t, o, m in entries:
+            bterm.append(t); bown.append(o); bmatch.append(m)
+        boff.append(len(bterm))
+        bnode.append(node)
+        bcls.append(len(boff) - 2)
+
+    gang_entries = [[] for _ in range(G)]
+    anti = rng.random(G) < one_per_host
+    ps = (rng.random(G) < ps_affine) & ~anti
+    missing = rng.random(G) < ps_missing
+    selfaff = (rng.random(G) < self_affine) & ~anti & ~ps
+    nsib = rng.integers(0, siblings + 1, G)
+    for g in range(G):
+        if anti[g]:
+            t = term(0)
+            gang_entries[g].append((t, IPF_ANTI))
+            for _ in range(int(rng.integers(0, siblings + 1))):
+                bound(int(rng.integers(0, max(N, 1))), [(t, 0, 1)])
+        elif ps[g]:
+            t = term(1)
+            gang_entries[g].append((t, IPF_AFFINITY))
+            if not missing[g]:
+                bound(int(rng.integers(0, max(N, 1))), [(t, 0, 1)])
+        elif selfaff[g]:
+            t = term(1)
+            gang_entries[g].append((t, IPF_AFFINITY))
+            for _ in range(int(nsib[g]) if N else 0):
+                bound(int(rng.integers(0, N)), [(t, 0, 1)])
+    for _ in range(n_blockers if N else 0):
+        w = term(1)
+        bound(int(rng.integers(0, N)), [(w, 1, 0)])
+        for g in np.flatnonzero(rng.random(G) < blocked):
+            gang_entries[g].append((w, IPF_EXISTING))
+    bnode += rng.integers(0, max(N, 1), filler * N).tolist()
+    bcls += [IPF_NONE] * (filler * N)
+    cls_of_gang = np.full(G, IPF_NONE, np.uint32)
+    poff, pterm, prole, pself = [0], [], [], []
+    for g in range(G):
+        ent = gang_entries[g][:64]
+        if not ent:
+            continue
+        cls_of_gang[g] = len(poff) - 1
+        pterm += [t for t, _ in ent]
+        prole += [r for _, r in ent]
+        poff.append(len(pterm))
+        pself.append(1 if selfaff[g] else 0)
+    ok = (gid >= 0) & (gid < G)
+    pod_class = np.where(ok, cls_of_gang[np.clip(gid, 0, max(G - 1, 0))] if G else IPF_NONE, IPF_NONE).astype(np.uint32)
+    node = (n_values, topo, np.array(term_key, np.uint32), np.array(bnode, np.uint32), np.array(bcls, np.uint32),
+            (np.array(boff, np.uint32), np.array(bterm, np.uint32), np.array(bown, np.int32), np.array(bmatch, np.uint8)))
+    pods = (pod_class, (np.array(poff, np.uint32), np.array(pterm, np.uint32), np.array(prole, np.uint8),
+                        np.array(pself, np.uint8)))
+    return node, pods
+
+
 # ----------------------------------------------------------------------------
 # splitmix64 stream (vectorised): value i of the stream with seed s is
 # mix(s + (i+1)*0x9E3779B97F4A7C15).

@@ -679,6 +679,78 @@ int bs_upload_node_interpod(bs_engine* e, const bs_interpod_nodes* t);
  * either side changes.  bs_upload_pods drops the side. */
 int bs_upload_pod_interpod(bs_engine* e, const bs_interpod_pods* t);
 
+/* ---- kube-scheduler v1.17's MatchInterPodAffinity filter: required pod affinity and anti-affinity in the fit set ----
+ * Off by default.  While it is on, every evaluation ANDs it into each pod's fit set: the fit bitmap, the scores,
+ * feasible_count, best_node, the top-K lists, the fit set of the BS_OUT_PRIORITY lists, the reason rows (through the
+ * companion rows below) and the Permit verdict.  It does not reach PreFilter's cluster scans or BS_OUT_FILTER
+ * (core.go's checkFit and Filter never call it).  All pods of a round check against the one uploaded snapshot: no pod
+ * sees another pending pod's placement.
+ *
+ * The caller resolves the objects into a dictionary of terms t = (namespaces, selector, topology key key(t)), with
+ * empty namespaces already replaced by the namespace of the pod that defines the term.  "Existing pods" are every pod of
+ * the snapshot's NodeInfo.Pods() (terminating and assumed pods included) on a node that has a Node(); they are the
+ * node side's bound pods.  Class entries of a bound pod are (t, own, match): own = 1 when t is one of its required
+ * anti-affinity terms, match = 1 when it matches t.  A required affinity set {t1..tk} of a pending pod is k dictionary
+ * terms of their own, and a bound pod's match on each of them means "matches every term of the set".  Class entries of
+ * a pending pod are (t, role): BS_IPF_AFFINITY (t is in its required affinity set), BS_IPF_ANTI (t is one of its
+ * required anti-affinity terms), BS_IPF_EXISTING (it matches t, a bound pod's required anti-affinity term), and each
+ * class has a self_match byte: the pod matches every term of its own affinity set.  For pod p and node n, the first
+ * failing step decides [upstream, from memory]:
+ *     1. E: some EXISTING entry w where n carries key(w) with value v and a bound pod with own on w sits on a node
+ *           with value v (satisfiesExistingPodsAntiAffinity); applies to pods without affinity of their own
+ *     2. a class without AFFINITY and ANTI entries passes
+ *     3. A: not every AFFINITY entry t has n carrying key(t) with value v and a bound pod matching t on a node with
+ *           value v, unless no bound pod matching the set sits on a node carrying any of the keys and self_match is 1
+ *           (the first-pod exception)
+ *     4. N: some ANTI entry u where n carries key(u) with value v and a bound pod matching u sits on a node with value v
+ * A node carries a key when its topo value is not BS_TOPO_NONE; an empty topologyKey is a key no node carries.  A
+ * selector that does not convert matches no pod.  A BS_IPF_NONE pod passes every node.
+ * An evaluation with the filter on is BS_E_STATE before anything is launched when either side is missing, BS_E_INDEX
+ * when a pod class's term is >= the node side's n_terms and BS_E_INVAL when the class bit planes pass
+ * BS_IPF_TABLE_MAX_BYTES.  bs_replay, bs_replay_priority, bs_preempt and bs_preempt_walk refuse to run (BS_E_INVAL)
+ * while the filter is on: their walks would need presence that follows their own placements and victim removals.
+ *
+ * Exactness: presence is one bit per (term, value) and plane, set with atomicOr, and the emptiness test of step 3 is a
+ * per-term count of at most BS_IPF_BOUND_MAX, so every verdict is exact whatever the order. */
+int bs_set_interpod_filter(bs_engine* e, int on);
+#define BS_IPF_NONE 0xffffffffu                 /* filter class of a pod without entries: passes every node */
+#define BS_IPF_AFFINITY 0u                      /* role: a term of the pod's required affinity set */
+#define BS_IPF_ANTI 1u                          /* role: one of the pod's required anti-affinity terms */
+#define BS_IPF_EXISTING 2u                      /* role: a bound pod's required anti-affinity term the pod matches */
+#define BS_IPF_CLASS_MAX 64                     /* entries of one class, pod or bound */
+#define BS_IPF_BOUND_MAX (1u << 24)             /* bound pods of one node side: a term's count fits 32 bits */
+#define BS_IPF_TERM_MAX_BYTES (1ull << 30)      /* 2 bit planes x sum over terms of n_values[term_key[t]] at most 1 GiB */
+#define BS_IPF_TABLE_MAX_BYTES (1ull << 30)     /* 3 bit planes x pod n_classes x Npad at most 1 GiB */
+typedef struct {
+  uint32_t n_pods;                /* the pod table's */
+  const uint32_t* pod_class;      /* [n_pods] < n_classes, or BS_IPF_NONE */
+  uint32_t n_classes;
+  const uint32_t* class_offset;   /* [n_classes + 1], class_offset[0] = 0, ascending, at most BS_IPF_CLASS_MAX apart */
+  const uint32_t* term;           /* [class_offset[n_classes]] term ids of the node side's dictionary */
+  const uint8_t* role;            /* [...] BS_IPF_AFFINITY, BS_IPF_ANTI or BS_IPF_EXISTING */
+  const uint8_t* self_match;      /* [n_classes] 0 or 1 */
+} bs_interpod_filter_pods;
+/* The node side, in the layout of bs_upload_node_interpod and with its checks, and own in {0, 1} (else BS_E_RANGE).
+ * The dictionary is the filter's own.  bs_upload_nodes and bs_update_nodes drop it; a failing call leaves it dropped. */
+int bs_upload_node_interpod_filter(bs_engine* e, const bs_interpod_nodes* t);
+/* The pod side.  A wrong n_pods, a malformed class table or a role > BS_IPF_EXISTING is BS_E_INVAL, a pod_class out of
+ * range BS_E_INDEX, a self_match > 1 BS_E_RANGE; a failing call leaves it dropped.  bs_upload_pods drops it. */
+int bs_upload_pod_interpod_filter(bs_engine* e, const bs_interpod_filter_pods* t);
+/* The companion of bs_fetch_reason_rows (BS_OUT_REASONS): dense [n][3] counters, the nodes that pass the guards,
+ * checkFit and every lane of pod pod0 + p and then fail the filter at step 1 (E), 3 (A) or 4 (N).  All zero for a
+ * round evaluated with the filter off. */
+int bs_fetch_interpod_reason_rows(bs_engine* e, uint32_t pod0, uint32_t n, uint32_t* counts);
+/* bs_format_fit_error with the three counters of a companion row (interpod[3] = E, A, N) as further entries, sorted
+ * with the rest as whole strings, each only when its count is non-zero:
+ *     "<E+A+N> node(s) didn't match pod affinity/anti-affinity"
+ *     "<E> node(s) didn't satisfy existing pods anti-affinity rules"
+ *     "<A> node(s) didn't match pod affinity rules"
+ *     "<N> node(s) didn't match pod anti-affinity rules"
+ * [upstream, from memory: a failing node reports ErrPodAffinityNotMatch and the specific reason].  A NULL interpod is
+ * bs_format_fit_error. */
+int bs_format_fit_error_interpod(const uint32_t* counts, uint32_t n_lanes, const uint32_t* interpod, uint32_t n_nodes,
+                                 const char* const* scalar_names, char* buf, size_t buf_len);
+
 /* ---- preemption: PreFilterExtensions.RemovePod and the node / victims kube-scheduler's preemption would pick ----
  * The bound-pod table lists the pods already running on the snapshot's nodes (NodeInfo.Pods()).  Rows may come in
  * any order; the engine groups them by node in MoreImportantPod order (priority descending, start time ascending,

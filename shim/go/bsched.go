@@ -355,6 +355,50 @@ func (e *Engine) UploadPodInterPodAffinity(t *C.bs_interpod_pods) error {
 	return e.rc(C.bs_upload_pod_interpod(e.h, t))
 }
 
+// MatchInterPodAffinity filter roles and the class of a pod without entries (include/bsched.h BS_IPF_*).
+const (
+	IPFNone     = uint32(C.BS_IPF_NONE)
+	IPFAffinity = uint8(C.BS_IPF_AFFINITY)
+	IPFAnti     = uint8(C.BS_IPF_ANTI)
+	IPFExisting = uint8(C.BS_IPF_EXISTING)
+	IPFClassMax = int(C.BS_IPF_CLASS_MAX)
+	IPFBoundMax = uint32(C.BS_IPF_BOUND_MAX)
+)
+
+// SetInterPodAffinityFilter: kube-scheduler v1.17's MatchInterPodAffinity filter in every pod's fit set (off by
+// default).  While it is on, each Evaluate needs both filter sides, and Replay, ReplayPriority, Preempt and
+// PreemptWalk refuse to run.
+func (e *Engine) SetInterPodAffinityFilter(on bool) error {
+	v := C.int(0)
+	if on {
+		v = 1
+	}
+	return e.rc(C.bs_set_interpod_filter(e.h, v))
+}
+
+// UploadNodeInterPodFilter / UploadPodInterPodFilter: the filter's sides in C-malloc'd (or pinned) columns.  The node
+// side has the layout of the InterPodAffinity node side, own = 1 for a bound pod's required anti-affinity terms.
+// UploadNodes / UpdateNodes drop the node side and UploadPods the pod side.
+func (e *Engine) UploadNodeInterPodFilter(t *C.bs_interpod_nodes) error {
+	return e.rc(C.bs_upload_node_interpod_filter(e.h, t))
+}
+func (e *Engine) UploadPodInterPodFilter(t *C.bs_interpod_filter_pods) error {
+	return e.rc(C.bs_upload_pod_interpod_filter(e.h, t))
+}
+
+// FetchInterPodReasonRows: the companion of FetchReasonRows, counts[n][3] (E, A, N) of the nodes that pass every
+// other check and fail the filter.
+func (e *Engine) FetchInterPodReasonRows(pod0, n uint32, counts []uint32) error {
+	if uint64(len(counts)) < uint64(n)*3 {
+		return fmt.Errorf("bsched: counts needs n*3 entries")
+	}
+	var p *C.uint32_t
+	if n > 0 {
+		p = (*C.uint32_t)(unsafe.Pointer(&counts[0]))
+	}
+	return e.rc(C.bs_fetch_interpod_reason_rows(e.h, C.uint32_t(pod0), C.uint32_t(n), p))
+}
+
 // UploadNodeNonZero / UploadPodNonZero: the non-zero request columns, nz[2][n] (cpu millicores, then memory bytes):
 // per pod the sum over its containers of GetNonzeroRequestForResource(Requests), per node NodeInfo.NonZeroRequest().
 // UploadNodes / UpdateNodes drop the node column and UploadPods the pod column: upload them again before Evaluate.
@@ -401,9 +445,22 @@ func (e *Engine) Reasons(pod0, n int) ([]uint32, error) {
 // FitError formats one reason row (4 + lanes counters) as kube-scheduler's FailedScheduling message,
 // "0/<nNodes> nodes are available: ...", naming lanes 4.. by scalarNames (nil: "lane<d>").  Needs no engine.
 func FitError(counts []uint32, nNodes int, scalarNames []string) (string, error) {
+	return FitErrorInterPod(counts, nil, nNodes, scalarNames)
+}
+
+// FitErrorInterPod is FitError with the row's MatchInterPodAffinity companion (E, A, N from FetchInterPodReasonRows)
+// as further entries (bs_format_fit_error_interpod); a nil interPod is FitError.
+func FitErrorInterPod(counts, interPod []uint32, nNodes int, scalarNames []string) (string, error) {
 	lanes := len(counts) - 4
 	if lanes < C.BS_FIXED_LANES {
 		return "", fmt.Errorf("bs_format_fit_error: a reason row has 4 + lanes bins")
+	}
+	var ip *C.uint32_t
+	if interPod != nil {
+		if len(interPod) != 3 {
+			return "", fmt.Errorf("bs_format_fit_error_interpod: a companion row has 3 counters")
+		}
+		ip = (*C.uint32_t)(unsafe.Pointer(&interPod[0]))
 	}
 	var names **C.char
 	if len(scalarNames) > 0 {
@@ -418,8 +475,8 @@ func FitError(counts []uint32, nNodes int, scalarNames []string) (string, error)
 	}
 	for size := 512; size <= 1<<20; size *= 4 {
 		buf := (*C.char)(C.malloc(C.size_t(size)))
-		rc := C.bs_format_fit_error((*C.uint32_t)(unsafe.Pointer(&counts[0])), C.uint32_t(lanes), C.uint32_t(nNodes),
-			names, buf, C.size_t(size))
+		rc := C.bs_format_fit_error_interpod((*C.uint32_t)(unsafe.Pointer(&counts[0])), C.uint32_t(lanes), ip,
+			C.uint32_t(nNodes), names, buf, C.size_t(size))
 		msg := C.GoString(buf)
 		C.free(unsafe.Pointer(buf))
 		if rc == 0 {
