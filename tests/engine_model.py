@@ -1,12 +1,15 @@
 """TEST INFRASTRUCTURE — a host model of one long-lived engine's logical state, and a seeded generator of call sequences.
 
-Model.apply(op) follows one call: it updates the tables, side columns and weights the engine keeps between calls and
-returns the error code the engine must answer (None for success).  The drop rules and check orders are
+Model.apply(op) follows one call: it updates the tables, side columns, filter halves and weights the engine keeps
+between calls and returns the error code the engine must answer (None for success).  The drop rules and check orders are
 include/bsched.h's; Model.expect(cfg) gives every output of a round on the current state from the existing CPU
 restatements only (the oracle, the reason rows, the priority lists, the lane classifier, the walks and preemption).
 
-generate(seed) is a list of ops: random uploads, row updates, side columns, weights, failing calls and rounds, plus
-the scripted bursts R1-R6 (every seed runs at least one; across seeds all of them):
+generate(seed) is a list of ops: random uploads, row updates, side columns, weights, failing calls and rounds, the
+MatchInterPodAffinity filter's switch and halves (both built with one seed, so that they describe one cluster),
+bound-pod tables with PodDisruptionBudget bits, preemption and preemption walks (now and then with a list that breaks
+one of bs_preempt_walk's rules), plus the scripted bursts R1-R9 (every seed runs at least one; across seeds all of
+them):
   R1  more than 4096 fit and representative classes, then a table with few (both persistent class indices clear),
       then bs_update_groups with a new representative class, then a round;
   R2  node tables of 0, 1, 511, 512, 513 and more nodes, growing and shrinking, every side uploaded again after each;
@@ -15,7 +18,13 @@ the scripted bursts R1-R6 (every seed runs at least one; across seeds all of the
   R4  each side dropped by the call that owns it: BS_E_STATE with its weight on, the lists without the term with it
       off, and the term back once the side is uploaded again;
   R5  a failing upload of each table kind, then a round;
-  R6  every list output at N = 0 and at P = 0 with every term on.
+  R6  every list output at N = 0 and at P = 0 with every term on;
+  R7  the filter's lifecycle: the switch without halves, each half dropped by bs_update_nodes, a node table of another
+      size and a pod table refused for its lane count and uploaded again, a failing pod half, the four refusals;
+  R8  more than 4096 fit classes under the filter, pod halves in new filter classes until the fit class index is
+      compacted, the switch toggled, a group row update and an affinity table in between, then a small pod table;
+  R9  preemption with budget bits and walks after a group row update, a node row update and a group upload, and one
+      walk per broken list rule.
 """
 from __future__ import annotations
 
@@ -23,9 +32,11 @@ import numpy as np
 
 import fit_reasons_ref as frr
 import fit_shape_cases as fsc
+import interpod_filter_ref as fr
 import interpod_priority_ref as ir
 import locality_priority_ref as lpr
-import preempt_ref
+import preempt_pdb_ref
+import preempt_walk_ref as pwr
 import ratio_priority_ref as rr
 from oracle import oracle
 from randsnap import S, random_snapshot
@@ -96,6 +107,9 @@ class Model:
         self.weights = (1, 0, 1)
         self.ratio = ir.NO_RATIO
         self.pw, self.lw, self.w_spread, self.w_ipa = (0, 0), (0, 0), 0, 0
+        # the MatchInterPodAffinity filter: the switch, its two halves (node: the node side's columns, pod: (pod_class,
+        # class table)), and whether the last successful round ran with the switch on (else its companion rows are 0)
+        self.ipf_on, self.ipf_node, self.ipf_pod, self.ipf_round = False, None, None, False
 
     # ---- state ---------------------------------------------------------------------------------------------------
     def snapshot(self):
@@ -119,6 +133,7 @@ class Model:
     def _upload_nodes(self, op):
         nt = op["table"]
         self._drop(NODE_SIDES)
+        self.ipf_node = None
         self.bound, self.aff = None, None   # they belong to the snapshot, also to one that fails validation
         if _out_of_range(nt.alloc, nt.requested):
             self.nodes = None
@@ -131,6 +146,7 @@ class Model:
         if self.nodes is None:
             return E_STATE
         self._drop(NODE_SIDES)   # every call, also one that changes no row or fails (bsched.h bs_update_nodes)
+        self.ipf_node = None
         if len(idx) == 0:
             return None
         if (np.asarray(idx) >= self.nodes.n).any():
@@ -167,6 +183,9 @@ class Model:
     def _upload_pods(self, op):
         pt = op["table"]
         self._drop(POD_SIDES)
+        self.ipf_pod = None      # also by a call refused for its lane count, which keeps the pod table of now
+        if pt.lanes != self.lanes:
+            return E_INVAL
         if _out_of_range(pt.req):
             self.pods = None
             return E_RANGE
@@ -198,6 +217,26 @@ class Model:
         self.side[key] = op["cols"]
         return None
 
+    def _ipf(self, op):
+        """One half of the filter's columns: half (node / pod), cols, n (its length)."""
+        key = "ipf_" + op["half"]
+        setattr(self, key, None)   # a failing call leaves the half dropped
+        table = self.nodes if op["half"] == "node" else self.pods
+        if table is None:
+            return E_STATE
+        if op["n"] != table.n:
+            return E_INVAL
+        if op["half"] == "pod" and _max_class(op["cols"][0], S.IPF_NONE) >= len(op["cols"][1][0]) - 1:
+            return E_INDEX
+        if op["half"] == "node" and (np.asarray(op["cols"][3], np.int64) >= table.n).any():
+            return E_INDEX     # a bound pod on a node the table lacks
+        setattr(self, key, op["cols"])
+        return None
+
+    def _ipf_switch(self, op):
+        self.ipf_on = bool(op["on"])
+        return None
+
     def _weights(self, op):
         for k, v in op.items():
             if k != "op":
@@ -205,8 +244,14 @@ class Model:
         return None
 
     def _evaluate(self, op):
+        rc = self._evaluate_check(op)
+        if rc is None:
+            self.ipf_round = self.ipf_on
+        return rc
+
+    def _evaluate_check(self, op):
         """The engine's check order: the tables, then (priority lists only) the non-zero columns, the node
-        priorities, locality, spread and inter-pod, then the affinity class ids."""
+        priorities, locality, spread and inter-pod, then the filter's halves and terms, then the affinity class ids."""
         if not self.complete():
             return E_STATE
         if op["priority"]:
@@ -231,6 +276,11 @@ class Model:
                     return E_STATE
                 if _max_class(sd["ipa_pod"][1][1], -1) >= len(sd["ipa_node"][2]):
                     return E_INDEX
+        if self.ipf_on:
+            if self.ipf_node is None or self.ipf_pod is None:
+                return E_STATE
+            if _max_class(self.ipf_pod[1][1], -1) >= len(self.ipf_node[2]):   # any class's term, used or not
+                return E_INDEX
         return self._affinity_check()
 
     def _locality_check(self):
@@ -253,6 +303,8 @@ class Model:
         return None
 
     def _replay(self, op):
+        if self.ipf_on:
+            return E_INVAL     # refused while the filter is on, before anything else
         if op["priority"] and (any(self.pw) or self.w_spread or self.w_ipa):
             return E_INVAL     # bs_replay_priority refuses these weights before anything else
         if not self.complete():
@@ -266,16 +318,50 @@ class Model:
         return self._affinity_check()
 
     def _preempt(self, op):
+        """bs_preempt's checks (preempt_pods in engine.cu): the switch, the tables, then each listed pod's index and
+        affinity class."""
+        if self.ipf_on:
+            return E_INVAL
         if not self.complete() or self.bound is None:
             return E_STATE
+        pods = np.asarray(op["pods"], np.int64)
+        if (pods >= self.pods.n).any():
+            return E_INDEX
         n_aff = 0 if self.aff is None else len(self.aff)
-        if self.pods.aff_class is not None and _max_class(self.pods.aff_class, S.AFF_NONE) >= n_aff:
+        if self.pods.aff_class is not None and _max_class(self.pods.aff_class[pods], S.AFF_NONE) >= n_aff:
             return E_INDEX
         return None
 
+    def _preempt_walk(self, op):
+        """bs_preempt's checks, then the list rules in the engine's order (include/bsched.h bs_preempt_walk): per list
+        position, a priority above the one before, a pod listed twice, and with gang a group (0 <= gid < n_groups)
+        whose run started before and was closed."""
+        rc = self._preempt(op)
+        if rc:
+            return rc
+        pods = np.asarray(op["pods"], np.int64)
+        prio, gid, G = self.pods.priority[pods], self.pods.gid[pods], self.groups.n
+        seen, closed = set(), set()
+        for i, p in enumerate(pods.tolist()):
+            if i and prio[i] > prio[i - 1]:
+                return E_INVAL
+            if p in seen:
+                return E_INVAL
+            seen.add(p)
+            if not op["gang"] or not 0 <= gid[i] < G or (i and gid[i - 1] == gid[i]):
+                continue
+            if gid[i] in closed:
+                return E_INVAL
+            closed.add(gid[i])
+        # the generator stays under the walk's BS_E_RANGE bound: every value is within +-LIMIT, so the live sums are
+        # at most (4 + n) * LIMIT plus the pod counts
+        pc = max([int(t.pod_count.max()) for t in self.history + [self.nodes] if t.n] + [0])
+        assert (4 + len(pods)) * LIMIT + pc + len(pods) <= 1 << 62, "a walk the engine refuses with BS_E_RANGE"
+        return None
+
     # ---- what a round gives ----------------------------------------------------------------------------------------
-    def priority_rows(self, K, pods=None):
-        sd, snap = self.side, self.snapshot()
+    def priority_rows(self, K, pods=None, snap=None):
+        sd, snap = self.side, snap or self.snapshot()
         N, P = self.nodes.n, self.pods.n
         zero = (([1], [np.zeros(N)], [0], [], [], ([0], [], [], [])), (np.full(P, S.IPA_NONE), ([0], [], [], [])))
         interpod = (sd["ipa_node"], sd["ipa_pod"]) if self.w_ipa else zero
@@ -291,8 +377,21 @@ class Model:
 
     def expect(self, cfg):
         """Every output of a round on this state for an engine built with cfg (score, fit_bitmap, filter, reasons,
-        topk, priority_k): a dict of arrays, keyed as the GPU test reads them back."""
+        topk, priority_k): a dict of arrays, keyed as the GPU test reads them back.  With the filter on, the round is
+        interpod_filter_ref.expected_round's; interpod_rows (with reasons) are the companion rows, zero when the last
+        round ran with the filter off."""
         snap = self.snapshot()
+        if self.ipf_round:
+            def lists(fsnap, score):
+                out = {}
+                if cfg.get("topk"):
+                    out["topk_nodes"], out["topk_scores"] = expected_topk(score, cfg["topk"])
+                if cfg.get("priority_k"):
+                    out["priority_nodes"], out["priority_scores"] = self.priority_rows(cfg["priority_k"], snap=fsnap)
+                return out
+            out, _ = fr.expected_round(snap, (self.ipf_node, self.ipf_pod), cfg, lists)
+            out["lanes"] = fsc.classify(self.nodes, self.pods, self.history)
+            return out
         orc = oracle.round(snap, want_bitmap=True, want_score=True, want_filter=cfg.get("filter", False))
         out = {f: getattr(orc, f) for f in ("prefilter", "feasible_count", "best_node", "best_score", "admit",
                                              "admit_bitmap", "new_denied", "order", "rank")}
@@ -307,6 +406,7 @@ class Model:
             out["topk_nodes"], out["topk_scores"] = expected_topk(orc.score, cfg["topk"])
         if cfg.get("reasons"):
             out["reason_rows"] = frr.fit_reasons(snap)
+            out["interpod_rows"] = np.zeros((self.pods.n, 3), np.uint32)
         if cfg.get("priority_k"):
             out["priority_nodes"], out["priority_scores"] = self.priority_rows(cfg["priority_k"])
         out["lanes"] = fsc.classify(self.nodes, self.pods, self.history)
@@ -328,9 +428,13 @@ class Model:
         return {"prefilter": pf, "node": node, "ready": ready}
 
     def expect_preempt(self, pods):
-        r = preempt_ref.preempt(self.snapshot(), self.bound, pods)
-        return {"node": r.node, "n_victims": r.n_victims, "n_candidates": r.n_candidates,
-                "victims": np.concatenate([r.victims_of(i) for i in range(len(pods))] + [np.zeros(0, np.uint32)])}
+        r = preempt_pdb_ref.preempt(self.snapshot(), self.bound, pods)
+        return {"node": r.node, "n_victims": r.n_victims, "n_candidates": r.n_candidates, "victims": r.victims}
+
+    def expect_preempt_walk(self, pods, gang):
+        r = pwr.walk(self.snapshot(), self.bound, pods, gang)
+        return {"node": r.node, "n_victims": r.n_victims, "n_candidates": r.n_candidates, "victims": r.victims,
+                "outcome": r.outcome, "evicted_by": r.evicted_by}
 
 
 # ---- the generator -----------------------------------------------------------------------------------------------
@@ -362,6 +466,7 @@ class Generator:
         self.ops = []
         self.regimes = set()
         self.max_p = 0
+        self.ipf_seed = seed   # both filter halves are built with it, so that they describe one cluster
 
     def _k(self):
         return int(self.rng.integers(0, 1 << 30))
@@ -472,10 +577,49 @@ class Generator:
         for name in ("nz", "pref", "loc", "spread", "ipa"):
             for half in halves:
                 self.side(name, half)
+        for half in halves:
+            self.ipf(half)
 
     def node_sides(self):
-        """The node halves again, as a caller does after bs_update_nodes dropped them."""
+        """The node halves again (the filter's too), as a caller does after bs_update_nodes dropped them."""
         self.all_sides(("node",))
+
+    def ipf(self, half, mismatch=False, wrong_len=False, bad=False, spread=0):
+        """One half of the filter's columns, built from the state of now with the seed of the pod half (another seed
+        with mismatch); wrong_len: one entry too many; bad: a pod class out of range; spread > 0: the pod half's class
+        table repeated `spread` times and each pod in a random copy of its class (verdicts unchanged, new fit classes)."""
+        m = self.model
+        table = m.nodes if half == "node" else m.pods
+        if table is None:
+            return
+        snap = S.Snapshot(m.nodes if m.nodes is not None else S.NodeTable.empty(0, self.L),
+                          m.pods if m.pods is not None else S.PodTable.empty(0, self.L),
+                          m.groups if m.groups is not None else S.GroupTable.empty(0, self.L))
+        node, pods = S.node_interpod_filter(snap, self._k() if mismatch else self.ipf_seed)
+        if half == "node":
+            nv, topo, tkey, bnode, bcls, bcl = node
+            if not m.nodes.n:   # the generator puts bound pods on node 0 of an empty table: none can be bound
+                bnode, bcls = bnode[:0], bcls[:0]
+            rest = (tkey, bnode, bcls, bcl)
+            if wrong_len:
+                topo = np.concatenate([topo, np.zeros((topo.shape[0], 1), np.uint32)], axis=1)
+            cols, n = (nv, topo, *rest), topo.shape[1]
+        else:
+            pcls, (off, term, role, selfm) = pods
+            C = len(off) - 1
+            if spread and C:
+                pcls = np.where(pcls == S.IPF_NONE, pcls, pcls + C * self.rng.integers(0, spread, len(pcls))).astype(np.uint32)
+                off = np.concatenate([off[:1]] + [off[1:] + k * off[-1] for k in range(spread)]).astype(np.uint32)
+                term, role, selfm = np.tile(term, spread), np.tile(role, spread), np.tile(selfm, spread)
+            if bad:
+                pcls = np.full(len(pcls), len(off) - 1, np.uint32)
+            if wrong_len:
+                pcls = np.r_[pcls, np.uint32(S.IPF_NONE)].astype(np.uint32)
+            cols, n = (pcls, (off, term, role, selfm)), len(pcls)
+        self.emit({"op": "ipf", "half": half, "n": n, "cols": cols})
+
+    def switch(self, on):
+        self.emit({"op": "ipf_switch", "on": on})
 
     def weights(self, on):
         L = self.L
@@ -490,12 +634,61 @@ class Generator:
 
     def walk(self, kind):
         if kind == "preempt":
-            if self.model.complete() and self.model.nodes is not None and self.model.groups is not None:
-                self.emit({"op": "upload_bound", "table": S.bound_pods(self.model.snapshot(), self._k(), max_per_node=6)})
+            if self.model.complete():
+                self.bound()
             self.emit({"op": "preempt", "pods": np.arange(min(self.model.pods.n if self.model.pods is not None else 0, 40),
                                                          dtype=np.uint32)})
         else:
             self.emit({"op": "replay", "priority": kind == "priority"})
+
+    def bound(self):
+        """A bound-pod table of the snapshot of now; none, some or all of its pods violate a PodDisruptionBudget."""
+        v = float(self.rng.choice([0.0, 0.3, 1.0]))
+        self.emit({"op": "upload_bound", "table": S.bound_pods(self.model.snapshot(), self._k(), max_per_node=6,
+                                                               violating=v)})
+
+    def walk_list(self, gang, n=24):
+        """Up to n pods in queue order (priority descending, then group, then index); with gang, a group whose members
+        the priorities split keeps its first run only, so that the list keeps bs_preempt_walk's rules."""
+        pt, G = self.model.pods, self.model.groups.n
+        pick = np.sort(self.rng.choice(pt.n, min(n, pt.n), replace=False)) if pt.n else np.zeros(0, np.int64)
+        pick = pick[np.lexsort((pick, pt.gid[pick], -pt.priority[pick].astype(np.int64)))]
+        keep, closed = [], set()
+        for p in pick.tolist():
+            g = int(pt.gid[p])
+            if gang and 0 <= g < G:
+                if keep and int(pt.gid[keep[-1]]) == g:
+                    keep.append(p)
+                    continue
+                if g in closed:
+                    continue
+                closed.add(g)
+            keep.append(p)
+        return np.array(keep, np.uint32)
+
+    def broken_list(self, rule, gang):
+        """A walk list that breaks one rule: "rising" (a priority above the one before), "twice" (a pod listed twice)
+        or "split" (under gang, a group's preemptors around another pod of their priority)."""
+        pt, G = self.model.pods, self.model.groups.n
+        pods = self.walk_list(gang)
+        if rule == "rising":
+            d = np.flatnonzero(pt.priority[pods[:-1]] != pt.priority[pods[1:]])
+            if len(d):
+                i = int(d[0])
+                pods[i], pods[i + 1] = pods[i + 1], pods[i]
+                return pods
+        if rule == "split":
+            for g in range(G):
+                for q in np.unique(pt.priority[pt.gid == g]):
+                    mine = np.flatnonzero((pt.gid == g) & (pt.priority == q))
+                    other = np.flatnonzero((pt.gid != g) & (pt.priority == q))
+                    if len(mine) >= 2 and len(other):
+                        return np.array([mine[0], other[0], mine[1]], np.uint32)
+        return np.insert(pods, 1, pods[0]) if len(pods) else np.zeros(2, np.uint32)
+
+    def preempt_walk(self, gang, rule=None):
+        pods = self.walk_list(gang) if rule is None else self.broken_list(rule, gang)
+        self.emit({"op": "preempt_walk", "pods": pods, "gang": gang, "rule": rule})
 
     def base(self, P=150, N=300, G=20):
         self.upload_nodes(N)
@@ -595,12 +788,16 @@ class Generator:
         return {"pref": {"pw": (0, 0)}, "loc": {"lw": (0, 0)}, "spread": {"w_spread": 0}, "ipa": {"w_ipa": 0}}[name]
 
     def all_sides_but(self, skip):
+        """Every missing side but `skip` (a side's name, or "ipf": the filter's halves)."""
         for name in ("nz", "pref", "loc", "spread", "ipa"):
             if name == skip:
                 continue
             for half in ("node", "pod"):
                 if self.model.side[name + "_" + half] is None:
                     self.side(name, half)
+        for half in ("node", "pod"):
+            if skip != "ipf" and getattr(self.model, "ipf_" + half) is None:
+                self.ipf(half)
 
     def r5(self):
         self.base()
@@ -649,40 +846,164 @@ class Generator:
         self.round()
         self.regimes.add("R6")
 
+    def r7(self):
+        """The filter's lifecycle: each half dropped by the call that owns it and uploaded again, a node table of
+        another size, a pod table refused for its lane count, a failing pod half, and the four refusals."""
+        self.upload_nodes(300)
+        self.upload_groups(20)
+        self.upload_pods(150)
+        self.all_sides_but("ipf")
+        self.weights(on=True)
+        self.switch(True)
+        self.round()                 # BS_E_STATE: no halves
+        self.ipf("node")
+        self.ipf("pod")
+        self.round()
+        self.update_nodes(str(self.rng.choice(["widen", "flags", "labels"])))
+        self.all_sides_but("ipf")
+        self.round()                 # BS_E_STATE: the node half went with the update
+        self.ipf("node")
+        self.round()
+        self.upload_nodes(int(self.rng.choice([513, 700])))   # another Npad for the pass planes
+        self.all_sides()
+        self.round()
+        lanes = random_snapshot(self._k(), P=40, N=1, G=1, L=self.L + 1).pods
+        self.emit({"op": "upload_pods", "table": lanes})   # BS_E_INVAL: the pod table stays, its sides go
+        self.all_sides_but("ipf")
+        self.round()                 # BS_E_STATE: the pod half went with the refused call
+        self.ipf("pod")
+        self.round()
+        self.ipf("pod", bad=True)    # BS_E_INDEX
+        self.round()                 # BS_E_STATE
+        self.ipf("pod")
+        self.round()
+        self.bound()
+        for kind in ("first_fit", "priority"):
+            self.emit({"op": "replay", "priority": kind == "priority"})   # BS_E_INVAL while the filter is on
+        self.emit({"op": "preempt", "pods": np.arange(min(self.model.pods.n, 40), dtype=np.uint32)})
+        self.preempt_walk(False)
+        self.switch(False)
+        self.emit({"op": "replay", "priority": False})
+        self.emit({"op": "preempt", "pods": np.arange(min(self.model.pods.n, 40), dtype=np.uint32)})
+        self.preempt_walk(True)
+        self.switch(True)
+        self.round()
+        self.regimes.add("R7")
+
+    def r8(self):
+        """More than 4096 fit classes under the filter, and pod halves that put the pods in new filter classes at
+        every round until compact_fit_index rebuilds the fit index, with the switch toggled, a group row update and a
+        new affinity table in between; then a small pod table with the switch off and on."""
+        self.upload_nodes(64)
+        self.upload_groups(40)
+        pt = self.snap(R8_PODS, 1, 40).pods
+        pt.tol_mask = self.rng.integers(0, 1 << 62, pt.n).astype(np.uint64)   # a fit class per pod
+        self.emit({"op": "upload_pods", "table": pt})
+        self.all_sides()
+        self.switch(True)
+        self.round("evaluate")
+        for k in range(R8_ROUNDS):
+            self.ipf("pod", spread=R8_SPREAD)
+            if k % 4 == 1:
+                self.switch(False)
+                self.round()
+                self.switch(True)
+            if k == R8_ROUNDS // 2:
+                self.update_groups("rep")
+                self.emit({"op": "upload_affinity", "bits": self.snap(1, 64, 1, aff=AFF).aff_bits})
+            self.round()
+        self.upload_pods(50)
+        self.all_sides()
+        self.switch(False)
+        self.round()
+        self.switch(True)
+        self.round()
+        self.regimes.add("R8")
+
+    def r9(self):
+        """Preemption with PodDisruptionBudget bits and the walk: after a group row update (the bound table stays),
+        after a node row update and after a group upload (both drop it), and one walk per broken list rule."""
+        self.switch(False)
+        self.base()
+        self.bound()
+        self.walk("preempt")
+        self.preempt_walk(False)
+        self.preempt_walk(True)
+        self.update_groups("creation")
+        self.emit({"op": "preempt", "pods": np.arange(min(self.model.pods.n, 40), dtype=np.uint32)})
+        self.update_nodes(str(self.rng.choice(["widen", "flags", "labels"])))
+        self.preempt_walk(False)     # BS_E_STATE: the update dropped the bound table
+        self.bound()
+        self.preempt_walk(bool(self.rng.random() < 0.5))
+        self.upload_groups(self.model.groups.n)
+        self.preempt_walk(True, "split")   # BS_E_STATE: the state checks come before the list rules
+        self.bound()
+        for rule, gang in (("rising", False), ("twice", False), ("split", True)):
+            self.preempt_walk(gang, rule)
+        self.preempt_walk(True)
+        self.regimes.add("R9")
+
     # -- random ops --
+    def filter_or_preempt_op(self):
+        m = self.model
+        r = self.rng.random()
+        if r < 0.25:
+            self.switch(not m.ipf_on)
+            self.round()
+        elif r < 0.5:
+            if self.rng.random() < 0.3:
+                self.ipf_seed = self._k()   # new halves: the pod half first, then the node half
+                self.ipf("pod")
+                self.ipf("node")
+            else:
+                self.ipf(str(self.rng.choice(["node", "pod"])), wrong_len=self.rng.random() < 0.2,
+                         mismatch=self.rng.random() < 0.1)
+            self.round()
+        elif r < 0.65:
+            self.bound()
+            self.walk("preempt")
+        else:
+            if m.bound is None or self.rng.random() < 0.4:
+                self.bound()
+            gang = bool(self.rng.random() < 0.5)
+            rule = str(self.rng.choice(["rising", "twice", "split"])) if self.rng.random() < 0.2 else None
+            self.preempt_walk(gang, rule)
+
     def random_op(self):
         m = self.model
         r = self.rng.random()
         if m.nodes is None or m.pods is None or m.groups is None:
             self.base()
-        elif r < 0.10:   # without its affinity table now and then: the pods' classes are BS_E_INDEX until it comes
+        elif r < 0.12:
+            self.filter_or_preempt_op()
+        elif r < 0.20:   # without its affinity table now and then: the pods' classes are BS_E_INDEX until it comes
             self.upload_nodes(int(self.rng.choice([1, 33, 511, 512, 513, 900])), aff=AFF if self.rng.random() < 0.85 else 0)
             self.all_sides(("node",))
-        elif r < 0.18:
+        elif r < 0.27:
             self.upload_pods(int(self.rng.choice([0, 1, 70, self.max_p + 13])), aff=AFF if self.rng.random() < 0.8 else 0)
             self.all_sides(("pod",))
-        elif r < 0.22:
+        elif r < 0.30:
             self.upload_groups(int(self.rng.choice([0, 1, 9, 31])), aff=AFF if self.rng.random() < 0.8 else 0)
-        elif r < 0.34 and m.nodes.n:
+        elif r < 0.41 and m.nodes.n:
             self.update_nodes(str(self.rng.choice(["widen", "back", "flags", "labels"])))
             if self.rng.random() < 0.85:   # else the next rounds answer BS_E_STATE until a side op brings them back
                 self.node_sides()
                 self.round()
-        elif r < 0.42 and m.groups.n:
+        elif r < 0.48 and m.groups.n:
             self.update_groups(str(self.rng.choice(["rep", "creation"])))
             self.round()
-        elif r < 0.50:   # a new table (the nodes' class fits change), or none (the pods' classes are out of range)
+        elif r < 0.55:   # a new table (the nodes' class fits change), or none (the pods' classes are out of range)
             bits = self.snap(1, m.nodes.n, 1, aff=AFF).aff_bits if self.rng.random() < 0.75 else None
             self.emit({"op": "upload_affinity", "bits": bits})
             self.round()
-        elif r < 0.62:
+        elif r < 0.65:
             name = str(self.rng.choice(["nz", "pref", "loc", "spread", "ipa"]))
             half = str(self.rng.choice(["node", "pod"]))
             self.side(name, half, mismatch=self.rng.random() < 0.3, wrong_len=self.rng.random() < 0.1)
-        elif r < 0.70:
+        elif r < 0.72:
             self.weights(on=bool(self.rng.random() < 0.6))
-        elif r < 0.76:
-            kind = str(self.rng.choice(["nodes", "groups", "pods", "index"]))
+        elif r < 0.78:
+            kind = str(self.rng.choice(["nodes", "groups", "pods", "index", "lanes"]))
             if kind == "index" and m.nodes.n:
                 self.emit({"op": "update_nodes", "idx": np.array([m.nodes.n], np.uint32), "rows": m.nodes.take([0])})
             elif kind == "groups":
@@ -694,20 +1015,23 @@ class Generator:
                 bad = m.pods.copy()
                 bad.req[0, 0] = -(LIMIT + 1)
                 self.emit({"op": "upload_pods", "table": bad})
-        elif r < 0.84:
+            elif kind == "lanes":   # refused for its lane count: the pod table stays, its sides go
+                self.emit({"op": "upload_pods", "table": random_snapshot(self._k(), P=20, N=1, G=1, L=self.L + 1).pods})
+        elif r < 0.85:
             self.walk(str(self.rng.choice(["first_fit", "priority", "preempt"])))
         else:
             self.round()
 
 
-BURSTS = ("r1", "r2", "r3", "r4", "r5", "r6")
+BURSTS = ("r1", "r2", "r3", "r4", "r5", "r6", "r7", "r8", "r9")
+R8_PODS, R8_ROUNDS, R8_SPREAD = 4200, 9, 64
 
 
 def generate(seed, n_ops=30, lanes=None):
-    """(ops, regimes): about n_ops random ops around one scripted burst (seed % 6 picks it; seeds >= 6 add another),
+    """(ops, regimes): about n_ops random ops around one scripted burst (seed % 9 picks it; seeds >= 6 add another),
     every op as the dict Model.apply takes; regimes names the bursts the sequence ran."""
     g = Generator(seed, lanes or [5, 6, 9][seed % 3])
-    bursts = [BURSTS[seed % 6]] + ([BURSTS[(seed // 6 + seed) % 6]] if seed >= 6 else [])
+    bursts = [BURSTS[seed % 9]] + ([BURSTS[(seed + 4) % 9]] if seed >= 6 else [])
     at = sorted(int(x) for x in g.rng.integers(0, n_ops, len(bursts)))
     g.base()
     for i in range(n_ops):

@@ -1,13 +1,16 @@
 """CPU: the host model of a long-lived engine (tests/engine_model.py) and its op generator, without a device: row
 updates through the model equal the tables built directly, the generator is deterministic and reaches every scripted
 regime across the seeds the GPU test runs, and the model's expected outputs come from the restatements on a short
-sequence (which keeps the reference side honest and bounds its cost)."""
+sequence (which keeps the reference side honest and bounds its cost).  The MatchInterPodAffinity filter's drop rules,
+check order and refusals, the preemption walk's list rules, and the invariants of a round under the filter are pinned
+on hand-built op lists."""
 import numpy as np
 
 import engine_model as em
+import interpod_filter_ref as fr
 from randsnap import S, random_snapshot
 
-SEEDS = range(8)
+SEEDS = range(9)   # the GPU test's seeds
 
 
 def _same(a, b):
@@ -88,7 +91,7 @@ def test_generator_is_deterministic_and_reaches_every_regime():
         seen |= regimes
         kinds = {o["op"] for o in ops}
         assert {"upload_nodes", "upload_pods", "upload_groups", "side", "weights", "evaluate"} <= kinds
-    assert seen == {"R1", "R2", "R3", "R4", "R5", "R6"}
+    assert seen == {f"R{k}" for k in range(1, 10)}
 
 
 def test_sequences_reach_the_edges():
@@ -180,3 +183,206 @@ def test_r1_updates_a_group_in_place_after_the_indices_cleared():
     last_pods = len(before) - 1 - before[::-1].index("upload_pods")
     assert "evaluate" in before[last_pods:]
     assert g.ops[last_pods]["table"].n < 4096 // 4
+
+
+def _loaded(seed=21, P=60, N=90, G=12, L=5):
+    """A model with every table, the non-zero columns and both filter halves of one cluster; the switch off."""
+    snap = random_snapshot(seed, P=P, N=N, G=G, L=L, aff=2)
+    m = em.Model(L)
+    for op in ({"op": "upload_nodes", "table": snap.nodes}, {"op": "upload_affinity", "bits": snap.aff_bits},
+               {"op": "upload_groups", "table": snap.groups}, {"op": "upload_pods", "table": snap.pods}):
+        assert m.apply(op) is None
+    nz = S.nonzero_requests(snap, 1)
+    for half, cols in (("node", nz[0]), ("pod", nz[1])):
+        assert m.apply({"op": "side", "name": "nz", "half": half, "n": cols.shape[1], "cols": cols}) is None
+    node, pods = S.node_interpod_filter(snap, 3)
+    assert m.apply({"op": "ipf", "half": "node", "n": N, "cols": node}) is None
+    assert m.apply({"op": "ipf", "half": "pod", "n": P, "cols": pods}) is None
+    return m, snap, node, pods
+
+
+def test_filter_drop_rules_and_check_order():
+    m, snap, node, pods = _loaded()
+    ev = {"op": "evaluate", "priority": True}
+    half = lambda h, cols, n=None: {"op": "ipf", "half": h, "cols": cols,
+                                    "n": (snap.nodes.n if h == "node" else snap.pods.n) if n is None else n}
+    assert m.apply(ev) is None and not m.ipf_round
+    assert m.apply({"op": "ipf_switch", "on": True}) is None
+    assert m.apply(ev) is None and m.ipf_round
+    # bs_update_nodes drops the node half, also a call that changes no row or fails
+    for idx, rows in ((np.zeros(0, np.uint32), snap.nodes.take(np.zeros(0, np.int64))), (np.array([snap.nodes.n], np.uint32),
+                                                                      snap.nodes.take([0]))):
+        m.apply({"op": "update_nodes", "idx": idx, "rows": rows})
+        assert m.ipf_node is None and m.ipf_pod is not None
+        assert m.apply(half("node", node)) is None
+    assert m.apply({"op": "update_nodes", "idx": np.array([1], np.uint32), "rows": snap.nodes.take([1])}) is None
+    assert m.apply({"op": "side", "name": "nz", "half": "node", "n": snap.nodes.n,
+                    "cols": S.nonzero_requests(snap, 1)[0]}) is None
+    assert m.apply(ev) == em.E_STATE            # the filter's half, after the priority sides are back
+    assert m.apply(half("node", node)) is None
+    assert m.apply(ev) is None
+    # bs_upload_nodes drops it, also one that fails validation
+    bad = snap.nodes.copy()
+    bad.alloc[0, 0] = em.LIMIT + 1
+    assert m.apply({"op": "upload_nodes", "table": bad}) == em.E_RANGE
+    assert m.ipf_node is None
+    assert m.apply(half("node", node)) == em.E_STATE    # without its table
+    assert m.apply({"op": "upload_nodes", "table": snap.nodes}) is None
+    assert m.apply({"op": "upload_affinity", "bits": snap.aff_bits}) is None
+    assert m.apply({"op": "side", "name": "nz", "half": "node", "n": snap.nodes.n,
+                    "cols": S.nonzero_requests(snap, 1)[0]}) is None
+    wide = (node[0], np.concatenate([node[1], node[1][:, :1]], axis=1), *node[2:])
+    assert m.apply(half("node", wide, snap.nodes.n + 1)) == em.E_INVAL and m.ipf_node is None
+    off_table = (*node[:3], np.r_[node[3][:-1], np.uint32(snap.nodes.n)], *node[4:])
+    assert m.apply(half("node", off_table)) == em.E_INDEX and m.ipf_node is None   # a bound pod on no node
+    assert m.apply(half("node", node)) is None
+    # bs_upload_pods drops the pod half, also a call refused for its lane count (which keeps the pod table)
+    other = random_snapshot(5, P=7, N=1, G=1, L=6).pods
+    assert m.apply({"op": "upload_pods", "table": other}) == em.E_INVAL
+    assert m.pods is snap.pods and m.ipf_pod is None and m.side["nz_pod"] is None
+    assert m.apply({"op": "side", "name": "nz", "half": "pod", "n": snap.pods.n,
+                    "cols": S.nonzero_requests(snap, 1)[1]}) is None
+    assert m.apply(ev) == em.E_STATE
+    # a failing half leaves it dropped: a pod class out of range is BS_E_INDEX, a wrong length BS_E_INVAL
+    pcls, cl = pods
+    assert m.apply(half("pod", (np.full(len(pcls), len(cl[0]) - 1, np.uint32), cl))) == em.E_INDEX
+    assert m.apply(half("pod", (pcls[:-1], cl), snap.pods.n - 1)) == em.E_INVAL
+    assert m.ipf_pod is None and m.apply(ev) == em.E_STATE
+    # a term outside the node half's dictionary is BS_E_INDEX at evaluation, after the priority sides' checks
+    far = (pcls, (cl[0], np.full_like(cl[1], len(node[2])), cl[2], cl[3]))
+    assert m.apply(half("pod", far)) is None
+    assert m.apply(ev) == em.E_INDEX
+    assert m.apply({"op": "weights", "w_spread": 1}) is None
+    assert m.apply(ev) == em.E_STATE            # the spread sides are checked first
+    assert m.apply({"op": "weights", "w_spread": 0}) is None
+    assert m.apply(half("pod", pods)) is None
+    assert m.apply(ev) is None
+    # ... and before the affinity ids
+    assert m.apply({"op": "upload_affinity", "bits": None}) is None
+    assert m.apply({"op": "ipf", "half": "pod", "n": snap.pods.n, "cols": far}) is None
+    assert m.apply(ev) == em.E_INDEX
+    assert m.apply(half("pod", pods)) is None
+    assert m.apply(ev) == em.E_INDEX            # now the affinity ids
+    assert m.apply({"op": "ipf_switch", "on": False}) is None
+    assert m.apply(ev) == em.E_INDEX and m.ipf_round
+
+
+def test_refusals_and_walk_rules():
+    m, snap, node, pods = _loaded()
+    pt = snap.pods
+    walk = lambda p, gang=False: {"op": "preempt_walk", "pods": np.asarray(p, np.uint32), "gang": gang}
+    refusals = ({"op": "replay", "priority": False}, {"op": "replay", "priority": True},
+                {"op": "preempt", "pods": np.arange(5, dtype=np.uint32)}, walk([0]))
+    assert m.apply({"op": "ipf_switch", "on": True}) is None
+    for op in refusals:   # before every other check: there is no bound table yet, and a broken list
+        assert m.apply(op) == em.E_INVAL
+    assert m.apply(walk([0, 0])) == em.E_INVAL
+    assert m.apply({"op": "ipf_switch", "on": False}) is None
+    assert m.apply(refusals[0]) is None
+    assert m.apply(refusals[2]) == em.E_STATE and m.apply(refusals[3]) == em.E_STATE
+    assert m.apply(walk([0, 0])) == em.E_STATE   # the state checks come before the list rules
+    assert m.apply({"op": "upload_bound", "table": S.bound_pods(snap, 2, max_per_node=4, violating=0.3)}) is None
+    assert m.apply(walk([pt.n])) == em.E_INDEX
+    order = np.lexsort((np.arange(pt.n), pt.gid, -pt.priority.astype(np.int64)))
+    assert m.apply(walk(order[:20])) is None
+    assert m.apply(walk(order[:20][::-1])) == em.E_INVAL                         # rising priorities
+    assert m.apply(walk(np.r_[order[:5], order[4]])) == em.E_INVAL               # a pod twice
+    # a group split around another pod of its priority: a rule under gang only; gids >= n_groups are units of one
+    g, q = next((g, q) for g in range(snap.groups.n) for q in np.unique(pt.priority[pt.gid == g])
+                if ((pt.gid == g) & (pt.priority == q)).sum() >= 2 and ((pt.gid != g) & (pt.priority == q)).any())
+    a, b = np.flatnonzero((pt.gid == g) & (pt.priority == q))[:2]
+    h = np.flatnonzero((pt.gid != g) & (pt.priority == q))[0]
+    assert m.apply(walk([a, h, b])) is None
+    assert m.apply(walk([a, h, b], gang=True)) == em.E_INVAL
+    far = pt.copy()
+    far.gid[[a, b]] = snap.groups.n + 3
+    far.gid[h] = snap.groups.n + 4
+    assert m.apply({"op": "upload_pods", "table": far}) is None
+    assert m.apply({"op": "upload_bound", "table": S.bound_pods(snap, 2, max_per_node=4)}) is None
+    assert m.apply(walk([a, h, b], gang=True)) is None
+    # the bound table stays through bs_update_groups and goes with bs_update_nodes and bs_upload_groups
+    assert m.apply({"op": "update_groups", "idx": np.array([0], np.uint32), "rows": snap.groups.take([0])}) is None
+    assert m.bound is not None
+    assert m.apply({"op": "upload_groups", "table": snap.groups}) is None and m.bound is None
+
+
+def _fit_keys(pt):
+    """Each pod's fit class key without the filter (engine.cu bs_upload_pods): (sel, tol, scalar keys requested with a
+    non-zero amount, affinity class)."""
+    nz = np.zeros(pt.n, np.uint64)
+    for d in range(4, pt.lanes):
+        nz |= ((((pt.req_present >> np.uint32(d)) & 1) == 1) & (pt.req[d] != 0)).astype(np.uint64) << np.uint64(d)
+    aff = pt.aff_class if pt.aff_class is not None else np.full(pt.n, S.AFF_NONE, np.uint32)
+    return list(zip(pt.sel_mask.tolist(), pt.tol_mask.tolist(), nz.tolist(), aff.tolist()))
+
+
+def test_filter_rounds_follow_every_change():
+    """Across the seeds, rounds with the filter on succeed right after a node table of another size, a node row
+    update, a pod table refused for its lane count and a compaction of the fit class index; walks and preemption with
+    PodDisruptionBudget bits succeed after row updates.  The compaction is certain once the (fit class, filter class)
+    keys assigned since the last pod table outnumber max(4096, 4 x 2P), since the index only grows until it is
+    compacted and a compaction keeps at most 2P classes (each pod's class and its class without the filter)."""
+    reached, walks, pdb = set(), 0, 0
+    for seed in SEEDS:
+        ops, _, L = em.generate(seed)
+        m = em.Model(L)
+        pending, keys, n_prev, updated = set(), set(), None, False
+        for op in ops:
+            rc = m.apply(op)
+            k = op["op"]
+            if k == "upload_nodes" and rc is None:
+                if n_prev is not None and op["table"].n != n_prev:
+                    pending.add("resize")
+                n_prev = op["table"].n
+            elif k == "update_nodes" and rc is None and len(op["idx"]):
+                pending.add("update_nodes")
+                updated = True
+            elif k == "update_groups" and rc is None:
+                updated = True
+            elif k == "upload_pods":
+                if rc == em.E_INVAL:
+                    pending.add("refused pods")
+                elif rc is None:
+                    keys = set()
+            elif k == "evaluate" and rc is None and m.ipf_on:
+                base = _fit_keys(m.pods)
+                keys |= set(zip(base, m.ipf_pod[0].tolist()))
+                if len(keys) > max(4096, 8 * m.pods.n):
+                    pending.add("compaction")
+                    keys = set()
+                reached |= pending
+                pending = set()
+            elif k == "preempt_walk" and rc is None and updated and len(op["pods"]):
+                walks += 1
+            elif k == "preempt" and rc is None and updated and (m.bound.flags & S.BOUND_PDB_VIOLATING).any():
+                pdb += 1
+    assert reached == {"resize", "update_nodes", "refused pods", "compaction"}, reached
+    assert walks >= 1 and pdb >= 1, (walks, pdb)
+
+
+def test_expect_under_the_filter():
+    """The round under the filter: filtered feasible counts never exceed the plain ones, each companion row sums to
+    the nodes that fit the plain round and fail the filter, the Filter matrix and its codes are the same with the
+    switch on and off, and the outputs the filter does not reach are the plain round's."""
+    cfg = dict(score=True, fit_bitmap=True, filter=True, reasons=True, priority_k=8)
+    for seed in (31, 32):
+        m, snap, node, pods = _loaded(seed, P=120, N=200, G=20, L=[5, 9][seed % 2])
+        assert m.apply({"op": "evaluate", "priority": True}) is None
+        off = m.expect(cfg)
+        assert not off["interpod_rows"].any()
+        assert m.apply({"op": "ipf_switch", "on": True}) is None
+        assert m.apply({"op": "evaluate", "priority": True}) is None
+        on = m.expect(cfg)
+        assert (on["feasible_count"] <= off["feasible_count"]).all()
+        assert (on["feasible_count"] < off["feasible_count"]).any()
+        N = snap.nodes.n
+        fit = np.unpackbits(off["fit_rows"].view(np.uint8), axis=1, bitorder="little")[:, :N].astype(bool)
+        v = fr.verdicts((node, pods), N)
+        np.testing.assert_array_equal(on["interpod_rows"].sum(1), (fit & (v != fr.PASS)).sum(1))
+        assert on["interpod_rows"].any()
+        for key in ("filter_rows", "filter_code", "prefilter", "new_denied", "order", "rank", "reason_rows",
+                    "max_group", "max_finished"):
+            np.testing.assert_array_equal(on[key], off[key], err_msg=key)
+        fit_on = np.unpackbits(on["fit_rows"].view(np.uint8), axis=1, bitorder="little")[:, :N].astype(bool)
+        np.testing.assert_array_equal(fit_on, fit & (v == fr.PASS))
+        assert (on["priority_nodes"] >= 0).sum(1).tolist() == np.minimum(8, on["feasible_count"]).tolist()

@@ -1,5 +1,6 @@
 """GPU: one long-lived engine through seeded sequences of uploads, row updates, affinity tables, side columns, weights,
-failing calls, rounds, walks and preemption (tests/engine_model.py), with every output on.  After each op the engine
+the MatchInterPodAffinity filter's switch and halves, failing calls, rounds, walks, preemption with
+PodDisruptionBudget bits and the preemption walk (tests/engine_model.py), with every output on.  After each op the engine
 answers the error code the host model predicts, and every round, walk and preemption is bit-exact against the CPU
 restatements on the model's state.  A mismatch reports the seed, the step, the ops up to it, the first differing
 output and whether a fresh engine loaded with the model's state agrees (stale engine state) or not (a kernel)."""
@@ -78,6 +79,7 @@ def _round(eng, cfg, how):
         out["topk_nodes"], out["topk_scores"] = eng.topk_rows()
     if cfg.get("reasons"):
         out["reason_rows"] = eng.reason_rows()
+        out["interpod_rows"] = eng.fetch_interpod_reason_rows()
     if cfg.get("priority_k"):
         out["priority_nodes"], out["priority_scores"] = eng.priority_rows()
     out["lanes"] = eng.fit_lanes()
@@ -104,6 +106,10 @@ def _call(pkg, eng, L, op, cfg):
             eng.upload_bound_pods(op["table"])
         elif k == "side":
             _side(eng, op)
+        elif k == "ipf":
+            eng.upload_interpod_filter(**{"node" if op["half"] == "node" else "pods": op["cols"]})
+        elif k == "ipf_switch":
+            eng.set_interpod_filter(op["on"])
         elif k == "weights":
             _weights(eng, L, op)
         elif k == "evaluate":
@@ -114,6 +120,10 @@ def _call(pkg, eng, L, op, cfg):
         elif k == "preempt":
             r = eng.preempt(op["pods"])
             return None, {"node": r.node, "n_victims": r.n_victims, "n_candidates": r.n_candidates, "victims": r.victims}
+        elif k == "preempt_walk":
+            r = eng.preempt_walk(op["pods"], gang=op["gang"])
+            return None, {"node": r.node, "n_victims": r.n_victims, "n_candidates": r.n_candidates, "victims": r.victims,
+                          "outcome": r.outcome, "evicted_by": r.evicted_by}
         else:
             raise ValueError(k)
     except pkg.capi.BsError as ex:
@@ -138,8 +148,19 @@ def _first_diff(got, want):
     return None
 
 
-def _fresh_agrees(pkg, model, cfg, L):
-    """A fresh engine loaded with the model's state: does its round equal the references?"""
+def _expect(model, op, cfg):
+    if op["op"] == "evaluate":
+        return model.expect(cfg)
+    if op["op"] == "replay":
+        return model.expect_walk(op["priority"], None)
+    if op["op"] == "preempt":
+        return model.expect_preempt(op["pods"])
+    return model.expect_preempt_walk(op["pods"], op["gang"])
+
+
+def _fresh_agrees(pkg, model, cfg, L, op):
+    """A fresh engine loaded with the model's state (tables, sides, weights, the filter's halves and switch, the
+    bound table): does `op` (a round, walk or preemption; else a round) on it equal the references?"""
     eng = _engine(pkg, L, cfg)
     try:
         eng.upload_nodes(model.nodes)
@@ -151,12 +172,22 @@ def _fresh_agrees(pkg, model, cfg, L):
             if cols is not None:
                 name, half = key.split("_")
                 _side(eng, {"name": name, "half": half, "cols": cols})
+        for half in ("node", "pod"):
+            if getattr(model, "ipf_" + half) is not None:
+                _call(pkg, eng, L, {"op": "ipf", "half": half, "cols": getattr(model, "ipf_" + half)}, cfg)
+        eng.set_interpod_filter(model.ipf_on)
+        if model.bound is not None:
+            eng.upload_bound_pods(model.bound)
         _weights(eng, L, dict(weights=model.weights, ratio=model.ratio, pw=model.pw, lw=model.lw,
                               w_spread=model.w_spread, w_ipa=model.w_ipa))
-        got = _round(eng, cfg, "evaluate")
-        want = model.expect(cfg)
-        want.pop("lanes")
-        got.pop("lanes")
+        if op["op"] not in ("evaluate", "replay", "preempt", "preempt_walk"):
+            op = {"op": "evaluate", "how": "evaluate"}
+        code, got = _call(pkg, eng, L, op, cfg)
+        if code is not None:
+            return f"fresh engine answered {code}"
+        want = _expect(model, op, cfg)
+        want.pop("lanes", None)
+        got.pop("lanes", None)
         return _first_diff(got, want) is None
     except Exception as ex:  # noqa: BLE001
         return f"fresh engine failed: {ex!r}"
@@ -175,7 +206,7 @@ def _run_seed(pkg, cfg, seed):
 
             def fail(what):
                 log = "\n".join(f"  {i:3d} {em.describe(o)}" for i, o in enumerate(ops[:step + 1]))
-                fresh = _fresh_agrees(pkg, model, cfg, L) if model.complete() else "n/a (tables missing)"
+                fresh = _fresh_agrees(pkg, model, cfg, L, op) if model.complete() else "n/a (tables missing)"
                 pytest.fail(f"seed {seed} step {step}: {what}\nfresh engine with the model's state agrees with the "
                             f"references: {fresh}\nops:\n{log}")
 
@@ -183,12 +214,7 @@ def _run_seed(pkg, cfg, seed):
                 fail(f"{em.describe(op)} answered {code}, the model predicts {want_code}")
             if got is None or want_code is not None:
                 continue
-            if op["op"] == "evaluate":
-                d = _first_diff(got, model.expect(cfg))
-            elif op["op"] == "replay":
-                d = _first_diff(got, model.expect_walk(op["priority"], None))
-            else:
-                d = _first_diff(got, model.expect_preempt(op["pods"]))
+            d = _first_diff(got, _expect(model, op, cfg))
             if d:
                 fail(f"{em.describe(op)}: {d}")
     finally:
@@ -196,6 +222,6 @@ def _run_seed(pkg, cfg, seed):
 
 
 @pytest.mark.parametrize("config", sorted(CONFIGS))
-@pytest.mark.parametrize("seed", range(8))
+@pytest.mark.parametrize("seed", range(9))
 def test_engine_sequences(pkg, oracle, config, seed):
     _run_seed(pkg, CONFIGS[config], seed)

@@ -6,7 +6,6 @@ Checked: the round's decisions, the fit bitmap, scores, top-K, the priority list
 the reason rows and their companion, every lane bound, unaligned sizes, more than 32768 filter classes, the switch
 against no sides at all, when the pre-pass runs, the drop rules, the caps and error codes, the four refusals, and
 sampled pods of a cfg4 round with the generator's columns."""
-import copy
 
 import numpy as np
 import pytest
@@ -19,35 +18,6 @@ from randsnap import S, random_snapshot
 
 pytestmark = pytest.mark.gpu
 
-AFF_NONE = 0xFFFFFFFF
-
-
-def _pack_bits(b: np.ndarray) -> np.ndarray:
-    """[P, N] bool -> [P, ceil(N/32)] uint32, bit n % 32 of word n / 32."""
-    P, N = b.shape
-    W = (N + 31) // 32
-    pad = np.zeros((P, W * 32), np.uint64)
-    pad[:, :N] = b
-    return (pad.reshape(P, W, 32) << np.arange(32, dtype=np.uint64)).sum(2).astype(np.uint32)
-
-
-def _filtered(snap, v):
-    """The snapshot with pod p's affinity row ANDed with the filter's pass bits (v[p] == PASS); groups keep theirs."""
-    P, N = v.shape
-    W = (N + 31) // 32
-    old = snap.aff_bits if snap.aff_bits is not None else np.zeros((0, W), np.uint32)
-    ac = snap.pods.aff_class if snap.pods.aff_class is not None else np.full(P, AFF_NONE, np.uint32)
-    base = np.where((ac == AFF_NONE)[:, None], np.uint32(0xFFFFFFFF), old[np.minimum(ac, max(len(old) - 1, 0))]
-                    if len(old) else np.uint32(0xFFFFFFFF))
-    rows = (base & _pack_bits(v == fr.PASS)).astype(np.uint32)
-    out = copy.deepcopy(snap)
-    out.aff_bits = np.ascontiguousarray(np.concatenate([old, rows]), dtype=np.uint32)
-    out.pods.aff_class = (len(old) + np.arange(P)).astype(np.uint32)
-    if out.groups.rep_aff is None:
-        out.groups.rep_aff = np.full(out.groups.n, AFF_NONE, np.uint32)
-    return out
-
-
 def _engine(pkg, snap, cols, on=True, **kw):
     eng = pkg.Engine(snap.lanes, 0, **kw)
     eng.upload(snap)
@@ -58,50 +28,23 @@ def _engine(pkg, snap, cols, on=True, **kw):
 
 
 ROUND = ("prefilter", "feasible_count", "best_node", "best_score", "admit", "admit_bitmap", "new_denied", "order", "rank")
-ADMIT, WAIT, UNSCHEDULABLE = range(3)   # BS_ADMIT, BS_WAIT, BS_UNSCHEDULABLE
-
-
-def _admit(snap, prefilter, feasible, idle):
-    """Permit readiness per group from each pod's PreFilter verdict and feasible count (gang_admit_kernel's rule);
-    groups without a pod in the round keep `idle`."""
-    gt, G = snap.groups, snap.groups.n
-    gid = snap.pods.gid
-    ok = (gid >= 0) & (gid < G)
-    in_round = np.bincount(gid[ok], minlength=G)
-    c = np.bincount(gid[ok], weights=((prefilter == 0) & (feasible > 0))[ok], minlength=G).astype(np.int64)
-    need = (gt.min_member.astype(np.int64) - gt.scheduled) & 0xFFFFFFFF
-    v = np.where(c == 0, UNSCHEDULABLE, np.where(gt.matched + c >= need, ADMIT, WAIT))
-    admit = np.where(in_round > 0, v, idle).astype(np.uint8)
-    bits = np.zeros(((G + 31) // 32) * 32, np.uint64)
-    bits[:G] = admit == ADMIT
-    return admit, (bits.reshape(-1, 32) << np.arange(32, dtype=np.uint64)).sum(1).astype(np.uint32)
 
 
 def _check_round(pkg, oracle, snap, cols):
-    """The round under the filter: the fit-set outputs are the filtered snapshot's, PreFilter's (and the sort's) the
-    plain snapshot's (a pod's affinity row also reaches PreFilter, the filter does not), and Permit readiness follows
-    from both."""
-    v = fr.verdicts(cols, snap.nodes.n)
-    fsnap = _filtered(snap, v)
-    orc = oracle.round(fsnap, want_bitmap=True, want_score=True)
-    plain = oracle.round(snap, want_bitmap=True)
-    a0, b0 = _admit(snap, plain.prefilter, plain.feasible_count, plain.admit)
-    np.testing.assert_array_equal(a0, plain.admit)   # the readiness rule restated reproduces the oracle's
-    np.testing.assert_array_equal(b0, plain.admit_bitmap)
-    admit, bitmap = _admit(snap, plain.prefilter, orc.feasible_count, plain.admit)
-    want = dict(prefilter=plain.prefilter, feasible_count=orc.feasible_count, best_node=orc.best_node,
-                best_score=orc.best_score, admit=admit, admit_bitmap=bitmap, new_denied=plain.new_denied,
-                order=plain.order, rank=plain.rank)
+    """The round under the filter against interpod_filter_ref.expected_round: the fit-set outputs are the filtered
+    snapshot's, PreFilter's (and the sort's) the plain snapshot's (a pod's affinity row also reaches PreFilter, the
+    filter does not), and Permit readiness follows from both."""
+    want, fsnap = fr.expected_round(snap, cols, dict(fit_bitmap=True, score=True))
     eng = _engine(pkg, snap, cols, fit_bitmap=True, score=True)
     try:
         res = eng.evaluate()
         for f in ROUND:
             np.testing.assert_array_equal(getattr(res, f), want[f], err_msg=f)
-        np.testing.assert_array_equal(eng.fit_rows(), orc.fit_bitmap)
-        np.testing.assert_array_equal(eng.score_rows(), orc.score)
+        np.testing.assert_array_equal(eng.fit_rows(), want["fit_rows"])
+        np.testing.assert_array_equal(eng.score_rows(), want["score_rows"])
     finally:
         eng.close()
-    return v, fsnap, plain
+    return fr.verdicts(cols, snap.nodes.n), fsnap, oracle.round(snap, want_bitmap=True)
 
 
 @pytest.mark.parametrize("L", [5, 9, 16])
@@ -245,7 +188,7 @@ def test_pod_side_reuploads(pkg, oracle):
             if k % 4 == 3:
                 eng.evaluate()
                 v = fr.verdicts((cols[0], pods), snap.nodes.n)
-                np.testing.assert_array_equal(eng.fit_rows()[:, :W], off & _pack_bits(v == fr.PASS), err_msg=str(k))
+                np.testing.assert_array_equal(eng.fit_rows()[:, :W], off & fr.pack_bits(v == fr.PASS), err_msg=str(k))
     finally:
         eng.close()
 
@@ -339,7 +282,7 @@ def test_cases_on_device(pkg, oracle):
             fit_off = eng.fit_rows()[:, :1]
         finally:
             eng.close()
-        np.testing.assert_array_equal(fit_on, fit_off & _pack_bits(v == fr.PASS), err_msg=name)
+        np.testing.assert_array_equal(fit_on, fit_off & fr.pack_bits(v == fr.PASS), err_msg=name)
 
 
 def test_cfg4_sampled(pkg, oracle):
@@ -358,5 +301,5 @@ def test_cfg4_sampled(pkg, oracle):
         eng.close()
     v = fr.verdicts(cols, snap.nodes.n, pods)
     W = (snap.nodes.n + 31) // 32
-    np.testing.assert_array_equal(on[:, :W], off[:, :W] & _pack_bits(v == fr.PASS))
+    np.testing.assert_array_equal(on[:, :W], off[:, :W] & fr.pack_bits(v == fr.PASS))
     assert (v != fr.PASS).any()
