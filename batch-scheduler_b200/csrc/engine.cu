@@ -365,6 +365,14 @@ void assign_classes(ClassIndex& global, uint32_t n, KeyFn key_of, uint32_t* out)
   merge_classes(global, local, ch, out);
 }
 
+// The node side of InterPodAffinity and of the MatchInterPodAffinity filter (bs_interpod_nodes): topology values
+// [keys][N], each term's key and first (term, value) slot, the bound pods and their class table.
+struct InterpodNodeSide {
+  DevBuf d_topo, d_term_key, d_term_off, d_bound_node, d_bound_class, d_boff, d_bterm, d_bown, d_bmatch;
+  uint32_t terms = 0, bound = 0, bclasses = 0;
+  uint64_t slots = 0;
+};
+
 }  // namespace
 
 struct bs_engine {
@@ -428,72 +436,79 @@ struct bs_engine {
   DevBuf d_left_full, d_reason_gate, d_reason_class, d_reasons;
   // BS_OUT_PRIORITY: the non-zero request columns (node [2][Npad] zero-padded, pod [2][P]; each dropped with its
   // table), the score weights, and the lists [P][topk]; the fit set is the reason rows' (d_left_full, d_reason_gate)
-  DevBuf d_nz_node, d_nz_pod, d_prio_node, d_prio_score;
-  bool have_nz_node = false, have_nz_pod = false;
-  int64_t nz_node_max[2] = {0, 0}, nz_pod_max[2] = {0, 0};   // per row, of the uploaded columns (bs_replay_priority)
+  DevBuf d_prio_node, d_prio_score;
+  struct {
+    DevBuf d_node, d_pod;
+    bool have_node = false, have_pod = false;
+    int64_t node_max[2] = {0, 0}, pod_max[2] = {0, 0};   // per row, of the uploaded columns (bs_replay_priority)
+  } nz;
   ScoreWeights weights{1, 0, 1};
   // RequestedToCapacityRatio (bs_set_ratio_priority): weight 0 = off; the shape table lives in d_ratio_tab
   RatioSetting ratio{};
   DevBuf d_ratio_tab;
   // TaintToleration and preferred NodeAffinity (bs_set_node_priority_weights; 0, 0 = off): the node side
   // (PreferNoSchedule masks [Npad], the class x node weights [classes][Npad]; dropped with the node table) and the pod
-  // side (tolerated masks [P], the class of each pod [P]; dropped with the pod table).  pref_class_max: the largest
-  // class a pod names (-1 none), checked against pref_classes at evaluation.
+  // side (tolerated masks [P], the class of each pod [P]; dropped with the pod table).  class_max: the largest class a
+  // pod names (-1 none), checked against classes at evaluation.
   uint32_t w_taint = 0, w_naff = 0;
-  DevBuf d_prefer_taints, d_pref_weights, d_prefer_tol, d_pref_class;
-  bool have_pref_node = false, have_pref_pod = false;
-  uint32_t pref_classes = 0;
-  int64_t pref_class_max = -1;
+  struct {
+    DevBuf d_prefer_taints, d_weights, d_prefer_tol, d_class;
+    bool have_node = false, have_pod = false;
+    uint32_t classes = 0;
+    int64_t class_max = -1;
+  } pref;
   // ImageLocality and NodePreferAvoidPods (bs_set_locality_weights; 0, 0 = off): the node side (the image bit rows
   // [n_images][ceil(N/32)] and sizes, the preferAvoidPods masks [Npad]; dropped with the node table) and the pod side
   // (each pod's image class [P], the classes' CSR, each pod's controller bit [P]; dropped with the pod table); each
-  // side has its image part and its avoid part.  d_img_scaled and the class x node IL table d_loc_il are built on the
-  // device when loc_dirty (priority.cuh image_spread_kernel, locality_class_kernel).  loc_class_max / loc_image_max:
-  // the largest class a pod names and the largest id a class lists (-1 none), checked at evaluation.
+  // side has its image part and its avoid part.  d_img_scaled and the class x node IL table d_il are built on the
+  // device when dirty (priority.cuh image_spread_kernel, locality_class_kernel).  class_max / image_max: the largest
+  // class a pod names and the largest id a class lists (-1 none), checked at evaluation.
   uint32_t w_img = 0, w_avoid = 0;
-  DevBuf d_img_bits, d_img_size, d_img_scaled, d_avoid_mask, d_loc_class, d_loc_off, d_loc_ids, d_avoid_bit, d_loc_il;
-  bool have_img_node = false, have_avoid_node = false, have_img_pod = false, have_avoid_pod = false;
-  bool loc_dirty = true;
-  uint32_t loc_images = 0, loc_classes = 0;
-  int64_t loc_class_max = -1, loc_image_max = -1;
+  struct {
+    DevBuf d_img_bits, d_img_size, d_img_scaled, d_avoid_mask, d_class, d_off, d_ids, d_avoid_bit, d_il;
+    bool have_img_node = false, have_avoid_node = false, have_img_pod = false, have_avoid_pod = false;
+    bool dirty = true;
+    uint32_t images = 0, classes = 0;
+    int64_t class_max = -1, image_max = -1;
+  } loc;
   // SelectorSpread (bs_set_spread_weight; 0 = off): the node side (each node's zone [Npad], the class x node counts
   // [classes][Npad]; dropped with the node table) and the pod side (each pod's class [P]; dropped with the pod table).
-  // spread_class_max: the largest class a pod names (-1 none), checked against spread_classes at evaluation.
+  // class_max: the largest class a pod names (-1 none), checked against classes at evaluation.
   uint32_t w_spread = 0;
-  DevBuf d_spread_zone, d_spread_counts, d_spread_class;
-  bool have_spread_node = false, have_spread_pod = false;
-  uint32_t spread_classes = 0;
-  int64_t spread_class_max = -1;
-  // InterPodAffinity (bs_set_interpod_weight; 0 = off): the node side (topology values [keys][N], each term's key and
-  // first (term, value) slot, the bound pods and their class table; dropped with the node table) and the pod side (each
-  // pod's class [P] and the class table; dropped with the pod table).  d_ipa_ms (M and S per slot) and the pod class x
-  // node raw table d_ipa_raw are built on the device when ipa_dirty (ipa_mass_dirty: M and S too).  ipa_term_max: the
-  // largest term a pod class names (-1 none), checked against ipa_terms at evaluation.
+  struct {
+    DevBuf d_zone, d_counts, d_class;
+    bool have_node = false, have_pod = false;
+    uint32_t classes = 0;
+    int64_t class_max = -1;
+  } spread;
+  // InterPodAffinity (bs_set_interpod_weight; 0 = off): the node side (InterpodNodeSide; dropped with the node table)
+  // and the pod side (each pod's class [P] and the class table; dropped with the pod table).  d_ms (M and S per slot)
+  // and the pod class x node raw table d_raw are built on the device when dirty (mass_dirty: M and S too).
+  // term_max: the largest term a pod class names (-1 none), checked against node.terms at evaluation.
   uint32_t w_ipa = 0;
-  DevBuf d_ipa_topo, d_ipa_term_key, d_ipa_term_off, d_ipa_bound_node, d_ipa_bound_class;
-  DevBuf d_ipa_boff, d_ipa_bterm, d_ipa_bown, d_ipa_bmatch, d_ipa_ms;
-  DevBuf d_ipa_class, d_ipa_poff, d_ipa_pterm, d_ipa_pown, d_ipa_pmatch, d_ipa_raw;
-  bool have_ipa_node = false, have_ipa_pod = false, ipa_dirty = true, ipa_mass_dirty = true;
-  uint32_t ipa_terms = 0, ipa_bound = 0, ipa_bclasses = 0, ipa_pclasses = 0;
-  uint64_t ipa_slots = 0;
-  int64_t ipa_term_max = -1;
-  // MatchInterPodAffinity filter (bs_set_interpod_filter; off by default): the node side (topology values, each term's
-  // key and first slot, the bound pods and their class table; dropped with the node table) and the pod side (each pod's
-  // filter class h_ipf_class, the class table; dropped with the pod table).  The presence planes d_ipf_presence
-  // ([2][words]: match, own), the per-term counts d_ipf_hits and the class planes d_ipf_bits ([3][classes][Npad/32]:
-  // pass, E, A) are built on the device when ipf_dirty.  ipf_assign_dirty: the pods' fit classes have to be assigned
-  // again (with their filter class while the filter is on, else their base class h_pfc_base).  d_fipf: each fit class's
-  // filter class, d_reason_gate_ipf the priority lists' gate, d_ipf_reasons the companion rows [P][3].
-  bool ipf_on = false, ipf_round = false;
-  DevBuf d_ipf_topo, d_ipf_term_key, d_ipf_term_off, d_ipf_bound_node, d_ipf_bound_class;
-  DevBuf d_ipf_boff, d_ipf_bterm, d_ipf_bown, d_ipf_bmatch, d_ipf_presence, d_ipf_hits;
-  DevBuf d_ipf_poff, d_ipf_pterm, d_ipf_prole, d_ipf_pself, d_ipf_bits, d_fipf, d_reason_gate_ipf, d_ipf_reasons;
-  bool have_ipf_node = false, have_ipf_pod = false, ipf_dirty = true, ipf_assign_dirty = false;
-  uint32_t ipf_terms = 0, ipf_bound = 0, ipf_pclasses = 0;
-  uint64_t ipf_slots = 0;
-  int64_t ipf_term_max = -1;
-  std::vector<uint32_t> h_ipf_class, h_pfc_base;   // h_pfc_base: the pods' fit classes without the filter
-  bool pfc_base_valid = false;                     // h_pfc_base holds the classes of the pod table of now
+  struct {
+    InterpodNodeSide node;
+    DevBuf d_ms, d_class, d_poff, d_pterm, d_pown, d_pmatch, d_raw;
+    bool have_node = false, have_pod = false, dirty = true, mass_dirty = true;
+    uint32_t pclasses = 0;
+    int64_t term_max = -1;
+  } ipa;
+  // MatchInterPodAffinity filter (bs_set_interpod_filter; off by default): the node side (InterpodNodeSide; dropped
+  // with the node table) and the pod side (each pod's filter class h_class, the class table; dropped with the pod
+  // table).  The presence planes d_presence ([2][words]: match, own), the per-term counts d_hits and the class planes
+  // d_bits ([3][classes][Npad/32]: pass, E, A) are built on the device when dirty.  assign_dirty: the pods' fit classes
+  // have to be assigned again (with their filter class while the filter is on, else their base class h_pfc_base).
+  // d_fipf: each fit class's filter class, d_reason_gate the priority lists' gate, d_reasons the companion rows [P][3].
+  struct {
+    bool on = false, round = false;
+    InterpodNodeSide node;
+    DevBuf d_presence, d_hits, d_poff, d_pterm, d_prole, d_pself, d_bits, d_fipf, d_reason_gate, d_reasons;
+    bool have_node = false, have_pod = false, dirty = true, assign_dirty = false;
+    uint32_t pclasses = 0;
+    int64_t term_max = -1;
+    std::vector<uint32_t> h_class, h_pfc_base;   // h_pfc_base: the pods' fit classes without the filter
+    bool pfc_base_valid = false;                 // h_pfc_base holds the classes of the pod table of now
+  } ipf;
   // sort scratch: views into one arena
   View d_gk0, d_gk1, d_pk0, d_pk1, d_idx_a, d_idx_b, d_ghist, d_group_rank, d_tilecnt, d_sort_barrier;
   uint32_t sort_max_grid = 1;
@@ -689,11 +704,12 @@ bool null_column(const std::array<Col, K>& cols) {
   return std::any_of(cols.begin(), cols.end(), [](const Col& c) { return !c.host; });
 }
 
-// upload a host column of n rows into its device column padded to npad rows (rows >= n zero)
-int upload_col(bs_engine* e, const Col& c, uint32_t n, uint32_t npad) {
+// upload a host column of n rows into its device column padded to npad >= n rows (at least one allocated), the
+// padding's bytes set to fill
+int upload_col(bs_engine* e, const Col& c, uint64_t n, uint64_t npad, int fill = 0) {
   const size_t row = (size_t)c.elem * n, prow = (size_t)c.elem * npad;
-  CK(c.dev->ensure(prow * c.lanes));
-  if (npad != n) CK(cudaMemsetAsync(c.dev->p, 0, prow * c.lanes, e->s));
+  CK(c.dev->ensure((size_t)c.elem * std::max<uint64_t>(npad, 1) * c.lanes));
+  if (npad > n) CK(cudaMemsetAsync(c.dev->p, fill, prow * c.lanes, e->s));
   if (n && c.lanes == 1) CK(cudaMemcpyAsync(c.dev->p, c.host, row, cudaMemcpyHostToDevice, e->s));
   else if (n) CK(cudaMemcpy2DAsync(c.dev->p, prow, c.host, row, row, c.lanes, cudaMemcpyHostToDevice, e->s));
   return BS_OK;
@@ -706,9 +722,33 @@ int upload_cols(bs_engine* e, const std::array<Col, K>& cols, uint32_t n, uint32
   return BS_OK;
 }
 template <class T>
-int upload_vec(bs_engine* e, DevBuf& dst, const T* src, uint32_t n, uint32_t npad) {
-  return upload_col(e, col(src, dst), n, npad);
+int upload_vec(bs_engine* e, DevBuf& dst, const T* src, uint64_t n, uint64_t npad, int fill = 0) {
+  return upload_col(e, col(src, dst), n, npad, fill);
 }
+
+// The largest class col[0, n) names, `none` aside (-1 when there is none).
+int64_t max_class(const uint32_t* col, uint32_t n, uint32_t none) {
+  int64_t mx = -1;
+  for (uint32_t k = 0; k < n; ++k)
+    if (col[k] != none) mx = std::max(mx, (int64_t)col[k]);
+  return mx;
+}
+
+// A refusal of the call `who`: its code, with "who: why" as the engine's last error.
+enum SideOf { NODE_SIDE, POD_SIDE };
+struct Refuse {
+  bs_engine* e;
+  const char* who;
+  int operator()(int rc, const char* why) const { return fail(e, rc, (std::string(who) + ": " + why).c_str()); }
+  // a side table's shape: the table it belongs to is uploaded (BS_E_STATE) and has n rows (BS_E_INVAL)
+  int shape(SideOf side, uint32_t n) const {
+    if (side == NODE_SIDE && !e->have_nodes) return (*this)(BS_E_STATE, "upload nodes first");
+    if (side == POD_SIDE && !e->have_pods) return (*this)(BS_E_STATE, "upload pods first");
+    if (side == NODE_SIDE && n != e->N) return (*this)(BS_E_INVAL, "n_nodes differs from the node table's");
+    if (side == POD_SIDE && n != e->P) return (*this)(BS_E_INVAL, "n_pods differs from the pod table's");
+    return BS_OK;
+  }
+};
 
 // Stages the n changed rows of every column, and idx, in d_stage, and scatters row k of each column to row
 // idx[k] of its device column (pitch rows per lane).  The caller synchronises before its arrays are reused.
@@ -986,7 +1026,7 @@ void compact_fit_index(bs_engine* e) {
   ClassIndex& fi = e->fit_index;
   const uint32_t P = e->P;
   uint32_t* pfc = e->h_pfc.data();
-  uint32_t* base = e->pfc_base_valid ? e->h_pfc_base.data() : nullptr;
+  uint32_t* base = e->ipf.pfc_base_valid ? e->ipf.h_pfc_base.data() : nullptr;
   std::vector<uint8_t> used(fi.size(), 0);
   size_t n_used = 0;
   auto mark = [&](uint32_t id) { n_used += used[id] ? 0 : 1; used[id] = 1; };
@@ -1022,25 +1062,25 @@ int rebuild_classes(bs_engine* e) {
     e->group_classes_dirty = false;
   }
   HP(e, "classes:assign-groups");
-  if (e->ipf_assign_dirty) {
+  if (e->ipf.assign_dirty) {
     // the pods' fit classes with their filter class while the filter is on, else the classes of the upload
     uint32_t* pfc = e->h_pfc.data();
-    if (e->ipf_on) {
-      if (!e->pfc_base_valid) e->h_pfc_base.assign(pfc, pfc + P);
-      e->pfc_base_valid = true;
-      const uint32_t* base = e->h_pfc_base.data();
-      const uint32_t* ipf = e->h_ipf_class.data();
+    if (e->ipf.on) {
+      if (!e->ipf.pfc_base_valid) e->ipf.h_pfc_base.assign(pfc, pfc + P);
+      e->ipf.pfc_base_valid = true;
+      const uint32_t* base = e->ipf.h_pfc_base.data();
+      const uint32_t* ipf = e->ipf.h_class.data();
       ClassIndex& fi = e->fit_index;
       assign_classes(fi, P, [&fi, base, ipf](uint32_t p) {
         ClassKey k = fi.keys[base[p]];
         k.ipf = ipf[p];
         return k;
       }, pfc);
-    } else if (e->pfc_base_valid) {
-      memcpy(pfc, e->h_pfc_base.data(), (size_t)P * 4);
+    } else if (e->ipf.pfc_base_valid) {
+      memcpy(pfc, e->ipf.h_pfc_base.data(), (size_t)P * 4);
     }
     compact_fit_index(e);
-    e->ipf_assign_dirty = false;
+    e->ipf.assign_dirty = false;
   }
   if (e->fit_index.size() == 0) e->fit_index.get_or_add(ClassKey{0, 0, 0, BS_AFF_NONE});
   if (e->rep_index.size() == 0) e->rep_index.get_or_add(ClassKey{0, 0, 0, BS_AFF_NONE});
@@ -1085,14 +1125,14 @@ int rebuild_classes(bs_engine* e) {
   if ((rc = upload_vec(e, e->d_raff, raff.data(), e->n_rep_classes, e->n_rep_classes))) return rc;
   if ((rc = upload_vec(e, e->d_rsel, rsel.data(), e->n_rep_classes, e->n_rep_classes))) return rc;
   if ((rc = upload_vec(e, e->d_rtol, rtol.data(), e->n_rep_classes, e->n_rep_classes))) return rc;
-  if (e->ipf_on) {
+  if (e->ipf.on) {
     // a stale class may name a filter class the pod side of now does not have: no pod uses it, so it passes
     std::vector<uint32_t> fipf(e->n_fit_classes);
     for (uint32_t c = 0; c < e->n_fit_classes; ++c) {
       const uint32_t f = e->fit_index.keys[c].ipf;
-      fipf[c] = f < e->ipf_pclasses ? f : BS_IPF_NONE;
+      fipf[c] = f < e->ipf.pclasses ? f : BS_IPF_NONE;
     }
-    if ((rc = upload_vec(e, e->d_fipf, fipf.data(), e->n_fit_classes, e->n_fit_classes))) return rc;
+    if ((rc = upload_vec(e, e->ipf.d_fipf, fipf.data(), e->n_fit_classes, e->n_fit_classes))) return rc;
   }
   if (e->pod_classes_dirty) {   // a group-only change (bs_update_groups) leaves the pods' ids alone
     if ((rc = upload_vec(e, e->d_pod_fit_class, e->h_pfc.data(), P, std::max(P, 1u)))) return rc;
@@ -1145,7 +1185,7 @@ int ensure_round_buffers(bs_engine* e) {
     CK(e->d_filter_bitmap.ensure(Prows * std::max(e->W, 1u) * 4));
   }
   if (e->out_flags & BS_OUT_REASONS) CK(e->d_reasons.ensure((size_t)P * (4 + L) * 4));
-  if ((e->out_flags & BS_OUT_REASONS) && e->ipf_on) CK(e->d_ipf_reasons.ensure((size_t)P * 3 * 4));
+  if ((e->out_flags & BS_OUT_REASONS) && e->ipf.on) CK(e->ipf.d_reasons.ensure((size_t)P * 3 * 4));
   if (e->out_flags & BS_OUT_PRIORITY) {
     CK(e->d_prio_node.ensure((size_t)P * e->topk * 4));
     CK(e->d_prio_score.ensure((size_t)P * e->topk * 8));
@@ -1205,11 +1245,11 @@ int prepare_nodes(bs_engine* e) {
   {
     for (uint32_t c0 = 0; c0 < e->n_fit_classes; c0 += 32768) {
       dim3 grid(cdiv(n_tiles * 32, 256), std::min(32768u, e->n_fit_classes - c0));
-      auto fn = e->ipf_on ? class_fit_kernel<true> : class_fit_kernel<false>;
+      auto fn = e->ipf.on ? class_fit_kernel<true> : class_fit_kernel<false>;
       fn<<<grid, 256, 0, e->s>>>(t, e->d_left_present.as<uint32_t>(), e->d_fsel.as<uint64_t>(), e->d_ftol.as<uint64_t>(),
                                  e->d_fnz.as<uint32_t>(), e->d_faff.as<uint32_t>(), e->n_fit_classes, n_tiles,
-                                 e->d_classfit.as<ColBits>(), c0, e->d_fipf.as<uint32_t>(),
-                                 e->d_ipf_bits.as<uint32_t>(), e->Npad / 32);
+                                 e->d_classfit.as<ColBits>(), c0, e->ipf.d_fipf.as<uint32_t>(),
+                                 e->ipf.d_bits.as<uint32_t>(), e->Npad / 32);
       tm.launched();
     }
   }
@@ -1219,15 +1259,15 @@ int prepare_nodes(bs_engine* e) {
     CK(e->d_reason_gate.ensure((size_t)e->n_fit_classes * Wg * 4));
     CK(e->d_reason_class.ensure((size_t)e->n_fit_classes * 4 * 4));
     CK(cudaMemsetAsync(e->d_reason_class.p, 0, (size_t)e->n_fit_classes * 4 * 4, e->s));
-    if (e->ipf_on) CK(e->d_reason_gate_ipf.ensure((size_t)e->n_fit_classes * Wg * 4));
+    if (e->ipf.on) CK(e->ipf.d_reason_gate.ensure((size_t)e->n_fit_classes * Wg * 4));
     for (uint32_t c0 = 0; c0 < e->n_fit_classes; c0 += 32768) {
       dim3 grid(cdiv(Wg * 32, REASON_CLASS_THREADS), std::min(32768u, e->n_fit_classes - c0));
-      auto fn = e->ipf_on ? reason_class_kernel<true> : reason_class_kernel<false>;
+      auto fn = e->ipf.on ? reason_class_kernel<true> : reason_class_kernel<false>;
       fn<<<grid, REASON_CLASS_THREADS, 0, e->s>>>(t, e->d_fsel.as<uint64_t>(), e->d_ftol.as<uint64_t>(),
                                                   e->d_faff.as<uint32_t>(), e->n_fit_classes, Wg,
                                                   e->d_reason_gate.as<uint32_t>(), e->d_reason_class.as<uint32_t>(), c0,
-                                                  e->d_fipf.as<uint32_t>(), e->d_ipf_bits.as<uint32_t>(),
-                                                  e->d_reason_gate_ipf.as<uint32_t>());
+                                                  e->ipf.d_fipf.as<uint32_t>(), e->ipf.d_bits.as<uint32_t>(),
+                                                  e->ipf.d_reason_gate.as<uint32_t>());
       tm.launched();
     }
   }
@@ -1236,66 +1276,115 @@ int prepare_nodes(bs_engine* e) {
   return BS_OK;
 }
 
-// The columns a non-zero bs_set_locality_weights weight reads (BS_E_STATE when one is missing) and the ids they hold
-// (BS_E_INDEX), checked before anything is launched.
+// The side tables' checks before anything is launched: the columns a non-zero weight (or the filter switch) reads,
+// BS_E_STATE when a side is missing, the ids they hold (BS_E_INDEX) and the tables they size (BS_E_INVAL).  The pod
+// sides outlive node uploads: their class x node tables are checked against the node table of now.
+int nonzero_check(bs_engine* e, const char* who) {
+  if (!(e->nz.have_node && e->nz.have_pod))
+    return Refuse{e, who}(BS_E_STATE, "BS_OUT_PRIORITY needs the node and pod non-zero columns");
+  return BS_OK;
+}
+
+int preference_check(bs_engine* e, const char* who) {
+  const Refuse bad{e, who};
+  if (!(e->w_taint || e->w_naff)) return BS_OK;
+  if (!(e->pref.have_node && e->pref.have_pod))
+    return bad(BS_E_STATE, "a non-zero node priority weight needs the node and pod preference columns");
+  if (e->w_naff && e->pref.class_max >= (int64_t)e->pref.classes)
+    return bad(BS_E_INDEX, "a pod's preference class is outside the uploaded weight table");
+  return BS_OK;
+}
+
 int locality_check(bs_engine* e, const char* who) {
-  const std::string w(who);
+  const Refuse bad{e, who};
   if (e->w_img) {
-    if (!(e->have_img_node && e->have_img_pod))
-      return fail(e, BS_E_STATE, (w + ": a non-zero ImageLocality weight needs the node and pod image columns").c_str());
-    if (e->loc_class_max >= (int64_t)e->loc_classes)
-      return fail(e, BS_E_INDEX, (w + ": a pod's image class is outside the uploaded classes").c_str());
-    if (e->loc_image_max >= (int64_t)e->loc_images)
-      return fail(e, BS_E_INDEX, (w + ": an image class lists an id outside the node side's image dictionary").c_str());
-    // the pod side outlives node uploads: its class x node table is checked against the node table of now
-    if ((uint64_t)e->loc_classes * e->Npad > BS_LOC_TABLE_MAX_BYTES)
-      return fail(e, BS_E_INVAL, (w + ": n_classes x padded nodes bytes exceeds BS_LOC_TABLE_MAX_BYTES").c_str());
+    if (!(e->loc.have_img_node && e->loc.have_img_pod))
+      return bad(BS_E_STATE, "a non-zero ImageLocality weight needs the node and pod image columns");
+    if (e->loc.class_max >= (int64_t)e->loc.classes)
+      return bad(BS_E_INDEX, "a pod's image class is outside the uploaded classes");
+    if (e->loc.image_max >= (int64_t)e->loc.images)
+      return bad(BS_E_INDEX, "an image class lists an id outside the node side's image dictionary");
+    if ((uint64_t)e->loc.classes * e->Npad > BS_LOC_TABLE_MAX_BYTES)
+      return bad(BS_E_INVAL, "n_classes x padded nodes bytes exceeds BS_LOC_TABLE_MAX_BYTES");
   }
-  if (e->w_avoid && !(e->have_avoid_node && e->have_avoid_pod))
-    return fail(e, BS_E_STATE, (w + ": a non-zero NodePreferAvoidPods weight needs the node and pod avoid columns").c_str());
+  if (e->w_avoid && !(e->loc.have_avoid_node && e->loc.have_avoid_pod))
+    return bad(BS_E_STATE, "a non-zero NodePreferAvoidPods weight needs the node and pod avoid columns");
+  return BS_OK;
+}
+
+int spread_check(bs_engine* e, const char* who) {
+  const Refuse bad{e, who};
+  if (!e->w_spread) return BS_OK;
+  if (!(e->spread.have_node && e->spread.have_pod))
+    return bad(BS_E_STATE, "a non-zero SelectorSpread weight needs the node and pod spread columns");
+  if (e->spread.class_max >= (int64_t)e->spread.classes)
+    return bad(BS_E_INDEX, "a pod's spread class is outside the uploaded count table");
+  return BS_OK;
+}
+
+int interpod_check(bs_engine* e, const char* who) {
+  const Refuse bad{e, who};
+  if (!e->w_ipa) return BS_OK;
+  if (!(e->ipa.have_node && e->ipa.have_pod))
+    return bad(BS_E_STATE, "a non-zero InterPodAffinity weight needs the node and pod inter-pod sides");
+  if (e->ipa.term_max >= (int64_t)e->ipa.node.terms)
+    return bad(BS_E_INDEX, "a pod class's term is outside the node side's term dictionary");
+  if ((uint64_t)e->ipa.pclasses * e->Npad * 8 > BS_IPA_TABLE_MAX_BYTES)
+    return bad(BS_E_INVAL, "pod n_classes x padded nodes x 8 bytes exceeds BS_IPA_TABLE_MAX_BYTES");
+  return BS_OK;
+}
+
+int interpod_filter_check(bs_engine* e, const char* who) {
+  const Refuse bad{e, who};
+  if (!(e->ipf.have_node && e->ipf.have_pod))
+    return bad(BS_E_STATE, "the MatchInterPodAffinity filter needs its node and pod sides");
+  if (e->ipf.term_max >= (int64_t)e->ipf.node.terms)
+    return bad(BS_E_INDEX, "a filter class's term is outside the node side's term dictionary");
+  if (3ull * e->ipf.pclasses * (e->Npad / 8) > BS_IPF_TABLE_MAX_BYTES)
+    return bad(BS_E_INVAL, "3 x filter n_classes x padded nodes / 8 bytes exceeds BS_IPF_TABLE_MAX_BYTES");
   return BS_OK;
 }
 
 // The LOC pre-pass on the main stream: each name's scaled size, then the class x node IL table.  Only after either
 // side or a weight changed, and only while the ImageLocality weight is non-zero (else the table is not read).
 int locality_prepass(bs_engine* e) {
-  if (!e->loc_dirty || !e->w_img) return BS_OK;
-  const uint32_t C = e->loc_classes, I = e->loc_images;
+  if (!e->loc.dirty || !e->w_img) return BS_OK;
+  const uint32_t C = e->loc.classes, I = e->loc.images;
   if (C && e->Npad) {
-    CK(e->d_loc_il.ensure((size_t)C * e->Npad));
-    CK(e->d_img_scaled.ensure((size_t)std::max(I, 1u) * 8));
-    CK(launch_locality_prepass(e->d_img_bits.as<uint32_t>(), e->d_img_size.as<int64_t>(), e->d_img_scaled.as<int64_t>(),
-                               I, e->d_loc_off.as<uint32_t>(), e->d_loc_ids.as<uint32_t>(), e->d_loc_il.as<uint8_t>(), C,
+    CK(e->loc.d_il.ensure((size_t)C * e->Npad));
+    CK(e->loc.d_img_scaled.ensure((size_t)std::max(I, 1u) * 8));
+    CK(launch_locality_prepass(e->loc.d_img_bits.as<uint32_t>(), e->loc.d_img_size.as<int64_t>(), e->loc.d_img_scaled.as<int64_t>(),
+                               I, e->loc.d_off.as<uint32_t>(), e->loc.d_ids.as<uint32_t>(), e->loc.d_il.as<uint8_t>(), C,
                                e->N, e->Npad, e->s));
     e->launches += 2;
   }
-  e->loc_dirty = false;
+  e->loc.dirty = false;
   return BS_OK;
 }
 
 // The IPA pre-pass on the main stream: M and S over the bound pods (after a node-side change), then the pod class x
 // node raw table.  Only after either side changed, and only while the weight is non-zero.
 int interpod_prepass(bs_engine* e) {
-  if (!e->ipa_dirty || !e->w_ipa) return BS_OK;
-  const uint32_t C = e->ipa_pclasses, Npad = e->Npad;
-  if (e->ipa_mass_dirty) {
-    CK(e->d_ipa_ms.ensure((size_t)std::max<uint64_t>(e->ipa_slots, 1) * 16));
-    CK(cudaMemsetAsync(e->d_ipa_ms.p, 0, (size_t)e->ipa_slots * 16, e->s));
+  if (!e->ipa.dirty || !e->w_ipa) return BS_OK;
+  const uint32_t C = e->ipa.pclasses, Npad = e->Npad;
+  const InterpodNodeSide& s = e->ipa.node;
+  if (e->ipa.mass_dirty) {
+    CK(e->ipa.d_ms.ensure((size_t)std::max<uint64_t>(s.slots, 1) * 16));
+    CK(cudaMemsetAsync(e->ipa.d_ms.p, 0, (size_t)s.slots * 16, e->s));
   }
   if (C && Npad) {
-    CK(e->d_ipa_raw.ensure((size_t)C * Npad * 8));
-    const InterpodClasses bound{e->d_ipa_boff.as<uint32_t>(), e->d_ipa_bterm.as<uint32_t>(), e->d_ipa_bown.as<int32_t>(),
-                                e->d_ipa_bmatch.as<uint8_t>(), e->ipa_bclasses};
-    const InterpodClasses pods{e->d_ipa_poff.as<uint32_t>(), e->d_ipa_pterm.as<uint32_t>(), e->d_ipa_pown.as<int32_t>(),
-                               e->d_ipa_pmatch.as<uint8_t>(), C};
-    CK(launch_interpod_prepass(e->ipa_mass_dirty, e->d_ipa_topo.as<uint32_t>(), e->d_ipa_term_key.as<uint32_t>(),
-                               e->d_ipa_term_off.as<uint32_t>(), e->d_ipa_bound_node.as<uint32_t>(),
-                               e->d_ipa_bound_class.as<uint32_t>(), e->ipa_bound, bound, pods,
-                               e->d_ipa_ms.as<int64_t>(), e->d_ipa_raw.as<int64_t>(), e->N, Npad, e->s));
-    e->launches += (e->ipa_mass_dirty && e->ipa_bound) ? 2 : 1;
-    e->ipa_mass_dirty = false;
+    CK(e->ipa.d_raw.ensure((size_t)C * Npad * 8));
+    const InterpodClasses bound{s.d_boff.as<uint32_t>(), s.d_bterm.as<uint32_t>(), s.d_bown.as<int32_t>(),
+                                s.d_bmatch.as<uint8_t>(), s.bclasses};
+    const InterpodClasses pods{e->ipa.d_poff.as<uint32_t>(), e->ipa.d_pterm.as<uint32_t>(), e->ipa.d_pown.as<int32_t>(),
+                               e->ipa.d_pmatch.as<uint8_t>(), C};
+    CK(launch_interpod_prepass(e->ipa.mass_dirty, s.d_topo.as<uint32_t>(), s.d_term_key.as<uint32_t>(),
+                               s.d_term_off.as<uint32_t>(), s.d_bound_node.as<uint32_t>(), s.d_bound_class.as<uint32_t>(),
+                               s.bound, bound, pods, e->ipa.d_ms.as<int64_t>(), e->ipa.d_raw.as<int64_t>(), e->N, Npad, e->s));
+    e->launches += (e->ipa.mass_dirty && s.bound) ? 2 : 1;
+    e->ipa.mass_dirty = false;
   }
-  e->ipa_dirty = false;
+  e->ipa.dirty = false;
   return BS_OK;
 }
 
@@ -1303,80 +1392,59 @@ int interpod_prepass(bs_engine* e) {
 // counts over the bound pods, then the class bit planes.  Only while the filter is on and after a side changed or the
 // filter was switched on.
 int interpod_filter_prepass(bs_engine* e) {
-  if (!e->ipf_on || !e->ipf_dirty) return BS_OK;
-  const uint32_t C = e->ipf_pclasses, Wg = e->Npad / 32;
-  const uint64_t words = (e->ipf_slots + 31) / 32;
-  CK(e->d_ipf_presence.ensure((size_t)std::max<uint64_t>(2 * words, 1) * 4));
-  CK(e->d_ipf_hits.ensure((size_t)std::max(e->ipf_terms, 1u) * 4));
-  CK(e->d_ipf_bits.ensure((size_t)std::max<uint64_t>(3ull * C * Wg, 1) * 4));
-  if (words) CK(cudaMemsetAsync(e->d_ipf_presence.p, 0, (size_t)2 * words * 4, e->s));
-  if (e->ipf_terms) CK(cudaMemsetAsync(e->d_ipf_hits.p, 0, (size_t)e->ipf_terms * 4, e->s));
-  const IpfTopo tp{e->d_ipf_topo.as<uint32_t>(), e->d_ipf_term_key.as<uint32_t>(), e->d_ipf_term_off.as<uint32_t>(), e->N};
-  uint32_t* mbits = e->d_ipf_presence.as<uint32_t>();
-  if (e->ipf_bound) {
-    const IpfBound b{e->d_ipf_bound_node.as<uint32_t>(), e->d_ipf_bound_class.as<uint32_t>(), e->d_ipf_boff.as<uint32_t>(),
-                     e->d_ipf_bterm.as<uint32_t>(), e->d_ipf_bown.as<int32_t>(), e->d_ipf_bmatch.as<uint8_t>(),
-                     e->ipf_bound};
-    ipf_presence_kernel<<<cdiv(e->ipf_bound, IPF_THREADS), IPF_THREADS, 0, e->s>>>(b, tp, mbits, mbits + words,
-                                                                                  e->d_ipf_hits.as<uint32_t>());
+  if (!e->ipf.on || !e->ipf.dirty) return BS_OK;
+  const uint32_t C = e->ipf.pclasses, Wg = e->Npad / 32;
+  const InterpodNodeSide& s = e->ipf.node;
+  const uint64_t words = (s.slots + 31) / 32;
+  CK(e->ipf.d_presence.ensure((size_t)std::max<uint64_t>(2 * words, 1) * 4));
+  CK(e->ipf.d_hits.ensure((size_t)std::max(s.terms, 1u) * 4));
+  CK(e->ipf.d_bits.ensure((size_t)std::max<uint64_t>(3ull * C * Wg, 1) * 4));
+  if (words) CK(cudaMemsetAsync(e->ipf.d_presence.p, 0, (size_t)2 * words * 4, e->s));
+  if (s.terms) CK(cudaMemsetAsync(e->ipf.d_hits.p, 0, (size_t)s.terms * 4, e->s));
+  const IpfTopo tp{s.d_topo.as<uint32_t>(), s.d_term_key.as<uint32_t>(), s.d_term_off.as<uint32_t>(), e->N};
+  uint32_t* mbits = e->ipf.d_presence.as<uint32_t>();
+  if (s.bound) {
+    const IpfBound b{s.d_bound_node.as<uint32_t>(), s.d_bound_class.as<uint32_t>(), s.d_boff.as<uint32_t>(),
+                     s.d_bterm.as<uint32_t>(), s.d_bown.as<int32_t>(), s.d_bmatch.as<uint8_t>(), s.bound};
+    ipf_presence_kernel<<<cdiv(s.bound, IPF_THREADS), IPF_THREADS, 0, e->s>>>(b, tp, mbits, mbits + words,
+                                                                         e->ipf.d_hits.as<uint32_t>());
     e->launches += 1;
   }
-  const IpfPods pc{e->d_ipf_poff.as<uint32_t>(), e->d_ipf_pterm.as<uint32_t>(), e->d_ipf_prole.as<uint8_t>(),
-                   e->d_ipf_pself.as<uint8_t>(), C};
+  const IpfPods pc{e->ipf.d_poff.as<uint32_t>(), e->ipf.d_pterm.as<uint32_t>(), e->ipf.d_prole.as<uint8_t>(),
+                   e->ipf.d_pself.as<uint8_t>(), C};
   for (uint32_t c0 = 0; c0 < C && Wg; c0 += 32768) {
     const dim3 grid(cdiv(Wg * 32, IPF_THREADS), std::min(32768u, C - c0));
-    ipf_class_kernel<<<grid, IPF_THREADS, 0, e->s>>>(pc, tp, mbits, mbits + words, e->d_ipf_hits.as<uint32_t>(),
-                                                     e->d_ipf_bits.as<uint32_t>(), Wg, c0);
+    ipf_class_kernel<<<grid, IPF_THREADS, 0, e->s>>>(pc, tp, mbits, mbits + words, e->ipf.d_hits.as<uint32_t>(),
+                                                     e->ipf.d_bits.as<uint32_t>(), Wg, c0);
     e->launches += 1;
   }
   CK(cudaGetLastError());
-  e->ipf_dirty = false;
+  e->ipf.dirty = false;
   return BS_OK;
 }
 
-// The filter's columns (BS_E_STATE when a side is missing), the terms its pod classes name (BS_E_INDEX) and its class
-// planes' size (BS_E_INVAL), checked before anything is launched.
-int interpod_filter_check(bs_engine* e, const char* who) {
-  const std::string w(who);
-  if (!(e->have_ipf_node && e->have_ipf_pod))
-    return fail(e, BS_E_STATE, (w + ": the MatchInterPodAffinity filter needs its node and pod sides").c_str());
-  if (e->ipf_term_max >= (int64_t)e->ipf_terms)
-    return fail(e, BS_E_INDEX, (w + ": a filter class's term is outside the node side's term dictionary").c_str());
-  // the pod side outlives node uploads: its planes are checked against the node table of now
-  if (3ull * e->ipf_pclasses * (e->Npad / 8) > BS_IPF_TABLE_MAX_BYTES)
-    return fail(e, BS_E_INVAL, (w + ": 3 x filter n_classes x padded nodes / 8 bytes exceeds BS_IPF_TABLE_MAX_BYTES").c_str());
-  return BS_OK;
+// The side tables belong to the node snapshot (the non-zero column, taints, labels, images and annotations of its
+// nodes, the pods bound to them) and to the pod table: each half falls with a new table or changed rows and is
+// uploaded again.
+void drop_node_sides(bs_engine* e) {
+  e->nz.have_node = e->pref.have_node = e->loc.have_img_node = e->loc.have_avoid_node = e->spread.have_node =
+      e->ipa.have_node = e->ipf.have_node = false;
+}
+void drop_pod_sides(bs_engine* e) {
+  e->nz.have_pod = e->pref.have_pod = e->loc.have_img_pod = e->loc.have_avoid_pod = e->spread.have_pod =
+      e->ipa.have_pod = e->ipf.have_pod = false;
 }
 
 int evaluate_async_locked(bs_engine* e) {
   int rc;
   if (!e->have_nodes || !e->have_pods || !e->have_groups)
     return fail(e, BS_E_STATE, "bs_evaluate: upload nodes, groups and pods first");
-  if ((e->out_flags & BS_OUT_PRIORITY) && !(e->have_nz_node && e->have_nz_pod))
-    return fail(e, BS_E_STATE, "bs_evaluate: BS_OUT_PRIORITY needs the node and pod non-zero columns");
-  if ((e->out_flags & BS_OUT_PRIORITY) && (e->w_taint || e->w_naff)) {
-    if (!(e->have_pref_node && e->have_pref_pod))
-      return fail(e, BS_E_STATE, "bs_evaluate: a non-zero node priority weight needs the node and pod preference columns");
-    if (e->w_naff && e->pref_class_max >= (int64_t)e->pref_classes)
-      return fail(e, BS_E_INDEX, "bs_evaluate: a pod's preference class is outside the uploaded weight table");
-  }
-  if ((e->out_flags & BS_OUT_PRIORITY) && (rc = locality_check(e, "bs_evaluate"))) return rc;
-  if ((e->out_flags & BS_OUT_PRIORITY) && e->w_spread) {
-    if (!(e->have_spread_node && e->have_spread_pod))
-      return fail(e, BS_E_STATE, "bs_evaluate: a non-zero SelectorSpread weight needs the node and pod spread columns");
-    if (e->spread_class_max >= (int64_t)e->spread_classes)
-      return fail(e, BS_E_INDEX, "bs_evaluate: a pod's spread class is outside the uploaded count table");
-  }
-  if ((e->out_flags & BS_OUT_PRIORITY) && e->w_ipa) {
-    if (!(e->have_ipa_node && e->have_ipa_pod))
-      return fail(e, BS_E_STATE, "bs_evaluate: a non-zero InterPodAffinity weight needs the node and pod inter-pod sides");
-    if (e->ipa_term_max >= (int64_t)e->ipa_terms)
-      return fail(e, BS_E_INDEX, "bs_evaluate: a pod class's term is outside the node side's term dictionary");
-    // the pod side outlives node uploads: its class x node table is checked against the node table of now
-    if ((uint64_t)e->ipa_pclasses * e->Npad * 8 > BS_IPA_TABLE_MAX_BYTES)
-      return fail(e, BS_E_INVAL, "bs_evaluate: pod n_classes x padded nodes x 8 bytes exceeds BS_IPA_TABLE_MAX_BYTES");
-  }
-  if (e->ipf_on && (rc = interpod_filter_check(e, "bs_evaluate"))) return rc;
+  if ((e->out_flags & BS_OUT_PRIORITY) &&
+      ((rc = nonzero_check(e, "bs_evaluate")) || (rc = preference_check(e, "bs_evaluate")) ||
+       (rc = locality_check(e, "bs_evaluate")) || (rc = spread_check(e, "bs_evaluate")) ||
+       (rc = interpod_check(e, "bs_evaluate"))))
+    return rc;
+  if (e->ipf.on && (rc = interpod_filter_check(e, "bs_evaluate"))) return rc;
   if (e->peer_broken)
     return fail(e, BS_E_PEER, "peer exchange is broken (a rank did not arrive): bs_peer_detach on every rank, then init/attach again");
   BS_DEVICE_GUARD(e);
@@ -1398,7 +1466,7 @@ int evaluate_async_locked(bs_engine* e) {
   }
   if ((rc = ensure_round_buffers(e))) return rc;
   for (int k = 0; k < BS_K_COUNT; ++k) e->k_valid[k] = false;
-  if (e->ipf_on && e->ipf_dirty) {   // new pass bits: the class fit bits and gates are built again
+  if (e->ipf.on && e->ipf.dirty) {   // new pass bits: the class fit bits and gates are built again
     if ((rc = interpod_filter_prepass(e))) return rc;
     reprepare = true;
   }
@@ -1621,11 +1689,11 @@ int evaluate_async_locked(bs_engine* e) {
       ra.fit_class = e->d_pod_fit_class.as<uint32_t>();
       ra.rows = e->d_reasons.as<uint32_t>();
       ra.P = P; ra.N = e->N; ra.Npad = e->Npad; ra.Wg = e->Npad / 32; ra.L = L;
-      ra.cipf = e->d_fipf.as<uint32_t>();
-      ra.ipf_bits = e->d_ipf_bits.as<uint32_t>();
-      ra.n_ipf = e->ipf_pclasses;
-      ra.ipf_rows = e->d_ipf_reasons.as<uint32_t>();
-      if (e->ipf_on) reason_pod_kernel<true><<<cdiv(P, REASON_PODS_PER_CTA), REASON_THREADS, 0, e->s>>>(ra);
+      ra.cipf = e->ipf.d_fipf.as<uint32_t>();
+      ra.ipf_bits = e->ipf.d_bits.as<uint32_t>();
+      ra.n_ipf = e->ipf.pclasses;
+      ra.ipf_rows = e->ipf.d_reasons.as<uint32_t>();
+      if (e->ipf.on) reason_pod_kernel<true><<<cdiv(P, REASON_PODS_PER_CTA), REASON_THREADS, 0, e->s>>>(ra);
       else reason_pod_kernel<false><<<cdiv(P, REASON_PODS_PER_CTA), REASON_THREADS, 0, e->s>>>(ra);
       tm.launched();
     }
@@ -1634,13 +1702,13 @@ int evaluate_async_locked(bs_engine* e) {
     PriorityRatioArgs pa;
     pa.left = e->d_left_full.as<int64_t>();
     pa.left_present = e->d_left_present.as<uint32_t>();
-    pa.gate = e->ipf_on ? e->d_reason_gate_ipf.as<uint32_t>() : e->d_reason_gate.as<uint32_t>();
+    pa.gate = e->ipf.on ? e->ipf.d_reason_gate.as<uint32_t>() : e->d_reason_gate.as<uint32_t>();
     pa.req = e->d_req.as<int64_t>();
     pa.req_present = e->d_ppres.as<uint32_t>();
     pa.fit_class = e->d_pod_fit_class.as<uint32_t>();
     pa.alloc = e->d_alloc.as<int64_t>();
-    pa.node_nz = e->d_nz_node.as<int64_t>();
-    pa.pod_nz = e->d_nz_pod.as<int64_t>();
+    pa.node_nz = e->nz.d_node.as<int64_t>();
+    pa.pod_nz = e->nz.d_pod.as<int64_t>();
     pa.out_node = e->d_prio_node.as<int32_t>();
     pa.out_score = e->d_prio_score.as<int64_t>();
     pa.w = e->weights;
@@ -1652,32 +1720,32 @@ int evaluate_async_locked(bs_engine* e) {
     const uint32_t grid = cdiv(P, PRIO_PODS_PER_CTA);
     PriorityIpaArgs la;
     static_cast<PriorityRatioArgs&>(la) = pa;
-    la.prefer_taints = e->d_prefer_taints.as<uint64_t>();
-    la.pref_weights = e->d_pref_weights.as<int32_t>();
-    la.prefer_tol = e->d_prefer_tol.as<uint64_t>();
-    la.pref_class = e->d_pref_class.as<uint32_t>();
+    la.prefer_taints = e->pref.d_prefer_taints.as<uint64_t>();
+    la.pref_weights = e->pref.d_weights.as<int32_t>();
+    la.prefer_tol = e->pref.d_prefer_tol.as<uint64_t>();
+    la.pref_class = e->pref.d_class.as<uint32_t>();
     la.w_taint = e->w_taint;
     la.w_naff = e->w_naff;
     const bool pref = e->w_taint || e->w_naff, ratio = e->ratio.weight != 0;
     if (e->w_img || e->w_avoid) {   // (the pre-pass runs on the same stream, ahead of the kernel)
       if ((rc = locality_prepass(e))) return rc;
-      la.il = e->d_loc_il.as<uint8_t>();
-      la.avoid_mask = e->d_avoid_mask.as<uint64_t>();
-      la.loc_class = e->d_loc_class.as<uint32_t>();
-      la.avoid_bit = e->d_avoid_bit.as<uint8_t>();
+      la.il = e->loc.d_il.as<uint8_t>();
+      la.avoid_mask = e->loc.d_avoid_mask.as<uint64_t>();
+      la.loc_class = e->loc.d_class.as<uint32_t>();
+      la.avoid_bit = e->loc.d_avoid_bit.as<uint8_t>();
       la.w_img = e->w_img;
       la.w_avoid = e->w_avoid;
     }
     if (e->w_spread) {
-      la.spread_zone = e->d_spread_zone.as<uint8_t>();
-      la.spread_counts = e->d_spread_counts.as<int32_t>();
-      la.spread_class = e->d_spread_class.as<uint32_t>();
+      la.spread_zone = e->spread.d_zone.as<uint8_t>();
+      la.spread_counts = e->spread.d_counts.as<int32_t>();
+      la.spread_class = e->spread.d_class.as<uint32_t>();
       la.w_spread = e->w_spread;
     }
     if (e->w_ipa) {   // (the pre-pass runs on the same stream, ahead of the kernel)
       if ((rc = interpod_prepass(e))) return rc;
-      la.ipa_raw = e->d_ipa_raw.as<int64_t>();
-      la.ipa_class = e->d_ipa_class.as<uint32_t>();
+      la.ipa_raw = e->ipa.d_raw.as<int64_t>();
+      la.ipa_class = e->ipa.d_class.as<uint32_t>();
       la.w_ipa = e->w_ipa;
     }
     CK(launch_priority(L, grid, ratio, pref, e->w_img || e->w_avoid, e->w_spread != 0, e->w_ipa != 0, la, e->s));
@@ -1710,7 +1778,7 @@ int evaluate_async_locked(bs_engine* e) {
   }
   CK(cudaStreamWaitEvent(e->s, e->ev_join, 0));
   CK(cudaGetLastError());
-  e->ipf_round = e->ipf_on;
+  e->ipf.round = e->ipf.on;
   e->evaluated = true;
   e->fetched = false;
   e->gang_applied = false;
@@ -1907,12 +1975,7 @@ void bs_destroy(bs_engine* e) {
 int bs_upload_nodes(bs_engine* e, const bs_node_table* t) {
   if (!e || !t) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
-  e->have_nz_node = false;   // the non-zero column belongs to the node snapshot
-  e->have_pref_node = false;   // and so do the PreferNoSchedule masks and the preferred-affinity table
-  e->have_img_node = e->have_avoid_node = false;   // and the image rows and preferAvoidPods masks
-  e->have_spread_node = false;   // and the zones and selector counts (counts change when pods bind)
-  e->have_ipa_node = false;   // and the topology values and bound pods of InterPodAffinity
-  e->have_ipf_node = false;   // and those of the MatchInterPodAffinity filter
+  drop_node_sides(e);
   if (t->n_lanes != e->L) return fail(e, BS_E_INVAL, "bs_upload_nodes: n_lanes differs from the engine's");
   const uint32_t N = t->n_nodes, L = e->L;
   const auto cols = node_cols(e, t);
@@ -1955,12 +2018,7 @@ int bs_update_nodes(bs_engine* e, const uint32_t* idx, const bs_node_table* t) {
   if (!e || !t || (t->n_nodes && !idx)) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
   if (!e->have_nodes) return fail(e, BS_E_STATE, "bs_update_nodes: upload nodes first");
-  e->have_nz_node = false;   // the changed rows' non-zero requests come with a new column
-  e->have_pref_node = false;   // ... and so do their taints and labels: the node preference side is uploaded again
-  e->have_img_node = e->have_avoid_node = false;   // ... and their images and annotations: so is the locality side
-  e->have_spread_node = false;   // ... and the pods on them and their zone labels: so is the spread side
-  e->have_ipa_node = false;   // ... and the inter-pod side, for the same reasons
-  e->have_ipf_node = false;   // ... and the filter's
+  drop_node_sides(e);   // the changed rows come with new side columns
   if (t->n_lanes != e->L) return fail(e, BS_E_INVAL, "bs_update_nodes: n_lanes differs from the engine's");
   const uint32_t n = t->n_nodes, L = e->L;
   if (!n) return BS_OK;
@@ -2091,14 +2149,9 @@ int bs_update_groups(bs_engine* e, const uint32_t* idx, const bs_group_table* t)
 int bs_upload_pods(bs_engine* e, const bs_pod_table* t) {
   if (!e || !t) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
-  e->have_nz_pod = false;   // the non-zero column belongs to the pod table
-  e->have_pref_pod = false;   // and so does the pod preference side
-  e->have_img_pod = e->have_avoid_pod = false;   // and the pod locality side
-  e->have_spread_pod = false;   // and the pod spread side
-  e->have_ipa_pod = false;   // and the pod inter-pod side
-  e->have_ipf_pod = false;   // and the filter's pod side; the new table's fit classes are its base classes
-  e->pfc_base_valid = false;
-  e->ipf_assign_dirty = false;
+  drop_pod_sides(e);
+  e->ipf.pfc_base_valid = false;   // the new table's fit classes are its base classes
+  e->ipf.assign_dirty = false;
   if (t->n_lanes != e->L) return fail(e, BS_E_INVAL, "bs_upload_pods: n_lanes differs from the engine's");
   const uint32_t P = t->n_pods, L = e->L;
   if (P && (!t->req || !t->req_present || !t->gid || !t->sel_mask || !t->tol_mask || !t->priority ||
@@ -2702,7 +2755,7 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
   const std::string w(who);
   if (!e->have_nodes || !e->have_pods || !e->have_groups)
     return fail(e, BS_E_STATE, (w + ": upload nodes, groups and pods first").c_str());
-  if (scored && !(e->have_nz_node && e->have_nz_pod))
+  if (scored && !(e->nz.have_node && e->nz.have_pod))
     return fail(e, BS_E_STATE, (w + ": upload both non-zero request columns first").c_str());
   const bool loc = scored && (e->w_img || e->w_avoid);
   int rc;
@@ -2716,7 +2769,7 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
       if (queue[i] >= P) return fail(e, BS_E_INDEX, (w + ": queue entry is not a pod of the table").c_str());
   // the live non-zero sums: at most the node column's maximum plus every queued pod's
   for (int r = 0; r < 2 && scored; ++r)
-    if ((long double)e->nz_node_max[r] + (long double)n_queue * (long double)e->nz_pod_max[r] > 0x1p62L)
+    if ((long double)e->nz.node_max[r] + (long double)n_queue * (long double)e->nz.pod_max[r] > 0x1p62L)
       return fail(e, BS_E_RANGE, (w + ": live non-zero requests could pass 2^62").c_str());
   if (e->classes_dirty && (rc = rebuild_classes(e))) return rc;
   if (loc && (rc = locality_prepass(e))) return rc;
@@ -2760,7 +2813,7 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
   CK(dup(s_grc, e->d_group_rep_class, (size_t)G * 4));
   CK(dup(s_minres, e->d_min_res, (size_t)L * G * 8));
   CK(dup(s_mrp, e->d_mrpres, (size_t)G * 4));
-  if (scored) CK(dup(n_nz, e->d_nz_node, (size_t)2 * Npad * 8));
+  if (scored) CK(dup(n_nz, e->nz.d_node, (size_t)2 * Npad * 8));
   if (queue && n_queue) CK(cudaMemcpyAsync(d_queue.p, queue, (size_t)n_queue * 4, cudaMemcpyHostToDevice, e->s));
   CK(cudaMemsetAsync(d_status.p, 0, 128, e->s));
   ReplayLocArgs la{};
@@ -2804,15 +2857,15 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
   a.status = d_status.as<int32_t>();
   if (scored) {
     a.nz_live = n_nz.as<int64_t>();
-    a.pod_nz = e->d_nz_pod.as<int64_t>();
+    a.pod_nz = e->nz.d_pod.as<int64_t>();
     a.w = e->weights;
     a.ratio = e->ratio;
   }
   if (loc) {
-    la.il = e->d_loc_il.as<uint8_t>();
-    la.avoid_mask = e->d_avoid_mask.as<uint64_t>();
-    la.loc_class = e->d_loc_class.as<uint32_t>();
-    la.avoid_bit = e->d_avoid_bit.as<uint8_t>();
+    la.il = e->loc.d_il.as<uint8_t>();
+    la.avoid_mask = e->loc.d_avoid_mask.as<uint64_t>();
+    la.loc_class = e->loc.d_class.as<uint32_t>();
+    la.avoid_bit = e->loc.d_avoid_bit.as<uint8_t>();
     la.w_img = e->w_img;
     la.w_avoid = e->w_avoid;
   }
@@ -2874,7 +2927,7 @@ static int interpod_filter_refuse(bs_engine* e, const char* who) {
 int bs_replay(bs_engine* e, const uint32_t* queue, uint32_t n_queue, bs_replay_result* out) {
   if (!e || !out) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
-  if (e->ipf_on) return interpod_filter_refuse(e, "bs_replay");
+  if (e->ipf.on) return interpod_filter_refuse(e, "bs_replay");
   return replay_walk(e, "bs_replay", queue, n_queue, out, false, nullptr);
 }
 
@@ -2882,7 +2935,7 @@ int bs_replay_priority(bs_engine* e, const uint32_t* queue, uint32_t n_queue, bs
                        int64_t* node_nonzero_after) {
   if (!e || !out) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
-  if (e->ipf_on) return interpod_filter_refuse(e, "bs_replay_priority");
+  if (e->ipf.on) return interpod_filter_refuse(e, "bs_replay_priority");
   if (e->w_taint || e->w_naff)   // their maxima would have to follow the walk's live fit set, which is not built yet
     return fail(e, BS_E_INVAL, "bs_replay_priority: TaintToleration and NodeAffinity are not supported in the walk; "
                                "set both weights of bs_set_node_priority_weights to 0");
@@ -3060,7 +3113,7 @@ int bs_preempt(bs_engine* e, const uint32_t* pods, uint32_t n, bs_preempt_result
   if (!e || !out || (n && (!pods || !out->node || !out->n_victims || !out->n_candidates)) || !out->victim_offset)
     return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
-  if (e->ipf_on) return interpod_filter_refuse(e, "bs_preempt");
+  if (e->ipf.on) return interpod_filter_refuse(e, "bs_preempt");
   std::vector<PreemptPod> pp;
   int rc;
   if ((rc = preempt_pods(e, "bs_preempt", pods, n, pp))) return rc;
@@ -3129,7 +3182,7 @@ int bs_preempt_walk(bs_engine* e, const uint32_t* pods, uint32_t n, uint32_t fla
   if (!e || !out || (n && (!pods || !out->node || !out->n_victims || !out->n_candidates)) || !out->victim_offset)
     return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
-  if (e->ipf_on) return interpod_filter_refuse(e, "bs_preempt_walk");
+  if (e->ipf.on) return interpod_filter_refuse(e, "bs_preempt_walk");
   if (flags & ~BS_PREEMPT_GANG) return fail(e, BS_E_INVAL, "bs_preempt_walk: unknown flag bits");
   const bool gang = flags & BS_PREEMPT_GANG;
   std::vector<PreemptPod> pp;
@@ -3512,12 +3565,17 @@ int bs_set_ratio_priority(bs_engine* e, uint32_t weight, uint32_t n_points, cons
 }
 
 namespace {
-// One non-zero column [2][n] into dst ([2][pitch], zero beyond n).  The caller has dropped the column already; it is
-// marked present only when every value lies in [0, BS_NONZERO_MAX].  mx gets each row's maximum (bs_replay_priority's
-// overflow bound).
-int upload_nonzero(bs_engine* e, DevBuf& dst, uint32_t n, uint32_t pitch, const int64_t* nz, const char* who,
-                   int64_t (&mx)[2]) {
-  if (n && !nz) return fail(e, BS_E_INVAL, who);
+// One non-zero column [2][n] (the node or the pod half) into its device column ([2][pitch], zero beyond n), marked
+// present only when every value lies in [0, BS_NONZERO_MAX].  Its maxima go to node_max / pod_max
+// (bs_replay_priority's overflow bound).
+int upload_nonzero(bs_engine* e, SideOf side, uint32_t n, const int64_t* nz) {
+  const bool node = side == NODE_SIDE;
+  const Refuse bad{e, node ? "bs_upload_node_nonzero" : "bs_upload_pod_nonzero"};
+  bool& have = node ? e->nz.have_node : e->nz.have_pod;
+  int64_t(&mx)[2] = node ? e->nz.node_max : e->nz.pod_max;
+  have = false;
+  if (int rc = bad.shape(side, n)) return rc;
+  if (n && !nz) return bad(BS_E_INVAL, "null column");
   mx[0] = mx[1] = 0;
   for (size_t k = 0; k < (size_t)2 * n; ++k) {
     if (nz[k] < 0 || nz[k] > BS_NONZERO_MAX) return fail(e, BS_E_RANGE, "non-zero request outside [0, 2^56]");
@@ -3525,11 +3583,9 @@ int upload_nonzero(bs_engine* e, DevBuf& dst, uint32_t n, uint32_t pitch, const 
     m = std::max(m, nz[k]);
   }
   BS_DEVICE_GUARD(e);
-  CK(dst.ensure((size_t)2 * std::max(pitch, 1u) * 8));
-  if (pitch > n) CK(cudaMemsetAsync(dst.p, 0, (size_t)2 * pitch * 8, e->s));
-  if (n)
-    CK(cudaMemcpy2DAsync(dst.p, (size_t)pitch * 8, nz, (size_t)n * 8, (size_t)n * 8, 2, cudaMemcpyHostToDevice, e->s));
+  if (int rc = upload_col(e, col(nz, node ? e->nz.d_node : e->nz.d_pod, 2), n, node ? e->Npad : n)) return rc;
   CK(cudaStreamSynchronize(e->s));
+  have = true;
   return BS_OK;
 }
 }  // namespace
@@ -3537,25 +3593,13 @@ int upload_nonzero(bs_engine* e, DevBuf& dst, uint32_t n, uint32_t pitch, const 
 int bs_upload_node_nonzero(bs_engine* e, uint32_t n_nodes, const int64_t* nz) {
   if (!e) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
-  e->have_nz_node = false;
-  if (!e->have_nodes) return fail(e, BS_E_STATE, "bs_upload_node_nonzero: upload nodes first");
-  if (n_nodes != e->N) return fail(e, BS_E_INVAL, "bs_upload_node_nonzero: n_nodes differs from the node table's");
-  const int rc = upload_nonzero(e, e->d_nz_node, n_nodes, e->Npad, nz, "bs_upload_node_nonzero: null column",
-                                e->nz_node_max);
-  e->have_nz_node = rc == BS_OK;
-  return rc;
+  return upload_nonzero(e, NODE_SIDE, n_nodes, nz);
 }
 
 int bs_upload_pod_nonzero(bs_engine* e, uint32_t n_pods, const int64_t* nz) {
   if (!e) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
-  e->have_nz_pod = false;
-  if (!e->have_pods) return fail(e, BS_E_STATE, "bs_upload_pod_nonzero: upload pods first");
-  if (n_pods != e->P) return fail(e, BS_E_INVAL, "bs_upload_pod_nonzero: n_pods differs from the pod table's");
-  const int rc = upload_nonzero(e, e->d_nz_pod, n_pods, n_pods, nz, "bs_upload_pod_nonzero: null column",
-                                e->nz_pod_max);
-  e->have_nz_pod = rc == BS_OK;
-  return rc;
+  return upload_nonzero(e, POD_SIDE, n_pods, nz);
 }
 
 int bs_set_node_priority_weights(bs_engine* e, uint32_t taint_toleration, uint32_t node_affinity) {
@@ -3570,11 +3614,9 @@ int bs_upload_node_preferences(bs_engine* e, uint32_t n_nodes, const uint64_t* p
                                const int32_t* pref_weights) {
   if (!e) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
-  const char* who = "bs_upload_node_preferences";
-  auto bad = [&](int rc, const char* why) { return fail(e, rc, (std::string(who) + ": " + why).c_str()); };
-  e->have_pref_node = false;
-  if (!e->have_nodes) return bad(BS_E_STATE, "upload nodes first");
-  if (n_nodes != e->N) return bad(BS_E_INVAL, "n_nodes differs from the node table's");
+  const Refuse bad{e, "bs_upload_node_preferences"};
+  e->pref.have_node = false;
+  if (int rc = bad.shape(NODE_SIDE, n_nodes)) return rc;
   const uint32_t Npad = e->Npad;
   if ((uint64_t)n_classes * Npad * 4 > BS_PREF_TABLE_MAX_BYTES)
     return bad(BS_E_INVAL, "n_classes x padded nodes x 4 bytes exceeds BS_PREF_TABLE_MAX_BYTES");
@@ -3583,51 +3625,37 @@ int bs_upload_node_preferences(bs_engine* e, uint32_t n_nodes, const uint64_t* p
   for (size_t k = 0; k < (size_t)n_classes * n_nodes; ++k)
     if (pref_weights[k] < 0) return bad(BS_E_RANGE, "a preferred-affinity weight is negative");
   BS_DEVICE_GUARD(e);
-  CK(e->d_prefer_taints.ensure((size_t)std::max(Npad, 1u) * 8));
-  CK(cudaMemsetAsync(e->d_prefer_taints.p, 0, (size_t)Npad * 8, e->s));
-  if (n_nodes) CK(cudaMemcpyAsync(e->d_prefer_taints.p, prefer_taints, (size_t)n_nodes * 8, cudaMemcpyHostToDevice, e->s));
-  if (n_classes) {
-    CK(e->d_pref_weights.ensure((size_t)n_classes * Npad * 4));
-    CK(cudaMemsetAsync(e->d_pref_weights.p, 0, (size_t)n_classes * Npad * 4, e->s));
-    if (n_nodes)
-      CK(cudaMemcpy2DAsync(e->d_pref_weights.p, (size_t)Npad * 4, pref_weights, (size_t)n_nodes * 4, (size_t)n_nodes * 4,
-                           n_classes, cudaMemcpyHostToDevice, e->s));
-  }
+  int rc;
+  if ((rc = upload_vec(e, e->pref.d_prefer_taints, prefer_taints, n_nodes, Npad))) return rc;
+  if (n_classes && (rc = upload_col(e, col(pref_weights, e->pref.d_weights, n_classes), n_nodes, Npad))) return rc;
   CK(cudaStreamSynchronize(e->s));
-  e->pref_classes = n_classes;
-  e->have_pref_node = true;
+  e->pref.classes = n_classes;
+  e->pref.have_node = true;
   return BS_OK;
 }
 
 int bs_upload_pod_preferences(bs_engine* e, uint32_t n_pods, const uint64_t* prefer_tol, const uint32_t* pref_class) {
   if (!e) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
-  const char* who = "bs_upload_pod_preferences";
-  auto bad = [&](int rc, const char* why) { return fail(e, rc, (std::string(who) + ": " + why).c_str()); };
-  e->have_pref_pod = false;
-  if (!e->have_pods) return bad(BS_E_STATE, "upload pods first");
-  if (n_pods != e->P) return bad(BS_E_INVAL, "n_pods differs from the pod table's");
+  const Refuse bad{e, "bs_upload_pod_preferences"};
+  e->pref.have_pod = false;
+  if (int rc = bad.shape(POD_SIDE, n_pods)) return rc;
   if (n_pods && (!prefer_tol || !pref_class)) return bad(BS_E_INVAL, "null column");
-  int64_t mx = -1;
-  for (uint32_t p = 0; p < n_pods; ++p)
-    if (pref_class[p] != BS_PREF_NONE) mx = std::max(mx, (int64_t)pref_class[p]);
+  const int64_t mx = max_class(pref_class, n_pods, BS_PREF_NONE);
   BS_DEVICE_GUARD(e);
-  CK(e->d_prefer_tol.ensure((size_t)std::max(n_pods, 1u) * 8));
-  CK(e->d_pref_class.ensure((size_t)std::max(n_pods, 1u) * 4));
-  if (n_pods) {
-    CK(cudaMemcpyAsync(e->d_prefer_tol.p, prefer_tol, (size_t)n_pods * 8, cudaMemcpyHostToDevice, e->s));
-    CK(cudaMemcpyAsync(e->d_pref_class.p, pref_class, (size_t)n_pods * 4, cudaMemcpyHostToDevice, e->s));
-  }
+  int rc;
+  if ((rc = upload_vec(e, e->pref.d_prefer_tol, prefer_tol, n_pods, n_pods))) return rc;
+  if ((rc = upload_vec(e, e->pref.d_class, pref_class, n_pods, n_pods))) return rc;
   CK(cudaStreamSynchronize(e->s));
-  e->pref_class_max = mx;
-  e->have_pref_pod = true;
+  e->pref.class_max = mx;
+  e->pref.have_pod = true;
   return BS_OK;
 }
 
 int bs_set_locality_weights(bs_engine* e, uint32_t image_locality, uint32_t prefer_avoid_pods) {
   if (!e) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
-  if (image_locality != e->w_img || prefer_avoid_pods != e->w_avoid) e->loc_dirty = true;
+  if (image_locality != e->w_img || prefer_avoid_pods != e->w_avoid) e->loc.dirty = true;
   e->w_img = image_locality;
   e->w_avoid = prefer_avoid_pods;
   return BS_OK;
@@ -3637,12 +3665,10 @@ int bs_upload_node_locality(bs_engine* e, uint32_t n_nodes, uint32_t n_images, c
                             const uint32_t* image_bits, const uint64_t* avoid_mask) {
   if (!e) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
-  const char* who = "bs_upload_node_locality";
-  auto bad = [&](int rc, const char* why) { return fail(e, rc, (std::string(who) + ": " + why).c_str()); };
-  e->have_img_node = e->have_avoid_node = false;
-  e->loc_dirty = true;
-  if (!e->have_nodes) return bad(BS_E_STATE, "upload nodes first");
-  if (n_nodes != e->N) return bad(BS_E_INVAL, "n_nodes differs from the node table's");
+  const Refuse bad{e, "bs_upload_node_locality"};
+  e->loc.have_img_node = e->loc.have_avoid_node = false;
+  e->loc.dirty = true;
+  if (int rc = bad.shape(NODE_SIDE, n_nodes)) return rc;
   const uint32_t Npad = e->Npad, words = cdiv(n_nodes, 32);
   const bool img = image_size && image_bits;
   if (img && (uint64_t)n_images * words * 4 > BS_LOC_TABLE_MAX_BYTES)
@@ -3650,23 +3676,15 @@ int bs_upload_node_locality(bs_engine* e, uint32_t n_nodes, uint32_t n_images, c
   for (uint32_t i = 0; img && i < n_images; ++i)
     if (image_size[i] < 0 || image_size[i] > BS_IMAGE_SIZE_MAX) return bad(BS_E_RANGE, "an image size is outside [0, 2^48]");
   BS_DEVICE_GUARD(e);
-  if (img) {
-    CK(e->d_img_size.ensure((size_t)std::max(n_images, 1u) * 8));
-    CK(e->d_img_bits.ensure((size_t)std::max<uint64_t>((uint64_t)n_images * words, 1) * 4));
-    if (n_images) {
-      CK(cudaMemcpyAsync(e->d_img_size.p, image_size, (size_t)n_images * 8, cudaMemcpyHostToDevice, e->s));
-      if (words) CK(cudaMemcpyAsync(e->d_img_bits.p, image_bits, (size_t)n_images * words * 4, cudaMemcpyHostToDevice, e->s));
-    }
-  }
-  if (avoid_mask) {
-    CK(e->d_avoid_mask.ensure((size_t)std::max(Npad, 1u) * 8));
-    CK(cudaMemsetAsync(e->d_avoid_mask.p, 0, (size_t)Npad * 8, e->s));
-    if (n_nodes) CK(cudaMemcpyAsync(e->d_avoid_mask.p, avoid_mask, (size_t)n_nodes * 8, cudaMemcpyHostToDevice, e->s));
-  }
+  int rc;
+  if (img && (rc = upload_vec(e, e->loc.d_img_size, image_size, n_images, n_images))) return rc;
+  const uint64_t bits = (uint64_t)n_images * words;
+  if (img && (rc = upload_vec(e, e->loc.d_img_bits, image_bits, bits, bits))) return rc;
+  if (avoid_mask && (rc = upload_vec(e, e->loc.d_avoid_mask, avoid_mask, n_nodes, Npad))) return rc;
   CK(cudaStreamSynchronize(e->s));
-  e->loc_images = img ? n_images : 0;
-  e->have_img_node = img;
-  e->have_avoid_node = avoid_mask != nullptr;
+  e->loc.images = img ? n_images : 0;
+  e->loc.have_img_node = img;
+  e->loc.have_avoid_node = avoid_mask != nullptr;
   return BS_OK;
 }
 
@@ -3674,12 +3692,10 @@ int bs_upload_pod_locality(bs_engine* e, uint32_t n_pods, const uint32_t* image_
                            const uint32_t* class_offset, const uint32_t* class_images, const uint8_t* avoid_bit) {
   if (!e) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
-  const char* who = "bs_upload_pod_locality";
-  auto bad = [&](int rc, const char* why) { return fail(e, rc, (std::string(who) + ": " + why).c_str()); };
-  e->have_img_pod = e->have_avoid_pod = false;
-  e->loc_dirty = true;
-  if (!e->have_pods) return bad(BS_E_STATE, "upload pods first");
-  if (n_pods != e->P) return bad(BS_E_INVAL, "n_pods differs from the pod table's");
+  const Refuse bad{e, "bs_upload_pod_locality"};
+  e->loc.have_img_pod = e->loc.have_avoid_pod = false;
+  e->loc.dirty = true;
+  if (int rc = bad.shape(POD_SIDE, n_pods)) return rc;
   const bool img = image_class && class_offset && class_images;
   int64_t cmax = -1, imax = -1;
   uint32_t nnz = 0;
@@ -3692,30 +3708,23 @@ int bs_upload_pod_locality(bs_engine* e, uint32_t n_pods, const uint32_t* image_
         return bad(BS_E_INVAL, "class_offset is not ascending, or a class lists more than BS_LOC_CLASS_MAX ids");
     nnz = class_offset[n_classes];
     for (uint32_t k = 0; k < nnz; ++k) imax = std::max(imax, (int64_t)class_images[k]);
-    for (uint32_t p = 0; p < n_pods; ++p)
-      if (image_class[p] != BS_IMAGE_NONE) cmax = std::max(cmax, (int64_t)image_class[p]);
+    cmax = max_class(image_class, n_pods, BS_IMAGE_NONE);
   }
   for (uint32_t p = 0; avoid_bit && p < n_pods; ++p)
     if (avoid_bit[p] > 63 && avoid_bit[p] != BS_AVOID_NONE) return bad(BS_E_RANGE, "an avoid bit is outside 0..63");
   BS_DEVICE_GUARD(e);
-  if (img) {
-    CK(e->d_loc_class.ensure((size_t)std::max(n_pods, 1u) * 4));
-    CK(e->d_loc_off.ensure((size_t)(n_classes + 1) * 4));
-    CK(e->d_loc_ids.ensure((size_t)std::max(nnz, 1u) * 4));
-    if (n_pods) CK(cudaMemcpyAsync(e->d_loc_class.p, image_class, (size_t)n_pods * 4, cudaMemcpyHostToDevice, e->s));
-    CK(cudaMemcpyAsync(e->d_loc_off.p, class_offset, (size_t)(n_classes + 1) * 4, cudaMemcpyHostToDevice, e->s));
-    if (nnz) CK(cudaMemcpyAsync(e->d_loc_ids.p, class_images, (size_t)nnz * 4, cudaMemcpyHostToDevice, e->s));
-  }
-  if (avoid_bit) {
-    CK(e->d_avoid_bit.ensure(std::max(n_pods, 1u)));
-    if (n_pods) CK(cudaMemcpyAsync(e->d_avoid_bit.p, avoid_bit, n_pods, cudaMemcpyHostToDevice, e->s));
-  }
+  int rc;
+  if (img && ((rc = upload_vec(e, e->loc.d_class, image_class, n_pods, n_pods)) ||
+              (rc = upload_vec(e, e->loc.d_off, class_offset, n_classes + 1, n_classes + 1)) ||
+              (rc = upload_vec(e, e->loc.d_ids, class_images, nnz, nnz))))
+    return rc;
+  if (avoid_bit && (rc = upload_vec(e, e->loc.d_avoid_bit, avoid_bit, n_pods, n_pods))) return rc;
   CK(cudaStreamSynchronize(e->s));
-  e->loc_classes = img ? n_classes : 0;
-  e->loc_class_max = cmax;
-  e->loc_image_max = imax;
-  e->have_img_pod = img;
-  e->have_avoid_pod = avoid_bit != nullptr;
+  e->loc.classes = img ? n_classes : 0;
+  e->loc.class_max = cmax;
+  e->loc.image_max = imax;
+  e->loc.have_img_pod = img;
+  e->loc.have_avoid_pod = avoid_bit != nullptr;
   return BS_OK;
 }
 
@@ -3730,11 +3739,9 @@ int bs_upload_node_spread(bs_engine* e, uint32_t n_nodes, uint32_t n_zones, cons
                           const int32_t* counts) {
   if (!e) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
-  const char* who = "bs_upload_node_spread";
-  auto bad = [&](int rc, const char* why) { return fail(e, rc, (std::string(who) + ": " + why).c_str()); };
-  e->have_spread_node = false;
-  if (!e->have_nodes) return bad(BS_E_STATE, "upload nodes first");
-  if (n_nodes != e->N) return bad(BS_E_INVAL, "n_nodes differs from the node table's");
+  const Refuse bad{e, "bs_upload_node_spread"};
+  e->spread.have_node = false;
+  if (int rc = bad.shape(NODE_SIDE, n_nodes)) return rc;
   if (n_zones > BS_SPREAD_ZONE_MAX) return bad(BS_E_INVAL, "n_zones exceeds BS_SPREAD_ZONE_MAX");
   const uint32_t Npad = e->Npad;
   if ((uint64_t)n_classes * Npad * 4 > BS_SPREAD_TABLE_MAX_BYTES)
@@ -3746,40 +3753,29 @@ int bs_upload_node_spread(bs_engine* e, uint32_t n_nodes, uint32_t n_zones, cons
   for (size_t k = 0; k < (size_t)n_classes * n_nodes; ++k)
     if (counts[k] < 0 || counts[k] > BS_SPREAD_COUNT_MAX) return bad(BS_E_RANGE, "a count is outside [0, 2^24]");
   BS_DEVICE_GUARD(e);
-  CK(e->d_spread_zone.ensure(std::max(Npad, 1u)));
-  CK(cudaMemsetAsync(e->d_spread_zone.p, BS_ZONE_NONE, Npad, e->s));   // padding nodes have no zone (and never fit)
-  if (n_nodes) CK(cudaMemcpyAsync(e->d_spread_zone.p, zone, n_nodes, cudaMemcpyHostToDevice, e->s));
-  if (n_classes) {
-    CK(e->d_spread_counts.ensure((size_t)n_classes * Npad * 4));
-    CK(cudaMemsetAsync(e->d_spread_counts.p, 0, (size_t)n_classes * Npad * 4, e->s));
-    if (n_nodes)
-      CK(cudaMemcpy2DAsync(e->d_spread_counts.p, (size_t)Npad * 4, counts, (size_t)n_nodes * 4, (size_t)n_nodes * 4,
-                           n_classes, cudaMemcpyHostToDevice, e->s));
-  }
+  int rc;
+  // padding nodes have no zone (and never fit)
+  if ((rc = upload_vec(e, e->spread.d_zone, zone, n_nodes, Npad, BS_ZONE_NONE))) return rc;
+  if (n_classes && (rc = upload_col(e, col(counts, e->spread.d_counts, n_classes), n_nodes, Npad))) return rc;
   CK(cudaStreamSynchronize(e->s));
-  e->spread_classes = n_classes;
-  e->have_spread_node = true;
+  e->spread.classes = n_classes;
+  e->spread.have_node = true;
   return BS_OK;
 }
 
 int bs_upload_pod_spread(bs_engine* e, uint32_t n_pods, const uint32_t* spread_class) {
   if (!e) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
-  const char* who = "bs_upload_pod_spread";
-  auto bad = [&](int rc, const char* why) { return fail(e, rc, (std::string(who) + ": " + why).c_str()); };
-  e->have_spread_pod = false;
-  if (!e->have_pods) return bad(BS_E_STATE, "upload pods first");
-  if (n_pods != e->P) return bad(BS_E_INVAL, "n_pods differs from the pod table's");
+  const Refuse bad{e, "bs_upload_pod_spread"};
+  e->spread.have_pod = false;
+  if (int rc = bad.shape(POD_SIDE, n_pods)) return rc;
   if (n_pods && !spread_class) return bad(BS_E_INVAL, "null spread_class");
-  int64_t mx = -1;
-  for (uint32_t p = 0; p < n_pods; ++p)
-    if (spread_class[p] != BS_SPREAD_NONE) mx = std::max(mx, (int64_t)spread_class[p]);
+  const int64_t mx = max_class(spread_class, n_pods, BS_SPREAD_NONE);
   BS_DEVICE_GUARD(e);
-  CK(e->d_spread_class.ensure((size_t)std::max(n_pods, 1u) * 4));
-  if (n_pods) CK(cudaMemcpyAsync(e->d_spread_class.p, spread_class, (size_t)n_pods * 4, cudaMemcpyHostToDevice, e->s));
+  if (int rc = upload_vec(e, e->spread.d_class, spread_class, n_pods, n_pods)) return rc;
   CK(cudaStreamSynchronize(e->s));
-  e->spread_class_max = mx;
-  e->have_spread_pod = true;
+  e->spread.class_max = mx;
+  e->spread.have_pod = true;
   return BS_OK;
 }
 
@@ -3819,21 +3815,78 @@ int interpod_classes_check(const bs_interpod_classes& c, uint32_t n_terms, int64
   return BS_OK;
 }
 
-// Device copies of a checked class table.
+// Device copies of a checked class table (an offset 0 alone for an empty one).
 int interpod_classes_upload(bs_engine* e, const bs_interpod_classes& c, DevBuf& off, DevBuf& term, DevBuf& own,
                             DevBuf& match) {
   const uint32_t nnz = c.n_classes ? c.class_offset[c.n_classes] : 0;
-  CK(off.ensure((size_t)(c.n_classes + 1) * 4));
-  CK(term.ensure((size_t)std::max(nnz, 1u) * 4));
-  CK(own.ensure((size_t)std::max(nnz, 1u) * 4));
-  CK(match.ensure(std::max(nnz, 1u)));
-  if (c.n_classes) CK(cudaMemcpyAsync(off.p, c.class_offset, (size_t)(c.n_classes + 1) * 4, cudaMemcpyHostToDevice, e->s));
-  else CK(cudaMemsetAsync(off.p, 0, 4, e->s));
-  if (nnz) {
-    CK(cudaMemcpyAsync(term.p, c.term, (size_t)nnz * 4, cudaMemcpyHostToDevice, e->s));
-    CK(cudaMemcpyAsync(own.p, c.own, (size_t)nnz * 4, cudaMemcpyHostToDevice, e->s));
-    CK(cudaMemcpyAsync(match.p, c.match, nnz, cudaMemcpyHostToDevice, e->s));
+  int rc;
+  if ((rc = upload_vec(e, off, c.class_offset, c.n_classes ? c.n_classes + 1 : 0, c.n_classes + 1)) ||
+      (rc = upload_vec(e, term, c.term, nnz, nnz)) || (rc = upload_vec(e, own, c.own, nnz, nnz)) ||
+      (rc = upload_vec(e, match, c.match, nnz, nnz)))
+    return rc;
+  return BS_OK;
+}
+
+// What the node sides of InterPodAffinity and of the MatchInterPodAffinity filter differ in.
+struct InterpodLimits {
+  uint32_t bound_max;   // bound pods at most
+  uint32_t none;        // the class of a bound pod without entries
+  bool planes;          // the slots are the filter's two presence bit planes, not the priority's 16-byte M and S
+  bool own_01;          // every own is 0 or 1 (the filter's anti-affinity flag)
+  const char *bound_why, *slots_why;
+};
+constexpr InterpodLimits IPA_LIMITS{BS_IPA_BOUND_MAX, BS_IPA_NONE, false, false, "n_bound exceeds BS_IPA_BOUND_MAX",
+                                    "the term tables exceed BS_IPA_TERM_MAX_BYTES"};
+constexpr InterpodLimits IPF_LIMITS{BS_IPF_BOUND_MAX, BS_IPF_NONE, true, true, "n_bound exceeds BS_IPF_BOUND_MAX",
+                                    "the presence planes exceed BS_IPF_TERM_MAX_BYTES"};
+
+// Checks a bs_interpod_nodes table against the node table and `lim`, and copies it into s.  The caller has dropped
+// the side already.
+int upload_interpod_nodes(bs_engine* e, const Refuse& bad, const bs_interpod_nodes* t, const InterpodLimits& lim,
+                          InterpodNodeSide& s) {
+  if (!t) return bad(BS_E_INVAL, "null table");
+  if (int rc = bad.shape(NODE_SIDE, t->n_nodes)) return rc;
+  const uint32_t N = t->n_nodes, K = t->n_keys, T = t->n_terms, V = t->n_bound;
+  if (K > BS_IPA_KEY_MAX) return bad(BS_E_INVAL, "n_keys exceeds BS_IPA_KEY_MAX");
+  if (V > lim.bound_max) return bad(BS_E_INVAL, lim.bound_why);
+  if ((K && !t->n_values) || (K && N && !t->topo) || (T && !t->term_key) || (V && !(t->bound_node && t->bound_class)))
+    return bad(BS_E_INVAL, "null column");
+  for (size_t k = 0; k < (size_t)K * N; ++k)
+    if (t->topo[k] != BS_TOPO_NONE && t->topo[k] >= t->n_values[k / N]) return bad(BS_E_INDEX, "a topo value is >= n_values");
+  std::vector<uint32_t> off(T);
+  uint64_t slots = 0;
+  for (uint32_t k = 0; k < T; ++k) {
+    if (t->term_key[k] >= K) return bad(BS_E_INDEX, "a term_key is >= n_keys");
+    off[k] = lim.planes ? (uint32_t)slots : (uint32_t)std::min<uint64_t>(slots, UINT32_MAX);
+    slots += t->n_values[t->term_key[k]];
+    if (lim.planes ? (slots + 31) / 32 * 2 * 4 > BS_IPF_TERM_MAX_BYTES : slots * 16 > BS_IPA_TERM_MAX_BYTES)
+      return bad(BS_E_INVAL, lim.slots_why);
   }
+  for (uint32_t k = 0; k < V; ++k) {
+    if (t->bound_node[k] >= N) return bad(BS_E_INDEX, "a bound_node is >= n_nodes");
+    if (t->bound_class[k] != lim.none && t->bound_class[k] >= t->classes.n_classes)
+      return bad(BS_E_INDEX, "a bound_class is >= n_classes");
+  }
+  int64_t tmax;
+  const char* why = nullptr;
+  if (int rc = interpod_classes_check(t->classes, T, tmax, why)) return bad(rc, why);
+  const uint32_t nnz = t->classes.n_classes ? t->classes.class_offset[t->classes.n_classes] : 0;
+  for (uint32_t k = 0; lim.own_01 && k < nnz; ++k)
+    if (t->classes.own[k] != 0 && t->classes.own[k] != 1) return bad(BS_E_RANGE, "an own is not 0 or 1");
+  BS_DEVICE_GUARD(e);
+  const uint64_t KN = (uint64_t)K * N;
+  int rc;
+  if ((rc = upload_vec(e, s.d_topo, t->topo, KN, KN)) || (rc = upload_vec(e, s.d_term_key, t->term_key, T, T)) ||
+      (rc = upload_vec(e, s.d_term_off, off.data(), T, T)) ||
+      (rc = upload_vec(e, s.d_bound_node, t->bound_node, V, V)) ||
+      (rc = upload_vec(e, s.d_bound_class, t->bound_class, V, V)) ||
+      (rc = interpod_classes_upload(e, t->classes, s.d_boff, s.d_bterm, s.d_bown, s.d_bmatch)))
+    return rc;
+  CK(cudaStreamSynchronize(e->s));   // the caller's columns may go once the call returns
+  s.terms = T;
+  s.slots = slots;
+  s.bound = V;
+  s.bclasses = t->classes.n_classes;
   return BS_OK;
 }
 
@@ -3842,101 +3895,49 @@ int interpod_classes_upload(bs_engine* e, const bs_interpod_classes& c, DevBuf& 
 int bs_upload_node_interpod(bs_engine* e, const bs_interpod_nodes* t) {
   if (!e) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
-  const char* who = "bs_upload_node_interpod";
-  auto bad = [&](int rc, const char* why) { return fail(e, rc, (std::string(who) + ": " + why).c_str()); };
-  e->have_ipa_node = false;
-  e->ipa_dirty = e->ipa_mass_dirty = true;
-  if (!t) return bad(BS_E_INVAL, "null table");
-  if (!e->have_nodes) return bad(BS_E_STATE, "upload nodes first");
-  const uint32_t N = t->n_nodes, K = t->n_keys, T = t->n_terms, V = t->n_bound;
-  if (N != e->N) return bad(BS_E_INVAL, "n_nodes differs from the node table's");
-  if (K > BS_IPA_KEY_MAX) return bad(BS_E_INVAL, "n_keys exceeds BS_IPA_KEY_MAX");
-  if (V > BS_IPA_BOUND_MAX) return bad(BS_E_INVAL, "n_bound exceeds BS_IPA_BOUND_MAX");
-  if ((K && !t->n_values) || (K && N && !t->topo) || (T && !t->term_key) || (V && !(t->bound_node && t->bound_class)))
-    return bad(BS_E_INVAL, "null column");
-  for (size_t k = 0; k < (size_t)K * N; ++k)
-    if (t->topo[k] != BS_TOPO_NONE && t->topo[k] >= t->n_values[k / N]) return bad(BS_E_INDEX, "a topo value is >= n_values");
-  std::vector<uint32_t> off(T);
-  uint64_t slots = 0;
-  for (uint32_t k = 0; k < T; ++k) {
-    if (t->term_key[k] >= K) return bad(BS_E_INDEX, "a term_key is >= n_keys");
-    off[k] = (uint32_t)std::min<uint64_t>(slots, UINT32_MAX);
-    slots += t->n_values[t->term_key[k]];
-    if (slots * 16 > BS_IPA_TERM_MAX_BYTES) return bad(BS_E_INVAL, "the term tables exceed BS_IPA_TERM_MAX_BYTES");
-  }
-  for (uint32_t k = 0; k < V; ++k) {
-    if (t->bound_node[k] >= N) return bad(BS_E_INDEX, "a bound_node is >= n_nodes");
-    if (t->bound_class[k] != BS_IPA_NONE && t->bound_class[k] >= t->classes.n_classes)
-      return bad(BS_E_INDEX, "a bound_class is >= n_classes");
-  }
-  int64_t tmax;
-  const char* why = nullptr;
-  if (int rc = interpod_classes_check(t->classes, T, tmax, why)) return bad(rc, why);
-  BS_DEVICE_GUARD(e);
-  CK(e->d_ipa_topo.ensure((size_t)std::max<uint64_t>((uint64_t)K * N, 1) * 4));
-  CK(e->d_ipa_term_key.ensure((size_t)std::max(T, 1u) * 4));
-  CK(e->d_ipa_term_off.ensure((size_t)std::max(T, 1u) * 4));
-  CK(e->d_ipa_bound_node.ensure((size_t)std::max(V, 1u) * 4));
-  CK(e->d_ipa_bound_class.ensure((size_t)std::max(V, 1u) * 4));
-  if (K && N) CK(cudaMemcpyAsync(e->d_ipa_topo.p, t->topo, (size_t)K * N * 4, cudaMemcpyHostToDevice, e->s));
-  if (T) {
-    CK(cudaMemcpyAsync(e->d_ipa_term_key.p, t->term_key, (size_t)T * 4, cudaMemcpyHostToDevice, e->s));
-    CK(cudaMemcpyAsync(e->d_ipa_term_off.p, off.data(), (size_t)T * 4, cudaMemcpyHostToDevice, e->s));
-  }
-  if (V) {
-    CK(cudaMemcpyAsync(e->d_ipa_bound_node.p, t->bound_node, (size_t)V * 4, cudaMemcpyHostToDevice, e->s));
-    CK(cudaMemcpyAsync(e->d_ipa_bound_class.p, t->bound_class, (size_t)V * 4, cudaMemcpyHostToDevice, e->s));
-  }
-  if (int rc = interpod_classes_upload(e, t->classes, e->d_ipa_boff, e->d_ipa_bterm, e->d_ipa_bown, e->d_ipa_bmatch))
-    return rc;
-  CK(cudaStreamSynchronize(e->s));   // the caller's columns may go once the call returns
-  e->ipa_terms = T;
-  e->ipa_slots = slots;
-  e->ipa_bound = V;
-  e->ipa_bclasses = t->classes.n_classes;
-  e->have_ipa_node = true;
-  return BS_OK;
+  e->ipa.have_node = false;
+  e->ipa.dirty = e->ipa.mass_dirty = true;
+  const int rc = upload_interpod_nodes(e, {e, "bs_upload_node_interpod"}, t, IPA_LIMITS, e->ipa.node);
+  e->ipa.have_node = rc == BS_OK;
+  return rc;
 }
 
 int bs_upload_pod_interpod(bs_engine* e, const bs_interpod_pods* t) {
   if (!e) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
-  const char* who = "bs_upload_pod_interpod";
-  auto bad = [&](int rc, const char* why) { return fail(e, rc, (std::string(who) + ": " + why).c_str()); };
-  e->have_ipa_pod = false;
-  e->ipa_dirty = true;
+  const Refuse bad{e, "bs_upload_pod_interpod"};
+  e->ipa.have_pod = false;
+  e->ipa.dirty = true;
   if (!t) return bad(BS_E_INVAL, "null table");
-  if (!e->have_pods) return bad(BS_E_STATE, "upload pods first");
   const uint32_t P = t->n_pods;
-  if (P != e->P) return bad(BS_E_INVAL, "n_pods differs from the pod table's");
+  if (int rc = bad.shape(POD_SIDE, P)) return rc;
   if (P && !t->pod_class) return bad(BS_E_INVAL, "null pod_class");
   if ((uint64_t)t->classes.n_classes * e->Npad * 8 > BS_IPA_TABLE_MAX_BYTES)
     return bad(BS_E_INVAL, "n_classes x padded nodes x 8 bytes exceeds BS_IPA_TABLE_MAX_BYTES");
-  for (uint32_t p = 0; p < P; ++p)
-    if (t->pod_class[p] != BS_IPA_NONE && t->pod_class[p] >= t->classes.n_classes)
-      return bad(BS_E_INDEX, "a pod_class is >= n_classes");
+  if (max_class(t->pod_class, P, BS_IPA_NONE) >= (int64_t)t->classes.n_classes)
+    return bad(BS_E_INDEX, "a pod_class is >= n_classes");
   int64_t tmax;
   const char* why = nullptr;
   if (int rc = interpod_classes_check(t->classes, UINT32_MAX, tmax, why)) return bad(rc, why);
   BS_DEVICE_GUARD(e);
-  CK(e->d_ipa_class.ensure((size_t)std::max(P, 1u) * 4));
-  if (P) CK(cudaMemcpyAsync(e->d_ipa_class.p, t->pod_class, (size_t)P * 4, cudaMemcpyHostToDevice, e->s));
-  if (int rc = interpod_classes_upload(e, t->classes, e->d_ipa_poff, e->d_ipa_pterm, e->d_ipa_pown, e->d_ipa_pmatch))
+  int rc;
+  if ((rc = upload_vec(e, e->ipa.d_class, t->pod_class, P, P)) ||
+      (rc = interpod_classes_upload(e, t->classes, e->ipa.d_poff, e->ipa.d_pterm, e->ipa.d_pown, e->ipa.d_pmatch)))
     return rc;
   CK(cudaStreamSynchronize(e->s));
-  e->ipa_pclasses = t->classes.n_classes;
-  e->ipa_term_max = tmax;
-  e->have_ipa_pod = true;
+  e->ipa.pclasses = t->classes.n_classes;
+  e->ipa.term_max = tmax;
+  e->ipa.have_pod = true;
   return BS_OK;
 }
 
 int bs_set_interpod_filter(bs_engine* e, int on) {
   if (!e) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
-  if ((on != 0) == e->ipf_on) return BS_OK;
-  e->ipf_on = on != 0;
-  e->ipf_dirty = true;   // the pass bits are built again at the next evaluation the filter is on for
-  e->ipf_assign_dirty = e->classes_dirty = e->pod_classes_dirty = true;   // and the pods' fit classes follow the switch
+  if ((on != 0) == e->ipf.on) return BS_OK;
+  e->ipf.on = on != 0;
+  e->ipf.dirty = true;   // the pass bits are built again at the next evaluation the filter is on for
+  e->ipf.assign_dirty = e->classes_dirty = e->pod_classes_dirty = true;   // and the pods' fit classes follow the switch
   e->evaluated = false;
   return BS_OK;
 }
@@ -3944,61 +3945,11 @@ int bs_set_interpod_filter(bs_engine* e, int on) {
 int bs_upload_node_interpod_filter(bs_engine* e, const bs_interpod_nodes* t) {
   if (!e) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
-  const char* who = "bs_upload_node_interpod_filter";
-  auto bad = [&](int rc, const char* why) { return fail(e, rc, (std::string(who) + ": " + why).c_str()); };
-  e->have_ipf_node = false;
-  e->ipf_dirty = true;
-  if (!t) return bad(BS_E_INVAL, "null table");
-  if (!e->have_nodes) return bad(BS_E_STATE, "upload nodes first");
-  const uint32_t N = t->n_nodes, K = t->n_keys, T = t->n_terms, V = t->n_bound;
-  if (N != e->N) return bad(BS_E_INVAL, "n_nodes differs from the node table's");
-  if (K > BS_IPA_KEY_MAX) return bad(BS_E_INVAL, "n_keys exceeds BS_IPA_KEY_MAX");
-  if (V > BS_IPF_BOUND_MAX) return bad(BS_E_INVAL, "n_bound exceeds BS_IPF_BOUND_MAX");
-  if ((K && !t->n_values) || (K && N && !t->topo) || (T && !t->term_key) || (V && !(t->bound_node && t->bound_class)))
-    return bad(BS_E_INVAL, "null column");
-  for (size_t k = 0; k < (size_t)K * N; ++k)
-    if (t->topo[k] != BS_TOPO_NONE && t->topo[k] >= t->n_values[k / N]) return bad(BS_E_INDEX, "a topo value is >= n_values");
-  std::vector<uint32_t> off(T);
-  uint64_t slots = 0;
-  for (uint32_t k = 0; k < T; ++k) {
-    if (t->term_key[k] >= K) return bad(BS_E_INDEX, "a term_key is >= n_keys");
-    off[k] = (uint32_t)slots;
-    slots += t->n_values[t->term_key[k]];
-    if ((slots + 31) / 32 * 2 * 4 > BS_IPF_TERM_MAX_BYTES) return bad(BS_E_INVAL, "the presence planes exceed BS_IPF_TERM_MAX_BYTES");
-  }
-  for (uint32_t k = 0; k < V; ++k) {
-    if (t->bound_node[k] >= N) return bad(BS_E_INDEX, "a bound_node is >= n_nodes");
-    if (t->bound_class[k] != BS_IPF_NONE && t->bound_class[k] >= t->classes.n_classes)
-      return bad(BS_E_INDEX, "a bound_class is >= n_classes");
-  }
-  int64_t tmax;
-  const char* why = nullptr;
-  if (int rc = interpod_classes_check(t->classes, T, tmax, why)) return bad(rc, why);
-  const uint32_t nnz = t->classes.n_classes ? t->classes.class_offset[t->classes.n_classes] : 0;
-  for (uint32_t k = 0; k < nnz; ++k)
-    if (t->classes.own[k] != 0 && t->classes.own[k] != 1) return bad(BS_E_RANGE, "an own is not 0 or 1");
-  BS_DEVICE_GUARD(e);
-  CK(e->d_ipf_topo.ensure((size_t)std::max<uint64_t>((uint64_t)K * N, 1) * 4));
-  CK(e->d_ipf_term_key.ensure((size_t)std::max(T, 1u) * 4));
-  CK(e->d_ipf_term_off.ensure((size_t)std::max(T, 1u) * 4));
-  CK(e->d_ipf_bound_node.ensure((size_t)std::max(V, 1u) * 4));
-  CK(e->d_ipf_bound_class.ensure((size_t)std::max(V, 1u) * 4));
-  if (K && N) CK(cudaMemcpyAsync(e->d_ipf_topo.p, t->topo, (size_t)K * N * 4, cudaMemcpyHostToDevice, e->s));
-  if (T) {
-    CK(cudaMemcpyAsync(e->d_ipf_term_key.p, t->term_key, (size_t)T * 4, cudaMemcpyHostToDevice, e->s));
-    CK(cudaMemcpyAsync(e->d_ipf_term_off.p, off.data(), (size_t)T * 4, cudaMemcpyHostToDevice, e->s));
-  }
-  if (V) {
-    CK(cudaMemcpyAsync(e->d_ipf_bound_node.p, t->bound_node, (size_t)V * 4, cudaMemcpyHostToDevice, e->s));
-    CK(cudaMemcpyAsync(e->d_ipf_bound_class.p, t->bound_class, (size_t)V * 4, cudaMemcpyHostToDevice, e->s));
-  }
-  if (int rc = interpod_classes_upload(e, t->classes, e->d_ipf_boff, e->d_ipf_bterm, e->d_ipf_bown, e->d_ipf_bmatch))
-    return rc;
-  CK(cudaStreamSynchronize(e->s));   // the caller's columns may go once the call returns
-  e->ipf_terms = T;
-  e->ipf_slots = slots;
-  e->ipf_bound = V;
-  e->have_ipf_node = true;
+  e->ipf.have_node = false;
+  e->ipf.dirty = true;
+  const int rc = upload_interpod_nodes(e, {e, "bs_upload_node_interpod_filter"}, t, IPF_LIMITS, e->ipf.node);
+  if (rc) return rc;
+  e->ipf.have_node = true;
   e->evaluated = false;
   return BS_OK;
 }
@@ -4006,14 +3957,12 @@ int bs_upload_node_interpod_filter(bs_engine* e, const bs_interpod_nodes* t) {
 int bs_upload_pod_interpod_filter(bs_engine* e, const bs_interpod_filter_pods* t) {
   if (!e) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
-  const char* who = "bs_upload_pod_interpod_filter";
-  auto bad = [&](int rc, const char* why) { return fail(e, rc, (std::string(who) + ": " + why).c_str()); };
-  e->have_ipf_pod = false;
-  e->ipf_dirty = true;
+  const Refuse bad{e, "bs_upload_pod_interpod_filter"};
+  e->ipf.have_pod = false;
+  e->ipf.dirty = true;
   if (!t) return bad(BS_E_INVAL, "null table");
-  if (!e->have_pods) return bad(BS_E_STATE, "upload pods first");
   const uint32_t P = t->n_pods, C = t->n_classes;
-  if (P != e->P) return bad(BS_E_INVAL, "n_pods differs from the pod table's");
+  if (int rc = bad.shape(POD_SIDE, P)) return rc;
   if (P && !t->pod_class) return bad(BS_E_INVAL, "null pod_class");
   if (C && !(t->class_offset && t->self_match)) return bad(BS_E_INVAL, "null class_offset or self_match");
   if (3ull * C * (e->Npad / 8) > BS_IPF_TABLE_MAX_BYTES)
@@ -4031,27 +3980,20 @@ int bs_upload_pod_interpod_filter(bs_engine* e, const bs_interpod_filter_pods* t
   }
   for (uint32_t k = 0; k < C; ++k)
     if (t->self_match[k] > 1) return bad(BS_E_RANGE, "a self_match is not 0 or 1");
-  for (uint32_t p = 0; p < P; ++p)
-    if (t->pod_class[p] != BS_IPF_NONE && t->pod_class[p] >= C) return bad(BS_E_INDEX, "a pod_class is >= n_classes");
+  if (max_class(t->pod_class, P, BS_IPF_NONE) >= (int64_t)C) return bad(BS_E_INDEX, "a pod_class is >= n_classes");
   BS_DEVICE_GUARD(e);
-  CK(e->d_ipf_poff.ensure((size_t)(C + 1) * 4));
-  CK(e->d_ipf_pterm.ensure((size_t)std::max(nnz, 1u) * 4));
-  CK(e->d_ipf_prole.ensure(std::max(nnz, 1u)));
-  CK(e->d_ipf_pself.ensure(std::max(C, 1u)));
-  if (C) {
-    CK(cudaMemcpyAsync(e->d_ipf_poff.p, t->class_offset, (size_t)(C + 1) * 4, cudaMemcpyHostToDevice, e->s));
-    CK(cudaMemcpyAsync(e->d_ipf_pself.p, t->self_match, C, cudaMemcpyHostToDevice, e->s));
-  }
-  if (nnz) {
-    CK(cudaMemcpyAsync(e->d_ipf_pterm.p, t->term, (size_t)nnz * 4, cudaMemcpyHostToDevice, e->s));
-    CK(cudaMemcpyAsync(e->d_ipf_prole.p, t->role, nnz, cudaMemcpyHostToDevice, e->s));
-  }
+  const uint32_t offs = C ? C + 1 : 0;   // (no offset at all for an empty table: no class is ever read)
+  int rc;
+  if ((rc = upload_vec(e, e->ipf.d_poff, t->class_offset, offs, offs)) ||
+      (rc = upload_vec(e, e->ipf.d_pterm, t->term, nnz, nnz)) || (rc = upload_vec(e, e->ipf.d_prole, t->role, nnz, nnz)) ||
+      (rc = upload_vec(e, e->ipf.d_pself, t->self_match, C, C)))
+    return rc;
   CK(cudaStreamSynchronize(e->s));
-  e->h_ipf_class.assign(t->pod_class, t->pod_class + P);
-  e->ipf_pclasses = C;
-  e->ipf_term_max = tmax;
-  e->have_ipf_pod = true;
-  e->ipf_assign_dirty = e->classes_dirty = e->pod_classes_dirty = true;   // the pods' fit classes carry the filter class
+  e->ipf.h_class.assign(t->pod_class, t->pod_class + P);
+  e->ipf.pclasses = C;
+  e->ipf.term_max = tmax;
+  e->ipf.have_pod = true;
+  e->ipf.assign_dirty = e->classes_dirty = e->pod_classes_dirty = true;   // the pods' fit classes carry the filter class
   e->evaluated = false;
   return BS_OK;
 }
@@ -4062,12 +4004,12 @@ int bs_fetch_interpod_reason_rows(bs_engine* e, uint32_t pod0, uint32_t n, uint3
   if (!e->evaluated || !(e->out_flags & BS_OUT_REASONS)) return fail(e, BS_E_STATE, "no reason rows materialised");
   if ((uint64_t)pod0 + n > e->P) return BS_E_INDEX;
   if (!n) return BS_OK;
-  if (!e->ipf_round) {
+  if (!e->ipf.round) {
     memset(counts, 0, (size_t)n * 3 * 4);
     return BS_OK;
   }
   BS_DEVICE_GUARD(e);
-  CK(cudaMemcpyAsync(counts, e->d_ipf_reasons.as<uint32_t>() + (size_t)pod0 * 3, (size_t)n * 3 * 4,
+  CK(cudaMemcpyAsync(counts, e->ipf.d_reasons.as<uint32_t>() + (size_t)pod0 * 3, (size_t)n * 3 * 4,
                      cudaMemcpyDeviceToHost, e->s));
   CK(cudaStreamSynchronize(e->s));
   return BS_OK;

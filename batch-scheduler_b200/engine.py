@@ -66,6 +66,15 @@ def _table_c(table):
     return cls(table.n, table.lanes, *(capi.ptr(getattr(table, c)) for c in cols))
 
 
+def _interpod_classes(cl, keep):
+    """The bs_interpod_classes of (class_offset [C + 1], term, own int32, match uint8); `keep` holds its arrays."""
+    off, term, own, match = cl
+    a = [np.ascontiguousarray(off, dtype=np.uint32).reshape(-1), np.ascontiguousarray(term, dtype=np.uint32),
+         np.ascontiguousarray(own, dtype=np.int32), np.ascontiguousarray(match, dtype=np.uint8)]
+    keep += a
+    return capi.InterpodClassesC(max(len(a[0]) - 1, 0), *(capi.ptr(x) for x in a))
+
+
 class Engine:
     def __init__(self, n_lanes: int, device: int = 0, fit_bitmap: bool = True, score: bool = False,
                  filter: bool = False, topk: int = 0, reasons: bool = False, priority_k: int = 0):
@@ -412,33 +421,28 @@ class Engine:
         (capi.TOPO_NONE: none), each term's key, the bound pods' nodes and classes (capi.IPA_NONE: none) and the bound
         classes.  pods = (pod_class [P], classes): each pod's class (capi.IPA_NONE: none) and the pod classes.  Uploading
         nodes (or updating node rows) drops the node side, uploading pods the pod side."""
-        def classes(cl, keep):
-            off, term, own, match = cl
-            a = [np.ascontiguousarray(off, dtype=np.uint32).reshape(-1), np.ascontiguousarray(term, dtype=np.uint32),
-                 np.ascontiguousarray(own, dtype=np.int32), np.ascontiguousarray(match, dtype=np.uint8)]
-            keep += a
-            return capi.InterpodClassesC(max(len(a[0]) - 1, 0), *(capi.ptr(x) for x in a))
+        keep = []
         if node is not None:
-            keep = []
-            nv, topo, tkey, bnode, bcls, cl = node
-            nv = np.ascontiguousarray(nv, dtype=np.uint32).reshape(-1)
-            topo = (np.ascontiguousarray(topo, dtype=np.uint32).reshape(len(nv), -1) if len(nv)
-                    else np.zeros((0, self.N), np.uint32))
-            tkey = np.ascontiguousarray(tkey, dtype=np.uint32).reshape(-1)
-            bnode = np.ascontiguousarray(bnode, dtype=np.uint32).reshape(-1)
-            bcls = np.ascontiguousarray(bcls, dtype=np.uint32).reshape(-1)
-            if len(bnode) != len(bcls):
-                raise ValueError("bound_node and bound_class must have one entry per bound pod")
-            t = capi.InterpodNodesC(topo.shape[1], len(nv), capi.ptr(nv), capi.ptr(topo),
-                                    len(tkey), capi.ptr(tkey), len(bnode), capi.ptr(bnode), capi.ptr(bcls),
-                                    classes(cl, keep))
-            self._check(self.lib.bs_upload_node_interpod(self.h, C.byref(t)))
+            self._check(self.lib.bs_upload_node_interpod(self.h, C.byref(self._interpod_nodes(node, keep))))
         if pods is not None:
-            keep = []
-            pcls, cl = pods
-            pcls = np.ascontiguousarray(pcls, dtype=np.uint32).reshape(-1)
-            t = capi.InterpodPodsC(len(pcls), capi.ptr(pcls), classes(cl, keep))
+            pcls = np.ascontiguousarray(pods[0], dtype=np.uint32).reshape(-1)
+            t = capi.InterpodPodsC(len(pcls), capi.ptr(pcls), _interpod_classes(pods[1], keep))
             self._check(self.lib.bs_upload_pod_interpod(self.h, C.byref(t)))
+
+    def _interpod_nodes(self, node, keep):
+        """The bs_interpod_nodes of upload_interpod's node tuple; `keep` holds its arrays for the call."""
+        nv, topo, tkey, bnode, bcls, cl = node
+        nv = np.ascontiguousarray(nv, dtype=np.uint32).reshape(-1)
+        topo = (np.ascontiguousarray(topo, dtype=np.uint32).reshape(len(nv), -1) if len(nv)
+                else np.zeros((0, self.N), np.uint32))
+        tkey = np.ascontiguousarray(tkey, dtype=np.uint32).reshape(-1)
+        bnode = np.ascontiguousarray(bnode, dtype=np.uint32).reshape(-1)
+        bcls = np.ascontiguousarray(bcls, dtype=np.uint32).reshape(-1)
+        if len(bnode) != len(bcls):
+            raise ValueError("bound_node and bound_class must have one entry per bound pod")
+        keep += [nv, topo, tkey, bnode, bcls]
+        return capi.InterpodNodesC(topo.shape[1], len(nv), capi.ptr(nv), capi.ptr(topo), len(tkey), capi.ptr(tkey),
+                                   len(bnode), capi.ptr(bnode), capi.ptr(bcls), _interpod_classes(cl, keep))
 
     def set_interpod_filter(self, on: bool = False):
         """Switch kube-scheduler's MatchInterPodAffinity filter (required pod affinity and anti-affinity) into every
@@ -453,21 +457,8 @@ class Engine:
         class (capi.IPF_NONE: none) and the class table with roles capi.IPF_AFFINITY / IPF_ANTI / IPF_EXISTING.
         Uploading nodes (or updating node rows) drops the node side, uploading pods the pod side."""
         if node is not None:
-            nv, topo, tkey, bnode, bcls, (off, term, own, match) = node
-            keep = [np.ascontiguousarray(off, dtype=np.uint32).reshape(-1), np.ascontiguousarray(term, dtype=np.uint32),
-                    np.ascontiguousarray(own, dtype=np.int32), np.ascontiguousarray(match, dtype=np.uint8)]
-            nv = np.ascontiguousarray(nv, dtype=np.uint32).reshape(-1)
-            topo = (np.ascontiguousarray(topo, dtype=np.uint32).reshape(len(nv), -1) if len(nv)
-                    else np.zeros((0, self.N), np.uint32))
-            tkey = np.ascontiguousarray(tkey, dtype=np.uint32).reshape(-1)
-            bnode = np.ascontiguousarray(bnode, dtype=np.uint32).reshape(-1)
-            bcls = np.ascontiguousarray(bcls, dtype=np.uint32).reshape(-1)
-            if len(bnode) != len(bcls):
-                raise ValueError("bound_node and bound_class must have one entry per bound pod")
-            cl = capi.InterpodClassesC(max(len(keep[0]) - 1, 0), *(capi.ptr(x) for x in keep))
-            t = capi.InterpodNodesC(topo.shape[1], len(nv), capi.ptr(nv), capi.ptr(topo), len(tkey), capi.ptr(tkey),
-                                    len(bnode), capi.ptr(bnode), capi.ptr(bcls), cl)
-            self._check(self.lib.bs_upload_node_interpod_filter(self.h, C.byref(t)))
+            keep = []
+            self._check(self.lib.bs_upload_node_interpod_filter(self.h, C.byref(self._interpod_nodes(node, keep))))
         if pods is not None:
             pcls, (off, term, role, self_match) = pods
             a = [np.ascontiguousarray(pcls, dtype=np.uint32).reshape(-1),
