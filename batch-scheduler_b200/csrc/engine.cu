@@ -1447,6 +1447,15 @@ int evaluate_async_locked(bs_engine* e) {
   if (e->ipf.on && (rc = interpod_filter_check(e, "bs_evaluate"))) return rc;
   if (e->peer_broken)
     return fail(e, BS_E_PEER, "peer exchange is broken (a rank did not arrive): bs_peer_detach on every rank, then init/attach again");
+  if (e->peer_attached && cdiv(std::max(e->G, 1u), 32) > e->peer_wpr) {
+    // the push carries words_per_rank words: a round whose admits cannot all reach the peers does not run (the
+    // group table is replicated, so every rank refuses the same round and none is left waiting)
+    const uint32_t need = cdiv(std::max(e->G, 1u), 32);
+    e->err = "bs_evaluate: the group table needs " + std::to_string(need) + " admit-bitmap words per rank, but the peer "
+             "exchange carries " + std::to_string(e->peer_wpr) + " (bs_peer_init with words_per_rank >= " +
+             std::to_string(need) + ")";
+    return BS_E_STATE;
+  }
   BS_DEVICE_GUARD(e);
   bool reprepare = e->nodes_dirty;
   if (e->classes_dirty) {
@@ -4098,6 +4107,14 @@ int bs_peer_detach(bs_engine* e) {
   e->peer_attached = false;
   e->peer_broken = false;
   e->peer_seq = 0;
+  // A new epoch may attach this buffer again without bs_peer_init: its round 1 must not find the last epoch's words
+  // and round numbers in the flags.  The peers' pushes of the last round have landed (this rank's wait for it
+  // finished above), and no peer pushes the next epoch before every rank has attached again.
+  if (e->d_gather.p && e->s) {
+    CK(cudaMemsetAsync(e->d_gather.p, 0, e->d_gather.cap, e->s));
+    CK(cudaMemsetAsync(e->d_peer_err.p, 0, sizeof(int), e->s));
+    CK(cudaStreamSynchronize(e->s));
+  }
   return BS_OK;
 }
 

@@ -862,10 +862,18 @@ int bs_format_remove_message(const bs_status* st, const char* pod_name, const ch
  *   bs_fetch_gathered_admit  copy [world][words_per_rank] words of the last round to the host
  * BS_BUF_GATHERED_ADMIT is the device address of the last round's slot set (rank r at word
  * r*words_per_rank); it alternates between two addresses from round to round.
+ * A round needs ceil(G / 32) <= words_per_rank: while attached, bs_evaluate* refuses a group table larger than
+ * 32 * words_per_rank groups with BS_E_STATE ("bs_evaluate: the group table needs W admit-bitmap words per rank,
+ * but the peer exchange carries w (bs_peer_init with words_per_rank >= W)") before anything runs; the group table
+ * is replicated, so every rank refuses the same round.  A smaller table works; its words past ceil(G / 32) are 0.
+ * A new epoch: bs_peer_detach on every rank (it waits for this rank's last round, then zeroes its gather buffer
+ * and error word), then bs_peer_attach on every rank, with the handles of the last bs_peer_init or after a new
+ * bs_peer_init and handle exchange; round numbers restart at 1.  No rank may evaluate before every rank has
+ * attached (exchanging handles is that barrier).
  * Failure: a rank that does not arrive within BS_PEER_TIMEOUT_MS (env, default 2000) makes bs_sync /
  * bs_fetch_gathered_admit return BS_E_PEER; from then on bs_evaluate* fails fast with BS_E_PEER (no
- * further spinning) until every rank has called bs_peer_detach and attached again (a new epoch:
- * buffers zeroed, round numbers restart at 1). */
+ * further spinning) until every rank has called bs_peer_detach, bs_peer_init and attached again (the
+ * late rank may still push into the old buffers). */
 int bs_peer_init(bs_engine* e, uint32_t rank, uint32_t world, uint32_t words_per_rank);
 int bs_peer_handle(bs_engine* e, unsigned char handle[64]);
 int bs_peer_attach(bs_engine* e, const unsigned char* handles /* [world][64] */);
