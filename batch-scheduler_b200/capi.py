@@ -38,6 +38,8 @@ IPA_NONE = 0xffffffff     # BS_IPA_NONE: class of a pod or bound pod without ent
 TOPO_NONE = 0xffffffff    # BS_TOPO_NONE: topo value of a node without the key
 IPF_NONE = 0xffffffff     # BS_IPF_NONE: filter class of a pod without entries (passes every node)
 IPF_AFFINITY, IPF_ANTI, IPF_EXISTING = range(3)   # BS_IPF_*: roles of a pod's filter class entries
+HOSTPORT_MAX = 64         # BS_HOSTPORT_MAX: entries of the host-port dictionary
+HOSTPORT_IP_ANY = 0       # BS_HOSTPORT_IP_ANY: ip id of "0.0.0.0"
 IPA_KEY_MAX = 64          # BS_IPA_KEY_MAX: topology keys of one node side
 IPA_BOUND_MAX = 1 << 24   # BS_IPA_BOUND_MAX: bound pods of one node side
 IPA_CLASS_MAX = 64        # BS_IPA_CLASS_MAX: entries of one class
@@ -123,6 +125,11 @@ class InterpodPodsC(C.Structure):
 class InterpodFilterPodsC(C.Structure):
     _fields_ = [("n_pods", C.c_uint32), ("pod_class", C.c_void_p), ("n_classes", C.c_uint32),
                 ("class_offset", C.c_void_p), ("term", C.c_void_p), ("role", C.c_void_p), ("self_match", C.c_void_p)]
+
+
+class HostPortNodesC(C.Structure):
+    _fields_ = [("n_nodes", C.c_uint32), ("n_entries", C.c_uint32), ("ip", C.c_void_p), ("protocol", C.c_void_p),
+                ("port", C.c_void_p), ("used", C.c_void_p)]
 
 
 class PreemptResultC(C.Structure):
@@ -225,6 +232,12 @@ SYMBOLS = {
     "bs_fetch_interpod_reason_rows": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]),
     "bs_format_fit_error_interpod": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_char_p,
                                                C.c_size_t]),
+    "bs_set_host_port_filter": (C.c_int, [C.c_void_p, C.c_int]),
+    "bs_upload_node_host_ports": (C.c_int, [C.c_void_p, _p(HostPortNodesC)]),
+    "bs_upload_pod_host_ports": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p]),
+    "bs_fetch_host_port_reason_rows": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]),
+    "bs_format_fit_error_filters": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p,
+                                              C.c_char_p, C.c_size_t]),
     "bs_peer_init": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32]),
     "bs_peer_handle": (C.c_int, [C.c_void_p, C.c_void_p]),
     "bs_peer_attach": (C.c_int, [C.c_void_p, C.c_void_p]),

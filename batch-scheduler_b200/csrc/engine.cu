@@ -168,8 +168,9 @@ struct ClassKey {
   uint32_t nz;
   uint32_t aff;   // affinity class (row of the bs_upload_affinity table) or BS_AFF_NONE
   uint32_t ipf = BS_IPF_NONE;   // MatchInterPodAffinity filter class while the filter is on, else BS_IPF_NONE
+  uint64_t hp = 0;              // PodFitsHostPorts conflict mask while the filter is on, else 0
   bool operator==(const ClassKey& o) const {
-    return sel == o.sel && tol == o.tol && nz == o.nz && aff == o.aff && ipf == o.ipf;
+    return sel == o.sel && tol == o.tol && nz == o.nz && aff == o.aff && ipf == o.ipf && hp == o.hp;
   }
 };
 
@@ -182,7 +183,8 @@ struct ClassIndex {
   uint32_t last_id = 0;
   static uint64_t hash(const ClassKey& k) {
     uint64_t h = k.sel * 0x9E3779B97F4A7C15ull ^ (k.tol + 0x7F4A7C15ull) * 0xBF58476D1CE4E5B9ull ^
-                 ((uint64_t)k.nz | ((uint64_t)k.aff << 32)) * 0x94D049BB133111EBull ^ (uint64_t)(k.ipf + 1u) * 0xD6E8FEB86659FD93ull;
+                 ((uint64_t)k.nz | ((uint64_t)k.aff << 32)) * 0x94D049BB133111EBull ^ (uint64_t)(k.ipf + 1u) * 0xD6E8FEB86659FD93ull ^
+                 k.hp * 0xC2B2AE3D27D4EB4Full;
     return h ^ (h >> 29);
   }
   void clear() {
@@ -496,19 +498,39 @@ struct bs_engine {
   // MatchInterPodAffinity filter (bs_set_interpod_filter; off by default): the node side (InterpodNodeSide; dropped
   // with the node table) and the pod side (each pod's filter class h_class, the class table; dropped with the pod
   // table).  The presence planes d_presence ([2][words]: match, own), the per-term counts d_hits and the class planes
-  // d_bits ([3][classes][Npad/32]: pass, E, A) are built on the device when dirty.  assign_dirty: the pods' fit classes
-  // have to be assigned again (with their filter class while the filter is on, else their base class h_pfc_base).
-  // d_fipf: each fit class's filter class, d_reason_gate the priority lists' gate, d_reasons the companion rows [P][3].
+  // d_bits ([3][classes][Npad/32]: pass, E, A) are built on the device when dirty.  d_fipf: each fit class's filter
+  // class, d_reasons the companion rows [P][3].
   struct {
     bool on = false, round = false;
     InterpodNodeSide node;
-    DevBuf d_presence, d_hits, d_poff, d_pterm, d_prole, d_pself, d_bits, d_fipf, d_reason_gate, d_reasons;
-    bool have_node = false, have_pod = false, dirty = true, assign_dirty = false;
+    DevBuf d_presence, d_hits, d_poff, d_pterm, d_prole, d_pself, d_bits, d_fipf, d_reasons;
+    bool have_node = false, have_pod = false, dirty = true;
     uint32_t pclasses = 0;
     int64_t term_max = -1;
-    std::vector<uint32_t> h_class, h_pfc_base;   // h_pfc_base: the pods' fit classes without the filter
-    bool pfc_base_valid = false;                 // h_pfc_base holds the classes of the pod table of now
+    std::vector<uint32_t> h_class;
   } ipf;
+  // PodFitsHostPorts filter (bs_set_host_port_filter; off by default): the node side (each entry's conflict mask
+  // h_conflict, each node's used mask d_used [Npad]; dropped with the node table) and the pod side (each pod's want
+  // mask h_want, want_all their OR; dropped with the pod table).  dirty: the used masks changed or the filter was
+  // switched on, so the class fit bits are built again.  d_fconf: each fit class's conflict mask, d_bins the ports bin
+  // of each fit class, d_reasons the companion rows [P].
+  struct {
+    bool on = false, round = false;
+    DevBuf d_used, d_fconf, d_bins, d_reasons;
+    bool have_node = false, have_pod = false, dirty = true;
+    uint32_t entries = 0;
+    uint64_t want_all = 0;
+    std::vector<uint64_t> h_conflict, h_want;
+  } hp;
+  // The filters' share of the fit classes.  assign_dirty: the pods' fit classes have to be assigned again (with their
+  // filter class and conflict mask while a filter is on, else their base class h_pfc_base).  d_gate: the priority
+  // lists' gate while a filter is on, the reason gate ANDed with the filters' pass bits.
+  struct {
+    bool assign_dirty = false;
+    std::vector<uint32_t> h_pfc_base;   // the pods' fit classes without the filters
+    bool pfc_base_valid = false;        // h_pfc_base holds the classes of the pod table of now
+    DevBuf d_gate;
+  } filt;
   // sort scratch: views into one arena
   View d_gk0, d_gk1, d_pk0, d_pk1, d_idx_a, d_idx_b, d_ghist, d_group_rank, d_tilecnt, d_sort_barrier;
   uint32_t sort_max_grid = 1;
@@ -914,23 +936,30 @@ void launch_prefix(uint32_t L, NodeTab t, PrefixSel ps, PrefixScratch sc, Prefix
   }
 }
 
-// loc: the scored walk with the locality terms (a is then a ReplayLocArgs)
-template <int MAXL>
+// loc: the scored walk with the locality terms (a is then a ReplayLocArgs); HP: the PodFitsHostPorts filter is on (a is
+// then a ReplayHpArgs)
+template <int MAXL, bool HP>
 void launch_replay_t(const ReplayArgs& a, bool scored, bool loc, cudaStream_t s) {
   if (loc) {
-    const ReplayLocArgs& la = static_cast<const ReplayLocArgs&>(a);
-    if (a.ratio.weight) replay_kernel<MAXL, true, true, true><<<1, REPLAY_THREADS, 0, s>>>(la);
-    else replay_kernel<MAXL, true, false, true><<<1, REPLAY_THREADS, 0, s>>>(la);
-  } else if (scored && a.ratio.weight) replay_kernel<MAXL, true, true><<<1, REPLAY_THREADS, 0, s>>>(a);
-  else if (scored) replay_kernel<MAXL, true><<<1, REPLAY_THREADS, 0, s>>>(a);
-  else replay_kernel<MAXL, false><<<1, REPLAY_THREADS, 0, s>>>(a);
+    const auto& la = static_cast<const ReplayArgsOf<true, HP>&>(a);
+    if (a.ratio.weight) replay_kernel<MAXL, true, true, true, HP><<<1, REPLAY_THREADS, 0, s>>>(la);
+    else replay_kernel<MAXL, true, false, true, HP><<<1, REPLAY_THREADS, 0, s>>>(la);
+    return;
+  }
+  const auto& ha = static_cast<const ReplayArgsOf<false, HP>&>(a);
+  if (scored && a.ratio.weight) replay_kernel<MAXL, true, true, false, HP><<<1, REPLAY_THREADS, 0, s>>>(ha);
+  else if (scored) replay_kernel<MAXL, true, false, false, HP><<<1, REPLAY_THREADS, 0, s>>>(ha);
+  else replay_kernel<MAXL, false, false, false, HP><<<1, REPLAY_THREADS, 0, s>>>(ha);
 }
 inline uint32_t replay_maxl(uint32_t L) { return L <= 5 ? 5u : L <= 9 ? 9u : 16u; }
-void launch_replay(uint32_t L, const ReplayArgs& a, bool scored, bool loc, cudaStream_t s) {
-  switch (replay_maxl(L)) {
-    case 5: launch_replay_t<5>(a, scored, loc, s); break;
-    case 9: launch_replay_t<9>(a, scored, loc, s); break;
-    default: launch_replay_t<16>(a, scored, loc, s); break;
+void launch_replay(uint32_t L, const ReplayArgs& a, bool scored, bool loc, bool hp, cudaStream_t s) {
+  switch (replay_maxl(L) + (hp ? 100u : 0u)) {
+    case 5: launch_replay_t<5, false>(a, scored, loc, s); break;
+    case 9: launch_replay_t<9, false>(a, scored, loc, s); break;
+    case 16: launch_replay_t<16, false>(a, scored, loc, s); break;
+    case 105: launch_replay_t<5, true>(a, scored, loc, s); break;
+    case 109: launch_replay_t<9, true>(a, scored, loc, s); break;
+    default: launch_replay_t<16, true>(a, scored, loc, s); break;
   }
 }
 
@@ -1019,14 +1048,14 @@ inline uint64_t low_bits_mask(uint32_t n) {  // mask covering every value in [0,
   return m;
 }
 
-// The fit index only grows.  While the filter is on, every pod-side upload and every switch adds (class, filter class)
-// keys, so after each re-assignment the index is rebuilt from the classes the pods use when those are a small share
-// of it (the bound bs_upload_pods applies to stale classes); the base ids of h_pfc_base follow.
+// The fit index only grows.  While a filter is on, every side upload and every switch adds (class, filter class,
+// conflict mask) keys, so after each re-assignment the index is rebuilt from the classes the pods use when those are a
+// small share of it (the bound bs_upload_pods applies to stale classes); the base ids of h_pfc_base follow.
 void compact_fit_index(bs_engine* e) {
   ClassIndex& fi = e->fit_index;
   const uint32_t P = e->P;
   uint32_t* pfc = e->h_pfc.data();
-  uint32_t* base = e->ipf.pfc_base_valid ? e->ipf.h_pfc_base.data() : nullptr;
+  uint32_t* base = e->filt.pfc_base_valid ? e->filt.h_pfc_base.data() : nullptr;
   std::vector<uint8_t> used(fi.size(), 0);
   size_t n_used = 0;
   auto mark = [&](uint32_t id) { n_used += used[id] ? 0 : 1; used[id] = 1; };
@@ -1062,25 +1091,30 @@ int rebuild_classes(bs_engine* e) {
     e->group_classes_dirty = false;
   }
   HP(e, "classes:assign-groups");
-  if (e->ipf.assign_dirty) {
-    // the pods' fit classes with their filter class while the filter is on, else the classes of the upload
+  if (e->filt.assign_dirty) {
+    // the pods' fit classes with their filter class and conflict mask while a filter is on, else the classes of the
+    // upload (the evaluation's checks have passed: both sides of each filter that is on are here and agree)
     uint32_t* pfc = e->h_pfc.data();
-    if (e->ipf.on) {
-      if (!e->ipf.pfc_base_valid) e->ipf.h_pfc_base.assign(pfc, pfc + P);
-      e->ipf.pfc_base_valid = true;
-      const uint32_t* base = e->ipf.h_pfc_base.data();
-      const uint32_t* ipf = e->ipf.h_class.data();
+    if (e->ipf.on || e->hp.on) {
+      if (!e->filt.pfc_base_valid) e->filt.h_pfc_base.assign(pfc, pfc + P);
+      e->filt.pfc_base_valid = true;
+      const uint32_t* base = e->filt.h_pfc_base.data();
+      const uint32_t* ipf = e->ipf.on ? e->ipf.h_class.data() : nullptr;
+      const uint64_t* want = e->hp.on ? e->hp.h_want.data() : nullptr;
+      const uint64_t* conflict = e->hp.h_conflict.data();
       ClassIndex& fi = e->fit_index;
-      assign_classes(fi, P, [&fi, base, ipf](uint32_t p) {
+      assign_classes(fi, P, [&fi, base, ipf, want, conflict](uint32_t p) {
         ClassKey k = fi.keys[base[p]];
-        k.ipf = ipf[p];
+        if (ipf) k.ipf = ipf[p];
+        if (want)
+          for (uint64_t w = want[p]; w; w &= w - 1) k.hp |= conflict[__builtin_ctzll(w)];
         return k;
       }, pfc);
-    } else if (e->ipf.pfc_base_valid) {
-      memcpy(pfc, e->ipf.h_pfc_base.data(), (size_t)P * 4);
+    } else if (e->filt.pfc_base_valid) {
+      memcpy(pfc, e->filt.h_pfc_base.data(), (size_t)P * 4);
     }
     compact_fit_index(e);
-    e->ipf.assign_dirty = false;
+    e->filt.assign_dirty = false;
   }
   if (e->fit_index.size() == 0) e->fit_index.get_or_add(ClassKey{0, 0, 0, BS_AFF_NONE});
   if (e->rep_index.size() == 0) e->rep_index.get_or_add(ClassKey{0, 0, 0, BS_AFF_NONE});
@@ -1134,6 +1168,11 @@ int rebuild_classes(bs_engine* e) {
     }
     if ((rc = upload_vec(e, e->ipf.d_fipf, fipf.data(), e->n_fit_classes, e->n_fit_classes))) return rc;
   }
+  if (e->hp.on) {
+    std::vector<uint64_t> fconf(e->n_fit_classes);
+    for (uint32_t c = 0; c < e->n_fit_classes; ++c) fconf[c] = e->fit_index.keys[c].hp;
+    if ((rc = upload_vec(e, e->hp.d_fconf, fconf.data(), e->n_fit_classes, e->n_fit_classes))) return rc;
+  }
   if (e->pod_classes_dirty) {   // a group-only change (bs_update_groups) leaves the pods' ids alone
     if ((rc = upload_vec(e, e->d_pod_fit_class, e->h_pfc.data(), P, std::max(P, 1u)))) return rc;
     if ((rc = upload_vec(e, e->d_pod_rep_class, e->h_prc.data(), P, std::max(P, 1u)))) return rc;
@@ -1186,6 +1225,7 @@ int ensure_round_buffers(bs_engine* e) {
   }
   if (e->out_flags & BS_OUT_REASONS) CK(e->d_reasons.ensure((size_t)P * (4 + L) * 4));
   if ((e->out_flags & BS_OUT_REASONS) && e->ipf.on) CK(e->ipf.d_reasons.ensure((size_t)P * 3 * 4));
+  if ((e->out_flags & BS_OUT_REASONS) && e->hp.on) CK(e->hp.d_reasons.ensure((size_t)P * 4));
   if (e->out_flags & BS_OUT_PRIORITY) {
     CK(e->d_prio_node.ensure((size_t)P * e->topk * 4));
     CK(e->d_prio_score.ensure((size_t)P * e->topk * 8));
@@ -1245,11 +1285,13 @@ int prepare_nodes(bs_engine* e) {
   {
     for (uint32_t c0 = 0; c0 < e->n_fit_classes; c0 += 32768) {
       dim3 grid(cdiv(n_tiles * 32, 256), std::min(32768u, e->n_fit_classes - c0));
-      auto fn = e->ipf.on ? class_fit_kernel<true> : class_fit_kernel<false>;
+      auto fn = e->ipf.on ? (e->hp.on ? class_fit_kernel<true, true> : class_fit_kernel<true, false>)
+                          : (e->hp.on ? class_fit_kernel<false, true> : class_fit_kernel<false, false>);
       fn<<<grid, 256, 0, e->s>>>(t, e->d_left_present.as<uint32_t>(), e->d_fsel.as<uint64_t>(), e->d_ftol.as<uint64_t>(),
                                  e->d_fnz.as<uint32_t>(), e->d_faff.as<uint32_t>(), e->n_fit_classes, n_tiles,
                                  e->d_classfit.as<ColBits>(), c0, e->ipf.d_fipf.as<uint32_t>(),
-                                 e->ipf.d_bits.as<uint32_t>(), e->Npad / 32);
+                                 e->ipf.d_bits.as<uint32_t>(), e->Npad / 32, e->hp.d_fconf.as<uint64_t>(),
+                                 e->hp.d_used.as<uint64_t>());
       tm.launched();
     }
   }
@@ -1259,15 +1301,21 @@ int prepare_nodes(bs_engine* e) {
     CK(e->d_reason_gate.ensure((size_t)e->n_fit_classes * Wg * 4));
     CK(e->d_reason_class.ensure((size_t)e->n_fit_classes * 4 * 4));
     CK(cudaMemsetAsync(e->d_reason_class.p, 0, (size_t)e->n_fit_classes * 4 * 4, e->s));
-    if (e->ipf.on) CK(e->ipf.d_reason_gate.ensure((size_t)e->n_fit_classes * Wg * 4));
+    if (e->ipf.on || e->hp.on) CK(e->filt.d_gate.ensure((size_t)e->n_fit_classes * Wg * 4));
+    if (e->hp.on) {
+      CK(e->hp.d_bins.ensure((size_t)e->n_fit_classes * 4));
+      CK(cudaMemsetAsync(e->hp.d_bins.p, 0, (size_t)e->n_fit_classes * 4, e->s));
+    }
+    const HostPortClassArgs hpa{e->hp.d_fconf.as<uint64_t>(), e->hp.d_used.as<uint64_t>(), e->hp.d_bins.as<uint32_t>()};
     for (uint32_t c0 = 0; c0 < e->n_fit_classes; c0 += 32768) {
       dim3 grid(cdiv(Wg * 32, REASON_CLASS_THREADS), std::min(32768u, e->n_fit_classes - c0));
-      auto fn = e->ipf.on ? reason_class_kernel<true> : reason_class_kernel<false>;
+      auto fn = e->ipf.on ? (e->hp.on ? reason_class_kernel<true, true> : reason_class_kernel<true, false>)
+                          : (e->hp.on ? reason_class_kernel<false, true> : reason_class_kernel<false, false>);
       fn<<<grid, REASON_CLASS_THREADS, 0, e->s>>>(t, e->d_fsel.as<uint64_t>(), e->d_ftol.as<uint64_t>(),
                                                   e->d_faff.as<uint32_t>(), e->n_fit_classes, Wg,
                                                   e->d_reason_gate.as<uint32_t>(), e->d_reason_class.as<uint32_t>(), c0,
                                                   e->ipf.d_fipf.as<uint32_t>(), e->ipf.d_bits.as<uint32_t>(),
-                                                  e->ipf.d_reason_gate.as<uint32_t>());
+                                                  e->filt.d_gate.as<uint32_t>(), hpa);
       tm.launched();
     }
   }
@@ -1342,6 +1390,15 @@ int interpod_filter_check(bs_engine* e, const char* who) {
     return bad(BS_E_INDEX, "a filter class's term is outside the node side's term dictionary");
   if (3ull * e->ipf.pclasses * (e->Npad / 8) > BS_IPF_TABLE_MAX_BYTES)
     return bad(BS_E_INVAL, "3 x filter n_classes x padded nodes / 8 bytes exceeds BS_IPF_TABLE_MAX_BYTES");
+  return BS_OK;
+}
+
+int host_port_check(bs_engine* e, const char* who) {
+  const Refuse bad{e, who};
+  if (!(e->hp.have_node && e->hp.have_pod))
+    return bad(BS_E_STATE, "the PodFitsHostPorts filter needs its node and pod sides");
+  if (e->hp.entries < 64 && (e->hp.want_all >> e->hp.entries))
+    return bad(BS_E_INDEX, "a pod's want bit is outside the node side's host-port dictionary");
   return BS_OK;
 }
 
@@ -1428,11 +1485,11 @@ int interpod_filter_prepass(bs_engine* e) {
 // uploaded again.
 void drop_node_sides(bs_engine* e) {
   e->nz.have_node = e->pref.have_node = e->loc.have_img_node = e->loc.have_avoid_node = e->spread.have_node =
-      e->ipa.have_node = e->ipf.have_node = false;
+      e->ipa.have_node = e->ipf.have_node = e->hp.have_node = false;
 }
 void drop_pod_sides(bs_engine* e) {
   e->nz.have_pod = e->pref.have_pod = e->loc.have_img_pod = e->loc.have_avoid_pod = e->spread.have_pod =
-      e->ipa.have_pod = e->ipf.have_pod = false;
+      e->ipa.have_pod = e->ipf.have_pod = e->hp.have_pod = false;
 }
 
 int evaluate_async_locked(bs_engine* e) {
@@ -1445,6 +1502,7 @@ int evaluate_async_locked(bs_engine* e) {
        (rc = interpod_check(e, "bs_evaluate"))))
     return rc;
   if (e->ipf.on && (rc = interpod_filter_check(e, "bs_evaluate"))) return rc;
+  if (e->hp.on && (rc = host_port_check(e, "bs_evaluate"))) return rc;
   if (e->peer_broken)
     return fail(e, BS_E_PEER, "peer exchange is broken (a rank did not arrive): bs_peer_detach on every rank, then init/attach again");
   if (e->peer_attached && cdiv(std::max(e->G, 1u), 32) > e->peer_wpr) {
@@ -1478,6 +1536,10 @@ int evaluate_async_locked(bs_engine* e) {
   if (e->ipf.on && e->ipf.dirty) {   // new pass bits: the class fit bits and gates are built again
     if ((rc = interpod_filter_prepass(e))) return rc;
     reprepare = true;
+  }
+  if (e->hp.on && e->hp.dirty) {   // new used masks: likewise
+    reprepare = true;
+    e->hp.dirty = false;
   }
   if (reprepare && (rc = prepare_nodes(e))) return rc;
 
@@ -1688,7 +1750,7 @@ int evaluate_async_locked(bs_engine* e) {
   {
     StageTimer tm(e, BS_K_REASONS, e->s);
     if (P && (e->out_flags & BS_OUT_REASONS)) {
-      ReasonArgs ra;
+      ReasonHpArgs ra;
       ra.left = e->d_left_full.as<int64_t>();
       ra.left_present = e->d_left_present.as<uint32_t>();
       ra.gate = e->d_reason_gate.as<uint32_t>();
@@ -1702,8 +1764,19 @@ int evaluate_async_locked(bs_engine* e) {
       ra.ipf_bits = e->ipf.d_bits.as<uint32_t>();
       ra.n_ipf = e->ipf.pclasses;
       ra.ipf_rows = e->ipf.d_reasons.as<uint32_t>();
-      if (e->ipf.on) reason_pod_kernel<true><<<cdiv(P, REASON_PODS_PER_CTA), REASON_THREADS, 0, e->s>>>(ra);
-      else reason_pod_kernel<false><<<cdiv(P, REASON_PODS_PER_CTA), REASON_THREADS, 0, e->s>>>(ra);
+      ra.cconf = e->hp.d_fconf.as<uint64_t>();
+      ra.hp_bins = e->hp.d_bins.as<uint32_t>();
+      ra.used = e->hp.d_used.as<uint64_t>();
+      ra.hp_rows = e->hp.d_reasons.as<uint32_t>();
+      const ReasonArgs& rb = ra;   // the filter-off builds take the base arguments
+      const uint32_t grid = cdiv(P, REASON_PODS_PER_CTA);
+      if (e->hp.on) {
+        auto fn = e->ipf.on ? reason_pod_kernel<true, true> : reason_pod_kernel<false, true>;
+        fn<<<grid, REASON_THREADS, 0, e->s>>>(ra);
+      } else {
+        auto fn = e->ipf.on ? reason_pod_kernel<true, false> : reason_pod_kernel<false, false>;
+        fn<<<grid, REASON_THREADS, 0, e->s>>>(rb);
+      }
       tm.launched();
     }
   }
@@ -1711,7 +1784,7 @@ int evaluate_async_locked(bs_engine* e) {
     PriorityRatioArgs pa;
     pa.left = e->d_left_full.as<int64_t>();
     pa.left_present = e->d_left_present.as<uint32_t>();
-    pa.gate = e->ipf.on ? e->ipf.d_reason_gate.as<uint32_t>() : e->d_reason_gate.as<uint32_t>();
+    pa.gate = (e->ipf.on || e->hp.on) ? e->filt.d_gate.as<uint32_t>() : e->d_reason_gate.as<uint32_t>();
     pa.req = e->d_req.as<int64_t>();
     pa.req_present = e->d_ppres.as<uint32_t>();
     pa.fit_class = e->d_pod_fit_class.as<uint32_t>();
@@ -1788,6 +1861,7 @@ int evaluate_async_locked(bs_engine* e) {
   CK(cudaStreamWaitEvent(e->s, e->ev_join, 0));
   CK(cudaGetLastError());
   e->ipf.round = e->ipf.on;
+  e->hp.round = e->hp.on;
   e->evaluated = true;
   e->fetched = false;
   e->gang_applied = false;
@@ -2159,8 +2233,8 @@ int bs_upload_pods(bs_engine* e, const bs_pod_table* t) {
   if (!e || !t) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
   drop_pod_sides(e);
-  e->ipf.pfc_base_valid = false;   // the new table's fit classes are its base classes
-  e->ipf.assign_dirty = false;
+  e->filt.pfc_base_valid = false;   // the new table's fit classes are its base classes
+  e->filt.assign_dirty = false;
   if (t->n_lanes != e->L) return fail(e, BS_E_INVAL, "bs_upload_pods: n_lanes differs from the engine's");
   const uint32_t P = t->n_pods, L = e->L;
   if (P && (!t->req || !t->req_present || !t->gid || !t->sel_mask || !t->tol_mask || !t->priority ||
@@ -2663,6 +2737,12 @@ int bs_format_fit_error(const uint32_t* counts, uint32_t n_lanes, uint32_t n_nod
 
 int bs_format_fit_error_interpod(const uint32_t* counts, uint32_t n_lanes, const uint32_t* interpod, uint32_t n_nodes,
                                  const char* const* scalar_names, char* buf, size_t buf_len) {
+  return bs_format_fit_error_filters(counts, n_lanes, interpod, nullptr, n_nodes, scalar_names, buf, buf_len);
+}
+
+int bs_format_fit_error_filters(const uint32_t* counts, uint32_t n_lanes, const uint32_t* interpod,
+                                const uint32_t* host_ports, uint32_t n_nodes, const char* const* scalar_names, char* buf,
+                                size_t buf_len) {
   if (!counts || !buf || !buf_len || n_lanes < BS_FIXED_LANES || n_lanes > BS_MAX_LANES) return BS_E_INVAL;
   static const char* const kFixed[4] = {"node(s) were unschedulable", "node(s) were unavailable",
                                         "node(s) didn't match node selector",
@@ -2691,6 +2771,8 @@ int bs_format_fit_error_interpod(const uint32_t* counts, uint32_t n_lanes, const
     for (int k = 0; k < 3; ++k)
       if (interpod[k]) entries.push_back(std::to_string(interpod[k]) + " " + kIpf[k]);
   }
+  if (host_ports && host_ports[0])   // ErrPodNotFitsHostPorts
+    entries.push_back(std::to_string(host_ports[0]) + " node(s) didn't have free ports for the requested pod ports");
   std::sort(entries.begin(), entries.end());   // byte-wise, as Go's sort.Strings
   std::string msg = "0/" + std::to_string(n_nodes) + " nodes are available: ";
   for (size_t k = 0; k < entries.size(); ++k) msg += (k ? ", " : "") + entries[k];
@@ -2767,8 +2849,10 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
   if (scored && !(e->nz.have_node && e->nz.have_pod))
     return fail(e, BS_E_STATE, (w + ": upload both non-zero request columns first").c_str());
   const bool loc = scored && (e->w_img || e->w_avoid);
+  const bool hp = e->hp.on;
   int rc;
   if (loc && (rc = locality_check(e, who))) return rc;
+  if (hp && (rc = host_port_check(e, who))) return rc;
   BS_DEVICE_GUARD(e);
   const uint32_t N = e->N, Npad = e->Npad, P = e->P, G = e->G, L = e->L;
   if (!queue) n_queue = P;
@@ -2801,7 +2885,7 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
   const bool cache = safe && fitmask && n_blocks >= 1 && n_blocks <= (uint32_t)REPLAY_MAX_BLOCKS;
   const size_t rows = cache ? (size_t)2 * e->n_rep_classes * n_blocks : 0, maxl = replay_maxl(L);
   View s_req, s_pc, s_rp, s_matched, s_gflags, s_grc, s_minres, s_mrp, d_queue, d_pf, d_node, d_ready, d_status,
-      n_left0, n_left1, n_both, n_stat, n_fit, c_sum, c_max, c_keys, n_nz;
+      n_left0, n_left1, n_both, n_stat, n_fit, c_sum, c_max, c_keys, n_nz, s_used, d_want, d_conf;
   // The node state and block cache every step reads come first: carved behind the copies, the same kernel took
   // 2 % longer at the bench shape on an H100.
   CK(carve(e->d_replay,
@@ -2810,7 +2894,8 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
             {&c_max, rows * maxl * 8}, {&c_keys, rows * 4}, {&s_req, (size_t)L * Npad * 8}, {&s_pc, (size_t)Npad * 4},
             {&s_rp, (size_t)Npad * 4}, {&s_matched, (size_t)Gp * 4}, {&s_gflags, Gp}, {&s_grc, (size_t)Gp * 4},
             {&s_minres, (size_t)L * Gp * 8}, {&s_mrp, (size_t)Gp * 4}, {&d_queue, (size_t)Qp * 4}, {&d_pf, Qp},
-            {&d_node, (size_t)Qp * 4}, {&d_ready, Qp}, {&d_status, 128}, {&n_nz, scored ? (size_t)2 * Npad * 8 : 0}}));
+            {&d_node, (size_t)Qp * 4}, {&d_ready, Qp}, {&d_status, 128}, {&n_nz, scored ? (size_t)2 * Npad * 8 : 0},
+            {&s_used, hp ? (size_t)Npad * 8 : 0}, {&d_want, hp ? (size_t)P * 8 : 0}, {&d_conf, hp ? (size_t)P * 8 : 0}}));
   auto dup = [&](const View& dst, const DevBuf& src, size_t bytes) {
     return bytes ? cudaMemcpyAsync(dst.p, src.p, bytes, cudaMemcpyDeviceToDevice, e->s) : cudaSuccess;
   };
@@ -2823,9 +2908,20 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
   CK(dup(s_minres, e->d_min_res, (size_t)L * G * 8));
   CK(dup(s_mrp, e->d_mrpres, (size_t)G * 4));
   if (scored) CK(dup(n_nz, e->nz.d_node, (size_t)2 * Npad * 8));
+  std::vector<uint64_t> conf;   // each pod's conflict mask (host_port_check has passed: every want bit is an entry)
+  if (hp) {
+    CK(dup(s_used, e->hp.d_used, (size_t)Npad * 8));
+    conf.assign(P, 0);
+    for (uint32_t p = 0; p < P; ++p)
+      for (uint64_t w = e->hp.h_want[p]; w; w &= w - 1) conf[p] |= e->hp.h_conflict[__builtin_ctzll(w)];
+    if (P) {
+      CK(cudaMemcpyAsync(d_want.p, e->hp.h_want.data(), (size_t)P * 8, cudaMemcpyHostToDevice, e->s));
+      CK(cudaMemcpyAsync(d_conf.p, conf.data(), (size_t)P * 8, cudaMemcpyHostToDevice, e->s));
+    }
+  }
   if (queue && n_queue) CK(cudaMemcpyAsync(d_queue.p, queue, (size_t)n_queue * 4, cudaMemcpyHostToDevice, e->s));
   CK(cudaMemsetAsync(d_status.p, 0, 128, e->s));
-  ReplayLocArgs la{};
+  ReplayHpArgs la{};
   ReplayArgs& a = la;
   a.nt = node_tab(e);
   a.nt.requested = s_req.as<int64_t>();
@@ -2878,9 +2974,14 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
     la.w_img = e->w_img;
     la.w_avoid = e->w_avoid;
   }
+  if (hp) {
+    la.hp_live = s_used.as<uint64_t>();
+    la.hp_want = d_want.as<uint64_t>();
+    la.hp_conf = d_conf.as<uint64_t>();
+  }
   {
     StageTimer tm(e, BS_K_REPLAY, e->s);
-    launch_replay(L, a, scored, loc, e->s);
+    launch_replay(L, a, scored, loc, hp, e->s);
     tm.launched();
     CK(cudaGetLastError());
   }
@@ -2927,10 +3028,16 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
 }  // namespace
 
 // The walks and preemption refuse to run under the MatchInterPodAffinity filter: its presence would have to follow their
-// own placements and victim removals (upstream's metadata AddPod / RemovePod).
+// own placements and victim removals (upstream's metadata AddPod / RemovePod).  Preemption refuses to run under the
+// PodFitsHostPorts filter: its victims' removal would have to take their ports out of the used masks (the walks follow
+// their own placements in a live copy of them).
 static int interpod_filter_refuse(bs_engine* e, const char* who) {
   return fail(e, BS_E_INVAL, (std::string(who) + ": the MatchInterPodAffinity filter is not supported here; "
                               "switch it off with bs_set_interpod_filter").c_str());
+}
+static int host_port_refuse(bs_engine* e, const char* who) {
+  return fail(e, BS_E_INVAL, (std::string(who) + ": the PodFitsHostPorts filter is not supported here; "
+                              "switch it off with bs_set_host_port_filter").c_str());
 }
 
 int bs_replay(bs_engine* e, const uint32_t* queue, uint32_t n_queue, bs_replay_result* out) {
@@ -3123,6 +3230,7 @@ int bs_preempt(bs_engine* e, const uint32_t* pods, uint32_t n, bs_preempt_result
     return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
   if (e->ipf.on) return interpod_filter_refuse(e, "bs_preempt");
+  if (e->hp.on) return host_port_refuse(e, "bs_preempt");
   std::vector<PreemptPod> pp;
   int rc;
   if ((rc = preempt_pods(e, "bs_preempt", pods, n, pp))) return rc;
@@ -3192,6 +3300,7 @@ int bs_preempt_walk(bs_engine* e, const uint32_t* pods, uint32_t n, uint32_t fla
     return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
   if (e->ipf.on) return interpod_filter_refuse(e, "bs_preempt_walk");
+  if (e->hp.on) return host_port_refuse(e, "bs_preempt_walk");
   if (flags & ~BS_PREEMPT_GANG) return fail(e, BS_E_INVAL, "bs_preempt_walk: unknown flag bits");
   const bool gang = flags & BS_PREEMPT_GANG;
   std::vector<PreemptPod> pp;
@@ -3946,7 +4055,7 @@ int bs_set_interpod_filter(bs_engine* e, int on) {
   if ((on != 0) == e->ipf.on) return BS_OK;
   e->ipf.on = on != 0;
   e->ipf.dirty = true;   // the pass bits are built again at the next evaluation the filter is on for
-  e->ipf.assign_dirty = e->classes_dirty = e->pod_classes_dirty = true;   // and the pods' fit classes follow the switch
+  e->filt.assign_dirty = e->classes_dirty = e->pod_classes_dirty = true;   // and the pods' fit classes follow the switch
   e->evaluated = false;
   return BS_OK;
 }
@@ -4002,7 +4111,7 @@ int bs_upload_pod_interpod_filter(bs_engine* e, const bs_interpod_filter_pods* t
   e->ipf.pclasses = C;
   e->ipf.term_max = tmax;
   e->ipf.have_pod = true;
-  e->ipf.assign_dirty = e->classes_dirty = e->pod_classes_dirty = true;   // the pods' fit classes carry the filter class
+  e->filt.assign_dirty = e->classes_dirty = e->pod_classes_dirty = true;   // the pods' fit classes carry the filter class
   e->evaluated = false;
   return BS_OK;
 }
@@ -4020,6 +4129,88 @@ int bs_fetch_interpod_reason_rows(bs_engine* e, uint32_t pod0, uint32_t n, uint3
   BS_DEVICE_GUARD(e);
   CK(cudaMemcpyAsync(counts, e->ipf.d_reasons.as<uint32_t>() + (size_t)pod0 * 3, (size_t)n * 3 * 4,
                      cudaMemcpyDeviceToHost, e->s));
+  CK(cudaStreamSynchronize(e->s));
+  return BS_OK;
+}
+
+int bs_set_host_port_filter(bs_engine* e, int on) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if ((on != 0) == e->hp.on) return BS_OK;
+  e->hp.on = on != 0;
+  e->hp.dirty = true;   // the class fit bits are built again at the next evaluation the filter is on for
+  e->filt.assign_dirty = e->classes_dirty = e->pod_classes_dirty = true;   // and the pods' fit classes follow the switch
+  e->evaluated = false;
+  return BS_OK;
+}
+
+int bs_upload_node_host_ports(bs_engine* e, const bs_host_port_nodes* t) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  const Refuse bad{e, "bs_upload_node_host_ports"};
+  e->hp.have_node = false;
+  if (!t) return bad(BS_E_INVAL, "null table");
+  const uint32_t N = t->n_nodes, K = t->n_entries;
+  if (int rc = bad.shape(NODE_SIDE, N)) return rc;
+  if (K > BS_HOSTPORT_MAX) return bad(BS_E_INVAL, "more than BS_HOSTPORT_MAX entries");
+  if (K && !(t->ip && t->protocol && t->port)) return bad(BS_E_INVAL, "null ip, protocol or port");
+  if (N && !t->used) return bad(BS_E_INVAL, "null used");
+  for (uint32_t a = 0; a < K; ++a)
+    if (t->port[a] < 1 || t->port[a] > 65535) return bad(BS_E_RANGE, "a port is outside 1..65535");
+  // entries a and b conflict: the same protocol and port, and the wildcard on either side or the same ip
+  std::vector<uint64_t> conflict(K, 0);
+  for (uint32_t a = 0; a < K; ++a)
+    for (uint32_t b = 0; b < K; ++b) {
+      if (t->protocol[a] != t->protocol[b] || t->port[a] != t->port[b]) continue;
+      if (a != b && t->ip[a] == t->ip[b]) return bad(BS_E_INVAL, "an entry is listed twice");
+      if (t->ip[a] == BS_HOSTPORT_IP_ANY || t->ip[b] == BS_HOSTPORT_IP_ANY || t->ip[a] == t->ip[b])
+        conflict[a] |= 1ull << b;
+    }
+  uint64_t any = 0;
+  for (uint32_t n = 0; n < N; ++n) any |= t->used[n];
+  if (K < 64 && (any >> K)) return bad(BS_E_INDEX, "a used bit is >= n_entries");
+  BS_DEVICE_GUARD(e);
+  if (int rc = upload_vec(e, e->hp.d_used, t->used, N, e->Npad)) return rc;
+  CK(cudaStreamSynchronize(e->s));
+  e->hp.h_conflict = std::move(conflict);
+  e->hp.h_conflict.resize(BS_HOSTPORT_MAX, 0);   // want bits past n_entries are refused at evaluation
+  e->hp.entries = K;
+  e->hp.have_node = true;
+  e->hp.dirty = true;
+  if (e->hp.on) e->filt.assign_dirty = e->classes_dirty = e->pod_classes_dirty = true;   // new conflict masks
+  e->evaluated = false;
+  return BS_OK;
+}
+
+int bs_upload_pod_host_ports(bs_engine* e, uint32_t n_pods, const uint64_t* want) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  const Refuse bad{e, "bs_upload_pod_host_ports"};
+  e->hp.have_pod = false;
+  if (int rc = bad.shape(POD_SIDE, n_pods)) return rc;
+  if (n_pods && !want) return bad(BS_E_INVAL, "null want");
+  e->hp.h_want.assign(want, want + n_pods);
+  uint64_t all = 0;
+  for (uint32_t p = 0; p < n_pods; ++p) all |= want[p];
+  e->hp.want_all = all;
+  e->hp.have_pod = true;
+  e->filt.assign_dirty = e->classes_dirty = e->pod_classes_dirty = true;   // the pods' fit classes carry the mask
+  e->evaluated = false;
+  return BS_OK;
+}
+
+int bs_fetch_host_port_reason_rows(bs_engine* e, uint32_t pod0, uint32_t n, uint32_t* counts) {
+  if (!e || (n && !counts)) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!e->evaluated || !(e->out_flags & BS_OUT_REASONS)) return fail(e, BS_E_STATE, "no reason rows materialised");
+  if ((uint64_t)pod0 + n > e->P) return BS_E_INDEX;
+  if (!n) return BS_OK;
+  if (!e->hp.round) {
+    memset(counts, 0, (size_t)n * 4);
+    return BS_OK;
+  }
+  BS_DEVICE_GUARD(e);
+  CK(cudaMemcpyAsync(counts, e->hp.d_reasons.as<uint32_t>() + pod0, (size_t)n * 4, cudaMemcpyDeviceToHost, e->s));
   CK(cudaStreamSynchronize(e->s));
   return BS_OK;
 }

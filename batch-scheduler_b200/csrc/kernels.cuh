@@ -7,6 +7,8 @@
 // padded to a multiple of NODE_TILE so tiles can be moved with 1-D TMA bulk
 // copies (cp.async.bulk, 16-byte granules).
 #pragma once
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace bsk {
@@ -365,14 +367,17 @@ __global__ void node_left_class_kernel(NodeTab t, uint64_t sel, uint64_t tol, fl
 // tile*NODE_TILE + j*32 + lane — exactly the TILE_WORDS nodes lane `lane` owns in
 // that tile, so the hot loop needs one coalesced 4-byte load per (pod, tile).  IPF: the MatchInterPodAffinity
 // filter is on, and the bit also needs the pass bit of the class's filter class cipf[c] (interpod_filter.cuh; bit
-// i % 32 of word ipf_pass[cipf[c] * Wg + i / 32]; BS_IPF_NONE passes).  The IPF = false build is the filter-off kernel.
-template <bool IPF>
+// i % 32 of word ipf_pass[cipf[c] * Wg + i / 32]; BS_IPF_NONE passes).  HP: the PodFitsHostPorts filter is on, and
+// the bit also needs (used[i] & cconf[c]) == 0, the node's used host ports against the class's conflict mask.  The
+// IPF = HP = false build is the filter-off kernel.
+template <bool IPF, bool HP>
 __global__ void class_fit_kernel(NodeTab t, const uint32_t* __restrict__ left_present,
                                  const uint64_t* __restrict__ csel, const uint64_t* __restrict__ ctol,
                                  const uint32_t* __restrict__ cnz, const uint32_t* __restrict__ caff,
                                  uint32_t n_classes, uint32_t n_tiles,
                                  ColBits* __restrict__ classfit, uint32_t class0,
-                                 const uint32_t* __restrict__ cipf, const uint32_t* __restrict__ ipf_pass, uint32_t Wg) {
+                                 const uint32_t* __restrict__ cipf, const uint32_t* __restrict__ ipf_pass, uint32_t Wg,
+                                 const uint64_t* __restrict__ cconf, const uint64_t* __restrict__ used) {
   const uint32_t c = class0 + blockIdx.y;   // gridDim.y is capped at 65535: classes go in chunks
   const uint32_t slot = blockIdx.x * blockDim.x + threadIdx.x;  // tile * 32 + lane
   if (slot >= n_tiles * 32 || c >= n_classes) return;
@@ -380,6 +385,7 @@ __global__ void class_fit_kernel(NodeTab t, const uint32_t* __restrict__ left_pr
   const uint64_t sel = csel[c], tol = ctol[c];
   const uint32_t nz = cnz[c], aff = caff[c];
   const uint32_t ipf = IPF ? cipf[c] : BS_IPF_NONE;
+  const uint64_t conf = HP ? cconf[c] : 0;
   ColBits bits = 0;
 #pragma unroll
   for (int j = 0; j < TILE_WORDS; ++j) {
@@ -390,6 +396,7 @@ __global__ void class_fit_kernel(NodeTab t, const uint32_t* __restrict__ left_pr
       ok = !node_skipped(f) && !(f & BS_NODE_TAINTS_ERR) && check_fit(t.label[i], t.taint[i], sel, tol) &&
            aff_ok(t, aff, i) && ((nz & ~left_present[i]) == 0);
       if (IPF && ipf != BS_IPF_NONE) ok = ok && ((ipf_pass[(size_t)ipf * Wg + (i >> 5)] >> (i & 31)) & 1u);
+      if (HP && conf) ok = ok && (used[i] & conf) == 0;
     }
     bits |= (ColBits)(ok ? 1u : 0u) << j;
   }
@@ -405,23 +412,32 @@ __global__ void class_fit_kernel(NodeTab t, const uint32_t* __restrict__ left_pr
 // (Wg * 32 threads cover the padded table: gate bits of padding nodes are 0), one ballot per warp and bin, one
 // global atomic per CTA and bin into class_bins[c][4] (zeroed before the launch).  IPF: the MatchInterPodAffinity
 // filter is on, and the kernel also writes gate_ipf = the gate AND the pass bits of the class's filter class, the fit
-// set's gate of the priority lists; the gate itself stays the lane sweep's.  The IPF = false build is the filter-off
-// kernel.
+// set's gate of the priority lists; the gate itself stays the lane sweep's.  HP: the PodFitsHostPorts filter is on;
+// the kernel counts into hp_bins[c] (zeroed before the launch) the nodes past the guards whose used host ports
+// conflict with the class's conflict mask, whatever their other bins, and gate_ipf also needs no conflict.  The
+// IPF = HP = false build is the filter-off kernel.
 constexpr int REASON_CLASS_THREADS = 256;
-template <bool IPF>
+struct HostPortClassArgs {
+  const uint64_t* cconf;   // [classes] conflict mask of each fit class
+  const uint64_t* used;    // [Npad] used host ports of each node
+  uint32_t* hp_bins;       // [classes]
+};
+template <bool IPF, bool HP>
 __global__ void __launch_bounds__(REASON_CLASS_THREADS)
 reason_class_kernel(NodeTab t, const uint64_t* __restrict__ csel, const uint64_t* __restrict__ ctol,
                     const uint32_t* __restrict__ caff, uint32_t n_classes, uint32_t Wg,
                     uint32_t* __restrict__ gate, uint32_t* __restrict__ class_bins, uint32_t class0,
                     const uint32_t* __restrict__ cipf, const uint32_t* __restrict__ ipf_pass,
-                    uint32_t* __restrict__ gate_ipf) {
+                    uint32_t* __restrict__ gate_ipf, HostPortClassArgs hpa) {
   const uint32_t c = class0 + blockIdx.y;   // gridDim.y is capped at 65535: classes go in chunks
   if (c >= n_classes) return;
   __shared__ uint32_t s_bins[4];
+  __shared__ uint32_t s_hp;
   if (threadIdx.x < 4) s_bins[threadIdx.x] = 0;
+  if (HP && threadIdx.x == 4) s_hp = 0;
   __syncthreads();
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x, lane = threadIdx.x & 31;
-  bool unsched = false, unavail = false, sel_bad = false, taint_bad = false, pass = false;
+  bool unsched = false, unavail = false, sel_bad = false, taint_bad = false, pass = false, port_bad = false;
   if (i < t.N) {
     const uint8_t f = t.flags[i];
     if (node_skipped(f) || (f & BS_NODE_TAINTS_ERR)) {
@@ -434,14 +450,18 @@ reason_class_kernel(NodeTab t, const uint64_t* __restrict__ csel, const uint64_t
       sel_bad = !check_fit(label, 0, sel, 0) || !aff_ok(t, caff[c], i);
       taint_bad = !check_fit(~0ull, taint, 0, tol);
       pass = !sel_bad && !taint_bad;
+      if (HP) port_bad = (hpa.used[i] & hpa.cconf[c]) != 0;
     }
   }
   const uint32_t gw = __ballot_sync(0xffffffffu, pass);
   if (lane == 0 && (i >> 5) < Wg) gate[(size_t)c * Wg + (i >> 5)] = gw;
-  if (IPF && lane == 0 && (i >> 5) < Wg) {
-    const uint32_t ipf = cipf[c];
-    gate_ipf[(size_t)c * Wg + (i >> 5)] = ipf == BS_IPF_NONE ? gw : gw & ipf_pass[(size_t)ipf * Wg + (i >> 5)];
+  const uint32_t pw = HP ? __ballot_sync(0xffffffffu, port_bad) : 0u;
+  if ((IPF || HP) && lane == 0 && (i >> 5) < Wg) {
+    const uint32_t ipf = IPF ? cipf[c] : BS_IPF_NONE;
+    const uint32_t g2 = HP ? gw & ~pw : gw;
+    gate_ipf[(size_t)c * Wg + (i >> 5)] = ipf == BS_IPF_NONE ? g2 : g2 & ipf_pass[(size_t)ipf * Wg + (i >> 5)];
   }
+  if (HP && lane == 0 && pw) atomicAdd(&s_hp, (uint32_t)__popc(pw));
   const uint32_t b0 = __popc(__ballot_sync(0xffffffffu, unsched)), b1 = __popc(__ballot_sync(0xffffffffu, unavail));
   const uint32_t b2 = __popc(__ballot_sync(0xffffffffu, sel_bad)), b3 = __popc(__ballot_sync(0xffffffffu, taint_bad));
   if (lane == 0) {
@@ -452,6 +472,7 @@ reason_class_kernel(NodeTab t, const uint64_t* __restrict__ csel, const uint64_t
   }
   __syncthreads();
   if (threadIdx.x < 4 && s_bins[threadIdx.x]) atomicAdd(&class_bins[(size_t)c * 4 + threadIdx.x], s_bins[threadIdx.x]);
+  if (HP && threadIdx.x == 0 && s_hp) atomicAdd(&hpa.hp_bins[c], s_hp);
 }
 
 // K1d reason_pod_kernel — the lane bins of a reason row.  A warp takes REASON_PPW pods and sweeps every node 32 at a
@@ -461,8 +482,9 @@ reason_class_kernel(NodeTab t, const uint64_t* __restrict__ csel, const uint64_t
 // req != 0, or when req > left.  Every short lane counts (the reference stops at the first).  Counters stay in
 // registers, are summed across the warp once at the end, and each (pod, bin) is stored once; bins 0-3 are copied
 // from the pod's class.  IPF: the MatchInterPodAffinity filter is on, and a gated node with no short lane that fails
-// the filter counts in ipf_rows[p][3] by the step that failed it (E, A, N; interpod_filter.cuh's planes).  The
-// IPF = false build is the filter-off kernel.
+// the filter counts in ipf_rows[p][3] by the step that failed it (E, A, N; interpod_filter.cuh's planes).  HP: the
+// PodFitsHostPorts filter is on; hp_rows[p] is copied from the pod's class (reason_class_kernel's hp_bins), and a
+// node with a port conflict counts in no ipf_rows bin.  The IPF = HP = false build is the filter-off kernel.
 constexpr int REASON_THREADS = 256;
 constexpr int REASON_PPW = 4;                                         // pods per warp
 constexpr int REASON_PODS_PER_CTA = (REASON_THREADS / 32) * REASON_PPW;
@@ -482,8 +504,17 @@ struct ReasonArgs {
   uint32_t n_ipf;
   uint32_t* ipf_rows;
 };
-template <bool IPF>
-__global__ void __launch_bounds__(REASON_THREADS) reason_pod_kernel(ReasonArgs a) {
+// HP only: each fit class's conflict mask and port bin, each node's used host ports [Npad] and the rows [P]
+struct ReasonHpArgs : ReasonArgs {
+  const uint64_t* cconf;
+  const uint32_t* hp_bins;
+  const uint64_t* used;
+  uint32_t* hp_rows;
+};
+template <bool HP>
+using ReasonArgsOf = typename std::conditional<HP, ReasonHpArgs, ReasonArgs>::type;
+template <bool IPF, bool HP>
+__global__ void __launch_bounds__(REASON_THREADS) reason_pod_kernel(ReasonArgsOf<HP> a) {
   __shared__ int64_t s_req[REASON_THREADS / 32][REASON_PPW][BS_MAX_LANES];
   const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const uint32_t p0 = (blockIdx.x * (REASON_THREADS / 32) + wid) * REASON_PPW;
@@ -496,6 +527,7 @@ __global__ void __launch_bounds__(REASON_THREADS) reason_pod_kernel(ReasonArgs a
   uint32_t rmask[REASON_PPW];   // lanes compared: 0-3 always, scalar lanes the pod requests
   const uint32_t* grow[REASON_PPW];
   const uint32_t* frow[REASON_PPW];   // IPF: the pass plane row of the pod's filter class, or null
+  uint64_t conf[REASON_PPW];          // HP: the conflict mask of the pod's class
 #pragma unroll
   for (int j = 0; j < REASON_PPW; ++j) {
     const uint32_t p = p0 + j;
@@ -505,6 +537,10 @@ __global__ void __launch_bounds__(REASON_THREADS) reason_pod_kernel(ReasonArgs a
     if (IPF) {
       const uint32_t f = ok ? a.cipf[a.fit_class[p]] : BS_IPF_NONE;
       frow[j] = f == BS_IPF_NONE ? nullptr : a.ipf_bits + (size_t)f * a.Wg;
+    }
+    if constexpr (HP) {
+      conf[j] = ok ? a.cconf[a.fit_class[p]] : 0ull;
+      if (ok && lane == 0) a.hp_rows[p] = a.hp_bins[a.fit_class[p]];
     }
   }
   uint32_t cnt[REASON_PPW][BS_MAX_LANES];
@@ -546,9 +582,12 @@ __global__ void __launch_bounds__(REASON_THREADS) reason_pod_kernel(ReasonArgs a
     }
     if (IPF) {
       const size_t plane = (size_t)a.n_ipf * a.Wg;
+      uint64_t used = 0;
+      if constexpr (HP) used = a.used[i];
 #pragma unroll
       for (int j = 0; j < REASON_PPW; ++j) {
         if (!g[j] || any_short[j] || !frow[j] || ((frow[j][w] >> lane) & 1u)) continue;
+        if (HP && (used & conf[j])) continue;   // GeneralPredicates failed first
         const bool e_bit = (frow[j][plane + w] >> lane) & 1u, a_bit = (frow[j][2 * plane + w] >> lane) & 1u;
         icnt[j][0] += e_bit ? 1u : 0u;
         icnt[j][1] += !e_bit && a_bit ? 1u : 0u;

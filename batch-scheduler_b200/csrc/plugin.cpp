@@ -983,6 +983,8 @@ Status BatchSchedulingPlugin::BeginRound(const std::vector<const NodeInfo*>& sna
     if (!nst.ok()) return nst;
     nst = UploadInterPodFilter();
     if (!nst.ok()) return nst;
+    nst = UploadHostPorts();
+    if (!nst.ok()) return nst;
   }
   {
     Status bst = UploadBound();   // after the groups: the bound rows' group indices refer to this table
@@ -1101,9 +1103,15 @@ int BatchSchedulingPlugin::FetchReasons() {
   reasons_.assign((size_t)P * (4 + packed_.lanes), 0);
   const int rc = bs_fetch_reason_rows(eng_, 0, P, reasons_.data());
   ipf_reasons_.clear();
-  if (rc || !interpod_filter_) return rc;
-  ipf_reasons_.assign((size_t)P * 3, 0);
-  return bs_fetch_interpod_reason_rows(eng_, 0, P, ipf_reasons_.data());
+  hp_reasons_.clear();
+  if (rc) return rc;
+  if (interpod_filter_) {
+    ipf_reasons_.assign((size_t)P * 3, 0);
+    if (int r = bs_fetch_interpod_reason_rows(eng_, 0, P, ipf_reasons_.data())) return r;
+  }
+  if (!host_port_filter_) return BS_OK;
+  hp_reasons_.assign(P, 0);
+  return bs_fetch_host_port_reason_rows(eng_, 0, P, hp_reasons_.data());
 }
 
 int BatchSchedulingPlugin::FetchPriority() {
@@ -2048,6 +2056,104 @@ Status BatchSchedulingPlugin::UploadInterPodFilter() {
   return rc ? fail(rc) : Status{};
 }
 
+void BatchSchedulingPlugin::SetHostPortFilter(bool on) {
+  std::lock_guard<std::mutex> lk(mu_);
+  host_port_filter_ = on;
+}
+
+namespace {
+struct HostPortTriple {
+  std::string ip, protocol;
+  int32_t port;
+  bool operator==(const HostPortTriple& o) const { return port == o.port && ip == o.ip && protocol == o.protocol; }
+};
+// HostPortInfo's sanitizing: port <= 0 is not a host port, "" ip is "0.0.0.0", "" protocol is "TCP"
+void add_triples(const std::vector<ContainerPort>& ports, std::vector<HostPortTriple>* out) {
+  for (const ContainerPort& cp : ports) {
+    if (cp.host_port <= 0) continue;
+    HostPortTriple t{cp.host_ip.empty() ? "0.0.0.0" : cp.host_ip, cp.protocol.empty() ? "TCP" : cp.protocol,
+                     cp.host_port};
+    if (std::find(out->begin(), out->end(), t) == out->end()) out->push_back(t);
+  }
+}
+bool triples_conflict(const HostPortTriple& a, const HostPortTriple& b) {
+  return a.protocol == b.protocol && a.port == b.port && (a.ip == "0.0.0.0" || b.ip == "0.0.0.0" || a.ip == b.ip);
+}
+}  // namespace
+
+Status BatchSchedulingPlugin::PackHostPorts(const std::vector<const NodeInfo*>& snapshot,
+                                            const std::vector<const Pod*>& pending, PackedHostPorts* out) {
+  if (!out) return Status{BS_CODE_ERROR, "PackHostPorts: null output"};
+  *out = PackedHostPorts{};
+  std::vector<HostPortTriple> dict;
+  std::vector<std::vector<HostPortTriple>> wanted(pending.size()), used(snapshot.size());
+  for (size_t p = 0; p < pending.size(); ++p) {
+    if (pending[p])
+      for (const Container& c : pending[p]->containers) add_triples(c.ports, &wanted[p]);
+    for (const HostPortTriple& t : wanted[p])
+      if (std::find(dict.begin(), dict.end(), t) == dict.end()) dict.push_back(t);
+  }
+  const size_t n_wanted = dict.size();
+  for (size_t n = 0; n < snapshot.size(); ++n) {
+    if (snapshot[n]) add_triples(snapshot[n]->used_ports, &used[n]);
+    for (const HostPortTriple& t : used[n]) {
+      if (std::find(dict.begin(), dict.end(), t) != dict.end()) continue;
+      for (size_t k = 0; k < n_wanted; ++k)
+        if (triples_conflict(dict[k], t)) {
+          dict.push_back(t);
+          break;
+        }
+    }
+  }
+  if (dict.size() > BS_HOSTPORT_MAX)
+    return Status{BS_CODE_ERROR, "PackHostPorts: " + std::to_string(dict.size()) + " host-port entries, more than BS_HOSTPORT_MAX"};
+  auto id = [](std::vector<std::string>& names, const std::string& s) {
+    const auto it = std::find(names.begin(), names.end(), s);
+    if (it != names.end()) return (uint32_t)(it - names.begin());
+    names.push_back(s);
+    return (uint32_t)names.size() - 1;
+  };
+  for (const HostPortTriple& t : dict) {
+    out->ip.push_back(id(out->ips, t.ip));
+    out->protocol.push_back(id(out->protocols, t.protocol));
+    out->port.push_back(t.port);
+  }
+  auto mask = [&dict](const std::vector<HostPortTriple>& ts) {
+    uint64_t m = 0;
+    for (const HostPortTriple& t : ts) {
+      const auto it = std::find(dict.begin(), dict.end(), t);
+      if (it != dict.end()) m |= 1ull << (it - dict.begin());
+    }
+    return m;
+  };
+  for (const auto& ts : used) out->used.push_back(mask(ts));
+  for (const auto& ts : wanted) out->want.push_back(mask(ts));
+  return Status{};
+}
+
+Status BatchSchedulingPlugin::UploadHostPorts() {
+  auto fail = [&](int rc) {
+    return Status{BS_CODE_ERROR, std::string("bsched: ") + bs_strerror(rc) + " (" + bs_last_error(eng_) + ")"};
+  };
+  int rc = bs_set_host_port_filter(eng_, host_port_filter_ ? 1 : 0);
+  if (rc) return fail(rc);
+  if (!host_port_filter_) return Status{};
+  PackedHostPorts pk;
+  Status st = PackHostPorts(snapshot_, pending_, &pk);
+  if (!st.ok()) return st;
+  bs_host_port_nodes nt{(uint32_t)snapshot_.size(), (uint32_t)pk.port.size(), pk.ip.data(), pk.protocol.data(),
+                        pk.port.data(), pk.used.data()};
+  rc = bs_upload_node_host_ports(eng_, &nt);
+  if (!rc) rc = bs_upload_pod_host_ports(eng_, (uint32_t)pending_.size(), pk.want.data());
+  return rc ? fail(rc) : Status{};
+}
+
+std::vector<uint32_t> BatchSchedulingPlugin::HostPortReasonCounts(const std::string& uid) const {
+  const int32_t row = pod_row_.find(uid);
+  if (row < 0 || hp_reasons_.size() <= (size_t)row) return {};
+  return {hp_reasons_[row]};
+}
+
 std::vector<uint32_t> BatchSchedulingPlugin::InterPodReasonCounts(const std::string& uid) const {
   const int32_t row = pod_row_.find(uid);
   if (row < 0 || ipf_reasons_.size() < ((size_t)row + 1) * 3) return {};
@@ -2094,11 +2200,12 @@ std::string BatchSchedulingPlugin::FitError(const std::string& uid) const {
   std::vector<const char*> names;
   for (auto& nm : packed_.scalar_names) names.push_back(nm.c_str());
   const std::vector<uint32_t> ipf = InterPodReasonCounts(uid);   // empty while the filter is off
+  const std::vector<uint32_t> hp = HostPortReasonCounts(uid);     // likewise
   std::vector<char> buf(256);
   for (;;) {   // grows until the whole message fits
-    const int rc = bs_format_fit_error_interpod(counts.data(), packed_.lanes, ipf.empty() ? nullptr : ipf.data(),
-                                                packed_.n_nodes, names.empty() ? nullptr : names.data(), buf.data(),
-                                                buf.size());
+    const int rc = bs_format_fit_error_filters(counts.data(), packed_.lanes, ipf.empty() ? nullptr : ipf.data(),
+                                               hp.empty() ? nullptr : hp.data(), packed_.n_nodes,
+                                               names.empty() ? nullptr : names.data(), buf.data(), buf.size());
     if (rc == BS_OK) return std::string(buf.data());
     if (buf.size() > (1u << 20)) return "";
     buf.resize(buf.size() * 4);
@@ -2123,6 +2230,8 @@ Status BatchSchedulingPlugin::UpdateRound(const std::vector<std::pair<uint32_t, 
     st = UploadInterPodAffinity();
     if (!st.ok()) return st;
     st = UploadInterPodFilter();
+    if (!st.ok()) return st;
+    st = UploadHostPorts();
     if (!st.ok()) return st;
   }
   return Reevaluate();
@@ -2183,6 +2292,8 @@ Status BatchSchedulingPlugin::UpdateNodes(const std::vector<std::pair<uint32_t, 
   st = UploadInterPodAffinity();   // ... and the inter-pod side (the changed NodeInfos' pods and labels: both sides)
   if (!st.ok()) return st;
   st = UploadInterPodFilter();     // ... and the filter's sides, for the same reasons
+  if (!st.ok()) return st;
+  st = UploadHostPorts();          // ... and the host-port sides (the changed NodeInfos' used ports)
   if (!st.ok()) return st;
   // the round's decisions follow the new snapshot: same pods, same groups, same result vectors
   return evaluate ? Reevaluate() : Status{};
@@ -2395,6 +2506,8 @@ Status BatchSchedulingPlugin::Preempt(const std::string& uid, std::string* node,
   std::lock_guard<std::mutex> lk(mu_);
   if (interpod_filter_)
     return Status{BS_CODE_ERROR, "Preempt: the MatchInterPodAffinity filter is on (SetInterPodAffinityFilter(false) first)"};
+  if (host_port_filter_)
+    return Status{BS_CODE_ERROR, "Preempt: the PodFitsHostPorts filter is on (SetHostPortFilter(false) first)"};
   const int32_t p = pod_row_.find(uid);
   if (!eng_ || p < 0) return Status{BS_CODE_ERROR, "Preempt: " + uid + " is not a pending pod of the round"};
   if (!bound_.n) {   // no NodeInfo lists pods: nothing to evict, the table was never uploaded
@@ -2415,6 +2528,8 @@ Status BatchSchedulingPlugin::PreemptAll(std::vector<Preemption>* out) {
   if (!eng_ || !out) return Status{BS_CODE_ERROR, "PreemptAll: no round has been started"};
   if (interpod_filter_)
     return Status{BS_CODE_ERROR, "PreemptAll: the MatchInterPodAffinity filter is on (SetInterPodAffinityFilter(false) first)"};
+  if (host_port_filter_)
+    return Status{BS_CODE_ERROR, "PreemptAll: the PodFitsHostPorts filter is on (SetHostPortFilter(false) first)"};
   out->clear();
   if (!bound_.n) return Status{};
   std::vector<uint32_t> rows;
@@ -2432,6 +2547,8 @@ Status BatchSchedulingPlugin::PreemptQueue(std::vector<Preemption>* out, bool ga
   if (!eng_ || !out) return Status{BS_CODE_ERROR, "PreemptQueue: no round has been started"};
   if (interpod_filter_)
     return Status{BS_CODE_ERROR, "PreemptQueue: the MatchInterPodAffinity filter is on (SetInterPodAffinityFilter(false) first)"};
+  if (host_port_filter_)
+    return Status{BS_CODE_ERROR, "PreemptQueue: the PodFitsHostPorts filter is on (SetHostPortFilter(false) first)"};
   out->clear();
   if (!bound_.n) return Status{};
   // PreemptAll's pods in queue order; with gang units, one unit per group at its first preemptor's place

@@ -31,11 +31,19 @@ using ResourceList = std::vector<std::pair<std::string, std::string>>;
 
 constexpr const char* kPodGroupLabel = "group.batch.scheduler.tencent.com";  // pkg/util/types.go:25
 
+// v1.ContainerPort: the fields PodFitsHostPorts reads (HostPort; ContainerPort is what hostNetwork defaults it from)
+struct ContainerPort {
+  std::string host_ip;      // "" = "0.0.0.0"
+  std::string protocol;     // "" = "TCP"
+  int32_t host_port = 0;    // <= 0: not a host port
+  int32_t container_port = 0;
+};
 struct Container {
   bool has_limits = false;  // Resources.Limits != nil  (core.go:765)
   ResourceList limits;
   ResourceList requests;
   std::string image;        // Spec.Containers[].Image as written (ImageLocality normalizes it)
+  std::vector<ContainerPort> ports;   // Spec.Containers[].Ports (init containers are not Containers)
 };
 struct Toleration {
   std::string key, op /* "", "Equal", "Exists" */, value, effect;
@@ -170,6 +178,7 @@ struct NodeInfo {          // k8s.io/kubernetes/pkg/scheduler/nodeinfo.NodeInfo,
   int32_t num_pods = 0;        // len(info.Pods())
   bool taints_error = false;   // info.Taints() returned an error (core.go:639)
   std::vector<const Pod*> pods;   // info.Pods(): the pods bound to the node, what preemption may evict (may be empty)
+  std::vector<ContainerPort> used_ports;   // info.UsedPorts() flattened, as the caller supplies it (not derived from pods)
 };
 struct PodGroup {          // pkg/apis/podgroup/v1/types.go:62-130 (fields on the path)
   std::string ns, name;
@@ -318,6 +327,16 @@ struct PackedInterPodAffinity {
 // bs_upload_pod_interpod_filter): keys, values and topo as PackedInterPodAffinity numbers them; the filter's own term
 // dictionary (term_signatures); the bound pods of NodeInfo::pods and their classes of (term, own, match); each pending
 // pod's class of (term, role) with its self_match byte.
+// The columns of the PodFitsHostPorts filter of one round (bs_upload_node_host_ports, bs_upload_pod_host_ports): the
+// dictionary (ip id, protocol id, port; ip id 0 = "0.0.0.0", the other ips and the protocols numbered by first
+// appearance), each node's used mask and each pending pod's want mask.
+struct PackedHostPorts {
+  std::vector<uint32_t> ip, protocol;
+  std::vector<int32_t> port;
+  std::vector<uint64_t> used;   // [n_nodes]
+  std::vector<uint64_t> want;   // [n_pods]
+  std::vector<std::string> ips{"0.0.0.0"}, protocols;   // id -> text
+};
 struct PackedInterPodFilter {
   std::vector<std::string> keys;
   std::vector<std::vector<std::string>> values;
@@ -529,6 +548,13 @@ class BatchSchedulingPlugin {
   // default), from the next round, delta round or UpdateNodes on: PackInterPodFilter's columns are uploaded with each
   // of them.  While it is on, ReplayQueue, Preempt, PreemptAll and PreemptQueue return an error.
   void SetInterPodAffinityFilter(bool on);
+  // kube-scheduler v1.17's PodFitsHostPorts filter in every pod's fit set and in ReplayQueue (bs_set_host_port_filter;
+  // off by default), from the next round, delta round or UpdateNodes on: PackHostPorts' columns are uploaded with each
+  // of them.  While it is on, Preempt, PreemptAll and PreemptQueue return an error.
+  void SetHostPortFilter(bool on);
+  // the last round's host-port companion count of a pending pod (bs_fetch_host_port_reason_rows); empty without
+  // BS_OUT_REASONS, while the filter is off or for an unknown uid
+  std::vector<uint32_t> HostPortReasonCounts(const std::string& uid) const;
   // the last round's companion reason row of a pending pod (bs_fetch_interpod_reason_rows: the nodes that pass every
   // other check and fail the filter at E, A, N); empty without BS_OUT_REASONS or for an unknown uid
   std::vector<uint32_t> InterPodReasonCounts(const std::string& uid) const;
@@ -657,6 +683,12 @@ class BatchSchedulingPlugin {
   // More than BS_IPA_KEY_MAX keys, BS_IPF_BOUND_MAX bound pods or BS_IPF_CLASS_MAX entries in a class is an error.
   static Status PackInterPodFilter(const std::vector<const NodeInfo*>& snapshot, const std::vector<const Pod*>& pending,
                                    PackedInterPodFilter* out);
+  // PodFitsHostPorts' columns: HostPortInfo's sanitizing (port <= 0 dropped, "" ip = "0.0.0.0", "" protocol = "TCP");
+  // the dictionary holds the pending pods' wanted (ip, protocol, port) in order of first appearance, then the nodes'
+  // used ones that conflict with one of them (a used entry that conflicts with nothing wanted never decides a verdict).
+  // More than BS_HOSTPORT_MAX entries is an error.
+  static Status PackHostPorts(const std::vector<const NodeInfo*>& snapshot, const std::vector<const Pod*>& pending,
+                              PackedHostPorts* out);
 
   static Status Pack(const std::vector<const NodeInfo*>& snapshot, const std::vector<const Pod*>& pending,
                      const std::vector<PodGroup>& groups, const std::vector<uint32_t>& matched,
@@ -693,6 +725,7 @@ class BatchSchedulingPlugin {
   uint32_t interpod_weight_ = 0;                        // SetInterPodAffinityWeight
   int32_t hard_pod_affinity_weight_ = 1;                // SetHardPodAffinityWeight
   bool interpod_filter_ = false;                        // SetInterPodAffinityFilter
+  bool host_port_filter_ = false;                       // SetHostPortFilter
   std::string init_error_;
   int64_t max_schedule_time_ns_;
   std::map<std::string, GroupState> groups_;                        // ordered: canonical table order
@@ -714,6 +747,7 @@ class BatchSchedulingPlugin {
   std::vector<int64_t> topk_score_;
   std::vector<uint32_t> reasons_;                                   // [P][4 + lanes] (BS_OUT_REASONS)
   std::vector<uint32_t> ipf_reasons_;                               // [P][3] companion rows (BS_OUT_REASONS)
+  std::vector<uint32_t> hp_reasons_;                                // [P] host-port companion (BS_OUT_REASONS)
   std::vector<int32_t> prio_node_;                                  // [P][priority_k_] (BS_OUT_PRIORITY)
   std::vector<int64_t> prio_score_;
   int64_t now_ns_ = 0;
@@ -732,6 +766,7 @@ class BatchSchedulingPlugin {
   Status UploadInterPodAffinity();   // both inter-pod sides of snapshot_ and pending_ and the weight; the columns
                                     // only while the weight is non-zero; no-op without priority_k
   Status UploadInterPodFilter();   // the filter switch and, while it is on, both filter sides of snapshot_ and pending_
+  Status UploadHostPorts();        // likewise for the PodFitsHostPorts filter
   Status UploadLocality();   // both locality sides of snapshot_ and pending_ and the two weights; the columns only
                              // while a weight is non-zero; no-op without priority_k
   Status UploadBound();  // packs and uploads the bound-pod table of snapshot_ (no-op when no NodeInfo lists pods)

@@ -37,9 +37,12 @@
 //                      which the walk does not change: the round's IL table and avoid masks.  In both,
 //                      requests only grow `requested`, so a leading run of nodes no pod of the table
 //                      can ever fit again (or that is skipped) is remembered and not rescanned; such
-//                      a node never fits, so it never scores either;
+//                      a node never fits, so it never scores either.  HP (the PodFitsHostPorts filter
+//                      is on): a node whose live used-port mask conflicts with the pod's is not a
+//                      candidate; the dead-node skip stays resource-only;
 //   assume + Permit    a handful of stores by the first lanes (SCORED: the chosen node's live
-//                      non-zero column grows by the pod's, NodeInfo.AddPod's nonzeroRequest).
+//                      non-zero column grows by the pod's, NodeInfo.AddPod's nonzeroRequest; HP: the
+//                      pod's wanted entries join the node's live used-port mask).
 // Mutable state lives in scratch copies (requested, pod_count, req_present, matched, group flags,
 // representative class, MinResources, the live non-zero column); the uploaded tables are untouched.
 #pragma once
@@ -108,6 +111,14 @@ struct ReplayLocArgs : ReplayArgs {
   const uint8_t* avoid_bit;     // [P]
   uint32_t w_img, w_avoid;
 };
+// HP's arguments: derived again, so that the kernels without the filter keep theirs
+struct ReplayHpArgs : ReplayLocArgs {
+  uint64_t* hp_live;            // [Npad] scratch copy of the node side's used masks
+  const uint64_t* hp_want;      // [P] each pod's want mask
+  const uint64_t* hp_conf;      // [P] each pod's conflict mask (the OR of its wanted entries')
+};
+template <bool LOC, bool HP>
+using ReplayArgsOf = std::conditional_t<HP, ReplayHpArgs, std::conditional_t<LOC, ReplayLocArgs, ReplayArgs>>;
 
 template <int MAXL>
 struct ReplaySmem {
@@ -225,8 +236,8 @@ __device__ __forceinline__ void block_scan(ReplaySmem<MAXL>& sm, int64_t (&v)[RE
   for (int k = 0; k < REPLAY_NPT; ++k) keys[k] |= fk;
 }
 
-template <int MAXL, bool SCORED, bool RATIO = false, bool LOC = false>
-__global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(std::conditional_t<LOC, ReplayLocArgs, ReplayArgs> a) {
+template <int MAXL, bool SCORED, bool RATIO = false, bool LOC = false, bool HP = false>
+__global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(ReplayArgsOf<LOC, HP> a) {
   static_assert(SCORED || !RATIO, "the ratio term belongs to the scored node choice");
   static_assert(SCORED || !LOC, "the locality terms belong to the scored node choice");
   __shared__ ReplaySmem<MAXL> sm;
@@ -320,6 +331,8 @@ __global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(std::conditio
   // SCORED: the pod's non-zero pair (cpu, memory), one slot per step parity like sm.req; a separate array, so that the
   // first-fit kernel's shared memory stays as it is
   __shared__ int64_t s_pod_nz[2][2];
+  // HP: the pod's want and conflict masks, likewise (in shared memory: the 16-lane build has no registers to spare)
+  __shared__ uint64_t s_hp[2][2];
   struct PodRow { uint32_t p; int32_t g; uint8_t pf; uint32_t keys, rc; };
   auto load_row = [&](uint32_t qi, int slot) {
     PodRow r;
@@ -329,6 +342,8 @@ __global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(std::conditio
     const uint32_t ppres = a.pt.req_present[r.p];
     r.keys = ppres & ~0xFu;
     r.rc = a.pt.rep_class[r.p];
+    if constexpr (HP)
+      if (tid < 2) s_hp[slot][tid] = tid ? a.hp_conf[r.p] : a.hp_want[r.p];
     if constexpr (SCORED)
       if (tid < 2) s_pod_nz[slot][tid] = a.pod_nz[(size_t)tid * P + r.p];
     if (tid < L)   // getPodResourceRequire (core.go:761-772): the packer summed the containers
@@ -638,6 +653,20 @@ __global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(std::conditio
           if (((usable & cf) >> k) & 1u)
             if (compare_lanes<MAXL>(v[k], keys[k], req, req_keys)) fit |= 1u << k;
         }
+        if constexpr (HP) {
+          const uint64_t conf = s_hp[par][1];
+          if (conf) {   // uniform: the pod's row
+            const uint32_t i0 = base + REPLAY_NPT * tid;
+            if (i0 < Npad) {
+              const ulonglong2* src = reinterpret_cast<const ulonglong2*>(a.hp_live + i0);
+              const ulonglong2 x = src[0], y = src[1];
+              const uint64_t u[REPLAY_NPT] = {x.x, x.y, y.x, y.y};
+#pragma unroll
+              for (int k = 0; k < REPLAY_NPT; ++k)
+                if (u[k] & conf) fit &= ~(1u << k);
+            }
+          }
+        }
         if constexpr (SCORED) {
           // nodes come in ascending order per thread: only a strictly higher score replaces the best
           const int64_t pnz0 = s_pod_nz[par][0], pnz1 = s_pod_nz[par][1];
@@ -753,6 +782,8 @@ __global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(std::conditio
         }
         if constexpr (SCORED)   // NodeInfo.AddPod grows the node's non-zero requests by the pod's
           if (tid >= 96 && tid < 98) a.nz_live[(size_t)(tid - 96) * Npad + n] += s_pod_nz[par][tid - 96];
+        if constexpr (HP)   // NodeInfo.AddPod adds the pod's ports to UsedPorts
+          if (tid == 128) a.hp_live[n] |= s_hp[par][0];
         if (tid == 0) {
           // ---- Permit (core.go:268-309) ----
           if (g < 0 || (uint32_t)g >= G) {

@@ -475,6 +475,37 @@ class Engine:
         self._check(self.lib.bs_fetch_interpod_reason_rows(self.h, pod0, n, capi.ptr(out)))
         return out
 
+    def set_host_port_filter(self, on: bool = False):
+        """Switch kube-scheduler's PodFitsHostPorts filter into every pod's fit set (off by default).  While it is on,
+        each round needs upload_host_ports' two sides, and replay and preempt refuse to run."""
+        self._check(self.lib.bs_set_host_port_filter(self.h, 1 if on else 0))
+
+    def upload_host_ports(self, node=None, pods=None):
+        """The columns of the PodFitsHostPorts filter (include/bsched.h bs_upload_node_host_ports).  node = (entries,
+        used): entries [K, 3] rows (ip id, protocol id, port), ip id capi.HOSTPORT_IP_ANY the wildcard "0.0.0.0", and
+        used [N] uint64, bit k = the node uses entry k.  pods = want [P] uint64, bit k = the pod asks for entry k.
+        Uploading nodes (or updating node rows) drops the node side, uploading pods the pod side."""
+        if node is not None:
+            entries, used = node
+            ent = np.asarray(entries, dtype=np.int64).reshape(-1, 3)
+            ip = np.ascontiguousarray(ent[:, 0], dtype=np.uint32)
+            proto = np.ascontiguousarray(ent[:, 1], dtype=np.uint32)
+            port = np.ascontiguousarray(np.clip(ent[:, 2], -1, 1 << 20), dtype=np.int32)
+            used = np.ascontiguousarray(used, dtype=np.uint64).reshape(-1)
+            t = capi.HostPortNodesC(len(used), len(ent), capi.ptr(ip), capi.ptr(proto), capi.ptr(port), capi.ptr(used))
+            self._check(self.lib.bs_upload_node_host_ports(self.h, C.byref(t)))
+        if pods is not None:
+            want = np.ascontiguousarray(pods, dtype=np.uint64).reshape(-1)
+            self._check(self.lib.bs_upload_pod_host_ports(self.h, len(want), capi.ptr(want)))
+
+    def fetch_host_port_reason_rows(self, pod0=0, n=None) -> np.ndarray:
+        """[n] uint32: the companion of reason_rows, the nodes past the guards that have a host-port conflict with the
+        pod, whatever their other bins."""
+        n = self.P - pod0 if n is None else n
+        out = np.zeros(n, np.uint32)
+        self._check(self.lib.bs_fetch_host_port_reason_rows(self.h, pod0, n, capi.ptr(out)))
+        return out
+
     def priority_rows(self, pod0=0, n=None):
         """(nodes [n, K] int32, scores [n, K] int64): each pod's fitting nodes by priority score descending, then node
         index ascending; min(K, feasible_count) entries, padded with node -1 and score INT64_MIN."""
@@ -764,10 +795,12 @@ def format_remove_message(reason: int, pod_name: str = "", victim_name: str = ""
     return buf.value.decode()
 
 
-def format_fit_error(counts, n_lanes: int, n_nodes: int, scalar_names=None, buf_len: int = 4096, interpod=None) -> str:
+def format_fit_error(counts, n_lanes: int, n_nodes: int, scalar_names=None, buf_len: int = 4096, interpod=None,
+                     host_ports=None) -> str:
     """kube-scheduler's FailedScheduling text for one reason row; needs no engine and no device.  scalar_names: the
     names of lanes 4.. (None: "lane<d>").  interpod: the row's companion (E, A, N) from fetch_interpod_reason_rows, whose
-    MatchInterPodAffinity entries join the message (bs_format_fit_error_interpod)."""
+    MatchInterPodAffinity entries join the message (bs_format_fit_error_interpod).  host_ports: the row's count from
+    fetch_host_port_reason_rows, whose PodFitsHostPorts entry joins it (bs_format_fit_error_filters)."""
     lib = capi.load()
     row = np.ascontiguousarray(counts, dtype=np.uint32)
     if row.shape != (4 + n_lanes,):
@@ -776,7 +809,16 @@ def format_fit_error(counts, n_lanes: int, n_nodes: int, scalar_names=None, buf_
     if scalar_names is not None:
         names = (C.c_char_p * max(1, n_lanes - 4))(*[s.encode() for s in scalar_names])
     buf = C.create_string_buffer(buf_len)
-    if interpod is not None:
+    if host_ports is not None:
+        ip = None if interpod is None else np.ascontiguousarray(interpod, dtype=np.uint32)
+        if ip is not None and ip.shape != (3,):
+            raise ValueError("an inter-pod companion row has 3 counters")
+        hp = np.ascontiguousarray(host_ports, dtype=np.uint32).reshape(-1)
+        if hp.shape != (1,):
+            raise ValueError("a host-port companion row has 1 counter")
+        rc = lib.bs_format_fit_error_filters(capi.ptr(row), n_lanes, capi.ptr(ip), capi.ptr(hp), n_nodes,
+                                             C.cast(names, C.c_void_p) if names is not None else None, buf, buf_len)
+    elif interpod is not None:
         ip = np.ascontiguousarray(interpod, dtype=np.uint32)
         if ip.shape != (3,):
             raise ValueError("an inter-pod companion row has 3 counters")

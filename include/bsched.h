@@ -751,6 +751,58 @@ int bs_fetch_interpod_reason_rows(bs_engine* e, uint32_t pod0, uint32_t n, uint3
 int bs_format_fit_error_interpod(const uint32_t* counts, uint32_t n_lanes, const uint32_t* interpod, uint32_t n_nodes,
                                  const char* const* scalar_names, char* buf, size_t buf_len);
 
+/* ---- kube-scheduler v1.17's PodFitsHostPorts filter: a pod's host ports in its fit set ----
+ * Off by default.  While it is on, every evaluation ANDs it into each pod's fit set, as the MatchInterPodAffinity
+ * filter above: the fit bitmap, the scores, feasible_count, best_node, the top-K lists, the fit set of the
+ * BS_OUT_PRIORITY lists, the reason rows (through the companion row below) and the Permit verdict.  It does not reach
+ * PreFilter's cluster scans or BS_OUT_FILTER.
+ *
+ * The caller resolves the objects into a dictionary of at most BS_HOSTPORT_MAX entries (ip id, protocol id, port)
+ * [upstream, from memory: schedutil.GetContainerPorts over Spec.Containers (init containers excluded), NodeInfo's
+ * HostPortInfo]: a port <= 0 is dropped, an empty HostIP is "0.0.0.0" and has ip id BS_HOSTPORT_IP_ANY, an empty
+ * protocol is "TCP"; the caller numbers the other IPs (compared as strings, so "::" is an ordinary IP) and the
+ * protocols.  A node's used mask and a pod's want mask are sets of entries.  The engine derives each entry's conflict
+ * mask: entries a and b conflict when they have the same protocol and port and either ip id is BS_HOSTPORT_IP_ANY or
+ * the ids are equal.  Pod p fails node n when some entry n uses conflicts with some entry p wants.
+ * An evaluation with the filter on is BS_E_STATE before anything is launched when either side is missing and BS_E_INDEX
+ * when a want bit is >= the node side's n_entries.  bs_replay and bs_replay_priority (every variant) apply the filter
+ * to each step's node choice on a live copy of the used masks: a node whose live mask conflicts with the pod's is not
+ * a candidate, and assuming a pod ORs its want mask into its node's live mask (NodeInfo.AddPod); the same checks run
+ * before the walk.  The live masks are not returned: they are the used masks ORed with the want masks of the pods
+ * placed on each node.  bs_preempt and bs_preempt_walk refuse to run (BS_E_INVAL) while the filter is on: removing a
+ * victim would have to take its ports out of the used masks. */
+int bs_set_host_port_filter(bs_engine* e, int on);
+#define BS_HOSTPORT_MAX 64        /* entries of the dictionary: one bit each of a uint64 mask */
+#define BS_HOSTPORT_IP_ANY 0u     /* ip id of "0.0.0.0" (and of an empty HostIP) */
+typedef struct {
+  uint32_t n_nodes;               /* the node table's */
+  uint32_t n_entries;             /* at most BS_HOSTPORT_MAX */
+  const uint32_t* ip;             /* [n_entries] ip id, BS_HOSTPORT_IP_ANY the wildcard */
+  const uint32_t* protocol;       /* [n_entries] protocol id */
+  const int32_t* port;            /* [n_entries] 1..65535 */
+  const uint64_t* used;           /* [n_nodes] bit k: the node's NodeInfo.UsedPorts() holds entry k */
+} bs_host_port_nodes;
+/* The node side.  A wrong n_nodes, more than BS_HOSTPORT_MAX entries or an entry listed twice is BS_E_INVAL, a port
+ * outside 1..65535 BS_E_RANGE, a used bit >= n_entries BS_E_INDEX; a failing call leaves it dropped.
+ * bs_upload_nodes and bs_update_nodes drop it. */
+int bs_upload_node_host_ports(bs_engine* e, const bs_host_port_nodes* t);
+/* The pod side: want[n_pods], bit k = the pod's containers ask for entry k.  A wrong n_pods is BS_E_INVAL; the bits are
+ * checked against the node side at evaluation, so the sides may come in either order.  A failing call leaves it
+ * dropped; bs_upload_pods drops it. */
+int bs_upload_pod_host_ports(bs_engine* e, uint32_t n_pods, const uint64_t* want);
+/* The companion of bs_fetch_reason_rows (BS_OUT_REASONS): dense [n] counters, the nodes that pass the guards (bins 0
+ * and 1) and have a port conflict with pod pod0 + p, whatever the other bins say.  All zero for a round evaluated with
+ * the filter off.  With both filters on, bs_fetch_interpod_reason_rows counts only nodes without a port conflict:
+ * upstream runs MatchInterPodAffinity after GeneralPredicates. */
+int bs_fetch_host_port_reason_rows(bs_engine* e, uint32_t pod0, uint32_t n, uint32_t* counts);
+/* bs_format_fit_error with both filters' companions as further entries, sorted with the rest as whole strings: interpod
+ * (NULL or [3]) as in bs_format_fit_error_interpod, host_ports (NULL or [1]) as
+ *     "<count> node(s) didn't have free ports for the requested pod ports"
+ * when its count is non-zero.  bs_format_fit_error_interpod is this call with host_ports NULL. */
+int bs_format_fit_error_filters(const uint32_t* counts, uint32_t n_lanes, const uint32_t* interpod,
+                                const uint32_t* host_ports, uint32_t n_nodes, const char* const* scalar_names, char* buf,
+                                size_t buf_len);
+
 /* ---- preemption: PreFilterExtensions.RemovePod and the node / victims kube-scheduler's preemption would pick ----
  * The bound-pod table lists the pods already running on the snapshot's nodes (NodeInfo.Pods()).  Rows may come in
  * any order; the engine groups them by node in MoreImportantPod order (priority descending, start time ascending,

@@ -399,6 +399,72 @@ func (e *Engine) FetchInterPodReasonRows(pod0, n uint32, counts []uint32) error 
 	return e.rc(C.bs_fetch_interpod_reason_rows(e.h, C.uint32_t(pod0), C.uint32_t(n), p))
 }
 
+// SetHostPortFilter: kube-scheduler v1.17's PodFitsHostPorts filter in every pod's fit set and in the Replay walks
+// (off by default).  While it is on, each Evaluate and Replay needs both sides, and Preempt and PreemptWalk refuse to
+// run.
+func (e *Engine) SetHostPortFilter(on bool) error {
+	v := C.int(0)
+	if on {
+		v = 1
+	}
+	return e.rc(C.bs_set_host_port_filter(e.h, v))
+}
+
+// HostPortEntry is one (ip id, protocol id, port) of the dictionary; ip id 0 (BS_HOSTPORT_IP_ANY) is "0.0.0.0".
+type HostPortEntry struct {
+	IP, Protocol uint32
+	Port         int32
+}
+
+// UploadNodeHostPorts: the dictionary (at most BS_HOSTPORT_MAX entries) and used[n_nodes], bit k = the node's
+// UsedPorts() holds entry k.  UploadNodes / UpdateNodes drop it.
+func (e *Engine) UploadNodeHostPorts(entries []HostPortEntry, used []uint64) error {
+	k := len(entries)
+	ip, proto, port := make([]uint32, k+1), make([]uint32, k+1), make([]int32, k+1)
+	for i, x := range entries {
+		ip[i], proto[i], port[i] = x.IP, x.Protocol, x.Port
+	}
+	cip := (*C.uint32_t)(C.malloc(C.size_t(4 * (k + 1))))
+	cproto := (*C.uint32_t)(C.malloc(C.size_t(4 * (k + 1))))
+	cport := (*C.int32_t)(C.malloc(C.size_t(4 * (k + 1))))
+	cused := (*C.uint64_t)(C.malloc(C.size_t(8 * (len(used) + 1))))
+	defer C.free(unsafe.Pointer(cip))
+	defer C.free(unsafe.Pointer(cproto))
+	defer C.free(unsafe.Pointer(cport))
+	defer C.free(unsafe.Pointer(cused))
+	copy(unsafe.Slice((*uint32)(unsafe.Pointer(cip)), k+1), ip)
+	copy(unsafe.Slice((*uint32)(unsafe.Pointer(cproto)), k+1), proto)
+	copy(unsafe.Slice((*int32)(unsafe.Pointer(cport)), k+1), port)
+	copy(unsafe.Slice((*uint64)(unsafe.Pointer(cused)), len(used)+1), used)
+	t := C.bs_host_port_nodes{n_nodes: C.uint32_t(len(used)), n_entries: C.uint32_t(k), ip: cip, protocol: cproto,
+		port: cport, used: cused}
+	return e.rc(C.bs_upload_node_host_ports(e.h, &t))
+}
+
+// UploadPodHostPorts: want[n_pods], bit k = the pod's containers ask for entry k.  UploadPods drops it.
+func (e *Engine) UploadPodHostPorts(want []uint64) error {
+	if len(want) == 0 {
+		return e.rc(C.bs_upload_pod_host_ports(e.h, 0, nil))
+	}
+	c := (*C.uint64_t)(C.malloc(C.size_t(8 * len(want))))
+	defer C.free(unsafe.Pointer(c))
+	copy(unsafe.Slice((*uint64)(unsafe.Pointer(c)), len(want)), want)
+	return e.rc(C.bs_upload_pod_host_ports(e.h, C.uint32_t(len(want)), c))
+}
+
+// FetchHostPortReasonRows: the companion of FetchReasonRows, counts[n] of the nodes past the guards with a host-port
+// conflict.
+func (e *Engine) FetchHostPortReasonRows(pod0, n uint32, counts []uint32) error {
+	if uint64(len(counts)) < uint64(n) {
+		return fmt.Errorf("bsched: counts needs n entries")
+	}
+	var p *C.uint32_t
+	if n > 0 {
+		p = (*C.uint32_t)(unsafe.Pointer(&counts[0]))
+	}
+	return e.rc(C.bs_fetch_host_port_reason_rows(e.h, C.uint32_t(pod0), C.uint32_t(n), p))
+}
+
 // UploadNodeNonZero / UploadPodNonZero: the non-zero request columns, nz[2][n] (cpu millicores, then memory bytes):
 // per pod the sum over its containers of GetNonzeroRequestForResource(Requests), per node NodeInfo.NonZeroRequest().
 // UploadNodes / UpdateNodes drop the node column and UploadPods the pod column: upload them again before Evaluate.
@@ -451,6 +517,12 @@ func FitError(counts []uint32, nNodes int, scalarNames []string) (string, error)
 // FitErrorInterPod is FitError with the row's MatchInterPodAffinity companion (E, A, N from FetchInterPodReasonRows)
 // as further entries (bs_format_fit_error_interpod); a nil interPod is FitError.
 func FitErrorInterPod(counts, interPod []uint32, nNodes int, scalarNames []string) (string, error) {
+	return FitErrorFilters(counts, interPod, nil, nNodes, scalarNames)
+}
+
+// FitErrorFilters is FitError with both filters' companions (nil: absent): interPod as FitErrorInterPod, hostPorts the
+// one counter of FetchHostPortReasonRows (bs_format_fit_error_filters).
+func FitErrorFilters(counts, interPod, hostPorts []uint32, nNodes int, scalarNames []string) (string, error) {
 	lanes := len(counts) - 4
 	if lanes < C.BS_FIXED_LANES {
 		return "", fmt.Errorf("bs_format_fit_error: a reason row has 4 + lanes bins")
@@ -461,6 +533,13 @@ func FitErrorInterPod(counts, interPod []uint32, nNodes int, scalarNames []strin
 			return "", fmt.Errorf("bs_format_fit_error_interpod: a companion row has 3 counters")
 		}
 		ip = (*C.uint32_t)(unsafe.Pointer(&interPod[0]))
+	}
+	var hp *C.uint32_t
+	if hostPorts != nil {
+		if len(hostPorts) != 1 {
+			return "", fmt.Errorf("bs_format_fit_error_filters: a host-port companion row has 1 counter")
+		}
+		hp = (*C.uint32_t)(unsafe.Pointer(&hostPorts[0]))
 	}
 	var names **C.char
 	if len(scalarNames) > 0 {
@@ -475,7 +554,7 @@ func FitErrorInterPod(counts, interPod []uint32, nNodes int, scalarNames []strin
 	}
 	for size := 512; size <= 1<<20; size *= 4 {
 		buf := (*C.char)(C.malloc(C.size_t(size)))
-		rc := C.bs_format_fit_error_interpod((*C.uint32_t)(unsafe.Pointer(&counts[0])), C.uint32_t(lanes), ip,
+		rc := C.bs_format_fit_error_filters((*C.uint32_t)(unsafe.Pointer(&counts[0])), C.uint32_t(lanes), ip, hp,
 			C.uint32_t(nNodes), names, buf, C.size_t(size))
 		msg := C.GoString(buf)
 		C.free(unsafe.Pointer(buf))
