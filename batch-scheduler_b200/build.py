@@ -6,6 +6,7 @@ Translation units (compiled in parallel, then linked into libbsched.so):
   priority_inst.cu     the priority lists' kernels (csrc/priority.cuh): priority_pod_kernel without SPREAD or IPA, LOC and IPA pre-passes
   priority_spread_inst.cu x 3   priority_pod_kernel's SPREAD variants, one unit per -DBS_PRIO_SPREAD_MAXL=5, 9, 16
   priority_interpod_inst.cu x 3 priority_pod_kernel's IPA variants, one unit per -DBS_PRIO_IPA_MAXL=5, 9, 16
+  replay_ipf_inst.cu x 3        replay_kernel's MatchInterPodAffinity builds, one unit per -DBS_REPLAY_IPF_MAXL=5, 9, 16
   fit_inst.cu x 9      the gang_fit_kernel variant table, one slice per -DBS_FIT_SLICE=n (csrc/fit.cuh)
 
     python -m importlib ...  # not importable by dotted name (hyphen); use __graft_entry__.build()
@@ -40,6 +41,7 @@ def _units():
     for m in (5, 9, 16):
         u.append(("priority_spread_inst.cu", f"priority_spread_inst_{m}.o", [f"-DBS_PRIO_SPREAD_MAXL={m}"]))
         u.append(("priority_interpod_inst.cu", f"priority_interpod_inst_{m}.o", [f"-DBS_PRIO_IPA_MAXL={m}"]))
+        u.append(("replay_ipf_inst.cu", f"replay_ipf_inst_{m}.o", [f"-DBS_REPLAY_IPF_MAXL={m}"]))
     for n in range(FIT_SLICES):
         u.append(("fit_inst.cu", f"fit_inst_{n}.o", [f"-DBS_FIT_SLICE={n}"]))
     return u

@@ -229,6 +229,7 @@ SYMBOLS = {
     "bs_set_interpod_filter": (C.c_int, [C.c_void_p, C.c_int]),
     "bs_upload_node_interpod_filter": (C.c_int, [C.c_void_p, _p(InterpodNodesC)]),
     "bs_upload_pod_interpod_filter": (C.c_int, [C.c_void_p, _p(InterpodFilterPodsC)]),
+    "bs_upload_pod_interpod_placed": (C.c_int, [C.c_void_p, _p(InterpodPodsC)]),
     "bs_fetch_interpod_reason_rows": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]),
     "bs_format_fit_error_interpod": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_char_p,
                                                C.c_size_t]),

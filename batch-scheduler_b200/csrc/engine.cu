@@ -499,14 +499,18 @@ struct bs_engine {
   // with the node table) and the pod side (each pod's filter class h_class, the class table; dropped with the pod
   // table).  The presence planes d_presence ([2][words]: match, own), the per-term counts d_hits and the class planes
   // d_bits ([3][classes][Npad/32]: pass, E, A) are built on the device when dirty.  d_fipf: each fit class's filter
-  // class, d_reasons the companion rows [P][3].
+  // class, d_reasons the companion rows [P][3].  The placed side (bs_upload_pod_interpod_placed; dropped with the pod
+  // table): each pod's placed class d_qclass [P] and the class table, what an assumed pod adds to presence in the walks;
+  // placed_term_max is checked against node.terms when a walk starts.  walk_prepass: a walk ran the pre-pass, so the
+  // next evaluation builds the class fit bits and gates again.
   struct {
     bool on = false, round = false;
     InterpodNodeSide node;
     DevBuf d_presence, d_hits, d_poff, d_pterm, d_prole, d_pself, d_bits, d_fipf, d_reasons;
-    bool have_node = false, have_pod = false, dirty = true;
+    DevBuf d_qclass, d_qoff, d_qterm, d_qown, d_qmatch;
+    bool have_node = false, have_pod = false, have_placed = false, dirty = true, walk_prepass = false;
     uint32_t pclasses = 0;
-    int64_t term_max = -1;
+    int64_t term_max = -1, placed_term_max = -1;
     std::vector<uint32_t> h_class;
   } ipf;
   // PodFitsHostPorts filter (bs_set_host_port_filter; off by default): the node side (each entry's conflict mask
@@ -936,30 +940,21 @@ void launch_prefix(uint32_t L, NodeTab t, PrefixSel ps, PrefixScratch sc, Prefix
   }
 }
 
-// loc: the scored walk with the locality terms (a is then a ReplayLocArgs); HP: the PodFitsHostPorts filter is on (a is
-// then a ReplayHpArgs)
-template <int MAXL, bool HP>
-void launch_replay_t(const ReplayArgs& a, bool scored, bool loc, cudaStream_t s) {
-  if (loc) {
-    const auto& la = static_cast<const ReplayArgsOf<true, HP>&>(a);
-    if (a.ratio.weight) replay_kernel<MAXL, true, true, true, HP><<<1, REPLAY_THREADS, 0, s>>>(la);
-    else replay_kernel<MAXL, true, false, true, HP><<<1, REPLAY_THREADS, 0, s>>>(la);
-    return;
-  }
-  const auto& ha = static_cast<const ReplayArgsOf<false, HP>&>(a);
-  if (scored && a.ratio.weight) replay_kernel<MAXL, true, true, false, HP><<<1, REPLAY_THREADS, 0, s>>>(ha);
-  else if (scored) replay_kernel<MAXL, true, false, false, HP><<<1, REPLAY_THREADS, 0, s>>>(ha);
-  else replay_kernel<MAXL, false, false, false, HP><<<1, REPLAY_THREADS, 0, s>>>(ha);
-}
 inline uint32_t replay_maxl(uint32_t L) { return L <= 5 ? 5u : L <= 9 ? 9u : 16u; }
-void launch_replay(uint32_t L, const ReplayArgs& a, bool scored, bool loc, bool hp, cudaStream_t s) {
-  switch (replay_maxl(L) + (hp ? 100u : 0u)) {
+void launch_replay(uint32_t L, const ReplayArgs& a, bool scored, bool loc, bool hp, bool ipf, cudaStream_t s) {
+  switch (replay_maxl(L) + (hp ? 100u : 0u) + (ipf ? 200u : 0u)) {
     case 5: launch_replay_t<5, false>(a, scored, loc, s); break;
     case 9: launch_replay_t<9, false>(a, scored, loc, s); break;
     case 16: launch_replay_t<16, false>(a, scored, loc, s); break;
     case 105: launch_replay_t<5, true>(a, scored, loc, s); break;
     case 109: launch_replay_t<9, true>(a, scored, loc, s); break;
-    default: launch_replay_t<16, true>(a, scored, loc, s); break;
+    case 116: launch_replay_t<16, true>(a, scored, loc, s); break;
+    case 205: launch_replay_ipf<5, false>(a, scored, loc, s); break;
+    case 209: launch_replay_ipf<9, false>(a, scored, loc, s); break;
+    case 216: launch_replay_ipf<16, false>(a, scored, loc, s); break;
+    case 305: launch_replay_ipf<5, true>(a, scored, loc, s); break;
+    case 309: launch_replay_ipf<9, true>(a, scored, loc, s); break;
+    default: launch_replay_ipf<16, true>(a, scored, loc, s); break;
   }
 }
 
@@ -1489,7 +1484,7 @@ void drop_node_sides(bs_engine* e) {
 }
 void drop_pod_sides(bs_engine* e) {
   e->nz.have_pod = e->pref.have_pod = e->loc.have_img_pod = e->loc.have_avoid_pod = e->spread.have_pod =
-      e->ipa.have_pod = e->ipf.have_pod = e->hp.have_pod = false;
+      e->ipa.have_pod = e->ipf.have_pod = e->ipf.have_placed = e->hp.have_pod = false;
 }
 
 int evaluate_async_locked(bs_engine* e) {
@@ -1533,9 +1528,10 @@ int evaluate_async_locked(bs_engine* e) {
   }
   if ((rc = ensure_round_buffers(e))) return rc;
   for (int k = 0; k < BS_K_COUNT; ++k) e->k_valid[k] = false;
-  if (e->ipf.on && e->ipf.dirty) {   // new pass bits: the class fit bits and gates are built again
+  if (e->ipf.on && (e->ipf.dirty || e->ipf.walk_prepass)) {   // new pass bits: the class fit bits and gates are built again
     if ((rc = interpod_filter_prepass(e))) return rc;
     reprepare = true;
+    e->ipf.walk_prepass = false;
   }
   if (e->hp.on && e->hp.dirty) {   // new used masks: likewise
     reprepare = true;
@@ -2849,10 +2845,13 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
   if (scored && !(e->nz.have_node && e->nz.have_pod))
     return fail(e, BS_E_STATE, (w + ": upload both non-zero request columns first").c_str());
   const bool loc = scored && (e->w_img || e->w_avoid);
-  const bool hp = e->hp.on;
+  const bool hp = e->hp.on, ipf = e->ipf.on;
   int rc;
   if (loc && (rc = locality_check(e, who))) return rc;
   if (hp && (rc = host_port_check(e, who))) return rc;
+  if (ipf && (rc = interpod_filter_check(e, who))) return rc;
+  if (ipf && e->ipf.placed_term_max >= (int64_t)e->ipf.node.terms)
+    return fail(e, BS_E_INDEX, (w + ": a placed class's term is outside the filter's term dictionary").c_str());
   BS_DEVICE_GUARD(e);
   const uint32_t N = e->N, Npad = e->Npad, P = e->P, G = e->G, L = e->L;
   if (!queue) n_queue = P;
@@ -2866,6 +2865,10 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
       return fail(e, BS_E_RANGE, (w + ": live non-zero requests could pass 2^62").c_str());
   if (e->classes_dirty && (rc = rebuild_classes(e))) return rc;
   if (loc && (rc = locality_prepass(e))) return rc;
+  if (ipf && e->ipf.dirty) {   // presence of the sides of now; the next evaluation builds its class fit bits again
+    if ((rc = interpod_filter_prepass(e))) return rc;
+    e->ipf.walk_prepass = true;
+  }
 
   // scratch copies of everything the cycle mutates, the queue and the outputs, and the compact node state and
   // block cache the kernel builds (replay.cuh)
@@ -2885,7 +2888,10 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
   const bool cache = safe && fitmask && n_blocks >= 1 && n_blocks <= (uint32_t)REPLAY_MAX_BLOCKS;
   const size_t rows = cache ? (size_t)2 * e->n_rep_classes * n_blocks : 0, maxl = replay_maxl(L);
   View s_req, s_pc, s_rp, s_matched, s_gflags, s_grc, s_minres, s_mrp, d_queue, d_pf, d_node, d_ready, d_status,
-      n_left0, n_left1, n_both, n_stat, n_fit, c_sum, c_max, c_keys, n_nz, s_used, d_want, d_conf;
+      n_left0, n_left1, n_both, n_stat, n_fit, c_sum, c_max, c_keys, n_nz, s_used, d_want, d_conf, s_pres, s_hits,
+      d_fclass;
+  const InterpodNodeSide& is = e->ipf.node;
+  const size_t ipf_words = ipf ? (is.slots + 31) / 32 : 0;
   // The node state and block cache every step reads come first: carved behind the copies, the same kernel took
   // 2 % longer at the bench shape on an H100.
   CK(carve(e->d_replay,
@@ -2895,7 +2901,9 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
             {&s_rp, (size_t)Npad * 4}, {&s_matched, (size_t)Gp * 4}, {&s_gflags, Gp}, {&s_grc, (size_t)Gp * 4},
             {&s_minres, (size_t)L * Gp * 8}, {&s_mrp, (size_t)Gp * 4}, {&d_queue, (size_t)Qp * 4}, {&d_pf, Qp},
             {&d_node, (size_t)Qp * 4}, {&d_ready, Qp}, {&d_status, 128}, {&n_nz, scored ? (size_t)2 * Npad * 8 : 0},
-            {&s_used, hp ? (size_t)Npad * 8 : 0}, {&d_want, hp ? (size_t)P * 8 : 0}, {&d_conf, hp ? (size_t)P * 8 : 0}}));
+            {&s_used, hp ? (size_t)Npad * 8 : 0}, {&d_want, hp ? (size_t)P * 8 : 0}, {&d_conf, hp ? (size_t)P * 8 : 0},
+            {&s_pres, ipf_words * 2 * 4}, {&s_hits, ipf ? (size_t)is.terms * 4 : 0},
+            {&d_fclass, ipf ? (size_t)P * 4 : 0}}));
   auto dup = [&](const View& dst, const DevBuf& src, size_t bytes) {
     return bytes ? cudaMemcpyAsync(dst.p, src.p, bytes, cudaMemcpyDeviceToDevice, e->s) : cudaSuccess;
   };
@@ -2919,9 +2927,14 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
       CK(cudaMemcpyAsync(d_conf.p, conf.data(), (size_t)P * 8, cudaMemcpyHostToDevice, e->s));
     }
   }
+  if (ipf) {   // the live presence starts as the snapshot's
+    CK(dup(s_pres, e->ipf.d_presence, ipf_words * 2 * 4));
+    CK(dup(s_hits, e->ipf.d_hits, (size_t)is.terms * 4));
+    if (P) CK(cudaMemcpyAsync(d_fclass.p, e->ipf.h_class.data(), (size_t)P * 4, cudaMemcpyHostToDevice, e->s));
+  }
   if (queue && n_queue) CK(cudaMemcpyAsync(d_queue.p, queue, (size_t)n_queue * 4, cudaMemcpyHostToDevice, e->s));
   CK(cudaMemsetAsync(d_status.p, 0, 128, e->s));
-  ReplayHpArgs la{};
+  ReplayIpfArgs la{};
   ReplayArgs& a = la;
   a.nt = node_tab(e);
   a.nt.requested = s_req.as<int64_t>();
@@ -2979,9 +2992,23 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
     la.hp_want = d_want.as<uint64_t>();
     la.hp_conf = d_conf.as<uint64_t>();
   }
+  if (ipf) {
+    la.ipf_mbits = s_pres.as<uint32_t>();
+    la.ipf_obits = s_pres.as<uint32_t>() + ipf_words;
+    la.ipf_hits = s_hits.as<uint32_t>();
+    la.tp = IpfTopo{is.d_topo.as<uint32_t>(), is.d_term_key.as<uint32_t>(), is.d_term_off.as<uint32_t>(), N};
+    la.fc = IpfPods{e->ipf.d_poff.as<uint32_t>(), e->ipf.d_pterm.as<uint32_t>(), e->ipf.d_prole.as<uint8_t>(),
+                    e->ipf.d_pself.as<uint8_t>(), e->ipf.pclasses};
+    la.f_class = d_fclass.as<uint32_t>();
+    la.q_class = e->ipf.d_qclass.as<uint32_t>();
+    la.q_off = e->ipf.d_qoff.as<uint32_t>();
+    la.q_term = e->ipf.d_qterm.as<uint32_t>();
+    la.q_own = e->ipf.d_qown.as<int32_t>();
+    la.q_match = e->ipf.d_qmatch.as<uint8_t>();
+  }
   {
     StageTimer tm(e, BS_K_REPLAY, e->s);
-    launch_replay(L, a, scored, loc, hp, e->s);
+    launch_replay(L, a, scored, loc, hp, ipf, e->s);
     tm.launched();
     CK(cudaGetLastError());
   }
@@ -3027,13 +3054,19 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
 }
 }  // namespace
 
-// The walks and preemption refuse to run under the MatchInterPodAffinity filter: its presence would have to follow their
-// own placements and victim removals (upstream's metadata AddPod / RemovePod).  Preemption refuses to run under the
-// PodFitsHostPorts filter: its victims' removal would have to take their ports out of the used masks (the walks follow
-// their own placements in a live copy of them).
+// Preemption refuses to run under the MatchInterPodAffinity filter: its presence would have to shrink when victims leave
+// (upstream's metadata RemovePod).  The walks follow their own placements in live presence, which needs each pod's
+// placed class: without it they refuse as well.  Preemption refuses to run under the PodFitsHostPorts filter: its
+// victims' removal would have to take their ports out of the used masks (the walks follow their own placements in a
+// live copy of them).
 static int interpod_filter_refuse(bs_engine* e, const char* who) {
   return fail(e, BS_E_INVAL, (std::string(who) + ": the MatchInterPodAffinity filter is not supported here; "
                               "switch it off with bs_set_interpod_filter").c_str());
+}
+static int interpod_placed_refuse(bs_engine* e, const char* who) {
+  return fail(e, BS_E_INVAL, (std::string(who) + ": the MatchInterPodAffinity filter needs the pods' placed classes in "
+                              "the walk; upload them with bs_upload_pod_interpod_placed or switch the filter off with "
+                              "bs_set_interpod_filter").c_str());
 }
 static int host_port_refuse(bs_engine* e, const char* who) {
   return fail(e, BS_E_INVAL, (std::string(who) + ": the PodFitsHostPorts filter is not supported here; "
@@ -3043,7 +3076,7 @@ static int host_port_refuse(bs_engine* e, const char* who) {
 int bs_replay(bs_engine* e, const uint32_t* queue, uint32_t n_queue, bs_replay_result* out) {
   if (!e || !out) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
-  if (e->ipf.on) return interpod_filter_refuse(e, "bs_replay");
+  if (e->ipf.on && !e->ipf.have_placed) return interpod_placed_refuse(e, "bs_replay");
   return replay_walk(e, "bs_replay", queue, n_queue, out, false, nullptr);
 }
 
@@ -3051,7 +3084,7 @@ int bs_replay_priority(bs_engine* e, const uint32_t* queue, uint32_t n_queue, bs
                        int64_t* node_nonzero_after) {
   if (!e || !out) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
-  if (e->ipf.on) return interpod_filter_refuse(e, "bs_replay_priority");
+  if (e->ipf.on && !e->ipf.have_placed) return interpod_placed_refuse(e, "bs_replay_priority");
   if (e->w_taint || e->w_naff)   // their maxima would have to follow the walk's live fit set, which is not built yet
     return fail(e, BS_E_INVAL, "bs_replay_priority: TaintToleration and NodeAffinity are not supported in the walk; "
                                "set both weights of bs_set_node_priority_weights to 0");
@@ -4113,6 +4146,34 @@ int bs_upload_pod_interpod_filter(bs_engine* e, const bs_interpod_filter_pods* t
   e->ipf.have_pod = true;
   e->filt.assign_dirty = e->classes_dirty = e->pod_classes_dirty = true;   // the pods' fit classes carry the filter class
   e->evaluated = false;
+  return BS_OK;
+}
+
+int bs_upload_pod_interpod_placed(bs_engine* e, const bs_interpod_pods* t) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  const Refuse bad{e, "bs_upload_pod_interpod_placed"};
+  e->ipf.have_placed = false;
+  if (!t) return bad(BS_E_INVAL, "null table");
+  const uint32_t P = t->n_pods;
+  if (int rc = bad.shape(POD_SIDE, P)) return rc;
+  if (P && !t->pod_class) return bad(BS_E_INVAL, "null pod_class");
+  if (max_class(t->pod_class, P, BS_IPF_NONE) >= (int64_t)t->classes.n_classes)
+    return bad(BS_E_INDEX, "a pod_class is >= n_classes");
+  int64_t tmax;
+  const char* why = nullptr;
+  if (int rc = interpod_classes_check(t->classes, UINT32_MAX, tmax, why)) return bad(rc, why);
+  const uint32_t nnz = t->classes.n_classes ? t->classes.class_offset[t->classes.n_classes] : 0;
+  for (uint32_t k = 0; k < nnz; ++k)
+    if (t->classes.own[k] != 0 && t->classes.own[k] != 1) return bad(BS_E_RANGE, "an own is not 0 or 1");
+  BS_DEVICE_GUARD(e);
+  int rc;
+  if ((rc = upload_vec(e, e->ipf.d_qclass, t->pod_class, P, P)) ||
+      (rc = interpod_classes_upload(e, t->classes, e->ipf.d_qoff, e->ipf.d_qterm, e->ipf.d_qown, e->ipf.d_qmatch)))
+    return rc;
+  CK(cudaStreamSynchronize(e->s));
+  e->ipf.placed_term_max = tmax;
+  e->ipf.have_placed = true;
   return BS_OK;
 }
 

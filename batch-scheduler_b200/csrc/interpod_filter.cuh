@@ -37,6 +37,8 @@ struct IpfTopo {
   uint32_t n_nodes;
 };
 
+// The kernels are defined once, in engine.cu; replay_ipf_inst.cu (BS_KERNELS_HELPERS_ONLY) needs the types above only.
+#ifndef BS_KERNELS_HELPERS_ONLY
 // K1j ipf_presence_kernel — a thread per bound pod, walking its class's entries in step with its warp (entry k of every
 // lane at once).  For an entry whose key the pod's node carries (value v): match sets bit term_off + v of the match
 // plane and adds one to the term's count, own sets the bit of the own plane.  Lanes that hit one plane word combine
@@ -142,5 +144,7 @@ __global__ void __launch_bounds__(IPF_THREADS) ipf_class_kernel(IpfPods pc, IpfT
     bits[2 * plane + at] = wa;
   }
 }
+
+#endif  // BS_KERNELS_HELPERS_ONLY
 
 }  // namespace bsk

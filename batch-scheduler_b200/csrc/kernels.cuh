@@ -243,8 +243,9 @@ __device__ __forceinline__ uint64_t ratio_term(uint32_t weight, uint32_t num, ui
   return (uint64_t)weight * (uint64_t)ratio_round(num, den);
 }
 
-// The round's kernels.  A translation unit that needs only the helpers above (priority_inst.cu) defines
-// BS_KERNELS_HELPERS_ONLY, so that these external kernels are defined once, in engine.cu.
+// The round's kernels.  A translation unit that needs only the helpers (priority_inst.cu, replay_ipf_inst.cu) defines
+// BS_KERNELS_HELPERS_ONLY, so that these external kernels are defined once, in engine.cu; the group and findMaxPG
+// helpers the walk shares sit between guarded stretches.
 #ifndef BS_KERNELS_HELPERS_ONLY
 // node_left_kernel's per-node code, shared with bs_preempt_walk's commit step: the scalar keys of the residuals
 // (alloc_present & req_present) and lane d's residual at percent 1.0 (singleNodeResource core.go:647-668), or
@@ -621,6 +622,8 @@ __global__ void __launch_bounds__(REASON_THREADS) reason_pod_kernel(ReasonArgsOf
   }
 }
 
+#endif  // BS_KERNELS_HELPERS_ONLY
+
 // ---------------------------------------------------------------------------
 // K2  group preparation: what fillOccupiedObj (core.go:477-512) leaves behind
 // once the first pod of each group (table order) has reached it.
@@ -654,6 +657,7 @@ struct GroupEff {
   uint32_t* done;       // pods whose fit row is finished (ticket)
 };
 
+#ifndef BS_KERNELS_HELPERS_ONLY
 __global__ void group_reset_kernel(GroupTab g, GroupEff e, uint8_t* __restrict__ new_denied,
                                    uint32_t* __restrict__ admit_bitmap, uint8_t* __restrict__ okA) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -722,6 +726,8 @@ __device__ __forceinline__ uint32_t pre_allocated(const GroupTab& g, const Group
   if (need[LANE_PODS] == 0) need[LANE_PODS] = mm + 1;                                         // :789-791
   return present;
 }
+
+#endif  // BS_KERNELS_HELPERS_ONLY
 
 // K3  findMaxPG (core.go:701-739) as ONE pass with an associative, order-insensitive merge
 // that reproduces the sequential table-order scan exactly (tie rule :725-735):
@@ -794,6 +800,7 @@ __device__ __forceinline__ MaxState max_state_block_reduce(MaxState v, MaxState*
   return v;  // valid in warp 0
 }
 
+#ifndef BS_KERNELS_HELPERS_ONLY
 constexpr int FINDMAX_THREADS = 256;
 constexpr int FINDMAX_PER_THREAD = 4;
 __global__ void __launch_bounds__(FINDMAX_THREADS)

@@ -1880,8 +1880,14 @@ void BatchSchedulingPlugin::SetInterPodAffinityFilter(bool on) {
   interpod_filter_ = on;
 }
 
+void BatchSchedulingPlugin::SetInterPodAffinityFilterInWalks(bool on) {
+  std::lock_guard<std::mutex> lk(mu_);
+  interpod_filter_walks_ = on;
+}
+
 Status BatchSchedulingPlugin::PackInterPodFilter(const std::vector<const NodeInfo*>& snapshot,
-                                                 const std::vector<const Pod*>& pending, PackedInterPodFilter* out) {
+                                                 const std::vector<const Pod*>& pending, PackedInterPodFilter* out,
+                                                 bool placed) {
   if (!out) return Status{BS_CODE_ERROR, "PackInterPodFilter: null output"};
   PackedInterPodFilter& pk = *out;
   pk = PackedInterPodFilter();
@@ -1936,6 +1942,7 @@ Status BatchSchedulingPlugin::PackInterPodFilter(const std::vector<const NodeInf
   std::vector<std::pair<ResolvedTerm, uint32_t>> antis;
   std::unordered_map<std::string, size_t> set_of;
   std::map<std::pair<std::vector<std::pair<uint32_t, uint8_t>>, uint8_t>, uint32_t> class_of;
+  std::vector<std::vector<uint32_t>> own_anti(placed ? P : 0);   // placed: each pending pod's anti-affinity terms
   pk.pod_class.assign(P, BS_IPF_NONE);
   for (size_t p = 0; p < P; ++p) {
     if (!pending[p]) continue;
@@ -1979,6 +1986,7 @@ Status BatchSchedulingPlugin::PackInterPodFilter(const std::vector<const NodeInf
       if (!(st = term_id("n\x1e" + r.sig, t.topology_key, &id, &fresh)).ok()) return st;
       if (fresh) antis.emplace_back(std::move(r), id);
       ent.emplace(id, (uint8_t)BS_IPF_ANTI);
+      if (placed) own_anti[p].push_back(id);
     }
     if (ent.empty()) continue;
     if (ent.size() > BS_IPF_CLASS_MAX)
@@ -2028,6 +2036,44 @@ Status BatchSchedulingPlugin::PackInterPodFilter(const std::vector<const NodeInf
     }
     pk.bound_class[k] = it->second;
   }
+  if (placed) {
+    // what each pending pod adds once assumed, as a bound pod's class: the bound pods' loop above from the other side
+    std::map<std::vector<std::tuple<uint32_t, int32_t, uint8_t>>, uint32_t> qclass_of;
+    pk.placed_class.assign(P, BS_IPF_NONE);
+    for (size_t p = 0; p < P; ++p) {
+      if (!pending[p]) continue;
+      const Pod& pod = *pending[p];
+      std::map<uint32_t, std::pair<int32_t, uint8_t>> ent;   // term -> (own, match)
+      for (uint32_t id : own_anti[p]) ent[id].first = 1;
+      for (auto& e : existing)
+        if (pod_matches_term(pod, e.first)) ent[e.second].second = 1;
+      for (const Set& s : sets) {
+        bool all = true;
+        for (const ResolvedTerm& r : s.terms) all = all && pod_matches_term(pod, r);
+        if (all)
+          for (uint32_t id : s.ids) ent[id].second = 1;
+      }
+      for (auto& a : antis)
+        if (pod_matches_term(pod, a.first)) ent[a.second].second = 1;
+      if (ent.empty()) continue;
+      if (ent.size() > BS_IPF_CLASS_MAX)
+        return Status{BS_CODE_ERROR, "PackInterPodFilter: a pending pod's placed class lists more than BS_IPF_CLASS_MAX terms"};
+      std::vector<std::tuple<uint32_t, int32_t, uint8_t>> key;
+      for (auto& kv : ent) key.emplace_back(kv.first, kv.second.first, kv.second.second);
+      auto it = qclass_of.find(key);
+      if (it == qclass_of.end()) {
+        PackedInterPodAffinity::Classes& cl = pk.placed_classes;
+        it = qclass_of.emplace(key, cl.n_classes()).first;
+        for (auto& e : key) {
+          cl.term.push_back(std::get<0>(e));
+          cl.own.push_back(std::get<1>(e));
+          cl.match.push_back(std::get<2>(e));
+        }
+        cl.offset.push_back((uint32_t)cl.term.size());
+      }
+      pk.placed_class[p] = it->second;
+    }
+  }
   number_topology(snapshot, pk.keys, &pk.values, &pk.n_values, &pk.topo);
   return Status{};
 }
@@ -2040,7 +2086,7 @@ Status BatchSchedulingPlugin::UploadInterPodFilter() {
   if (rc) return fail(rc);
   if (!interpod_filter_) return Status{};
   PackedInterPodFilter pk;
-  Status st = PackInterPodFilter(snapshot_, pending_, &pk);
+  Status st = PackInterPodFilter(snapshot_, pending_, &pk, interpod_filter_walks_);
   if (!st.ok()) return st;
   const PackedInterPodAffinity::Classes& c = pk.bound_classes;
   bs_interpod_nodes nt{(uint32_t)snapshot_.size(), (uint32_t)pk.keys.size(), pk.n_values.data(), pk.topo.data(),
@@ -2052,6 +2098,12 @@ Status BatchSchedulingPlugin::UploadInterPodFilter() {
     bs_interpod_filter_pods pt{(uint32_t)pending_.size(), pk.pod_class.data(), pk.n_pod_classes(), pk.pod_offset.data(),
                                pk.pod_term.data(), pk.pod_role.data(), pk.self_match.data()};
     rc = bs_upload_pod_interpod_filter(eng_, &pt);
+  }
+  if (!rc && interpod_filter_walks_) {
+    const PackedInterPodAffinity::Classes& q = pk.placed_classes;
+    bs_interpod_pods qt{(uint32_t)pending_.size(), pk.placed_class.data(),
+                        bs_interpod_classes{q.n_classes(), q.offset.data(), q.term.data(), q.own.data(), q.match.data()}};
+    rc = bs_upload_pod_interpod_placed(eng_, &qt);
   }
   return rc ? fail(rc) : Status{};
 }
@@ -2583,7 +2635,7 @@ Status BatchSchedulingPlugin::PreemptQueue(std::vector<Preemption>* out, bool ga
 Status BatchSchedulingPlugin::ReplayQueue(std::vector<ReplayDecision>* out, ReplayNodeChoice choice) {
   if (!out) return Status{BS_CODE_ERROR, "ReplayQueue: null output"};
   if (!eng_) return Status{BS_CODE_ERROR, "ReplayQueue: no round has been started"};
-  if (interpod_filter_)
+  if (interpod_filter_ && !interpod_filter_walks_)
     return Status{BS_CODE_ERROR, "ReplayQueue: the MatchInterPodAffinity filter is on (SetInterPodAffinityFilter(false) first)"};
   const bool prio = choice == ReplayNodeChoice::kPriority;
   if (prio && !priority_k_)

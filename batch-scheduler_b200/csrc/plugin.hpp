@@ -352,6 +352,10 @@ struct PackedInterPodFilter {
   std::vector<uint8_t> pod_role;                // BS_IPF_AFFINITY / BS_IPF_ANTI / BS_IPF_EXISTING
   std::vector<uint8_t> self_match;              // [n_classes]
   uint32_t n_pod_classes() const { return (uint32_t)pod_offset.size() - 1; }
+  // the placed side (bs_upload_pod_interpod_placed), packed only on request: what each pending pod adds to presence
+  // once a walk assumes it, as a bound pod's class
+  std::vector<uint32_t> placed_class;           // [n_pods], BS_IPF_NONE = no entries; empty when not packed
+  PackedInterPodAffinity::Classes placed_classes;
 };
 // normalizedImageName (ImageLocality): ":latest" appended when the last ':' does not follow the last '/'
 std::string normalized_image_name(const std::string& name);
@@ -546,8 +550,14 @@ class BatchSchedulingPlugin {
   void SetInterPodAffinityWeight(uint32_t inter_pod_affinity);
   // kube-scheduler v1.17's MatchInterPodAffinity filter in every pod's fit set (bs_set_interpod_filter; off by
   // default), from the next round, delta round or UpdateNodes on: PackInterPodFilter's columns are uploaded with each
-  // of them.  While it is on, ReplayQueue, Preempt, PreemptAll and PreemptQueue return an error.
+  // of them.  While it is on, Preempt, PreemptAll and PreemptQueue return an error, and so does ReplayQueue unless
+  // SetInterPodAffinityFilterInWalks is on.
   void SetInterPodAffinityFilter(bool on);
+  // the MatchInterPodAffinity filter in ReplayQueue as well (off by default): while this and the filter are on, the
+  // next round, delta round or UpdateNodes packs and uploads the pending pods' placed classes too
+  // (PackInterPodFilter(..., placed = true), bs_upload_pod_interpod_placed), and ReplayQueue (both choices) walks under
+  // the filter on presence that follows its own placements.  Off, the rounds pack and upload what they did before.
+  void SetInterPodAffinityFilterInWalks(bool on);
   // kube-scheduler v1.17's PodFitsHostPorts filter in every pod's fit set and in ReplayQueue (bs_set_host_port_filter;
   // off by default), from the next round, delta round or UpdateNodes on: PackHostPorts' columns are uploaded with each
   // of them.  While it is on, Preempt, PreemptAll and PreemptQueue return an error.
@@ -680,9 +690,13 @@ class BatchSchedulingPlugin {
   // (BS_IPF_ANTI; match = it matches the term); equal sets and equal anti terms share their terms.  A selector that
   // fails to convert matches no pod; an empty key is a key no node carries.  self_match: the pending pod matches its
   // whole set.  Classes are numbered in order of first appearance; a pod without entries has none (BS_IPF_NONE).
+  // With `placed`, also each pending pod's placed class over the same dictionary: own = 1 on its required
+  // anti-affinity terms, match = 1 on the bound pods' anti-affinity terms it matches, on every term of each affinity set
+  // it matches as a whole (its own included) and on each pending anti-affinity term it matches (P x terms selector
+  // matching, hence on request).  Its match entries on bound pods' terms are exactly its BS_IPF_EXISTING entries.
   // More than BS_IPA_KEY_MAX keys, BS_IPF_BOUND_MAX bound pods or BS_IPF_CLASS_MAX entries in a class is an error.
   static Status PackInterPodFilter(const std::vector<const NodeInfo*>& snapshot, const std::vector<const Pod*>& pending,
-                                   PackedInterPodFilter* out);
+                                   PackedInterPodFilter* out, bool placed = false);
   // PodFitsHostPorts' columns: HostPortInfo's sanitizing (port <= 0 dropped, "" ip = "0.0.0.0", "" protocol = "TCP");
   // the dictionary holds the pending pods' wanted (ip, protocol, port) in order of first appearance, then the nodes'
   // used ones that conflict with one of them (a used entry that conflicts with nothing wanted never decides a verdict).
@@ -725,6 +739,7 @@ class BatchSchedulingPlugin {
   uint32_t interpod_weight_ = 0;                        // SetInterPodAffinityWeight
   int32_t hard_pod_affinity_weight_ = 1;                // SetHardPodAffinityWeight
   bool interpod_filter_ = false;                        // SetInterPodAffinityFilter
+  bool interpod_filter_walks_ = false;                  // SetInterPodAffinityFilterInWalks
   bool host_port_filter_ = false;                       // SetHostPortFilter
   std::string init_error_;
   int64_t max_schedule_time_ns_;

@@ -39,13 +39,18 @@
 //                      can ever fit again (or that is skipped) is remembered and not rescanned; such
 //                      a node never fits, so it never scores either.  HP (the PodFitsHostPorts filter
 //                      is on): a node whose live used-port mask conflicts with the pod's is not a
-//                      candidate; the dead-node skip stays resource-only;
+//                      candidate; IPF (the MatchInterPodAffinity filter is on): a node that fails steps 1, 3 or 4 of
+//                      include/bsched.h on the live presence planes is not a candidate, step 1 over the pod's
+//                      EXISTING entries and its placed class's match entries; the dead-node skip stays resource-only;
 //   assume + Permit    a handful of stores by the first lanes (SCORED: the chosen node's live
 //                      non-zero column grows by the pod's, NodeInfo.AddPod's nonzeroRequest; HP: the
-//                      pod's wanted entries join the node's live used-port mask).
+//                      pod's wanted entries join the node's live used-port mask; IPF: the pod's placed class joins the
+//                      live presence at the node, as a bound pod there would: match and own bits, per-term counts).
 // Mutable state lives in scratch copies (requested, pod_count, req_present, matched, group flags,
-// representative class, MinResources, the live non-zero column); the uploaded tables are untouched.
+// representative class, MinResources, the live non-zero column, the live presence planes); the uploaded tables are
+// untouched.
 #pragma once
+#include "interpod_filter.cuh"
 #include "kernels.cuh"
 
 #include <type_traits>
@@ -117,8 +122,29 @@ struct ReplayHpArgs : ReplayLocArgs {
   const uint64_t* hp_want;      // [P] each pod's want mask
   const uint64_t* hp_conf;      // [P] each pod's conflict mask (the OR of its wanted entries')
 };
-template <bool LOC, bool HP>
-using ReplayArgsOf = std::conditional_t<HP, ReplayHpArgs, std::conditional_t<LOC, ReplayLocArgs, ReplayArgs>>;
+// IPF's arguments: derived once more, so that the kernels without the filter keep theirs
+struct ReplayIpfArgs : ReplayHpArgs {
+  uint32_t* ipf_mbits;          // live match plane: scratch copy of the pre-pass's
+  uint32_t* ipf_obits;          // live own plane, likewise
+  uint32_t* ipf_hits;           // live per-term counts, likewise
+  IpfTopo tp;                   // the node side's topo (n_nodes = N), term keys and slot offsets
+  IpfPods fc;                   // the filter classes: (term, role), self_match
+  const uint32_t* f_class;      // [P] each pod's filter class or BS_IPF_NONE
+  const uint32_t* q_class;      // [P] each pod's placed class or BS_IPF_NONE
+  const uint32_t* q_off;        // placed classes: (term, own, match), own and match 0 or 1
+  const uint32_t* q_term;
+  const int32_t* q_own;
+  const uint8_t* q_match;
+};
+template <bool LOC, bool HP, bool IPF = false>
+using ReplayArgsOf = std::conditional_t<
+    IPF, ReplayIpfArgs, std::conditional_t<HP, ReplayHpArgs, std::conditional_t<LOC, ReplayLocArgs, ReplayArgs>>>;
+
+// the kind of a staged IPF check: the plane it reads and whether a set bit passes or fails the node
+constexpr uint8_t RIPF_AFFINITY = 0;   // match plane, must be set (step 3)
+constexpr uint8_t RIPF_ANTI = 1;       // match plane, must be clear (step 4)
+constexpr uint8_t RIPF_EXISTING = 2;   // own plane, must be clear (step 1)
+constexpr uint8_t RIPF_SKIP = 3;       // a placed entry without match: nothing to check
 
 template <int MAXL>
 struct ReplaySmem {
@@ -236,8 +262,8 @@ __device__ __forceinline__ void block_scan(ReplaySmem<MAXL>& sm, int64_t (&v)[RE
   for (int k = 0; k < REPLAY_NPT; ++k) keys[k] |= fk;
 }
 
-template <int MAXL, bool SCORED, bool RATIO = false, bool LOC = false, bool HP = false>
-__global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(ReplayArgsOf<LOC, HP> a) {
+template <int MAXL, bool SCORED, bool RATIO = false, bool LOC = false, bool HP = false, bool IPF = false>
+__global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(ReplayArgsOf<LOC, HP, IPF> a) {
   static_assert(SCORED || !RATIO, "the ratio term belongs to the scored node choice");
   static_assert(SCORED || !LOC, "the locality terms belong to the scored node choice");
   __shared__ ReplaySmem<MAXL> sm;
@@ -333,6 +359,12 @@ __global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(ReplayArgsOf<
   __shared__ int64_t s_pod_nz[2][2];
   // HP: the pod's want and conflict masks, likewise (in shared memory: the 16-lane build has no registers to spare)
   __shared__ uint64_t s_hp[2][2];
+  // IPF: the pod's checks, likewise: its filter class's entries, then its placed class's (an E check on each match
+  // entry); per entry the key, the term's first slot and the kind.  s_ipf_meta: entries, filter entries, the filter
+  // class's first entry, its self_match
+  __shared__ uint32_t s_ipf_off[2][2 * BS_IPF_CLASS_MAX];
+  __shared__ uint8_t s_ipf_key[2][2 * BS_IPF_CLASS_MAX], s_ipf_kind[2][2 * BS_IPF_CLASS_MAX];
+  __shared__ uint32_t s_ipf_meta[2][4];
   struct PodRow { uint32_t p; int32_t g; uint8_t pf; uint32_t keys, rc; };
   auto load_row = [&](uint32_t qi, int slot) {
     PodRow r;
@@ -344,6 +376,32 @@ __global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(ReplayArgsOf<
     r.rc = a.pt.rep_class[r.p];
     if constexpr (HP)
       if (tid < 2) s_hp[slot][tid] = tid ? a.hp_conf[r.p] : a.hp_want[r.p];
+    if constexpr (IPF) {
+      const uint32_t fc = a.f_class[r.p], qc = a.q_class[r.p];
+      const uint32_t fo = fc != BS_IPF_NONE ? a.fc.offset[fc] : 0u, nf = fc != BS_IPF_NONE ? a.fc.offset[fc + 1] - fo : 0u;
+      const uint32_t qo = qc != BS_IPF_NONE ? a.q_off[qc] : 0u, nq = qc != BS_IPF_NONE ? a.q_off[qc + 1] - qo : 0u;
+      uint32_t t = 0;
+      uint8_t kind = RIPF_SKIP;
+      if (tid < nf) {
+        t = a.fc.term[fo + tid];
+        const uint8_t role = a.fc.role[fo + tid];
+        kind = role == BS_IPF_AFFINITY ? RIPF_AFFINITY : role == BS_IPF_ANTI ? RIPF_ANTI : RIPF_EXISTING;
+      } else if (tid < nf + nq) {
+        t = a.q_term[qo + tid - nf];
+        if (a.q_match[qo + tid - nf]) kind = RIPF_EXISTING;
+      }
+      if (tid < nf + nq) {
+        s_ipf_key[slot][tid] = (uint8_t)a.tp.term_key[t];
+        s_ipf_off[slot][tid] = a.tp.term_off[t];
+        s_ipf_kind[slot][tid] = kind;
+      }
+      if (tid == 0) {
+        s_ipf_meta[slot][0] = nf + nq;
+        s_ipf_meta[slot][1] = nf;
+        s_ipf_meta[slot][2] = fo;
+        s_ipf_meta[slot][3] = nf ? a.fc.self_match[fc] : 0u;
+      }
+    }
     if constexpr (SCORED)
       if (tid < 2) s_pod_nz[slot][tid] = a.pod_nz[(size_t)tid * P + r.p];
     if (tid < L)   // getPodResourceRequire (core.go:761-772): the packer summed the containers
@@ -639,6 +697,34 @@ __global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(ReplayArgsOf<
       const uint64_t sel = a.rsel[rc], tol = a.rtol[rc];
       int64_t best_s = INT64_MIN;   // SCORED: this thread's best (score, node) so far; node -1 = none
       int32_t best_n = -1;
+      // IPF: the first-pod exception reads the live counts, so it is decided here, after the last step's assume
+      [[maybe_unused]] uint32_t ipf_n = 0;
+      [[maybe_unused]] bool ipf_exempt = false;
+      if constexpr (IPF) {
+        ipf_n = s_ipf_meta[par][0];
+        const uint32_t nf = s_ipf_meta[par][1];
+        if (nf) {   // uniform
+          const bool hit = tid < nf && s_ipf_kind[par][tid] == RIPF_AFFINITY &&
+                           a.ipf_hits[a.fc.term[s_ipf_meta[par][2] + tid]] != 0;
+          ipf_exempt = s_ipf_meta[par][3] && !__syncthreads_or(hit ? 1 : 0);
+        }
+      }
+      // steps 1, 3 and 4 of node n (< N) on the live planes; the order of the steps does not change the verdict
+      [[maybe_unused]] auto ipf_pass = [&](const auto& ia, uint32_t n) -> bool {   // generic: IPF builds only
+        for (uint32_t j = 0; j < ipf_n; ++j) {
+          const uint8_t kind = s_ipf_kind[par][j];
+          if (kind == RIPF_SKIP) continue;
+          const uint32_t v = ia.tp.topo[(size_t)s_ipf_key[par][j] * N + n];
+          bool set = false;
+          if (v != BS_TOPO_NONE) {
+            const uint64_t slot = (uint64_t)s_ipf_off[par][j] + v;
+            const uint32_t* plane = kind == RIPF_EXISTING ? ia.ipf_obits : ia.ipf_mbits;
+            set = ((plane[slot >> 5] >> (slot & 31)) & 1u) != 0;
+          }
+          if (kind == RIPF_AFFINITY ? !(set || ipf_exempt) : set) return false;
+        }
+        return true;
+      };
       for (uint32_t base = lo; base < N; base += REPLAY_BLOCK) {
         int64_t v[REPLAY_NPT][MAXL];
         uint32_t keys[REPLAY_NPT], vis, tok, cf;
@@ -665,6 +751,13 @@ __global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(ReplayArgsOf<
               for (int k = 0; k < REPLAY_NPT; ++k)
                 if (u[k] & conf) fit &= ~(1u << k);
             }
+          }
+        }
+        if constexpr (IPF) {
+          if (ipf_n) {   // uniform: the pod's row
+#pragma unroll
+            for (int k = 0; k < REPLAY_NPT; ++k)
+              if (((fit >> k) & 1u) && !ipf_pass(a, base + REPLAY_NPT * tid + k)) fit &= ~(1u << k);
           }
         }
         if constexpr (SCORED) {
@@ -784,6 +877,25 @@ __global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(ReplayArgsOf<
           if (tid >= 96 && tid < 98) a.nz_live[(size_t)(tid - 96) * Npad + n] += s_pod_nz[par][tid - 96];
         if constexpr (HP)   // NodeInfo.AddPod adds the pod's ports to UsedPorts
           if (tid == 128) a.hp_live[n] |= s_hp[par][0];
+        if constexpr (IPF) {   // the pod joins the node's existing pods: its placed class, one entry per thread
+          const uint32_t qc = a.q_class[cur.p];
+          if (qc != BS_IPF_NONE && tid >= 160) {
+            const uint32_t j = a.q_off[qc] + (tid - 160);
+            if (j < a.q_off[qc + 1]) {
+              const uint32_t t = a.q_term[j];
+              const uint32_t v = a.tp.topo[(size_t)a.tp.term_key[t] * N + n];
+              if (v != BS_TOPO_NONE) {
+                const uint64_t slot = (uint64_t)a.tp.term_off[t] + v;
+                const uint32_t bit = 1u << (slot & 31);
+                if (a.q_match[j]) {
+                  atomicOr(&a.ipf_mbits[slot >> 5], bit);
+                  atomicAdd(&a.ipf_hits[t], 1u);
+                }
+                if (a.q_own[j]) atomicOr(&a.ipf_obits[slot >> 5], bit);
+              }
+            }
+          }
+        }
         if (tid == 0) {
           // ---- Permit (core.go:268-309) ----
           if (g < 0 || (uint32_t)g >= G) {
@@ -808,5 +920,24 @@ __global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(ReplayArgsOf<
   }
   if (tid == 0) { a.status[0] = sm.panic; a.status[1] = (int32_t)lo; a.status[2] = sm.monotone; }
 }
+
+// loc: the scored walk with the locality terms (a is then a ReplayLocArgs); HP: the PodFitsHostPorts filter is on (a is
+// then a ReplayHpArgs); IPF: the MatchInterPodAffinity filter is on (a is then a ReplayIpfArgs)
+template <int MAXL, bool HP, bool IPF = false>
+void launch_replay_t(const ReplayArgs& a, bool scored, bool loc, cudaStream_t s) {
+  if (loc) {
+    const auto& la = static_cast<const ReplayArgsOf<true, HP, IPF>&>(a);
+    if (a.ratio.weight) replay_kernel<MAXL, true, true, true, HP, IPF><<<1, REPLAY_THREADS, 0, s>>>(la);
+    else replay_kernel<MAXL, true, false, true, HP, IPF><<<1, REPLAY_THREADS, 0, s>>>(la);
+    return;
+  }
+  const auto& ha = static_cast<const ReplayArgsOf<false, HP, IPF>&>(a);
+  if (scored && a.ratio.weight) replay_kernel<MAXL, true, true, false, HP, IPF><<<1, REPLAY_THREADS, 0, s>>>(ha);
+  else if (scored) replay_kernel<MAXL, true, false, false, HP, IPF><<<1, REPLAY_THREADS, 0, s>>>(ha);
+  else replay_kernel<MAXL, false, false, false, HP, IPF><<<1, REPLAY_THREADS, 0, s>>>(ha);
+}
+// replay_ipf_inst.cu, one translation unit per MAXL (-DBS_REPLAY_IPF_MAXL): the IPF builds, launch_replay_t<MAXL, HP, true>
+template <int MAXL, bool HP>
+void launch_replay_ipf(const ReplayArgs& a, bool scored, bool loc, cudaStream_t s);
 
 }  // namespace bsk

@@ -446,8 +446,8 @@ class Engine:
 
     def set_interpod_filter(self, on: bool = False):
         """Switch kube-scheduler's MatchInterPodAffinity filter (required pod affinity and anti-affinity) into every
-        pod's fit set (off by default).  While it is on, each round needs upload_interpod_filter's two sides, and
-        replay and preempt refuse to run."""
+        pod's fit set (off by default).  While it is on, each round needs upload_interpod_filter's two sides, replay
+        needs upload_interpod_placed as well (it refuses to run without it), and preempt refuses to run."""
         self._check(self.lib.bs_set_interpod_filter(self.h, 1 if on else 0))
 
     def upload_interpod_filter(self, node=None, pods=None):
@@ -466,6 +466,16 @@ class Engine:
                  np.ascontiguousarray(role, dtype=np.uint8), np.ascontiguousarray(self_match, dtype=np.uint8)]
             t = capi.InterpodFilterPodsC(len(a[0]), capi.ptr(a[0]), max(len(a[1]) - 1, 0), *(capi.ptr(x) for x in a[1:]))
             self._check(self.lib.bs_upload_pod_interpod_filter(self.h, C.byref(t)))
+
+    def upload_interpod_placed(self, pod_class, classes):
+        """The placed side of the MatchInterPodAffinity filter (include/bsched.h bs_upload_pod_interpod_placed): what
+        each pending pod adds to presence once replay assumes it.  pod_class [P] (capi.IPF_NONE: nothing) and classes
+        (class_offset [C + 1], term, own int32, match uint8) over the filter's dictionary, as a bound pod's class: own 1
+        on the pod's required anti-affinity terms, match 1 on the terms it matches.  Uploading pods drops it."""
+        keep = []
+        pcls = np.ascontiguousarray(pod_class, dtype=np.uint32).reshape(-1)
+        t = capi.InterpodPodsC(len(pcls), capi.ptr(pcls), _interpod_classes(classes, keep))
+        self._check(self.lib.bs_upload_pod_interpod_placed(self.h, C.byref(t)))
 
     def fetch_interpod_reason_rows(self, pod0=0, n=None) -> np.ndarray:
         """[n, 3] uint32: the companion of reason_rows, the nodes that fail MatchInterPodAffinity after every other
@@ -548,7 +558,9 @@ class Engine:
         node and group columns (the uploaded tables themselves are left untouched).
         priority=True places each passing pod on its best node under the resource priorities on the live
         state (bs_replay_priority; needs upload_nonzero, weights from set_score_weights) instead of the first
-        fitting one; with after_state the dict also holds the live non-zero column node_nonzero [2, N]."""
+        fitting one; with after_state the dict also holds the live non-zero column node_nonzero [2, N].
+        Both walks apply the filters that are on: PodFitsHostPorts on live used ports, and MatchInterPodAffinity on
+        live presence that each assumed pod's placed class (upload_interpod_placed) joins."""
         q = None if queue is None else np.ascontiguousarray(queue, dtype=np.uint32)
         n = self.P if q is None else len(q)
         L, N, G = self.n_lanes, self.N, self.G

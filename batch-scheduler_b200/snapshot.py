@@ -613,6 +613,48 @@ def node_interpod_filter(snap: Snapshot, seed: int, n_zones: int = 8, unlabelled
     return node, pods
 
 
+def node_interpod_walk(snap: Snapshot, seed: int, pending_ps: float = 0.8, **kw):
+    """node_interpod_filter's columns (same seed and keywords, same draws) plus a placed side consistent with them, as
+    Engine.upload_interpod_placed takes it: (node, pods, placed).  A gang's pods own and match their hostname
+    anti-affinity term, match their self-affine set and match the blockers' terms their filter class lists as EXISTING.
+    For a share pending_ps of the parameter-server gangs, one pod of the table without a filter class becomes the
+    pending parameter server: its placed class matches the gang's affinity term.  Own generator: other draws keep
+    their seeds."""
+    node, pods = node_interpod_filter(snap, seed, **kw)
+    pod_class, (poff, pterm, prole, pself) = pods
+    rng = np.random.default_rng(seed + 0x5EED)
+    qoff, qterm, qown, qmatch = [0], [], [], []
+    qcls_of = np.full(len(pself), IPF_NONE, np.uint32)
+    ps_terms = []
+    for c in range(len(pself)):
+        ent = []
+        for k in range(poff[c], poff[c + 1]):
+            t, r = int(pterm[k]), int(prole[k])
+            if r == IPF_ANTI:
+                ent.append((t, 1, 1))
+            elif r == IPF_EXISTING or (r == IPF_AFFINITY and pself[c]):
+                ent.append((t, 0, 1))
+            elif r == IPF_AFFINITY:
+                ps_terms.append(t)
+        if ent:
+            qcls_of[c] = len(qoff) - 1
+            for t, o, m in ent:
+                qterm.append(t); qown.append(o); qmatch.append(m)
+            qoff.append(len(qterm))
+    placed_class = np.where(pod_class != IPF_NONE, qcls_of[np.minimum(pod_class, max(len(pself) - 1, 0))]
+                            if len(pself) else IPF_NONE, IPF_NONE).astype(np.uint32)
+    free = list(rng.permutation(np.flatnonzero(pod_class == IPF_NONE)))
+    for t in sorted(set(ps_terms)):
+        if rng.random() >= pending_ps or not free:
+            continue
+        placed_class[free.pop()] = len(qoff) - 1
+        qterm.append(t); qown.append(0); qmatch.append(1)
+        qoff.append(len(qterm))
+    placed = (placed_class, (np.array(qoff, np.uint32), np.array(qterm, np.uint32), np.array(qown, np.int32),
+                             np.array(qmatch, np.uint8)))
+    return node, pods, placed
+
+
 # ----------------------------------------------------------------------------
 # splitmix64 stream (vectorised): value i of the stream with seed s is
 # mix(s + (i+1)*0x9E3779B97F4A7C15).

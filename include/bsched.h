@@ -707,8 +707,19 @@ int bs_upload_pod_interpod(bs_engine* e, const bs_interpod_pods* t);
  * selector that does not convert matches no pod.  A BS_IPF_NONE pod passes every node.
  * An evaluation with the filter on is BS_E_STATE before anything is launched when either side is missing, BS_E_INDEX
  * when a pod class's term is >= the node side's n_terms and BS_E_INVAL when the class bit planes pass
- * BS_IPF_TABLE_MAX_BYTES.  bs_replay, bs_replay_priority, bs_preempt and bs_preempt_walk refuse to run (BS_E_INVAL)
- * while the filter is on: their walks would need presence that follows their own placements and victim removals.
+ * BS_IPF_TABLE_MAX_BYTES.  bs_preempt and bs_preempt_walk refuse to run (BS_E_INVAL) while the filter is on: their
+ * walks would need presence that shrinks when victims leave.
+ *
+ * The walks.  bs_replay and bs_replay_priority apply the filter on live presence once the pods' placed classes are
+ * uploaded (bs_upload_pod_interpod_placed); without them they refuse to run (BS_E_INVAL).  Live presence starts as the
+ * snapshot's, and each assume adds the pod's placed class at its node as a bound pod there would add its class.  For
+ * step i's pod and a candidate node the four steps above run on live presence, with one widening of step 1: besides
+ * the EXISTING entries of the pod's filter class, every match entry of its placed class is checked against the own
+ * bits, so that an anti-affinity term a previously assumed pod owns keeps out a pod whose filter class is BS_IPF_NONE.
+ * The first-pod exception reads the live counts.  A node that fails is not a candidate; PreFilter, the cluster scans,
+ * findMaxPG, Permit, the dead-node skip and the after-state are unchanged, and presence only grows.  When every placed
+ * match entry on a term some bound pod owns is also an EXISTING entry of the pod's filter class, the first step sees
+ * exactly the round's verdicts.
  *
  * Exactness: presence is one bit per (term, value) and plane, set with atomicOr, and the emptiness test of step 3 is a
  * per-term count of at most BS_IPF_BOUND_MAX, so every verdict is exact whatever the order. */
@@ -736,6 +747,14 @@ int bs_upload_node_interpod_filter(bs_engine* e, const bs_interpod_nodes* t);
 /* The pod side.  A wrong n_pods, a malformed class table or a role > BS_IPF_EXISTING is BS_E_INVAL, a pod_class out of
  * range BS_E_INDEX, a self_match > 1 BS_E_RANGE; a failing call leaves it dropped.  bs_upload_pods drops it. */
 int bs_upload_pod_interpod_filter(bs_engine* e, const bs_interpod_filter_pods* t);
+/* The placed side: what each pending pod adds to presence once a walk assumes it, in the layout of a bound pod's class
+ * over the filter's dictionary: (t, own, match) with own = 1 when t is one of the pod's required anti-affinity terms and
+ * match = 1 when the pod matches t (an affinity set's term: every term of the set); entries with both 0 are left out,
+ * BS_IPF_NONE is no entries, at most BS_IPF_CLASS_MAX entries per class.  A wrong n_pods or a malformed class table is
+ * BS_E_INVAL, a pod_class out of range BS_E_INDEX, an own or match outside {0, 1} BS_E_RANGE; a failing call leaves it
+ * dropped.  Its terms are checked against the node side's n_terms when a walk starts (BS_E_INDEX, before anything is
+ * launched).  With the filter off it is not read.  bs_upload_pods drops it. */
+int bs_upload_pod_interpod_placed(bs_engine* e, const bs_interpod_pods* t);
 /* The companion of bs_fetch_reason_rows (BS_OUT_REASONS): dense [n][3] counters, the nodes that pass the guards,
  * checkFit and every lane of pod pod0 + p and then fail the filter at step 1 (E), 3 (A) or 4 (N).  All zero for a
  * round evaluated with the filter off. */

@@ -366,8 +366,8 @@ const (
 )
 
 // SetInterPodAffinityFilter: kube-scheduler v1.17's MatchInterPodAffinity filter in every pod's fit set (off by
-// default).  While it is on, each Evaluate needs both filter sides, and Replay, ReplayPriority, Preempt and
-// PreemptWalk refuse to run.
+// default).  While it is on, each Evaluate needs both filter sides, Replay and ReplayPriority need the placed side
+// as well (UploadPodInterPodPlaced; they refuse to run without it), and Preempt and PreemptWalk refuse to run.
 func (e *Engine) SetInterPodAffinityFilter(on bool) error {
 	v := C.int(0)
 	if on {
@@ -384,6 +384,13 @@ func (e *Engine) UploadNodeInterPodFilter(t *C.bs_interpod_nodes) error {
 }
 func (e *Engine) UploadPodInterPodFilter(t *C.bs_interpod_filter_pods) error {
 	return e.rc(C.bs_upload_pod_interpod_filter(e.h, t))
+}
+
+// UploadPodInterPodPlaced: the filter's placed side, what each pending pod adds to presence once a walk assumes it, in
+// the layout of a bound pod's class (own on its anti-affinity terms, match on the terms it matches).  UploadPods drops
+// it.
+func (e *Engine) UploadPodInterPodPlaced(t *C.bs_interpod_pods) error {
+	return e.rc(C.bs_upload_pod_interpod_placed(e.h, t))
 }
 
 // FetchInterPodReasonRows: the companion of FetchReasonRows, counts[n][3] (E, A, N) of the nodes that pass every
