@@ -2229,13 +2229,15 @@ int bs_upload_pods(bs_engine* e, const bs_pod_table* t) {
   if (!e || !t) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
   drop_pod_sides(e);
-  e->filt.pfc_base_valid = false;   // the new table's fit classes are its base classes
-  e->filt.assign_dirty = false;
   if (t->n_lanes != e->L) return fail(e, BS_E_INVAL, "bs_upload_pods: n_lanes differs from the engine's");
   const uint32_t P = t->n_pods, L = e->L;
   if (P && (!t->req || !t->req_present || !t->gid || !t->sel_mask || !t->tol_mask || !t->priority ||
             !t->ts_ns || !t->flags))
     return fail(e, BS_E_INVAL, "bs_upload_pods: null column");
+  // Only now does the new table replace the old one: a call refused above keeps the old table, whose h_pfc may hold
+  // the classes the filters gave it, and h_pfc_base its base classes.
+  e->filt.pfc_base_valid = false;   // the new table's fit classes are its base classes
+  e->filt.assign_dirty = false;
   // ONE parallel pass over the table before anything is committed: per-lane maxima (range check and
   // wide/narrow lane classification), the varying bits of the sort keys, thread-local class indices
   // (fit class = (sel, tol, scalar keys requested with a non-zero amount, core.go:688-690);

@@ -6,10 +6,11 @@ include/bsched.h's; Model.expect(cfg) gives every output of a round on the curre
 restatements only (the oracle, the reason rows, the priority lists, the lane classifier, the walks and preemption).
 
 generate(seed) is a list of ops: random uploads, row updates, side columns, weights, failing calls and rounds, the
-MatchInterPodAffinity filter's switch and halves (both built with one seed, so that they describe one cluster),
+MatchInterPodAffinity filter's switch, halves and placed side (all built with one seed, so that they describe one
+cluster), the PodFitsHostPorts filter's switch and halves (failing ones too), walks with either filter or both,
 bound-pod tables with PodDisruptionBudget bits, preemption and preemption walks (now and then with a list that breaks
-one of bs_preempt_walk's rules), plus the scripted bursts R1-R9 (every seed runs at least one; across seeds all of
-them):
+one of bs_preempt_walk's rules), plus the scripted bursts R1-R12 (every seed runs at least one; across seeds all of
+them, each first in some seed):
   R1  more than 4096 fit and representative classes, then a table with few (both persistent class indices clear),
       then bs_update_groups with a new representative class, then a round;
   R2  node tables of 0, 1, 511, 512, 513 and more nodes, growing and shrinking, every side uploaded again after each;
@@ -24,7 +25,15 @@ them):
   R8  more than 4096 fit classes under the filter, pod halves in new filter classes until the fit class index is
       compacted, the switch toggled, a group row update and an affinity table in between, then a small pod table;
   R9  preemption with budget bits and walks after a group row update, a node row update and a group upload, and one
-      walk per broken list rule.
+      walk per broken list rule;
+  R10 the ports filter's lifecycle: the switch without halves, each half dropped by the call that owns it, a node
+      table of another size, a pod table refused for its lane count followed by another want half and a round, every
+      failing node half, a dictionary the want bits pass, preemption refused, the switch off;
+  R11 more than 4096 fit classes under the ports filter, want halves in new conflict classes until the fit class index
+      is compacted, the inter-pod switch toggled and a group row update in between, then a small pod table;
+  R12 walks under the inter-pod filter, the ports filter and both: right after a filter half and before any round,
+      after a node row update and the node halves again; the placed side dropped by a refused pod upload, a placed
+      term past the filter's dictionary, and the placed side not read with the filter off.
 """
 from __future__ import annotations
 
@@ -32,8 +41,10 @@ import numpy as np
 
 import fit_reasons_ref as frr
 import fit_shape_cases as fsc
+import host_ports_ref as hr
 import interpod_filter_ref as fr
 import interpod_priority_ref as ir
+import interpod_walk_ref as iwr
 import locality_priority_ref as lpr
 import preempt_pdb_ref
 import preempt_walk_ref as pwr
@@ -88,6 +99,23 @@ def _apply_rows(table, idx, rows):
     return out
 
 
+def _or(masks):
+    """The OR of a uint64 mask column, as a Python int."""
+    return int(np.bitwise_or.reduce(np.asarray(masks, np.uint64).reshape(-1), initial=np.uint64(0)))
+
+
+def no_interpod_filter(N, P):
+    """((node, pods), placed): MatchInterPodAffinity filter columns without a term, every pod without a class and a
+    placed side without a class.  interpod_walk_ref.replay passes every node with them, so that it walks the ports
+    filter alone around any chooser."""
+    none = np.full(P, S.IPF_NONE, np.uint32)
+    u32 = lambda n: np.zeros(n, np.uint32)
+    node = (u32(0), np.zeros((0, N), np.uint32), u32(0), u32(0), u32(0),
+            (u32(1), u32(0), np.zeros(0, np.int32), np.zeros(0, np.uint8)))
+    pods = (none, (u32(1), u32(0), np.zeros(0, np.uint8), np.zeros(0, np.uint8)))
+    return (node, pods), (none.copy(), (u32(1), u32(0), np.zeros(0, np.int32), np.zeros(0, np.uint8)))
+
+
 def _max_class(cls, none):
     c = np.asarray(cls, np.int64)
     c = c[c != none]
@@ -110,6 +138,11 @@ class Model:
         # the MatchInterPodAffinity filter: the switch, its two halves (node: the node side's columns, pod: (pod_class,
         # class table)), and whether the last successful round ran with the switch on (else its companion rows are 0)
         self.ipf_on, self.ipf_node, self.ipf_pod, self.ipf_round = False, None, None, False
+        # the filter's placed side (pod_class, class table): what the walks add to presence for each pod they assume
+        self.ipf_placed = None
+        # the PodFitsHostPorts filter: the switch, its two halves (node: (entries [K, 3], used [N]), pod: want [P]) and
+        # whether the last successful round ran with it on (else its companion rows are 0)
+        self.hp_on, self.hp_node, self.hp_pod, self.hp_round = False, None, None, False
 
     # ---- state ---------------------------------------------------------------------------------------------------
     def snapshot(self):
@@ -133,7 +166,7 @@ class Model:
     def _upload_nodes(self, op):
         nt = op["table"]
         self._drop(NODE_SIDES)
-        self.ipf_node = None
+        self.ipf_node = self.hp_node = None
         self.bound, self.aff = None, None   # they belong to the snapshot, also to one that fails validation
         if _out_of_range(nt.alloc, nt.requested):
             self.nodes = None
@@ -146,7 +179,7 @@ class Model:
         if self.nodes is None:
             return E_STATE
         self._drop(NODE_SIDES)   # every call, also one that changes no row or fails (bsched.h bs_update_nodes)
-        self.ipf_node = None
+        self.ipf_node = self.hp_node = None
         if len(idx) == 0:
             return None
         if (np.asarray(idx) >= self.nodes.n).any():
@@ -183,7 +216,8 @@ class Model:
     def _upload_pods(self, op):
         pt = op["table"]
         self._drop(POD_SIDES)
-        self.ipf_pod = None      # also by a call refused for its lane count, which keeps the pod table of now
+        self.ipf_pod = self.ipf_placed = self.hp_pod = None   # also by a call refused for its lane count, which keeps
+        # the pod table of now
         if pt.lanes != self.lanes:
             return E_INVAL
         if _out_of_range(pt.req):
@@ -237,6 +271,50 @@ class Model:
         self.ipf_on = bool(op["on"])
         return None
 
+    def _placed(self, op):
+        """The filter's placed side: cols = (pod_class, (class_offset, term, own, match)), n (its length)."""
+        self.ipf_placed = None   # a failing call leaves it dropped
+        if self.pods is None:
+            return E_STATE
+        if op["n"] != self.pods.n:
+            return E_INVAL
+        pcls, (off, _, own, _) = op["cols"]
+        if _max_class(pcls, S.IPF_NONE) >= len(off) - 1:
+            return E_INDEX
+        if not np.isin(np.asarray(own, np.int64), (0, 1)).all():
+            return E_RANGE
+        self.ipf_placed = op["cols"]
+        return None
+
+    def _hp(self, op):
+        """One half of the ports filter's columns: half (node: cols = (entries [K, 3], used [N]); pod: cols = want
+        [P]), n (its length).  The node half's checks in the engine's order: the length, more than 64 entries, a port
+        outside 1..65535, an entry listed twice, a used bit past the entries."""
+        key = "hp_" + op["half"]
+        setattr(self, key, None)   # a failing call leaves the half dropped
+        table = self.nodes if op["half"] == "node" else self.pods
+        if table is None:
+            return E_STATE
+        if op["n"] != table.n:
+            return E_INVAL
+        if op["half"] == "node":
+            ent = np.asarray(op["cols"][0], np.int64).reshape(-1, 3)
+            K = len(ent)
+            if K > 64:
+                return E_INVAL
+            if ((ent[:, 2] < 1) | (ent[:, 2] > 65535)).any():
+                return E_RANGE
+            if len(set(map(tuple, ent.tolist()))) < K:
+                return E_INVAL
+            if K < 64 and _or(op["cols"][1]) >> K:
+                return E_INDEX
+        setattr(self, key, op["cols"])
+        return None
+
+    def _hp_switch(self, op):
+        self.hp_on = bool(op["on"])
+        return None
+
     def _weights(self, op):
         for k, v in op.items():
             if k != "op":
@@ -246,7 +324,7 @@ class Model:
     def _evaluate(self, op):
         rc = self._evaluate_check(op)
         if rc is None:
-            self.ipf_round = self.ipf_on
+            self.ipf_round, self.hp_round = self.ipf_on, self.hp_on
         return rc
 
     def _evaluate_check(self, op):
@@ -276,12 +354,23 @@ class Model:
                     return E_STATE
                 if _max_class(sd["ipa_pod"][1][1], -1) >= len(sd["ipa_node"][2]):
                     return E_INDEX
-        if self.ipf_on:
-            if self.ipf_node is None or self.ipf_pod is None:
-                return E_STATE
-            if _max_class(self.ipf_pod[1][1], -1) >= len(self.ipf_node[2]):   # any class's term, used or not
-                return E_INDEX
-        return self._affinity_check()
+        rc = (self.ipf_on and self._interpod_filter_check()) or (self.hp_on and self._host_port_check())
+        return rc or self._affinity_check()
+
+    def _interpod_filter_check(self):
+        if self.ipf_node is None or self.ipf_pod is None:
+            return E_STATE
+        if _max_class(self.ipf_pod[1][1], -1) >= len(self.ipf_node[2]):   # any class's term, used or not
+            return E_INDEX
+        return None
+
+    def _host_port_check(self):
+        if self.hp_node is None or self.hp_pod is None:
+            return E_STATE
+        K = len(np.asarray(self.hp_node[0]).reshape(-1, 3))
+        if K < 64 and _or(self.hp_pod) >> K:   # a want bit past the node half's entries
+            return E_INDEX
+        return None
 
     def _locality_check(self):
         sd = self.side
@@ -303,10 +392,13 @@ class Model:
         return None
 
     def _replay(self, op):
-        if self.ipf_on:
-            return E_INVAL     # refused while the filter is on, before anything else
+        """bs_replay / bs_replay_priority (engine.cu replay_walk): the filter on without the placed side and then
+        bs_replay_priority's weights before anything else; the tables, the non-zero columns, locality, the ports
+        filter, the inter-pod filter, a placed term past the filter's dictionary, then the affinity class ids."""
+        if self.ipf_on and self.ipf_placed is None:
+            return E_INVAL
         if op["priority"] and (any(self.pw) or self.w_spread or self.w_ipa):
-            return E_INVAL     # bs_replay_priority refuses these weights before anything else
+            return E_INVAL
         if not self.complete():
             return E_STATE
         if op["priority"]:
@@ -315,12 +407,17 @@ class Model:
             rc = self._locality_check() if any(self.lw) else None
             if rc:
                 return rc
+        rc = (self.hp_on and self._host_port_check()) or (self.ipf_on and self._interpod_filter_check())
+        if rc:
+            return rc
+        if self.ipf_on and _max_class(self.ipf_placed[1][1], -1) >= len(self.ipf_node[2]):
+            return E_INDEX
         return self._affinity_check()
 
     def _preempt(self, op):
-        """bs_preempt's checks (preempt_pods in engine.cu): the switch, the tables, then each listed pod's index and
-        affinity class."""
-        if self.ipf_on:
+        """bs_preempt's checks (preempt_pods in engine.cu): the filters' switches, the tables, then each listed pod's
+        index and affinity class."""
+        if self.ipf_on or self.hp_on:
             return E_INVAL
         if not self.complete() or self.bound is None:
             return E_STATE
@@ -378,10 +475,11 @@ class Model:
     def expect(self, cfg):
         """Every output of a round on this state for an engine built with cfg (score, fit_bitmap, filter, reasons,
         topk, priority_k): a dict of arrays, keyed as the GPU test reads them back.  With the filter on, the round is
-        interpod_filter_ref.expected_round's; interpod_rows (with reasons) are the companion rows, zero when the last
-        round ran with the filter off."""
+        interpod_filter_ref.expected_round's, with the ports filter on host_ports_ref.expected_round's (with the
+        inter-pod verdicts when both are on); interpod_rows and host_port_rows (with reasons) are the companion rows,
+        zero when the last round ran with that filter off."""
         snap = self.snapshot()
-        if self.ipf_round:
+        if self.ipf_round or self.hp_round:
             def lists(fsnap, score):
                 out = {}
                 if cfg.get("topk"):
@@ -389,7 +487,16 @@ class Model:
                 if cfg.get("priority_k"):
                     out["priority_nodes"], out["priority_scores"] = self.priority_rows(cfg["priority_k"], snap=fsnap)
                 return out
-            out, _ = fr.expected_round(snap, (self.ipf_node, self.ipf_pod), cfg, lists)
+            ipf = (self.ipf_node, self.ipf_pod)
+            if self.hp_round:
+                (entries, used), want = self.hp_node, self.hp_pod
+                ipf_v = fr.verdicts(ipf, self.nodes.n) if self.ipf_round else None
+                out, _ = hr.expected_round(snap, hr.passes(entries, used, want), cfg, lists, ipf_v)
+            else:
+                out, _ = fr.expected_round(snap, ipf, cfg, lists)
+            if cfg.get("reasons"):
+                out.setdefault("interpod_rows", np.zeros((self.pods.n, 3), np.uint32))
+                out.setdefault("host_port_rows", np.zeros(self.pods.n, np.uint32))
             out["lanes"] = fsc.classify(self.nodes, self.pods, self.history)
             return out
         orc = oracle.round(snap, want_bitmap=True, want_score=True, want_filter=cfg.get("filter", False))
@@ -407,20 +514,32 @@ class Model:
         if cfg.get("reasons"):
             out["reason_rows"] = frr.fit_reasons(snap)
             out["interpod_rows"] = np.zeros((self.pods.n, 3), np.uint32)
+            out["host_port_rows"] = np.zeros(self.pods.n, np.uint32)
         if cfg.get("priority_k"):
             out["priority_nodes"], out["priority_scores"] = self.priority_rows(cfg["priority_k"])
         out["lanes"] = fsc.classify(self.nodes, self.pods, self.history)
         return out
 
     def expect_walk(self, priority, queue):
+        """The walk on this state: with either filter on interpod_walk_ref.replay (with the ports filter inside it;
+        with the inter-pod filter off, one without terms), else the oracle's walk or bs_replay_priority's."""
         snap = self.snapshot()
+        sd = self.side
+        loc = None
         if priority:
-            sd = self.side
             loc = (sd["loc_node"], sd["loc_pod"]) if any(self.lw) else \
                 ((np.zeros(0, np.int64), np.zeros((0, (self.nodes.n + 31) // 32), np.uint32),
                   np.zeros(self.nodes.n, np.uint64)),
                  (np.full(self.pods.n, S.IMAGE_NONE, np.uint32), np.zeros(1, np.uint32), np.zeros(0, np.uint32),
                   np.full(self.pods.n, S.AVOID_NONE, np.uint8)))
+        if self.ipf_on or self.hp_on:
+            cols, placed = ((self.ipf_node, self.ipf_pod), self.ipf_placed) if self.ipf_on else \
+                no_interpod_filter(self.nodes.n, self.pods.n)
+            nz = (sd["nz_node"], sd["nz_pod"]) if priority else None
+            hp = (self.hp_node, self.hp_pod) if self.hp_on else None
+            pf, node, ready, _, _, _ = iwr.replay(snap, cols, placed, queue, nz, self.weights, self.ratio_setting(), loc,
+                                                  self.lw, hp)
+        elif priority:
             pf, node, ready, _, _ = lpr.replay_locality(snap, sd["nz_node"], sd["nz_pod"], loc, self.lw,
                                                         self.ratio_setting(), queue, self.weights)
         else:
@@ -466,7 +585,8 @@ class Generator:
         self.ops = []
         self.regimes = set()
         self.max_p = 0
-        self.ipf_seed = seed   # both filter halves are built with it, so that they describe one cluster
+        self.ipf_seed = seed   # both filter halves and the placed side are built with it: they describe one cluster
+        self.hp_seed = seed    # both ports halves are built with it: they draw the same dictionary
 
     def _k(self):
         return int(self.rng.integers(0, 1 << 30))
@@ -534,14 +654,19 @@ class Generator:
         self.emit({"op": "update_groups", "idx": idx, "rows": rows})
 
     # -- sides --
+    def _now(self):
+        """The snapshot of now, with empty tables for the missing ones."""
+        m = self.model
+        return S.Snapshot(m.nodes if m.nodes is not None else S.NodeTable.empty(0, self.L),
+                          m.pods if m.pods is not None else S.PodTable.empty(0, self.L),
+                          m.groups if m.groups is not None else S.GroupTable.empty(0, self.L))
+
     def side(self, name, half, mismatch=False, wrong_len=False):
         m = self.model
         table = m.nodes if half == "node" else m.pods
         if table is None:
             return
-        snap = S.Snapshot(m.nodes if m.nodes is not None else S.NodeTable.empty(0, self.L),
-                          m.pods if m.pods is not None else S.PodTable.empty(0, self.L),
-                          m.groups if m.groups is not None else S.GroupTable.empty(0, self.L))
+        snap = self._now()
         k = self._k()
         if name == "nz":
             cols = S.nonzero_requests(snap, k)[0 if half == "node" else 1]
@@ -579,6 +704,9 @@ class Generator:
                 self.side(name, half)
         for half in halves:
             self.ipf(half)
+            self.hp(half)
+        if "pod" in halves:
+            self.placed()
 
     def node_sides(self):
         """The node halves again (the filter's too), as a caller does after bs_update_nodes dropped them."""
@@ -592,10 +720,7 @@ class Generator:
         table = m.nodes if half == "node" else m.pods
         if table is None:
             return
-        snap = S.Snapshot(m.nodes if m.nodes is not None else S.NodeTable.empty(0, self.L),
-                          m.pods if m.pods is not None else S.PodTable.empty(0, self.L),
-                          m.groups if m.groups is not None else S.GroupTable.empty(0, self.L))
-        node, pods = S.node_interpod_filter(snap, self._k() if mismatch else self.ipf_seed)
+        node, pods = S.node_interpod_filter(self._now(), self._k() if mismatch else self.ipf_seed)
         if half == "node":
             nv, topo, tkey, bnode, bcls, bcl = node
             if not m.nodes.n:   # the generator puts bound pods on node 0 of an empty table: none can be bound
@@ -618,8 +743,63 @@ class Generator:
             cols, n = (pcls, (off, term, role, selfm)), len(pcls)
         self.emit({"op": "ipf", "half": half, "n": n, "cols": cols})
 
+    def hp(self, half, wrong_len=False, bad=None, n_entries=12):
+        """One half of the ports filter's columns: host_ports_ref.random_columns on the state of now with hp_seed (both
+        halves draw the same dictionary first, so a node half of fewer n_entries is a prefix of it); wrong_len: one
+        entry too many; bad (node half): "port" (a port 0), "twice" (an entry listed twice), "used" (a used bit past
+        the entries) or "many" (65 entries)."""
+        m = self.model
+        table = m.nodes if half == "node" else m.pods
+        if table is None:
+            return
+        (entries, used), want = hr.random_columns(self._now(), self.hp_seed, n_entries=n_entries)
+        if half == "pod":
+            cols = np.r_[want, np.uint64(0)].astype(np.uint64) if wrong_len else want
+            self.emit({"op": "hp", "half": half, "n": len(cols), "cols": cols})
+            return
+        entries, used = entries.copy(), used.copy()
+        if bad == "port":
+            entries[-1, 2] = 0
+        elif bad == "twice":
+            entries[-1] = entries[0]
+        elif bad == "used" and len(used):
+            used[-1] |= np.uint64(1) << np.uint64(len(entries))
+        elif bad == "many":
+            entries = np.array([(1, 0, 1000 + k) for k in range(65)], np.int64)
+        if wrong_len:
+            used = np.r_[used, np.uint64(0)].astype(np.uint64)
+        self.emit({"op": "hp", "half": half, "n": len(used), "cols": (entries, used), "bad": bad})
+
+    def placed(self, wrong_len=False, bad=None):
+        """The filter's placed side from snapshot.node_interpod_walk on the state of now with ipf_seed (the draws of
+        the filter's halves); wrong_len: one entry too many; bad: "class" (a pod class out of range), "own" (an own of
+        2) or "term" (a term one past the node half's dictionary, or past 24 terms without one)."""
+        m = self.model
+        if m.pods is None:
+            return
+        pcls, (off, term, own, match) = S.node_interpod_walk(self._now(), self.ipf_seed)[2]
+        if bad == "class":
+            pcls = np.full(len(pcls), len(off) - 1, np.uint32)
+        elif bad in ("own", "term"):   # one more class of one entry, the last pod in it
+            T = len(m.ipf_node[2]) if m.ipf_node is not None else 24
+            off, term = np.r_[off, off[-1] + 1].astype(np.uint32), np.r_[term, T if bad == "term" else 0].astype(np.uint32)
+            own, match = np.r_[own, 2 if bad == "own" else 0].astype(np.int32), np.r_[match, 1].astype(np.uint8)
+            if len(pcls):
+                pcls = pcls.copy()
+                pcls[-1] = len(off) - 2
+        if wrong_len:
+            pcls = np.r_[pcls, np.uint32(S.IPF_NONE)].astype(np.uint32)
+        self.emit({"op": "placed", "n": len(pcls), "cols": (pcls, (off, term, own, match)), "bad": bad})
+
     def switch(self, on):
         self.emit({"op": "ipf_switch", "on": on})
+
+    def hp_switch(self, on):
+        self.emit({"op": "hp_switch", "on": on})
+
+    def walk_weights(self):
+        """The weights bs_replay_priority refuses set to 0 (the resource, ratio and locality terms stay)."""
+        self.emit({"op": "weights", "pw": (0, 0), "w_spread": 0, "w_ipa": 0})
 
     def weights(self, on):
         L = self.L
@@ -788,16 +968,22 @@ class Generator:
         return {"pref": {"pw": (0, 0)}, "loc": {"lw": (0, 0)}, "spread": {"w_spread": 0}, "ipa": {"w_ipa": 0}}[name]
 
     def all_sides_but(self, skip):
-        """Every missing side but `skip` (a side's name, or "ipf": the filter's halves)."""
+        """Every missing side but `skip` (a side's name, "ipf": the filter's halves and its placed side, "hp": the
+        ports filter's halves, or "placed")."""
+        m = self.model
         for name in ("nz", "pref", "loc", "spread", "ipa"):
             if name == skip:
                 continue
             for half in ("node", "pod"):
-                if self.model.side[name + "_" + half] is None:
+                if m.side[name + "_" + half] is None:
                     self.side(name, half)
         for half in ("node", "pod"):
-            if skip != "ipf" and getattr(self.model, "ipf_" + half) is None:
+            if skip != "ipf" and getattr(m, "ipf_" + half) is None:
                 self.ipf(half)
+            if skip != "hp" and getattr(m, "hp_" + half) is None:
+                self.hp(half)
+        if skip not in ("ipf", "placed") and m.ipf_placed is None:
+            self.placed()
 
     def r5(self):
         self.base()
@@ -924,6 +1110,7 @@ class Generator:
         """Preemption with PodDisruptionBudget bits and the walk: after a group row update (the bound table stays),
         after a node row update and after a group upload (both drop it), and one walk per broken list rule."""
         self.switch(False)
+        self.hp_switch(False)
         self.base()
         self.bound()
         self.walk("preempt")
@@ -943,7 +1130,177 @@ class Generator:
         self.preempt_walk(True)
         self.regimes.add("R9")
 
+    def r10(self):
+        """The ports filter's lifecycle: the switch without halves, each half dropped by the call that owns it, a node
+        table of another size, a pod table refused for its lane count followed by a want half other than the one before
+        and a round (the pods' fit classes are built again from their base classes, not from the classes the filter
+        gave them), each failing node half, a dictionary that the want bits pass, preemption refused, the switch off."""
+        self.upload_nodes(300)
+        self.upload_groups(20)
+        self.upload_pods(150)
+        self.all_sides_but("hp")
+        self.weights(on=True)
+        self.switch(False)
+        self.hp_switch(True)
+        self.round()                 # BS_E_STATE: no halves
+        self.hp("node")
+        self.round()                 # BS_E_STATE: no pod half
+        self.hp("pod")
+        self.round()
+        self.update_nodes(str(self.rng.choice(["widen", "flags", "labels"])))
+        self.all_sides_but("hp")
+        self.round()                 # BS_E_STATE: the node half went with the update
+        self.hp("node")
+        self.round()
+        self.upload_pods(150)
+        self.all_sides_but("hp")
+        self.round()                 # BS_E_STATE: the pod half went with the pod table
+        self.hp("pod")
+        self.round()
+        self.upload_nodes(int(self.rng.choice([513, 700])))   # another Npad
+        self.all_sides()
+        self.round()
+        lanes = random_snapshot(self._k(), P=40, N=1, G=1, L=self.L + 1).pods
+        self.emit({"op": "upload_pods", "table": lanes})   # BS_E_INVAL: the pod table stays, its sides go
+        self.all_sides_but("hp")
+        self.round()                 # BS_E_STATE: the pod half went with the refused call
+        self.emit({"op": "hp", "half": "pod", "n": self.model.pods.n, "cols": np.zeros(self.model.pods.n, np.uint64)})
+        self.round()                 # no pod wants a port: every node passes the filter
+        self.hp("pod")
+        self.round()
+        for bad in ("port", "twice", "used", "many"):
+            self.hp("node", bad=bad)     # BS_E_RANGE, BS_E_INVAL, BS_E_INDEX, BS_E_INVAL
+        self.hp("node", wrong_len=True)  # BS_E_INVAL
+        self.round()                 # BS_E_STATE
+        self.hp("pod", wrong_len=True)
+        self.hp("node", n_entries=3)
+        self.round()                 # BS_E_STATE: the pod half failed
+        self.hp("pod")
+        self.round()                 # BS_E_INDEX: want bits past the 3 entries
+        self.hp("node")
+        self.round()
+        self.bound()
+        self.emit({"op": "preempt", "pods": np.arange(min(self.model.pods.n, 40), dtype=np.uint32)})   # BS_E_INVAL
+        self.preempt_walk(False)     # BS_E_INVAL
+        self.hp_switch(False)
+        self.round()
+        self.regimes.add("R10")
+
+    def r11(self):
+        """More than 4096 fit classes under the ports filter, and want halves that put every pod in a new conflict
+        class at each round until compact_fit_index rebuilds the fit index; the inter-pod switch toggled in between and
+        a group row update; then a small pod table.  The dictionary's entries have distinct ports, so each entry
+        conflicts with itself alone and a pod's conflict mask is its want mask."""
+        self.upload_nodes(64)
+        self.upload_groups(40)
+        pt = self.snap(R8_PODS, 1, 40).pods
+        pt.tol_mask = self.rng.integers(0, 1 << 62, pt.n).astype(np.uint64)   # a fit class per pod
+        self.emit({"op": "upload_pods", "table": pt})
+        self.all_sides_but("hp")
+        K = R11_ENTRIES
+        entries = np.array([(1 + k % 2, k % 2, 2000 + k) for k in range(K)], np.int64)
+        used = np.bitwise_or.reduce(self._bits(self.model.nodes.n, K, 0.04), axis=1)
+        self.emit({"op": "hp", "half": "node", "n": len(used), "cols": (entries, used)})
+        self.switch(True)
+        self.hp_switch(True)
+        for k in range(R11_ROUNDS):
+            want = np.bitwise_or.reduce(self._bits(pt.n, K, 0.06), axis=1)
+            self.emit({"op": "hp", "half": "pod", "n": pt.n, "cols": want})
+            if k % 3 == 1:
+                self.switch(not self.model.ipf_on)
+            if k == R11_ROUNDS // 2:
+                self.update_groups("rep")
+            self.round("evaluate" if k == 0 else None)
+        self.upload_pods(50)
+        self.all_sides()
+        self.round()
+        self.switch(False)
+        self.round()
+        self.regimes.add("R11")
+
+    def _bits(self, n, K, p):
+        """[n, K] uint64: bit k of column k with probability p."""
+        return np.where(self.rng.random((n, K)) < p, np.uint64(1) << np.arange(K, dtype=np.uint64), np.uint64(0))
+
+    def r12(self):
+        """Walks under the inter-pod filter, the ports filter and both: right after a new filter half and before any
+        round (the walk runs the filter's pre-pass for the next evaluation), after bs_update_nodes and the node halves
+        again; a refused pod upload drops the placed side, a placed term past the node half's dictionary, and with the
+        filter off the placed side is not read."""
+        self.upload_nodes(300)
+        self.upload_groups(20)
+        self.upload_pods(150)
+        self.all_sides()
+        self.weights(on=True)
+        self.walk_weights()
+        for on in ("ipf", "hp", "both"):
+            self.switch(on != "hp")
+            self.hp_switch(on != "ipf")
+            self.round()
+            if on != "hp":
+                self.ipf("node")
+            if on != "ipf":
+                self.hp("node")
+            for kind in ("first_fit", "priority"):
+                self.walk(kind)
+            self.round()
+            self.update_nodes(str(self.rng.choice(["widen", "flags", "labels"])))
+            self.node_sides()
+            for kind in ("first_fit", "priority"):
+                self.walk(kind)
+            self.round()
+        lanes = random_snapshot(self._k(), P=40, N=1, G=1, L=self.L + 1).pods
+        self.emit({"op": "upload_pods", "table": lanes})   # BS_E_INVAL: the placed side goes with the pod sides
+        self.all_sides_but("placed")
+        self.walk("first_fit")       # BS_E_INVAL: the filter is on without the placed side
+        self.placed()
+        self.walk("priority")
+        self.placed(bad="term")
+        self.walk("first_fit")       # BS_E_INDEX: a placed term past the node half's dictionary
+        self.placed(bad="class")     # BS_E_INDEX
+        self.placed(bad="own")       # BS_E_RANGE
+        self.placed(bad="term")
+        self.switch(False)
+        self.walk("priority")        # the placed side is not read
+        self.hp_switch(False)
+        self.walk("first_fit")
+        self.switch(True)
+        self.placed()
+        self.round()
+        self.regimes.add("R12")
+
     # -- random ops --
+    def ports_or_walk_op(self):
+        m = self.model
+        r = self.rng.random()
+        if r < 0.2:
+            self.hp_switch(not m.hp_on)
+            self.round()
+        elif r < 0.45:
+            if self.rng.random() < 0.3:
+                self.hp_seed = self._k()   # new halves: the pod half first, then the node half
+                self.hp("pod")
+                self.hp("node")
+            else:
+                half = str(self.rng.choice(["node", "pod"]))
+                bad = self.rng.choice([None, "port", "twice", "used", "many"]) if self.rng.random() < 0.15 else None
+                self.hp(half, wrong_len=self.rng.random() < 0.1, bad=bad,
+                        n_entries=3 if self.rng.random() < 0.1 else 12)
+            self.round()
+        elif r < 0.6:
+            bad = self.rng.choice([None, "class", "own", "term"]) if self.rng.random() < 0.2 else None
+            self.placed(wrong_len=self.rng.random() < 0.1, bad=bad)
+            self.walk(str(self.rng.choice(["first_fit", "priority"])))
+        else:
+            on = str(self.rng.choice(["ipf", "hp", "both"]))
+            self.switch(on != "hp")
+            self.hp_switch(on != "ipf")
+            if m.ipf_placed is None and self.rng.random() < 0.8:
+                self.placed()
+            if self.rng.random() < 0.5:
+                self.walk_weights()
+            self.walk(str(self.rng.choice(["first_fit", "priority"])))
+
     def filter_or_preempt_op(self):
         m = self.model
         r = self.rng.random()
@@ -974,17 +1331,19 @@ class Generator:
         r = self.rng.random()
         if m.nodes is None or m.pods is None or m.groups is None:
             self.base()
-        elif r < 0.12:
+        elif r < 0.10:
             self.filter_or_preempt_op()
-        elif r < 0.20:   # without its affinity table now and then: the pods' classes are BS_E_INDEX until it comes
+        elif r < 0.17:
+            self.ports_or_walk_op()
+        elif r < 0.23:   # without its affinity table now and then: the pods' classes are BS_E_INDEX until it comes
             self.upload_nodes(int(self.rng.choice([1, 33, 511, 512, 513, 900])), aff=AFF if self.rng.random() < 0.85 else 0)
             self.all_sides(("node",))
-        elif r < 0.27:
+        elif r < 0.29:
             self.upload_pods(int(self.rng.choice([0, 1, 70, self.max_p + 13])), aff=AFF if self.rng.random() < 0.8 else 0)
             self.all_sides(("pod",))
-        elif r < 0.30:
+        elif r < 0.32:
             self.upload_groups(int(self.rng.choice([0, 1, 9, 31])), aff=AFF if self.rng.random() < 0.8 else 0)
-        elif r < 0.41 and m.nodes.n:
+        elif r < 0.42 and m.nodes.n:
             self.update_nodes(str(self.rng.choice(["widen", "back", "flags", "labels"])))
             if self.rng.random() < 0.85:   # else the next rounds answer BS_E_STATE until a side op brings them back
                 self.node_sides()
@@ -1023,15 +1382,17 @@ class Generator:
             self.round()
 
 
-BURSTS = ("r1", "r2", "r3", "r4", "r5", "r6", "r7", "r8", "r9")
+BURSTS = ("r1", "r2", "r3", "r4", "r5", "r6", "r7", "r8", "r9", "r10", "r11", "r12")
 R8_PODS, R8_ROUNDS, R8_SPREAD = 4200, 9, 64
+R11_ENTRIES, R11_ROUNDS = 40, 10
 
 
 def generate(seed, n_ops=30, lanes=None):
-    """(ops, regimes): about n_ops random ops around one scripted burst (seed % 9 picks it; seeds >= 6 add another),
-    every op as the dict Model.apply takes; regimes names the bursts the sequence ran."""
+    """(ops, regimes): about n_ops random ops around one scripted burst (seed % len(BURSTS) picks it; seeds >= 6 add
+    another), every op as the dict Model.apply takes; regimes names the bursts the sequence ran."""
     g = Generator(seed, lanes or [5, 6, 9][seed % 3])
-    bursts = [BURSTS[seed % 9]] + ([BURSTS[(seed + 4) % 9]] if seed >= 6 else [])
+    n = len(BURSTS)
+    bursts = [BURSTS[seed % n]] + ([BURSTS[(seed + 4) % n]] if seed >= 6 else [])
     at = sorted(int(x) for x in g.rng.integers(0, n_ops, len(bursts)))
     g.base()
     for i in range(n_ops):

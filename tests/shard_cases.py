@@ -3,10 +3,10 @@
 Snapshot.shard_groups cuts the three tables: the node and group tables are replicated, the pods of the rank's group
 range (and the ungrouped pods with index % world == rank) stay, in table order, at local.meta["pod_index"].  shard()
 cuts the side columns the same way: every pod half (the non-zero [2][P] column, the preference, locality, spread and
-inter-pod pod classes, the MatchInterPodAffinity filter's pod classes) is sliced by pod, every node half and every
-class table is replicated as it is.  A case is an engine_model.Model holding the whole state with every side column,
-all six priority weights and the filter on, so that Model.expect gives every output of a round on the whole snapshot
-and on a shard alike.
+inter-pod pod classes, the MatchInterPodAffinity filter's pod classes, the PodFitsHostPorts filter's want masks) is
+sliced by pod, every node half and every class table is replicated as it is.  A case is an engine_model.Model holding
+the whole state with every side column, all six priority weights and both filters on, so that Model.expect gives every
+output of a round on the whole snapshot and on a shard alike.
 
 The cases (each one's rounds move admits and max_group through identical group row updates, group_updates):
   unbalanced    three groups hold three quarters of the pods;
@@ -25,6 +25,7 @@ from __future__ import annotations
 import numpy as np
 
 import engine_model as em
+import host_ports_ref as hr
 from randsnap import S, random_snapshot
 
 L = 6
@@ -33,7 +34,7 @@ ROUNDS = 3          # the loaded state, then two group row updates
 CASES = ("unbalanced", "ungrouped", "empty_shard", "many_groups", "many_groups3", "tail", "idle")
 WORLDS = (2, 3, 4)
 PER_POD = ("prefilter", "feasible_count", "best_node", "best_score", "fit_rows", "score_rows", "filter_rows",
-           "filter_code", "reason_rows", "interpod_rows", "topk_nodes", "topk_scores", "priority_nodes",
+           "filter_code", "reason_rows", "interpod_rows", "host_port_rows", "topk_nodes", "topk_scores", "priority_nodes",
            "priority_scores")
 
 
@@ -70,7 +71,7 @@ def _gids(name, rng):
 
 def case(name, seed=None) -> em.Model:
     """The whole state of case `name`: its tables (groups resolved), every side column, all six priority weights and
-    the MatchInterPodAffinity filter on."""
+    both filters on."""
     seed = CASES.index(name) + 11 if seed is None else seed
     rng = np.random.default_rng(seed)
     P, N, G, gid = _gids(name, rng)
@@ -93,6 +94,8 @@ def case(name, seed=None) -> em.Model:
     m.ratio = (em.RATIO_ON[0], em.RATIO_ON[1], [1, 1, 0, 0] + [1] * (L - 4), em.RATIO_ON[3])
     m.pw, m.lw, m.w_spread, m.w_ipa = em.PW, em.LW, em.W_SPREAD, em.W_IPA
     m.ipf_on = m.ipf_round = True
+    m.hp_node, m.hp_pod = hr.random_columns(snap, k + 6)
+    m.hp_on = m.hp_round = True
     return m
 
 
@@ -113,10 +116,11 @@ def shard(m: em.Model, rank: int, world: int):
     local = m.snapshot().shard_groups(rank, world)
     idx = local.meta["pod_index"]
     s = em.Model(m.lanes)
-    s.__dict__.update({k: v for k, v in m.__dict__.items() if k not in ("side", "pods", "ipf_pod")})
+    s.__dict__.update({k: v for k, v in m.__dict__.items() if k not in ("side", "pods", "ipf_pod", "hp_pod")})
     s.pods = local.pods
     s.side = {k: (v if k.endswith("_node") else _pod_half(k.split("_")[0], v, idx)) for k, v in m.side.items()}
     s.ipf_pod = _pod_half("ipf", m.ipf_pod, idx)
+    s.hp_pod = np.ascontiguousarray(m.hp_pod[idx])
     return s, idx, local.meta["group_range"]
 
 

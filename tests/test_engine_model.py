@@ -1,16 +1,24 @@
 """CPU: the host model of a long-lived engine (tests/engine_model.py) and its op generator, without a device: row
 updates through the model equal the tables built directly, the generator is deterministic and reaches every scripted
 regime across the seeds the GPU test runs, and the model's expected outputs come from the restatements on a short
-sequence (which keeps the reference side honest and bounds its cost).  The MatchInterPodAffinity filter's drop rules,
-check order and refusals, the preemption walk's list rules, and the invariants of a round under the filter are pinned
-on hand-built op lists."""
+sequence (which keeps the reference side honest and bounds its cost).  The drop rules, check orders and refusals of
+the MatchInterPodAffinity filter, its placed side and the PodFitsHostPorts filter, the preemption walk's list rules,
+and the invariants of a round under the filter are pinned on hand-built op lists; the walk references the model picks
+agree with each other wherever more than one applies."""
+import functools
+import operator
+
 import numpy as np
 
 import engine_model as em
+import host_ports_ref as hr
 import interpod_filter_ref as fr
+import interpod_walk_ref as iwr
+import locality_priority_ref as lpr
+from oracle import oracle
 from randsnap import S, random_snapshot
 
-SEEDS = range(9)   # the GPU test's seeds
+SEEDS = range(len(em.BURSTS))   # the GPU test's seeds
 
 
 def _same(a, b):
@@ -91,18 +99,21 @@ def test_generator_is_deterministic_and_reaches_every_regime():
         seen |= regimes
         kinds = {o["op"] for o in ops}
         assert {"upload_nodes", "upload_pods", "upload_groups", "side", "weights", "evaluate"} <= kinds
-    assert seen == {f"R{k}" for k in range(1, 10)}
+    assert seen == {f"R{k}" for k in range(1, len(em.BURSTS) + 1)}
+    assert {em.BURSTS[s % len(em.BURSTS)] for s in SEEDS} == set(em.BURSTS)   # each burst runs first in some seed
 
 
 def test_sequences_reach_the_edges():
     """Across the seeds: N, P and G of 0, node counts on both sides of the 512-node tile, the class indices past
     4096, every side refused once (wrong length), every error the model predicts, and a round after each."""
-    codes, sizes, P_max = set(), set(), 0
+    codes, sizes, P_max, by_op = set(), set(), 0, {}
     for seed in SEEDS:
         ops, _, L = em.generate(seed)
         m = em.Model(L)
         for op in ops:
-            codes.add(m.apply(op))
+            rc = m.apply(op)
+            codes.add(rc)
+            by_op.setdefault(op["op"], set()).add(rc)
             if op["op"] == "upload_nodes":
                 sizes.add(op["table"].n)
             if op["op"] == "upload_pods":
@@ -111,6 +122,11 @@ def test_sequences_reach_the_edges():
             if op["op"] == "upload_groups":
                 sizes.add(("G", op["table"].n))
     assert {None, em.E_STATE, em.E_RANGE, em.E_INDEX, em.E_INVAL} <= codes
+    # every refusal of the ports filter's node half and of the placed side, and the walks' own ones
+    assert {None, em.E_INVAL, em.E_RANGE, em.E_INDEX} <= by_op["hp"], by_op["hp"]
+    assert {None, em.E_INDEX, em.E_RANGE} <= by_op["placed"], by_op["placed"]
+    assert {None, em.E_INVAL, em.E_INDEX} <= by_op["replay"], by_op["replay"]
+    assert {None, em.E_STATE, em.E_INDEX} <= by_op["evaluate"]
     assert {0, 1, 511, 512, 513, ("P", 0), ("G", 0)} <= sizes
     assert P_max >= 4097
 
@@ -386,3 +402,262 @@ def test_expect_under_the_filter():
         fit_on = np.unpackbits(on["fit_rows"].view(np.uint8), axis=1, bitorder="little")[:, :N].astype(bool)
         np.testing.assert_array_equal(fit_on, fit & (v == fr.PASS))
         assert (on["priority_nodes"] >= 0).sum(1).tolist() == np.minimum(8, on["feasible_count"]).tolist()
+
+
+def _hp_half(snap, h, cols, n=None):
+    return {"op": "hp", "half": h, "cols": cols, "n": (snap.nodes.n if h == "node" else snap.pods.n) if n is None else n}
+
+
+def test_host_port_drop_rules_and_check_order():
+    m, snap, node, pods = _loaded()
+    N, P = snap.nodes.n, snap.pods.n
+    (entries, used), want = hr.random_columns(snap, 4)
+    assert want.any()
+    ev = {"op": "evaluate", "priority": True}
+    nz_node = {"op": "side", "name": "nz", "half": "node", "n": N, "cols": S.nonzero_requests(snap, 1)[0]}
+    nz_pod = {"op": "side", "name": "nz", "half": "pod", "n": P, "cols": S.nonzero_requests(snap, 1)[1]}
+    assert m.apply({"op": "hp_switch", "on": True}) is None
+    assert m.apply(ev) == em.E_STATE                       # no halves
+    assert m.apply(_hp_half(snap, "node", (entries, used))) is None
+    assert m.apply(ev) == em.E_STATE                       # no pod half
+    assert m.apply(_hp_half(snap, "pod", want)) is None
+    assert m.apply(ev) is None and m.hp_round and not m.ipf_round
+    # bs_update_nodes drops the node half, also a call that changes no row or fails
+    for idx, rows in ((np.zeros(0, np.uint32), snap.nodes.take(np.zeros(0, np.int64))),
+                      (np.array([N], np.uint32), snap.nodes.take([0])), (np.array([1], np.uint32), snap.nodes.take([1]))):
+        m.apply({"op": "update_nodes", "idx": idx, "rows": rows})
+        assert m.hp_node is None and m.hp_pod is not None
+        assert m.apply(nz_node) is None
+        assert m.apply(ev) == em.E_STATE
+        assert m.apply(_hp_half(snap, "node", (entries, used))) is None
+        assert m.apply(ev) is None
+    # bs_upload_nodes drops it, also one that fails validation
+    bad = snap.nodes.copy()
+    bad.alloc[0, 0] = em.LIMIT + 1
+    assert m.apply({"op": "upload_nodes", "table": bad}) == em.E_RANGE and m.hp_node is None
+    assert m.apply(_hp_half(snap, "node", (entries, used))) == em.E_STATE   # without its table
+    for op in ({"op": "upload_nodes", "table": snap.nodes}, {"op": "upload_affinity", "bits": snap.aff_bits}, nz_node,
+               {"op": "ipf", "half": "node", "n": N, "cols": node}):
+        assert m.apply(op) is None
+    assert m.hp_node is None and m.apply(ev) == em.E_STATE
+    # each failing node half leaves it dropped: a wrong length, more than 64 entries, a port outside 1..65535 (before
+    # an entry listed twice), an entry listed twice (before a used bit past the entries), a used bit past the entries
+    K = len(entries)
+    twice = np.r_[entries[:-1], entries[:1]]
+    zero_port = twice.copy()
+    zero_port[0, 2] = 0
+    past = used.copy()
+    past[3] |= np.uint64(1) << np.uint64(K)
+    many = np.array([(1, 0, 1000 + k) for k in range(65)], np.int64)
+    for cols, n, rc in (((entries, used[:-1]), N - 1, em.E_INVAL), ((many, np.zeros(N, np.uint64)), N, em.E_INVAL),
+                        ((zero_port, past), N, em.E_RANGE), ((twice, past), N, em.E_INVAL),
+                        ((entries, past), N, em.E_INDEX)):
+        assert m.apply(_hp_half(snap, "node", (entries, used))) is None
+        assert m.apply(_hp_half(snap, "node", cols, n)) == rc and m.hp_node is None
+    assert m.apply(_hp_half(snap, "node", (many[:64], np.zeros(N, np.uint64)))) is None   # 64 entries: every bit
+    assert m.apply(ev) is None
+    assert m.apply(_hp_half(snap, "node", (entries, used))) is None
+    # bs_upload_pods drops the pod half and the placed side, also a call refused for its lane count (which keeps the
+    # pod table and the node half)
+    placed = S.node_interpod_walk(snap, 3)[2]
+    assert m.apply({"op": "placed", "n": P, "cols": placed}) is None
+    other = random_snapshot(5, P=7, N=1, G=1, L=6).pods
+    assert m.apply({"op": "upload_pods", "table": other}) == em.E_INVAL
+    assert m.pods is snap.pods and m.hp_pod is None and m.ipf_placed is None and m.hp_node is not None
+    assert m.apply(nz_pod) is None
+    assert m.apply(ev) == em.E_STATE
+    assert m.apply(_hp_half(snap, "pod", want[:-1], P - 1)) == em.E_INVAL and m.hp_pod is None
+    assert m.apply(_hp_half(snap, "pod", want)) is None
+    assert m.apply(ev) is None
+    # bs_evaluate: the priority sides, then the inter-pod filter, then the ports filter, then the affinity ids
+    small = (entries[:1], used & np.uint64(1))     # the pods want entries past this dictionary
+    assert m.apply(_hp_half(snap, "node", small)) is None
+    assert m.apply(ev) == em.E_INDEX
+    assert m.apply({"op": "weights", "w_spread": 1}) is None
+    assert m.apply(ev) == em.E_STATE                       # the spread sides come first
+    assert m.apply({"op": "weights", "w_spread": 0}) is None
+    assert m.apply({"op": "ipf_switch", "on": True}) is None
+    assert m.apply({"op": "ipf", "half": "pod", "n": P, "cols": (np.r_[pods[0][:-1], 0], pods[1])}) is None
+    assert m.apply({"op": "ipf", "half": "node", "n": N + 1, "cols": node}) == em.E_INVAL
+    assert m.apply(ev) == em.E_STATE                       # the inter-pod filter's half before the ports' dictionary
+    assert m.apply({"op": "ipf", "half": "node", "n": N, "cols": node}) is None
+    assert m.apply(ev) == em.E_INDEX
+    assert m.apply({"op": "ipf_switch", "on": False}) is None
+    assert m.apply({"op": "upload_affinity", "bits": None}) is None
+    assert m.apply(_hp_half(snap, "pod", want[:-1], P - 1)) == em.E_INVAL
+    assert m.apply(ev) == em.E_STATE                       # the ports filter before the affinity ids
+    assert m.apply(_hp_half(snap, "pod", np.zeros(P, np.uint64))) is None
+    assert m.apply(ev) == em.E_INDEX                       # now the affinity ids
+    assert m.apply({"op": "upload_affinity", "bits": snap.aff_bits}) is None
+    assert m.apply(ev) is None
+    # preemption and the preemption walk are refused with the switch on, before the bound table is looked at
+    for op in ({"op": "preempt", "pods": np.arange(5, dtype=np.uint32)},
+               {"op": "preempt_walk", "pods": np.zeros(2, np.uint32), "gang": False}):
+        assert m.apply(op) == em.E_INVAL
+    assert m.apply({"op": "hp_switch", "on": False}) is None
+    assert m.apply(ev) is None and not m.hp_round
+    assert m.apply({"op": "preempt", "pods": np.arange(5, dtype=np.uint32)}) == em.E_STATE
+
+
+def test_walk_refusals_under_the_filters():
+    """bs_replay / bs_replay_priority with the filters: the inter-pod filter without the placed side first, then the
+    priority weights, the tables, the non-zero columns, locality, the ports filter, the inter-pod filter, a placed
+    term past the filter's dictionary; the placed side's own refusals; with the filter off it is not read."""
+    m, snap, node, pods = _loaded()
+    N, P = snap.nodes.n, snap.pods.n
+    ff, pr = {"op": "replay", "priority": False}, {"op": "replay", "priority": True}
+    placed = S.node_interpod_walk(snap, 3)[2]
+    pcls, (off, term, own, match) = placed
+    T = len(node[2])
+    far = (pcls, (off, np.where(np.arange(len(term)) == 0, T, term).astype(np.uint32), own, match))
+    pl = lambda cols, n=P: {"op": "placed", "n": n, "cols": cols}
+    assert m.apply(ff) is None and m.apply(pr) is None
+    assert m.apply({"op": "ipf_switch", "on": True}) is None
+    assert m.apply({"op": "hp_switch", "on": True}) is None
+    assert m.apply(ff) == em.E_INVAL                        # no placed side, before the ports filter's E_STATE
+    assert m.apply({"op": "weights", "w_spread": 1}) is None
+    assert m.apply(pr) == em.E_INVAL
+    # the placed side's refusals: its table, its length, a class out of range, an own outside {0, 1}
+    assert m.apply(pl(placed, P + 1)) == em.E_INVAL and m.ipf_placed is None
+    assert m.apply(pl((np.full(P, len(off) - 1, np.uint32), placed[1]))) == em.E_INDEX
+    bad_own = (pcls, (off, term, np.where(np.arange(len(own)) == 0, 2, own).astype(np.int32), match))
+    assert len(own) and m.apply(pl(bad_own)) == em.E_RANGE and m.ipf_placed is None
+    assert m.apply(pl(far)) is None                          # a term past the dictionary is checked by the walk
+    assert m.apply(pr) == em.E_INVAL                         # bs_replay_priority's weights next
+    assert m.apply({"op": "weights", "w_spread": 0}) is None
+    assert m.apply(pr) == em.E_STATE and m.apply(ff) == em.E_STATE   # the ports filter's halves before the placed term
+    (entries, used), want = hr.random_columns(snap, 4)
+    assert m.apply(_hp_half(snap, "node", (entries[:1], used & np.uint64(1)))) is None
+    assert m.apply(_hp_half(snap, "pod", want)) is None
+    assert m.apply(ff) == em.E_INDEX                         # want bits past the dictionary
+    assert m.apply({"op": "weights", "lw": (1, 0)}) is None
+    assert m.apply(pr) == em.E_STATE                         # locality before the ports filter
+    assert m.apply({"op": "weights", "lw": (0, 0)}) is None
+    assert m.apply(_hp_half(snap, "node", (entries, used))) is None
+    assert m.apply({"op": "ipf", "half": "pod", "n": P, "cols": (pods[0], (pods[1][0], np.full_like(pods[1][1], T),
+                                                                          *pods[1][2:]))}) is None
+    assert m.apply(ff) == em.E_INDEX                         # the pods' filter terms
+    assert m.apply({"op": "ipf", "half": "pod", "n": P, "cols": pods}) is None
+    assert m.apply(ff) == em.E_INDEX and m.apply(pr) == em.E_INDEX   # now the placed term
+    assert m.apply({"op": "ipf_switch", "on": False}) is None
+    assert m.apply(ff) is None and m.apply(pr) is None       # the placed side is not read
+    assert m.apply({"op": "upload_pods", "table": snap.pods}) is None and m.ipf_placed is None
+    assert m.apply({"op": "ipf_switch", "on": True}) is None
+    assert m.apply(ff) == em.E_INVAL
+
+
+def _conflicts(entries):
+    """Each entry's conflict mask (engine.cu bs_upload_node_host_ports)."""
+    ent = np.asarray(entries, np.int64).reshape(-1, 3)
+    out = []
+    for a in ent:
+        same = (ent[:, 1] == a[1]) & (ent[:, 2] == a[2]) & ((ent[:, 0] == 0) | (a[0] == 0) | (ent[:, 0] == a[0]))
+        out.append(sum(1 << int(b) for b in np.flatnonzero(same)))
+    return out
+
+
+def _fit_index_grows(seed):
+    """(rounds that certainly compacted the fit class index with the ports filter on, ops, Model): a round is certain
+    to compact once the (base class, filter class, conflict mask) keys assigned since the last pod table outnumber
+    max(4096, 4 x 2P), as test_filter_rounds_follow_every_change reasons."""
+    ops, _, L = em.generate(seed)
+    m = em.Model(L)
+    keys, hits = set(), []
+    for i, op in enumerate(ops):
+        rc = m.apply(op)
+        if op["op"] == "upload_pods" and rc is None:
+            keys = set()
+        if op["op"] == "evaluate" and rc is None and (m.ipf_on or m.hp_on):
+            ipf = m.ipf_pod[0].tolist() if m.ipf_on else [S.IPF_NONE] * m.pods.n
+            conf = [0] * m.pods.n
+            if m.hp_on:
+                c = _conflicts(m.hp_node[0])
+                conf = [functools.reduce(operator.or_, (c[b] for b in range(len(c)) if (int(w) >> b) & 1), 0)
+                        for w in m.hp_pod]
+            keys |= set(zip(_fit_keys(m.pods), ipf, conf))
+            if len(keys) > max(4096, 8 * m.pods.n):
+                hits.append(i)
+                keys = set()
+    return hits, ops, m
+
+
+def test_r11_compacts_the_fit_index_under_the_ports_filter():
+    seed = next(s for s in SEEDS if em.BURSTS[s % len(em.BURSTS)] == "r11")
+    hits, ops, _ = _fit_index_grows(seed)
+    assert hits, "R11 never outgrew the fit index"
+    assert any(ops[i]["op"] == "evaluate" for i in hits)
+    last_pods = max(i for i, op in enumerate(ops) if op["op"] == "upload_pods" and op["table"].n == 50)
+    assert hits[0] < last_pods     # ... and then the small pod table
+
+
+def test_r10_wants_again_after_a_refused_pod_table():
+    """R10: a pod table refused for its lane count while the ports filter is on (after a round that gave the pods
+    their conflict classes), then a want half other than the one before, then a successful round that changes what
+    passes: the engine must build the classes from the base classes, not from the ones the filter gave them."""
+    seed = next(s for s in SEEDS if em.BURSTS[s % len(em.BURSTS)] == "r10")
+    ops, _, L = em.generate(seed)
+    m = em.Model(L)
+    found = False
+    refused, want_before, want_after = None, None, None
+    for op in ops:
+        rc = m.apply(op)
+        if op["op"] == "upload_pods":
+            refused = m.hp_round and m.hp_on and rc == em.E_INVAL
+            want_after = None
+        elif op["op"] == "hp" and op["half"] == "pod" and rc is None:
+            if refused and want_after is None:
+                want_after = op["cols"]
+            else:
+                want_before = op["cols"]
+        elif op["op"] == "evaluate" and rc is None and refused and want_after is not None and m.hp_on:
+            found = found or not np.array_equal(want_after, want_before)
+            refused = False
+    assert found
+
+
+def test_r12_walks_right_after_a_filter_half():
+    """Across the seeds: successful filtered walks (first fit and priority) right after a filter half and before any
+    round, under the inter-pod filter, the ports filter and both, and walks with the placed side refused."""
+    reached = set()
+    for seed in SEEDS:
+        ops, _, L = em.generate(seed)
+        m = em.Model(L)
+        fresh = False
+        for op in ops:
+            rc = m.apply(op)
+            if op["op"] in ("ipf", "hp") and rc is None:
+                fresh = True
+            elif op["op"] == "evaluate":
+                fresh = False
+            elif op["op"] == "replay" and rc is None and fresh and (m.ipf_on or m.hp_on):
+                on = "both" if m.ipf_on and m.hp_on else ("ipf" if m.ipf_on else "hp")
+                reached.add((on, "priority" if op["priority"] else "first_fit"))
+    assert reached == {(on, k) for on in ("ipf", "hp", "both") for k in ("first_fit", "priority")}, reached
+
+
+def test_walk_references_agree():
+    """The model's walk references where two apply: interpod_walk_ref.replay with a filter without terms equals
+    host_ports_ref.replay with the ports filter on, and the oracle's walk and locality_priority_ref.replay_locality
+    with it off."""
+    for seed, L in ((41, 5), (42, 6), (43, 9)):
+        snap = random_snapshot(seed, P=90, N=120, G=14, L=L, aff=2)
+        cols, placed = em.no_interpod_filter(snap.nodes.n, snap.pods.n)
+        hp = hr.random_columns(snap, seed, node_bits=3, grouped=0.6)
+        nz = S.nonzero_requests(snap, seed)
+        for chooser in (None, nz):
+            got = iwr.replay(snap, cols, placed, None, chooser, (1, 0, 1), None, None, (0, 0), hp)
+            want = hr.replay(snap, hp, None, chooser, (1, 0, 1))
+            for a, b in zip(got[:3], want[:3]):
+                np.testing.assert_array_equal(a, b)
+            np.testing.assert_array_equal(got[5], want[4])      # the live used masks
+        assert (got[1] >= 0).any() and (hr.passes(*hp[0], hp[1]) == 0).any()
+        got = iwr.replay(snap, cols, placed)
+        want = oracle.replay(snap)
+        for a, b in zip(got[:3], want[:3]):
+            np.testing.assert_array_equal(a, b)
+        loc = S.node_locality(snap, seed)
+        ratio = (2, em.RATIO_ON[1], [1, 1, 0, 0] + [1] * (L - 4), 1)
+        got = iwr.replay(snap, cols, placed, None, nz, (1, 0, 1), ratio, loc, em.LW)
+        want = lpr.replay_locality(snap, nz[0], nz[1], loc, em.LW, ratio, None, (1, 0, 1))
+        for a, b in zip(got[:3], want[:3]):
+            np.testing.assert_array_equal(a, b)

@@ -1,6 +1,6 @@
 """GPU: one long-lived engine through seeded sequences of uploads, row updates, affinity tables, side columns, weights,
-the MatchInterPodAffinity filter's switch and halves, failing calls, rounds, walks, preemption with
-PodDisruptionBudget bits and the preemption walk (tests/engine_model.py), with every output on.  After each op the engine
+the MatchInterPodAffinity filter's switch, halves and placed side, the PodFitsHostPorts filter's switch and halves,
+failing calls, rounds, walks with either filter or both, preemption with PodDisruptionBudget bits and the preemption walk (tests/engine_model.py), with every output on.  After each op the engine
 answers the error code the host model predicts, and every round, walk and preemption is bit-exact against the CPU
 restatements on the model's state.  A mismatch reports the seed, the step, the ops up to it, the first differing
 output and whether a fresh engine loaded with the model's state agrees (stale engine state) or not (a kernel)."""
@@ -80,6 +80,7 @@ def _round(eng, cfg, how):
     if cfg.get("reasons"):
         out["reason_rows"] = eng.reason_rows()
         out["interpod_rows"] = eng.fetch_interpod_reason_rows()
+        out["host_port_rows"] = eng.fetch_host_port_reason_rows()
     if cfg.get("priority_k"):
         out["priority_nodes"], out["priority_scores"] = eng.priority_rows()
     out["lanes"] = eng.fit_lanes()
@@ -110,6 +111,12 @@ def _call(pkg, eng, L, op, cfg):
             eng.upload_interpod_filter(**{"node" if op["half"] == "node" else "pods": op["cols"]})
         elif k == "ipf_switch":
             eng.set_interpod_filter(op["on"])
+        elif k == "placed":
+            eng.upload_interpod_placed(*op["cols"])
+        elif k == "hp":
+            eng.upload_host_ports(**{"node" if op["half"] == "node" else "pods": op["cols"]})
+        elif k == "hp_switch":
+            eng.set_host_port_filter(op["on"])
         elif k == "weights":
             _weights(eng, L, op)
         elif k == "evaluate":
@@ -159,8 +166,8 @@ def _expect(model, op, cfg):
 
 
 def _fresh_agrees(pkg, model, cfg, L, op):
-    """A fresh engine loaded with the model's state (tables, sides, weights, the filter's halves and switch, the
-    bound table): does `op` (a round, walk or preemption; else a round) on it equal the references?"""
+    """A fresh engine loaded with the model's state (tables, sides, weights, both filters' halves and switches, the
+    placed side, the bound table): does `op` (a round, walk or preemption; else a round) on it equal the references?"""
     eng = _engine(pkg, L, cfg)
     try:
         eng.upload_nodes(model.nodes)
@@ -172,10 +179,14 @@ def _fresh_agrees(pkg, model, cfg, L, op):
             if cols is not None:
                 name, half = key.split("_")
                 _side(eng, {"name": name, "half": half, "cols": cols})
-        for half in ("node", "pod"):
-            if getattr(model, "ipf_" + half) is not None:
-                _call(pkg, eng, L, {"op": "ipf", "half": half, "cols": getattr(model, "ipf_" + half)}, cfg)
+        for kind in ("ipf", "hp"):
+            for half in ("node", "pod"):
+                if getattr(model, kind + "_" + half) is not None:
+                    _call(pkg, eng, L, {"op": kind, "half": half, "cols": getattr(model, kind + "_" + half)}, cfg)
+        if model.ipf_placed is not None:
+            eng.upload_interpod_placed(*model.ipf_placed)
         eng.set_interpod_filter(model.ipf_on)
+        eng.set_host_port_filter(model.hp_on)
         if model.bound is not None:
             eng.upload_bound_pods(model.bound)
         _weights(eng, L, dict(weights=model.weights, ratio=model.ratio, pw=model.pw, lw=model.lw,
@@ -222,6 +233,6 @@ def _run_seed(pkg, cfg, seed):
 
 
 @pytest.mark.parametrize("config", sorted(CONFIGS))
-@pytest.mark.parametrize("seed", range(9))
+@pytest.mark.parametrize("seed", range(len(em.BURSTS)))
 def test_engine_sequences(pkg, oracle, config, seed):
     _run_seed(pkg, CONFIGS[config], seed)

@@ -1,7 +1,7 @@
 """GPU, 2-4 ranks: the group-sharded round on every rank with peers attached, against the unsharded references.
 
 Each rank loads its shard of every case of tests/shard_cases.py (tables and side columns, all six priority weights and
-the MatchInterPodAffinity filter on) into both engine configurations of test_gpu_engine_sequences.CONFIGS, attaches the
+both filters on) into both engine configurations of test_gpu_engine_sequences.CONFIGS, attaches the
 peer exchange, and runs shard_cases.ROUNDS rounds with the same group row updates in between.  After each round every
 rank checks its own outputs bit-exact against the whole snapshot's references restricted to its shard
 (shard_cases.first_diff: the CPU test pins that decomposition), and the gathered bitmap: every rank's bits in its own
@@ -72,7 +72,7 @@ def _engine(pkg, dev, cfg):
 
 
 def _load(eng, m):
-    """Every table, side column, filter half and weight of the Model m."""
+    """Every table, side column, both filters' halves and switches, and every weight of the Model m."""
     import test_gpu_engine_sequences as seq
     eng.upload_nodes(m.nodes)
     eng.upload_affinity(m.aff)
@@ -84,6 +84,8 @@ def _load(eng, m):
     eng.upload_interpod_filter(node=m.ipf_node)
     eng.upload_interpod_filter(pods=m.ipf_pod)
     eng.set_interpod_filter(m.ipf_on)
+    eng.upload_host_ports(node=m.hp_node, pods=m.hp_pod)
+    eng.set_host_port_filter(m.hp_on)
     seq._weights(eng, m.lanes, dict(weights=m.weights, ratio=m.ratio, pw=m.pw, lw=m.lw, w_spread=m.w_spread,
                                     w_ipa=m.w_ipa))
 
@@ -256,9 +258,9 @@ def _h1_worker(rank, world, port, data_path, out_dir, shared_gpu):
 
 
 def _plain_tail():
-    """Case tail with the filter off: these engines load the tables only."""
+    """Case tail with the filters off: these engines load the tables only."""
     m = sc.case("tail")
-    m.ipf_on = m.ipf_round = False
+    m.ipf_on = m.ipf_round = m.hp_on = m.hp_round = False
     return m
 
 

@@ -3,7 +3,7 @@
 For every case of tests/shard_cases.py, every world size of 2, 3 and 4 and every rank, each round's references on the
 rank's shard (tables and side columns cut by shard_cases.shard) equal the references on the whole snapshot restricted
 to the shard: every per-pod row (PreFilter, the feasible count, best node and score, the fit, score and Filter rows, the
-reason and companion rows, top-K and the priority lists with every weight and the MatchInterPodAffinity filter on),
+reason and both filters' companion rows, top-K and the priority lists with every weight and both filters on),
 admit and new_denied of the rank's own group range and of the groups no rank holds pods of, max_group and max_finished
 on every rank, and the queue order as the whole order filtered to the shard.  The rounds in between apply the same
 group row updates on every rank, and the cases are checked to do what their names say."""
