@@ -1,12 +1,12 @@
 """Builds the C-ABI shared library in-tree: nvcc, sm_90a (H100) only.
 
 Translation units (compiled in parallel, then linked into libbsched.so):
-  engine.cu            the C ABI, host sequencing and every kernel but the dominant one
+  engine.cu            the C ABI, host sequencing and every kernel the units below do not hold
   plugin.cpp           the C++ host mirror of the reference plugin + snapshot packer
-  priority_inst.cu     the priority lists' kernels (csrc/priority.cuh): priority_pod_kernel without SPREAD or IPA, LOC and IPA pre-passes
-  priority_spread_inst.cu x 3   priority_pod_kernel's SPREAD variants, one unit per -DBS_PRIO_SPREAD_MAXL=5, 9, 16
-  priority_interpod_inst.cu x 3 priority_pod_kernel's IPA variants, one unit per -DBS_PRIO_IPA_MAXL=5, 9, 16
-  replay_ipf_inst.cu x 3        replay_kernel's MatchInterPodAffinity builds, one unit per -DBS_REPLAY_IPF_MAXL=5, 9, 16
+  priority_inst.cu x 6 the 96 priority_pod_kernel builds (csrc/priority.cuh), one slice per -DBS_PRIO_SLICE=k: lane
+                       bound 5, 9, 16 by k / 2, IPA off or on by k % 2; slice 0 also the LOC and IPA pre-passes
+  replay_inst.cu x 6   the 60 replay_kernel builds (csrc/replay.cuh), one slice per -DBS_REPLAY_SLICE=k: lane bound
+                       5, 9, 16 by k / 2, IPF off or on by k % 2
   fit_inst.cu x 9      the gang_fit_kernel variant table, one slice per -DBS_FIT_SLICE=n (csrc/fit.cuh)
 
     python -m importlib ...  # not importable by dotted name (hyphen); use __graft_entry__.build()
@@ -26,6 +26,8 @@ HEADERS = ["devmem.hpp", "common.cuh", "kernels.cuh", "fit.cuh", "sort.cuh", "re
            "plugin.hpp",
            os.path.join("..", "..", "include", "bsched.h")]
 FIT_SLICES = 9
+PRIO_SLICES = 6
+REPLAY_SLICES = 6
 
 
 def nvcc_path() -> str:
@@ -37,11 +39,11 @@ def nvcc_path() -> str:
 
 def _units():
     """(source, object, extra flags) of every translation unit."""
-    u = [("engine.cu", "engine.o", []), ("plugin.cpp", "plugin.o", []), ("priority_inst.cu", "priority_inst.o", [])]
-    for m in (5, 9, 16):
-        u.append(("priority_spread_inst.cu", f"priority_spread_inst_{m}.o", [f"-DBS_PRIO_SPREAD_MAXL={m}"]))
-        u.append(("priority_interpod_inst.cu", f"priority_interpod_inst_{m}.o", [f"-DBS_PRIO_IPA_MAXL={m}"]))
-        u.append(("replay_ipf_inst.cu", f"replay_ipf_inst_{m}.o", [f"-DBS_REPLAY_IPF_MAXL={m}"]))
+    u = [("engine.cu", "engine.o", []), ("plugin.cpp", "plugin.o", [])]
+    for k in range(PRIO_SLICES):
+        u.append(("priority_inst.cu", f"priority_inst_{k}.o", [f"-DBS_PRIO_SLICE={k}"]))
+    for k in range(REPLAY_SLICES):
+        u.append(("replay_inst.cu", f"replay_inst_{k}.o", [f"-DBS_REPLAY_SLICE={k}"]))
     for n in range(FIT_SLICES):
         u.append(("fit_inst.cu", f"fit_inst_{n}.o", [f"-DBS_FIT_SLICE={n}"]))
     return u

@@ -3,9 +3,32 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+#include <utility>
+
 #include "../../include/bsched.h"
 
 namespace bsk {
+
+// Kernel builds are chosen with two helpers.  with_maxl<B...>(L, f) calls f(std::integral_constant<int, M>{}), M the
+// smallest of the ascending lane bounds B... that is at least L, or the last when L passes them all; it returns what f
+// returns.
+template <int B, int... Rest, class F>
+decltype(auto) with_maxl(uint32_t L, F&& f) {
+  if constexpr (sizeof...(Rest) == 0) return f(std::integral_constant<int, B>{});
+  else if (L <= (uint32_t)B) return f(std::integral_constant<int, B>{});
+  else return with_maxl<Rest...>(L, f);
+}
+// with_flags<N>(mask, f) calls f(std::integral_constant<uint32_t, mask>{}) for a mask below N, so that every bit of a
+// runtime mask becomes a compile-time flag; it calls nothing for a mask of N or more.
+template <uint32_t... M, class F>
+void with_flags_of(uint32_t mask, F& f, std::integer_sequence<uint32_t, M...>) {
+  ((mask == M ? f(std::integral_constant<uint32_t, M>{}) : void()), ...);
+}
+template <uint32_t N, class F>
+void with_flags(uint32_t mask, F&& f) {
+  with_flags_of(mask, f, std::make_integer_sequence<uint32_t, N>{});
+}
 
 constexpr int LANE_CPU = 0, LANE_MEM = 1, LANE_EPH = 2, LANE_PODS = 3;
 // Sentinels for lanes without a map key.  With |table values| <= BS_VALUE_LIMIT = 2^56,

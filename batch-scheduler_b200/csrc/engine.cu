@@ -916,46 +916,30 @@ struct StageTimer {
   }
 };
 
-inline int prefix_maxl(uint32_t L) {
-  return L <= 4 ? 4 : L <= 5 ? 5 : L <= 6 ? 6 : L <= 8 ? 8 : L <= 9 ? 9 : L <= 12 ? 12 : 16;
-}
-template <int MAXL>
-void launch_prefix_t(NodeTab t, PrefixSel ps, PrefixScratch sc, PrefixOut po, uint32_t n_classes, cudaStream_t s) {
-  const uint32_t n_chunks = cdiv(t.N, PREFIX_CHUNK);
-  dim3 grid(n_chunks, n_classes);
-  prefix_partial_kernel<MAXL><<<grid, PREFIX_CHUNK, 0, s>>>(t, ps, sc, n_chunks);
-  prefix_scan_kernel<MAXL><<<grid, PREFIX_CHUNK, 0, s>>>(t, ps, sc, n_chunks, po);
-}
 // two launches: chunk totals, then offsets + in-chunk scan + statistics
 void launch_prefix(uint32_t L, NodeTab t, PrefixSel ps, PrefixScratch sc, PrefixOut po, uint32_t n_classes,
                    cudaStream_t s) {
-  switch (prefix_maxl(L)) {
-    case 4: launch_prefix_t<4>(t, ps, sc, po, n_classes, s); break;
-    case 5: launch_prefix_t<5>(t, ps, sc, po, n_classes, s); break;
-    case 6: launch_prefix_t<6>(t, ps, sc, po, n_classes, s); break;
-    case 8: launch_prefix_t<8>(t, ps, sc, po, n_classes, s); break;
-    case 9: launch_prefix_t<9>(t, ps, sc, po, n_classes, s); break;
-    case 12: launch_prefix_t<12>(t, ps, sc, po, n_classes, s); break;
-    default: launch_prefix_t<16>(t, ps, sc, po, n_classes, s); break;
-  }
+  const uint32_t n_chunks = cdiv(t.N, PREFIX_CHUNK);
+  dim3 grid(n_chunks, n_classes);
+  with_maxl<4, 5, 6, 8, 9, 12, 16>(L, [&](auto M) {
+    prefix_partial_kernel<M><<<grid, PREFIX_CHUNK, 0, s>>>(t, ps, sc, n_chunks);
+    prefix_scan_kernel<M><<<grid, PREFIX_CHUNK, 0, s>>>(t, ps, sc, n_chunks, po);
+  });
 }
 
-inline uint32_t replay_maxl(uint32_t L) { return L <= 5 ? 5u : L <= 9 ? 9u : 16u; }
-void launch_replay(uint32_t L, const ReplayArgs& a, bool scored, bool loc, bool hp, bool ipf, cudaStream_t s) {
-  switch (replay_maxl(L) + (hp ? 100u : 0u) + (ipf ? 200u : 0u)) {
-    case 5: launch_replay_t<5, false>(a, scored, loc, s); break;
-    case 9: launch_replay_t<9, false>(a, scored, loc, s); break;
-    case 16: launch_replay_t<16, false>(a, scored, loc, s); break;
-    case 105: launch_replay_t<5, true>(a, scored, loc, s); break;
-    case 109: launch_replay_t<9, true>(a, scored, loc, s); break;
-    case 116: launch_replay_t<16, true>(a, scored, loc, s); break;
-    case 205: launch_replay_ipf<5, false>(a, scored, loc, s); break;
-    case 209: launch_replay_ipf<9, false>(a, scored, loc, s); break;
-    case 216: launch_replay_ipf<16, false>(a, scored, loc, s); break;
-    case 305: launch_replay_ipf<5, true>(a, scored, loc, s); break;
-    case 309: launch_replay_ipf<9, true>(a, scored, loc, s); break;
-    default: launch_replay_ipf<16, true>(a, scored, loc, s); break;
-  }
+// priority.cuh: the build of priority_pod_kernel for L lanes and `terms` (PRIO_*)
+cudaError_t launch_priority(uint32_t L, uint32_t grid, uint32_t terms, const PriorityIpaArgs& a, cudaStream_t s) {
+  with_maxl<5, 9, 16>(L, [&](auto M) {
+    (terms & PRIO_IPA ? launch_priority_slice<M, PRIO_IPA> : launch_priority_slice<M, 0>)(terms, grid, a, s);
+  });
+  return cudaGetLastError();
+}
+
+// replay.cuh: the build of replay_kernel for L lanes and `build` (REPLAY_*)
+void launch_replay(uint32_t L, uint32_t build, const ReplayIpfArgs& a, cudaStream_t s) {
+  with_maxl<5, 9, 16>(L, [&](auto M) {
+    (build & REPLAY_IPF ? launch_replay_slice<M, REPLAY_IPF> : launch_replay_slice<M, 0>)(build, a, s);
+  });
 }
 
 cudaError_t launch_fit(const FitArgs& a, uint32_t units, cudaStream_t s, uint32_t* launches, cudaEvent_t ev_a, cudaEvent_t ev_b) {
@@ -1764,15 +1748,10 @@ int evaluate_async_locked(bs_engine* e) {
       ra.hp_bins = e->hp.d_bins.as<uint32_t>();
       ra.used = e->hp.d_used.as<uint64_t>();
       ra.hp_rows = e->hp.d_reasons.as<uint32_t>();
-      const ReasonArgs& rb = ra;   // the filter-off builds take the base arguments
       const uint32_t grid = cdiv(P, REASON_PODS_PER_CTA);
-      if (e->hp.on) {
-        auto fn = e->ipf.on ? reason_pod_kernel<true, true> : reason_pod_kernel<false, true>;
-        fn<<<grid, REASON_THREADS, 0, e->s>>>(ra);
-      } else {
-        auto fn = e->ipf.on ? reason_pod_kernel<true, false> : reason_pod_kernel<false, false>;
-        fn<<<grid, REASON_THREADS, 0, e->s>>>(rb);
-      }
+      with_flags<4>((e->ipf.on ? 1u : 0u) | (e->hp.on ? 2u : 0u), [&](auto f) {   // bit 0 IPF, bit 1 HP
+        reason_pod_kernel<(f & 1u) != 0, (f & 2u) != 0><<<grid, REASON_THREADS, 0, e->s>>>(ra);
+      });
       tm.launched();
     }
   }
@@ -1804,8 +1783,10 @@ int evaluate_async_locked(bs_engine* e) {
     la.pref_class = e->pref.d_class.as<uint32_t>();
     la.w_taint = e->w_taint;
     la.w_naff = e->w_naff;
-    const bool pref = e->w_taint || e->w_naff, ratio = e->ratio.weight != 0;
-    if (e->w_img || e->w_avoid) {   // (the pre-pass runs on the same stream, ahead of the kernel)
+    const uint32_t terms = (e->ratio.weight ? PRIO_RATIO : 0u) | (e->w_taint || e->w_naff ? PRIO_PREF : 0u) |
+                           (e->w_img || e->w_avoid ? PRIO_LOC : 0u) | (e->w_spread ? PRIO_SPREAD : 0u) |
+                           (e->w_ipa ? PRIO_IPA : 0u);
+    if (terms & PRIO_LOC) {   // (the pre-pass runs on the same stream, ahead of the kernel)
       if ((rc = locality_prepass(e))) return rc;
       la.il = e->loc.d_il.as<uint8_t>();
       la.avoid_mask = e->loc.d_avoid_mask.as<uint64_t>();
@@ -1814,19 +1795,19 @@ int evaluate_async_locked(bs_engine* e) {
       la.w_img = e->w_img;
       la.w_avoid = e->w_avoid;
     }
-    if (e->w_spread) {
+    if (terms & PRIO_SPREAD) {
       la.spread_zone = e->spread.d_zone.as<uint8_t>();
       la.spread_counts = e->spread.d_counts.as<int32_t>();
       la.spread_class = e->spread.d_class.as<uint32_t>();
       la.w_spread = e->w_spread;
     }
-    if (e->w_ipa) {   // (the pre-pass runs on the same stream, ahead of the kernel)
+    if (terms & PRIO_IPA) {   // (the pre-pass runs on the same stream, ahead of the kernel)
       if ((rc = interpod_prepass(e))) return rc;
       la.ipa_raw = e->ipa.d_raw.as<int64_t>();
       la.ipa_class = e->ipa.d_class.as<uint32_t>();
       la.w_ipa = e->w_ipa;
     }
-    CK(launch_priority(L, grid, ratio, pref, e->w_img || e->w_avoid, e->w_spread != 0, e->w_ipa != 0, la, e->s));
+    CK(launch_priority(L, grid, terms, la, e->s));
     e->launches += 1;
   }
   if (e->peer_attached) {
@@ -1920,30 +1901,6 @@ int fetch_locked(bs_engine* e, bs_results* out, bool view = false) {
 }
 
 // ---- preemption (preempt.cuh) ----
-// Launches a MAXL instance of a preemption kernel: 5, 9 or 16 lanes of registers
-template <template <int> class K, class... A>
-void launch_maxl(uint32_t L, A&&... args) {
-  if (L <= 5) K<5>::go(args...);
-  else if (L <= 9) K<9>::go(args...);
-  else K<16>::go(args...);
-}
-template <int MAXL>
-struct PreemptNodeLaunch {
-  static void go(dim3 grid, cudaStream_t s, const PreemptArgs& a) {
-    preempt_node_kernel<MAXL><<<grid, PREEMPT_THREADS, 0, s>>>(a);
-  }
-};
-template <int MAXL>
-struct PreemptEmitLaunch {
-  static void go(dim3 grid, cudaStream_t s, const PreemptArgs& a) { preempt_emit_kernel<MAXL><<<grid, 256, 0, s>>>(a); }
-};
-template <int MAXL>
-struct PreemptCommitLaunch {
-  static void go(cudaStream_t s, const PreemptArgs& a, const WalkArgs& w, uint32_t i) {
-    preempt_commit_kernel<MAXL><<<1, PREEMPT_THREADS, 0, s>>>(a, w, i);
-  }
-};
-
 // What the bound-table pass finds wrong, in the order the errors are reported.
 struct BoundStats {
   bool bad_index = false, bad_count = false, bad_keys = false, bad_range = false;   // bad_index: node or gid
@@ -2888,7 +2845,8 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
   const bool safe = worst * (long double)std::max(N, 1u) < 4.0e18L;
   const uint32_t n_blocks = cdiv(N, REPLAY_BLOCK);
   const bool cache = safe && fitmask && n_blocks >= 1 && n_blocks <= (uint32_t)REPLAY_MAX_BLOCKS;
-  const size_t rows = cache ? (size_t)2 * e->n_rep_classes * n_blocks : 0, maxl = replay_maxl(L);
+  const size_t rows = cache ? (size_t)2 * e->n_rep_classes * n_blocks : 0;
+  const size_t maxl = with_maxl<5, 9, 16>(L, [](auto M) { return (size_t)M; });   // launch_replay's lane bound
   View s_req, s_pc, s_rp, s_matched, s_gflags, s_grc, s_minres, s_mrp, d_queue, d_pf, d_node, d_ready, d_status,
       n_left0, n_left1, n_both, n_stat, n_fit, c_sum, c_max, c_keys, n_nz, s_used, d_want, d_conf, s_pres, s_hits,
       d_fclass;
@@ -3010,7 +2968,9 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
   }
   {
     StageTimer tm(e, BS_K_REPLAY, e->s);
-    launch_replay(L, a, scored, loc, hp, ipf, e->s);
+    const uint32_t build = (scored ? REPLAY_SCORED : 0u) | (scored && e->ratio.weight ? REPLAY_RATIO : 0u) |
+                           (loc ? REPLAY_LOC : 0u) | (hp ? REPLAY_HP : 0u) | (ipf ? REPLAY_IPF : 0u);
+    launch_replay(L, build, la, e->s);
     tm.launched();
     CK(cudaGetLastError());
   }
@@ -3297,7 +3257,9 @@ int bs_preempt(bs_engine* e, const uint32_t* pods, uint32_t n, bs_preempt_result
     for (uint32_t p0 = 0; p0 < n; p0 += chunk) {
       const uint32_t cnt = std::min(chunk, n - p0);
       a.p0 = p0;
-      launch_maxl<PreemptNodeLaunch>(L, dim3(a.n_tiles, cnt), (cudaStream_t)e->s, a);
+      with_maxl<5, 9, 16>(L, [&](auto M) {
+        preempt_node_kernel<M><<<dim3(a.n_tiles, cnt), PREEMPT_THREADS, 0, e->s>>>(a);
+      });
       preempt_reduce_kernel<<<cdiv(cnt, 256), 256, 0, e->s>>>(a, cnt);
       e->launches += 2;
     }
@@ -3321,7 +3283,7 @@ int bs_preempt(bs_engine* e, const uint32_t* pods, uint32_t n, bs_preempt_result
   CK(cudaMemcpyAsync(e->d_poff.p, out->victim_offset, (size_t)n * 4, cudaMemcpyHostToDevice, e->s));
   a.offset = e->d_poff.as<uint32_t>();
   a.victims = e->d_pvict.as<uint32_t>();
-  launch_maxl<PreemptEmitLaunch>(L, dim3(cdiv(n, 256)), (cudaStream_t)e->s, a);
+  with_maxl<5, 9, 16>(L, [&](auto M) { preempt_emit_kernel<M><<<dim3(cdiv(n, 256)), 256, 0, e->s>>>(a); });
   ++e->launches;
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(out->victims, a.victims, (size_t)total * 4, cudaMemcpyDeviceToHost, e->s));
@@ -3467,10 +3429,12 @@ int bs_preempt_walk(bs_engine* e, const uint32_t* pods, uint32_t n, uint32_t fla
   for (uint32_t i = 0; i < n; ++i) {   // stream-ordered: no host synchronisation inside the walk
     if (N) {
       a.p0 = i;
-      launch_maxl<PreemptNodeLaunch>(L, dim3(a.n_tiles, 1), (cudaStream_t)e->s, a);
+      with_maxl<5, 9, 16>(L, [&](auto M) {
+        preempt_node_kernel<M><<<dim3(a.n_tiles, 1), PREEMPT_THREADS, 0, e->s>>>(a);
+      });
       ++e->launches;
     }
-    launch_maxl<PreemptCommitLaunch>(L, (cudaStream_t)e->s, a, w, i);
+    with_maxl<5, 9, 16>(L, [&](auto M) { preempt_commit_kernel<M><<<1, PREEMPT_THREADS, 0, e->s>>>(a, w, i); });
     ++e->launches;
   }
   CK(cudaGetLastError());

@@ -37,7 +37,7 @@ struct IpfTopo {
   uint32_t n_nodes;
 };
 
-// The kernels are defined once, in engine.cu; replay_ipf_inst.cu (BS_KERNELS_HELPERS_ONLY) needs the types above only.
+// The kernels are defined once, in engine.cu; replay_inst.cu (BS_KERNELS_HELPERS_ONLY) needs the types above only.
 #ifndef BS_KERNELS_HELPERS_ONLY
 // K1j ipf_presence_kernel — a thread per bound pod, walking its class's entries in step with its warp (entry k of every
 // lane at once).  For an entry whose key the pod's node carries (value v): match sets bit term_off + v of the match

@@ -243,7 +243,7 @@ __device__ __forceinline__ uint64_t ratio_term(uint32_t weight, uint32_t num, ui
   return (uint64_t)weight * (uint64_t)ratio_round(num, den);
 }
 
-// The round's kernels.  A translation unit that needs only the helpers (priority_inst.cu, replay_ipf_inst.cu) defines
+// The round's kernels.  A translation unit that needs only the helpers (priority_inst.cu, replay_inst.cu) defines
 // BS_KERNELS_HELPERS_ONLY, so that these external kernels are defined once, in engine.cu; the group and findMaxPG
 // helpers the walk shares sit between guarded stretches.
 #ifndef BS_KERNELS_HELPERS_ONLY

@@ -480,21 +480,15 @@ priority_pod_kernel(std::conditional_t<IPA, PriorityIpaArgs,
   }
 }
 
-// priority_inst.cu, a translation unit of its own so that the variants compile in parallel with engine.cu:
-// priority_pod_kernel<MAXL, ratio, pref, loc, spread, ipa> for the engine's lane count L; `a` is read as the flags'
-// argument type (PriorityArgs without any flag, PriorityRatioArgs with ratio alone, PriorityPrefArgs with pref,
-// PriorityLocArgs with loc, PrioritySpreadArgs with spread, all of it with ipa).
-cudaError_t launch_priority(uint32_t L, uint32_t grid, bool ratio, bool pref, bool loc, bool spread, bool ipa,
-                            const PriorityIpaArgs& a, cudaStream_t s);
-// priority_spread_inst.cu, one translation unit per MAXL (-DBS_PRIO_SPREAD_MAXL): the SPREAD variants, reached through
-// launch_priority
-template <int MAXL>
-void launch_priority_spread(uint32_t grid, bool ratio, bool pref, bool loc, const PrioritySpreadArgs& a, cudaStream_t s);
-// priority_interpod_inst.cu, one translation unit per MAXL (-DBS_PRIO_IPA_MAXL): the IPA variants, reached through
-// launch_priority
-template <int MAXL>
-void launch_priority_interpod(uint32_t grid, bool ratio, bool pref, bool loc, bool spread, const PriorityIpaArgs& a,
-                              cudaStream_t s);
+// The builds of priority_pod_kernel: one per lane bound MAXL = 5, 9, 16 and mask of the terms below, 96 in all.  The host
+// sets a term's bit when its weight is non-zero; `a` is read as the build's argument type (PriorityArgs without any
+// term, PriorityRatioArgs with RATIO alone, PriorityPrefArgs with PREF, PriorityLocArgs with LOC, PrioritySpreadArgs
+// with SPREAD, all of it with IPA).
+constexpr uint32_t PRIO_RATIO = 1, PRIO_PREF = 2, PRIO_LOC = 4, PRIO_SPREAD = 8, PRIO_IPA = 16;
+// priority_inst.cu, one slice per (MAXL, IPA bit): launches the build of lane bound MAXL for `terms`, whose IPA bit is
+// IPA (engine.cu's launch_priority picks the slice)
+template <int MAXL, uint32_t IPA>
+void launch_priority_slice(uint32_t terms, uint32_t grid, const PriorityIpaArgs& a, cudaStream_t s);
 // the LOC pre-pass: scaled[n_images] from the bit rows and sizes, then il[n_classes][Npad]; 2 launches
 cudaError_t launch_locality_prepass(const uint32_t* bits, const int64_t* size, int64_t* scaled, uint32_t n_images,
                                     const uint32_t* class_offset, const uint32_t* class_images, uint8_t* il,

@@ -1,11 +1,30 @@
-// priority_inst.cu — the priority lists' kernels (priority.cuh): every priority_pod_kernel variant and the LOC and IPA
-// pre-passes, except the SPREAD and IPA variants (priority_spread_inst.cu, priority_interpod_inst.cu).  A translation
-// unit of its own (build.py), compiled in parallel with engine.cu, which reaches the kernels through launch_priority,
+// priority_inst.cu — the priority lists' kernels (priority.cuh), compiled once per slice (build.py, -DBS_PRIO_SLICE=k
+// for k = 0..5) so that the 96 builds of priority_pod_kernel compile in parallel with the other units: slice k holds
+// the 16 builds of lane bound 5, 9 or 16 (k / 2 = 0, 1, 2) with IPA off (even k) or on (odd k), and slice 0 also the
+// LOC and IPA pre-passes.  engine.cu reaches the builds through launch_priority_slice and the pre-passes through
 // launch_locality_prepass and launch_interpod_prepass.
 #define BS_KERNELS_HELPERS_ONLY   // kernels.cuh's round kernels live in engine.cu
 #include "priority.cuh"
 
+#ifndef BS_PRIO_SLICE
+#error "compile with -DBS_PRIO_SLICE=0..5"
+#endif
+
 namespace bsk {
+
+template <int MAXL, uint32_t IPA>
+void launch_priority_slice(uint32_t terms, uint32_t grid, const PriorityIpaArgs& a, cudaStream_t s) {
+  with_flags<PRIO_IPA>(terms % PRIO_IPA, [&](auto low) {
+    constexpr uint32_t T = IPA | decltype(low)::value;
+    priority_pod_kernel<MAXL, (T & PRIO_RATIO) != 0, (T & PRIO_PREF) != 0, (T & PRIO_LOC) != 0, (T & PRIO_SPREAD) != 0,
+                        (T & PRIO_IPA) != 0><<<grid, PRIO_THREADS, 0, s>>>(a);
+  });
+}
+constexpr int SLICE_MAXL[] = {5, 9, 16};
+template void launch_priority_slice<SLICE_MAXL[BS_PRIO_SLICE / 2], BS_PRIO_SLICE % 2 * PRIO_IPA>(
+    uint32_t, uint32_t, const PriorityIpaArgs&, cudaStream_t);
+
+#if BS_PRIO_SLICE == 0
 namespace {
 
 // The LOC pre-pass.  ImageLocality's per-name score depends on how many snapshot nodes report the name, and its sum
@@ -147,45 +166,7 @@ __global__ void __launch_bounds__(LOC_THREADS) interpod_class_kernel(InterpodCla
   }
 }
 
-template <bool RATIO, bool PREF, bool LOC, class Args>
-void launch_t(uint32_t L, uint32_t grid, const Args& a, cudaStream_t s) {
-  if (L <= 5) priority_pod_kernel<5, RATIO, PREF, LOC><<<grid, PRIO_THREADS, 0, s>>>(a);
-  else if (L <= 9) priority_pod_kernel<9, RATIO, PREF, LOC><<<grid, PRIO_THREADS, 0, s>>>(a);
-  else priority_pod_kernel<16, RATIO, PREF, LOC><<<grid, PRIO_THREADS, 0, s>>>(a);
-}
-
 }  // namespace
-
-cudaError_t launch_priority(uint32_t L, uint32_t grid, bool ratio, bool pref, bool loc, bool spread, bool ipa,
-                            const PriorityIpaArgs& a, cudaStream_t s) {
-  const PrioritySpreadArgs& ps = a;
-  const PriorityLocArgs& pl = a;
-  const PriorityPrefArgs& pp = a;
-  const PriorityRatioArgs& pr = a;
-  const PriorityArgs& pb = a;
-  if (ipa) {
-    if (L <= 5) launch_priority_interpod<5>(grid, ratio, pref, loc, spread, a, s);
-    else if (L <= 9) launch_priority_interpod<9>(grid, ratio, pref, loc, spread, a, s);
-    else launch_priority_interpod<16>(grid, ratio, pref, loc, spread, a, s);
-  } else if (spread) {
-    if (L <= 5) launch_priority_spread<5>(grid, ratio, pref, loc, ps, s);
-    else if (L <= 9) launch_priority_spread<9>(grid, ratio, pref, loc, ps, s);
-    else launch_priority_spread<16>(grid, ratio, pref, loc, ps, s);
-  } else if (loc) {
-    if (pref && ratio) launch_t<true, true, true>(L, grid, pl, s);
-    else if (pref) launch_t<false, true, true>(L, grid, pl, s);
-    else if (ratio) launch_t<true, false, true>(L, grid, pl, s);
-    else launch_t<false, false, true>(L, grid, pl, s);
-  } else if (pref) {
-    if (ratio) launch_t<true, true, false>(L, grid, pp, s);
-    else launch_t<false, true, false>(L, grid, pp, s);
-  } else if (ratio) {
-    launch_t<true, false, false>(L, grid, pr, s);
-  } else {
-    launch_t<false, false, false>(L, grid, pb, s);
-  }
-  return cudaGetLastError();
-}
 
 cudaError_t launch_locality_prepass(const uint32_t* bits, const int64_t* size, int64_t* scaled, uint32_t n_images,
                                     const uint32_t* class_offset, const uint32_t* class_images, uint8_t* il,
@@ -211,5 +192,7 @@ cudaError_t launch_interpod_prepass(bool mass, const uint32_t* topo, const uint3
   interpod_class_kernel<<<grid, LOC_THREADS, 0, s>>>(pods, topo, term_key, term_off, ms, raw, n_nodes, Npad);
   return cudaGetLastError();
 }
+
+#endif
 
 }  // namespace bsk

@@ -921,23 +921,18 @@ __global__ void __launch_bounds__(REPLAY_THREADS, 1) replay_kernel(ReplayArgsOf<
   if (tid == 0) { a.status[0] = sm.panic; a.status[1] = (int32_t)lo; a.status[2] = sm.monotone; }
 }
 
-// loc: the scored walk with the locality terms (a is then a ReplayLocArgs); HP: the PodFitsHostPorts filter is on (a is
-// then a ReplayHpArgs); IPF: the MatchInterPodAffinity filter is on (a is then a ReplayIpfArgs)
-template <int MAXL, bool HP, bool IPF = false>
-void launch_replay_t(const ReplayArgs& a, bool scored, bool loc, cudaStream_t s) {
-  if (loc) {
-    const auto& la = static_cast<const ReplayArgsOf<true, HP, IPF>&>(a);
-    if (a.ratio.weight) replay_kernel<MAXL, true, true, true, HP, IPF><<<1, REPLAY_THREADS, 0, s>>>(la);
-    else replay_kernel<MAXL, true, false, true, HP, IPF><<<1, REPLAY_THREADS, 0, s>>>(la);
-    return;
-  }
-  const auto& ha = static_cast<const ReplayArgsOf<false, HP, IPF>&>(a);
-  if (scored && a.ratio.weight) replay_kernel<MAXL, true, true, false, HP, IPF><<<1, REPLAY_THREADS, 0, s>>>(ha);
-  else if (scored) replay_kernel<MAXL, true, false, false, HP, IPF><<<1, REPLAY_THREADS, 0, s>>>(ha);
-  else replay_kernel<MAXL, false, false, false, HP, IPF><<<1, REPLAY_THREADS, 0, s>>>(ha);
+// The builds of replay_kernel: one per lane bound MAXL = 5, 9, 16 and mask of the bits below, 60 in all.  SCORED:
+// bs_replay_priority's node choice; RATIO: with the ratio term; LOC: with the locality terms (a is read as a
+// ReplayLocArgs); HP: the PodFitsHostPorts filter is on (a ReplayHpArgs); IPF: the MatchInterPodAffinity filter is on (a
+// ReplayIpfArgs).  RATIO and LOC belong to the scored node choice, so a mask with either and without SCORED is not a
+// build.
+constexpr uint32_t REPLAY_SCORED = 1, REPLAY_RATIO = 2, REPLAY_LOC = 4, REPLAY_HP = 8, REPLAY_IPF = 16;
+constexpr bool replay_build_exists(uint32_t build) {
+  return (build & REPLAY_SCORED) || !(build & (REPLAY_RATIO | REPLAY_LOC));
 }
-// replay_ipf_inst.cu, one translation unit per MAXL (-DBS_REPLAY_IPF_MAXL): the IPF builds, launch_replay_t<MAXL, HP, true>
-template <int MAXL, bool HP>
-void launch_replay_ipf(const ReplayArgs& a, bool scored, bool loc, cudaStream_t s);
+// replay_inst.cu, one slice per (MAXL, IPF bit): launches the build of lane bound MAXL for `build`, whose IPF bit is
+// IPF (engine.cu's launch_replay picks the slice)
+template <int MAXL, uint32_t IPF>
+void launch_replay_slice(uint32_t build, const ReplayIpfArgs& a, cudaStream_t s);
 
 }  // namespace bsk

@@ -1,7 +1,7 @@
 """Designed rounds in which one lane decides every outcome, for every lane count L = 4..16.
 
-The lane count picks the build of the prefix scans (prefix_maxl: 4, 5, 6, 8, 9, 12, 16) and of bs_replay
-(replay_maxl: 5, 9, 16), and the lane classes of the fit kernel.  Random snapshots put small values on every scalar
+The lane count picks the build of the prefix scans (lane bounds 4, 5, 6, 8, 9, 12, 16) and of bs_replay
+(lane bounds 5, 9, 16), and the lane classes of the fit kernel.  Random snapshots put small values on every scalar
 lane, so the top lane seldom decides a verdict.  Here every lane but one is generous and never decides anything; the
 deciding lane is present on some nodes and absent on others, its residuals sit at, just above and just below the
 pods' requests, and the groups' MinResources on it decide the cluster checks:
