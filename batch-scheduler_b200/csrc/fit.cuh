@@ -21,8 +21,8 @@ namespace bsk {
 //   INPUT: the producer lane streams the tiles of the residual table into a FIT_STAGES-deep
 //     shared-memory ring with 1-D TMA bulk copies (cp.async.bulk global->shared, one per lane
 //     row), guarded by full/empty mbarrier pairs; consumers never meet at a CTA-wide barrier.
-//   OUTPUT: score rows do NOT leave through the LSU.  In score mode a warp sweeps the tile range
-//     once per pod (its rows front to back), writes that pod's NODE_TILE scores into a private staging slab in shared
+//   OUTPUT: score rows do NOT leave through the LSU.  In score mode a warp sweeps each tile one
+//     pod at a time, writes that pod's NODE_TILE scores into a private staging slab in shared
 //     memory (st.shared.u64, conflict-free) and one lane hands the row segment — NODE_TILE*8 =
 //     4 KB contiguous bytes of one matrix row — to the TMA engine (cp.async.bulk shared->global,
 //     bulk_group completion); FIT_NB slabs per warp rotate, a slab is refilled once its bulk read
@@ -37,7 +37,7 @@ namespace bsk {
 //     lines leave through the same bulk path (profiles/store_ladder_h100.jsonl).
 // A lane owns nodes lane, lane+32, ... of the tile.  The bitmap and decisions-only modes evaluate
 // the warp's PODS_PER_WARP pods against each node's `left` in registers; the score sweep reads a
-// node's `left` from the stage once per pod (the producer streams the tiles once per pass).
+// node's `left` from the stage once per pod (the producer streams the tiles once per CTA in every mode).
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return (uint32_t)__cvta_generic_to_shared(p);
 }
@@ -406,20 +406,10 @@ __global__ void __launch_bounds__(FIT_THREADS, FIT_MIN_BLOCKS) gang_fit_kernel(F
   // complete on `full`.  Consumers never meet at a CTA-wide barrier during the sweep.
   if (wid == FIT_WARPS) {
     if (lane == 0) {
-      if constexpr (SCORE) {
-        // the score sweep passes over the tile range once per pod of a warp (below)
-        const uint32_t range = tile_hi - tile_lo;
-        for (uint32_t i = 0; i < PODS_PER_WARP * range; ++i) {
-          const uint32_t st = i % FIT_STAGES, use = i / FIT_STAGES;
-          if (use > 0) mbar_wait(&s_empty[st], (use - 1) & 1);
-          issue(tile_lo + i % range, st);
-        }
-      } else {
-        for (uint32_t tile = tile_lo; tile < tile_hi; ++tile) {
-          const uint32_t st = (tile - tile_lo) % FIT_STAGES, use = (tile - tile_lo) / FIT_STAGES;
-          if (use > 0) mbar_wait(&s_empty[st], (use - 1) & 1);
-          issue(tile, st);
-        }
+      for (uint32_t tile = tile_lo; tile < tile_hi; ++tile) {
+        const uint32_t st = (tile - tile_lo) % FIT_STAGES, use = (tile - tile_lo) / FIT_STAGES;
+        if (use > 0) mbar_wait(&s_empty[st], (use - 1) & 1);
+        issue(tile, st);
       }
     }
     return;
@@ -454,7 +444,7 @@ __global__ void __launch_bounds__(FIT_THREADS, FIT_MIN_BLOCKS) gang_fit_kernel(F
     best_s[r] = LN > 0 ? (typename BestT<(LN > 0)>::type)(-1) : (typename BestT<(LN > 0)>::type)INT64_MIN;
     const uint32_t p = wpod0 + r;
     coff[r] = (p < a.P ? a.fit_class[p] : 0u) * n_tiles * 32 + lane;
-    if (!SCORE) load_req(r);   // score mode: at the start of the pod's pass
+    if (!SCORE) load_req(r);   // score mode: before each of the pod's row segments
   }
   const uint32_t slab0 = smem_u32(smem_raw + fit_smem_front(LW, LN, LS)) + wid * (uint32_t)(FIT_NB * fit_slab_bytes());
   int64_t* srow = SCORE ? a.score + (size_t)wpod0 * a.score_pitch : nullptr;
@@ -462,25 +452,15 @@ __global__ void __launch_bounds__(FIT_THREADS, FIT_MIN_BLOCKS) gang_fit_kernel(F
   // Consumers: a warp releases a stage by arriving on its `empty` mbarrier and may run up to
   // FIT_STAGES-1 tiles ahead of the slowest warp.
   uint32_t stage = 0, phase = 0;
-  // Score mode sweeps the tile range once per pod (pass = the pod), writing each of the warp's rows front to back:
-  // a warp has one matrix row in flight instead of four.  On an H100 the store stream of four rows written a tile
-  // at a time took 0.03-0.04 ms more than the same rows one after another (profiles/microbench/store_ladder.cu).  The
-  // other modes make one pass with all of the warp's pods.
-  constexpr int PASSES = SCORE ? PODS_PER_WARP : 1;
-  uint32_t nseg = 0, nline = 0;   // SCORE: bulk groups committed, bitmap lines sent
+  uint32_t nseg = 0;   // SCORE: bulk groups committed
   ColBits colnext[PODS_PER_WARP];   // class bits are fetched one tile ahead (their L2 latency stays off the tile's critical path)
 #pragma unroll
-  for (int pass = 0; pass < PASSES; ++pass) {
-  if (SCORE) load_req(pass);   // only the pass's pod has its requests in registers
-#pragma unroll
-  for (int r = 0; r < PODS_PER_WARP; ++r)
-    if (!SCORE || r == pass) colnext[r] = __ldg(a.classfit + coff[r] + min(tile_lo, n_tiles - 1) * 32);
+  for (int r = 0; r < PODS_PER_WARP; ++r) colnext[r] = __ldg(a.classfit + coff[r] + min(tile_lo, n_tiles - 1) * 32);
   for (uint32_t tile = tile_lo; tile < tile_hi; ++tile) {
     ColBits colbits[PODS_PER_WARP];
     const uint32_t tnext = tile + 1 < tile_hi ? tile + 1 : tile;
 #pragma unroll
     for (int r = 0; r < PODS_PER_WARP; ++r) {
-      if (SCORE && r != pass) continue;
       colbits[r] = colnext[r];
       colnext[r] = __ldg(a.classfit + coff[r] + tnext * 32);
     }
@@ -490,38 +470,45 @@ __global__ void __launch_bounds__(FIT_THREADS, FIT_MIN_BLOCKS) gang_fit_kernel(F
     const uint32_t node_base = tile * NODE_TILE;
     const uint32_t wbase = (tile % TILES_PER_LINE) * TILE_WORDS;
     if constexpr (SCORE) {
-      // staged scores: the pod's row of the tile goes to the next of the warp's FIT_NB staging slabs and leaves as one
-      // NODE_TILE*8-byte bulk store while the next tile is computed.
+      // Staged scores, one pod at a time: the pod's row of the tile goes to the next of the warp's FIT_NB staging
+      // slabs and leaves as one NODE_TILE*8-byte bulk store while the next pod is computed.  The producer streams
+      // the tile range once per CTA.  Only the pod being swept has its requests in registers (read back from shared
+      // memory per segment), so the register count stays that of a one-pod sweep.
+      // On compressible memory this order (four rows a tile at a time) is the faster one: on an H100 the store ladder
+      // took 2.127 ms for it against 2.165-2.169 ms with each warp's rows front to back and the tiles streamed once
+      // per row (profiles/fit_multicast_h100.jsonl); on cudaMalloc memory the order went the other way.
       // The pod's fit-bitmap line leaves the same way, from its ballot words in s_words, in the bulk group of the
       // segment that completes it: written from the LSU (st.global) beside the bulk stream, the lines cost the
-      // kernel 0.13 ms on an H100, as bulk stores 0.05 ms (profiles/microbench/store_ladder.cu).  Consecutive lines
-      // take the warp's PODS_PER_WARP word rows in turn, so a row is rewritten PODS_PER_WARP lines later, behind
-      // slab waits that leave at most FIT_NB - 1 bulk groups pending: the line's read is done by then.
+      // kernel 0.13 ms on an H100, as bulk stores 0.05 ms (profiles/microbench/store_ladder.cu).  Pod r's word row
+      // is rewritten PODS_PER_WARP segments later, behind slab waits that leave at most FIT_NB - 1 bulk groups
+      // pending: the line's read is done by then.
       static_assert(PODS_PER_WARP >= FIT_NB, "a bitmap line's word row must be read before it is rewritten");
-      const uint32_t wrow = nline % PODS_PER_WARP;
-      const uint32_t slab = slab0 + (nseg % FIT_NB) * (uint32_t)fit_slab_bytes();
-      if (nseg >= (uint32_t)FIT_NB) {
-        if (lane == 0) bulk_wait_read<FIT_NB - 1>();   // the bulk store that last read this slab is done with it
-        __syncwarp();
-      }
-      // fit_tile writes pod `pass`'s ballot words to row `pass` of the words it is given: shift them to row wrow
-      fit_tile<LW, LN, LS, OUT, 1>(a, tlw, tln, rqw, rqn, colbits, pass, slab, s_words + ((int)wrow - pass) * 32, wbase,
-                                   node_base, lane, best_s, best_n, kb, cnt, tks, tkn, thr);
-      fence_async_smem();
-      __syncwarp();
-      if (lane == 0) {
-        // the tile's scores, or what is left of the row (pitch is even: 16-byte sizes)
-        if (node_base < (uint32_t)a.score_pitch) {
-          const uint32_t cols = min((uint32_t)NODE_TILE, (uint32_t)a.score_pitch - node_base);
-          tma_bulk_s2g(srow + (size_t)pass * a.score_pitch + node_base, slab, cols * 8, l2_evict_first());
+#pragma unroll
+      for (int r = 0; r < PODS_PER_WARP; ++r) {
+        load_req(r);
+        const uint32_t slab = slab0 + (nseg % FIT_NB) * (uint32_t)fit_slab_bytes();
+        if (nseg >= (uint32_t)FIT_NB) {
+          if (lane == 0) bulk_wait_read<FIT_NB - 1>();   // the bulk store that last read this slab is done with it
+          __syncwarp();
         }
-        // the tile completes the pod's bitmap line (TILES_PER_LINE tiles, or the range's last tile)
-        if (want_bitmap && ((tile + 1) % TILES_PER_LINE == 0 || tile + 1 == tile_hi))
-          tma_bulk_s2g(a.fit_bitmap + (size_t)(wpod0 + pass) * a.bitmap_pitch + (tile / TILES_PER_LINE) * 32,
-                       smem_u32(s_words + wrow * 32), (tile % TILES_PER_LINE + 1) * TILE_WORDS * 4, l2_evict_first());
-        bulk_commit();
+        fit_tile<LW, LN, LS, OUT, 1>(a, tlw, tln, rqw, rqn, colbits, r, slab, s_words, wbase, node_base, lane, best_s,
+                                     best_n, kb, cnt, tks, tkn, thr);
+        fence_async_smem();
+        __syncwarp();
+        if (lane == 0) {
+          // the tile's scores, or what is left of the row (pitch is even: 16-byte sizes)
+          if (node_base < (uint32_t)a.score_pitch) {
+            const uint32_t cols = min((uint32_t)NODE_TILE, (uint32_t)a.score_pitch - node_base);
+            tma_bulk_s2g(srow + (size_t)r * a.score_pitch + node_base, slab, cols * 8, l2_evict_first());
+          }
+          // the tile completes the pod's bitmap line (TILES_PER_LINE tiles, or the range's last tile)
+          if (want_bitmap && ((tile + 1) % TILES_PER_LINE == 0 || tile + 1 == tile_hi))
+            tma_bulk_s2g(a.fit_bitmap + (size_t)(wpod0 + r) * a.bitmap_pitch + (tile / TILES_PER_LINE) * 32,
+                         smem_u32(s_words + r * 32), (tile % TILES_PER_LINE + 1) * TILE_WORDS * 4, l2_evict_first());
+          bulk_commit();
+        }
+        ++nseg;
       }
-      ++nseg;
     } else {
       fit_tile<LW, LN, LS, OUT, PODS_PER_WARP>(a, tlw, tln, rqw, rqn, colbits, 0, 0, s_words, wbase, node_base, lane,
                                                best_s, best_n, kb, cnt, tks, tkn, thr);
@@ -531,7 +518,6 @@ __global__ void __launch_bounds__(FIT_THREADS, FIT_MIN_BLOCKS) gang_fit_kernel(F
       // (an equal score in a later tile loses to the earlier node)
 #pragma unroll
       for (int r = 0; r < PODS_PER_WARP; ++r) {
-        if (SCORE && r != pass) continue;
         if (kb[r] >= kthr[r]) {
           best_s[r] = kb[r] >> KEY_BITS;
           best_n[r] = (int32_t)(node_base + lane) + (TILE_WORDS - 1 - (kb[r] & (TILE_WORDS - 1))) * 32;
@@ -548,22 +534,18 @@ __global__ void __launch_bounds__(FIT_THREADS, FIT_MIN_BLOCKS) gang_fit_kernel(F
     if ((WORDS || (TOPK && want_bitmap)) && ((tile + 1) % TILES_PER_LINE == 0 || tile + 1 == tile_hi)) {
       const uint32_t line = tile / TILES_PER_LINE;
       const uint32_t valid = (tile % TILES_PER_LINE + 1) * TILE_WORDS;   // words assembled in this line
-      if constexpr (SCORE) {
-        if (lane < valid) cnt[pass] += __popc(s_words[(nline % PODS_PER_WARP) * 32 + lane]);
-        ++nline;
-      } else if (lane < valid) {
+      if (lane < valid) {
 #pragma unroll
         for (int r = 0; r < PODS_PER_WARP; ++r) {
           const uint32_t w = s_words[r * 32 + lane];
           if (WORDS) cnt[r] += __popc(w);
-          if (want_bitmap) a.fit_bitmap[(size_t)(wpod0 + r) * a.bitmap_pitch + line * 32 + lane] = w;
+          if (!SCORE && want_bitmap) a.fit_bitmap[(size_t)(wpod0 + r) * a.bitmap_pitch + line * 32 + lane] = w;
         }
       }
     }
     __syncwarp();                                   // the ballot slab is rewritten by the next tile
     if (++stage == FIT_STAGES) { stage = 0; phase ^= 1; }
   }
-  }  // pass
   if (SCORE && lane == 0) bulk_wait_read<0>();      // the slabs must outlive their bulk reads
   if (TOPK && lane < a.topk_k) {
     // the lists leave as [Ppad][K] rows (padded rows: no pod guard); lane i writes entry i
