@@ -237,6 +237,7 @@ SYMBOLS = {
     "bs_upload_node_host_ports": (C.c_int, [C.c_void_p, _p(HostPortNodesC)]),
     "bs_upload_pod_host_ports": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p]),
     "bs_fetch_host_port_reason_rows": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]),
+    "bs_upload_bound_host_ports": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p]),
     "bs_format_fit_error_filters": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p,
                                               C.c_char_p, C.c_size_t]),
     "bs_peer_init": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32]),

@@ -517,14 +517,17 @@ struct bs_engine {
   // h_conflict, each node's used mask d_used [Npad]; dropped with the node table) and the pod side (each pod's want
   // mask h_want, want_all their OR; dropped with the pod table).  dirty: the used masks changed or the filter was
   // switched on, so the class fit bits are built again.  d_fconf: each fit class's conflict mask, d_bins the ports bin
-  // of each fit class, d_reasons the companion rows [P].
+  // of each fit class, d_reasons the companion rows [P].  The bound side (bs_upload_bound_host_ports; dropped with the
+  // bound-pod table): each bound row's mask h_bports in table order, d_bports / d_bsuf the masks in CSR order and their
+  // suffix OR; h_used keeps the node side's used masks for its checks.
   struct {
     bool on = false, round = false;
     DevBuf d_used, d_fconf, d_bins, d_reasons;
-    bool have_node = false, have_pod = false, dirty = true;
+    bool have_node = false, have_pod = false, dirty = true, have_bound = false;
     uint32_t entries = 0;
     uint64_t want_all = 0;
-    std::vector<uint64_t> h_conflict, h_want;
+    std::vector<uint64_t> h_conflict, h_want, h_used, h_bports;
+    DevBuf d_bstage, d_bports, d_bsuf, d_pconf;   // d_pconf: bs_preempt's per-preemptor conflict masks
   } hp;
   // The filters' share of the fit classes.  assign_dirty: the pods' fit classes have to be assigned again (with their
   // filter class and conflict mask while a filter is on, else their base class h_pfc_base).  d_gate: the priority
@@ -588,6 +591,7 @@ struct bs_engine {
   uint32_t V = 0;
   int32_t bound_max_gid = -1;
   std::vector<int32_t> h_bgid;        // by bound-table index: bs_remove_pod
+  std::vector<uint32_t> h_bnode;      // by bound-table index: the bound host-port checks
   std::vector<uint8_t> h_bflags;
   std::vector<int32_t> h_npc;         // node pod_count and req_present as uploaded (bound-table validation)
   std::vector<uint32_t> h_nrpres;
@@ -2020,7 +2024,7 @@ int bs_upload_nodes(bs_engine* e, const bs_node_table* t) {
   // or an error partway through the copy) leaves no snapshot behind, and the engine answers BS_E_STATE until a valid
   // one arrives instead of evaluating the previous snapshot (or a half-written one)
   e->have_nodes = false;
-  e->have_bound = false;   // the bound-pod table belongs to the node snapshot
+  e->have_bound = e->hp.have_bound = false;   // the bound-pod table belongs to the node snapshot
   if (e->n_aff) e->classes_dirty = true;   // class ids are validated again: the affinity table belongs to the
   e->n_aff = 0;                            // node snapshot and goes with it
   e->evaluated = false;
@@ -2077,7 +2081,7 @@ int bs_update_nodes(bs_engine* e, const uint32_t* idx, const bs_node_table* t) {
     e->h_npc[idx[k]] = t->pod_count[k];
     e->h_nrpres[idx[k]] = t->req_present[k];
   }
-  e->have_bound = false;
+  e->have_bound = e->hp.have_bound = false;
   e->nodes_dirty = true;
   e->evaluated = false;
   return BS_OK;
@@ -2095,7 +2099,7 @@ int bs_upload_groups(bs_engine* e, const bs_group_table* t) {
   BS_DEVICE_GUARD(e);
   HP_BEGIN(e);
   e->have_groups = false;
-  e->have_bound = false;   // the bound rows' group indices refer to the old table
+  e->have_bound = e->hp.have_bound = false;   // the bound rows' group indices refer to the old table
   e->evaluated = false;
   const uint32_t Gp = std::max(G, 1u);
   int rc;
@@ -3020,7 +3024,8 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
 // (upstream's metadata RemovePod).  The walks follow their own placements in live presence, which needs each pod's
 // placed class: without it they refuse as well.  Preemption refuses to run under the PodFitsHostPorts filter: its
 // victims' removal would have to take their ports out of the used masks (the walks follow their own placements in a
-// live copy of them).
+// live copy of them).  With the bound pods' host-port masks (bs_upload_bound_host_ports) it runs: see
+// host_port_preempt_check.
 static int interpod_filter_refuse(bs_engine* e, const char* who) {
   return fail(e, BS_E_INVAL, (std::string(who) + ": the MatchInterPodAffinity filter is not supported here; "
                               "switch it off with bs_set_interpod_filter").c_str());
@@ -3031,8 +3036,36 @@ static int interpod_placed_refuse(bs_engine* e, const char* who) {
                               "bs_set_interpod_filter").c_str());
 }
 static int host_port_refuse(bs_engine* e, const char* who) {
-  return fail(e, BS_E_INVAL, (std::string(who) + ": the PodFitsHostPorts filter is not supported here; "
-                              "switch it off with bs_set_host_port_filter").c_str());
+  return fail(e, BS_E_INVAL, (std::string(who) + ": the PodFitsHostPorts filter needs the bound pods' host ports in "
+                              "preemption; upload them with bs_upload_bound_host_ports or switch the filter off with "
+                              "bs_set_host_port_filter").c_str());
+}
+
+// bs_preempt and bs_preempt_walk under the PodFitsHostPorts filter: both sides of the filter as the round needs them,
+// and each bound row's bits entries of the node side's dictionary that its node uses (a NodeInfo's used ports include
+// its pods').  Then each preemptor's want and conflict masks.  The caller holds the engine's lock.
+static int host_port_preempt_check(bs_engine* e, const char* who, const uint32_t* pods, uint32_t n,
+                                   std::vector<uint64_t>& want, std::vector<uint64_t>& conf) {
+  if (int rc = host_port_check(e, who)) return rc;
+  const Refuse bad{e, who};
+  const std::vector<uint64_t>& bp = e->hp.h_bports;
+  uint64_t all = 0;
+  bool outside = false;
+  for (uint32_t v = 0; v < (uint32_t)bp.size(); ++v) {
+    all |= bp[v];
+    outside = outside || (bp[v] & ~e->hp.h_used[e->h_bnode[v]]) != 0;
+  }
+  if (e->hp.entries < 64 && (all >> e->hp.entries))
+    return bad(BS_E_INDEX, "a bound pod's host-port bit is outside the node side's dictionary");
+  if (outside) return bad(BS_E_INVAL, "a bound pod holds a host port its node's used mask does not have");
+  want.assign(std::max(n, 1u), 0);
+  conf.assign(std::max(n, 1u), 0);
+  for (uint32_t i = 0; i < n; ++i) {
+    if (pods[i] >= e->P) continue;   // preempt_pods refuses it
+    want[i] = e->hp.h_want[pods[i]];
+    for (uint64_t w = want[i]; w; w &= w - 1) conf[i] |= e->hp.h_conflict[__builtin_ctzll(w)];
+  }
+  return BS_OK;
 }
 
 int bs_replay(bs_engine* e, const uint32_t* queue, uint32_t n_queue, bs_replay_result* out) {
@@ -3068,7 +3101,7 @@ int bs_upload_bound_pods(bs_engine* e, const bs_bound_table* t) {
   const uint32_t V = t->n_pods, L = e->L, N = e->N;
   if (V && (!t->node || !t->req || !t->req_present || !t->gid || !t->priority || !t->start_ns || !t->flags))
     return fail(e, BS_E_INVAL, "bs_upload_bound_pods: null column");
-  e->have_bound = false;   // a failing table is dropped
+  e->have_bound = e->hp.have_bound = false;   // a failing table is dropped, and the host-port masks go with it
   // rows: node index, scalar keys within the node's, value range
   BoundStats bs = Chunks(V, 8192).reduce<BoundStats>([&](int, uint32_t a0, uint32_t a1, BoundStats& st) {
     for (uint32_t v = a0; v < a1; ++v) {
@@ -3172,6 +3205,7 @@ int bs_upload_bound_pods(bs_engine* e, const bs_bound_table* t) {
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(e->s));   // the host vectors die here
   e->h_bgid.assign(t->gid, t->gid + V);
+  e->h_bnode.assign(t->node, t->node + V);
   e->h_bflags.assign(t->flags, t->flags + V);
   e->V = V;
   e->bound_max_gid = bs.max_gid;
@@ -3225,9 +3259,12 @@ int bs_preempt(bs_engine* e, const uint32_t* pods, uint32_t n, bs_preempt_result
     return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
   if (e->ipf.on) return interpod_filter_refuse(e, "bs_preempt");
-  if (e->hp.on) return host_port_refuse(e, "bs_preempt");
+  const bool hp = e->hp.on;
+  if (hp && !e->hp.have_bound) return host_port_refuse(e, "bs_preempt");
   std::vector<PreemptPod> pp;
+  std::vector<uint64_t> want, conf;
   int rc;
+  if (hp && (rc = host_port_preempt_check(e, "bs_preempt", pods, n, want, conf))) return rc;
   if ((rc = preempt_pods(e, "bs_preempt", pods, n, pp))) return rc;
   const uint32_t L = e->L, N = e->N;
   out->victim_offset[0] = 0;
@@ -3240,7 +3277,17 @@ int bs_preempt(bs_engine* e, const uint32_t* pods, uint32_t n, bs_preempt_result
   CK(e->d_pcand.ensure((size_t)n * 4));
   CK(e->d_poff.ensure((size_t)n * 4));
   CK(cudaMemcpyAsync(e->d_pp.p, pp.data(), (size_t)n * sizeof(PreemptPod), cudaMemcpyHostToDevice, e->s));
-  PreemptArgs a = preempt_args(e, n);
+  PreemptHpArgs ha{};
+  PreemptArgs& a = ha;
+  a = preempt_args(e, n);
+  if (hp) {
+    CK(e->hp.d_pconf.ensure((size_t)n * 8));
+    CK(cudaMemcpyAsync(e->hp.d_pconf.p, conf.data(), (size_t)n * 8, cudaMemcpyHostToDevice, e->s));
+    ha.hp_used = e->hp.d_used.as<uint64_t>();
+    ha.hp_ports = e->hp.d_bports.as<uint64_t>();
+    ha.hp_suf = e->hp.d_bsuf.as<uint64_t>();
+    ha.hp_conf = e->hp.d_pconf.as<uint64_t>();
+  }
   a.out_node = e->d_pnode.as<int32_t>();
   a.out_nv = e->d_pnv.as<uint32_t>();
   a.out_cand = e->d_pcand.as<uint32_t>();
@@ -3258,7 +3305,8 @@ int bs_preempt(bs_engine* e, const uint32_t* pods, uint32_t n, bs_preempt_result
       const uint32_t cnt = std::min(chunk, n - p0);
       a.p0 = p0;
       with_maxl<5, 9, 16>(L, [&](auto M) {
-        preempt_node_kernel<M><<<dim3(a.n_tiles, cnt), PREEMPT_THREADS, 0, e->s>>>(a);
+        if (hp) preempt_node_kernel<M, true><<<dim3(a.n_tiles, cnt), PREEMPT_THREADS, 0, e->s>>>(ha);
+        else preempt_node_kernel<M, false><<<dim3(a.n_tiles, cnt), PREEMPT_THREADS, 0, e->s>>>(a);
       });
       preempt_reduce_kernel<<<cdiv(cnt, 256), 256, 0, e->s>>>(a, cnt);
       e->launches += 2;
@@ -3283,7 +3331,10 @@ int bs_preempt(bs_engine* e, const uint32_t* pods, uint32_t n, bs_preempt_result
   CK(cudaMemcpyAsync(e->d_poff.p, out->victim_offset, (size_t)n * 4, cudaMemcpyHostToDevice, e->s));
   a.offset = e->d_poff.as<uint32_t>();
   a.victims = e->d_pvict.as<uint32_t>();
-  with_maxl<5, 9, 16>(L, [&](auto M) { preempt_emit_kernel<M><<<dim3(cdiv(n, 256)), 256, 0, e->s>>>(a); });
+  with_maxl<5, 9, 16>(L, [&](auto M) {
+    if (hp) preempt_emit_kernel<M, true><<<dim3(cdiv(n, 256)), 256, 0, e->s>>>(ha);
+    else preempt_emit_kernel<M, false><<<dim3(cdiv(n, 256)), 256, 0, e->s>>>(a);
+  });
   ++e->launches;
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(out->victims, a.victims, (size_t)total * 4, cudaMemcpyDeviceToHost, e->s));
@@ -3297,11 +3348,14 @@ int bs_preempt_walk(bs_engine* e, const uint32_t* pods, uint32_t n, uint32_t fla
     return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
   if (e->ipf.on) return interpod_filter_refuse(e, "bs_preempt_walk");
-  if (e->hp.on) return host_port_refuse(e, "bs_preempt_walk");
+  const bool hp = e->hp.on;
+  if (hp && !e->hp.have_bound) return host_port_refuse(e, "bs_preempt_walk");
   if (flags & ~BS_PREEMPT_GANG) return fail(e, BS_E_INVAL, "bs_preempt_walk: unknown flag bits");
   const bool gang = flags & BS_PREEMPT_GANG;
   std::vector<PreemptPod> pp;
+  std::vector<uint64_t> want, conf;
   int rc;
+  if (hp && (rc = host_port_preempt_check(e, "bs_preempt_walk", pods, n, want, conf))) return rc;
   if ((rc = preempt_pods(e, "bs_preempt_walk", pods, n, pp))) return rc;
   // queue order: every earlier nomination has a priority >= the current preemptor's, so all of them count
   // (addNominatedPods) and none is ever cleared (getLowerPriorityNominatedPods)
@@ -3334,11 +3388,14 @@ int bs_preempt_walk(bs_engine* e, const uint32_t* pods, uint32_t n, uint32_t fla
   out->victims_total = 0;
   if (!n) return BS_OK;
   BS_DEVICE_GUARD(e);
-  PreemptArgs a = preempt_args(e, n);
-  const size_t g_n = gang ? n : 0, g_v = gang ? Vp : 0;
+  PreemptHpArgs ha{};
+  PreemptArgs& a = ha;
+  a = preempt_args(e, n);
+  const size_t g_n = gang ? n : 0, g_v = gang ? Vp : 0, h_n = hp ? n : 0, h_v = hp ? Vp : 0;
   View w_pp, w_node, w_nv, w_cand, w_outcome, w_last, w_tiles, w_vict, w_ctl, w_end, w_prio, w_start, w_gid, w_flags,
       w_idx, w_req, w_suf, w_son, w_sbad, w_svio, w_requested, w_rp, w_pc, w_left, w_lp, w_evby, e_node, e_end, e_nv,
-      e_row, e_req, e_rp, e_pc, r_pos, r_prio, r_start, r_gid, r_flags, r_idx, r_req;
+      e_row, e_req, e_rp, e_pc, r_pos, r_prio, r_start, r_gid, r_flags, r_idx, r_req, h_conf, h_want, h_used, h_nom,
+      h_ports, h_suf, he_used, he_nom, hr_ports;
   CK(carve(e->d_walk,
            {{&w_pp, (size_t)n * sizeof(PreemptPod)}, {&w_node, (size_t)n * 4}, {&w_nv, (size_t)n * 4},
             {&w_cand, (size_t)n * 4}, {&w_outcome, (size_t)n * 4}, {&w_last, n}, {&w_tiles, a.n_tiles * sizeof(PickKey)},
@@ -3350,7 +3407,10 @@ int bs_preempt_walk(bs_engine* e, const uint32_t* pods, uint32_t n, uint32_t fla
             {&w_lp, (size_t)Npad * 4}, {&w_evby, (size_t)Vp * 4}, {&e_node, g_n * 4}, {&e_end, g_n * 4},
             {&e_nv, g_n * 4}, {&e_row, g_n * 4}, {&e_req, L * g_n * 8}, {&e_rp, g_n * 4}, {&e_pc, g_n * 4},
             {&r_pos, g_v * 4}, {&r_prio, g_v * 4}, {&r_start, g_v * 8}, {&r_gid, g_v * 4}, {&r_flags, g_v},
-            {&r_idx, g_v * 4}, {&r_req, L * g_v * 8}}));
+            {&r_idx, g_v * 4}, {&r_req, L * g_v * 8}, {&h_conf, h_n * 8}, {&h_want, h_n * 8},
+            {&h_used, hp ? (size_t)Npad * 8 : 0}, {&h_nom, hp ? (size_t)Npad * 8 : 0}, {&h_ports, h_v * 8},
+            {&h_suf, h_v * 8}, {&he_used, hp ? g_n * 8 : 0}, {&he_nom, hp ? g_n * 8 : 0},
+            {&hr_ports, hp ? g_v * 8 : 0}}));
   auto dup = [&](const View& dst, const void* src, size_t bytes) {
     return bytes ? cudaMemcpyAsync(dst.p, src, bytes, cudaMemcpyDeviceToDevice, e->s) : cudaSuccess;
   };
@@ -3374,7 +3434,8 @@ int bs_preempt_walk(bs_engine* e, const uint32_t* pods, uint32_t n, uint32_t fla
   CK(dup(w_pc, e->d_pod_count.p, (size_t)Npad * 4));
   CK(dup(w_left, e->d_pl_left.p, (size_t)L * Npad * 8));
   CK(dup(w_lp, e->d_pl_present.p, (size_t)Npad * 4));
-  WalkArgs w{};
+  WalkHpArgs hw{};
+  WalkArgs& w = hw;
   w.end = w_end.as<uint32_t>();
   w.prio = w_prio.as<int32_t>();
   w.start = w_start.as<int64_t>();
@@ -3421,6 +3482,29 @@ int bs_preempt_walk(bs_engine* e, const uint32_t* pods, uint32_t n, uint32_t fla
   a.b = BoundTab{a.b.row, w.end, w.prio, w.start, w.gid, w.flags, w.idx, w.req, w.suf, w.suf_online, w.suf_bad,
                  w.suf_vio, Vp};
   a.pp = w_pp.as<PreemptPod>();
+  if (hp) {   // the live masks: the bound ones start as the node side's, the nominated ones empty
+    CK(cudaMemcpyAsync(h_conf.p, conf.data(), (size_t)n * 8, cudaMemcpyHostToDevice, e->s));
+    CK(cudaMemcpyAsync(h_want.p, want.data(), (size_t)n * 8, cudaMemcpyHostToDevice, e->s));
+    CK(dup(h_used, e->hp.d_used.p, (size_t)Npad * 8));
+    CK(cudaMemsetAsync(h_nom.p, 0, (size_t)Npad * 8, e->s));
+    CK(dup(h_ports, e->hp.d_bports.p, (size_t)Vp * 8));
+    CK(dup(h_suf, e->hp.d_bsuf.p, (size_t)Vp * 8));
+    hw.used = h_used.as<uint64_t>();
+    hw.nom = h_nom.as<uint64_t>();
+    hw.ports = h_ports.as<uint64_t>();
+    hw.suf_ports = h_suf.as<uint64_t>();
+    if (gang) {
+      hw.ent_used = he_used.as<uint64_t>();
+      hw.ent_nom = he_nom.as<uint64_t>();
+      hw.row_ports = hr_ports.as<uint64_t>();
+    }
+    ha.hp_used = hw.used;
+    ha.hp_nom = hw.nom;
+    ha.hp_ports = hw.ports;
+    ha.hp_suf = hw.suf_ports;
+    ha.hp_conf = h_conf.as<uint64_t>();
+    ha.hp_want = h_want.as<uint64_t>();
+  }
   a.tiles = w_tiles.as<PickKey>();
   a.out_node = w_node.as<int32_t>();
   a.out_nv = w_nv.as<uint32_t>();
@@ -3430,11 +3514,15 @@ int bs_preempt_walk(bs_engine* e, const uint32_t* pods, uint32_t n, uint32_t fla
     if (N) {
       a.p0 = i;
       with_maxl<5, 9, 16>(L, [&](auto M) {
-        preempt_node_kernel<M><<<dim3(a.n_tiles, 1), PREEMPT_THREADS, 0, e->s>>>(a);
+        if (hp) preempt_node_kernel<M, true><<<dim3(a.n_tiles, 1), PREEMPT_THREADS, 0, e->s>>>(ha);
+        else preempt_node_kernel<M, false><<<dim3(a.n_tiles, 1), PREEMPT_THREADS, 0, e->s>>>(a);
       });
       ++e->launches;
     }
-    with_maxl<5, 9, 16>(L, [&](auto M) { preempt_commit_kernel<M><<<1, PREEMPT_THREADS, 0, e->s>>>(a, w, i); });
+    with_maxl<5, 9, 16>(L, [&](auto M) {
+      if (hp) preempt_commit_kernel<M, true><<<1, PREEMPT_THREADS, 0, e->s>>>(ha, hw, i);
+      else preempt_commit_kernel<M, false><<<1, PREEMPT_THREADS, 0, e->s>>>(a, w, i);
+    });
     ++e->launches;
   }
   CK(cudaGetLastError());
@@ -4200,6 +4288,7 @@ int bs_upload_node_host_ports(bs_engine* e, const bs_host_port_nodes* t) {
   if (int rc = upload_vec(e, e->hp.d_used, t->used, N, e->Npad)) return rc;
   CK(cudaStreamSynchronize(e->s));
   e->hp.h_conflict = std::move(conflict);
+  e->hp.h_used.assign(t->used, t->used + N);
   e->hp.h_conflict.resize(BS_HOSTPORT_MAX, 0);   // want bits past n_entries are refused at evaluation
   e->hp.entries = K;
   e->hp.have_node = true;
@@ -4223,6 +4312,33 @@ int bs_upload_pod_host_ports(bs_engine* e, uint32_t n_pods, const uint64_t* want
   e->hp.have_pod = true;
   e->filt.assign_dirty = e->classes_dirty = e->pod_classes_dirty = true;   // the pods' fit classes carry the mask
   e->evaluated = false;
+  return BS_OK;
+}
+
+int bs_upload_bound_host_ports(bs_engine* e, uint32_t n_pods, const uint64_t* ports) {
+  if (!e) return BS_E_INVAL;
+  std::lock_guard<std::mutex> lk(e->mu);
+  const Refuse bad{e, "bs_upload_bound_host_ports"};
+  e->hp.have_bound = false;
+  if (!e->have_bound) return bad(BS_E_STATE, "upload the bound-pod table first");
+  if (n_pods != e->V) return bad(BS_E_INVAL, "n_pods differs from the bound-pod table's");
+  if (n_pods && !ports) return bad(BS_E_INVAL, "null ports");
+  // the bits are checked against the node side when a preemption starts: the sides may come in any order
+  const uint32_t V = e->V, N = e->N, Vp = std::max(V, 1u);
+  BS_DEVICE_GUARD(e);
+  if (int rc = upload_vec(e, e->hp.d_bstage, ports, V, Vp)) return rc;   // table order
+  CK(e->hp.d_bports.ensure((size_t)Vp * 8));
+  CK(e->hp.d_bsuf.ensure((size_t)Vp * 8));
+  if (N) {
+    preempt_ports_prep_kernel<<<cdiv(N, 256), 256, 0, e->s>>>(e->d_brow.as<uint32_t>(), e->d_bidx.as<uint32_t>(),
+                                                             e->hp.d_bstage.as<uint64_t>(), e->hp.d_bports.as<uint64_t>(),
+                                                             e->hp.d_bsuf.as<uint64_t>(), N);
+    ++e->launches;
+  }
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(e->s));
+  e->hp.h_bports.assign(ports, ports + V);
+  e->hp.have_bound = true;
   return BS_OK;
 }
 

@@ -2113,6 +2113,11 @@ void BatchSchedulingPlugin::SetHostPortFilter(bool on) {
   host_port_filter_ = on;
 }
 
+void BatchSchedulingPlugin::SetHostPortFilterInPreemption(bool on) {
+  std::lock_guard<std::mutex> lk(mu_);
+  host_port_preempt_ = on;
+}
+
 namespace {
 struct HostPortTriple {
   std::string ip, protocol;
@@ -2134,7 +2139,7 @@ bool triples_conflict(const HostPortTriple& a, const HostPortTriple& b) {
 }  // namespace
 
 Status BatchSchedulingPlugin::PackHostPorts(const std::vector<const NodeInfo*>& snapshot,
-                                            const std::vector<const Pod*>& pending, PackedHostPorts* out) {
+                                            const std::vector<const Pod*>& pending, PackedHostPorts* out, bool bound) {
   if (!out) return Status{BS_CODE_ERROR, "PackHostPorts: null output"};
   *out = PackedHostPorts{};
   std::vector<HostPortTriple> dict;
@@ -2180,6 +2185,17 @@ Status BatchSchedulingPlugin::PackHostPorts(const std::vector<const NodeInfo*>& 
   };
   for (const auto& ts : used) out->used.push_back(mask(ts));
   for (const auto& ts : wanted) out->want.push_back(mask(ts));
+  if (bound) {   // PackBoundPods' rows: the snapshot's NodeInfo::pods in order
+    std::vector<HostPortTriple> held;
+    for (const NodeInfo* ni : snapshot)
+      if (ni)
+        for (const Pod* p : ni->pods) {
+          if (!p) continue;
+          held.clear();
+          for (const Container& c : p->containers) add_triples(c.ports, &held);
+          out->bound.push_back(mask(held));
+        }
+  }
   return Status{};
 }
 
@@ -2198,6 +2214,18 @@ Status BatchSchedulingPlugin::UploadHostPorts() {
   rc = bs_upload_node_host_ports(eng_, &nt);
   if (!rc) rc = bs_upload_pod_host_ports(eng_, (uint32_t)pending_.size(), pk.want.data());
   return rc ? fail(rc) : Status{};
+}
+
+// Called right after every bound-table upload.  PackHostPorts numbers the dictionary from snapshot_ and pending_ alone,
+// so the masks agree with the node and pod sides UploadHostPorts uploads in the same round or UpdateNodes.
+Status BatchSchedulingPlugin::UploadBoundHostPorts() {
+  if (!host_port_filter_ || !host_port_preempt_ || !bound_.n) return Status{};
+  PackedHostPorts pk;
+  Status st = PackHostPorts(snapshot_, pending_, &pk, true);
+  if (!st.ok()) return st;
+  const int rc = bs_upload_bound_host_ports(eng_, (uint32_t)pk.bound.size(), pk.bound.data());
+  if (rc) return Status{BS_CODE_ERROR, std::string("bsched: ") + bs_strerror(rc) + " (" + bs_last_error(eng_) + ")"};
+  return Status{};
 }
 
 std::vector<uint32_t> BatchSchedulingPlugin::HostPortReasonCounts(const std::string& uid) const {
@@ -2506,7 +2534,7 @@ Status BatchSchedulingPlugin::UploadBound() {
   const bs_bound_table t = bound_.table();
   const int rc = bs_upload_bound_pods(eng_, &t);
   if (rc) return Status{BS_CODE_ERROR, std::string("bsched: ") + bs_strerror(rc) + " (" + bs_last_error(eng_) + ")"};
-  return Status{};
+  return UploadBoundHostPorts();   // the masks belong to the table just uploaded
 }
 
 Status BatchSchedulingPlugin::RemovePod(const Pod& preemptor, const Pod& victim) {
@@ -2558,7 +2586,7 @@ Status BatchSchedulingPlugin::Preempt(const std::string& uid, std::string* node,
   std::lock_guard<std::mutex> lk(mu_);
   if (interpod_filter_)
     return Status{BS_CODE_ERROR, "Preempt: the MatchInterPodAffinity filter is on (SetInterPodAffinityFilter(false) first)"};
-  if (host_port_filter_)
+  if (host_port_filter_ && !host_port_preempt_)
     return Status{BS_CODE_ERROR, "Preempt: the PodFitsHostPorts filter is on (SetHostPortFilter(false) first)"};
   const int32_t p = pod_row_.find(uid);
   if (!eng_ || p < 0) return Status{BS_CODE_ERROR, "Preempt: " + uid + " is not a pending pod of the round"};
@@ -2580,7 +2608,7 @@ Status BatchSchedulingPlugin::PreemptAll(std::vector<Preemption>* out) {
   if (!eng_ || !out) return Status{BS_CODE_ERROR, "PreemptAll: no round has been started"};
   if (interpod_filter_)
     return Status{BS_CODE_ERROR, "PreemptAll: the MatchInterPodAffinity filter is on (SetInterPodAffinityFilter(false) first)"};
-  if (host_port_filter_)
+  if (host_port_filter_ && !host_port_preempt_)
     return Status{BS_CODE_ERROR, "PreemptAll: the PodFitsHostPorts filter is on (SetHostPortFilter(false) first)"};
   out->clear();
   if (!bound_.n) return Status{};
@@ -2599,7 +2627,7 @@ Status BatchSchedulingPlugin::PreemptQueue(std::vector<Preemption>* out, bool ga
   if (!eng_ || !out) return Status{BS_CODE_ERROR, "PreemptQueue: no round has been started"};
   if (interpod_filter_)
     return Status{BS_CODE_ERROR, "PreemptQueue: the MatchInterPodAffinity filter is on (SetInterPodAffinityFilter(false) first)"};
-  if (host_port_filter_)
+  if (host_port_filter_ && !host_port_preempt_)
     return Status{BS_CODE_ERROR, "PreemptQueue: the PodFitsHostPorts filter is on (SetHostPortFilter(false) first)"};
   out->clear();
   if (!bound_.n) return Status{};

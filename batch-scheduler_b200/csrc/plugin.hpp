@@ -329,12 +329,13 @@ struct PackedInterPodAffinity {
 // pod's class of (term, role) with its self_match byte.
 // The columns of the PodFitsHostPorts filter of one round (bs_upload_node_host_ports, bs_upload_pod_host_ports): the
 // dictionary (ip id, protocol id, port; ip id 0 = "0.0.0.0", the other ips and the protocols numbered by first
-// appearance), each node's used mask and each pending pod's want mask.
+// appearance), each node's used mask and each pending pod's want mask; with bound, each bound pod's mask too.
 struct PackedHostPorts {
   std::vector<uint32_t> ip, protocol;
   std::vector<int32_t> port;
   std::vector<uint64_t> used;   // [n_nodes]
   std::vector<uint64_t> want;   // [n_pods]
+  std::vector<uint64_t> bound;  // [bound pods] NodeInfo::pods in PackBoundPods' row order (bs_upload_bound_host_ports)
   std::vector<std::string> ips{"0.0.0.0"}, protocols;   // id -> text
 };
 struct PackedInterPodFilter {
@@ -560,8 +561,15 @@ class BatchSchedulingPlugin {
   void SetInterPodAffinityFilterInWalks(bool on);
   // kube-scheduler v1.17's PodFitsHostPorts filter in every pod's fit set and in ReplayQueue (bs_set_host_port_filter;
   // off by default), from the next round, delta round or UpdateNodes on: PackHostPorts' columns are uploaded with each
-  // of them.  While it is on, Preempt, PreemptAll and PreemptQueue return an error.
+  // of them.  While it is on, Preempt, PreemptAll and PreemptQueue return an error unless
+  // SetHostPortFilterInPreemption is on too.
   void SetHostPortFilter(bool on);
+  // the PodFitsHostPorts filter in preemption as well (off by default): while this and the filter are on, every upload
+  // of the bound-pod table and of the filter's sides is followed by the bound pods' host-port masks
+  // (PackHostPorts(..., bound = true), bs_upload_bound_host_ports), from the next round, delta round or UpdateNodes
+  // on, and Preempt, PreemptAll and PreemptQueue run under the filter.  Off, the rounds pack and upload what they did
+  // before and the three calls refuse under the filter.
+  void SetHostPortFilterInPreemption(bool on);
   // the last round's host-port companion count of a pending pod (bs_fetch_host_port_reason_rows); empty without
   // BS_OUT_REASONS, while the filter is off or for an unknown uid
   std::vector<uint32_t> HostPortReasonCounts(const std::string& uid) const;
@@ -700,9 +708,11 @@ class BatchSchedulingPlugin {
   // PodFitsHostPorts' columns: HostPortInfo's sanitizing (port <= 0 dropped, "" ip = "0.0.0.0", "" protocol = "TCP");
   // the dictionary holds the pending pods' wanted (ip, protocol, port) in order of first appearance, then the nodes'
   // used ones that conflict with one of them (a used entry that conflicts with nothing wanted never decides a verdict).
-  // More than BS_HOSTPORT_MAX entries is an error.
+  // More than BS_HOSTPORT_MAX entries is an error.  bound: also each NodeInfo::pods row's mask from its
+  // Container::ports, sanitized the same way, with the bit of the dictionary entry each port equals (a port in no
+  // entry conflicts with no pending pod and is left out).
   static Status PackHostPorts(const std::vector<const NodeInfo*>& snapshot, const std::vector<const Pod*>& pending,
-                              PackedHostPorts* out);
+                              PackedHostPorts* out, bool bound = false);
 
   static Status Pack(const std::vector<const NodeInfo*>& snapshot, const std::vector<const Pod*>& pending,
                      const std::vector<PodGroup>& groups, const std::vector<uint32_t>& matched,
@@ -741,6 +751,7 @@ class BatchSchedulingPlugin {
   bool interpod_filter_ = false;                        // SetInterPodAffinityFilter
   bool interpod_filter_walks_ = false;                  // SetInterPodAffinityFilterInWalks
   bool host_port_filter_ = false;                       // SetHostPortFilter
+  bool host_port_preempt_ = false;                      // SetHostPortFilterInPreemption
   std::string init_error_;
   int64_t max_schedule_time_ns_;
   std::map<std::string, GroupState> groups_;                        // ordered: canonical table order
@@ -782,6 +793,7 @@ class BatchSchedulingPlugin {
                                     // only while the weight is non-zero; no-op without priority_k
   Status UploadInterPodFilter();   // the filter switch and, while it is on, both filter sides of snapshot_ and pending_
   Status UploadHostPorts();        // likewise for the PodFitsHostPorts filter
+  Status UploadBoundHostPorts();   // the bound pods' host-port masks while the filter is on in preemption
   Status UploadLocality();   // both locality sides of snapshot_ and pending_ and the two weights; the columns only
                              // while a weight is non-zero; no-op without priority_k
   Status UploadBound();  // packs and uploads the bound-pod table of snapshot_ (no-op when no NodeInfo lists pods)

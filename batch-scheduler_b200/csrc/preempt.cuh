@@ -10,6 +10,13 @@
 // hot kernel answers "all victims removed" with one binary search and one suffix read per (preemptor, node) and walks
 // the suffix only for the pairs that survive that test.  The oracles in the tests mutate a copy of the node instead:
 // the two must agree.
+//
+// Under the PodFitsHostPorts filter (the HP builds) each CSR position also carries its row's host-port mask and the
+// suffix OR of those masks.  Removing every potential victim is a set delete on the node's used mask
+// (HostPortInfo.Remove: an entry goes even when a more important row lists it too): base = used & ~suf_ports[s].  The
+// node is a candidate when (base | nominated) holds no entry the preemptor conflicts with.  Since neither side of that
+// OR conflicts afterwards, re-adding row k in the reprieve conflicts exactly when the row's own mask does: a row holding
+// a conflicting port is always a victim.
 #pragma once
 #include "kernels.cuh"
 
@@ -118,6 +125,26 @@ __global__ void preempt_prep_kernel(const uint32_t* __restrict__ row, const int3
   prep_node(row[n], row[n + 1], gid, flags, req, suf, suf_online, suf_bad, suf_vio, V, L);
 }
 
+// The suffix OR of the host-port masks of one node's segment [b, e).
+__device__ __forceinline__ void prep_node_ports(uint32_t b, uint32_t e, const uint64_t* ports, uint64_t* suf_ports) {
+  uint64_t m = 0;
+  for (uint32_t k = e; k-- > b;) {
+    m |= ports[k];
+    suf_ports[k] = m;
+  }
+}
+
+// preempt_ports_prep_kernel — once per bound host-port upload, one thread per node: the masks into CSR order (by_row
+// is in bound-table order) and their suffix OR.
+__global__ void preempt_ports_prep_kernel(const uint32_t* __restrict__ row, const uint32_t* __restrict__ idx,
+                                          const uint64_t* __restrict__ by_row, uint64_t* __restrict__ ports,
+                                          uint64_t* __restrict__ suf_ports, uint32_t N) {
+  const uint32_t n = blockIdx.x * blockDim.x + threadIdx.x;
+  if (n >= N) return;
+  for (uint32_t k = row[n]; k < row[n + 1]; ++k) ports[k] = by_row[idx[k]];
+  prep_node_ports(row[n], row[n + 1], ports, suf_ports);
+}
+
 struct PreemptArgs {
   NodeTab t;                  // node table (guards, masks, affinity bits, requested lane 3)
   const int64_t* left;        // [L][Npad] node_left_kernel's full-width residuals at percent 1.0 (0 = key absent)
@@ -137,6 +164,24 @@ struct PreemptArgs {
   const uint32_t* offset;     // [n] exclusive scan of out_nv (emit)
   uint32_t* victims;          // emit output
 };
+// HP's arguments: a derived type, so that the kernels without the filter keep theirs
+struct PreemptHpArgs : PreemptArgs {
+  const uint64_t* hp_used;    // [Npad] the bound pods' used masks (bs_preempt_walk: live, evictions delete from it)
+  const uint64_t* hp_nom;     // [Npad] the nominated pods' want masks (bs_preempt_walk), null in bs_preempt
+  const uint64_t* hp_ports;   // [V] each CSR position's host-port mask
+  const uint64_t* hp_suf;     // [V] OR of hp_ports over positions k .. end of the segment
+  const uint64_t* hp_conf;    // [n] each preemptor's conflict mask (the OR of its wanted entries')
+  const uint64_t* hp_want;    // [n] each preemptor's want mask (bs_preempt_walk's nominations)
+};
+template <bool HP>
+using PreemptArgsOf = std::conditional_t<HP, PreemptHpArgs, PreemptArgs>;
+
+// preemptor slot i's conflict mask, 0 without the filter
+template <bool HP>
+__device__ __forceinline__ uint64_t hp_conf_of(const PreemptArgsOf<HP>& a, uint32_t i) {
+  if constexpr (HP) return a.hp_conf[i];
+  else return 0;
+}
 
 constexpr int PREEMPT_THREADS = 256;   // nodes per tile of the hot kernel
 
@@ -163,10 +208,11 @@ struct BoolC {
 // selectVictimsOnNode for preemptor slot i on node n.  Returns false when the node is not a candidate; else the
 // key of the node, and with EMIT the victims' bound-table indices at out[0..): the PDB-violating victims first, then
 // the others, each part in MoreImportantPod order (filterPodsWithPDBViolation splits the potential victims and the
-// violating ones are reprieved first).
-template <int MAXL, bool EMIT>
-__device__ bool select_victims(const PreemptArgs& a, const PreemptPod& q, const int64_t* req, uint32_t rpres,
-                               uint32_t n, PickKey& key, uint32_t* out) {
+// violating ones are reprieved first).  HP: under the PodFitsHostPorts filter, with conf the preemptor's conflict mask
+// (the header's rule: the node's used mask after the set delete, and each reprieved row's own mask).
+template <int MAXL, bool EMIT, bool HP>
+__device__ bool select_victims(const PreemptArgsOf<HP>& a, const PreemptPod& q, const int64_t* req, uint32_t rpres,
+                               uint32_t n, PickKey& key, uint32_t* out, uint64_t conf) {
   const NodeTab& t = a.t;
   const uint8_t f = t.flags[n];
   // the gate: the pod's fit-class bit (guards core.go:606-617 and :639, checkFit :741-759, absent-key rule :688-690)
@@ -190,6 +236,11 @@ __device__ bool select_victims(const PreemptArgs& a, const PreemptPod& q, const 
     if (offline && q.gid >= 0)
       for (uint32_t k = s; k < end; ++k)
         if (a.b.gid[k] == q.gid) return false;
+  }
+  if constexpr (HP) {   // every potential victim's ports leave; the nominated pods' stay
+    const uint64_t nom = a.hp_nom ? a.hp_nom[n] : 0ull;
+    const uint64_t base = a.hp_used[n] & ~(s < end ? a.hp_suf[s] : 0ull);
+    if ((base | nom) & conf) return false;
   }
   const uint32_t cmask = 0x7u | (rpres & a.left_present[n] & ~0xFu);
   const bool pods_by_count = t.requested[(size_t)LANE_PODS * t.Npad + n] == 0;
@@ -217,7 +268,13 @@ __device__ bool select_victims(const PreemptArgs& a, const PreemptPod& q, const 
     for (int d = 0; d < MAXL; ++d)
       if (d < (int)t.L) freed[d] -= a.b.req[(size_t)d * a.b.V + k];
     --removed;
-    if (fits_freed<MAXL>(left, freed, req, cmask, pods_left + (pods_by_count ? removed : 0), pods_req)) return;
+    if constexpr (HP) {
+      if (fits_freed<MAXL>(left, freed, req, cmask, pods_left + (pods_by_count ? removed : 0), pods_req) &&
+          (a.hp_ports[k] & conf) == 0)
+        return;
+    } else {
+      if (fits_freed<MAXL>(left, freed, req, cmask, pods_left + (pods_by_count ? removed : 0), pods_req)) return;
+    }
 #pragma unroll
     for (int d = 0; d < MAXL; ++d)
       if (d < (int)t.L) freed[d] += a.b.req[(size_t)d * a.b.V + k];
@@ -282,15 +339,16 @@ __device__ __forceinline__ PickKey block_pick_min(PickKey key) {
 // writes the tile's best key (and its candidate count).  The key is a total order (the node index decides last),
 // so the tree below gives the same winner as a walk in node order.  At MAXL 5 the bound holds 64 registers, four
 // blocks per SM, without spills (the PDB pass would otherwise take it to 72 and three blocks).
-template <int MAXL>
-__global__ void __launch_bounds__(PREEMPT_THREADS, MAXL <= 5 ? 4 : 1) preempt_node_kernel(PreemptArgs a) {
+template <int MAXL, bool HP>
+__global__ void __launch_bounds__(PREEMPT_THREADS, MAXL <= 5 ? 4 : 1) preempt_node_kernel(PreemptArgsOf<HP> a) {
   const uint32_t i = a.p0 + blockIdx.y;
   const uint32_t n = blockIdx.x * PREEMPT_THREADS + threadIdx.x;
   const PreemptPod q = a.pp[i];
   int64_t req[MAXL];
   const uint32_t rpres = load_req<MAXL>(a, q, req);
+  const uint64_t conf = hp_conf_of<HP>(a, i);
   PickKey key = pick_none();
-  if (n < a.t.N && !select_victims<MAXL, false>(a, q, req, rpres, n, key, nullptr)) key = pick_none();
+  if (n < a.t.N && !select_victims<MAXL, false, HP>(a, q, req, rpres, n, key, nullptr, conf)) key = pick_none();
   key = block_pick_min(key);
   if (threadIdx.x == 0) a.tiles[(size_t)blockIdx.y * a.n_tiles + blockIdx.x] = key;
 }
@@ -308,8 +366,8 @@ __global__ void preempt_reduce_kernel(PreemptArgs a, uint32_t count) {
 }
 
 // preempt_emit_kernel — one thread per preemptor with a node: the reprieve again on that node, writing the victims
-template <int MAXL>
-__global__ void preempt_emit_kernel(PreemptArgs a) {
+template <int MAXL, bool HP>
+__global__ void preempt_emit_kernel(PreemptArgsOf<HP> a) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= a.n) return;
   const int32_t n = a.out_node[i];
@@ -318,7 +376,7 @@ __global__ void preempt_emit_kernel(PreemptArgs a) {
   int64_t req[MAXL];
   const uint32_t rpres = load_req<MAXL>(a, q, req);
   PickKey key;
-  select_victims<MAXL, true>(a, q, req, rpres, (uint32_t)n, key, a.victims + a.offset[i]);
+  select_victims<MAXL, true, HP>(a, q, req, rpres, (uint32_t)n, key, a.victims + a.offset[i], hp_conf_of<HP>(a, i));
 }
 
 // ---------------------------------------------------------------------------
@@ -376,6 +434,17 @@ struct WalkArgs {
   int64_t* row_req;         // [L][V]
   uint32_t n;
 };
+// HP's live state and its share of the undo log: derived, so that the kernels without the filter keep theirs
+struct WalkHpArgs : WalkArgs {
+  uint64_t* used;           // [Npad] the bound pods' used masks (PreemptHpArgs::hp_used): evictions set-delete
+  uint64_t* nom;            // [Npad] the nominated pods' want masks (PreemptHpArgs::hp_nom): nominations OR in
+  uint64_t* ports;          // [V] each live CSR position's mask (PreemptHpArgs::hp_ports)
+  uint64_t* suf_ports;      // [V] their suffix OR (PreemptHpArgs::hp_suf)
+  uint64_t *ent_used, *ent_nom;   // [n] per commit: the node's two masks before it
+  uint64_t* row_ports;      // [V] per logged row: its mask
+};
+template <bool HP>
+using WalkArgsOf = std::conditional_t<HP, WalkHpArgs, WalkArgs>;
 
 // Rebuilds node n's suffixes and residuals from its live segment and its live requested / req_present / pod_count.
 __device__ __forceinline__ void walk_refresh_node(const PreemptArgs& a, const WalkArgs& w, uint32_t n) {
@@ -392,8 +461,9 @@ __device__ __forceinline__ void walk_refresh_node(const PreemptArgs& a, const Wa
 
 // Step i's pick, victims, eviction and nomination, and at the end of a failed unit its undo.  One CTA; the tiles of
 // preempt_node_kernel are reduced by the whole block, the rest runs on thread 0 (one node's segment).
-template <int MAXL>
-__global__ void __launch_bounds__(PREEMPT_THREADS) preempt_commit_kernel(PreemptArgs a, WalkArgs w, uint32_t i) {
+template <int MAXL, bool HP>
+__global__ void __launch_bounds__(PREEMPT_THREADS) preempt_commit_kernel(PreemptArgsOf<HP> a, WalkArgsOf<HP> w,
+                                                                         uint32_t i) {
   PickKey key = pick_none();
   for (uint32_t tl = threadIdx.x; tl < a.n_tiles; tl += PREEMPT_THREADS) key = pick_min(key, a.tiles[tl]);
   key = block_pick_min(key);
@@ -413,7 +483,7 @@ __global__ void __launch_bounds__(PREEMPT_THREADS) preempt_commit_kernel(Preempt
     const uint32_t rpres = load_req<MAXL>(a, q, req);
     uint32_t* vict = a.victims + c.voff;
     PickKey k2;
-    select_victims<MAXL, true>(a, q, req, rpres, n, k2, vict);
+    select_victims<MAXL, true, HP>(a, q, req, rpres, n, k2, vict, hp_conf_of<HP>(a, i));
     const uint32_t nv = k2.nv;
     a.out_node[i] = (int32_t)n;
     a.out_nv[i] = nv;
@@ -430,12 +500,17 @@ __global__ void __launch_bounds__(PREEMPT_THREADS) preempt_commit_kernel(Preempt
       for (uint32_t d = 0; d < L; ++d) w.ent_req[(size_t)d * w.n + e] = w.requested[(size_t)d * Npad + n];
       w.ent_rp[e] = w.req_present[n];
       w.ent_pc[e] = w.pod_count[n];
+      if constexpr (HP) {
+        w.ent_used[e] = w.used[n];
+        w.ent_nom[e] = w.nom[n];
+      }
     }
     // evict: the victims leave the segment (order kept) and NodeInfo.RemovePod takes their Requests
     uint32_t dst = beg;
     for (uint32_t k = beg; k < end; ++k) {
       if (w.evicted_by[w.idx[k]] == (int32_t)i) {
         for (uint32_t d = 0; d < L; ++d) w.requested[(size_t)d * Npad + n] -= w.req[(size_t)d * V + k];
+        if constexpr (HP) w.used[n] &= ~w.ports[k];   // HostPortInfo.Remove: a set delete
         if (w.ent_node) {
           const uint32_t r = c.n_rows++;
           w.row_pos[r] = k - beg;
@@ -445,6 +520,7 @@ __global__ void __launch_bounds__(PREEMPT_THREADS) preempt_commit_kernel(Preempt
           w.row_flags[r] = w.flags[k];
           w.row_idx[r] = w.idx[k];
           for (uint32_t d = 0; d < L; ++d) w.row_req[(size_t)d * V + r] = w.req[(size_t)d * V + k];
+          if constexpr (HP) w.row_ports[r] = w.ports[k];
         }
         continue;
       }
@@ -455,6 +531,7 @@ __global__ void __launch_bounds__(PREEMPT_THREADS) preempt_commit_kernel(Preempt
         w.flags[dst] = w.flags[k];
         w.idx[dst] = w.idx[k];
         for (uint32_t d = 0; d < L; ++d) w.req[(size_t)d * V + dst] = w.req[(size_t)d * V + k];
+        if constexpr (HP) w.ports[dst] = w.ports[k];
       }
       ++dst;
     }
@@ -466,6 +543,10 @@ __global__ void __launch_bounds__(PREEMPT_THREADS) preempt_commit_kernel(Preempt
     w.req_present[n] |= rpres & ~0xFu;
     w.pod_count[n] += 1 - (int32_t)nv;
     walk_refresh_node(a, w, n);
+    if constexpr (HP) {   // the nominated pod's ports, kept apart from the bound ones (addNominatedPods' clone)
+      w.nom[n] |= a.hp_want[i];
+      prep_node_ports(beg, w.end[n], w.ports, w.suf_ports);
+    }
   }
   if (!w.unit_last[i]) return;
   if (c.failed && w.ent_node) {   // undo the unit, last commit first
@@ -481,6 +562,7 @@ __global__ void __launch_bounds__(PREEMPT_THREADS) preempt_commit_kernel(Preempt
           w.flags[k] = w.row_flags[r];
           w.idx[k] = w.row_idx[r];
           for (uint32_t d = 0; d < L; ++d) w.req[(size_t)d * V + k] = w.row_req[(size_t)d * V + r];
+          if constexpr (HP) w.ports[k] = w.row_ports[r];
           w.evicted_by[w.row_idx[r]] = -1;
         } else if (--src != k) {
           w.prio[k] = w.prio[src];
@@ -489,6 +571,7 @@ __global__ void __launch_bounds__(PREEMPT_THREADS) preempt_commit_kernel(Preempt
           w.flags[k] = w.flags[src];
           w.idx[k] = w.idx[src];
           for (uint32_t d = 0; d < L; ++d) w.req[(size_t)d * V + k] = w.req[(size_t)d * V + src];
+          if constexpr (HP) w.ports[k] = w.ports[src];
         }
       }
       w.end[n] = w.ent_end[e];
@@ -496,6 +579,11 @@ __global__ void __launch_bounds__(PREEMPT_THREADS) preempt_commit_kernel(Preempt
       w.req_present[n] = w.ent_rp[e];
       w.pod_count[n] = w.ent_pc[e];
       walk_refresh_node(a, w, n);
+      if constexpr (HP) {
+        w.used[n] = w.ent_used[e];
+        w.nom[n] = w.ent_nom[e];
+        prep_node_ports(beg, w.end[n], w.ports, w.suf_ports);
+      }
     }
     for (uint32_t k = c.unit_first; k <= i; ++k) {
       a.out_node[k] = -1;

@@ -487,7 +487,8 @@ class Engine:
 
     def set_host_port_filter(self, on: bool = False):
         """Switch kube-scheduler's PodFitsHostPorts filter into every pod's fit set (off by default).  While it is on,
-        each round needs upload_host_ports' two sides, and replay and preempt refuse to run."""
+        each round needs upload_host_ports' two sides; replay applies it, and preempt and preempt_walk apply it once
+        upload_bound_host_ports has given the bound pods' ports (they refuse to run without them)."""
         self._check(self.lib.bs_set_host_port_filter(self.h, 1 if on else 0))
 
     def upload_host_ports(self, node=None, pods=None):
@@ -589,6 +590,13 @@ class Engine:
         """The pods bound to the uploaded nodes (upload nodes and groups first; either upload drops this table)."""
         self._check(self.lib.bs_upload_bound_pods(self.h, C.byref(_table_c(bt))))
         self._bound_rows = bt.n
+
+    def upload_bound_host_ports(self, ports):
+        """[V] uint64, bit k = bound row v holds entry k of upload_host_ports' dictionary: what preemption under the
+        PodFitsHostPorts filter frees when it evicts the row (upload the bound pods first; uploading them again drops
+        it).  The bits are checked against the node side when a preemption starts."""
+        ports = np.ascontiguousarray(ports, dtype=np.uint64).reshape(-1)
+        self._check(self.lib.bs_upload_bound_host_ports(self.h, len(ports), capi.ptr(ports)))
 
     def preempt(self, pods, victims_cap=None) -> PreemptResult:
         """For every pod index in `pods`: the node preemption would pick and the pods it would evict there.

@@ -788,8 +788,9 @@ int bs_format_fit_error_interpod(const uint32_t* counts, uint32_t n_lanes, const
  * to each step's node choice on a live copy of the used masks: a node whose live mask conflicts with the pod's is not
  * a candidate, and assuming a pod ORs its want mask into its node's live mask (NodeInfo.AddPod); the same checks run
  * before the walk.  The live masks are not returned: they are the used masks ORed with the want masks of the pods
- * placed on each node.  bs_preempt and bs_preempt_walk refuse to run (BS_E_INVAL) while the filter is on: removing a
- * victim would have to take its ports out of the used masks. */
+ * placed on each node.  bs_preempt and bs_preempt_walk apply the filter while it is on, given the bound side
+ * (bs_upload_bound_host_ports below): removing a victim takes its ports out of its node's used mask.  Without the bound
+ * side they refuse to run (BS_E_INVAL, before any other check but the MatchInterPodAffinity filter's refusal). */
 int bs_set_host_port_filter(bs_engine* e, int on);
 #define BS_HOSTPORT_MAX 64        /* entries of the dictionary: one bit each of a uint64 mask */
 #define BS_HOSTPORT_IP_ANY 0u     /* ip id of "0.0.0.0" (and of an empty HostIP) */
@@ -814,6 +815,14 @@ int bs_upload_pod_host_ports(bs_engine* e, uint32_t n_pods, const uint64_t* want
  * the filter off.  With both filters on, bs_fetch_interpod_reason_rows counts only nodes without a port conflict:
  * upstream runs MatchInterPodAffinity after GeneralPredicates. */
 int bs_fetch_host_port_reason_rows(bs_engine* e, uint32_t pod0, uint32_t n, uint32_t* counts);
+/* The bound side: ports[n_pods], bit k = bound row v of bs_upload_bound_pods holds exactly entry k of the node side's
+ * dictionary (its containers' host ports, resolved as above).  It belongs to the bound-pod table: no table is
+ * BS_E_STATE, an n_pods other than the table's BS_E_INVAL, and bs_upload_bound_pods and every call that drops the
+ * table drop it; a failing call leaves it dropped.  The bits are checked against the node side when a preemption
+ * starts, so the sides may come in any order: a bit >= the node side's n_entries is BS_E_INDEX, and a bit its row's
+ * node's used mask does not have is BS_E_INVAL (a NodeInfo's used ports include its pods' ports).  Read only by
+ * bs_preempt and bs_preempt_walk while the filter is on. */
+int bs_upload_bound_host_ports(bs_engine* e, uint32_t n_pods, const uint64_t* ports);
 /* bs_format_fit_error with both filters' companions as further entries, sorted with the rest as whole strings: interpod
  * (NULL or [3]) as in bs_format_fit_error_interpod, host_ports (NULL or [1]) as
  *     "<count> node(s) didn't have free ports for the requested pod ports"
@@ -864,7 +873,17 @@ typedef struct {
 } bs_preempt_result;
 /* Every pods[i] (an index of the uploaded pod table) is an independent what-if against the uploaded node and bound
  * tables (DESIGN.md §2 "Preemption").  Needs nodes, groups, pods and the bound table; does not depend on, and does not
- * change, any round's state or outputs. */
+ * change, any round's state or outputs.
+ *
+ * The filters (k8s v1.17.5 selectVictimsOnNode / podPassesFiltersOnNode / NodeInfo.RemovePod [upstream, from
+ * memory]): under MatchInterPodAffinity the call refuses (BS_E_INVAL).  Under PodFitsHostPorts it needs the bound
+ * side (else BS_E_INVAL, checked next), both other sides as an evaluation does (BS_E_STATE, BS_E_INDEX) and the bound
+ * side's bits as bs_upload_bound_host_ports says.  With conf the OR of the conflict masks of the preemptor's wanted
+ * entries: removing every potential victim deletes each entry any of them holds from the node's used mask (a set
+ * delete, so an entry goes even when a more important row holds it too, as HostPortInfo.Remove does), and the node is
+ * a candidate when the resources fit and what is left has no entry in conf.  In the reprieve a row is kept when the
+ * resources fit and its own mask has no entry in conf (it is added back to the used mask); a row holding a conflicting
+ * entry is always a victim.  A node that fails only on ports is still considered. */
 int bs_preempt(bs_engine* e, const uint32_t* pods, uint32_t n, bs_preempt_result* out);
 
 /* bs_preempt_walk: the preemptors one after another, as kube-scheduler preempts one pod per cycle (DESIGN.md §2
@@ -874,6 +893,10 @@ int bs_preempt(bs_engine* e, const uint32_t* pods, uint32_t n, bs_preempt_result
  * row is never a potential victim again), and the preemptor is nominated there by bs_replay's assume rule (the pod
  * table's request on every lane but 3, its scalar keys ORed into req_present, one pod more).  A nominated pod is
  * never a victim.  Victims leave at once (graceful termination is not modelled); PreemptionPolicy is not modelled.
+ * Under PodFitsHostPorts each node has two live masks: the bound one starts as the used mask and each eviction deletes
+ * the victims' entries from it; the nominated one starts empty and each nomination ORs in the preemptor's want mask.
+ * The test of bs_preempt reads their OR.  They stay apart because upstream adds nominated pods to a clone at filter
+ * time, not to the NodeInfo its evictions edit: a later eviction never frees a nominated pod's entry.
  *
  * Rules, each BS_E_INVAL: priorities must be non-increasing along the list (queue order satisfies it; every earlier
  * nomination then counts for later preemptors and none is ever cleared); a pod listed twice; flag bits other than
@@ -882,7 +905,8 @@ int bs_preempt(bs_engine* e, const uint32_t* pods, uint32_t n, bs_preempt_result
  * BS_PREEMPT_GANG: the preemptors of one group form a unit (online and missing-group pods, and pods whose gid is
  * >= n_groups, are units of one).  When
  * a unit's last member has been walked and some member got no node, the unit is undone: the state is the one before
- * it, and every member reports node -1, 0 victims and BS_WALK_ROLLED_BACK.  A gang succeeds when every listed member
+ * it (both host-port masks and the evicted rows' ports included), and every member reports node -1, 0 victims and
+ * BS_WALK_ROLLED_BACK.  A gang succeeds when every listed member
  * got a node, so the caller lists the members the gang needs.
  *
  * out is bs_preempt's result: n_candidates counts against the live state; victims come per preemptor in reprieve

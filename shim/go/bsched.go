@@ -407,8 +407,8 @@ func (e *Engine) FetchInterPodReasonRows(pod0, n uint32, counts []uint32) error 
 }
 
 // SetHostPortFilter: kube-scheduler v1.17's PodFitsHostPorts filter in every pod's fit set and in the Replay walks
-// (off by default).  While it is on, each Evaluate and Replay needs both sides, and Preempt and PreemptWalk refuse to
-// run.
+// (off by default).  While it is on, each Evaluate and Replay needs both sides, and Preempt and PreemptWalk apply it
+// once UploadBoundHostPorts has given the bound pods' masks (they refuse to run without them).
 func (e *Engine) SetHostPortFilter(on bool) error {
 	v := C.int(0)
 	if on {
@@ -457,6 +457,19 @@ func (e *Engine) UploadPodHostPorts(want []uint64) error {
 	defer C.free(unsafe.Pointer(c))
 	copy(unsafe.Slice((*uint64)(unsafe.Pointer(c)), len(want)), want)
 	return e.rc(C.bs_upload_pod_host_ports(e.h, C.uint32_t(len(want)), c))
+}
+
+// UploadBoundHostPorts: ports[n_bound_pods], bit k = bound row v of UploadBoundPods holds exactly entry k of the
+// node side's dictionary, what preemption under the filter frees when it evicts the row.  UploadBoundPods and every
+// call that drops the bound table drop it; the bits are checked against the node side when a preemption starts.
+func (e *Engine) UploadBoundHostPorts(ports []uint64) error {
+	if len(ports) == 0 {
+		return e.rc(C.bs_upload_bound_host_ports(e.h, 0, nil))
+	}
+	c := (*C.uint64_t)(C.malloc(C.size_t(8 * len(ports))))
+	defer C.free(unsafe.Pointer(c))
+	copy(unsafe.Slice((*uint64)(unsafe.Pointer(c)), len(ports)), ports)
+	return e.rc(C.bs_upload_bound_host_ports(e.h, C.uint32_t(len(ports)), c))
 }
 
 // FetchHostPortReasonRows: the companion of FetchReasonRows, counts[n] of the nodes past the guards with a host-port
