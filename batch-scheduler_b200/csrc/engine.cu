@@ -1056,6 +1056,13 @@ void compact_fit_index(bs_engine* e) {
   fi = std::move(ni);
 }
 
+// A PodFitsHostPorts want mask's conflict mask: the OR of the node side's conflict masks of the entries it wants.
+uint64_t hp_conflict_of(const bs_engine* e, uint64_t want) {
+  uint64_t conf = 0;
+  for (; want; want &= want - 1) conf |= e->hp.h_conflict[__builtin_ctzll(want)];
+  return conf;
+}
+
 int rebuild_classes(bs_engine* e) {
   // Pod classes were indexed while the pod table was uploaded; group representative classes are
   // looked up here (the representative index must already hold the pods' (sel, tol) pairs so that
@@ -1084,13 +1091,11 @@ int rebuild_classes(bs_engine* e) {
       const uint32_t* base = e->filt.h_pfc_base.data();
       const uint32_t* ipf = e->ipf.on ? e->ipf.h_class.data() : nullptr;
       const uint64_t* want = e->hp.on ? e->hp.h_want.data() : nullptr;
-      const uint64_t* conflict = e->hp.h_conflict.data();
       ClassIndex& fi = e->fit_index;
-      assign_classes(fi, P, [&fi, base, ipf, want, conflict](uint32_t p) {
+      assign_classes(fi, P, [e, &fi, base, ipf, want](uint32_t p) {
         ClassKey k = fi.keys[base[p]];
         if (ipf) k.ipf = ipf[p];
-        if (want)
-          for (uint64_t w = want[p]; w; w &= w - 1) k.hp |= conflict[__builtin_ctzll(w)];
+        if (want) k.hp |= hp_conflict_of(e, want[p]);
         return k;
       }, pfc);
     } else if (e->filt.pfc_base_valid) {
@@ -1917,6 +1922,47 @@ struct BoundStats {
     max_gid = std::max(max_gid, o.max_gid);
   }
 };
+
+// preempt.cuh: the build of the preemption kernels for L lanes and the PodFitsHostPorts switch.  f(M, H) launches
+// with PreemptArgsOf<H> and WalkArgsOf<H>: without the filter, the base part of PreemptHpArgs and WalkHpArgs.
+template <class F>
+void with_preempt_build(uint32_t L, bool hp, F&& f) {
+  with_maxl<5, 9, 16>(L, [&](auto M) {
+    if (hp) f(M, std::true_type{});
+    else f(M, std::false_type{});
+  });
+}
+
+// bs_preempt's and bs_preempt_walk's read-back: the per-preemptor columns, with the caller's other copies (more())
+// before the synchronisation, the victim offsets and total (clamped to 32 bits; the walk's total is at most V, a row
+// is evicted once), the victim list's checks, and the victims from a.victims, which emit(total) fills first where the
+// kernels have not.
+template <class More, class Emit>
+int preempt_read_back(bs_engine* e, const char* who, PreemptArgs& a, uint32_t n, bs_preempt_result* out, More&& more,
+                      Emit&& emit) {
+  const Refuse bad{e, who};
+  int rc;
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(out->node, a.out_node, (size_t)n * 4, cudaMemcpyDeviceToHost, e->s));
+  CK(cudaMemcpyAsync(out->n_victims, a.out_nv, (size_t)n * 4, cudaMemcpyDeviceToHost, e->s));
+  CK(cudaMemcpyAsync(out->n_candidates, a.out_cand, (size_t)n * 4, cudaMemcpyDeviceToHost, e->s));
+  if ((rc = more())) return rc;
+  CK(cudaStreamSynchronize(e->s));
+  uint64_t total = 0;
+  for (uint32_t i = 0; i < n; ++i) {
+    out->victim_offset[i] = (uint32_t)std::min<uint64_t>(total, UINT32_MAX);
+    total += out->n_victims[i];
+  }
+  out->victim_offset[n] = (uint32_t)std::min<uint64_t>(total, UINT32_MAX);
+  out->victims_total = (uint32_t)std::min<uint64_t>(total, UINT32_MAX);
+  if (total > out->victims_cap) return bad(BS_E_INVAL, "victims_cap is smaller than victims_total");
+  if (!total) return BS_OK;
+  if (!out->victims) return bad(BS_E_INVAL, "null victims buffer");
+  if ((rc = emit(total))) return rc;
+  CK(cudaMemcpyAsync(out->victims, a.victims, (size_t)total * 4, cudaMemcpyDeviceToHost, e->s));
+  CK(cudaStreamSynchronize(e->s));
+  return BS_OK;
+}
 
 }  // namespace
 
@@ -2884,8 +2930,7 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
   if (hp) {
     CK(dup(s_used, e->hp.d_used, (size_t)Npad * 8));
     conf.assign(P, 0);
-    for (uint32_t p = 0; p < P; ++p)
-      for (uint64_t w = e->hp.h_want[p]; w; w &= w - 1) conf[p] |= e->hp.h_conflict[__builtin_ctzll(w)];
+    for (uint32_t p = 0; p < P; ++p) conf[p] = hp_conflict_of(e, e->hp.h_want[p]);
     if (P) {
       CK(cudaMemcpyAsync(d_want.p, e->hp.h_want.data(), (size_t)P * 8, cudaMemcpyHostToDevice, e->s));
       CK(cudaMemcpyAsync(d_conf.p, conf.data(), (size_t)P * 8, cudaMemcpyHostToDevice, e->s));
@@ -3020,52 +3065,12 @@ int replay_walk(bs_engine* e, const char* who, const uint32_t* queue, uint32_t n
 }
 }  // namespace
 
-// Preemption refuses to run under the MatchInterPodAffinity filter: its presence would have to shrink when victims leave
-// (upstream's metadata RemovePod).  The walks follow their own placements in live presence, which needs each pod's
-// placed class: without it they refuse as well.  Preemption refuses to run under the PodFitsHostPorts filter: its
-// victims' removal would have to take their ports out of the used masks (the walks follow their own placements in a
-// live copy of them).  With the bound pods' host-port masks (bs_upload_bound_host_ports) it runs: see
-// host_port_preempt_check.
-static int interpod_filter_refuse(bs_engine* e, const char* who) {
-  return fail(e, BS_E_INVAL, (std::string(who) + ": the MatchInterPodAffinity filter is not supported here; "
-                              "switch it off with bs_set_interpod_filter").c_str());
-}
+// The walks follow their own placements in live MatchInterPodAffinity presence, which needs each pod's placed class:
+// without it they refuse.
 static int interpod_placed_refuse(bs_engine* e, const char* who) {
   return fail(e, BS_E_INVAL, (std::string(who) + ": the MatchInterPodAffinity filter needs the pods' placed classes in "
                               "the walk; upload them with bs_upload_pod_interpod_placed or switch the filter off with "
                               "bs_set_interpod_filter").c_str());
-}
-static int host_port_refuse(bs_engine* e, const char* who) {
-  return fail(e, BS_E_INVAL, (std::string(who) + ": the PodFitsHostPorts filter needs the bound pods' host ports in "
-                              "preemption; upload them with bs_upload_bound_host_ports or switch the filter off with "
-                              "bs_set_host_port_filter").c_str());
-}
-
-// bs_preempt and bs_preempt_walk under the PodFitsHostPorts filter: both sides of the filter as the round needs them,
-// and each bound row's bits entries of the node side's dictionary that its node uses (a NodeInfo's used ports include
-// its pods').  Then each preemptor's want and conflict masks.  The caller holds the engine's lock.
-static int host_port_preempt_check(bs_engine* e, const char* who, const uint32_t* pods, uint32_t n,
-                                   std::vector<uint64_t>& want, std::vector<uint64_t>& conf) {
-  if (int rc = host_port_check(e, who)) return rc;
-  const Refuse bad{e, who};
-  const std::vector<uint64_t>& bp = e->hp.h_bports;
-  uint64_t all = 0;
-  bool outside = false;
-  for (uint32_t v = 0; v < (uint32_t)bp.size(); ++v) {
-    all |= bp[v];
-    outside = outside || (bp[v] & ~e->hp.h_used[e->h_bnode[v]]) != 0;
-  }
-  if (e->hp.entries < 64 && (all >> e->hp.entries))
-    return bad(BS_E_INDEX, "a bound pod's host-port bit is outside the node side's dictionary");
-  if (outside) return bad(BS_E_INVAL, "a bound pod holds a host port its node's used mask does not have");
-  want.assign(std::max(n, 1u), 0);
-  conf.assign(std::max(n, 1u), 0);
-  for (uint32_t i = 0; i < n; ++i) {
-    if (pods[i] >= e->P) continue;   // preempt_pods refuses it
-    want[i] = e->hp.h_want[pods[i]];
-    for (uint64_t w = want[i]; w; w &= w - 1) conf[i] |= e->hp.h_conflict[__builtin_ctzll(w)];
-  }
-  return BS_OK;
 }
 
 int bs_replay(bs_engine* e, const uint32_t* queue, uint32_t n_queue, bs_replay_result* out) {
@@ -3214,22 +3219,61 @@ int bs_upload_bound_pods(bs_engine* e, const bs_bound_table* t) {
 }
 
 namespace {
-// bs_preempt and bs_preempt_walk: the state checks and each preemptor as the kernels take it.  The caller holds the
+// What bs_preempt and bs_preempt_walk hand their kernels for each preemptor: its row, and while the PodFitsHostPorts
+// filter is on (hp) its conflict mask and, in the walk, its want mask (what its nomination adds to its node's).
+struct Preemptors {
+  bool hp = false;
+  std::vector<PreemptPod> pp;
+  std::vector<uint64_t> conf, want;
+};
+
+// bs_preempt's and bs_preempt_walk's checks, in this order: the arguments; the MatchInterPodAffinity filter, which
+// preemption refuses (its presence would have to shrink when victims leave: upstream's metadata RemovePod); the
+// PodFitsHostPorts filter without the bound pods' host-port masks (bs_upload_bound_host_ports), which preemption needs
+// to take its victims' ports out of the used masks; flag bits other than BS_PREEMPT_GANG; both sides of the ports
+// filter as the round needs them, and each bound row's bits entries of the node side's dictionary that its node uses
+// (a NodeInfo's used ports include its pods'); the tables; each preemptor.  `walk` fills q.want.  The caller holds the
 // engine's lock.
-int preempt_pods(bs_engine* e, const char* who, const uint32_t* pods, uint32_t n, std::vector<PreemptPod>& pp) {
-  const std::string w(who);
+int preempt_prologue(bs_engine* e, const char* who, const uint32_t* pods, uint32_t n, const bs_preempt_result* out,
+                     uint32_t flags, bool walk, Preemptors& q) {
+  if (!out || (n && (!pods || !out->node || !out->n_victims || !out->n_candidates)) || !out->victim_offset)
+    return BS_E_INVAL;
+  const Refuse bad{e, who};
+  if (e->ipf.on)
+    return bad(BS_E_INVAL, "the MatchInterPodAffinity filter is not supported here; switch it off with "
+                           "bs_set_interpod_filter");
+  q.hp = e->hp.on;
+  if (q.hp && !e->hp.have_bound)
+    return bad(BS_E_INVAL, "the PodFitsHostPorts filter needs the bound pods' host ports in preemption; upload them "
+                           "with bs_upload_bound_host_ports or switch the filter off with bs_set_host_port_filter");
+  if (flags & ~BS_PREEMPT_GANG) return bad(BS_E_INVAL, "unknown flag bits");
+  if (q.hp) {
+    if (int rc = host_port_check(e, who)) return rc;
+    const std::vector<uint64_t>& bp = e->hp.h_bports;
+    uint64_t all = 0;
+    bool outside = false;
+    for (uint32_t v = 0; v < (uint32_t)bp.size(); ++v) {
+      all |= bp[v];
+      outside = outside || (bp[v] & ~e->hp.h_used[e->h_bnode[v]]) != 0;
+    }
+    if (e->hp.entries < 64 && (all >> e->hp.entries))
+      return bad(BS_E_INDEX, "a bound pod's host-port bit is outside the node side's dictionary");
+    if (outside) return bad(BS_E_INVAL, "a bound pod holds a host port its node's used mask does not have");
+  }
   if (!e->have_nodes || !e->have_groups || !e->have_pods || !e->have_bound)
-    return fail(e, BS_E_STATE, (w + ": upload nodes, groups, pods and the bound-pod table first").c_str());
-  if (e->bound_max_gid >= (int32_t)e->G)
-    return fail(e, BS_E_INDEX, (w + ": a bound pod's group index >= n_groups").c_str());
-  pp.assign(std::max(n, 1u), PreemptPod{});
+    return bad(BS_E_STATE, "upload nodes, groups, pods and the bound-pod table first");
+  if (e->bound_max_gid >= (int32_t)e->G) return bad(BS_E_INDEX, "a bound pod's group index >= n_groups");
+  q.pp.assign(std::max(n, 1u), PreemptPod{});
+  if (q.hp) q.conf.assign(std::max(n, 1u), 0);
+  if (q.hp && walk) q.want.assign(std::max(n, 1u), 0);
   for (uint32_t i = 0; i < n; ++i) {
     const uint32_t p = pods[i];
-    if (p >= e->P) return fail(e, BS_E_INDEX, (w + ": pod index outside the pod table").c_str());
+    if (p >= e->P) return bad(BS_E_INDEX, "pod index outside the pod table");
     const ClassKey& k = e->fit_index.keys[e->h_pfc[p]];
-    if (k.aff != BS_AFF_NONE && k.aff >= e->n_aff)
-      return fail(e, BS_E_INDEX, (w + ": affinity class outside the uploaded table").c_str());
-    pp[i] = PreemptPod{k.sel, k.tol, p, k.nz, k.aff, e->h_prio[p], e->h_gid[p]};
+    if (k.aff != BS_AFF_NONE && k.aff >= e->n_aff) return bad(BS_E_INDEX, "affinity class outside the uploaded table");
+    q.pp[i] = PreemptPod{k.sel, k.tol, p, k.nz, k.aff, e->h_prio[p], e->h_gid[p]};
+    if (q.hp) q.conf[i] = hp_conflict_of(e, e->hp.h_want[p]);
+    if (q.hp && walk) q.want[i] = e->hp.h_want[p];
   }
   return BS_OK;
 }
@@ -3252,20 +3296,25 @@ PreemptArgs preempt_args(const bs_engine* e, uint32_t n) {
   a.n_tiles = cdiv(e->N, PREEMPT_THREADS);
   return a;
 }
+
+// The PodFitsHostPorts views of PreemptHpArgs: bs_preempt passes the uploaded masks and no nominated or want masks,
+// bs_preempt_walk its live copies.
+void hp_views(PreemptHpArgs& ha, const uint64_t* used, const uint64_t* nom, const uint64_t* ports, const uint64_t* suf,
+              const uint64_t* conf, const uint64_t* want) {
+  ha.hp_used = used;
+  ha.hp_nom = nom;
+  ha.hp_ports = ports;
+  ha.hp_suf = suf;
+  ha.hp_conf = conf;
+  ha.hp_want = want;
+}
 }  // namespace
 
 int bs_preempt(bs_engine* e, const uint32_t* pods, uint32_t n, bs_preempt_result* out) {
-  if (!e || !out || (n && (!pods || !out->node || !out->n_victims || !out->n_candidates)) || !out->victim_offset)
-    return BS_E_INVAL;
+  if (!e) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
-  if (e->ipf.on) return interpod_filter_refuse(e, "bs_preempt");
-  const bool hp = e->hp.on;
-  if (hp && !e->hp.have_bound) return host_port_refuse(e, "bs_preempt");
-  std::vector<PreemptPod> pp;
-  std::vector<uint64_t> want, conf;
-  int rc;
-  if (hp && (rc = host_port_preempt_check(e, "bs_preempt", pods, n, want, conf))) return rc;
-  if ((rc = preempt_pods(e, "bs_preempt", pods, n, pp))) return rc;
+  Preemptors q;
+  if (int rc = preempt_prologue(e, "bs_preempt", pods, n, out, 0, false, q)) return rc;
   const uint32_t L = e->L, N = e->N;
   out->victim_offset[0] = 0;
   out->victims_total = 0;
@@ -3276,17 +3325,15 @@ int bs_preempt(bs_engine* e, const uint32_t* pods, uint32_t n, bs_preempt_result
   CK(e->d_pnv.ensure((size_t)n * 4));
   CK(e->d_pcand.ensure((size_t)n * 4));
   CK(e->d_poff.ensure((size_t)n * 4));
-  CK(cudaMemcpyAsync(e->d_pp.p, pp.data(), (size_t)n * sizeof(PreemptPod), cudaMemcpyHostToDevice, e->s));
+  CK(cudaMemcpyAsync(e->d_pp.p, q.pp.data(), (size_t)n * sizeof(PreemptPod), cudaMemcpyHostToDevice, e->s));
   PreemptHpArgs ha{};
   PreemptArgs& a = ha;
   a = preempt_args(e, n);
-  if (hp) {
+  if (q.hp) {
     CK(e->hp.d_pconf.ensure((size_t)n * 8));
-    CK(cudaMemcpyAsync(e->hp.d_pconf.p, conf.data(), (size_t)n * 8, cudaMemcpyHostToDevice, e->s));
-    ha.hp_used = e->hp.d_used.as<uint64_t>();
-    ha.hp_ports = e->hp.d_bports.as<uint64_t>();
-    ha.hp_suf = e->hp.d_bsuf.as<uint64_t>();
-    ha.hp_conf = e->hp.d_pconf.as<uint64_t>();
+    CK(cudaMemcpyAsync(e->hp.d_pconf.p, q.conf.data(), (size_t)n * 8, cudaMemcpyHostToDevice, e->s));
+    hp_views(ha, e->hp.d_used.as<uint64_t>(), nullptr, e->hp.d_bports.as<uint64_t>(), e->hp.d_bsuf.as<uint64_t>(),
+             e->hp.d_pconf.as<uint64_t>(), nullptr);
   }
   a.out_node = e->d_pnode.as<int32_t>();
   a.out_nv = e->d_pnv.as<uint32_t>();
@@ -3304,59 +3351,35 @@ int bs_preempt(bs_engine* e, const uint32_t* pods, uint32_t n, bs_preempt_result
     for (uint32_t p0 = 0; p0 < n; p0 += chunk) {
       const uint32_t cnt = std::min(chunk, n - p0);
       a.p0 = p0;
-      with_maxl<5, 9, 16>(L, [&](auto M) {
-        if (hp) preempt_node_kernel<M, true><<<dim3(a.n_tiles, cnt), PREEMPT_THREADS, 0, e->s>>>(ha);
-        else preempt_node_kernel<M, false><<<dim3(a.n_tiles, cnt), PREEMPT_THREADS, 0, e->s>>>(a);
+      with_preempt_build(L, q.hp, [&](auto M, auto H) {
+        preempt_node_kernel<M, H><<<dim3(a.n_tiles, cnt), PREEMPT_THREADS, 0, e->s>>>(PreemptArgsOf<H>(ha));
       });
       preempt_reduce_kernel<<<cdiv(cnt, 256), 256, 0, e->s>>>(a, cnt);
       e->launches += 2;
     }
   }
-  CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(out->node, a.out_node, (size_t)n * 4, cudaMemcpyDeviceToHost, e->s));
-  CK(cudaMemcpyAsync(out->n_victims, a.out_nv, (size_t)n * 4, cudaMemcpyDeviceToHost, e->s));
-  CK(cudaMemcpyAsync(out->n_candidates, a.out_cand, (size_t)n * 4, cudaMemcpyDeviceToHost, e->s));
-  CK(cudaStreamSynchronize(e->s));
-  uint64_t total = 0;
-  for (uint32_t i = 0; i < n; ++i) {
-    out->victim_offset[i] = (uint32_t)std::min<uint64_t>(total, UINT32_MAX);
-    total += out->n_victims[i];
-  }
-  out->victim_offset[n] = (uint32_t)std::min<uint64_t>(total, UINT32_MAX);
-  out->victims_total = (uint32_t)std::min<uint64_t>(total, UINT32_MAX);
-  if (total > out->victims_cap) return fail(e, BS_E_INVAL, "bs_preempt: victims_cap is smaller than victims_total");
-  if (!total) return BS_OK;
-  if (!out->victims) return fail(e, BS_E_INVAL, "bs_preempt: null victims buffer");
-  CK(e->d_pvict.ensure((size_t)total * 4));
-  CK(cudaMemcpyAsync(e->d_poff.p, out->victim_offset, (size_t)n * 4, cudaMemcpyHostToDevice, e->s));
-  a.offset = e->d_poff.as<uint32_t>();
-  a.victims = e->d_pvict.as<uint32_t>();
-  with_maxl<5, 9, 16>(L, [&](auto M) {
-    if (hp) preempt_emit_kernel<M, true><<<dim3(cdiv(n, 256)), 256, 0, e->s>>>(ha);
-    else preempt_emit_kernel<M, false><<<dim3(cdiv(n, 256)), 256, 0, e->s>>>(a);
+  return preempt_read_back(e, "bs_preempt", a, n, out, [] { return BS_OK; }, [&](uint64_t total) -> int {
+    CK(e->d_pvict.ensure((size_t)total * 4));
+    CK(cudaMemcpyAsync(e->d_poff.p, out->victim_offset, (size_t)n * 4, cudaMemcpyHostToDevice, e->s));
+    a.offset = e->d_poff.as<uint32_t>();
+    a.victims = e->d_pvict.as<uint32_t>();
+    with_preempt_build(L, q.hp, [&](auto M, auto H) {
+      preempt_emit_kernel<M, H><<<dim3(cdiv(n, 256)), 256, 0, e->s>>>(PreemptArgsOf<H>(ha));
+    });
+    ++e->launches;
+    CK(cudaGetLastError());
+    return BS_OK;
   });
-  ++e->launches;
-  CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(out->victims, a.victims, (size_t)total * 4, cudaMemcpyDeviceToHost, e->s));
-  CK(cudaStreamSynchronize(e->s));
-  return BS_OK;
 }
 
 int bs_preempt_walk(bs_engine* e, const uint32_t* pods, uint32_t n, uint32_t flags, bs_preempt_result* out,
                     uint32_t* outcome, int32_t* evicted_by) {
-  if (!e || !out || (n && (!pods || !out->node || !out->n_victims || !out->n_candidates)) || !out->victim_offset)
-    return BS_E_INVAL;
+  if (!e) return BS_E_INVAL;
   std::lock_guard<std::mutex> lk(e->mu);
-  if (e->ipf.on) return interpod_filter_refuse(e, "bs_preempt_walk");
-  const bool hp = e->hp.on;
-  if (hp && !e->hp.have_bound) return host_port_refuse(e, "bs_preempt_walk");
-  if (flags & ~BS_PREEMPT_GANG) return fail(e, BS_E_INVAL, "bs_preempt_walk: unknown flag bits");
-  const bool gang = flags & BS_PREEMPT_GANG;
-  std::vector<PreemptPod> pp;
-  std::vector<uint64_t> want, conf;
-  int rc;
-  if (hp && (rc = host_port_preempt_check(e, "bs_preempt_walk", pods, n, want, conf))) return rc;
-  if ((rc = preempt_pods(e, "bs_preempt_walk", pods, n, pp))) return rc;
+  Preemptors q;
+  if (int rc = preempt_prologue(e, "bs_preempt_walk", pods, n, out, flags, true, q)) return rc;
+  const bool gang = flags & BS_PREEMPT_GANG, hp = q.hp;
+  const std::vector<PreemptPod>& pp = q.pp;
   // queue order: every earlier nomination has a priority >= the current preemptor's, so all of them count
   // (addNominatedPods) and none is ever cleared (getLowerPriorityNominatedPods)
   std::vector<uint8_t> seen(e->P, 0), closed(gang ? e->G : 0, 0), unit_last(std::max(n, 1u), 1);
@@ -3483,8 +3506,8 @@ int bs_preempt_walk(bs_engine* e, const uint32_t* pods, uint32_t n, uint32_t fla
                  w.suf_vio, Vp};
   a.pp = w_pp.as<PreemptPod>();
   if (hp) {   // the live masks: the bound ones start as the node side's, the nominated ones empty
-    CK(cudaMemcpyAsync(h_conf.p, conf.data(), (size_t)n * 8, cudaMemcpyHostToDevice, e->s));
-    CK(cudaMemcpyAsync(h_want.p, want.data(), (size_t)n * 8, cudaMemcpyHostToDevice, e->s));
+    CK(cudaMemcpyAsync(h_conf.p, q.conf.data(), (size_t)n * 8, cudaMemcpyHostToDevice, e->s));
+    CK(cudaMemcpyAsync(h_want.p, q.want.data(), (size_t)n * 8, cudaMemcpyHostToDevice, e->s));
     CK(dup(h_used, e->hp.d_used.p, (size_t)Npad * 8));
     CK(cudaMemsetAsync(h_nom.p, 0, (size_t)Npad * 8, e->s));
     CK(dup(h_ports, e->hp.d_bports.p, (size_t)Vp * 8));
@@ -3498,12 +3521,7 @@ int bs_preempt_walk(bs_engine* e, const uint32_t* pods, uint32_t n, uint32_t fla
       hw.ent_nom = he_nom.as<uint64_t>();
       hw.row_ports = hr_ports.as<uint64_t>();
     }
-    ha.hp_used = hw.used;
-    ha.hp_nom = hw.nom;
-    ha.hp_ports = hw.ports;
-    ha.hp_suf = hw.suf_ports;
-    ha.hp_conf = h_conf.as<uint64_t>();
-    ha.hp_want = h_want.as<uint64_t>();
+    hp_views(ha, hw.used, hw.nom, hw.ports, hw.suf_ports, h_conf.as<uint64_t>(), h_want.as<uint64_t>());
   }
   a.tiles = w_tiles.as<PickKey>();
   a.out_node = w_node.as<int32_t>();
@@ -3511,40 +3529,21 @@ int bs_preempt_walk(bs_engine* e, const uint32_t* pods, uint32_t n, uint32_t fla
   a.out_cand = w_cand.as<uint32_t>();
   a.victims = w_vict.as<uint32_t>();
   for (uint32_t i = 0; i < n; ++i) {   // stream-ordered: no host synchronisation inside the walk
-    if (N) {
-      a.p0 = i;
-      with_maxl<5, 9, 16>(L, [&](auto M) {
-        if (hp) preempt_node_kernel<M, true><<<dim3(a.n_tiles, 1), PREEMPT_THREADS, 0, e->s>>>(ha);
-        else preempt_node_kernel<M, false><<<dim3(a.n_tiles, 1), PREEMPT_THREADS, 0, e->s>>>(a);
-      });
+    with_preempt_build(L, hp, [&](auto M, auto H) {
+      if (N) {
+        a.p0 = i;
+        preempt_node_kernel<M, H><<<dim3(a.n_tiles, 1), PREEMPT_THREADS, 0, e->s>>>(PreemptArgsOf<H>(ha));
+        ++e->launches;
+      }
+      preempt_commit_kernel<M, H><<<1, PREEMPT_THREADS, 0, e->s>>>(PreemptArgsOf<H>(ha), WalkArgsOf<H>(hw), i);
       ++e->launches;
-    }
-    with_maxl<5, 9, 16>(L, [&](auto M) {
-      if (hp) preempt_commit_kernel<M, true><<<1, PREEMPT_THREADS, 0, e->s>>>(ha, hw, i);
-      else preempt_commit_kernel<M, false><<<1, PREEMPT_THREADS, 0, e->s>>>(a, w, i);
     });
-    ++e->launches;
   }
-  CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(out->node, a.out_node, (size_t)n * 4, cudaMemcpyDeviceToHost, e->s));
-  CK(cudaMemcpyAsync(out->n_victims, a.out_nv, (size_t)n * 4, cudaMemcpyDeviceToHost, e->s));
-  CK(cudaMemcpyAsync(out->n_candidates, a.out_cand, (size_t)n * 4, cudaMemcpyDeviceToHost, e->s));
-  if (outcome) CK(cudaMemcpyAsync(outcome, w.outcome, (size_t)n * 4, cudaMemcpyDeviceToHost, e->s));
-  if (evicted_by && V) CK(cudaMemcpyAsync(evicted_by, w.evicted_by, (size_t)V * 4, cudaMemcpyDeviceToHost, e->s));
-  CK(cudaStreamSynchronize(e->s));
-  uint32_t total = 0;   // at most V: a row is evicted once
-  for (uint32_t i = 0; i < n; ++i) {
-    out->victim_offset[i] = total;
-    total += out->n_victims[i];
-  }
-  out->victim_offset[n] = total;
-  out->victims_total = total;
-  if (total > out->victims_cap) return fail(e, BS_E_INVAL, "bs_preempt_walk: victims_cap is smaller than victims_total");
-  if (!total) return BS_OK;
-  if (!out->victims) return fail(e, BS_E_INVAL, "bs_preempt_walk: null victims buffer");
-  CK(cudaMemcpyAsync(out->victims, a.victims, (size_t)total * 4, cudaMemcpyDeviceToHost, e->s));
-  CK(cudaStreamSynchronize(e->s));
-  return BS_OK;
+  return preempt_read_back(e, "bs_preempt_walk", a, n, out, [&]() -> int {
+    if (outcome) CK(cudaMemcpyAsync(outcome, w.outcome, (size_t)n * 4, cudaMemcpyDeviceToHost, e->s));
+    if (evicted_by && V) CK(cudaMemcpyAsync(evicted_by, w.evicted_by, (size_t)V * 4, cudaMemcpyDeviceToHost, e->s));
+    return BS_OK;
+  }, [](uint64_t) { return BS_OK; });
 }
 
 // core.PreemptRemovePod (core.go:203-260).  "Offline" = carries the group label (VerifyPodLabelSatisfied,

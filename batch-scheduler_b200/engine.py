@@ -598,9 +598,9 @@ class Engine:
         ports = np.ascontiguousarray(ports, dtype=np.uint64).reshape(-1)
         self._check(self.lib.bs_upload_bound_host_ports(self.h, len(ports), capi.ptr(ports)))
 
-    def preempt(self, pods, victims_cap=None) -> PreemptResult:
-        """For every pod index in `pods`: the node preemption would pick and the pods it would evict there.
-        victims_cap: capacity of the victim list (None: as large as the answer needs, found with a first call)."""
+    def _preempt_call(self, pods, victims_cap, call):
+        """bs_preempt or bs_preempt_walk as call(pods pointer, n, result) into fresh result arrays, with a first call
+        to size the victim list when victims_cap is None: (node, n_victims, n_candidates, victim_offset, victims)."""
         idx = np.ascontiguousarray(pods, dtype=np.uint32)
         n = len(idx)
         node, nv, cand = np.zeros(n, np.int32), np.zeros(n, np.uint32), np.zeros(n, np.uint32)
@@ -609,34 +609,29 @@ class Engine:
         while True:
             vict = np.zeros(max(cap, 1), np.uint32)
             r = capi.PreemptResultC(capi.ptr(node), capi.ptr(nv), capi.ptr(cand), capi.ptr(off), capi.ptr(vict), cap, 0)
-            rc = self.lib.bs_preempt(self.h, capi.ptr(idx) if n else None, n, C.byref(r))
+            rc = call(capi.ptr(idx) if n else None, n, C.byref(r))
             if rc == capi.BS_E_INVAL and victims_cap is None and r.victims_total > cap:
                 cap = r.victims_total
                 continue
             self._check(rc)
-            return PreemptResult(node, nv, cand, off, vict[:r.victims_total].copy())
+            return node, nv, cand, off, vict[:r.victims_total].copy()
+
+    def preempt(self, pods, victims_cap=None) -> PreemptResult:
+        """For every pod index in `pods`: the node preemption would pick and the pods it would evict there.
+        victims_cap: capacity of the victim list (None: as large as the answer needs, found with a first call)."""
+        return PreemptResult(*self._preempt_call(pods, victims_cap,
+                                                 lambda p, n, r: self.lib.bs_preempt(self.h, p, n, r)))
 
     def preempt_walk(self, pods, gang=False, victims_cap=None) -> PreemptWalkResult:
         """The preemptors of `pods` one after another in list order (priorities non-increasing), each seeing the
         evictions and nominations of those before it; with `gang`, the preemptors of one group (contiguous in the
         list) are preempted for all together or not at all.  victims_cap as in preempt()."""
         idx = np.ascontiguousarray(pods, dtype=np.uint32)
-        n = len(idx)
-        node, nv, cand = np.zeros(n, np.int32), np.zeros(n, np.uint32), np.zeros(n, np.uint32)
-        off, outcome = np.zeros(n + 1, np.uint32), np.zeros(n, np.uint32)
-        evicted_by = np.zeros(self._bound_rows, np.int32)
+        outcome, evicted_by = np.zeros(len(idx), np.uint32), np.zeros(self._bound_rows, np.int32)
         flags = capi.PREEMPT_GANG if gang else 0
-        cap = 0 if victims_cap is None else victims_cap
-        while True:
-            vict = np.zeros(max(cap, 1), np.uint32)
-            r = capi.PreemptResultC(capi.ptr(node), capi.ptr(nv), capi.ptr(cand), capi.ptr(off), capi.ptr(vict), cap, 0)
-            rc = self.lib.bs_preempt_walk(self.h, capi.ptr(idx) if n else None, n, flags, C.byref(r),
-                                          capi.ptr(outcome) if n else None, capi.ptr(evicted_by))
-            if rc == capi.BS_E_INVAL and victims_cap is None and r.victims_total > cap:
-                cap = r.victims_total
-                continue
-            self._check(rc)
-            return PreemptWalkResult(node, nv, cand, off, vict[:r.victims_total].copy(), outcome, evicted_by)
+        res = self._preempt_call(idx, victims_cap, lambda p, n, r: self.lib.bs_preempt_walk(
+            self.h, p, n, flags, r, capi.ptr(outcome) if n else None, capi.ptr(evicted_by)))
+        return PreemptWalkResult(*res, outcome, evicted_by)
 
     def remove_pod(self, pod: int, bound: int):
         """batchSchedulingPluginExtension.RemovePod for pod `pod` and bound pod `bound`: (code, reason, group)."""

@@ -415,8 +415,8 @@ class Model:
         return self._affinity_check()
 
     def _preempt(self, op):
-        """bs_preempt's checks (preempt_pods in engine.cu): the filters' switches, the tables, then each listed pod's
-        index and affinity class."""
+        """bs_preempt's checks (preempt_prologue in engine.cu): the filters' switches, the tables, then each listed
+        pod's index and affinity class."""
         if self.ipf_on or self.hp_on:
             return E_INVAL
         if not self.complete() or self.bound is None:
